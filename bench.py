@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- the reference's headline metric on B200: separated frames/s (8 ms hops of a 16 kHz
+"""bench.py -- the reference's headline metric on one H100: separated frames/s (8 ms hops of a 16 kHz
 binaural stream) and the real-time factor, for BASELINE.json configs[1]: separation in 8 ms chunks,
 batch 1, fp32, one stream per GPU.
 
@@ -16,10 +16,13 @@ through the C-ABI host-buffer call (l2h_sep_stream_host): per round of up to 500
 copy of the round's samples from pinned memory and ONE device->host copy of its output, inside the
 timed region.  Further blocks on the line: `batched_streaming` (configs[4] per-GPU shape, 256 streams
 per rank, at every N), `offline_bf16_256` (configs[2]), `enrollment_1024` (configs[3]).
-`--impl reference` times the reference's own CPU path (the reference modules when the checkout is
-present, else the oracle port) on the host cores with the same workload.
+`--impl reference` times the reference's CPU path (the oracle port, oracle/restate.py, pinned to the reference
+by tests/test_oracle.py) on the host cores with the same workload.
+`--dump-outputs DIR` writes, after the timed steps, what the timed path returned in its last step:
+DIR/separated.npy (float32 [1, 2, 64000], the separated binaural clip; separated_rank<r>.npy on rank r > 0).
+Inputs and weights are seeded, so two builds can be compared output for output.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--chunks-per-call C] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--chunks-per-call C] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
 """
 import argparse
@@ -53,11 +56,9 @@ def workload_name():
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.isfile(p):
-        d = json.load(open(p))
-        return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d.get("bf16_tflops_sustained", 1412.4), source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W card): HBM3 bandwidth and dense BF16 tensor rate.  Not reached figures: a
+    # card with a lower power limit (the `clocks` block) runs below them.
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, source="NVIDIA H100 SXM data sheet (not measured)")
 
 
 class ClockSampler(threading.Thread):
@@ -115,34 +116,25 @@ def cpu_model_name():
 
 
 def time_cpu_streaming(frames, chunks_per_call, passes, threads, seed=0):
-    """The CPU path on the host cores: chunked predict(pad=False) over `frames` hops, B=1.
-    Uses the reference's own modules when the checkout exists, else the oracle port."""
+    """The CPU path on the host cores: chunked predict(pad=False) over `frames` hops, B=1, through the oracle port
+    of the reference (same ops: ATen's fused LSTM, like the reference's nn.LSTM)."""
     from lookoncetohear_b200 import Net, synth
     from lookoncetohear_b200.configs import TSH_PARAMS
-    from oracle import ref_loader, restate
+    from oracle import restate
     torch.set_num_threads(threads)
     x, _ = synth.mixture(1, frames * HOP)
     e = synth.embedding(1)[:, 0]
     xp = torch.nn.functional.pad(x, (0, 64))
     step = HOP * chunks_per_call
-    if ref_loader.available():
-        kind = "reference"
-        net = ref_loader.reference_net(seed)
+    kind = "port"
+    restate.set_fast(True)
+    torch.manual_seed(seed)
+    sd = {k: v.detach().clone() for k, v in Net(**TSH_PARAMS).state_dict().items()}
 
-        def one_pass():
-            st = net.init_buffers(1, "cpu")
-            for i in range(0, frames, chunks_per_call):
-                net.predict(xp[..., HOP * i:HOP * i + step + 64], e, st, pad=False)
-    else:
-        kind = "port"
-        restate.set_fast(True)            # ATen's fused LSTM, like the reference's nn.LSTM
-        torch.manual_seed(seed)
-        sd = {k: v.detach().clone() for k, v in Net(**TSH_PARAMS).state_dict().items()}
-
-        def one_pass():
-            st = restate.sep_init_state(sd, 1)
-            for i in range(0, frames, chunks_per_call):
-                restate.sep_predict(sd, xp[..., HOP * i:HOP * i + step + 64], e, st, pad=False)
+    def one_pass():
+        st = restate.sep_init_state(sd, 1)
+        for i in range(0, frames, chunks_per_call):
+            restate.sep_predict(sd, xp[..., HOP * i:HOP * i + step + 64], e, st, pad=False)
     best = None
     with torch.no_grad():
         for _ in range(passes):
@@ -277,6 +269,8 @@ def main():
     ap.add_argument("--no-extras", action="store_true", help="skip the latency / buffered-throughput extras")
     ap.add_argument("--clip-hops", type=int, default=0,
                     help="profiling aid: shorten the clip to this many hops (the default, 0, is the 4 s = 500-hop clip)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the separated clip of the last timed step as DIR/separated.npy")
     args = ap.parse_args()
 
     global CLIP_SAMPLES, FRAMES
@@ -321,7 +315,7 @@ def main():
     x_dev = x_cpu.to(dev)
     x_pin = x_cpu.pin_memory()
     y_dev = torch.empty(1, 2, CLIP_SAMPLES, device=dev)
-    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)      # 256 MiB > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)      # 256 MiB > 50 MB L2
     L = _cabi.lib()
 
     def step_dev():
@@ -356,6 +350,11 @@ def main():
         evs.append((a, b))
     barrier()
     t_wall = time.perf_counter() - t_wall0
+    if args.dump_outputs:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        name = "separated.npy" if rank == 0 else f"separated_rank{rank}.npy"
+        np.save(os.path.join(args.dump_outputs, name), y_dev.cpu().numpy().astype(np.float32))
     n_launched = ctypes.c_int64()
     _cabi.check(L.l2h_sep_launch_count(net._engine(), ctypes.byref(n_launched), 0))
     dev_ms = sum(a.elapsed_time(b) for a, b in evs)
@@ -526,34 +525,27 @@ def main():
         tr = trace_one_hop(net, x_dev, emb, dev)
         fps_seq = extras.get("frames_per_s_unpipelined")
         chain_us = 1e6 / fps_seq if fps_seq else tr["span_us"]      # device time per hop of back-to-back one-hop calls (chain + the gap between two graph launches)
-        latency_model = {"serial_steps": 3 * 97, "t_step_floor_us": 0.23, "t_step_measured_us": tr["t_step_us"],
+        latency_model = {"serial_steps": 3 * 97, "t_step_measured_us": tr["t_step_us"],
                          "chain_us": chain_us, "kernels_per_hop": tr["kernels"],
-                         "latency_frac": 3 * 97 * 0.23 / chain_us, "recurrence_share_of_chain": 3 * 97 * (tr["t_step_us"] or 0.0) / chain_us,
-                         "fma_pipe_pct_of_dominant_kernel": 15.6,
+                         "recurrence_share_of_chain": 3 * 97 * (tr["t_step_us"] or 0.0) / chain_us,
                          "source": "chain_us = 1e6 / frames_per_s_unpipelined (untraced); t_step, kernels and the timeline from the device-side "
                                    "trace of one one-hop call (l2h_sep_trace_*; with tracing on every kernel exit also flushes its time stamps)",
                          "traced_span_us": tr["span_us"], "timeline_us": tr["timeline_us"]}
         roof = {"bound": "hbm", "kernel": dom[0], "achieved": ach, "peak": pk["hbm_gbs"], "unit": "GB/s",
-                "frac": ach / pk["hbm_gbs"],
-                # dram__bytes_read.sum + dram__bytes_write.sum per launch of this kernel, from the committed
-                # ncu --set full capture profiles/r01e_lstm_rec3_full.md (warm L2: the launch's 379 KB of
-                # algorithmic bytes are L2 hits; 0.9 KB read + 10.5 KB written reach DRAM)
-                "traffic": 11392.0 if dom[0] == "lstm_intra" else None, "peak_source": pk["source"],
+                "frac": ach / pk["hbm_gbs"], "peak_source": pk["source"],
                 "alg_bytes_per_launch": alg, "mean_us_per_launch": 1e3 * dom[1]["ms_mean"],
                 "share_of_chain": dom[1]["ms_total"] / sum(v["ms_total"] for v in prof.values()),
-                # fma_pipe_pct from the ncu capture profiles/r01e_lstm_rec3_full.md
-                # the model that governs batch 1: the chain cannot be shorter than its 3 x 97 dependent recurrent steps.
-                # t_step_floor = 0.23 us: the FMA + shuffle + barrier floor of one 256x64 step on one SM
-                # (profiles/r01c_lstm_microbench.txt); chain_us / t_step_measured from the device-side trace of one hop
+                # the model that governs batch 1: the chain cannot be shorter than its 3 x 97 dependent recurrent steps;
+                # chain_us / t_step_measured from the device-side trace of one hop
                 "latency_model": latency_model,
-                "note": "batch-1 streaming is latency-bound (serial LSTM chain, 13 MB working set resident in L2); "
+                "note": "batch-1 streaming is latency-bound (serial LSTM chain, 13 MB working set resident in the 50 MB L2); "
                         "whole-chain algorithmic rate: %.1f GB/s, %.2f TFLOP/s fp32" % (
                             value / world * BYTES_PER_FRAME / 1e9, value / world * FLOP_PER_FRAME / 1e12)}
         extras["kernel_us"] = {k: round(1e3 * v["ms_mean"], 2) for k, v in prof.items()}
         if world == 1 and not args.no_extras:
             allc = os.cpu_count() or 1
-            # chunk-by-chunk streaming on CPU is dispatch-bound: more threads are slower (0.14 frames/s on 128
-            # threads vs 190 on one, measured); probe 1 thread vs min(all, 8) briefly and keep the faster
+            # chunk-by-chunk streaming on CPU is dispatch-bound: more threads can be slower; probe 1 thread vs
+            # min(all, 8) briefly and keep the faster
             probe = {t: time_cpu_streaming(4, cpc, 1, t)[0] for t in sorted({1, min(allc, 8)})}
             threads = max(probe, key=probe.get)
             fps, kind, _ = time_cpu_streaming(125, cpc, 2, threads)

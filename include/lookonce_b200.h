@@ -1,8 +1,8 @@
-/* lookonce_b200.h -- C ABI of the B200-native LookOnceToHear inference engine.
+/* lookonce_b200.h -- C ABI of the LookOnceToHear inference engine for the H100 (sm_90a).
  *
  * Drop-in boundary for ONE path of vb000/LookOnceToHear: the inference forward of its two
  * networks.  The reference is pure Python; the interface each entry point stands in for is the
- * Python method the reference's evaluation path calls (all paths relative to /root/reference):
+ * Python method the reference's evaluation path calls (all paths relative to the reference repository):
  *
  *   l2h_sep_create / l2h_sep_load_weight / l2h_sep_commit_weights
  *        <- Net.__init__ + load_state_dict      src/models/tfgridnet_realtime/net.py:20-49,
@@ -140,7 +140,7 @@ int l2h_sep_pipeline_frames(void* handle, int32_t* frames);
  * the BiLSTM and the 16-CTA tail_kernel; default 1), "back_many" (calls of several frames / many streams through the persistent
  * front_many / back_many kernels; default 1), "pipeline_split_mid" (mid section as mid_a | mid_b | mid_c in the graph),
  * "mid_split_large" (the same three kernels for many streams), "fold_mid_c" (default 0: no mid_c -- the inter Linear moves into
- * the serial kernel, the Q/K/V projection into qkv_kernel; changes rounding, not the maths; measured slower, tested),
+ * the serial kernel, the Q/K/V projection into qkv_kernel; changes rounding, not the maths; it lengthens the serial stage of the pipeline; tested),
  * "tensor_cores" (default 1), "fuse_ih" (default 0), "graph_stats".  Values: "bf16" (0 = bf16x3 split products, 1 = bf16 weights x
  * split activations, 2 = plain bf16), "tc_lstm_min" (sequence-directions from which the recurrence runs on the tensor cores,
  * default 4096), "tc_pdl" (bit mask, default 7: programmatic launches around the tensor-core GEMMs of many-row chains),

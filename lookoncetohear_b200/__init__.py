@@ -1,11 +1,11 @@
-"""lookoncetohear_b200 -- B200-native inference engine for the two networks of
+"""lookoncetohear_b200 -- H100 (sm_90a) inference engine for the two networks of
 vb000/LookOnceToHear (speaker-conditioned streaming TF-GridNet separator + enrollment embedding
 net), behind the reference's own Python call signatures.
 
     from lookoncetohear_b200 import Net            # drop-in for src.models.tfgridnet_realtime.net.Net
     from lookoncetohear_b200 import EmbedTFGridNet # drop-in for src.models.tfgridnet_orig.tfgridnet.EmbedTFGridNet
 
-Compute happens only in lib/liblookonce_b200.so (hand-written sm_100a CUDA, C ABI declared in
+Compute happens only in lib/liblookonce_b200.so (hand-written sm_90a CUDA, C ABI declared in
 include/lookonce_b200.h); importing this package never falls back to PyTorch math.
 """
 from .embed import EmbedTFGridNet  # noqa: F401

@@ -1,4 +1,4 @@
-// Shared device helpers for the lookonce-b200 engine (sm_100a only).
+// Shared device helpers for the lookonce engine (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -7,27 +7,12 @@ namespace l2h {
 
 #define L2H_DEVINL __device__ __forceinline__
 
-// ---- d.xy = a.xy * b.xy + c.xy ------------------------------------------------------------------------------------
-// L2H_FFMA2 = 1: the packed fma.rn.f32x2 (SASS FFMA2); 0: two scalar fma.rn.f32 (SASS FFMA) -- the same two roundings, bit-identical.
-// tools/ffma_microbench.cu on a B200 SM: FFMA 1.0 cycle per warp-instruction and scheduler with one operand shared between
-// neighbouring instructions (127 FMA/clk/SM), 1.2-2.3 with three distinct registers; FFMA2 2.35 (109 FMA/clk/SM) resp. 3.15 (81).  The
-// packed form is no faster per FMA -- it halves the instruction count, which is what the latency-shaped kernels here are short of:
-// built with scalar FFMAs the one-hop chain is 1 % faster, the many-sequence recurrences 7-9 % and the pipelined clip 5 % slower.
-#ifndef L2H_FFMA2
-#define L2H_FFMA2 1
-#endif
+// SMs of an H100 SXM: the grid size of the persistent and work-splitting kernels (a smaller part only queues a wave)
+constexpr int NUM_SMS = 132;
+
+// ---- d.xy = a.xy * b.xy + c.xy: two fp32 FMAs (Hopper has no packed fp32 FMA; the kernels keep their pairwise form) ----
 L2H_DEVINL float2 ffma2(float2 a, float2 b, float2 c) {
-#if L2H_FFMA2
-    unsigned long long d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;"
-        : "=l"(d)
-        : "l"(*reinterpret_cast<unsigned long long*>(&a)),
-          "l"(*reinterpret_cast<unsigned long long*>(&b)),
-          "l"(*reinterpret_cast<unsigned long long*>(&c)));
-    return *reinterpret_cast<float2*>(&d);
-#else
     return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
-#endif
 }
 
 L2H_DEVINL float warp_sum(float v) {
@@ -92,9 +77,8 @@ L2H_DEVINL void tma_load_1d(void* dst_smem, const void* src_gmem, unsigned bytes
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
-// Stage a contiguous block with ONE bulk copy issued by thread 0.  Measured on B200 for a single CTA
-// and an L2-resident source (profiles/r01c_copy_microbench.txt): 150 KB in 0.88 us (170 GB/s) with one
-// cp.async.bulk, vs 1.26 us as 74 x 2 KB bulk copies and 2.35 us as an LDG.128 -> STS.128 loop.
+// Stage a contiguous block with ONE bulk copy issued by thread 0 (fewer instructions and barrier arrivals than a
+// loop of smaller bulk copies or an LDG.128 -> STS.128 loop).
 // Called by all threads (uniform call sites); the caller arms the barrier with the byte total.
 L2H_DEVINL void tma_load_split(void* dst_smem, const void* src_gmem, unsigned bytes, unsigned long long* bar,
                                int tid, int /*nthreads*/) {
@@ -188,6 +172,23 @@ struct TraceScope {
         if (rec != nullptr) marks()[point] = globaltimer_ns();
     }
 };
+
+// How many CTAs of `kernel` (with `threads` threads and `smem` bytes of dynamic shared memory) the CURRENT device holds
+// at once: occupancy per SM x SM count, cached per device in `cache` (one array per call site, 0 = not asked yet).  The
+// one-wave limit of the persistent and work-splitting launches: a persistent grid larger than this runs a second wave.
+template <typename... KArgs>
+inline int resident_ctas(int (&cache)[64], void (*kernel)(KArgs...), int threads, size_t smem) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) { cudaGetLastError(); return NUM_SMS; }
+    if (cache[dev] == 0) {
+        int sms = 0, per = 0;
+        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = NUM_SMS;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, kernel, threads, smem) != cudaSuccess || per <= 0) per = 1;
+        cudaGetLastError();
+        cache[dev] = per * sms;
+    }
+    return cache[dev];
+}
 
 // every kernel launch the engines issue goes through launch_k / launch_cluster / umma::launch: this counter makes the
 // "kernels launched" figure of the C ABI exact for directly launched chains (graph replays count their kernel nodes)

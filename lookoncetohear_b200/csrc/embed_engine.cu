@@ -1,5 +1,5 @@
 // Enrollment engine: weight packing, the kernel chain and the C ABI (include/lookonce_b200.h).
-// Reference path: EmbedTFGridNet.forward, /root/reference/src/models/tfgridnet_orig/tfgridnet.py:100-127
+// Reference path: EmbedTFGridNet.forward, reference src/models/tfgridnet_orig/tfgridnet.py:100-127
 // (trunk = espnet2 TF-GridNet block, SURVEY.md Appendix B).
 #include <cuda_runtime.h>
 
@@ -418,7 +418,7 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
             g.C = O; g.ldc = VDIM; g.c_seq_stride = (int64_t)Tp * VDIM;
             CKU(umma::launch(g, st, &_why));
         }
-        eattn_out_kernel<<<dim3((unsigned)std::min<int64_t>((int64_t)T * B, 148 * 4)), 256, EAOUT_SMEM, st>>>(O, X, W, T, Tp, T * B);
+        eattn_out_kernel<<<dim3((unsigned)std::min<int64_t>((int64_t)T * B, NUM_SMS * 4)), 256, EAOUT_SMEM, st>>>(O, X, W, T, Tp, T * B);
         CK(cudaGetLastError());
     }
     // ---- head: Linear(4160 -> 256) over rows (b,t) [features f*64+c], LN, mean over T -----------

@@ -1,5 +1,5 @@
 // On-GPU evaluation epilogue (SURVEY.md section 8 f-2): the three per-mixture figures the reference's evaluation
-// driver computes on the CPU after `outputs.cpu()` -- /root/reference/src/ts_hear_test.py:139-146 --
+// driver computes on the CPU after `outputs.cpu()` -- reference src/ts_hear_test.py:139-146 --
 //   output_sisnr  = mean over ears of SI-SNR(estimate, target)
 //   si_snr_i      = mean over ears of SI-SNR(estimate, target) - SI-SNR(mixture, target)
 //   embedding_sim = cosine_similarity(embedding, embedding_gt)

@@ -1,5 +1,5 @@
 // rows_gemm: C[m, n] = epi( sum_k A(m)[k] * Wt[k][n] + bias[n] ),  fp32 on the CUDA cores with
-// packed FFMA2.  "Rows" are (stream, frame, freq-bin) activations: M is huge or tiny, K and N are
+// paired fp32 FMAs.  "Rows" are (stream, frame, freq-bin) activations: M is huge or tiny, K and N are
 // small (64..512), so W^T lives in shared memory and A streams through once.
 //
 // A rows may be overlapping windows of a [seq][pos][lda] tensor (the enrollment net's unfold /
@@ -186,7 +186,7 @@ rows_gemm_kernel(const GemmArgs g) {
 // ------------------------------------------------------------------------------------------------
 // Large-M variant.  Persistent CTAs keep the whole k-major weight slab W^T[K][BN] resident in shared
 // memory and stream 128-row tiles of A through it in 64-deep k chunks; each thread owns an 8 x TN
-// register tile (TN = BN/16), fed by 2 + TN/4 LDS.128 per k for 8*TN/2 FFMA2 -- twice the FMAs per
+// register tile (TN = BN/16), fed by 2 + TN/4 LDS.128 per k for 8*TN/2 FMA pairs -- twice the FMAs per
 // shared-memory instruction of the small-tile kernel and no weight re-loads per row tile.
 // Same GemmArgs contract (windowed A rows, LN prologue for K == 64, bias / PReLU / residual epilogues).
 template <int BN>
@@ -324,11 +324,11 @@ inline cudaError_t launch_rows_gemm_big(const GemmArgs& g, cudaStream_t st, bool
     const int col_tiles = g.N / BN;
     // resident CTAs per SM: the 128-column variant holds 105 registers x 256 threads -> two; the 64-column variant
     // three (as far as shared memory allows).  The grid must not exceed what is resident (a second wave of a
-    // persistent kernel doubles its time: ncu, profiles/r01f_ncu_batch256.md), and the row tiles are dealt out
+    // persistent kernel doubles its time), and the row tiles are dealt out
     // evenly: every CTA takes ceil(tiles / gx_max) of them.
     const int by_smem = (smem <= 72 * 1024) ? 3 : (smem <= 110 * 1024 ? 2 : 1);
     const int per_sm = std::min(by_smem, BN == 128 ? 2 : 3);
-    int gx = std::max(1, (148 * per_sm) / col_tiles);
+    int gx = std::max(1, (NUM_SMS * per_sm) / col_tiles);
     if (gx > n_row_tiles) gx = n_row_tiles;
     const int per_cta = (n_row_tiles + gx - 1) / gx;
     gx = (n_row_tiles + per_cta - 1) / per_cta;

@@ -14,7 +14,7 @@
 //             GX = LN(x) W_ih^T + b, with W_ih (128 KB) brought by TMA into the shared memory the mid weights occupied (:505-512)
 //
 // Replaces mid_kernel + qkv_kernel + attn_cluster_kernel + attn_out_kernel + the next rows_gemm launch: 5 launches and
-// 4 global round trips become one launch with 5 cluster barriers (~0.2 us each, tools/cluster16_probe.cu).
+// 4 global round trips become one launch with 5 cluster barriers (tools/cluster16_probe.cu times one).
 // The 16-CTA cluster is a non-portable size: the engine asks cudaOccupancyMaxActiveClusters first and keeps the separate
 // kernels when it cannot be scheduled.
 #pragma once
@@ -47,7 +47,7 @@ __device__ __forceinline__ int tail_rows(int p) { return min(MID_RT, NF - p * MI
 // Input projection of an intra BiLSTM for one tile of MID_RT rows: GX[r][0..511] = LN(x[r]) W_ih^T + b.
 // xrows: the tile's rows [8][64] in shared memory (all 8 rows defined); xn: [64][8] scratch; wih: W_ih^T [64][512] in shared
 // memory (its TMA has completed); (g0, g1, b0, b1): LayerNorm gamma / beta of channels lane, lane + 32; bias: b[2 tid .. +1].
-// Thread t owns gate columns 2t, 2t+1 for all 8 rows (row pairs packed for FFMA2).  Ends without a barrier.
+// Thread t owns gate columns 2t, 2t+1 for all 8 rows (row pairs as float2 FMA pairs).  Ends without a barrier.
 __device__ __forceinline__ void ih_rows_tile(const float* xrows, float* xn, const float* wih, float g0, float g1, float b0, float b1,
                                              float2 bias, float* gx_rows, int nr, int tid) {
     const int warp = tid >> 5, lane = tid & 31;
@@ -483,7 +483,7 @@ tail_kernel(const float* __restrict__ Y, float* X, float* __restrict__ state, in
 
 // ------------------------------------------------------------------------------------------------------------------
 // front1_kernel: the head of a one-hop call on the latency path.  front_kernel runs a frame in ONE CTA (150 KB of analysis
-// filters for 194 dot products, then a 3x3 conv that one CTA needs 6 us for: profiles/r02k_hop_trace.md) and is followed by
+// filters for 194 dot products, then a 3x3 conv, all on one SM) and is followed by
 // the W_ih GEMM launch of block 0.  Here the frame is 13 row tiles of 8 bins like tail_kernel's: CTA p computes the
 // spectrum only for the bins its conv rows touch (f0-1 .. f0+8: 20 filter rows instead of 194), the conv for its rows, and
 // block 0's input projection GX = LN(x) W_ih^T + b for them (W_ih arrives by TMA meanwhile).  One more CTA (blockIdx.x == 13)

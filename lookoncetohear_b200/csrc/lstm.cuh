@@ -5,7 +5,7 @@
 // column tid).  What is left is, per step, a 256x64 mat-vec with W_hh, the cell update and
 // one barrier -- a latency chain.  One CTA (128 threads: hidden unit x k-half) runs NSEQ independent
 // sequences in lock-step with its W_hh slice in registers and h broadcast through shared memory; the
-// FMAs are packed FFMA2 along k.  lstm_rec3_kernel: few sequences (latency), lstm_rec4_kernel: many
+// FMAs are paired (float2) along k.  lstm_rec3_kernel: few sequences (latency), lstm_rec4_kernel: many
 // sequences, the step written stage by stage across the CTA's sequences (throughput).
 //
 // Row addressing (rows of gx / out are activation rows of the [B,T,F,C] tensors):
@@ -199,8 +199,8 @@ lstm_rec3_kernel(const LstmArgs a) {
 }
 
 // ---- variant 4: variant 3's thread layout, throughput mode --------------------------------------
-// With many sequences per CTA, variant 3 measured ~410 ns per (sequence, step) however many sequences the
-// CTA holds (profiles/r01e_kernel_us_batch256.jsonl: 855 ns/step at NSEQ = 2): 214-226 registers leave the
+// With many sequences per CTA, variant 3's time per (sequence, step) does not fall with the number of sequences
+// the CTA holds: 214-226 registers leave the
 // scheduler no room to overlap the sequences' dependent chains.  Here the step is written stage by stage
 // ACROSS the CTA's sequences (all dot products, then all reductions, then all activations) with one
 // accumulator pair per gate, so NSEQ independent chains are in flight at every stage.
@@ -277,7 +277,7 @@ lstm_rec4_kernel(const LstmArgs a) {
     int cur = 0;
     for (int it = 0; it < a.L; ++it) {
         if ((it & 3) == 0) issue_group((it >> 2) + 1);              // overwrites the group consumed 4 steps ago
-        // stage A: all dot products (4 NSEQ independent FFMA2 chains)
+        // stage A: all dot products (4 NSEQ independent FMA-pair chains)
         float2 acc[NSEQ][4];
         float2 g2[NSEQ];
 #pragma unroll
@@ -377,12 +377,16 @@ inline cudaError_t configure_lstm() {
 inline cudaError_t launch_lstm_rec(const LstmArgs& a, cudaStream_t st, bool pdl = false) {
     if (a.nseq <= 0 || a.L <= 0) return cudaErrorInvalidValue;
     const int ctas1 = a.nseq * a.ndir;
-    if (ctas1 <= 148 && (size_t)a.L * 1024 <= 200 * 1024)      // latency mode: one sequence per CTA, preloaded
+    if (ctas1 <= NUM_SMS && (size_t)a.L * 1024 <= 200 * 1024)      // latency mode: one sequence per CTA, preloaded
         return launch_k(pdl, lstm_rec3_kernel<1, true>, dim3(a.nseq, a.ndir), dim3(128), (size_t)a.L * 1024, st, a);
-    // many sequences: NSEQ per CTA in lock-step (stage by stage), at most 4.  (Six per CTA, to fit 1 552 sequences in ONE wave of
-    // 259 CTAs instead of 388 CTAs in two, was measured: 6.9 us per step against 2 x 2.7 -- slower, 226 registers; not kept.)
+    // many sequences: NSEQ per CTA in lock-step (stage by stage), at most 4: more sequences per CTA only while one sequence
+    // per CTA (resp. two) would not fit the device in one wave.  (Six per CTA would need 226 registers; not kept.)
+    static int wave1[64] = {}, wave2[64] = {};
     int per = 1;
-    while (per < 4 && ((a.nseq + per - 1) / per) * a.ndir > 296) per *= 2;
+    if ((int64_t)a.nseq * a.ndir > resident_ctas(wave1, lstm_rec3_kernel<1, false>, 128, 0)) {
+        per = 2;
+        if ((int64_t)((a.nseq + 1) / 2) * a.ndir > resident_ctas(wave2, lstm_rec4_kernel<2>, 128, lstm_rec4_smem(2))) per = 4;
+    }
     dim3 grid((a.nseq + per - 1) / per, a.ndir);
     if (per == 2) return launch_k(pdl, lstm_rec4_kernel<2>, grid, dim3(128), lstm_rec4_smem(2), st, a);   // many sequences: stage by stage
     if (per == 4) return launch_k(pdl, lstm_rec4_kernel<4>, grid, dim3(128), lstm_rec4_smem(4), st, a);

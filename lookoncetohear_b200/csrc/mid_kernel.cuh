@@ -11,10 +11,9 @@
 // loading the weights ONCE and looping over (stream, row-tile) items.
 //
 // Tiling (v2).  With only 8 rows per tile the activations are the broadcast operand, and a broadcast
-// LDS costs one shared-memory wavefront per 4 B per lane whatever its width (profiles/r01c_lstm_microbench.txt),
+// LDS costs one shared-memory wavefront per 4 B per lane whatever its width,
 // so a warp computing R rows x C columns per lane gets 32 R C / (R + C) FMAs per wavefront: v1 (C = 1,
-// R = 2 or 8) was bound by the shared-memory pipe at 12 k wavefronts and 9.7 us per tile (ncu,
-// profiles/r01f_ncu_batch256.md).  v2 splits K across KQ adjacent lanes instead of giving every lane its own
+// R = 2 or 8) was bound by the shared-memory pipe.  v2 splits K across KQ adjacent lanes instead of giving every lane its own
 // column: a lane accumulates 8 rows x C = 4 or 8 columns over K/KQ values of k, the KQ partial tiles are
 // summed by a shuffle reduce-scatter, and every lane ends up owning 8 C / KQ finished outputs for the
 // epilogue.  Weights and activations are stored in k-slices padded by 4 floats so that the 8 lanes of a
@@ -507,7 +506,7 @@ mid_c_kernel(const float* __restrict__ Hn, float* __restrict__ X, float* __restr
 }
 
 // The fused kernel without phase 6 (engine option "fold_mid_c": qkv_kernel projects Q/K/V itself, and the pipelined graph has
-// no mid_c).  Same text as mid_kernel up to X2.  Off by default: measured slower in the pipeline (profiles/r02e_fold_mid_c_pipeline.jsonl);
+// no mid_c).  Same text as mid_kernel up to X2.  Off by default: it lengthens the serial stage of the pipeline;
 // covered by tests/test_sep_gpu.py::test_fold_mid_c_option.
 __global__ void __launch_bounds__(256)
 mid_noproj_kernel(const float* __restrict__ Y, float* __restrict__ X, float* __restrict__ QKV, float* __restrict__ state,
@@ -622,7 +621,7 @@ mid_noproj_kernel(const float* __restrict__ Y, float* __restrict__ X, float* __r
 
 // mid_b + the inter Linear (engine option "fold_mid_c", with qkv_kernel doing its own Q/K/V projection): the serial stage also
 // finishes X2 = X1 + h' W_l2 + b, so that no mid_c launch (and no graph edge for it) is left between it and qkv.
-// Off by default (8.64 vs 7.27 us per hop, profiles/r02e_fold_mid_c_pipeline.jsonl); covered by tests/test_sep_gpu.py::test_fold_mid_c_option.
+// Off by default (it lengthens the serial stage of the pipeline); covered by tests/test_sep_gpu.py::test_fold_mid_c_option.
 constexpr size_t MID_B2_SMEM = (size_t)((MID_W5 - MID_W3B) + MID_A3 + (MID_W6 - MID_W5) + MID_A5) * sizeof(float);
 __global__ void __launch_bounds__(256)
 mid_b2_kernel(const float* __restrict__ GI, float* __restrict__ X, int64_t hop_stride, int n_hops, float* __restrict__ state,

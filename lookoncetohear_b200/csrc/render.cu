@@ -1,9 +1,9 @@
 // GPU binaural renderer (SURVEY.md section 8 f-3): the data-side arithmetic that feeds the two networks, so that
 // synthetic evaluation inputs can be produced at the rate the engine consumes them.
 //   * per event and ear: causal FIR with the head-related / room impulse response, truncated to the source length --
-//     SOFASimulator._convolve, /root/reference/src/datasets/multi_ch_simulator.py:56-58
+//     SOFASimulator._convolve, reference src/datasets/multi_ch_simulator.py:56-58
 //     (`convolve(src, rir[0])[:len(src)]`, `convolve(src, rir[1])[:len(src)]`);
-//   * mixture assembly -- /root/reference/src/datasets/MixLibriSpeechNoisyEnrollNorm.py:179-202: noise scaled by
+//   * mixture assembly -- reference src/datasets/MixLibriSpeechNoisyEnrollNorm.py:179-202: noise scaled by
 //     `noise_scale`, `norm_factor = |sum(events) + noise|.max()`; if it exceeds 1 every event and the noise are
 //     divided by it; `mixture = sum(events) + noise`.
 // Direct-form convolution in fp32 on the CUDA cores (HRIRs are a few hundred taps, BRIRs a few thousand: 2 n_src N L
@@ -13,6 +13,7 @@
 #include <string>
 
 #include "../../include/lookonce_b200.h"
+#include "common.cuh"
 
 namespace l2h {
 int fail(int code, const std::string& msg);
@@ -116,7 +117,7 @@ extern "C" int l2h_render_binaural(const float* src_dev, const float* rir_dev, c
         fir_kernel<<<dim3((n_samples + FIR_TILE - 1) / FIR_TILE, 2 * n_src, batch), 256, 0, st>>>(src_dev, rir_dev, events_dev, n_src, n_samples, rir_len);
         e = cudaGetLastError();
     }
-    const int gx = (int)((2ll * n_samples + 255) / 256 < 148 ? (2ll * n_samples + 255) / 256 : 148);
+    const int gx = (int)((2ll * n_samples + 255) / 256 < NUM_SMS ? (2ll * n_samples + 255) / 256 : NUM_SMS);
     if (e == cudaSuccess) {
         mix_peak_kernel<<<dim3(gx, batch), 256, 0, st>>>(events_dev, noise_dev, noise_scale_dev, n_src, n_samples, peak);
         e = cudaGetLastError();

@@ -47,9 +47,9 @@ struct Slot {
     std::vector<float> raw;    // accumulate slots keep their tensor; the sum is formed at commit
 };
 
-// (sequence, direction) pairs from which the recurrence runs on the tensor cores (tc_lstm: 32 sequences per CTA, 9 472 per wave of
-// 296 CTAs at 16.8 us per step; CUDA cores: 4 per CTA, 1 184 per wave at 2.7 us).  Measured at the offline shape
-// (tools/offline_split_experiment.py): 3 492 inter sequences are faster as three CUDA-core waves than as 110 tensor-core CTAs.
+// (sequence, direction) pairs from which the recurrence runs on the tensor cores (tc_lstm: 32 sequences per CTA; CUDA cores:
+// up to 4 per CTA).  The threshold was chosen with an earlier tensor-core recurrence on another GPU and has not been
+// re-measured for the wgmma kernel on the H100; tools/offline_split_experiment.py measures the split (option "tc_lstm_min").
 constexpr int TCL_MIN_SEQDIRS = 4096;
 
 struct SepEngine {
@@ -68,9 +68,8 @@ struct SepEngine {
     __nv_bfloat16* planes = nullptr;
     int64_t planes_total = 0;
     bool cur_pdl = false;               // PDL attribute for the tensor-core launches of the chain being enqueued
-    bool fuse_ih = false;               // many sequences: W_ih + LayerNorm inside the tensor-core recurrence (option "fuse_ih").  Off:
-                                        // measured slower than GEMM + tc_lstm (offline B=16: 5.48 vs 4.50 ms per chain, profiles/r02i)
-    bool use_tc = true;                 // rows > TC_MIN_ROWS: dense contractions on tcgen05 (option "tensor_cores")
+    bool fuse_ih = false;               // many sequences: W_ih + LayerNorm inside the tensor-core recurrence (option "fuse_ih", default off)
+    bool use_tc = true;                 // rows > TC_MIN_ROWS: dense contractions on the tensor cores, wgmma (option "tensor_cores")
     int tc_passes = 3;                  // 3 = bf16x3 split products (fp32 configs); 2 = bf16 weights x split activations (option
                                         // "bf16" = 1: the offline bf16 configuration); 1 = plain bf16 operands ("bf16" = 2)
     int64_t total = 0;
@@ -109,7 +108,7 @@ struct SepEngine {
     bool mid_split_large = true;  // many streams: run the fused mid section as mid_a | mid_b | mid_c (2-4 CTAs per SM)
     bool use_mid = true;     // fused row-local mid-section for one-frame calls (option "fused_mid")
     int tcl_min_seqdirs = TCL_MIN_SEQDIRS;  // (sequence, direction) pairs from which the recurrence runs on the tensor cores (option "tc_lstm_min")
-    int tc_pdl = 7;              // programmatic dependent launch around the tensor-core GEMMs of many-row calls: bit 0 the many-stream mid section, bit 1 W_ih and the out projection + its LayerNorm kernel, bit 2 the persistent qkv kernel (256 streams: 0.847 -> 0.828 ms per hop-step; PDL on EVERY kernel of that chain was slower: 0.939; option "tc_pdl")
+    int tc_pdl = 7;              // programmatic dependent launch around the tensor-core GEMMs of many-row calls: bit 0 the many-stream mid section, bit 1 W_ih and the out projection + its LayerNorm kernel, bit 2 the persistent qkv kernel (PDL on EVERY kernel of that chain parks early-launched dependents on the SMs the big kernels need; option "tc_pdl")
     bool use_back_many = true;   // calls of several frames: front_many_kernel / back_many_kernel (one CTA / cluster per chunk of frames) instead of one per frame (option "back_many")
     bool use_tail = true;    // one-hop calls of a few streams: mid + qkv + attention + attn_out (+ next W_ih) as ONE 16-CTA cluster kernel (option "fused_tail")
     bool use_pdl = true;     // programmatic dependent launch between the kernels of a chain (option "pdl")
@@ -297,8 +296,9 @@ struct Workspace {
 };
 // few frames in flight -> split every head's 50-row window over several CTAs
 static int attn_splits(int B, int T) {
+    static int wave[64] = {};
     const int ctas = B * T * NHEAD;
-    return (ctas * ATT_CL <= 296) ? ATT_CL : 1;      // 8-CTA clusters while they all fit in one wave
+    return (ctas * ATT_CL <= resident_ctas(wave, attn_cluster_kernel, 256, 0)) ? ATT_CL : 1;      // 8-CTA clusters while they all fit in one wave
 }
 
 static Workspace carve(int n_blocks, int B, int T, uint32_t flags) {
@@ -323,10 +323,10 @@ static Workspace carve(int n_blocks, int B, int T, uint32_t flags) {
 // grids of the mid-section kernels: persistent over (stream, row tile) items, as many CTAs per SM as their shared memory
 // allows (fused 225 KB -> 1, mid_a 107 KB -> 2, mid_b 68 KB -> 3, mid_c 50 KB -> 4)
 static inline int mid_items(int B) { return B * ((NF + MID_RT - 1) / MID_RT); }
-static inline dim3 mid_grid_for(int B, int ctas_per_sm) { return dim3(std::min(148 * ctas_per_sm, mid_items(B))); }
+static inline dim3 mid_grid_for(int B, int ctas_per_sm) { return dim3(std::min(NUM_SMS * ctas_per_sm, mid_items(B))); }
 // many streams: the section is throughput-bound and one fused CTA per SM (8 warps) cannot hide its own latencies; the
 // three smaller kernels run 2-4 CTAs per SM (same arithmetic, +3 small global round trips)
-static inline bool mid_split_for_throughput(int B) { return mid_items(B) > 148; }
+static inline bool mid_split_for_throughput(int B) { return mid_items(B) > NUM_SMS; }
 
 // cudaFuncSetAttribute applies to the CURRENT device: keep one flag per device ordinal
 static bool g_attr_done[64] = {};
@@ -474,8 +474,7 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
         return 0;
     };
     float* sbase = state + sizeof(StateHeader) / 4;
-    // programmatic dependent launch pays on the latency chain of a few rows; with many rows it is slower (256 streams: 0.939 vs
-    // 0.865 ms per hop-step, profiles/r02j_b256_options.jsonl): early-launched dependents park on the SMs the big kernels need
+    // programmatic dependent launch pays on the latency chain of a few rows; with many rows early-launched dependents park on the SMs the big kernels need
     const bool pdl = e->use_pdl && a.prof == nullptr && !(flags & L2H_FLAG_TAPS) && !(e->use_tc && rows > TC_MIN_ROWS);
     e->cur_pdl = false;
 #define MARK(name) do { if (a.prof) { if (int _rc = a.prof->mark(name, st)) return _rc; } } while (0)
@@ -484,10 +483,10 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
         CK(launch_k(false, front1_kernel, dim3(TAIL_TILES + 1, B), dim3(256), FRONT1_SMEM, st, x, xbs, xcs, x_len, X, state, ss, e->w,
                     e->bw[0], GX, a.pos_rel, emb, PRE));
     } else if ((T > 1 || tc) && e->use_back_many) {      // many frames / streams: one CTA walks (stream, chunk) items (one CTA per SM: 150 KB of filters)
-        const int per_stream = std::max(1, 148 / B);
+        const int per_stream = std::max(1, NUM_SMS / B);
         const int chunk = (T + per_stream - 1) / per_stream;
         const int n_chunks = (T + chunk - 1) / chunk;
-        const int n_workers = std::min(148, B * n_chunks);
+        const int n_workers = std::min(NUM_SMS, B * n_chunks);
         CK(launch_k(false, front_many_kernel, dim3(n_workers + B, 1), dim3(256), FRONT_SMEM, st, x, xbs, xcs, x_len, X, state, ss, e->w, T,
                     a.pos_rel, emb, PRE, chunk, n_chunks, B, n_workers));
     } else {
@@ -644,8 +643,10 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
         if (tc && !tc_mid) {      // Q|K|V projections of all rows as one tensor-core GEMM (+ bias + PReLU per column)
             if (int rc = tc_rows_gemm(e, b, PL_QKV, X, 64, 64, NQKV, nullptr, nullptr, W.bqkv, W.slope_vec, nullptr, QKVRAW, NQKV, rows, st)) return rc;
         }
-        if (tc && (int64_t)B * T >= 148) {      // many frames: persistent form (LayerNorm parameters staged once per CTA, two CTAs per SM)
-            CK(launch_k(pdl || ((e->tc_pdl & 4) != 0 && a.prof == nullptr), qkv_many_kernel, dim3((unsigned)std::min<int64_t>(296, (int64_t)B * T)), dim3(QKV_THREADS), QKV_MANY_SMEM, st, (const float*)QKVRAW, Q, KALL, VALL, state, ss,
+        if (tc && (int64_t)B * T >= NUM_SMS) {      // many frames: persistent form (LayerNorm parameters staged once per CTA), one wave
+            static int wave[64] = {};
+            const int64_t grid_q = std::min<int64_t>(resident_ctas(wave, qkv_many_kernel, QKV_THREADS, QKV_MANY_SMEM), (int64_t)B * T);
+            CK(launch_k(pdl || ((e->tc_pdl & 4) != 0 && a.prof == nullptr), qkv_many_kernel, dim3((unsigned)grid_q), dim3(QKV_THREADS), QKV_MANY_SMEM, st, (const float*)QKVRAW, Q, KALL, VALL, state, ss,
                         b, W, T, B * T));
         } else {
             CK(launch_k(pdl, qkv_kernel, dim3(T, B), dim3(QKV_THREADS), QKV_SMEM, st, (const float*)X,
@@ -655,7 +656,7 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
         if (nsplit > 1) {
             CK(launch_cluster(pdl, dim3(1, ATT_CL, 1), attn_cluster_kernel, dim3(T, NHEAD * ATT_CL, B), dim3(256), 0, st,
                               (const float*)Q, (const float*)KALL, (const float*)VALL, (const float*)state, ss, b, Z, T, 0));
-        } else if (T > 1 && (int64_t)B * NHEAD * ((T + ATT_TQ - 1) / ATT_TQ) >= 148) {   // enough tiles to fill the GPU: query-tiled,
+        } else if (T > 1 && (int64_t)B * NHEAD * ((T + ATT_TQ - 1) / ATT_TQ) >= NUM_SMS) {   // enough tiles to fill the GPU: query-tiled,
             // one pass over 57 rows serves 8 queries
             CK(launch_k(pdl, attn_tile_kernel, dim3((T + ATT_TQ - 1) / ATT_TQ, NHEAD, B), dim3(256), 0, st, (const float*)Q,
                         (const float*)KALL, (const float*)VALL, Z, T));
@@ -681,7 +682,7 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
     if ((T > 1 || tc) && e->use_back_many) {
         // many frames (or many streams): one cluster walks (stream, chunk-of-frames) items -- filters loaded once per cluster, rows
         // staged once; as many clusters as stay resident together (3 CTAs of 72 KB per SM)
-        const int max_cl = 148 * 3 / BACK_CL;
+        const int max_cl = NUM_SMS * 3 / BACK_CL;
         const int per_stream = std::max(1, max_cl / B);
         const int chunk = (T + per_stream - 1) / per_stream;
         const int n_chunks = (T + chunk - 1) / chunk;
@@ -706,7 +707,7 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
 //   B2b = attn_out                           needs Z_t, X_t only
 // A graph of K consecutive one-hop chains is captured on 1 + 3*(PIPE_LANES+3) + 1 streams with event edges
 // for exactly these dependencies; hops flow through the stages like a systolic wavefront and the
-// steady-state cost per hop is the slowest SERIAL stage instead of the whole 250 us chain.  Every hop owns a
+// steady-state cost per hop is the slowest SERIAL stage instead of the whole chain.  Every hop owns a
 // workspace slot; state addressing uses pos + frame_k / parity(ncalls + frame_k); the header advances once,
 // at the last hop of the graph.  The arithmetic and its order per stream are unchanged: results are
 // bit-identical to running the hops one after the other (tests/test_sep_gpu.py).
@@ -726,7 +727,7 @@ constexpr int PIPE_QKV_AHEAD = RING - ATT;         // qkv of hop t+3 overwrites 
 static_assert(PIPE_STREAMS <= 128, "pipe_streams[]");
 
 static int64_t pipe_slot_floats(SepEngine* e, int B) { return carve(e->n_blocks, B, 1, 0).total; }
-// hops per pipelined graph: fill + drain cost one chain latency (~0.25 ms) per graph, so as many as possible -- every hop
+// hops per pipelined graph: fill + drain cost one chain latency per graph, so as many as possible -- every hop
 // in flight owns a workspace slot (350 KB per stream), which is what bounds it for many streams
 static int pipe_frames_for(SepEngine* e, int B) {
     if (e->pipe_frames > 0) return e->pipe_frames;
@@ -752,7 +753,7 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
     // programmatic dependent launch, per stage: the kernel's prologue (weight staging) overlaps its stream predecessor's
     // tail; every kernel reaches griddepcontrol.wait before it touches activations or state.  Worth it only on the
     // serial stage (mid_b -> mid_b of the next hop): everywhere, the parked dependents hold shared memory and CTA
-    // slots the running kernels need (measured 14.0 vs 9.4 us per hop, profiles/r01f_pipeline_sweeps.jsonl)
+    // slots the running kernels need
     const int ppdl = e->pipe_pdl;         // stage bit mask (same bits as pipe_skip)
     const bool fold = e->fold_mid_c;
     const bool many = mid_split_for_throughput(B);
@@ -804,7 +805,7 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
     };
     for (int i = 1; i < PIPE_STREAMS; ++i)                             // fork: bring the worker streams into the capture
         if (int rc = edge(origin, e->pipe_streams[i])) return rc;
-    // The serial stage (mid_b) takes `mb` consecutive hops per launch: its ~3 us of launch overhead and its 64 KB of
+    // The serial stage (mid_b) takes `mb` consecutive hops per launch: its launch overhead and its 64 KB of
     // weights are paid once per batch, h stays in shared memory and c in registers from hop to hop.  A batch waits
     // for stage A of all its hops; the upstream block is that far ahead anyway once the pipeline is full.
     const int mb = (split_mid && !many) ? std::max(1, std::min(e->pipe_midb_hops, PIPE_MIDB_MAX)) : 1;

@@ -1,5 +1,5 @@
 // Separation-network kernels that are not plain row-GEMMs / LSTM recurrences.
-// Reference: /root/reference/src/models/tfgridnet_realtime/tfgridnet_causal.py (cited per kernel).
+// Reference: reference src/models/tfgridnet_realtime/tfgridnet_causal.py (cited per kernel).
 // Activations are [B, T, F=97, C=64] fp32 rows of 256 B.
 #pragma once
 #include <cooperative_groups.h>
@@ -168,8 +168,8 @@ front_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride, 
 #pragma unroll
         for (int k = 0; k < 36; ++k) wr[k] = __ldg(w.wc + o * 36 + k);
         const float bias = __ldg(w.bc + o);
-        // four rows at a time: four independent 36-long FMA chains per thread instead of one (the single chain made the conv
-        // 6 us of a frame's 11: profiles/r02k_one_hop_latency_path.md); per output the same order of additions as before
+        // four rows at a time: four independent 36-long FMA chains per thread instead of one (a single chain makes the
+        // conv the longest part of the frame); per output the same order of additions as before
         for (int f = fg; f < NF; f += 16) {
             float acc[4] = {bias, bias, bias, bias};
 #pragma unroll
@@ -547,8 +547,8 @@ qkv_kernel(const float* __restrict__ X, const float* __restrict__ pre, float* __
 // K4a for MANY frames (offline batches, many streams) when the projections come from a tensor-core GEMM: the same
 // LayerNorm + head split + ring append as qkv_kernel, but persistent -- each CTA stages the LayerNorm parameters ONCE
 // (22 KB) and walks frames fi = blockIdx.x, + gridDim.x, ... with the 43 KB projection tile of the next frame in flight
-// (two TMA-filled buffers) while the 12 warps normalise the current one.  qkv_kernel's one-CTA-per-frame form costs
-// ~18 us per frame in staging latency (profiles/r02h); this form is bound by the 86 KB each frame moves.
+// (two TMA-filled buffers) while the 12 warps normalise the current one.  qkv_kernel's one-CTA-per-frame form pays
+// the staging latency per frame; this form is bound by the 86 KB each frame moves.
 constexpr size_t QKV_MANY_SMEM = (size_t)(2 * NF * QKV_PLD + QKV_LNP) * sizeof(float);
 
 __global__ void __launch_bounds__(QKV_THREADS)
@@ -1076,7 +1076,7 @@ attn_out_kernel(const float* __restrict__ Z, float* __restrict__ X, const float*
 // -- it stages those rows (+ halo) of the four frames it needs by TMA, runs the deconv for them, and sums
 // the synthesis filterbank over ITS rows only (its 2 x ~24 filter rows, 37 KB, prefetched by TMA before the
 // dependency wait).  The four partial windows meet in CTA 0 through distributed shared memory, in a fixed
-// order, and CTA 0 does the overlap-add and the store.  (v1 ran the frame in one CTA: 28 us per hop, the
+// order, and CTA 0 does the overlap-add and the store.  (v1 ran the frame in one CTA, which made it the
 // slowest stage of the one-hop pipeline once the mid section was split.)
 // The last CTA to finish advances the state header (pos += T, ncalls += 1).
 constexpr int BACK_CL = 4;
@@ -1265,8 +1265,8 @@ back_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_bstrid
 // same order (results are bit-identical), but one cluster walks a contiguous CHUNK of frames of a stream: its synthesis
 // filter slices (37 KB per CTA) are loaded once instead of once per frame, every frame's rows are staged once (4-slot ring,
 // the next frame's TMA in flight under the current frame's work) instead of four times, and the deconvolved spectrum of
-// frame t-1 is carried in shared memory instead of being recomputed -- back_kernel's one-cluster-per-frame form was 12 % of
-// the offline step (8 000 clusters of 4 CTAs per 16 x 500 frames, profiles/r02d_kernel_us_by_call_size.jsonl).
+// frame t-1 is carried in shared memory instead of being recomputed -- back_kernel's one-cluster-per-frame form launches
+// 8 000 clusters of 4 CTAs per 16 x 500 frames.
 // grid (BACK_CL * n_chunks, B) in clusters of BACK_CL, 256 threads; frames [c*chunk, min(T, (c+1)*chunk)) for cluster c.
 constexpr size_t BACK_MANY_SMEM = (size_t)(4 * (BACK_FMAX + 2) * 64 + 2 * BACK_FMAX * NFFT + 2 * NSRC * NROW + 2 * NSRC * NFFT) * sizeof(float);
 

@@ -21,8 +21,8 @@ constexpr int VD = 16;         // D / heads
 constexpr int ATT = 50;        // local_atten_len
 constexpr int RING = 56;       // K/V ring slots per head: the 50-frame window + 6 spare, so that the ring writes of
                                // hops t+1 .. t+6 never touch a row hop t's attention still reads (pipelined streaming;
-                               // with 2 spare rows the qkv -> attention -> qkv(t+3) cycle, 21 us per 3 hops, bound the
-                               // pipeline: profiles/r01f_pipeline_trace.md)
+                               // with 2 spare rows the qkv -> attention -> qkv(t+3) cycle bounds the
+                               // pipeline)
 constexpr int SPK = 256;
 constexpr int QK_DIM = NF * QE;     // 582
 constexpr int QK_LD = 584;          // padded to a multiple of 4 floats (16 B rows)

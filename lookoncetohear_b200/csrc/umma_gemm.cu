@@ -1,4 +1,4 @@
-// umma_gemm.cu: the tcgen05 GEMM kernel (umma_gemm.cuh) and its host side -- tensor maps (cuTensorMapEncodeTiled
+// umma_gemm.cu: the wgmma GEMM kernel (umma_gemm.cuh) and its host side -- tensor maps (cuTensorMapEncodeTiled
 // through the runtime's driver entry point, so the library does not link libcuda), shared-memory plan, launch.
 #include "umma_host.cuh"
 #include "umma_kernel.cuh"
@@ -41,15 +41,12 @@ inline cudaError_t make_tmap4(CUtensorMap* m, CUtensorMapDataType dt, int elem_b
     return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
 }
 
-// column tile: at most 256, a multiple of 16, N split into equal tiles
-inline int pick_bn(int N, int max_bn = 256) {
-    const int nt = (N + max_bn - 1) / max_bn;
-    const int bn = ((N + nt - 1) / nt + 15) & ~15;
-    return std::min(max_bn, std::max(16, bn));
-}
+// column tile: 64 for N <= 64, else 128 (the wgmma shapes the kernel is built for; the accumulators of a 64 x 128 tile
+// are 64 registers per thread).  Columns beyond N are zero-filled by TMA and never stored.
+inline int pick_bn(int N) { return N <= 64 ? 64 : 128; }
 
 constexpr size_t SMEM_LIMIT = 227 * 1024 - 2048;      // dynamic shared memory budget (static barriers etc. come on top)
-constexpr size_t EPI_BYTES = 4 * 4096;                // epilogue transpose buffers
+constexpr size_t EPI_BYTES = 8 * 2048;                // epilogue transpose buffers
 
 cudaError_t configure() {
     static thread_local int done_dev = -1;
@@ -57,7 +54,8 @@ cudaError_t configure() {
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return e;
     if (done_dev == dev) return cudaSuccess;
-    e = cudaFuncSetAttribute(umma_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_LIMIT);
+    for (auto k : {umma_gemm_kernel<64, 0>, umma_gemm_kernel<64, 1>, umma_gemm_kernel<128, 0>, umma_gemm_kernel<128, 1>})
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_LIMIT);
     if (e == cudaSuccess) done_dev = dev;
     return e;
 }
@@ -67,7 +65,7 @@ inline int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     if (ndev != dev) { cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); ndev = dev; }
-    return n > 0 ? n : 148;
+    return n > 0 ? n : 132;
 }
 
 struct Plan { int BN, resident, nstg, nop; size_t smem; bool ok; };
@@ -124,17 +122,13 @@ cudaError_t launch(const GemmDesc& g, cudaStream_t st, std::string* why) {
     p.seq_inner = (int)g.a0.n_inner;
     p.pos_bias = g.pos_bias;
     Plan pl = plan_for(g, pick_bn(g.N));
-    if ((!pl.ok || (!pl.resident && pl.nop < 2)) && pl.BN > 128) pl = plan_for(g, pick_bn(g.N, 128));   // keep two operand slots
+    if ((!pl.ok || (!pl.resident && pl.nop < 2)) && pl.BN > 64) pl = plan_for(g, 64);   // keep two operand slots
     if (!pl.ok) return bad("operand tile does not fit shared memory");
     p.N = g.N; p.BN = pl.BN; p.n_tiles_n = (g.N + p.BN - 1) / p.BN;
     p.passes = g.passes; p.b_mn_major = g.b.mn_major ? 1 : 0; p.b_by_seq = g.b_by_seq ? 1 : 0;
-    p.idesc = make_idesc_bf16(p.BN, p.b_mn_major);
     p.b_resident = pl.resident; p.nstg = pl.nstg; p.nop = pl.nop;
     const size_t smem = pl.smem;
     const int planes = g.passes > 2 ? 2 : 1;      // B planes the tensor map exposes
-    int cols = 32;
-    while (cols < 2 * p.BN) cols <<= 1;
-    p.tmem_cols = cols;
     // ---- tensor maps ----
     {
         const int tile_box[4] = {32, p.P_TILE, p.S_TILE, 1};
@@ -184,7 +178,8 @@ cudaError_t launch(const GemmDesc& g, cudaStream_t st, std::string* why) {
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = g.pdl ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, umma_gemm_kernel, p);
+    if (p.BN == 64) return p.b_mn_major ? cudaLaunchKernelEx(&cfg, umma_gemm_kernel<64, 1>, p) : cudaLaunchKernelEx(&cfg, umma_gemm_kernel<64, 0>, p);
+    return p.b_mn_major ? cudaLaunchKernelEx(&cfg, umma_gemm_kernel<128, 1>, p) : cudaLaunchKernelEx(&cfg, umma_gemm_kernel<128, 0>, p);
 }
 
 // ---- B operand preparation: fp32 matrix (any strides) -> bf16 hi/lo planes [2][rows][cols] ---------------------

@@ -1,21 +1,21 @@
-// umma_gemm: the dense contractions of both networks on the 5th-generation tensor cores.
+// umma_gemm: the dense contractions of both networks on the Hopper tensor cores (wgmma).
 //
 //     C[m, n] = epi( alpha * sum_k A(m)[k] * B[n][k] + bias[n] )          (fp32 in, fp32 out)
 //
-// One persistent CTA per SM, 128-row tiles, the Blackwell way:
+// One persistent CTA per SM, 128-row tiles:
 //   * operands arrive through TENSOR-MAP TMA (cp.async.bulk.tensor, SASS UTMALDG) with 128-byte swizzle:
 //     the fp32 activation tile [128 rows x 64 k] into a staging ring, the weight tile (bf16, split on the host
 //     side of the engine into hi/lo planes) straight into the operand ring;
 //   * a converter warpgroup (thread = row) turns the staged fp32 rows into bf16 hi/lo operand tiles in the
 //     canonical K-major SWIZZLE_128B layout (optionally applying LayerNorm over the 64 channels of the row first
 //     -- nn.LayerNorm semantics -- so that LN -> Linear pairs are one kernel);
-//   * ONE thread issues tcgen05.mma (kind::f16, bf16 x bf16 -> fp32, M = 128, N = BN <= 256) with the accumulator in
-//     TENSOR MEMORY.  passes = 3 gives fp32-grade products from three bf16 MMAs
+//   * two math warpgroups, 64 rows each, issue wgmma (bf16 x bf16 -> fp32, M = 64, N = BN in {64, 128}) with the
+//     accumulators in registers.  passes = 3 gives fp32-grade products from three bf16 MMAs
 //     (a_hi*b_hi + a_lo*b_hi + a_hi*b_lo, relative error ~2^-16 per product: the "bf16x3" split); passes = 2 drops the
 //     b_lo term (bf16 weights, activations still split: the offline bf16 configuration); passes = 1 is plain bf16;
-//   * the epilogue warpgroup reads the accumulator back with tcgen05.ld (thread = row = TMEM lane), applies
-//     bias / PReLU / residual / scale and stores fp32 rows; accumulators are double-buffered in TMEM so the epilogue
-//     of tile i overlaps the MMAs of tile i+1.
+//   * the same warpgroups then apply bias / PReLU / residual / scale and store fp32 rows (transposed through shared
+//     memory so that every warp store writes whole 128-byte lines); the TMA warp and the converter keep filling the
+//     operand ring for the next tile meanwhile.
 //
 // "Rows" (the M space) are (sequence, position) pairs described by a 4-D tensor map (channel, position,
 // seq_inner, seq_outer); a k-chunk of 64 channels may come from a position offset `dp` (overlapping windows: the
@@ -32,9 +32,9 @@
 namespace l2h {
 namespace umma {
 
-constexpr int BM = 128;          // rows per tile == TMEM lanes
+constexpr int BM = 128;          // rows per tile: two math warpgroups of 64
 constexpr int KC = 64;           // k-chunk: 64 bf16 = one 128-byte swizzle row
-constexpr int NTHREADS = 320;    // warp 0: TMA, warp 1: MMA + TMEM alloc, warps 2-5: converter, warps 6-9: epilogue
+constexpr int NTHREADS = 416;    // warps 0-3: converter, 4-7 and 8-11: math (rows 0-63, 64-127), warp 12: TMA
 constexpr int MAX_NSTG = 2;      // fp32 staging ring slots (32 KB each)
 constexpr int STG_BYTES = BM * KC * 4;
 constexpr int OPA_PLANE = BM * KC * 2;   // 16 KB per bf16 plane
@@ -55,10 +55,8 @@ struct Params {
     int seq_inner;             // sequence -> tensor-map coordinates (seq % seq_inner, seq / seq_inner)
     int pos_bias;              // added to every position coordinate (may be negative: zero-filled halo)
     int N, BN, n_tiles_n, passes, b_mn_major, b_by_seq;
-    unsigned idesc;
     int nop;                   // operand ring slots
     int nstg;                  // fp32 staging ring slots (1 or 2)
-    int tmem_cols;
     int vec_ok;                // C/R rows 16-byte aligned: float4 epilogue accesses
     int b_resident;            // all k-chunks of the B tile stay in shared memory for the CTA's whole life
     // epilogue
@@ -73,12 +71,6 @@ struct Params {
     const float* ln_b;
     float alpha;
 };
-
-__host__ __device__ inline unsigned make_idesc_bf16(int n, int b_mn_major) {
-    // c_format F32 (bits 4-5 = 1), a/b format BF16 (bits 7-9, 10-12 = 1), b_major bit 16, N>>3 at 17, M>>4 at 24
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((unsigned)(b_mn_major ? 1 : 0) << 16) | ((unsigned)(n >> 3) << 17) |
-           ((unsigned)(BM >> 4) << 24);
-}
 
 }  // namespace umma
 }  // namespace l2h

@@ -49,7 +49,7 @@ class _EmbedBlockParams(nn.Module):
 
 
 class EmbedTFGridNet(nn.Module):
-    """B200-native replacement of the reference ``EmbedTFGridNet``."""
+    """CUDA (H100) replacement of the reference ``EmbedTFGridNet``."""
 
     def __init__(self, embed_dim, num_ch, n_fft, stride, num_blocks):
         super().__init__()
@@ -117,7 +117,7 @@ class EmbedTFGridNet(nn.Module):
     def forward(self, input):
         """input [B, M, N] -> [B, embed_dim]   (reference tfgridnet.py:100-127)."""
         if not input.is_cuda:
-            raise RuntimeError("lookoncetohear_b200.EmbedTFGridNet runs only on a CUDA (sm_100a) device: "
+            raise RuntimeError("lookoncetohear_b200.EmbedTFGridNet runs only on a CUDA (sm_90a) device: "
                                "hand-written CUDA hot path, no CPU fallback")
         dev = input.device
         self._sync_weights(dev)

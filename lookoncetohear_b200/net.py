@@ -5,7 +5,7 @@ Select it from the reference's config by pointing ``pl_module_args.model`` at
 ts_hear_embed_pl_module.py:25).  Same constructor keywords, same parameter names and shapes (a
 Lightning checkpoint's ``state_dict`` loads unchanged), same ``forward / predict /
 init_buffers`` signatures.  The arithmetic is NOT here: every call goes through the C ABI of
-``liblookonce_b200.so`` (hand-written sm_100a CUDA).  There is no PyTorch/CPU fallback -- on a
+``liblookonce_b200.so`` (hand-written sm_90a CUDA).  There is no PyTorch/CPU fallback -- on a
 machine without the built library or without a CUDA device the calls raise.
 
 The torch modules held below (nn.Conv2d, nn.LSTM, ...) are used purely as parameter containers,
@@ -183,7 +183,7 @@ class SepState(dict):
 
 
 class Net(nn.Module):
-    """B200-native replacement of the reference ``Net`` (net.py:20-76)."""
+    """CUDA (H100) replacement of the reference ``Net`` (net.py:20-76)."""
 
     def __init__(self, stft_chunk_size=160, stft_pad_size=120, embed_dim=256, num_ch=2, D=64, B=6, I=1, J=1,
                  L=0, H=128, use_attn=False, lookahead=True, local_atten_len=100, chunk_causal=False,
@@ -203,9 +203,9 @@ class Net(nn.Module):
         self._handle = None
         self._dirty = True                      # weights need (re)packing into the engine
         self._ws = None
-        # batch*frames per kernel chain.  36 clips of 500 frames: the intra recurrence (2 x 18 000 sequences, 32 per tensor-core CTA) is
-        # 3.8 waves of the 296 resident CTAs and the inter recurrence (3 492 sequences, 4 per CUDA-core CTA) 2.95 waves; measured
-        # 651 k frames/s against 628 k at 18 clips, 600 k at 16 (tools/offline_split_experiment.py)
+        # batch*frames per kernel chain: 36 clips of 500 frames (the intra recurrence then has 2 x 18 000 sequences, the inter
+        # recurrence 3 492).  Chosen with an earlier tensor-core recurrence on another GPU; not re-measured on the H100
+        # (tools/offline_split_experiment.py measures it)
         self.max_frames_per_launch = 18432
 
     # ---- engine plumbing -------------------------------------------------------------------
@@ -300,7 +300,7 @@ class Net(nn.Module):
     @staticmethod
     def _require_cuda(t):
         if not t.is_cuda:
-            raise RuntimeError("lookoncetohear_b200.Net runs only on a CUDA (sm_100a) device: the hot path is "
+            raise RuntimeError("lookoncetohear_b200.Net runs only on a CUDA (sm_90a) device: the hot path is "
                                "hand-written CUDA with no CPU fallback")
 
     # ---- reference API ---------------------------------------------------------------------

@@ -1,8 +1,8 @@
 """ORACLE (test infrastructure): import the reference's own modules, unmodified, by path.
 
-Works only where the reference checkout exists (/root/reference in the build container, or a
-driver-placed copy under baseline/_ref); the GPU box has neither, there the checker is
-oracle/restate.py + the committed fixtures under tests/golden/.
+Works only where a reference checkout exists; its path is taken from the environment variable
+LOOKONCE_REFERENCE.  Only the fixture generator (tests/golden/make_golden.py) uses it: the tests check against
+oracle/restate.py + the committed fixtures under tests/golden/, which were generated from the reference.
 
 The reference's two third-party packages that are absent from this image (asteroid_filterbanks,
 espnet2 -- SURVEY.md section 8c) are satisfied by the restatements in oracle/shims/.
@@ -15,13 +15,12 @@ import sys
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SHIMS = os.path.join(_HERE, "shims")
-_CANDIDATES = ["/root/reference", os.path.join(os.path.dirname(_HERE), "baseline", "_ref")]
 
 
 def reference_root():
-    for c in _CANDIDATES:
-        if os.path.isfile(os.path.join(c, "src", "models", "tfgridnet_realtime", "net.py")):
-            return c
+    c = os.environ.get("LOOKONCE_REFERENCE")
+    if c and os.path.isfile(os.path.join(c, "src", "models", "tfgridnet_realtime", "net.py")):
+        return c
     return None
 
 
@@ -32,7 +31,7 @@ def available():
 def _prepare():
     root = reference_root()
     if root is None:
-        raise RuntimeError("reference checkout not present (expected on the GPU box)")
+        raise RuntimeError("reference checkout not found: set LOOKONCE_REFERENCE to its path")
     for p in (root, _SHIMS):
         if p not in sys.path:
             sys.path.insert(0, p)

@@ -1,11 +1,11 @@
 """ORACLE SHIM (test infrastructure, never shipped / never on the product path).
 
 Restatement of the one entry point of the un-vendored third-party package
-``asteroid-filterbanks`` (pulled in by ``asteroid``, /root/reference/requirements.txt:15,
+``asteroid-filterbanks`` (pulled in by ``asteroid``, reference requirements.txt:15,
 no version pinned) that the reference's separation model calls:
 
     make_enc_dec('stft', n_filters, kernel_size, stride, window_type=...)
-        -- call site /root/reference/src/models/tfgridnet_realtime/tfgridnet_causal.py:131-135
+        -- call site reference src/models/tfgridnet_realtime/tfgridnet_causal.py:131-135
     enc(x[B,M,N]) -> [B,M,n_filters+2,T]           -- call site :229
     dec(spec[B,S,n_filters+2,T]) -> [B,S,(T-1)*stride+kernel]   -- call site :272
 

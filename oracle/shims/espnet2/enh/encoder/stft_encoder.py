@@ -1,6 +1,6 @@
 """ORACLE SHIM: restatement of espnet2 STFTEncoder (package absent, no version pinned:
-/root/reference/requirements.txt:19).  Semantics = the Stft.forward the reference vendors at
-/root/reference/src/models/tfgridnet_orig/stft.py:68-195: torch.stft(center=True -> reflect
+reference requirements.txt:19).  Semantics = the Stft.forward the reference vendors at
+reference src/models/tfgridnet_orig/stft.py:68-195: torch.stft(center=True -> reflect
 pad n_fft//2, periodic Hann, onesided, not normalised); multi-channel input [B,N,M] gives a
 complex spectrum [B,T,M,F]."""
 import torch

@@ -1,9 +1,9 @@
 """ORACLE SHIM (test infrastructure, never on the product path).
 
 Restatement of ``espnet2.enh.separator.tfgridnet_separator`` -- the base class of the
-reference's enrollment network (/root/reference/src/models/tfgridnet_orig/tfgridnet.py:8,
+reference's enrollment network (reference src/models/tfgridnet_orig/tfgridnet.py:8,
 ``class TFGridNet(TFGridNet)`` :11, ``EmbedTFGridNet`` :88-98).  espnet is an un-vendored,
-un-pinned dependency (/root/reference/requirements.txt:19) and is absent from this image, so
+un-pinned dependency (reference requirements.txt:19) and is absent from this image, so
 the constructor and ``GridNetBlock`` are restated from the package's published algorithm
 (TF-GridNet, Wang et al. 2022; SURVEY.md Appendix B / C.2).  Only ``__init__`` and
 ``GridNetBlock.forward`` matter: the reference overrides ``TFGridNet.forward``.

@@ -1,5 +1,6 @@
-"""Generate the committed fixtures from the REFERENCE ITSELF (run in the build container, where
-/root/reference exists):  python tests/golden/make_golden.py
+"""Generate the committed fixtures from the REFERENCE ITSELF (a checkout of vb000/LookOnceToHear):
+
+    LOOKONCE_REFERENCE=<checkout> python tests/golden/make_golden.py
 
 Weights are not stored (8 MB): they are the PyTorch default init under torch.manual_seed(seed),
 which the reference modules and the engine's parameter containers reproduce identically
@@ -23,6 +24,76 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 def weight_checksum(sd):
     return np.array([float(sum(v.double().abs().sum() for v in sd.values())),
                      float(sum((v.double() ** 2).sum() for v in sd.values()))])
+
+
+def sample(t, k, seed):
+    """A fixed, seeded sample of at most k elements of t: (flat indices, values, L2 norm of the whole tensor)."""
+    flat = t.detach().reshape(-1)
+    g = torch.Generator().manual_seed(seed)
+    idx = torch.randperm(flat.numel(), generator=g)[:k].sort().values if flat.numel() > k else torch.arange(flat.numel())
+    return idx.numpy().astype(np.int32), flat[idx].numpy(), float(flat.double().norm())
+
+
+def ref_pins():
+    """What the reference-pinning tests compare against (tests/test_oracle.py, tests/test_ckpt.py): outputs and
+    state of the reference modules on the tests' seeded inputs, and the vendored STFT; large tensors as samples."""
+    import importlib
+    pins = {}
+
+    def put(name, t, k=512, seed=0):
+        pins[name + "/idx"], pins[name + "/val"], pins[name + "/norm"] = sample(t, k, seed)
+        pins[name + "/shape"] = np.array(t.shape)
+
+    # seeded default init of both networks: 16 sampled values and the norm of every state_dict entry
+    for tag, net in (("init_sep", rl.reference_net(0)), ("init_embed", rl.reference_embed_net(0))):
+        sd = net.state_dict()
+        rows = []
+        for i, v in enumerate(sd.values()):
+            flat = v.reshape(-1)
+            g = torch.Generator().manual_seed(i)
+            idx = torch.randperm(flat.numel(), generator=g)[:16] if flat.numel() >= 16 else torch.arange(16) % flat.numel()
+            rows.append((idx.numpy().astype(np.int32), flat[idx].numpy(), float(flat.double().norm())))
+        pins[f"{tag}/keys"] = np.array(list(sd))
+        pins[f"{tag}/idx"] = np.stack([r[0] for r in rows])
+        pins[f"{tag}/val"] = np.stack([r[1] for r in rows])
+        pins[f"{tag}/norm"] = np.array([r[2] for r in rows])
+        pins[f"{tag}/n_params"] = np.array(sum(p.numel() for p in net.parameters()))
+    # forward + final state, seed 3, B = 2, ragged length
+    net = rl.reference_net(3)
+    x, _ = synth.mixture(2, 128 * 9 + 77, seed0=50)
+    e = synth.embedding(2, seed0=60)
+    with torch.no_grad():
+        pins["fwd3/y"] = net(x, e).numpy()
+        st = net.init_buffers(2, "cpu")
+        _, st = net.predict(x, e[:, 0], st)
+    for k in ("conv_buf", "deconv_buf", "istft_buf"):
+        put(f"fwd3/{k}", st[k])
+    for i in range(3):
+        for k in ("K_buf", "V_buf", "h0", "c0"):
+            put(f"fwd3/buf{i}/{k}", st["gridnet_bufs"][f"buf{i}"][k], 512, 10 * i)
+    # forward, seed 1, B = 1 (the fp64 floor of the restatement)
+    net = rl.reference_net(1)
+    x, _ = synth.mixture(1, 128 * 8)
+    with torch.no_grad():
+        pins["fwd1/y"] = net(x, synth.embedding(1)).numpy()
+    # enrollment, seed 2
+    en = rl.reference_embed_net(2)
+    with torch.no_grad():
+        pins["emb2/emb"] = en(synth.enrollment(2, 5000)).numpy()
+    # checkpoint -> outputs on the GPU: the reference network of seed 13 on a 12-hop clip
+    net = rl.reference_net(13)
+    x, _ = synth.mixture(1, 128 * 12)
+    with torch.no_grad():
+        pins["ckpt13/y"] = net(x, synth.embedding(1)).numpy()
+    pins["ckpt13/wsum"] = weight_checksum(net.state_dict())
+    # the STFT the reference vendors (src/models/tfgridnet_orig/stft.py)
+    Stft = importlib.import_module("src.models.tfgridnet_orig.stft").Stft
+    for i, (n_fft, hop, n) in enumerate(((128, 64, 5000), (128, 64, 4999), (192, 128, 3001))):
+        xs = synth.enrollment(3, n).transpose(1, 2).contiguous()
+        ref, olens = Stft(n_fft=n_fft, win_length=n_fft, hop_length=hop, window="hann")(xs, torch.tensor([n, n, n]))
+        put(f"stft{i}/spec", ref, 1024, 100 + i)
+        pins[f"stft{i}/olens"] = olens.numpy()
+    np.savez_compressed(os.path.join(HERE, "ref_pins.npz"), **pins)
 
 
 def main():
@@ -62,8 +133,9 @@ def main():
             "embed": {k: list(v.shape) for k, v in en.state_dict().items()}}
     with open(os.path.join(HERE, "ckpt_keys.json"), "w") as f:
         json.dump(keys, f, indent=0, sort_keys=True)
+    ref_pins()
     print("written", os.listdir(HERE))
 
 
 if __name__ == "__main__":
-    main()
+    main() if "--pins-only" not in sys.argv else ref_pins()

@@ -1,26 +1,25 @@
 """SURVEY section 8(f1): a Lightning checkpoint of the reference loads UNCHANGED into the engine's classes.
 
 The evaluation driver does ``torch.load(run_dir/best.ckpt)['state_dict']`` and ``load_state_dict`` on a
-LightningModule whose ``self.model`` is the network (/root/reference/src/ts_hear_test.py:18-34,
+LightningModule whose ``self.model`` is the network (reference src/ts_hear_test.py:18-34,
 ts_hear_embed_pl_module.py:25), so every key carries a ``model.`` prefix; real asteroid registers one extra buffer
-per filterbank (``torch_window``).  Where the reference checkout exists the checkpoint is written from the
-reference's own modules; everywhere, the key names and shapes are pinned by a committed fixture generated from
-the reference (tests/golden/make_golden.py -> ckpt_keys.json).
+per filterbank (``torch_window``).  The checkpoints here carry exactly the key names and shapes of the reference
+modules (committed fixture generated from the reference: tests/golden/make_golden.py -> ckpt_keys.json), and the
+outputs of the reference network of a seeded checkpoint are pinned by tests/golden/ref_pins.npz.
 """
 import json
 import os
 
+import numpy as np
 import pytest
 import torch
 import torch.nn as nn
 
 from lookoncetohear_b200 import EmbedTFGridNet, Net, synth
 from lookoncetohear_b200.net import SepState
-from oracle import ref_loader as rl
 from oracle import restate as rs
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-needs_ref = pytest.mark.skipif(not rl.available(), reason="reference checkout not present on this box")
 
 
 class _PLShaped(nn.Module):
@@ -31,20 +30,26 @@ class _PLShaped(nn.Module):
         self.model = model
 
 
-def _write_ckpt(path, module, extra=None):
-    sd = {k: v.detach().clone() for k, v in _PLShaped(module).state_dict().items()}
+def _write_ckpt(path, sd, extra=None):
+    sd = {"model." + k: v for k, v in sd.items()}
     sd.update(extra or {})
     torch.save({"state_dict": sd, "epoch": 7, "global_step": 1234}, path)
     return sd
 
 
-@needs_ref
+def _reference_shaped(name, seed):
+    """A state_dict with the reference module's key names and shapes (fixture) and seeded random values."""
+    with open(os.path.join(GOLD, "ckpt_keys.json")) as f:
+        keys = json.load(f)[name]
+    g = torch.Generator().manual_seed(seed)
+    return {k: torch.randn(shape, generator=g) for k, shape in keys.items()}
+
+
 def test_separator_checkpoint_loads_strict(tmp_path, tsh_params):
-    ref = rl.reference_net(11)
     path = os.path.join(tmp_path, "best.ckpt")
     extra = {"model.tfgridnet.enc.filterbank.torch_window": torch.hann_window(192),
              "model.tfgridnet.dec.filterbank.torch_window": torch.hann_window(192)}
-    sd = _write_ckpt(path, ref, extra)
+    sd = _write_ckpt(path, _reference_shaped("sep", 11), extra)
     torch.manual_seed(99)                                   # different init: everything must come from the file
     mine = _PLShaped(Net(**tsh_params))
     state = torch.load(path, map_location="cpu")["state_dict"]
@@ -56,11 +61,9 @@ def test_separator_checkpoint_loads_strict(tmp_path, tsh_params):
     assert mine.model._dirty                                # the engine repacks on the next call
 
 
-@needs_ref
 def test_enrollment_checkpoint_loads_strict(tmp_path, embed_params):
-    ref = rl.reference_embed_net(12)
     path = os.path.join(tmp_path, "embed.ckpt")
-    sd = _write_ckpt(path, ref)
+    sd = _write_ckpt(path, _reference_shaped("embed", 12))
     torch.manual_seed(98)
     mine = _PLShaped(EmbedTFGridNet(**embed_params))
     mine.load_state_dict(torch.load(path, map_location="cpu")["state_dict"], strict=True)
@@ -109,11 +112,18 @@ def test_net_deepcopy_and_pickle(tsh_params):
 
 
 @pytest.mark.gpu
-@needs_ref
 def test_checkpoint_outputs_on_gpu(tmp_path, tsh_params):
-    ref = rl.reference_net(13)
+    """The reference network of seed 13 as a Lightning checkpoint (its weights = the seeded default init, pinned by
+    a checksum of the reference's) -> the engine's outputs == the reference's outputs (fixture)."""
+    pins = np.load(os.path.join(GOLD, "ref_pins.npz"))
+    torch.manual_seed(13)
+    ref_sd = {k: v.detach().clone() for k, v in Net(**tsh_params).state_dict().items()}
+    wsum = np.array([float(sum(v.double().abs().sum() for v in ref_sd.values())),
+                     float(sum((v.double() ** 2).sum() for v in ref_sd.values()))])
+    assert np.allclose(wsum, pins["ckpt13/wsum"], rtol=1e-9), "seeded init differs from the build that made the fixture"
     path = os.path.join(tmp_path, "best.ckpt")
-    _write_ckpt(path, ref)
+    _write_ckpt(path, ref_sd)
+    torch.manual_seed(99)
     mine = _PLShaped(Net(**tsh_params))
     mine.load_state_dict(torch.load(path, map_location="cpu")["state_dict"], strict=True)
     mine = mine.eval().cuda()
@@ -121,8 +131,7 @@ def test_checkpoint_outputs_on_gpu(tmp_path, tsh_params):
     e = synth.embedding(1)
     with torch.no_grad():
         y = mine.model(x.cuda(), e.cuda()).cpu()
-        y_ref = ref(x, e)
-    assert rs.rel_l2(y, y_ref) <= 1e-3
+    assert rs.rel_l2(y, torch.from_numpy(pins["ckpt13/y"])) <= 1e-3
 
 
 @pytest.mark.gpu

@@ -172,7 +172,7 @@ def test_enrollment_batch_1024(embed_params, dev):
 
 def test_fused_input_projection_recurrence_option(sep, dev):
     """Engine option "fuse_ih": LayerNorm + W_ih + the recurrence as ONE tensor-core kernel (tc_lstm_x_kernel) for calls
-    with >= 4096 sequence-directions.  Off by default (measured slower than GEMM + tc_lstm, profiles/r02i); same gates."""
+    with >= 4096 sequence-directions.  Off by default; same gates."""
     net, sd = sep
     B = 20
     x, tgt = synth.mixture(B, 128 * 110, seed0=2400)            # 20 x 110 frames: 4400 intra sequence-directions, 1940 inter

@@ -1,5 +1,5 @@
 """On-GPU evaluation epilogue (l2h_eval_metrics) against the formulas of the reference's evaluation loop
-(/root/reference/src/ts_hear_test.py:139-146): torchmetrics SI-SNR (restated in oracle/restate.py::si_sdr and pinned
+(reference src/ts_hear_test.py:139-146): torchmetrics SI-SNR (restated in oracle/restate.py::si_sdr and pinned
 by a known-answer test) and torch's cosine_similarity."""
 import pytest
 import torch

@@ -333,8 +333,8 @@ def test_one_hop_cluster_kernel_equals_separate_kernels(model, dev):
 
 
 def test_one_hop_form_switches_with_the_number_of_streams(model, dev):
-    """A one-hop call takes the cluster-kernel form only while all its 16-CTA clusters fit on the device at once (7 on a
-    B200); a call with more streams runs the separate kernels.  The same stream must come out the same (1e-5) from a
+    """A one-hop call takes the cluster-kernel form only while all its 16-CTA clusters fit on the device at once (as
+    cudaOccupancyMaxActiveClusters reports it); a call with more streams runs the separate kernels.  The same stream must come out the same (1e-5) from a
     4-stream call (cluster form) and from a 12-stream call (separate kernels), state carried over 8 hops."""
     net, _ = model
     B, T = 12, 8

@@ -1,5 +1,5 @@
 // Probe: can a 16-CTA (non-portable) cluster with ~226 KB of shared memory per CTA be scheduled, and what do a
-// cluster barrier and a DSMEM gather cost at that size?   nvcc -arch=sm_100a -o cluster16_probe cluster16_probe.cu
+// cluster barrier and a DSMEM gather cost at that size?   nvcc -gencode arch=compute_90a,code=sm_90a -o cluster16_probe cluster16_probe.cu
 #include <cooperative_groups.h>
 #include <cstdio>
 #include <cuda_runtime.h>

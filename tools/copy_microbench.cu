@@ -1,5 +1,5 @@
 // How fast can ONE CTA stage a contiguous block from (L2-resident) global memory into shared memory?
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o tools/copy_microbench tools/copy_microbench.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/copy_microbench tools/copy_microbench.cu
 #include <cstdio>
 #include "../lookoncetohear_b200/csrc/common.cuh"
 using namespace l2h;

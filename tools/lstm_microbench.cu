@@ -1,5 +1,5 @@
 // Micro-benchmark of LSTM recurrence step variants (one CTA = one sequence, one direction).
-// Build:  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o tools/lstm_microbench tools/lstm_microbench.cu
+// Build:  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/lstm_microbench tools/lstm_microbench.cu
 // Prints ns per recurrent step for each variant (timing only; E* variants change the math).
 #include <cstdio>
 #include <vector>

@@ -1,5 +1,5 @@
 """configs[2] (256 clips of 4 s, bf16 option) against the number of clips per kernel chain: wave quantisation of the recurrences
-(tc_lstm: 32 sequences per CTA, 296 resident; lstm_rec4: NSEQ per CTA) decides the best split.   python tools/offline_split_experiment.py"""
+(tc_lstm: 32 sequences per CTA; lstm_rec4: NSEQ per CTA) decides the best split.   python tools/offline_split_experiment.py"""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,5 +1,5 @@
-// Standalone correctness + throughput harness for csrc/umma_gemm.cuh (tcgen05 / TMEM / tensor-map TMA GEMM).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -o tools/umma_gemm_test tools/umma_gemm_test.cu lookoncetohear_b200/csrc/umma_gemm.cu
+// Standalone correctness + throughput harness for csrc/umma_gemm.cuh (wgmma / tensor-map TMA GEMM).
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -o tools/umma_gemm_test tools/umma_gemm_test.cu lookoncetohear_b200/csrc/umma_gemm.cu
 // Every case is checked against a double-precision CPU product of the same fp32 inputs.
 #include <cuda_runtime.h>
 #include <cmath>
