@@ -1,13 +1,15 @@
 """The reference's evaluation loop (src/ts_hear_test.py:93-166) with every arithmetic step on the GPU engine:
 
-    mono events + impulse responses --render_binaural--> mixture, target          (multi_ch_simulator.py:56-58,
+    mono events + 44.1 kHz impulse responses --render_binaural--> mixture, target  (multi_ch_simulator.py:49-58: resampled
+                                                                                     to 16 kHz, then convolved;
                                                                                      MixLibriSpeechNoisyEnrollNorm.py:179-202)
     enrollment recording --EmbedTFGridNet--> embedding                             (ts_hear_test.py:133-135)
     model(mixture, embedding) --Net--> outputs                                     (ts_hear_test.py:138)
     eval_metrics(outputs, target, mixture, embedding, embedding_gt)                (ts_hear_test.py:139-146)
 
-Synthetic inputs (no dataset in the image): white-noise events, exponentially decaying random impulse responses.  Only the
-three metric floats per mixture leave the device.  Usage: python examples/eval_gpu.py [n_batches] [batch]"""
+Synthetic inputs (no dataset at hand): white-noise events, exponentially decaying random impulse responses drawn at
+44.1 kHz like CIPIC's HRIRs and resampled on the device.  Only the three metric floats per mixture leave the device.
+Usage: python examples/eval_gpu.py [n_batches] [batch]"""
 import os
 import sys
 import time
@@ -20,8 +22,11 @@ from lookoncetohear_b200.configs import EMBED_PARAMS, TSH_PARAMS
 from lookoncetohear_b200.metrics import eval_metrics
 from lookoncetohear_b200.render import render_binaural
 
+RIR_SR = 44100
+
 
 def synthetic_batch(batch, n_src, n, rir_len, gen, dev):
+    """Events at 16 kHz, responses of rir_len taps at RIR_SR."""
     srcs = 0.1 * torch.randn(batch, n_src, n, generator=gen, device=dev)
     decay = torch.exp(-torch.arange(rir_len, device=dev) / (rir_len / 6.0))
     rirs = torch.randn(batch, n_src, 2, rir_len, generator=gen, device=dev) * decay
@@ -42,12 +47,12 @@ def main():
     t0 = time.perf_counter()
     with torch.no_grad():
         for _ in range(n_batches):
-            srcs, rirs, noise, scale = synthetic_batch(batch, 3, 80000, 200, gen, dev)
-            events, mixture, _ = render_binaural(srcs, rirs, noise, scale)
+            srcs, rirs, noise, scale = synthetic_batch(batch, 3, 80000, 551, gen, dev)
+            events, mixture, _ = render_binaural(srcs, rirs, noise, scale, rir_sr=RIR_SR, sr=16000)
             target = events[:, 0]                                              # tgt_idx = 0
             # noisy enrollment: the target speaker's other utterance rendered with another response, plus background
-            e_src, e_rir, e_noise, e_scale = synthetic_batch(batch, 1, 80000, 200, gen, dev)
-            _, enrollment, _ = render_binaural(e_src, e_rir, e_noise, e_scale)
+            e_src, e_rir, e_noise, e_scale = synthetic_batch(batch, 1, 80000, 551, gen, dev)
+            _, enrollment, _ = render_binaural(e_src, e_rir, e_noise, e_scale, rir_sr=RIR_SR, sr=16000)
             embedding = enroll_model(enrollment).unsqueeze(1)                  # [B, 1, 256]
             embedding_gt = torch.nn.functional.normalize(torch.rand(batch, 1, 256, generator=gen, device=dev), dim=-1)
             outputs = model(mixture, embedding)

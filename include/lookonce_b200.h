@@ -229,12 +229,29 @@ int l2h_eval_metrics(const float* est_dev, const float* target_dev, const float*
  *   events[b][s][ear] = convolve(src[b][s], rir[b][s][ear])[:n_samples]      src/datasets/multi_ch_simulator.py:56-58
  *   noise scaled by noise_scale[b]; norm = max|sum(events) + noise|; if norm > 1 events and noise are divided by it;
  *   mixture = sum(events) + noise                                   src/datasets/MixLibriSpeechNoisyEnrollNorm.py:179-202
- * src_dev [batch][n_src][n_samples] mono; rir_dev [batch][n_src][2][rir_len] (already at the sampling rate of src);
- * noise_dev [batch][2][n_samples] or NULL; noise_scale_dev [batch] or NULL (= 1); events_dev [batch][n_src][2][n_samples];
- * mixture_dev [batch][2][n_samples]; norm_dev [batch] or NULL; scratch_dev: batch * 4 bytes.  Asynchronous on `stream`. */
+ * src_dev [batch][n_src][n_samples] mono; rir_dev [batch][n_src][2][rir_len] (already at the sampling rate of src:
+ * l2h_resample brings responses stored at another rate there); noise_dev [batch][2][n_samples] or NULL; noise_scale_dev
+ * [batch] or NULL (= 1); events_dev [batch][n_src][2][n_samples]; mixture_dev [batch][2][n_samples]; norm_dev [batch] or
+ * NULL; scratch_dev: batch * 4 bytes.  Asynchronous on `stream`. */
 int l2h_render_binaural(const float* src_dev, const float* rir_dev, const float* noise_dev, const float* noise_scale_dev,
                         int32_t batch, int32_t n_src, int32_t n_samples, int32_t rir_len, float* events_dev,
                         float* mixture_dev, float* norm_dev, void* scratch_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Band-limited resampling of many rows in one call: torchaudio.functional.resample(row, orig_freq[r], new_freq) at its
+ * defaults (Hann-windowed sinc, lowpass_filter_width 6, rolloff 0.99) -- impulse responses from the rate of their file
+ * to the dataset rate (src/datasets/multi_ch_simulator.py:49) and the dataset's resample_rate step
+ * (MixLibriSpeechNoisyEnrollNorm.py:69-75).  Other methods or parameters are not implemented.
+ *   x_dev       [n_rows] rows of n_in fp32 samples, x_row_stride floats apart (>= n_in)
+ *   orig_freq   HOST array of n_rows rates in Hz, one per row; new_freq the rate of every output row
+ *   y_dev       [n_rows] rows of y_capacity fp32 samples, y_row_stride floats apart (>= y_capacity); must not overlap x
+ * Row r gets n_out(r) = ceil(new_freq * n_in / orig_freq[r]) resampled samples (computed exactly in integers; a row
+ * with orig_freq[r] == new_freq is copied bit for bit), then zeros up to y_capacity -- rows of different rates come out
+ * zero-padded to a common length.  Errors, returned before anything is enqueued: 1 = null pointer, bad size or stride,
+ * a rate <= 0, or some n_out(r) > y_capacity; 2 = a reduced rate ratio orig/new too large for the kernel's input
+ * window (downsampling by more than about 45x).  Asynchronous on `stream`; orig_freq is read during the call only. */
+int l2h_resample(const float* x_dev, int64_t x_row_stride, int32_t n_in, int32_t n_rows, const int32_t* orig_freq,
+                 int32_t new_freq, float* y_dev, int64_t y_row_stride, int32_t y_capacity, void* stream);
 
 #ifdef __cplusplus
 }
