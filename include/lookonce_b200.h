@@ -203,8 +203,9 @@ int l2h_embed_load_weight(void* handle, const char* name, const float* host_data
 int l2h_embed_weights_expected(void* handle, int32_t* n_expected, int32_t* n_loaded);
 int l2h_embed_commit_weights(void* handle, void* stream);
 int l2h_embed_workspace_bytes(void* handle, int32_t batch, int32_t n_samples, size_t* bytes);
-/* "bf16" = 1: the tensor-core GEMMs take plain bf16 operands (one MMA pass); 0 (default): every product is formed from
- * bf16 hi/lo splits of both fp32 operands in three MMA passes (fp32-grade, relative error ~2^-16 per product). */
+/* "bf16" (the separator's mapping): 0 (default): every tensor-core product is formed from bf16 hi/lo splits of both fp32
+ * operands in three MMA passes (fp32-grade, relative error ~2^-16 per product); 1: bf16 weights x split activations (two
+ * passes); 2: plain bf16 operands (one pass). */
 int l2h_embed_set_option(void* handle, const char* name, int32_t value);
 /* largest batch one l2h_embed_forward call should be given for utterances of n_samples (workspace bound) */
 int l2h_embed_max_batch(void* handle, int32_t n_samples, int32_t* max_batch);

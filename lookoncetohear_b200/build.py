@@ -18,7 +18,14 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-
               "--compiler-options", "-fPIC", "-shared", "-Xptxas", "-v"]
 
 
-def _fingerprint():
+# test-only library: direct C entry points into the tensor-core GEMM and the LSTM recurrences (tests/kernels/).
+# Hidden visibility + -Bsymbolic: its copy of the engine's symbols never binds to the product library's copy.
+HARNESS_SRC = os.path.join(os.path.dirname(HERE), "tests", "kernels", "kernel_harness.cu")
+HARNESS_LIB = os.path.join(LIBDIR, "libl2h_kernel_harness.so")
+HARNESS_FLAGS = ["--compiler-options", "-fvisibility=hidden", "-Xlinker", "-Bsymbolic", "-I", CSRC]
+
+
+def _fingerprint(extra_files=(), extra_flags=()):
     h = hashlib.sha256()
     inc = os.path.join(os.path.dirname(HERE), "include")
     for d in (CSRC, inc):
@@ -27,7 +34,11 @@ def _fingerprint():
                 with open(os.path.join(d, fn), "rb") as f:
                     h.update(fn.encode())
                     h.update(f.read())
-    h.update(" ".join(NVCC_FLAGS).encode())
+    for p in extra_files:
+        with open(p, "rb") as f:
+            h.update(os.path.basename(p).encode())
+            h.update(f.read())
+    h.update(" ".join(NVCC_FLAGS + list(extra_flags)).encode())
     return h.hexdigest()
 
 
@@ -38,17 +49,15 @@ def nvcc_path():
     return "nvcc"
 
 
-def build(force=False, verbose=False):
-    """Compile if sources changed since the last build.  Returns the library path."""
+def _compile(out, sources, fp, extra_flags, log_name, force, verbose):
     os.makedirs(LIBDIR, exist_ok=True)
-    stamp = LIB + ".sha256"
-    fp = _fingerprint()
-    if not force and os.path.isfile(LIB) and os.path.isfile(stamp) and open(stamp).read().strip() == fp:
-        return LIB
-    cmd = [nvcc_path()] + NVCC_FLAGS + ["-o", LIB] + [os.path.join(CSRC, s) for s in SOURCES]
+    stamp = out + ".sha256"
+    if not force and os.path.isfile(out) and os.path.isfile(stamp) and open(stamp).read().strip() == fp:
+        return out
+    cmd = [nvcc_path()] + NVCC_FLAGS + list(extra_flags) + ["-o", out] + list(sources)
     res = subprocess.run(cmd, capture_output=True, text=True)
     log = res.stdout + res.stderr
-    with open(os.path.join(LIBDIR, "build.log"), "w") as f:
+    with open(os.path.join(LIBDIR, log_name), "w") as f:
         f.write(" ".join(cmd) + "\n" + log)
     if res.returncode != 0:
         raise RuntimeError("nvcc failed:\n" + log[-4000:])
@@ -56,8 +65,20 @@ def build(force=False, verbose=False):
         print(log)
     with open(stamp, "w") as f:
         f.write(fp)
-    return LIB
+    return out
+
+
+def build(force=False, verbose=False):
+    """Compile if sources changed since the last build.  Returns the library path."""
+    return _compile(LIB, [os.path.join(CSRC, s) for s in SOURCES], _fingerprint(), [], "build.log", force, verbose)
+
+
+def build_harness(force=False, verbose=False):
+    """The test-only kernel harness library (same flags as the product library), if its sources changed."""
+    fp = _fingerprint([HARNESS_SRC], HARNESS_FLAGS)
+    return _compile(HARNESS_LIB, [HARNESS_SRC], fp, HARNESS_FLAGS, "build_harness.log", force, verbose)
 
 
 if __name__ == "__main__":
     print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))
+    print(build_harness(force="--force" in sys.argv, verbose="-v" in sys.argv))

@@ -58,7 +58,7 @@ struct EmbedEngine {
     std::vector<PlaneSrc> plane_srcs;
     __nv_bfloat16* planes = nullptr;
     int64_t planes_total = 0;
-    int passes = 3;                 // 3: bf16x3 split products (fp32-grade), 1: plain bf16 operands
+    int passes = 3;                 // 3: bf16x3 split products (fp32-grade), 2: bf16 weights x split activations, 1: plain bf16
 };
 
 static umma::BPlanes wplanes(const EmbedEngine* e, const float* wt, int K, int N) {

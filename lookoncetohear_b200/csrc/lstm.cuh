@@ -28,7 +28,7 @@ struct LstmArgs {
     float* out;            // rows x out_ld; direction d writes columns [d*64, d*64+64)
     int64_t out_ld;
     const float* whh;      // [ndir][256 (j*4+q)][64]
-    float* h_state;        // carried state (read at start, written at end) or null;
+    float* h_state;        // carried state (read at start, written at end) or null; one direction only (ndir == 1):
     float* c_state;        //   element (seq, j) at (seq/inner_count)*hc_outer_stride + (seq%inner_count)*64 + j
     int64_t hc_outer_stride;
     int nseq, L;
@@ -374,8 +374,14 @@ inline cudaError_t configure_lstm() {
     return e;
 }
 
+// the state slot of a sequence has no direction term: a bidirectional call with carried state would have both
+// directions read and write the same (h, c)
+inline bool lstm_state_ok(const LstmArgs& a) {
+    return (a.ndir == 1 || a.ndir == 2) && (a.h_state == nullptr || a.ndir == 1) && ((a.h_state == nullptr) == (a.c_state == nullptr));
+}
+
 inline cudaError_t launch_lstm_rec(const LstmArgs& a, cudaStream_t st, bool pdl = false) {
-    if (a.nseq <= 0 || a.L <= 0) return cudaErrorInvalidValue;
+    if (a.nseq <= 0 || a.L <= 0 || !lstm_state_ok(a)) return cudaErrorInvalidValue;
     const int ctas1 = a.nseq * a.ndir;
     if (ctas1 <= NUM_SMS && (size_t)a.L * 1024 <= 200 * 1024)      // latency mode: one sequence per CTA, preloaded
         return launch_k(pdl, lstm_rec3_kernel<1, true>, dim3(a.nseq, a.ndir), dim3(128), (size_t)a.L * 1024, st, a);

@@ -4,7 +4,8 @@
 // Per step and direction the recurrent product is gates^T[256 x NS] = W_hh[256 x 64] . h^T[64 x NS]: "swap-AB" --
 // the 256 gate rows are the MMA's M dimension (four M = 64 wgmma tiles, W_hh bf16 hi/lo resident in shared memory for
 // the CTA's whole life), the CTA's NS = 32 sequences are its N dimension.  Products are bf16x3 split
-// (W_hi h_hi + W_lo h_hi + W_hi h_lo; `passes` = 2 drops the W_lo term for the bf16 configuration), accumulators in the
+// (W_hi h_hi + W_lo h_hi + W_hi h_lo; `passes` = 2 drops the W_lo term for the bf16 configuration, `passes` = 1 keeps
+// only W_hi h_hi: plain bf16), accumulators in the
 // registers of the CTA's single warpgroup.  A step:
 //   1. wgmma of the four gate tiles (48 MMAs of N = 32); meanwhile the input projection gx of this step is in flight
 //      (loaded at the end of the previous step; coalesced float4: the four gates of a unit are adjacent columns);
@@ -218,6 +219,7 @@ tc_lstm_kernel(const LstmXArgs xa, int passes) {
                 const unsigned long long b_hi = umma::smem_desc(bb, 16, 1024), b_lo = umma::smem_desc(bb + NS * 128, 16, 1024);
                 for (int ps = 0; ps < 3; ++ps) {
                     if (ps == 1 && passes < 3) continue;            // W_lo term only for the fp32-grade split
+                    if (ps == 2 && passes < 2) continue;            // h_lo / x_lo term: not for plain bf16
                     const unsigned long long da = (ps == 1) ? w_lo : w_hi, db = (ps == 2) ? b_lo : b_hi;
 #pragma unroll
                     for (unsigned kk = 0; kk < 4; ++kk)
@@ -279,7 +281,7 @@ static inline cudaError_t configure_tc_lstm() {
 }
 // ... with the input projection (and its LayerNorm) inside
 static inline cudaError_t launch_tc_lstm_x(const tcl::LstmXArgs& xa, int passes, cudaStream_t st, bool pdl = false) {
-    if (xa.l.nseq <= 0 || xa.l.L <= 0) return cudaErrorInvalidValue;
+    if (xa.l.nseq <= 0 || xa.l.L <= 0 || !lstm_state_ok(xa.l) || passes < 1 || passes > 3) return cudaErrorInvalidValue;
     if ((xa.x_ld & 3) != 0 || (reinterpret_cast<uintptr_t>(xa.x) & 15) != 0 || (reinterpret_cast<uintptr_t>(xa.bias) & 15) != 0)
         return cudaErrorInvalidValue;
     dim3 grid((xa.l.nseq + tcl::NS - 1) / tcl::NS, xa.l.ndir);
@@ -287,7 +289,7 @@ static inline cudaError_t launch_tc_lstm_x(const tcl::LstmXArgs& xa, int passes,
 }
 // many sequences: the recurrence on the tensor cores
 static inline cudaError_t launch_tc_lstm(const LstmArgs& a, int passes, cudaStream_t st, bool pdl = false) {
-    if (a.nseq <= 0 || a.L <= 0) return cudaErrorInvalidValue;
+    if (a.nseq <= 0 || a.L <= 0 || !lstm_state_ok(a) || passes < 1 || passes > 3) return cudaErrorInvalidValue;
     if ((a.gx_ld & 3) != 0 || (reinterpret_cast<uintptr_t>(a.gx) & 15) != 0) return cudaErrorInvalidValue;   // float4 gate loads
     tcl::LstmXArgs xa{};
     xa.l = a;

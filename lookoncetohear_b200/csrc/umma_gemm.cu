@@ -95,17 +95,11 @@ inline Plan plan_for(const GemmDesc& g, int BN) {
     return pl;
 }
 
-cudaError_t launch(const GemmDesc& g, cudaStream_t st, std::string* why) {
-    auto bad = [&](const char* m) { if (why) *why = m; return cudaErrorInvalidValue; };
-    if (g.n_chunks <= 0 || g.n_chunks > MAX_CHUNKS) return bad("k-chunk count");
-    if (g.N <= 0 || g.rows_per_seq <= 0 || g.nseq <= 0) return bad("empty problem");
-    if (g.passes < 1 || g.passes > 3) return bad("passes must be 1, 2 or 3");
-    cudaError_t e = configure();
-    if (e != cudaSuccess) return e;
-    Params p;
-    memset(&p, 0, sizeof(p));
-    memcpy(p.chunks, g.chunks, sizeof(KChunk) * g.n_chunks);
-    p.n_chunks = g.n_chunks;
+// what launch() decides before it encodes the tensor maps: tile shape, shared-memory plan, persistent grid, epilogue width
+struct LaunchPlan { Plan pl; int P_TILE, S_TILE, n_tiles_n, grid, vec_ok; long long m_tiles; };
+
+// null, or why the problem cannot be launched
+inline const char* plan_launch(const GemmDesc& g, LaunchPlan& L) {
     {   // rows per tile = P_TILE positions x S_TILE sequences: pick the shape that wastes the fewest of the 128 rows
         const bool flat = g.a0.n_outer == 1 && (!g.a1.base || g.a1.n_outer == 1) && !g.b_by_seq;
         const int cand[3][2] = {{BM, 1}, {std::min(g.rows_per_seq, BM), std::max(1, BM / std::max(1, std::min(g.rows_per_seq, BM)))}, {1, BM}};
@@ -115,16 +109,51 @@ cudaError_t launch(const GemmDesc& g, cudaStream_t st, std::string* why) {
             if (S > 1 && !flat) continue;
             const long long pt = (g.rows_per_seq + P - 1) / P, stl = (g.nseq + S - 1) / S;
             const double eff = (double)g.rows_per_seq * g.nseq / ((double)pt * stl * BM);
-            if (eff > best + 1e-9) { best = eff; p.P_TILE = P; p.S_TILE = S; }
+            if (eff > best + 1e-9) { best = eff; L.P_TILE = P; L.S_TILE = S; }
         }
     }
+    Plan pl = plan_for(g, pick_bn(g.N));
+    if ((!pl.ok || (!pl.resident && pl.nop < 2)) && pl.BN > 64) pl = plan_for(g, 64);   // keep two operand slots
+    if (!pl.ok) return "operand tile does not fit shared memory";
+    L.pl = pl;
+    L.n_tiles_n = (g.N + pl.BN - 1) / pl.BN;
+    const int p_tiles = (g.rows_per_seq + L.P_TILE - 1) / L.P_TILE, s_tiles = (g.nseq + L.S_TILE - 1) / L.S_TILE;
+    L.m_tiles = (long long)p_tiles * s_tiles;
+    if (L.m_tiles * L.n_tiles_n > 0x7fffffff) return "too many tiles";
+    // persistent grid: `groups` CTAs per column tile, every group member gets the same number of row tiles (+-1)
+    const int sms = sm_count();
+    long long groups = std::max(1, sms / L.n_tiles_n);
+    groups = std::min(groups, L.m_tiles);
+    const long long per = (L.m_tiles + groups - 1) / groups;
+    groups = (L.m_tiles + per - 1) / per;
+    L.grid = (int)groups * L.n_tiles_n;
+    // float4 epilogue accesses: C / R rows and the per-column operands 16-byte aligned
+    L.vec_ok = (g.ldc % 4 == 0 && g.c_seq_stride % 4 == 0 && g.c_inner_stride % 4 == 0 && (reinterpret_cast<uintptr_t>(g.C) & 15) == 0 &&
+                (reinterpret_cast<uintptr_t>(g.R) & 15) == 0 && (reinterpret_cast<uintptr_t>(g.bias) & 15) == 0 &&
+                (reinterpret_cast<uintptr_t>(g.prelu_vec) & 15) == 0) ? 1 : 0;
+    return nullptr;
+}
+
+cudaError_t launch(const GemmDesc& g, cudaStream_t st, std::string* why) {
+    auto bad = [&](const char* m) { if (why) *why = m; return cudaErrorInvalidValue; };
+    if (g.n_chunks <= 0 || g.n_chunks > MAX_CHUNKS) return bad("k-chunk count");
+    if (g.N <= 0 || g.rows_per_seq <= 0 || g.nseq <= 0) return bad("empty problem");
+    if (g.passes < 1 || g.passes > 3) return bad("passes must be 1, 2 or 3");
+    if (g.prelu && g.prelu_vec) return bad("scalar and vector PReLU slopes are exclusive");
+    LaunchPlan lp;
+    if (const char* m = plan_launch(g, lp)) return bad(m);
+    const Plan& pl = lp.pl;
+    cudaError_t e = configure();
+    if (e != cudaSuccess) return e;
+    Params p;
+    memset(&p, 0, sizeof(p));
+    memcpy(p.chunks, g.chunks, sizeof(KChunk) * g.n_chunks);
+    p.n_chunks = g.n_chunks;
+    p.P_TILE = lp.P_TILE; p.S_TILE = lp.S_TILE;
     p.rows_per_seq = g.rows_per_seq; p.nseq = g.nseq;
     p.seq_inner = (int)g.a0.n_inner;
     p.pos_bias = g.pos_bias;
-    Plan pl = plan_for(g, pick_bn(g.N));
-    if ((!pl.ok || (!pl.resident && pl.nop < 2)) && pl.BN > 64) pl = plan_for(g, 64);   // keep two operand slots
-    if (!pl.ok) return bad("operand tile does not fit shared memory");
-    p.N = g.N; p.BN = pl.BN; p.n_tiles_n = (g.N + p.BN - 1) / p.BN;
+    p.N = g.N; p.BN = pl.BN; p.n_tiles_n = lp.n_tiles_n;
     p.passes = g.passes; p.b_mn_major = g.b.mn_major ? 1 : 0; p.b_by_seq = g.b_by_seq ? 1 : 0;
     p.b_resident = pl.resident; p.nstg = pl.nstg; p.nop = pl.nop;
     const size_t smem = pl.smem;
@@ -157,19 +186,8 @@ cudaError_t launch(const GemmDesc& g, cudaStream_t st, std::string* why) {
     }
     p.C = g.C; p.R = g.R; p.ldc = g.ldc; p.c_seq_stride = g.c_seq_stride; p.c_inner_stride = g.c_inner_stride; p.c_inner = g.c_inner;
     p.bias = g.bias; p.prelu = g.prelu; p.prelu_vec = g.prelu_vec; p.ln_g = g.ln_g; p.ln_b = g.ln_b; p.alpha = g.alpha;
-    p.vec_ok = (g.ldc % 4 == 0 && g.c_seq_stride % 4 == 0 && g.c_inner_stride % 4 == 0 && (reinterpret_cast<uintptr_t>(g.C) & 15) == 0 &&
-                (reinterpret_cast<uintptr_t>(g.R) & 15) == 0 && (reinterpret_cast<uintptr_t>(g.bias) & 15) == 0 &&
-                (reinterpret_cast<uintptr_t>(g.prelu_vec) & 15) == 0) ? 1 : 0;
-    const int p_tiles = (p.rows_per_seq + p.P_TILE - 1) / p.P_TILE, s_tiles = (p.nseq + p.S_TILE - 1) / p.S_TILE;
-    const long long m_tiles = (long long)p_tiles * s_tiles;
-    if (m_tiles * p.n_tiles_n > 0x7fffffff) return bad("too many tiles");
-    // persistent grid: `groups` CTAs per column tile, every group member gets the same number of row tiles (+-1)
-    const int sms = sm_count();
-    long long groups = std::max(1, sms / p.n_tiles_n);
-    groups = std::min(groups, m_tiles);
-    const long long per = (m_tiles + groups - 1) / groups;
-    groups = (m_tiles + per - 1) / per;
-    const int grid = (int)groups * p.n_tiles_n;
+    p.vec_ok = lp.vec_ok;
+    const int grid = lp.grid;
     ++g_launches;
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(grid); cfg.blockDim = dim3(NTHREADS); cfg.dynamicSmemBytes = smem; cfg.stream = st;

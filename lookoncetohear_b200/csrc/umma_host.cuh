@@ -45,8 +45,8 @@ struct GemmDesc {
     int64_t ldc = 0, c_seq_stride = 0, c_inner_stride = 0;
     int c_inner = 0;
     const float* bias = nullptr;
-    const float* prelu = nullptr;
-    const float* prelu_vec = nullptr;
+    const float* prelu = nullptr;     // scalar PReLU slope, or
+    const float* prelu_vec = nullptr; // one slope per column (at most one of the two)
     const float* ln_g = nullptr;
     const float* ln_b = nullptr;
     float alpha = 1.f;

@@ -85,7 +85,8 @@ class EmbedTFGridNet(nn.Module):
         return d
 
     def set_option(self, name, value):
-        """"bf16": 1 = plain bf16 tensor-core operands (one MMA pass), 0 = bf16x3 split products (default, fp32-grade)."""
+        """"bf16": 0 = bf16x3 split products (default, fp32-grade), 1 = bf16 weights x split activations (two MMA passes),
+        2 = plain bf16 tensor-core operands (one MMA pass)."""
         _cabi.check(_cabi.lib().l2h_embed_set_option(self._engine(), name.encode(), int(value)))
 
     def __del__(self):

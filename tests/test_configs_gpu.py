@@ -187,3 +187,48 @@ def test_fused_input_projection_recurrence_option(sep, dev):
     assert rs.rel_l2(y1, y0) < 1e-4
     for b in (0, 19):
         assert rs.rel_l2(y1[b:b + 1], rs.sep_forward(sd, x[b:b + 1], e[b:b + 1])) <= 1e-3
+
+
+def _flat_state(ref):
+    out = {}
+    for k, v in ref.items():
+        if isinstance(v, dict):
+            out.update({f"{k}.{kk}": vv for kk, vv in _flat_state(v).items()})
+        else:
+            out[k] = v
+    return out
+
+
+@pytest.mark.parametrize("fuse_ih", [0, 1])
+@pytest.mark.parametrize("chunks_per_call", [2, 5])
+def test_tensor_core_recurrence_with_carried_state(sep, dev, chunks_per_call, fuse_ih):
+    """Streaming calls of several hops run the inter LSTM over T > 1 steps with the (h, c) carried in the state.  With
+    option "tc_lstm_min" = 1 that recurrence (and the intra one) runs on the tensor cores (tc_lstm_kernel, or with
+    "fuse_ih" tc_lstm_x_kernel) even for 3 streams: output and final state must match the CUDA-core recurrences and the
+    oracle."""
+    net, sd = sep
+    B = 3
+    x, _ = synth.mixture(B, 128 * 20, seed0=2600)
+    e = synth.embedding(B, seed0=2700)
+    xd, ed = x.to(dev), e[:, 0].to(dev)
+    with torch.no_grad():
+        st0 = net.init_buffers(B, dev)
+        y0 = net.stream_dev(xd, ed, chunks_per_call=chunks_per_call, state=st0).cpu()
+        s0 = _flat_state(st0.to_reference())
+        net.set_option("tc_lstm_min", 1)
+        net.set_option("fuse_ih", fuse_ih)
+        try:
+            st1 = net.init_buffers(B, dev)
+            y1 = net.stream_dev(xd, ed, chunks_per_call=chunks_per_call, state=st1).cpu()
+            s1 = _flat_state(st1.to_reference())
+        finally:
+            net.set_option("tc_lstm_min", 4096)
+            net.set_option("fuse_ih", 0)
+    assert rs.rel_l2(y1, y0) < 1e-4
+    for k in s0:
+        if s0[k].abs().max() > 0:
+            assert rs.rel_l2(s1[k].cpu(), s0[k].cpu()) < 1e-4, k
+        else:
+            assert torch.equal(s1[k], s0[k]), k
+    for b in (0, 2):
+        assert rs.rel_l2(y1[b:b + 1], rs.sep_forward(sd, x[b:b + 1], e[b:b + 1])) <= 1e-3
