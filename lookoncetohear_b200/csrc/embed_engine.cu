@@ -6,12 +6,12 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
-#include <functional>
-#include <map>
 #include <string>
 #include <vector>
 
 #include "../../include/lookonce_b200.h"
+#include "host_errors.h"
+#include "weight_pack.h"
 #include "embed_kernels.cuh"
 #include "lstm.cuh"
 #include "umma_host.cuh"
@@ -19,156 +19,106 @@
 
 namespace l2h {
 
-extern thread_local std::string g_err;
-int fail(int code, const std::string& msg);
-#define CK(expr)                                                                                   \
-    do {                                                                                           \
-        cudaError_t _e = (expr);                                                                   \
-        if (_e != cudaSuccess)                                                                     \
-            return fail(3, std::string(#expr) + ": " + cudaGetErrorString(_e));                    \
-    } while (0)
-
 using namespace emb;
-
-struct ESlot {
-    int64_t numel;
-    std::function<void(const float*, float*)> repack;   // (src, packed host base)
-    bool loaded = false;
-    bool accumulate = false;
-    bool ignored = false;
-    int64_t off = 0;
-    std::vector<float> raw;
-};
 
 struct EmbedEngine {
     l2h_embed_config cfg;
     int n_blocks;
-    std::vector<float> host;
-    float* dev = nullptr;
-    int64_t total = 0;
-    std::map<std::string, ESlot> slots;
+    // packed weights; every tensor-core B operand also as bf16 hi/lo planes [2][N][K] (csrc/umma_host.cuh: split_planes)
+    WeightPack pack;
     EmbWeights w;
     std::vector<EmbBlockWeights> bw;
-    bool committed = false;
+    // plane offsets (pack.plane) of the head Linear and, per block, of both W_ih, both ConvTranspose1d and Q|K|V
+    int64_t head_plane = 0;
+    struct BlockPlanes { int64_t ih1, l1, ih2, l2, qkv; };
+    std::vector<BlockPlanes> bplanes;
     int attrs_dev = -1;
-    int device = -1;
-    // bf16 hi/lo planes [2][N][K] of every tensor-core B operand, built on the device at commit from the packed fp32
-    // k-major matrices (csrc/umma_host.cuh: split_planes)
-    struct PlaneSrc { int64_t wt_off; int K, N; int64_t plane_off; };
-    std::vector<PlaneSrc> plane_srcs;
-    __nv_bfloat16* planes = nullptr;
-    int64_t planes_total = 0;
     int passes = 3;                 // 3: bf16x3 split products (fp32-grade), 2: bf16 weights x split activations, 1: plain bf16
 };
 
-static umma::BPlanes wplanes(const EmbedEngine* e, const float* wt, int K, int N) {
-    // the packed matrices were registered in order; look the plane set up by device address
-    const int64_t off = wt - e->dev;
-    for (const auto& ps : e->plane_srcs)
-        if (ps.wt_off == off) {
-            umma::BPlanes b;
-            b.base = e->planes + ps.plane_off; b.ld = K; b.z_stride = 0; b.plane_stride = e->planes_total; b.nz = 1; b.mn_major = false;
-            (void)N;
-            return b;
-        }
-    return umma::BPlanes{};
-}
-
-static inline int perm_row(int p) { return (p & 3) * 64 + (p >> 2); }
-
 static void build_layout(EmbedEngine* e) {
-    int64_t cur = 0;
-    auto alloc = [&](int64_t n) { int64_t o = cur; cur = (cur + n + 3) & ~int64_t(3); return o; };
-    auto& S = e->slots;
-    std::vector<std::pair<const float**, int64_t>> fix;
-    auto bind = [&](const float** f, int64_t off) { fix.push_back({f, off}); };
-    auto plain = [&](const std::string& name, int64_t n) {
-        int64_t o = alloc(n);
-        ESlot s; s.numel = n; s.repack = [o, n](const float* src, float* d) { memcpy(d + o, src, n * sizeof(float)); };
-        S[name] = s;
-        return o;
-    };
-    auto ignored = [&](const std::string& name, int64_t n) {
-        ESlot s; s.numel = n; s.ignored = true; s.repack = [](const float*, float*) {};
-        S[name] = s;
-    };
+    WeightPack& pk = e->pack;
     // DFT table generated here (torch.stft: periodic Hann, onesided, not normalised)
-    const int64_t dft = alloc(NFFT * DFT_LD);
-    bind(&e->w.dft, dft);
-    bind(&e->w.wc, plain("conv.0.weight", 64 * 36));
-    bind(&e->w.bc, plain("conv.0.bias", 64));
-    bind(&e->w.gn_g, plain("conv.1.weight", 64));
-    bind(&e->w.gn_b, plain("conv.1.bias", 64));
-    ignored("deconv.weight", 64 * 2 * 9);
-    ignored("deconv.bias", 2);
+    const int64_t dft = pk.alloc(NFFT * DFT_LD);
+    for (int n = 0; n < NFFT; ++n) {
+        const double win = 0.5 - 0.5 * std::cos(2.0 * M_PI * n / NFFT);
+        for (int k = 0; k < NF; ++k) {
+            const double ang = 2.0 * M_PI * k * n / NFFT;
+            pk.host[dft + n * DFT_LD + k] = (float)(win * std::cos(ang));
+            pk.host[dft + n * DFT_LD + NF + k] = (float)(-win * std::sin(ang));
+        }
+    }
+    pk.bind(&e->w.dft, dft);
+    pk.bind(&e->w.wc, pk.plain("conv.0.weight", 64 * 36));
+    pk.bind(&e->w.bc, pk.plain("conv.0.bias", 64));
+    pk.bind(&e->w.gn_g, pk.plain("conv.1.weight", 64));
+    pk.bind(&e->w.gn_b, pk.plain("conv.1.bias", 64));
+    pk.ignore("deconv.weight", 64 * 2 * 9);
+    pk.ignore("deconv.bias", 2);
     {   // head Linear [256][4160 (c*65+f)] -> [4160 (f*64+c)][256]
-        const int64_t o = alloc((int64_t)FC * 256);
-        ESlot s; s.numel = (int64_t)256 * FC;
-        s.repack = [o](const float* src, float* d) {
+        const int64_t o = pk.alloc((int64_t)FC * 256);
+        pk.repacked("embed_proj.0.weight", (int64_t)256 * FC, [o](const float* src, float* d) {
             for (int n = 0; n < 256; ++n)
                 for (int c = 0; c < CH; ++c)
                     for (int f = 0; f < NF; ++f) d[o + (int64_t)(f * 64 + c) * 256 + n] = src[(int64_t)n * FC + c * NF + f];
-        };
-        S["embed_proj.0.weight"] = s;
-        bind(&e->w.wh_t, o);
+        });
+        pk.bind(&e->w.wh_t, o);
+        e->head_plane = pk.plane(o, FC, 256, FC);
     }
-    bind(&e->w.bh, plain("embed_proj.0.bias", 256));
-    bind(&e->w.lnh_g, plain("embed_proj.1.weight", 256));
-    bind(&e->w.lnh_b, plain("embed_proj.1.bias", 256));
+    pk.bind(&e->w.bh, pk.plain("embed_proj.0.bias", 256));
+    pk.bind(&e->w.lnh_g, pk.plain("embed_proj.1.weight", 256));
+    pk.bind(&e->w.lnh_b, pk.plain("embed_proj.1.bias", 256));
 
     e->bw.resize(e->n_blocks);
+    e->bplanes.resize(e->n_blocks);
     for (int b = 0; b < e->n_blocks; ++b) {
         EmbBlockWeights& W = e->bw[b];
+        EmbedEngine::BlockPlanes& PL = e->bplanes[b];
         const std::string B = "blocks." + std::to_string(b) + ".";
         auto rnn = [&](const std::string& nm, const float** ln_g, const float** ln_b, const float** wih, const float** bb,
-                       const float** whh, const float** wl, const float** bl) {
-            bind(ln_g, plain(B + nm + "_norm.gamma", 64));
-            bind(ln_b, plain(B + nm + "_norm.beta", 64));
-            const int64_t o_ih = alloc(256 * 512), o_b = alloc(512), o_hh = alloc(2 * 256 * 64);
+                       const float** whh, const float** wl, const float** bl, int64_t& p_ih, int64_t& p_l) {
+            pk.bind(ln_g, pk.plain(B + nm + "_norm.gamma", 64));
+            pk.bind(ln_b, pk.plain(B + nm + "_norm.beta", 64));
+            const int64_t o_ih = pk.alloc(256 * 512), o_b = pk.alloc(512), o_hh = pk.alloc(2 * 256 * 64);
             for (int dir = 0; dir < 2; ++dir) {
                 const std::string sfx = dir ? "_reverse" : "";
-                ESlot s; s.numel = 256 * 256;
-                s.repack = [o_ih, dir](const float* src, float* d) {   // [256 rows][256 = c*4+k] -> [k*64+c][dir*256+p]
-                    for (int p = 0; p < 256; ++p) {
+                pk.repacked(B + nm + "_rnn.weight_ih_l0" + sfx, 256 * 256, [o_ih, dir](const float* src, float* d) {
+                    for (int p = 0; p < 256; ++p) {     // [256 rows][256 = c*4+k] -> [k*64+c][dir*256+p]
                         const int r = perm_row(p);
                         for (int c = 0; c < 64; ++c)
                             for (int k = 0; k < 4; ++k)
                                 d[o_ih + (int64_t)(k * 64 + c) * 512 + dir * 256 + p] = src[(int64_t)r * 256 + c * 4 + k];
                     }
-                };
-                S[B + nm + "_rnn.weight_ih_l0" + sfx] = s;
-                ESlot h; h.numel = 256 * 64;
-                h.repack = [o_hh, dir](const float* src, float* d) {
+                });
+                pk.repacked(B + nm + "_rnn.weight_hh_l0" + sfx, 256 * 64, [o_hh, dir](const float* src, float* d) {
                     for (int p = 0; p < 256; ++p)
                         memcpy(d + o_hh + (int64_t)(dir * 256 + p) * 64, src + perm_row(p) * 64, 64 * sizeof(float));
-                };
-                S[B + nm + "_rnn.weight_hh_l0" + sfx] = h;
-                for (const char* bn : {"_rnn.bias_ih_l0", "_rnn.bias_hh_l0"}) {
-                    ESlot bs; bs.numel = 256; bs.accumulate = true; bs.off = o_b + dir * 256;
-                    const int64_t ob = o_b + dir * 256;
-                    bs.repack = [ob](const float* src, float* d) { for (int p = 0; p < 256; ++p) d[ob + p] += src[perm_row(p)]; };
-                    S[B + nm + bn + sfx] = bs;
-                }
+                });
+                const int64_t ob = o_b + dir * 256;
+                for (const char* bn : {"_rnn.bias_ih_l0", "_rnn.bias_hh_l0"})
+                    pk.accumulate(B + nm + bn + sfx, ob, 256, [ob](const float* src, float* d) {
+                        for (int p = 0; p < 256; ++p) d[ob + p] += src[perm_row(p)];
+                    });
             }
-            bind(wih, o_ih); bind(bb, o_b); bind(whh, o_hh);
+            pk.bind(wih, o_ih); pk.bind(bb, o_b); pk.bind(whh, o_hh);
+            p_ih = pk.plane(o_ih, 256, 512, 256);
             {   // ConvTranspose1d weight [128 h][64 c][4 k] -> [(kk*128+h)][c] with k = 3-kk
-                const int64_t o = alloc(512 * 64);
-                ESlot s; s.numel = 128 * 64 * 4;
-                s.repack = [o](const float* src, float* d) {
+                const int64_t o = pk.alloc(512 * 64);
+                pk.repacked(B + nm + "_linear.weight", 128 * 64 * 4, [o](const float* src, float* d) {
                     for (int kk = 0; kk < 4; ++kk)
                         for (int h = 0; h < 128; ++h)
                             for (int c = 0; c < 64; ++c) d[o + (int64_t)(kk * 128 + h) * 64 + c] = src[((int64_t)h * 64 + c) * 4 + (3 - kk)];
-                };
-                S[B + nm + "_linear.weight"] = s;
-                bind(wl, o);
+                });
+                pk.bind(wl, o);
+                p_l = pk.plane(o, 512, 64, 512);
             }
-            bind(bl, plain(B + nm + "_linear.bias", 64));
+            pk.bind(bl, pk.plain(B + nm + "_linear.bias", 64));
         };
-        rnn("intra", &W.ln1_g, &W.ln1_b, &W.wih1_t, &W.b1, &W.whh1, &W.wl1_t, &W.bl1);
-        rnn("inter", &W.ln2_g, &W.ln2_b, &W.wih2_t, &W.b2, &W.whh2, &W.wl2_t, &W.bl2);
-        const int64_t wqkv = alloc(64 * NQKV), bqkv = alloc(NQKV), sl = alloc(NQKV);
-        const int64_t gq = alloc(NH * QK), bq = alloc(NH * QK), gk = alloc(NH * QK), bk = alloc(NH * QK);
-        const int64_t gv = alloc(NH * VDIM), bv = alloc(NH * VDIM);
+        rnn("intra", &W.ln1_g, &W.ln1_b, &W.wih1_t, &W.b1, &W.whh1, &W.wl1_t, &W.bl1, PL.ih1, PL.l1);
+        rnn("inter", &W.ln2_g, &W.ln2_b, &W.wih2_t, &W.b2, &W.whh2, &W.wl2_t, &W.bl2, PL.ih2, PL.l2);
+        const int64_t wqkv = pk.alloc(64 * NQKV), bqkv = pk.alloc(NQKV), sl = pk.alloc(NQKV);
+        const int64_t gq = pk.alloc(NH * QK), bq = pk.alloc(NH * QK), gk = pk.alloc(NH * QK), bk = pk.alloc(NH * QK);
+        const int64_t gv = pk.alloc(NH * VDIM), bv = pk.alloc(NH * VDIM);
         for (int h = 0; h < NH; ++h) {
             struct Br { const char* nm; int d; int col0; int64_t g; int64_t bt; };
             const Br brs[3] = {{"attn_conv_Q_", QE, h * QE, gq, bq}, {"attn_conv_K_", QE, 32 + h * QE, gk, bk},
@@ -176,90 +126,43 @@ static void build_layout(EmbedEngine* e) {
             for (const Br& br : brs) {
                 const std::string M = B + br.nm + std::to_string(h);
                 const int d = br.d, col0 = br.col0;
-                ESlot ws; ws.numel = d * 64;
-                ws.repack = [wqkv, d, col0](const float* src, float* dd) {
+                pk.repacked(M + ".0.weight", d * 64, [wqkv, d, col0](const float* src, float* dd) {
                     for (int r = 0; r < d; ++r)
                         for (int k = 0; k < 64; ++k) dd[wqkv + (int64_t)k * NQKV + col0 + r] = src[r * 64 + k];
-                };
-                S[M + ".0.weight"] = ws;
-                ESlot bs; bs.numel = d;
-                bs.repack = [bqkv, d, col0](const float* src, float* dd) { memcpy(dd + bqkv + col0, src, d * sizeof(float)); };
-                S[M + ".0.bias"] = bs;
-                ESlot ps; ps.numel = 1;
-                ps.repack = [sl, d, col0](const float* src, float* dd) { for (int r = 0; r < d; ++r) dd[sl + col0 + r] = src[0]; };
-                S[M + ".1.weight"] = ps;
+                });
+                pk.repacked(M + ".0.bias", d, [bqkv, d, col0](const float* src, float* dd) { memcpy(dd + bqkv + col0, src, d * sizeof(float)); });
+                pk.repacked(M + ".1.weight", 1, [sl, d, col0](const float* src, float* dd) { for (int r = 0; r < d; ++r) dd[sl + col0 + r] = src[0]; });
                 // gamma/beta [1][d][1][65] -> per head [(f*d + e)]
                 for (int gb = 0; gb < 2; ++gb) {
                     const int64_t base = (gb == 0 ? br.g : br.bt) + (int64_t)h * NF * d;
-                    ESlot gs; gs.numel = d * NF;
-                    gs.repack = [base, d](const float* src, float* dd) {
+                    pk.repacked(M + (gb == 0 ? ".2.gamma" : ".2.beta"), d * NF, [base, d](const float* src, float* dd) {
                         for (int e2 = 0; e2 < d; ++e2)
                             for (int f = 0; f < NF; ++f) dd[base + f * d + e2] = src[e2 * NF + f];
-                    };
-                    S[M + (gb == 0 ? ".2.gamma" : ".2.beta")] = gs;
+                    });
                 }
             }
         }
-        bind(&W.wqkv_t, wqkv); bind(&W.bqkv, bqkv); bind(&W.slope_qkv, sl);
-        bind(&W.gq, gq); bind(&W.bq, bq); bind(&W.gk, gk); bind(&W.bk, bk); bind(&W.gv, gv); bind(&W.bv, bv);
+        pk.bind(&W.wqkv_t, wqkv); pk.bind(&W.bqkv, bqkv); pk.bind(&W.slope_qkv, sl);
+        pk.bind(&W.gq, gq); pk.bind(&W.bq, bq); pk.bind(&W.gk, gk); pk.bind(&W.bk, bk); pk.bind(&W.gv, gv); pk.bind(&W.bv, bv);
+        PL.qkv = pk.plane(wqkv, 64, NQKV, 64);
         {   // concat proj [64][64][1][1] -> [k][n]
-            const int64_t o = alloc(64 * 64);
-            ESlot s; s.numel = 64 * 64;
-            s.repack = [o](const float* src, float* d) {
+            const int64_t o = pk.alloc(64 * 64);
+            pk.repacked(B + "attn_concat_proj.0.weight", 64 * 64, [o](const float* src, float* d) {
                 for (int n = 0; n < 64; ++n)
                     for (int k = 0; k < 64; ++k) d[o + (int64_t)k * 64 + n] = src[n * 64 + k];
-            };
-            S[B + "attn_concat_proj.0.weight"] = s;
-            bind(&W.wp_t, o);
+            });
+            pk.bind(&W.wp_t, o);
         }
-        bind(&W.bp, plain(B + "attn_concat_proj.0.bias", 64));
-        bind(&W.slope_p, plain(B + "attn_concat_proj.1.weight", 1));
+        pk.bind(&W.bp, pk.plain(B + "attn_concat_proj.0.bias", 64));
+        pk.bind(&W.slope_p, pk.plain(B + "attn_concat_proj.1.weight", 1));
         for (int gb = 0; gb < 2; ++gb) {   // [1][64][1][65] -> (f*64 + c)
-            const int64_t o = alloc(FC);
-            ESlot s; s.numel = FC;
-            s.repack = [o](const float* src, float* d) {
+            const int64_t o = pk.alloc(FC);
+            pk.repacked(B + (gb == 0 ? "attn_concat_proj.2.gamma" : "attn_concat_proj.2.beta"), FC, [o](const float* src, float* d) {
                 for (int c = 0; c < CH; ++c)
                     for (int f = 0; f < NF; ++f) d[o + f * 64 + c] = src[c * NF + f];
-            };
-            S[B + (gb == 0 ? "attn_concat_proj.2.gamma" : "attn_concat_proj.2.beta")] = s;
-            bind(gb == 0 ? &W.gp : &W.bpn, o);
+            });
+            pk.bind(gb == 0 ? &W.gp : &W.bpn, o);
         }
-    }
-    e->total = cur;
-    e->host.assign(cur, 0.f);
-    {   // tensor-core B operands (offsets are still offsets here)
-        int64_t pc = 0;
-        auto reg = [&](const float* field, int K, int N) {
-            e->plane_srcs.push_back({reinterpret_cast<int64_t>(field), K, N, pc});
-            pc += ((int64_t)K * N + 63) & ~int64_t(63);
-        };
-        for (auto& f : fix) *f.first = reinterpret_cast<const float*>(f.second);      // stash offsets first
-        reg(e->w.wh_t, FC, 256);
-        for (auto& W : e->bw) {
-            reg(W.wih1_t, 256, 512); reg(W.wl1_t, 512, 64); reg(W.wih2_t, 256, 512); reg(W.wl2_t, 512, 64); reg(W.wqkv_t, 64, NQKV);
-        }
-        e->planes_total = pc;
-    }
-    for (int n = 0; n < NFFT; ++n) {
-        const double win = 0.5 - 0.5 * std::cos(2.0 * M_PI * n / NFFT);
-        for (int k = 0; k < NF; ++k) {
-            const double ang = 2.0 * M_PI * k * n / NFFT;
-            e->host[dft + n * DFT_LD + k] = (float)(win * std::cos(ang));
-            e->host[dft + n * DFT_LD + NF + k] = (float)(-win * std::sin(ang));
-        }
-    }
-    for (auto& f : fix) *f.first = reinterpret_cast<const float*>(f.second);
-}
-
-static void resolve(EmbedEngine* e) {
-    auto fx = [&](const float*& p) { p = e->dev + reinterpret_cast<int64_t>(p); };
-    EmbWeights& w = e->w;
-    fx(w.dft); fx(w.wc); fx(w.bc); fx(w.gn_g); fx(w.gn_b); fx(w.wh_t); fx(w.bh); fx(w.lnh_g); fx(w.lnh_b);
-    for (auto& W : e->bw) {
-        fx(W.ln1_g); fx(W.ln1_b); fx(W.wih1_t); fx(W.b1); fx(W.whh1); fx(W.wl1_t); fx(W.bl1);
-        fx(W.ln2_g); fx(W.ln2_b); fx(W.wih2_t); fx(W.b2); fx(W.whh2); fx(W.wl2_t); fx(W.bl2);
-        fx(W.wqkv_t); fx(W.bqkv); fx(W.slope_qkv); fx(W.gq); fx(W.bq); fx(W.gk); fx(W.bk); fx(W.gv); fx(W.bv);
-        fx(W.wp_t); fx(W.bp); fx(W.slope_p); fx(W.gp); fx(W.bpn);
     }
 }
 
@@ -299,7 +202,7 @@ static EWs ecarve(int B, int N) {
 
 static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B, int N, float* wsp, size_t ws_bytes,
                               cudaStream_t st) {
-    if (!e->committed) return fail(4, "weights not committed");
+    if (!e->pack.committed) return fail(4, "weights not committed");
     if (B <= 0 || N < NFFT) return fail(1, "need batch >= 1 and at least 128 samples");
     const EWs ws = ecarve(B, N);
     if ((size_t)ws.total * sizeof(float) > ws_bytes) return fail(1, "workspace too small");
@@ -309,9 +212,10 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
     if (rows * 2 > 0x7fffffff) return fail(1, "batch too large for one call; split it (l2h_embed_max_batch)");
     int cur_dev = -1;
     CK(cudaGetDevice(&cur_dev));
-    if (cur_dev != e->device)
-        return fail(1, "this handle's weights live on device " + std::to_string(e->device) + ", device " + std::to_string(cur_dev) +
-                       " is current: commit the weights again there (EmbedTFGridNet.to(device) does)");
+    if (cur_dev != e->pack.device)
+        return fail(1, "this handle's weights live on device " + std::to_string(e->pack.device) + " but device " + std::to_string(cur_dev) +
+                       " is current: commit the weights again with the new device current (EmbedTFGridNet.to(device) does), or use one "
+                       "handle per device");
     if (e->attrs_dev != cur_dev) {
         CK(configure_lstm());
         CK(configure_tc_lstm());
@@ -328,6 +232,7 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
     const int Z = B * NH;
     const int64_t k_plane = (int64_t)Z * Tp * QK, v_plane = (int64_t)Z * Tp * VDIM;
     const int passes = e->passes;
+    const WeightPack& pk = e->pack;
 
     estd_kernel<<<B, 256, 0, st>>>(x, (int64_t)2 * N, INV);
     CK(cudaGetLastError());
@@ -342,6 +247,7 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
 
     for (int blk = 0; blk < e->n_blocks; ++blk) {
         const EmbBlockWeights& W = e->bw[blk];
+        const EmbedEngine::BlockPlanes& PL = e->bplanes[blk];
         for (int path = 0; path < 2; ++path) {          // 0: intra (along F), 1: inter (along T)
             const bool inter = path == 1;
             const int Ls = inter ? T : NF;               // positions per sequence
@@ -360,7 +266,7 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
             umma::set_window_chunks(g, 64, KS, true);
             g.ln_g = inter ? W.ln2_g : W.ln1_g; g.ln_b = inter ? W.ln2_b : W.ln1_b;
             g.rows_per_seq = steps; g.nseq = nseq;
-            g.b = wplanes(e, inter ? W.wih2_t : W.wih1_t, 256, 512); g.N = 512; g.K = 256; g.passes = passes;
+            g.b = pk.bplanes(inter ? PL.ih2 : PL.ih1, 256); g.N = 512; g.K = 256; g.passes = passes;
             g.bias = inter ? W.b2 : W.b1; g.C = GX; g.ldc = 512; g.c_seq_stride = (int64_t)steps * 512;
             CKU(umma::launch(g, st, &_why));
             LstmArgs l{};
@@ -378,7 +284,7 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
             umma::set_window_chunks(c, 128, KS, false);
             c.pos_bias = -(KS - 1);
             c.rows_per_seq = Ls; c.nseq = nseq;
-            c.b = wplanes(e, inter ? W.wl2_t : W.wl1_t, 512, 64); c.N = 64; c.K = 512; c.passes = passes;
+            c.b = pk.bplanes(inter ? PL.l2 : PL.l1, 512); c.N = 64; c.K = 512; c.passes = passes;
             c.bias = inter ? W.bl2 : W.bl1; c.C = X; c.R = X;
             if (!inter) { c.ldc = 64; c.c_seq_stride = (int64_t)NF * 64; }                 // row ((b,t), f) -> X[b][t][f]
             else { c.ldc = (int64_t)NF * 64; c.c_inner = NF; c.c_seq_stride = (int64_t)T * NF * 64; c.c_inner_stride = 64; }   // ((b,f), t)
@@ -390,7 +296,7 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
             g.a0.base = X; g.a0.channels = 64; g.a0.n_pos = rows; g.a0.pos_stride = 64;
             umma::set_plain_chunks(g, 64);
             g.rows_per_seq = (int)rows; g.nseq = 1;
-            g.b = wplanes(e, W.wqkv_t, 64, NQKV); g.N = NQKV; g.K = 64; g.passes = passes;
+            g.b = pk.bplanes(PL.qkv, 64); g.N = NQKV; g.K = 64; g.passes = passes;
             g.bias = W.bqkv; g.prelu_vec = W.slope_qkv; g.C = QKV; g.ldc = NQKV; g.c_seq_stride = 0;
             CKU(umma::launch(g, st, &_why));
         }
@@ -427,7 +333,7 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
         g.a0.base = X; g.a0.channels = FC; g.a0.n_pos = (int64_t)B * T; g.a0.pos_stride = FC;
         umma::set_plain_chunks(g, FC);
         g.rows_per_seq = B * T; g.nseq = 1;
-        g.b = wplanes(e, e->w.wh_t, FC, 256); g.N = 256; g.K = FC; g.passes = passes;
+        g.b = pk.bplanes(e->head_plane, FC); g.N = 256; g.K = FC; g.passes = passes;
         g.bias = e->w.bh; g.C = HD; g.ldc = 256;
         CKU(umma::launch(g, st, &_why));
     }
@@ -459,8 +365,7 @@ int l2h_embed_create(const l2h_embed_config* c, void** handle) {
 int l2h_embed_destroy(void* handle) {
     EmbedEngine* e = static_cast<EmbedEngine*>(handle);
     if (!e) return 0;
-    if (e->dev) cudaFree(e->dev);
-    if (e->planes) cudaFree(e->planes);
+    e->pack.release();
     delete e;
     return 0;
 }
@@ -468,54 +373,22 @@ int l2h_embed_destroy(void* handle) {
 int l2h_embed_load_weight(void* handle, const char* name, const float* data, int64_t numel) {
     EmbedEngine* e = static_cast<EmbedEngine*>(handle);
     if (!e || !name || !data) return fail(1, "null argument");
-    auto it = e->slots.find(name);
-    if (it == e->slots.end()) return fail(2, std::string("unknown weight name: ") + name);
-    ESlot& s = it->second;
-    if (numel != s.numel) return fail(1, std::string("wrong element count for ") + name);
-    if (s.accumulate) s.raw.assign(data, data + numel);
-    else s.repack(data, e->host.data());
-    s.loaded = true;
-    e->committed = false;
-    return 0;
+    return e->pack.load(name, data, numel);
 }
 
 int l2h_embed_weights_expected(void* handle, int32_t* n_expected, int32_t* n_loaded) {
     EmbedEngine* e = static_cast<EmbedEngine*>(handle);
     if (!e) return fail(1, "null handle");
-    int n = 0;
-    for (auto& kv : e->slots) n += kv.second.loaded ? 1 : 0;
-    if (n_expected) *n_expected = (int)e->slots.size();
-    if (n_loaded) *n_loaded = n;
+    e->pack.counts(n_expected, n_loaded);
     return 0;
 }
 
+// the handle is bound to the device current here: a commit on another device releases the old buffers and rebuilds them
 int l2h_embed_commit_weights(void* handle, void* stream) {
     EmbedEngine* e = static_cast<EmbedEngine*>(handle);
     if (!e) return fail(1, "null handle");
-    for (auto& kv : e->slots)
-        if (!kv.second.loaded) return fail(4, "weight not loaded: " + kv.first);
-    for (auto& kv : e->slots)
-        if (kv.second.accumulate) std::fill(e->host.begin() + kv.second.off, e->host.begin() + kv.second.off + 256, 0.f);
-    for (auto& kv : e->slots)
-        if (kv.second.accumulate) kv.second.repack(kv.second.raw.data(), e->host.data());
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    int cur = -1;
-    CK(cudaGetDevice(&cur));
-    if (e->dev != nullptr && e->device != cur) return fail(1, "an enrollment handle is bound to the device of its first commit; create one handle per device");
-    const bool first = e->dev == nullptr;
-    if (first) {
-        CK(cudaMalloc(&e->dev, e->total * sizeof(float)));
-        CK(cudaMalloc(&e->planes, 2 * e->planes_total * sizeof(__nv_bfloat16)));
-        e->device = cur;
-    }
-    CK(cudaMemcpyAsync(e->dev, e->host.data(), e->total * sizeof(float), cudaMemcpyHostToDevice, st));
-    for (const auto& ps : e->plane_srcs)        // k-major fp32 [K][N] -> bf16 hi/lo planes [N][K]
-        CK(umma::split_planes(e->dev + ps.wt_off, 1, ps.N, ps.N, ps.K, ps.K, e->planes + ps.plane_off,
-                              e->planes + e->planes_total + ps.plane_off, st));
-    CK(cudaStreamSynchronize(st));
-    if (first) resolve(e);
-    e->committed = true;
-    return 0;
+    if (int rc = e->pack.finish()) return rc;
+    return e->pack.upload(static_cast<cudaStream_t>(stream));
 }
 
 int l2h_embed_set_option(void* handle, const char* name, int32_t value) {

@@ -11,9 +11,9 @@
 #include <string>
 
 #include "../../include/lookonce_b200.h"
+#include "host_errors.h"
 
 namespace l2h {
-int fail(int code, const std::string& msg);
 
 __device__ __forceinline__ double blk_sum(double v, double* red) {
 #pragma unroll

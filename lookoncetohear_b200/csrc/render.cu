@@ -13,10 +13,10 @@
 #include <string>
 
 #include "../../include/lookonce_b200.h"
+#include "host_errors.h"
 #include "common.cuh"
 
 namespace l2h {
-int fail(int code, const std::string& msg);
 
 constexpr int FIR_TILE = 1024, FIR_CHUNK = 256;
 

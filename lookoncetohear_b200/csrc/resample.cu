@@ -24,9 +24,9 @@
 #include <string>
 
 #include "../../include/lookonce_b200.h"
+#include "host_errors.h"
 
 namespace l2h {
-int fail(int code, const std::string& msg);
 
 constexpr int RS_TILE = 256;              // outputs (threads) per CTA
 constexpr int RS_MAX_RATES = 16;          // distinct `orig` per launch

@@ -7,14 +7,14 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <functional>
-#include <iterator>
 #include <map>
 #include <tuple>
 #include <string>
 #include <vector>
 
 #include "../../include/lookonce_b200.h"
+#include "host_errors.h"
+#include "weight_pack.h"
 #include "gemm.cuh"
 #include "umma_host.cuh"
 #include "tc_lstm.cuh"
@@ -30,22 +30,6 @@ int fail(int code, const std::string& msg) {
     g_err = msg;
     return code;
 }
-#define CK(expr)                                                                                   \
-    do {                                                                                           \
-        cudaError_t _e = (expr);                                                                   \
-        if (_e != cudaSuccess)                                                                     \
-            return fail(3, std::string(#expr) + ": " + cudaGetErrorString(_e));                    \
-    } while (0)
-
-struct Slot {
-    int64_t off;    // floats into the packed buffer
-    int64_t numel;  // of the reference tensor
-    // repack(src_host, dst_host_base)
-    std::function<void(const float*, float*)> repack;
-    bool loaded = false;
-    bool accumulate = false;   // LSTM biases: b_ih and b_hh of one direction sum into one destination
-    std::vector<float> raw;    // accumulate slots keep their tensor; the sum is formed at commit
-};
 
 // (sequence, direction) pairs from which the recurrence runs on the tensor cores (tc_lstm: 32 sequences per CTA; CUDA cores:
 // up to 4 per CTA).  The threshold was chosen with an earlier tensor-core recurrence on another GPU and has not been
@@ -55,32 +39,21 @@ constexpr int TCL_MIN_SEQDIRS = 4096;
 struct SepEngine {
     l2h_sep_config cfg;
     int n_blocks;
-    std::vector<float> host;        // staging
-    float* dev = nullptr;           // packed weights
-    int device = -1;                // ordinal of the device that owns `dev`, the streams, events and cached graphs
+    WeightPack pack;                // packed weights; pack.device also owns the streams, events and cached graphs below
     int64_t weight_gen = 0;         // bumped by every commit
     bool graph_stats = false;
-    // tensor-core path: bf16 hi/lo planes [2][N][K] of the GEMM weights, built on the device at commit
-    struct PlaneSrc { int64_t wt_off; int K, N, ld, col0; int64_t plane_off; };
-    std::vector<PlaneSrc> plane_srcs;
-    std::vector<int64_t> plane_of;      // per block: plane offsets of wih1, wl1, wih2, wl2, wqkv, [wih2|whh2], wp
-    std::vector<int64_t> plane_stash;
-    __nv_bfloat16* planes = nullptr;
-    int64_t planes_total = 0;
-    bool cur_pdl = false;               // PDL attribute for the tensor-core launches of the chain being enqueued
+    std::vector<int64_t> plane_of;      // per block: plane offsets (pack.plane) of wih1, wl1, wih2, wl2, wqkv, [wih2|whh2], wp
+    bool cur_pdl = false;              // PDL attribute for the tensor-core launches of the chain being enqueued
     bool fuse_ih = false;               // many sequences: W_ih + LayerNorm inside the tensor-core recurrence (option "fuse_ih", default off)
     bool use_tc = true;                 // rows > TC_MIN_ROWS: dense contractions on the tensor cores, wgmma (option "tensor_cores")
     int tc_passes = 3;                  // 3 = bf16x3 split products (fp32 configs); 2 = bf16 weights x split activations (option
                                         // "bf16" = 1: the offline bf16 configuration); 1 = plain bf16 operands ("bf16" = 2)
-    int64_t total = 0;
-    std::map<std::string, Slot> slots;
     SepWeights w;
     std::vector<BlockWeights> bw;
-    bool committed = false;
     // CUDA-graph cache of whole kernel chains (the T=1 streaming chain is ~30 tiny kernels:
     // launch-bound unless replayed as a graph)
-    std::map<std::vector<int64_t>, cudaGraphExec_t> graphs;
-    std::map<cudaGraphExec_t, int> graph_kernels;   // kernel nodes per cached graph
+    struct CachedGraph { cudaGraphExec_t exec; int kernels; };   // kernels = kernel nodes, for the launch counter
+    std::map<std::vector<int64_t>, CachedGraph> graphs;
     TraceRec* trace_dev = nullptr;                  // device trace buffer (l2h_sep_trace_start)
     int trace_cap = 0;
     int64_t launch_count = 0;                       // kernels launched so far (graph replays counted by their kernel nodes)
@@ -114,179 +87,126 @@ struct SepEngine {
     bool use_pdl = true;     // programmatic dependent launch between the kernels of a chain (option "pdl")
 };
 
-static int64_t align4(int64_t x) { return (x + 3) & ~int64_t(3); }
-
-// gate-row permutation: packed row j*4+q <- reference row q*64+j
-static inline int perm_row(int p) { return (p & 3) * 64 + (p >> 2); }
-
 static void build_layout(SepEngine* e) {
-    int64_t cur = 0;
-    auto alloc = [&](int64_t n) { int64_t o = cur; cur = align4(cur + n); return o; };
-    auto& S = e->slots;
-    auto plain = [&](const std::string& name, int64_t n) {
-        int64_t o = alloc(n);
-        S[name] = Slot{o, n, [o, n](const float* s, float* d) { memcpy(d + o, s, n * sizeof(float)); }};
-        return o;
-    };
+    WeightPack& pk = e->pack;
     auto transposed = [&](const std::string& name, int rows, int cols, int ld_out) {
         // reference [rows][cols] -> packed [cols][ld_out] (k-major)
-        int64_t o = alloc((int64_t)cols * ld_out);
-        S[name] = Slot{o, (int64_t)rows * cols, [o, rows, cols, ld_out](const float* s, float* d) {
+        const int64_t o = pk.alloc((int64_t)cols * ld_out);
+        pk.repacked(name, (int64_t)rows * cols, [o, rows, cols, ld_out](const float* s, float* d) {
             for (int r = 0; r < rows; ++r)
                 for (int c = 0; c < cols; ++c) d[o + (int64_t)c * ld_out + r] = s[(int64_t)r * cols + c];
-        }};
+        });
         return o;
     };
     const std::string P = "tfgridnet.";
-    std::vector<std::pair<const float**, int64_t>> fix;   // pointer fields to resolve after alloc
-    auto bind = [&](const float** field, int64_t off) { fix.push_back({field, off}); };
 
     // STFT filterbanks [194][1][192]
-    bind(&e->w.wat, transposed(P + "enc.filterbank._filters", NROW, NFFT, 196));
-    bind(&e->w.ws, plain(P + "dec.filterbank._filters", (int64_t)NROW * NFFT));
-    bind(&e->w.wc, plain(P + "conv.0.weight", 64 * 36));
-    bind(&e->w.bc, plain(P + "conv.0.bias", 64));
-    bind(&e->w.we, plain(P + "embed_to_feats_proj.0.weight", (int64_t)FC * SPK));
-    bind(&e->w.be, plain(P + "embed_to_feats_proj.0.bias", FC));
-    bind(&e->w.lne_g, plain(P + "embed_to_feats_proj.1.weight", FC));
-    bind(&e->w.lne_b, plain(P + "embed_to_feats_proj.1.bias", FC));
-    bind(&e->w.wd, plain(P + "deconv.weight", 64 * 36));
-    bind(&e->w.bd, plain(P + "deconv.bias", 4));
+    pk.bind(&e->w.wat, transposed(P + "enc.filterbank._filters", NROW, NFFT, 196));
+    pk.bind(&e->w.ws, pk.plain(P + "dec.filterbank._filters", (int64_t)NROW * NFFT));
+    pk.bind(&e->w.wc, pk.plain(P + "conv.0.weight", 64 * 36));
+    pk.bind(&e->w.bc, pk.plain(P + "conv.0.bias", 64));
+    pk.bind(&e->w.we, pk.plain(P + "embed_to_feats_proj.0.weight", (int64_t)FC * SPK));
+    pk.bind(&e->w.be, pk.plain(P + "embed_to_feats_proj.0.bias", FC));
+    pk.bind(&e->w.lne_g, pk.plain(P + "embed_to_feats_proj.1.weight", FC));
+    pk.bind(&e->w.lne_b, pk.plain(P + "embed_to_feats_proj.1.bias", FC));
+    pk.bind(&e->w.wd, pk.plain(P + "deconv.weight", 64 * 36));
+    pk.bind(&e->w.bd, pk.plain(P + "deconv.bias", 4));
 
     e->bw.resize(e->n_blocks);
     for (int b = 0; b < e->n_blocks; ++b) {
         BlockWeights& W = e->bw[b];
         const std::string B = P + "blocks." + std::to_string(b) + ".";
-        bind(&W.ln1_g, plain(B + "intra_norm.norm.weight", 64));
-        bind(&W.ln1_b, plain(B + "intra_norm.norm.bias", 64));
-        bind(&W.ln2_g, plain(B + "inter_norm.norm.weight", 64));
-        bind(&W.ln2_b, plain(B + "inter_norm.norm.bias", 64));
+        pk.bind(&W.ln1_g, pk.plain(B + "intra_norm.norm.weight", 64));
+        pk.bind(&W.ln1_b, pk.plain(B + "intra_norm.norm.bias", 64));
+        pk.bind(&W.ln2_g, pk.plain(B + "inter_norm.norm.weight", 64));
+        pk.bind(&W.ln2_b, pk.plain(B + "inter_norm.norm.bias", 64));
         // LSTM input weights [256][64] -> Wt[k][dirofs + p], p = j*4+q
         auto ih = [&](const std::string& name, int64_t base, int ld, int dirofs) {
-            S[name] = Slot{base, 256 * 64, [base, ld, dirofs](const float* s, float* d) {
+            pk.repacked(name, 256 * 64, [base, ld, dirofs](const float* s, float* d) {
                 for (int p = 0; p < 256; ++p) {
                     const int r = perm_row(p);
                     for (int k = 0; k < 64; ++k) d[base + (int64_t)k * ld + dirofs + p] = s[r * 64 + k];
                 }
-            }};
+            });
         };
         auto hh = [&](const std::string& name, int64_t base) {
-            S[name] = Slot{base, 256 * 64, [base](const float* s, float* d) {
+            pk.repacked(name, 256 * 64, [base](const float* s, float* d) {
                 for (int p = 0; p < 256; ++p) memcpy(d + base + (int64_t)p * 64, s + perm_row(p) * 64, 64 * sizeof(float));
-            }};
+            });
         };
-        auto bias = [&](const std::string& name, int64_t base, bool) {
-            Slot sl{base, 256, [base](const float* s, float* d) {
+        auto bias = [&](const std::string& name, int64_t base) {
+            pk.accumulate(name, base, 256, [base](const float* s, float* d) {
                 for (int p = 0; p < 256; ++p) d[base + p] += s[perm_row(p)];
-            }};
-            sl.accumulate = true;
-            S[name] = sl;
+            });
         };
-        const int64_t wih1 = alloc(64 * 512), b1 = alloc(512), whh1 = alloc(2 * 256 * 64);
+        const int64_t wih1 = pk.alloc(64 * 512), b1 = pk.alloc(512), whh1 = pk.alloc(2 * 256 * 64);
         ih(B + "intra_rnn.weight_ih_l0", wih1, 512, 0);
         ih(B + "intra_rnn.weight_ih_l0_reverse", wih1, 512, 256);
         hh(B + "intra_rnn.weight_hh_l0", whh1);
         hh(B + "intra_rnn.weight_hh_l0_reverse", whh1 + 256 * 64);
-        bias(B + "intra_rnn.bias_ih_l0", b1, true);
-        bias(B + "intra_rnn.bias_hh_l0", b1, true);
-        bias(B + "intra_rnn.bias_ih_l0_reverse", b1 + 256, true);
-        bias(B + "intra_rnn.bias_hh_l0_reverse", b1 + 256, true);
-        bind(&W.wih1_t, wih1); bind(&W.b1, b1); bind(&W.whh1, whh1);
+        bias(B + "intra_rnn.bias_ih_l0", b1);
+        bias(B + "intra_rnn.bias_hh_l0", b1);
+        bias(B + "intra_rnn.bias_ih_l0_reverse", b1 + 256);
+        bias(B + "intra_rnn.bias_hh_l0_reverse", b1 + 256);
+        pk.bind(&W.wih1_t, wih1); pk.bind(&W.b1, b1); pk.bind(&W.whh1, whh1);
         const int64_t wl1 = transposed(B + "intra_linear.weight", 64, 128, 64);
-        bind(&W.wl1_t, wl1);
-        bind(&W.bl1, plain(B + "intra_linear.bias", 64));
-        const int64_t wih2 = alloc(64 * 256), b2 = alloc(256), whh2 = alloc(256 * 64), whh2t = alloc(64 * 256);
+        pk.bind(&W.wl1_t, wl1);
+        pk.bind(&W.bl1, pk.plain(B + "intra_linear.bias", 64));
+        const int64_t wih2 = pk.alloc(64 * 256), b2 = pk.alloc(256), whh2 = pk.alloc(256 * 64), whh2t = pk.alloc(64 * 256);
         ih(B + "inter_rnn.weight_ih_l0", wih2, 256, 0);
-        S[B + "inter_rnn.weight_hh_l0"] = Slot{whh2, 256 * 64, [whh2, whh2t](const float* s, float* d) {
+        pk.repacked(B + "inter_rnn.weight_hh_l0", 256 * 64, [whh2, whh2t](const float* s, float* d) {
             for (int p = 0; p < 256; ++p) {
                 const int r = perm_row(p);
                 memcpy(d + whh2 + (int64_t)p * 64, s + r * 64, 64 * sizeof(float));
                 for (int k = 0; k < 64; ++k) d[whh2t + (int64_t)k * 256 + p] = s[r * 64 + k];
             }
-        }};
-        bind(&W.whh2_t, whh2t);
-        bias(B + "inter_rnn.bias_ih_l0", b2, true);
-        bias(B + "inter_rnn.bias_hh_l0", b2, true);
-        bind(&W.wih2_t, wih2); bind(&W.b2, b2); bind(&W.whh2, whh2);
+        });
+        pk.bind(&W.whh2_t, whh2t);
+        bias(B + "inter_rnn.bias_ih_l0", b2);
+        bias(B + "inter_rnn.bias_hh_l0", b2);
+        pk.bind(&W.wih2_t, wih2); pk.bind(&W.b2, b2); pk.bind(&W.whh2, whh2);
         const int64_t wl2 = transposed(B + "inter_linear.weight", 64, 64, 64);
-        bind(&W.wl2_t, wl2);
-        bind(&W.bl2, plain(B + "inter_linear.bias", 64));
+        pk.bind(&W.wl2_t, wl2);
+        pk.bind(&W.bl2, pk.plain(B + "inter_linear.bias", 64));
         // Q | K | V projections -> one [64][112] k-major matrix
-        const int64_t wqkv = alloc(64 * NQKV), bqkv = alloc(NQKV), slopes = alloc(4);
+        const int64_t wqkv = pk.alloc(64 * NQKV), bqkv = pk.alloc(NQKV), slopes = pk.alloc(4);
         auto proj = [&](const std::string& mod, int rows, int col0, int slope_idx) {
-            S[B + mod + ".0.weight"] = Slot{wqkv, (int64_t)rows * 64, [wqkv, rows, col0](const float* s, float* d) {
+            pk.repacked(B + mod + ".0.weight", (int64_t)rows * 64, [wqkv, rows, col0](const float* s, float* d) {
                 for (int r = 0; r < rows; ++r)
                     for (int k = 0; k < 64; ++k) d[wqkv + (int64_t)k * NQKV + col0 + r] = s[r * 64 + k];
-            }};
-            S[B + mod + ".0.bias"] = Slot{bqkv, rows, [bqkv, rows, col0](const float* s, float* d) {
+            });
+            pk.repacked(B + mod + ".0.bias", rows, [bqkv, rows, col0](const float* s, float* d) {
                 memcpy(d + bqkv + col0, s, rows * sizeof(float));
-            }};
-            S[B + mod + ".1.weight"] = Slot{slopes, 1, [slopes, slope_idx](const float* s, float* d) {
-                d[slopes + slope_idx] = s[0];
-            }};
+            });
+            pk.repacked(B + mod + ".1.weight", 1, [slopes, slope_idx](const float* s, float* d) { d[slopes + slope_idx] = s[0]; });
         };
         proj("attn_conv_Q", NHEAD * QE, 0, 0);
         proj("attn_conv_K", NHEAD * QE, NHEAD * QE, 1);
         proj("attn_conv_V", NHEAD * VD, 2 * NHEAD * QE, 2);
-        bind(&W.wqkv_t, wqkv); bind(&W.bqkv, bqkv); bind(&W.slopes, slopes);
-        const int64_t slope_vec = alloc(NQKV);
-        bind(&W.slope_vec, slope_vec);
-        const int64_t midp = alloc(MID_PACK);
-        bind(&W.mid_pack, midp);
+        pk.bind(&W.wqkv_t, wqkv); pk.bind(&W.bqkv, bqkv); pk.bind(&W.slopes, slopes);
+        const int64_t slope_vec = pk.alloc(NQKV);
+        pk.bind(&W.slope_vec, slope_vec);
+        const int64_t midp = pk.alloc(MID_PACK);
+        pk.bind(&W.mid_pack, midp);
         e->mid_src.push_back({wl1, wih2, whh2t, wl2, wqkv, midp, slopes, slope_vec});
-        {   // tensor-core B operands of this block (offsets into the packed fp32 buffer; planes are made at commit)
-            auto reg = [&](int64_t wt, int K, int N, int ld, int col0, int64_t at) {
-                e->plane_srcs.push_back({wt, K, N, ld, col0, at});
-            };
-            auto take = [&](int K, int N) { const int64_t o = e->planes_total; e->planes_total += ((int64_t)K * N + 63) & ~int64_t(63); return o; };
-            const int64_t p_ih1 = take(64, 512), p_l1 = take(128, 64), p_ih2 = take(64, 256), p_l2 = take(64, 64), p_qkv = take(64, NQKV),
-                          p_cat = take(128, 256);
-            reg(wih1, 64, 512, 64, 0, p_ih1); reg(wl1, 128, 64, 128, 0, p_l1); reg(wih2, 64, 256, 64, 0, p_ih2);
-            reg(wl2, 64, 64, 64, 0, p_l2); reg(wqkv, 64, NQKV, 64, 0, p_qkv);
-            reg(wih2, 64, 256, 128, 0, p_cat); reg(whh2t, 64, 256, 128, 64, p_cat);      // [W_ih | W_hh]: k = [x | h]
-            e->plane_stash = {p_ih1, p_l1, p_ih2, p_l2, p_qkv, p_cat};
-        }
-        bind(&W.lnq_g, plain(B + "attn_conv_Q.3.norm.weight", QK_DIM));
-        bind(&W.lnq_b, plain(B + "attn_conv_Q.3.norm.bias", QK_DIM));
-        bind(&W.lnk_g, plain(B + "attn_conv_K.3.norm.weight", QK_DIM));
-        bind(&W.lnk_b, plain(B + "attn_conv_K.3.norm.bias", QK_DIM));
-        bind(&W.lnv_g, plain(B + "attn_conv_V.3.norm.weight", V_DIM));
-        bind(&W.lnv_b, plain(B + "attn_conv_V.3.norm.bias", V_DIM));
+        pk.bind(&W.lnq_g, pk.plain(B + "attn_conv_Q.3.norm.weight", QK_DIM));
+        pk.bind(&W.lnq_b, pk.plain(B + "attn_conv_Q.3.norm.bias", QK_DIM));
+        pk.bind(&W.lnk_g, pk.plain(B + "attn_conv_K.3.norm.weight", QK_DIM));
+        pk.bind(&W.lnk_b, pk.plain(B + "attn_conv_K.3.norm.bias", QK_DIM));
+        pk.bind(&W.lnv_g, pk.plain(B + "attn_conv_V.3.norm.weight", V_DIM));
+        pk.bind(&W.lnv_b, pk.plain(B + "attn_conv_V.3.norm.bias", V_DIM));
         const int64_t wp = transposed(B + "attn_concat_proj.0.weight", 64, 64, 64);
-        bind(&W.wp_t, wp);
-        {
-            const int64_t p_p = e->planes_total;
-            e->planes_total += 64 * 64;
-            e->plane_srcs.push_back({wp, 64, 64, 64, 0, p_p});
-            for (int64_t v : e->plane_stash) e->plane_of.push_back(v);
-            e->plane_of.push_back(p_p);
-        }
-        bind(&W.bp, plain(B + "attn_concat_proj.0.bias", 64));
-        S[B + "attn_concat_proj.1.weight"] = Slot{slopes, 1, [slopes](const float* s, float* d) { d[slopes + 3] = s[0]; }};
-        bind(&W.lnp_g, plain(B + "attn_concat_proj.3.norm.weight", FC));
-        bind(&W.lnp_b, plain(B + "attn_concat_proj.3.norm.bias", FC));
-    }
-    e->total = cur;
-    e->host.assign(cur, 0.f);
-    // stash offsets in the pointer fields; resolved to device addresses at commit
-    for (auto& f : fix) *f.first = reinterpret_cast<const float*>(f.second);
-}
-
-// pointer fields hold offsets (floats) until the first commit; `base` turns them into device addresses, and a
-// later re-commit on another device shifts them by (new base - old base)
-static void shift_pointers(SepEngine* e, const float* new_base, const float* old_base) {
-    auto fixp = [&](const float*& p) {
-        if (old_base == nullptr) p = new_base + reinterpret_cast<int64_t>(p);      // offset -> address
-        else p = new_base + (p - old_base);                                        // address on the old device -> new one
-    };
-    SepWeights& w = e->w;
-    fixp(w.wat); fixp(w.ws); fixp(w.wc); fixp(w.bc); fixp(w.we); fixp(w.be); fixp(w.lne_g); fixp(w.lne_b);
-    fixp(w.wd); fixp(w.bd);
-    for (auto& W : e->bw) {
-        fixp(W.ln1_g); fixp(W.ln1_b); fixp(W.wih1_t); fixp(W.b1); fixp(W.whh1); fixp(W.wl1_t); fixp(W.bl1);
-        fixp(W.ln2_g); fixp(W.ln2_b); fixp(W.wih2_t); fixp(W.b2); fixp(W.whh2); fixp(W.whh2_t); fixp(W.mid_pack); fixp(W.wl2_t); fixp(W.bl2);
-        fixp(W.wqkv_t); fixp(W.bqkv); fixp(W.slopes); fixp(W.slope_vec); fixp(W.lnq_g); fixp(W.lnq_b); fixp(W.lnk_g);
-        fixp(W.lnk_b); fixp(W.lnv_g); fixp(W.lnv_b); fixp(W.wp_t); fixp(W.bp); fixp(W.lnp_g); fixp(W.lnp_b);
+        pk.bind(&W.wp_t, wp);
+        pk.bind(&W.bp, pk.plain(B + "attn_concat_proj.0.bias", 64));
+        pk.repacked(B + "attn_concat_proj.1.weight", 1, [slopes](const float* s, float* d) { d[slopes + 3] = s[0]; });
+        pk.bind(&W.lnp_g, pk.plain(B + "attn_concat_proj.3.norm.weight", FC));
+        pk.bind(&W.lnp_b, pk.plain(B + "attn_concat_proj.3.norm.bias", FC));
+        // tensor-core B operands of this block, in PL_* order
+        auto reg = [&](int64_t wt, int K, int N, int ld) { e->plane_of.push_back(pk.plane(wt, K, N, ld)); };
+        reg(wih1, 64, 512, 64); reg(wl1, 128, 64, 128); reg(wih2, 64, 256, 64); reg(wl2, 64, 64, 64); reg(wqkv, 64, NQKV, 64);
+        reg(wih2, 64, 256, 128);
+        pk.plane(whh2t, 64, 256, 128, 64);      // [W_ih | W_hh]: k = [x | h], one plane
+        reg(wp, 64, 64, 64);
     }
 }
 
@@ -379,10 +299,7 @@ constexpr int64_t TC_MIN_ROWS = 2048;      // below this the 16-row CUDA-core ti
 enum { PL_IH1 = 0, PL_L1, PL_IH2, PL_L2, PL_QKV, PL_CAT, PL_P, PL_PER_BLOCK };
 
 static umma::BPlanes tc_planes(const SepEngine* e, int blk, int which, int ld) {
-    umma::BPlanes b;
-    b.base = e->planes + e->plane_of[(size_t)blk * PL_PER_BLOCK + which];
-    b.ld = ld; b.plane_stride = e->planes_total; b.nz = 1;
-    return b;
+    return e->pack.bplanes(e->plane_of[(size_t)blk * PL_PER_BLOCK + which], ld);
 }
 
 // the recurrence: tensor cores when there are enough sequences to fill the GPU with 32-sequence CTAs, else lstm.cuh
@@ -439,7 +356,7 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
     const float* emb = a.emb; float* state = a.state; float* y = a.y;
     const int64_t ybs = a.ybs, ycs = a.ycs; const int y_len = a.y_len, B = a.B, T = a.T;
     float* wsp = a.wsp; const size_t ws_bytes = a.ws_bytes; const uint32_t flags = a.flags;
-    if (!e->committed) return fail(4, "weights not committed");
+    if (!e->pack.committed) return fail(4, "weights not committed");
     if (B <= 0 || T <= 0) return fail(1, "batch and frames must be positive");
     const Workspace ws = carve(e->n_blocks, B, T, flags);
     if ((size_t)ws.total * sizeof(float) > ws_bytes) return fail(1, "workspace too small");
@@ -508,7 +425,7 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
             // many sequences: LayerNorm, W_ih and the recurrence in ONE tensor-core kernel (no [rows x 512] projection in HBM)
             tcl::LstmXArgs xa{};
             xa.l = l; xa.x = X; xa.x_ld = 64;
-            xa.wih_hi = e->planes + e->plane_of[(size_t)b * PL_PER_BLOCK + PL_IH1]; xa.wih_lo = xa.wih_hi + e->planes_total;
+            xa.wih_hi = e->pack.planes + e->plane_of[(size_t)b * PL_PER_BLOCK + PL_IH1]; xa.wih_lo = xa.wih_hi + e->pack.planes_total;
             xa.bias = W.b1; xa.ln_g = W.ln1_g; xa.ln_b = W.ln1_b;
             CK(launch_tc_lstm_x(xa, e->tc_passes, st, false));
             MARK("gemm_ih_intra");
@@ -606,7 +523,7 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
             if (tc_fused_lstm(e, l)) {
                 tcl::LstmXArgs xa{};
                 xa.l = l; xa.x = X; xa.x_ld = 64;
-                xa.wih_hi = e->planes + e->plane_of[(size_t)b * PL_PER_BLOCK + PL_IH2]; xa.wih_lo = xa.wih_hi + e->planes_total;
+                xa.wih_hi = e->pack.planes + e->plane_of[(size_t)b * PL_PER_BLOCK + PL_IH2]; xa.wih_lo = xa.wih_hi + e->pack.planes_total;
                 xa.bias = W.b2; xa.ln_g = W.ln2_g; xa.ln_b = W.ln2_b;
                 CK(launch_tc_lstm_x(xa, e->tc_passes, st, false));
                 MARK("gemm_ih_inter");
@@ -952,28 +869,36 @@ static int count_kernel_nodes(cudaGraph_t graph) {
     return k;
 }
 
-// K chained one-frame calls as one pipelined graph (cached on the argument set + K)
-static int run_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_t st) {
-    std::vector<int64_t> key = {(int64_t)a.x, a.xbs, a.xcs, a.x_len, (int64_t)a.emb, (int64_t)a.state, (int64_t)a.y,
-                                a.ybs, a.ycs, a.y_len, a.B, -K, (int64_t)a.wsp, (int64_t)a.flags, a.pos_rel};
+static void drop_graphs(SepEngine* e) {
+    for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);
+    e->graphs.clear();
+}
+
+// cache key of a chain graph: every argument its kernels bake in (`t`: frames, or -hops for the pipelined form)
+static std::vector<int64_t> graph_key(const ChainArgs& a, int t) {
+    return {(int64_t)a.x, a.xbs, a.xcs, a.x_len, (int64_t)a.emb, (int64_t)a.state, (int64_t)a.y,
+            a.ybs, a.ycs, a.y_len, a.B, t, (int64_t)a.wsp, (int64_t)a.flags, a.pos_rel};
+}
+
+// Launch the graph cached under `key` on `st`.  The first time a key is seen, `enqueue(cap)` is captured on the private
+// stream `cap` (made on first use) and instantiated; at most 32 graphs are kept.  `census_hops` > 0 marks a pipelined
+// graph, whose node / edge census option "graph_stats" prints.
+template <class Enqueue>
+static int run_graph(SepEngine* e, const std::vector<int64_t>& key, cudaStream_t& cap, cudaStream_t st, Enqueue enqueue,
+                     int census_hops = 0) {
     auto it = e->graphs.find(key);
     if (it == e->graphs.end()) {
-        if (!e->committed) return fail(4, "weights not committed");
+        if (!e->pack.committed) return fail(4, "weights not committed");
         if (int rc = set_attrs()) return rc;
-        if (!e->pipe_streams[0]) CK(cudaStreamCreateWithFlags(&e->pipe_streams[0], cudaStreamNonBlocking));
-        if (e->graphs.size() >= 32) {
-            for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second);
-            e->graphs.clear();
-            e->graph_kernels.clear();
-        }
-        cudaStream_t origin = e->pipe_streams[0];
-        CK(cudaStreamBeginCapture(origin, cudaStreamCaptureModeThreadLocal));
-        const int rc = enqueue_pipeline(e, a, K, origin);
+        if (!cap) CK(cudaStreamCreateWithFlags(&cap, cudaStreamNonBlocking));
+        if (e->graphs.size() >= 32) drop_graphs(e);
+        CK(cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal));
+        const int rc = enqueue(cap);
         cudaGraph_t graph = nullptr;
-        const cudaError_t ce = cudaStreamEndCapture(origin, &graph);
+        const cudaError_t ce = cudaStreamEndCapture(cap, &graph);
         if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-        if (ce != cudaSuccess) return fail(3, std::string("cudaStreamEndCapture (pipeline): ") + cudaGetErrorString(ce));
-        if (e->graph_stats) {                       // debug (option "graph_stats"): node / edge census of the captured pipeline graph
+        if (ce != cudaSuccess) return fail(3, std::string("cudaStreamEndCapture: ") + cudaGetErrorString(ce));
+        if (census_hops > 0 && e->graph_stats) {
             size_t n_nodes = 0, n_edges = 0;
             cudaGraphGetNodes(graph, nullptr, &n_nodes);
             cudaGraphGetEdges_v2(graph, nullptr, nullptr, nullptr, &n_edges);
@@ -982,22 +907,26 @@ static int run_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_t st
             cudaGraphGetEdges_v2(graph, from.data(), to.data(), ed.data(), &n_edges);
             size_t prog = 0;
             for (const auto& d : ed) prog += (d.type == cudaGraphDependencyTypeProgrammatic) ? 1 : 0;
-            fprintf(stderr, "[l2h] pipeline graph: hops %d, nodes %zu, edges %zu, programmatic edges %zu\n", K, n_nodes, n_edges, prog);
+            fprintf(stderr, "[l2h] pipeline graph: hops %d, nodes %zu, edges %zu, programmatic edges %zu\n", census_hops, n_nodes,
+                    n_edges, prog);
         }
         cudaGraphExec_t exec = nullptr;
         const int nk = count_kernel_nodes(graph);
         CK(cudaGraphInstantiate(&exec, graph, 0));
         cudaGraphDestroy(graph);
-        e->graph_kernels[exec] = nk;
-        it = e->graphs.emplace(key, exec).first;
+        it = e->graphs.emplace(key, SepEngine::CachedGraph{exec, nk}).first;
     }
-    CK(cudaGraphLaunch(it->second, st));
-    e->launch_count += e->graph_kernels[it->second];
+    CK(cudaGraphLaunch(it->second.exec, st));
+    e->launch_count += it->second.kernels;
     return 0;
 }
 
-// Launch the chain directly, or replay it from a cached CUDA graph (captured on a private
-// stream the first time this exact argument set is seen; graph launches go to the caller's stream).
+// K chained one-frame calls as one pipelined graph
+static int run_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_t st) {
+    return run_graph(e, graph_key(a, -K), e->pipe_streams[0], st, [&](cudaStream_t origin) { return enqueue_pipeline(e, a, K, origin); }, K);
+}
+
+// Launch the chain directly, or replay it from a cached CUDA graph (graph launches go to the caller's stream).
 static int run_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st, bool use_graph) {
     if (!use_graph || (a.flags & L2H_FLAG_TAPS)) {
         const long long before = g_launches;
@@ -1005,34 +934,7 @@ static int run_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st, bool use
         e->launch_count += g_launches - before;
         return rc;
     }
-    std::vector<int64_t> key = {(int64_t)a.x, a.xbs, a.xcs, a.x_len, (int64_t)a.emb, (int64_t)a.state, (int64_t)a.y,
-                                a.ybs, a.ycs, a.y_len, a.B, a.T, (int64_t)a.wsp, (int64_t)a.flags, a.pos_rel};
-    auto it = e->graphs.find(key);
-    if (it == e->graphs.end()) {
-        if (!e->committed) return fail(4, "weights not committed");
-        if (int rc = set_attrs()) return rc;
-        if (!e->cap_stream) CK(cudaStreamCreateWithFlags(&e->cap_stream, cudaStreamNonBlocking));
-        if (e->graphs.size() >= 32) {
-            for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second);
-            e->graphs.clear();
-            e->graph_kernels.clear();
-        }
-        CK(cudaStreamBeginCapture(e->cap_stream, cudaStreamCaptureModeThreadLocal));
-        const int rc = enqueue_chain(e, a, e->cap_stream);
-        cudaGraph_t graph = nullptr;
-        const cudaError_t ce = cudaStreamEndCapture(e->cap_stream, &graph);
-        if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-        if (ce != cudaSuccess) return fail(3, std::string("cudaStreamEndCapture: ") + cudaGetErrorString(ce));
-        cudaGraphExec_t exec = nullptr;
-        const int nk = count_kernel_nodes(graph);
-        CK(cudaGraphInstantiate(&exec, graph, 0));
-        cudaGraphDestroy(graph);
-        e->graph_kernels[exec] = nk;
-        it = e->graphs.emplace(key, exec).first;
-    }
-    CK(cudaGraphLaunch(it->second, st));
-    e->launch_count += e->graph_kernels[it->second];
-    return 0;
+    return run_graph(e, graph_key(a, a.T), e->cap_stream, st, [&](cudaStream_t cs) { return enqueue_chain(e, a, cs); });
 }
 
 }  // namespace l2h
@@ -1059,21 +961,19 @@ int l2h_sep_create(const l2h_sep_config* c, void** handle) {
     return 0;
 }
 
-// everything the handle owns on its device: cached graphs, capture / pipeline streams, events, the weight buffer
+// everything the handle owns on its device: cached graphs, capture / pipeline streams, events, the weight buffers
 static void release_device_resources(SepEngine* e) {
     int cur = -1;
-    const bool sw = e->device >= 0 && cudaGetDevice(&cur) == cudaSuccess && cur != e->device;
-    if (sw) cudaSetDevice(e->device);
-    for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second);
-    e->graphs.clear();
-    e->graph_kernels.clear();
+    const int dev = e->pack.device;
+    const bool sw = dev >= 0 && cudaGetDevice(&cur) == cudaSuccess && cur != dev;
+    if (sw) cudaSetDevice(dev);
+    drop_graphs(e);
     if (e->cap_stream) { cudaStreamDestroy(e->cap_stream); e->cap_stream = nullptr; }
     for (auto& ps : e->pipe_streams) if (ps) { cudaStreamDestroy(ps); ps = nullptr; }
     for (auto& ev : e->pipe_events) cudaEventDestroy(ev);
     e->pipe_events.clear();
     if (e->trace_dev) { cudaFree(e->trace_dev); e->trace_dev = nullptr; e->trace_cap = 0; }
-    if (e->dev) { cudaFree(e->dev); e->dev = nullptr; }
-    if (e->planes) { cudaFree(e->planes); e->planes = nullptr; }
+    e->pack.release();
     if (sw) cudaSetDevice(cur);
 }
 
@@ -1081,8 +981,9 @@ static void release_device_resources(SepEngine* e) {
 static int check_device(SepEngine* e) {
     int cur = -1;
     CK(cudaGetDevice(&cur));
-    if (e->device >= 0 && cur != e->device)
-        return fail(1, "this handle's weights live on device " + std::to_string(e->device) + " but device " + std::to_string(cur) +
+    const int dev = e->pack.device;
+    if (dev >= 0 && cur != dev)
+        return fail(1, "this handle's weights live on device " + std::to_string(dev) + " but device " + std::to_string(cur) +
                        " is current: commit the weights again with the new device current (Net.to(device) does), or use one handle per device");
     return 0;
 }
@@ -1098,51 +999,30 @@ int l2h_sep_destroy(void* handle) {
 int l2h_sep_load_weight(void* handle, const char* name, const float* data, int64_t numel) {
     SepEngine* e = static_cast<SepEngine*>(handle);
     if (!e || !name || !data) return fail(1, "null argument");
-    auto it = e->slots.find(name);
-    if (it == e->slots.end()) return fail(2, std::string("unknown weight name: ") + name);
-    Slot& s = it->second;
-    if (numel != s.numel) return fail(1, std::string("wrong element count for ") + name);
-    if (s.accumulate) s.raw.assign(data, data + numel);
-    else s.repack(data, e->host.data());
-    s.loaded = true;
-    e->committed = false;
-    return 0;
+    return e->pack.load(name, data, numel);
 }
 
 int l2h_sep_weights_expected(void* handle, int32_t* n_expected, int32_t* n_loaded) {
     SepEngine* e = static_cast<SepEngine*>(handle);
     if (!e) return fail(1, "null handle");
-    int n = 0;
-    for (auto& kv : e->slots) n += kv.second.loaded ? 1 : 0;
-    if (n_expected) *n_expected = (int)e->slots.size();
-    if (n_loaded) *n_loaded = n;
+    e->pack.counts(n_expected, n_loaded);
     return 0;
 }
 
 int l2h_sep_weight_info(void* handle, int32_t index, const char** name, int64_t* numel) {
     SepEngine* e = static_cast<SepEngine*>(handle);
     if (!e) return fail(1, "null handle");
-    if (index < 0 || index >= (int32_t)e->slots.size()) return fail(1, "weight index out of range");
-    auto it = e->slots.begin();
-    std::advance(it, index);
-    if (name) *name = it->first.c_str();             // owned by the handle, valid until l2h_sep_destroy
-    if (numel) *numel = it->second.numel;
-    return 0;
+    return e->pack.info(index, name, numel);       // the name is valid until l2h_sep_destroy
 }
 
 int l2h_sep_commit_weights(void* handle, void* stream) {
     SepEngine* e = static_cast<SepEngine*>(handle);
     if (!e) return fail(1, "null handle");
-    for (auto& kv : e->slots)
-        if (!kv.second.loaded) return fail(4, "weight not loaded: " + kv.first);
-    for (auto& kv : e->slots)
-        if (kv.second.accumulate) std::fill(e->host.begin() + kv.second.off, e->host.begin() + kv.second.off + 256, 0.f);
-    for (auto& kv : e->slots)
-        if (kv.second.accumulate) kv.second.repack(kv.second.raw.data(), e->host.data());
+    if (int rc = e->pack.finish()) return rc;
+    float* h = e->pack.host.data();
     for (const auto& m : e->mid_src)        // per-column PReLU slopes of the fused Q|K|V projection
-        for (int n = 0; n < NQKV; ++n) e->host[m.slope_vec + n] = e->host[m.slopes + (n < NHEAD * QE ? 0 : (n < 2 * NHEAD * QE ? 1 : 2))];
+        for (int n = 0; n < NQKV; ++n) h[m.slope_vec + n] = h[m.slopes + (n < NHEAD * QE ? 0 : (n < 2 * NHEAD * QE ? 1 : 2))];
     for (const auto& m : e->mid_src) {      // k-sliced, bank-padded copies for mid_kernel (layout: mid_kernel.cuh)
-        float* h = e->host.data();
         std::fill(h + m.dst, h + m.dst + MID_PACK, 0.f);
         for (int k = 0; k < M1_K; ++k)
             for (int n = 0; n < M1_N; ++n) h[m.dst + MID_W1 + mid_widx(M1_KS, M1_N, k, n)] = h[m.wl1 + (int64_t)k * 64 + n];
@@ -1156,29 +1036,13 @@ int l2h_sep_commit_weights(void* handle, void* stream) {
         for (int k = 0; k < M6_K; ++k)
             for (int n = 0; n < M6_N; ++n) h[m.dst + MID_W6 + mid_widx(M6_KS, M6_N, k, n)] = h[m.wqkv + (int64_t)k * NQKV + n];
     }
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
     int cur = -1;
     CK(cudaGetDevice(&cur));
-    const float* old_base = e->dev;              // null before the first commit (pointer fields then hold offsets)
-    if (e->dev != nullptr && e->device != cur) {  // the module moved to another GPU: everything device-side is rebuilt there
+    if (e->pack.dev != nullptr && e->pack.device != cur)    // the module moved to another GPU: everything device-side is rebuilt there
         release_device_resources(e);
-    }
-    if (e->dev == nullptr) {
-        CK(cudaMalloc(&e->dev, e->total * sizeof(float)));
-        e->device = cur;
-        shift_pointers(e, e->dev, old_base);
-        CK(cudaMalloc(&e->planes, 2 * e->planes_total * sizeof(__nv_bfloat16)));
-    }
-    CK(cudaMemcpyAsync(e->dev, e->host.data(), e->total * sizeof(float), cudaMemcpyHostToDevice, st));
-    for (const auto& ps : e->plane_srcs)        // k-major fp32 [K][N] -> bf16 hi/lo planes [N][ld] (tensor-core B operands)
-        CK(umma::split_planes(e->dev + ps.wt_off, 1, ps.N, ps.N, ps.K, ps.ld, e->planes + ps.plane_off + ps.col0,
-                              e->planes + e->planes_total + ps.plane_off + ps.col0, st));
-    CK(cudaStreamSynchronize(st));
-    e->committed = true;
+    if (int rc = e->pack.upload(static_cast<cudaStream_t>(stream))) return rc;
     e->w.gen = (int)(++e->weight_gen & 0x7fffff) + 1;      // never 0 (= a freshly initialised state)
-    for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second);     // cached graphs carry the old generation in their kernel arguments
-    e->graphs.clear();
-    e->graph_kernels.clear();
+    drop_graphs(e);                                         // cached graphs carry the old generation in their kernel arguments
     return 0;
 }
 
@@ -1428,9 +1292,7 @@ int l2h_sep_set_option(void* handle, const char* name, int32_t value) {
     else if (n == "bf16") e->tc_passes = value == 0 ? 3 : (value == 2 ? 1 : 2);   // 1: bf16 weights x split activations; 2: plain bf16 both
     else if (n == "graph_stats") e->graph_stats = value != 0;
     else return fail(2, "unknown option: " + n);
-    for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second);     // cached graphs were built with the old setting
-    e->graphs.clear();
-    e->graph_kernels.clear();
+    drop_graphs(e);                             // cached graphs were built with the old setting
     return 0;
 }
 

@@ -112,6 +112,9 @@ def test_embed_weight_table_matches_reference_state_dict(lib, embed_params):
     ne, nl = ctypes.c_int32(), ctypes.c_int32()
     assert lib.l2h_embed_weights_expected(h, ctypes.byref(ne), ctypes.byref(nl)) == 0
     assert ne.value == nl.value == len(net.state_dict())
+    z = torch.zeros(4)
+    assert lib.l2h_embed_load_weight(h, b"blocks.0.nope", z.data_ptr(), 4) == 2
+    assert lib.l2h_embed_load_weight(h, b"conv.0.bias", z.data_ptr(), 4) == 1
     n = ctypes.c_size_t()
     assert lib.l2h_embed_workspace_bytes(h, 1, 80000, ctypes.byref(n)) == 0 and n.value > 0
     mb = ctypes.c_int32()
