@@ -202,16 +202,34 @@ int l2h_embed_destroy(void* handle);
 int l2h_embed_load_weight(void* handle, const char* name, const float* host_data, int64_t numel);
 int l2h_embed_weights_expected(void* handle, int32_t* n_expected, int32_t* n_loaded);
 int l2h_embed_commit_weights(void* handle, void* stream);
+/* workspace of one forward call of `batch` utterances padded to n_samples; it includes batch * 4 bytes for the device
+ * copy of the lengths of l2h_embed_forward_lengths */
 int l2h_embed_workspace_bytes(void* handle, int32_t batch, int32_t n_samples, size_t* bytes);
 /* "bf16" (the separator's mapping): 0 (default): every tensor-core product is formed from bf16 hi/lo splits of both fp32
  * operands in three MMA passes (fp32-grade, relative error ~2^-16 per product); 1: bf16 weights x split activations (two
- * passes); 2: plain bf16 operands (one pass). */
+ * passes); 2: plain bf16 operands (one pass).
+ * "tc_lstm_min" (default 2048): the sequence-directions of one recurrence from which it runs on the tensor cores
+ * (tc_lstm) instead of the CUDA cores (lstm_rec).  The choice is made per call from the padded batch, so a short
+ * utterance alone can take the other kernel family than inside a long batch; set it to 1 (always tensor cores) or
+ * above any batch (never) to compare results of the same recurrence arithmetic. */
 int l2h_embed_set_option(void* handle, const char* name, int32_t value);
 /* largest batch one l2h_embed_forward call should be given for utterances of n_samples (workspace bound) */
 int l2h_embed_max_batch(void* handle, int32_t n_samples, int32_t* max_batch);
-/* x_dev [batch][2][n_samples] fp32 contiguous -> emb_dev [batch][256].  Asynchronous on `stream`. */
+/* x_dev [batch][2][n_samples] fp32 contiguous -> emb_dev [batch][256].  Asynchronous on `stream`.
+ * The same as l2h_embed_forward_lengths with lengths_host = NULL. */
 int l2h_embed_forward(void* handle, const float* x_dev, float* emb_dev, int32_t batch, int32_t n_samples,
                       void* workspace_dev, size_t workspace_bytes, void* stream);
+/* Utterances of different lengths in one call.  x_dev [batch][2][n_max] fp32 contiguous; utterance b is
+ * x_dev[b][:][0 .. lengths_host[b]) and row b of emb_dev [batch][256] is its embedding as if it were embedded alone.
+ * Samples at index >= lengths_host[b] are never read (they may hold anything, NaN included).  lengths_host is a HOST
+ * array of `batch` sample counts, read during the call only; NULL means every utterance is n_max long.  Each length must
+ * lie in [192, n_max] (192 samples = the 4 STFT frames of the unfold).  Size the workspace with
+ * l2h_embed_workspace_bytes(batch, n_max) and the batch with l2h_embed_max_batch(n_max).  The utterances are computed
+ * padded to n_max, so the cost is that of `batch` utterances of n_max samples.
+ * Errors, returned before anything is enqueued and before the weights are checked: 1 = a null pointer, batch <= 0, a
+ * length outside [192, n_max], or a workspace smaller than the query.  Asynchronous on `stream`. */
+int l2h_embed_forward_lengths(void* handle, const float* x_dev, int32_t n_max, const int32_t* lengths_host, int32_t batch,
+                              float* emb_dev, void* workspace_dev, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Evaluation epilogue on the device (replaces the CPU metric code after `outputs.cpu()` in

@@ -96,6 +96,9 @@ _SIGS = {
     "l2h_embed_max_batch": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int32, ctypes.POINTER(ctypes.c_int32)]),
     "l2h_embed_forward": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
                                         ctypes.c_int32, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
+    "l2h_embed_forward_lengths": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
+                                                ctypes.POINTER(ctypes.c_int32), ctypes.c_int32, ctypes.c_void_p,
+                                                ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
 }
 
 

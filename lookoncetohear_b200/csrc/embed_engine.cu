@@ -34,6 +34,7 @@ struct EmbedEngine {
     std::vector<BlockPlanes> bplanes;
     int attrs_dev = -1;
     int passes = 3;                 // 3: bf16x3 split products (fp32-grade), 2: bf16 weights x split activations, 1: plain bf16
+    int tcl_min_seqdirs = 2048;     // (sequence, direction) pairs from which a recurrence runs on the tensor cores (option "tc_lstm_min")
 };
 
 static void build_layout(EmbedEngine* e) {
@@ -166,7 +167,7 @@ static void build_layout(EmbedEngine* e) {
     }
 }
 
-struct EWs { int64_t INV, GN, X, GX, HC, QKV, QN, KP, VP, S, O, HD, total; int T, Tp; };
+struct EWs { int64_t INV, GN, X, GX, HC, QKV, QN, KP, VP, S, O, HD, LENS, total; int T, Tp; };
 
 static EWs ecarve(int B, int N) {
     EWs w;
@@ -188,6 +189,7 @@ static EWs ecarve(int B, int N) {
     w.S = alloc((int64_t)B * NH * T * Tp);
     w.O = alloc((int64_t)B * NH * Tp * VDIM);
     w.HD = alloc((int64_t)B * T * 256);
+    w.LENS = alloc(B);                         // int32 per utterance: the device copy of the lengths of a mixed batch
     w.total = cur;
     return w;
 }
@@ -200,16 +202,29 @@ static EWs ecarve(int B, int N) {
             return fail(3, std::string(#expr) + ": " + cudaGetErrorString(_e) + " " + _why);       \
     } while (0)
 
-static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B, int N, float* wsp, size_t ws_bytes,
-                              cudaStream_t st) {
-    if (!e->pack.committed) return fail(4, "weights not committed");
-    if (B <= 0 || N < NFFT) return fail(1, "need batch >= 1 and at least 128 samples");
+// The shortest utterance: T = 1 + n / HOP >= KS frames for the 4-frame unfold.
+constexpr int MIN_SAMPLES = HOP * (KS - 1);
+
+// x [B][2][N]; utterance b is x[b, :, :lens_host[b]] (lens_host null: every utterance is N long).  Every argument is
+// checked before the committed-weights check and before any device work.
+static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B, int N, const int32_t* lens_host, float* wsp,
+                              size_t ws_bytes, cudaStream_t st) {
+    if (B <= 0) return fail(1, "need batch >= 1");
+    if (N < MIN_SAMPLES) return fail(1, "utterance too short for the 4-frame unfold: need at least 192 samples");
+    bool mixed = false;                        // some utterance shorter than N: the padded-frame path
+    if (lens_host != nullptr)
+        for (int b = 0; b < B; ++b) {
+            if (lens_host[b] < MIN_SAMPLES || lens_host[b] > N)
+                return fail(1, "length " + std::to_string(lens_host[b]) + " of utterance " + std::to_string(b) + " is outside [192, n_max = " +
+                                   std::to_string(N) + "]");
+            mixed |= lens_host[b] != N;
+        }
     const EWs ws = ecarve(B, N);
     if ((size_t)ws.total * sizeof(float) > ws_bytes) return fail(1, "workspace too small");
     const int T = ws.T, Tp = ws.Tp;
-    if (T < KS) return fail(1, "utterance too short for the 4-frame unfold");
     const int64_t rows = (int64_t)B * T * NF;
     if (rows * 2 > 0x7fffffff) return fail(1, "batch too large for one call; split it (l2h_embed_max_batch)");
+    if (!e->pack.committed) return fail(4, "weights not committed");
     int cur_dev = -1;
     CK(cudaGetDevice(&cur_dev));
     if (cur_dev != e->pack.device)
@@ -234,14 +249,27 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
     const int passes = e->passes;
     const WeightPack& pk = e->pack;
 
-    estd_kernel<<<B, 256, 0, st>>>(x, (int64_t)2 * N, INV);
+    // lengths on the device only for a mixed batch; equal lengths run exactly the equal-length path
+    int32_t* lens = nullptr;
+    if (mixed) {
+        lens = reinterpret_cast<int32_t*>(wsp + ws.LENS);
+        for (int b0 = 0; b0 < B; b0 += LENS_PER_LAUNCH) {
+            const int n = std::min(LENS_PER_LAUNCH, B - b0);
+            LensBlock blk;
+            memcpy(blk.v, lens_host + b0, sizeof(int32_t) * n);
+            eput_lens_kernel<<<1, 256, 0, st>>>(lens + b0, blk, n);
+            CK(cudaGetLastError());
+        }
+    }
+
+    estd_kernel<<<B, 256, 0, st>>>(x, N, lens, INV);
     CK(cudaGetLastError());
     CK(cudaMemsetAsync(GN, 0, sizeof(double) * 2 * B, st));
-    efront_kernel<<<dim3(T, B), 256, 0, st>>>(x, N, INV, X, GN, e->w, T);
+    efront_kernel<<<dim3(T, B), 256, 0, st>>>(x, N, lens, INV, X, GN, e->w, T);
     CK(cudaGetLastError());
     {
         const int64_t per_b = (int64_t)T * NF * CH, total4 = (int64_t)B * per_b / 4;
-        egn_apply_kernel<<<(unsigned)((total4 + 255) / 256), 256, 0, st>>>(X, GN, per_b, total4, e->w);
+        egn_apply_kernel<<<(unsigned)((total4 + 255) / 256), 256, 0, st>>>(X, GN, per_b, total4, lens, e->w);
         CK(cudaGetLastError());
     }
 
@@ -269,11 +297,15 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
             g.b = pk.bplanes(inter ? PL.ih2 : PL.ih1, 256); g.N = 512; g.K = 256; g.passes = passes;
             g.bias = inter ? W.b2 : W.b1; g.C = GX; g.ldc = 512; g.c_seq_stride = (int64_t)steps * 512;
             CKU(umma::launch(g, st, &_why));
+            if (inter && lens != nullptr) {             // windows past an utterance's own frames: zero state, zero h
+                einter_mask_kernel<<<dim3(NF, B), 128, 0, st>>>(GX, lens, steps);
+                CK(cudaGetLastError());
+            }
             LstmArgs l{};
             l.gx = GX; l.gx_ld = 512; l.out = HC; l.out_ld = 128; l.whh = inter ? W.whh2 : W.whh1;
             l.nseq = nseq; l.L = steps; l.inner_count = 1; l.outer_stride = steps; l.inner_stride = 0; l.step_stride = 1;
             l.ndir = 2;
-            if ((int64_t)l.nseq * l.ndir >= 2048) CK(launch_tc_lstm(l, passes, st));      // many sequences: recurrence on the tensor cores
+            if ((int64_t)l.nseq * l.ndir >= e->tcl_min_seqdirs) CK(launch_tc_lstm(l, passes, st));   // many sequences: recurrence on the tensor cores
             else CK(launch_lstm_rec(l, st));
             // ---- ConvTranspose1d(128->64, k=4) + residual: output position p reads h rows p-3 .. p; rows outside the
             // sequence are the zero-filled halo of the tensor map ----------------------------------------------------
@@ -312,7 +344,7 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
             g.C = S; g.ldc = Tp; g.c_seq_stride = (int64_t)T * Tp;
             CKU(umma::launch(g, st, &_why));
         }
-        softmax_rows_kernel<<<(unsigned)((int64_t)Z * T), 128, 0, st>>>(S, Tp, T, T, (int64_t)T * Tp);
+        softmax_rows_kernel<<<(unsigned)((int64_t)Z * T), 128, 0, st>>>(S, Tp, T, T, (int64_t)T * Tp, lens);
         CK(cudaGetLastError());
         {
             umma::GemmDesc g;                          // O = P V (V is the MN-major B operand: [frame][f*16+c])
@@ -337,7 +369,7 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
         g.bias = e->w.bh; g.C = HD; g.ldc = 256;
         CKU(umma::launch(g, st, &_why));
     }
-    ehead_kernel<<<B, 256, 0, st>>>(HD, out, e->w, T);
+    ehead_kernel<<<B, 256, 0, st>>>(HD, out, e->w, T, lens);
     CK(cudaGetLastError());
     return 0;
 }
@@ -397,6 +429,7 @@ int l2h_embed_set_option(void* handle, const char* name, int32_t value) {
     const std::string n(name);
     if (n == "bf16") e->passes = value == 0 ? 3 : (value == 2 ? 1 : 2);   // 0 (default): bf16x3 split, fp32-grade; 1: bf16 weights x
                                                                           // split activations; 2: plain bf16 operands
+    else if (n == "tc_lstm_min") e->tcl_min_seqdirs = std::max(1, (int)value);
     else return fail(2, "unknown option: " + n);
     return 0;
 }
@@ -417,12 +450,17 @@ int l2h_embed_max_batch(void* handle, int32_t n_samples, int32_t* max_batch) {
     return 0;
 }
 
-int l2h_embed_forward(void* handle, const float* x_dev, float* emb_dev, int32_t batch, int32_t n_samples, void* ws,
-                      size_t ws_bytes, void* stream) {
+int l2h_embed_forward_lengths(void* handle, const float* x_dev, int32_t n_max, const int32_t* lengths_host, int32_t batch,
+                              float* emb_dev, void* ws, size_t ws_bytes, void* stream) {
     EmbedEngine* e = static_cast<EmbedEngine*>(handle);
     if (!e || !x_dev || !emb_dev || !ws) return fail(1, "null argument");
-    return embed_forward_impl(e, x_dev, emb_dev, batch, n_samples, static_cast<float*>(ws), ws_bytes,
+    return embed_forward_impl(e, x_dev, emb_dev, batch, n_max, lengths_host, static_cast<float*>(ws), ws_bytes,
                               static_cast<cudaStream_t>(stream));
+}
+
+int l2h_embed_forward(void* handle, const float* x_dev, float* emb_dev, int32_t batch, int32_t n_samples, void* ws,
+                      size_t ws_bytes, void* stream) {
+    return l2h_embed_forward_lengths(handle, x_dev, n_samples, nullptr, batch, emb_dev, ws, ws_bytes, stream);
 }
 
 }  // extern "C"

@@ -10,6 +10,7 @@ containers only; the forward goes through the C ABI.
 """
 import ctypes
 import math
+import numbers
 
 import torch
 import torch.nn as nn
@@ -86,7 +87,8 @@ class EmbedTFGridNet(nn.Module):
 
     def set_option(self, name, value):
         """"bf16": 0 = bf16x3 split products (default, fp32-grade), 1 = bf16 weights x split activations (two MMA passes),
-        2 = plain bf16 tensor-core operands (one MMA pass)."""
+        2 = plain bf16 tensor-core operands (one MMA pass).
+        "tc_lstm_min" (default 2048): sequence-directions from which a recurrence runs on the tensor cores."""
         _cabi.check(_cabi.lib().l2h_embed_set_option(self._engine(), name.encode(), int(value)))
 
     def __del__(self):
@@ -115,28 +117,96 @@ class EmbedTFGridNet(nn.Module):
             _cabi.check(L.l2h_embed_commit_weights(h, torch.cuda.current_stream(device).cuda_stream))
         self._dirty = False
 
-    def forward(self, input):
-        """input [B, M, N] -> [B, embed_dim]   (reference tfgridnet.py:100-127)."""
+    def max_batch(self, n_samples):
+        """Largest batch one engine call takes for utterances padded to n_samples (workspace bound)."""
+        per = ctypes.c_int32()
+        _cabi.check(_cabi.lib().l2h_embed_max_batch(self._engine(), int(n_samples), ctypes.byref(per)))
+        return max(1, per.value)
+
+    def _run(self, x, out, lens):
+        """One engine call: x [nb, M, n] contiguous on the device, lens None or nb ints, out [nb, embed_dim]."""
+        dev = x.device
+        nb, _, n = x.shape
+        L, h = _cabi.lib(), self._engine()
+        ws = ctypes.c_size_t()
+        _cabi.check(L.l2h_embed_workspace_bytes(h, nb, n, ctypes.byref(ws)))
+        if self._ws is None or self._ws.numel() < ws.value or self._ws.device != dev:
+            self._ws = torch.empty(ws.value, dtype=torch.uint8, device=dev)
+        lens_c = None if lens is None else (ctypes.c_int32 * nb)(*lens)
+        with torch.cuda.device(dev):
+            _cabi.check(L.l2h_embed_forward_lengths(h, x.data_ptr(), n, lens_c, nb, out.data_ptr(),
+                                                    self._ws.data_ptr(), self._ws.numel(),
+                                                    torch.cuda.current_stream(dev).cuda_stream))
+
+    def forward(self, input, lengths=None):
+        """input [B, M, N] -> [B, embed_dim]   (reference tfgridnet.py:100-127).
+
+        ``lengths`` (optional: B ints, or a 1-D integer tensor on any device) gives each utterance's own sample count,
+        192 <= lengths[b] <= N: row b is then the embedding of ``input[b, :, :lengths[b]]`` alone, and the samples past
+        it are never read.  A batch larger than one engine call takes is sorted by length and cut into calls padded
+        only to their own longest utterance."""
         if not input.is_cuda:
             raise RuntimeError("lookoncetohear_b200.EmbedTFGridNet runs only on a CUDA (sm_90a) device: "
                                "hand-written CUDA hot path, no CPU fallback")
+        B, M, N = input.shape
+        lens = None if lengths is None else check_lengths(lengths, B, N)
+        if lens is not None and all(n == N for n in lens):
+            lens = None                                   # equal lengths: the equal-length call
         dev = input.device
         self._sync_weights(dev)
         x = input.contiguous().float()
-        B, M, N = x.shape
         out = torch.empty(B, self.embed_dim, dtype=torch.float32, device=dev)
-        L, h = _cabi.lib(), self._engine()
-        per = ctypes.c_int32()
-        _cabi.check(L.l2h_embed_max_batch(h, N, ctypes.byref(per)))
-        per = max(1, per.value)
-        for b0 in range(0, B, per):
-            nb = min(per, B - b0)
-            n = ctypes.c_size_t()
-            _cabi.check(L.l2h_embed_workspace_bytes(h, nb, N, ctypes.byref(n)))
-            if self._ws is None or self._ws.numel() < n.value or self._ws.device != dev:
-                self._ws = torch.empty(n.value, dtype=torch.uint8, device=dev)
-            with torch.cuda.device(dev):
-                _cabi.check(L.l2h_embed_forward(h, x[b0:].data_ptr(), out[b0:].data_ptr(), nb, N,
-                                                self._ws.data_ptr(), self._ws.numel(),
-                                                torch.cuda.current_stream(dev).cuda_stream))
+        per = self.max_batch(N)
+        if lens is None or B <= per:
+            for b0 in range(0, B, per):
+                nb = min(per, B - b0)
+                self._run(x[b0:b0 + nb], out[b0:b0 + nb], None if lens is None else lens[b0:b0 + nb])
+            return out
+        for idx, m in group_by_length(lens, self.max_batch):
+            ii = torch.tensor(idx, dtype=torch.long, device=dev)
+            xc = x[ii, :, :m].contiguous()
+            oc = torch.empty(len(idx), self.embed_dim, dtype=torch.float32, device=dev)
+            self._run(xc, oc, [lens[i] for i in idx])
+            out[ii] = oc
         return out
+
+
+MIN_SAMPLES = 192          # 1 + n // 64 >= 4 STFT frames for the 4-frame unfold
+
+
+def check_lengths(lengths, batch, n_max):
+    """Validate per-utterance lengths on the host: a list of ``batch`` Python ints in [192, n_max], else ValueError."""
+    if isinstance(lengths, torch.Tensor):
+        if lengths.dim() != 1 or lengths.dtype.is_floating_point or lengths.dtype.is_complex or lengths.dtype == torch.bool:
+            raise ValueError(f"lengths must be a 1-D integer tensor, got {lengths.dtype} of shape {tuple(lengths.shape)}")
+        lens = [int(v) for v in lengths.tolist()]
+    else:
+        try:
+            lens = list(lengths)
+        except TypeError:
+            raise ValueError("lengths must be a sequence of ints or a 1-D integer tensor") from None
+        for v in lens:
+            if isinstance(v, bool) or not isinstance(v, numbers.Integral):
+                raise ValueError(f"lengths must be integers, got {v!r}")
+        lens = [int(v) for v in lens]
+    if len(lens) != batch:
+        raise ValueError(f"{len(lens)} lengths for a batch of {batch}")
+    for b, v in enumerate(lens):
+        if not MIN_SAMPLES <= v <= n_max:
+            raise ValueError(f"length {v} of utterance {b} is outside [{MIN_SAMPLES}, {n_max}]")
+    return lens
+
+
+def group_by_length(lengths, max_batch):
+    """Cut a batch into engine calls: utterances sorted by length, from the longest down, at most
+    ``max_batch(longest in the call)`` per call.  Returns [(indices, pad)]: each call's indices in ascending length and
+    the length it is padded to, its own longest."""
+    order = sorted(range(len(lengths)), key=lambda i: lengths[i])
+    chunks = []
+    end = len(order)
+    while end > 0:
+        m = lengths[order[end - 1]]
+        start = max(0, end - max(1, int(max_batch(m))))
+        chunks.append((order[start:end], m))
+        end = start
+    return chunks
