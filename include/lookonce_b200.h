@@ -126,7 +126,7 @@ int l2h_sep_stream_host(void* handle, const float* x_host, int32_t x_len, const 
  * works on is derived on the device from the state's frame counter.  With chunks_per_call == 1 the
  * one-hop chains of up to l2h_sep_pipeline_frames() consecutive hops are captured as ONE graph on 8
  * streams with (block, frame) wavefront dependencies, so different blocks work on different hops
- * concurrently (set L2H_PIPE=0 to run the hops strictly one after the other).  Asynchronous. */
+ * concurrently (option "pipeline" = 0 runs the hops strictly one after the other).  Asynchronous. */
 int l2h_sep_stream_dev(void* handle, const float* x_dev, int32_t x_len, const float* emb_dev,
                        void* state_dev, float* y_dev, int32_t y_len, int32_t batch, int32_t n_calls,
                        int32_t chunks_per_call, void* workspace_dev, size_t workspace_bytes, void* stream);
@@ -136,23 +136,19 @@ int l2h_sep_stream_dev(void* handle, const float* x_dev, int32_t x_len, const fl
 int l2h_sep_stream_workspace_bytes(void* handle, int32_t batch, int32_t chunks_per_call, size_t* bytes);
 int l2h_sep_pipeline_frames(void* handle, int32_t* frames);
 /* runtime switches (the only way to change them: there are no environment variables).  0 | 1: "pipeline" (wavefront graph for
- * streams of one-hop calls), "pdl", "fused_mid", "fused_tail" (one-hop calls of a few streams as 8 launches: front1_kernel, per block
+ * streams of one-hop calls), "pdl", "fused_tail" (one-hop calls of a few streams as 8 launches: front1_kernel, per block
  * the BiLSTM and the 16-CTA tail_kernel; default 1), "back_many" (calls of several frames / many streams through the persistent
- * front_many / back_many kernels; default 1), "pipeline_split_mid" (mid section as mid_a | mid_b | mid_c in the graph),
- * "mid_split_large" (the same three kernels for many streams), "fold_mid_c" (default 0: no mid_c -- the inter Linear moves into
- * the serial kernel, the Q/K/V projection into qkv_kernel; changes rounding, not the maths; it lengthens the serial stage of the pipeline; tested),
- * "tensor_cores" (default 1), "fuse_ih" (default 0), "graph_stats".  Values: "bf16" (0 = bf16x3 split products, 1 = bf16 weights x
+ * front_many / back_many kernels; default 1), "fuse_ih" (default 0).  Values: "bf16" (0 = bf16x3 split products, 1 = bf16 weights x
  * split activations, 2 = plain bf16), "tc_lstm_min" (sequence-directions from which the recurrence runs on the tensor cores,
  * default 4096), "tc_pdl" (bit mask, default 7: programmatic launches around the tensor-core GEMMs of many-row chains),
  * "pipeline_gemm_shape" (0 | 1 | 2).  Counts: "pipeline_frames" (hops per graph, <= 500; 0 = as many as the workspace budget
  * holds), "pipeline_midb_hops" (hops per launch of the serial stage, <= 8) and the hops in flight per stage: "pipeline_lanes"
  * (BiLSTM, <= 16), "pipeline_midc_lanes" (<= 3), "pipeline_qkv_lanes" (<= 4), "pipeline_attn_lanes" (<= 4),
- * "pipeline_out_lanes" (<= 4), "pipeline_front_lanes" (<= 8), "pipeline_back_lanes" (<= 6).  Bit masks over the stages
- * front=1, W_ih gemm=2, bilstm=4, mid_a=8, mid_b=16, mid_c=32, qkv=64, attention=128, attn_out=256, back=512:
- * "pipeline_pdl" (stages launched with programmatic dependent launch; default 16) and "pipeline_debug_skip" (stages NOT
- * launched -- timing experiments only, the output is garbage).  "defaults" restores all pipeline settings.  The pipeline
- * settings never change results (bit-identical, tests/test_sep_gpu.py); "fused_tail", "fold_mid_c", "bf16", "fuse_ih" and the
- * tensor-core switches change rounding only (gates in tests/). */
+ * "pipeline_out_lanes" (<= 4), "pipeline_front_lanes" (<= 8), "pipeline_back_lanes" (<= 6).  "pipeline_pdl": bit mask of the
+ * stages launched with programmatic dependent launch (front=1, W_ih gemm=2, bilstm=4, mid_a=8, mid_b=16, mid_c=32, qkv=64,
+ * attention=128, attn_out=256, back=512; default 16).  "defaults" restores all pipeline settings.  The pipeline settings never
+ * change results (bit-identical, tests/test_sep_gpu.py); "fused_tail", "bf16", "fuse_ih" and "tc_lstm_min" change rounding
+ * only (gates in tests/). */
 int l2h_sep_set_option(void* handle, const char* name, int32_t value);
 
 /* where the tap area starts inside the workspace (floats) and its stage count; stage s holds

@@ -505,202 +505,4 @@ mid_c_kernel(const float* __restrict__ Hn, float* __restrict__ X, float* __restr
     }
 }
 
-// The fused kernel without phase 6 (engine option "fold_mid_c": qkv_kernel projects Q/K/V itself, and the pipelined graph has
-// no mid_c).  Same text as mid_kernel up to X2.  Off by default: it lengthens the serial stage of the pipeline;
-// covered by tests/test_sep_gpu.py::test_fold_mid_c_option.
-__global__ void __launch_bounds__(256)
-mid_noproj_kernel(const float* __restrict__ Y, float* __restrict__ X, float* __restrict__ QKV, float* __restrict__ state,
-           int64_t sstride, int blk, BlockWeights w, int n_streams) {
-    extern __shared__ __align__(16) float sm[];
-    float* Wp = sm;                       // the packed weights (BlockWeights::mid_pack)
-    float* A1 = Wp + MID_PACK;            // intra LSTM outputs Y, k-sliced for phase 1
-    float* A3 = A1 + MID_A1;              // LN(X1), k-sliced for phase 3
-    float* A3h = A3 + MID_A3;             // h, k-sliced for phase 3
-    float* A5 = A3h + MID_A3;             // h', k-sliced for phase 5
-    float* A6 = A5 + MID_A5;              // X2, k-sliced for phase 6
-    float* x1s = A6 + MID_A6;             // [RT][64] X1 (LayerNorm input)
-
-    __shared__ __align__(8) unsigned long long wbar;
-    TraceScope trace_(TK_MID, Y);   // QKV is not written
-    griddep_launch();
-    const int tid = threadIdx.x;
-    constexpr int TILES = (NF + MID_RT - 1) / MID_RT;       // row tiles per stream
-    // ---- weights -> smem: TMA bulk copies (independent of the chain, so issued before the wait) ------
-    if (tid == 0) {
-        mbar_init(&wbar, 1);
-        mbar_fence_init();
-        mbar_expect_tx(&wbar, MID_PACK * 4);
-        tma_load_1d(Wp + MID_W1, w.mid_pack + MID_W1, (MID_W3B - MID_W1) * 4, &wbar);
-        tma_load_1d(Wp + MID_W3B, w.mid_pack + MID_W3B, (MID_W5 - MID_W3B) * 4, &wbar);
-        tma_load_1d(Wp + MID_W5, w.mid_pack + MID_W5, (MID_PACK - MID_W5) * 4, &wbar);
-    }
-    __syncthreads();
-    griddep_wait();
-    for (int item = blockIdx.x; item < n_streams * TILES; item += gridDim.x) {
-        const int b = item / TILES;
-        const int r0 = (item % TILES) * MID_RT;
-        const int nr = min(MID_RT, NF - r0);
-        __syncthreads();                    // the previous item's tiles are fully consumed
-        float* sb = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride + ST_BLK + (int64_t)blk * BK_STRIDE;
-        float* hst = sb + BK_H;
-        float* cst = sb + BK_C;
-        const int64_t row0 = (int64_t)b * NF + r0;
-        // ---- tile loads: Y -> A1, h -> A3h ------------------------------------------------------------
-        {
-            const int r = tid >> 5, k4 = tid & 31;
-            const float4 v = (r < nr) ? *reinterpret_cast<const float4*>(Y + (row0 + r) * 128 + k4 * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
-            A1[mid_aidx(M1_KS, k4 * 4 + 0, r)] = v.x; A1[mid_aidx(M1_KS, k4 * 4 + 1, r)] = v.y;
-            A1[mid_aidx(M1_KS, k4 * 4 + 2, r)] = v.z; A1[mid_aidx(M1_KS, k4 * 4 + 3, r)] = v.w;
-        }
-        if (tid < 128) {
-            const int r = tid >> 4, k4 = tid & 15;
-            const float4 v = (r < nr) ? *reinterpret_cast<const float4*>(hst + (r0 + r) * 64 + k4 * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
-            A3h[mid_aidx(M3_KS, k4 * 4 + 0, r)] = v.x; A3h[mid_aidx(M3_KS, k4 * 4 + 1, r)] = v.y;
-            A3h[mid_aidx(M3_KS, k4 * 4 + 2, r)] = v.z; A3h[mid_aidx(M3_KS, k4 * 4 + 3, r)] = v.w;
-        }
-        mbar_wait(&wbar, 0);
-        __syncthreads();
-        // ---- phase 1: X1 = X + Y W1 + b ;  lane (cg, kq) finishes row kq/2, columns cg*4 + (kq&1)*2 + {0,1}
-        float2 x1v;
-        const int r1 = (tid & 15) >> 1, n1 = (tid >> 4) * 4 + (tid & 1) * 2;
-        {
-            float v[MID_RT * M1_C];
-            mid_mm<M1_C, M1_KQ, M1_KS, M1_N>(Wp + MID_W1, A1, tid >> 4, tid & 15, v);
-            const float2 bias = __ldg(reinterpret_cast<const float2*>(w.bl1 + n1));
-            const float2 xo = (r1 < nr) ? *reinterpret_cast<const float2*>(X + (row0 + r1) * 64 + n1) : make_float2(0.f, 0.f);
-            x1v = make_float2(xo.x + v[0] + bias.x, xo.y + v[1] + bias.y);
-            *reinterpret_cast<float2*>(x1s + r1 * 64 + n1) = x1v;
-        }
-        __syncthreads();
-        // ---- phase 2: LayerNorm over channels, one warp per row -> A3 ------------------------------------
-        {
-            const int r = tid >> 5, lane = tid & 31;
-            const float v0 = x1s[r * 64 + lane], v1 = x1s[r * 64 + lane + 32];
-            const float mu = warp_sum(v0 + v1) * (1.f / 64.f);
-            const float d0 = v0 - mu, d1 = v1 - mu;
-            const float rs = rsqrtf(warp_sum(d0 * d0 + d1 * d1) * (1.f / 64.f) + 1e-5f);
-            A3[mid_aidx(M3_KS, lane, r)] = d0 * rs * __ldg(w.ln2_g + lane) + __ldg(w.ln2_b + lane);
-            A3[mid_aidx(M3_KS, lane + 32, r)] = d1 * rs * __ldg(w.ln2_g + lane + 32) + __ldg(w.ln2_b + lane + 32);
-        }
-        __syncthreads();
-        // ---- phase 3 + 4: gates and LSTM cell; lane (jp, kq) finishes row kq, hidden units 2jp, 2jp+1 ----
-        {
-            // two K = 64 products, combined as (x W_ih + b) + h W_hh: the arithmetic of mid_a_kernel + mid_b_kernel
-            float u[MID_RT * M3_C], v[MID_RT * M3_C];
-            const int jp = tid >> 3, r = tid & 7;
-            mid_mm<M3_C, M3_KQ, M3_KS, M3_N>(Wp + MID_W3A, A3, jp, r, u);
-            mid_mm<M3_C, M3_KQ, M3_KS, M3_N>(Wp + MID_W3B, A3h, jp, r, v);
-            const float4 ba = __ldg(reinterpret_cast<const float4*>(w.b2 + jp * 8));
-            const float4 bb = __ldg(reinterpret_cast<const float4*>(w.b2 + jp * 8 + 4));
-            const float4 ga = make_float4(u[0] + ba.x, u[1] + ba.y, u[2] + ba.z, u[3] + ba.w);
-            const float4 gb = make_float4(u[4] + bb.x, u[5] + bb.y, u[6] + bb.z, u[7] + bb.w);
-            const float2 cold = (r < nr) ? *reinterpret_cast<const float2*>(cst + (r0 + r) * 64 + jp * 2) : make_float2(0.f, 0.f);
-            const float gi0 = fast_sigmoid(v[0] + ga.x), gf0 = fast_sigmoid(v[1] + ga.y), gg0 = fast_tanh(v[2] + ga.z), go0 = fast_sigmoid(v[3] + ga.w);
-            const float gi1 = fast_sigmoid(v[4] + gb.x), gf1 = fast_sigmoid(v[5] + gb.y), gg1 = fast_tanh(v[6] + gb.z), go1 = fast_sigmoid(v[7] + gb.w);
-            const float c0 = gf0 * cold.x + gi0 * gg0, c1 = gf1 * cold.y + gi1 * gg1;
-            const float h0 = go0 * fast_tanh(c0), h1 = go1 * fast_tanh(c1);
-            if (r < nr) {
-                *reinterpret_cast<float2*>(cst + (r0 + r) * 64 + jp * 2) = make_float2(c0, c1);
-                *reinterpret_cast<float2*>(hst + (r0 + r) * 64 + jp * 2) = make_float2(h0, h1);
-            }
-            A5[mid_aidx(M5_KS, jp * 2, r)] = h0;
-            A5[mid_aidx(M5_KS, jp * 2 + 1, r)] = h1;
-        }
-        __syncthreads();
-        // ---- phase 5: X2 = X1 + h' W_l2 + b ; same lane -> output mapping as phase 1 -------------------
-        {
-            float v[MID_RT * M5_C];
-            mid_mm<M5_C, M5_KQ, M5_KS, M5_N>(Wp + MID_W5, A5, tid >> 4, tid & 15, v);
-            const float2 bias = __ldg(reinterpret_cast<const float2*>(w.bl2 + n1));
-            const float2 x2v = make_float2(x1v.x + v[0] + bias.x, x1v.y + v[1] + bias.y);
-            if (r1 < nr) *reinterpret_cast<float2*>(X + (row0 + r1) * 64 + n1) = x2v;
-        }
-    }
-}
-
-
-// mid_b + the inter Linear (engine option "fold_mid_c", with qkv_kernel doing its own Q/K/V projection): the serial stage also
-// finishes X2 = X1 + h' W_l2 + b, so that no mid_c launch (and no graph edge for it) is left between it and qkv.
-// Off by default (it lengthens the serial stage of the pipeline); covered by tests/test_sep_gpu.py::test_fold_mid_c_option.
-constexpr size_t MID_B2_SMEM = (size_t)((MID_W5 - MID_W3B) + MID_A3 + (MID_W6 - MID_W5) + MID_A5) * sizeof(float);
-__global__ void __launch_bounds__(256)
-mid_b2_kernel(const float* __restrict__ GI, float* __restrict__ X, int64_t hop_stride, int n_hops, float* __restrict__ state,
-              int64_t sstride, int blk, BlockWeights w, int n_streams) {
-    extern __shared__ __align__(16) float sm[];
-    float* W3b = sm;                                  // W_hh, k-sliced
-    float* A3 = W3b + (MID_W5 - MID_W3B);             // h, k-sliced
-    float* W5 = A3 + MID_A3;                          // inter linear, k-sliced
-    float* A5 = W5 + (MID_W6 - MID_W5);               // h', k-sliced for the linear
-    __shared__ __align__(8) unsigned long long wbar;
-    TraceScope trace_(TK_MID_B, GI);
-    griddep_launch();
-    const int tid = threadIdx.x;
-    constexpr int TILES = (NF + MID_RT - 1) / MID_RT;
-    if (tid == 0) {
-        mbar_init(&wbar, 1);
-        mbar_fence_init();
-        mbar_expect_tx(&wbar, ((MID_W5 - MID_W3B) + (MID_W6 - MID_W5)) * 4);
-        tma_load_1d(W3b, w.mid_pack + MID_W3B, (MID_W5 - MID_W3B) * 4, &wbar);
-        tma_load_1d(W5, w.mid_pack + MID_W5, (MID_W6 - MID_W5) * 4, &wbar);
-    }
-    __syncthreads();
-    griddep_wait();
-    for (int item = blockIdx.x; item < n_streams * TILES; item += gridDim.x) {
-        const int b = item / TILES;
-        const int r0 = (item % TILES) * MID_RT;
-        const int nr = min(MID_RT, NF - r0);
-        __syncthreads();
-        float* sb = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride + ST_BLK + (int64_t)blk * BK_STRIDE;
-        float* hst = sb + BK_H;
-        float* cst = sb + BK_C;
-        const int64_t row0 = (int64_t)b * NF + r0;
-        if (tid < 128) {
-            const int r = tid >> 4, k4 = tid & 15;
-            const float4 v = (r < nr) ? *reinterpret_cast<const float4*>(hst + (r0 + r) * 64 + k4 * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
-            A3[mid_aidx(M3_KS, k4 * 4 + 0, r)] = v.x; A3[mid_aidx(M3_KS, k4 * 4 + 1, r)] = v.y;
-            A3[mid_aidx(M3_KS, k4 * 4 + 2, r)] = v.z; A3[mid_aidx(M3_KS, k4 * 4 + 3, r)] = v.w;
-        }
-        const int jp = tid >> 3, r = tid & 7;
-        const bool live = r < nr;
-        const int r1 = (tid & 15) >> 1, n1 = (tid >> 4) * 4 + (tid & 1) * 2;      // this lane's outputs of the linear
-        float2 cc = live ? *reinterpret_cast<const float2*>(cst + (r0 + r) * 64 + jp * 2) : make_float2(0.f, 0.f);
-        float2 hh = make_float2(0.f, 0.f);
-        const float4* gp = reinterpret_cast<const float4*>(GI + (row0 + r) * 256 + jp * 8);
-        float4 ga = make_float4(0.f, 0.f, 0.f, 0.f), gb = ga;
-        if (live) { ga = gp[0]; gb = gp[1]; }
-        const float2 bias5 = __ldg(reinterpret_cast<const float2*>(w.bl2 + n1));
-        mbar_wait(&wbar, 0);
-        for (int j = 0; j < n_hops; ++j) {
-            __syncthreads();                          // h of this hop is in A3; the previous hop's linear is done with A5
-            float4 na = make_float4(0.f, 0.f, 0.f, 0.f), nb = na;
-            if (live && j + 1 < n_hops) {
-                const float4* np = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(gp) + (int64_t)(j + 1) * hop_stride);
-                na = np[0]; nb = np[1];
-            }
-            float* Xj = X + (int64_t)j * hop_stride;
-            const float2 x1v = (r1 < nr) ? *reinterpret_cast<const float2*>(Xj + (row0 + r1) * 64 + n1) : make_float2(0.f, 0.f);
-            float v[MID_RT * M3_C];
-            mid_mm<M3_C, M3_KQ, M3_KS, M3_N>(W3b, A3, jp, r, v);
-            const float gi0 = fast_sigmoid(v[0] + ga.x), gf0 = fast_sigmoid(v[1] + ga.y), gg0 = fast_tanh(v[2] + ga.z), go0 = fast_sigmoid(v[3] + ga.w);
-            const float gi1 = fast_sigmoid(v[4] + gb.x), gf1 = fast_sigmoid(v[5] + gb.y), gg1 = fast_tanh(v[6] + gb.z), go1 = fast_sigmoid(v[7] + gb.w);
-            cc = make_float2(gf0 * cc.x + gi0 * gg0, gf1 * cc.y + gi1 * gg1);
-            hh = make_float2(go0 * fast_tanh(cc.x), go1 * fast_tanh(cc.y));
-            ga = na; gb = nb;
-            __syncthreads();                          // every lane has read the old h
-            A3[mid_aidx(M3_KS, jp * 2, r)] = hh.x;
-            A3[mid_aidx(M3_KS, jp * 2 + 1, r)] = hh.y;
-            A5[mid_aidx(M5_KS, jp * 2, r)] = hh.x;
-            A5[mid_aidx(M5_KS, jp * 2 + 1, r)] = hh.y;
-            __syncthreads();
-            float u[MID_RT * M5_C];
-            mid_mm<M5_C, M5_KQ, M5_KS, M5_N>(W5, A5, tid >> 4, tid & 15, u);
-            if (r1 < nr) *reinterpret_cast<float2*>(Xj + (row0 + r1) * 64 + n1) = make_float2(x1v.x + u[0] + bias5.x, x1v.y + u[1] + bias5.y);
-        }
-        if (live) {
-            *reinterpret_cast<float2*>(cst + (r0 + r) * 64 + jp * 2) = cc;
-            *reinterpret_cast<float2*>(hst + (r0 + r) * 64 + jp * 2) = hh;
-        }
-    }
-}
-
 }  // namespace l2h

@@ -41,11 +41,9 @@ struct SepEngine {
     int n_blocks;
     WeightPack pack;                // packed weights; pack.device also owns the streams, events and cached graphs below
     int64_t weight_gen = 0;         // bumped by every commit
-    bool graph_stats = false;
     std::vector<int64_t> plane_of;      // per block: plane offsets (pack.plane) of wih1, wl1, wih2, wl2, wqkv, [wih2|whh2], wp
     bool cur_pdl = false;              // PDL attribute for the tensor-core launches of the chain being enqueued
     bool fuse_ih = false;               // many sequences: W_ih + LayerNorm inside the tensor-core recurrence (option "fuse_ih", default off)
-    bool use_tc = true;                 // rows > TC_MIN_ROWS: dense contractions on the tensor cores, wgmma (option "tensor_cores")
     int tc_passes = 3;                  // 3 = bf16x3 split products (fp32 configs); 2 = bf16 weights x split activations (option
                                         // "bf16" = 1: the offline bf16 configuration); 1 = plain bf16 operands ("bf16" = 2)
     SepWeights w;
@@ -67,9 +65,7 @@ struct SepEngine {
     int pipe_alanes = 12;    // BiLSTM (stage A) hops in flight per block (<= PIPE_LANES)
     int pipe_gemm_shape = 0; // tile shape of the pipelined W_ih GEMM (gemm.cuh: launch_rows_gemm), option "pipeline_gemm_shape"
     int pipe_midb_hops = 4;       // pipeline: consecutive hops one mid_b launch takes (<= PIPE_MIDB_MAX)
-    int pipe_skip = 0;            // DEBUG (timing experiments only): bit mask of pipeline stages NOT to launch
     int pipe_pdl = 16;            // pipeline: stages launched with programmatic dependent launch (bit mask; 16 = mid_b)
-    bool pipe_split_mid = true;   // pipeline: mid section as mid_a | mid_b (serial) | mid_c
     int pipe_qlanes = 3;     // qkv hops in flight per block (<= PIPE_QLANES)
     int pipe_clanes = 2;     // mid_c hops in flight per block (<= PIPE_CLANES)
     int pipe_tlanes = 3;     // attention hops in flight per block (<= PIPE_TLANES)
@@ -77,9 +73,6 @@ struct SepEngine {
     int pipe_flanes = 6;     // front_kernel hops in flight (<= PIPE_FLANES)
     int pipe_blanes = 6;     // back_kernel hops in flight (<= PIPE_BLANES)
     bool use_pipe = true;    // wavefront pipelining of one-frame calls inside a multi-frame graph (option "pipeline")
-    bool fold_mid_c = false;      // no mid_c / no projection in the mid kernels: Linear in mid_b2, Q/K/V projection in qkv (untested)
-    bool mid_split_large = true;  // many streams: run the fused mid section as mid_a | mid_b | mid_c (2-4 CTAs per SM)
-    bool use_mid = true;     // fused row-local mid-section for one-frame calls (option "fused_mid")
     int tcl_min_seqdirs = TCL_MIN_SEQDIRS;  // (sequence, direction) pairs from which the recurrence runs on the tensor cores (option "tc_lstm_min")
     int tc_pdl = 7;              // programmatic dependent launch around the tensor-core GEMMs of many-row calls: bit 0 the many-stream mid section, bit 1 W_ih and the out projection + its LayerNorm kernel, bit 2 the persistent qkv kernel (PDL on EVERY kernel of that chain parks early-launched dependents on the SMs the big kernels need; option "tc_pdl")
     bool use_back_many = true;   // calls of several frames: front_many_kernel / back_many_kernel (one CTA / cluster per chunk of frames) instead of one per frame (option "back_many")
@@ -264,8 +257,6 @@ static int set_attrs() {
     CK(cudaFuncSetAttribute(front_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FRONT_SMEM));
     CK(cudaFuncSetAttribute(front_many_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FRONT_SMEM));
     CK(cudaFuncSetAttribute(mid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_SMEM));
-    CK(cudaFuncSetAttribute(mid_noproj_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_SMEM));
-    CK(cudaFuncSetAttribute(mid_b2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_B2_SMEM));
     CK(cudaFuncSetAttribute(mid_a_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_A_SMEM));
     CK(cudaFuncSetAttribute(mid_b_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_B_SMEM));
     CK(cudaFuncSetAttribute(mid_c_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_C_SMEM));
@@ -304,13 +295,13 @@ static umma::BPlanes tc_planes(const SepEngine* e, int blk, int which, int ld) {
 
 // the recurrence: tensor cores when there are enough sequences to fill the GPU with 32-sequence CTAs, else lstm.cuh
 static cudaError_t lstm_any(SepEngine* e, const LstmArgs& l, cudaStream_t st, bool pdl) {
-    if (e->use_tc && (int64_t)l.nseq * l.ndir >= e->tcl_min_seqdirs) return launch_tc_lstm(l, e->tc_passes, st, pdl);
+    if ((int64_t)l.nseq * l.ndir >= e->tcl_min_seqdirs) return launch_tc_lstm(l, e->tc_passes, st, pdl);
     return launch_lstm_rec(l, st, pdl);
 }
 
 // ... and with enough sequences the input projection moves into the recurrence kernel too (tc_lstm_x_kernel)
 static bool tc_fused_lstm(const SepEngine* e, const LstmArgs& l) {
-    return e->use_tc && e->fuse_ih && (int64_t)l.nseq * l.ndir >= e->tcl_min_seqdirs;
+    return e->fuse_ih && (int64_t)l.nseq * l.ndir >= e->tcl_min_seqdirs;
 }
 
 // C[rows][N] = epi(LN?(A[rows][lda, first K]) W^T + bias) (+ R), plain row-major rows
@@ -371,13 +362,13 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
     const int nsplit = attn_splits(B, T);
     // one-frame calls: the row-local middle of every block runs as ONE fused kernel (mid_kernel.cuh).
     // (Taps want the intermediate activations of the generic chain, so they keep it.)
-    const bool fused_mid = (T == 1) && e->use_mid && !(flags & L2H_FLAG_TAPS);
+    const bool row_mid = (T == 1) && !(flags & L2H_FLAG_TAPS);
     // many rows (whole utterances, offline batches, many streams): the dense contractions run on the tensor cores
-    const bool tc = e->use_tc && rows > TC_MIN_ROWS;
+    const bool tc = rows > TC_MIN_ROWS;
     const bool tc_mid = tc && T == 1 && !(flags & L2H_FLAG_TAPS);
     // few streams, one hop (the latency path): everything after the BiLSTM as one cluster kernel per stream
     bool fused_tail = false;
-    if (fused_mid && !tc && e->use_tail && !e->fold_mid_c) {
+    if (row_mid && !tc && e->use_tail) {
         int dev_ord = 0;
         CK(cudaGetDevice(&dev_ord));
         fused_tail = B <= g_tail_clusters[dev_ord];      // all clusters of the launch resident at once
@@ -392,7 +383,7 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
     };
     float* sbase = state + sizeof(StateHeader) / 4;
     // programmatic dependent launch pays on the latency chain of a few rows; with many rows early-launched dependents park on the SMs the big kernels need
-    const bool pdl = e->use_pdl && a.prof == nullptr && !(flags & L2H_FLAG_TAPS) && !(e->use_tc && rows > TC_MIN_ROWS);
+    const bool pdl = e->use_pdl && a.prof == nullptr && !(flags & L2H_FLAG_TAPS) && !tc;
     e->cur_pdl = false;
 #define MARK(name) do { if (a.prof) { if (int _rc = a.prof->mark(name, st)) return _rc; } } while (0)
     MARK("start");
@@ -474,15 +465,11 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
             if (int rc = tc_rows_gemm(e, b, PL_QKV, X, 64, 64, NQKV, nullptr, nullptr, W.bqkv, W.slope_vec, nullptr, QKVRAW, NQKV, rows, st)) return rc;
             e->cur_pdl = false;
             MARK("mid");
-        } else if (fused_mid && mid_split_for_throughput(B) && e->mid_split_large) {
+        } else if (row_mid && mid_split_for_throughput(B)) {
             float* GI = GX; float* HN = GX + rows * 256;         // the BiLSTM is done with GX
             CK(launch_k(pdl, mid_a_kernel, mid_grid_for(B, 2), dim3(256), MID_A_SMEM, st, (const float*)Y, X, GI, W, B, (int64_t)0, 1));
-            if (e->fold_mid_c) {
-                CK(launch_k(pdl, mid_b2_kernel, mid_grid_for(B, 2), dim3(256), MID_B2_SMEM, st, (const float*)GI, X, (int64_t)0, 1, state, ss, b, W, B));
-            } else {
-                CK(launch_k(pdl, mid_b_kernel, mid_grid_for(B, 3), dim3(256), MID_B_SMEM, st, (const float*)GI, HN, (int64_t)0, 1, state, ss, b, W, B));
-                CK(launch_k(pdl, mid_c_kernel, mid_grid_for(B, 4), dim3(256), MID_C_SMEM, st, (const float*)HN, X, QKVRAW, W, B, (int64_t)0, 1));
-            }
+            CK(launch_k(pdl, mid_b_kernel, mid_grid_for(B, 3), dim3(256), MID_B_SMEM, st, (const float*)GI, HN, (int64_t)0, 1, state, ss, b, W, B));
+            CK(launch_k(pdl, mid_c_kernel, mid_grid_for(B, 4), dim3(256), MID_C_SMEM, st, (const float*)HN, X, QKVRAW, W, B, (int64_t)0, 1));
             MARK("mid");
         } else if (fused_tail) {
             NextIh nx{};
@@ -495,11 +482,8 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
             MARK("tail");
             if (int rc = do_tap()) return rc;
             continue;
-        } else if (fused_mid) {
-            if (e->fold_mid_c)
-                CK(launch_k(pdl, mid_noproj_kernel, mid_grid_for(B, 1), dim3(256), MID_SMEM, st, (const float*)Y, X, QKVRAW, state, ss, b, W, B));
-            else
-                CK(launch_k(pdl, mid_kernel, mid_grid_for(B, 1), dim3(256), MID_SMEM, st, (const float*)Y, X, QKVRAW, state, ss, b, W, B));
+        } else if (row_mid) {
+            CK(launch_k(pdl, mid_kernel, mid_grid_for(B, 1), dim3(256), MID_SMEM, st, (const float*)Y, X, QKVRAW, state, ss, b, W, B));
             MARK("mid");
         } else {
             if (tc) {
@@ -567,7 +551,7 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
                         b, W, T, B * T));
         } else {
             CK(launch_k(pdl, qkv_kernel, dim3(T, B), dim3(QKV_THREADS), QKV_SMEM, st, (const float*)X,
-                        (const float*)((tc || (fused_mid && !e->fold_mid_c)) ? QKVRAW : nullptr), Q, KALL, VALL, state, ss, b, W, T, 0));
+                        (const float*)((tc || row_mid) ? QKVRAW : nullptr), Q, KALL, VALL, state, ss, b, W, T, 0));
         }
         MARK("qkv");
         if (nsplit > 1) {
@@ -618,8 +602,9 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
 // ---- wavefront pipeline over (block, frame) for one-frame calls ---------------------------------------
 // Work item (block b, hop t) depends only on (b-1, t) and (b, t-1) (SURVEY.md 3.3), and inside a block
 // only part of the work carries state from hop to hop:
-//   A   = W_ih GEMM + 97-step BiLSTM        needs X_t only            -> PIPE_LANES hops of it run side by side
-//   B1  = mid_kernel (inter-LSTM step ...)   carries (h, c)            -> serial per block
+//   A   = W_ih GEMM + 97-step BiLSTM + mid_a needs X_t only           -> PIPE_LANES hops of it run side by side
+//   B1  = mid_b (inter-LSTM step)            carries (h, c)            -> serial per block
+//   Bc  = mid_c (inter Linear + Q|K|V)       needs h'_t, X_t only
 //   B2a = qkv + attention                    carries the K/V rings     -> serial per block
 //   B2b = attn_out                           needs Z_t, X_t only
 // A graph of K consecutive one-hop chains is captured on 1 + 3*(PIPE_LANES+3) + 1 streams with event edges
@@ -671,10 +656,8 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
     // tail; every kernel reaches griddepcontrol.wait before it touches activations or state.  Worth it only on the
     // serial stage (mid_b -> mid_b of the next hop): everywhere, the parked dependents hold shared memory and CTA
     // slots the running kernels need
-    const int ppdl = e->pipe_pdl;         // stage bit mask (same bits as pipe_skip)
-    const bool fold = e->fold_mid_c;
+    const int ppdl = e->pipe_pdl;         // stage bit mask (bits: include/lookonce_b200.h, l2h_sep_set_option)
     const bool many = mid_split_for_throughput(B);
-    const bool split_mid = many ? e->mid_split_large : e->pipe_split_mid;
     float* state = a.state;
     for (int i = 0; i < PIPE_STREAMS; ++i)
         if (!e->pipe_streams[i]) CK(cudaStreamCreateWithFlags(&e->pipe_streams[i], cudaStreamNonBlocking));
@@ -725,7 +708,7 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
     // The serial stage (mid_b) takes `mb` consecutive hops per launch: its launch overhead and its 64 KB of
     // weights are paid once per batch, h stays in shared memory and c in registers from hop to hop.  A batch waits
     // for stage A of all its hops; the upstream block is that far ahead anyway once the pipeline is full.
-    const int mb = (split_mid && !many) ? std::max(1, std::min(e->pipe_midb_hops, PIPE_MIDB_MAX)) : 1;
+    const int mb = many ? 1 : std::max(1, std::min(e->pipe_midb_hops, PIPE_MIDB_MAX));
     float* PRE = a.wsp + ws.PRE;                                       // speaker-gate scratch: front stream only
     for (int k0 = 0; k0 < K; k0 += mb) {
         const int k1 = std::min(K, k0 + mb);                           // this batch: hops [k0, k1)
@@ -744,8 +727,8 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
                         // position the device derives from the state header)
                         cudaStream_t sF = sFront(k);
                         // the speaker-gate memo CTA (blockIdx.x == 1) rides with hop 0 only: one builder of ST_GATE per group
-                        if (!(e->pipe_skip & 1)) CK(launch_k((ppdl & 1) != 0, front_kernel, dim3(k == 0 ? 2 : 1, B), dim3(256), FRONT_SMEM, sF, a.x, a.xbs, a.xcs,
-                                                             a.x_len, a.wsp + (int64_t)k * slot + ws.X, state, ss, e->w, 1, a.pos_rel, a.emb, PRE, k, K, k * HOP));
+                        CK(launch_k((ppdl & 1) != 0, front_kernel, dim3(k == 0 ? 2 : 1, B), dim3(256), FRONT_SMEM, sF, a.x, a.xbs, a.xcs,
+                                    a.x_len, a.wsp + (int64_t)k * slot + ws.X, state, ss, e->w, 1, a.pos_rel, a.emb, PRE, k, K, k * HOP));
                         if (k == 0) {                  // ... and every attn_out lane of block 0 (the gate's only reader) waits for it once
                             cudaEvent_t gate_ev;
                             if (int rc = record(&gate_ev, sF)) return rc;
@@ -760,16 +743,15 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
                 g.A = X; g.lda = 64; g.a_rows_per_seq = rows; g.a_seq_stride = slot;
                 g.Wt = W.wih1_t; g.bias = W.b1; g.C = GX; g.ldc = 512; g.c_rows_per_seq = rows; g.c_seq_stride = slot;
                 g.ln_g = W.ln1_g; g.ln_b = W.ln1_b; g.M = rows * nh; g.N = 512; g.K = 64;
-                if (!(e->pipe_skip & 2)) CK(launch_rows_gemm(g, st_a, (ppdl & 2) != 0, e->pipe_gemm_shape));
+                CK(launch_rows_gemm(g, st_a, (ppdl & 2) != 0, e->pipe_gemm_shape));
                 LstmArgs l{};
                 l.gx = GX; l.gx_ld = 512; l.out = Y; l.out_ld = 128; l.whh = W.whh1;
                 l.nseq = B * nh; l.L = NF; l.inner_count = B; l.outer_stride = slot / 512; l.inner_stride = NF; l.step_stride = 1;
                 l.out_outer_stride = slot / 128; l.out_inner_stride = NF; l.out_step_stride = 1; l.ndir = 2;
-                if (!(e->pipe_skip & 4)) CK(launch_lstm_rec(l, st_a, (ppdl & 4) != 0));
+                CK(launch_lstm_rec(l, st_a, (ppdl & 4) != 0));
                 // only the W_hh product + cell (mid_b) is serial per block; the rest rides on the parallel lanes.
                 // GI / H' live in the hop's GX slot, which the BiLSTM has finished with.
-                if (split_mid && !(e->pipe_skip & 8))
-                    CK(launch_k((ppdl & 8) != 0, mid_a_kernel, mid_grid_for(B * nh, 2), dim3(256), MID_A_SMEM, st_a, (const float*)Y, X, GX, W, B, slot, nh));
+                CK(launch_k((ppdl & 8) != 0, mid_a_kernel, mid_grid_for(B * nh, 2), dim3(256), MID_A_SMEM, st_a, (const float*)Y, X, GX, W, B, slot, nh));
                 cudaEvent_t ev_a;
                 if (int rc = record(&ev_a, st_a)) return rc;
                 for (int k = k0; k < k1; ++k) a_done[b][k] = ev_a;
@@ -779,36 +761,19 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
             {
                 float* wsp = a.wsp + (int64_t)k0 * slot;
                 float* GI = wsp + ws.GX; float* HN = GI + (int64_t)rows * 256;
-                if (split_mid && fold) {
-                    if (!(e->pipe_skip & 16))
-                        CK(launch_k((ppdl & 16) != 0, mid_b2_kernel, mid_grid_for(B, 2), dim3(256), MID_B2_SMEM, sB1(b), (const float*)GI, wsp + ws.X,
-                                    slot, k1 - k0, state, ss, b, W, B));
-                } else if (split_mid) {
-                    if (!(e->pipe_skip & 16))
-                        CK(launch_k((ppdl & 16) != 0, mid_b_kernel, mid_grid_for(B, 3), dim3(256), MID_B_SMEM, sB1(b), (const float*)GI, HN, slot,
-                                    k1 - k0, state, ss, b, W, B));
-                } else if (!(e->pipe_skip & 16)) {
-                    if (fold)
-                        CK(launch_k((ppdl & 16) != 0, mid_noproj_kernel, mid_grid_for(B, 1), dim3(256), MID_SMEM, sB1(b), (const float*)(wsp + ws.Y),
-                                    wsp + ws.X, wsp + ws.QKVRAW, state, ss, b, W, B));
-                    else
-                        CK(launch_k((ppdl & 16) != 0, mid_kernel, mid_grid_for(B, 1), dim3(256), MID_SMEM, sB1(b), (const float*)(wsp + ws.Y),
-                                    wsp + ws.X, wsp + ws.QKVRAW, state, ss, b, W, B));
-                }
+                CK(launch_k((ppdl & 16) != 0, mid_b_kernel, mid_grid_for(B, 3), dim3(256), MID_B_SMEM, sB1(b), (const float*)GI, HN, slot,
+                            k1 - k0, state, ss, b, W, B));
             }
             cudaEvent_t midb_done;
             if (int rc = record(&midb_done, sB1(b))) return rc;
             // ---- mid_c for the whole batch (one launch), then per hop: qkv -> attention -> attn_out (lanes, ring guards) ----
-            cudaEvent_t midc_done = midb_done;
-            if (split_mid && !fold) {
-                cudaStream_t st_c = sBc(b, k0 / mb);
-                float* wsp0 = a.wsp + (int64_t)k0 * slot;
-                CK(cudaStreamWaitEvent(st_c, midb_done, 0));
-                if (!(e->pipe_skip & 32))
-                    CK(launch_k((ppdl & 32) != 0, mid_c_kernel, mid_grid_for(B * (k1 - k0), 4), dim3(256), MID_C_SMEM, st_c,
-                                (const float*)(wsp0 + ws.GX + (int64_t)rows * 256), wsp0 + ws.X, wsp0 + ws.QKVRAW, W, B, slot, k1 - k0));
-                if (int rc = record(&midc_done, st_c)) return rc;
-            }
+            cudaStream_t st_c = sBc(b, k0 / mb);
+            float* wsp0 = a.wsp + (int64_t)k0 * slot;
+            CK(cudaStreamWaitEvent(st_c, midb_done, 0));
+            CK(launch_k((ppdl & 32) != 0, mid_c_kernel, mid_grid_for(B * (k1 - k0), 4), dim3(256), MID_C_SMEM, st_c,
+                        (const float*)(wsp0 + ws.GX + (int64_t)rows * 256), wsp0 + ws.X, wsp0 + ws.QKVRAW, W, B, slot, k1 - k0));
+            cudaEvent_t midc_done;
+            if (int rc = record(&midc_done, st_c)) return rc;
             for (int k = k0; k < k1; ++k) {
                 float* wsp = a.wsp + (int64_t)k * slot;
                 float* X = wsp + ws.X; float* Z = wsp + ws.Z; float* Q = wsp + ws.Q; float* QKVRAW = wsp + ws.QKVRAW;
@@ -818,24 +783,24 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
                 // attention (one per attention lane) must be done
                 for (int d = 0; d < e->pipe_tlanes && k - PIPE_QKV_AHEAD - 1 - d >= 0; ++d)
                     CK(cudaStreamWaitEvent(st_q, att_done[b][k - PIPE_QKV_AHEAD - 1 - d], 0));
-                if (!(e->pipe_skip & 64)) CK(launch_k((ppdl & 64) != 0, qkv_kernel, dim3(1, B), dim3(QKV_THREADS), QKV_SMEM, st_q, (const float*)X,
-                                                      (const float*)(fold ? nullptr : QKVRAW), Q, (float*)nullptr, (float*)nullptr, state, ss, b, W, 1, k));
+                CK(launch_k((ppdl & 64) != 0, qkv_kernel, dim3(1, B), dim3(QKV_THREADS), QKV_SMEM, st_q, (const float*)X,
+                            (const float*)QKVRAW, Q, (float*)nullptr, (float*)nullptr, state, ss, b, W, 1, k));
                 if (int rc = record(&qkv_done[b][k], st_q)) return rc;
                 // the attention reads this hop's ring row and the 49 before it: the other qkv lanes' latest hops must be in
                 cudaStream_t st_t = sBa(b, k);
                 for (int d = 0; d < e->pipe_qlanes && d <= k; ++d) CK(cudaStreamWaitEvent(st_t, qkv_done[b][k - d], 0));
                 if (nsplit > 1) {
-                    if (!(e->pipe_skip & 128)) CK(launch_cluster((ppdl & 128) != 0, dim3(1, ATT_CL, 1), attn_cluster_kernel, dim3(1, NHEAD * ATT_CL, B),
-                                                                 dim3(256), 0, st_t, (const float*)Q, (const float*)nullptr, (const float*)nullptr,
-                                                                 (const float*)state, ss, b, Z, 1, k));
+                    CK(launch_cluster((ppdl & 128) != 0, dim3(1, ATT_CL, 1), attn_cluster_kernel, dim3(1, NHEAD * ATT_CL, B),
+                                      dim3(256), 0, st_t, (const float*)Q, (const float*)nullptr, (const float*)nullptr,
+                                      (const float*)state, ss, b, Z, 1, k));
                 } else {
-                    if (!(e->pipe_skip & 128)) CK(launch_k((ppdl & 128) != 0, attn_kernel, dim3(1, NHEAD, B), dim3(256), 0, st_t, (const float*)Q,
-                                                           (const float*)nullptr, (const float*)nullptr, (const float*)state, ss, b, Z, 1, k));
+                    CK(launch_k((ppdl & 128) != 0, attn_kernel, dim3(1, NHEAD, B), dim3(256), 0, st_t, (const float*)Q,
+                                (const float*)nullptr, (const float*)nullptr, (const float*)state, ss, b, Z, 1, k));
                 }
                 if (int rc = record(&att_done[b][k], st_t)) return rc;
                 CK(cudaStreamWaitEvent(sBo(b, k), att_done[b][k], 0));
-                if (!(e->pipe_skip & 256)) CK(launch_k((ppdl & 256) != 0, attn_out_kernel, dim3(1, B), dim3(256), AOUT_SMEM, sBo(b, k), (const float*)Z, X,
-                                                       (const float*)state, ss, W, b == 0 ? 1 : 0, 1));
+                CK(launch_k((ppdl & 256) != 0, attn_out_kernel, dim3(1, B), dim3(256), AOUT_SMEM, sBo(b, k), (const float*)Z, X,
+                            (const float*)state, ss, W, b == 0 ? 1 : 0, 1));
                 if (int rc = record(&out_done[b][k], sBo(b, k))) return rc;
             }
         }
@@ -844,8 +809,8 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
             cudaStream_t sBack = sBackL(k);
             // this hop's output and the three before it (deconv / overlap-add context) sit on different attn_out lanes
             for (int d = 0; d <= 3 && d <= k; ++d) CK(cudaStreamWaitEvent(sBack, out_done[2][k - d], 0));
-            if (!(e->pipe_skip & 512)) CK(launch_cluster((ppdl & 512) != 0, dim3(BACK_CL, 1, 1), back_kernel, dim3(BACK_CL, B), dim3(256), BACK_SMEM, sBack,
-                                                         (const float*)X, a.y, a.ybs, a.ycs, a.y_len, state, ss, e->w, 1, a.pos_rel, k, K, k * HOP, slot));
+            CK(launch_cluster((ppdl & 512) != 0, dim3(BACK_CL, 1, 1), back_kernel, dim3(BACK_CL, B), dim3(256), BACK_SMEM, sBack,
+                              (const float*)X, a.y, a.ybs, a.ycs, a.y_len, state, ss, e->w, 1, a.pos_rel, k, K, k * HOP, slot));
         }
     }
     for (int i = 1; i < PIPE_STREAMS; ++i)                             // join
@@ -881,11 +846,9 @@ static std::vector<int64_t> graph_key(const ChainArgs& a, int t) {
 }
 
 // Launch the graph cached under `key` on `st`.  The first time a key is seen, `enqueue(cap)` is captured on the private
-// stream `cap` (made on first use) and instantiated; at most 32 graphs are kept.  `census_hops` > 0 marks a pipelined
-// graph, whose node / edge census option "graph_stats" prints.
+// stream `cap` (made on first use) and instantiated; at most 32 graphs are kept.
 template <class Enqueue>
-static int run_graph(SepEngine* e, const std::vector<int64_t>& key, cudaStream_t& cap, cudaStream_t st, Enqueue enqueue,
-                     int census_hops = 0) {
+static int run_graph(SepEngine* e, const std::vector<int64_t>& key, cudaStream_t& cap, cudaStream_t st, Enqueue enqueue) {
     auto it = e->graphs.find(key);
     if (it == e->graphs.end()) {
         if (!e->pack.committed) return fail(4, "weights not committed");
@@ -898,18 +861,6 @@ static int run_graph(SepEngine* e, const std::vector<int64_t>& key, cudaStream_t
         const cudaError_t ce = cudaStreamEndCapture(cap, &graph);
         if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
         if (ce != cudaSuccess) return fail(3, std::string("cudaStreamEndCapture: ") + cudaGetErrorString(ce));
-        if (census_hops > 0 && e->graph_stats) {
-            size_t n_nodes = 0, n_edges = 0;
-            cudaGraphGetNodes(graph, nullptr, &n_nodes);
-            cudaGraphGetEdges_v2(graph, nullptr, nullptr, nullptr, &n_edges);
-            std::vector<cudaGraphNode_t> from(n_edges), to(n_edges);
-            std::vector<cudaGraphEdgeData> ed(n_edges);
-            cudaGraphGetEdges_v2(graph, from.data(), to.data(), ed.data(), &n_edges);
-            size_t prog = 0;
-            for (const auto& d : ed) prog += (d.type == cudaGraphDependencyTypeProgrammatic) ? 1 : 0;
-            fprintf(stderr, "[l2h] pipeline graph: hops %d, nodes %zu, edges %zu, programmatic edges %zu\n", census_hops, n_nodes,
-                    n_edges, prog);
-        }
         cudaGraphExec_t exec = nullptr;
         const int nk = count_kernel_nodes(graph);
         CK(cudaGraphInstantiate(&exec, graph, 0));
@@ -923,7 +874,7 @@ static int run_graph(SepEngine* e, const std::vector<int64_t>& key, cudaStream_t
 
 // K chained one-frame calls as one pipelined graph
 static int run_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_t st) {
-    return run_graph(e, graph_key(a, -K), e->pipe_streams[0], st, [&](cudaStream_t origin) { return enqueue_pipeline(e, a, K, origin); }, K);
+    return run_graph(e, graph_key(a, -K), e->pipe_streams[0], st, [&](cudaStream_t origin) { return enqueue_pipeline(e, a, K, origin); });
 }
 
 // Launch the chain directly, or replay it from a cached CUDA graph (graph launches go to the caller's stream).
@@ -1103,13 +1054,12 @@ int l2h_sep_launches_per_forward(void* handle, int32_t frames, int32_t* n) {
     // one l2h_sep_forward: a one-hop call is 6 kernels per block (gemm, bilstm, mid, qkv, attn, attn_out; 8 with many
     // streams, where the mid section runs as three kernels), a multi-hop call 10.  Streams of one-hop calls go through
     // the pipelined graph instead -- l2h_sep_launch_count has the exact figure for everything this handle launched.
-    const int one_hop = e->use_mid ? 6 : 9;
     int dev_ord = 0;
     cudaGetDevice(&dev_ord);
-    if (frames == 1 && e->use_mid && e->use_tail && !e->fold_mid_c && dev_ord >= 0 && dev_ord < 64 && g_tail_clusters[dev_ord] > 0)
+    if (frames == 1 && e->use_tail && dev_ord >= 0 && dev_ord < 64 && g_tail_clusters[dev_ord] > 0)
         *n = 1 + e->n_blocks * 2 + 1;       // front1, (BiLSTM, tail_kernel) per block, back
     else
-        *n = 1 + e->n_blocks * (frames == 1 ? one_hop : 10) + 1;
+        *n = 1 + e->n_blocks * (frames == 1 ? 6 : 10) + 1;
     return 0;
 }
 
@@ -1169,8 +1119,8 @@ int l2h_sep_forward(void* handle, const float* x, int64_t xbs, int64_t xcs, int3
 // One-hop calls are pipelined over hops (wavefront graph) only for FEW streams: with many streams every kernel of a hop
 // already fills the GPU, the dense stages run on the tensor cores (enqueue_chain) and the hops replay one chain graph.
 static bool pipeline_applies(const SepEngine* e, int batch, int cpc, int n_calls) {
-    if (!(cpc == 1 && e->use_pipe && e->use_mid && e->n_blocks == 3 && n_calls > 1)) return false;
-    return !(e->use_tc && (int64_t)batch * NF > TC_MIN_ROWS);
+    if (!(cpc == 1 && e->use_pipe && e->n_blocks == 3 && n_calls > 1)) return false;
+    return (int64_t)batch * NF <= TC_MIN_ROWS;
 }
 
 int l2h_sep_stream_host(void* handle, const float* x_host, int32_t x_len, const float* emb, void* state,
@@ -1259,20 +1209,18 @@ int l2h_sep_set_option(void* handle, const char* name, int32_t value) {
     SepEngine* e = static_cast<SepEngine*>(handle);
     if (!e || !name) return fail(1, "bad argument");
     const std::string n(name);
-    if (n == "defaults") {                      // lane counts and mid split back to the built-in defaults
+    if (n == "defaults") {                      // pipeline settings back to the built-in defaults
         const SepEngine d{};
         e->pipe_alanes = d.pipe_alanes; e->pipe_qlanes = d.pipe_qlanes; e->pipe_clanes = d.pipe_clanes; e->pipe_tlanes = d.pipe_tlanes;
         e->pipe_olanes = d.pipe_olanes; e->pipe_flanes = d.pipe_flanes; e->pipe_blanes = d.pipe_blanes;
-        e->pipe_split_mid = d.pipe_split_mid; e->pipe_frames = d.pipe_frames; e->pipe_skip = 0; e->pipe_pdl = d.pipe_pdl; e->pipe_midb_hops = d.pipe_midb_hops;
+        e->pipe_frames = d.pipe_frames; e->pipe_pdl = d.pipe_pdl; e->pipe_midb_hops = d.pipe_midb_hops;
     }
     else if (n == "pipeline") e->use_pipe = value != 0;
     else if (n == "pipeline_frames") e->pipe_frames = value <= 0 ? 0 : std::max(2, std::min(PIPE_MAX_FRAMES, (int)value));
     else if (n == "pipeline_lanes") e->pipe_alanes = std::max(1, std::min(PIPE_LANES, (int)value));
-    else if (n == "pipeline_debug_skip") e->pipe_skip = value;
     else if (n == "pipeline_pdl") e->pipe_pdl = value;
     else if (n == "pipeline_gemm_shape") e->pipe_gemm_shape = std::max(0, std::min(2, (int)value));
     else if (n == "pipeline_midb_hops") e->pipe_midb_hops = std::max(1, std::min(PIPE_MIDB_MAX, (int)value));
-    else if (n == "pipeline_split_mid") e->pipe_split_mid = value != 0;
     else if (n == "pipeline_qkv_lanes") e->pipe_qlanes = std::max(1, std::min(PIPE_QLANES, (int)value));
     else if (n == "pipeline_midc_lanes") e->pipe_clanes = std::max(1, std::min(PIPE_CLANES, (int)value));
     else if (n == "pipeline_attn_lanes") e->pipe_tlanes = std::max(1, std::min(PIPE_TLANES, (int)value));
@@ -1280,17 +1228,12 @@ int l2h_sep_set_option(void* handle, const char* name, int32_t value) {
     else if (n == "pipeline_front_lanes") e->pipe_flanes = std::max(1, std::min(PIPE_FLANES, (int)value));
     else if (n == "pipeline_back_lanes") e->pipe_blanes = std::max(1, std::min(PIPE_BLANES, (int)value));
     else if (n == "pdl") e->use_pdl = value != 0;
-    else if (n == "fused_mid") e->use_mid = value != 0;
     else if (n == "fused_tail") e->use_tail = value != 0;
     else if (n == "back_many") e->use_back_many = value != 0;
     else if (n == "tc_pdl") e->tc_pdl = (int)value;
     else if (n == "tc_lstm_min") e->tcl_min_seqdirs = std::max(1, (int)value);
-    else if (n == "mid_split_large") e->mid_split_large = value != 0;
-    else if (n == "fold_mid_c") e->fold_mid_c = value != 0;
-    else if (n == "tensor_cores") e->use_tc = value != 0;
     else if (n == "fuse_ih") e->fuse_ih = value != 0;
     else if (n == "bf16") e->tc_passes = value == 0 ? 3 : (value == 2 ? 1 : 2);   // 1: bf16 weights x split activations; 2: plain bf16 both
-    else if (n == "graph_stats") e->graph_stats = value != 0;
     else return fail(2, "unknown option: " + n);
     drop_graphs(e);                             // cached graphs were built with the old setting
     return 0;
@@ -1299,7 +1242,7 @@ int l2h_sep_set_option(void* handle, const char* name, int32_t value) {
 int l2h_sep_pipeline_frames(void* handle, int32_t* frames) {
     SepEngine* e = static_cast<SepEngine*>(handle);
     if (!e || !frames) return fail(1, "bad argument");
-    *frames = (e->use_pipe && e->use_mid && e->n_blocks == 3) ? pipe_frames_for(e, 1) : 1;
+    *frames = (e->use_pipe && e->n_blocks == 3) ? pipe_frames_for(e, 1) : 1;
     return 0;
 }
 

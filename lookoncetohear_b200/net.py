@@ -283,13 +283,14 @@ class Net(nn.Module):
         return self._ws, n.value
 
     def set_option(self, name, value):
-        """Engine switches: "pipeline" (wavefront pipelining of one-hop calls), "pdl", "fused_mid", "pipeline_frames",
-        "pipeline_split_mid" and the lanes per pipeline stage: "pipeline_lanes" (BiLSTM), "pipeline_qkv_lanes",
-        "pipeline_attn_lanes", "pipeline_out_lanes", "pipeline_front_lanes", "pipeline_back_lanes"."""
+        """Engine switches: "pipeline" (wavefront pipelining of one-hop calls), "pdl", "fused_tail", "pipeline_frames"
+        and the lanes per pipeline stage: "pipeline_lanes" (BiLSTM), "pipeline_qkv_lanes", "pipeline_midc_lanes",
+        "pipeline_attn_lanes", "pipeline_out_lanes", "pipeline_front_lanes", "pipeline_back_lanes".  The full list is in
+        include/lookonce_b200.h (l2h_sep_set_option)."""
         _cabi.check(_cabi.lib().l2h_sep_set_option(self._engine(), name.encode(), int(value)))
 
     def reset_options(self):
-        """Pipeline lane counts / mid split / hops per graph back to the engine defaults."""
+        """Pipeline lane counts / hops per graph / PDL stages back to the engine defaults."""
         self.set_option("defaults", 0)
 
     def pipeline_frames(self):

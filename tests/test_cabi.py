@@ -163,12 +163,16 @@ def test_cpp_host_example_builds(lib, tmp_path):
 
 
 def test_every_engine_option_is_documented_in_the_header():
-    """l2h_sep_set_option takes its switches by name: every name the engine accepts must appear in the header's description of
-    the call (and no environment variable may select a code path: the only getenv allowed in csrc/ would be none)."""
+    """l2h_sep_set_option takes its switches by name: the engine accepts exactly the names below, and every one must appear in
+    the header's description of the call (and no environment variable may select a code path: the only getenv allowed in
+    csrc/ would be none)."""
     src = open(os.path.join(ROOT, "lookoncetohear_b200", "csrc", "sep_engine.cu")).read()
     hdr = open(os.path.join(ROOT, "include", "lookonce_b200.h")).read()
     names = sorted(set(re.findall(r'n == "([a-z_0-9]+)"', src)))
-    assert len(names) >= 20
+    assert set(names) == {
+        "defaults", "pipeline", "pipeline_frames", "pipeline_lanes", "pipeline_pdl", "pipeline_gemm_shape", "pipeline_midb_hops",
+        "pipeline_qkv_lanes", "pipeline_midc_lanes", "pipeline_attn_lanes", "pipeline_out_lanes", "pipeline_front_lanes",
+        "pipeline_back_lanes", "pdl", "fused_tail", "back_many", "tc_pdl", "tc_lstm_min", "fuse_ih", "bf16"}
     for n in names:
         assert f'"{n}"' in hdr, f'option "{n}" is accepted by l2h_sep_set_option but not documented in include/lookonce_b200.h'
     csrc = os.path.join(ROOT, "lookoncetohear_b200", "csrc")

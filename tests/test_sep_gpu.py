@@ -226,11 +226,11 @@ def test_device_streaming_entry_point(model, dev, cpc):
 
 
 PIPE_OPTIONS = ("pipeline_lanes", "pipeline_qkv_lanes", "pipeline_attn_lanes", "pipeline_out_lanes", "pipeline_front_lanes",
-                "pipeline_back_lanes", "pipeline_split_mid", "pipeline_pdl", "pipeline_midb_hops", "pipeline_midc_lanes")
+                "pipeline_back_lanes", "pipeline_pdl", "pipeline_midb_hops", "pipeline_midc_lanes")
 
 
-@pytest.mark.parametrize("lanes", [None, (16, 4, 4, 4, 8, 6, 1, 1023, 8, 3), (3, 1, 1, 1, 1, 2, 0, 16, 1, 1), (5, 2, 2, 3, 3, 3, 1, 0, 3, 2)],
-                         ids=["default", "max-lanes-pdl-everywhere-midb8", "few-lanes-fused-mid", "odd-lanes-no-pdl-midb3"])
+@pytest.mark.parametrize("lanes", [None, (16, 4, 4, 4, 8, 6, 1023, 8, 3), (3, 1, 1, 1, 1, 2, 16, 1, 1), (5, 2, 2, 3, 3, 3, 0, 3, 2)],
+                         ids=["default", "max-lanes-pdl-all-stages-midb8", "few-lanes-midb1", "odd-lanes-no-pdl-midb3-midc2"])
 def test_wavefront_pipeline_equals_sequential(model, dev, lanes):
     """One-hop calls captured as a (block, hop) wavefront graph must reproduce the strictly sequential
     hop-by-hop run bit for bit (same arithmetic, only the schedule and the kernel boundaries of the mid
@@ -419,30 +419,6 @@ def test_init_buffers_in_place(model, dev):
     assert torch.equal(y0, y1)
     with pytest.raises(ValueError):
         net.init_buffers(2, dev, out=st)
-
-
-def test_fold_mid_c_option(model, dev):
-    """Engine option "fold_mid_c": the inter Linear runs inside the serial mid kernel and the Q/K/V projection inside
-    qkv_kernel (three kernels fewer per hop).  A different kernel split, so not bit-identical to the default -- the
-    gate is the usual 1e-3 against the oracle plus 1e-5 against the default path; pipelined == sequential bit for bit
-    holds within the option."""
-    net, sd = model
-    T, B = 70, 2
-    x, _ = synth.mixture(B, 128 * T, seed0=191)
-    e = synth.embedding(B, seed0=192)
-    xd, ed = x.to(dev), e[:, 0].to(dev)
-    y_def = net.stream_dev(xd, ed, chunks_per_call=1).cpu()
-    try:
-        net.set_option("fold_mid_c", 1)             # (also keeps the one-hop chain on its separate kernels)
-        y_pipe = net.stream_dev(xd, ed, chunks_per_call=1).cpu()
-        net.set_option("pipeline", 0)
-        y_seq = net.stream_dev(xd, ed, chunks_per_call=1).cpu()
-    finally:
-        net.set_option("pipeline", 1)
-        net.set_option("fold_mid_c", 0)
-    assert torch.equal(y_pipe, y_seq)
-    assert rs.rel_l2(y_pipe, y_def) < 1e-5
-    _check(y_pipe[:1], rs.sep_forward(sd, x[:1], e[:1]))
 
 
 def test_gate_memo_follows_weight_changes(tsh_params, dev):

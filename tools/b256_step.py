@@ -25,4 +25,4 @@ for g in groups:
     print(json.dumps({"options": g, "ms_per_hop_step": round(ms / 50, 4), "frames_per_s": round(256 * 50 / (ms * 1e-3))}), flush=True)
     for kv in g:
         k, _ = kv.split("=")
-        net.set_option(k, {"pdl": 1, "tensor_cores": 1, "fuse_ih": 0, "bf16": 0}.get(k, 0))
+        net.set_option(k, {"pdl": 1, "fuse_ih": 0, "bf16": 0}.get(k, 0))

@@ -1,6 +1,6 @@
 """Pipeline sweep: lane counts per stage -> frames/s (device-resident clip, B=1), plus the CPU time the host
 spends inside l2h_sep_stream_dev (graph launches) per 500-hop clip.
-    python tools/pipe_experiment.py [A:Q:T:O:F:B[:split_mid[:pdl_mask[:midb_hops[:midc_lanes[:hops_per_graph[:fold_mid_c]]]]]] ...]      lanes of BiLSTM : qkv : attention : attn_out : front : back"""
+    python tools/pipe_experiment.py [A:Q:T:O:F:B[:pdl_mask[:midb_hops[:midc_lanes[:hops_per_graph]]]] ...]      lanes of BiLSTM : qkv : attention : attn_out : front : back"""
 import os, sys, time, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -14,12 +14,12 @@ x, _ = synth.mixture(1, 64000)
 x = x.to(dev)
 emb = synth.embedding(1)[:, 0].to(dev)
 y = torch.empty(1, 2, 64000, device=dev)
-combos = sys.argv[1:] or ["12:3:3:4:6:6", "12:3:3:4:4:4", "16:3:3:4:6:6", "12:3:3:4:6:6:1:16:8", "12:3:3:4:6:6:1:16:4:2:250"]
+combos = sys.argv[1:] or ["12:3:3:4:6:6", "12:3:3:4:4:4", "16:3:3:4:6:6", "12:3:3:4:6:6:16:8", "12:3:3:4:6:6:16:4:2:250"]
 names = ("pipeline_lanes", "pipeline_qkv_lanes", "pipeline_attn_lanes", "pipeline_out_lanes", "pipeline_front_lanes",
-         "pipeline_back_lanes", "pipeline_split_mid", "pipeline_pdl", "pipeline_midb_hops", "pipeline_midc_lanes", "pipeline_frames", "fold_mid_c")
+         "pipeline_back_lanes", "pipeline_pdl", "pipeline_midb_hops", "pipeline_midc_lanes", "pipeline_frames")
 for combo in combos:
     vals = [int(v) for v in combo.split(":")]
-    defaults = [12, 3, 3, 4, 6, 6, 1, 16, 4, 2, 0, 0]
+    defaults = [12, 3, 3, 4, 6, 6, 16, 4, 2, 0]
     vals += defaults[len(vals):]
     for n, v in zip(names, vals):
         net.set_option(n, v)
