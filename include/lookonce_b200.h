@@ -88,9 +88,32 @@ int l2h_sep_state_layout(void* handle, int64_t* header_bytes, int64_t* stream_st
  * state dict (tfgridnet_causal.py:173-186, :408-427) -- SepState.to_reference() / load_reference().  out[i]:
  * 0 ring slots per head, 1 K row stride, 2 K row length (582), 3 V row length (1552), 4 attention window (50),
  * 5 embedding copy, 6 cached speaker gate, 7 conv tail, 8 deconv tail, 9 iSTFT tail, 10 first block, then inside a
- * block: 11 K ring, 12 V ring, 13 h, 14 c, 15 block stride. */
-#define L2H_STATE_OFFSETS 16
+ * block: 11 K ring, 12 V ring, 13 h, 14 c, 15 block stride; then the stream's own clock: 16 its frame count (int64),
+ * 17 its call count (int32; bit 0 = which copy of the double-buffered tails is current).  n may be 16 (the first 16
+ * values only) or more; at most L2H_STATE_OFFSETS values are written.
+ *
+ * Every stream of a state has its own clock: the K/V ring slot of a frame and the current tails come from it, not from
+ * the state's header (which counts the calls and addresses the clip of l2h_sep_stream_dev).  l2h_sep_state_init sets
+ * every clock to 0, and without the three calls below every clock equals the header's. */
+#define L2H_STATE_OFFSETS 18
 int l2h_sep_state_offsets(void* handle, int64_t* out, int32_t n);
+
+/* Serving many listeners from one state (INTEGRATION.md).  Argument errors (null pointers, batch or n <= 0, a slot outside
+ * [0, batch), a slot listed twice) return 1 before anything is enqueued.  Asynchronous on `stream`.
+ *
+ * l2h_sep_state_reset_streams: records slots_host[0 .. n) of a state of `batch` streams become fresh streams (zero rings,
+ * h / c and tails, clock 0, speaker-gate memo invalidated), as in a state just initialised; the other records are not
+ * touched.  One kernel launch per 960 slots.
+ *
+ * l2h_sep_state_copy_streams: record src_slots_host[i] of src_state -> record dst_slots_host[i] of dst_state, the clock
+ * included, so the stream continues in its new slot exactly as it would have in the old one.  Both states belong to this
+ * handle's configuration and device (they may be the same state; then no slot may be both a source and a destination).
+ * The copied records' gate memo is invalidated (it is rebuilt at their next call).  A stream moves to another device by a
+ * host copy of its record (SepState views) into an initialised state there. */
+int l2h_sep_state_reset_streams(void* handle, void* state_dev, int32_t batch, const int32_t* slots_host, int32_t n, void* stream);
+int l2h_sep_state_copy_streams(void* handle, void* dst_state_dev, int32_t dst_batch, const int32_t* dst_slots_host,
+                               const void* src_state_dev, int32_t src_batch, const int32_t* src_slots_host, int32_t n,
+                               void* stream);
 
 int l2h_sep_workspace_bytes(void* handle, int32_t batch, int32_t frames, uint32_t flags, size_t* bytes);
 
@@ -105,6 +128,16 @@ int l2h_sep_forward(void* handle, const float* x_dev, int64_t x_batch_stride, in
                     int64_t y_batch_stride, int64_t y_ch_stride, int32_t y_len, int32_t batch,
                     int32_t frames, void* workspace_dev, size_t workspace_bytes, uint32_t flags,
                     void* stream);
+/* l2h_sep_forward for a one-hop call (frames == 1) in which only some streams advance: stream b advances when
+ * active_dev[b] != 0.  For any other stream nothing in its record changes (rings, h / c, tails, clock, gate memo), and its
+ * rows of y_dev are not written; it may still be computed.  active_dev is [batch] bytes of DEVICE memory read when the
+ * kernels run, so with L2H_FLAG_GRAPH a caller rewrites it in place before every hop and replays the same cached graph.
+ * active_dev == NULL is l2h_sep_forward.  Errors 1: a mask with frames != 1 or with L2H_FLAG_TAPS. */
+int l2h_sep_forward_active(void* handle, const float* x_dev, int64_t x_batch_stride, int64_t x_ch_stride,
+                           int32_t x_len, const float* emb_dev, void* state_dev, float* y_dev,
+                           int64_t y_batch_stride, int64_t y_ch_stride, int32_t y_len, int32_t batch,
+                           int32_t frames, void* workspace_dev, size_t workspace_bytes, uint32_t flags,
+                           void* stream, const uint8_t* active_dev);
 
 /* Streaming with HOST buffers (the end-to-end path).  Per round: H2D of the round's samples (+64
  * look-ahead) from pinned memory, the kernel chains, D2H of the new samples; one stream synchronise at

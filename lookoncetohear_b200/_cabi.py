@@ -41,6 +41,11 @@ _SIGS = {
     "l2h_sep_state_layout": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int64),
                                            ctypes.POINTER(ctypes.c_int64)]),
     "l2h_sep_state_offsets": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int64), ctypes.c_int32]),
+    "l2h_sep_state_reset_streams": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
+                                                  ctypes.POINTER(ctypes.c_int32), ctypes.c_int32, ctypes.c_void_p]),
+    "l2h_sep_state_copy_streams": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
+                                                 ctypes.POINTER(ctypes.c_int32), ctypes.c_void_p, ctypes.c_int32,
+                                                 ctypes.POINTER(ctypes.c_int32), ctypes.c_int32, ctypes.c_void_p]),
     "l2h_sep_workspace_bytes": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_uint32,
                                               ctypes.POINTER(ctypes.c_size_t)]),
     "l2h_sep_forward": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64,
@@ -48,6 +53,11 @@ _SIGS = {
                                       ctypes.c_int64, ctypes.c_int64, ctypes.c_int32, ctypes.c_int32,
                                       ctypes.c_int32, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_uint32,
                                       ctypes.c_void_p]),
+    "l2h_sep_forward_active": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64,
+                                             ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                             ctypes.c_int64, ctypes.c_int64, ctypes.c_int32, ctypes.c_int32,
+                                             ctypes.c_int32, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_uint32,
+                                             ctypes.c_void_p, ctypes.c_void_p]),
     "l2h_sep_stream_host": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p,
                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
                                           ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p,
@@ -123,6 +133,13 @@ def lib():
 def check(rc):
     if rc != 0:
         raise RuntimeError(f"lookonce_b200 error {rc}: {lib().l2h_last_error().decode()}")
+
+
+def check_args(rc):
+    """check() for entry points whose error 1 means an argument the caller passed is invalid: that one raises ValueError."""
+    if rc == 1:
+        raise ValueError(lib().l2h_last_error().decode())
+    check(rc)
 
 
 def declared_symbols():

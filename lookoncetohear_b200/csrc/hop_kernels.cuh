@@ -97,7 +97,7 @@ __device__ __forceinline__ void tail_col(int col, int& which, int& h, int& e, in
 
 __global__ void __launch_bounds__(256)
 tail_kernel(const float* __restrict__ Y, float* X, float* __restrict__ state, int64_t sstride, int blk, BlockWeights w,
-            NextIh nx, int apply_gate, int frame_k) {
+            NextIh nx, int apply_gate, int frame_k, const uint8_t* __restrict__ active) {
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
     extern __shared__ __align__(16) float sm[];
@@ -123,9 +123,10 @@ tail_kernel(const float* __restrict__ Y, float* X, float* __restrict__ state, in
     const int rk = (int)cluster.block_rank(), b = blockIdx.y;
     const bool has_tile = rk < TAIL_TILES;
     const int r0 = rk * MID_RT, nr = has_tile ? tail_rows(rk) : 0;
-    float* st = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride;
+    float* st = stream_rec(state, sstride, b);
     float* sb = st + ST_BLK + (int64_t)blk * BK_STRIDE;
     const bool has_next = nx.wih_t != nullptr;
+    const bool live = stream_active(active, b);          // false: the stream skips this hop, its record is not written
     if (tid == 0) {
         mbar_init(&wbar, 1); mbar_init(&pbar, 1); mbar_init(&gbar, 1);
         mbar_fence_init();
@@ -175,7 +176,7 @@ tail_kernel(const float* __restrict__ Y, float* X, float* __restrict__ state, in
         mid_h_product(S, sb + BK_H, sb + BK_C, r0, nr, tid, hv, cold);
     }
     griddep_wait();
-    const long long pos = reinterpret_cast<const StateHeader*>(state)->pos + frame_k;
+    const long long pos = rec_pos(st) + frame_k;
     trace_.mark(0);
 
     // ---- phase M ------------------------------------------------------------------------------------------------
@@ -186,7 +187,7 @@ tail_kernel(const float* __restrict__ Y, float* X, float* __restrict__ state, in
             if (ok1) gate1 = st[ST_GATE + (r0 + rp + 4) * 64 + n_o];
         }
         const int64_t row0 = (int64_t)b * NF + r0;
-        mid_tile<true>(S, Y + row0 * 128, X + row0 * 64, x2s, Ps, sb + BK_H, sb + BK_C, r0, nr, vs, tid, hv, cold);
+        mid_tile<true>(S, Y + row0 * 128, X + row0 * 64, x2s, Ps, sb + BK_H, sb + BK_C, r0, nr, vs, tid, live, hv, cold);
         __syncthreads();
         if (tid == 0) {                    // the mid weights are dead: W_p (and the next block's W_ih) take their place
             fence_proxy_async();
@@ -288,11 +289,11 @@ tail_kernel(const float* __restrict__ Y, float* X, float* __restrict__ state, in
                 const int g = which * 4 + h, i = (r0 + r) * d + e;
                 const float v = (Ps[idx] - gstat[g][0]) * gstat[g][1] * ng[it] + nb[it];
                 if (which == 0) qn[h * (MID_RT * QE) + r * QE + e] = v;
-                else if (which == 1) sb[BK_K + ((int64_t)h * RING + slot) * QK_LD + i] = v;
-                else sb[BK_V + ((int64_t)h * RING + slot) * V_DIM + i] = v;
+                else if (live && which == 1) sb[BK_K + ((int64_t)h * RING + slot) * QK_LD + i] = v;
+                else if (live) sb[BK_V + ((int64_t)h * RING + slot) * V_DIM + i] = v;
             }
         }
-        if (rk == TAIL_TILES - 1 && tid < 2 * NHEAD)                  // the two pad columns 582, 583 of the K row
+        if (live && rk == TAIL_TILES - 1 && tid < 2 * NHEAD)          // the two pad columns 582, 583 of the K row
             sb[BK_K + ((int64_t)(tid >> 1) * RING + slot) * QK_LD + QK_DIM + (tid & 1)] = 0.f;
     }
     trace_.mark(4);
@@ -494,7 +495,7 @@ constexpr size_t FRONT1_SMEM = (size_t)(64 * 512) * sizeof(float);
 __global__ void __launch_bounds__(256)
 front1_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride, int x_len, float* __restrict__ X,
               float* __restrict__ state, int64_t sstride, SepWeights w, BlockWeights w0, float* __restrict__ GX, int pos_rel,
-              const float* __restrict__ emb, float* __restrict__ spk_pre) {
+              const float* __restrict__ emb, float* __restrict__ spk_pre, const uint8_t* __restrict__ active) {
     extern __shared__ __align__(16) float wih[];       // [64][512] block 0's W_ih^T
     __shared__ __align__(16) float xs[NMIC][NFFT];      // the frame's samples (reused as scratch by the gate CTA: >= 288 floats)
     __shared__ float U[3][4][F1_NB];                    // [frame t-2..t][ch][halo + bin], zero outside 0..96
@@ -506,7 +507,7 @@ front1_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride,
     const int p = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     if (p == TAIL_TILES) {                 // the extra CTA of this stream: speaker-gate memo
         griddep_wait();
-        spk_gate_cta(emb, spk_pre, state, sstride, w, b, &xs[0][0]);
+        spk_gate_cta(emb, spk_pre, state, sstride, w, b, &xs[0][0], active);
         return;
     }
     const int f0 = p * MID_RT, nr = tail_rows(p);
@@ -540,8 +541,8 @@ front1_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride,
     __syncthreads();
     griddep_wait();
     const StateHeader* hdr = reinterpret_cast<const StateHeader*>(state);
-    const int par = (int)(hdr->ncalls & 1);
-    float* st = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride;
+    float* st = stream_rec(state, sstride, b);
+    const int par = rec_par(st);
     const float* cb = st + ST_CONV + par * (2 * 4 * NF);
     float* cb_next = st + ST_CONV + (par ^ 1) * (2 * 4 * NF);
     // samples of the frame: x[s0 .. s0 + 191] (zero past the end: the look-ahead padding of net.py:8-18,56-58)
@@ -598,9 +599,11 @@ front1_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride,
         if (ok1) xr[(fq + 4) * 64 + o] = acc1;
     }
     // next conv tails = spectrogram rows of frames t-1, t (own bins)
-    for (int i = tid; i < 2 * 4 * nr; i += 256) {
-        const int fr = i / (4 * nr), c = (i / nr) % 4, r = i % nr;
-        cb_next[(fr * 4 + c) * NF + f0 + r] = U[1 + fr][c][1 + r];
+    if (stream_active(active, b)) {
+        for (int i = tid; i < 2 * 4 * nr; i += 256) {
+            const int fr = i / (4 * nr), c = (i / nr) % 4, r = i % nr;
+            cb_next[(fr * 4 + c) * NF + f0 + r] = U[1 + fr][c][1 + r];
+        }
     }
     __syncthreads();
     trace_.mark(2);

@@ -154,9 +154,10 @@ __device__ __forceinline__ void mid_h_product(const MidSmem& S, const float* hst
 }
 
 // PRE_H: the h W_hh product and the old cell state come from mid_h_product (hv_in, cold_in) instead of being computed here.
+// store_hc = false: the new (h, c) are computed but not written back (a stream that skips this hop).
 template <bool PRE_H = false>
 __device__ __forceinline__ void mid_tile(const MidSmem& S, const float* Yrows, const float* Xin, float* X2out, float* Pout,
-                                         float* hst, float* cst, int r0, int nr, const float* vs, int tid,
+                                         float* hst, float* cst, int r0, int nr, const float* vs, int tid, bool store_hc,
                                          const float* hv_in = nullptr, float2 cold_in = make_float2(0.f, 0.f)) {
     float* Wp = S.Wp; float* A1 = S.A1; float* A3 = S.A3; float* A3h = S.A3h; float* A5 = S.A5; float* A6 = S.A6; float* x1s = S.x1s;
     // ---- tile loads: Y -> A1, h -> A3h ------------------------------------------------------------
@@ -219,7 +220,7 @@ __device__ __forceinline__ void mid_tile(const MidSmem& S, const float* Yrows, c
         const float gi1 = fast_sigmoid(v[4] + gb.x), gf1 = fast_sigmoid(v[5] + gb.y), gg1 = fast_tanh(v[6] + gb.z), go1 = fast_sigmoid(v[7] + gb.w);
         const float c0 = gf0 * cold.x + gi0 * gg0, c1 = gf1 * cold.y + gi1 * gg1;
         const float h0 = go0 * fast_tanh(c0), h1 = go1 * fast_tanh(c1);
-        if (r < nr) {
+        if (store_hc && r < nr) {
             *reinterpret_cast<float2*>(cst + (r0 + r) * 64 + jp * 2) = make_float2(c0, c1);
             *reinterpret_cast<float2*>(hst + (r0 + r) * 64 + jp * 2) = make_float2(h0, h1);
         }
@@ -254,7 +255,7 @@ __device__ __forceinline__ void mid_tile(const MidSmem& S, const float* Yrows, c
 
 __global__ void __launch_bounds__(256)
 mid_kernel(const float* __restrict__ Y, float* X, float* __restrict__ QKV, float* __restrict__ state,
-           int64_t sstride, int blk, BlockWeights w, int n_streams) {
+           int64_t sstride, int blk, BlockWeights w, int n_streams, const uint8_t* __restrict__ active) {
     extern __shared__ __align__(16) float sm[];
     const MidSmem S(sm);
     __shared__ __align__(8) unsigned long long wbar;
@@ -281,9 +282,10 @@ mid_kernel(const float* __restrict__ Y, float* X, float* __restrict__ QKV, float
         const int r0 = (item % TILES) * MID_RT;
         const int nr = min(MID_RT, NF - r0);
         __syncthreads();                    // the previous item's tiles are fully consumed
-        float* sb = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride + ST_BLK + (int64_t)blk * BK_STRIDE;
+        float* sb = stream_rec(state, sstride, b) + ST_BLK + (int64_t)blk * BK_STRIDE;
         const int64_t row0 = (int64_t)b * NF + r0;
-        mid_tile(S, Y + row0 * 128, X + row0 * 64, X + row0 * 64, QKV + row0 * NQKV, sb + BK_H, sb + BK_C, r0, nr, vs, tid);
+        mid_tile(S, Y + row0 * 128, X + row0 * 64, X + row0 * 64, QKV + row0 * NQKV, sb + BK_H, sb + BK_C, r0, nr, vs, tid,
+                 stream_active(active, b));
     }
 }
 
@@ -372,7 +374,7 @@ mid_a_kernel(const float* __restrict__ Y, float* __restrict__ X, float* __restri
 // registers between them, the state is read before the first and written after the last.
 __global__ void __launch_bounds__(256)
 mid_b_kernel(const float* __restrict__ GI, float* __restrict__ Hn, int64_t hop_stride, int n_hops, float* __restrict__ state,
-             int64_t sstride, int blk, BlockWeights w, int n_streams) {
+             int64_t sstride, int blk, BlockWeights w, int n_streams, const uint8_t* __restrict__ active) {
     extern __shared__ __align__(16) float sm[];
     float* W3b = sm;                                  // W_hh, k-sliced
     float* A3 = W3b + (MID_W5 - MID_W3B);             // h, k-sliced
@@ -394,7 +396,7 @@ mid_b_kernel(const float* __restrict__ GI, float* __restrict__ Hn, int64_t hop_s
         const int r0 = (item % TILES) * MID_RT;
         const int nr = min(MID_RT, NF - r0);
         __syncthreads();
-        float* sb = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride + ST_BLK + (int64_t)blk * BK_STRIDE;
+        float* sb = stream_rec(state, sstride, b) + ST_BLK + (int64_t)blk * BK_STRIDE;
         float* hst = sb + BK_H;
         float* cst = sb + BK_C;
         const int64_t row0 = (int64_t)b * NF + r0;
@@ -434,7 +436,7 @@ mid_b_kernel(const float* __restrict__ GI, float* __restrict__ Hn, int64_t hop_s
                 A3[mid_aidx(M3_KS, jp * 2 + 1, r)] = hh.y;
             }
         }
-        if (live) {
+        if (live && stream_active(active, b)) {
             *reinterpret_cast<float2*>(cst + (r0 + r) * 64 + jp * 2) = cc;
             *reinterpret_cast<float2*>(hst + (r0 + r) * 64 + jp * 2) = hh;
         }

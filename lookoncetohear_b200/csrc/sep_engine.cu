@@ -340,6 +340,7 @@ struct ChainArgs {
     float* y; int64_t ybs, ycs; int y_len;
     int B, T; float* wsp; size_t ws_bytes; uint32_t flags; int pos_rel;
     Profiler* prof = nullptr;
+    const uint8_t* active = nullptr;     // one-hop calls: [B] device mask of the streams that advance (null: all)
 };
 
 static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
@@ -347,6 +348,7 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
     const float* emb = a.emb; float* state = a.state; float* y = a.y;
     const int64_t ybs = a.ybs, ycs = a.ycs; const int y_len = a.y_len, B = a.B, T = a.T;
     float* wsp = a.wsp; const size_t ws_bytes = a.ws_bytes; const uint32_t flags = a.flags;
+    const uint8_t* active = a.active;
     if (!e->pack.committed) return fail(4, "weights not committed");
     if (B <= 0 || T <= 0) return fail(1, "batch and frames must be positive");
     const Workspace ws = carve(e->n_blocks, B, T, flags);
@@ -389,17 +391,17 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
     MARK("start");
     if (fused_tail) {      // the frame as 13 row tiles: spectrum of the tile's bins, conv, and block 0's input projection
         CK(launch_k(false, front1_kernel, dim3(TAIL_TILES + 1, B), dim3(256), FRONT1_SMEM, st, x, xbs, xcs, x_len, X, state, ss, e->w,
-                    e->bw[0], GX, a.pos_rel, emb, PRE));
+                    e->bw[0], GX, a.pos_rel, emb, PRE, active));
     } else if ((T > 1 || tc) && e->use_back_many) {      // many frames / streams: one CTA walks (stream, chunk) items (one CTA per SM: 150 KB of filters)
         const int per_stream = std::max(1, NUM_SMS / B);
         const int chunk = (T + per_stream - 1) / per_stream;
         const int n_chunks = (T + chunk - 1) / chunk;
         const int n_workers = std::min(NUM_SMS, B * n_chunks);
         CK(launch_k(false, front_many_kernel, dim3(n_workers + B, 1), dim3(256), FRONT_SMEM, st, x, xbs, xcs, x_len, X, state, ss, e->w, T,
-                    a.pos_rel, emb, PRE, chunk, n_chunks, B, n_workers));
+                    a.pos_rel, emb, PRE, chunk, n_chunks, B, n_workers, active));
     } else {
         CK(launch_k(false, front_kernel, dim3(T + 1, B), dim3(256), FRONT_SMEM, st, x, xbs, xcs, x_len, X, state, ss, e->w, T,
-                    a.pos_rel, emb, PRE, 0, 1, 0));
+                    a.pos_rel, emb, PRE, 0, 1, 0, active));
     }
     MARK("front");
     if (int rc = do_tap()) return rc;
@@ -460,7 +462,8 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
                 const cudaError_t ce = umma::launch(q, st, &why);
                 if (ce != cudaSuccess) return fail(3, std::string("umma_gemm (inter step): ") + cudaGetErrorString(ce) + " " + why);
             }
-            CK(launch_k(pdl || mp, lstm_cell_rows_kernel, dim3((unsigned)((rows * 64 + 255) / 256)), dim3(256), 0, st, (const float*)GX, state, ss, b, Y, (int)rows));
+            CK(launch_k(pdl || mp, lstm_cell_rows_kernel, dim3((unsigned)((rows * 64 + 255) / 256)), dim3(256), 0, st, (const float*)GX, state, ss, b, Y, (int)rows,
+                      active));
             if (int rc = tc_rows_gemm(e, b, PL_L2, Y, 64, 64, 64, nullptr, nullptr, W.bl2, nullptr, X, X, 64, rows, st)) return rc;
             if (int rc = tc_rows_gemm(e, b, PL_QKV, X, 64, 64, NQKV, nullptr, nullptr, W.bqkv, W.slope_vec, nullptr, QKVRAW, NQKV, rows, st)) return rc;
             e->cur_pdl = false;
@@ -468,7 +471,8 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
         } else if (row_mid && mid_split_for_throughput(B)) {
             float* GI = GX; float* HN = GX + rows * 256;         // the BiLSTM is done with GX
             CK(launch_k(pdl, mid_a_kernel, mid_grid_for(B, 2), dim3(256), MID_A_SMEM, st, (const float*)Y, X, GI, W, B, (int64_t)0, 1));
-            CK(launch_k(pdl, mid_b_kernel, mid_grid_for(B, 3), dim3(256), MID_B_SMEM, st, (const float*)GI, HN, (int64_t)0, 1, state, ss, b, W, B));
+            CK(launch_k(pdl, mid_b_kernel, mid_grid_for(B, 3), dim3(256), MID_B_SMEM, st, (const float*)GI, HN, (int64_t)0, 1, state, ss, b, W, B,
+                        active));
             CK(launch_k(pdl, mid_c_kernel, mid_grid_for(B, 4), dim3(256), MID_C_SMEM, st, (const float*)HN, X, QKVRAW, W, B, (int64_t)0, 1));
             MARK("mid");
         } else if (fused_tail) {
@@ -478,12 +482,12 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
                 nx.ln_g = Wn.ln1_g; nx.ln_b = Wn.ln1_b; nx.wih_t = Wn.wih1_t; nx.bias = Wn.b1; nx.GX = GX;
             }
             CK(launch_cluster(pdl, dim3(TAIL_CL, 1, 1), tail_kernel, dim3(TAIL_CL, B), dim3(256), TAIL_SMEM, st, (const float*)Y, X, state, ss,
-                              b, W, nx, (b == 0 && e->n_blocks > 1) ? 1 : 0, 0));
+                              b, W, nx, (b == 0 && e->n_blocks > 1) ? 1 : 0, 0, active));
             MARK("tail");
             if (int rc = do_tap()) return rc;
             continue;
         } else if (row_mid) {
-            CK(launch_k(pdl, mid_kernel, mid_grid_for(B, 1), dim3(256), MID_SMEM, st, (const float*)Y, X, QKVRAW, state, ss, b, W, B));
+            CK(launch_k(pdl, mid_kernel, mid_grid_for(B, 1), dim3(256), MID_SMEM, st, (const float*)Y, X, QKVRAW, state, ss, b, W, B, active));
             MARK("mid");
         } else {
             if (tc) {
@@ -548,10 +552,10 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
             static int wave[64] = {};
             const int64_t grid_q = std::min<int64_t>(resident_ctas(wave, qkv_many_kernel, QKV_THREADS, QKV_MANY_SMEM), (int64_t)B * T);
             CK(launch_k(pdl || ((e->tc_pdl & 4) != 0 && a.prof == nullptr), qkv_many_kernel, dim3((unsigned)grid_q), dim3(QKV_THREADS), QKV_MANY_SMEM, st, (const float*)QKVRAW, Q, KALL, VALL, state, ss,
-                        b, W, T, B * T));
+                        b, W, T, B * T, active));
         } else {
             CK(launch_k(pdl, qkv_kernel, dim3(T, B), dim3(QKV_THREADS), QKV_SMEM, st, (const float*)X,
-                        (const float*)((tc || row_mid) ? QKVRAW : nullptr), Q, KALL, VALL, state, ss, b, W, T, 0));
+                        (const float*)((tc || row_mid) ? QKVRAW : nullptr), Q, KALL, VALL, state, ss, b, W, T, 0, active));
         }
         MARK("qkv");
         if (nsplit > 1) {
@@ -589,10 +593,10 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
         const int n_chunks = (T + chunk - 1) / chunk;
         const int n_cl = std::min(max_cl, B * n_chunks);
         CK(launch_cluster(pdl, dim3(BACK_CL, 1, 1), back_many_kernel, dim3(BACK_CL * n_cl, 1), dim3(256), BACK_MANY_SMEM, st, (const float*)X, y, ybs,
-                          ycs, y_len, state, ss, e->w, T, a.pos_rel, chunk, n_chunks, B));
+                          ycs, y_len, state, ss, e->w, T, a.pos_rel, chunk, n_chunks, B, active));
     } else {
         CK(launch_cluster(pdl, dim3(BACK_CL, 1, 1), back_kernel, dim3(BACK_CL * T, B), dim3(256), BACK_SMEM, st, (const float*)X, y, ybs, ycs, y_len, state, ss, e->w, T,
-                    a.pos_rel, 0, 1, 0, (int64_t)0));
+                    a.pos_rel, 0, 1, 0, (int64_t)0, active));
     }
     MARK("back");
 #undef MARK
@@ -610,8 +614,8 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
 // A graph of K consecutive one-hop chains is captured on 1 + 3*(PIPE_LANES+3) + 1 streams with event edges
 // for exactly these dependencies; hops flow through the stages like a systolic wavefront and the
 // steady-state cost per hop is the slowest SERIAL stage instead of the whole chain.  Every hop owns a
-// workspace slot; state addressing uses pos + frame_k / parity(ncalls + frame_k); the header advances once,
-// at the last hop of the graph.  The arithmetic and its order per stream are unchanged: results are
+// workspace slot; state addressing uses each stream's own clock (pos + frame_k, the parity of its calls); the
+// clocks advance once, at the last hop of the graph.  The arithmetic and its order per stream are unchanged: results are
 // bit-identical to running the hops one after the other (tests/test_sep_gpu.py).
 constexpr int PIPE_MAX_FRAMES = 500;
 constexpr int PIPE_LANES = 16;     // max hops of stage A (BiLSTM) in flight per block (engine->pipe_alanes used)
@@ -659,6 +663,7 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
     const int ppdl = e->pipe_pdl;         // stage bit mask (bits: include/lookonce_b200.h, l2h_sep_set_option)
     const bool many = mid_split_for_throughput(B);
     float* state = a.state;
+    const uint8_t* all_active = nullptr;      // every stream of a pipelined graph advances
     for (int i = 0; i < PIPE_STREAMS; ++i)
         if (!e->pipe_streams[i]) CK(cudaStreamCreateWithFlags(&e->pipe_streams[i], cudaStreamNonBlocking));
     size_t ev_used = 0;
@@ -728,7 +733,8 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
                         cudaStream_t sF = sFront(k);
                         // the speaker-gate memo CTA (blockIdx.x == 1) rides with hop 0 only: one builder of ST_GATE per group
                         CK(launch_k((ppdl & 1) != 0, front_kernel, dim3(k == 0 ? 2 : 1, B), dim3(256), FRONT_SMEM, sF, a.x, a.xbs, a.xcs,
-                                    a.x_len, a.wsp + (int64_t)k * slot + ws.X, state, ss, e->w, 1, a.pos_rel, a.emb, PRE, k, K, k * HOP));
+                                    a.x_len, a.wsp + (int64_t)k * slot + ws.X, state, ss, e->w, 1, a.pos_rel, a.emb, PRE, k, K, k * HOP,
+                                    all_active));
                         if (k == 0) {                  // ... and every attn_out lane of block 0 (the gate's only reader) waits for it once
                             cudaEvent_t gate_ev;
                             if (int rc = record(&gate_ev, sF)) return rc;
@@ -762,7 +768,7 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
                 float* wsp = a.wsp + (int64_t)k0 * slot;
                 float* GI = wsp + ws.GX; float* HN = GI + (int64_t)rows * 256;
                 CK(launch_k((ppdl & 16) != 0, mid_b_kernel, mid_grid_for(B, 3), dim3(256), MID_B_SMEM, sB1(b), (const float*)GI, HN, slot,
-                            k1 - k0, state, ss, b, W, B));
+                            k1 - k0, state, ss, b, W, B, all_active));
             }
             cudaEvent_t midb_done;
             if (int rc = record(&midb_done, sB1(b))) return rc;
@@ -784,7 +790,7 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
                 for (int d = 0; d < e->pipe_tlanes && k - PIPE_QKV_AHEAD - 1 - d >= 0; ++d)
                     CK(cudaStreamWaitEvent(st_q, att_done[b][k - PIPE_QKV_AHEAD - 1 - d], 0));
                 CK(launch_k((ppdl & 64) != 0, qkv_kernel, dim3(1, B), dim3(QKV_THREADS), QKV_SMEM, st_q, (const float*)X,
-                            (const float*)QKVRAW, Q, (float*)nullptr, (float*)nullptr, state, ss, b, W, 1, k));
+                            (const float*)QKVRAW, Q, (float*)nullptr, (float*)nullptr, state, ss, b, W, 1, k, all_active));
                 if (int rc = record(&qkv_done[b][k], st_q)) return rc;
                 // the attention reads this hop's ring row and the 49 before it: the other qkv lanes' latest hops must be in
                 cudaStream_t st_t = sBa(b, k);
@@ -810,12 +816,13 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
             // this hop's output and the three before it (deconv / overlap-add context) sit on different attn_out lanes
             for (int d = 0; d <= 3 && d <= k; ++d) CK(cudaStreamWaitEvent(sBack, out_done[2][k - d], 0));
             CK(launch_cluster((ppdl & 512) != 0, dim3(BACK_CL, 1, 1), back_kernel, dim3(BACK_CL, B), dim3(256), BACK_SMEM, sBack,
-                              (const float*)X, a.y, a.ybs, a.ycs, a.y_len, state, ss, e->w, 1, a.pos_rel, k, K, k * HOP, slot));
+                              (const float*)X, a.y, a.ybs, a.ycs, a.y_len, state, ss, e->w, 1, a.pos_rel, k, K, k * HOP, slot,
+                              all_active));
         }
     }
     for (int i = 1; i < PIPE_STREAMS; ++i)                             // join
         if (int rc = edge(e->pipe_streams[i], origin)) return rc;
-    advance_header_kernel<<<1, 1, 0, origin>>>(state, K);                // pos += K, ncalls += 1: after every hop of the group
+    advance_header_kernel<<<1, 256, 0, origin>>>(state, ss, B, K);       // every clock: pos += K, calls += 1, after every hop of the group
     CK(cudaGetLastError());
     return 0;
 }
@@ -842,7 +849,7 @@ static void drop_graphs(SepEngine* e) {
 // cache key of a chain graph: every argument its kernels bake in (`t`: frames, or -hops for the pipelined form)
 static std::vector<int64_t> graph_key(const ChainArgs& a, int t) {
     return {(int64_t)a.x, a.xbs, a.xcs, a.x_len, (int64_t)a.emb, (int64_t)a.state, (int64_t)a.y,
-            a.ybs, a.ycs, a.y_len, a.B, t, (int64_t)a.wsp, (int64_t)a.flags, a.pos_rel};
+            a.ybs, a.ycs, a.y_len, a.B, t, (int64_t)a.wsp, (int64_t)a.flags, a.pos_rel, (int64_t)a.active};
 }
 
 // Launch the graph cached under `key` on `st`.  The first time a key is seen, `enqueue(cap)` is captured on the private
@@ -1001,9 +1008,9 @@ int l2h_sep_state_offsets(void* handle, int64_t* out, int32_t n) {
     SepEngine* e = static_cast<SepEngine*>(handle);
     if (!e || !out) return fail(1, "null argument");
     const int64_t v[L2H_STATE_OFFSETS] = {RING, QK_LD, QK_DIM, V_DIM, ATT, ST_EMB, ST_GATE, ST_CONV, ST_DECONV, ST_ISTFT, ST_BLK,
-                                          BK_K, BK_V, BK_H, BK_C, BK_STRIDE};
-    if (n < L2H_STATE_OFFSETS) return fail(1, "need room for L2H_STATE_OFFSETS values");
-    for (int i = 0; i < L2H_STATE_OFFSETS; ++i) out[i] = v[i];
+                                          BK_K, BK_V, BK_H, BK_C, BK_STRIDE, ST_POS, ST_CALLS};
+    if (n < 16) return fail(1, "need room for at least 16 values");      // 16: the layout before the per-stream clocks
+    for (int i = 0; i < std::min<int>(n, L2H_STATE_OFFSETS); ++i) out[i] = v[i];
     return 0;
 }
 
@@ -1030,6 +1037,71 @@ int l2h_sep_state_init(void* handle, void* state, int32_t batch, void* stream) {
     state_init_kernel<<<592, 256, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<float*>(state), total, ss, batch);
     CK(cudaGetLastError());
     e->launch_count += 1;
+    return 0;
+}
+
+// slot lists of the stream-record calls: every slot in [0, batch), none twice
+static int check_slots(const int32_t* slots, int32_t n, int32_t batch, const char* what) {
+    std::vector<char> seen((size_t)batch, 0);
+    for (int32_t i = 0; i < n; ++i) {
+        const int32_t s = slots[i];
+        if (s < 0 || s >= batch)
+            return fail(1, std::string(what) + ": slot " + std::to_string(s) + " outside [0, " + std::to_string(batch) + ")");
+        if (seen[(size_t)s]) return fail(1, std::string(what) + ": slot " + std::to_string(s) + " listed twice");
+        seen[(size_t)s] = 1;
+    }
+    return 0;
+}
+
+int l2h_sep_state_reset_streams(void* handle, void* state, int32_t batch, const int32_t* slots_host, int32_t n, void* stream) {
+    SepEngine* e = static_cast<SepEngine*>(handle);
+    if (!e || !state || !slots_host) return fail(1, "null argument");
+    if (batch <= 0 || n <= 0 || n > batch) return fail(1, "batch and the slot count must be positive, slots at most batch");
+    if (int rc = check_slots(slots_host, n, batch, "reset_streams")) return rc;
+    if (int rc = check_device(e)) return rc;
+    const int64_t ss = stream_stride(e->n_blocks);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    for (int32_t i0 = 0; i0 < n; i0 += RESET_MAX_SLOTS) {       // one launch for up to RESET_MAX_SLOTS records
+        const int32_t k = std::min<int32_t>(RESET_MAX_SLOTS, n - i0);
+        SlotList sl{};
+        std::copy(slots_host + i0, slots_host + i0 + k, sl.s);
+        // ~2 CTAs per SM over all records: each record is 6 MB of stores
+        const unsigned per_rec = (unsigned)std::max(1, 2 * NUM_SMS / k);
+        reset_streams_kernel<<<dim3(per_rec, k), 256, 0, st>>>(static_cast<float*>(state), ss, sl);
+        CK(cudaGetLastError());
+        e->launch_count += 1;
+    }
+    return 0;
+}
+
+int l2h_sep_state_copy_streams(void* handle, void* dst_state, int32_t dst_batch, const int32_t* dst_slots_host,
+                               const void* src_state, int32_t src_batch, const int32_t* src_slots_host, int32_t n, void* stream) {
+    SepEngine* e = static_cast<SepEngine*>(handle);
+    if (!e || !dst_state || !src_state || !dst_slots_host || !src_slots_host) return fail(1, "null argument");
+    if (dst_batch <= 0 || src_batch <= 0 || n <= 0 || n > dst_batch) return fail(1, "batches and the slot count must be positive");
+    if (int rc = check_slots(dst_slots_host, n, dst_batch, "copy_streams (destination)")) return rc;
+    for (int32_t i = 0; i < n; ++i)
+        if (src_slots_host[i] < 0 || src_slots_host[i] >= src_batch)
+            return fail(1, "copy_streams: source slot " + std::to_string(src_slots_host[i]) + " outside [0, " + std::to_string(src_batch) + ")");
+    if (dst_state == src_state) {         // within one state: no record may be both read and overwritten
+        std::vector<char> src_used((size_t)src_batch, 0);
+        for (int32_t i = 0; i < n; ++i) src_used[(size_t)src_slots_host[i]] = 1;
+        for (int32_t i = 0; i < n; ++i)
+            if (src_used[(size_t)dst_slots_host[i]])
+                return fail(1, "copy_streams: slot " + std::to_string(dst_slots_host[i]) + " is both a source and a destination");
+    }
+    if (int rc = check_device(e)) return rc;
+    const int64_t ss = stream_stride(e->n_blocks);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    float* dst = static_cast<float*>(dst_state) + sizeof(StateHeader) / 4;
+    const float* src = static_cast<const float*>(src_state) + sizeof(StateHeader) / 4;
+    for (int32_t i = 0; i < n; ++i) {
+        float* d = dst + (int64_t)dst_slots_host[i] * ss;
+        // the whole record, its clock included; then the gate memo is invalidated (generation 0 is never a handle's):
+        // weight generations are per handle, so a memo built by another handle must not be trusted
+        CK(cudaMemcpyAsync(d, src + (int64_t)src_slots_host[i] * ss, (size_t)ss * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        CK(cudaMemsetAsync(d + ST_GEN, 0, sizeof(float), st));
+    }
     return 0;
 }
 
@@ -1108,11 +1180,21 @@ int l2h_sep_launch_count(void* handle, int64_t* kernels, int32_t reset) {
 int l2h_sep_forward(void* handle, const float* x, int64_t xbs, int64_t xcs, int32_t x_len, const float* emb,
                     void* state, float* y, int64_t ybs, int64_t ycs, int32_t y_len, int32_t batch, int32_t frames,
                     void* ws, size_t ws_bytes, uint32_t flags, void* stream) {
+    return l2h_sep_forward_active(handle, x, xbs, xcs, x_len, emb, state, y, ybs, ycs, y_len, batch, frames, ws, ws_bytes, flags,
+                                  stream, nullptr);
+}
+
+int l2h_sep_forward_active(void* handle, const float* x, int64_t xbs, int64_t xcs, int32_t x_len, const float* emb,
+                           void* state, float* y, int64_t ybs, int64_t ycs, int32_t y_len, int32_t batch, int32_t frames,
+                           void* ws, size_t ws_bytes, uint32_t flags, void* stream, const uint8_t* active_dev) {
     SepEngine* e = static_cast<SepEngine*>(handle);
+    if (active_dev && frames != 1) return fail(1, "an activity mask needs a one-hop call (frames == 1)");
+    if (active_dev && (flags & L2H_FLAG_TAPS)) return fail(1, "an activity mask cannot be combined with L2H_FLAG_TAPS");
     if (e) { if (int rc_dev = check_device(e)) return rc_dev; }
     if (!e || !x || !emb || !state || !y || !ws) return fail(1, "null argument");
     ChainArgs a{x, xbs, xcs, x_len, emb, static_cast<float*>(state), y, ybs, ycs, y_len, batch, frames,
                 static_cast<float*>(ws), ws_bytes, flags & ~L2H_FLAG_GRAPH, 0};
+    a.active = active_dev;
     return run_chain(e, a, static_cast<cudaStream_t>(stream), (flags & L2H_FLAG_GRAPH) != 0);
 }
 

@@ -65,10 +65,62 @@ __global__ void state_init_kernel(float* state, int64_t total_floats, int64_t st
     }
 }
 
-__global__ void advance_header_kernel(float* state, int frames) {
-    StateHeader* hdr = reinterpret_cast<StateHeader*>(state);
-    hdr->pos += frames;
-    hdr->ncalls += 1;
+// ---- per-stream clocks (sep_layout.h) and the activity mask of one-hop calls ----------------------------------
+__device__ __forceinline__ float* stream_rec(float* state, int64_t sstride, int b) {
+    return state + sizeof(StateHeader) / 4 + (int64_t)b * sstride;
+}
+__device__ __forceinline__ const float* stream_rec(const float* state, int64_t sstride, int b) {
+    return state + sizeof(StateHeader) / 4 + (int64_t)b * sstride;
+}
+__device__ __forceinline__ long long rec_pos(const float* rec) { return *reinterpret_cast<const long long*>(rec + ST_POS); }
+__device__ __forceinline__ int rec_par(const float* rec) { return __float_as_int(rec[ST_CALLS]) & 1; }
+// active == nullptr: every stream advances (all calls except l2h_sep_forward_active with a mask)
+__device__ __forceinline__ bool stream_active(const uint8_t* active, int b) { return active == nullptr || active[b] != 0; }
+
+// End of a call, run by every thread of ONE CTA after all others have finished reading the clocks: the header advances by
+// `frames` frames and one call, and so does the clock of every active stream.
+__device__ void advance_clocks(float* state, int64_t sstride, int n_streams, int frames, const uint8_t* active) {
+    if (threadIdx.x == 0) {
+        StateHeader* hdr = reinterpret_cast<StateHeader*>(state);
+        hdr->pos += frames;
+        hdr->ncalls += 1;
+        hdr->done = 0;
+    }
+    for (int b = threadIdx.x; b < n_streams; b += blockDim.x) {
+        if (!stream_active(active, b)) continue;
+        float* rec = stream_rec(state, sstride, b);
+        *reinterpret_cast<long long*>(rec + ST_POS) += frames;
+        rec[ST_CALLS] = __int_as_float(__float_as_int(rec[ST_CALLS]) + 1);
+    }
+    __threadfence();
+}
+
+// The last CTA of a call's final kernel advances the clocks (advance_clocks).
+__device__ __forceinline__ void finish_call(float* state, int64_t sstride, int n_streams, int frames, const uint8_t* active) {
+    __shared__ int last;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        const int prev = atomicAdd(&reinterpret_cast<StateHeader*>(state)->done, 1);
+        last = prev == (int)(gridDim.x * gridDim.y) - 1;
+    }
+    __syncthreads();
+    if (last) advance_clocks(state, sstride, n_streams, frames, active);
+}
+
+__global__ void advance_header_kernel(float* state, int64_t sstride, int n_streams, int frames) {
+    advance_clocks(state, sstride, n_streams, frames, nullptr);
+}
+
+// l2h_sep_state_reset_streams: the listed records become fresh streams, as state_init_kernel leaves them (zero rings,
+// h / c and tails, clock 0, NaN embedding = gate memo invalid).  grid (any, n), record of slots.s[blockIdx.y].
+constexpr int RESET_MAX_SLOTS = 960;      // slots per launch: the kernel parameters stay under 4 KB
+struct SlotList { int32_t s[RESET_MAX_SLOTS]; };
+__global__ void reset_streams_kernel(float* state, int64_t sstride, SlotList slots) {
+    float4* rec = reinterpret_cast<float4*>(stream_rec(state, sstride, slots.s[blockIdx.y]));
+    const float nan = __int_as_float(0x7fc00000);
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < sstride / 4; i += (int64_t)gridDim.x * blockDim.x)
+        rec[i] = (i < SPK / 4) ? make_float4(nan, nan, nan, nan) : make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
 __global__ void set_clip_base_kernel(float* state) {
@@ -83,13 +135,13 @@ __global__ void set_clip_base_kernel(float* state) {
 constexpr size_t FRONT_SMEM = (size_t)NFFT * 196 * sizeof(float);     // analysis filters, staged by TMA
 
 __device__ void spk_gate_cta(const float* __restrict__ emb, float* __restrict__ pre, float* __restrict__ state,
-                             int64_t sstride, const SepWeights& w, int b, float* red);
+                             int64_t sstride, const SepWeights& w, int b, float* red, const uint8_t* __restrict__ active);
 
 __global__ void __launch_bounds__(256)
 front_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride, int x_len,
              float* __restrict__ X, float* __restrict__ state, int64_t sstride, SepWeights w, int T,
              int pos_rel, const float* __restrict__ emb, float* __restrict__ spk_pre, int frame_k, int frames_total,
-             int sample_off) {
+             int sample_off, const uint8_t* __restrict__ active) {
     extern __shared__ __align__(16) float wat_s[];     // [192][196]
     __shared__ __align__(16) float xs[NMIC][448];
     __shared__ float U[3][4][100];      // [frame t-2..t][ch][1 + f], zero-padded in f
@@ -99,7 +151,7 @@ front_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride, 
     const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
     if (t == T) {                      // the extra CTA of this stream: speaker-gate memo
         griddep_wait();
-        spk_gate_cta(emb, spk_pre, state, sstride, w, b, &xs[0][0]);
+        spk_gate_cta(emb, spk_pre, state, sstride, w, b, &xs[0][0], active);
         return;
     }
     if (tid == 0) { mbar_init(&wbar, 1); mbar_fence_init(); }
@@ -108,15 +160,15 @@ front_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride, 
     __syncthreads();
     tma_load_split(wat_s, w.wat, (unsigned)FRONT_SMEM, &wbar, tid, 256);     // 74 bulk copies in flight
     griddep_wait();
-    // A "group" is what advances the state header once: the T frames of an ordinary call, or the
+    // A "group" is what advances the clocks once: the T frames of an ordinary call, or the
     // frames_total one-frame calls of a pipelined graph (frame_k = index inside it).  gi = frame index in
-    // the group.  All frames of a group read the tails the PREVIOUS group left (parity ncalls & 1) and
-    // recompute what they need of their predecessors inside the group; only the group's last frame writes
-    // the new tails (other parity) -- so the frames of a group never depend on each other here.
+    // the group.  All frames of a group read the tails the stream's PREVIOUS group left (parity of its call
+    // count) and recompute what they need of their predecessors inside the group; only the group's last frame
+    // writes the new tails (other parity) -- so the frames of a group never depend on each other here.
     const StateHeader* hdr = reinterpret_cast<const StateHeader*>(state);
-    const int par = (int)(hdr->ncalls & 1);
     const int gi = frame_k + t, GN = (frames_total > 1) ? frames_total : T;
-    float* st = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride;
+    float* st = stream_rec(state, sstride, b);
+    const int par = rec_par(st);
     const float* cb = st + ST_CONV + par * (2 * 4 * NF);
     float* cb_next = st + ST_CONV + (par ^ 1) * (2 * 4 * NF);
 
@@ -189,7 +241,7 @@ front_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride, 
     }
     trace_.mark(3);
     // next conv_buf = spectrogram rows of the last two frames of the group, written by its last frame
-    if (gi == GN - 1) {
+    if (gi == GN - 1 && stream_active(active, b)) {
         for (int e = tid; e < 4 * NF; e += 256) {
             cb_next[e] = U[1][e / NF][1 + e % NF];
             cb_next[4 * NF + e] = U[2][e / NF][1 + e % NF];
@@ -205,7 +257,8 @@ front_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride, 
 __global__ void __launch_bounds__(256)
 front_many_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride, int x_len, float* __restrict__ X,
                   float* __restrict__ state, int64_t sstride, SepWeights w, int T, int pos_rel, const float* __restrict__ emb,
-                  float* __restrict__ spk_pre, int chunk, int n_chunks, int n_streams, int n_workers) {
+                  float* __restrict__ spk_pre, int chunk, int n_chunks, int n_streams, int n_workers,
+                  const uint8_t* __restrict__ active) {
     extern __shared__ __align__(16) float wat_s[];     // [192][196]
     __shared__ __align__(16) float xs[NMIC][NFFT];      // the samples of the frame being transformed (>= 288 floats: gate CTA scratch)
     __shared__ float U[3][4][100];      // ring: frame g -> slot (g + 3) % 3; [ch][1 + f], zero-padded in f
@@ -214,7 +267,7 @@ front_many_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstr
     const int tid = threadIdx.x;
     if ((int)blockIdx.x >= n_workers) {        // one more CTA per stream: speaker-gate memo
         griddep_wait();
-        spk_gate_cta(emb, spk_pre, state, sstride, w, (int)blockIdx.x - n_workers, &xs[0][0]);
+        spk_gate_cta(emb, spk_pre, state, sstride, w, (int)blockIdx.x - n_workers, &xs[0][0], active);
         return;
     }
     if (tid == 0) { mbar_init(&wbar, 1); mbar_fence_init(); }
@@ -228,14 +281,15 @@ front_many_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstr
     const float bias = __ldg(w.bc + o);
     griddep_wait();
     const StateHeader* hdr = reinterpret_cast<const StateHeader*>(state);
-    const int par = (int)(hdr->ncalls & 1);
     const int sbase = pos_rel ? (int)(hdr->pos - hdr->clip_base) * HOP : 0;
     mbar_wait(&wbar, 0);
     // one CTA walks (stream, chunk) items: frames [c*chunk, min(T, (c+1)*chunk)) of stream b
     for (int item = blockIdx.x; item < n_streams * n_chunks; item += n_workers) {
     const int b = item / n_chunks, c = item % n_chunks;
     const int t0 = c * chunk, t1 = min(T, t0 + chunk);
-    float* st = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride;
+    float* st = stream_rec(state, sstride, b);
+    const int par = rec_par(st);
+    const bool live = stream_active(active, b);
     const float* cb = st + ST_CONV + par * (2 * 4 * NF);
     float* cb_next = st + ST_CONV + (par ^ 1) * (2 * 4 * NF);
     const float* xb = x + (int64_t)b * x_bstride;
@@ -310,7 +364,7 @@ front_many_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstr
                     if (f + 4 * u < NF) X[(((int64_t)b * T + t) * NF + f + 4 * u) * CH + o] = acc[u];
             }
         }
-        if (t == T - 1) {                          // next conv tails = spectrogram rows of the call's last two frames
+        if (t == T - 1 && live) {                  // next conv tails = spectrogram rows of the call's last two frames
             for (int e = tid; e < 4 * NF; e += 256) {
                 cb_next[e] = U[(t - 1 + 3) % 3][e / NF][1 + e % NF];
                 cb_next[4 * NF + e] = U[(t + 3) % 3][e / NF][1 + e % NF];
@@ -328,9 +382,11 @@ front_many_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstr
 // embedding with the one the cached gate was built from and returns at once if they are equal
 // (the streaming steady state).  Otherwise that CTA rebuilds the gate (6208x256 GEMV + LayerNorm).
 __device__ void spk_gate_cta(const float* __restrict__ emb, float* __restrict__ pre, float* __restrict__ state,
-                             int64_t sstride, const SepWeights& w, int b, float* red /* >= 288 floats smem */) {
+                             int64_t sstride, const SepWeights& w, int b, float* red /* >= 288 floats smem */,
+                             const uint8_t* __restrict__ active) {
+    if (!stream_active(active, b)) return;     // a stream that skips this hop keeps its record as it is, memo included
     const int tid = threadIdx.x;
-    float* st = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride;
+    float* st = stream_rec(state, sstride, b);
     const float e = emb[(int64_t)b * SPK + tid];
     // memo key: the embedding AND the weight generation (a reused state must not keep a gate built from old weights)
     const int same = __syncthreads_and(e == st[ST_EMB + tid] && __float_as_int(st[ST_GEN]) == w.gen);
@@ -375,16 +431,16 @@ __device__ void spk_gate_cta(const float* __restrict__ emb, float* __restrict__ 
 
 // ------------------------------------------------------------------------------------------
 // K/V history -> linear scratch for multi-frame calls.  Kall[b*4+h][0..48] = ring slots of frames
-// pos-49 .. pos-1 (never-written slots are zero = the reference's zero-initialised K_buf/V_buf).
+// pos-49 .. pos-1 of stream b's clock (frames before its start are zero = the reference's zero-initialised K_buf/V_buf).
 __global__ void kv_gather_kernel(const float* __restrict__ state, int64_t sstride, int blk,
                                  float* __restrict__ Kall, float* __restrict__ Vall, int T) {
     griddep_launch();
     griddep_wait();
     const int i = blockIdx.x, bh = blockIdx.y, b = bh / NHEAD, h = bh % NHEAD;
-    const StateHeader* hdr = reinterpret_cast<const StateHeader*>(state);
-    const long long fr = hdr->pos - (ATT - 1) + i;
+    const float* rec = stream_rec(state, sstride, b);
+    const long long fr = rec_pos(rec) - (ATT - 1) + i;
     const int slot = (int)(((fr % RING) + RING) % RING);
-    const float* sb = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride + ST_BLK + (int64_t)blk * BK_STRIDE;
+    const float* sb = rec + ST_BLK + (int64_t)blk * BK_STRIDE;
     const float4* ks = reinterpret_cast<const float4*>(sb + BK_K + ((int64_t)h * RING + slot) * QK_LD);
     const float4* vs = reinterpret_cast<const float4*>(sb + BK_V + ((int64_t)h * RING + slot) * V_DIM);
     float4* kd = reinterpret_cast<float4*>(Kall + ((int64_t)bh * (ATT - 1 + T) + i) * QK_LD);
@@ -407,7 +463,7 @@ constexpr size_t QKV_SMEM = (size_t)(64 * 100 + 64 * NQKV + NF * QKV_PLD + QKV_L
 __global__ void __launch_bounds__(QKV_THREADS)
 qkv_kernel(const float* __restrict__ X, const float* __restrict__ pre, float* __restrict__ Qbuf,
            float* __restrict__ Kall, float* __restrict__ Vall, float* __restrict__ state, int64_t sstride, int blk,
-           BlockWeights w, int T, int frame_k) {
+           BlockWeights w, int T, int frame_k, const uint8_t* __restrict__ active) {
     extern __shared__ __align__(16) float sm[];
     float* Xt = sm;                      // [64][100]  k-major, rows padded to 100 (zeros)
     float* Ws = Xt + 64 * 100;           // [64][112]
@@ -512,8 +568,8 @@ qkv_kernel(const float* __restrict__ X, const float* __restrict__ pre, float* __
     const float rs = rsqrtf(warp_sum(q) / (float)n + 1e-5f);
     const float* gam = LNP + (which == 0 ? 0 : (which == 1 ? 2 * QK_LD : 4 * QK_LD));
     const float* bet = LNP + (which == 0 ? QK_LD : (which == 1 ? 3 * QK_LD : 4 * QK_LD + V_DIM));
-    const StateHeader* hdr = reinterpret_cast<const StateHeader*>(state);
-    const long long pos = hdr->pos + frame_k;
+    float* rec = stream_rec(state, sstride, b);
+    const long long pos = rec_pos(rec) + frame_k;
     const int ld = (which == 2) ? V_DIM : QK_LD;
     float* dst0 = nullptr;   // linear scratch / Q buffer
     float* dst1 = nullptr;   // ring slot
@@ -521,9 +577,9 @@ qkv_kernel(const float* __restrict__ X, const float* __restrict__ pre, float* __
     if (which == 0) {
         dst0 = Qbuf + (bh * T + t) * QK_LD;
     } else {
-        float* sb = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride + ST_BLK + (int64_t)blk * BK_STRIDE;
+        float* sb = rec + ST_BLK + (int64_t)blk * BK_STRIDE;
         const int slot = (int)((pos + t) % RING);
-        if (t >= T - ATT)
+        if (t >= T - ATT && stream_active(active, b))
             dst1 = sb + (which == 1 ? BK_K : BK_V) + ((int64_t)h * RING + slot) * ld;
         if (T > 1) dst0 = (which == 1 ? Kall : Vall) + (bh * (ATT - 1 + T) + (ATT - 1) + t) * ld;
     }
@@ -553,7 +609,8 @@ constexpr size_t QKV_MANY_SMEM = (size_t)(2 * NF * QKV_PLD + QKV_LNP) * sizeof(f
 
 __global__ void __launch_bounds__(QKV_THREADS)
 qkv_many_kernel(const float* __restrict__ pre, float* __restrict__ Qbuf, float* __restrict__ Kall, float* __restrict__ Vall,
-                float* __restrict__ state, int64_t sstride, int blk, BlockWeights w, int T, int n_frames) {
+                float* __restrict__ state, int64_t sstride, int blk, BlockWeights w, int T, int n_frames,
+                const uint8_t* __restrict__ active) {
     extern __shared__ __align__(16) float sm[];
     float* Pb[2] = {sm, sm + NF * QKV_PLD};
     float* LNP = sm + 2 * NF * QKV_PLD;
@@ -570,8 +627,6 @@ qkv_many_kernel(const float* __restrict__ pre, float* __restrict__ Qbuf, float* 
         tma_load_1d(dst, src, (tid < 4 ? QK_LD : V_DIM) * 4, &bars[2]);
     }
     griddep_wait();
-    const StateHeader* hdr = reinterpret_cast<const StateHeader*>(state);
-    const long long pos0 = hdr->pos;
     int fi = blockIdx.x;
     if (fi < n_frames && tid == 0) {
         mbar_expect_tx(&bars[0], NF * NQKV * 4);
@@ -626,9 +681,10 @@ qkv_many_kernel(const float* __restrict__ pre, float* __restrict__ Qbuf, float* 
         if (which == 0) {
             dst0 = Qbuf + (bh * T + t) * QK_LD;
         } else {
-            float* sb = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride + ST_BLK + (int64_t)blk * BK_STRIDE;
-            const int slot = (int)((pos0 + t) % RING);
-            if (t >= T - ATT) dst1 = sb + (which == 1 ? BK_K : BK_V) + ((int64_t)h * RING + slot) * ld;
+            float* rec = stream_rec(state, sstride, b);
+            float* sb = rec + ST_BLK + (int64_t)blk * BK_STRIDE;
+            const int slot = (int)((rec_pos(rec) + t) % RING);
+            if (t >= T - ATT && stream_active(active, b)) dst1 = sb + (which == 1 ? BK_K : BK_V) + ((int64_t)h * RING + slot) * ld;
             if (T > 1) dst0 = (which == 1 ? Kall : Vall) + (bh * (ATT - 1 + T) + (ATT - 1) + t) * ld;
         }
         {
@@ -667,11 +723,12 @@ attn_kernel(const float* __restrict__ Qbuf, const float* __restrict__ Kall, cons
     const float* kb;
     const float* vb;
     int first = 0, wrap = 0x7fffffff;       // window row j -> storage row (first + j) % wrap
-    if (T == 1) {                           // ring: window = frames pos-49 .. pos
-        const float* sb = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride + ST_BLK + (int64_t)blk * BK_STRIDE;
+    if (T == 1) {                           // ring: window = frames pos-49 .. pos of the stream's clock
+        const float* rec = stream_rec(state, sstride, b);
+        const float* sb = rec + ST_BLK + (int64_t)blk * BK_STRIDE;
         kb = sb + BK_K + (int64_t)h * RING * QK_LD;
         vb = sb + BK_V + (int64_t)h * RING * V_DIM;
-        const long long p0 = reinterpret_cast<const StateHeader*>(state)->pos + frame_k - (ATT - 1);
+        const long long p0 = rec_pos(rec) + frame_k - (ATT - 1);
         first = (int)(((p0 % RING) + RING) % RING);
         wrap = RING;
     } else {
@@ -863,11 +920,12 @@ attn_cluster_kernel(const float* __restrict__ Qbuf, const float* __restrict__ Ka
     const float* kb;
     const float* vb;
     int first = j0, wrap = 0x7fffffff;      // window row j -> storage row (first + j) % wrap
-    if (T == 1) {                           // ring: window = frames pos-49 .. pos, frame n lives in slot n mod RING
-        const float* sb = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride + ST_BLK + (int64_t)blk * BK_STRIDE;
+    if (T == 1) {                           // ring: window = frames pos-49 .. pos of the stream's clock, frame n in slot n mod RING
+        const float* rec = stream_rec(state, sstride, b);
+        const float* sb = rec + ST_BLK + (int64_t)blk * BK_STRIDE;
         kb = sb + BK_K + (int64_t)h * RING * QK_LD;
         vb = sb + BK_V + (int64_t)h * RING * V_DIM;
-        const long long p0 = reinterpret_cast<const StateHeader*>(state)->pos + frame_k - (ATT - 1) + j0;
+        const long long p0 = rec_pos(rec) + frame_k - (ATT - 1) + j0;
         first = (int)(((p0 % RING) + RING) % RING);
         wrap = RING;
     } else {
@@ -1078,7 +1136,7 @@ attn_out_kernel(const float* __restrict__ Z, float* __restrict__ X, const float*
 // dependency wait).  The four partial windows meet in CTA 0 through distributed shared memory, in a fixed
 // order, and CTA 0 does the overlap-add and the store.  (v1 ran the frame in one CTA, which made it the
 // slowest stage of the one-hop pipeline once the mid section was split.)
-// The last CTA to finish advances the state header (pos += T, ncalls += 1).
+// The last CTA to finish advances the header and the clocks of the active streams (finish_call).
 constexpr int BACK_CL = 4;
 constexpr int BACK_FMAX = (NF + BACK_CL - 1) / BACK_CL;       // 25 bins per CTA at most
 constexpr size_t BACK_SMEM = (size_t)(4 * (BACK_FMAX + 2) * 64 + 2 * BACK_FMAX * NFFT + 2 * NSRC * NROW + NSRC * NFFT) * sizeof(float);
@@ -1088,7 +1146,7 @@ __device__ __forceinline__ int back_f0(int part) { return (part * NF) / BACK_CL;
 __global__ void __launch_bounds__(256)
 back_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_bstride, int64_t y_cstride,
             int y_len, float* __restrict__ state, int64_t sstride, SepWeights w, int T, int pos_rel, int frame_k,
-            int frames_total, int sample_off, int64_t hist_stride) {
+            int frames_total, int sample_off, int64_t hist_stride, const uint8_t* __restrict__ active) {
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
     extern __shared__ __align__(16) float sm[];
@@ -1131,10 +1189,11 @@ back_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_bstrid
     __syncthreads();
     griddep_wait();
     trace_.mark(0);
-    StateHeader* hdr = reinterpret_cast<StateHeader*>(state);
-    const int par = (int)(hdr->ncalls & 1);
+    const StateHeader* hdr = reinterpret_cast<const StateHeader*>(state);
     const int soff = sample_off + (pos_rel ? (int)(hdr->pos - hdr->clip_base) * HOP : 0);
-    float* st = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride;
+    float* st = stream_rec(state, sstride, b);
+    const int par = rec_par(st);
+    const bool live = stream_active(active, b);
     const float* db = st + ST_DECONV + par * (2 * FC);
     float* db_next = st + ST_DECONV + (par ^ 1) * (2 * FC);
     const float* ib = st + ST_ISTFT + par * (NSRC * NROW);
@@ -1191,7 +1250,7 @@ back_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_bstrid
             }
     }
     // next deconv tails (frames GN-2, GN-1) come straight from the staged frames of the group's last frame
-    if (gi == GN - 1) {
+    if (gi == GN - 1 && live) {
         for (int i = tid; i < nf * 16; i += 256) {
             const int r = i / 16, c4 = i % 16;
             reinterpret_cast<float4*>(db_next + (f0 + r) * 64)[c4] = reinterpret_cast<const float4*>(Xs + (2 * ld + 1 + r) * 64)[c4];
@@ -1218,7 +1277,7 @@ back_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_bstrid
             wacc[item] = acc;
         }
     }
-    if (gi == GN - 1)
+    if (gi == GN - 1 && live)
         for (int i = tid; i < NSRC * 2 * nf; i += 256) {
             const int idx = (i / (2 * nf)) * NROW + ((i / nf) & 1) * NF + f0 + i % nf;
             ib_next[idx] = R[NSRC * NROW + idx];
@@ -1226,7 +1285,7 @@ back_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_bstrid
     trace_.mark(3);
     cluster.sync();                         // all four partial windows are complete and visible cluster-wide
     trace_.mark(4);
-    if (part == 0) {
+    if (part == 0 && live) {
         for (int i = tid; i < NSRC * HOP; i += 256) {
             const int ear = i / HOP, n = i % HOP;
             const int s = HOP * t + n + soff;
@@ -1246,18 +1305,9 @@ back_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_bstrid
     trace_.mark(5);
     cluster.sync();                         // nobody leaves while CTA 0 may still read its shared memory
     trace_.mark(6);
-    // ordinary call: the last CTA to finish advances the header (a pipelined graph runs several back_kernels
-    // at once and advances it with advance_header_kernel after all of its frames instead)
-    if (frames_total == 1 && tid == 0) {
-        __threadfence();
-        const int prev = atomicAdd(&hdr->done, 1);
-        if (prev == (int)(gridDim.x * gridDim.y) - 1) {
-            hdr->pos += T;
-            hdr->ncalls += 1;
-            hdr->done = 0;
-            __threadfence();
-        }
-    }
+    // ordinary call: the last CTA to finish advances the clocks (a pipelined graph runs several back_kernels
+    // at once and advances them with advance_header_kernel after all of its frames instead)
+    if (frames_total == 1) finish_call(state, sstride, gridDim.y, T, active);
 }
 
 
@@ -1272,7 +1322,8 @@ constexpr size_t BACK_MANY_SMEM = (size_t)(4 * (BACK_FMAX + 2) * 64 + 2 * BACK_F
 
 __global__ void __launch_bounds__(256)
 back_many_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_bstride, int64_t y_cstride, int y_len,
-                 float* __restrict__ state, int64_t sstride, SepWeights w, int T, int pos_rel, int chunk, int n_chunks, int n_streams) {
+                 float* __restrict__ state, int64_t sstride, SepWeights w, int T, int pos_rel, int chunk, int n_chunks, int n_streams,
+                 const uint8_t* __restrict__ active) {
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
     extern __shared__ __align__(16) float sm[];
@@ -1309,8 +1360,7 @@ back_many_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_b
     for (int o = 0; o < 4; ++o) bd[o] = __ldg(w.bd + o);
     __syncthreads();
     griddep_wait();
-    StateHeader* hdr = reinterpret_cast<StateHeader*>(state);
-    const int par = (int)(hdr->ncalls & 1);
+    const StateHeader* hdr = reinterpret_cast<const StateHeader*>(state);
     const int soff = pos_rel ? (int)(hdr->pos - hdr->clip_base) * HOP : 0;
     const int lo = max(f0 - 1, 0), hi = min(f1 + 1, NF);          // staged bins that exist: [lo, hi)
     // ring-slot barriers: bit s of usebits = parity the NEXT staging into slot s completes; waitbits = parity to wait for the latest one
@@ -1321,7 +1371,9 @@ back_many_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_b
     for (int item = cl; item < n_streams * n_chunks; item += n_cl) {
         const int b = item / n_chunks, c = item % n_chunks;
         const int t0 = c * chunk, t1 = min(T, t0 + chunk);
-        float* st = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride;
+        float* st = stream_rec(state, sstride, b);
+        const int par = rec_par(st);
+        const bool live = stream_active(active, b);
         const float* db = st + ST_DECONV + par * (2 * FC);
         float* db_next = st + ST_DECONV + (par ^ 1) * (2 * FC);
         const float* ib = st + ST_ISTFT + par * (NSRC * NROW);
@@ -1381,7 +1433,7 @@ back_many_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_b
             __syncthreads();                           // frame t-1's readers of frame t-3's slot are done; R[(t-1)&1] complete
             if (t + 1 < t1) stage(t + 1);              // into the slot of frame t-3
             deconv(t);
-            if (t == T - 1) {                          // next deconv tails: frames T-2, T-1 (own bins)
+            if (t == T - 1 && live) {                  // next deconv tails: frames T-2, T-1 (own bins)
                 for (int i = tid; i < nf * 16; i += 256) {
                     const int r = i / 16, c4 = i % 16;
                     reinterpret_cast<float4*>(db_next + (f0 + r) * 64)[c4] =
@@ -1408,13 +1460,13 @@ back_many_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_b
                     wa[it2] = acc;
                 }
             }
-            if (t == T - 1)
+            if (t == T - 1 && live)
                 for (int i = tid; i < NSRC * 2 * nf; i += 256) {
                     const int idx = (i / (2 * nf)) * NROW + ((i / nf) & 1) * NF + f0 + i % nf;
                     ib_next[idx] = R[(t & 1) * NSRC * NROW + idx];
                 }
             cluster.sync();                            // the four partial windows of frame t are complete and visible cluster-wide
-            if (part == 0) {                           // (wacc is double-buffered: the peers go on with the next frame meanwhile)
+            if (part == 0 && live) {                   // (wacc is double-buffered: the peers go on with the next frame meanwhile)
                 for (int i = tid; i < NSRC * HOP; i += 256) {
                     const int ear = i / HOP, n = i % HOP;
                     const int s2 = HOP * t + n + soff;
@@ -1434,16 +1486,7 @@ back_many_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_b
         }
     }
     cluster.sync();                         // nobody leaves while CTA 0 may still read its shared memory
-    if (tid == 0) {                         // the last CTA to finish advances the header
-        __threadfence();
-        const int prev = atomicAdd(&hdr->done, 1);
-        if (prev == (int)(gridDim.x * gridDim.y) - 1) {
-            hdr->pos += T;
-            hdr->ncalls += 1;
-            hdr->done = 0;
-            __threadfence();
-        }
-    }
+    finish_call(state, sstride, n_streams, T, active);      // the last CTA to finish advances the clocks
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1493,7 +1536,7 @@ ln_frame_res_kernel(const float* __restrict__ P, float* __restrict__ X, const fl
 // state records, and h again as contiguous rows for the Linear that follows.  One thread per (row, hidden unit).
 __global__ void __launch_bounds__(256)
 lstm_cell_rows_kernel(const float* __restrict__ gates, float* __restrict__ state, int64_t sstride, int blk, float* __restrict__ Hout,
-                      int rows) {
+                      int rows, const uint8_t* __restrict__ active) {
     griddep_launch();
     griddep_wait();
     const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
@@ -1501,7 +1544,7 @@ lstm_cell_rows_kernel(const float* __restrict__ gates, float* __restrict__ state
     const int row = (int)(i >> 6), j = (int)(i & 63);
     const int b = row / NF, f = row % NF;
     const float4 g = *reinterpret_cast<const float4*>(gates + (int64_t)row * 256 + j * 4);
-    float* base = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride + ST_BLK + (int64_t)blk * BK_STRIDE;
+    float* base = stream_rec(state, sstride, b) + ST_BLK + (int64_t)blk * BK_STRIDE;
     float* hp = base + BK_H + f * 64 + j;
     float* cp = base + BK_C + f * 64 + j;
     constexpr float LOG2E = 1.4426950408889634f;
@@ -1511,8 +1554,10 @@ lstm_cell_rows_kernel(const float* __restrict__ gates, float* __restrict__ state
     const float og = __fdividef(1.f, 1.f + ex2_ftz(-LOG2E * g.w));
     const float c = fg * *cp + ig * gg;
     const float h = og * (__fdividef(2.f, 1.f + ex2_ftz(-2.f * LOG2E * c)) - 1.f);
-    *cp = c;
-    *hp = h;
+    if (stream_active(active, b)) {
+        *cp = c;
+        *hp = h;
+    }
     Hout[i] = h;
 }
 

@@ -31,10 +31,14 @@ constexpr int FC = NF * CH;         // 6208
 constexpr int NQKV = 2 * NHEAD * QE + NHEAD * VD;  // 112
 
 // ---- state: one allocation = header + B stream records ---------------------------------------
-// header (64 B): int64 pos (frames consumed so far), int64 ncalls (parity for the small
-// double-buffered tails), int64 clip_base (pos at the start of the clip being streamed: lets a
-// captured CUDA graph address "chunk pos - clip_base" of a whole-clip buffer without any
+// header (64 B): the CALL clock of the whole state: int64 pos (frames the calls have covered so
+// far), int64 ncalls (calls so far), int64 clip_base (pos at the start of the clip being streamed:
+// lets a captured CUDA graph address "chunk pos - clip_base" of a whole-clip buffer without any
 // per-launch parameter), int32 done (last-CTA counter of the final kernel).
+// Every stream record carries its OWN frame clock (ST_POS, ST_CALLS below): the K/V ring slot of a
+// frame and the parity of the double-buffered tails come from it, so streams of one state may start,
+// restart and skip hops independently.  Until a stream is reset, copied or skipped, its clock equals
+// the header's.
 struct StateHeader {
     long long pos;
     long long ncalls;
@@ -47,6 +51,8 @@ static_assert(sizeof(StateHeader) == 64, "header");
 // per-stream record, offsets in floats
 constexpr int64_t ST_EMB = 0;                                   // [256] embedding the gate was built from
 constexpr int64_t ST_GEN = ST_EMB + SPK;                        // [4] slot 0: weight generation (int bits) the gate was built with
+constexpr int64_t ST_CALLS = ST_GEN + 1;                        // int32: the stream's calls so far (bit 0 = parity of its tails)
+constexpr int64_t ST_POS = ST_GEN + 2;                          // int64 (slots 2-3): frames the stream has consumed
 constexpr int64_t ST_GATE = ST_GEN + 4;                         // [97][64]  LN(W e + b), (f, c) order
 constexpr int64_t ST_CONV = ST_GATE + FC;                       // [2 parity][2 frames][4][97]
 constexpr int64_t ST_DECONV = ST_CONV + 2 * 2 * 4 * NF;         // [2][2][97][64]
@@ -58,6 +64,7 @@ constexpr int64_t BK_H = BK_V + (int64_t)NHEAD * RING * V_DIM;  // [97][64]
 constexpr int64_t BK_C = BK_H + FC;                             // [97][64]
 constexpr int64_t BK_STRIDE = BK_C + FC;
 static_assert(ST_BLK % 4 == 0 && BK_STRIDE % 4 == 0 && BK_V % 4 == 0, "16 B alignment");
+static_assert(ST_POS % 2 == 0, "the int64 stream clock is 8 B aligned (records start 16 B aligned)");
 
 inline int64_t stream_stride(int n_blocks) { return ST_BLK + (int64_t)n_blocks * BK_STRIDE; }
 

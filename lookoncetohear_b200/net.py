@@ -99,16 +99,21 @@ class SepState(dict):
     is kept because reference callers treat the state as an opaque dict they pass back.
     ``to_reference()`` / ``load_reference()`` convert to / from the reference's nested dict of
     tensors (tfgridnet_causal.py:173-186, :408-427).
+
+    Every stream (slot) has its own frame clock, so the streams of one state need not start together or
+    advance on every hop: ``reset_streams`` starts fresh streams in some slots, ``Net.predict(..., active=)``
+    advances only some streams, ``copy_streams_from`` moves streams between slots and states.
     """
 
     _OFFSET_NAMES = ("ring", "k_ld", "k_dim", "v_dim", "att", "st_emb", "st_gate", "st_conv", "st_deconv",
-                     "st_istft", "st_blk", "bk_k", "bk_v", "bk_h", "bk_c", "bk_stride")
+                     "st_istft", "st_blk", "bk_k", "bk_v", "bk_h", "bk_c", "bk_stride", "st_pos", "st_calls")
 
-    def __init__(self, buf, batch, n_blocks, header_bytes, stride, offsets):
+    def __init__(self, buf, batch, n_blocks, header_bytes, stride, offsets, net=None):
         super().__init__()
         self.buf, self.batch, self.n_blocks = buf, batch, n_blocks
         self.header_floats, self.stride = header_bytes // 4, stride
         self.lay = dict(zip(self._OFFSET_NAMES, offsets))
+        self._net = net                  # the Net whose engine runs reset_streams / copy_streams_from
         self["buf"] = buf
 
     # ---- views ------------------------------------------------------------------------------
@@ -116,15 +121,28 @@ class SepState(dict):
         return self.buf[self.header_floats:].view(self.batch, self.stride)
 
     def header(self):
-        """(pos, ncalls) -- synchronises."""
+        """(pos, ncalls) of the whole state: frames and calls the predict calls have covered -- synchronises."""
         h = self.buf[:4].view(torch.int64).cpu()
         return int(h[0]), int(h[1])
 
+    def _clocks(self):
+        """Views of the per-stream clocks: frames consumed [B] int64, calls [B] int32."""
+        r, L = self._rec(), self.lay
+        pos = r[:, L["st_pos"]:L["st_pos"] + 2].view(torch.int64)[:, 0]
+        calls = r[:, L["st_calls"]:L["st_calls"] + 1].view(torch.int32)[:, 0]
+        return pos, calls
+
+    def stream_pos(self):
+        """Frames each stream has consumed, a list of `batch` ints -- synchronises."""
+        return self._clocks()[0].cpu().tolist()
+
     def _tails(self, r, par):
+        """Current tails of every stream; par: one parity for all streams (views) or a [B] tensor of parities (copies)."""
         L, B = self.lay, self.batch
-        conv = r[:, L["st_conv"]:L["st_deconv"]].view(B, 2, 2, 4, 97)[:, par]            # [B,slot,ch,F]
-        deconv = r[:, L["st_deconv"]:L["st_istft"]].view(B, 2, 2, 97, 64)[:, par]        # [B,slot,F,C]
-        istft = r[:, L["st_istft"]:L["st_blk"]].view(B, 2, 2, 194)[:, par]               # [B,ear,2F]
+        sel = (slice(None), par) if isinstance(par, int) else (torch.arange(B, device=r.device), par)
+        conv = r[:, L["st_conv"]:L["st_deconv"]].view(B, 2, 2, 4, 97)[sel]            # [B,slot,ch,F]
+        deconv = r[:, L["st_deconv"]:L["st_istft"]].view(B, 2, 2, 97, 64)[sel]        # [B,slot,F,C]
+        istft = r[:, L["st_istft"]:L["st_blk"]].view(B, 2, 2, 194)[sel]               # [B,ear,2F]
         return conv, deconv, istft
 
     def _block(self, r, i):
@@ -138,29 +156,34 @@ class SepState(dict):
 
     def to_reference(self):
         """Nested dict with the reference's keys and shapes (copies; synchronises)."""
-        pos, ncalls = self.header()
         L, r, B = self.lay, self._rec(), self.batch
+        dev = self.buf.device
+        pos, calls = self._clocks()
         hist = L["att"] - 1
-        conv, deconv, istft = self._tails(r, ncalls & 1)
+        conv, deconv, istft = self._tails(r, (calls & 1).long())
         out = dict(conv_buf=conv.permute(0, 2, 1, 3).contiguous(),
                    deconv_buf=deconv.permute(0, 3, 1, 2).contiguous(),
                    istft_buf=istft.unsqueeze(-1).contiguous(), gridnet_bufs={})
-        # ring slot of frame n is n % ring; history rows are frames pos-49 .. pos-1
-        frames = torch.arange(pos - hist, pos)
-        slots = torch.remainder(frames, L["ring"]).to(self.buf.device)
-        live = (frames >= 0).to(self.buf.device, self.buf.dtype)[None, None, :, None]
+        # ring slot of frame n is n % ring; the history rows of stream b are frames pos_b-49 .. pos_b-1 of its own clock
+        frames = pos.cpu()[:, None] - hist + torch.arange(hist)[None, :]                  # [B, hist]
+        slots = torch.remainder(frames, L["ring"]).to(dev)
+        live = (frames >= 0).to(dev, self.buf.dtype)[:, None, :, None]
+        rows = torch.arange(B, device=dev)[:, None]
         for i in range(self.n_blocks):
             K, V, h, c = self._block(r, i)
+            Kh = K[rows, :, slots].permute(0, 2, 1, 3)                                     # [B, 4, hist, k_ld]
+            Vh = V[rows, :, slots].permute(0, 2, 1, 3)
             out["gridnet_bufs"][f"buf{i}"] = dict(
-                K_buf=(K[:, :, slots, :L["k_dim"]] * live).reshape(B * 4, hist, L["k_dim"]).contiguous(),
-                V_buf=(V[:, :, slots] * live).reshape(B * 4, hist, L["v_dim"]).contiguous(),
+                K_buf=(Kh[..., :L["k_dim"]] * live).reshape(B * 4, hist, L["k_dim"]).contiguous(),
+                V_buf=(Vh * live).reshape(B * 4, hist, L["v_dim"]).contiguous(),
                 h0=h.reshape(1, B * 97, 64).clone(), c0=c.reshape(1, B * 97, 64).clone())
         return out
 
     def load_reference(self, ref_state):
         """Import a state in the reference's format (the nested dict ``Net.init_buffers`` /
         ``predict`` of the reference produce) so a stream started on the reference implementation can
-        be continued here.  The 49 history rows become frames 0..48 of the rings (pos = 49)."""
+        be continued here.  The 49 history rows become frames 0..48 of the rings (pos = 49 for the
+        header and every stream)."""
         L, r, B = self.lay, self._rec(), self.batch
         hist = L["att"] - 1
         dev, dt = self.buf.device, self.buf.dtype
@@ -168,6 +191,9 @@ class SepState(dict):
         hdr = self.buf[:4].view(torch.int64)
         hdr[0] = hist            # pos: frames consumed so far
         hdr[1] = 0               # ncalls: tails live in parity slot 0
+        pos, calls = self._clocks()
+        pos.fill_(hist)
+        calls.fill_(0)
         conv, deconv, istft = self._tails(r, 0)
         conv.copy_(ref_state["conv_buf"].to(dev, dt).permute(0, 2, 1, 3))
         deconv.copy_(ref_state["deconv_buf"].to(dev, dt).permute(0, 2, 3, 1))
@@ -180,6 +206,56 @@ class SepState(dict):
             h.copy_(g["h0"].to(dev, dt).reshape(B, 97 * 64))
             c.copy_(g["c0"].to(dev, dt).reshape(B, 97 * 64))
         return self
+
+    # ---- serving many listeners ---------------------------------------------------------------
+    def _engine_call(self):
+        if self._net is None:
+            raise ValueError("this state was not made by Net.init_buffers: it has no engine to run on")
+        if self.buf.is_cuda:
+            self._net._sync_weights(self.buf.device)      # the engine is bound to the device of its weights
+        return self._net._engine(), _cabi.lib()
+
+    @staticmethod
+    def _slots(slots):
+        s = torch.as_tensor(slots, dtype=torch.int64).flatten()
+        if s.numel() == 0:
+            raise ValueError("no slots given")
+        return (ctypes.c_int32 * s.numel())(*s.tolist())
+
+    def reset_streams(self, slots):
+        """Start fresh streams in `slots` (a list of slot indices): their records become those of a just-initialised
+        state, the other streams keep running undisturbed.  Asynchronous on the current stream."""
+        h, L = self._engine_call()
+        sl = self._slots(slots)
+        with torch.cuda.device(self.buf.device):
+            _cabi.check_args(L.l2h_sep_state_reset_streams(h, self.buf.data_ptr(), self.batch, sl, len(sl),
+                                                           torch.cuda.current_stream(self.buf.device).cuda_stream))
+        return self
+
+    def copy_streams_from(self, src_state, src_slots, dst_slots):
+        """Continue stream src_slots[i] of `src_state` in slot dst_slots[i] of this state: its whole record, its clock
+        included, is copied, so it goes on exactly as it would have in its old slot.  The states may be the same one, or
+        lie on different devices (then the records travel through host memory).  Asynchronous on the current stream."""
+        if not isinstance(src_state, SepState) or src_state.stride != self.stride:
+            raise ValueError("copy_streams_from: the source must be a SepState of the same network configuration")
+        h, L = self._engine_call()
+        ss, ds = self._slots(src_slots), self._slots(dst_slots)
+        if len(ss) != len(ds):
+            raise ValueError("copy_streams_from: src_slots and dst_slots differ in length")
+        dev = self.buf.device
+        if src_state.buf.device == dev:
+            with torch.cuda.device(dev):
+                _cabi.check_args(L.l2h_sep_state_copy_streams(h, self.buf.data_ptr(), self.batch, ds, src_state.buf.data_ptr(),
+                                                              src_state.batch, ss, len(ss),
+                                                              torch.cuda.current_stream(dev).cuda_stream))
+            return self
+        # another device: the records travel through host memory into a staging state here, then a same-device copy
+        # imports them (its argument checks and gate-memo invalidation are the engine's)
+        if min(ss) < 0 or max(ss) >= src_state.batch:
+            raise ValueError(f"copy_streams_from: a source slot lies outside [0, {src_state.batch})")
+        staged = self._net.init_buffers(len(ss), dev)
+        staged._rec().copy_(src_state._rec()[list(ss)].cpu().to(dev))
+        return self.copy_streams_from(staged, list(range(len(ss))), list(ds))
 
 
 class Net(nn.Module):
@@ -325,19 +401,20 @@ class Net(nn.Module):
         with torch.cuda.device(device):
             _cabi.check(L.l2h_sep_state_init(h, buf.data_ptr(), batch_size,
                                              torch.cuda.current_stream(device).cuda_stream))
-        return SepState(buf, batch_size, self.n_blocks, hb, stride, offs)
+        return SepState(buf, batch_size, self.n_blocks, hb, stride, offs, net=self)
 
     def _state_layout(self):
         """(header bytes, floats per stream record, record offsets) from the C side."""
         L, h = _cabi.lib(), self._engine()
         hb, stride = ctypes.c_int64(), ctypes.c_int64()
         _cabi.check(L.l2h_sep_state_layout(h, ctypes.byref(hb), ctypes.byref(stride)))
-        offs = (ctypes.c_int64 * 16)()
-        _cabi.check(L.l2h_sep_state_offsets(h, offs, 16))
+        n = len(SepState._OFFSET_NAMES)
+        offs = (ctypes.c_int64 * n)()
+        _cabi.check(L.l2h_sep_state_offsets(h, offs, n))
         return hb.value, stride.value, list(offs)
 
-    def _run(self, x, embed, state, frames, out_len, flags=0):
-        """x [B,M,n] (any length; samples beyond n read as zero), embed [B,256]."""
+    def _run(self, x, embed, state, frames, out_len, flags=0, active=None):
+        """x [B,M,n] (any length; samples beyond n read as zero), embed [B,256], active: [B] uint8 device mask or None."""
         self._require_cuda(x)
         dev = x.device
         self._sync_weights(dev)
@@ -349,14 +426,29 @@ class Net(nn.Module):
         y = torch.empty(Bsz, self.num_src, out_len, dtype=torch.float32, device=dev)
         ws, nbytes = self._workspace(dev, Bsz, frames, flags)
         with torch.cuda.device(dev):
-            _cabi.check(_cabi.lib().l2h_sep_forward(
+            _cabi.check(_cabi.lib().l2h_sep_forward_active(
                 self._engine(), x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], embed.data_ptr(),
                 state.buf.data_ptr(), y.data_ptr(), y.stride(0), y.stride(1), out_len, Bsz, frames,
-                ws.data_ptr(), ws.numel(), flags, torch.cuda.current_stream(dev).cuda_stream))
+                ws.data_ptr(), ws.numel(), flags, torch.cuda.current_stream(dev).cuda_stream,
+                None if active is None else active.data_ptr()))
         return y
 
-    def predict(self, x, embed, input_state, pad=True):
-        """Reference net.py:54-66.  x [B,M,N]; embed [B,256]; returns (y [B,S,*], state)."""
+    @staticmethod
+    def _active_mask(active, dev, batch):
+        """`active` of predict as the [batch] uint8 device tensor the engine reads."""
+        if not isinstance(active, torch.Tensor) or active.dtype not in (torch.bool, torch.uint8):
+            raise ValueError("active must be a bool or uint8 tensor")
+        if active.device != dev:
+            raise ValueError(f"active must live on the input's device {dev}, not {active.device}")
+        if tuple(active.shape) != (batch,):
+            raise ValueError(f"active must have shape ({batch},), got {tuple(active.shape)}")
+        return active.contiguous().view(torch.uint8)
+
+    def predict(self, x, embed, input_state, pad=True, active=None):
+        """Reference net.py:54-66.  x [B,M,N]; embed [B,256]; returns (y [B,S,*], state).
+
+        active: None, or for a one-hop call a [B] bool / uint8 CUDA tensor: only the streams with a true entry advance.
+        The others are untouched -- record, clock and speaker-gate memo -- and their rows of y are left unwritten."""
         hop, la = self.stft_chunk_size, self.stft_pad_size
         n = x.shape[-1]
         if pad:
@@ -369,7 +461,12 @@ class Net(nn.Module):
             out_len = frames * hop
         if not isinstance(input_state, SepState):
             raise TypeError("input_state must come from Net.init_buffers()")
-        y = self._run(x, embed, input_state, frames, out_len)
+        if active is not None:
+            if frames != 1:
+                raise ValueError(f"active needs a one-hop call ({hop}+{la} samples with pad=False), this call has {frames} hops")
+            self._require_cuda(x)
+            active = self._active_mask(active, x.device, x.shape[0])
+        y = self._run(x, embed, input_state, frames, out_len, active=active)
         return y, input_state
 
     def forward(self, x, embeds, input_state=None, pad=True):
