@@ -59,8 +59,20 @@ class Lstm(ctypes.Structure):
                 ("bias", ctypes.c_void_p), ("ln_g", ctypes.c_void_p), ("ln_b", ctypes.c_void_p)]
 
 
-MIRRORS = {"kh_sizeof_asource": ASource, "kh_sizeof_gemm": Gemm, "kh_sizeof_plan": Plan, "kh_sizeof_lstm": Lstm}
-SYMBOLS = ("kh_gemm", "kh_gemm_plan", "kh_split_planes", "kh_lstm", "kh_launch_count") + tuple(MIRRORS)
+class SepWeights(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_void_p) for n in ("wqkv_t", "bqkv", "slopes", "lnq_g", "lnq_b", "lnk_g", "lnk_b", "lnv_g", "lnv_b",
+                                                "wp_t", "bp", "lnp_g", "lnp_b")]
+
+
+MIRRORS = {"kh_sizeof_asource": ASource, "kh_sizeof_gemm": Gemm, "kh_sizeof_plan": Plan, "kh_sizeof_lstm": Lstm,
+           "kh_sizeof_sep_weights": SepWeights}
+SYMBOLS = ("kh_gemm", "kh_gemm_plan", "kh_split_planes", "kh_lstm", "kh_launch_count", "kh_sep_layout", "kh_qkv",
+           "kh_qkv_many", "kh_kv_gather", "kh_attention", "kh_attn_out", "kh_ln_frame_res",
+           "kh_attn_cluster_resident") + tuple(MIRRORS)
+
+ATTN_FORMS = {"query": 0, "tile": 1, "cluster": 2}
+SEP_LAYOUT_NAMES = ("RING", "QK_LD", "QK_DIM", "V_DIM", "ATT", "ST_GATE", "ST_BLK", "BK_K", "BK_V", "BK_H", "BK_C",
+                    "BK_STRIDE", "ST_POS", "ST_CALLS", "HEADER_BYTES", "STREAM_STRIDE")
 
 _lib = None
 
@@ -82,6 +94,20 @@ def lib():
                                       ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
         L.kh_lstm.restype = ctypes.c_int
         L.kh_lstm.argtypes = [ctypes.POINTER(Lstm), ctypes.c_int, ctypes.c_int, ctypes.c_char_p, ctypes.c_int, ctypes.c_void_p]
+        P, I, I64, W = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.POINTER(SepWeights)
+        sigs = {
+            "kh_sep_layout": [I, ctypes.POINTER(ctypes.c_int64)],
+            "kh_attn_cluster_resident": [],
+            "kh_qkv": [W, P, P, P, P, P, P, I64, I, I, I, I, P, P],
+            "kh_qkv_many": [W, P, P, P, P, P, I64, I, I, I, I, P, P],
+            "kh_kv_gather": [P, I64, I, P, P, I, I, P],
+            "kh_attention": [I, P, P, P, P, I64, I, P, I, I, I, P],
+            "kh_attn_out": [W, P, P, P, I64, I, I, I, P],
+            "kh_ln_frame_res": [W, P, P, P, I64, I, I, I, P],
+        }
+        for s, args in sigs.items():
+            getattr(L, s).restype = ctypes.c_int
+            getattr(L, s).argtypes = args
         _lib = L
     return _lib
 
@@ -113,6 +139,40 @@ def lstm(args, variant, passes=3):
     return rc, why.value.decode()
 
 
+def sep_layout(n_blocks):
+    """kh_sep_layout as {name: value} (SEP_LAYOUT_NAMES): offsets in floats, HEADER_BYTES in bytes"""
+    out = (ctypes.c_int64 * 32)()
+    n = lib().kh_sep_layout(n_blocks, out)
+    return dict(zip(SEP_LAYOUT_NAMES, list(out)[:n]))
+
+
+def qkv(w, X, pre, Q, K, V, state, sstride, blk, B, T, frame_k=0, active=None):
+    return lib().kh_qkv(ctypes.byref(w), ptr(X), ptr(pre), ptr(Q), ptr(K), ptr(V), ptr(state), sstride, blk, B, T, frame_k,
+                        ptr(active), stream())
+
+
+def qkv_many(w, pre, Q, K, V, state, sstride, blk, T, grid, n_frames, active=None):
+    return lib().kh_qkv_many(ctypes.byref(w), ptr(pre), ptr(Q), ptr(K), ptr(V), ptr(state), sstride, blk, T, grid, n_frames,
+                             ptr(active), stream())
+
+
+def kv_gather(state, sstride, blk, K, V, B, T):
+    return lib().kh_kv_gather(ptr(state), sstride, blk, ptr(K), ptr(V), B, T, stream())
+
+
+def attention(form, Q, K, V, state, sstride, blk, Z, B, T, frame_k=0):
+    return lib().kh_attention(ATTN_FORMS[form], ptr(Q), ptr(K), ptr(V), ptr(state), sstride, blk, ptr(Z), B, T, frame_k,
+                              stream())
+
+
+def attn_out(w, Z, X, state, sstride, B, T, apply_gate):
+    return lib().kh_attn_out(ctypes.byref(w), ptr(Z), ptr(X), ptr(state), sstride, B, T, apply_gate, stream())
+
+
+def ln_frame_res(w, P, X, state, sstride, B, T, apply_gate):
+    return lib().kh_ln_frame_res(ctypes.byref(w), ptr(P), ptr(X), ptr(state), sstride, B, T, apply_gate, stream())
+
+
 # ---- float64 references ---------------------------------------------------------------------------------------------
 def split_bf16(x):
     """bf16 hi/lo planes of fp32 x, as the kernels form them (round to nearest even; x - hi exact in fp32)."""
@@ -134,11 +194,130 @@ def split_product(a, b, passes):
     return out
 
 
-def layer_norm64(x, g, b, eps=1e-5):
+def layer_norm64(x, g, b, eps=1e-5, unbiased=False):
+    """LayerNorm over the last dimension: biased variance, eps inside the sqrt (unbiased=True: a mutated reference)"""
     x = x.double()
     mu = x.mean(-1, keepdim=True)
     var = ((x - mu) ** 2).mean(-1, keepdim=True)
+    if unbiased:
+        var = var * x.shape[-1] / (x.shape[-1] - 1)
     return (x - mu) / torch.sqrt(var + eps) * g.double() + b.double()
+
+
+# ---- the separator's attention section (tfgridnet_causal.py:540-588; oracle/restate.py::sep_block) ------------------
+# Shapes: NF = 97 bins, CH = 64 channels, NHEAD = 4 heads, QE = 6 (Q/K features per bin and head), VD = 16 (V), a
+# window of ATT = 50 frames.  Q/K rows are QK_DIM = 582 = 97*6 values (element f*6 + e), stored QK_LD = 584 wide; V rows
+# are V_DIM = 1552 = 97*16 values (f*16 + c).  The mutated references (keyword flags) restate the plausible mistakes a
+# kernel could make; the tests show that each one is far outside the bound the kernels meet.
+NF, CH, NHEAD, QE, VD, ATT, RING = 97, 64, 4, 6, 16, 50, 56
+QK_DIM, QK_LD, V_DIM, FC, NQKV = NF * QE, 584, NF * VD, NF * CH, 2 * 4 * 6 + 4 * 16
+
+
+def prelu64(x, a):
+    return torch.where(x >= 0, x, a * x)
+
+
+def qkv_proj64(X, wqkv_t, bqkv, slopes, swap_qk_slopes=False):
+    """Linear 64 -> 112 + bias + PReLU (slope slopes[0] on the Q columns 0..23, [1] on K 24..47, [2] on V 48..111) of
+    X [..., 97, 64] -> [..., 97, 112] (tfgridnet_causal.py:354-387: attn_conv_Q/K/V, layers .0 and .1)"""
+    s = slopes.double()
+    sq, sk = (s[1], s[0]) if swap_qk_slopes else (s[0], s[1])
+    a = torch.cat([sq.expand(24), sk.expand(24), s[2].expand(64)])
+    return prelu64(X.double() @ wqkv_t.double() + bqkv.double(), a)
+
+
+def qkv_ln64(P, lnq, lnk, lnv, unbiased=False, heads_transposed=False):
+    """head split + LayerNorm over (F, E) per (Q/K/V, head) of projections P [N, 97, 112] -> Q, K [N, 4, 582] and
+    V [N, 4, 1552].  Head h of Q owns columns h*6 + e, element i = f*6 + e (K: 24 + h*6 + e; V: 48 + h*16 + c).
+    lnq / lnk / lnv: (gain, bias), of at least 582 / 1552 values.  heads_transposed: column e*4 + h (a mutant)."""
+    N = P.shape[0]
+    out = []
+    for d, c0, (g, b) in ((QE, 0, lnq), (QE, 24, lnk), (VD, 48, lnv)):
+        cols = P[:, :, c0:c0 + NHEAD * d].double()
+        y = cols.view(N, NF, d, NHEAD).permute(0, 3, 1, 2) if heads_transposed else cols.view(N, NF, NHEAD, d).permute(0, 2, 1, 3)
+        n = NF * d
+        out.append(layer_norm64(y.reshape(N, NHEAD, n), g[:n], b[:n], unbiased=unbiased))
+    return tuple(out)
+
+
+def window_mask(qframes, kframes, lo=-(ATT - 1), hi=0, mask_before_start=False):
+    """[T, n] bool: query frame qframes[t] attends to key frame kframes[j] iff qframes[t] + lo <= kframes[j] <=
+    qframes[t] + hi -- the model's window is the 50 frames ending at the query's (lo = -49, hi = 0).  Frames before the
+    stream start are zero rows that TAKE PART in the softmax (the reference's zero-initialised K_buf / V_buf);
+    mask_before_start=True leaves them out instead (a mutant)."""
+    q = torch.as_tensor(qframes, dtype=torch.int64)[:, None]
+    k = torch.as_tensor(kframes, dtype=torch.int64)[None, :]
+    w = (k >= q + lo) & (k <= q + hi)
+    return w & (k >= 0) if mask_before_start else w
+
+
+def attention64(q, K, V, window, scale=1.0 / QK_DIM ** 0.5):
+    """softmax(q . k * scale) V over each query's window: q [T, H, >=582], K [n, H, >=582] and V [n, H, 1552] the rows
+    of n frames, window [T, n] (window_mask) -> [T, H, 1552]"""
+    s = torch.einsum("thd,nhd->htn", q[..., :QK_DIM].double(), K[..., :QK_DIM].double()) * scale
+    s = s.masked_fill(~window[None], float("-inf"))
+    return torch.einsum("htn,nhd->thd", torch.softmax(s, dim=-1), V.double())
+
+
+def merge_heads64(o, transposed=False):
+    """head outputs o [N, 4, 1552] (feature f*16 + c) -> Z [N, 97, 64] with channel h*16 + c of bin f
+    (tfgridnet_causal.py:575-581); transposed: channel c*4 + h (a mutant)"""
+    N = o.shape[0]
+    z = o.double().view(N, NHEAD, NF, VD).permute(0, 2, 1, 3)          # [N, 97, 4, 16]
+    if transposed:
+        z = z.transpose(2, 3)
+    return z.reshape(N, NF, CH)
+
+
+def ln_frame_res64(P, X, g, b, gate=None, per_bin=False, gate_first=False, unbiased=False):
+    """X + LayerNorm over the frame's 6208 values (f, c) of P [N, 97, 64], times the speaker gate [N, 97, 64] if given
+    (tfgridnet_causal.py:583-588, :250-251).  Mutants: per_bin (LayerNorm over each bin's 64 values), gate_first
+    (X * gate + LN), unbiased (variance over n - 1)."""
+    N = P.shape[0]
+    if per_bin:
+        y = layer_norm64(P, g.view(NF, CH), b.view(NF, CH), unbiased=unbiased)
+    else:
+        y = layer_norm64(P.reshape(N, FC), g, b, unbiased=unbiased).view(N, NF, CH)
+    x = X.double()
+    if gate is None:
+        return x + y
+    gate = gate.double().view(N, NF, CH)
+    return x * gate + y if gate_first else (x + y) * gate
+
+
+def attn_out64(Z, X, wp_t, bp, slope, g, b, gate=None, **mutant):
+    """Linear 64 -> 64 + bias + PReLU (slopes[3]) of Z [N, 97, 64], then ln_frame_res64"""
+    return ln_frame_res64(prelu64(Z.double() @ wp_t.double() + bp.double(), float(slope)), X, g, b, gate, **mutant)
+
+
+class Ring:
+    """Where the kernels keep a stream's K/V history (sep_layout.h): frame n of head h lives in slot n mod RING of the
+    block's K ring (and V ring), at ST_BLK + blk*BK_STRIDE + BK_K (BK_V) + (h*RING + slot) * row floats of the stream's
+    record.  The attention window of frame n is frames n-49 .. n; the other RING - ATT slots ("spare": frames n-55 ..
+    n-50) hold rows that later hops of the pipelined graph may already have overwritten."""
+
+    def __init__(self, lay):
+        self.lay = lay
+        assert lay["RING"] == RING and lay["ATT"] == ATT and lay["QK_LD"] == QK_LD and lay["V_DIM"] == V_DIM
+
+    @staticmethod
+    def slot(n):
+        return n % RING                                  # Python's % is non-negative: frame -1 -> slot 55
+
+    def row(self, blk, which, h, n):
+        """offset (floats) of frame n's row of head h inside a stream record; which = 'k' or 'v'"""
+        base = self.lay["ST_BLK"] + blk * self.lay["BK_STRIDE"]
+        if which == "k":
+            return base + self.lay["BK_K"] + (h * RING + self.slot(n)) * QK_LD
+        return base + self.lay["BK_V"] + (h * RING + self.slot(n)) * V_DIM
+
+    @staticmethod
+    def window(n, lo=-(ATT - 1), hi=0):
+        return list(range(n + lo, n + hi + 1))
+
+    @staticmethod
+    def spare(n):
+        return list(range(n - RING + 1, n - ATT + 1))
 
 
 def lstm_ref(gx, whh, nseq, L, ndir, row_of, h0=None, c0=None):

@@ -1,13 +1,16 @@
-// Test-only C entry points into the engine's tensor-core GEMM (umma::launch) and LSTM recurrences (lstm.cuh,
-// tc_lstm.cuh), so that tests/test_umma_gemm_gpu.py and tests/test_lstm_kernels_gpu.py can drive each kernel directly
-// with arbitrary shapes and compare it element by element with a float64 reference.
+// Test-only C entry points into the engine's tensor-core GEMM (umma::launch), LSTM recurrences (lstm.cuh,
+// tc_lstm.cuh) and the separator's attention section (sep_kernels.cuh), so that tests/test_umma_gemm_gpu.py,
+// tests/test_lstm_kernels_gpu.py and tests/test_attention_kernels_gpu.py can drive each kernel directly with arbitrary
+// shapes and compare it element by element with a float64 reference.
 //
 // The argument structs below are plain C (mirrored with ctypes in the tests); every function fills the engine's own
-// descriptor and calls the engine's own launcher.  Built by lookoncetohear_b200/build.py as lib/libl2h_kernel_harness.so
-// with hidden visibility, so this library's copy of the l2h symbols never binds to the product library's copy.
+// descriptor and calls the engine's own launcher (or launches the kernel with the engine's own geometry).  Built by
+// lookoncetohear_b200/build.py as lib/libl2h_kernel_harness.so with hidden visibility, so this library's copy of the
+// l2h symbols never binds to the product library's copy.
 #include <cstdio>
 #include "umma_gemm.cu"
 #include "tc_lstm.cuh"
+#include "sep_kernels.cuh"
 
 #define KH_API extern "C" __attribute__((visibility("default")))
 
@@ -199,4 +202,122 @@ KH_API int kh_lstm(const KhLstm* k, int variant, int passes, char* why, int why_
     }
     if (e != cudaSuccess) put_why(why, why_len, cudaGetErrorString(e));
     return (int)e;
+}
+
+// ---- the separator's attention section (sep_kernels.cuh) -------------------------------------------------------------
+// The fields of BlockWeights that qkv_kernel, qkv_many_kernel, attn_out_kernel and ln_frame_res_kernel read.  The four
+// Q/K LayerNorm vectors are read as QK_LD (584) floats: 582 values and 2 floats of padding.
+struct KhSepWeights {
+    const float *wqkv_t, *bqkv, *slopes;
+    const float *lnq_g, *lnq_b, *lnk_g, *lnk_b, *lnv_g, *lnv_b;
+    const float *wp_t, *bp, *lnp_g, *lnp_b;
+};
+
+enum KhAttnForm { KH_ATTN_QUERY = 0, KH_ATTN_TILE = 1, KH_ATTN_CLUSTER = 2 };   // attn_kernel, attn_tile_kernel, attn_cluster_kernel
+
+static BlockWeights to_block(const KhSepWeights& k) {
+    BlockWeights w{};
+    w.wqkv_t = k.wqkv_t; w.bqkv = k.bqkv; w.slopes = k.slopes;
+    w.lnq_g = k.lnq_g; w.lnq_b = k.lnq_b; w.lnk_g = k.lnk_g; w.lnk_b = k.lnk_b; w.lnv_g = k.lnv_g; w.lnv_b = k.lnv_b;
+    w.wp_t = k.wp_t; w.bp = k.bp; w.lnp_g = k.lnp_g; w.lnp_b = k.lnp_b;
+    return w;
+}
+
+KH_API int kh_sizeof_sep_weights() { return (int)sizeof(KhSepWeights); }
+
+// RING, QK_LD, QK_DIM, V_DIM, ATT, ST_GATE, ST_BLK, BK_K, BK_V, BK_H, BK_C, BK_STRIDE, ST_POS, ST_CALLS,
+// sizeof(StateHeader), stream_stride(n_blocks); returns the count written (16)
+KH_API int kh_sep_layout(int n_blocks, int64_t* out) {
+    const int64_t v[] = {RING, QK_LD, QK_DIM, V_DIM, ATT, ST_GATE, ST_BLK, BK_K, BK_V, BK_H, BK_C, BK_STRIDE, ST_POS, ST_CALLS,
+                         (int64_t)sizeof(StateHeader), stream_stride(n_blocks)};
+    const int n = (int)(sizeof(v) / sizeof(v[0]));
+    for (int i = 0; i < n; ++i) out[i] = v[i];
+    return n;
+}
+
+// dynamic shared memory of the section's kernels, set once per device (as the engine's set_attrs does)
+static cudaError_t configure_sep() {
+    static thread_local int configured_dev = -1;
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess || configured_dev == dev) return e;
+    e = cudaFuncSetAttribute(qkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)QKV_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(qkv_many_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)QKV_MANY_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(attn_out_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AOUT_SMEM);
+    if (e == cudaSuccess) configured_dev = dev;
+    return e;
+}
+
+// CTAs of attn_cluster_kernel the current device holds at once: the engine splits a call's windows over 8-CTA
+// clusters while B * T * NHEAD * ATT_CL fits in this (attn_splits)
+KH_API int kh_attn_cluster_resident() {
+    static int wave[64] = {};
+    return resident_ctas(wave, attn_cluster_kernel, 256, 0);
+}
+
+// qkv_kernel: grid (T, B).  pre == nullptr: the Linear 64 -> 112 (+ bias + PReLU) runs inside, from X [B][T][97][64];
+// otherwise pre holds the projections [B][T][97][112].
+KH_API int kh_qkv(const KhSepWeights* w, const float* X, const float* pre, float* Q, float* Kall, float* Vall, float* state,
+                  int64_t sstride, int blk, int B, int T, int frame_k, const uint8_t* active, void* stream) {
+    if (B <= 0 || T <= 0 || frame_k < 0) return (int)cudaErrorInvalidValue;
+    cudaError_t e = configure_sep();
+    if (e != cudaSuccess) return (int)e;
+    return (int)launch_k(false, qkv_kernel, dim3(T, B), dim3(QKV_THREADS), QKV_SMEM, static_cast<cudaStream_t>(stream), X, pre,
+                         Q, Kall, Vall, state, sstride, blk, to_block(*w), T, frame_k, active);
+}
+
+// qkv_many_kernel over frames 0 .. n_frames-1 (frame fi = stream fi / T, row fi % T) with `grid` persistent CTAs
+KH_API int kh_qkv_many(const KhSepWeights* w, const float* pre, float* Q, float* Kall, float* Vall, float* state,
+                       int64_t sstride, int blk, int T, int grid, int n_frames, const uint8_t* active, void* stream) {
+    if (T <= 0 || grid <= 0 || n_frames <= 0) return (int)cudaErrorInvalidValue;
+    cudaError_t e = configure_sep();
+    if (e != cudaSuccess) return (int)e;
+    return (int)launch_k(false, qkv_many_kernel, dim3(grid), dim3(QKV_THREADS), QKV_MANY_SMEM, static_cast<cudaStream_t>(stream),
+                         pre, Q, Kall, Vall, state, sstride, blk, to_block(*w), T, n_frames, active);
+}
+
+// kv_gather_kernel: grid (ATT - 1, B * NHEAD), 128 threads
+KH_API int kh_kv_gather(const float* state, int64_t sstride, int blk, float* Kall, float* Vall, int B, int T, void* stream) {
+    if (B <= 0 || T <= 1) return (int)cudaErrorInvalidValue;
+    return (int)launch_k(false, kv_gather_kernel, dim3(ATT - 1, B * NHEAD), dim3(128), 0, static_cast<cudaStream_t>(stream),
+                         state, sstride, blk, Kall, Vall, T);
+}
+
+// One attention form: T == 1 reads the ring (window of frame clock + frame_k), T > 1 the linear scratch.  The tile form
+// reads the scratch only; the engine never launches it with T == 1, and it has no frame_k.
+KH_API int kh_attention(int form, const float* Q, const float* Kall, const float* Vall, const float* state, int64_t sstride,
+                        int blk, float* Z, int B, int T, int frame_k, void* stream) {
+    if (B <= 0 || T <= 0 || frame_k < 0 || (T > 1 && frame_k != 0)) return (int)cudaErrorInvalidValue;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    switch (form) {
+        case KH_ATTN_QUERY:
+            return (int)launch_k(false, attn_kernel, dim3(T, NHEAD, B), dim3(256), 0, st, Q, Kall, Vall, state, sstride, blk, Z, T,
+                                 frame_k);
+        case KH_ATTN_TILE:
+            if (T == 1) return (int)cudaErrorInvalidValue;
+            return (int)launch_k(false, attn_tile_kernel, dim3((T + ATT_TQ - 1) / ATT_TQ, NHEAD, B), dim3(256), 0, st, Q, Kall,
+                                 Vall, Z, T);
+        case KH_ATTN_CLUSTER:
+            return (int)launch_cluster(false, dim3(1, ATT_CL, 1), attn_cluster_kernel, dim3(T, NHEAD * ATT_CL, B), dim3(256), 0,
+                                       st, Q, Kall, Vall, state, sstride, blk, Z, T, frame_k);
+        default: return (int)cudaErrorInvalidValue;
+    }
+}
+
+// attn_out_kernel: grid (T, B); X [B][T][97][64] updated in place; the gate is ST_GATE of each stream's record
+KH_API int kh_attn_out(const KhSepWeights* w, const float* Z, float* X, const float* state, int64_t sstride, int B, int T,
+                       int apply_gate, void* stream) {
+    if (B <= 0 || T <= 0) return (int)cudaErrorInvalidValue;
+    cudaError_t e = configure_sep();
+    if (e != cudaSuccess) return (int)e;
+    return (int)launch_k(false, attn_out_kernel, dim3(T, B), dim3(256), AOUT_SMEM, static_cast<cudaStream_t>(stream), Z, X,
+                         state, sstride, to_block(*w), apply_gate, T);
+}
+
+// ln_frame_res_kernel: grid (T, B); P [B][T][97][64] = the projection after PReLU
+KH_API int kh_ln_frame_res(const KhSepWeights* w, const float* P, float* X, const float* state, int64_t sstride, int B, int T,
+                           int apply_gate, void* stream) {
+    if (B <= 0 || T <= 0) return (int)cudaErrorInvalidValue;
+    return (int)launch_k(false, ln_frame_res_kernel, dim3(T, B), dim3(256), 0, static_cast<cudaStream_t>(stream), P, X, state,
+                         sstride, to_block(*w), apply_gate, T);
 }

@@ -1,6 +1,7 @@
 """The kernel harness library (tests/kernels/) and the float64 references the kernel-level GPU tests
-(test_umma_gemm_gpu.py, test_lstm_kernels_gpu.py) rely on.  No device needed."""
+(test_umma_gemm_gpu.py, test_lstm_kernels_gpu.py, test_attention_kernels_gpu.py) rely on.  No device needed."""
 import ctypes
+import math
 
 import torch
 
@@ -121,3 +122,107 @@ def test_split_product_passes():
     err = {p: float(((kh.split_product(a, b, p) - exact).abs() / P).max()) for p in (1, 2, 3)}
     assert err[3] <= 3 * 2.0 ** -17 and err[2] <= 2.0 ** -8 and err[1] <= 2.0 ** -7
     assert err[3] < err[2] / 20 and err[2] < err[1]
+
+
+# ---- the attention section ------------------------------------------------------------------------------------------
+def test_sep_layout_matches_the_product_library(tsh_params):
+    """the harness's state layout (kh_sep_layout) is the one the product library reports, so the state buffers the
+    attention tests build are the engine's"""
+    from lookoncetohear_b200 import Net, build, _cabi
+    build.build()
+    net = Net(**tsh_params)
+    h, L = net._engine(), _cabi.lib()
+    offs = (ctypes.c_int64 * 18)()
+    assert L.l2h_sep_state_offsets(h, offs, 18) == 0
+    hb, stride = ctypes.c_int64(), ctypes.c_int64()
+    assert L.l2h_sep_state_layout(h, ctypes.byref(hb), ctypes.byref(stride)) == 0
+    one = kh.sep_layout(1)
+    n_blocks = (stride.value - one["ST_BLK"]) // one["BK_STRIDE"]
+    names = {"RING": 0, "QK_LD": 1, "QK_DIM": 2, "V_DIM": 3, "ATT": 4, "ST_GATE": 6, "ST_BLK": 10, "BK_K": 11, "BK_V": 12,
+             "BK_H": 13, "BK_C": 14, "BK_STRIDE": 15, "ST_POS": 16, "ST_CALLS": 17}
+    want = {n: offs[i] for n, i in names.items()}
+    want.update(HEADER_BYTES=hb.value, STREAM_STRIDE=stride.value)
+    assert kh.sep_layout(n_blocks) == want
+    assert (kh.RING, kh.QK_LD, kh.QK_DIM, kh.V_DIM, kh.ATT) == tuple(offs[:5])
+
+
+def test_ring_model():
+    """frame n in slot n mod 56; a window and its 6 spare slots cover the ring once, also across the wrap, for
+    negative frames and above 2^31; rows are laid out head by head, K ring then V ring, block by block"""
+    lay = kh.sep_layout(2)
+    ring = kh.Ring(lay)
+    for n in (0, 1, 48, 49, 50, 55, 56, 57, 111, 2 ** 31 + 7):
+        w, sp = ring.window(n), ring.spare(n)
+        assert len(w) == kh.ATT and w[-1] == n and len(sp) == kh.RING - kh.ATT and sp[-1] == n - kh.ATT
+        assert sorted(ring.slot(m) for m in w + sp) == list(range(kh.RING))
+    assert ring.slot(-1) == 55 and ring.slot(56) == 0 and ring.slot(2 ** 31 + 7) == 23
+    blk1 = lay["ST_BLK"] + lay["BK_STRIDE"]
+    assert ring.row(1, "k", 0, 0) == blk1 + lay["BK_K"]
+    assert ring.row(1, "k", 1, 57) == blk1 + lay["BK_K"] + (kh.RING + 1) * kh.QK_LD
+    assert ring.row(1, "k", 3, 55) + kh.QK_LD == blk1 + lay["BK_V"]
+    assert ring.row(1, "v", 3, -1) + kh.V_DIM == blk1 + lay["BK_H"]
+    assert ring.row(0, "v", 2, 2 ** 31 + 7) == lay["ST_BLK"] + lay["BK_V"] + (2 * kh.RING + 23) * kh.V_DIM
+
+
+def test_window_attention_is_the_reference_loop():
+    """attention64 over window_mask equals the model's loop (oracle/restate.py::sep_block): Kall = [K_buf (49 zero rows
+    of a fresh stream) ; k], query t attends to rows t .. t+49"""
+    torch.manual_seed(3)
+    T, H = 7, 2
+    q = torch.randn(T, H, kh.QK_DIM, dtype=torch.float64)
+    k = torch.randn(T, H, kh.QK_DIM, dtype=torch.float64)
+    v = torch.randn(T, H, kh.V_DIM, dtype=torch.float64)
+    Kall = torch.cat([torch.zeros(kh.ATT - 1, H, kh.QK_DIM, dtype=torch.float64), k])
+    Vall = torch.cat([torch.zeros(kh.ATT - 1, H, kh.V_DIM, dtype=torch.float64), v])
+    want = torch.stack([torch.einsum("hj,jhd->hd", torch.softmax(
+        torch.einsum("hd,jhd->hj", q[t], Kall[t:t + kh.ATT]) / math.sqrt(kh.QK_DIM), -1), Vall[t:t + kh.ATT])
+        for t in range(T)])
+    frames = list(range(-(kh.ATT - 1), T))
+    got = kh.attention64(q, Kall, Vall, kh.window_mask(list(range(T)), frames))
+    assert torch.allclose(got, want, rtol=0, atol=1e-12)
+
+
+def test_mutated_references_differ():
+    """each mutated reference the attention tests use moves a small case (scores ~ N(0, 1)) by more than 10x the
+    kernels' bounds at such scores (<= 2e-5), so the sensitivity checks cannot pass vacuously"""
+    g = torch.Generator().manual_seed(5)
+    N = 3
+    X = torch.randn(N, kh.NF, kh.CH, generator=g)
+    w = (torch.rand(64, kh.NQKV, generator=g) * 2 - 1) * 0.25
+    bias = 0.1 * torch.randn(kh.NQKV, generator=g)
+    slopes = torch.tensor([0.25, -0.1, 0.05, 0.2])
+    ln = [(1 + 0.2 * torch.randn(n, generator=g), 0.2 * torch.randn(n, generator=g)) for n in (kh.QK_DIM, kh.QK_DIM, kh.V_DIM)]
+    P = kh.qkv_proj64(X, w, bias, slopes)
+    ref = kh.qkv_ln64(P, *ln)
+    assert [tuple(t.shape) for t in ref] == [(N, 4, kh.QK_DIM), (N, 4, kh.QK_DIM), (N, 4, kh.V_DIM)]
+    for mut in (kh.qkv_ln64(P, *ln, unbiased=True), kh.qkv_ln64(P, *ln, heads_transposed=True),
+                kh.qkv_ln64(kh.qkv_proj64(X, w, bias, slopes, swap_qk_slopes=True), *ln)):
+        assert max(float((a - b).abs().max()) for a, b in zip(mut, ref)) > 1e-3
+    # attention: frames -3 .. 60 of one stream (zero rows before 0), queries at frames 1 and 55
+    n = 64
+    kf = list(range(-3, n - 3))
+    K = torch.randn(n, 4, kh.QK_LD, generator=g, dtype=torch.float64)
+    V = torch.randn(n, 4, kh.V_DIM, generator=g, dtype=torch.float64)
+    K[:3], V[:3] = 0, 0
+    q = torch.randn(2, 4, kh.QK_LD, generator=g, dtype=torch.float64)
+    qf = [1, 55]
+    ref = kh.merge_heads64(kh.attention64(q, K, V, kh.window_mask(qf, kf)))
+    muts = [kh.attention64(q, K, V, kh.window_mask(qf, kf, -kh.ATT, -1)),
+            kh.attention64(q, K, V, kh.window_mask(qf, kf, -(kh.ATT - 2))),
+            kh.attention64(q, K, V, kh.window_mask(qf, kf, -kh.ATT)),
+            kh.attention64(q, K, V, kh.window_mask(qf, kf, mask_before_start=True)),
+            kh.attention64(q, K, V, kh.window_mask(qf, kf), scale=1 / math.sqrt(kh.QK_LD))]
+    for m in muts:
+        assert float((kh.merge_heads64(m) - ref).abs().max()) > 1e-3
+    o = kh.attention64(q, K, V, kh.window_mask(qf, kf))
+    assert float((kh.merge_heads64(o, transposed=True) - ref).abs().max()) > 1e-3
+    # the head merge: channel h*16 + c of bin f is feature f*16 + c of head h
+    assert torch.equal(ref[1, 5, 2 * 16 + 3], o[1, 2, 5 * 16 + 3])
+    # attention output: LayerNorm over the frame's 6208 values, then the gate
+    Pp = torch.randn(N, kh.NF, kh.CH, generator=g)
+    Xr = torch.randn(N, kh.NF, kh.CH, generator=g)
+    gate = 1 + 0.5 * torch.randn(N, kh.NF, kh.CH, generator=g)
+    lg, lb = 1 + 0.2 * torch.randn(kh.FC, generator=g), 0.2 * torch.randn(kh.FC, generator=g)
+    ref = kh.ln_frame_res64(Pp, Xr, lg, lb, gate)
+    for mut in (dict(per_bin=True), dict(gate_first=True), dict(unbiased=True)):
+        assert float((kh.ln_frame_res64(Pp, Xr, lg, lb, gate, **mut) - ref).abs().max()) > 3e-4, mut
