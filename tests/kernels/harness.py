@@ -10,6 +10,7 @@ with a = the activation (GEMM: the A row; recurrence: h or LN(x)) and b = the we
 bf16 weights times split activations.
 """
 import ctypes
+import math
 
 import torch
 
@@ -64,15 +65,22 @@ class SepWeights(ctypes.Structure):
                                                 "wp_t", "bp", "lnp_g", "lnp_b")]
 
 
+class SepFrontBack(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_void_p) for n in ("wat", "ws", "wc", "bc", "we", "be", "lne_g", "lne_b", "wd", "bd")] + \
+               [("gen", ctypes.c_int32)] + [(n, ctypes.c_void_p) for n in ("ln1_g", "ln1_b", "wih1_t", "b1")]
+
+
 MIRRORS = {"kh_sizeof_asource": ASource, "kh_sizeof_gemm": Gemm, "kh_sizeof_plan": Plan, "kh_sizeof_lstm": Lstm,
-           "kh_sizeof_sep_weights": SepWeights}
+           "kh_sizeof_sep_weights": SepWeights, "kh_sizeof_sep_front_back": SepFrontBack}
 SYMBOLS = ("kh_gemm", "kh_gemm_plan", "kh_split_planes", "kh_lstm", "kh_launch_count", "kh_sep_layout", "kh_qkv",
            "kh_qkv_many", "kh_kv_gather", "kh_attention", "kh_attn_out", "kh_ln_frame_res",
-           "kh_attn_cluster_resident") + tuple(MIRRORS)
+           "kh_attn_cluster_resident", "kh_front", "kh_front_many", "kh_front_many_geometry", "kh_front1", "kh_back",
+           "kh_back_many", "kh_back_many_geometry") + tuple(MIRRORS)
 
 ATTN_FORMS = {"query": 0, "tile": 1, "cluster": 2}
 SEP_LAYOUT_NAMES = ("RING", "QK_LD", "QK_DIM", "V_DIM", "ATT", "ST_GATE", "ST_BLK", "BK_K", "BK_V", "BK_H", "BK_C",
-                    "BK_STRIDE", "ST_POS", "ST_CALLS", "HEADER_BYTES", "STREAM_STRIDE")
+                    "BK_STRIDE", "ST_POS", "ST_CALLS", "HEADER_BYTES", "STREAM_STRIDE", "ST_EMB", "ST_GEN", "ST_CONV",
+                    "ST_DECONV", "ST_ISTFT")
 
 _lib = None
 
@@ -105,6 +113,17 @@ def lib():
             "kh_attn_out": [W, P, P, P, I64, I, I, I, P],
             "kh_ln_frame_res": [W, P, P, P, I64, I, I, I, P],
         }
+        FB, IP = ctypes.POINTER(SepFrontBack), ctypes.POINTER(ctypes.c_int)
+        sigs.update({
+            "kh_front": [FB, P, I64, I64, I, P, P, I64, I, I, I, P, P, I, I, P, P],
+            "kh_front_many": [FB, P, I64, I64, I, P, P, I64, I, I, I, P, P, I, I, P, P],
+            "kh_front1": [FB, P, I64, I64, I, P, P, P, I64, I, I, P, P, P, P],
+            "kh_back": [FB, P, P, I64, I64, I, P, I64, I, I, I, I, I, I64, P, P],
+            "kh_back_many": [FB, P, P, I64, I64, I, P, I64, I, I, I, I, I, P, P],
+        })
+        for s in ("kh_front_many_geometry", "kh_back_many_geometry"):
+            getattr(L, s).restype = None
+            getattr(L, s).argtypes = [I, I, IP, IP]
         for s, args in sigs.items():
             getattr(L, s).restype = ctypes.c_int
             getattr(L, s).argtypes = args
@@ -171,6 +190,46 @@ def attn_out(w, Z, X, state, sstride, B, T, apply_gate):
 
 def ln_frame_res(w, P, X, state, sstride, B, T, apply_gate):
     return lib().kh_ln_frame_res(ctypes.byref(w), ptr(P), ptr(X), ptr(state), sstride, B, T, apply_gate, stream())
+
+
+# x, y: [B][2][n] (any strides along the first two dimensions); x_len / y_len count samples of the last dimension
+def front(w, x, x_len, X, state, sstride, B, T, pos_rel, emb, spk_pre, frame_k=0, frames_total=1, active=None):
+    return lib().kh_front(ctypes.byref(w), ptr(x), x.stride(0), x.stride(1), x_len, ptr(X), ptr(state), sstride, B, T, pos_rel,
+                          ptr(emb), ptr(spk_pre), frame_k, frames_total, ptr(active), stream())
+
+
+def front_many_geometry(B, T):
+    """(chunk, n_workers) the engine launches front_many_kernel with"""
+    c, n = ctypes.c_int(), ctypes.c_int()
+    lib().kh_front_many_geometry(B, T, ctypes.byref(c), ctypes.byref(n))
+    return c.value, n.value
+
+
+def front_many(w, x, x_len, X, state, sstride, B, T, pos_rel, emb, spk_pre, chunk, n_workers, active=None):
+    return lib().kh_front_many(ctypes.byref(w), ptr(x), x.stride(0), x.stride(1), x_len, ptr(X), ptr(state), sstride, B, T,
+                               pos_rel, ptr(emb), ptr(spk_pre), chunk, n_workers, ptr(active), stream())
+
+
+def front1(w, x, x_len, X, GX, state, sstride, B, pos_rel, emb, spk_pre, active=None):
+    return lib().kh_front1(ctypes.byref(w), ptr(x), x.stride(0), x.stride(1), x_len, ptr(X), ptr(GX), ptr(state), sstride, B,
+                           pos_rel, ptr(emb), ptr(spk_pre), ptr(active), stream())
+
+
+def back(w, X, y, y_len, state, sstride, B, T, pos_rel, frame_k=0, frames_total=1, hist_stride=0, active=None):
+    return lib().kh_back(ctypes.byref(w), ptr(X), ptr(y), y.stride(0), y.stride(1), y_len, ptr(state), sstride, B, T, pos_rel,
+                         frame_k, frames_total, hist_stride, ptr(active), stream())
+
+
+def back_many_geometry(B, T):
+    """(chunk, n_cl) the engine launches back_many_kernel with"""
+    c, n = ctypes.c_int(), ctypes.c_int()
+    lib().kh_back_many_geometry(B, T, ctypes.byref(c), ctypes.byref(n))
+    return c.value, n.value
+
+
+def back_many(w, X, y, y_len, state, sstride, B, T, pos_rel, chunk, n_cl, active=None):
+    return lib().kh_back_many(ctypes.byref(w), ptr(X), ptr(y), y.stride(0), y.stride(1), y_len, ptr(state), sstride, B, T,
+                              pos_rel, chunk, n_cl, ptr(active), stream())
 
 
 # ---- float64 references ---------------------------------------------------------------------------------------------
@@ -345,3 +404,167 @@ def lstm_ref(gx, whh, nseq, L, ndir, row_of, h0=None, c0=None):
 def packed_from_torch(w):
     """torch.nn.LSTM gate rows (q*64 + j) -> the packed rows of lstm.cuh (j*4 + q)."""
     return w.view(4, 64, *w.shape[1:]).transpose(0, 1).reshape(w.shape)
+
+
+# ---- the separator's front and back (tfgridnet_causal.py:229-273; oracle/restate.py::sep_core) -----------------------
+# One stream at a time.  Frame t of a call covers samples s0 + 128 t .. + 191 (128 new samples and the 64-sample
+# look-ahead); the spectrum has channels [Re m0, Re m1, Im m0, Im m1] and bins f = 0..96; the conv reads the two frames
+# before the call from the conv tail [2][4][97] and zero-pads in F; the transposed conv reads the deconv tail [2][97][64];
+# the synthesis of frame t-1 comes from the iSTFT tail [2 ears][194].  Each reference returns, next to every value, an
+# element-wise bound on the fp32 rounding error of a kernel that computes it: u sqrt(n) sum |terms| for each sum of n
+# terms (with the bounds of its inputs carried through), u = 2^-24.  The mutant flags restate plausible kernel mistakes.
+HOP, NFFT, LOOKAHEAD, NROW, SPK = 128, 192, 64, 194, 256
+U32 = 2.0 ** -24
+# A LayerNorm's own rounding, relative to a normalised value: the variance is a block sum of <= 25 sequential terms per
+# thread and an 8-level tree (<= 33 roundings of positive terms, 17 u on its square root), rsqrtf adds <= 2 ulp (4 u)
+# and the final multiply-add 3 roundings: at most this many u (the 64-value LayerNorms of front1_kernel round less)
+LN_U = 24
+
+
+def frames64(x, x_len, s0, T):
+    """[2, T, 192] float64: frame t of mic m = x[m, s0 + 128 t + n], zero outside [0, x_len) (x [2][>= x_len])"""
+    idx = s0 + HOP * torch.arange(T)[:, None] + torch.arange(NFFT)[None, :]
+    ok = (idx >= 0) & (idx < x_len)
+    out = torch.zeros(x.shape[0], T, NFFT, dtype=torch.float64)
+    out[:, ok] = x[:, idx[ok]].double()
+    return out
+
+
+def _pad_f(u, clamp=False):
+    """[..., 97, ...] with F on dim -2 (X-like) -> zero-padded (or edge-clamped: a mutant) to 99 bins"""
+    lo, hi = (u[..., :1, :], u[..., -1:, :]) if clamp else (torch.zeros_like(u[..., :1, :]),) * 2
+    return torch.cat([lo, u, hi], dim=-2)
+
+
+def front64(x, x_len, s0, T, conv_tail, Wa, Wc, bc, shift=0, reim_interleaved=False, conv_flip_time=False,
+            edge_clamp=False):
+    """STFT analysis, channel regroup and the causal 3x3 conv of one stream (tfgridnet_causal.py:229-242).
+    x [2][n] (fp32), conv_tail [2][4][97] (frames -2, -1), Wa [194][192] analysis filters, Wc [64][4][3][3], bc [64].
+    Returns X [T][97][64], the new conv tail [2][4][97] (spectra of the call's last two frames) and their bounds.
+    Mutants: shift (frames one hop late), reim_interleaved (channels [Re m0, Im m0, Re m1, Im m1]), conv_flip_time
+    (kernel rows i -> 2 - i), edge_clamp (bins -1 and 97 copy bins 0 and 96)."""
+    fr = frames64(x, x_len, s0 + HOP * shift, T)
+    Wa = Wa.double()
+    S, Sa = fr @ Wa.T, fr.abs() @ Wa.abs().T                              # [2, T, 194]
+    order = [0, 2, 1, 3] if reim_interleaved else [0, 1, 2, 3]              # channel ri*2 + m (mutant: m*2 + ri)
+
+    def regroup(s):
+        u = torch.stack([s[0, :, :NF], s[1, :, :NF], s[0, :, NF:], s[1, :, NF:]], dim=1)   # [T, 4, 97]
+        return u[:, order]
+    tail = conv_tail.double()
+    Up = torch.cat([tail, regroup(S)])                                      # [T + 2, 4, 97]
+    Ua = torch.cat([tail.abs(), regroup(Sa)])
+    Ue = torch.cat([torch.zeros_like(tail), regroup(Sa) * (U32 * math.sqrt(NFFT))])     # bound of each spectrum value
+    W = Wc.double()
+    if conv_flip_time:
+        W = W.flip(2)
+    X = torch.zeros(T, NF, CH, dtype=torch.float64) + bc.double()
+    Xa = torch.zeros_like(X) + bc.double().abs()
+    Xe = torch.zeros_like(X)
+    pads = [_pad_f(u.transpose(1, 2), edge_clamp) for u in (Up, Ua, Ue)]  # [T + 2, 99, 4]
+    for i in range(3):
+        for j in range(3):
+            w = W[:, :, i, j]
+            X = X + pads[0][i:i + T, j:j + NF] @ w.T
+            Xa = Xa + pads[1][i:i + T, j:j + NF] @ w.abs().T
+            Xe = Xe + pads[2][i:i + T, j:j + NF] @ w.abs().T
+    return dict(X=X, X_bound=Xe + U32 * math.sqrt(37) * Xa, tail=Up[-2:], tail_bound=Ue[-2:])
+
+
+def gate64(e, We, be, g, b, cf_order=False, unbiased=False):
+    """speaker gate LN_6208(We e + be) (tfgridnet_causal.py:247-248), element c*97 + f stored at [f][c] -> ([97][64],
+    bound).  Mutants: cf_order (element i stored at flat i), unbiased (variance over 6207)."""
+    # each row is a 256-term dot product whose longest rounding chain is 8 products per lane, a 5-level warp tree and
+    # the bias: 16 roundings; an error pe in p moves y by |g| (pe + mean pe) / sigma, and |g xh| mean pe / sigma more
+    # through sigma
+    p = We.double() @ e.double() + be.double()
+    pe = U32 * math.sqrt(16) * (We.double().abs() @ e.double().abs() + be.double().abs())
+    y = layer_norm64(p, g, b, unbiased=unbiased)
+    sd = p.std(unbiased=False)
+    gx = (g.double() * (p - p.mean()) / sd).abs()
+    bound = (g.double().abs() * (pe + pe.mean()) + gx * pe.mean()) / sd + U32 * (LN_U * gx + 2 * b.double().abs())
+    if cf_order:
+        return y.view(NF, CH), bound.view(NF, CH)
+    return y.view(CH, NF).T, bound.view(CH, NF).T
+
+
+
+def ih64(X, g, b, wih_t, bias):
+    """block 0's intra input projection LN_64(X) W_ih^T + b of X [97][64] -> ([97][512], bound); wih_t [64][512] and
+    bias [512] in the packed column order d*256 + j*4 + q of lstm.cuh"""
+    xn = layer_norm64(X, g, b)
+    xh = (X.double() - X.double().mean(-1, keepdim=True)) / X.double().std(-1, unbiased=False, keepdim=True)
+    W = wih_t.double()
+    out = xn @ W + bias.double()
+    bound = U32 * (math.sqrt(65) * (xn.abs() @ W.abs() + bias.double().abs()) + LN_U * ((g.double() * xh).abs() @ W.abs()))
+    return out, bound
+
+
+def back64(X, deconv_tail, istft_tail, Wd, bd, Ws, plain_conv=False, swap_ear_ri=False, ola="model", carry_istft=True):
+    """causal 3x3 transposed conv, Re/Im regroup, synthesis and overlap-add of one stream (tfgridnet_causal.py:256-273,
+    net.py:61).  X [T][97][64], deconv_tail [2][97][64] (frames -2, -1), istft_tail [2 ears][194] (frame -1), Wd
+    [64][4][3][3] (c, o, i, j), bd [4], Ws [194][192] synthesis filters.  D[o,t,f] = bd[o] + sum Wd[c,o,i,j]
+    Xp[c,t+2-i,f+1-j]; channel o = 2 ear + ri; output sample 128 t + n = w_t[n] (+ w_{t-1}[128 + n] for n < 64).
+    Returns y [2][128 T], the new deconv tail [2][97][64], the new iSTFT tail [2][194] and bounds.
+    Mutants: plain_conv (kernel flipped in both axes), swap_ear_ri (o = 2 ri + ear), ola = "dropped" (no tail added) or
+    "wrong_half" (w_{t-1}[n] added), carry_istft=False (frame -1 synthesised from zeros)."""
+    T = X.shape[0]
+    Xp = torch.cat([deconv_tail.double(), X.double()])                     # [T + 2, 97, 64]
+    Xpp, Xpa = _pad_f(Xp), _pad_f(Xp.abs())                                # [T + 2, 99, 64]
+    W = Wd.double()
+    if plain_conv:
+        W = W.flip(2, 3)
+    D = torch.zeros(4, T, NF, dtype=torch.float64) + bd.double()[:, None, None]
+    Da = torch.zeros_like(D) + bd.double().abs()[:, None, None]
+    for i in range(3):
+        for j in range(3):
+            D = D + torch.einsum("tfc,co->otf", Xpp[2 - i:2 - i + T, 2 - j:2 - j + NF], W[:, :, i, j])
+            Da = Da + torch.einsum("tfc,co->otf", Xpa[2 - i:2 - i + T, 2 - j:2 - j + NF], W[:, :, i, j].abs())
+    De = U32 * math.sqrt(4 * 9 * 64) * Da
+
+    def regroup(d):                                                        # [4, T, 97] -> [2 ears, T, 194]
+        pairs = [(0, 2), (1, 3)] if swap_ear_ri else [(0, 1), (2, 3)]
+        return torch.stack([torch.cat([d[a], d[c]], dim=-1) for a, c in pairs])
+    R, Ra, Re = regroup(D), regroup(D.abs()), regroup(De)
+    tail = istft_tail.double() if carry_istft else torch.zeros(2, NROW, dtype=torch.float64)
+    Rp = torch.cat([tail[:, None], R], dim=1)                              # [2, T + 1, 194]
+    Rpa = torch.cat([istft_tail.double().abs()[:, None], Ra], dim=1)
+    Rpe = torch.cat([torch.zeros(2, 1, NROW, dtype=torch.float64), Re], dim=1)
+    Wsd = Ws.double()
+    w = Rp @ Wsd                                                           # [2, T + 1, 192]
+    wa = Rpa @ Wsd.abs()
+    we = Rpe @ Wsd.abs()
+
+    def ola_(v, mode):
+        head = v[:, 1:, :HOP].clone()
+        if mode == "model":
+            head[..., :LOOKAHEAD] += v[:, :-1, HOP:]
+        elif mode == "wrong_half":
+            head[..., :LOOKAHEAD] += v[:, :-1, :LOOKAHEAD]
+        return head.reshape(2, T * HOP)
+    bound = ola_(we, "model") + U32 * math.sqrt(NROW + 2 * 4) * ola_(wa, "model")
+    return dict(y=ola_(w, ola), y_bound=bound, deconv_tail=Xp[-2:], istft_tail=R[:, -1], istft_bound=Re[:, -1])
+
+
+def pack_front_back(sd, pad=float("nan"), prefix="tfgridnet."):
+    """the front / back weights of a state dict in the kernels' layouts (SepWeights): wat [192][196] (the analysis
+    filters transposed, 2 pad columns = pad), ws [194][192], wc [64][36], wd [64][4][9], we [6208][256], be, and the
+    gate LayerNorm's lne_g / lne_b in c*97 + f order (the model's own)"""
+    g = lambda k: sd[prefix + k].detach().float()
+    wa = g("enc.filterbank._filters")[:, 0]
+    wat = torch.full((NFFT, NROW + 2), pad, dtype=torch.float32)
+    wat[:, :NROW] = wa.T
+    return dict(wat=wat, ws=g("dec.filterbank._filters")[:, 0].contiguous(), wc=g("conv.0.weight").reshape(CH, 36),
+                bc=g("conv.0.bias"), we=g("embed_to_feats_proj.0.weight"), be=g("embed_to_feats_proj.0.bias"),
+                lne_g=g("embed_to_feats_proj.1.weight"), lne_b=g("embed_to_feats_proj.1.bias"),
+                wd=g("deconv.weight").reshape(CH, 4, 9), bd=g("deconv.bias"))
+
+
+def unpack_front_back(p, prefix="tfgridnet."):
+    """pack_front_back's inverse: the state-dict tensors"""
+    return {prefix + "enc.filterbank._filters": p["wat"][:, :NROW].T.reshape(NROW, 1, NFFT),
+            prefix + "dec.filterbank._filters": p["ws"].reshape(NROW, 1, NFFT),
+            prefix + "conv.0.weight": p["wc"].reshape(CH, 4, 3, 3), prefix + "conv.0.bias": p["bc"],
+            prefix + "embed_to_feats_proj.0.weight": p["we"], prefix + "embed_to_feats_proj.0.bias": p["be"],
+            prefix + "embed_to_feats_proj.1.weight": p["lne_g"], prefix + "embed_to_feats_proj.1.bias": p["lne_b"],
+            prefix + "deconv.weight": p["wd"].reshape(CH, 4, 3, 3), prefix + "deconv.bias": p["bd"]}

@@ -1,7 +1,8 @@
 // Test-only C entry points into the engine's tensor-core GEMM (umma::launch), LSTM recurrences (lstm.cuh,
-// tc_lstm.cuh) and the separator's attention section (sep_kernels.cuh), so that tests/test_umma_gemm_gpu.py,
-// tests/test_lstm_kernels_gpu.py and tests/test_attention_kernels_gpu.py can drive each kernel directly with arbitrary
-// shapes and compare it element by element with a float64 reference.
+// tc_lstm.cuh), the separator's attention section (sep_kernels.cuh) and its front and back (sep_kernels.cuh,
+// hop_kernels.cuh), so that tests/test_umma_gemm_gpu.py, tests/test_lstm_kernels_gpu.py,
+// tests/test_attention_kernels_gpu.py and tests/test_front_back_kernels_gpu.py can drive each kernel directly with
+// arbitrary shapes and compare it element by element with a float64 reference.
 //
 // The argument structs below are plain C (mirrored with ctypes in the tests); every function fills the engine's own
 // descriptor and calls the engine's own launcher (or launches the kernel with the engine's own geometry).  Built by
@@ -11,6 +12,7 @@
 #include "umma_gemm.cu"
 #include "tc_lstm.cuh"
 #include "sep_kernels.cuh"
+#include "hop_kernels.cuh"
 
 #define KH_API extern "C" __attribute__((visibility("default")))
 
@@ -226,16 +228,16 @@ static BlockWeights to_block(const KhSepWeights& k) {
 KH_API int kh_sizeof_sep_weights() { return (int)sizeof(KhSepWeights); }
 
 // RING, QK_LD, QK_DIM, V_DIM, ATT, ST_GATE, ST_BLK, BK_K, BK_V, BK_H, BK_C, BK_STRIDE, ST_POS, ST_CALLS,
-// sizeof(StateHeader), stream_stride(n_blocks); returns the count written (16)
+// sizeof(StateHeader), stream_stride(n_blocks), ST_EMB, ST_GEN, ST_CONV, ST_DECONV, ST_ISTFT; returns the count written (21)
 KH_API int kh_sep_layout(int n_blocks, int64_t* out) {
     const int64_t v[] = {RING, QK_LD, QK_DIM, V_DIM, ATT, ST_GATE, ST_BLK, BK_K, BK_V, BK_H, BK_C, BK_STRIDE, ST_POS, ST_CALLS,
-                         (int64_t)sizeof(StateHeader), stream_stride(n_blocks)};
+                         (int64_t)sizeof(StateHeader), stream_stride(n_blocks), ST_EMB, ST_GEN, ST_CONV, ST_DECONV, ST_ISTFT};
     const int n = (int)(sizeof(v) / sizeof(v[0]));
     for (int i = 0; i < n; ++i) out[i] = v[i];
     return n;
 }
 
-// dynamic shared memory of the section's kernels, set once per device (as the engine's set_attrs does)
+// dynamic shared memory of the separator kernels launched here, set once per device (as the engine's set_attrs does)
 static cudaError_t configure_sep() {
     static thread_local int configured_dev = -1;
     int dev = 0;
@@ -244,6 +246,11 @@ static cudaError_t configure_sep() {
     e = cudaFuncSetAttribute(qkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)QKV_SMEM);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(qkv_many_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)QKV_MANY_SMEM);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(attn_out_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AOUT_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(front_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FRONT_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(front_many_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FRONT_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(front1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FRONT1_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(back_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BACK_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(back_many_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BACK_MANY_SMEM);
     if (e == cudaSuccess) configured_dev = dev;
     return e;
 }
@@ -320,4 +327,111 @@ KH_API int kh_ln_frame_res(const KhSepWeights* w, const float* P, float* X, cons
     if (B <= 0 || T <= 0) return (int)cudaErrorInvalidValue;
     return (int)launch_k(false, ln_frame_res_kernel, dim3(T, B), dim3(256), 0, static_cast<cudaStream_t>(stream), P, X, state,
                          sstride, to_block(*w), apply_gate, T);
+}
+
+// ---- the separator's front and back (sep_kernels.cuh, hop_kernels.cuh) ----------------------------------------------
+// The SepWeights fields, and for front1_kernel the block-0 fields of its input projection.
+struct KhSepFrontBack {
+    const float *wat, *ws, *wc, *bc, *we, *be, *lne_g, *lne_b, *wd, *bd;
+    int32_t gen;
+    const float *ln1_g, *ln1_b, *wih1_t, *b1;
+};
+
+static SepWeights to_sep(const KhSepFrontBack& k) {
+    SepWeights w{};
+    w.wat = k.wat; w.ws = k.ws; w.wc = k.wc; w.bc = k.bc; w.we = k.we; w.be = k.be; w.lne_g = k.lne_g; w.lne_b = k.lne_b;
+    w.wd = k.wd; w.bd = k.bd; w.gen = k.gen;
+    return w;
+}
+
+KH_API int kh_sizeof_sep_front_back() { return (int)sizeof(KhSepFrontBack); }
+
+// front_kernel.  frames_total <= 1: an ordinary call of T frames, grid (T + 1, B).  frames_total > 1: hop frame_k of a
+// group of frames_total one-frame calls of the pipelined graph (T must be 1): grid (frame_k == 0 ? 2 : 1, B), samples
+// from offset frame_k * 128 -- only hop 0 carries the speaker-gate CTA.
+KH_API int kh_front(const KhSepFrontBack* w, const float* x, int64_t x_bstride, int64_t x_cstride, int x_len, float* X,
+                    float* state, int64_t sstride, int B, int T, int pos_rel, const float* emb, float* spk_pre, int frame_k,
+                    int frames_total, const uint8_t* active, void* stream) {
+    const bool group = frames_total > 1;
+    if (B <= 0 || T <= 0 || (group && (T != 1 || frame_k < 0 || frame_k >= frames_total)) || (!group && frame_k != 0))
+        return (int)cudaErrorInvalidValue;
+    cudaError_t e = configure_sep();
+    if (e != cudaSuccess) return (int)e;
+    const dim3 grid(group ? (frame_k == 0 ? 2 : 1) : T + 1, B);
+    return (int)launch_k(false, front_kernel, grid, dim3(256), FRONT_SMEM, static_cast<cudaStream_t>(stream), x, x_bstride,
+                         x_cstride, x_len, X, state, sstride, to_sep(*w), T, pos_rel, emb, spk_pre, group ? frame_k : 0,
+                         group ? frames_total : 1, group ? frame_k * HOP : 0, active);
+}
+
+// the engine's front_many_kernel geometry for (B, T) (sep_engine.cu, the many-frame branch of the front)
+KH_API void kh_front_many_geometry(int B, int T, int* chunk, int* n_workers) {
+    const int per_stream = std::max(1, NUM_SMS / B);
+    *chunk = (T + per_stream - 1) / per_stream;
+    const int n_chunks = (T + *chunk - 1) / *chunk;
+    *n_workers = std::min(NUM_SMS, B * n_chunks);
+}
+
+// front_many_kernel: n_workers CTAs walk the (stream, chunk-of-`chunk`-frames) items, then one speaker-gate CTA per stream
+KH_API int kh_front_many(const KhSepFrontBack* w, const float* x, int64_t x_bstride, int64_t x_cstride, int x_len, float* X,
+                         float* state, int64_t sstride, int B, int T, int pos_rel, const float* emb, float* spk_pre, int chunk,
+                         int n_workers, const uint8_t* active, void* stream) {
+    if (B <= 0 || T <= 0 || chunk <= 0 || n_workers <= 0) return (int)cudaErrorInvalidValue;
+    cudaError_t e = configure_sep();
+    if (e != cudaSuccess) return (int)e;
+    const int n_chunks = (T + chunk - 1) / chunk;
+    return (int)launch_k(false, front_many_kernel, dim3(n_workers + B, 1), dim3(256), FRONT_SMEM, static_cast<cudaStream_t>(stream),
+                         x, x_bstride, x_cstride, x_len, X, state, sstride, to_sep(*w), T, pos_rel, emb, spk_pre, chunk, n_chunks,
+                         B, n_workers, active);
+}
+
+// front1_kernel: one frame as 13 tiles of 8 bins plus the speaker-gate CTA, grid (14, B); GX [B][97][512]
+KH_API int kh_front1(const KhSepFrontBack* w, const float* x, int64_t x_bstride, int64_t x_cstride, int x_len, float* X,
+                     float* GX, float* state, int64_t sstride, int B, int pos_rel, const float* emb, float* spk_pre,
+                     const uint8_t* active, void* stream) {
+    if (B <= 0) return (int)cudaErrorInvalidValue;
+    cudaError_t e = configure_sep();
+    if (e != cudaSuccess) return (int)e;
+    BlockWeights w0{};
+    w0.ln1_g = w->ln1_g; w0.ln1_b = w->ln1_b; w0.wih1_t = w->wih1_t; w0.b1 = w->b1;
+    return (int)launch_k(false, front1_kernel, dim3(TAIL_TILES + 1, B), dim3(256), FRONT1_SMEM, static_cast<cudaStream_t>(stream),
+                         x, x_bstride, x_cstride, x_len, X, state, sstride, to_sep(*w), w0, GX, pos_rel, emb, spk_pre, active);
+}
+
+// back_kernel in clusters of BACK_CL.  frames_total <= 1: an ordinary call of T frames, grid (4 T, B); it advances the
+// clocks.  frames_total > 1: hop frame_k of a pipelined group (T must be 1), grid (4, B), samples from offset
+// frame_k * 128, X = this hop's rows with the previous hops' hist_stride floats apart; it advances no clock.
+KH_API int kh_back(const KhSepFrontBack* w, const float* X, float* y, int64_t y_bstride, int64_t y_cstride, int y_len,
+                   float* state, int64_t sstride, int B, int T, int pos_rel, int frame_k, int frames_total, int64_t hist_stride,
+                   const uint8_t* active, void* stream) {
+    const bool group = frames_total > 1;
+    if (B <= 0 || T <= 0 || (group && (T != 1 || frame_k < 0 || frame_k >= frames_total)) || (!group && frame_k != 0))
+        return (int)cudaErrorInvalidValue;
+    cudaError_t e = configure_sep();
+    if (e != cudaSuccess) return (int)e;
+    return (int)launch_cluster(false, dim3(BACK_CL, 1, 1), back_kernel, dim3(BACK_CL * T, B), dim3(256), BACK_SMEM,
+                               static_cast<cudaStream_t>(stream), X, y, y_bstride, y_cstride, y_len, state, sstride, to_sep(*w), T,
+                               pos_rel, group ? frame_k : 0, group ? frames_total : 1, group ? frame_k * HOP : 0,
+                               group ? hist_stride : (int64_t)0, active);
+}
+
+// the engine's back_many_kernel geometry for (B, T) (sep_engine.cu, the many-frame branch of the back)
+KH_API void kh_back_many_geometry(int B, int T, int* chunk, int* n_cl) {
+    const int max_cl = NUM_SMS * 3 / BACK_CL;
+    const int per_stream = std::max(1, max_cl / B);
+    *chunk = (T + per_stream - 1) / per_stream;
+    const int n_chunks = (T + *chunk - 1) / *chunk;
+    *n_cl = std::min(max_cl, B * n_chunks);
+}
+
+// back_many_kernel: n_cl clusters of BACK_CL walk the (stream, chunk-of-`chunk`-frames) items; it advances the clocks
+KH_API int kh_back_many(const KhSepFrontBack* w, const float* X, float* y, int64_t y_bstride, int64_t y_cstride, int y_len,
+                        float* state, int64_t sstride, int B, int T, int pos_rel, int chunk, int n_cl, const uint8_t* active,
+                        void* stream) {
+    if (B <= 0 || T <= 0 || chunk <= 0 || n_cl <= 0) return (int)cudaErrorInvalidValue;
+    cudaError_t e = configure_sep();
+    if (e != cudaSuccess) return (int)e;
+    const int n_chunks = (T + chunk - 1) / chunk;
+    return (int)launch_cluster(false, dim3(BACK_CL, 1, 1), back_many_kernel, dim3(BACK_CL * n_cl, 1), dim3(256), BACK_MANY_SMEM,
+                               static_cast<cudaStream_t>(stream), X, y, y_bstride, y_cstride, y_len, state, sstride, to_sep(*w), T,
+                               pos_rel, chunk, n_chunks, B, active);
 }

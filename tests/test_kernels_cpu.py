@@ -1,5 +1,6 @@
 """The kernel harness library (tests/kernels/) and the float64 references the kernel-level GPU tests
-(test_umma_gemm_gpu.py, test_lstm_kernels_gpu.py, test_attention_kernels_gpu.py) rely on.  No device needed."""
+(test_umma_gemm_gpu.py, test_lstm_kernels_gpu.py, test_attention_kernels_gpu.py, test_front_back_kernels_gpu.py) rely on.
+No device needed."""
 import ctypes
 import math
 
@@ -127,7 +128,7 @@ def test_split_product_passes():
 # ---- the attention section ------------------------------------------------------------------------------------------
 def test_sep_layout_matches_the_product_library(tsh_params):
     """the harness's state layout (kh_sep_layout) is the one the product library reports, so the state buffers the
-    attention tests build are the engine's"""
+    attention, front and back tests build are the engine's"""
     from lookoncetohear_b200 import Net, build, _cabi
     build.build()
     net = Net(**tsh_params)
@@ -138,10 +139,12 @@ def test_sep_layout_matches_the_product_library(tsh_params):
     assert L.l2h_sep_state_layout(h, ctypes.byref(hb), ctypes.byref(stride)) == 0
     one = kh.sep_layout(1)
     n_blocks = (stride.value - one["ST_BLK"]) // one["BK_STRIDE"]
-    names = {"RING": 0, "QK_LD": 1, "QK_DIM": 2, "V_DIM": 3, "ATT": 4, "ST_GATE": 6, "ST_BLK": 10, "BK_K": 11, "BK_V": 12,
-             "BK_H": 13, "BK_C": 14, "BK_STRIDE": 15, "ST_POS": 16, "ST_CALLS": 17}
+    names = {"RING": 0, "QK_LD": 1, "QK_DIM": 2, "V_DIM": 3, "ATT": 4, "ST_EMB": 5, "ST_GATE": 6, "ST_CONV": 7,
+             "ST_DECONV": 8, "ST_ISTFT": 9, "ST_BLK": 10, "BK_K": 11, "BK_V": 12, "BK_H": 13, "BK_C": 14, "BK_STRIDE": 15,
+             "ST_POS": 16, "ST_CALLS": 17}
     want = {n: offs[i] for n, i in names.items()}
-    want.update(HEADER_BYTES=hb.value, STREAM_STRIDE=stride.value)
+    # the weight generation of the gate memo is the word before the stream's call count
+    want.update(HEADER_BYTES=hb.value, STREAM_STRIDE=stride.value, ST_GEN=offs[17] - 1)
     assert kh.sep_layout(n_blocks) == want
     assert (kh.RING, kh.QK_LD, kh.QK_DIM, kh.V_DIM, kh.ATT) == tuple(offs[:5])
 
@@ -226,3 +229,107 @@ def test_mutated_references_differ():
     ref = kh.ln_frame_res64(Pp, Xr, lg, lb, gate)
     for mut in (dict(per_bin=True), dict(gate_first=True), dict(unbiased=True)):
         assert float((kh.ln_frame_res64(Pp, Xr, lg, lb, gate, **mut) - ref).abs().max()) > 3e-4, mut
+
+
+# ---- the front and the back -----------------------------------------------------------------------------------------
+def _net_sd(tsh_params, seed=0):
+    from lookoncetohear_b200 import Net
+    torch.manual_seed(seed)
+    return Net(**tsh_params).state_dict()
+
+
+def _fb(sd64):
+    g = lambda k: sd64["tfgridnet." + k]
+    return dict(Wa=g("enc.filterbank._filters")[:, 0], Wc=g("conv.0.weight"), bc=g("conv.0.bias"),
+                Wd=g("deconv.weight"), bd=g("deconv.bias"), Ws=g("dec.filterbank._filters")[:, 0],
+                We=g("embed_to_feats_proj.0.weight"), be=g("embed_to_feats_proj.0.bias"),
+                lg=g("embed_to_feats_proj.1.weight"), lb=g("embed_to_feats_proj.1.bias"))
+
+
+def test_front_and_back_references_are_the_model(tsh_params):
+    """over three consecutive calls of 1, 2 and 5 frames of one stream, front64 and back64 (fed the tails of the model's
+    state, in the kernels' layouts) reproduce oracle/restate.py::sep_core: the encoder output taps["enc"], the new
+    conv / deconv / iSTFT tails, and the 128 T samples of the output before the look-ahead; gate64 is taps["gate"]"""
+    from oracle import restate
+    sd = _net_sd(tsh_params)
+    sd["tfgridnet.embed_to_feats_proj.1.weight"] = 1 + 0.3 * torch.randn(kh.FC)
+    sd["tfgridnet.embed_to_feats_proj.1.bias"] = 0.3 * torch.randn(kh.FC)
+    sd64 = restate.cast_sd(sd, torch.float64)
+    w = _fb(sd64)
+    g = torch.Generator().manual_seed(7)
+    x = torch.randn(2, kh.HOP * 8 + kh.LOOKAHEAD, generator=g, dtype=torch.float64)
+    emb = torch.randn(kh.SPK, generator=g, dtype=torch.float64)
+    state = restate.sep_init_state(sd64, 1, dtype=torch.float64)
+    pos = 0
+    for T in (1, 2, 5):
+        conv_tail = state["conv_buf"][0].permute(1, 0, 2)                 # [4][2][97] -> [2 frames][4][97]
+        deconv_tail = state["deconv_buf"][0].permute(1, 2, 0)             # [64][2][97] -> [2][97][64]
+        istft_tail = state["istft_buf"][0, :, :, 0]                       # [2 ears][194]
+        end = kh.HOP * (pos + T) + kh.LOOKAHEAD
+        taps = {}
+        y, state = restate.sep_core(sd64, x[None, :, kh.HOP * pos:end], emb[None], state, taps=taps)
+        f = kh.front64(x, end, kh.HOP * pos, T, conv_tail, w["Wa"], w["Wc"], w["bc"])
+        assert torch.allclose(f["X"], taps["enc"][0], rtol=0, atol=1e-12)
+        assert torch.allclose(f["tail"], state["conv_buf"][0].permute(1, 0, 2), rtol=0, atol=1e-12)
+        b = kh.back64(taps["block2"][0], deconv_tail, istft_tail, w["Wd"], w["bd"], w["Ws"])
+        assert torch.allclose(b["y"], y[0, :, :kh.HOP * T], rtol=0, atol=1e-12)
+        assert torch.equal(b["deconv_tail"], state["deconv_buf"][0].permute(1, 2, 0))
+        assert torch.allclose(b["istft_tail"], state["istft_buf"][0, :, :, 0], rtol=0, atol=1e-12)
+        gate, _ = kh.gate64(emb, w["We"], w["be"], w["lg"], w["lb"])
+        assert torch.allclose(gate, taps["gate"][0, 0], rtol=0, atol=1e-12)
+        pos += T
+
+
+def test_front_and_back_mutants_differ(tsh_params):
+    """every mutated reference the front / back tests use moves a small case far from the reference (by more than 1 %
+    of the largest value): the kernels' bounds are ~1e-5 of it, so the >= 10x margins cannot pass vacuously.  The
+    gate's unbiased variance moves a value by |LN| / 12416 only: more than 12x gate64's own bound somewhere."""
+    from oracle import restate
+    w = _fb(restate.cast_sd(_net_sd(tsh_params), torch.float64))
+    g = torch.Generator().manual_seed(8)
+    T = 3
+    x = torch.randn(2, 2000, generator=g, dtype=torch.float64)
+    ct, ct2 = torch.randn(2, 2, 4, kh.NF, generator=g, dtype=torch.float64)
+    dt, dt2 = torch.randn(2, 2, kh.NF, kh.CH, generator=g, dtype=torch.float64)
+    it, it2 = torch.randn(2, 2, kh.NROW, generator=g, dtype=torch.float64)
+    X = torch.randn(T, kh.NF, kh.CH, generator=g, dtype=torch.float64)
+    front = lambda s0=300, tail=ct, **m: kh.front64(x, 1900, s0, T, tail, w["Wa"], w["Wc"], w["bc"], **m)
+    ref = front()
+    for m in (dict(shift=1), dict(reim_interleaved=True), dict(conv_flip_time=True), dict(edge_clamp=True),
+              dict(tail=ct2), dict(s0=300 + kh.HOP * 5)):
+        mut = front(**m)
+        d = max(float((mut[k] - ref[k]).abs().max()) for k in ("X", "tail"))
+        assert d > 1e-2 * float(ref["X"].abs().max()), m
+    # the edge clamp changes bins 0 and 96 only
+    mut = front(edge_clamp=True)
+    assert torch.equal(mut["X"][:, 1:-1], ref["X"][:, 1:-1])
+    back = lambda d=dt, i=it, **m: kh.back64(X, d, i, w["Wd"], w["bd"], w["Ws"], **m)
+    ref = back()
+    for m in (dict(plain_conv=True), dict(swap_ear_ri=True), dict(ola="dropped"), dict(ola="wrong_half"),
+              dict(carry_istft=False), dict(d=dt2), dict(i=it2)):
+        mut = back(**m)
+        d = max(float((mut[k] - ref[k]).abs().max()) for k in ("y", "istft_tail"))
+        assert d > 1e-2 * float(ref["y"].abs().max()), m
+    # the overlap-add mutants change the first 64 samples of each frame only
+    assert torch.equal(back(ola="dropped")["y"].view(2, T, kh.HOP)[..., kh.LOOKAHEAD:], ref["y"].view(2, T, kh.HOP)[..., kh.LOOKAHEAD:])
+    e = torch.randn(kh.SPK, generator=g, dtype=torch.float64)
+    lg, lb = 1 + 0.3 * torch.randn(kh.FC, generator=g), 0.3 * torch.randn(kh.FC, generator=g)
+    ref, bound = kh.gate64(e, w["We"], w["be"], lg, lb)
+    for m in (dict(cf_order=True), dict(unbiased=True)):
+        mut, _ = kh.gate64(e, w["We"], w["be"], lg, lb, **m)
+        assert float(((mut - ref).abs() / bound).max()) > 12, m
+
+
+def test_front_back_packing_round_trips(tsh_params):
+    """pack_front_back gives the kernels' layouts; unpacked again they are the state-dict tensors bit for bit, and the
+    two pad columns of the transposed analysis filters hold the pad value"""
+    sd = _net_sd(tsh_params)
+    p = kh.pack_front_back(sd)
+    shapes = dict(wat=(192, 196), ws=(194, 192), wc=(64, 36), bc=(64,), we=(kh.FC, 256), be=(kh.FC,), lne_g=(kh.FC,),
+                  lne_b=(kh.FC,), wd=(64, 4, 9), bd=(4,))
+    assert {k: tuple(v.shape) for k, v in p.items()} == shapes
+    assert bool(p["wat"][:, 194:].isnan().all()) and not bool(p["wat"][:, :194].isnan().any())
+    for k, v in kh.unpack_front_back(p).items():
+        assert torch.equal(v, sd[k]), k
+    assert torch.equal(p["wat"][5, 100], sd["tfgridnet.enc.filterbank._filters"][100, 0, 5])
+    assert torch.equal(p["wd"][7, 3, 2 * 3 + 1], sd["tfgridnet.deconv.weight"][7, 3, 2, 1])
