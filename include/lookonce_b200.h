@@ -12,6 +12,8 @@
  *   l2h_sep_forward
  *        <- Net.predict / Net.forward           net.py:54-76  -> TFGridNet.forward
  *                                               tfgridnet_causal.py:188-283
+ *   l2h_sep_forward_active / l2h_sep_forward_slots
+ *        <- one Net.predict hop for some of a state's streams (serving many listeners: INTEGRATION.md)
  *   l2h_sep_stream_host
  *        <- the chunk loop around Net.predict(chunk, embed, state, pad=False)  (SURVEY.md 3.3)
  *           with host buffers: H2D of each chunk and D2H of each result inside the call
@@ -138,6 +140,20 @@ int l2h_sep_forward_active(void* handle, const float* x_dev, int64_t x_batch_str
                            int64_t y_batch_stride, int64_t y_ch_stride, int32_t y_len, int32_t batch,
                            int32_t frames, void* workspace_dev, size_t workspace_bytes, uint32_t flags,
                            void* stream, const uint8_t* active_dev);
+/* A one-hop call over a chosen list of a state's records, so a hop costs what its n listed streams need, not what the
+ * state's capacity needs.  Call row i reads x / emb row i, writes y row i and advances record slots_dev[i] of a state of
+ * state_batch records.  The work, the kernel form and the workspace (l2h_sep_workspace_bytes(handle, n, 1, flags)) are
+ * those of a dense call of n streams.  Records not listed are neither read nor written (rings, h / c, tails, gate memo,
+ * clock); the header advances as for any call, and so do the clocks of the listed records.
+ *   slots_dev  [n] int32 of DEVICE memory read when the kernels run: with L2H_FLAG_GRAPH a caller rewrites the list in place
+ *              before every hop and replays the same cached graph (its key holds n, not the list's contents).  An entry
+ *              outside [0, state_batch) marks a row that is computed but stores nothing (no record, no y row): a stream
+ *              skipping this hop.  A slot listed twice is a caller error the call does not detect.
+ * Errors 1, before anything is enqueued: null pointers, n <= 0, n > state_batch, L2H_FLAG_TAPS. */
+int l2h_sep_forward_slots(void* handle, const float* x_dev, int64_t x_batch_stride, int64_t x_ch_stride, int32_t x_len,
+                          const float* emb_dev, void* state_dev, int32_t state_batch, const int32_t* slots_dev, int32_t n,
+                          float* y_dev, int64_t y_batch_stride, int64_t y_ch_stride, int32_t y_len,
+                          void* workspace_dev, size_t workspace_bytes, uint32_t flags, void* stream);
 
 /* Streaming with HOST buffers (the end-to-end path).  Per round: H2D of the round's samples (+64
  * look-ahead) from pinned memory, the kernel chains, D2H of the new samples; one stream synchronise at

@@ -95,9 +95,10 @@ __device__ __forceinline__ void tail_col(int col, int& which, int& h, int& e, in
     h = cc / d; e = cc % d;
 }
 
+template <class Map>
 __global__ void __launch_bounds__(256)
-tail_kernel(const float* __restrict__ Y, float* X, float* __restrict__ state, int64_t sstride, int blk, BlockWeights w,
-            NextIh nx, int apply_gate, int frame_k, const uint8_t* __restrict__ active) {
+tail_kernel_t(const float* __restrict__ Y, float* X, float* __restrict__ state, Map recs, int blk, BlockWeights w,
+              NextIh nx, int apply_gate, int frame_k, const uint8_t* __restrict__ active) {
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
     extern __shared__ __align__(16) float sm[];
@@ -123,10 +124,10 @@ tail_kernel(const float* __restrict__ Y, float* X, float* __restrict__ state, in
     const int rk = (int)cluster.block_rank(), b = blockIdx.y;
     const bool has_tile = rk < TAIL_TILES;
     const int r0 = rk * MID_RT, nr = has_tile ? tail_rows(rk) : 0;
-    float* st = stream_rec(state, sstride, b);
+    float* st = stream_rec(state, recs, b);
     float* sb = st + ST_BLK + (int64_t)blk * BK_STRIDE;
     const bool has_next = nx.wih_t != nullptr;
-    const bool live = stream_active(active, b);          // false: the stream skips this hop, its record is not written
+    const bool live = stream_active(recs, active, b);          // false: the stream skips this hop, its record is not written
     if (tid == 0) {
         mbar_init(&wbar, 1); mbar_init(&pbar, 1); mbar_init(&gbar, 1);
         mbar_fence_init();
@@ -492,10 +493,11 @@ tail_kernel(const float* __restrict__ Y, float* X, float* __restrict__ state, in
 constexpr int F1_NB = MID_RT + 2;                      // bins per CTA with the conv halo
 constexpr size_t FRONT1_SMEM = (size_t)(64 * 512) * sizeof(float);
 
+template <class Map>
 __global__ void __launch_bounds__(256)
-front1_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride, int x_len, float* __restrict__ X,
-              float* __restrict__ state, int64_t sstride, SepWeights w, BlockWeights w0, float* __restrict__ GX, int pos_rel,
-              const float* __restrict__ emb, float* __restrict__ spk_pre, const uint8_t* __restrict__ active) {
+front1_kernel_t(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride, int x_len, float* __restrict__ X,
+                float* __restrict__ state, Map recs, SepWeights w, BlockWeights w0, float* __restrict__ GX, int pos_rel,
+                const float* __restrict__ emb, float* __restrict__ spk_pre, const uint8_t* __restrict__ active) {
     extern __shared__ __align__(16) float wih[];       // [64][512] block 0's W_ih^T
     __shared__ __align__(16) float xs[NMIC][NFFT];      // the frame's samples (reused as scratch by the gate CTA: >= 288 floats)
     __shared__ float U[3][4][F1_NB];                    // [frame t-2..t][ch][halo + bin], zero outside 0..96
@@ -507,7 +509,7 @@ front1_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride,
     const int p = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     if (p == TAIL_TILES) {                 // the extra CTA of this stream: speaker-gate memo
         griddep_wait();
-        spk_gate_cta(emb, spk_pre, state, sstride, w, b, &xs[0][0], active);
+        spk_gate_cta(emb, spk_pre, state, recs, w, b, &xs[0][0], active);
         return;
     }
     const int f0 = p * MID_RT, nr = tail_rows(p);
@@ -541,7 +543,7 @@ front1_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride,
     __syncthreads();
     griddep_wait();
     const StateHeader* hdr = reinterpret_cast<const StateHeader*>(state);
-    float* st = stream_rec(state, sstride, b);
+    float* st = stream_rec(state, recs, b);
     const int par = rec_par(st);
     const float* cb = st + ST_CONV + par * (2 * 4 * NF);
     float* cb_next = st + ST_CONV + (par ^ 1) * (2 * 4 * NF);
@@ -599,7 +601,7 @@ front1_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride,
         if (ok1) xr[(fq + 4) * 64 + o] = acc1;
     }
     // next conv tails = spectrogram rows of frames t-1, t (own bins)
-    if (stream_active(active, b)) {
+    if (stream_active(recs, active, b)) {
         for (int i = tid; i < 2 * 4 * nr; i += 256) {
             const int fr = i / (4 * nr), c = (i / nr) % 4, r = i % nr;
             cb_next[(fr * 4 + c) * NF + f0 + r] = U[1 + fr][c][1 + r];
@@ -610,5 +612,9 @@ front1_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride,
     mbar_wait(&gbar, 0);
     ih_rows_tile(xrows, xn, wih, gg0, gg1, gb0, gb1, gbias, GX + ((int64_t)b * NF + f0) * 512, nr, tid);
 }
+
+// the dense forms (call row b = record b); the `_t<Records>` forms serve slot-list calls (l2h_sep_forward_slots)
+constexpr auto tail_kernel = tail_kernel_t<int64_t>;
+constexpr auto front1_kernel = front1_kernel_t<int64_t>;
 
 }  // namespace l2h

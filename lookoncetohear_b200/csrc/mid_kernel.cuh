@@ -253,9 +253,10 @@ __device__ __forceinline__ void mid_tile(const MidSmem& S, const float* Yrows, c
     }
 }
 
+template <class Map>
 __global__ void __launch_bounds__(256)
-mid_kernel(const float* __restrict__ Y, float* X, float* __restrict__ QKV, float* __restrict__ state,
-           int64_t sstride, int blk, BlockWeights w, int n_streams, const uint8_t* __restrict__ active) {
+mid_kernel_t(const float* __restrict__ Y, float* X, float* __restrict__ QKV, float* __restrict__ state,
+             Map recs, int blk, BlockWeights w, int n_streams, const uint8_t* __restrict__ active) {
     extern __shared__ __align__(16) float sm[];
     const MidSmem S(sm);
     __shared__ __align__(8) unsigned long long wbar;
@@ -282,10 +283,10 @@ mid_kernel(const float* __restrict__ Y, float* X, float* __restrict__ QKV, float
         const int r0 = (item % TILES) * MID_RT;
         const int nr = min(MID_RT, NF - r0);
         __syncthreads();                    // the previous item's tiles are fully consumed
-        float* sb = stream_rec(state, sstride, b) + ST_BLK + (int64_t)blk * BK_STRIDE;
+        float* sb = stream_rec(state, recs, b) + ST_BLK + (int64_t)blk * BK_STRIDE;
         const int64_t row0 = (int64_t)b * NF + r0;
         mid_tile(S, Y + row0 * 128, X + row0 * 64, X + row0 * 64, QKV + row0 * NQKV, sb + BK_H, sb + BK_C, r0, nr, vs, tid,
-                 stream_active(active, b));
+                 stream_active(recs, active, b));
     }
 }
 
@@ -372,9 +373,10 @@ mid_a_kernel(const float* __restrict__ Y, float* __restrict__ X, float* __restri
 
 // n_hops consecutive hops per launch (GI / Hn of hop j at + j * hop_stride floats): h stays in shared memory and c in
 // registers between them, the state is read before the first and written after the last.
+template <class Map>
 __global__ void __launch_bounds__(256)
-mid_b_kernel(const float* __restrict__ GI, float* __restrict__ Hn, int64_t hop_stride, int n_hops, float* __restrict__ state,
-             int64_t sstride, int blk, BlockWeights w, int n_streams, const uint8_t* __restrict__ active) {
+mid_b_kernel_t(const float* __restrict__ GI, float* __restrict__ Hn, int64_t hop_stride, int n_hops, float* __restrict__ state,
+               Map recs, int blk, BlockWeights w, int n_streams, const uint8_t* __restrict__ active) {
     extern __shared__ __align__(16) float sm[];
     float* W3b = sm;                                  // W_hh, k-sliced
     float* A3 = W3b + (MID_W5 - MID_W3B);             // h, k-sliced
@@ -396,7 +398,7 @@ mid_b_kernel(const float* __restrict__ GI, float* __restrict__ Hn, int64_t hop_s
         const int r0 = (item % TILES) * MID_RT;
         const int nr = min(MID_RT, NF - r0);
         __syncthreads();
-        float* sb = stream_rec(state, sstride, b) + ST_BLK + (int64_t)blk * BK_STRIDE;
+        float* sb = stream_rec(state, recs, b) + ST_BLK + (int64_t)blk * BK_STRIDE;
         float* hst = sb + BK_H;
         float* cst = sb + BK_C;
         const int64_t row0 = (int64_t)b * NF + r0;
@@ -436,7 +438,7 @@ mid_b_kernel(const float* __restrict__ GI, float* __restrict__ Hn, int64_t hop_s
                 A3[mid_aidx(M3_KS, jp * 2 + 1, r)] = hh.y;
             }
         }
-        if (live && stream_active(active, b)) {
+        if (live && stream_active(recs, active, b)) {
             *reinterpret_cast<float2*>(cst + (r0 + r) * 64 + jp * 2) = cc;
             *reinterpret_cast<float2*>(hst + (r0 + r) * 64 + jp * 2) = hh;
         }
@@ -506,5 +508,9 @@ mid_c_kernel(const float* __restrict__ Hn, float* __restrict__ X, float* __restr
         }
     }
 }
+
+// the dense forms (call row b = record b); the `_t<Records>` forms serve slot-list calls (l2h_sep_forward_slots)
+constexpr auto mid_kernel = mid_kernel_t<int64_t>;
+constexpr auto mid_b_kernel = mid_b_kernel_t<int64_t>;
 
 }  // namespace l2h

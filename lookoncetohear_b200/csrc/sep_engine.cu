@@ -9,6 +9,7 @@
 #include <cstring>
 #include <map>
 #include <tuple>
+#include <type_traits>
 #include <string>
 #include <vector>
 
@@ -204,8 +205,10 @@ static void build_layout(SepEngine* e) {
 }
 
 // ---- workspace carve-up (floats) ---------------------------------------------------------------
+constexpr int64_t TC_MIN_ROWS = 2048;      // calls of more rows run their dense contractions on the tensor cores: below this
+                                           // the 16-row CUDA-core tiles win (one streaming frame = 97 rows)
 struct Workspace {
-    int64_t X, GX, Y, Z, Q, KALL, VALL, PRE, QKVRAW, TAPS, total;
+    int64_t X, GX, Y, Z, Q, KALL, VALL, PRE, QKVRAW, TAPS, HG, total;
 };
 // few frames in flight -> split every head's 50-row window over several CTAs
 static int attn_splits(int B, int T) {
@@ -229,6 +232,9 @@ static Workspace carve(int n_blocks, int B, int T, uint32_t flags) {
     ws.PRE = alloc((int64_t)B * FC);
     ws.QKVRAW = alloc(rows * NQKV);
     ws.TAPS = alloc((flags & L2H_FLAG_TAPS) ? (int64_t)(1 + 3 * n_blocks) * rows * 64 : 0);
+    // one-hop calls in the tensor-core form: the listed records' h of every block for a slot-list call (gather_h_kernel)
+    const bool tc_hop = T == 1 && rows > TC_MIN_ROWS && !(flags & L2H_FLAG_TAPS);
+    ws.HG = alloc(tc_hop ? (int64_t)n_blocks * rows * 64 : 0);
     ws.total = (cur + 511) & ~int64_t(511);      // a multiple of one GX row: pipelined hops address their slots as rows of one tensor
     return ws;
 }
@@ -265,6 +271,17 @@ static int set_attrs() {
     CK(umma::configure());
     CK(configure_tc_lstm());
     CK(cudaFuncSetAttribute(front1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FRONT1_SMEM));
+    // the slot-list forms of the kernels above (l2h_sep_forward_slots)
+    CK(cudaFuncSetAttribute(qkv_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)QKV_SMEM));
+    CK(cudaFuncSetAttribute(qkv_many_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)QKV_MANY_SMEM));
+    CK(cudaFuncSetAttribute(attn_out_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AOUT_SMEM));
+    CK(cudaFuncSetAttribute(back_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BACK_SMEM));
+    CK(cudaFuncSetAttribute(back_many_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BACK_MANY_SMEM));
+    CK(cudaFuncSetAttribute(front_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FRONT_SMEM));
+    CK(cudaFuncSetAttribute(front_many_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FRONT_SMEM));
+    CK(cudaFuncSetAttribute(mid_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_SMEM));
+    CK(cudaFuncSetAttribute(mid_b_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_B_SMEM));
+    CK(cudaFuncSetAttribute(front1_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FRONT1_SMEM));
     {   // tail_kernel: 16 CTAs per cluster is a non-portable size; ask whether this device can place it
         g_tail_clusters[dev_ord] = 0;
         if (cudaFuncSetAttribute(tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TAIL_SMEM) == cudaSuccess &&
@@ -278,6 +295,10 @@ static int set_attrs() {
             int ncl = 0;
             if (cudaOccupancyMaxActiveClusters(&ncl, tail_kernel, &cfg) == cudaSuccess) g_tail_clusters[dev_ord] = ncl;
         }
+        if (g_tail_clusters[dev_ord] > 0 &&      // the slot-list form: same resources, so the same cluster count
+            (cudaFuncSetAttribute(tail_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TAIL_SMEM) != cudaSuccess ||
+             cudaFuncSetAttribute(tail_kernel_t<Records>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess))
+            g_tail_clusters[dev_ord] = 0;
         cudaGetLastError();
     }
     g_attr_done[dev_ord] = true;
@@ -286,7 +307,6 @@ static int set_attrs() {
 
 
 // ---- dense contractions on the tensor cores (csrc/umma_gemm.cuh) for calls with many rows --------------------------
-constexpr int64_t TC_MIN_ROWS = 2048;      // below this the 16-row CUDA-core tiles win (one streaming frame = 97 rows)
 enum { PL_IH1 = 0, PL_L1, PL_IH2, PL_L2, PL_QKV, PL_CAT, PL_P, PL_PER_BLOCK };
 
 static umma::BPlanes tc_planes(const SepEngine* e, int blk, int which, int ld) {
@@ -341,9 +361,13 @@ struct ChainArgs {
     int B, T; float* wsp; size_t ws_bytes; uint32_t flags; int pos_rel;
     Profiler* prof = nullptr;
     const uint8_t* active = nullptr;     // one-hop calls: [B] device mask of the streams that advance (null: all)
+    const int32_t* slots = nullptr;      // one-hop calls: [B] device list, row b -> record slots[b] (null: row b -> record b)
+    int state_batch = 0;                 // records in the state (slot lists only)
 };
 
-static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
+// Map: the record stride (dense calls) or Records (slot-list calls), see row_record in sep_kernels.cuh
+template <class Map>
+static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Map recs) {
     const float* x = a.x; const int64_t xbs = a.xbs, xcs = a.xcs; const int x_len = a.x_len;
     const float* emb = a.emb; float* state = a.state; float* y = a.y;
     const int64_t ybs = a.ybs, ycs = a.ycs; const int y_len = a.y_len, B = a.B, T = a.T;
@@ -361,6 +385,7 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
     float* Q = wsp + ws.Q; float* KALL = wsp + ws.KALL; float* VALL = wsp + ws.VALL; float* PRE = wsp + ws.PRE;
     float* TAPS = wsp + ws.TAPS;
     float* QKVRAW = wsp + ws.QKVRAW;
+    float* HG = wsp + ws.HG;
     const int nsplit = attn_splits(B, T);
     // one-frame calls: the row-local middle of every block runs as ONE fused kernel (mid_kernel.cuh).
     // (Taps want the intermediate activations of the generic chain, so they keep it.)
@@ -389,18 +414,25 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
     e->cur_pdl = false;
 #define MARK(name) do { if (a.prof) { if (int _rc = a.prof->mark(name, st)) return _rc; } } while (0)
     MARK("start");
+    if constexpr (std::is_same_v<Map, Records>) {
+        if (tc_mid) {      // the listed records' h of every block, for the inter-step GEMMs below
+            const int64_t n4 = (int64_t)e->n_blocks * B * FC / 4;
+            CK(launch_k(false, gather_h_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, st, (const float*)state, recs,
+                        e->n_blocks, B, HG));
+        }
+    }
     if (fused_tail) {      // the frame as 13 row tiles: spectrum of the tile's bins, conv, and block 0's input projection
-        CK(launch_k(false, front1_kernel, dim3(TAIL_TILES + 1, B), dim3(256), FRONT1_SMEM, st, x, xbs, xcs, x_len, X, state, ss, e->w,
+        CK(launch_k(false, front1_kernel_t<Map>, dim3(TAIL_TILES + 1, B), dim3(256), FRONT1_SMEM, st, x, xbs, xcs, x_len, X, state, recs, e->w,
                     e->bw[0], GX, a.pos_rel, emb, PRE, active));
     } else if ((T > 1 || tc) && e->use_back_many) {      // many frames / streams: one CTA walks (stream, chunk) items (one CTA per SM: 150 KB of filters)
         const int per_stream = std::max(1, NUM_SMS / B);
         const int chunk = (T + per_stream - 1) / per_stream;
         const int n_chunks = (T + chunk - 1) / chunk;
         const int n_workers = std::min(NUM_SMS, B * n_chunks);
-        CK(launch_k(false, front_many_kernel, dim3(n_workers + B, 1), dim3(256), FRONT_SMEM, st, x, xbs, xcs, x_len, X, state, ss, e->w, T,
+        CK(launch_k(false, front_many_kernel_t<Map>, dim3(n_workers + B, 1), dim3(256), FRONT_SMEM, st, x, xbs, xcs, x_len, X, state, recs, e->w, T,
                     a.pos_rel, emb, PRE, chunk, n_chunks, B, n_workers, active));
     } else {
-        CK(launch_k(false, front_kernel, dim3(T + 1, B), dim3(256), FRONT_SMEM, st, x, xbs, xcs, x_len, X, state, ss, e->w, T,
+        CK(launch_k(false, front_kernel_t<Map>, dim3(T + 1, B), dim3(256), FRONT_SMEM, st, x, xbs, xcs, x_len, X, state, recs, e->w, T,
                     a.pos_rel, emb, PRE, 0, 1, 0, active));
     }
     MARK("front");
@@ -450,6 +482,7 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
                 q.a0.base = X; q.a0.channels = 64; q.a0.n_pos = NF; q.a0.pos_stride = 64; q.a0.n_inner = B; q.a0.inner_stride = (int64_t)NF * 64;
                 q.a1.base = sbase + ST_BLK + (int64_t)b * BK_STRIDE + BK_H;
                 q.a1.channels = 64; q.a1.n_pos = NF; q.a1.pos_stride = 64; q.a1.n_inner = B; q.a1.inner_stride = ss;
+                if (a.slots) { q.a1.base = HG + (int64_t)b * B * FC; q.a1.inner_stride = FC; }      // gathered by gather_h_kernel
                 q.n_chunks = 2;
                 q.chunks[0].c0 = 0; q.chunks[0].dp = 0; q.chunks[0].flags = 2;      // x: LayerNorm
                 q.chunks[1].c0 = 0; q.chunks[1].dp = 0; q.chunks[1].flags = 1;      // h: second source
@@ -462,7 +495,7 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
                 const cudaError_t ce = umma::launch(q, st, &why);
                 if (ce != cudaSuccess) return fail(3, std::string("umma_gemm (inter step): ") + cudaGetErrorString(ce) + " " + why);
             }
-            CK(launch_k(pdl || mp, lstm_cell_rows_kernel, dim3((unsigned)((rows * 64 + 255) / 256)), dim3(256), 0, st, (const float*)GX, state, ss, b, Y, (int)rows,
+            CK(launch_k(pdl || mp, lstm_cell_rows_kernel_t<Map>, dim3((unsigned)((rows * 64 + 255) / 256)), dim3(256), 0, st, (const float*)GX, state, recs, b, Y, (int)rows,
                       active));
             if (int rc = tc_rows_gemm(e, b, PL_L2, Y, 64, 64, 64, nullptr, nullptr, W.bl2, nullptr, X, X, 64, rows, st)) return rc;
             if (int rc = tc_rows_gemm(e, b, PL_QKV, X, 64, 64, NQKV, nullptr, nullptr, W.bqkv, W.slope_vec, nullptr, QKVRAW, NQKV, rows, st)) return rc;
@@ -471,7 +504,7 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
         } else if (row_mid && mid_split_for_throughput(B)) {
             float* GI = GX; float* HN = GX + rows * 256;         // the BiLSTM is done with GX
             CK(launch_k(pdl, mid_a_kernel, mid_grid_for(B, 2), dim3(256), MID_A_SMEM, st, (const float*)Y, X, GI, W, B, (int64_t)0, 1));
-            CK(launch_k(pdl, mid_b_kernel, mid_grid_for(B, 3), dim3(256), MID_B_SMEM, st, (const float*)GI, HN, (int64_t)0, 1, state, ss, b, W, B,
+            CK(launch_k(pdl, mid_b_kernel_t<Map>, mid_grid_for(B, 3), dim3(256), MID_B_SMEM, st, (const float*)GI, HN, (int64_t)0, 1, state, recs, b, W, B,
                         active));
             CK(launch_k(pdl, mid_c_kernel, mid_grid_for(B, 4), dim3(256), MID_C_SMEM, st, (const float*)HN, X, QKVRAW, W, B, (int64_t)0, 1));
             MARK("mid");
@@ -481,13 +514,13 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
                 const BlockWeights& Wn = e->bw[b + 1];
                 nx.ln_g = Wn.ln1_g; nx.ln_b = Wn.ln1_b; nx.wih_t = Wn.wih1_t; nx.bias = Wn.b1; nx.GX = GX;
             }
-            CK(launch_cluster(pdl, dim3(TAIL_CL, 1, 1), tail_kernel, dim3(TAIL_CL, B), dim3(256), TAIL_SMEM, st, (const float*)Y, X, state, ss,
+            CK(launch_cluster(pdl, dim3(TAIL_CL, 1, 1), tail_kernel_t<Map>, dim3(TAIL_CL, B), dim3(256), TAIL_SMEM, st, (const float*)Y, X, state, recs,
                               b, W, nx, (b == 0 && e->n_blocks > 1) ? 1 : 0, 0, active));
             MARK("tail");
             if (int rc = do_tap()) return rc;
             continue;
         } else if (row_mid) {
-            CK(launch_k(pdl, mid_kernel, mid_grid_for(B, 1), dim3(256), MID_SMEM, st, (const float*)Y, X, QKVRAW, state, ss, b, W, B, active));
+            CK(launch_k(pdl, mid_kernel_t<Map>, mid_grid_for(B, 1), dim3(256), MID_SMEM, st, (const float*)Y, X, QKVRAW, state, recs, b, W, B, active));
             MARK("mid");
         } else {
             if (tc) {
@@ -550,24 +583,24 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
         }
         if (tc && (int64_t)B * T >= NUM_SMS) {      // many frames: persistent form (LayerNorm parameters staged once per CTA), one wave
             static int wave[64] = {};
-            const int64_t grid_q = std::min<int64_t>(resident_ctas(wave, qkv_many_kernel, QKV_THREADS, QKV_MANY_SMEM), (int64_t)B * T);
-            CK(launch_k(pdl || ((e->tc_pdl & 4) != 0 && a.prof == nullptr), qkv_many_kernel, dim3((unsigned)grid_q), dim3(QKV_THREADS), QKV_MANY_SMEM, st, (const float*)QKVRAW, Q, KALL, VALL, state, ss,
+            const int64_t grid_q = std::min<int64_t>(resident_ctas(wave, qkv_many_kernel_t<Map>, QKV_THREADS, QKV_MANY_SMEM), (int64_t)B * T);
+            CK(launch_k(pdl || ((e->tc_pdl & 4) != 0 && a.prof == nullptr), qkv_many_kernel_t<Map>, dim3((unsigned)grid_q), dim3(QKV_THREADS), QKV_MANY_SMEM, st, (const float*)QKVRAW, Q, KALL, VALL, state, recs,
                         b, W, T, B * T, active));
         } else {
-            CK(launch_k(pdl, qkv_kernel, dim3(T, B), dim3(QKV_THREADS), QKV_SMEM, st, (const float*)X,
-                        (const float*)((tc || row_mid) ? QKVRAW : nullptr), Q, KALL, VALL, state, ss, b, W, T, 0, active));
+            CK(launch_k(pdl, qkv_kernel_t<Map>, dim3(T, B), dim3(QKV_THREADS), QKV_SMEM, st, (const float*)X,
+                        (const float*)((tc || row_mid) ? QKVRAW : nullptr), Q, KALL, VALL, state, recs, b, W, T, 0, active));
         }
         MARK("qkv");
         if (nsplit > 1) {
-            CK(launch_cluster(pdl, dim3(1, ATT_CL, 1), attn_cluster_kernel, dim3(T, NHEAD * ATT_CL, B), dim3(256), 0, st,
-                              (const float*)Q, (const float*)KALL, (const float*)VALL, (const float*)state, ss, b, Z, T, 0));
+            CK(launch_cluster(pdl, dim3(1, ATT_CL, 1), attn_cluster_kernel_t<Map>, dim3(T, NHEAD * ATT_CL, B), dim3(256), 0, st,
+                              (const float*)Q, (const float*)KALL, (const float*)VALL, (const float*)state, recs, b, Z, T, 0));
         } else if (T > 1 && (int64_t)B * NHEAD * ((T + ATT_TQ - 1) / ATT_TQ) >= NUM_SMS) {   // enough tiles to fill the GPU: query-tiled,
             // one pass over 57 rows serves 8 queries
             CK(launch_k(pdl, attn_tile_kernel, dim3((T + ATT_TQ - 1) / ATT_TQ, NHEAD, B), dim3(256), 0, st, (const float*)Q,
                         (const float*)KALL, (const float*)VALL, Z, T));
         } else {
-            CK(launch_k(pdl, attn_kernel, dim3(T, NHEAD, B), dim3(256), 0, st, (const float*)Q, (const float*)KALL,
-                        (const float*)VALL, (const float*)state, ss, b, Z, T, 0));
+            CK(launch_k(pdl, attn_kernel_t<Map>, dim3(T, NHEAD, B), dim3(256), 0, st, (const float*)Q, (const float*)KALL,
+                        (const float*)VALL, (const float*)state, recs, b, Z, T, 0));
         }
         MARK("attn");
         if (tc) {      // Linear(64->64) + PReLU of all rows on the tensor cores, then LayerNorm(6208) + residual (+ gate) per frame
@@ -575,10 +608,10 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
             e->cur_pdl = p2;
             if (int rc = tc_rows_gemm(e, b, PL_P, Z, 64, 64, 64, nullptr, nullptr, W.bp, nullptr, nullptr, Y, 64, rows, st, W.slopes + 3)) return rc;
             e->cur_pdl = false;
-            CK(launch_k(pdl || p2, ln_frame_res_kernel, dim3(T, B), dim3(256), 0, st, (const float*)Y, X, (const float*)state, ss, W,
+            CK(launch_k(pdl || p2, ln_frame_res_kernel_t<Map>, dim3(T, B), dim3(256), 0, st, (const float*)Y, X, (const float*)state, recs, W,
                         (b == 0 && e->n_blocks > 1) ? 1 : 0, T));
         } else {
-            CK(launch_k(pdl, attn_out_kernel, dim3(T, B), dim3(256), AOUT_SMEM, st, (const float*)Z, X, (const float*)state, ss, W,
+            CK(launch_k(pdl, attn_out_kernel_t<Map>, dim3(T, B), dim3(256), AOUT_SMEM, st, (const float*)Z, X, (const float*)state, recs, W,
                         (b == 0 && e->n_blocks > 1) ? 1 : 0, T));
         }
         MARK("attn_out");
@@ -592,15 +625,21 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
         const int chunk = (T + per_stream - 1) / per_stream;
         const int n_chunks = (T + chunk - 1) / chunk;
         const int n_cl = std::min(max_cl, B * n_chunks);
-        CK(launch_cluster(pdl, dim3(BACK_CL, 1, 1), back_many_kernel, dim3(BACK_CL * n_cl, 1), dim3(256), BACK_MANY_SMEM, st, (const float*)X, y, ybs,
-                          ycs, y_len, state, ss, e->w, T, a.pos_rel, chunk, n_chunks, B, active));
+        CK(launch_cluster(pdl, dim3(BACK_CL, 1, 1), back_many_kernel_t<Map>, dim3(BACK_CL * n_cl, 1), dim3(256), BACK_MANY_SMEM, st, (const float*)X, y, ybs,
+                          ycs, y_len, state, recs, e->w, T, a.pos_rel, chunk, n_chunks, B, active));
     } else {
-        CK(launch_cluster(pdl, dim3(BACK_CL, 1, 1), back_kernel, dim3(BACK_CL * T, B), dim3(256), BACK_SMEM, st, (const float*)X, y, ybs, ycs, y_len, state, ss, e->w, T,
+        CK(launch_cluster(pdl, dim3(BACK_CL, 1, 1), back_kernel_t<Map>, dim3(BACK_CL * T, B), dim3(256), BACK_SMEM, st, (const float*)X, y, ybs, ycs, y_len, state, recs, e->w, T,
                     a.pos_rel, 0, 1, 0, (int64_t)0, active));
     }
     MARK("back");
 #undef MARK
     return 0;
+}
+
+static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
+    const int64_t ss = stream_stride(e->n_blocks);
+    if (a.slots) return enqueue_chain_t(e, a, st, Records{ss, a.slots, a.state_batch});
+    return enqueue_chain_t(e, a, st, ss);
 }
 
 // ---- wavefront pipeline over (block, frame) for one-frame calls ---------------------------------------
@@ -849,7 +888,8 @@ static void drop_graphs(SepEngine* e) {
 // cache key of a chain graph: every argument its kernels bake in (`t`: frames, or -hops for the pipelined form)
 static std::vector<int64_t> graph_key(const ChainArgs& a, int t) {
     return {(int64_t)a.x, a.xbs, a.xcs, a.x_len, (int64_t)a.emb, (int64_t)a.state, (int64_t)a.y,
-            a.ybs, a.ycs, a.y_len, a.B, t, (int64_t)a.wsp, (int64_t)a.flags, a.pos_rel, (int64_t)a.active};
+            a.ybs, a.ycs, a.y_len, a.B, t, (int64_t)a.wsp, (int64_t)a.flags, a.pos_rel, (int64_t)a.active,
+            (int64_t)a.slots, a.state_batch};
 }
 
 // Launch the graph cached under `key` on `st`.  The first time a key is seen, `enqueue(cap)` is captured on the private
@@ -1195,6 +1235,23 @@ int l2h_sep_forward_active(void* handle, const float* x, int64_t xbs, int64_t xc
     ChainArgs a{x, xbs, xcs, x_len, emb, static_cast<float*>(state), y, ybs, ycs, y_len, batch, frames,
                 static_cast<float*>(ws), ws_bytes, flags & ~L2H_FLAG_GRAPH, 0};
     a.active = active_dev;
+    return run_chain(e, a, static_cast<cudaStream_t>(stream), (flags & L2H_FLAG_GRAPH) != 0);
+}
+
+int l2h_sep_forward_slots(void* handle, const float* x, int64_t xbs, int64_t xcs, int32_t x_len, const float* emb,
+                          void* state, int32_t state_batch, const int32_t* slots_dev, int32_t n, float* y, int64_t ybs,
+                          int64_t ycs, int32_t y_len, void* ws, size_t ws_bytes, uint32_t flags, void* stream) {
+    SepEngine* e = static_cast<SepEngine*>(handle);
+    if (!e || !x || !emb || !state || !y || !ws || !slots_dev) return fail(1, "null argument");
+    if (state_batch <= 0 || n <= 0 || n > state_batch)
+        return fail(1, "a slot list needs 0 < n <= state_batch (n = " + std::to_string(n) + ", state_batch = " +
+                           std::to_string(state_batch) + ")");
+    if (flags & L2H_FLAG_TAPS) return fail(1, "a slot list cannot be combined with L2H_FLAG_TAPS");
+    if (int rc_dev = check_device(e)) return rc_dev;
+    ChainArgs a{x, xbs, xcs, x_len, emb, static_cast<float*>(state), y, ybs, ycs, y_len, n, 1,
+                static_cast<float*>(ws), ws_bytes, flags & ~L2H_FLAG_GRAPH, 0};
+    a.slots = slots_dev;
+    a.state_batch = state_batch;
     return run_chain(e, a, static_cast<cudaStream_t>(stream), (flags & L2H_FLAG_GRAPH) != 0);
 }
 

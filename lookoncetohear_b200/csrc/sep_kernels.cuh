@@ -65,21 +65,44 @@ __global__ void state_init_kernel(float* state, int64_t total_floats, int64_t st
     }
 }
 
-// ---- per-stream clocks (sep_layout.h) and the activity mask of one-hop calls ----------------------------------
-__device__ __forceinline__ float* stream_rec(float* state, int64_t sstride, int b) {
-    return state + sizeof(StateHeader) / 4 + (int64_t)b * sstride;
+// ---- call rows -> stream records, per-stream clocks (sep_layout.h) and the rows that store -------------------------
+// Where the records of a slot-list call's rows live (l2h_sep_forward_slots): row b is record slots[b] of a state of
+// `batch` records.  Dense calls pass the record stride instead (row b is record b).  The kernels that address records
+// are templates over the two (`Map`): the dense forms compile to the arithmetic they had before slot lists existed.
+struct Records {
+    int64_t stride;            // floats per record
+    const int32_t* slots;      // device, one entry per call row
+    int32_t batch;             // records in the state
+};
+
+// The one decision of which record call row b reads and writes, and whether the row stores anything (its record and its
+// y row).  Dense rows store unless the activity mask of l2h_sep_forward_active clears them.  A slot-list entry outside
+// [0, batch) marks a row that is computed from record 0 (so every read stays inside the state) and stores nothing.
+struct RowRecord { int64_t off; bool stores; };
+__device__ __forceinline__ RowRecord row_record(int64_t stride, const uint8_t* active, int b) {
+    return {(int64_t)(sizeof(StateHeader) / 4) + (int64_t)b * stride, active == nullptr || active[b] != 0};
 }
-__device__ __forceinline__ const float* stream_rec(const float* state, int64_t sstride, int b) {
-    return state + sizeof(StateHeader) / 4 + (int64_t)b * sstride;
+__device__ __forceinline__ RowRecord row_record(const Records& r, const uint8_t*, int b) {
+    const int s = __ldg(r.slots + b);
+    const bool in = (unsigned)s < (unsigned)r.batch;
+    return {(int64_t)(sizeof(StateHeader) / 4) + (int64_t)(in ? s : 0) * r.stride, in};
+}
+template <class Map> __device__ __forceinline__ float* stream_rec(float* state, const Map& r, int b) {
+    return state + row_record(r, nullptr, b).off;
+}
+template <class Map> __device__ __forceinline__ const float* stream_rec(const float* state, const Map& r, int b) {
+    return state + row_record(r, nullptr, b).off;
+}
+template <class Map> __device__ __forceinline__ bool stream_active(const Map& r, const uint8_t* active, int b) {
+    return row_record(r, active, b).stores;
 }
 __device__ __forceinline__ long long rec_pos(const float* rec) { return *reinterpret_cast<const long long*>(rec + ST_POS); }
 __device__ __forceinline__ int rec_par(const float* rec) { return __float_as_int(rec[ST_CALLS]) & 1; }
-// active == nullptr: every stream advances (all calls except l2h_sep_forward_active with a mask)
-__device__ __forceinline__ bool stream_active(const uint8_t* active, int b) { return active == nullptr || active[b] != 0; }
 
 // End of a call, run by every thread of ONE CTA after all others have finished reading the clocks: the header advances by
-// `frames` frames and one call, and so does the clock of every active stream.
-__device__ void advance_clocks(float* state, int64_t sstride, int n_streams, int frames, const uint8_t* active) {
+// `frames` frames and one call, and so does the clock of every row that stores.
+template <class Map>
+__device__ void advance_clocks(float* state, Map recs, int n_streams, int frames, const uint8_t* active) {
     if (threadIdx.x == 0) {
         StateHeader* hdr = reinterpret_cast<StateHeader*>(state);
         hdr->pos += frames;
@@ -87,8 +110,8 @@ __device__ void advance_clocks(float* state, int64_t sstride, int n_streams, int
         hdr->done = 0;
     }
     for (int b = threadIdx.x; b < n_streams; b += blockDim.x) {
-        if (!stream_active(active, b)) continue;
-        float* rec = stream_rec(state, sstride, b);
+        if (!stream_active(recs, active, b)) continue;
+        float* rec = stream_rec(state, recs, b);
         *reinterpret_cast<long long*>(rec + ST_POS) += frames;
         rec[ST_CALLS] = __int_as_float(__float_as_int(rec[ST_CALLS]) + 1);
     }
@@ -96,7 +119,8 @@ __device__ void advance_clocks(float* state, int64_t sstride, int n_streams, int
 }
 
 // The last CTA of a call's final kernel advances the clocks (advance_clocks).
-__device__ __forceinline__ void finish_call(float* state, int64_t sstride, int n_streams, int frames, const uint8_t* active) {
+template <class Map>
+__device__ __forceinline__ void finish_call(float* state, Map recs, int n_streams, int frames, const uint8_t* active) {
     __shared__ int last;
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -105,7 +129,7 @@ __device__ __forceinline__ void finish_call(float* state, int64_t sstride, int n
         last = prev == (int)(gridDim.x * gridDim.y) - 1;
     }
     __syncthreads();
-    if (last) advance_clocks(state, sstride, n_streams, frames, active);
+    if (last) advance_clocks(state, recs, n_streams, frames, active);
 }
 
 __global__ void advance_header_kernel(float* state, int64_t sstride, int n_streams, int frames) {
@@ -134,14 +158,16 @@ __global__ void set_clip_base_kernel(float* state) {
 // look-ahead zeros of net.py:8-18,56-58).  Frames before the call start come from conv_buf.
 constexpr size_t FRONT_SMEM = (size_t)NFFT * 196 * sizeof(float);     // analysis filters, staged by TMA
 
+template <class Map>
 __device__ void spk_gate_cta(const float* __restrict__ emb, float* __restrict__ pre, float* __restrict__ state,
-                             int64_t sstride, const SepWeights& w, int b, float* red, const uint8_t* __restrict__ active);
+                             Map recs, const SepWeights& w, int b, float* red, const uint8_t* __restrict__ active);
 
+template <class Map>
 __global__ void __launch_bounds__(256)
-front_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride, int x_len,
-             float* __restrict__ X, float* __restrict__ state, int64_t sstride, SepWeights w, int T,
-             int pos_rel, const float* __restrict__ emb, float* __restrict__ spk_pre, int frame_k, int frames_total,
-             int sample_off, const uint8_t* __restrict__ active) {
+front_kernel_t(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride, int x_len,
+               float* __restrict__ X, float* __restrict__ state, Map recs, SepWeights w, int T,
+               int pos_rel, const float* __restrict__ emb, float* __restrict__ spk_pre, int frame_k, int frames_total,
+               int sample_off, const uint8_t* __restrict__ active) {
     extern __shared__ __align__(16) float wat_s[];     // [192][196]
     __shared__ __align__(16) float xs[NMIC][448];
     __shared__ float U[3][4][100];      // [frame t-2..t][ch][1 + f], zero-padded in f
@@ -151,7 +177,7 @@ front_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride, 
     const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
     if (t == T) {                      // the extra CTA of this stream: speaker-gate memo
         griddep_wait();
-        spk_gate_cta(emb, spk_pre, state, sstride, w, b, &xs[0][0], active);
+        spk_gate_cta(emb, spk_pre, state, recs, w, b, &xs[0][0], active);
         return;
     }
     if (tid == 0) { mbar_init(&wbar, 1); mbar_fence_init(); }
@@ -167,7 +193,7 @@ front_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride, 
     // writes the new tails (other parity) -- so the frames of a group never depend on each other here.
     const StateHeader* hdr = reinterpret_cast<const StateHeader*>(state);
     const int gi = frame_k + t, GN = (frames_total > 1) ? frames_total : T;
-    float* st = stream_rec(state, sstride, b);
+    float* st = stream_rec(state, recs, b);
     const int par = rec_par(st);
     const float* cb = st + ST_CONV + par * (2 * 4 * NF);
     float* cb_next = st + ST_CONV + (par ^ 1) * (2 * 4 * NF);
@@ -241,7 +267,7 @@ front_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride, 
     }
     trace_.mark(3);
     // next conv_buf = spectrogram rows of the last two frames of the group, written by its last frame
-    if (gi == GN - 1 && stream_active(active, b)) {
+    if (gi == GN - 1 && stream_active(recs, active, b)) {
         for (int e = tid; e < 4 * NF; e += 256) {
             cb_next[e] = U[1][e / NF][1 + e % NF];
             cb_next[4 * NF + e] = U[2][e / NF][1 + e % NF];
@@ -254,11 +280,12 @@ front_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride, 
 // only the NEW frame's spectrum is computed (the two before it stay in a 3-slot ring; front_kernel recomputes them: 3x the STFT),
 // and the next frame's samples are fetched while the current frame is worked on.  grid (n_chunks + 1, B): the last CTA of a
 // stream is the speaker-gate memo.  Frames [c*chunk, min(T, (c+1)*chunk)) for CTA c.
+template <class Map>
 __global__ void __launch_bounds__(256)
-front_many_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride, int x_len, float* __restrict__ X,
-                  float* __restrict__ state, int64_t sstride, SepWeights w, int T, int pos_rel, const float* __restrict__ emb,
-                  float* __restrict__ spk_pre, int chunk, int n_chunks, int n_streams, int n_workers,
-                  const uint8_t* __restrict__ active) {
+front_many_kernel_t(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride, int x_len, float* __restrict__ X,
+                    float* __restrict__ state, Map recs, SepWeights w, int T, int pos_rel, const float* __restrict__ emb,
+                    float* __restrict__ spk_pre, int chunk, int n_chunks, int n_streams, int n_workers,
+                    const uint8_t* __restrict__ active) {
     extern __shared__ __align__(16) float wat_s[];     // [192][196]
     __shared__ __align__(16) float xs[NMIC][NFFT];      // the samples of the frame being transformed (>= 288 floats: gate CTA scratch)
     __shared__ float U[3][4][100];      // ring: frame g -> slot (g + 3) % 3; [ch][1 + f], zero-padded in f
@@ -267,7 +294,7 @@ front_many_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstr
     const int tid = threadIdx.x;
     if ((int)blockIdx.x >= n_workers) {        // one more CTA per stream: speaker-gate memo
         griddep_wait();
-        spk_gate_cta(emb, spk_pre, state, sstride, w, (int)blockIdx.x - n_workers, &xs[0][0], active);
+        spk_gate_cta(emb, spk_pre, state, recs, w, (int)blockIdx.x - n_workers, &xs[0][0], active);
         return;
     }
     if (tid == 0) { mbar_init(&wbar, 1); mbar_fence_init(); }
@@ -287,9 +314,9 @@ front_many_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstr
     for (int item = blockIdx.x; item < n_streams * n_chunks; item += n_workers) {
     const int b = item / n_chunks, c = item % n_chunks;
     const int t0 = c * chunk, t1 = min(T, t0 + chunk);
-    float* st = stream_rec(state, sstride, b);
+    float* st = stream_rec(state, recs, b);
     const int par = rec_par(st);
-    const bool live = stream_active(active, b);
+    const bool live = stream_active(recs, active, b);
     const float* cb = st + ST_CONV + par * (2 * 4 * NF);
     float* cb_next = st + ST_CONV + (par ^ 1) * (2 * 4 * NF);
     const float* xb = x + (int64_t)b * x_bstride;
@@ -381,12 +408,13 @@ front_many_kernel(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstr
 // memoised ON THE DEVICE: one extra CTA per stream rides along with front_kernel, compares the
 // embedding with the one the cached gate was built from and returns at once if they are equal
 // (the streaming steady state).  Otherwise that CTA rebuilds the gate (6208x256 GEMV + LayerNorm).
+template <class Map>
 __device__ void spk_gate_cta(const float* __restrict__ emb, float* __restrict__ pre, float* __restrict__ state,
-                             int64_t sstride, const SepWeights& w, int b, float* red /* >= 288 floats smem */,
+                             Map recs, const SepWeights& w, int b, float* red /* >= 288 floats smem */,
                              const uint8_t* __restrict__ active) {
-    if (!stream_active(active, b)) return;     // a stream that skips this hop keeps its record as it is, memo included
+    if (!stream_active(recs, active, b)) return;     // a stream that skips this hop keeps its record as it is, memo included
     const int tid = threadIdx.x;
-    float* st = stream_rec(state, sstride, b);
+    float* st = stream_rec(state, recs, b);
     const float e = emb[(int64_t)b * SPK + tid];
     // memo key: the embedding AND the weight generation (a reused state must not keep a gate built from old weights)
     const int same = __syncthreads_and(e == st[ST_EMB + tid] && __float_as_int(st[ST_GEN]) == w.gen);
@@ -460,10 +488,11 @@ constexpr int QKV_PLD = NQKV;                 // 112: a frame's projections are 
 constexpr int QKV_LNP = 4 * QK_LD + 2 * V_DIM;  // staged LayerNorm params: gq | bq | gk | bk | gv | bv
 constexpr size_t QKV_SMEM = (size_t)(64 * 100 + 64 * NQKV + NF * QKV_PLD + QKV_LNP) * sizeof(float);
 
+template <class Map>
 __global__ void __launch_bounds__(QKV_THREADS)
-qkv_kernel(const float* __restrict__ X, const float* __restrict__ pre, float* __restrict__ Qbuf,
-           float* __restrict__ Kall, float* __restrict__ Vall, float* __restrict__ state, int64_t sstride, int blk,
-           BlockWeights w, int T, int frame_k, const uint8_t* __restrict__ active) {
+qkv_kernel_t(const float* __restrict__ X, const float* __restrict__ pre, float* __restrict__ Qbuf,
+             float* __restrict__ Kall, float* __restrict__ Vall, float* __restrict__ state, Map recs, int blk,
+             BlockWeights w, int T, int frame_k, const uint8_t* __restrict__ active) {
     extern __shared__ __align__(16) float sm[];
     float* Xt = sm;                      // [64][100]  k-major, rows padded to 100 (zeros)
     float* Ws = Xt + 64 * 100;           // [64][112]
@@ -568,7 +597,7 @@ qkv_kernel(const float* __restrict__ X, const float* __restrict__ pre, float* __
     const float rs = rsqrtf(warp_sum(q) / (float)n + 1e-5f);
     const float* gam = LNP + (which == 0 ? 0 : (which == 1 ? 2 * QK_LD : 4 * QK_LD));
     const float* bet = LNP + (which == 0 ? QK_LD : (which == 1 ? 3 * QK_LD : 4 * QK_LD + V_DIM));
-    float* rec = stream_rec(state, sstride, b);
+    float* rec = stream_rec(state, recs, b);
     const long long pos = rec_pos(rec) + frame_k;
     const int ld = (which == 2) ? V_DIM : QK_LD;
     float* dst0 = nullptr;   // linear scratch / Q buffer
@@ -579,7 +608,7 @@ qkv_kernel(const float* __restrict__ X, const float* __restrict__ pre, float* __
     } else {
         float* sb = rec + ST_BLK + (int64_t)blk * BK_STRIDE;
         const int slot = (int)((pos + t) % RING);
-        if (t >= T - ATT && stream_active(active, b))
+        if (t >= T - ATT && stream_active(recs, active, b))
             dst1 = sb + (which == 1 ? BK_K : BK_V) + ((int64_t)h * RING + slot) * ld;
         if (T > 1) dst0 = (which == 1 ? Kall : Vall) + (bh * (ATT - 1 + T) + (ATT - 1) + t) * ld;
     }
@@ -607,10 +636,11 @@ qkv_kernel(const float* __restrict__ X, const float* __restrict__ pre, float* __
 // the staging latency per frame; this form is bound by the 86 KB each frame moves.
 constexpr size_t QKV_MANY_SMEM = (size_t)(2 * NF * QKV_PLD + QKV_LNP) * sizeof(float);
 
+template <class Map>
 __global__ void __launch_bounds__(QKV_THREADS)
-qkv_many_kernel(const float* __restrict__ pre, float* __restrict__ Qbuf, float* __restrict__ Kall, float* __restrict__ Vall,
-                float* __restrict__ state, int64_t sstride, int blk, BlockWeights w, int T, int n_frames,
-                const uint8_t* __restrict__ active) {
+qkv_many_kernel_t(const float* __restrict__ pre, float* __restrict__ Qbuf, float* __restrict__ Kall, float* __restrict__ Vall,
+                  float* __restrict__ state, Map recs, int blk, BlockWeights w, int T, int n_frames,
+                  const uint8_t* __restrict__ active) {
     extern __shared__ __align__(16) float sm[];
     float* Pb[2] = {sm, sm + NF * QKV_PLD};
     float* LNP = sm + 2 * NF * QKV_PLD;
@@ -681,10 +711,10 @@ qkv_many_kernel(const float* __restrict__ pre, float* __restrict__ Qbuf, float* 
         if (which == 0) {
             dst0 = Qbuf + (bh * T + t) * QK_LD;
         } else {
-            float* rec = stream_rec(state, sstride, b);
+            float* rec = stream_rec(state, recs, b);
             float* sb = rec + ST_BLK + (int64_t)blk * BK_STRIDE;
             const int slot = (int)((rec_pos(rec) + t) % RING);
-            if (t >= T - ATT && stream_active(active, b)) dst1 = sb + (which == 1 ? BK_K : BK_V) + ((int64_t)h * RING + slot) * ld;
+            if (t >= T - ATT && stream_active(recs, active, b)) dst1 = sb + (which == 1 ? BK_K : BK_V) + ((int64_t)h * RING + slot) * ld;
             if (T > 1) dst0 = (which == 1 ? Kall : Vall) + (bh * (ATT - 1 + T) + (ATT - 1) + t) * ld;
         }
         {
@@ -711,9 +741,10 @@ qkv_many_kernel(const float* __restrict__ pre, float* __restrict__ Qbuf, float* 
 // T == 1: K/V rows are ring slots (frame n lives in slot n mod RING); T > 1: rows t .. t+49 of the
 // linear scratch.  Used when there are enough (frame, head, stream) items to fill the GPU but too few
 // frames per stream to tile (e.g. 256 streams x 1 hop); see attn_cluster_kernel / attn_tile_kernel.
+template <class Map>
 __global__ void __launch_bounds__(256)
-attn_kernel(const float* __restrict__ Qbuf, const float* __restrict__ Kall, const float* __restrict__ Vall,
-            const float* __restrict__ state, int64_t sstride, int blk, float* __restrict__ Z, int T, int frame_k) {
+attn_kernel_t(const float* __restrict__ Qbuf, const float* __restrict__ Kall, const float* __restrict__ Vall,
+              const float* __restrict__ state, Map recs, int blk, float* __restrict__ Z, int T, int frame_k) {
     __shared__ __align__(16) float qs[QK_LD];
     __shared__ float sc[64];
     griddep_launch();
@@ -724,7 +755,7 @@ attn_kernel(const float* __restrict__ Qbuf, const float* __restrict__ Kall, cons
     const float* vb;
     int first = 0, wrap = 0x7fffffff;       // window row j -> storage row (first + j) % wrap
     if (T == 1) {                           // ring: window = frames pos-49 .. pos of the stream's clock
-        const float* rec = stream_rec(state, sstride, b);
+        const float* rec = stream_rec(state, recs, b);
         const float* sb = rec + ST_BLK + (int64_t)blk * BK_STRIDE;
         kb = sb + BK_K + (int64_t)h * RING * QK_LD;
         vb = sb + BK_V + (int64_t)h * RING * V_DIM;
@@ -899,10 +930,11 @@ attn_tile_kernel(const float* __restrict__ Qbuf, const float* __restrict__ Kall,
 // through L2/HBM, no separate merge pass.  grid (T, 4*8, B), cluster (1, 8, 1), 256 threads.
 constexpr int ATT_CL = 8;
 
+template <class Map>
 __global__ void __launch_bounds__(256)
-attn_cluster_kernel(const float* __restrict__ Qbuf, const float* __restrict__ Kall, const float* __restrict__ Vall,
-                    const float* __restrict__ state, int64_t sstride, int blk, float* __restrict__ Z, int T,
-                    int frame_k) {
+attn_cluster_kernel_t(const float* __restrict__ Qbuf, const float* __restrict__ Kall, const float* __restrict__ Vall,
+                      const float* __restrict__ state, Map recs, int blk, float* __restrict__ Z, int T,
+                      int frame_k) {
     namespace cg = cooperative_groups;
     __shared__ __align__(16) float qs[QK_LD];
     __shared__ __align__(16) float os[V_DIM];     // this CTA's partial output
@@ -921,7 +953,7 @@ attn_cluster_kernel(const float* __restrict__ Qbuf, const float* __restrict__ Ka
     const float* vb;
     int first = j0, wrap = 0x7fffffff;      // window row j -> storage row (first + j) % wrap
     if (T == 1) {                           // ring: window = frames pos-49 .. pos of the stream's clock, frame n in slot n mod RING
-        const float* rec = stream_rec(state, sstride, b);
+        const float* rec = stream_rec(state, recs, b);
         const float* sb = rec + ST_BLK + (int64_t)blk * BK_STRIDE;
         kb = sb + BK_K + (int64_t)h * RING * QK_LD;
         vb = sb + BK_V + (int64_t)h * RING * V_DIM;
@@ -1026,9 +1058,10 @@ attn_cluster_kernel(const float* __restrict__ Qbuf, const float* __restrict__ Ka
 // input of block 1 (:250-251) is folded into this epilogue.  grid (T, B), 256 threads.
 constexpr size_t AOUT_SMEM = (size_t)(64 * 100 + 64 * 64 + NF * 64 + 4 * FC) * sizeof(float);   // + gamma, beta, X row, gate
 
+template <class Map>
 __global__ void __launch_bounds__(256)
-attn_out_kernel(const float* __restrict__ Z, float* __restrict__ X, const float* __restrict__ state,
-                int64_t sstride, BlockWeights w, int apply_gate, int T) {
+attn_out_kernel_t(const float* __restrict__ Z, float* __restrict__ X, const float* __restrict__ state,
+                  Map recs, BlockWeights w, int apply_gate, int T) {
     extern __shared__ __align__(16) float sm[];
     __shared__ float red[32];
     float* Zt = sm;                 // [64][100]
@@ -1041,7 +1074,7 @@ attn_out_kernel(const float* __restrict__ Z, float* __restrict__ X, const float*
     __shared__ __align__(8) unsigned long long bars[2];
     const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
     float* xr = X + ((int64_t)b * T + t) * NF * CH;
-    const float* gate = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride + ST_GATE;
+    const float* gate = stream_rec(state, recs, b) + ST_GATE;
     TraceScope trace_(TK_ATTN_OUT, Z);
     griddep_launch();
     if (tid == 0) { mbar_init(&bars[0], 1); mbar_init(&bars[1], 1); mbar_fence_init(); }
@@ -1143,10 +1176,11 @@ constexpr size_t BACK_SMEM = (size_t)(4 * (BACK_FMAX + 2) * 64 + 2 * BACK_FMAX *
 
 __device__ __forceinline__ int back_f0(int part) { return (part * NF) / BACK_CL; }
 
+template <class Map>
 __global__ void __launch_bounds__(256)
-back_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_bstride, int64_t y_cstride,
-            int y_len, float* __restrict__ state, int64_t sstride, SepWeights w, int T, int pos_rel, int frame_k,
-            int frames_total, int sample_off, int64_t hist_stride, const uint8_t* __restrict__ active) {
+back_kernel_t(const float* __restrict__ X, float* __restrict__ y, int64_t y_bstride, int64_t y_cstride,
+              int y_len, float* __restrict__ state, Map recs, SepWeights w, int T, int pos_rel, int frame_k,
+              int frames_total, int sample_off, int64_t hist_stride, const uint8_t* __restrict__ active) {
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
     extern __shared__ __align__(16) float sm[];
@@ -1191,9 +1225,9 @@ back_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_bstrid
     trace_.mark(0);
     const StateHeader* hdr = reinterpret_cast<const StateHeader*>(state);
     const int soff = sample_off + (pos_rel ? (int)(hdr->pos - hdr->clip_base) * HOP : 0);
-    float* st = stream_rec(state, sstride, b);
+    float* st = stream_rec(state, recs, b);
     const int par = rec_par(st);
-    const bool live = stream_active(active, b);
+    const bool live = stream_active(recs, active, b);
     const float* db = st + ST_DECONV + par * (2 * FC);
     float* db_next = st + ST_DECONV + (par ^ 1) * (2 * FC);
     const float* ib = st + ST_ISTFT + par * (NSRC * NROW);
@@ -1307,7 +1341,7 @@ back_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_bstrid
     trace_.mark(6);
     // ordinary call: the last CTA to finish advances the clocks (a pipelined graph runs several back_kernels
     // at once and advances them with advance_header_kernel after all of its frames instead)
-    if (frames_total == 1) finish_call(state, sstride, gridDim.y, T, active);
+    if (frames_total == 1) finish_call(state, recs, gridDim.y, T, active);
 }
 
 
@@ -1320,10 +1354,11 @@ back_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_bstrid
 // grid (BACK_CL * n_chunks, B) in clusters of BACK_CL, 256 threads; frames [c*chunk, min(T, (c+1)*chunk)) for cluster c.
 constexpr size_t BACK_MANY_SMEM = (size_t)(4 * (BACK_FMAX + 2) * 64 + 2 * BACK_FMAX * NFFT + 2 * NSRC * NROW + 2 * NSRC * NFFT) * sizeof(float);
 
+template <class Map>
 __global__ void __launch_bounds__(256)
-back_many_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_bstride, int64_t y_cstride, int y_len,
-                 float* __restrict__ state, int64_t sstride, SepWeights w, int T, int pos_rel, int chunk, int n_chunks, int n_streams,
-                 const uint8_t* __restrict__ active) {
+back_many_kernel_t(const float* __restrict__ X, float* __restrict__ y, int64_t y_bstride, int64_t y_cstride, int y_len,
+                   float* __restrict__ state, Map recs, SepWeights w, int T, int pos_rel, int chunk, int n_chunks, int n_streams,
+                   const uint8_t* __restrict__ active) {
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
     extern __shared__ __align__(16) float sm[];
@@ -1371,9 +1406,9 @@ back_many_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_b
     for (int item = cl; item < n_streams * n_chunks; item += n_cl) {
         const int b = item / n_chunks, c = item % n_chunks;
         const int t0 = c * chunk, t1 = min(T, t0 + chunk);
-        float* st = stream_rec(state, sstride, b);
+        float* st = stream_rec(state, recs, b);
         const int par = rec_par(st);
-        const bool live = stream_active(active, b);
+        const bool live = stream_active(recs, active, b);
         const float* db = st + ST_DECONV + par * (2 * FC);
         float* db_next = st + ST_DECONV + (par ^ 1) * (2 * FC);
         const float* ib = st + ST_ISTFT + par * (NSRC * NROW);
@@ -1486,16 +1521,17 @@ back_many_kernel(const float* __restrict__ X, float* __restrict__ y, int64_t y_b
         }
     }
     cluster.sync();                         // nobody leaves while CTA 0 may still read its shared memory
-    finish_call(state, sstride, n_streams, T, active);      // the last CTA to finish advances the clocks
+    finish_call(state, recs, n_streams, T, active);      // the last CTA to finish advances the clocks
 }
 
 // ------------------------------------------------------------------------------------------
 // Tail of the attention output for calls with many rows, where the Linear(64->64) + PReLU ran as a tensor-core GEMM
 // into P: LayerNorm over the frame's (F, C) = 6208 values + residual (+ the speaker gate after block 0)
 // (tfgridnet_causal.py:583-588, :250-251).  Same arithmetic as the tail of attn_out_kernel.  grid (T, B), 256 threads.
+template <class Map>
 __global__ void __launch_bounds__(256)
-ln_frame_res_kernel(const float* __restrict__ P, float* __restrict__ X, const float* __restrict__ state, int64_t sstride,
-                    BlockWeights w, int apply_gate, int T) {
+ln_frame_res_kernel_t(const float* __restrict__ P, float* __restrict__ X, const float* __restrict__ state, Map recs,
+                      BlockWeights w, int apply_gate, int T) {
     __shared__ float red[32];
     __shared__ __align__(16) float Ps[FC];
     const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
@@ -1512,7 +1548,7 @@ ln_frame_res_kernel(const float* __restrict__ P, float* __restrict__ X, const fl
     float q = 0.f;
     for (int i = tid; i < FC; i += 256) { const float d = Ps[i] - mu; q += d * d; }
     const float rs = rsqrtf(block_sum(q, red) * (1.f / FC) + 1e-5f);
-    const float* gate = state + sizeof(StateHeader) / 4 + (int64_t)b * sstride + ST_GATE;
+    const float* gate = stream_rec(state, recs, b) + ST_GATE;
     float* xr = X + off;
     for (int i = tid; i < FC / 4; i += 256) {
         float4 x4 = reinterpret_cast<const float4*>(xr)[i];
@@ -1534,9 +1570,10 @@ ln_frame_res_kernel(const float* __restrict__ P, float* __restrict__ X, const fl
 // pre-activations [rows][256] (column j*4+q, q in i,f,g,o; = LN(x) W_ih^T + h W_hh^T + b from ONE tensor-core GEMM
 // over the concatenated k = [x | h]) and the carried cell state give the new (h, c), written back to the per-stream
 // state records, and h again as contiguous rows for the Linear that follows.  One thread per (row, hidden unit).
+template <class Map>
 __global__ void __launch_bounds__(256)
-lstm_cell_rows_kernel(const float* __restrict__ gates, float* __restrict__ state, int64_t sstride, int blk, float* __restrict__ Hout,
-                      int rows, const uint8_t* __restrict__ active) {
+lstm_cell_rows_kernel_t(const float* __restrict__ gates, float* __restrict__ state, Map recs, int blk, float* __restrict__ Hout,
+                        int rows, const uint8_t* __restrict__ active) {
     griddep_launch();
     griddep_wait();
     const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
@@ -1544,7 +1581,7 @@ lstm_cell_rows_kernel(const float* __restrict__ gates, float* __restrict__ state
     const int row = (int)(i >> 6), j = (int)(i & 63);
     const int b = row / NF, f = row % NF;
     const float4 g = *reinterpret_cast<const float4*>(gates + (int64_t)row * 256 + j * 4);
-    float* base = stream_rec(state, sstride, b) + ST_BLK + (int64_t)blk * BK_STRIDE;
+    float* base = stream_rec(state, recs, b) + ST_BLK + (int64_t)blk * BK_STRIDE;
     float* hp = base + BK_H + f * 64 + j;
     float* cp = base + BK_C + f * 64 + j;
     constexpr float LOG2E = 1.4426950408889634f;
@@ -1554,11 +1591,38 @@ lstm_cell_rows_kernel(const float* __restrict__ gates, float* __restrict__ state
     const float og = __fdividef(1.f, 1.f + ex2_ftz(-LOG2E * g.w));
     const float c = fg * *cp + ig * gg;
     const float h = og * (__fdividef(2.f, 1.f + ex2_ftz(-2.f * LOG2E * c)) - 1.f);
-    if (stream_active(active, b)) {
+    if (stream_active(recs, active, b)) {
         *cp = c;
         *hp = h;
     }
     Hout[i] = h;
 }
+
+// Slot-list calls in the tensor-core form: the inter-step GEMM reads the previous h through a strided tensor map over the
+// records, which a slot list cannot express.  Once per call, before any block's cell update, this copies the h of every
+// block of every row's record to Hg[blk][row][f][c] for the GEMM to read instead.  One thread per float4.
+__global__ void __launch_bounds__(256)
+gather_h_kernel(const float* __restrict__ state, Records recs, int n_blocks, int n_streams, float* __restrict__ Hg) {
+    constexpr int PER = FC / 4;                        // float4s of one block's h
+    const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    if (i >= (int64_t)n_blocks * n_streams * PER) return;
+    const int k = (int)(i % PER), row = (int)(i / PER);
+    const int b = row % n_streams, blk = row / n_streams;
+    const float* h = stream_rec(state, recs, b) + ST_BLK + (int64_t)blk * BK_STRIDE + BK_H;
+    reinterpret_cast<float4*>(Hg)[i] = reinterpret_cast<const float4*>(h)[k];
+}
+
+// the dense forms (call row b = record b); the `_t<Records>` forms serve slot-list calls (l2h_sep_forward_slots)
+constexpr auto front_kernel = front_kernel_t<int64_t>;
+constexpr auto front_many_kernel = front_many_kernel_t<int64_t>;
+constexpr auto qkv_kernel = qkv_kernel_t<int64_t>;
+constexpr auto qkv_many_kernel = qkv_many_kernel_t<int64_t>;
+constexpr auto attn_kernel = attn_kernel_t<int64_t>;
+constexpr auto attn_cluster_kernel = attn_cluster_kernel_t<int64_t>;
+constexpr auto attn_out_kernel = attn_out_kernel_t<int64_t>;
+constexpr auto back_kernel = back_kernel_t<int64_t>;
+constexpr auto back_many_kernel = back_many_kernel_t<int64_t>;
+constexpr auto ln_frame_res_kernel = ln_frame_res_kernel_t<int64_t>;
+constexpr auto lstm_cell_rows_kernel = lstm_cell_rows_kernel_t<int64_t>;
 
 }  // namespace l2h

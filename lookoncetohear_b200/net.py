@@ -413,24 +413,31 @@ class Net(nn.Module):
         _cabi.check(L.l2h_sep_state_offsets(h, offs, n))
         return hb.value, stride.value, list(offs)
 
-    def _run(self, x, embed, state, frames, out_len, flags=0, active=None):
-        """x [B,M,n] (any length; samples beyond n read as zero), embed [B,256], active: [B] uint8 device mask or None."""
+    def _run(self, x, embed, state, frames, out_len, flags=0, active=None, slots=None):
+        """x [B,M,n] (any length; samples beyond n read as zero), embed [B,256], active: [B] uint8 device mask or None,
+        slots: [B] int32 device list of the state's records the rows advance (one-hop calls) or None."""
         self._require_cuda(x)
         dev = x.device
         self._sync_weights(dev)
         x = x.contiguous().float()
         embed = embed.to(dev, torch.float32).contiguous()
         Bsz = x.shape[0]
-        if state.batch != Bsz:
+        if slots is None and state.batch != Bsz:
             raise ValueError(f"state was built for batch {state.batch}, input has batch {Bsz}")
         y = torch.empty(Bsz, self.num_src, out_len, dtype=torch.float32, device=dev)
         ws, nbytes = self._workspace(dev, Bsz, frames, flags)
+        L, st = _cabi.lib(), torch.cuda.current_stream(dev).cuda_stream
         with torch.cuda.device(dev):
-            _cabi.check(_cabi.lib().l2h_sep_forward_active(
-                self._engine(), x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], embed.data_ptr(),
-                state.buf.data_ptr(), y.data_ptr(), y.stride(0), y.stride(1), out_len, Bsz, frames,
-                ws.data_ptr(), ws.numel(), flags, torch.cuda.current_stream(dev).cuda_stream,
-                None if active is None else active.data_ptr()))
+            if slots is not None:
+                _cabi.check_args(L.l2h_sep_forward_slots(
+                    self._engine(), x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], embed.data_ptr(),
+                    state.buf.data_ptr(), state.batch, slots.data_ptr(), Bsz, y.data_ptr(), y.stride(0), y.stride(1),
+                    out_len, ws.data_ptr(), ws.numel(), flags, st))
+            else:
+                _cabi.check(L.l2h_sep_forward_active(
+                    self._engine(), x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], embed.data_ptr(),
+                    state.buf.data_ptr(), y.data_ptr(), y.stride(0), y.stride(1), out_len, Bsz, frames,
+                    ws.data_ptr(), ws.numel(), flags, st, None if active is None else active.data_ptr()))
         return y
 
     @staticmethod
@@ -444,11 +451,38 @@ class Net(nn.Module):
             raise ValueError(f"active must have shape ({batch},), got {tuple(active.shape)}")
         return active.contiguous().view(torch.uint8)
 
-    def predict(self, x, embed, input_state, pad=True, active=None):
+    @staticmethod
+    def _slot_list(slots, dev, n, batch):
+        """`slots` of predict as the [n] int32 device tensor the engine reads.  A CUDA int32 tensor is used as it is (its
+        entries are read when the kernels run); anything else is checked here and uploaded."""
+        if isinstance(slots, torch.Tensor) and slots.is_cuda:
+            if slots.dtype != torch.int32 or tuple(slots.shape) != (n,) or not slots.is_contiguous():
+                raise ValueError(f"a CUDA slot list must be a contiguous int32 tensor of shape ({n},)")
+            if slots.device != dev:
+                raise ValueError(f"slots must live on the input's device {dev}, not {slots.device}")
+            return slots
+        s = torch.as_tensor(slots)
+        if s.dtype.is_floating_point or s.dtype.is_complex or s.dtype == torch.bool or s.dim() != 1:
+            raise ValueError("slots must be a sequence or 1-d tensor of integer slot indices")
+        if s.numel() != n:
+            raise ValueError(f"slots lists {s.numel()} records for {n} input rows")
+        if n > 0 and (int(s.min()) < 0 or int(s.max()) >= batch):
+            raise ValueError(f"a slot lies outside [0, {batch})")
+        if len(set(s.tolist())) != n:
+            raise ValueError("a slot is listed twice")
+        return s.to(torch.int32).to(dev)
+
+    def predict(self, x, embed, input_state, pad=True, active=None, slots=None):
         """Reference net.py:54-66.  x [B,M,N]; embed [B,256]; returns (y [B,S,*], state).
 
         active: None, or for a one-hop call a [B] bool / uint8 CUDA tensor: only the streams with a true entry advance.
-        The others are untouched -- record, clock and speaker-gate memo -- and their rows of y are left unwritten."""
+        The others are untouched -- record, clock and speaker-gate memo -- and their rows of y are left unwritten.
+
+        slots: None, or for a one-hop call the records of `input_state` the B input rows advance: row i continues stream
+        slots[i], and the call costs what B streams cost, whatever the state's size.  Records not listed are not read or
+        written.  Either B distinct ints in [0, state.batch) (a sequence or CPU tensor, checked and uploaded), or a CUDA
+        int32 tensor used in place: there an entry outside [0, state.batch) marks a row that stores nothing (its y row is
+        left unwritten), and listing a slot twice is the caller's error.  Cannot be combined with `active`."""
         hop, la = self.stft_chunk_size, self.stft_pad_size
         n = x.shape[-1]
         if pad:
@@ -461,12 +495,19 @@ class Net(nn.Module):
             out_len = frames * hop
         if not isinstance(input_state, SepState):
             raise TypeError("input_state must come from Net.init_buffers()")
+        if slots is not None:
+            if active is not None:
+                raise ValueError("slots and active cannot be combined: skip a stream by leaving it out of the list")
+            if frames != 1:
+                raise ValueError(f"slots needs a one-hop call ({hop}+{la} samples with pad=False), this call has {frames} hops")
+            self._require_cuda(x)
+            slots = self._slot_list(slots, x.device, x.shape[0], input_state.batch)
         if active is not None:
             if frames != 1:
                 raise ValueError(f"active needs a one-hop call ({hop}+{la} samples with pad=False), this call has {frames} hops")
             self._require_cuda(x)
             active = self._active_mask(active, x.device, x.shape[0])
-        y = self._run(x, embed, input_state, frames, out_len, active=active)
+        y = self._run(x, embed, input_state, frames, out_len, active=active, slots=slots)
         return y, input_state
 
     def forward(self, x, embeds, input_state=None, pad=True):
