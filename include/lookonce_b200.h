@@ -14,6 +14,8 @@
  *                                               tfgridnet_causal.py:188-283
  *   l2h_sep_forward_active / l2h_sep_forward_slots
  *        <- one Net.predict hop for some of a state's streams (serving many listeners: INTEGRATION.md)
+ *   l2h_sep_forward_slots_frames
+ *        <- several Net.predict hops for a list of a state's streams (Net.advance_slots)
  *   l2h_sep_stream_host
  *        <- the chunk loop around Net.predict(chunk, embed, state, pad=False)  (SURVEY.md 3.3)
  *           with host buffers: H2D of each chunk and D2H of each result inside the call
@@ -154,6 +156,23 @@ int l2h_sep_forward_slots(void* handle, const float* x_dev, int64_t x_batch_stri
                           const float* emb_dev, void* state_dev, int32_t state_batch, const int32_t* slots_dev, int32_t n,
                           float* y_dev, int64_t y_batch_stride, int64_t y_ch_stride, int32_t y_len,
                           void* workspace_dev, size_t workspace_bytes, uint32_t flags, void* stream);
+/* l2h_sep_forward_slots for `frames` hops: every call row advances its record by `frames` hops in one call, so a listener
+ * that fell behind catches up its backlog at once, or listed listeners run at a cadence of several hops.  The T hops of a
+ * row run their BiLSTMs side by side as in a dense multi-hop call; only the inter-LSTM cells and the attention run in
+ * frame order.  l2h_sep_forward_slots is this call with frames == 1.
+ *   x_dev      row i holds 128*frames + 64 samples (x_len); y_dev row i receives 128*frames samples
+ *   workspace  l2h_sep_workspace_bytes(handle, n, frames, flags), as for a dense call of n streams and `frames` hops
+ *   slots_dev  as for l2h_sep_forward_slots; with L2H_FLAG_GRAPH the cached graph's key holds n and frames.  An entry
+ *              outside [0, state_batch) marks a row that is computed from record 0 and stores nothing (no record, no y
+ *              row) for all of its frames.
+ * Every row advances by the same number of hops: listeners with different backlogs go in different calls.  Records not
+ * listed are neither read nor written; the header advances by `frames` as for any call.
+ * Errors 1, before anything is enqueued: null pointers, n <= 0, n > state_batch, frames <= 0, L2H_FLAG_TAPS. */
+int l2h_sep_forward_slots_frames(void* handle, const float* x_dev, int64_t x_batch_stride, int64_t x_ch_stride,
+                                 int32_t x_len, const float* emb_dev, void* state_dev, int32_t state_batch,
+                                 const int32_t* slots_dev, int32_t n, int32_t frames, float* y_dev,
+                                 int64_t y_batch_stride, int64_t y_ch_stride, int32_t y_len, void* workspace_dev,
+                                 size_t workspace_bytes, uint32_t flags, void* stream);
 
 /* Streaming with HOST buffers (the end-to-end path).  Per round: H2D of the round's samples (+64
  * look-ahead) from pinned memory, the kernel chains, D2H of the new samples; one stream synchronise at

@@ -232,9 +232,10 @@ static Workspace carve(int n_blocks, int B, int T, uint32_t flags) {
     ws.PRE = alloc((int64_t)B * FC);
     ws.QKVRAW = alloc(rows * NQKV);
     ws.TAPS = alloc((flags & L2H_FLAG_TAPS) ? (int64_t)(1 + 3 * n_blocks) * rows * 64 : 0);
-    // one-hop calls in the tensor-core form: the listed records' h of every block for a slot-list call (gather_h_kernel)
+    // the listed records' carried inter-LSTM state of every block for a slot-list call (gather_h_kernel): h for one-hop
+    // calls in the tensor-core form, h and c ([n_blocks][B][97][64] each) for every multi-hop call
     const bool tc_hop = T == 1 && rows > TC_MIN_ROWS && !(flags & L2H_FLAG_TAPS);
-    ws.HG = alloc(tc_hop ? (int64_t)n_blocks * rows * 64 : 0);
+    ws.HG = alloc((T > 1 ? 2 : tc_hop ? 1 : 0) * (int64_t)n_blocks * B * FC);
     ws.total = (cur + 511) & ~int64_t(511);      // a multiple of one GX row: pipelined hops address their slots as rows of one tensor
     return ws;
 }
@@ -361,7 +362,7 @@ struct ChainArgs {
     int B, T; float* wsp; size_t ws_bytes; uint32_t flags; int pos_rel;
     Profiler* prof = nullptr;
     const uint8_t* active = nullptr;     // one-hop calls: [B] device mask of the streams that advance (null: all)
-    const int32_t* slots = nullptr;      // one-hop calls: [B] device list, row b -> record slots[b] (null: row b -> record b)
+    const int32_t* slots = nullptr;      // [B] device list, row b -> record slots[b] (null: row b -> record b)
     int state_batch = 0;                 // records in the state (slot lists only)
 };
 
@@ -414,12 +415,14 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
     e->cur_pdl = false;
 #define MARK(name) do { if (a.prof) { if (int _rc = a.prof->mark(name, st)) return _rc; } } while (0)
     MARK("start");
+    // slot lists: the listed records' h of every block, for the one-hop inter-step GEMMs, or their (h, c) for the
+    // multi-hop inter recurrences, which carry them in the workspace (HG, CG) until scatter_hc_kernel stores them back
+    const int64_t hc4 = (int64_t)e->n_blocks * B * FC / 4;      // float4s of one of them
+    float* CG = HG + (int64_t)e->n_blocks * B * FC;
     if constexpr (std::is_same_v<Map, Records>) {
-        if (tc_mid) {      // the listed records' h of every block, for the inter-step GEMMs below
-            const int64_t n4 = (int64_t)e->n_blocks * B * FC / 4;
-            CK(launch_k(false, gather_h_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, st, (const float*)state, recs,
-                        e->n_blocks, B, HG));
-        }
+        if (tc_mid || T > 1)
+            CK(launch_k(false, gather_h_kernel, dim3((unsigned)((hc4 + 255) / 256)), dim3(256), 0, st, (const float*)state, recs,
+                        e->n_blocks, B, HG, T > 1 ? CG : nullptr));
     }
     if (fused_tail) {      // the frame as 13 row tiles: spectrum of the tile's bins, conv, and block 0's input projection
         CK(launch_k(false, front1_kernel_t<Map>, dim3(TAIL_TILES + 1, B), dim3(256), FRONT1_SMEM, st, x, xbs, xcs, x_len, X, state, recs, e->w,
@@ -536,9 +539,15 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
             // ---- inter: LN -> W_ih -> LSTM over T with carried (h, c) -> Linear -> +res ------------
             l = LstmArgs{};
             l.gx = GX; l.gx_ld = 256; l.out = Y; l.out_ld = 64; l.whh = W.whh2;
-            l.h_state = sbase + ST_BLK + (int64_t)b * BK_STRIDE + BK_H;
-            l.c_state = sbase + ST_BLK + (int64_t)b * BK_STRIDE + BK_C;
-            l.hc_outer_stride = ss;
+            if constexpr (std::is_same_v<Map, Records>) {      // the copy gather_h_kernel made of the listed records' (h, c)
+                l.h_state = HG + (int64_t)b * B * FC;
+                l.c_state = CG + (int64_t)b * B * FC;
+                l.hc_outer_stride = FC;
+            } else {
+                l.h_state = sbase + ST_BLK + (int64_t)b * BK_STRIDE + BK_H;
+                l.c_state = sbase + ST_BLK + (int64_t)b * BK_STRIDE + BK_C;
+                l.hc_outer_stride = ss;
+            }
             l.nseq = B * NF; l.L = T; l.inner_count = NF; l.outer_stride = (int64_t)T * NF; l.inner_stride = 1;
             l.step_stride = NF; l.ndir = 1;
             if (tc_fused_lstm(e, l)) {
@@ -561,6 +570,11 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
                 CK(lstm_any(e, l, st, pdl));
             }
             MARK("lstm_inter");
+            if constexpr (std::is_same_v<Map, Records>) {
+                if (b == e->n_blocks - 1)
+                    CK(launch_k(false, scatter_hc_kernel, dim3((unsigned)((hc4 + 255) / 256)), dim3(256), 0, st, state, recs,
+                                e->n_blocks, B, (const float*)HG, (const float*)CG));
+            }
             if (tc) {
                 if (int rc = tc_rows_gemm(e, b, PL_L2, Y, 64, 64, 64, nullptr, nullptr, W.bl2, nullptr, X, X, 64, rows, st)) return rc;
             } else {
@@ -574,7 +588,7 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
         }
         // ---- attention --------------------------------------------------------------------------
         if (T > 1) {
-            CK(launch_k(pdl, kv_gather_kernel, dim3(ATT - 1, B * NHEAD), dim3(128), 0, st, (const float*)state, ss, b, KALL,
+            CK(launch_k(pdl, kv_gather_kernel_t<Map>, dim3(ATT - 1, B * NHEAD), dim3(128), 0, st, (const float*)state, recs, b, KALL,
                         VALL, T));
             MARK("kv_gather");
         }
@@ -1241,14 +1255,23 @@ int l2h_sep_forward_active(void* handle, const float* x, int64_t xbs, int64_t xc
 int l2h_sep_forward_slots(void* handle, const float* x, int64_t xbs, int64_t xcs, int32_t x_len, const float* emb,
                           void* state, int32_t state_batch, const int32_t* slots_dev, int32_t n, float* y, int64_t ybs,
                           int64_t ycs, int32_t y_len, void* ws, size_t ws_bytes, uint32_t flags, void* stream) {
+    return l2h_sep_forward_slots_frames(handle, x, xbs, xcs, x_len, emb, state, state_batch, slots_dev, n, 1, y, ybs, ycs,
+                                        y_len, ws, ws_bytes, flags, stream);
+}
+
+int l2h_sep_forward_slots_frames(void* handle, const float* x, int64_t xbs, int64_t xcs, int32_t x_len, const float* emb,
+                                 void* state, int32_t state_batch, const int32_t* slots_dev, int32_t n, int32_t frames,
+                                 float* y, int64_t ybs, int64_t ycs, int32_t y_len, void* ws, size_t ws_bytes,
+                                 uint32_t flags, void* stream) {
     SepEngine* e = static_cast<SepEngine*>(handle);
     if (!e || !x || !emb || !state || !y || !ws || !slots_dev) return fail(1, "null argument");
     if (state_batch <= 0 || n <= 0 || n > state_batch)
         return fail(1, "a slot list needs 0 < n <= state_batch (n = " + std::to_string(n) + ", state_batch = " +
                            std::to_string(state_batch) + ")");
+    if (frames <= 0) return fail(1, "a slot-list call needs frames > 0 (frames = " + std::to_string(frames) + ")");
     if (flags & L2H_FLAG_TAPS) return fail(1, "a slot list cannot be combined with L2H_FLAG_TAPS");
     if (int rc_dev = check_device(e)) return rc_dev;
-    ChainArgs a{x, xbs, xcs, x_len, emb, static_cast<float*>(state), y, ybs, ycs, y_len, n, 1,
+    ChainArgs a{x, xbs, xcs, x_len, emb, static_cast<float*>(state), y, ybs, ycs, y_len, n, frames,
                 static_cast<float*>(ws), ws_bytes, flags & ~L2H_FLAG_GRAPH, 0};
     a.slots = slots_dev;
     a.state_batch = state_batch;

@@ -460,12 +460,13 @@ __device__ void spk_gate_cta(const float* __restrict__ emb, float* __restrict__ 
 // ------------------------------------------------------------------------------------------
 // K/V history -> linear scratch for multi-frame calls.  Kall[b*4+h][0..48] = ring slots of frames
 // pos-49 .. pos-1 of stream b's clock (frames before its start are zero = the reference's zero-initialised K_buf/V_buf).
-__global__ void kv_gather_kernel(const float* __restrict__ state, int64_t sstride, int blk,
-                                 float* __restrict__ Kall, float* __restrict__ Vall, int T) {
+template <class Map>
+__global__ void kv_gather_kernel_t(const float* __restrict__ state, Map recs, int blk,
+                                   float* __restrict__ Kall, float* __restrict__ Vall, int T) {
     griddep_launch();
     griddep_wait();
     const int i = blockIdx.x, bh = blockIdx.y, b = bh / NHEAD, h = bh % NHEAD;
-    const float* rec = stream_rec(state, sstride, b);
+    const float* rec = stream_rec(state, recs, b);
     const long long fr = rec_pos(rec) - (ATT - 1) + i;
     const int slot = (int)(((fr % RING) + RING) % RING);
     const float* sb = rec + ST_BLK + (int64_t)blk * BK_STRIDE;
@@ -1598,11 +1599,14 @@ lstm_cell_rows_kernel_t(const float* __restrict__ gates, float* __restrict__ sta
     Hout[i] = h;
 }
 
-// Slot-list calls in the tensor-core form: the inter-step GEMM reads the previous h through a strided tensor map over the
-// records, which a slot list cannot express.  Once per call, before any block's cell update, this copies the h of every
-// block of every row's record to Hg[blk][row][f][c] for the GEMM to read instead.  One thread per float4.
+// Slot-list calls read the carried inter-LSTM state of their records through a base pointer and a stride in two places,
+// and a slot list cannot be expressed that way: the one-hop tensor-core chain's inter-step GEMM (a strided tensor map over
+// the records' h) and the recurrence over T of multi-hop calls (LstmArgs::h_state / c_state).  Once per call, before any
+// block reads them, this copies the h (and, with Cg, the c) of every block of every row's record to Hg[blk][row][f][c]
+// (Cg alike) for those to use instead.  One thread per float4.
 __global__ void __launch_bounds__(256)
-gather_h_kernel(const float* __restrict__ state, Records recs, int n_blocks, int n_streams, float* __restrict__ Hg) {
+gather_h_kernel(const float* __restrict__ state, Records recs, int n_blocks, int n_streams, float* __restrict__ Hg,
+                float* __restrict__ Cg) {
     constexpr int PER = FC / 4;                        // float4s of one block's h
     const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
     if (i >= (int64_t)n_blocks * n_streams * PER) return;
@@ -1610,6 +1614,24 @@ gather_h_kernel(const float* __restrict__ state, Records recs, int n_blocks, int
     const int b = row % n_streams, blk = row / n_streams;
     const float* h = stream_rec(state, recs, b) + ST_BLK + (int64_t)blk * BK_STRIDE + BK_H;
     reinterpret_cast<float4*>(Hg)[i] = reinterpret_cast<const float4*>(h)[k];
+    if (Cg != nullptr) reinterpret_cast<float4*>(Cg)[i] = reinterpret_cast<const float4*>(h + (BK_C - BK_H))[k];
+}
+
+// Multi-hop slot-list calls: after the last block's recurrence, the new (h, c) that gather_h_kernel's copy carried through
+// the call go back to the records of the rows that store (an entry outside the state stores nothing).  One thread per float4.
+__global__ void __launch_bounds__(256)
+scatter_hc_kernel(float* __restrict__ state, Records recs, int n_blocks, int n_streams, const float* __restrict__ Hg,
+                  const float* __restrict__ Cg) {
+    constexpr int PER = FC / 4;
+    const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    if (i >= (int64_t)n_blocks * n_streams * PER) return;
+    const int k = (int)(i % PER), row = (int)(i / PER);
+    const int b = row % n_streams, blk = row / n_streams;
+    const RowRecord r = row_record(recs, nullptr, b);
+    if (!r.stores) return;
+    float* h = state + r.off + ST_BLK + (int64_t)blk * BK_STRIDE + BK_H;
+    reinterpret_cast<float4*>(h)[k] = reinterpret_cast<const float4*>(Hg)[i];
+    reinterpret_cast<float4*>(h + (BK_C - BK_H))[k] = reinterpret_cast<const float4*>(Cg)[i];
 }
 
 // the dense forms (call row b = record b); the `_t<Records>` forms serve slot-list calls (l2h_sep_forward_slots)
@@ -1624,5 +1646,6 @@ constexpr auto back_kernel = back_kernel_t<int64_t>;
 constexpr auto back_many_kernel = back_many_kernel_t<int64_t>;
 constexpr auto ln_frame_res_kernel = ln_frame_res_kernel_t<int64_t>;
 constexpr auto lstm_cell_rows_kernel = lstm_cell_rows_kernel_t<int64_t>;
+constexpr auto kv_gather_kernel = kv_gather_kernel_t<int64_t>;
 
 }  // namespace l2h

@@ -415,7 +415,7 @@ class Net(nn.Module):
 
     def _run(self, x, embed, state, frames, out_len, flags=0, active=None, slots=None):
         """x [B,M,n] (any length; samples beyond n read as zero), embed [B,256], active: [B] uint8 device mask or None,
-        slots: [B] int32 device list of the state's records the rows advance (one-hop calls) or None."""
+        slots: [B] int32 device list of the state's records the rows advance by `frames` hops, or None."""
         self._require_cuda(x)
         dev = x.device
         self._sync_weights(dev)
@@ -429,10 +429,10 @@ class Net(nn.Module):
         L, st = _cabi.lib(), torch.cuda.current_stream(dev).cuda_stream
         with torch.cuda.device(dev):
             if slots is not None:
-                _cabi.check_args(L.l2h_sep_forward_slots(
+                _cabi.check_args(L.l2h_sep_forward_slots_frames(
                     self._engine(), x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], embed.data_ptr(),
-                    state.buf.data_ptr(), state.batch, slots.data_ptr(), Bsz, y.data_ptr(), y.stride(0), y.stride(1),
-                    out_len, ws.data_ptr(), ws.numel(), flags, st))
+                    state.buf.data_ptr(), state.batch, slots.data_ptr(), Bsz, frames, y.data_ptr(), y.stride(0),
+                    y.stride(1), out_len, ws.data_ptr(), ws.numel(), flags, st))
             else:
                 _cabi.check(L.l2h_sep_forward_active(
                     self._engine(), x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], embed.data_ptr(),
@@ -509,6 +509,28 @@ class Net(nn.Module):
             active = self._active_mask(active, x.device, x.shape[0])
         y = self._run(x, embed, input_state, frames, out_len, active=active, slots=slots)
         return y, input_state
+
+    def advance_slots(self, x, embed, state, slots):
+        """Advance record slots[i] of `state` by T hops with row i of x [n, M, 128*T + 64] (the pad=False shape) and
+        embed [n, 256]; returns y [n, S, 128*T].  A listener whose chunks arrived late catches up its backlog of T hops
+        in one call: the T hops' BiLSTMs run side by side, as in a dense multi-hop predict.  Every row advances by the
+        same T, so listeners with different backlogs go in different calls.
+
+        `slots` is checked as for predict(slots=): n distinct ints in [0, state.batch) (a sequence or CPU tensor, checked
+        and uploaded), or a CUDA int32 tensor used in place, where an entry outside [0, state.batch) marks a row that
+        stores nothing for all of its hops.  predict(slots=) remains the one-hop form."""
+        hop, la = self.stft_chunk_size, self.stft_pad_size
+        if x.dim() != 3:
+            raise ValueError(f"advance_slots needs x of shape [n, channels, {hop}*T+{la}], got {tuple(x.shape)}")
+        n = x.shape[-1]
+        if (n - la) % hop != 0 or n < hop + la:
+            raise ValueError(f"advance_slots needs {hop}*T+{la} samples per row, got {n}")
+        if not isinstance(state, SepState):
+            raise TypeError("state must come from Net.init_buffers()")
+        frames = (n - la) // hop
+        self._require_cuda(x)
+        slots = self._slot_list(slots, x.device, x.shape[0], state.batch)
+        return self._run(x, embed, state, frames, frames * hop, slots=slots)
 
     def forward(self, x, embeds, input_state=None, pad=True):
         """Reference net.py:68-76.  x [B,M,N]; embeds [B,1,256] -> [B,S,N]."""
