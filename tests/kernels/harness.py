@@ -70,12 +70,24 @@ class SepFrontBack(ctypes.Structure):
                [("gen", ctypes.c_int32)] + [(n, ctypes.c_void_p) for n in ("ln1_g", "ln1_b", "wih1_t", "b1")]
 
 
+class EmbWeights(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_void_p) for n in ("dft", "wc", "bc", "gn_g", "gn_b", "lnh_g", "lnh_b")]
+
+
+class EmbBlock(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_void_p) for n in ("gq", "bq", "gk", "bk", "gv", "bv", "wp_t", "bp", "slope_p", "gp", "bpn")]
+
+
 MIRRORS = {"kh_sizeof_asource": ASource, "kh_sizeof_gemm": Gemm, "kh_sizeof_plan": Plan, "kh_sizeof_lstm": Lstm,
-           "kh_sizeof_sep_weights": SepWeights, "kh_sizeof_sep_front_back": SepFrontBack}
+           "kh_sizeof_sep_weights": SepWeights, "kh_sizeof_sep_front_back": SepFrontBack,
+           "kh_sizeof_emb_weights": EmbWeights, "kh_sizeof_emb_block": EmbBlock}
+EMBED_SYMBOLS = ("kh_embed_layout", "kh_estd", "kh_efront", "kh_egn_apply", "kh_eqkv_ln", "kh_softmax_rows",
+                 "kh_eattn_out_grid", "kh_eattn_out", "kh_ehead", "kh_einter_mask", "kh_eput_lens")
 SYMBOLS = ("kh_gemm", "kh_gemm_plan", "kh_split_planes", "kh_lstm", "kh_launch_count", "kh_sep_layout", "kh_qkv",
            "kh_qkv_many", "kh_kv_gather", "kh_attention", "kh_attn_out", "kh_ln_frame_res",
            "kh_attn_cluster_resident", "kh_front", "kh_front_many", "kh_front_many_geometry", "kh_front1", "kh_back",
-           "kh_back_many", "kh_back_many_geometry") + tuple(MIRRORS)
+           "kh_back_many", "kh_back_many_geometry") + EMBED_SYMBOLS + tuple(MIRRORS)
+EMBED_LAYOUT_NAMES = ("NFFT", "HOP", "NF", "CH", "QK", "VDIM", "FC", "NQKV", "DFT_LD", "EAOUT_SMEM", "LENS_PER_LAUNCH")
 
 ATTN_FORMS = {"query": 0, "tile": 1, "cluster": 2}
 SEP_LAYOUT_NAMES = ("RING", "QK_LD", "QK_DIM", "V_DIM", "ATT", "ST_GATE", "ST_BLK", "BK_K", "BK_V", "BK_H", "BK_C",
@@ -124,6 +136,20 @@ def lib():
         for s in ("kh_front_many_geometry", "kh_back_many_geometry"):
             getattr(L, s).restype = None
             getattr(L, s).argtypes = [I, I, IP, IP]
+        EW, EB = ctypes.POINTER(EmbWeights), ctypes.POINTER(EmbBlock)
+        sigs.update({
+            "kh_embed_layout": [ctypes.POINTER(ctypes.c_int64)],
+            "kh_estd": [P, I, P, P, I, P],
+            "kh_efront": [EW, P, I, P, P, P, P, I, I, P],
+            "kh_egn_apply": [EW, P, P, I64, I64, P, P],
+            "kh_eqkv_ln": [EB, P, P, P, P, I64, I64, I, I, I, P],
+            "kh_softmax_rows": [P, I64, I, I, I64, I, P, P],
+            "kh_eattn_out_grid": [I, I],
+            "kh_eattn_out": [EB, P, P, I, I, I, I, P],
+            "kh_ehead": [EW, P, P, I, I, P, P],
+            "kh_einter_mask": [P, P, I, I, P],
+            "kh_eput_lens": [P, P, I, P],
+        })
         for s, args in sigs.items():
             getattr(L, s).restype = ctypes.c_int
             getattr(L, s).argtypes = args
@@ -568,3 +594,331 @@ def unpack_front_back(p, prefix="tfgridnet."):
             prefix + "embed_to_feats_proj.0.weight": p["we"], prefix + "embed_to_feats_proj.0.bias": p["be"],
             prefix + "embed_to_feats_proj.1.weight": p["lne_g"], prefix + "embed_to_feats_proj.1.bias": p["lne_b"],
             prefix + "deconv.weight": p["wd"].reshape(CH, 4, 3, 3), prefix + "deconv.bias": p["bd"]}
+
+
+# ---- the enrollment network's own kernels (embed_kernels.cuh; tfgridnet.py:100-127, oracle/restate.py::embed_forward
+# and embed_block) ----------------------------------------------------------------------------------------------------
+# Activations [T][F = 65][C = 64] per utterance.  An utterance of n own samples has T_b = 1 + n // 64 frames; frames
+# t >= T_b of a padded batch are padding.  Every reference takes float64 copies of the kernel's fp32 inputs and returns,
+# next to every value, an element-wise bound on the kernel's fp32 rounding (u = 2^-24 per rounding, u sqrt(n) sum |terms|
+# for a sum of n terms, input bounds carried through).  The keyword flags are the mutants: plausible kernel mistakes.
+E_NFFT, E_HOP, E_NF, E_CH, E_NH, E_QE, E_VD = 128, 64, 65, 64, 4, 8, 16
+E_QK, E_VDIM, E_FC, E_NQKV, E_DFT_LD, E_LENS_PER_LAUNCH = 520, 1040, 4160, 128, 132, 1000
+E_PAD_GATES = (float("-inf"), float("-inf"), 0.0, 0.0)      # (i, f, g, o) of a padded inter window
+
+
+def embed_layout():
+    """kh_embed_layout as {name: value} (EMBED_LAYOUT_NAMES; EAOUT_SMEM in bytes)"""
+    out = (ctypes.c_int64 * 16)()
+    n = lib().kh_embed_layout(out)
+    return dict(zip(EMBED_LAYOUT_NAMES, list(out)[:n]))
+
+
+def estd(x, N, lens, inv_std, B):
+    return lib().kh_estd(ptr(x), N, ptr(lens), ptr(inv_std), B, stream())
+
+
+def efront(w, x, N, lens, inv_std, X, gn_sums, B, T):
+    return lib().kh_efront(ctypes.byref(w), ptr(x), N, ptr(lens), ptr(inv_std), ptr(X), ptr(gn_sums), B, T, stream())
+
+
+def egn_apply(w, X, gn_sums, per_b, total4, lens):
+    return lib().kh_egn_apply(ctypes.byref(w), ptr(X), ptr(gn_sums), per_b, total4, ptr(lens), stream())
+
+
+def eqkv_ln(w, QKV, Qn, Kp, Vp, k_plane, v_plane, B, T, Tp):
+    return lib().kh_eqkv_ln(ctypes.byref(w), ptr(QKV), ptr(Qn), ptr(Kp), ptr(Vp), k_plane, v_plane, B, T, Tp, stream())
+
+
+def softmax_rows(S, ld, n, rows_per_z, z_stride, Z, lens):
+    return lib().kh_softmax_rows(ptr(S), ld, n, rows_per_z, z_stride, Z, ptr(lens), stream())
+
+
+def eattn_out_grid(T, B):
+    """the engine's eattn_out_kernel grid: min(T B, 4 CTAs per SM)"""
+    return lib().kh_eattn_out_grid(T, B)
+
+
+def eattn_out(w, O, X, T, Tp, n_frames, grid):
+    return lib().kh_eattn_out(ctypes.byref(w), ptr(O), ptr(X), T, Tp, n_frames, grid, stream())
+
+
+def ehead(w, HD, out, B, T, lens):
+    return lib().kh_ehead(ctypes.byref(w), ptr(HD), ptr(out), B, T, ptr(lens), stream())
+
+
+def einter_mask(gx, lens, B, steps):
+    return lib().kh_einter_mask(ptr(gx), ptr(lens), B, steps, stream())
+
+
+def eput_lens(dst, lens_host, n):
+    arr = (ctypes.c_int32 * len(lens_host))(*lens_host)
+    return lib().kh_eput_lens(ptr(dst), arr, n, stream())
+
+
+def e_frames(n):
+    return 1 + n // E_HOP
+
+
+def _ln_bound64(y, g, b, chain, ye=None, dims=(-1,)):
+    """LayerNorm (biased variance, eps 1e-5 inside the sqrt) of y over `dims`, and the bound on a kernel that computes it
+    with fp32 two-pass statistics whose longest rounding chain is `chain` (the per-thread sums plus the reduction tree),
+    rsqrtf (2 ulp = 4 u), the final (y - mu) rs g + b (3 roundings and |b|) and one more rounding for a residual add.
+    ye: bounds on the inputs, carried through as in gate64 (|g| (ye + mean ye) + |g xh| mean ye) / sigma."""
+    mu = y.mean(dims, keepdim=True)
+    sd = torch.sqrt(((y - mu) ** 2).mean(dims, keepdim=True) + 1e-5)
+    xh = (y - mu) / sd
+    out = xh * g + b
+    gx = (g * xh).abs()
+    bound = U32 * ((0.5 * chain + 12) * gx + chain * y.abs().mean(dims, keepdim=True) / sd * g.abs() + 2 * b.abs())
+    if ye is not None:
+        m = ye.mean(dims, keepdim=True)
+        bound = bound + (g.abs() * (ye + m) + gx * m) / sd
+    return out, bound
+
+
+def estd64(x, n, unbiased=True, mic0_only=False):
+    """1 / std over the utterance's own 2n samples of both mics (x [2][>= n]), unbiased (tfgridnet.py:109-110), and its
+    bound: the kernel sums in double, so one rounding to fp32.  Mutants: unbiased=False, mic0_only."""
+    v = (x[:1, :n] if mic0_only else x[:, :n]).double().reshape(-1)
+    inv = 1.0 / v.std(unbiased=unbiased)
+    return inv, inv * (U32 + 1e-12)
+
+
+def dft_table64(symmetric_hann=False):
+    """[128][130]: window[n] (cos | -sin)(2 pi k n / 128), k = 0..64, with the periodic Hann window of torch.stft
+    (symmetric_hann: the symmetric one, a mutant)"""
+    n = torch.arange(E_NFFT, dtype=torch.float64)
+    win = 0.5 - 0.5 * torch.cos(2 * math.pi * n / (E_NFFT - 1 if symmetric_hann else E_NFFT))
+    ang = 2 * math.pi * n[:, None] * torch.arange(E_NF, dtype=torch.float64)[None, :] / E_NFFT
+    return torch.cat([win[:, None] * torch.cos(ang), -win[:, None] * torch.sin(ang)], dim=1)
+
+
+def efront64(x, n, T, inv, Wc, bc, edge_repeat=False, reflect_at=None, symmetric_hann=False, reim_interleaved=False,
+             conv_flip_time=False):
+    """the centred STFT (reflect padding about the utterance's own last sample n - 1, no edge repeat; periodic Hann) of
+    x [2][>= n] * inv, channels [Re m0, Re m1, Im m0, Im m1], then Conv2d(4 -> 64, 3x3) zero-padded in T (frames outside
+    [0, T_b)) and in F, for the T frames of the padded layout: rows t >= T_b are exactly zero.  Wc [64][4][3][3], bc [64].
+    Returns X [T][65][64], its bound, and the GroupNorm sums (sum X, sum X^2 over the real frames) with their bounds.
+    Mutants: edge_repeat (reflect with the edge sample repeated), reflect_at (reflect at another length, e.g. N),
+    symmetric_hann, reim_interleaved ([Re m0, Im m0, Re m1, Im m1]), conv_flip_time."""
+    Tb = e_frames(n)
+    L = n if reflect_at is None else reflect_at
+    s = E_HOP * torch.arange(Tb)[:, None] - E_NFFT // 2 + torch.arange(E_NFFT)[None, :]
+    if edge_repeat:
+        s = torch.where(s < 0, -s - 1, s)
+        s = torch.where(s >= L, 2 * L - 1 - s, s)
+    else:
+        s = s.abs()
+        s = torch.where(s >= L, 2 * (L - 1) - s, s)
+    xs = x.double()[:, s] * float(inv)                                     # [2, Tb, 128]
+    D = dft_table64(symmetric_hann)
+    S, Sa = xs @ D, xs.abs() @ D.abs()                                     # [2, Tb, 130]
+    order = [0, 2, 1, 3] if reim_interleaved else [0, 1, 2, 3]
+
+    def regroup(v):
+        u = torch.stack([v[0, :, :E_NF], v[1, :, :E_NF], v[0, :, E_NF:], v[1, :, E_NF:]])[order]     # [4, Tb, 65]
+        p = torch.zeros(4, Tb + 2, E_NF + 2, dtype=torch.float64)
+        p[:, 1:Tb + 1, 1:E_NF + 1] = u
+        return p
+    # the spectrum: 128 products (x * inv and the fp32 table each add one rounding per term)
+    Up, Ua, Ue = regroup(S), regroup(Sa), regroup(Sa) * (U32 * (math.sqrt(E_NFFT) + 2))
+    W = Wc.double().flip(2) if conv_flip_time else Wc.double()
+    X = torch.zeros(T, E_NF, E_CH, dtype=torch.float64)
+    Xa = torch.zeros_like(X)
+    Xe = torch.zeros_like(X)
+    X[:Tb] += bc.double()
+    Xa[:Tb] += bc.double().abs()
+    for i in range(3):
+        for j in range(3):
+            w = W[:, :, i, j]
+            X[:Tb] += torch.einsum("ctf,oc->tfo", Up[:, i:i + Tb, j:j + E_NF], w)
+            Xa[:Tb] += torch.einsum("ctf,oc->tfo", Ua[:, i:i + Tb, j:j + E_NF], w.abs())
+            Xe[:Tb] += torch.einsum("ctf,oc->tfo", Ue[:, i:i + Tb, j:j + E_NF], w.abs())
+    Xb = Xe + U32 * math.sqrt(37) * Xa
+    r = X[:Tb]
+    sums = torch.stack([r.sum(), (r * r).sum()])
+    sums_bound = torch.stack([Xb[:Tb].sum(), (2 * r.abs() * Xb[:Tb] + Xb[:Tb] ** 2).sum()]) + 1e-12 * sums.abs()
+    return dict(X=X, X_bound=Xb, sums=sums, sums_bound=sums_bound)
+
+
+def egn64(X, sums, Tb, g, b, padded_count=False, unbiased=False):
+    """GroupNorm(1 group) of one utterance X [T][65][64] from its sums (sum X, sum X^2 over the real frames): population
+    variance over T_b 65 64 values, eps 1e-5, affine per channel; frames t >= T_b come back exactly as they are.  The
+    kernel forms mean and variance in double and rounds them to fp32 once, then 4 fp32 roundings.
+    Mutants: padded_count (count T 65 64), unbiased (variance over count - 1)."""
+    X = X.double()
+    T = X.shape[0]
+    cnt = float((T if padded_count else Tb) * E_FC)
+    mu = float(sums[0]) / cnt
+    var = float(sums[1]) / cnt - mu * mu
+    if unbiased:
+        var = var * cnt / (cnt - 1)
+    rs = 1.0 / math.sqrt(var + 1e-5)
+    out, bound = X.clone(), torch.zeros_like(X)
+    xh = (X[:Tb] - mu) * rs
+    gg, bb = g.double(), b.double()
+    out[:Tb] = xh * gg + bb
+    bound[:Tb] = U32 * (5 * (xh * gg).abs() + abs(mu) * rs * gg.abs() + 2 * bb.abs())
+    return out, bound
+
+
+def eqkv_ln64(QKV, gq, bq, gk, bk, gv, bv, per_bin=False, heads_transposed=False, swap_qk_gains=False):
+    """per head, the LayerNorm over (f, e) of the PReLU'd projections QKV [T][65][128] (columns Q h*8 + e | 32 + K h*8 + e
+    | 64 + V h*16 + c), element f*d + e; gains / biases [4][65 d].  Returns {"Q", "K", "V"}: ([4][T][65 d], bound).
+    The kernel's statistics: each lane sums 65 d / 32 values, then a 5-level warp tree.
+    Mutants: per_bin (a LayerNorm over each bin's d values), heads_transposed (column e*4 + h), swap_qk_gains."""
+    P = QKV.double()
+    T = P.shape[0]
+    if swap_qk_gains:
+        (gq, bq), (gk, bk) = (gk, bk), (gq, bq)
+    out = {}
+    for name, d, c0, g, b in (("Q", E_QE, 0, gq, bq), ("K", E_QE, 32, gk, bk), ("V", E_VD, 64, gv, bv)):
+        cols = P[:, :, c0:c0 + E_NH * d]
+        y = (cols.view(T, E_NF, d, E_NH).permute(3, 0, 1, 2) if heads_transposed
+             else cols.view(T, E_NF, E_NH, d).permute(2, 0, 1, 3))                    # [4, T, 65, d]
+        g4, b4 = g.double().view(E_NH, 1, E_NF, d), b.double().view(E_NH, 1, E_NF, d)
+        n = E_NF * d
+        v, bound = _ln_bound64(y, g4, b4, n / 32 + 5, dims=(-1,) if per_bin else (-2, -1))
+        out[name] = (v.reshape(E_NH, T, n), bound.reshape(E_NH, T, n))
+    return out
+
+
+def softmax_row_lens(Z, rows_per_z, lens, n, by_mod=False):
+    """the column count of each of the Z rows_per_z rows of softmax_rows_kernel: the own frame count of utterance z / 4
+    (lens None: n).  by_mod: utterance z % 4 (a mutant)."""
+    z = torch.arange(Z * rows_per_z) // rows_per_z
+    if lens is None:
+        return torch.full_like(z, n)
+    u = z % E_NH if by_mod else z // E_NH
+    return torch.tensor([e_frames(int(lens[int(i)])) for i in u])
+
+
+def softmax64(S, ncols, zero_pad=True):
+    """softmax over the first ncols[r] columns of each row of S [rows][ld]; columns ncols[r] .. ld - 1 become exactly 0
+    (zero_pad=False: left as they are, a mutant).  Bound of each weight p: its own __expf error (2 + 1.2 |s - max| ulp,
+    plus the rounding of s - max) and the weighted mean of all of them (through the sum), plus the sum's rounding
+    (n / 128 terms per thread and a 10-level tree) and the reciprocal and product."""
+    S = S.double()
+    ncols = torch.as_tensor(ncols)
+    out = S.clone() if not zero_pad else torch.zeros_like(S)
+    bound = torch.zeros_like(S)
+    for n in ncols.unique().tolist():
+        r = (ncols == n).nonzero()[:, 0]
+        s = S[r, :n]
+        d = s - s.max(1, keepdim=True).values
+        p = torch.softmax(s, 1)
+        re = U32 * (6 + 4.4 * d.abs())
+        out[r, :n] = p
+        bound[r, :n] = p * (re + (p * re).sum(1, keepdim=True) + U32 * (n / 128 + 14)) + 2.0 ** -126
+    return out, bound
+
+
+def eattn_out64(O, X, wp_t, bp, slope, gp, bpn, heads_cf=False, ignore_slope=False, ln_per_bin=False):
+    """the attention output of one utterance's frames: gather heads O [T][4][1040] (feature f*16 + c) to channel h*16 + c
+    of bin f, Linear 64 -> 64 (wp_t [64 in][64 out]) + bias, scalar PReLU, LayerNorm over the frame's 4160 values in
+    (f*64 + c) order (gp, bpn [4160]), then the residual X [T][65][64].  Returns (X', bound).
+    Mutants: heads_cf (channel c*4 + h), ignore_slope (no PReLU), ln_per_bin (LayerNorm over C per bin)."""
+    T = O.shape[0]
+    z = O.double().view(T, E_NH, E_NF, E_VD).permute(0, 2, 1, 3)               # [T, 65, 4, 16]
+    if heads_cf:
+        z = z.transpose(2, 3)
+    Z = z.reshape(T, E_NF, E_CH)
+    W, bpd = wp_t.double(), bp.double()
+    P = Z @ W + bpd
+    a = 1.0 if ignore_slope else float(slope)
+    Pe = U32 * math.sqrt(65) * (Z.abs() @ W.abs() + bpd.abs()) * max(1.0, abs(a))
+    P = prelu64(P, a)
+    g, b = gp.double().view(E_NF, E_CH), bpn.double().view(E_NF, E_CH)
+    if ln_per_bin:
+        y, yb = _ln_bound64(P, g, b, 64 / 256 + 10, ye=Pe, dims=(-1,))
+    else:
+        y, yb = _ln_bound64(P, g, b, E_FC / 256 + 10, ye=Pe, dims=(-2, -1))
+    out = X.double() + y
+    return out, yb + U32 * out.abs()
+
+
+def ehead64(HD, Tb, g, b, div_T=False, mean_before_ln=False):
+    """LayerNorm(256) of each of the utterance's own T_b frames of HD [T][256], then their mean (tfgridnet.py:124-125),
+    and its bound: the mean of the frames' LayerNorm bounds (8 values per lane, 5-level tree) plus the sum's rounding
+    (T_b / 8 terms per warp, 8 warps, the division).  Mutants: div_T (the sum over T_b frames divided by the padded T),
+    mean_before_ln (the LayerNorm of the mean frame)."""
+    H = HD.double()
+    T = H.shape[0]
+    gd, bd = g.double(), b.double()
+    if mean_before_ln:
+        y, yb = _ln_bound64(H[:Tb].mean(0), gd, bd, 13)
+        return y, yb
+    y, yb = _ln_bound64(H[:Tb], gd, bd, 13)
+    out = y.sum(0) / (T if div_T else Tb)
+    bound = yb.sum(0) / Tb + U32 * (math.ceil(Tb / 8) + 9) * y.abs().sum(0) / Tb
+    return out, bound
+
+
+def einter_mask_expected(gx, lens, steps, start=3, fwd_only=False, pad=E_PAD_GATES):
+    """what einter_mask_kernel leaves in gx [(b*65 + f)][steps][512] (columns dir*256 + j*4 + q, q = i, f, g, o): every
+    unit's four gates of the windows s >= T_b - start of each (b, f) sequence become pad, in both directions; every other
+    float is bit-unchanged.  Mutants: start = 4 or 2 (one window early / late), fwd_only, pad in another gate order."""
+    out = gx.clone().view(len(lens), E_NF, steps, 2, 64, 4)
+    p = torch.tensor(pad, dtype=gx.dtype)
+    for b, n in enumerate(lens):
+        s0 = max(0, e_frames(int(n)) - start)
+        if fwd_only:
+            out[b, :, s0:, 0] = p
+        else:
+            out[b, :, s0:] = p
+    return out.view(gx.shape)
+
+
+def pack_embed(sd, n_blocks=1):
+    """the weights the enrollment kernels read, in the engine's packed layouts (embed_engine.cu: build_layout), as fp32:
+    wc [64][36], bc, gn_g, gn_b, lnh_g, lnh_b, and per block i: wqkv_t [64][128] (columns Q h*8 + e | 32 + K h*8 + e |
+    64 + V h*16 + c), bqkv, slope_qkv [128], gq / bq / gk / bk [4][520] and gv / bv [4][1040] in (f*d + e) order, wp_t
+    [64 in][64 out], bp, slope_p [1], gp / bpn [4160] in (f*64 + c) order (keys "i.name")"""
+    g = lambda k: sd[k].detach().float()
+    out = dict(wc=g("conv.0.weight").reshape(E_CH, 36), bc=g("conv.0.bias"), gn_g=g("conv.1.weight"),
+               gn_b=g("conv.1.bias"), lnh_g=g("embed_proj.1.weight"), lnh_b=g("embed_proj.1.bias"))
+    for i in range(n_blocks):
+        p = f"blocks.{i}."
+        w = torch.zeros(E_CH, E_NQKV)
+        bias, slope = torch.zeros(E_NQKV), torch.zeros(E_NQKV)
+        ln = {k: torch.zeros(E_NH, E_NF * d) for k, d in (("gq", 8), ("bq", 8), ("gk", 8), ("bk", 8), ("gv", 16), ("bv", 16))}
+        for h in range(E_NH):
+            for nm, d, c0, gk, bk in (("Q", E_QE, h * E_QE, "gq", "bq"), ("K", E_QE, 32 + h * E_QE, "gk", "bk"),
+                                      ("V", E_VD, 64 + h * E_VD, "gv", "bv")):
+                m = f"{p}attn_conv_{nm}_{h}."
+                w[:, c0:c0 + d] = g(m + "0.weight")[:, :, 0, 0].T
+                bias[c0:c0 + d] = g(m + "0.bias")
+                slope[c0:c0 + d] = g(m + "1.weight")[0]
+                ln[gk][h] = g(m + "2.gamma")[0, :, 0, :].T.reshape(-1)
+                ln[bk][h] = g(m + "2.beta")[0, :, 0, :].T.reshape(-1)
+        out.update({f"{i}.wqkv_t": w, f"{i}.bqkv": bias, f"{i}.slope_qkv": slope})
+        out.update({f"{i}.{k}": v for k, v in ln.items()})
+        out[f"{i}.wp_t"] = g(p + "attn_concat_proj.0.weight")[:, :, 0, 0].T.contiguous()
+        out[f"{i}.bp"] = g(p + "attn_concat_proj.0.bias")
+        out[f"{i}.slope_p"] = g(p + "attn_concat_proj.1.weight").reshape(1)
+        out[f"{i}.gp"] = g(p + "attn_concat_proj.2.gamma")[0, :, 0, :].T.reshape(-1).contiguous()
+        out[f"{i}.bpn"] = g(p + "attn_concat_proj.2.beta")[0, :, 0, :].T.reshape(-1).contiguous()
+    return out
+
+
+def dft_table32(pad=float("nan")):
+    """the engine's fp32 DFT table [128][132] (build_layout: periodic Hann, cos | -sin), its 2 pad columns = pad"""
+    t = torch.full((E_NFFT, E_DFT_LD), pad, dtype=torch.float32)
+    t[:, :2 * E_NF] = dft_table64().float()
+    return t
+
+
+def eattention64(X2, pk, blk=0, **mut):
+    """the attention section of one utterance's T_b frames X2 [T_b][65][64] through the references (the Q|K|V projection,
+    Q.K^T / sqrt(520), P.V and the GEMMs in float64): eqkv_ln64 -> softmax64 -> eattn_out64; mut goes to eattn_out64"""
+    T = X2.shape[0]
+    q = lambda k: pk[f"{blk}.{k}"]
+    QKV = prelu64(X2.double() @ q("wqkv_t").double() + q("bqkv").double(), q("slope_qkv").double())
+    r = eqkv_ln64(QKV, q("gq"), q("bq"), q("gk"), q("bk"), q("gv"), q("bv"))
+    O = torch.zeros(T, E_NH, E_VDIM, dtype=torch.float64)
+    for h in range(E_NH):
+        S = r["Q"][0][h] @ r["K"][0][h].T / math.sqrt(E_QK)
+        P, _ = softmax64(S, [T] * T)
+        O[:, h] = P @ r["V"][0][h]
+    return eattn_out64(O, X2, q("wp_t"), q("bp"), q("slope_p"), q("gp"), q("bpn"), **mut)[0]

@@ -1,8 +1,10 @@
 // Test-only C entry points into the engine's tensor-core GEMM (umma::launch), LSTM recurrences (lstm.cuh,
-// tc_lstm.cuh), the separator's attention section (sep_kernels.cuh) and its front and back (sep_kernels.cuh,
-// hop_kernels.cuh), so that tests/test_umma_gemm_gpu.py, tests/test_lstm_kernels_gpu.py,
-// tests/test_attention_kernels_gpu.py and tests/test_front_back_kernels_gpu.py can drive each kernel directly with
-// arbitrary shapes and compare it element by element with a float64 reference.
+// tc_lstm.cuh), the separator's attention section (sep_kernels.cuh), its front and back (sep_kernels.cuh,
+// hop_kernels.cuh) and the enrollment network's own kernels (embed_kernels.cuh: estd, efront, egn_apply, eqkv_ln,
+// softmax_rows, eattn_out, ehead, einter_mask, eput_lens), so that tests/test_umma_gemm_gpu.py,
+// tests/test_lstm_kernels_gpu.py, tests/test_attention_kernels_gpu.py, tests/test_front_back_kernels_gpu.py and
+// tests/test_embed_kernels_gpu.py can drive each kernel directly with arbitrary shapes and compare it element by element
+// with a float64 reference.
 //
 // The argument structs below are plain C (mirrored with ctypes in the tests); every function fills the engine's own
 // descriptor and calls the engine's own launcher (or launches the kernel with the engine's own geometry).  Built by
@@ -13,6 +15,7 @@
 #include "tc_lstm.cuh"
 #include "sep_kernels.cuh"
 #include "hop_kernels.cuh"
+#include "embed_kernels.cuh"
 
 #define KH_API extern "C" __attribute__((visibility("default")))
 
@@ -434,4 +437,128 @@ KH_API int kh_back_many(const KhSepFrontBack* w, const float* X, float* y, int64
     return (int)launch_cluster(false, dim3(BACK_CL, 1, 1), back_many_kernel, dim3(BACK_CL * n_cl, 1), dim3(256), BACK_MANY_SMEM,
                                static_cast<cudaStream_t>(stream), X, y, y_bstride, y_cstride, y_len, state, sstride, to_sep(*w), T,
                                pos_rel, chunk, n_chunks, B, active);
+}
+
+// ---- the enrollment network's own kernels (embed_kernels.cuh) --------------------------------------------------------
+// Launched with embed_forward_impl's geometry.  Every `lens` (device, [B] int32) may be null: the equal-length path.
+// The fields of EmbWeights that estd / efront / egn_apply / ehead read, and of EmbBlockWeights that eqkv_ln and eattn_out
+// read.
+struct KhEmbWeights {
+    const float *dft, *wc, *bc, *gn_g, *gn_b, *lnh_g, *lnh_b;
+};
+
+struct KhEmbBlock {
+    const float *gq, *bq, *gk, *bk, *gv, *bv;
+    const float *wp_t, *bp, *slope_p, *gp, *bpn;
+};
+
+static emb::EmbWeights to_emb(const KhEmbWeights& k) {
+    emb::EmbWeights w{};
+    w.dft = k.dft; w.wc = k.wc; w.bc = k.bc; w.gn_g = k.gn_g; w.gn_b = k.gn_b; w.lnh_g = k.lnh_g; w.lnh_b = k.lnh_b;
+    return w;
+}
+
+static emb::EmbBlockWeights to_emb_block(const KhEmbBlock& k) {
+    emb::EmbBlockWeights w{};
+    w.gq = k.gq; w.bq = k.bq; w.gk = k.gk; w.bk = k.bk; w.gv = k.gv; w.bv = k.bv;
+    w.wp_t = k.wp_t; w.bp = k.bp; w.slope_p = k.slope_p; w.gp = k.gp; w.bpn = k.bpn;
+    return w;
+}
+
+KH_API int kh_sizeof_emb_weights() { return (int)sizeof(KhEmbWeights); }
+KH_API int kh_sizeof_emb_block() { return (int)sizeof(KhEmbBlock); }
+
+// NFFT, HOP, NF, CH, QK, VDIM, FC, NQKV, DFT_LD, EAOUT_SMEM, LENS_PER_LAUNCH; returns the count written (11)
+KH_API int kh_embed_layout(int64_t* out) {
+    const int64_t v[] = {emb::NFFT, emb::HOP, emb::NF, emb::CH, emb::QK, emb::VDIM, emb::FC, emb::NQKV, emb::DFT_LD,
+                         (int64_t)emb::EAOUT_SMEM, emb::LENS_PER_LAUNCH};
+    const int n = (int)(sizeof(v) / sizeof(v[0]));
+    for (int i = 0; i < n; ++i) out[i] = v[i];
+    return n;
+}
+
+// estd_kernel: grid B, 256 threads; x [B][2][N]
+KH_API int kh_estd(const float* x, int N, const int32_t* lens, float* inv_std, int B, void* stream) {
+    if (B <= 0 || N <= 0) return (int)cudaErrorInvalidValue;
+    return (int)launch_k(false, emb::estd_kernel, dim3(B), dim3(256), 0, static_cast<cudaStream_t>(stream), x, N, lens, inv_std);
+}
+
+// efront_kernel: grid (T, B), 256 threads; the caller zeroes gn_sums [B][2] (double)
+KH_API int kh_efront(const KhEmbWeights* w, const float* x, int N, const int32_t* lens, const float* inv_std, float* X,
+                     double* gn_sums, int B, int T, void* stream) {
+    if (B <= 0 || T <= 0) return (int)cudaErrorInvalidValue;
+    return (int)launch_k(false, emb::efront_kernel, dim3(T, B), dim3(256), 0, static_cast<cudaStream_t>(stream), x, N, lens,
+                         inv_std, X, gn_sums, to_emb(*w), T);
+}
+
+// egn_apply_kernel: ceil(total4 / 256) CTAs of 256 threads
+KH_API int kh_egn_apply(const KhEmbWeights* w, float* X, const double* gn_sums, int64_t per_b, int64_t total4,
+                        const int32_t* lens, void* stream) {
+    if (per_b <= 0 || total4 <= 0) return (int)cudaErrorInvalidValue;
+    return (int)launch_k(false, emb::egn_apply_kernel, dim3((unsigned)((total4 + 255) / 256)), dim3(256), 0,
+                         static_cast<cudaStream_t>(stream), X, gn_sums, per_b, total4, lens, to_emb(*w));
+}
+
+// eqkv_ln_kernel: grid (T, B), 384 threads; QKV [B][T][65][128]
+KH_API int kh_eqkv_ln(const KhEmbBlock* w, const float* QKV, float* Qn, void* Kp, void* Vp, int64_t k_plane, int64_t v_plane,
+                      int B, int T, int Tp, void* stream) {
+    if (B <= 0 || T <= 0 || Tp < T) return (int)cudaErrorInvalidValue;
+    return (int)launch_k(false, emb::eqkv_ln_kernel, dim3(T, B), dim3(384), 0, static_cast<cudaStream_t>(stream), QKV, Qn,
+                         static_cast<__nv_bfloat16*>(Kp), static_cast<__nv_bfloat16*>(Vp), k_plane, v_plane, to_emb_block(*w),
+                         T, Tp);
+}
+
+// softmax_rows_kernel: one CTA of 128 threads per row, Z * rows_per_z rows
+KH_API int kh_softmax_rows(float* S, int64_t ld, int n, int rows_per_z, int64_t z_stride, int Z, const int32_t* lens,
+                           void* stream) {
+    if (Z <= 0 || rows_per_z <= 0 || n <= 0 || ld < n) return (int)cudaErrorInvalidValue;
+    return (int)launch_k(false, emb::softmax_rows_kernel, dim3((unsigned)((int64_t)Z * rows_per_z)), dim3(128), 0,
+                         static_cast<cudaStream_t>(stream), S, ld, n, rows_per_z, z_stride, lens);
+}
+
+// the engine's eattn_out_kernel grid for (T, B)
+KH_API int kh_eattn_out_grid(int T, int B) { return (int)std::min<int64_t>((int64_t)T * B, NUM_SMS * 4); }
+
+// eattn_out_kernel with `grid` persistent CTAs over frames 0 .. n_frames-1 (frame item = b * T + t)
+KH_API int kh_eattn_out(const KhEmbBlock* w, const float* O, float* X, int T, int Tp, int n_frames, int grid, void* stream) {
+    if (T <= 0 || Tp < T || n_frames <= 0 || grid <= 0) return (int)cudaErrorInvalidValue;
+    static thread_local int configured_dev = -1;
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return (int)e;
+    if (configured_dev != dev) {
+        e = cudaFuncSetAttribute(emb::eattn_out_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)emb::EAOUT_SMEM);
+        if (e != cudaSuccess) return (int)e;
+        configured_dev = dev;
+    }
+    return (int)launch_k(false, emb::eattn_out_kernel, dim3(grid), dim3(256), emb::EAOUT_SMEM, static_cast<cudaStream_t>(stream),
+                         O, X, to_emb_block(*w), T, Tp, n_frames);
+}
+
+// ehead_kernel: grid B, 256 threads; HD [B][T][256]
+KH_API int kh_ehead(const KhEmbWeights* w, const float* HD, float* out, int B, int T, const int32_t* lens, void* stream) {
+    if (B <= 0 || T <= 0) return (int)cudaErrorInvalidValue;
+    return (int)launch_k(false, emb::ehead_kernel, dim3(B), dim3(256), 0, static_cast<cudaStream_t>(stream), HD, out, to_emb(*w),
+                         T, lens);
+}
+
+// einter_mask_kernel: grid (NF, B), 128 threads; gx [(b*NF + f)][steps][512]
+KH_API int kh_einter_mask(float* gx, const int32_t* lens, int B, int steps, void* stream) {
+    if (B <= 0 || steps <= 0 || lens == nullptr) return (int)cudaErrorInvalidValue;
+    return (int)launch_k(false, emb::einter_mask_kernel, dim3(emb::NF, B), dim3(128), 0, static_cast<cudaStream_t>(stream), gx,
+                         lens, steps);
+}
+
+// eput_lens_kernel: the host lengths lens_host[0 .. n-1] to dst, one launch per block of LENS_PER_LAUNCH, as the engine loops
+KH_API int kh_eput_lens(int32_t* dst, const int32_t* lens_host, int n, void* stream) {
+    if (n <= 0) return (int)cudaErrorInvalidValue;
+    for (int b0 = 0; b0 < n; b0 += emb::LENS_PER_LAUNCH) {
+        const int m = std::min(emb::LENS_PER_LAUNCH, n - b0);
+        emb::LensBlock blk;
+        memcpy(blk.v, lens_host + b0, sizeof(int32_t) * m);
+        const cudaError_t e = launch_k(false, emb::eput_lens_kernel, dim3(1), dim3(256), 0, static_cast<cudaStream_t>(stream),
+                                       dst + b0, blk, m);
+        if (e != cudaSuccess) return (int)e;
+    }
+    return 0;
 }

@@ -1,6 +1,8 @@
 """The kernel harness library (tests/kernels/) and the float64 references the kernel-level GPU tests
-(test_umma_gemm_gpu.py, test_lstm_kernels_gpu.py, test_attention_kernels_gpu.py, test_front_back_kernels_gpu.py) rely on.
-No device needed."""
+(test_umma_gemm_gpu.py, test_lstm_kernels_gpu.py, test_attention_kernels_gpu.py, test_front_back_kernels_gpu.py,
+test_embed_kernels_gpu.py) rely on.  The enrollment references (estd64, efront64, egn64, eqkv_ln64, softmax64,
+eattn_out64, ehead64) are pinned to oracle/restate.py; each of their mutants is shown to miss the reference by more than
+10x its bound, and einter_mask_expected's mutants to change it.  No device needed."""
 import ctypes
 import math
 
@@ -333,3 +335,137 @@ def test_front_back_packing_round_trips(tsh_params):
         assert torch.equal(v, sd[k]), k
     assert torch.equal(p["wat"][5, 100], sd["tfgridnet.enc.filterbank._filters"][100, 0, 5])
     assert torch.equal(p["wd"][7, 3, 2 * 3 + 1], sd["tfgridnet.deconv.weight"][7, 3, 2, 1])
+
+
+# ---- the enrollment network's own kernels ---------------------------------------------------------------------------
+def test_embed_layout():
+    """the constants the enrollment tests build their buffers from are the kernels' own"""
+    lay = kh.embed_layout()
+    assert lay == dict(NFFT=kh.E_NFFT, HOP=kh.E_HOP, NF=kh.E_NF, CH=kh.E_CH, QK=kh.E_QK, VDIM=kh.E_VDIM, FC=kh.E_FC,
+                       NQKV=kh.E_NQKV, DFT_LD=kh.E_DFT_LD, EAOUT_SMEM=(64 * 68 + 64 * 64 + 65 * 64) * 4,
+                       LENS_PER_LAUNCH=kh.E_LENS_PER_LAUNCH)
+
+
+def _embed_sd(embed_params, seed=0):
+    """a seeded EmbedTFGridNet's state dict with random affine parameters (the defaults are ones and zeros, under which
+    swapped or transposed gains would go unseen)"""
+    from lookoncetohear_b200 import EmbedTFGridNet
+    torch.manual_seed(seed)
+    sd = {k: v.detach().clone() for k, v in EmbedTFGridNet(**embed_params).state_dict().items()}
+    g = torch.Generator().manual_seed(seed + 1)
+    for k, v in sd.items():
+        if k.endswith((".gamma", "conv.1.weight", "embed_proj.1.weight")):
+            sd[k] = 1 + 0.3 * torch.randn(v.shape, generator=g)
+        elif k.endswith((".beta", "conv.1.bias", "embed_proj.1.bias")):
+            sd[k] = 0.3 * torch.randn(v.shape, generator=g)
+    return sd
+
+
+def _embed_front(x, n, T, sd64):
+    """estd64 -> efront64 -> egn64 of one utterance x [2][>= n]"""
+    inv, _ = kh.estd64(x, n)
+    f = kh.efront64(x, n, T, inv, sd64["conv.0.weight"], sd64["conv.0.bias"])
+    X, _ = kh.egn64(f["X"], f["sums"], kh.e_frames(n), sd64["conv.1.weight"], sd64["conv.1.bias"])
+    return X, f
+
+
+def test_embed_references_are_the_model(embed_params):
+    """the chained references reproduce oracle/restate.py::embed_forward and embed_block to 1e-12: estd64 -> efront64 ->
+    egn64 the encoder output taps["enc"], eqkv_ln64 -> softmax64 -> eattn_out64 the attention section of every block
+    (its input is embed_block's output with the attention's LayerNorm affine zeroed), ehead64 the embedding; for a batch
+    of equal lengths and for an utterance of a padded batch alone (its rows t >= T_b are exactly zero)"""
+    from oracle import restate
+    sd = _embed_sd(embed_params)
+    sd64 = restate.cast_sd(sd, torch.float64)
+    pk = kh.pack_embed(sd64, embed_params["num_blocks"])
+    g = torch.Generator().manual_seed(21)
+    N, n = 700, 450
+    x = torch.randn(2, 2, N, generator=g)
+    T = kh.e_frames(N)
+    for xb, nb in ((x, N), (x[1:2, :, :n], n)):
+        taps = {}
+        emb = restate.embed_forward(sd64, xb.double(), taps=taps)
+        for b in range(xb.shape[0]):
+            X, _ = _embed_front(x[1 if nb == n else b], nb, T, sd64)
+            Tb = kh.e_frames(nb)
+            assert torch.allclose(X[:Tb], taps["enc"][b], rtol=0, atol=1e-12)
+            assert bool((X[Tb:] == 0).all())
+            for blk in range(embed_params["num_blocks"]):
+                Xin = taps["enc"][b:b + 1] if blk == 0 else taps[f"block{blk - 1}"][b:b + 1]
+                sdz = dict(sd64)
+                p = f"blocks.{blk}.attn_concat_proj.2."
+                sdz[p + "gamma"], sdz[p + "beta"] = torch.zeros_like(sd64[p + "gamma"]), torch.zeros_like(sd64[p + "beta"])
+                X2 = restate.embed_block(sdz, f"blocks.{blk}.", Xin)[0]
+                got = kh.eattention64(X2, {k: v.double() for k, v in pk.items()}, blk)
+                assert torch.allclose(got, taps[f"block{blk}"][b], rtol=0, atol=1e-12)
+            Xl = taps[f"block{embed_params['num_blocks'] - 1}"][b]
+            HD = Xl.permute(0, 2, 1).reshape(Tb, -1) @ sd64["embed_proj.0.weight"].T + sd64["embed_proj.0.bias"]
+            out, _ = kh.ehead64(HD, Tb, sd64["embed_proj.1.weight"], sd64["embed_proj.1.bias"])
+            assert torch.allclose(out, emb[b], rtol=0, atol=1e-12)
+
+
+def _far(mut, ref, bound, k=10):
+    """mut differs from ref by more than k times the bound somewhere"""
+    return float(((mut.double() - ref.double()).abs() / bound.clamp_min(1e-300)).max()) > k
+
+
+def test_embed_mutants_differ(embed_params):
+    """every mutated reference the enrollment kernel tests use misses the reference by more than 10x its bound on a
+    small case, so their >= 10x margins cannot pass vacuously"""
+    from oracle import restate
+    sd64 = restate.cast_sd(_embed_sd(embed_params), torch.float64)
+    pk = {k: v.double() for k, v in kh.pack_embed(sd64).items()}
+    g = torch.Generator().manual_seed(22)
+    N, n = 1000, 450
+    x = torch.randn(2, N, generator=g).float()
+    inv, ib = kh.estd64(x, n)
+    for m in (dict(unbiased=False), dict(mic0_only=True)):
+        assert _far(kh.estd64(x, n, **m)[0], inv, ib), m
+    T = kh.e_frames(N)
+    Wc, bc = sd64["conv.0.weight"], sd64["conv.0.bias"]
+    ref = kh.efront64(x, n, T, inv, Wc, bc)
+    for m in (dict(edge_repeat=True), dict(reflect_at=N), dict(symmetric_hann=True), dict(reim_interleaved=True),
+              dict(conv_flip_time=True)):
+        assert _far(kh.efront64(x, n, T, inv, Wc, bc, **m)["X"], ref["X"], ref["X_bound"]), m
+    Tb = kh.e_frames(n)
+    X = torch.randn(T, kh.E_NF, kh.E_CH, generator=g).double()
+    sums = torch.stack([X[:Tb].sum(), (X[:Tb] ** 2).sum()])
+    gg, gb = sd64["conv.1.weight"], sd64["conv.1.bias"]
+    ref, bound = kh.egn64(X, sums, Tb, gg, gb)
+    assert torch.equal(ref[Tb:], X[Tb:])
+    for m in (dict(padded_count=True), dict(unbiased=True)):
+        assert _far(kh.egn64(X, sums, Tb, gg, gb, **m)[0], ref, bound), m
+    QKV = torch.randn(5, kh.E_NF, kh.E_NQKV, generator=g).double()
+    ln = [pk["0." + k] for k in ("gq", "bq", "gk", "bk", "gv", "bv")]
+    ref = kh.eqkv_ln64(QKV, *ln)
+    for m in (dict(per_bin=True), dict(heads_transposed=True), dict(swap_qk_gains=True)):
+        mut = kh.eqkv_ln64(QKV, *ln, **m)
+        assert any(_far(mut[k][0], ref[k][0], ref[k][1]) for k in "QKV"), m
+    # softmax: 4 utterances of different lengths (z % 4 picks another utterance's length for most heads)
+    lens, Tp = [450, 1000, 300, 700], 64
+    S = 3 * torch.randn(4 * kh.E_NH * T, Tp, generator=g)
+    ncols = kh.softmax_row_lens(4 * kh.E_NH, T, lens, T)
+    ref, bound = kh.softmax64(S, ncols)
+    assert _far(kh.softmax64(S, kh.softmax_row_lens(4 * kh.E_NH, T, lens, T, by_mod=True))[0], ref, bound)
+    assert _far(kh.softmax64(S, ncols, zero_pad=False)[0], ref, bound)
+    O = torch.randn(3, kh.E_NH, kh.E_VDIM, generator=g).double()
+    Xr = torch.randn(3, kh.E_NF, kh.E_CH, generator=g).double()
+    a = [pk["0." + k] for k in ("wp_t", "bp", "slope_p", "gp", "bpn")]
+    ref, bound = kh.eattn_out64(O, Xr, *a)
+    for m in (dict(heads_cf=True), dict(ignore_slope=True), dict(ln_per_bin=True)):
+        assert _far(kh.eattn_out64(O, Xr, *a, **m)[0], ref, bound), m
+    HD = torch.randn(T, 256, generator=g).double()
+    hg, hb = sd64["embed_proj.1.weight"], sd64["embed_proj.1.bias"]
+    ref, bound = kh.ehead64(HD, Tb, hg, hb)
+    for m in (dict(div_T=True), dict(mean_before_ln=True)):
+        assert _far(kh.ehead64(HD, Tb, hg, hb, **m)[0], ref, bound), m
+    # the inter mask: exact, so any change is a miss; the longest utterance is left as it is
+    steps = T - 3
+    lens = lens[:2]
+    gx = torch.randn(2 * kh.E_NF, steps, 512, generator=g)
+    ref = kh.einter_mask_expected(gx, lens, steps)
+    assert torch.equal(ref.view(2, kh.E_NF, steps, 512)[1], gx.view(2, kh.E_NF, steps, 512)[1])
+    assert bool(ref.view(2, kh.E_NF, steps, 512)[0, :, Tb - 3:, 0::4].isneginf().all())
+    assert torch.equal(ref.view(2, kh.E_NF, steps, 512)[0, :, :Tb - 3], gx.view(2, kh.E_NF, steps, 512)[0, :, :Tb - 3])
+    for m in (dict(start=4), dict(start=2), dict(fwd_only=True), dict(pad=(float("-inf"), 0.0, float("-inf"), 0.0))):
+        assert not torch.equal(kh.einter_mask_expected(gx, lens, steps, **m), ref), m
