@@ -214,7 +214,7 @@ int l2h_sep_pipeline_frames(void* handle, int32_t* frames);
  * (BiLSTM, <= 16), "pipeline_midc_lanes" (<= 3), "pipeline_qkv_lanes" (<= 4), "pipeline_attn_lanes" (<= 4),
  * "pipeline_out_lanes" (<= 4), "pipeline_front_lanes" (<= 8), "pipeline_back_lanes" (<= 6).  "pipeline_pdl": bit mask of the
  * stages launched with programmatic dependent launch (front=1, W_ih gemm=2, bilstm=4, mid_a=8, mid_b=16, mid_c=32, qkv=64,
- * attention=128, attn_out=256, back=512; default 16).  "defaults" restores all pipeline settings.  The pipeline settings never
+ * attention=128, attn_out=256, back=512; default 0).  "defaults" restores all pipeline settings.  The pipeline settings never
  * change results (bit-identical, tests/test_sep_gpu.py); "fused_tail", "bf16", "fuse_ih" and "tc_lstm_min" change rounding
  * only (gates in tests/). */
 int l2h_sep_set_option(void* handle, const char* name, int32_t value);

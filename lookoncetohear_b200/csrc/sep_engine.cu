@@ -66,7 +66,7 @@ struct SepEngine {
     int pipe_alanes = 12;    // BiLSTM (stage A) hops in flight per block (<= PIPE_LANES)
     int pipe_gemm_shape = 0; // tile shape of the pipelined W_ih GEMM (gemm.cuh: launch_rows_gemm), option "pipeline_gemm_shape"
     int pipe_midb_hops = 4;       // pipeline: consecutive hops one mid_b launch takes (<= PIPE_MIDB_MAX)
-    int pipe_pdl = 16;            // pipeline: stages launched with programmatic dependent launch (bit mask; 16 = mid_b)
+    int pipe_pdl = 0;             // pipeline: stages launched with programmatic dependent launch (bit mask; 16 = mid_b)
     int pipe_qlanes = 3;     // qkv hops in flight per block (<= PIPE_QLANES)
     int pipe_clanes = 2;     // mid_c hops in flight per block (<= PIPE_CLANES)
     int pipe_tlanes = 3;     // attention hops in flight per block (<= PIPE_TLANES)
@@ -601,7 +601,7 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
             CK(launch_k(pdl || ((e->tc_pdl & 4) != 0 && a.prof == nullptr), qkv_many_kernel_t<Map>, dim3((unsigned)grid_q), dim3(QKV_THREADS), QKV_MANY_SMEM, st, (const float*)QKVRAW, Q, KALL, VALL, state, recs,
                         b, W, T, B * T, active));
         } else {
-            CK(launch_k(pdl, qkv_kernel_t<Map>, dim3(T, B), dim3(QKV_THREADS), QKV_SMEM, st, (const float*)X,
+            CK(launch_k(pdl, qkv_kernel_t<Map>, dim3(T, B), dim3(QKV_THREADS), (tc || row_mid) ? QKV_PRE_SMEM : QKV_SMEM, st, (const float*)X,
                         (const float*)((tc || row_mid) ? QKVRAW : nullptr), Q, KALL, VALL, state, recs, b, W, T, 0, active));
         }
         MARK("qkv");
@@ -710,9 +710,9 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
     const int rows = B * NF;
     const int nsplit = attn_splits(B, 1);
     // programmatic dependent launch, per stage: the kernel's prologue (weight staging) overlaps its stream predecessor's
-    // tail; every kernel reaches griddepcontrol.wait before it touches activations or state.  Worth it only on the
-    // serial stage (mid_b -> mid_b of the next hop): everywhere, the parked dependents hold shared memory and CTA
-    // slots the running kernels need
+    // tail; every kernel reaches griddepcontrol.wait before it touches activations or state.  Off by default: a parked
+    // dependent holds shared memory and CTA slots the running kernels need, on the serial stage too (mid_b -> mid_b of the
+    // next batch): its 13 CTAs would sit on half an SM each while mid_a walks its batch
     const int ppdl = e->pipe_pdl;         // stage bit mask (bits: include/lookonce_b200.h, l2h_sep_set_option)
     const bool many = mid_split_for_throughput(B);
     float* state = a.state;
@@ -809,8 +809,9 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
                 l.out_outer_stride = slot / 128; l.out_inner_stride = NF; l.out_step_stride = 1; l.ndir = 2;
                 CK(launch_lstm_rec(l, st_a, (ppdl & 4) != 0));
                 // only the W_hh product + cell (mid_b) is serial per block; the rest rides on the parallel lanes.
-                // GI / H' live in the hop's GX slot, which the BiLSTM has finished with.
-                CK(launch_k((ppdl & 8) != 0, mid_a_kernel, mid_grid_for(B * nh, 2), dim3(256), MID_A_SMEM, st_a, (const float*)Y, X, GX, W, B, slot, nh));
+                // GI / H' live in the hop's GX slot, which the BiLSTM has finished with.  One CTA per (stream, row
+                // tile) walks the batch's hops: its 100 KB of weights are staged once per batch, not once per hop.
+                CK(launch_k((ppdl & 8) != 0, mid_a_kernel, mid_grid_for(B, 2), dim3(256), MID_A_SMEM, st_a, (const float*)Y, X, GX, W, B, slot, nh));
                 cudaEvent_t ev_a;
                 if (int rc = record(&ev_a, st_a)) return rc;
                 for (int k = k0; k < k1; ++k) a_done[b][k] = ev_a;
@@ -829,7 +830,7 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
             cudaStream_t st_c = sBc(b, k0 / mb);
             float* wsp0 = a.wsp + (int64_t)k0 * slot;
             CK(cudaStreamWaitEvent(st_c, midb_done, 0));
-            CK(launch_k((ppdl & 32) != 0, mid_c_kernel, mid_grid_for(B * (k1 - k0), 4), dim3(256), MID_C_SMEM, st_c,
+            CK(launch_k((ppdl & 32) != 0, mid_c_kernel, mid_grid_for(B, 4), dim3(256), MID_C_SMEM, st_c,      // as mid_a: a CTA walks the hops of its tile
                         (const float*)(wsp0 + ws.GX + (int64_t)rows * 256), wsp0 + ws.X, wsp0 + ws.QKVRAW, W, B, slot, k1 - k0));
             cudaEvent_t midc_done;
             if (int rc = record(&midc_done, st_c)) return rc;
@@ -842,7 +843,7 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
                 // attention (one per attention lane) must be done
                 for (int d = 0; d < e->pipe_tlanes && k - PIPE_QKV_AHEAD - 1 - d >= 0; ++d)
                     CK(cudaStreamWaitEvent(st_q, att_done[b][k - PIPE_QKV_AHEAD - 1 - d], 0));
-                CK(launch_k((ppdl & 64) != 0, qkv_kernel, dim3(1, B), dim3(QKV_THREADS), QKV_SMEM, st_q, (const float*)X,
+                CK(launch_k((ppdl & 64) != 0, qkv_kernel, dim3(1, B), dim3(QKV_THREADS), QKV_PRE_SMEM, st_q, (const float*)X,
                             (const float*)QKVRAW, Q, (float*)nullptr, (float*)nullptr, state, ss, b, W, 1, k, all_active));
                 if (int rc = record(&qkv_done[b][k], st_q)) return rc;
                 // the attention reads this hop's ring row and the 49 before it: the other qkv lanes' latest hops must be in

@@ -488,6 +488,9 @@ constexpr int QKV_THREADS = 384;
 constexpr int QKV_PLD = NQKV;                 // 112: a frame's projections are one contiguous 43 KB tile
 constexpr int QKV_LNP = 4 * QK_LD + 2 * V_DIM;  // staged LayerNorm params: gq | bq | gk | bk | gv | bv
 constexpr size_t QKV_SMEM = (size_t)(64 * 100 + 64 * NQKV + NF * QKV_PLD + QKV_LNP) * sizeof(float);
+// with the projections given (`pre`), X and W_qkv are not staged: launches that pass `pre` need only this much, which lets
+// two such CTAs, or one and a BiLSTM, share an SM
+constexpr size_t QKV_PRE_SMEM = (size_t)(NF * QKV_PLD + QKV_LNP) * sizeof(float);
 
 template <class Map>
 __global__ void __launch_bounds__(QKV_THREADS)
@@ -495,9 +498,9 @@ qkv_kernel_t(const float* __restrict__ X, const float* __restrict__ pre, float* 
              float* __restrict__ Kall, float* __restrict__ Vall, float* __restrict__ state, Map recs, int blk,
              BlockWeights w, int T, int frame_k, const uint8_t* __restrict__ active) {
     extern __shared__ __align__(16) float sm[];
-    float* Xt = sm;                      // [64][100]  k-major, rows padded to 100 (zeros)
+    float* Xt = sm;                      // [64][100]  k-major, rows padded to 100 (zeros); not staged when pre != nullptr
     float* Ws = Xt + 64 * 100;           // [64][112]
-    float* P = Ws + 64 * NQKV;           // [97][112]
+    float* P = pre != nullptr ? sm : Ws + 64 * NQKV;     // [97][112]
     float* LNP = P + NF * QKV_PLD;       // gq[584] bq[584] gk[584] bk[584] gv[1552] bv[1552]
     __shared__ __align__(8) unsigned long long bars[2];
     const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
@@ -1057,7 +1060,11 @@ attn_cluster_kernel_t(const float* __restrict__ Qbuf, const float* __restrict__ 
 // K4c attention output: Linear(64->64) + PReLU + LayerNorm over (F, C) + residual
 // (tfgridnet_causal.py:583-588); for block 0 the speaker gate that the reference applies to the
 // input of block 1 (:250-251) is folded into this epilogue.  grid (T, B), 256 threads.
-constexpr size_t AOUT_SMEM = (size_t)(64 * 100 + 64 * 64 + NF * 64 + 4 * FC) * sizeof(float);   // + gamma, beta, X row, gate
+// The residual rows, the gate and the LayerNorm parameters are read once per element, so none is staged in shared memory
+// (the residual rows go to registers during the projection, the rest is read where it is used): 67 KB per CTA lets three
+// of them, or one next to a BiLSTM, share an SM.
+constexpr size_t AOUT_SMEM = (size_t)(64 * 100 + 64 * 64 + NF * 64) * sizeof(float);
+constexpr int AOUT_EPI = (FC / 4 + 255) / 256;      // float4s of the frame per thread in the epilogue
 
 template <class Map>
 __global__ void __launch_bounds__(256)
@@ -1068,30 +1075,26 @@ attn_out_kernel_t(const float* __restrict__ Z, float* __restrict__ X, const floa
     float* Zt = sm;                 // [64][100]
     float* Ws = Zt + 64 * 100;      // [64][64]
     float* P = Ws + 64 * 64;        // [97][64]
-    float* Gs = P + NF * 64;        // LN gamma  [6208]
-    float* Bs = Gs + FC;            // LN beta
-    float* Xr = Bs + FC;            // the frame's rows of X (residual)
-    float* Gt = Xr + FC;            // speaker gate (block 0 only)
-    __shared__ __align__(8) unsigned long long bars[2];
+    __shared__ __align__(8) unsigned long long bars[1];
     const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
     float* xr = X + ((int64_t)b * T + t) * NF * CH;
     const float* gate = stream_rec(state, recs, b) + ST_GATE;
     TraceScope trace_(TK_ATTN_OUT, Z);
     griddep_launch();
-    if (tid == 0) { mbar_init(&bars[0], 1); mbar_init(&bars[1], 1); mbar_fence_init(); }
+    if (tid == 0) { mbar_init(&bars[0], 1); mbar_fence_init(); }
     __syncthreads();
     // parameters: before the dependency wait
-    if (tid == 0) mbar_expect_tx(&bars[0], (64 * 64 + 2 * FC) * 4);
+    if (tid == 0) mbar_expect_tx(&bars[0], 64 * 64 * 4);
     __syncthreads();
     tma_load_split(Ws, w.wp_t, 64 * 64 * 4, &bars[0], tid, 256);
-    tma_load_split(Gs, w.lnp_g, FC * 4, &bars[0], tid, 256);
-    tma_load_split(Bs, w.lnp_b, FC * 4, &bars[0], tid, 256);
     griddep_wait();
-    // chain data: the residual rows and (block 0) the gate
-    if (tid == 0) mbar_expect_tx(&bars[1], (apply_gate ? 2 : 1) * FC * 4);
-    __syncthreads();
-    tma_load_split(Xr, xr, FC * 4, &bars[1], tid, 256);
-    if (apply_gate) tma_load_split(Gt, gate, FC * 4, &bars[1], tid, 256);
+    // chain data: the residual rows, in flight during the projection
+    float4 xv[AOUT_EPI];
+#pragma unroll
+    for (int j = 0; j < AOUT_EPI; ++j) {
+        const int i = tid + j * 256;
+        xv[j] = (i < FC / 4) ? reinterpret_cast<const float4*>(xr)[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
     {
         const float* zr = Z + ((int64_t)b * T + t) * NF * CH;
         for (int i = tid; i < 100 * 16; i += 256) {
@@ -1144,19 +1147,22 @@ attn_out_kernel_t(const float* __restrict__ Z, float* __restrict__ X, const floa
     float q = 0.f;
     for (int i = tid; i < FC; i += 256) { const float d = P[i] - mu; q += d * d; }
     const float rs = rsqrtf(block_sum(q, red) * (1.f / FC) + 1e-5f);
-    mbar_wait(&bars[1], 0);
-    for (int i = tid; i < FC / 4; i += 256) {
-        float4 x4 = reinterpret_cast<const float4*>(Xr)[i];
-        const float4 p4 = reinterpret_cast<const float4*>(P)[i];
-        const float4 g4 = reinterpret_cast<const float4*>(Gs)[i];
-        const float4 b4 = reinterpret_cast<const float4*>(Bs)[i];
-        x4.x += (p4.x - mu) * rs * g4.x + b4.x; x4.y += (p4.y - mu) * rs * g4.y + b4.y;
-        x4.z += (p4.z - mu) * rs * g4.z + b4.z; x4.w += (p4.w - mu) * rs * g4.w + b4.w;
-        if (apply_gate) {
-            const float4 t4 = reinterpret_cast<const float4*>(Gt)[i];
-            x4.x *= t4.x; x4.y *= t4.y; x4.z *= t4.z; x4.w *= t4.w;
+#pragma unroll
+    for (int j = 0; j < AOUT_EPI; ++j) {
+        const int i = tid + j * 256;
+        if (i < FC / 4) {
+            float4 x4 = xv[j];
+            const float4 p4 = reinterpret_cast<const float4*>(P)[i];
+            const float4 g4 = __ldg(reinterpret_cast<const float4*>(w.lnp_g) + i);
+            const float4 b4 = __ldg(reinterpret_cast<const float4*>(w.lnp_b) + i);
+            x4.x += (p4.x - mu) * rs * g4.x + b4.x; x4.y += (p4.y - mu) * rs * g4.y + b4.y;
+            x4.z += (p4.z - mu) * rs * g4.z + b4.z; x4.w += (p4.w - mu) * rs * g4.w + b4.w;
+            if (apply_gate) {
+                const float4 t4 = __ldg(reinterpret_cast<const float4*>(gate) + i);
+                x4.x *= t4.x; x4.y *= t4.y; x4.z *= t4.z; x4.w *= t4.w;
+            }
+            reinterpret_cast<float4*>(xr)[i] = x4;
         }
-        reinterpret_cast<float4*>(xr)[i] = x4;
     }
 }
 

@@ -1,11 +1,13 @@
 """Timeline of the pipelined one-hop graph from the device-side trace (l2h_sep_trace_start / _read): per kernel the
 duration, the wait between its last dependency finishing and its own start, the start-to-start interval of each stage,
-and how many kernels are in flight.   python tools/pipe_trace.py [out_prefix]"""
+and how many kernels are in flight; then a census of the SM time each stage holds per hop (DESIGN.md 4.2).
+python tools/pipe_trace.py [out_prefix]"""
 import ctypes, json, os, sys, tempfile
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
 from lookoncetohear_b200 import Net, synth, _cabi
+from lookoncetohear_b200 import build as _build
 from lookoncetohear_b200.configs import TSH_PARAMS
 
 NAMES = ["front", "gemm_ih", "lstm", "mid_a", "mid_b", "mid_c", "qkv", "attn", "attn_out", "back", "mid"]
@@ -104,3 +106,58 @@ for b in range(3):
     lat = [t1[key[(8, b, h)]] - t0[key[(1, b, h)]] for h in range(100, 400) if (8, b, h) in key and (1, b, h) in key]
     if lat:
         print(json.dumps({"block": b, "hop_latency_through_block_us_median": round(float(np.median(lat)), 1)}))
+
+# ---- census: how much SM time each stage holds per hop --------------------------------------------------------------
+# A CTA reserves max(smem / 228 KB, threads / 2048, registers / 64 K, 1 / 32) of an SM for as long as it runs.
+# Launch geometry of enqueue_pipeline (csrc/sep_engine.cu) at one stream and the default options (4-hop batches):
+# stage -> (kernel symbol, CTAs per launch, threads per CTA, dynamic smem bytes, hops per launch per block)
+GEOMETRY = {
+    "front": ("front_kernel_tIl", 1, 256, 192 * 196 * 4, 1),
+    "gemm_ih": ("rows_gemm_kernelILi16ELi64ELi2ELi4E", 25 * 8, 128, (64 * 20 + 64 * 64) * 4, mb),
+    "lstm": ("lstm_rec3_kernelILi1ELb1E", 2 * mb, 128, 97 * 1024, mb),
+    "mid_a": ("mid_a_kernel", 13, 256, 107264, mb),
+    "mid_b": ("mid_b_kernel_tIl", 13, 256, 67840, mb),
+    "mid_c": ("mid_c_kernel", 13, 256, 49920, mb),
+    "qkv": ("qkv_kernel_tIl", 1, 384, 65216, 1),
+    "attn": ("attn_cluster_kernel_tIl", 32, 256, 0, 1),
+    "attn_out": ("attn_out_kernel_tIl", 1, 256, 66816, 1),
+    "back": ("back_kernel_tIl", 4, 256, 70688, 1),
+}
+SM_SMEM, SM_THREADS, SM_REGS, SM_CTAS, N_SMS = 228 * 1024, 2048, 65536, 32, 132
+
+
+def ptxas_usage(log_path):
+    """{mangled kernel name: (registers, static smem bytes)} from the -Xptxas -v log of the build"""
+    use, cur = {}, None
+    for line in open(log_path):
+        if "Compiling entry function" in line:
+            cur = line.split("'")[1]
+        elif cur and "Used" in line and "registers" in line:
+            w = line.split()
+            regs = int(w[w.index("registers,") - 1])
+            smem = int(w[w.index("smem") - 2]) if "smem" in w else 0
+            use[cur] = (regs, smem)
+            cur = None
+    return use
+
+
+usage = ptxas_usage(os.path.join(_build.LIBDIR, "build.log"))
+print("| stage | duration us (median) | CTAs | threads | regs | smem KB per CTA | SM share per CTA | hops per launch | SM us per hop |")
+print("|---|---|---|---|---|---|---|---|---|")
+total_smus = 0.0
+for k, name in enumerate(NAMES[:10]):
+    m = (kern == k) & steady
+    if not m.any():
+        continue
+    sym, ctas, threads, dsmem, hops = GEOMETRY[name]
+    hits = [(n, u) for n, u in usage.items() if sym in n and "Records" not in n]
+    regs, ssmem = hits[0][1]
+    smem = dsmem + ssmem + 1024                              # + the 1 KB the SM reserves per CTA
+    share = max(smem / SM_SMEM, threads / SM_THREADS, -(-regs * 32 // 256) * 256 * (threads // 32) / SM_REGS, 1 / SM_CTAS)
+    dur = float(np.median(t1[m] - t0[m]))
+    smus = share * ctas * dur / hops
+    total_smus += smus
+    print("| %s | %.1f | %d | %d | %d | %.1f | %.3f | %d | %.2f |" % (name, dur, ctas, threads, regs, smem / 1024, share, hops, smus))
+us_hop = total / HOPS
+print(json.dumps({"sm_us_per_hop": round(total_smus, 1), "us_per_hop": round(us_hop, 2),
+                  "machine_fill": round(total_smus / (N_SMS * us_hop), 3)}))
