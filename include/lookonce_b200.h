@@ -14,8 +14,9 @@
  *                                               tfgridnet_causal.py:188-283
  *   l2h_sep_forward_active / l2h_sep_forward_slots
  *        <- one Net.predict hop for some of a state's streams (serving many listeners: INTEGRATION.md)
- *   l2h_sep_forward_slots_frames
- *        <- several Net.predict hops for a list of a state's streams (Net.advance_slots)
+ *   l2h_sep_forward_slots_frames / l2h_sep_forward_slots_hops
+ *        <- several Net.predict hops for a list of a state's streams, the same number for every row or one per row
+ *           (Net.advance_slots)
  *   l2h_sep_stream_host
  *        <- the chunk loop around Net.predict(chunk, embed, state, pad=False)  (SURVEY.md 3.3)
  *           with host buffers: H2D of each chunk and D2H of each result inside the call
@@ -165,14 +166,35 @@ int l2h_sep_forward_slots(void* handle, const float* x_dev, int64_t x_batch_stri
  *   slots_dev  as for l2h_sep_forward_slots; with L2H_FLAG_GRAPH the cached graph's key holds n and frames.  An entry
  *              outside [0, state_batch) marks a row that is computed from record 0 and stores nothing (no record, no y
  *              row) for all of its frames.
- * Every row advances by the same number of hops: listeners with different backlogs go in different calls.  Records not
- * listed are neither read nor written; the header advances by `frames` as for any call.
+ * Every row advances by the same number of hops; listeners with different backlogs share one call through
+ * l2h_sep_forward_slots_hops below, which gives each row its own count.  Records not listed are neither read nor
+ * written; the header advances by `frames` as for any call.
  * Errors 1, before anything is enqueued: null pointers, n <= 0, n > state_batch, frames <= 0, L2H_FLAG_TAPS. */
 int l2h_sep_forward_slots_frames(void* handle, const float* x_dev, int64_t x_batch_stride, int64_t x_ch_stride,
                                  int32_t x_len, const float* emb_dev, void* state_dev, int32_t state_batch,
                                  const int32_t* slots_dev, int32_t n, int32_t frames, float* y_dev,
                                  int64_t y_batch_stride, int64_t y_ch_stride, int32_t y_len, void* workspace_dev,
                                  size_t workspace_bytes, uint32_t flags, void* stream);
+/* l2h_sep_forward_slots_frames in which row i advances its record by its own number of hops h = hops_dev[i], from 0 to
+ * `frames` (T, the call's maximum), so listeners with different backlogs catch up in one call, and one graph cached for
+ * (n, T) serves every mix of backlogs up to T.  The model is causal in time, so a row's first h hops of a T-hop call are
+ * exactly those of an h-hop call; the call computes all T and stores only what h hops leave:
+ *   x_dev      x_len = 128*frames + 64 as for l2h_sep_forward_slots_frames, but row i reads only its samples
+ *              0 .. 128*h + 63: samples past 128*h + 64 are never read
+ *   y_dev      row i receives samples 0 .. 128*h - 1; its later samples are not written
+ *   record     its clock advances by h hops and by one call if h > 0; its rings, h / c, tails and gate memo end where h
+ *              hops leave them.  h = 0 stores nothing (as a slot outside [0, state_batch) does)
+ *   hops_dev   [n] int32 of DEVICE memory read when the kernels run, like slots_dev: with L2H_FLAG_GRAPH a caller rewrites
+ *              it in place before every tick and replays the same cached graph (its key holds the pointer, not the
+ *              contents).  An entry outside [0, frames] counts as 0.  NULL: every row advances `frames` hops, which is
+ *              l2h_sep_forward_slots_frames.
+ * The workspace, the argument errors (1, before anything is enqueued) and the header's advance by `frames` are those of
+ * l2h_sep_forward_slots_frames. */
+int l2h_sep_forward_slots_hops(void* handle, const float* x_dev, int64_t x_batch_stride, int64_t x_ch_stride,
+                               int32_t x_len, const float* emb_dev, void* state_dev, int32_t state_batch,
+                               const int32_t* slots_dev, const int32_t* hops_dev, int32_t n, int32_t frames,
+                               float* y_dev, int64_t y_batch_stride, int64_t y_ch_stride, int32_t y_len,
+                               void* workspace_dev, size_t workspace_bytes, uint32_t flags, void* stream);
 
 /* Streaming with HOST buffers (the end-to-end path).  Per round: H2D of the round's samples (+64
  * look-ahead) from pinned memory, the kernel chains, D2H of the new samples; one stream synchronise at

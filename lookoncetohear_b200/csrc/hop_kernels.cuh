@@ -549,9 +549,10 @@ front1_kernel_t(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstrid
     float* cb_next = st + ST_CONV + (par ^ 1) * (2 * 4 * NF);
     // samples of the frame: x[s0 .. s0 + 191] (zero past the end: the look-ahead padding of net.py:8-18,56-58)
     const int s0 = pos_rel ? (int)(hdr->pos - hdr->clip_base) * HOP : 0;
+    const int xl = row_len(recs, b, 1, x_len, LOOKAHEAD);
     for (int i = tid; i < NMIC * NFFT; i += 256) {
         const int m = i / NFFT, n = i % NFFT, sidx = s0 + n;
-        xs[m][n] = (sidx < x_len) ? x[(int64_t)b * x_bstride + (int64_t)m * x_cstride + sidx] : 0.f;
+        xs[m][n] = (sidx < xl) ? x[(int64_t)b * x_bstride + (int64_t)m * x_cstride + sidx] : 0.f;
     }
     // the two history frames of the conv come from the tails the previous call left
     for (int i = tid; i < 2 * 4 * F1_NB; i += 256) {

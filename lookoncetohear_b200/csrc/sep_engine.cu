@@ -364,6 +364,7 @@ struct ChainArgs {
     const uint8_t* active = nullptr;     // one-hop calls: [B] device mask of the streams that advance (null: all)
     const int32_t* slots = nullptr;      // [B] device list, row b -> record slots[b] (null: row b -> record b)
     int state_batch = 0;                 // records in the state (slot lists only)
+    const int32_t* hops = nullptr;       // slot lists: [B] device list of the frames each row advances (null: all T)
 };
 
 // Map: the record stride (dense calls) or Records (slot-list calls), see row_record in sep_kernels.cuh
@@ -555,6 +556,7 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
                 xa.l = l; xa.x = X; xa.x_ld = 64;
                 xa.wih_hi = e->pack.planes + e->plane_of[(size_t)b * PL_PER_BLOCK + PL_IH2]; xa.wih_lo = xa.wih_hi + e->pack.planes_total;
                 xa.bias = W.b2; xa.ln_g = W.ln2_g; xa.ln_b = W.ln2_b;
+                if constexpr (std::is_same_v<Map, Records>) xa.steps = recs.hops;     // ragged rows: masked inside
                 CK(launch_tc_lstm_x(xa, e->tc_passes, st, false));
                 MARK("gemm_ih_inter");
             } else {
@@ -567,10 +569,16 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
                     CK(launch_rows_gemm(g, st, pdl));
                 }
                 MARK("gemm_ih_inter");
+                if constexpr (std::is_same_v<Map, Records>) {
+                    if (recs.hops) CK(launch_k(false, inter_gate_mask_kernel, dim3(T, B), dim3(256), 0, st, GX, recs, T));
+                }
                 CK(lstm_any(e, l, st, pdl));
             }
             MARK("lstm_inter");
             if constexpr (std::is_same_v<Map, Records>) {
+                if (recs.hops)      // a ragged row's h is that of its own last frame
+                    CK(launch_k(false, inter_h_last_kernel, dim3(B), dim3(256), 0, st, (const float*)Y,
+                                HG + (int64_t)b * B * FC, recs, T));
                 if (b == e->n_blocks - 1)
                     CK(launch_k(false, scatter_hc_kernel, dim3((unsigned)((hc4 + 255) / 256)), dim3(256), 0, st, state, recs,
                                 e->n_blocks, B, (const float*)HG, (const float*)CG));
@@ -652,7 +660,7 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
 
 static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
     const int64_t ss = stream_stride(e->n_blocks);
-    if (a.slots) return enqueue_chain_t(e, a, st, Records{ss, a.slots, a.state_batch});
+    if (a.slots) return enqueue_chain_t(e, a, st, Records{ss, a.slots, a.state_batch, a.hops, a.T});
     return enqueue_chain_t(e, a, st, ss);
 }
 
@@ -904,7 +912,7 @@ static void drop_graphs(SepEngine* e) {
 static std::vector<int64_t> graph_key(const ChainArgs& a, int t) {
     return {(int64_t)a.x, a.xbs, a.xcs, a.x_len, (int64_t)a.emb, (int64_t)a.state, (int64_t)a.y,
             a.ybs, a.ycs, a.y_len, a.B, t, (int64_t)a.wsp, (int64_t)a.flags, a.pos_rel, (int64_t)a.active,
-            (int64_t)a.slots, a.state_batch};
+            (int64_t)a.slots, a.state_batch, (int64_t)a.hops};
 }
 
 // Launch the graph cached under `key` on `st`.  The first time a key is seen, `enqueue(cap)` is captured on the private
@@ -1264,6 +1272,14 @@ int l2h_sep_forward_slots_frames(void* handle, const float* x, int64_t xbs, int6
                                  void* state, int32_t state_batch, const int32_t* slots_dev, int32_t n, int32_t frames,
                                  float* y, int64_t ybs, int64_t ycs, int32_t y_len, void* ws, size_t ws_bytes,
                                  uint32_t flags, void* stream) {
+    return l2h_sep_forward_slots_hops(handle, x, xbs, xcs, x_len, emb, state, state_batch, slots_dev, nullptr, n, frames, y,
+                                      ybs, ycs, y_len, ws, ws_bytes, flags, stream);
+}
+
+int l2h_sep_forward_slots_hops(void* handle, const float* x, int64_t xbs, int64_t xcs, int32_t x_len, const float* emb,
+                               void* state, int32_t state_batch, const int32_t* slots_dev, const int32_t* hops_dev,
+                               int32_t n, int32_t frames, float* y, int64_t ybs, int64_t ycs, int32_t y_len, void* ws,
+                               size_t ws_bytes, uint32_t flags, void* stream) {
     SepEngine* e = static_cast<SepEngine*>(handle);
     if (!e || !x || !emb || !state || !y || !ws || !slots_dev) return fail(1, "null argument");
     if (state_batch <= 0 || n <= 0 || n > state_batch)
@@ -1276,6 +1292,7 @@ int l2h_sep_forward_slots_frames(void* handle, const float* x, int64_t xbs, int6
                 static_cast<float*>(ws), ws_bytes, flags & ~L2H_FLAG_GRAPH, 0};
     a.slots = slots_dev;
     a.state_batch = state_batch;
+    a.hops = hops_dev;
     return run_chain(e, a, static_cast<cudaStream_t>(stream), (flags & L2H_FLAG_GRAPH) != 0);
 }
 

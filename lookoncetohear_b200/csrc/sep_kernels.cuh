@@ -73,11 +73,32 @@ struct Records {
     int64_t stride;            // floats per record
     const int32_t* slots;      // device, one entry per call row
     int32_t batch;             // records in the state
+    const int32_t* hops;       // device, frames each row advances (l2h_sep_forward_slots_hops), or null: every row all of them
+    int32_t frames;            // frames of the call (T)
 };
+
+// How many of a call's T frames row b advances: all of them for dense rows and plain slot lists; hops[b] for a ragged
+// slot list, where an entry outside [0, T] counts as 0.  A ragged row computes all T frames (its first T_b are exactly
+// those of a T_b-frame call: every stage is causal in time) but stores only what its T_b frames leave.
+__device__ __forceinline__ int row_frames(int64_t, int, int T) { return T; }
+__device__ __forceinline__ int row_frames(const Records& r, int b, int T) {
+    if (r.hops == nullptr) return T;
+    const int h = __ldg(r.hops + b);
+    return (unsigned)h <= (unsigned)T ? h : 0;
+}
+// ... whether frame t (< T) is one of them, given T_b = row_frames(): always for a dense row
+__device__ __forceinline__ bool row_has_frame(int64_t, int, int) { return true; }
+__device__ __forceinline__ bool row_has_frame(const Records&, int t, int Tb) { return t < Tb; }
+// ... and the samples of row b's x (extra = LOOKAHEAD) or y (extra = 0) those frames read or write: `len` for a dense row
+__device__ __forceinline__ int row_len(int64_t, int, int, int len, int) { return len; }
+__device__ __forceinline__ int row_len(const Records& r, int b, int T, int len, int extra) {
+    return r.hops == nullptr ? len : min(len, HOP * row_frames(r, b, T) + extra);
+}
 
 // The one decision of which record call row b reads and writes, and whether the row stores anything (its record and its
 // y row).  Dense rows store unless the activity mask of l2h_sep_forward_active clears them.  A slot-list entry outside
-// [0, batch) marks a row that is computed from record 0 (so every read stays inside the state) and stores nothing.
+// [0, batch) marks a row that is computed from record 0 (so every read stays inside the state) and stores nothing, and so
+// does a ragged row that advances no frame.
 struct RowRecord { int64_t off; bool stores; };
 __device__ __forceinline__ RowRecord row_record(int64_t stride, const uint8_t* active, int b) {
     return {(int64_t)(sizeof(StateHeader) / 4) + (int64_t)b * stride, active == nullptr || active[b] != 0};
@@ -85,7 +106,7 @@ __device__ __forceinline__ RowRecord row_record(int64_t stride, const uint8_t* a
 __device__ __forceinline__ RowRecord row_record(const Records& r, const uint8_t*, int b) {
     const int s = __ldg(r.slots + b);
     const bool in = (unsigned)s < (unsigned)r.batch;
-    return {(int64_t)(sizeof(StateHeader) / 4) + (int64_t)(in ? s : 0) * r.stride, in};
+    return {(int64_t)(sizeof(StateHeader) / 4) + (int64_t)(in ? s : 0) * r.stride, in && row_frames(r, b, r.frames) > 0};
 }
 template <class Map> __device__ __forceinline__ float* stream_rec(float* state, const Map& r, int b) {
     return state + row_record(r, nullptr, b).off;
@@ -100,7 +121,7 @@ __device__ __forceinline__ long long rec_pos(const float* rec) { return *reinter
 __device__ __forceinline__ int rec_par(const float* rec) { return __float_as_int(rec[ST_CALLS]) & 1; }
 
 // End of a call, run by every thread of ONE CTA after all others have finished reading the clocks: the header advances by
-// `frames` frames and one call, and so does the clock of every row that stores.
+// `frames` frames and one call, and the clock of every row that stores by one call and the frames it advances.
 template <class Map>
 __device__ void advance_clocks(float* state, Map recs, int n_streams, int frames, const uint8_t* active) {
     if (threadIdx.x == 0) {
@@ -112,7 +133,7 @@ __device__ void advance_clocks(float* state, Map recs, int n_streams, int frames
     for (int b = threadIdx.x; b < n_streams; b += blockDim.x) {
         if (!stream_active(recs, active, b)) continue;
         float* rec = stream_rec(state, recs, b);
-        *reinterpret_cast<long long*>(rec + ST_POS) += frames;
+        *reinterpret_cast<long long*>(rec + ST_POS) += row_frames(recs, b, frames);
         rec[ST_CALLS] = __int_as_float(__float_as_int(rec[ST_CALLS]) + 1);
     }
     __threadfence();
@@ -192,7 +213,7 @@ front_kernel_t(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride
     // count) and recompute what they need of their predecessors inside the group; only the group's last frame
     // writes the new tails (other parity) -- so the frames of a group never depend on each other here.
     const StateHeader* hdr = reinterpret_cast<const StateHeader*>(state);
-    const int gi = frame_k + t, GN = (frames_total > 1) ? frames_total : T;
+    const int gi = frame_k + t, GN = row_frames(recs, b, (frames_total > 1) ? frames_total : T);
     float* st = stream_rec(state, recs, b);
     const int par = rec_par(st);
     const float* cb = st + ST_CONV + par * (2 * 4 * NF);
@@ -201,9 +222,10 @@ front_kernel_t(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride
     for (int i = tid; i < 3 * 4 * 100; i += 256) (&U[0][0][0])[i] = 0.f;
     // pos_rel: x is a whole clip and this call starts at frame (pos - clip_base) of it
     const int s0 = HOP * (t - 2) + sample_off + (pos_rel ? (int)(hdr->pos - hdr->clip_base) * HOP : 0);
+    const int xl = row_len(recs, b, T, x_len, LOOKAHEAD);
     for (int i = tid; i < NMIC * 448; i += 256) {
         const int m = i / 448, n = i % 448, s = s0 + n;
-        xs[m][n] = (s >= 0 && s < x_len) ? x[(int64_t)b * x_bstride + (int64_t)m * x_cstride + s] : 0.f;
+        xs[m][n] = (s >= 0 && s < xl) ? x[(int64_t)b * x_bstride + (int64_t)m * x_cstride + s] : 0.f;
     }
     __syncthreads();
     trace_.mark(0);
@@ -266,7 +288,8 @@ front_kernel_t(const float* __restrict__ x, int64_t x_bstride, int64_t x_cstride
         }
     }
     trace_.mark(3);
-    // next conv_buf = spectrogram rows of the last two frames of the group, written by its last frame
+    // next conv_buf = spectrogram rows of the last two frames of the group (a ragged row's own last two), written by its
+    // last frame
     if (gi == GN - 1 && stream_active(recs, active, b)) {
         for (int e = tid; e < 4 * NF; e += 256) {
             cb_next[e] = U[1][e / NF][1 + e % NF];
@@ -317,15 +340,16 @@ front_many_kernel_t(const float* __restrict__ x, int64_t x_bstride, int64_t x_cs
     float* st = stream_rec(state, recs, b);
     const int par = rec_par(st);
     const bool live = stream_active(recs, active, b);
+    const int Tb = row_frames(recs, b, T), xl = row_len(recs, b, T, x_len, LOOKAHEAD);
     const float* cb = st + ST_CONV + par * (2 * 4 * NF);
     float* cb_next = st + ST_CONV + (par ^ 1) * (2 * 4 * NF);
     const float* xb = x + (int64_t)b * x_bstride;
     // samples of frame g: x[sbase + 128 g .. + 191] (zero outside the clip); thread tid fetches entries tid and tid + 256 of [2][192]
     auto fetch = [&](int g, float& a0, float& a1) {
         const int s0 = sbase + HOP * g;
-        { const int m = tid / NFFT, n = tid % NFFT, sidx = s0 + n; a0 = (sidx >= 0 && sidx < x_len) ? xb[(int64_t)m * x_cstride + sidx] : 0.f; }
+        { const int m = tid / NFFT, n = tid % NFFT, sidx = s0 + n; a0 = (sidx >= 0 && sidx < xl) ? xb[(int64_t)m * x_cstride + sidx] : 0.f; }
         a1 = 0.f;
-        if (tid + 256 < NMIC * NFFT) { const int i = tid + 256, m = i / NFFT, n = i % NFFT, sidx = s0 + n; a1 = (sidx >= 0 && sidx < x_len) ? xb[(int64_t)m * x_cstride + sidx] : 0.f; }
+        if (tid + 256 < NMIC * NFFT) { const int i = tid + 256, m = i / NFFT, n = i % NFFT, sidx = s0 + n; a1 = (sidx >= 0 && sidx < xl) ? xb[(int64_t)m * x_cstride + sidx] : 0.f; }
     };
     auto put = [&](float a0, float a1) {
         (&xs[0][0])[tid] = a0;
@@ -391,7 +415,7 @@ front_many_kernel_t(const float* __restrict__ x, int64_t x_bstride, int64_t x_cs
                     if (f + 4 * u < NF) X[(((int64_t)b * T + t) * NF + f + 4 * u) * CH + o] = acc[u];
             }
         }
-        if (t == T - 1 && live) {                  // next conv tails = spectrogram rows of the call's last two frames
+        if (t == Tb - 1 && live) {                 // next conv tails = spectrogram rows of the row's last two frames
             for (int e = tid; e < 4 * NF; e += 256) {
                 cb_next[e] = U[(t - 1 + 3) % 3][e / NF][1 + e % NF];
                 cb_next[4 * NF + e] = U[(t + 3) % 3][e / NF][1 + e % NF];
@@ -612,7 +636,10 @@ qkv_kernel_t(const float* __restrict__ X, const float* __restrict__ pre, float* 
     } else {
         float* sb = rec + ST_BLK + (int64_t)blk * BK_STRIDE;
         const int slot = (int)((pos + t) % RING);
-        if (t >= T - ATT && stream_active(recs, active, b))
+        // the ring keeps the last ATT of the frames the row advances; a frame past them (t >= T_b + RING - ATT + 1) would
+        // overwrite a row the next call's window still reads
+        const int Tb = row_frames(recs, b, T);
+        if (t >= Tb - ATT && row_has_frame(recs, t, Tb) && stream_active(recs, active, b))
             dst1 = sb + (which == 1 ? BK_K : BK_V) + ((int64_t)h * RING + slot) * ld;
         if (T > 1) dst0 = (which == 1 ? Kall : Vall) + (bh * (ATT - 1 + T) + (ATT - 1) + t) * ld;
     }
@@ -718,7 +745,9 @@ qkv_many_kernel_t(const float* __restrict__ pre, float* __restrict__ Qbuf, float
             float* rec = stream_rec(state, recs, b);
             float* sb = rec + ST_BLK + (int64_t)blk * BK_STRIDE;
             const int slot = (int)((rec_pos(rec) + t) % RING);
-            if (t >= T - ATT && stream_active(recs, active, b)) dst1 = sb + (which == 1 ? BK_K : BK_V) + ((int64_t)h * RING + slot) * ld;
+            const int Tb = row_frames(recs, b, T);      // as in qkv_kernel
+            if (t >= Tb - ATT && row_has_frame(recs, t, Tb) && stream_active(recs, active, b))
+                dst1 = sb + (which == 1 ? BK_K : BK_V) + ((int64_t)h * RING + slot) * ld;
             if (T > 1) dst0 = (which == 1 ? Kall : Vall) + (bh * (ATT - 1 + T) + (ATT - 1) + t) * ld;
         }
         {
@@ -1212,7 +1241,7 @@ back_kernel_t(const float* __restrict__ X, float* __restrict__ y, int64_t y_bstr
     // group bookkeeping as in front_kernel: gi = frame index in the group, frames before the group come
     // from the deconv tails the previous group left, frames inside it from X (T > 1) or from the
     // workspace slots of the previous one-frame calls of the pipelined graph (hist_stride apart)
-    const int gi = frame_k + t, GN = (frames_total > 1) ? frames_total : T;
+    const int gi = frame_k + t, GN = row_frames(recs, b, (frames_total > 1) ? frames_total : T);
     // zero the halo rows that fall outside 0 .. 96 and whole slots that stay empty
     for (int i = tid; i < 4 * ld * 64; i += 256) {
         const int slot = i / (ld * 64), r = (i / 64) % ld;
@@ -1327,10 +1356,11 @@ back_kernel_t(const float* __restrict__ X, float* __restrict__ y, int64_t y_bstr
     cluster.sync();                         // all four partial windows are complete and visible cluster-wide
     trace_.mark(4);
     if (part == 0 && live) {
+        const int yl = row_len(recs, b, T, y_len, 0);
         for (int i = tid; i < NSRC * HOP; i += 256) {
             const int ear = i / HOP, n = i % HOP;
             const int s = HOP * t + n + soff;
-            if (s < y_len) {
+            if (s < yl) {
                 float v = 0.f, tail = 0.f;
 #pragma unroll
                 for (int p = 0; p < BACK_CL; ++p) {
@@ -1416,6 +1446,7 @@ back_many_kernel_t(const float* __restrict__ X, float* __restrict__ y, int64_t y
         float* st = stream_rec(state, recs, b);
         const int par = rec_par(st);
         const bool live = stream_active(recs, active, b);
+        const int Tb = row_frames(recs, b, T), yl = row_len(recs, b, T, y_len, 0);
         const float* db = st + ST_DECONV + par * (2 * FC);
         float* db_next = st + ST_DECONV + (par ^ 1) * (2 * FC);
         const float* ib = st + ST_ISTFT + par * (NSRC * NROW);
@@ -1475,7 +1506,7 @@ back_many_kernel_t(const float* __restrict__ X, float* __restrict__ y, int64_t y
             __syncthreads();                           // frame t-1's readers of frame t-3's slot are done; R[(t-1)&1] complete
             if (t + 1 < t1) stage(t + 1);              // into the slot of frame t-3
             deconv(t);
-            if (t == T - 1 && live) {                  // next deconv tails: frames T-2, T-1 (own bins)
+            if (t == Tb - 1 && live) {                 // next deconv tails: the row's last two frames (own bins)
                 for (int i = tid; i < nf * 16; i += 256) {
                     const int r = i / 16, c4 = i % 16;
                     reinterpret_cast<float4*>(db_next + (f0 + r) * 64)[c4] =
@@ -1502,7 +1533,7 @@ back_many_kernel_t(const float* __restrict__ X, float* __restrict__ y, int64_t y
                     wa[it2] = acc;
                 }
             }
-            if (t == T - 1 && live)
+            if (t == Tb - 1 && live)
                 for (int i = tid; i < NSRC * 2 * nf; i += 256) {
                     const int idx = (i / (2 * nf)) * NROW + ((i / nf) & 1) * NF + f0 + i % nf;
                     ib_next[idx] = R[(t & 1) * NSRC * NROW + idx];
@@ -1512,7 +1543,7 @@ back_many_kernel_t(const float* __restrict__ X, float* __restrict__ y, int64_t y
                 for (int i = tid; i < NSRC * HOP; i += 256) {
                     const int ear = i / HOP, n = i % HOP;
                     const int s2 = HOP * t + n + soff;
-                    if (s2 < y_len) {
+                    if (s2 < yl) {
                         float v = 0.f, tail = 0.f;
 #pragma unroll
                         for (int p = 0; p < BACK_CL; ++p) {
@@ -1638,6 +1669,35 @@ scatter_hc_kernel(float* __restrict__ state, Records recs, int n_blocks, int n_s
     float* h = state + r.off + ST_BLK + (int64_t)blk * BK_STRIDE + BK_H;
     reinterpret_cast<float4*>(h)[k] = reinterpret_cast<const float4*>(Hg)[i];
     reinterpret_cast<float4*>(h + (BK_C - BK_H))[k] = reinterpret_cast<const float4*>(Cg)[i];
+}
+
+// Ragged slot-list calls (l2h_sep_forward_slots_hops), inter LSTM over T: the gate pre-activations GX [B][T][97][256]
+// (column j*4 + q, q = i, f, g, o) of the frames t >= T_b a row does not advance become i = -inf, f = +inf, g = 0, so that
+// the recurrence carries c through them unchanged (sigma(+inf) = 1, sigma(-inf) = 0) and ends with the c of frame T_b - 1.
+// grid (T, B), 256 threads; CTAs of frames a row advances return at once.
+__global__ void __launch_bounds__(256)
+inter_gate_mask_kernel(float* __restrict__ gx, Records recs, int T) {
+    const int t = blockIdx.x, b = blockIdx.y;
+    if (t < row_frames(recs, b, T)) return;
+    float* g = gx + ((int64_t)b * T + t) * NF * 256;
+    for (int u = threadIdx.x; u < NF * 64; u += 256) {
+        g[4 * u + 0] = -INFINITY;
+        g[4 * u + 1] = INFINITY;
+        g[4 * u + 2] = 0.f;
+    }
+}
+
+// ... and its h: the recurrence ends with the h of frame T - 1, a row with 0 < T_b < T carries that of frame T_b - 1, which
+// is its row of the recurrence's output Y [B][T][97][64].  That row goes into Hg [B][97][64] (the block's part of
+// gather_h_kernel's copy) before Y is reused.  grid (B), 256 threads.
+__global__ void __launch_bounds__(256)
+inter_h_last_kernel(const float* __restrict__ Y, float* __restrict__ Hg, Records recs, int T) {
+    const int b = blockIdx.x;
+    const int Tb = row_frames(recs, b, T);
+    if (Tb <= 0 || Tb >= T) return;
+    const float4* src = reinterpret_cast<const float4*>(Y + ((int64_t)b * T + Tb - 1) * FC);
+    float4* dst = reinterpret_cast<float4*>(Hg + (int64_t)b * FC);
+    for (int i = threadIdx.x; i < FC / 4; i += 256) dst[i] = src[i];
 }
 
 // the dense forms (call row b = record b); the `_t<Records>` forms serve slot-list calls (l2h_sep_forward_slots)

@@ -46,6 +46,10 @@ struct LstmXArgs {
     const float* bias;                // [ndir*256]  b_ih + b_hh
     const float* ln_g;                // [64] LayerNorm over the input channels (nn.LayerNorm semantics)
     const float* ln_b;
+    // or null: [outer index] device step counts (an entry outside [0, L] counts as 0).  Steps s >= steps[o] of the
+    // sequences of outer index o get gates i = -inf, f = +inf, g = 0, so c passes through them unchanged and the final c
+    // is the one steps[o] steps leave (one direction: the separator's inter LSTM in ragged slot-list calls)
+    const int32_t* steps;
 };
 
 L2H_DEVINL float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
@@ -62,12 +66,13 @@ L2H_DEVINL void put_split(unsigned base, int n, int j, float v) {
     asm volatile("st.shared.b16 [%0], %1;" ::"r"(off + NS * 128), "h"(*reinterpret_cast<const unsigned short*>(&hl)) : "memory");
 }
 
-template <bool FX>
+template <bool FX, bool STEPS = false>
 static __global__ void __launch_bounds__(NTHREADS, FX ? 1 : 2)
 tc_lstm_kernel(const LstmXArgs xa, int passes) {
     const LstmArgs& a = xa.l;
     extern __shared__ uint8_t smem_raw[];
     __shared__ long long in_row[NS], out_row[NS], hc_off[NS];
+    __shared__ int n_steps[STEPS ? NS : 1];       // STEPS: the sequence's own step count (LstmXArgs::steps)
     __shared__ float lng[64], lnb[64];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int dir = blockIdx.y, seq0 = blockIdx.x * NS;
@@ -87,8 +92,13 @@ tc_lstm_kernel(const LstmXArgs xa, int passes) {
             in_row[tid] = o * a.outer_stride + i * a.inner_stride;
             out_row[tid] = o * o_outer + i * o_inner;
             hc_off[tid] = o * a.hc_outer_stride + i * 64;
+            if constexpr (STEPS) {
+                const int k = xa.steps[o];
+                n_steps[tid] = (unsigned)k <= (unsigned)a.L ? k : 0;
+            }
         } else {
             in_row[tid] = -1; out_row[tid] = -1; hc_off[tid] = -1;
+            if constexpr (STEPS) n_steps[tid] = 0;
         }
     }
     if (FX && tid < 64) { lng[tid] = __ldg(xa.ln_g + tid); lnb[tid] = __ldg(xa.ln_b + tid); }
@@ -253,6 +263,9 @@ tc_lstm_kernel(const LstmXArgs xa, int passes) {
                 float4 g = *reinterpret_cast<const float4*>(xt + n * XLD + 4 * j);     // i, f, g, o
                 const float4 add = FX ? bias4[jj] : g_in[k][jj];
                 g.x += add.x; g.y += add.y; g.z += add.z; g.w += add.w;
+                if constexpr (STEPS) {
+                    if (st >= n_steps[n]) { g.x = -INFINITY; g.y = INFINITY; g.z = 0.f; }
+                }
                 const float cc = sigm(g.y) * c[k][jj] + sigm(g.x) * tanh_g(g.z);
                 c[k][jj] = cc;
                 const float h = sigm(g.w) * (__fdividef(2.f, 1.f + ex2_ftz(-2.f * LOG2E * cc)) - 1.f);
@@ -277,6 +290,7 @@ tc_lstm_kernel(const LstmXArgs xa, int passes) {
 static inline cudaError_t configure_tc_lstm() {
     cudaError_t e = cudaFuncSetAttribute(tcl::tc_lstm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tcl::SMEM);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(tcl::tc_lstm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tcl::XSMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tcl::tc_lstm_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tcl::XSMEM);
     return e;
 }
 // ... with the input projection (and its LayerNorm) inside
@@ -284,7 +298,9 @@ static inline cudaError_t launch_tc_lstm_x(const tcl::LstmXArgs& xa, int passes,
     if (xa.l.nseq <= 0 || xa.l.L <= 0 || !lstm_state_ok(xa.l) || passes < 1 || passes > 3) return cudaErrorInvalidValue;
     if ((xa.x_ld & 3) != 0 || (reinterpret_cast<uintptr_t>(xa.x) & 15) != 0 || (reinterpret_cast<uintptr_t>(xa.bias) & 15) != 0)
         return cudaErrorInvalidValue;
+    if (xa.steps != nullptr && xa.l.ndir != 1) return cudaErrorInvalidValue;
     dim3 grid((xa.l.nseq + tcl::NS - 1) / tcl::NS, xa.l.ndir);
+    if (xa.steps != nullptr) return launch_k(pdl, tcl::tc_lstm_kernel<true, true>, grid, dim3(tcl::NTHREADS), tcl::XSMEM, st, xa, passes);
     return launch_k(pdl, tcl::tc_lstm_kernel<true>, grid, dim3(tcl::NTHREADS), tcl::XSMEM, st, xa, passes);
 }
 // many sequences: the recurrence on the tensor cores

@@ -413,9 +413,10 @@ class Net(nn.Module):
         _cabi.check(L.l2h_sep_state_offsets(h, offs, n))
         return hb.value, stride.value, list(offs)
 
-    def _run(self, x, embed, state, frames, out_len, flags=0, active=None, slots=None):
+    def _run(self, x, embed, state, frames, out_len, flags=0, active=None, slots=None, hops=None):
         """x [B,M,n] (any length; samples beyond n read as zero), embed [B,256], active: [B] uint8 device mask or None,
-        slots: [B] int32 device list of the state's records the rows advance by `frames` hops, or None."""
+        slots: [B] int32 device list of the state's records the rows advance by `frames` hops, or None; hops: with
+        slots, [B] int32 device list of the hops each row advances instead (at most `frames`), or None."""
         self._require_cuda(x)
         dev = x.device
         self._sync_weights(dev)
@@ -429,10 +430,11 @@ class Net(nn.Module):
         L, st = _cabi.lib(), torch.cuda.current_stream(dev).cuda_stream
         with torch.cuda.device(dev):
             if slots is not None:
-                _cabi.check_args(L.l2h_sep_forward_slots_frames(
+                _cabi.check_args(L.l2h_sep_forward_slots_hops(
                     self._engine(), x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], embed.data_ptr(),
-                    state.buf.data_ptr(), state.batch, slots.data_ptr(), Bsz, frames, y.data_ptr(), y.stride(0),
-                    y.stride(1), out_len, ws.data_ptr(), ws.numel(), flags, st))
+                    state.buf.data_ptr(), state.batch, slots.data_ptr(), None if hops is None else hops.data_ptr(),
+                    Bsz, frames, y.data_ptr(), y.stride(0), y.stride(1), out_len, ws.data_ptr(), ws.numel(), flags,
+                    st))
             else:
                 _cabi.check(L.l2h_sep_forward_active(
                     self._engine(), x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], embed.data_ptr(),
@@ -472,6 +474,25 @@ class Net(nn.Module):
             raise ValueError("a slot is listed twice")
         return s.to(torch.int32).to(dev)
 
+    @staticmethod
+    def _hop_counts(hops, dev, n, frames):
+        """`hops` of advance_slots as the [n] int32 device tensor the engine reads.  A CUDA int32 tensor is used as it is
+        (its entries are read when the kernels run); anything else is checked here and uploaded."""
+        if isinstance(hops, torch.Tensor) and hops.is_cuda:
+            if hops.dtype != torch.int32 or tuple(hops.shape) != (n,) or not hops.is_contiguous():
+                raise ValueError(f"a CUDA hop list must be a contiguous int32 tensor of shape ({n},)")
+            if hops.device != dev:
+                raise ValueError(f"hops must live on the input's device {dev}, not {hops.device}")
+            return hops
+        h = torch.as_tensor(hops)
+        if h.dtype.is_floating_point or h.dtype.is_complex or h.dtype == torch.bool or h.dim() != 1:
+            raise ValueError("hops must be a sequence or 1-d tensor of integer hop counts")
+        if h.numel() != n:
+            raise ValueError(f"hops gives {h.numel()} counts for {n} input rows")
+        if n > 0 and (int(h.min()) < 0 or int(h.max()) > frames):
+            raise ValueError(f"a hop count lies outside [0, {frames}] (the call's {frames} hops)")
+        return h.to(torch.int32).to(dev)
+
     def predict(self, x, embed, input_state, pad=True, active=None, slots=None):
         """Reference net.py:54-66.  x [B,M,N]; embed [B,256]; returns (y [B,S,*], state).
 
@@ -510,15 +531,22 @@ class Net(nn.Module):
         y = self._run(x, embed, input_state, frames, out_len, active=active, slots=slots)
         return y, input_state
 
-    def advance_slots(self, x, embed, state, slots):
+    def advance_slots(self, x, embed, state, slots, hops=None):
         """Advance record slots[i] of `state` by T hops with row i of x [n, M, 128*T + 64] (the pad=False shape) and
         embed [n, 256]; returns y [n, S, 128*T].  A listener whose chunks arrived late catches up its backlog of T hops
-        in one call: the T hops' BiLSTMs run side by side, as in a dense multi-hop predict.  Every row advances by the
-        same T, so listeners with different backlogs go in different calls.
+        in one call: the T hops' BiLSTMs run side by side, as in a dense multi-hop predict.
 
         `slots` is checked as for predict(slots=): n distinct ints in [0, state.batch) (a sequence or CPU tensor, checked
         and uploaded), or a CUDA int32 tensor used in place, where an entry outside [0, state.batch) marks a row that
-        stores nothing for all of its hops.  predict(slots=) remains the one-hop form."""
+        stores nothing for all of its hops.  predict(slots=) remains the one-hop form.
+
+        `hops`: None (every row advances T hops), or the hops h_i in [0, T] row i advances, so listeners with different
+        backlogs catch up in one call (l2h_sep_forward_slots_hops).  Row i reads only samples 0 .. 128*h_i + 63 of its x
+        row and writes only y[i, :, :128*h_i]: its later y samples are left unwritten.  Its record ends exactly where h_i
+        hops leave it, and h_i = 0 stores nothing.  Either n ints (a sequence or CPU tensor, checked and uploaded), or a
+        contiguous CUDA int32 tensor of shape (n,) used in place, as for `slots`: there an entry outside [0, T] counts
+        as 0.  With fixed slot and hop tensors rewritten in place every tick, one cached graph per (n, T) serves every
+        mix of backlogs up to T."""
         hop, la = self.stft_chunk_size, self.stft_pad_size
         if x.dim() != 3:
             raise ValueError(f"advance_slots needs x of shape [n, channels, {hop}*T+{la}], got {tuple(x.shape)}")
@@ -528,9 +556,11 @@ class Net(nn.Module):
         if not isinstance(state, SepState):
             raise TypeError("state must come from Net.init_buffers()")
         frames = (n - la) // hop
+        if hops is not None:
+            hops = self._hop_counts(hops, x.device, x.shape[0], frames)
         self._require_cuda(x)
         slots = self._slot_list(slots, x.device, x.shape[0], state.batch)
-        return self._run(x, embed, state, frames, frames * hop, slots=slots)
+        return self._run(x, embed, state, frames, frames * hop, slots=slots, hops=hops)
 
     def forward(self, x, embeds, input_state=None, pad=True):
         """Reference net.py:68-76.  x [B,M,N]; embeds [B,1,256] -> [B,S,N]."""
