@@ -195,6 +195,32 @@ int l2h_sep_forward_slots_hops(void* handle, const float* x_dev, int64_t x_batch
                                const int32_t* slots_dev, const int32_t* hops_dev, int32_t n, int32_t frames,
                                float* y_dev, int64_t y_batch_stride, int64_t y_ch_stride, int32_t y_len,
                                void* workspace_dev, size_t workspace_bytes, uint32_t flags, void* stream);
+/* Several enrolled speakers (targets) extracted from one mixture in one call: `batch` mixtures, K = n_targets targets each.
+ * The front (STFT, conv encoder) and all of block 0 do not depend on the speaker (the speaker gate applies after block 0,
+ * tfgridnet_causal.py:250-251), so they run once per mixture; blocks 1 .. B-1 and the back run once per target.
+ *   x_dev      [batch] mixture rows, as for l2h_sep_forward
+ *   emb_dev    [batch*K][256]: target row i*K + k is target k of mixture i
+ *   y_dev      [batch*K] target rows, same order; y_batch_stride is the stride between consecutive target rows
+ *   state_dev  an ordinary state of batch*K records (l2h_sep_state_bytes(handle, batch*K)), in groups of K: record i*K + k
+ *              is target k of mixture i.  The group's lead record i*K also holds the mixture's conv tails and block 0's K/V
+ *              rings and (h, c); in the group's other records those regions are never read or written.  Every record keeps
+ *              its own embedding and gate memo, deconv and iSTFT tails, blocks 1 .. B-1 and clock, and the records of a
+ *              group advance together, so their clocks stay equal.  A non-lead record is therefore not a standalone stream:
+ *              it continues only inside its group (l2h_sep_state_reset_streams / _copy_streams of whole groups keep working).
+ *   workspace  l2h_sep_workspace_bytes(handle, batch*K, frames, flags), as for a dense call of batch*K streams
+ * Every kernel form is chosen for the batch*K target rows, and block 0 runs those same forms over the mixtures, so a target
+ * row gets the arithmetic of a dense l2h_sep_forward of batch*K streams with each mixture repeated K times; one stage
+ * differs: in the fused one-hop form (option "fused_tail") block 1's input projection runs as a separate rows GEMM rather
+ * than inside block 0's tail kernel (rounding only).  n_targets == 1 is l2h_sep_forward, bit for bit.  L2H_FLAG_GRAPH works
+ * (the cached graph's key holds K).
+ * Not supported with targets: slot lists, activity masks and per-row hop counts; the pipelined wavefront graph and
+ * l2h_sep_stream_host / _dev; taps.  Non-lead records keep their (unused) block-0 area: there is no compact record.
+ * Errors 1, before anything is enqueued: null pointers, batch, n_targets or frames <= 0, batch*n_targets*frames*97 rows
+ * beyond the limit of one call, L2H_FLAG_TAPS. */
+int l2h_sep_forward_targets(void* handle, const float* x_dev, int64_t x_batch_stride, int64_t x_ch_stride, int32_t x_len,
+                            const float* emb_dev, void* state_dev, float* y_dev, int64_t y_batch_stride,
+                            int64_t y_ch_stride, int32_t y_len, int32_t batch, int32_t n_targets, int32_t frames,
+                            void* workspace_dev, size_t workspace_bytes, uint32_t flags, void* stream);
 
 /* Streaming with HOST buffers (the end-to-end path).  Per round: H2D of the round's samples (+64
  * look-ahead) from pinned memory, the kernel chains, D2H of the new samples; one stream synchronise at

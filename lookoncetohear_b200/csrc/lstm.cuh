@@ -380,18 +380,21 @@ inline bool lstm_state_ok(const LstmArgs& a) {
     return (a.ndir == 1 || a.ndir == 2) && (a.h_state == nullptr || a.ndir == 1) && ((a.h_state == nullptr) == (a.c_state == nullptr));
 }
 
-inline cudaError_t launch_lstm_rec(const LstmArgs& a, cudaStream_t st, bool pdl = false) {
+// `form_nseq` > 0: choose the kernel (and its sequences per CTA) as for that many sequences, so that a call over a subset of
+// a larger batch runs exactly the arithmetic the whole batch would (sep_engine.cu: block 0 of a targets call)
+inline cudaError_t launch_lstm_rec(const LstmArgs& a, cudaStream_t st, bool pdl = false, int form_nseq = 0) {
     if (a.nseq <= 0 || a.L <= 0 || !lstm_state_ok(a)) return cudaErrorInvalidValue;
-    const int ctas1 = a.nseq * a.ndir;
+    const int fseq = form_nseq > 0 ? form_nseq : a.nseq;
+    const int ctas1 = fseq * a.ndir;
     if (ctas1 <= NUM_SMS && (size_t)a.L * 1024 <= 200 * 1024)      // latency mode: one sequence per CTA, preloaded
         return launch_k(pdl, lstm_rec3_kernel<1, true>, dim3(a.nseq, a.ndir), dim3(128), (size_t)a.L * 1024, st, a);
     // many sequences: NSEQ per CTA in lock-step (stage by stage), at most 4: more sequences per CTA only while one sequence
     // per CTA (resp. two) would not fit the device in one wave.  (Six per CTA would need 226 registers; not kept.)
     static int wave1[64] = {}, wave2[64] = {};
     int per = 1;
-    if ((int64_t)a.nseq * a.ndir > resident_ctas(wave1, lstm_rec3_kernel<1, false>, 128, 0)) {
+    if ((int64_t)fseq * a.ndir > resident_ctas(wave1, lstm_rec3_kernel<1, false>, 128, 0)) {
         per = 2;
-        if ((int64_t)((a.nseq + 1) / 2) * a.ndir > resident_ctas(wave2, lstm_rec4_kernel<2>, 128, lstm_rec4_smem(2))) per = 4;
+        if ((int64_t)((fseq + 1) / 2) * a.ndir > resident_ctas(wave2, lstm_rec4_kernel<2>, 128, lstm_rec4_smem(2))) per = 4;
     }
     dim3 grid((a.nseq + per - 1) / per, a.ndir);
     if (per == 2) return launch_k(pdl, lstm_rec4_kernel<2>, grid, dim3(128), lstm_rec4_smem(2), st, a);   // many sequences: stage by stage

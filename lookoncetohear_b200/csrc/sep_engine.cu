@@ -23,6 +23,7 @@
 #include "sep_kernels.cuh"
 #include "mid_kernel.cuh"
 #include "hop_kernels.cuh"
+#include "targets_kernels.cuh"
 
 namespace l2h {
 
@@ -314,15 +315,16 @@ static umma::BPlanes tc_planes(const SepEngine* e, int blk, int which, int ld) {
     return e->pack.bplanes(e->plane_of[(size_t)blk * PL_PER_BLOCK + which], ld);
 }
 
-// the recurrence: tensor cores when there are enough sequences to fill the GPU with 32-sequence CTAs, else lstm.cuh
-static cudaError_t lstm_any(SepEngine* e, const LstmArgs& l, cudaStream_t st, bool pdl) {
-    if ((int64_t)l.nseq * l.ndir >= e->tcl_min_seqdirs) return launch_tc_lstm(l, e->tc_passes, st, pdl);
-    return launch_lstm_rec(l, st, pdl);
+// the recurrence: tensor cores when there are enough sequences to fill the GPU with 32-sequence CTAs, else lstm.cuh.
+// `scale`: the form is chosen for scale times l's sequences (block 0 of a targets call runs for all the target rows)
+static cudaError_t lstm_any(SepEngine* e, const LstmArgs& l, cudaStream_t st, bool pdl, int scale = 1) {
+    if ((int64_t)l.nseq * l.ndir * scale >= e->tcl_min_seqdirs) return launch_tc_lstm(l, e->tc_passes, st, pdl);
+    return launch_lstm_rec(l, st, pdl, scale > 1 ? l.nseq * scale : 0);
 }
 
 // ... and with enough sequences the input projection moves into the recurrence kernel too (tc_lstm_x_kernel)
-static bool tc_fused_lstm(const SepEngine* e, const LstmArgs& l) {
-    return e->fuse_ih && (int64_t)l.nseq * l.ndir >= e->tcl_min_seqdirs;
+static bool tc_fused_lstm(const SepEngine* e, const LstmArgs& l, int scale = 1) {
+    return e->fuse_ih && (int64_t)l.nseq * l.ndir * scale >= e->tcl_min_seqdirs;
 }
 
 // C[rows][N] = epi(LN?(A[rows][lda, first K]) W^T + bias) (+ R), plain row-major rows
@@ -365,6 +367,7 @@ struct ChainArgs {
     const int32_t* slots = nullptr;      // [B] device list, row b -> record slots[b] (null: row b -> record b)
     int state_batch = 0;                 // records in the state (slot lists only)
     const int32_t* hops = nullptr;       // slot lists: [B] device list of the frames each row advances (null: all T)
+    int targets = 1;                     // l2h_sep_forward_targets: rows per mixture (B counts target rows; x has B / targets)
 };
 
 // Map: the record stride (dense calls) or Records (slot-list calls), see row_record in sep_kernels.cuh
@@ -425,24 +428,67 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
             CK(launch_k(false, gather_h_kernel, dim3((unsigned)((hc4 + 255) / 256)), dim3(256), 0, st, (const float*)state, recs,
                         e->n_blocks, B, HG, T > 1 ? CG : nullptr));
     }
+    // Several targets per mixture (l2h_sep_forward_targets): B counts target rows, K per mixture, row i*K + k = target k of
+    // mixture i.  The front and block 0 do not depend on the speaker (its gate applies after block 0), so they run once
+    // per mixture: over B0 rows, on the lead records i*K (record stride K*ss), without the gate, into X0 (room in GX that
+    // block 0 leaves unused).  fan_out() then builds every target row's gate memo and its gated copy of block 0's output
+    // in X, and blocks 1 .. n_blocks-1 and the back run over all B rows.  Every form above was chosen for the B rows, and
+    // block 0 runs those same forms, so a target row gets the arithmetic of a dense call with its mixture duplicated.
+    const int K = a.targets;
+    const int B0 = B / K;
+    Map recs0 = recs;
+    float* X0 = X;
+    if constexpr (std::is_same_v<Map, int64_t>) {
+        recs0 = recs * K;
+        if (K > 1) X0 = GX + (int64_t)B0 * T * NF * 512;
+    } else {
+        if (K > 1) return fail(1, "targets cannot be combined with a slot list");
+    }
+    const int gate_ctas = K > 1 ? 0 : 1;      // the front's speaker-gate memo CTAs (one per row); fan_out() builds them here
+    auto fan_out = [&]() -> int {
+        if constexpr (std::is_same_v<Map, int64_t>) {
+            CK(launch_k(pdl, spk_gate_kernel, dim3(B), dim3(256), 0, st, emb, PRE, state, recs, e->w));
+            CK(launch_k(pdl, gate_fanout_kernel, dim3(T, B), dim3(256), 0, st, (const float*)X0, X, (const float*)state, ss, K, T,
+                        e->n_blocks > 1 ? 1 : 0));
+            MARK("gate_fanout");
+        }
+        return 0;
+    };
+    const bool mid_split = mid_split_for_throughput(B);
+    const bool qkv_many = tc && (int64_t)B * T >= NUM_SMS;
+    const bool attn_tiled = T > 1 && (int64_t)B * NHEAD * ((T + ATT_TQ - 1) / ATT_TQ) >= NUM_SMS;
     if (fused_tail) {      // the frame as 13 row tiles: spectrum of the tile's bins, conv, and block 0's input projection
-        CK(launch_k(false, front1_kernel_t<Map>, dim3(TAIL_TILES + 1, B), dim3(256), FRONT1_SMEM, st, x, xbs, xcs, x_len, X, state, recs, e->w,
-                    e->bw[0], GX, a.pos_rel, emb, PRE, active));
+        CK(launch_k(false, front1_kernel_t<Map>, dim3(TAIL_TILES + gate_ctas, B0), dim3(256), FRONT1_SMEM, st, x, xbs, xcs, x_len, X0, state,
+                    recs0, e->w, e->bw[0], GX, a.pos_rel, emb, PRE, active));
     } else if ((T > 1 || tc) && e->use_back_many) {      // many frames / streams: one CTA walks (stream, chunk) items (one CTA per SM: 150 KB of filters)
-        const int per_stream = std::max(1, NUM_SMS / B);
+        const int per_stream = std::max(1, NUM_SMS / B0);
         const int chunk = (T + per_stream - 1) / per_stream;
         const int n_chunks = (T + chunk - 1) / chunk;
-        const int n_workers = std::min(NUM_SMS, B * n_chunks);
-        CK(launch_k(false, front_many_kernel_t<Map>, dim3(n_workers + B, 1), dim3(256), FRONT_SMEM, st, x, xbs, xcs, x_len, X, state, recs, e->w, T,
-                    a.pos_rel, emb, PRE, chunk, n_chunks, B, n_workers, active));
+        const int n_workers = std::min(NUM_SMS, B0 * n_chunks);
+        CK(launch_k(false, front_many_kernel_t<Map>, dim3(n_workers + gate_ctas * B0, 1), dim3(256), FRONT_SMEM, st, x, xbs, xcs, x_len, X0, state,
+                    recs0, e->w, T, a.pos_rel, emb, PRE, chunk, n_chunks, B0, n_workers, active));
     } else {
-        CK(launch_k(false, front_kernel_t<Map>, dim3(T + 1, B), dim3(256), FRONT_SMEM, st, x, xbs, xcs, x_len, X, state, recs, e->w, T,
+        CK(launch_k(false, front_kernel_t<Map>, dim3(T + gate_ctas, B0), dim3(256), FRONT_SMEM, st, x, xbs, xcs, x_len, X0, state, recs0, e->w, T,
                     a.pos_rel, emb, PRE, 0, 1, 0, active));
     }
     MARK("front");
     if (int rc = do_tap()) return rc;
 
+    const int B_all = B;
+    const int64_t ss_all = ss;
+    const Map recs_all = recs;
+    float* const X_all = X;
     for (int b = 0; b < e->n_blocks; ++b) {
+        if (K > 1 && b == 1) { if (int rc = fan_out()) return rc; }
+        // inside a block, B / rows / ss / recs / X are the block's own: for block 0 of a targets call those of the mixtures'
+        // lead records (see above), else the call's
+        const bool lead = K > 1 && b == 0;
+        const int B = lead ? B0 : B_all;
+        const int64_t rows = (int64_t)B * T * NF;
+        const int64_t ss = lead ? ss_all * K : ss_all;
+        const Map recs = lead ? recs0 : recs_all;
+        float* const X = lead ? X0 : X_all;
+        const int form_scale = lead ? K : 1;      // the recurrences' forms are chosen for the call's rows too
         const BlockWeights& W = e->bw[b];
         // ---- intra: LN -> W_ih (both directions) -> BiLSTM over F -> Linear -> +res ------------
         GemmArgs g{};
@@ -450,7 +496,7 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
         l.gx = GX; l.gx_ld = 512; l.out = Y; l.out_ld = 128; l.whh = W.whh1;
         l.nseq = B * T; l.L = NF; l.inner_count = 1; l.outer_stride = NF; l.inner_stride = 0; l.step_stride = 1;
         l.ndir = 2;
-        if (tc_fused_lstm(e, l)) {
+        if (tc_fused_lstm(e, l, form_scale)) {
             // many sequences: LayerNorm, W_ih and the recurrence in ONE tensor-core kernel (no [rows x 512] projection in HBM)
             tcl::LstmXArgs xa{};
             xa.l = l; xa.x = X; xa.x_ld = 64;
@@ -459,8 +505,9 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
             CK(launch_tc_lstm_x(xa, e->tc_passes, st, false));
             MARK("gemm_ih_intra");
         } else {
-            if (fused_tail) {
+            if (fused_tail && !(K > 1 && b == 1)) {
                 // front1_kernel (block 0) / the previous block's tail_kernel (its phase G) already wrote this block's input projection
+                // (not for block 1 of a targets call: block 0's tail ran per mixture, before the gate; the rows GEMM below does)
             } else if (tc) {
                 e->cur_pdl = (e->tc_pdl & 2) != 0 && a.prof == nullptr;
                 if (int rc = tc_rows_gemm(e, b, PL_IH1, X, 64, 64, 512, W.ln1_g, W.ln1_b, W.b1, nullptr, nullptr, GX, 512, rows, st)) return rc;
@@ -471,7 +518,7 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
                 CK(launch_rows_gemm(g, st, pdl));
             }
             MARK("gemm_ih_intra");
-            CK(lstm_any(e, l, st, pdl));
+            CK(lstm_any(e, l, st, pdl, form_scale));
         }
         MARK("lstm_intra");
         if (tc_mid) {
@@ -505,7 +552,7 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
             if (int rc = tc_rows_gemm(e, b, PL_QKV, X, 64, 64, NQKV, nullptr, nullptr, W.bqkv, W.slope_vec, nullptr, QKVRAW, NQKV, rows, st)) return rc;
             e->cur_pdl = false;
             MARK("mid");
-        } else if (row_mid && mid_split_for_throughput(B)) {
+        } else if (row_mid && mid_split) {
             float* GI = GX; float* HN = GX + rows * 256;         // the BiLSTM is done with GX
             CK(launch_k(pdl, mid_a_kernel, mid_grid_for(B, 2), dim3(256), MID_A_SMEM, st, (const float*)Y, X, GI, W, B, (int64_t)0, 1));
             CK(launch_k(pdl, mid_b_kernel_t<Map>, mid_grid_for(B, 3), dim3(256), MID_B_SMEM, st, (const float*)GI, HN, (int64_t)0, 1, state, recs, b, W, B,
@@ -514,12 +561,12 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
             MARK("mid");
         } else if (fused_tail) {
             NextIh nx{};
-            if (b + 1 < e->n_blocks) {
+            if (b + 1 < e->n_blocks && !lead) {
                 const BlockWeights& Wn = e->bw[b + 1];
                 nx.ln_g = Wn.ln1_g; nx.ln_b = Wn.ln1_b; nx.wih_t = Wn.wih1_t; nx.bias = Wn.b1; nx.GX = GX;
             }
             CK(launch_cluster(pdl, dim3(TAIL_CL, 1, 1), tail_kernel_t<Map>, dim3(TAIL_CL, B), dim3(256), TAIL_SMEM, st, (const float*)Y, X, state, recs,
-                              b, W, nx, (b == 0 && e->n_blocks > 1) ? 1 : 0, 0, active));
+                              b, W, nx, (b == 0 && e->n_blocks > 1 && K == 1) ? 1 : 0, 0, active));
             MARK("tail");
             if (int rc = do_tap()) return rc;
             continue;
@@ -551,7 +598,7 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
             }
             l.nseq = B * NF; l.L = T; l.inner_count = NF; l.outer_stride = (int64_t)T * NF; l.inner_stride = 1;
             l.step_stride = NF; l.ndir = 1;
-            if (tc_fused_lstm(e, l)) {
+            if (tc_fused_lstm(e, l, form_scale)) {
                 tcl::LstmXArgs xa{};
                 xa.l = l; xa.x = X; xa.x_ld = 64;
                 xa.wih_hi = e->pack.planes + e->plane_of[(size_t)b * PL_PER_BLOCK + PL_IH2]; xa.wih_lo = xa.wih_hi + e->pack.planes_total;
@@ -572,7 +619,7 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
                 if constexpr (std::is_same_v<Map, Records>) {
                     if (recs.hops) CK(launch_k(false, inter_gate_mask_kernel, dim3(T, B), dim3(256), 0, st, GX, recs, T));
                 }
-                CK(lstm_any(e, l, st, pdl));
+                CK(lstm_any(e, l, st, pdl, form_scale));
             }
             MARK("lstm_inter");
             if constexpr (std::is_same_v<Map, Records>) {
@@ -603,7 +650,7 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
         if (tc && !tc_mid) {      // Q|K|V projections of all rows as one tensor-core GEMM (+ bias + PReLU per column)
             if (int rc = tc_rows_gemm(e, b, PL_QKV, X, 64, 64, NQKV, nullptr, nullptr, W.bqkv, W.slope_vec, nullptr, QKVRAW, NQKV, rows, st)) return rc;
         }
-        if (tc && (int64_t)B * T >= NUM_SMS) {      // many frames: persistent form (LayerNorm parameters staged once per CTA), one wave
+        if (qkv_many) {      // many frames: persistent form (LayerNorm parameters staged once per CTA), one wave
             static int wave[64] = {};
             const int64_t grid_q = std::min<int64_t>(resident_ctas(wave, qkv_many_kernel_t<Map>, QKV_THREADS, QKV_MANY_SMEM), (int64_t)B * T);
             CK(launch_k(pdl || ((e->tc_pdl & 4) != 0 && a.prof == nullptr), qkv_many_kernel_t<Map>, dim3((unsigned)grid_q), dim3(QKV_THREADS), QKV_MANY_SMEM, st, (const float*)QKVRAW, Q, KALL, VALL, state, recs,
@@ -616,7 +663,7 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
         if (nsplit > 1) {
             CK(launch_cluster(pdl, dim3(1, ATT_CL, 1), attn_cluster_kernel_t<Map>, dim3(T, NHEAD * ATT_CL, B), dim3(256), 0, st,
                               (const float*)Q, (const float*)KALL, (const float*)VALL, (const float*)state, recs, b, Z, T, 0));
-        } else if (T > 1 && (int64_t)B * NHEAD * ((T + ATT_TQ - 1) / ATT_TQ) >= NUM_SMS) {   // enough tiles to fill the GPU: query-tiled,
+        } else if (attn_tiled) {   // enough tiles to fill the GPU: query-tiled,
             // one pass over 57 rows serves 8 queries
             CK(launch_k(pdl, attn_tile_kernel, dim3((T + ATT_TQ - 1) / ATT_TQ, NHEAD, B), dim3(256), 0, st, (const float*)Q,
                         (const float*)KALL, (const float*)VALL, Z, T));
@@ -631,14 +678,15 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
             if (int rc = tc_rows_gemm(e, b, PL_P, Z, 64, 64, 64, nullptr, nullptr, W.bp, nullptr, nullptr, Y, 64, rows, st, W.slopes + 3)) return rc;
             e->cur_pdl = false;
             CK(launch_k(pdl || p2, ln_frame_res_kernel_t<Map>, dim3(T, B), dim3(256), 0, st, (const float*)Y, X, (const float*)state, recs, W,
-                        (b == 0 && e->n_blocks > 1) ? 1 : 0, T));
+                        (b == 0 && e->n_blocks > 1 && K == 1) ? 1 : 0, T));
         } else {
             CK(launch_k(pdl, attn_out_kernel_t<Map>, dim3(T, B), dim3(256), AOUT_SMEM, st, (const float*)Z, X, (const float*)state, recs, W,
-                        (b == 0 && e->n_blocks > 1) ? 1 : 0, T));
+                        (b == 0 && e->n_blocks > 1 && K == 1) ? 1 : 0, T));
         }
         MARK("attn_out");
         if (int rc = do_tap()) return rc;
     }
+    if (K > 1 && e->n_blocks == 1) { if (int rc = fan_out()) return rc; }
     if ((T > 1 || tc) && e->use_back_many) {
         // many frames (or many streams): one cluster walks (stream, chunk-of-frames) items -- filters loaded once per cluster, rows
         // staged once; as many clusters as stay resident together (3 CTAs of 72 KB per SM)
@@ -912,7 +960,7 @@ static void drop_graphs(SepEngine* e) {
 static std::vector<int64_t> graph_key(const ChainArgs& a, int t) {
     return {(int64_t)a.x, a.xbs, a.xcs, a.x_len, (int64_t)a.emb, (int64_t)a.state, (int64_t)a.y,
             a.ybs, a.ycs, a.y_len, a.B, t, (int64_t)a.wsp, (int64_t)a.flags, a.pos_rel, (int64_t)a.active,
-            (int64_t)a.slots, a.state_batch, (int64_t)a.hops};
+            (int64_t)a.slots, a.state_batch, (int64_t)a.hops, a.targets};
 }
 
 // Launch the graph cached under `key` on `st`.  The first time a key is seen, `enqueue(cap)` is captured on the private
@@ -1258,6 +1306,24 @@ int l2h_sep_forward_active(void* handle, const float* x, int64_t xbs, int64_t xc
     ChainArgs a{x, xbs, xcs, x_len, emb, static_cast<float*>(state), y, ybs, ycs, y_len, batch, frames,
                 static_cast<float*>(ws), ws_bytes, flags & ~L2H_FLAG_GRAPH, 0};
     a.active = active_dev;
+    return run_chain(e, a, static_cast<cudaStream_t>(stream), (flags & L2H_FLAG_GRAPH) != 0);
+}
+
+int l2h_sep_forward_targets(void* handle, const float* x, int64_t xbs, int64_t xcs, int32_t x_len, const float* emb,
+                            void* state, float* y, int64_t ybs, int64_t ycs, int32_t y_len, int32_t batch, int32_t n_targets,
+                            int32_t frames, void* ws, size_t ws_bytes, uint32_t flags, void* stream) {
+    SepEngine* e = static_cast<SepEngine*>(handle);
+    if (!e || !x || !emb || !state || !y || !ws) return fail(1, "null argument");
+    if (batch <= 0 || n_targets <= 0 || frames <= 0)
+        return fail(1, "a targets call needs batch, n_targets and frames > 0 (batch = " + std::to_string(batch) + ", n_targets = " +
+                           std::to_string(n_targets) + ", frames = " + std::to_string(frames) + ")");
+    if ((int64_t)batch * n_targets * frames * NF > 0x7fffffff / 2)
+        return fail(1, "batch*n_targets*frames too large for one call; split the batch");
+    if (flags & L2H_FLAG_TAPS) return fail(1, "a targets call cannot be combined with L2H_FLAG_TAPS");
+    if (int rc_dev = check_device(e)) return rc_dev;
+    ChainArgs a{x, xbs, xcs, x_len, emb, static_cast<float*>(state), y, ybs, ycs, y_len, batch * n_targets, frames,
+                static_cast<float*>(ws), ws_bytes, flags & ~L2H_FLAG_GRAPH, 0};
+    a.targets = n_targets;
     return run_chain(e, a, static_cast<cudaStream_t>(stream), (flags & L2H_FLAG_GRAPH) != 0);
 }
 

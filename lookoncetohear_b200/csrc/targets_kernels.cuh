@@ -1,0 +1,46 @@
+// Kernels of the calls that extract several targets per mixture (l2h_sep_forward_targets).  The front and block 0 do not
+// depend on the speaker, so such a call runs them once per mixture, without the gate; the two kernels below then give each
+// target row its own gated copy of block 0's output.  (Included after every other kernel header: defining them earlier in
+// the module would move the code generated for kernels that do not use them.)
+#pragma once
+#include "sep_kernels.cuh"
+
+namespace l2h {
+
+// The speaker-gate memo of every target row: one CTA per row, as the extra CTA of front_kernel builds or validates it in a
+// dense call.  grid (target rows), 256 threads.
+template <class Map>
+__global__ void __launch_bounds__(256)
+spk_gate_kernel_t(const float* __restrict__ emb, float* __restrict__ spk_pre, float* __restrict__ state, Map recs, SepWeights w) {
+    __shared__ __align__(16) float red[288];
+    griddep_launch();
+    griddep_wait();
+    spk_gate_cta(emb, spk_pre, state, recs, w, (int)blockIdx.x, red, nullptr);
+}
+
+// X[i*K + k] = X0[i] * gate of record i*K + k, elementwise over the [T][97][64] rows: block 0's output of mixture i becomes
+// block 1's input for each of its K targets.  The multiply is the one attn_out_kernel / ln_frame_res_kernel / tail_kernel
+// apply with their gate flag (tfgridnet_causal.py:250-251); with one block the gate never applies (apply_gate = 0) and this
+// is a plain copy.  X0 and X do not overlap.  grid (T, target rows), 256 threads.
+__global__ void __launch_bounds__(256)
+gate_fanout_kernel(const float* __restrict__ X0, float* __restrict__ X, const float* __restrict__ state, int64_t sstride,
+                   int n_targets, int T, int apply_gate) {
+    griddep_launch();
+    griddep_wait();
+    const int t = blockIdx.x, r = blockIdx.y;
+    const float4* src = reinterpret_cast<const float4*>(X0 + ((int64_t)(r / n_targets) * T + t) * FC);
+    float4* dst = reinterpret_cast<float4*>(X + ((int64_t)r * T + t) * FC);
+    const float4* gate = reinterpret_cast<const float4*>(stream_rec(state, sstride, r) + ST_GATE);
+    for (int i = threadIdx.x; i < FC / 4; i += 256) {
+        float4 v = src[i];
+        if (apply_gate) {
+            const float4 g = gate[i];
+            v.x *= g.x; v.y *= g.y; v.z *= g.z; v.w *= g.w;
+        }
+        dst[i] = v;
+    }
+}
+
+constexpr auto spk_gate_kernel = spk_gate_kernel_t<int64_t>;
+
+}  // namespace l2h

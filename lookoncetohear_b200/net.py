@@ -103,6 +103,10 @@ class SepState(dict):
     Every stream (slot) has its own frame clock, so the streams of one state need not start together or
     advance on every hop: ``reset_streams`` starts fresh streams in some slots, ``Net.predict(..., active=)``
     advances only some streams, ``copy_streams_from`` moves streams between slots and states.
+
+    A state that ``Net.predict_targets`` runs holds groups of K records, one per target of a mixture.  Only the group's
+    lead record (slot i*K) holds the mixture's conv tails and block 0's rings and (h, c), so a non-lead record is not a
+    standalone stream: it continues only inside its group.  Resetting or copying whole groups keeps working.
     """
 
     _OFFSET_NAMES = ("ring", "k_ld", "k_dim", "v_dim", "att", "st_emb", "st_gate", "st_conv", "st_deconv",
@@ -581,6 +585,70 @@ class Net(nn.Module):
             st = self.init_buffers(xs.shape[0], x.device)
             outs.append(self.predict(xs, es, st, pad)[0])
         return torch.cat(outs, dim=0)
+
+    # ---- several targets per mixture ---------------------------------------------------------
+    def _targets_shape(self, x, embeds):
+        """(B, K) of x [B, M, N] and embeds [B, K, 256], or ValueError."""
+        if x.dim() != 3:
+            raise ValueError(f"x must have shape [B, channels, N], got {tuple(x.shape)}")
+        if (not isinstance(embeds, torch.Tensor) or embeds.dim() != 3 or embeds.shape[0] != x.shape[0]
+                or embeds.shape[1] < 1 or embeds.shape[2] != self.embed_dim):
+            shape = tuple(embeds.shape) if isinstance(embeds, torch.Tensor) else type(embeds).__name__
+            raise ValueError(f"embeds must have shape [B, K, {self.embed_dim}] with B = {x.shape[0]} mixtures and K >= 1 "
+                             f"targets, got {shape}")
+        return x.shape[0], embeds.shape[1]
+
+    def predict_targets(self, x, embeds, state, pad=True):
+        """Extract K enrolled speakers from each of B mixtures in one call (l2h_sep_forward_targets).  x [B,M,N]; embeds
+        [B,K,256], one embedding per target; state from init_buffers(B*K), in groups of K records: record i*K + k is target
+        k of mixture i.  Returns (y [B,K,S,*], state); `pad` as for predict (pad=False with 128*T + 64 samples is a T-hop
+        call).
+
+        The front and block 0 do not depend on the speaker, so they run once per mixture, on the group's lead record
+        i*K; the other records of a group never hold them, which makes a non-lead record no standalone stream (see
+        SepState).  Each target gets the output of predict on its mixture alone, up to the rounding of one stage in the
+        fused one-hop form (include/lookonce_b200.h)."""
+        Bsz, K = self._targets_shape(x, embeds)
+        hop, la = self.stft_chunk_size, self.stft_pad_size
+        n = x.shape[-1]
+        if pad:
+            frames, out_len = (n + hop - 1) // hop, n
+        else:
+            if (n - la) % hop != 0 or n < hop + la:
+                raise ValueError(f"pad=False needs {hop}*T+{la} samples, got {n}")
+            frames = (n - la) // hop
+            out_len = frames * hop
+        if not isinstance(state, SepState):
+            raise TypeError("state must come from Net.init_buffers()")
+        if state.batch != Bsz * K:
+            raise ValueError(f"state was built for batch {state.batch}, a call of {Bsz} mixtures x {K} targets needs "
+                             f"init_buffers({Bsz * K})")
+        self._require_cuda(x)
+        dev = x.device
+        self._sync_weights(dev)
+        x = x.contiguous().float()
+        emb = embeds.to(dev, torch.float32).reshape(Bsz * K, self.embed_dim).contiguous()
+        y = torch.empty(Bsz, K, self.num_src, out_len, dtype=torch.float32, device=dev)
+        ws, _ = self._workspace(dev, Bsz * K, frames)
+        with torch.cuda.device(dev):
+            _cabi.check_args(_cabi.lib().l2h_sep_forward_targets(
+                self._engine(), x.data_ptr(), x.stride(0), x.stride(1), n, emb.data_ptr(), state.buf.data_ptr(),
+                y.data_ptr(), y.stride(1), y.stride(2), out_len, Bsz, K, frames, ws.data_ptr(), ws.numel(), 0,
+                torch.cuda.current_stream(dev).cuda_stream))
+        return y, state
+
+    def forward_targets(self, x, embeds):
+        """x [B,M,N], embeds [B,K,256] -> [B,K,S,N]: every mixture separated for each of its K targets, on a fresh state,
+        padded as forward() pads.  Long batches are split as forward() splits them, counting target rows."""
+        Bsz, K = self._targets_shape(x, embeds)
+        frames = (x.shape[-1] + self.stft_chunk_size - 1) // self.stft_chunk_size
+        per = max(1, self.max_frames_per_launch // max(frames * K, 1))
+        outs = []
+        for b0 in range(0, Bsz, per):
+            xs, es = x[b0:b0 + per], embeds[b0:b0 + per]
+            st = self.init_buffers(xs.shape[0] * K, x.device)
+            outs.append(self.predict_targets(xs, es, st)[0])
+        return outs[0] if len(outs) == 1 else torch.cat(outs, dim=0)
 
     def stream_dev(self, x_dev, embed_dev, chunks_per_call=1, state=None, n_calls=None, out=None):
         """Streaming over a device-resident clip (l2h_sep_stream_dev): x_dev [B,M,N] is consumed
