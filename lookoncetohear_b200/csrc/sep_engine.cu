@@ -20,9 +20,7 @@
 #include "umma_host.cuh"
 #include "tc_lstm.cuh"
 #include "lstm.cuh"
-#include "sep_kernels.cuh"
-#include "mid_kernel.cuh"
-#include "hop_kernels.cuh"
+#include "sep_launch.cuh"
 #include "targets_kernels.cuh"
 
 namespace l2h {
@@ -44,7 +42,6 @@ struct SepEngine {
     WeightPack pack;                // packed weights; pack.device also owns the streams, events and cached graphs below
     int64_t weight_gen = 0;         // bumped by every commit
     std::vector<int64_t> plane_of;      // per block: plane offsets (pack.plane) of wih1, wl1, wih2, wl2, wqkv, [wih2|whh2], wp
-    bool cur_pdl = false;              // PDL attribute for the tensor-core launches of the chain being enqueued
     bool fuse_ih = false;               // many sequences: W_ih + LayerNorm inside the tensor-core recurrence (option "fuse_ih", default off)
     int tc_passes = 3;                  // 3 = bf16x3 split products (fp32 configs); 2 = bf16 weights x split activations (option
                                         // "bf16" = 1: the offline bf16 configuration); 1 = plain bf16 operands ("bf16" = 2)
@@ -205,18 +202,21 @@ static void build_layout(SepEngine* e) {
     }
 }
 
-// ---- workspace carve-up (floats) ---------------------------------------------------------------
+// ---- the call's form: predicates shared by the chain (chain_form), the workspace and the entry points ------------------
 constexpr int64_t TC_MIN_ROWS = 2048;      // calls of more rows run their dense contractions on the tensor cores: below this
                                            // the 16-row CUDA-core tiles win (one streaming frame = 97 rows)
+// many rows (whole utterances, offline batches, many streams): the dense contractions run on the tensor cores
+static bool tc_form(int B, int T) { return (int64_t)B * T * NF > TC_MIN_ROWS; }
+// one-frame calls: the row-local middle of every block runs as fused kernels (mid_kernel.cuh).  (Taps want the
+// intermediate activations of the generic chain, so they keep it.)
+static bool row_mid_form(int T, uint32_t flags) { return T == 1 && !(flags & L2H_FLAG_TAPS); }
+// both: the middle as tensor-core GEMMs and the cell update
+static bool tc_mid_form(int B, int T, uint32_t flags) { return tc_form(B, T) && row_mid_form(T, flags); }
+
+// ---- workspace carve-up (floats) ---------------------------------------------------------------
 struct Workspace {
     int64_t X, GX, Y, Z, Q, KALL, VALL, PRE, QKVRAW, TAPS, HG, total;
 };
-// few frames in flight -> split every head's 50-row window over several CTAs
-static int attn_splits(int B, int T) {
-    static int wave[64] = {};
-    const int ctas = B * T * NHEAD;
-    return (ctas * ATT_CL <= resident_ctas(wave, attn_cluster_kernel, 256, 0)) ? ATT_CL : 1;      // 8-CTA clusters while they all fit in one wave
-}
 
 static Workspace carve(int n_blocks, int B, int T, uint32_t flags) {
     Workspace ws;
@@ -235,19 +235,10 @@ static Workspace carve(int n_blocks, int B, int T, uint32_t flags) {
     ws.TAPS = alloc((flags & L2H_FLAG_TAPS) ? (int64_t)(1 + 3 * n_blocks) * rows * 64 : 0);
     // the listed records' carried inter-LSTM state of every block for a slot-list call (gather_h_kernel): h for one-hop
     // calls in the tensor-core form, h and c ([n_blocks][B][97][64] each) for every multi-hop call
-    const bool tc_hop = T == 1 && rows > TC_MIN_ROWS && !(flags & L2H_FLAG_TAPS);
-    ws.HG = alloc((T > 1 ? 2 : tc_hop ? 1 : 0) * (int64_t)n_blocks * B * FC);
+    ws.HG = alloc((T > 1 ? 2 : tc_mid_form(B, T, flags) ? 1 : 0) * (int64_t)n_blocks * B * FC);
     ws.total = (cur + 511) & ~int64_t(511);      // a multiple of one GX row: pipelined hops address their slots as rows of one tensor
     return ws;
 }
-
-// grids of the mid-section kernels: persistent over (stream, row tile) items, as many CTAs per SM as their shared memory
-// allows (fused 225 KB -> 1, mid_a 107 KB -> 2, mid_b 68 KB -> 3, mid_c 50 KB -> 4)
-static inline int mid_items(int B) { return B * ((NF + MID_RT - 1) / MID_RT); }
-static inline dim3 mid_grid_for(int B, int ctas_per_sm) { return dim3(std::min(NUM_SMS * ctas_per_sm, mid_items(B))); }
-// many streams: the section is throughput-bound and one fused CTA per SM (8 warps) cannot hide its own latencies; the
-// three smaller kernels run 2-4 CTAs per SM (same arithmetic, +3 small global round trips)
-static inline bool mid_split_for_throughput(int B) { return mid_items(B) > NUM_SMS; }
 
 // cudaFuncSetAttribute applies to the CURRENT device: keep one flag per device ordinal
 static bool g_attr_done[64] = {};
@@ -257,33 +248,14 @@ static int set_attrs() {
     CK(cudaGetDevice(&dev_ord));
     if (dev_ord < 0 || dev_ord >= 64) return fail(1, "device ordinal out of range");
     if (g_attr_done[dev_ord]) return 0;
-    CK(cudaFuncSetAttribute(qkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)QKV_SMEM));
-    CK(cudaFuncSetAttribute(qkv_many_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)QKV_MANY_SMEM));
-    CK(cudaFuncSetAttribute(attn_out_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AOUT_SMEM));
-    CK(cudaFuncSetAttribute(back_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BACK_SMEM));
-    CK(cudaFuncSetAttribute(back_many_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BACK_MANY_SMEM));
-    CK(cudaFuncSetAttribute(front_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FRONT_SMEM));
-    CK(cudaFuncSetAttribute(front_many_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FRONT_SMEM));
-    CK(cudaFuncSetAttribute(mid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_SMEM));
+    CK(set_sep_smem<int64_t>());
+    CK(set_sep_smem<Records>());      // the slot-list forms (l2h_sep_forward_slots)
     CK(cudaFuncSetAttribute(mid_a_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_A_SMEM));
-    CK(cudaFuncSetAttribute(mid_b_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_B_SMEM));
     CK(cudaFuncSetAttribute(mid_c_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_C_SMEM));
     CK(configure_rows_gemm());
     CK(configure_lstm());
     CK(umma::configure());
     CK(configure_tc_lstm());
-    CK(cudaFuncSetAttribute(front1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FRONT1_SMEM));
-    // the slot-list forms of the kernels above (l2h_sep_forward_slots)
-    CK(cudaFuncSetAttribute(qkv_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)QKV_SMEM));
-    CK(cudaFuncSetAttribute(qkv_many_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)QKV_MANY_SMEM));
-    CK(cudaFuncSetAttribute(attn_out_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AOUT_SMEM));
-    CK(cudaFuncSetAttribute(back_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BACK_SMEM));
-    CK(cudaFuncSetAttribute(back_many_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BACK_MANY_SMEM));
-    CK(cudaFuncSetAttribute(front_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FRONT_SMEM));
-    CK(cudaFuncSetAttribute(front_many_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FRONT_SMEM));
-    CK(cudaFuncSetAttribute(mid_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_SMEM));
-    CK(cudaFuncSetAttribute(mid_b_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_B_SMEM));
-    CK(cudaFuncSetAttribute(front1_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FRONT1_SMEM));
     {   // tail_kernel: 16 CTAs per cluster is a non-portable size; ask whether this device can place it
         g_tail_clusters[dev_ord] = 0;
         if (cudaFuncSetAttribute(tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TAIL_SMEM) == cudaSuccess &&
@@ -315,22 +287,10 @@ static umma::BPlanes tc_planes(const SepEngine* e, int blk, int which, int ld) {
     return e->pack.bplanes(e->plane_of[(size_t)blk * PL_PER_BLOCK + which], ld);
 }
 
-// the recurrence: tensor cores when there are enough sequences to fill the GPU with 32-sequence CTAs, else lstm.cuh.
-// `scale`: the form is chosen for scale times l's sequences (block 0 of a targets call runs for all the target rows)
-static cudaError_t lstm_any(SepEngine* e, const LstmArgs& l, cudaStream_t st, bool pdl, int scale = 1) {
-    if ((int64_t)l.nseq * l.ndir * scale >= e->tcl_min_seqdirs) return launch_tc_lstm(l, e->tc_passes, st, pdl);
-    return launch_lstm_rec(l, st, pdl, scale > 1 ? l.nseq * scale : 0);
-}
-
-// ... and with enough sequences the input projection moves into the recurrence kernel too (tc_lstm_x_kernel)
-static bool tc_fused_lstm(const SepEngine* e, const LstmArgs& l, int scale = 1) {
-    return e->fuse_ih && (int64_t)l.nseq * l.ndir * scale >= e->tcl_min_seqdirs;
-}
-
 // C[rows][N] = epi(LN?(A[rows][lda, first K]) W^T + bias) (+ R), plain row-major rows
 static int tc_rows_gemm(SepEngine* e, int blk, int which, const float* A, int64_t lda, int K, int N, const float* ln_g, const float* ln_b,
                         const float* bias, const float* prelu_vec, const float* R, float* C, int64_t ldc, int64_t rows, cudaStream_t st,
-                        const float* prelu_scalar = nullptr) {
+                        bool pdl, const float* prelu_scalar = nullptr) {
     umma::GemmDesc g;
     g.a0.base = A; g.a0.channels = K; g.a0.n_pos = rows; g.a0.pos_stride = lda;
     umma::set_plain_chunks(g, K, ln_g != nullptr);
@@ -338,7 +298,7 @@ static int tc_rows_gemm(SepEngine* e, int blk, int which, const float* A, int64_
     g.rows_per_seq = (int)rows; g.nseq = 1;
     g.b = tc_planes(e, blk, which, K); g.N = N; g.K = K; g.passes = e->tc_passes;
     g.bias = bias; g.prelu_vec = prelu_vec; g.prelu = prelu_scalar; g.R = R; g.C = C; g.ldc = ldc;
-    g.pdl = e->cur_pdl;
+    g.pdl = pdl;
     std::string why;
     const cudaError_t ce = umma::launch(g, st, &why);
     if (ce != cudaSuccess) return fail(3, std::string("umma_gemm: ") + cudaGetErrorString(ce) + " " + why);
@@ -370,341 +330,386 @@ struct ChainArgs {
     int targets = 1;                     // l2h_sep_forward_targets: rows per mixture (B counts target rows; x has B / targets)
 };
 
-// Map: the record stride (dense calls) or Records (slot-list calls), see row_record in sep_kernels.cuh
+// few streams, one hop (the latency path): everything after the BiLSTM as one 16-CTA cluster kernel per stream, while all
+// B clusters of the launch are resident at once
+static bool tail_fits(const SepEngine* e, int B) {
+    int dev_ord = 0;
+    cudaGetDevice(&dev_ord);
+    return e->use_tail && dev_ord >= 0 && dev_ord < 64 && B <= g_tail_clusters[dev_ord];
+}
+
+// The form of one call, chosen once from its rows (B, T), its flags and the engine's options.  Block 0 of a targets call
+// runs these same forms over the mixtures' rows; grids follow the rows of the block being launched.
+struct RecForm {
+    bool tc;       // the recurrence on the tensor cores (enough sequences to fill the GPU with 32-sequence CTAs), else lstm.cuh
+    bool fused;    // ... with LayerNorm and W_ih inside the recurrence kernel (tc_lstm_x_kernel, option "fuse_ih")
+};
+struct ChainForm {
+    bool row_mid, tc, tc_mid, fused_tail;
+    bool mid_split;     // row_mid: mid_a / mid_b / mid_c instead of one mid_kernel (mid_split_for_throughput)
+    bool walkers;       // front_many_kernel / back_many_kernel: CTAs (clusters) walk (stream, chunk-of-frames) items
+    bool qkv_many;      // many frames: the persistent qkv_many_kernel, on at most qkv_ctas CTAs (one wave)
+    int qkv_ctas;
+    bool attn_tiled;    // enough query tiles to fill the GPU: attn_tile_kernel (one pass over 57 rows serves 8 queries)
+    int nsplit;         // attn_splits
+    RecForm intra, inter;
+    // programmatic dependent launch pays on the latency chain of a few rows; with many rows early-launched dependents park
+    // on the SMs the big kernels need, so tensor-core chains take it only where option "tc_pdl" asks: bit 0 the many-stream
+    // mid section, bit 1 W_ih and the out projection + its LayerNorm kernel, bit 2 the persistent qkv kernel
+    bool pdl, mid_pdl, gemm_pdl, qkv_pdl;
+};
+
 template <class Map>
-static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Map recs) {
-    const float* x = a.x; const int64_t xbs = a.xbs, xcs = a.xcs; const int x_len = a.x_len;
-    const float* emb = a.emb; float* state = a.state; float* y = a.y;
-    const int64_t ybs = a.ybs, ycs = a.ycs; const int y_len = a.y_len, B = a.B, T = a.T;
-    float* wsp = a.wsp; const size_t ws_bytes = a.ws_bytes; const uint32_t flags = a.flags;
-    const uint8_t* active = a.active;
-    if (!e->pack.committed) return fail(4, "weights not committed");
-    if (B <= 0 || T <= 0) return fail(1, "batch and frames must be positive");
-    const Workspace ws = carve(e->n_blocks, B, T, flags);
-    if ((size_t)ws.total * sizeof(float) > ws_bytes) return fail(1, "workspace too small");
-    if (int rc = set_attrs()) return rc;
-    const int64_t ss = stream_stride(e->n_blocks);
-    const int64_t rows = (int64_t)B * T * NF;
-    if (rows > 0x7fffffff / 2) return fail(1, "batch*frames too large for one call; split the batch");
-    float* X = wsp + ws.X; float* GX = wsp + ws.GX; float* Y = wsp + ws.Y; float* Z = wsp + ws.Z;
-    float* Q = wsp + ws.Q; float* KALL = wsp + ws.KALL; float* VALL = wsp + ws.VALL; float* PRE = wsp + ws.PRE;
-    float* TAPS = wsp + ws.TAPS;
-    float* QKVRAW = wsp + ws.QKVRAW;
-    float* HG = wsp + ws.HG;
-    const int nsplit = attn_splits(B, T);
-    // one-frame calls: the row-local middle of every block runs as ONE fused kernel (mid_kernel.cuh).
-    // (Taps want the intermediate activations of the generic chain, so they keep it.)
-    const bool row_mid = (T == 1) && !(flags & L2H_FLAG_TAPS);
-    // many rows (whole utterances, offline batches, many streams): the dense contractions run on the tensor cores
-    const bool tc = rows > TC_MIN_ROWS;
-    const bool tc_mid = tc && T == 1 && !(flags & L2H_FLAG_TAPS);
-    // few streams, one hop (the latency path): everything after the BiLSTM as one cluster kernel per stream
-    bool fused_tail = false;
-    if (row_mid && !tc && e->use_tail) {
-        int dev_ord = 0;
-        CK(cudaGetDevice(&dev_ord));
-        fused_tail = B <= g_tail_clusters[dev_ord];      // all clusters of the launch resident at once
+static ChainForm chain_form(const SepEngine* e, int B, int T, uint32_t flags, bool profiled) {
+    ChainForm f{};
+    f.row_mid = row_mid_form(T, flags);
+    f.tc = tc_form(B, T);
+    f.tc_mid = tc_mid_form(B, T, flags);
+    f.fused_tail = f.row_mid && !f.tc && tail_fits(e, B);
+    f.mid_split = mid_split_for_throughput(B);
+    f.walkers = (T > 1 || f.tc) && e->use_back_many;
+    f.qkv_many = f.tc && (int64_t)B * T >= NUM_SMS;
+    if (f.qkv_many) {
+        static int wave[64] = {};
+        f.qkv_ctas = resident_ctas(wave, qkv_many_kernel_t<Map>, QKV_THREADS, QKV_MANY_SMEM);
     }
+    f.attn_tiled = T > 1 && (int64_t)B * NHEAD * ((T + ATT_TQ - 1) / ATT_TQ) >= NUM_SMS;
+    f.nsplit = attn_splits(B, T);
+    const auto rec = [e](int64_t seqdirs) { const bool tc = seqdirs >= e->tcl_min_seqdirs; return RecForm{tc, tc && e->fuse_ih}; };
+    f.intra = rec((int64_t)B * T * 2);      // (stream, frame) sequences over F, both directions
+    f.inter = rec((int64_t)B * NF);         // (stream, bin) sequences over T
+    f.pdl = e->use_pdl && !profiled && !(flags & L2H_FLAG_TAPS) && !f.tc;
+    f.mid_pdl = (e->tc_pdl & 1) != 0 && !profiled;
+    f.gemm_pdl = (e->tc_pdl & 2) != 0 && !profiled;
+    f.qkv_pdl = (e->tc_pdl & 4) != 0 && !profiled;
+    return f;
+}
+
+// The rows one block runs over: the call's, or for block 0 of a targets call the mixtures' (Chain::rows_of)
+template <class Map>
+struct BlockRows {
+    int B;              // streams
+    int64_t rows;       // B * T * 97
+    int64_t ss;         // record stride
+    Map recs;           // record map
+    float* X;           // the block's input and output
+    int scale;          // the recurrences take the form of scale x this block's sequences: the call's
+    bool ih_written;    // GX holds the intra input projection already: front1_kernel / the previous tail_kernel wrote it
+    int gate;           // 1: this block's attn_out (tail_kernel) builds the speaker gate
+};
+
+#define MARK(name) do { if (a.prof) { if (int _rc = a.prof->mark(name, st)) return _rc; } } while (0)
+
+// One call's chain: its arguments, form and workspace, and the steps enqueue_chain_t takes in several places or in one
+// record map's form only
+template <class Map>
+struct Chain {
+    static constexpr bool slots = std::is_same_v<Map, Records>;
+    SepEngine* e; const ChainArgs& a; cudaStream_t st; const ChainForm& f; Map recs;
+    int K;              // targets per mixture
+    int64_t ss;         // record stride
+    float *X, *GX, *Y, *Z, *Q, *KALL, *VALL, *PRE, *QKVRAW, *TAPS, *HG, *CG, *sbase;
     int tap = 0;
-    auto do_tap = [&]() -> int {
-        if (flags & L2H_FLAG_TAPS) {
+
+    Chain(SepEngine* e_, const ChainArgs& a_, cudaStream_t st_, const ChainForm& f_, Map recs_, const Workspace& ws)
+        : e(e_), a(a_), st(st_), f(f_), recs(recs_), K(a_.targets), ss(stream_stride(e_->n_blocks)) {
+        float* w = a.wsp;
+        X = w + ws.X; GX = w + ws.GX; Y = w + ws.Y; Z = w + ws.Z; Q = w + ws.Q; KALL = w + ws.KALL; VALL = w + ws.VALL;
+        PRE = w + ws.PRE; QKVRAW = w + ws.QKVRAW; TAPS = w + ws.TAPS; HG = w + ws.HG;
+        CG = HG + (int64_t)e->n_blocks * a.B * FC;
+        sbase = a.state + sizeof(StateHeader) / 4;
+    }
+
+    // Several targets per mixture (l2h_sep_forward_targets): B counts target rows, K per mixture, row i*K + k = target k of
+    // mixture i.  The front and block 0 do not depend on the speaker (its gate applies after block 0), so they run once
+    // per mixture: over B / K rows, on the lead records i*K (record stride K*ss), without the gate, into room in GX that
+    // block 0 leaves unused.  fan_out() then builds every target row's gate memo and its gated copy of block 0's output
+    // in X, and blocks 1 .. n_blocks-1 and the back run over all B rows.  Every form was chosen for the B rows, and
+    // block 0 runs those same forms, so a target row gets the arithmetic of a dense call with its mixture duplicated.
+    BlockRows<Map> rows_of(int b) const {
+        const bool lead = K > 1 && b == 0;
+        BlockRows<Map> r{lead ? a.B / K : a.B, 0, lead ? ss * K : ss, recs, X, lead ? K : 1,
+                         f.fused_tail && !fans_out_before(b), (b == 0 && e->n_blocks > 1 && K == 1) ? 1 : 0};
+        r.rows = (int64_t)r.B * a.T * NF;
+        if constexpr (!slots) {
+            if (lead) { r.recs = recs * K; r.X = GX + r.rows * 512; }
+        }
+        return r;
+    }
+    bool fans_out_before(int b) const { return K > 1 && b == 1; }      // b == n_blocks: before the back
+    int fan_out() {
+        if constexpr (!slots) {
+            CK(launch_k(f.pdl, spk_gate_kernel, dim3(a.B), dim3(256), 0, st, a.emb, PRE, a.state, recs, e->w));
+            CK(launch_k(f.pdl, gate_fanout_kernel, dim3(a.T, a.B), dim3(256), 0, st, (const float*)rows_of(0).X, X,
+                        (const float*)a.state, ss, K, a.T, e->n_blocks > 1 ? 1 : 0));
+            MARK("gate_fanout");
+        }
+        return 0;
+    }
+
+    int do_tap() {
+        if (a.flags & L2H_FLAG_TAPS) {
+            const int64_t rows = (int64_t)a.B * a.T * NF;
             CK(cudaMemcpyAsync(TAPS + (int64_t)tap * rows * 64, X, rows * 64 * sizeof(float), cudaMemcpyDeviceToDevice, st));
             ++tap;
         }
         return 0;
-    };
-    float* sbase = state + sizeof(StateHeader) / 4;
-    // programmatic dependent launch pays on the latency chain of a few rows; with many rows early-launched dependents park on the SMs the big kernels need
-    const bool pdl = e->use_pdl && a.prof == nullptr && !(flags & L2H_FLAG_TAPS) && !tc;
-    e->cur_pdl = false;
-#define MARK(name) do { if (a.prof) { if (int _rc = a.prof->mark(name, st)) return _rc; } } while (0)
-    MARK("start");
-    // slot lists: the listed records' h of every block, for the one-hop inter-step GEMMs, or their (h, c) for the
-    // multi-hop inter recurrences, which carry them in the workspace (HG, CG) until scatter_hc_kernel stores them back
-    const int64_t hc4 = (int64_t)e->n_blocks * B * FC / 4;      // float4s of one of them
-    float* CG = HG + (int64_t)e->n_blocks * B * FC;
-    if constexpr (std::is_same_v<Map, Records>) {
-        if (tc_mid || T > 1)
-            CK(launch_k(false, gather_h_kernel, dim3((unsigned)((hc4 + 255) / 256)), dim3(256), 0, st, (const float*)state, recs,
-                        e->n_blocks, B, HG, T > 1 ? CG : nullptr));
     }
-    // Several targets per mixture (l2h_sep_forward_targets): B counts target rows, K per mixture, row i*K + k = target k of
-    // mixture i.  The front and block 0 do not depend on the speaker (its gate applies after block 0), so they run once
-    // per mixture: over B0 rows, on the lead records i*K (record stride K*ss), without the gate, into X0 (room in GX that
-    // block 0 leaves unused).  fan_out() then builds every target row's gate memo and its gated copy of block 0's output
-    // in X, and blocks 1 .. n_blocks-1 and the back run over all B rows.  Every form above was chosen for the B rows, and
-    // block 0 runs those same forms, so a target row gets the arithmetic of a dense call with its mixture duplicated.
-    const int K = a.targets;
-    const int B0 = B / K;
-    Map recs0 = recs;
-    float* X0 = X;
-    if constexpr (std::is_same_v<Map, int64_t>) {
-        recs0 = recs * K;
-        if (K > 1) X0 = GX + (int64_t)B0 * T * NF * 512;
-    } else {
-        if (K > 1) return fail(1, "targets cannot be combined with a slot list");
+
+    // block b's dense layer `which` over R's rows, on the tensor cores or as the CUDA-core rows GEMM:
+    // LN -> W_ih (PL_IH1, PL_IH2: X -> GX) or Linear + residual (PL_L1, PL_L2: Y -> X)
+    int dense(int b, int which, const BlockRows<Map>& R, bool pdl) {
+        const BlockWeights& W = e->bw[b];
+        GemmArgs g{};
+        switch (which) {
+            case PL_IH1:
+                g.A = R.X; g.lda = 64; g.Wt = W.wih1_t; g.bias = W.b1; g.C = GX; g.ldc = 512; g.ln_g = W.ln1_g; g.ln_b = W.ln1_b; g.N = 512;
+                g.K = 64; break;
+            case PL_L1: g.A = Y; g.lda = 128; g.Wt = W.wl1_t; g.bias = W.bl1; g.C = R.X; g.ldc = 64; g.R = R.X; g.N = 64; g.K = 128; break;
+            case PL_IH2:
+                g.A = R.X; g.lda = 64; g.Wt = W.wih2_t; g.bias = W.b2; g.C = GX; g.ldc = 256; g.ln_g = W.ln2_g; g.ln_b = W.ln2_b; g.N = 256;
+                g.K = 64; break;
+            default: g.A = Y; g.lda = 64; g.Wt = W.wl2_t; g.bias = W.bl2; g.C = R.X; g.ldc = 64; g.R = R.X; g.N = 64; g.K = 64; break;
+        }
+        if (f.tc) return tc_rows_gemm(e, b, which, g.A, g.lda, g.K, g.N, g.ln_g, g.ln_b, g.bias, nullptr, g.R, g.C, g.ldc, R.rows, st, pdl);
+        g.M = (int)R.rows;
+        CK(launch_rows_gemm(g, st, pdl));
+        return 0;
     }
-    const int gate_ctas = K > 1 ? 0 : 1;      // the front's speaker-gate memo CTAs (one per row); fan_out() builds them here
-    auto fan_out = [&]() -> int {
-        if constexpr (std::is_same_v<Map, int64_t>) {
-            CK(launch_k(pdl, spk_gate_kernel, dim3(B), dim3(256), 0, st, emb, PRE, state, recs, e->w));
-            CK(launch_k(pdl, gate_fanout_kernel, dim3(T, B), dim3(256), 0, st, (const float*)X0, X, (const float*)state, ss, K, T,
-                        e->n_blocks > 1 ? 1 : 0));
-            MARK("gate_fanout");
+
+    // LayerNorm + W_ih + the recurrence of block b's intra (PL_IH1) or inter (PL_IH2) LSTM: one tensor-core kernel
+    // (no [rows x 512] projection in HBM), or the projection (unless written already), the ragged rows' gate mask and the
+    // recurrence
+    int ln_ih_recurrence(int b, const BlockRows<Map>& R, int which, const LstmArgs& l) {
+        const bool inter = which == PL_IH2;
+        const RecForm rf = inter ? f.inter : f.intra;
+        const BlockWeights& W = e->bw[b];
+        if (rf.fused) {
+            tcl::LstmXArgs xa{};
+            xa.l = l; xa.x = R.X; xa.x_ld = 64;
+            xa.wih_hi = e->pack.planes + e->plane_of[(size_t)b * PL_PER_BLOCK + which]; xa.wih_lo = xa.wih_hi + e->pack.planes_total;
+            xa.bias = inter ? W.b2 : W.b1; xa.ln_g = inter ? W.ln2_g : W.ln1_g; xa.ln_b = inter ? W.ln2_b : W.ln1_b;
+            if constexpr (slots) { if (inter) xa.steps = recs.hops; }      // ragged rows: masked inside
+            CK(launch_tc_lstm_x(xa, e->tc_passes, st, false));
+            MARK(inter ? "gemm_ih_inter" : "gemm_ih_intra");
+        } else {
+            if (!R.ih_written) {      // a tensor-core chain's intra W_ih takes "tc_pdl" bit 1
+                if (int rc = dense(b, which, R, f.tc && !inter ? f.gemm_pdl : f.pdl)) return rc;
+            }
+            MARK(inter ? "gemm_ih_inter" : "gemm_ih_intra");
+            if constexpr (slots) {
+                if (inter && recs.hops) CK(launch_k(false, inter_gate_mask_kernel, dim3(a.T, R.B), dim3(256), 0, st, GX, recs, a.T));
+            }
+            if (rf.tc) CK(launch_tc_lstm(l, e->tc_passes, st, f.pdl));
+            else CK(launch_lstm_rec(l, st, f.pdl, l.nseq * R.scale));
+        }
+        MARK(inter ? "lstm_inter" : "lstm_intra");
+        return 0;
+    }
+
+    // Slot lists: one-hop tensor-core chains read the listed records' h of every block for the inter-step GEMMs, and
+    // multi-hop calls carry their (h, c) through the inter recurrences, from a copy in the workspace (HG, CG) that
+    // gather_hc() takes before block 0 and scatter_hc() stores back after the last block's inter recurrence
+    int64_t hc4() const { return (int64_t)e->n_blocks * a.B * FC / 4; }      // float4s of one of h, c
+    int gather_hc() {
+        if constexpr (slots) {
+            if (f.tc_mid || a.T > 1)
+                CK(launch_k(false, gather_h_kernel, dim3((unsigned)((hc4() + 255) / 256)), dim3(256), 0, st, (const float*)a.state,
+                            recs, e->n_blocks, a.B, HG, a.T > 1 ? CG : nullptr));
         }
         return 0;
-    };
-    const bool mid_split = mid_split_for_throughput(B);
-    const bool qkv_many = tc && (int64_t)B * T >= NUM_SMS;
-    const bool attn_tiled = T > 1 && (int64_t)B * NHEAD * ((T + ATT_TQ - 1) / ATT_TQ) >= NUM_SMS;
-    if (fused_tail) {      // the frame as 13 row tiles: spectrum of the tile's bins, conv, and block 0's input projection
-        CK(launch_k(false, front1_kernel_t<Map>, dim3(TAIL_TILES + gate_ctas, B0), dim3(256), FRONT1_SMEM, st, x, xbs, xcs, x_len, X0, state,
-                    recs0, e->w, e->bw[0], GX, a.pos_rel, emb, PRE, active));
-    } else if ((T > 1 || tc) && e->use_back_many) {      // many frames / streams: one CTA walks (stream, chunk) items (one CTA per SM: 150 KB of filters)
-        const int per_stream = std::max(1, NUM_SMS / B0);
-        const int chunk = (T + per_stream - 1) / per_stream;
-        const int n_chunks = (T + chunk - 1) / chunk;
-        const int n_workers = std::min(NUM_SMS, B0 * n_chunks);
-        CK(launch_k(false, front_many_kernel_t<Map>, dim3(n_workers + gate_ctas * B0, 1), dim3(256), FRONT_SMEM, st, x, xbs, xcs, x_len, X0, state,
-                    recs0, e->w, T, a.pos_rel, emb, PRE, chunk, n_chunks, B0, n_workers, active));
+    }
+    void inter_hc(LstmArgs& l, int b, const BlockRows<Map>& R) const {      // where block b's inter recurrence carries (h, c)
+        if constexpr (slots) {
+            l.h_state = HG + (int64_t)b * R.B * FC;
+            l.c_state = CG + (int64_t)b * R.B * FC;
+            l.hc_outer_stride = FC;
+        } else {
+            l.h_state = sbase + ST_BLK + (int64_t)b * BK_STRIDE + BK_H;
+            l.c_state = sbase + ST_BLK + (int64_t)b * BK_STRIDE + BK_C;
+            l.hc_outer_stride = R.ss;
+        }
+    }
+    int h_last(int b) {      // a ragged row's h is that of its own last frame
+        if constexpr (slots) {
+            if (recs.hops)
+                CK(launch_k(false, inter_h_last_kernel, dim3(a.B), dim3(256), 0, st, (const float*)Y, HG + (int64_t)b * a.B * FC, recs, a.T));
+        }
+        return 0;
+    }
+    int scatter_hc() {
+        if constexpr (slots)
+            CK(launch_k(false, scatter_hc_kernel, dim3((unsigned)((hc4() + 255) / 256)), dim3(256), 0, st, a.state, recs, e->n_blocks,
+                        a.B, (const float*)HG, (const float*)CG));
+        return 0;
+    }
+};
+
+// Map: the record stride (dense calls) or Records (slot-list calls), see row_record in sep_kernels.cuh
+template <class Map>
+static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Map recs) {
+    const int T = a.T;
+    if (!e->pack.committed) return fail(4, "weights not committed");
+    if (a.B <= 0 || T <= 0) return fail(1, "batch and frames must be positive");
+    const Workspace ws = carve(e->n_blocks, a.B, T, a.flags);
+    if ((size_t)ws.total * sizeof(float) > a.ws_bytes) return fail(1, "workspace too small");
+    if (int rc = set_attrs()) return rc;
+    if ((int64_t)a.B * T * NF > 0x7fffffff / 2) return fail(1, "batch*frames too large for one call; split the batch");
+    if (Chain<Map>::slots && a.targets > 1) return fail(1, "targets cannot be combined with a slot list");
+    const ChainForm f = chain_form<Map>(e, a.B, T, a.flags, a.prof != nullptr);
+    Chain<Map> c(e, a, st, f, recs, ws);
+    MARK("start");
+    if (int rc = c.gather_hc()) return rc;
+    const BlockRows<Map> R0 = c.rows_of(0);           // the front runs over block 0's rows
+    const int gate_ctas = c.K > 1 ? 0 : 1;            // the front's speaker-gate memo CTAs (one per row); fan_out() builds them here
+    if (f.fused_tail) {      // the frame as 13 row tiles: spectrum of the tile's bins, conv, and block 0's input projection
+        CK(launch_k(false, front1_kernel_t<Map>, dim3(TAIL_TILES + gate_ctas, R0.B), dim3(256), FRONT1_SMEM, st, a.x, a.xbs, a.xcs, a.x_len,
+                    R0.X, a.state, R0.recs, e->w, e->bw[0], c.GX, a.pos_rel, a.emb, c.PRE, a.active));
+    } else if (f.walkers) {
+        const ChunkWalk g = front_many_walk(R0.B, T);
+        CK(launch_k(false, front_many_kernel_t<Map>, dim3(g.workers + gate_ctas * R0.B, 1), dim3(256), FRONT_SMEM, st, a.x, a.xbs, a.xcs,
+                    a.x_len, R0.X, a.state, R0.recs, e->w, T, a.pos_rel, a.emb, c.PRE, g.chunk, g.n_chunks, R0.B, g.workers, a.active));
     } else {
-        CK(launch_k(false, front_kernel_t<Map>, dim3(T + gate_ctas, B0), dim3(256), FRONT_SMEM, st, x, xbs, xcs, x_len, X0, state, recs0, e->w, T,
-                    a.pos_rel, emb, PRE, 0, 1, 0, active));
+        CK(launch_k(false, front_kernel_t<Map>, dim3(T + gate_ctas, R0.B), dim3(256), FRONT_SMEM, st, a.x, a.xbs, a.xcs, a.x_len, R0.X,
+                    a.state, R0.recs, e->w, T, a.pos_rel, a.emb, c.PRE, 0, 1, 0, a.active));
     }
     MARK("front");
-    if (int rc = do_tap()) return rc;
+    if (int rc = c.do_tap()) return rc;
 
-    const int B_all = B;
-    const int64_t ss_all = ss;
-    const Map recs_all = recs;
-    float* const X_all = X;
     for (int b = 0; b < e->n_blocks; ++b) {
-        if (K > 1 && b == 1) { if (int rc = fan_out()) return rc; }
-        // inside a block, B / rows / ss / recs / X are the block's own: for block 0 of a targets call those of the mixtures'
-        // lead records (see above), else the call's
-        const bool lead = K > 1 && b == 0;
-        const int B = lead ? B0 : B_all;
-        const int64_t rows = (int64_t)B * T * NF;
-        const int64_t ss = lead ? ss_all * K : ss_all;
-        const Map recs = lead ? recs0 : recs_all;
-        float* const X = lead ? X0 : X_all;
-        const int form_scale = lead ? K : 1;      // the recurrences' forms are chosen for the call's rows too
+        if (c.fans_out_before(b)) { if (int rc = c.fan_out()) return rc; }
+        const BlockRows<Map> R = c.rows_of(b);
         const BlockWeights& W = e->bw[b];
         // ---- intra: LN -> W_ih (both directions) -> BiLSTM over F -> Linear -> +res ------------
-        GemmArgs g{};
         LstmArgs l{};
-        l.gx = GX; l.gx_ld = 512; l.out = Y; l.out_ld = 128; l.whh = W.whh1;
-        l.nseq = B * T; l.L = NF; l.inner_count = 1; l.outer_stride = NF; l.inner_stride = 0; l.step_stride = 1;
+        l.gx = c.GX; l.gx_ld = 512; l.out = c.Y; l.out_ld = 128; l.whh = W.whh1;
+        l.nseq = R.B * T; l.L = NF; l.inner_count = 1; l.outer_stride = NF; l.inner_stride = 0; l.step_stride = 1;
         l.ndir = 2;
-        if (tc_fused_lstm(e, l, form_scale)) {
-            // many sequences: LayerNorm, W_ih and the recurrence in ONE tensor-core kernel (no [rows x 512] projection in HBM)
-            tcl::LstmXArgs xa{};
-            xa.l = l; xa.x = X; xa.x_ld = 64;
-            xa.wih_hi = e->pack.planes + e->plane_of[(size_t)b * PL_PER_BLOCK + PL_IH1]; xa.wih_lo = xa.wih_hi + e->pack.planes_total;
-            xa.bias = W.b1; xa.ln_g = W.ln1_g; xa.ln_b = W.ln1_b;
-            CK(launch_tc_lstm_x(xa, e->tc_passes, st, false));
-            MARK("gemm_ih_intra");
-        } else {
-            if (fused_tail && !(K > 1 && b == 1)) {
-                // front1_kernel (block 0) / the previous block's tail_kernel (its phase G) already wrote this block's input projection
-                // (not for block 1 of a targets call: block 0's tail ran per mixture, before the gate; the rows GEMM below does)
-            } else if (tc) {
-                e->cur_pdl = (e->tc_pdl & 2) != 0 && a.prof == nullptr;
-                if (int rc = tc_rows_gemm(e, b, PL_IH1, X, 64, 64, 512, W.ln1_g, W.ln1_b, W.b1, nullptr, nullptr, GX, 512, rows, st)) return rc;
-                e->cur_pdl = false;
-            } else {
-                g.A = X; g.lda = 64; g.Wt = W.wih1_t; g.bias = W.b1; g.C = GX; g.ldc = 512;
-                g.ln_g = W.ln1_g; g.ln_b = W.ln1_b; g.M = (int)rows; g.N = 512; g.K = 64;
-                CK(launch_rows_gemm(g, st, pdl));
-            }
-            MARK("gemm_ih_intra");
-            CK(lstm_any(e, l, st, pdl, form_scale));
-        }
-        MARK("lstm_intra");
-        if (tc_mid) {
+        if (int rc = c.ln_ih_recurrence(b, R, PL_IH1, l)) return rc;
+        if (f.tc_mid) {
             // many streams, one hop: the row-local middle of the block as four tensor-core GEMMs and the cell update.
             // The inter-LSTM step is ONE GEMM over the concatenated k = [LN(x) | h_prev] (h read in place from the
             // per-stream state records through a strided tensor map) against [W_ih | W_hh].
-            const bool mp = (e->tc_pdl & 1) != 0 && a.prof == nullptr;      // programmatic launches inside the section (experiment, option "tc_pdl")
-            e->cur_pdl = mp;
-            if (int rc = tc_rows_gemm(e, b, PL_L1, Y, 128, 128, 64, nullptr, nullptr, W.bl1, nullptr, X, X, 64, rows, st)) return rc;
+            if (int rc = c.dense(b, PL_L1, R, f.mid_pdl)) return rc;
             {
                 umma::GemmDesc q;
-                q.a0.base = X; q.a0.channels = 64; q.a0.n_pos = NF; q.a0.pos_stride = 64; q.a0.n_inner = B; q.a0.inner_stride = (int64_t)NF * 64;
-                q.a1.base = sbase + ST_BLK + (int64_t)b * BK_STRIDE + BK_H;
-                q.a1.channels = 64; q.a1.n_pos = NF; q.a1.pos_stride = 64; q.a1.n_inner = B; q.a1.inner_stride = ss;
-                if (a.slots) { q.a1.base = HG + (int64_t)b * B * FC; q.a1.inner_stride = FC; }      // gathered by gather_h_kernel
+                q.a0.base = R.X; q.a0.channels = 64; q.a0.n_pos = NF; q.a0.pos_stride = 64; q.a0.n_inner = R.B; q.a0.inner_stride = (int64_t)NF * 64;
+                q.a1.base = c.sbase + ST_BLK + (int64_t)b * BK_STRIDE + BK_H;
+                q.a1.channels = 64; q.a1.n_pos = NF; q.a1.pos_stride = 64; q.a1.n_inner = R.B; q.a1.inner_stride = R.ss;
+                if (a.slots) { q.a1.base = c.HG + (int64_t)b * R.B * FC; q.a1.inner_stride = FC; }      // gathered by gather_hc()
                 q.n_chunks = 2;
                 q.chunks[0].c0 = 0; q.chunks[0].dp = 0; q.chunks[0].flags = 2;      // x: LayerNorm
                 q.chunks[1].c0 = 0; q.chunks[1].dp = 0; q.chunks[1].flags = 1;      // h: second source
                 q.ln_g = W.ln2_g; q.ln_b = W.ln2_b;
-                q.rows_per_seq = NF; q.nseq = B;
+                q.rows_per_seq = NF; q.nseq = R.B;
                 q.b = tc_planes(e, b, PL_CAT, 128); q.N = 256; q.K = 128; q.passes = e->tc_passes;
-                q.bias = W.b2; q.C = GX; q.ldc = 256; q.c_seq_stride = (int64_t)NF * 256;
-                q.pdl = mp;
+                q.bias = W.b2; q.C = c.GX; q.ldc = 256; q.c_seq_stride = (int64_t)NF * 256;
+                q.pdl = f.mid_pdl;
                 std::string why;
                 const cudaError_t ce = umma::launch(q, st, &why);
                 if (ce != cudaSuccess) return fail(3, std::string("umma_gemm (inter step): ") + cudaGetErrorString(ce) + " " + why);
             }
-            CK(launch_k(pdl || mp, lstm_cell_rows_kernel_t<Map>, dim3((unsigned)((rows * 64 + 255) / 256)), dim3(256), 0, st, (const float*)GX, state, recs, b, Y, (int)rows,
-                      active));
-            if (int rc = tc_rows_gemm(e, b, PL_L2, Y, 64, 64, 64, nullptr, nullptr, W.bl2, nullptr, X, X, 64, rows, st)) return rc;
-            if (int rc = tc_rows_gemm(e, b, PL_QKV, X, 64, 64, NQKV, nullptr, nullptr, W.bqkv, W.slope_vec, nullptr, QKVRAW, NQKV, rows, st)) return rc;
-            e->cur_pdl = false;
+            CK(launch_k(f.mid_pdl, lstm_cell_rows_kernel_t<Map>, dim3((unsigned)((R.rows * 64 + 255) / 256)), dim3(256), 0, st,
+                        (const float*)c.GX, a.state, R.recs, b, c.Y, (int)R.rows, a.active));
+            if (int rc = c.dense(b, PL_L2, R, f.mid_pdl)) return rc;
+            if (int rc = tc_rows_gemm(e, b, PL_QKV, R.X, 64, 64, NQKV, nullptr, nullptr, W.bqkv, W.slope_vec, nullptr, c.QKVRAW, NQKV, R.rows,
+                                      st, f.mid_pdl)) return rc;
             MARK("mid");
-        } else if (row_mid && mid_split) {
-            float* GI = GX; float* HN = GX + rows * 256;         // the BiLSTM is done with GX
-            CK(launch_k(pdl, mid_a_kernel, mid_grid_for(B, 2), dim3(256), MID_A_SMEM, st, (const float*)Y, X, GI, W, B, (int64_t)0, 1));
-            CK(launch_k(pdl, mid_b_kernel_t<Map>, mid_grid_for(B, 3), dim3(256), MID_B_SMEM, st, (const float*)GI, HN, (int64_t)0, 1, state, recs, b, W, B,
-                        active));
-            CK(launch_k(pdl, mid_c_kernel, mid_grid_for(B, 4), dim3(256), MID_C_SMEM, st, (const float*)HN, X, QKVRAW, W, B, (int64_t)0, 1));
+        } else if (f.row_mid && f.mid_split) {
+            float* GI = c.GX; float* HN = c.GX + R.rows * 256;         // the BiLSTM is done with GX
+            CK(launch_k(f.pdl, mid_a_kernel, mid_grid_for(R.B, 2), dim3(256), MID_A_SMEM, st, (const float*)c.Y, R.X, GI, W, R.B, (int64_t)0, 1));
+            CK(launch_k(f.pdl, mid_b_kernel_t<Map>, mid_grid_for(R.B, 3), dim3(256), MID_B_SMEM, st, (const float*)GI, HN, (int64_t)0, 1, a.state,
+                        R.recs, b, W, R.B, a.active));
+            CK(launch_k(f.pdl, mid_c_kernel, mid_grid_for(R.B, 4), dim3(256), MID_C_SMEM, st, (const float*)HN, R.X, c.QKVRAW, W, R.B, (int64_t)0, 1));
             MARK("mid");
-        } else if (fused_tail) {
-            NextIh nx{};
-            if (b + 1 < e->n_blocks && !lead) {
+        } else if (f.fused_tail) {
+            NextIh nx{};      // the next block's input projection, where that block reads it from GX
+            if (b + 1 < e->n_blocks && c.rows_of(b + 1).ih_written) {
                 const BlockWeights& Wn = e->bw[b + 1];
-                nx.ln_g = Wn.ln1_g; nx.ln_b = Wn.ln1_b; nx.wih_t = Wn.wih1_t; nx.bias = Wn.b1; nx.GX = GX;
+                nx.ln_g = Wn.ln1_g; nx.ln_b = Wn.ln1_b; nx.wih_t = Wn.wih1_t; nx.bias = Wn.b1; nx.GX = c.GX;
             }
-            CK(launch_cluster(pdl, dim3(TAIL_CL, 1, 1), tail_kernel_t<Map>, dim3(TAIL_CL, B), dim3(256), TAIL_SMEM, st, (const float*)Y, X, state, recs,
-                              b, W, nx, (b == 0 && e->n_blocks > 1 && K == 1) ? 1 : 0, 0, active));
+            CK(launch_cluster(f.pdl, dim3(TAIL_CL, 1, 1), tail_kernel_t<Map>, dim3(TAIL_CL, R.B), dim3(256), TAIL_SMEM, st, (const float*)c.Y, R.X,
+                              a.state, R.recs, b, W, nx, R.gate, 0, a.active));
             MARK("tail");
-            if (int rc = do_tap()) return rc;
+            if (int rc = c.do_tap()) return rc;
             continue;
-        } else if (row_mid) {
-            CK(launch_k(pdl, mid_kernel_t<Map>, mid_grid_for(B, 1), dim3(256), MID_SMEM, st, (const float*)Y, X, QKVRAW, state, recs, b, W, B, active));
+        } else if (f.row_mid) {
+            CK(launch_k(f.pdl, mid_kernel_t<Map>, mid_grid_for(R.B, 1), dim3(256), MID_SMEM, st, (const float*)c.Y, R.X, c.QKVRAW, a.state, R.recs,
+                        b, W, R.B, a.active));
             MARK("mid");
         } else {
-            if (tc) {
-                if (int rc = tc_rows_gemm(e, b, PL_L1, Y, 128, 128, 64, nullptr, nullptr, W.bl1, nullptr, X, X, 64, rows, st)) return rc;
-            } else {
-                g = GemmArgs{};
-                g.A = Y; g.lda = 128; g.Wt = W.wl1_t; g.bias = W.bl1; g.C = X; g.ldc = 64; g.R = X;
-                g.M = (int)rows; g.N = 64; g.K = 128;
-                CK(launch_rows_gemm(g, st, pdl));
-            }
+            if (int rc = c.dense(b, PL_L1, R, f.pdl)) return rc;
             MARK("gemm_lin_intra");
-            if (int rc = do_tap()) return rc;
+            if (int rc = c.do_tap()) return rc;
             // ---- inter: LN -> W_ih -> LSTM over T with carried (h, c) -> Linear -> +res ------------
             l = LstmArgs{};
-            l.gx = GX; l.gx_ld = 256; l.out = Y; l.out_ld = 64; l.whh = W.whh2;
-            if constexpr (std::is_same_v<Map, Records>) {      // the copy gather_h_kernel made of the listed records' (h, c)
-                l.h_state = HG + (int64_t)b * B * FC;
-                l.c_state = CG + (int64_t)b * B * FC;
-                l.hc_outer_stride = FC;
-            } else {
-                l.h_state = sbase + ST_BLK + (int64_t)b * BK_STRIDE + BK_H;
-                l.c_state = sbase + ST_BLK + (int64_t)b * BK_STRIDE + BK_C;
-                l.hc_outer_stride = ss;
-            }
-            l.nseq = B * NF; l.L = T; l.inner_count = NF; l.outer_stride = (int64_t)T * NF; l.inner_stride = 1;
+            l.gx = c.GX; l.gx_ld = 256; l.out = c.Y; l.out_ld = 64; l.whh = W.whh2;
+            c.inter_hc(l, b, R);
+            l.nseq = R.B * NF; l.L = T; l.inner_count = NF; l.outer_stride = (int64_t)T * NF; l.inner_stride = 1;
             l.step_stride = NF; l.ndir = 1;
-            if (tc_fused_lstm(e, l, form_scale)) {
-                tcl::LstmXArgs xa{};
-                xa.l = l; xa.x = X; xa.x_ld = 64;
-                xa.wih_hi = e->pack.planes + e->plane_of[(size_t)b * PL_PER_BLOCK + PL_IH2]; xa.wih_lo = xa.wih_hi + e->pack.planes_total;
-                xa.bias = W.b2; xa.ln_g = W.ln2_g; xa.ln_b = W.ln2_b;
-                if constexpr (std::is_same_v<Map, Records>) xa.steps = recs.hops;     // ragged rows: masked inside
-                CK(launch_tc_lstm_x(xa, e->tc_passes, st, false));
-                MARK("gemm_ih_inter");
-            } else {
-                if (tc) {
-                    if (int rc = tc_rows_gemm(e, b, PL_IH2, X, 64, 64, 256, W.ln2_g, W.ln2_b, W.b2, nullptr, nullptr, GX, 256, rows, st)) return rc;
-                } else {
-                    g = GemmArgs{};
-                    g.A = X; g.lda = 64; g.Wt = W.wih2_t; g.bias = W.b2; g.C = GX; g.ldc = 256;
-                    g.ln_g = W.ln2_g; g.ln_b = W.ln2_b; g.M = (int)rows; g.N = 256; g.K = 64;
-                    CK(launch_rows_gemm(g, st, pdl));
-                }
-                MARK("gemm_ih_inter");
-                if constexpr (std::is_same_v<Map, Records>) {
-                    if (recs.hops) CK(launch_k(false, inter_gate_mask_kernel, dim3(T, B), dim3(256), 0, st, GX, recs, T));
-                }
-                CK(lstm_any(e, l, st, pdl, form_scale));
-            }
-            MARK("lstm_inter");
-            if constexpr (std::is_same_v<Map, Records>) {
-                if (recs.hops)      // a ragged row's h is that of its own last frame
-                    CK(launch_k(false, inter_h_last_kernel, dim3(B), dim3(256), 0, st, (const float*)Y,
-                                HG + (int64_t)b * B * FC, recs, T));
-                if (b == e->n_blocks - 1)
-                    CK(launch_k(false, scatter_hc_kernel, dim3((unsigned)((hc4 + 255) / 256)), dim3(256), 0, st, state, recs,
-                                e->n_blocks, B, (const float*)HG, (const float*)CG));
-            }
-            if (tc) {
-                if (int rc = tc_rows_gemm(e, b, PL_L2, Y, 64, 64, 64, nullptr, nullptr, W.bl2, nullptr, X, X, 64, rows, st)) return rc;
-            } else {
-                g = GemmArgs{};
-                g.A = Y; g.lda = 64; g.Wt = W.wl2_t; g.bias = W.bl2; g.C = X; g.ldc = 64; g.R = X;
-                g.M = (int)rows; g.N = 64; g.K = 64;
-                CK(launch_rows_gemm(g, st, pdl));
-            }
+            if (int rc = c.ln_ih_recurrence(b, R, PL_IH2, l)) return rc;
+            if (int rc = c.h_last(b)) return rc;
+            if (b == e->n_blocks - 1) { if (int rc = c.scatter_hc()) return rc; }
+            if (int rc = c.dense(b, PL_L2, R, f.pdl)) return rc;
             MARK("gemm_lin_inter");
-            if (int rc = do_tap()) return rc;
+            if (int rc = c.do_tap()) return rc;
         }
         // ---- attention --------------------------------------------------------------------------
         if (T > 1) {
-            CK(launch_k(pdl, kv_gather_kernel_t<Map>, dim3(ATT - 1, B * NHEAD), dim3(128), 0, st, (const float*)state, recs, b, KALL,
-                        VALL, T));
+            CK(launch_k(f.pdl, kv_gather_kernel_t<Map>, dim3(ATT - 1, R.B * NHEAD), dim3(128), 0, st, (const float*)a.state, R.recs, b, c.KALL,
+                        c.VALL, T));
             MARK("kv_gather");
         }
-        if (tc && !tc_mid) {      // Q|K|V projections of all rows as one tensor-core GEMM (+ bias + PReLU per column)
-            if (int rc = tc_rows_gemm(e, b, PL_QKV, X, 64, 64, NQKV, nullptr, nullptr, W.bqkv, W.slope_vec, nullptr, QKVRAW, NQKV, rows, st)) return rc;
+        if (f.tc && !f.tc_mid) {      // Q|K|V projections of all rows as one tensor-core GEMM (+ bias + PReLU per column)
+            if (int rc = tc_rows_gemm(e, b, PL_QKV, R.X, 64, 64, NQKV, nullptr, nullptr, W.bqkv, W.slope_vec, nullptr, c.QKVRAW, NQKV, R.rows,
+                                      st, false)) return rc;
         }
-        if (qkv_many) {      // many frames: persistent form (LayerNorm parameters staged once per CTA), one wave
-            static int wave[64] = {};
-            const int64_t grid_q = std::min<int64_t>(resident_ctas(wave, qkv_many_kernel_t<Map>, QKV_THREADS, QKV_MANY_SMEM), (int64_t)B * T);
-            CK(launch_k(pdl || ((e->tc_pdl & 4) != 0 && a.prof == nullptr), qkv_many_kernel_t<Map>, dim3((unsigned)grid_q), dim3(QKV_THREADS), QKV_MANY_SMEM, st, (const float*)QKVRAW, Q, KALL, VALL, state, recs,
-                        b, W, T, B * T, active));
+        if (f.qkv_many) {      // many frames: persistent form (LayerNorm parameters staged once per CTA), one wave
+            const int64_t grid_q = std::min<int64_t>(f.qkv_ctas, (int64_t)R.B * T);
+            CK(launch_k(f.qkv_pdl, qkv_many_kernel_t<Map>, dim3((unsigned)grid_q), dim3(QKV_THREADS), QKV_MANY_SMEM, st, (const float*)c.QKVRAW,
+                        c.Q, c.KALL, c.VALL, a.state, R.recs, b, W, T, R.B * T, a.active));
         } else {
-            CK(launch_k(pdl, qkv_kernel_t<Map>, dim3(T, B), dim3(QKV_THREADS), (tc || row_mid) ? QKV_PRE_SMEM : QKV_SMEM, st, (const float*)X,
-                        (const float*)((tc || row_mid) ? QKVRAW : nullptr), Q, KALL, VALL, state, recs, b, W, T, 0, active));
+            const bool pre = f.tc || f.row_mid;      // the projections are in QKVRAW already
+            CK(launch_k(f.pdl, qkv_kernel_t<Map>, dim3(T, R.B), dim3(QKV_THREADS), pre ? QKV_PRE_SMEM : QKV_SMEM, st, (const float*)R.X,
+                        (const float*)(pre ? c.QKVRAW : nullptr), c.Q, c.KALL, c.VALL, a.state, R.recs, b, W, T, 0, a.active));
         }
         MARK("qkv");
-        if (nsplit > 1) {
-            CK(launch_cluster(pdl, dim3(1, ATT_CL, 1), attn_cluster_kernel_t<Map>, dim3(T, NHEAD * ATT_CL, B), dim3(256), 0, st,
-                              (const float*)Q, (const float*)KALL, (const float*)VALL, (const float*)state, recs, b, Z, T, 0));
-        } else if (attn_tiled) {   // enough tiles to fill the GPU: query-tiled,
-            // one pass over 57 rows serves 8 queries
-            CK(launch_k(pdl, attn_tile_kernel, dim3((T + ATT_TQ - 1) / ATT_TQ, NHEAD, B), dim3(256), 0, st, (const float*)Q,
-                        (const float*)KALL, (const float*)VALL, Z, T));
+        if (f.nsplit > 1) {
+            CK(launch_cluster(f.pdl, dim3(1, ATT_CL, 1), attn_cluster_kernel_t<Map>, dim3(T, NHEAD * ATT_CL, R.B), dim3(256), 0, st,
+                              (const float*)c.Q, (const float*)c.KALL, (const float*)c.VALL, (const float*)a.state, R.recs, b, c.Z, T, 0));
+        } else if (f.attn_tiled) {
+            CK(launch_k(f.pdl, attn_tile_kernel, dim3((T + ATT_TQ - 1) / ATT_TQ, NHEAD, R.B), dim3(256), 0, st, (const float*)c.Q,
+                        (const float*)c.KALL, (const float*)c.VALL, c.Z, T));
         } else {
-            CK(launch_k(pdl, attn_kernel_t<Map>, dim3(T, NHEAD, B), dim3(256), 0, st, (const float*)Q, (const float*)KALL,
-                        (const float*)VALL, (const float*)state, recs, b, Z, T, 0));
+            CK(launch_k(f.pdl, attn_kernel_t<Map>, dim3(T, NHEAD, R.B), dim3(256), 0, st, (const float*)c.Q, (const float*)c.KALL,
+                        (const float*)c.VALL, (const float*)a.state, R.recs, b, c.Z, T, 0));
         }
         MARK("attn");
-        if (tc) {      // Linear(64->64) + PReLU of all rows on the tensor cores, then LayerNorm(6208) + residual (+ gate) per frame
-            const bool p2 = (e->tc_pdl & 2) != 0 && a.prof == nullptr;
-            e->cur_pdl = p2;
-            if (int rc = tc_rows_gemm(e, b, PL_P, Z, 64, 64, 64, nullptr, nullptr, W.bp, nullptr, nullptr, Y, 64, rows, st, W.slopes + 3)) return rc;
-            e->cur_pdl = false;
-            CK(launch_k(pdl || p2, ln_frame_res_kernel_t<Map>, dim3(T, B), dim3(256), 0, st, (const float*)Y, X, (const float*)state, recs, W,
-                        (b == 0 && e->n_blocks > 1 && K == 1) ? 1 : 0, T));
+        if (f.tc) {      // Linear(64->64) + PReLU of all rows on the tensor cores, then LayerNorm(6208) + residual (+ gate) per frame
+            if (int rc = tc_rows_gemm(e, b, PL_P, c.Z, 64, 64, 64, nullptr, nullptr, W.bp, nullptr, nullptr, c.Y, 64, R.rows, st, f.gemm_pdl,
+                                      W.slopes + 3)) return rc;
+            CK(launch_k(f.gemm_pdl, ln_frame_res_kernel_t<Map>, dim3(T, R.B), dim3(256), 0, st, (const float*)c.Y, R.X, (const float*)a.state,
+                        R.recs, W, R.gate, T));
         } else {
-            CK(launch_k(pdl, attn_out_kernel_t<Map>, dim3(T, B), dim3(256), AOUT_SMEM, st, (const float*)Z, X, (const float*)state, recs, W,
-                        (b == 0 && e->n_blocks > 1 && K == 1) ? 1 : 0, T));
+            CK(launch_k(f.pdl, attn_out_kernel_t<Map>, dim3(T, R.B), dim3(256), AOUT_SMEM, st, (const float*)c.Z, R.X, (const float*)a.state,
+                        R.recs, W, R.gate, T));
         }
         MARK("attn_out");
-        if (int rc = do_tap()) return rc;
+        if (int rc = c.do_tap()) return rc;
     }
-    if (K > 1 && e->n_blocks == 1) { if (int rc = fan_out()) return rc; }
-    if ((T > 1 || tc) && e->use_back_many) {
-        // many frames (or many streams): one cluster walks (stream, chunk-of-frames) items -- filters loaded once per cluster, rows
-        // staged once; as many clusters as stay resident together (3 CTAs of 72 KB per SM)
-        const int max_cl = NUM_SMS * 3 / BACK_CL;
-        const int per_stream = std::max(1, max_cl / B);
-        const int chunk = (T + per_stream - 1) / per_stream;
-        const int n_chunks = (T + chunk - 1) / chunk;
-        const int n_cl = std::min(max_cl, B * n_chunks);
-        CK(launch_cluster(pdl, dim3(BACK_CL, 1, 1), back_many_kernel_t<Map>, dim3(BACK_CL * n_cl, 1), dim3(256), BACK_MANY_SMEM, st, (const float*)X, y, ybs,
-                          ycs, y_len, state, recs, e->w, T, a.pos_rel, chunk, n_chunks, B, active));
+    if (c.fans_out_before(e->n_blocks)) { if (int rc = c.fan_out()) return rc; }
+    if (f.walkers) {
+        const ChunkWalk g = back_many_walk(a.B, T);
+        CK(launch_cluster(f.pdl, dim3(BACK_CL, 1, 1), back_many_kernel_t<Map>, dim3(BACK_CL * g.workers, 1), dim3(256), BACK_MANY_SMEM, st,
+                          (const float*)c.X, a.y, a.ybs, a.ycs, a.y_len, a.state, recs, e->w, T, a.pos_rel, g.chunk, g.n_chunks, a.B, a.active));
     } else {
-        CK(launch_cluster(pdl, dim3(BACK_CL, 1, 1), back_kernel_t<Map>, dim3(BACK_CL * T, B), dim3(256), BACK_SMEM, st, (const float*)X, y, ybs, ycs, y_len, state, recs, e->w, T,
-                    a.pos_rel, 0, 1, 0, (int64_t)0, active));
+        CK(launch_cluster(f.pdl, dim3(BACK_CL, 1, 1), back_kernel_t<Map>, dim3(BACK_CL * T, a.B), dim3(256), BACK_SMEM, st, (const float*)c.X,
+                          a.y, a.ybs, a.ycs, a.y_len, a.state, recs, e->w, T, a.pos_rel, 0, 1, 0, (int64_t)0, a.active));
     }
     MARK("back");
-#undef MARK
     return 0;
 }
+#undef MARK
 
 static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
     const int64_t ss = stream_stride(e->n_blocks);
@@ -1237,9 +1242,7 @@ int l2h_sep_launches_per_forward(void* handle, int32_t frames, int32_t* n) {
     // one l2h_sep_forward: a one-hop call is 6 kernels per block (gemm, bilstm, mid, qkv, attn, attn_out; 8 with many
     // streams, where the mid section runs as three kernels), a multi-hop call 10.  Streams of one-hop calls go through
     // the pipelined graph instead -- l2h_sep_launch_count has the exact figure for everything this handle launched.
-    int dev_ord = 0;
-    cudaGetDevice(&dev_ord);
-    if (frames == 1 && e->use_tail && dev_ord >= 0 && dev_ord < 64 && g_tail_clusters[dev_ord] > 0)
+    if (frames == 1 && tail_fits(e, 1))
         *n = 1 + e->n_blocks * 2 + 1;       // front1, (BiLSTM, tail_kernel) per block, back
     else
         *n = 1 + e->n_blocks * (frames == 1 ? 6 : 10) + 1;
@@ -1365,8 +1368,7 @@ int l2h_sep_forward_slots_hops(void* handle, const float* x, int64_t xbs, int64_
 // One-hop calls are pipelined over hops (wavefront graph) only for FEW streams: with many streams every kernel of a hop
 // already fills the GPU, the dense stages run on the tensor cores (enqueue_chain) and the hops replay one chain graph.
 static bool pipeline_applies(const SepEngine* e, int batch, int cpc, int n_calls) {
-    if (!(cpc == 1 && e->use_pipe && e->n_blocks == 3 && n_calls > 1)) return false;
-    return (int64_t)batch * NF <= TC_MIN_ROWS;
+    return cpc == 1 && e->use_pipe && e->n_blocks == 3 && n_calls > 1 && !tc_form(batch, 1);
 }
 
 int l2h_sep_stream_host(void* handle, const float* x_host, int32_t x_len, const float* emb, void* state,

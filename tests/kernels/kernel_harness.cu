@@ -13,8 +13,7 @@
 #include <cstdio>
 #include "umma_gemm.cu"
 #include "tc_lstm.cuh"
-#include "sep_kernels.cuh"
-#include "hop_kernels.cuh"
+#include "sep_launch.cuh"
 #include "embed_kernels.cuh"
 
 #define KH_API extern "C" __attribute__((visibility("default")))
@@ -240,30 +239,20 @@ KH_API int kh_sep_layout(int n_blocks, int64_t* out) {
     return n;
 }
 
-// dynamic shared memory of the separator kernels launched here, set once per device (as the engine's set_attrs does)
+// dynamic shared memory of the separator kernels (dense forms), set once per device with the engine's own list
 static cudaError_t configure_sep() {
     static thread_local int configured_dev = -1;
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess || configured_dev == dev) return e;
-    e = cudaFuncSetAttribute(qkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)QKV_SMEM);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(qkv_many_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)QKV_MANY_SMEM);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(attn_out_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AOUT_SMEM);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(front_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FRONT_SMEM);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(front_many_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FRONT_SMEM);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(front1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FRONT1_SMEM);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(back_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BACK_SMEM);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(back_many_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BACK_MANY_SMEM);
+    e = set_sep_smem<int64_t>();
     if (e == cudaSuccess) configured_dev = dev;
     return e;
 }
 
 // CTAs of attn_cluster_kernel the current device holds at once: the engine splits a call's windows over 8-CTA
 // clusters while B * T * NHEAD * ATT_CL fits in this (attn_splits)
-KH_API int kh_attn_cluster_resident() {
-    static int wave[64] = {};
-    return resident_ctas(wave, attn_cluster_kernel, 256, 0);
-}
+KH_API int kh_attn_cluster_resident() { return attn_cluster_resident(); }
 
 // qkv_kernel: grid (T, B).  pre == nullptr: the Linear 64 -> 112 (+ bias + PReLU) runs inside, from X [B][T][97][64];
 // otherwise pre holds the projections [B][T][97][112].
@@ -366,12 +355,10 @@ KH_API int kh_front(const KhSepFrontBack* w, const float* x, int64_t x_bstride, 
                          group ? frames_total : 1, group ? frame_k * HOP : 0, active);
 }
 
-// the engine's front_many_kernel geometry for (B, T) (sep_engine.cu, the many-frame branch of the front)
+// the engine's front_many_kernel geometry for (B, T) (sep_launch.cuh)
 KH_API void kh_front_many_geometry(int B, int T, int* chunk, int* n_workers) {
-    const int per_stream = std::max(1, NUM_SMS / B);
-    *chunk = (T + per_stream - 1) / per_stream;
-    const int n_chunks = (T + *chunk - 1) / *chunk;
-    *n_workers = std::min(NUM_SMS, B * n_chunks);
+    const ChunkWalk g = front_many_walk(B, T);
+    *chunk = g.chunk; *n_workers = g.workers;
 }
 
 // front_many_kernel: n_workers CTAs walk the (stream, chunk-of-`chunk`-frames) items, then one speaker-gate CTA per stream
@@ -417,13 +404,10 @@ KH_API int kh_back(const KhSepFrontBack* w, const float* X, float* y, int64_t y_
                                group ? hist_stride : (int64_t)0, active);
 }
 
-// the engine's back_many_kernel geometry for (B, T) (sep_engine.cu, the many-frame branch of the back)
+// the engine's back_many_kernel geometry for (B, T) (sep_launch.cuh)
 KH_API void kh_back_many_geometry(int B, int T, int* chunk, int* n_cl) {
-    const int max_cl = NUM_SMS * 3 / BACK_CL;
-    const int per_stream = std::max(1, max_cl / B);
-    *chunk = (T + per_stream - 1) / per_stream;
-    const int n_chunks = (T + *chunk - 1) / *chunk;
-    *n_cl = std::min(max_cl, B * n_chunks);
+    const ChunkWalk g = back_many_walk(B, T);
+    *chunk = g.chunk; *n_cl = g.workers;
 }
 
 // back_many_kernel: n_cl clusters of BACK_CL walk the (stream, chunk-of-`chunk`-frames) items; it advances the clocks
