@@ -17,6 +17,9 @@
  *   l2h_sep_forward_slots_frames / l2h_sep_forward_slots_hops
  *        <- several Net.predict hops for a list of a state's streams, the same number for every row or one per row
  *           (Net.advance_slots)
+ *   l2h_sep_forward_targets / l2h_sep_forward_targets_groups
+ *        <- Net.predict for several enrolled speakers of each mixture, for a whole state or a list of its listener
+ *           groups (Net.predict_targets, Net.advance_targets)
  *   l2h_sep_stream_host
  *        <- the chunk loop around Net.predict(chunk, embed, state, pad=False)  (SURVEY.md 3.3)
  *           with host buffers: H2D of each chunk and D2H of each result inside the call
@@ -213,7 +216,8 @@ int l2h_sep_forward_slots_hops(void* handle, const float* x_dev, int64_t x_batch
  * differs: in the fused one-hop form (option "fused_tail") block 1's input projection runs as a separate rows GEMM rather
  * than inside block 0's tail kernel (rounding only).  n_targets == 1 is l2h_sep_forward, bit for bit.  L2H_FLAG_GRAPH works
  * (the cached graph's key holds K).
- * Not supported with targets: slot lists, activity masks and per-row hop counts; the pipelined wavefront graph and
+ * With targets, slot lists and per-row hop counts go through l2h_sep_forward_targets_groups below, which runs listed
+ * groups of a larger state.  Not supported with targets: activity masks; the pipelined wavefront graph and
  * l2h_sep_stream_host / _dev; taps.  Non-lead records keep their (unused) block-0 area: there is no compact record.
  * Errors 1, before anything is enqueued: null pointers, batch, n_targets or frames <= 0, batch*n_targets*frames*97 rows
  * beyond the limit of one call, L2H_FLAG_TAPS. */
@@ -221,6 +225,35 @@ int l2h_sep_forward_targets(void* handle, const float* x_dev, int64_t x_batch_st
                             const float* emb_dev, void* state_dev, float* y_dev, int64_t y_batch_stride,
                             int64_t y_ch_stride, int32_t y_len, int32_t batch, int32_t n_targets, int32_t frames,
                             void* workspace_dev, size_t workspace_bytes, uint32_t flags, void* stream);
+/* l2h_sep_forward_targets over a chosen list of a state's groups, each group advancing by its own number of hops: the
+ * slot-list calls (l2h_sep_forward_slots_hops) for listeners who each want K = n_targets speakers.  The front and block 0
+ * still run once per listed group, blocks 1 .. B-1 and the back once per target.
+ *   state_dev  a state of state_batch = G*K records in the targets layout: record g*K + k is target k of group g, and g*K is
+ *              the group's lead record (the state l2h_sep_forward_targets runs for G mixtures)
+ *   groups_dev [n] int32 of DEVICE memory read when the kernels run: call row i is group groups_dev[i].  An entry outside
+ *              [0, G) marks a group that is computed but stores nothing (no record, no y row): with a fixed n, a group
+ *              missing the tick.  A group listed twice is a caller error the call does not detect.
+ *   hops_dev   [n] int32 of DEVICE memory read when the kernels run, or NULL: every group advances `frames` hops.  Otherwise
+ *              group i advances h = hops_dev[i] hops, from 0 to `frames` (T), as a row of l2h_sep_forward_slots_hops does:
+ *              it reads only x samples 0 .. 128*h + 63 of its row, its K y rows receive samples 0 .. 128*h - 1 only, every
+ *              record of the group advances its clock by h (and by one call if h > 0), and h = 0 stores nothing.  An entry
+ *              outside [0, frames] counts as 0.
+ *   x_dev      [n] mixture rows of 128*frames + 64 samples (x_len); row i is the mixture of group groups_dev[i]
+ *   emb_dev    [n*K][256]: row i*K + k is target k of call row i, as for l2h_sep_forward_targets
+ *   y_dev      [n*K] target rows, same order; y_batch_stride is the stride between consecutive target rows
+ *   workspace  l2h_sep_workspace_bytes(handle, n*K, frames, flags), as for a targets call of n mixtures
+ * Groups not listed are neither read nor written; the header advances by `frames` as for any call.  Every kernel form is
+ * chosen for the n*K target rows, so a listed group gets the arithmetic of a dense l2h_sep_forward_targets of n groups, bit
+ * for bit, in every form.  With L2H_FLAG_GRAPH one graph cached for (n, K, T) serves every tick: its key holds the list
+ * pointers, not their contents, so a caller rewrites groups_dev and hops_dev in place before every tick.  n_targets == 1
+ * is l2h_sep_forward_slots_hops.
+ * Errors 1, before anything is enqueued: null pointers, n, n_targets or frames <= 0, a state_batch that is not a positive
+ * multiple of n_targets, n > G, n*n_targets*frames*97 rows beyond the limit of one call, L2H_FLAG_TAPS. */
+int l2h_sep_forward_targets_groups(void* handle, const float* x_dev, int64_t x_batch_stride, int64_t x_ch_stride,
+                                   int32_t x_len, const float* emb_dev, void* state_dev, int32_t state_batch,
+                                   const int32_t* groups_dev, const int32_t* hops_dev, int32_t n, int32_t n_targets,
+                                   int32_t frames, float* y_dev, int64_t y_batch_stride, int64_t y_ch_stride,
+                                   int32_t y_len, void* workspace_dev, size_t workspace_bytes, uint32_t flags, void* stream);
 
 /* Streaming with HOST buffers (the end-to-end path).  Per round: H2D of the round's samples (+64
  * look-ahead) from pinned memory, the kernel chains, D2H of the new samples; one stream synchronise at

@@ -215,7 +215,7 @@ static bool tc_mid_form(int B, int T, uint32_t flags) { return tc_form(B, T) && 
 
 // ---- workspace carve-up (floats) ---------------------------------------------------------------
 struct Workspace {
-    int64_t X, GX, Y, Z, Q, KALL, VALL, PRE, QKVRAW, TAPS, HG, total;
+    int64_t X, GX, Y, Z, Q, KALL, VALL, PRE, QKVRAW, TAPS, HG, LISTS, total;
 };
 
 static Workspace carve(int n_blocks, int B, int T, uint32_t flags) {
@@ -236,6 +236,9 @@ static Workspace carve(int n_blocks, int B, int T, uint32_t flags) {
     // the listed records' carried inter-LSTM state of every block for a slot-list call (gather_h_kernel): h for one-hop
     // calls in the tensor-core form, h and c ([n_blocks][B][97][64] each) for every multi-hop call
     ws.HG = alloc((T > 1 ? 2 : tc_mid_form(B, T, flags) ? 1 : 0) * (int64_t)n_blocks * B * FC);
+    // a call over a list of groups (l2h_sep_forward_targets_groups): the record and hop lists of its target rows
+    // (group_rows_kernel), two int32 per row.  Reserved for every call, so that one size query serves every kind of call.
+    ws.LISTS = alloc(2 * (int64_t)B);
     ws.total = (cur + 511) & ~int64_t(511);      // a multiple of one GX row: pipelined hops address their slots as rows of one tensor
     return ws;
 }
@@ -324,9 +327,10 @@ struct ChainArgs {
     int B, T; float* wsp; size_t ws_bytes; uint32_t flags; int pos_rel;
     Profiler* prof = nullptr;
     const uint8_t* active = nullptr;     // one-hop calls: [B] device mask of the streams that advance (null: all)
-    const int32_t* slots = nullptr;      // [B] device list, row b -> record slots[b] (null: row b -> record b)
+    const int32_t* slots = nullptr;      // [B] device list, row b -> record slots[b] (null: row b -> record b); with targets > 1
+                                         // the [B / targets] group list of l2h_sep_forward_targets_groups
     int state_batch = 0;                 // records in the state (slot lists only)
-    const int32_t* hops = nullptr;       // slot lists: [B] device list of the frames each row advances (null: all T)
+    const int32_t* hops = nullptr;       // slot lists: [B] device list of the frames each row advances (null: all T); per group
     int targets = 1;                     // l2h_sep_forward_targets: rows per mixture (B counts target rows; x has B / targets)
 };
 
@@ -408,7 +412,9 @@ struct Chain {
     SepEngine* e; const ChainArgs& a; cudaStream_t st; const ChainForm& f; Map recs;
     int K;              // targets per mixture
     int64_t ss;         // record stride
+    Map lead;           // K > 1: the record map of block 0's rows, the groups' lead records (rows_of)
     float *X, *GX, *Y, *Z, *Q, *KALL, *VALL, *PRE, *QKVRAW, *TAPS, *HG, *CG, *sbase;
+    int32_t* lists;     // a list of groups: the target rows' record list, then their hop list (group_rows)
     int tap = 0;
 
     Chain(SepEngine* e_, const ChainArgs& a_, cudaStream_t st_, const ChainForm& f_, Map recs_, const Workspace& ws)
@@ -417,7 +423,10 @@ struct Chain {
         X = w + ws.X; GX = w + ws.GX; Y = w + ws.Y; Z = w + ws.Z; Q = w + ws.Q; KALL = w + ws.KALL; VALL = w + ws.VALL;
         PRE = w + ws.PRE; QKVRAW = w + ws.QKVRAW; TAPS = w + ws.TAPS; HG = w + ws.HG;
         CG = HG + (int64_t)e->n_blocks * a.B * FC;
+        lists = reinterpret_cast<int32_t*>(w + ws.LISTS);
         sbase = a.state + sizeof(StateHeader) / 4;
+        if constexpr (slots) lead = Records{ss * K, a.slots, a.state_batch / K, a.hops, a.T};      // a.slots: the groups
+        else lead = recs * K;
     }
 
     // Several targets per mixture (l2h_sep_forward_targets): B counts target rows, K per mixture, row i*K + k = target k of
@@ -426,23 +435,32 @@ struct Chain {
     // block 0 leaves unused.  fan_out() then builds every target row's gate memo and its gated copy of block 0's output
     // in X, and blocks 1 .. n_blocks-1 and the back run over all B rows.  Every form was chosen for the B rows, and
     // block 0 runs those same forms, so a target row gets the arithmetic of a dense call with its mixture duplicated.
+    // Over a list of groups (l2h_sep_forward_targets_groups) block 0's map is the group list with record stride K*ss and
+    // the groups' hop counts, which addresses lead record g*K; the target rows' map is the list group_rows() builds.
     BlockRows<Map> rows_of(int b) const {
-        const bool lead = K > 1 && b == 0;
-        BlockRows<Map> r{lead ? a.B / K : a.B, 0, lead ? ss * K : ss, recs, X, lead ? K : 1,
+        const bool lead_rows = K > 1 && b == 0;
+        BlockRows<Map> r{lead_rows ? a.B / K : a.B, 0, lead_rows ? ss * K : ss, lead_rows ? lead : recs, X, lead_rows ? K : 1,
                          f.fused_tail && !fans_out_before(b), (b == 0 && e->n_blocks > 1 && K == 1) ? 1 : 0};
         r.rows = (int64_t)r.B * a.T * NF;
-        if constexpr (!slots) {
-            if (lead) { r.recs = recs * K; r.X = GX + r.rows * 512; }
-        }
+        if (lead_rows) r.X = GX + r.rows * 512;
         return r;
     }
     bool fans_out_before(int b) const { return K > 1 && b == 1; }      // b == n_blocks: before the back
     int fan_out() {
-        if constexpr (!slots) {
-            CK(launch_k(f.pdl, spk_gate_kernel, dim3(a.B), dim3(256), 0, st, a.emb, PRE, a.state, recs, e->w));
-            CK(launch_k(f.pdl, gate_fanout_kernel, dim3(a.T, a.B), dim3(256), 0, st, (const float*)rows_of(0).X, X,
-                        (const float*)a.state, ss, K, a.T, e->n_blocks > 1 ? 1 : 0));
-            MARK("gate_fanout");
+        CK(launch_k(f.pdl, spk_gate_kernel_t<Map>, dim3(a.B), dim3(256), 0, st, a.emb, PRE, a.state, recs, e->w));
+        CK(launch_k(f.pdl, gate_fanout_kernel_t<Map>, dim3(a.T, a.B), dim3(256), 0, st, (const float*)rows_of(0).X, X,
+                    (const float*)a.state, recs, K, a.T, e->n_blocks > 1 ? 1 : 0));
+        MARK("gate_fanout");
+        return 0;
+    }
+    // a list of groups: the target rows' record list (and hop list) from the group list, before any kernel reads them
+    int group_rows() {
+        if constexpr (slots) {
+            if (K > 1) {
+                CK(launch_k(false, group_rows_kernel, dim3((unsigned)((a.B + 255) / 256)), dim3(256), 0, st, a.slots, a.hops,
+                            a.state_batch / K, K, a.B, lists, lists + a.B));
+                MARK("group_rows");
+            }
         }
         return 0;
     }
@@ -489,7 +507,7 @@ struct Chain {
             xa.l = l; xa.x = R.X; xa.x_ld = 64;
             xa.wih_hi = e->pack.planes + e->plane_of[(size_t)b * PL_PER_BLOCK + which]; xa.wih_lo = xa.wih_hi + e->pack.planes_total;
             xa.bias = inter ? W.b2 : W.b1; xa.ln_g = inter ? W.ln2_g : W.ln1_g; xa.ln_b = inter ? W.ln2_b : W.ln1_b;
-            if constexpr (slots) { if (inter) xa.steps = recs.hops; }      // ragged rows: masked inside
+            if constexpr (slots) { if (inter) xa.steps = R.recs.hops; }      // ragged rows: masked inside
             CK(launch_tc_lstm_x(xa, e->tc_passes, st, false));
             MARK(inter ? "gemm_ih_inter" : "gemm_ih_intra");
         } else {
@@ -498,7 +516,7 @@ struct Chain {
             }
             MARK(inter ? "gemm_ih_inter" : "gemm_ih_intra");
             if constexpr (slots) {
-                if (inter && recs.hops) CK(launch_k(false, inter_gate_mask_kernel, dim3(a.T, R.B), dim3(256), 0, st, GX, recs, a.T));
+                if (inter && R.recs.hops) CK(launch_k(false, inter_gate_mask_kernel, dim3(a.T, R.B), dim3(256), 0, st, GX, R.recs, a.T));
             }
             if (rf.tc) CK(launch_tc_lstm(l, e->tc_passes, st, f.pdl));
             else CK(launch_lstm_rec(l, st, f.pdl, l.nseq * R.scale));
@@ -509,13 +527,30 @@ struct Chain {
 
     // Slot lists: one-hop tensor-core chains read the listed records' h of every block for the inter-step GEMMs, and
     // multi-hop calls carry their (h, c) through the inter recurrences, from a copy in the workspace (HG, CG) that
-    // gather_hc() takes before block 0 and scatter_hc() stores back after the last block's inter recurrence
-    int64_t hc4() const { return (int64_t)e->n_blocks * a.B * FC / 4; }      // float4s of one of h, c
+    // gather_hc() takes before block 0 and scatter_hc() stores back after the last block's inter recurrence.  Block b's
+    // part holds the rows of rows_of(b) (inter_hc): over a list of groups, block 0's part holds the lead rows.
+    // hc_copy: gather_h_kernel or scatter_hc_kernel over the blocks from b0 on that share rows_of(b0)'s record map.  The
+    // kernels address block `blk` of a record from the state pointer they get, so a pointer b0 blocks further makes their
+    // block 0 block b0 of the records.
+    int hc_copy(bool scatter, int b0) {
+        const BlockRows<Map> R = rows_of(b0);
+        const int nb = (K > 1 && b0 == 0) ? 1 : e->n_blocks - b0;
+        const int64_t o = (int64_t)b0 * R.B * FC;
+        const dim3 grid((unsigned)(((int64_t)nb * R.B * FC / 4 + 255) / 256));      // one thread per float4 of h (and c)
+        if (scatter)
+            CK(launch_k(false, scatter_hc_kernel, grid, dim3(256), 0, st, a.state + b0 * BK_STRIDE, R.recs, nb, R.B,
+                        (const float*)HG + o, (const float*)CG + o));
+        else
+            CK(launch_k(false, gather_h_kernel, grid, dim3(256), 0, st, (const float*)a.state + b0 * BK_STRIDE, R.recs, nb, R.B,
+                        HG + o, a.T > 1 ? CG + o : nullptr));
+        return 0;
+    }
     int gather_hc() {
         if constexpr (slots) {
-            if (f.tc_mid || a.T > 1)
-                CK(launch_k(false, gather_h_kernel, dim3((unsigned)((hc4() + 255) / 256)), dim3(256), 0, st, (const float*)a.state,
-                            recs, e->n_blocks, a.B, HG, a.T > 1 ? CG : nullptr));
+            if (f.tc_mid || a.T > 1) {
+                if (int rc = hc_copy(false, 0)) return rc;
+                if (K > 1 && e->n_blocks > 1) { if (int rc = hc_copy(false, 1)) return rc; }
+            }
         }
         return 0;
     }
@@ -530,17 +565,19 @@ struct Chain {
             l.hc_outer_stride = R.ss;
         }
     }
-    int h_last(int b) {      // a ragged row's h is that of its own last frame
+    int h_last(int b, const BlockRows<Map>& R) {      // a ragged row's h is that of its own last frame
         if constexpr (slots) {
-            if (recs.hops)
-                CK(launch_k(false, inter_h_last_kernel, dim3(a.B), dim3(256), 0, st, (const float*)Y, HG + (int64_t)b * a.B * FC, recs, a.T));
+            if (R.recs.hops)
+                CK(launch_k(false, inter_h_last_kernel, dim3(R.B), dim3(256), 0, st, (const float*)Y, HG + (int64_t)b * R.B * FC, R.recs,
+                            a.T));
         }
         return 0;
     }
     int scatter_hc() {
-        if constexpr (slots)
-            CK(launch_k(false, scatter_hc_kernel, dim3((unsigned)((hc4() + 255) / 256)), dim3(256), 0, st, a.state, recs, e->n_blocks,
-                        a.B, (const float*)HG, (const float*)CG));
+        if constexpr (slots) {
+            if (int rc = hc_copy(true, 0)) return rc;
+            if (K > 1 && e->n_blocks > 1) { if (int rc = hc_copy(true, 1)) return rc; }
+        }
         return 0;
     }
 };
@@ -555,10 +592,10 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
     if ((size_t)ws.total * sizeof(float) > a.ws_bytes) return fail(1, "workspace too small");
     if (int rc = set_attrs()) return rc;
     if ((int64_t)a.B * T * NF > 0x7fffffff / 2) return fail(1, "batch*frames too large for one call; split the batch");
-    if (Chain<Map>::slots && a.targets > 1) return fail(1, "targets cannot be combined with a slot list");
     const ChainForm f = chain_form<Map>(e, a.B, T, a.flags, a.prof != nullptr);
     Chain<Map> c(e, a, st, f, recs, ws);
     MARK("start");
+    if (int rc = c.group_rows()) return rc;
     if (int rc = c.gather_hc()) return rc;
     const BlockRows<Map> R0 = c.rows_of(0);           // the front runs over block 0's rows
     const int gate_ctas = c.K > 1 ? 0 : 1;            // the front's speaker-gate memo CTAs (one per row); fan_out() builds them here
@@ -648,7 +685,7 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
             l.nseq = R.B * NF; l.L = T; l.inner_count = NF; l.outer_stride = (int64_t)T * NF; l.inner_stride = 1;
             l.step_stride = NF; l.ndir = 1;
             if (int rc = c.ln_ih_recurrence(b, R, PL_IH2, l)) return rc;
-            if (int rc = c.h_last(b)) return rc;
+            if (int rc = c.h_last(b, R)) return rc;
             if (b == e->n_blocks - 1) { if (int rc = c.scatter_hc()) return rc; }
             if (int rc = c.dense(b, PL_L2, R, f.pdl)) return rc;
             MARK("gemm_lin_inter");
@@ -713,6 +750,11 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
 
 static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
     const int64_t ss = stream_stride(e->n_blocks);
+    if (a.slots && a.targets > 1) {      // a list of groups: the target rows' record (and hop) lists that Chain::group_rows
+                                         // builds in the workspace at the start of the call
+        const int32_t* lists = reinterpret_cast<const int32_t*>(a.wsp + carve(e->n_blocks, a.B, a.T, a.flags).LISTS);
+        return enqueue_chain_t(e, a, st, Records{ss, lists, a.state_batch, a.hops ? lists + a.B : nullptr, a.T});
+    }
     if (a.slots) return enqueue_chain_t(e, a, st, Records{ss, a.slots, a.state_batch, a.hops, a.T});
     return enqueue_chain_t(e, a, st, ss);
 }
@@ -1326,6 +1368,33 @@ int l2h_sep_forward_targets(void* handle, const float* x, int64_t xbs, int64_t x
     if (int rc_dev = check_device(e)) return rc_dev;
     ChainArgs a{x, xbs, xcs, x_len, emb, static_cast<float*>(state), y, ybs, ycs, y_len, batch * n_targets, frames,
                 static_cast<float*>(ws), ws_bytes, flags & ~L2H_FLAG_GRAPH, 0};
+    a.targets = n_targets;
+    return run_chain(e, a, static_cast<cudaStream_t>(stream), (flags & L2H_FLAG_GRAPH) != 0);
+}
+
+int l2h_sep_forward_targets_groups(void* handle, const float* x, int64_t xbs, int64_t xcs, int32_t x_len, const float* emb,
+                                   void* state, int32_t state_batch, const int32_t* groups_dev, const int32_t* hops_dev, int32_t n,
+                                   int32_t n_targets, int32_t frames, float* y, int64_t ybs, int64_t ycs, int32_t y_len, void* ws,
+                                   size_t ws_bytes, uint32_t flags, void* stream) {
+    SepEngine* e = static_cast<SepEngine*>(handle);
+    if (!e || !x || !emb || !state || !y || !ws || !groups_dev) return fail(1, "null argument");
+    if (n <= 0 || n_targets <= 0 || frames <= 0)
+        return fail(1, "a groups call needs n, n_targets and frames > 0 (n = " + std::to_string(n) + ", n_targets = " +
+                           std::to_string(n_targets) + ", frames = " + std::to_string(frames) + ")");
+    if (state_batch <= 0 || state_batch % n_targets != 0)
+        return fail(1, "a groups call needs a state of groups of n_targets records (state_batch = " + std::to_string(state_batch) +
+                           ", n_targets = " + std::to_string(n_targets) + ")");
+    if (n > state_batch / n_targets)
+        return fail(1, "a group list needs n <= state_batch / n_targets groups (n = " + std::to_string(n) + ", groups = " +
+                           std::to_string(state_batch / n_targets) + ")");
+    if ((int64_t)n * n_targets * frames * NF > 0x7fffffff / 2) return fail(1, "n*n_targets*frames too large for one call; split the list");
+    if (flags & L2H_FLAG_TAPS) return fail(1, "a groups call cannot be combined with L2H_FLAG_TAPS");
+    if (int rc_dev = check_device(e)) return rc_dev;
+    ChainArgs a{x, xbs, xcs, x_len, emb, static_cast<float*>(state), y, ybs, ycs, y_len, n * n_targets, frames,
+                static_cast<float*>(ws), ws_bytes, flags & ~L2H_FLAG_GRAPH, 0};
+    a.slots = groups_dev;
+    a.state_batch = state_batch;
+    a.hops = hops_dev;
     a.targets = n_targets;
     return run_chain(e, a, static_cast<cudaStream_t>(stream), (flags & L2H_FLAG_GRAPH) != 0);
 }

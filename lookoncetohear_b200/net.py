@@ -650,6 +650,46 @@ class Net(nn.Module):
             outs.append(self.predict_targets(xs, es, st)[0])
         return outs[0] if len(outs) == 1 else torch.cat(outs, dim=0)
 
+    def advance_targets(self, x, embeds, state, groups, hops=None):
+        """Advance listed groups of a targets state by T hops each (l2h_sep_forward_targets_groups): the slot-list calls of
+        advance_slots for listeners who each want K speakers.  x [n, M, 128*T + 64] (the pad=False shape), row i the mixture
+        of group groups[i]; embeds [n, K, 256]; state from init_buffers(G*K), in the layout of predict_targets: record
+        g*K + k is target k of group g.  Returns y [n, K, S, 128*T].  The front and block 0 run once per listed group, the
+        rest once per target; groups not listed are neither read nor written.  T = 1 is the one-hop tick.
+
+        `groups` follows the rules of predict(slots=), counted in groups: n distinct ints in [0, G) (a sequence or CPU tensor,
+        checked and uploaded), or a contiguous CUDA int32 tensor of shape (n,) used in place, where an entry outside [0, G)
+        marks a group that stores nothing.  `hops` follows advance_slots(hops=): None (every group advances T hops), or the
+        hops h_i in [0, T] group i advances; its K rows of y receive only y[i, :, :, :128*h_i].  With fixed tensors rewritten
+        in place every tick, one cached graph per (n, K, T) serves every tick.  Reset or copy whole groups of K records
+        (reset_streams(range(g*K, g*K + K)))."""
+        hop, la = self.stft_chunk_size, self.stft_pad_size
+        n, K = self._targets_shape(x, embeds)
+        N = x.shape[-1]
+        if (N - la) % hop != 0 or N < hop + la:
+            raise ValueError(f"advance_targets needs {hop}*T+{la} samples per row, got {N}")
+        if not isinstance(state, SepState):
+            raise TypeError("state must come from Net.init_buffers()")
+        if state.batch % K != 0:
+            raise ValueError(f"a state of {state.batch} records does not hold groups of {K} targets: use init_buffers(G*{K})")
+        frames = (N - la) // hop
+        if hops is not None:
+            hops = self._hop_counts(hops, x.device, n, frames)
+        groups = self._slot_list(groups, x.device, n, state.batch // K)
+        self._require_cuda(x)
+        dev = x.device
+        self._sync_weights(dev)
+        x = x.contiguous().float()
+        emb = embeds.to(dev, torch.float32).reshape(n * K, self.embed_dim).contiguous()
+        y = torch.empty(n, K, self.num_src, frames * hop, dtype=torch.float32, device=dev)
+        ws, _ = self._workspace(dev, n * K, frames)
+        with torch.cuda.device(dev):
+            _cabi.check_args(_cabi.lib().l2h_sep_forward_targets_groups(
+                self._engine(), x.data_ptr(), x.stride(0), x.stride(1), N, emb.data_ptr(), state.buf.data_ptr(), state.batch,
+                groups.data_ptr(), None if hops is None else hops.data_ptr(), n, K, frames, y.data_ptr(), y.stride(1),
+                y.stride(2), frames * hop, ws.data_ptr(), ws.numel(), 0, torch.cuda.current_stream(dev).cuda_stream))
+        return y
+
     def stream_dev(self, x_dev, embed_dev, chunks_per_call=1, state=None, n_calls=None, out=None):
         """Streaming over a device-resident clip (l2h_sep_stream_dev): x_dev [B,M,N] is consumed
         chunks_per_call hops per call with the state carried, every call one CUDA-graph replay.
