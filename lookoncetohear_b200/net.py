@@ -348,19 +348,59 @@ class Net(nn.Module):
         self._dirty = True
         return super()._load_from_state_dict(state_dict, prefix, *args, **kwargs)
 
-    def _workspace(self, device, batch, frames, flags=0):
+    def _cached_workspace(self, device, size_query, *args):
+        """(the net's workspace, grown on `device` to what size_query(handle, *args, &bytes) asks, those bytes)"""
         n = ctypes.c_size_t()
-        _cabi.check(_cabi.lib().l2h_sep_workspace_bytes(self._engine(), batch, frames, flags, ctypes.byref(n)))
+        _cabi.check(size_query(self._engine(), *args, ctypes.byref(n)))
         if self._ws is None or self._ws.numel() < n.value or self._ws.device != device:
             self._ws = torch.empty(n.value, dtype=torch.uint8, device=device)
         return self._ws, n.value
 
+    def _workspace(self, device, batch, frames, flags=0):
+        return self._cached_workspace(device, _cabi.lib().l2h_sep_workspace_bytes, batch, frames, flags)
+
     def _stream_workspace(self, device, batch, chunks_per_call):
-        n = ctypes.c_size_t()
-        _cabi.check(_cabi.lib().l2h_sep_stream_workspace_bytes(self._engine(), batch, chunks_per_call, ctypes.byref(n)))
-        if self._ws is None or self._ws.numel() < n.value or self._ws.device != device:
-            self._ws = torch.empty(n.value, dtype=torch.uint8, device=device)
-        return self._ws, n.value
+        return self._cached_workspace(device, _cabi.lib().l2h_sep_stream_workspace_bytes, batch, chunks_per_call)
+
+    def _launch(self, entry, x, emb, state, y, frames, flags=0, mask=None, slots=None, hops=None, K=1, ws=None):
+        """Run the separator forward C entry point `entry` on the current stream of x's device, on the caller's tensors as
+        they are (a service's fixed buffers keep the cached graph's key).  entry: "forward", "forward_active", "slots",
+        "slots_frames", "slots_hops", "targets" or "targets_groups" (l2h_sep_forward, l2h_sep_forward_<entry>).
+
+        x [rows_x, M, N]; emb [rows, 256]; y [rows, S, N], or for the targets calls [rows_x, K, S, N], passed as its
+        [rows, S, N] view; rows = rows_x * K.  mask: the [rows] uint8 activity mask of forward_active (None: all);
+        slots: the int32 slot list (the group list of targets_groups); hops: the int32 hop counts (None: every row all
+        frames).  ws: a workspace to use, else the net's own, sized for rows and frames.  A rejected argument raises
+        ValueError, except on the dense entries, where every error is a RuntimeError."""
+        dev = x.device
+        self._sync_weights(dev)
+        if y.dim() == 4:
+            y = y.view(-1, *y.shape[2:])
+        if ws is None:
+            ws = self._workspace(dev, y.shape[0], frames, flags)[0]
+        n = x.shape[0]
+        head = (self._engine(), x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], emb.data_ptr(), state.buf.data_ptr())
+        out = (y.data_ptr(), y.stride(0), y.stride(1), y.shape[-1])
+        listed = (state.batch, None if slots is None else slots.data_ptr())
+        hop_list = None if hops is None else hops.data_ptr()
+        with torch.cuda.device(dev):
+            tail = (ws.data_ptr(), ws.numel(), flags, torch.cuda.current_stream(dev).cuda_stream)
+            if entry == "forward":
+                args = (*head, *out, n, frames, *tail)
+            elif entry == "forward_active":
+                args = (*head, *out, n, frames, *tail, None if mask is None else mask.data_ptr())
+            elif entry == "slots":
+                args = (*head, *listed, n, *out, *tail)
+            elif entry == "slots_frames":
+                args = (*head, *listed, n, frames, *out, *tail)
+            elif entry == "slots_hops":
+                args = (*head, *listed, hop_list, n, frames, *out, *tail)
+            elif entry == "targets":
+                args = (*head, *out, n, K, frames, *tail)
+            else:
+                args = (*head, *listed, hop_list, n, K, frames, *out, *tail)
+            fn = getattr(_cabi.lib(), "l2h_sep_" + entry if entry.startswith("forward") else "l2h_sep_forward_" + entry)
+            (_cabi.check if entry.startswith("forward") else _cabi.check_args)(fn(*args))
 
     def set_option(self, name, value):
         """Engine switches: "pipeline" (wavefront pipelining of one-hop calls), "pdl", "fused_tail", "pipeline_frames"
@@ -422,28 +462,13 @@ class Net(nn.Module):
         slots: [B] int32 device list of the state's records the rows advance by `frames` hops, or None; hops: with
         slots, [B] int32 device list of the hops each row advances instead (at most `frames`), or None."""
         self._require_cuda(x)
-        dev = x.device
-        self._sync_weights(dev)
-        x = x.contiguous().float()
-        embed = embed.to(dev, torch.float32).contiguous()
         Bsz = x.shape[0]
         if slots is None and state.batch != Bsz:
             raise ValueError(f"state was built for batch {state.batch}, input has batch {Bsz}")
-        y = torch.empty(Bsz, self.num_src, out_len, dtype=torch.float32, device=dev)
-        ws, nbytes = self._workspace(dev, Bsz, frames, flags)
-        L, st = _cabi.lib(), torch.cuda.current_stream(dev).cuda_stream
-        with torch.cuda.device(dev):
-            if slots is not None:
-                _cabi.check_args(L.l2h_sep_forward_slots_hops(
-                    self._engine(), x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], embed.data_ptr(),
-                    state.buf.data_ptr(), state.batch, slots.data_ptr(), None if hops is None else hops.data_ptr(),
-                    Bsz, frames, y.data_ptr(), y.stride(0), y.stride(1), out_len, ws.data_ptr(), ws.numel(), flags,
-                    st))
-            else:
-                _cabi.check(L.l2h_sep_forward_active(
-                    self._engine(), x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], embed.data_ptr(),
-                    state.buf.data_ptr(), y.data_ptr(), y.stride(0), y.stride(1), out_len, Bsz, frames,
-                    ws.data_ptr(), ws.numel(), flags, st, None if active is None else active.data_ptr()))
+        y = torch.empty(Bsz, self.num_src, out_len, dtype=torch.float32, device=x.device)
+        self._launch("forward_active" if slots is None else "slots_hops", x.contiguous().float(),
+                     embed.to(x.device, torch.float32).contiguous(), state, y, frames, flags, mask=active, slots=slots,
+                     hops=hops)
         return y
 
     @staticmethod
@@ -457,45 +482,54 @@ class Net(nn.Module):
             raise ValueError(f"active must have shape ({batch},), got {tuple(active.shape)}")
         return active.contiguous().view(torch.uint8)
 
-    @staticmethod
-    def _slot_list(slots, dev, n, batch):
-        """`slots` of predict as the [n] int32 device tensor the engine reads.  A CUDA int32 tensor is used as it is (its
-        entries are read when the kernels run); anything else is checked here and uploaded."""
-        if isinstance(slots, torch.Tensor) and slots.is_cuda:
-            if slots.dtype != torch.int32 or tuple(slots.shape) != (n,) or not slots.is_contiguous():
-                raise ValueError(f"a CUDA slot list must be a contiguous int32 tensor of shape ({n},)")
-            if slots.device != dev:
-                raise ValueError(f"slots must live on the input's device {dev}, not {slots.device}")
-            return slots
-        s = torch.as_tensor(slots)
-        if s.dtype.is_floating_point or s.dtype.is_complex or s.dtype == torch.bool or s.dim() != 1:
-            raise ValueError("slots must be a sequence or 1-d tensor of integer slot indices")
-        if s.numel() != n:
-            raise ValueError(f"slots lists {s.numel()} records for {n} input rows")
-        if n > 0 and (int(s.min()) < 0 or int(s.max()) >= batch):
-            raise ValueError(f"a slot lies outside [0, {batch})")
-        if len(set(s.tolist())) != n:
-            raise ValueError("a slot is listed twice")
-        return s.to(torch.int32).to(dev)
+    # the wording of _device_list's errors per list: what its entries are, a wrong count, an entry outside [0, end)
+    _LIST_WORDS = {"slot": ("integer slot indices", "slots lists {} records for {} input rows",
+                            "a slot lies outside [0, {end})"),
+                   "hop": ("integer hop counts", "hops gives {} counts for {} input rows",
+                           "a hop count lies outside [0, {last}] (the call's {last} hops)")}
 
-    @staticmethod
-    def _hop_counts(hops, dev, n, frames):
-        """`hops` of advance_slots as the [n] int32 device tensor the engine reads.  A CUDA int32 tensor is used as it is
-        (its entries are read when the kernels run); anything else is checked here and uploaded."""
-        if isinstance(hops, torch.Tensor) and hops.is_cuda:
-            if hops.dtype != torch.int32 or tuple(hops.shape) != (n,) or not hops.is_contiguous():
-                raise ValueError(f"a CUDA hop list must be a contiguous int32 tensor of shape ({n},)")
-            if hops.device != dev:
-                raise ValueError(f"hops must live on the input's device {dev}, not {hops.device}")
-            return hops
-        h = torch.as_tensor(hops)
-        if h.dtype.is_floating_point or h.dtype.is_complex or h.dtype == torch.bool or h.dim() != 1:
-            raise ValueError("hops must be a sequence or 1-d tensor of integer hop counts")
-        if h.numel() != n:
-            raise ValueError(f"hops gives {h.numel()} counts for {n} input rows")
-        if n > 0 and (int(h.min()) < 0 or int(h.max()) > frames):
-            raise ValueError(f"a hop count lies outside [0, {frames}] (the call's {frames} hops)")
-        return h.to(torch.int32).to(dev)
+    @classmethod
+    def _device_list(cls, values, dev, n, end, distinct, noun):
+        """`values` (slots, groups or hop counts of a call of n rows) as the [n] int32 device tensor the engine reads.  A
+        CUDA int32 tensor is used as it is (its entries are read when the kernels run); anything else is checked here (n
+        ints in [0, end), each listed once if `distinct`) and uploaded.  noun: "slot" or "hop", for the messages."""
+        entries, count, outside = cls._LIST_WORDS[noun]
+        if isinstance(values, torch.Tensor) and values.is_cuda:
+            if values.dtype != torch.int32 or tuple(values.shape) != (n,) or not values.is_contiguous():
+                raise ValueError(f"a CUDA {noun} list must be a contiguous int32 tensor of shape ({n},)")
+            if values.device != dev:
+                raise ValueError(f"{noun}s must live on the input's device {dev}, not {values.device}")
+            return values
+        v = torch.as_tensor(values)
+        if v.dtype.is_floating_point or v.dtype.is_complex or v.dtype == torch.bool or v.dim() != 1:
+            raise ValueError(f"{noun}s must be a sequence or 1-d tensor of {entries}")
+        if v.numel() != n:
+            raise ValueError(count.format(v.numel(), n))
+        if n > 0 and (int(v.min()) < 0 or int(v.max()) >= end):
+            raise ValueError(outside.format(end=end, last=end - 1))
+        if distinct and len(set(v.tolist())) != n:
+            raise ValueError(f"a {noun} is listed twice")
+        return v.to(torch.int32).to(dev)
+
+    @classmethod
+    def _slot_list(cls, slots, dev, n, batch):
+        """slots (or groups) of a call of n rows: n distinct ints in [0, batch), or a CUDA int32 list used in place"""
+        return cls._device_list(slots, dev, n, batch, True, "slot")
+
+    @classmethod
+    def _hop_counts(cls, hops, dev, n, frames):
+        """hop counts of a call of n rows and `frames` hops: n ints in [0, frames], or a CUDA int32 list used in place"""
+        return cls._device_list(hops, dev, n, frames + 1, False, "hop")
+
+    def _frames(self, n, pad=False, who="pad=False", per=""):
+        """(frames, output samples) of a call on n input samples: pad=True rounds up to whole hops and returns n samples;
+        pad=False takes 128*T + 64 samples (the look-ahead included) and returns 128*T.  who / per word the ValueError."""
+        hop, la = self.stft_chunk_size, self.stft_pad_size
+        if pad:
+            return (n + hop - 1) // hop, n
+        if (n - la) % hop != 0 or n < hop + la:
+            raise ValueError(f"{who} needs {hop}*T+{la} samples{per}, got {n}")
+        return (n - la) // hop, (n - la) // hop * hop
 
     def predict(self, x, embed, input_state, pad=True, active=None, slots=None):
         """Reference net.py:54-66.  x [B,M,N]; embed [B,256]; returns (y [B,S,*], state).
@@ -509,15 +543,7 @@ class Net(nn.Module):
         int32 tensor used in place: there an entry outside [0, state.batch) marks a row that stores nothing (its y row is
         left unwritten), and listing a slot twice is the caller's error.  Cannot be combined with `active`."""
         hop, la = self.stft_chunk_size, self.stft_pad_size
-        n = x.shape[-1]
-        if pad:
-            frames = (n + hop - 1) // hop          # mod-pad to whole hops, + look-ahead zeros
-            out_len = n
-        else:
-            if (n - la) % hop != 0 or n < hop + la:
-                raise ValueError(f"pad=False needs {hop}*T+{la} samples, got {n}")
-            frames = (n - la) // hop
-            out_len = frames * hop
+        frames, out_len = self._frames(x.shape[-1], pad)
         if not isinstance(input_state, SepState):
             raise TypeError("input_state must come from Net.init_buffers()")
         if slots is not None:
@@ -551,27 +577,23 @@ class Net(nn.Module):
         contiguous CUDA int32 tensor of shape (n,) used in place, as for `slots`: there an entry outside [0, T] counts
         as 0.  With fixed slot and hop tensors rewritten in place every tick, one cached graph per (n, T) serves every
         mix of backlogs up to T."""
-        hop, la = self.stft_chunk_size, self.stft_pad_size
         if x.dim() != 3:
-            raise ValueError(f"advance_slots needs x of shape [n, channels, {hop}*T+{la}], got {tuple(x.shape)}")
-        n = x.shape[-1]
-        if (n - la) % hop != 0 or n < hop + la:
-            raise ValueError(f"advance_slots needs {hop}*T+{la} samples per row, got {n}")
+            raise ValueError(f"advance_slots needs x of shape [n, channels, {self.stft_chunk_size}*T+{self.stft_pad_size}], "
+                             f"got {tuple(x.shape)}")
+        frames, out_len = self._frames(x.shape[-1], who="advance_slots", per=" per row")
         if not isinstance(state, SepState):
             raise TypeError("state must come from Net.init_buffers()")
-        frames = (n - la) // hop
         if hops is not None:
             hops = self._hop_counts(hops, x.device, x.shape[0], frames)
         self._require_cuda(x)
         slots = self._slot_list(slots, x.device, x.shape[0], state.batch)
-        return self._run(x, embed, state, frames, frames * hop, slots=slots, hops=hops)
+        return self._run(x, embed, state, frames, out_len, slots=slots, hops=hops)
 
     def forward(self, x, embeds, input_state=None, pad=True):
         """Reference net.py:68-76.  x [B,M,N]; embeds [B,1,256] -> [B,S,N]."""
         embeds = embeds[:, 0]
         Bsz = x.shape[0]
-        hop = self.stft_chunk_size
-        frames = (x.shape[-1] + hop - 1) // hop
+        frames = self._frames(x.shape[-1], pad=True)[0]
         # independent streams: split the batch so batch*frames stays inside the workspace bound
         per = max(1, self.max_frames_per_launch // max(frames, 1))
         if input_state is not None or Bsz <= per:
@@ -609,39 +631,28 @@ class Net(nn.Module):
         SepState).  Each target gets the output of predict on its mixture alone, up to the rounding of one stage in the
         fused one-hop form (include/lookonce_b200.h)."""
         Bsz, K = self._targets_shape(x, embeds)
-        hop, la = self.stft_chunk_size, self.stft_pad_size
-        n = x.shape[-1]
-        if pad:
-            frames, out_len = (n + hop - 1) // hop, n
-        else:
-            if (n - la) % hop != 0 or n < hop + la:
-                raise ValueError(f"pad=False needs {hop}*T+{la} samples, got {n}")
-            frames = (n - la) // hop
-            out_len = frames * hop
+        frames, out_len = self._frames(x.shape[-1], pad)
         if not isinstance(state, SepState):
             raise TypeError("state must come from Net.init_buffers()")
         if state.batch != Bsz * K:
             raise ValueError(f"state was built for batch {state.batch}, a call of {Bsz} mixtures x {K} targets needs "
                              f"init_buffers({Bsz * K})")
+        return self._run_targets("targets", x, embeds, state, frames, out_len), state
+
+    def _run_targets(self, entry, x, embeds, state, frames, out_len, groups=None, hops=None):
+        """y [B, K, S, out_len] of the targets call `entry` on x [B, M, N] and embeds [B, K, 256]"""
         self._require_cuda(x)
-        dev = x.device
-        self._sync_weights(dev)
-        x = x.contiguous().float()
-        emb = embeds.to(dev, torch.float32).reshape(Bsz * K, self.embed_dim).contiguous()
-        y = torch.empty(Bsz, K, self.num_src, out_len, dtype=torch.float32, device=dev)
-        ws, _ = self._workspace(dev, Bsz * K, frames)
-        with torch.cuda.device(dev):
-            _cabi.check_args(_cabi.lib().l2h_sep_forward_targets(
-                self._engine(), x.data_ptr(), x.stride(0), x.stride(1), n, emb.data_ptr(), state.buf.data_ptr(),
-                y.data_ptr(), y.stride(1), y.stride(2), out_len, Bsz, K, frames, ws.data_ptr(), ws.numel(), 0,
-                torch.cuda.current_stream(dev).cuda_stream))
-        return y, state
+        Bsz, K = embeds.shape[:2]
+        y = torch.empty(Bsz, K, self.num_src, out_len, dtype=torch.float32, device=x.device)
+        self._launch(entry, x.contiguous().float(), embeds.to(x.device, torch.float32).reshape(Bsz * K, self.embed_dim)
+                     .contiguous(), state, y, frames, slots=groups, hops=hops, K=K)
+        return y
 
     def forward_targets(self, x, embeds):
         """x [B,M,N], embeds [B,K,256] -> [B,K,S,N]: every mixture separated for each of its K targets, on a fresh state,
         padded as forward() pads.  Long batches are split as forward() splits them, counting target rows."""
         Bsz, K = self._targets_shape(x, embeds)
-        frames = (x.shape[-1] + self.stft_chunk_size - 1) // self.stft_chunk_size
+        frames = self._frames(x.shape[-1], pad=True)[0]
         per = max(1, self.max_frames_per_launch // max(frames * K, 1))
         outs = []
         for b0 in range(0, Bsz, per):
@@ -663,32 +674,16 @@ class Net(nn.Module):
         hops h_i in [0, T] group i advances; its K rows of y receive only y[i, :, :, :128*h_i].  With fixed tensors rewritten
         in place every tick, one cached graph per (n, K, T) serves every tick.  Reset or copy whole groups of K records
         (reset_streams(range(g*K, g*K + K)))."""
-        hop, la = self.stft_chunk_size, self.stft_pad_size
         n, K = self._targets_shape(x, embeds)
-        N = x.shape[-1]
-        if (N - la) % hop != 0 or N < hop + la:
-            raise ValueError(f"advance_targets needs {hop}*T+{la} samples per row, got {N}")
+        frames, out_len = self._frames(x.shape[-1], who="advance_targets", per=" per row")
         if not isinstance(state, SepState):
             raise TypeError("state must come from Net.init_buffers()")
         if state.batch % K != 0:
             raise ValueError(f"a state of {state.batch} records does not hold groups of {K} targets: use init_buffers(G*{K})")
-        frames = (N - la) // hop
         if hops is not None:
             hops = self._hop_counts(hops, x.device, n, frames)
         groups = self._slot_list(groups, x.device, n, state.batch // K)
-        self._require_cuda(x)
-        dev = x.device
-        self._sync_weights(dev)
-        x = x.contiguous().float()
-        emb = embeds.to(dev, torch.float32).reshape(n * K, self.embed_dim).contiguous()
-        y = torch.empty(n, K, self.num_src, frames * hop, dtype=torch.float32, device=dev)
-        ws, _ = self._workspace(dev, n * K, frames)
-        with torch.cuda.device(dev):
-            _cabi.check_args(_cabi.lib().l2h_sep_forward_targets_groups(
-                self._engine(), x.data_ptr(), x.stride(0), x.stride(1), N, emb.data_ptr(), state.buf.data_ptr(), state.batch,
-                groups.data_ptr(), None if hops is None else hops.data_ptr(), n, K, frames, y.data_ptr(), y.stride(1),
-                y.stride(2), frames * hop, ws.data_ptr(), ws.numel(), 0, torch.cuda.current_stream(dev).cuda_stream))
-        return y
+        return self._run_targets("targets_groups", x, embeds, state, frames, out_len, groups, hops)
 
     def stream_dev(self, x_dev, embed_dev, chunks_per_call=1, state=None, n_calls=None, out=None):
         """Streaming over a device-resident clip (l2h_sep_stream_dev): x_dev [B,M,N] is consumed
@@ -764,11 +759,8 @@ class Net(nn.Module):
         dev = embed_dev.device
         self._require_cuda(embed_dev)
         self._sync_weights(dev)
-        hop, la = self.stft_chunk_size, self.stft_pad_size
         Bsz, _, n = x_host.shape
-        if (n - la) % hop != 0 or n < hop + la:
-            raise ValueError(f"predict_host needs {hop}*T+{la} samples, got {n}")
-        frames = (n - la) // hop
+        frames, out_len = self._frames(n, who="predict_host")
         if not (x_host.is_pinned() and x_host.is_contiguous() and x_host.dtype == torch.float32):
             raise ValueError("x_host must be a contiguous pinned float32 tensor")
         if not isinstance(state, SepState):
@@ -776,19 +768,19 @@ class Net(nn.Module):
         key = (Bsz, frames, str(dev))
         cache = getattr(self, "_predict_stage", None)
         if cache is None or cache[0] != key:
-            cache = (key, torch.empty(Bsz, self.num_src, hop * frames, dtype=torch.float32).pin_memory(),
+            cache = (key, torch.empty(Bsz, self.num_src, out_len, dtype=torch.float32).pin_memory(),
                      torch.empty(Bsz, self.num_ch, n, dtype=torch.float32, device=dev),
-                     torch.empty(Bsz, self.num_src, hop * frames, dtype=torch.float32, device=dev),
+                     torch.empty(Bsz, self.num_src, out_len, dtype=torch.float32, device=dev),
                      self._stream_workspace(dev, Bsz, frames)[0])
             self._predict_stage = cache
         _, yh_c, xs, ys, ws = cache
         emb = embed_dev if (embed_dev.dtype == torch.float32 and embed_dev.is_contiguous()) else embed_dev.to(torch.float32).contiguous()
         yh = out if out is not None else yh_c
-        if not yh.is_pinned() or not yh.is_contiguous() or tuple(yh.shape) != (Bsz, self.num_src, hop * frames):
+        if not yh.is_pinned() or not yh.is_contiguous() or tuple(yh.shape) != (Bsz, self.num_src, out_len):
             raise ValueError("out must be a contiguous pinned [B, S, 128*T] float32 tensor")
         with torch.cuda.device(dev):
             _cabi.check(_cabi.lib().l2h_sep_stream_host(
-                self._engine(), x_host.data_ptr(), n, emb.data_ptr(), state.buf.data_ptr(), yh.data_ptr(), hop * frames, Bsz, 1,
+                self._engine(), x_host.data_ptr(), n, emb.data_ptr(), state.buf.data_ptr(), yh.data_ptr(), out_len, Bsz, 1,
                 frames, xs.data_ptr(), ys.data_ptr(), ws.data_ptr(), ws.numel(), torch.cuda.current_stream(dev).cuda_stream))
         return yh, state
 
@@ -797,8 +789,7 @@ class Net(nn.Module):
         """Whole-utterance forward that also returns the activations after every stage
         ([B,T,97,64] each): encoder, then per block (after intra, after inter, block output)."""
         embeds = embeds[:, 0]
-        hop = self.stft_chunk_size
-        frames = (x.shape[-1] + hop - 1) // hop
+        frames = self._frames(x.shape[-1], pad=True)[0]
         st = self.init_buffers(x.shape[0], x.device)
         y = self._run(x, embeds, st, frames, x.shape[-1], flags=1)
         off, ns = ctypes.c_int64(), ctypes.c_int32()

@@ -2,23 +2,12 @@
 argument errors the C call returns before it touches the device, the Python ValueErrors, and the header's description
 (no GPU needed; the handle below never commits weights)."""
 import ctypes
-import os
-import re
 
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-FAKE_DEV = ctypes.c_void_p(0x10000)          # never dereferenced: every call below fails its argument checks first
-L2H_FLAG_TAPS = 1
-
-
-@pytest.fixture(scope="module")
-def eng(tsh_params):
-    from lookoncetohear_b200 import Net, build, _cabi
-    build.build()
-    net = Net(**tsh_params)
-    return net, net._engine(), _cabi.lib()
+import serving_util as su
+from serving_util import FAKE_DEV, L2H_FLAG_TAPS, eng  # noqa: F401
 
 
 def _call(L, h, state_batch, slots, n, flags=0, p=FAKE_DEV):
@@ -45,7 +34,6 @@ def test_forward_slots_argument_errors(eng):
 
 def test_python_slot_lists_raise_value_error(eng):
     net, _, _ = eng
-    from lookoncetohear_b200.net import SepState
     cpu = torch.device("cpu")
     for bad in ([0, 0, 1], [0, 1, 4], [-1, 0, 1], [0, 1], [0, 1, 2, 3], [[0, 1, 2]], [0.0, 1.0, 2.0],
                 torch.tensor([True, False, True])):
@@ -54,8 +42,7 @@ def test_python_slot_lists_raise_value_error(eng):
     got = net._slot_list(torch.tensor([3, 0, 2]), cpu, 3, 4)
     assert got.dtype == torch.int32 and got.tolist() == [3, 0, 2]
     assert net._slot_list((1, 2, 0), cpu, 3, 4).tolist() == [1, 2, 0]
-    hb, stride, offs = net._state_layout()
-    st = SepState(torch.zeros(hb // 4 + 4 * stride), 4, 3, hb, stride, offs)
+    st = su.host_state(net, 4)
     one_hop, two_hops = torch.zeros(2, 2, 192), torch.zeros(2, 2, 320)
     emb = torch.zeros(2, 256)
     with pytest.raises(ValueError):          # a list needs a one-hop call
@@ -65,14 +52,13 @@ def test_python_slot_lists_raise_value_error(eng):
 
 
 def test_header_documents_forward_slots():
-    hdr = open(os.path.join(ROOT, "include", "lookonce_b200.h")).read()
-    decl = re.search(r"int l2h_sep_forward_slots\((.*?)\);", hdr, flags=re.S)
+    hdr = su.header()
+    decl, args = su.declaration(hdr, "l2h_sep_forward_slots")
     assert decl, "l2h_sep_forward_slots is not declared"
-    args = [a.split()[-1].lstrip("*") for a in " ".join(decl.group(1).split()).split(",")]
     assert args == ["handle", "x_dev", "x_batch_stride", "x_ch_stride", "x_len", "emb_dev", "state_dev", "state_batch",
                     "slots_dev", "n", "y_dev", "y_batch_stride", "y_ch_stride", "y_len", "workspace_dev", "workspace_bytes",
                     "flags", "stream"]
-    doc = " ".join(re.sub(r"\n\s*\*", " ", hdr[:decl.start()].rsplit("/*", 1)[1]).split())
+    doc = su.doc_before(hdr, decl.start())
     for phrase in ("slots_dev[i]", "l2h_sep_workspace_bytes(handle, n, 1, flags)", "outside [0, state_batch)",
                    "L2H_FLAG_GRAPH", "n > state_batch", "L2H_FLAG_TAPS", "neither read nor written"):
         assert phrase in doc, phrase

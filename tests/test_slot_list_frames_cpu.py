@@ -2,23 +2,12 @@
 Net.advance_slots): the argument errors the C call returns before it touches the device, the Python ValueErrors, and the
 header's description (no GPU needed; the handle below never commits weights)."""
 import ctypes
-import os
-import re
 
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-FAKE_DEV = ctypes.c_void_p(0x10000)          # never dereferenced: every call below fails its argument checks first
-L2H_FLAG_TAPS = 1
-
-
-@pytest.fixture(scope="module")
-def eng(tsh_params):
-    from lookoncetohear_b200 import Net, build, _cabi
-    build.build()
-    net = Net(**tsh_params)
-    return net, net._engine(), _cabi.lib()
+import serving_util as su
+from serving_util import FAKE_DEV, L2H_FLAG_TAPS, eng  # noqa: F401
 
 
 def _call(L, h, state_batch, slots, n, frames, flags=0, p=FAKE_DEV):
@@ -57,9 +46,7 @@ def test_forward_slots_is_the_one_hop_form(eng):
 
 def test_python_advance_slots_raises_value_error(eng):
     net, _, _ = eng
-    from lookoncetohear_b200.net import SepState
-    hb, stride, offs = net._state_layout()
-    st = SepState(torch.zeros(hb // 4 + 4 * stride), 4, 3, hb, stride, offs)
+    st = su.host_state(net, 4)
     emb = torch.zeros(2, 256)
     for n in (128 * 3, 128 * 3 + 63, 128 * 3 + 65, 64, 0, 191):          # not 128*T + 64 with T >= 1
         with pytest.raises(ValueError):
@@ -71,14 +58,13 @@ def test_python_advance_slots_raises_value_error(eng):
 
 
 def test_header_documents_forward_slots_frames():
-    hdr = open(os.path.join(ROOT, "include", "lookonce_b200.h")).read()
-    decl = re.search(r"int l2h_sep_forward_slots_frames\((.*?)\);", hdr, flags=re.S)
+    hdr = su.header()
+    decl, args = su.declaration(hdr, "l2h_sep_forward_slots_frames")
     assert decl, "l2h_sep_forward_slots_frames is not declared"
-    args = [a.split()[-1].lstrip("*") for a in " ".join(decl.group(1).split()).split(",")]
     assert args == ["handle", "x_dev", "x_batch_stride", "x_ch_stride", "x_len", "emb_dev", "state_dev", "state_batch",
                     "slots_dev", "n", "frames", "y_dev", "y_batch_stride", "y_ch_stride", "y_len", "workspace_dev",
                     "workspace_bytes", "flags", "stream"]
-    doc = " ".join(re.sub(r"\n\s*\*", " ", hdr[:decl.start()].rsplit("/*", 1)[1]).split())
+    doc = su.doc_before(hdr, decl.start())
     for phrase in ("128*frames + 64", "128*frames samples", "l2h_sep_workspace_bytes(handle, n, frames, flags)",
                    "outside [0, state_batch)", "for all of its frames", "L2H_FLAG_GRAPH", "frames <= 0", "n > state_batch",
                    "L2H_FLAG_TAPS", "neither read nor written", "frames == 1"):

@@ -9,12 +9,12 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from lookoncetohear_b200 import Net, synth, _cabi
+from lookoncetohear_b200 import synth
 from oracle import restate as rs
+import serving_util as su
+from serving_util import HOP, LA, L2H_FLAG_GRAPH, dev, model  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-HOP, LA = 128, 64
-L2H_FLAG_GRAPH = 2
 # (records in the state, listed rows per call, hops per call, engine options)
 FORMS = [pytest.param((12, 2, 3, {"back_many": 1}), id="n2-T3"),
          pytest.param((12, 2, 3, {"back_many": 0}), id="n2-T3-per-frame"),
@@ -23,26 +23,6 @@ FORMS = [pytest.param((12, 2, 3, {"back_many": 1}), id="n2-T3"),
          pytest.param((16, 8, 3, {}), id="n8-T3-tc"),
          pytest.param((56, 48, 2, {}), id="n48-T2-tc-lstm"),
          pytest.param((56, 48, 2, {"fuse_ih": 1}), id="n48-T2-tc-lstm-x")]
-DEFAULTS = {"back_many": 1, "fuse_ih": 0}
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda", 0)
-
-
-@pytest.fixture(scope="module")
-def model(tsh_params, dev):
-    torch.manual_seed(0)
-    net = Net(**tsh_params).eval()
-    sd = {k: v.detach().clone() for k, v in net.state_dict().items()}
-    return net.to(dev), sd
-
-
-def _switched(net, opts):
-    for k, v in opts.items():
-        net.set_option(k, v)
 
 
 @pytest.fixture(params=FORMS)
@@ -50,63 +30,8 @@ def form(request, model):
     """(net, sd, S, n, T): the network switched to the kernel form under test for the test's duration."""
     S, n, T, opts = request.param
     net, sd = model
-    _switched(net, opts)
-    yield net, sd, S, n, T
-    _switched(net, {k: DEFAULTS[k] for k in opts})
-
-
-def _clips(n, hops, seed, dev):
-    x, tgt = synth.mixture(n, HOP * hops, seed0=seed)
-    return F.pad(x, (0, LA)).to(dev), tgt
-
-
-def _emb(n, seed, dev):
-    return synth.embedding(n, seed0=seed)[:, 0].to(dev)
-
-
-def _chunk(clip, t, T):
-    """hops t .. t+T-1 of one padded clip [2, N]: their 128*T samples + the 64 look-ahead samples"""
-    return clip[:, HOP * t:HOP * (t + T) + LA]
-
-
-def _subsets(S, n, calls, seed):
-    """a different unsorted list of n distinct slots for every call"""
-    g = torch.Generator().manual_seed(seed)
-    return [torch.randperm(S, generator=g)[:n].tolist() for _ in range(calls)]
-
-
-def _bits(t):
-    """a float tensor as its bit patterns: records hold NaN (the embedding of a fresh stream), which torch.equal rejects"""
-    return t.contiguous().view(torch.int32)
-
-
-def _records(st):
-    """every record of the state as bits, the gate memo's weight generation word cleared: copy_streams_from invalidates
-    the memo of the records it writes (by design), so the oracle's records carry generation 0 where a slot-list call
-    keeps it."""
-    r = _bits(st._rec()).clone()
-    r[:, st.lay["st_emb"] + 256] = 0
-    return r
-
-
-def _oracle(net, ref, x, e, sl):
-    """the listed records of `ref` advanced by a dense predict of len(sl) streams: copy in, run, copy back"""
-    n = len(sl)
-    dense = net.init_buffers(n, x.device)
-    dense.copy_streams_from(ref, sl, list(range(n)))
-    y, _ = net.predict(x, e, dense, pad=False)
-    ref.copy_streams_from(dense, list(range(n)), sl)
-    return y
-
-
-def _forward_slots_frames(net, st, x, e, slots, y, T, flags, dev):
-    """l2h_sep_forward_slots_frames on fixed buffers (a service's staging buffers; with L2H_FLAG_GRAPH one cached graph)"""
-    n = x.shape[0]
-    ws, _ = net._workspace(dev, n, T)
-    _cabi.check(_cabi.lib().l2h_sep_forward_slots_frames(
-        net._engine(), x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], e.data_ptr(), st.buf.data_ptr(), st.batch,
-        slots.data_ptr(), n, T, y.data_ptr(), y.stride(0), y.stride(1), y.shape[-1], ws.data_ptr(), ws.numel(), flags,
-        torch.cuda.current_stream(dev).cuda_stream))
+    with su.switched(net, opts):
+        yield net, sd, S, n, T
 
 
 def test_slots_frames_equal_copy_run_copy_back(form, dev):
@@ -114,23 +39,23 @@ def test_slots_frames_equal_copy_run_copy_back(form, dev):
     records (untouched) equal the copy / dense T-hop predict / copy back oracle bit for bit."""
     net, _, S, n, T = form
     calls = 6
-    clips, _ = _clips(S, calls * T, 4100, dev)
-    e = _emb(S, 4200, dev)
+    clips, _ = su.clips(S, calls * T, 4100, dev)
+    e = su.emb(S, 4200, dev)
     got, ref = net.init_buffers(S, dev), net.init_buffers(S, dev)
     fed = [0] * S
     with torch.no_grad():
-        for c, sl in enumerate(_subsets(S, n, calls, 4300)):
-            x = torch.stack([_chunk(clips[s], fed[s], T) for s in sl])
+        for c, sl in enumerate(su.subsets(S, n, calls, 4300)):
+            x = torch.stack([su.chunk(clips[s], fed[s], T) for s in sl])
             before = got._rec().clone()
             y = net.advance_slots(x, e[sl], got, sl)
-            y_ref = _oracle(net, ref, x, e[sl], sl)
+            y_ref = su.oracle(net, ref, sl, x, e[sl])
             for s in sl:
                 fed[s] += T
             assert y.shape == (n, 2, HOP * T)
             assert torch.equal(y, y_ref), f"call {c}: y"
             unlisted = [s for s in range(S) if s not in sl]
-            assert torch.equal(_bits(got._rec()[unlisted]), _bits(before[unlisted])), f"call {c}: an unlisted record changed"
-            assert torch.equal(_records(got), _records(ref)), f"call {c}: records"
+            assert torch.equal(su.bits(got._rec()[unlisted]), su.bits(before[unlisted])), f"call {c}: an unlisted record changed"
+            assert torch.equal(su.records(got), su.records(ref)), f"call {c}: records"
     assert got.stream_pos() == fed and got.header() == (calls * T, calls)
 
 
@@ -141,24 +66,23 @@ def test_mixed_clocks_and_hop_counts(model, dev, S, n, opts):
     records, calls whose hops cross a multiple of the 56-slot K/V ring, and records reset mid-test: every call equals
     the oracle bit for bit."""
     net, _ = model
-    _switched(net, opts)
-    try:
-        clips, _ = _clips(S, 120, 4400, dev)
-        e = _emb(S, 4500, dev)
+    with su.switched(net, opts):
+        clips, _ = su.clips(S, 120, 4400, dev)
+        e = su.emb(S, 4500, dev)
         got = net.init_buffers(S, dev)
         warm = 50 + torch.arange(S) % 5                    # clocks 50 .. 54: 2 to 6 hops below the ring's wrap
         fed = warm.tolist()
         with torch.no_grad():
             for s in range(S):                              # one dense multi-hop call per record, in a state of one
                 one = net.init_buffers(1, dev)
-                net.predict(_chunk(clips[s], 0, fed[s])[None], e[s:s + 1], one, pad=False)
+                net.predict(su.chunk(clips[s], 0, fed[s])[None], e[s:s + 1], one, pad=False)
                 got.copy_streams_from(one, [0], [s])
             ref = net.init_buffers(S, dev)
             ref.buf.copy_(got.buf)
             # (hops, how): "p" = predict(slots=), "a" = advance_slots
             plan = [(2, "a"), (5, "a"), (1, "p"), (5, "a"), (1, "a"), (2, "a"), ("reset", None), (5, "a"), (1, "p"),
                     (5, "a"), (2, "a"), (1, "p"), (5, "a")]
-            lists = iter(_subsets(S, n, len(plan), 4600))
+            lists = iter(su.subsets(S, n, len(plan), 4600))
             frames = calls = 0
             for step, (T, how) in enumerate(plan):
                 sl = next(lists)
@@ -168,21 +92,19 @@ def test_mixed_clocks_and_hop_counts(model, dev, S, n, opts):
                     for s in sl[:2]:
                         fed[s] = 0
                     continue
-                x = torch.stack([_chunk(clips[s], fed[s], T) for s in sl])
+                x = torch.stack([su.chunk(clips[s], fed[s], T) for s in sl])
                 if how == "p":
                     y, _ = net.predict(x, e[sl], got, pad=False, slots=sl)
                 else:
                     y = net.advance_slots(x, e[sl], got, sl)
-                y_ref = _oracle(net, ref, x, e[sl], sl)
+                y_ref = su.oracle(net, ref, sl, x, e[sl])
                 for s in sl:
                     fed[s] += T
                 frames, calls = frames + T, calls + 1
                 assert torch.equal(y, y_ref), f"step {step}: y"
-                assert torch.equal(_records(got), _records(ref)), f"step {step}: records"
+                assert torch.equal(su.records(got), su.records(ref)), f"step {step}: records"
         assert got.stream_pos() == fed and max(fed) > 56
         assert got.header() == (frames, calls)          # copying records in leaves the header as it was
-    finally:
-        _switched(net, {k: DEFAULTS[k] for k in opts})
 
 
 def test_entries_outside_the_state_store_nothing(form, dev):
@@ -190,20 +112,20 @@ def test_entries_outside_the_state_store_nothing(form, dev):
     untouched for all of their hops; the other rows equal the same call with those entries pointing at spare records of
     a copy of the state."""
     net, _, S, n, T = form
-    clips, _ = _clips(S, 4 * T, 4700, dev)
-    e = _emb(S, 4800, dev)
+    clips, _ = su.clips(S, 4 * T, 4700, dev)
+    e = su.emb(S, 4800, dev)
     st = net.init_buffers(S, dev)
     with torch.no_grad():
-        for c, sl in enumerate(_subsets(S, n, 3, 4900)):     # records with history and different clocks
-            net.advance_slots(torch.stack([_chunk(clips[s], c * T, T) for s in sl]), e[sl], st, sl)
-    sl = _subsets(S, n, 1, 5000)[0]
+        for c, sl in enumerate(su.subsets(S, n, 3, 4900)):     # records with history and different clocks
+            net.advance_slots(torch.stack([su.chunk(clips[s], c * T, T) for s in sl]), e[sl], st, sl)
+    sl = su.subsets(S, n, 1, 5000)[0]
     bad = {0: -1, n - 1: S + 3} if n > 2 else {0: -1}
     spare = [s for s in range(S) if s not in sl][:len(bad)]
     with_bad = [bad.get(i, s) for i, s in enumerate(sl)]
     with_spare = list(with_bad)
     for i, sp in zip(bad, spare):
         with_spare[i] = sp
-    x = torch.stack([_chunk(clips[s], 3 * T, T) for s in sl])
+    x = torch.stack([su.chunk(clips[s], 3 * T, T) for s in sl])
     ee = e[sl].contiguous()
     net._sync_weights(dev)
     twin = net.init_buffers(S, dev)
@@ -211,8 +133,8 @@ def test_entries_outside_the_state_store_nothing(form, dev):
     before = st._rec().clone()
     y = torch.full((n, 2, HOP * T), float("nan"), device=dev)
     y_twin = torch.full_like(y, float("nan"))
-    _forward_slots_frames(net, st, x, ee, torch.tensor(with_bad, dtype=torch.int32, device=dev), y, T, 0, dev)
-    _forward_slots_frames(net, twin, x, ee, torch.tensor(with_spare, dtype=torch.int32, device=dev), y_twin, T, 0, dev)
+    net._launch("slots_frames", x, ee, st, y, T, slots=torch.tensor(with_bad, dtype=torch.int32, device=dev))
+    net._launch("slots_frames", x, ee, twin, y_twin, T, slots=torch.tensor(with_spare, dtype=torch.int32, device=dev))
     torch.cuda.synchronize()
     stored = [s for s in with_bad if 0 <= s < S]
     for i in range(n):
@@ -222,8 +144,8 @@ def test_entries_outside_the_state_store_nothing(form, dev):
             assert torch.equal(y[i], y_twin[i]), f"row {i}"
             assert not bool(torch.isnan(y[i]).any())
     others = [s for s in range(S) if s not in stored]
-    assert torch.equal(_bits(st._rec()[others]), _bits(before[others])), "a record not listed (or listed out of range) changed"
-    assert torch.equal(_bits(st._rec()[stored]), _bits(twin._rec()[stored]))
+    assert torch.equal(su.bits(st._rec()[others]), su.bits(before[others])), "a record not listed (or listed out of range) changed"
+    assert torch.equal(su.bits(st._rec()[stored]), su.bits(twin._rec()[stored]))
     assert [st.stream_pos()[s] for s in spare] == [twin.stream_pos()[s] - T for s in spare]
 
 
@@ -232,24 +154,24 @@ def test_graph_replay_with_list_rewritten_in_place(form, dev):
     is replayed: y and the whole state equal direct calls."""
     net, _, S, n, T = form
     calls = 4
-    clips, _ = _clips(S, calls * T, 5100, dev)
-    e = _emb(S, 5200, dev)
+    clips, _ = su.clips(S, calls * T, 5100, dev)
+    e = su.emb(S, 5200, dev)
     net._sync_weights(dev)
     xbuf, ebuf = torch.empty(n, 2, HOP * T + LA, device=dev), torch.empty(n, 256, device=dev)
     slots = torch.empty(n, dtype=torch.int32, device=dev)
     yg, yd = torch.empty(n, 2, HOP * T, device=dev), torch.empty(n, 2, HOP * T, device=dev)
     sg, sdir = net.init_buffers(S, dev), net.init_buffers(S, dev)
     fed = [0] * S
-    for c, sl in enumerate(_subsets(S, n, calls, 5300)):
-        xbuf.copy_(torch.stack([_chunk(clips[s], fed[s], T) for s in sl]))
+    for c, sl in enumerate(su.subsets(S, n, calls, 5300)):
+        xbuf.copy_(torch.stack([su.chunk(clips[s], fed[s], T) for s in sl]))
         ebuf.copy_(e[sl])
         slots.copy_(torch.tensor(sl, dtype=torch.int32))
-        _forward_slots_frames(net, sg, xbuf, ebuf, slots, yg, T, L2H_FLAG_GRAPH, dev)
-        _forward_slots_frames(net, sdir, xbuf, ebuf, slots, yd, T, 0, dev)
+        net._launch("slots_frames", xbuf, ebuf, sg, yg, T, L2H_FLAG_GRAPH, slots=slots)
+        net._launch("slots_frames", xbuf, ebuf, sdir, yd, T, slots=slots)
         for s in sl:
             fed[s] += T
         assert torch.equal(yg, yd), c
-    assert torch.equal(_bits(sg.buf), _bits(sdir.buf))
+    assert torch.equal(su.bits(sg.buf), su.bits(sdir.buf))
 
 
 @pytest.mark.parametrize("S, n", [pytest.param(6, 2, id="n2"), pytest.param(16, 8, id="n8-tc")])
@@ -264,15 +186,15 @@ def test_listed_stream_vs_oracle(model, dev, S, n):
     n_fed = sum(T for c, T in enumerate(plan) if c not in skipped)
     x_cpu, tgt = synth.mixture(1, HOP * n_fed, seed0=5400)
     xc = F.pad(x_cpu, (0, LA)).to(dev)
-    others, _ = _clips(S, sum(plan), 5500, dev)
-    e = _emb(S, 5600, dev)
+    others, _ = su.clips(S, sum(plan), 5500, dev)
+    e = su.emb(S, 5600, dev)
     st = net.init_buffers(S, dev)
     got, fed, t0 = [], 0, 0
     with torch.no_grad():
-        for c, (T, sl) in enumerate(zip(plan, _subsets(S - 1, n, len(plan), 5700))):
+        for c, (T, sl) in enumerate(zip(plan, su.subsets(S - 1, n, len(plan), 5700))):
             if c not in skipped:
                 sl[c % n] = s
-            x = torch.stack([_chunk(xc[0], fed, T) if b == s else _chunk(others[b], t0, T) for b in sl])
+            x = torch.stack([su.chunk(xc[0], fed, T) if b == s else su.chunk(others[b], t0, T) for b in sl])
             y = net.advance_slots(x, e[sl], st, sl)
             if c not in skipped:
                 got.append(y[c % n])

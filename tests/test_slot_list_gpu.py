@@ -7,29 +7,15 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from lookoncetohear_b200 import Net, synth, _cabi
+from lookoncetohear_b200 import synth
 from oracle import restate as rs
+import serving_util as su
+from serving_util import HOP, LA, L2H_FLAG_GRAPH, dev, model  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-HOP, LA = 128, 64
-L2H_FLAG_GRAPH = 2
 # (records in the state, listed rows per call, fused_tail)
 FORMS = [pytest.param((40, 2, 1), id="n2-fused"), pytest.param((40, 2, 0), id="n2-separate"),
          pytest.param((40, 16, 1), id="n16-mid-split"), pytest.param((64, 24, 1), id="n24-tc")]
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda", 0)
-
-
-@pytest.fixture(scope="module")
-def model(tsh_params, dev):
-    torch.manual_seed(0)
-    net = Net(**tsh_params).eval()
-    sd = {k: v.detach().clone() for k, v in net.state_dict().items()}
-    return net.to(dev), sd
 
 
 @pytest.fixture(params=FORMS)
@@ -37,53 +23,8 @@ def form(request, model):
     """(net, sd, S, n): the network switched to the kernel form under test for the test's duration."""
     S, n, fused = request.param
     net, sd = model
-    net.set_option("fused_tail", fused)
-    yield net, sd, S, n
-    net.set_option("fused_tail", 1)
-
-
-def _clips(n, hops, seed, dev):
-    x, tgt = synth.mixture(n, HOP * hops, seed0=seed)
-    return F.pad(x, (0, LA)).to(dev), tgt
-
-
-def _emb(n, seed, dev):
-    return synth.embedding(n, seed0=seed)[:, 0].to(dev)
-
-
-def _chunk(clip, t):
-    """hop t of one padded clip [2, N]: its 128 samples + the 64 look-ahead samples"""
-    return clip[:, HOP * t:HOP * t + HOP + LA]
-
-
-def _subsets(S, n, hops, seed):
-    """a different unsorted list of n distinct slots for every hop"""
-    g = torch.Generator().manual_seed(seed)
-    return [torch.randperm(S, generator=g)[:n].tolist() for _ in range(hops)]
-
-
-def _bits(t):
-    """a float tensor as its bit patterns: records hold NaN (the embedding of a fresh stream), which torch.equal rejects"""
-    return t.contiguous().view(torch.int32)
-
-
-def _records(st):
-    """every record of the state as bits, the gate memo's weight generation word cleared: copy_streams_from invalidates
-    the memo of the records it writes (by design), so the oracle's records carry generation 0 where a slot-list call
-    keeps it."""
-    r = _bits(st._rec()).clone()
-    r[:, st.lay["st_emb"] + 256] = 0
-    return r
-
-
-def _forward_slots(net, st, x, e, slots, y, flags, dev):
-    """l2h_sep_forward_slots on fixed buffers (a service's staging buffers; with L2H_FLAG_GRAPH one cached graph)."""
-    n = x.shape[0]
-    ws, _ = net._workspace(dev, n, 1)
-    _cabi.check(_cabi.lib().l2h_sep_forward_slots(
-        net._engine(), x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], e.data_ptr(), st.buf.data_ptr(), st.batch,
-        slots.data_ptr(), n, y.data_ptr(), y.stride(0), y.stride(1), y.shape[-1], ws.data_ptr(), ws.numel(), flags,
-        torch.cuda.current_stream(dev).cuda_stream))
+    with su.switched(net, {"fused_tail": fused}):
+        yield net, sd, S, n
 
 
 def test_slots_equal_copy_run_copy_back(form, dev):
@@ -91,33 +32,31 @@ def test_slots_equal_copy_run_copy_back(form, dev):
     (untouched) equal the copy / dense predict / copy back oracle bit for bit."""
     net, _, S, n = form
     T = 12
-    clips, _ = _clips(S, T, 2100, dev)
-    e = _emb(S, 2200, dev)
+    clips, _ = su.clips(S, T, 2100, dev)
+    e = su.emb(S, 2200, dev)
     got, ref = net.init_buffers(S, dev), net.init_buffers(S, dev)
     dense = net.init_buffers(n, dev)
     fed = [0] * S
     with torch.no_grad():
-        for t, sl in enumerate(_subsets(S, n, T, 2300)):
-            x = torch.stack([_chunk(clips[s], fed[s]) for s in sl])
+        for t, sl in enumerate(su.subsets(S, n, T, 2300)):
+            x = torch.stack([su.chunk(clips[s], fed[s]) for s in sl])
             before = got._rec().clone()
             y, _ = net.predict(x, e[sl], got, pad=False, slots=sl)
-            dense.copy_streams_from(ref, sl, list(range(n)))
-            y_ref, _ = net.predict(x, e[sl], dense, pad=False)
-            ref.copy_streams_from(dense, list(range(n)), sl)
+            y_ref = su.oracle(net, ref, sl, x, e[sl], dense)
             for s in sl:
                 fed[s] += 1
             assert torch.equal(y, y_ref), f"hop {t}: y"
             unlisted = [s for s in range(S) if s not in sl]
-            assert torch.equal(_bits(got._rec()[unlisted]), _bits(before[unlisted])), f"hop {t}: an unlisted record changed"
-            assert torch.equal(_records(got), _records(ref)), f"hop {t}: records"
+            assert torch.equal(su.bits(got._rec()[unlisted]), su.bits(before[unlisted])), f"hop {t}: an unlisted record changed"
+            assert torch.equal(su.records(got), su.records(ref)), f"hop {t}: records"
     assert got.stream_pos() == fed and got.header() == (T, T)
 
 
 def test_identity_list_equals_dense_predict(form, dev):
     """slots = 0 .. n-1 (as a CUDA int32 tensor, used in place) over a state of n records is a plain predict."""
     net, _, _, n = form
-    clips, _ = _clips(n, 3, 2400, dev)
-    e = _emb(n, 2500, dev)
+    clips, _ = su.clips(n, 3, 2400, dev)
+    e = su.emb(n, 2500, dev)
     a, b = net.init_buffers(n, dev), net.init_buffers(n, dev)
     ident = torch.arange(n, dtype=torch.int32, device=dev)
     with torch.no_grad():
@@ -126,28 +65,28 @@ def test_identity_list_equals_dense_predict(form, dev):
             ya, _ = net.predict(x, e, a, pad=False, slots=ident)
             yb, _ = net.predict(x, e, b, pad=False)
             assert torch.equal(ya, yb), t
-    assert torch.equal(_bits(a.buf), _bits(b.buf))
+    assert torch.equal(su.bits(a.buf), su.bits(b.buf))
 
 
 def test_entries_outside_the_state_store_nothing(form, dev):
     """Rows whose entry lies outside [0, S) are computed but leave every record and their NaN-filled y row untouched; the
     other rows equal the same call with those entries pointing at spare records of a copy of the state."""
     net, _, S, n = form
-    clips, _ = _clips(S, 4, 2600, dev)
-    e = _emb(S, 2700, dev)
+    clips, _ = su.clips(S, 4, 2600, dev)
+    e = su.emb(S, 2700, dev)
     st = net.init_buffers(S, dev)
-    warm = _subsets(S, n, 3, 2800)
+    warm = su.subsets(S, n, 3, 2800)
     with torch.no_grad():
         for t, sl in enumerate(warm):        # records with history and different clocks
-            net.predict(torch.stack([_chunk(clips[s], t) for s in sl]), e[sl], st, pad=False, slots=sl)
-    sl = _subsets(S, n, 1, 2900)[0]
+            net.predict(torch.stack([su.chunk(clips[s], t) for s in sl]), e[sl], st, pad=False, slots=sl)
+    sl = su.subsets(S, n, 1, 2900)[0]
     bad = {0: -1, n - 1: S + 3} if n > 2 else {0: -1}
     spare = [s for s in range(S) if s not in sl][:len(bad)]
     with_bad = [bad.get(i, s) for i, s in enumerate(sl)]
     with_spare = list(with_bad)
     for i, sp in zip(bad, spare):
         with_spare[i] = sp
-    x = torch.stack([_chunk(clips[s], 3) for s in sl])
+    x = torch.stack([su.chunk(clips[s], 3) for s in sl])
     ee = e[sl].contiguous()
     net._sync_weights(dev)
     twin = net.init_buffers(S, dev)
@@ -155,8 +94,8 @@ def test_entries_outside_the_state_store_nothing(form, dev):
     before = st._rec().clone()
     y = torch.full((n, 2, HOP), float("nan"), device=dev)
     y_twin = torch.full_like(y, float("nan"))
-    _forward_slots(net, st, x, ee, torch.tensor(with_bad, dtype=torch.int32, device=dev), y, 0, dev)
-    _forward_slots(net, twin, x, ee, torch.tensor(with_spare, dtype=torch.int32, device=dev), y_twin, 0, dev)
+    net._launch("slots", x, ee, st, y, 1, slots=torch.tensor(with_bad, dtype=torch.int32, device=dev))
+    net._launch("slots", x, ee, twin, y_twin, 1, slots=torch.tensor(with_spare, dtype=torch.int32, device=dev))
     torch.cuda.synchronize()
     stored = [s for s in with_bad if 0 <= s < S]
     for i in range(n):
@@ -166,8 +105,8 @@ def test_entries_outside_the_state_store_nothing(form, dev):
             assert torch.equal(y[i], y_twin[i]), f"row {i}"
             assert not bool(torch.isnan(y[i]).any())
     others = [s for s in range(S) if s not in stored]
-    assert torch.equal(_bits(st._rec()[others]), _bits(before[others])), "a record not listed (or listed out of range) changed"
-    assert torch.equal(_bits(st._rec()[stored]), _bits(twin._rec()[stored]))
+    assert torch.equal(su.bits(st._rec()[others]), su.bits(before[others])), "a record not listed (or listed out of range) changed"
+    assert torch.equal(su.bits(st._rec()[stored]), su.bits(twin._rec()[stored]))
     assert [st.stream_pos()[s] for s in spare] == [twin.stream_pos()[s] - 1 for s in spare]
 
 
@@ -176,24 +115,24 @@ def test_graph_replay_with_list_rewritten_in_place(form, dev):
     is replayed: y and the whole state equal direct calls."""
     net, _, S, n = form
     T = 6
-    clips, _ = _clips(S, T, 3000, dev)
-    e = _emb(S, 3100, dev)
+    clips, _ = su.clips(S, T, 3000, dev)
+    e = su.emb(S, 3100, dev)
     net._sync_weights(dev)
     xbuf, ebuf = torch.empty(n, 2, HOP + LA, device=dev), torch.empty(n, 256, device=dev)
     slots = torch.empty(n, dtype=torch.int32, device=dev)
     yg, yd = torch.empty(n, 2, HOP, device=dev), torch.empty(n, 2, HOP, device=dev)
     sg, sdir = net.init_buffers(S, dev), net.init_buffers(S, dev)
     fed = [0] * S
-    for t, sl in enumerate(_subsets(S, n, T, 3200)):
-        xbuf.copy_(torch.stack([_chunk(clips[s], fed[s]) for s in sl]))
+    for t, sl in enumerate(su.subsets(S, n, T, 3200)):
+        xbuf.copy_(torch.stack([su.chunk(clips[s], fed[s]) for s in sl]))
         ebuf.copy_(e[sl])
         slots.copy_(torch.tensor(sl, dtype=torch.int32))
-        _forward_slots(net, sg, xbuf, ebuf, slots, yg, L2H_FLAG_GRAPH, dev)
-        _forward_slots(net, sdir, xbuf, ebuf, slots, yd, 0, dev)
+        net._launch("slots", xbuf, ebuf, sg, yg, 1, L2H_FLAG_GRAPH, slots=slots)
+        net._launch("slots", xbuf, ebuf, sdir, yd, 1, slots=slots)
         for s in sl:
             fed[s] += 1
         assert torch.equal(yg, yd), t
-    assert torch.equal(_bits(sg.buf), _bits(sdir.buf))
+    assert torch.equal(su.bits(sg.buf), su.bits(sdir.buf))
 
 
 def test_listed_stream_vs_oracle(form, dev):
@@ -205,15 +144,15 @@ def test_listed_stream_vs_oracle(form, dev):
     n_fed = T - len(skipped)
     x_cpu, tgt = synth.mixture(1, HOP * n_fed, seed0=3300)
     xc = F.pad(x_cpu, (0, LA)).to(dev)
-    others, _ = _clips(S, T, 3400, dev)
-    e = _emb(S, 3500, dev)
+    others, _ = su.clips(S, T, 3400, dev)
+    e = su.emb(S, 3500, dev)
     st = net.init_buffers(S, dev)
     got, fed = [], 0
     with torch.no_grad():
-        for t, sl in enumerate(_subsets(S - 1, n, T, 3600)):
+        for t, sl in enumerate(su.subsets(S - 1, n, T, 3600)):
             if t not in skipped:
                 sl[t % n] = s
-            x = torch.stack([_chunk(xc[0], fed) if b == s else _chunk(others[b], t) for b in sl])
+            x = torch.stack([su.chunk(xc[0], fed) if b == s else su.chunk(others[b], t) for b in sl])
             y, _ = net.predict(x, e[sl], st, pad=False, slots=sl)
             if t not in skipped:
                 got.append(y[t % n])

@@ -2,23 +2,13 @@
 Net.advance_slots(hops=)): the argument errors the C call returns before it touches the device, the header's description,
 and the Python ValueErrors for `hops` (no GPU needed; the handle below never commits weights)."""
 import ctypes
-import os
 import re
 
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-FAKE_DEV = ctypes.c_void_p(0x10000)          # never dereferenced: every call below fails its argument checks first
-L2H_FLAG_TAPS = 1
-
-
-@pytest.fixture(scope="module")
-def eng(tsh_params):
-    from lookoncetohear_b200 import Net, build, _cabi
-    build.build()
-    net = Net(**tsh_params)
-    return net, net._engine(), _cabi.lib()
+import serving_util as su
+from serving_util import FAKE_DEV, L2H_FLAG_TAPS, eng  # noqa: F401
 
 
 def _call(L, h, state_batch, slots, hops, n, frames, flags=0, p=FAKE_DEV):
@@ -48,30 +38,27 @@ def test_forward_slots_hops_argument_errors(eng, hops):
 
 
 def test_header_documents_forward_slots_hops():
-    hdr = open(os.path.join(ROOT, "include", "lookonce_b200.h")).read()
-    decl = re.search(r"int l2h_sep_forward_slots_hops\((.*?)\);", hdr, flags=re.S)
+    hdr = su.header()
+    decl, args = su.declaration(hdr, "l2h_sep_forward_slots_hops")
     assert decl, "l2h_sep_forward_slots_hops is not declared"
-    args = [a.split()[-1].lstrip("*") for a in " ".join(decl.group(1).split()).split(",")]
     assert args == ["handle", "x_dev", "x_batch_stride", "x_ch_stride", "x_len", "emb_dev", "state_dev", "state_batch",
                     "slots_dev", "hops_dev", "n", "frames", "y_dev", "y_batch_stride", "y_ch_stride", "y_len",
                     "workspace_dev", "workspace_bytes", "flags", "stream"]
     prev = re.search(r"int l2h_sep_forward_slots_frames\(", hdr)
     assert prev and prev.start() < decl.start(), "declared after l2h_sep_forward_slots_frames"
-    doc = " ".join(re.sub(r"\n\s*\*", " ", hdr[:decl.start()].rsplit("/*", 1)[1]).split())
+    doc = su.doc_before(hdr, decl.start())
     for phrase in ("hops_dev", "[0, frames]", "128*h + 64", "L2H_FLAG_GRAPH", "NULL", "128*h - 1", "h = 0 stores nothing",
                    "l2h_sep_forward_slots_frames"):
         assert phrase in doc, phrase
     # the multi-hop call's description points at the ragged call for listeners with different backlogs
-    frames_doc = " ".join(re.sub(r"\n\s*\*", " ", hdr[:prev.start()].rsplit("/*", 1)[1]).split())
+    frames_doc = su.doc_before(hdr, prev.start())
     assert "l2h_sep_forward_slots_hops" in frames_doc
     assert "#define L2H_ABI_VERSION 1" in hdr
 
 
 def test_python_hops_raise_value_error(eng):
     net, _, _ = eng
-    from lookoncetohear_b200.net import SepState
-    hb, stride, offs = net._state_layout()
-    st = SepState(torch.zeros(hb // 4 + 4 * stride), 4, 3, hb, stride, offs)
+    st = su.host_state(net, 4)
     emb = torch.zeros(2, 256)
     x = torch.zeros(2, 2, 128 * 3 + 64)                               # T = 3
     for bad in ([1], [1, 2, 3], [], [[1, 2]], [0, 4], [-1, 2], [3, 7], [1.0, 2.0], [True, False],

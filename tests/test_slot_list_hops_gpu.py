@@ -10,14 +10,13 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from lookoncetohear_b200 import Net, synth, _cabi
+from lookoncetohear_b200 import synth
 from oracle import restate as rs
 from kernels import harness as kh
+import serving_util as su
+from serving_util import HOP, LA, L2H_FLAG_GRAPH, SENTINEL, dev, model  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-HOP, LA = 128, 64
-L2H_FLAG_GRAPH = 2
-SENTINEL = float("nan")
 FORMS = [pytest.param((12, 2, 3, {"back_many": 1}), id="n2-T3"),
          pytest.param((12, 2, 3, {"back_many": 0}), id="n2-T3-per-frame"),
          pytest.param((12, 4, 5, {"back_many": 1}), id="n4-T5"),
@@ -25,157 +24,50 @@ FORMS = [pytest.param((12, 2, 3, {"back_many": 1}), id="n2-T3"),
          pytest.param((16, 8, 3, {}), id="n8-T3-tc"),
          pytest.param((56, 48, 2, {}), id="n48-T2-tc-lstm"),
          pytest.param((56, 48, 2, {"fuse_ih": 1}), id="n48-T2-tc-lstm-x")]
-DEFAULTS = {"back_many": 1, "fuse_ih": 0}
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda", 0)
-
-
-@pytest.fixture(scope="module")
-def model(tsh_params, dev):
-    torch.manual_seed(0)
-    net = Net(**tsh_params).eval()
-    sd = {k: v.detach().clone() for k, v in net.state_dict().items()}
-    net = net.to(dev)
-    net._sync_weights(dev)
-    return net, sd
-
-
-def _switched(net, opts):
-    for k, v in opts.items():
-        net.set_option(k, v)
 
 
 @pytest.fixture(params=FORMS)
 def form(request, model):
     S, n, T, opts = request.param
     net, sd = model
-    _switched(net, opts)
-    yield net, sd, S, n, T
-    _switched(net, {k: DEFAULTS[k] for k in opts})
-
-
-def _clips(n, hops, seed, dev):
-    x, tgt = synth.mixture(n, HOP * hops, seed0=seed)
-    return F.pad(x, (0, LA)).to(dev), tgt
-
-
-def _emb(n, seed, dev):
-    return synth.embedding(n, seed0=seed)[:, 0].to(dev)
-
-
-def _chunk(clip, t, T):
-    return clip[:, HOP * t:HOP * (t + T) + LA]
-
-
-def _subsets(S, n, calls, seed):
-    g = torch.Generator().manual_seed(seed)
-    return [torch.randperm(S, generator=g)[:n].tolist() for _ in range(calls)]
-
-
-def _hops(n, T, seed):
-    """n hop counts in [0, T] that include 0, 1 and T (n >= 3), else 1 and T"""
-    g = torch.Generator().manual_seed(seed)
-    h = torch.randint(0, T + 1, (n,), generator=g)
-    fixed = [0, 1, T] if n >= 3 else [1, T]
-    h[torch.randperm(n, generator=g)[:len(fixed)]] = torch.tensor(fixed)
-    return h.tolist()
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def _warm_state(net, S, n, T, seed, dev):
-    """a state whose records have history and different clocks"""
-    clips, _ = _clips(S, 3 * T, seed, dev)
-    e = _emb(S, seed + 1, dev)
-    st = net.init_buffers(S, dev)
-    with torch.no_grad():
-        for c, sl in enumerate(_subsets(S, n, 3, seed + 2)):
-            net.advance_slots(torch.stack([_chunk(clips[s], c * T, T) for s in sl]), e[sl], st, sl)
-    return st
-
-
-def _copy(net, st, dev):
-    twin = net.init_buffers(st.batch, dev)
-    twin.buf.copy_(st.buf)
-    return twin
-
-
-def _forward(net, st, x, e, slots, hops, y, T, flags, dev):
-    """l2h_sep_forward_slots_hops on fixed buffers (hops None: l2h_sep_forward_slots_frames)"""
-    n = x.shape[0]
-    ws, _ = net._workspace(dev, n, T)
-    L = _cabi.lib()
-    args = [net._engine(), x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], e.data_ptr(), st.buf.data_ptr(), st.batch,
-            slots.data_ptr()]
-    rest = [y.data_ptr(), y.stride(0), y.stride(1), y.shape[-1], ws.data_ptr(), ws.numel(), flags,
-            torch.cuda.current_stream(dev).cuda_stream]
-    if hops is None:
-        _cabi.check(L.l2h_sep_forward_slots_frames(*args, n, T, *rest))
-    else:
-        _cabi.check(L.l2h_sep_forward_slots_hops(*args, hops.data_ptr(), n, T, *rest))
-
-
-def _ring_mask(st, s, frames):
-    """bool [stride]: the ring rows of record s holding the given frames (every block, head, K and V)"""
-    L = st.lay
-    m = torch.zeros(st.stride, dtype=torch.bool, device=st.buf.device)
-    for blk in range(st.n_blocks):
-        base = L["st_blk"] + blk * L["bk_stride"]
-        for h in range(4):
-            for f in frames:
-                slot = f % L["ring"]
-                k0 = base + L["bk_k"] + (h * L["ring"] + slot) * L["k_ld"]
-                v0 = base + L["bk_v"] + (h * L["ring"] + slot) * L["v_dim"]
-                m[k0:k0 + L["k_ld"]] = True
-                m[v0:v0 + L["v_dim"]] = True
-    return m
-
-
-def _ring_all(st):
-    L = st.lay
-    return _ring_mask(st, 0, range(L["ring"]))
+    with su.switched(net, opts):
+        yield net, sd, S, n, T
 
 
 # ---- all hops = T: the ragged call is l2h_sep_forward_slots_frames --------------------------------------------------
 def test_all_hops_T_equal_slots_frames(form, dev):
     net, _, S, n, T = form
-    st = _warm_state(net, S, n, T, 6100, dev)
-    twin = _copy(net, st, dev)
-    clips, _ = _clips(n, T, 6200, dev)
+    st = su.warm_slots(net, S, n, T, 6100, dev)
+    twin = su.copy(net, st)
+    clips, _ = su.clips(n, T, 6200, dev)
     x = clips.contiguous()
-    e = _emb(n, 6300, dev)
-    sl = torch.tensor(_subsets(S, n, 1, 6400)[0], dtype=torch.int32, device=dev)
+    e = su.emb(n, 6300, dev)
+    sl = torch.tensor(su.subsets(S, n, 1, 6400)[0], dtype=torch.int32, device=dev)
     y = torch.full((n, 2, HOP * T), SENTINEL, device=dev)
     y_ref = torch.full_like(y, SENTINEL)
-    _forward(net, st, x, e, sl, torch.full((n,), T, dtype=torch.int32, device=dev), y, T, 0, dev)
-    _forward(net, twin, x, e, sl, None, y_ref, T, 0, dev)
+    net._launch("slots_hops", x, e, st, y, T, slots=sl, hops=torch.full((n,), T, dtype=torch.int32, device=dev))
+    net._launch("slots_frames", x, e, twin, y_ref, T, slots=sl)
     torch.cuda.synchronize()
-    assert torch.equal(_bits(y), _bits(y_ref))
-    assert torch.equal(_bits(st.buf), _bits(twin.buf))
+    assert torch.equal(su.bits(y), su.bits(y_ref))
+    assert torch.equal(su.bits(st.buf), su.bits(twin.buf))
 
 
 # ---- all hops 0, and slots out of range: nothing stored --------------------------------------------------------------
 def test_zero_hops_and_outside_slots_store_nothing(form, dev):
     net, _, S, n, T = form
-    st = _warm_state(net, S, n, T, 6500, dev)
-    before = _bits(st._rec()).clone()
-    clips, _ = _clips(n, T, 6600, dev)
-    e = _emb(n, 6700, dev)
-    sl = _subsets(S, n, 1, 6800)[0]
+    st = su.warm_slots(net, S, n, T, 6500, dev)
+    before = su.bits(st._rec()).clone()
+    clips, _ = su.clips(n, T, 6600, dev)
+    e = su.emb(n, 6700, dev)
+    sl = su.subsets(S, n, 1, 6800)[0]
     for slots, hops in ((sl, [0] * n), ([-1 - i if i % 2 else S + i for i in range(n)], [T] * n),
                         (sl, [T + 1 + i if i % 2 else -1 - i for i in range(n)])):      # counts outside [0, T] count as 0
         y = torch.full((n, 2, HOP * T), SENTINEL, device=dev)
-        _forward(net, st, clips.contiguous(), e, torch.tensor(slots, dtype=torch.int32, device=dev),
-                 torch.tensor(hops, dtype=torch.int32, device=dev), y, T, 0, dev)
+        net._launch("slots_hops", clips.contiguous(), e, st, y, T, slots=torch.tensor(slots, dtype=torch.int32, device=dev),
+                    hops=torch.tensor(hops, dtype=torch.int32, device=dev))
         torch.cuda.synchronize()
         assert bool(torch.isnan(y).all()), "a y row was written"
-        assert torch.equal(_bits(st._rec()), before), "a record changed"
+        assert torch.equal(su.bits(st._rec()), before), "a record changed"
 
 
 # ---- mixed hops against a uniform T-hop call on a copy ---------------------------------------------------------------
@@ -184,37 +76,37 @@ def test_mixed_hops_match_uniform_call_where_they_advance(form, dev):
     uniform T-hop call on a copy bit for bit; later y samples keep the sentinel; other ring rows, and unlisted records,
     are as before; clocks advance by h_i (calls by 1 if h_i > 0)."""
     net, _, S, n, T = form
-    st = _warm_state(net, S, n, T, 6900, dev)
-    twin = _copy(net, st, dev)
+    st = su.warm_slots(net, S, n, T, 6900, dev)
+    twin = su.copy(net, st)
     before = st._rec().clone()
     pos0 = st.stream_pos()
     calls0 = st._clocks()[1].cpu().tolist()
-    clips, _ = _clips(n, T, 7000, dev)
+    clips, _ = su.clips(n, T, 7000, dev)
     x = clips.contiguous().clone()
-    hops = _hops(n, T, 7100)
+    hops = su.hop_mix(n, T, 7100)
     for i, h in enumerate(hops):
         x[i, :, HOP * h + LA:] = float("nan")
-    e = _emb(n, 7200, dev)
-    sl = _subsets(S, n, 1, 7300)[0]
+    e = su.emb(n, 7200, dev)
+    sl = su.subsets(S, n, 1, 7300)[0]
     slots = torch.tensor(sl, dtype=torch.int32, device=dev)
     y = torch.full((n, 2, HOP * T), SENTINEL, device=dev)
     y_ref = torch.full_like(y, SENTINEL)
-    _forward(net, st, x, e, slots, torch.tensor(hops, dtype=torch.int32, device=dev), y, T, 0, dev)
-    _forward(net, twin, clips.contiguous(), e, slots, None, y_ref, T, 0, dev)
+    net._launch("slots_hops", x, e, st, y, T, slots=slots, hops=torch.tensor(hops, dtype=torch.int32, device=dev))
+    net._launch("slots_frames", clips.contiguous(), e, twin, y_ref, T, slots=slots)
     torch.cuda.synchronize()
     for i, (s, h) in enumerate(zip(sl, hops)):
-        assert torch.equal(_bits(y[i, :, :HOP * h]), _bits(y_ref[i, :, :HOP * h])), (i, h)
+        assert torch.equal(su.bits(y[i, :, :HOP * h]), su.bits(y_ref[i, :, :HOP * h])), (i, h)
         assert bool(torch.isnan(y[i, :, HOP * h:]).all()), (i, h, "y written past the row's hops")
-        new = _ring_mask(st, s, range(pos0[s], pos0[s] + h))
-        assert torch.equal(_bits(st._rec()[s][new]), _bits(twin._rec()[s][new])), (i, h, "ring rows of the new frames")
-        other = _ring_all(st) & ~new
-        assert torch.equal(_bits(st._rec()[s][other]), _bits(before[s][other])), (i, h, "another ring row changed")
+        new = su.ring_mask(st, range(pos0[s], pos0[s] + h))
+        assert torch.equal(su.bits(st._rec()[s][new]), su.bits(twin._rec()[s][new])), (i, h, "ring rows of the new frames")
+        other = su.ring_all(st) & ~new
+        assert torch.equal(su.bits(st._rec()[s][other]), su.bits(before[s][other])), (i, h, "another ring row changed")
         if h == 0:
-            assert torch.equal(_bits(st._rec()[s]), _bits(before[s])), (i, "h = 0 stored something")
+            assert torch.equal(su.bits(st._rec()[s]), su.bits(before[s])), (i, "h = 0 stored something")
         if h == T:
-            assert torch.equal(_bits(st._rec()[s]), _bits(twin._rec()[s])), (i, "h = T")
+            assert torch.equal(su.bits(st._rec()[s]), su.bits(twin._rec()[s])), (i, "h = T")
     unlisted = [s for s in range(S) if s not in sl]
-    assert torch.equal(_bits(st._rec()[unlisted]), _bits(before[unlisted]))
+    assert torch.equal(su.bits(st._rec()[unlisted]), su.bits(before[unlisted]))
     pos, calls = st.stream_pos(), st._clocks()[1].cpu().tolist()
     for s, h in zip(sl, hops):
         assert pos[s] == pos0[s] + h and calls[s] == calls0[s] + (1 if h > 0 else 0), (s, h)
@@ -230,7 +122,7 @@ def _state_parts(st, s):
     """the parts of record s a call stores, as float tensors: rings, (h, c) of every block, the current tails"""
     L, r = st.lay, st._rec()[s]
     par = int(st._clocks()[1][s]) & 1
-    parts = {"ring": r[_ring_all(st)]}
+    parts = {"ring": r[su.ring_all(st)]}
     for blk in range(st.n_blocks):
         base = L["st_blk"] + blk * L["bk_stride"]
         parts[f"h{blk}"] = r[base + L["bk_h"]:base + L["bk_h"] + 97 * 64]
@@ -249,24 +141,24 @@ def test_mixed_hops_match_per_depth_recipe(form, dev, record_property):
     other the fp32 CUDA-core one; then 10 one-hop predict(slots=) calls on both, with y within the same bound.  Which
     depths came out bit-identical is recorded as the test's `bit_identical_by_depth` property."""
     net, _, S, n, T = form
-    st = _warm_state(net, S, n, T, 7400, dev)
-    ref = _copy(net, st, dev)
-    clips, _ = _clips(S, T + 70, 7500, dev)
-    e = _emb(S, 7600, dev)
-    sl = _subsets(S, n, 1, 7700)[0]
-    hops = _hops(n, T, 7800)
+    st = su.warm_slots(net, S, n, T, 7400, dev)
+    ref = su.copy(net, st)
+    clips, _ = su.clips(S, T + 70, 7500, dev)
+    e = su.emb(S, 7600, dev)
+    sl = su.subsets(S, n, 1, 7700)[0]
+    hops = su.hop_mix(n, T, 7800)
     pos0 = st.stream_pos()
     tc = lambda rows, hops_: rows * hops_ * 97 > 2048          # the engine's tensor-core threshold (TC_MIN_ROWS)
     bound = 1e-5 if all(tc(hops.count(h), h) == tc(n, T) for h in set(hops) - {0}) else 5e-5
     with torch.no_grad():
-        x = torch.stack([_chunk(clips[s], 0, T) for s in sl])
+        x = torch.stack([su.chunk(clips[s], 0, T) for s in sl])
         y = net.advance_slots(x, e[sl], st, sl, hops=hops)
         for h in sorted(set(hops) - {0}):
             rows = [i for i in range(n) if hops[i] == h]
             ss = [sl[i] for i in rows]
             tmp = net.init_buffers(len(ss), dev)
             tmp.copy_streams_from(ref, ss, list(range(len(ss))))
-            y_h = net.advance_slots(torch.stack([_chunk(clips[s], 0, h) for s in ss]), e[ss], tmp, list(range(len(ss))))
+            y_h = net.advance_slots(torch.stack([su.chunk(clips[s], 0, h) for s in ss]), e[ss], tmp, list(range(len(ss))))
             ref.copy_streams_from(tmp, list(range(len(ss))), ss)
             for j, i in enumerate(rows):
                 assert _rel(y[i, :, :HOP * h], y_h[j]) <= bound, (i, h)
@@ -276,7 +168,7 @@ def test_mixed_hops_match_per_depth_recipe(form, dev, record_property):
     for s, h in zip(sl, hops):
         a, b = _state_parts(st, s), _state_parts(ref, s)
         for k in a:
-            same = torch.equal(_bits(a[k]), _bits(b[k]))
+            same = torch.equal(su.bits(a[k]), su.bits(b[k]))
             exact[f"h{h}"] = exact.get(f"h{h}", True) and same
             if not same:
                 worst[k] = max(worst.get(k, 0.0), _rel(a[k], b[k]))
@@ -286,7 +178,7 @@ def test_mixed_hops_match_per_depth_recipe(form, dev, record_property):
     fed = {s: h for s, h in zip(sl, hops)}
     with torch.no_grad():
         for k in range(10):                 # (records near the ring's wrap: test_recipe_calls_cross_the_ring)
-            xs = torch.stack([_chunk(clips[s], fed[s] + k, 1) for s in sl])
+            xs = torch.stack([su.chunk(clips[s], fed[s] + k, 1) for s in sl])
             ya, _ = net.predict(xs, e[sl], st, pad=False, slots=sl)
             yb, _ = net.predict(xs, e[sl], ref, pad=False, slots=sl)
             assert _rel(ya, yb) <= bound, k
@@ -298,29 +190,29 @@ def test_recipe_calls_cross_the_ring(model, dev):
     per-depth recipe, y within 1e-5 on every call and the clocks exact."""
     net, _ = model
     S, n, T = 10, 4, 5
-    clips, _ = _clips(S, 120, 7900, dev)
-    e = _emb(S, 8000, dev)
+    clips, _ = su.clips(S, 120, 7900, dev)
+    e = su.emb(S, 8000, dev)
     st = net.init_buffers(S, dev)
     fed = (50 + torch.arange(S) % 4).tolist()
     with torch.no_grad():
         for s in range(S):
             one = net.init_buffers(1, dev)
-            net.predict(_chunk(clips[s], 0, fed[s])[None], e[s:s + 1], one, pad=False)
+            net.predict(su.chunk(clips[s], 0, fed[s])[None], e[s:s + 1], one, pad=False)
             st.copy_streams_from(one, [0], [s])
-        ref = _copy(net, st, dev)
+        ref = su.copy(net, st)
         sl = [1, 4, 6, 9]
         hops = [0, 1, 5, 3]
-        y = net.advance_slots(torch.stack([_chunk(clips[s], fed[s], T) for s in sl]), e[sl], st, sl, hops=hops)
+        y = net.advance_slots(torch.stack([su.chunk(clips[s], fed[s], T) for s in sl]), e[sl], st, sl, hops=hops)
         for h in (1, 3, 5):
             ss = [s for s, hh in zip(sl, hops) if hh == h]
-            yy = net.advance_slots(torch.stack([_chunk(clips[s], fed[s], h) for s in ss]), e[ss], ref, ss)
+            yy = net.advance_slots(torch.stack([su.chunk(clips[s], fed[s], h) for s in ss]), e[ss], ref, ss)
             i = hops.index(h)
             assert _rel(y[i, :, :HOP * h], yy[0]) <= 1e-5, h
         for s, h in zip(sl, hops):
             fed[s] += h
         assert st.stream_pos() == ref.stream_pos() == fed
         for k in range(10):
-            xs = torch.stack([_chunk(clips[s], fed[s] + k, 1) for s in sl])
+            xs = torch.stack([su.chunk(clips[s], fed[s] + k, 1) for s in sl])
             ya, _ = net.predict(xs, e[sl], st, pad=False, slots=sl)
             yb, _ = net.predict(xs, e[sl], ref, pad=False, slots=sl)
             assert _rel(ya, yb) <= 1e-5, k
@@ -367,11 +259,11 @@ def test_masked_inter_steps_carry_c(variant, passes, dev):
     assert bool(torch.isfinite(out).all()) and bool(torch.isfinite(c).all())
     for b, tb in enumerate(Tbs):
         if tb == 0:
-            assert torch.equal(_bits(c[b]), _bits(c0[b])), (b, "c moved through masked steps only")
+            assert torch.equal(su.bits(c[b]), su.bits(c0[b])), (b, "c moved through masked steps only")
             continue
         o1, _, c1 = run(gx[b:b + 1], tb, slice(b, b + 1))
-        assert torch.equal(_bits(out[b, :tb]), _bits(o1[0, :tb])), (b, variant, passes)
-        assert torch.equal(_bits(c[b]), _bits(c1[0])), (b, variant, passes, "final c")
+        assert torch.equal(su.bits(out[b, :tb]), su.bits(o1[0, :tb])), (b, variant, passes)
+        assert torch.equal(su.bits(c[b]), su.bits(c1[0])), (b, variant, passes, "final c")
 
 
 # ---- one stream against the reference ---------------------------------------------------------------------------------
@@ -385,17 +277,17 @@ def test_ragged_stream_vs_oracle(model, dev, S, n):
     n_fed = sum(h for _, h in plan)
     x_cpu, tgt = synth.mixture(1, HOP * n_fed, seed0=8200)
     xc = F.pad(F.pad(x_cpu, (0, LA)), (0, HOP * 5), value=float("nan")).to(dev)     # never read past its own hops
-    others, _ = _clips(S, 5 * len(plan), 8300, dev)
-    e = _emb(S, 8400, dev)
+    others, _ = su.clips(S, 5 * len(plan), 8300, dev)
+    e = su.emb(S, 8400, dev)
     st = net.init_buffers(S, dev)
     fed_o = [0] * S
     got, fed = [], 0
     with torch.no_grad():
-        for c, ((T, h), sl) in enumerate(zip(plan, _subsets(S - 1, n, len(plan), 8500))):
+        for c, ((T, h), sl) in enumerate(zip(plan, su.subsets(S - 1, n, len(plan), 8500))):
             sl[c % n] = s
-            hops = _hops(n, T, 8600 + c)
+            hops = su.hop_mix(n, T, 8600 + c)
             hops[c % n] = h
-            x = torch.stack([_chunk(xc[0], fed, T) if b == s else _chunk(others[b], fed_o[b], T) for b in sl])
+            x = torch.stack([su.chunk(xc[0], fed, T) if b == s else su.chunk(others[b], fed_o[b], T) for b in sl])
             y = net.advance_slots(x, e[sl], st, sl, hops=hops)
             got.append(y[c % n, :, :HOP * h])
             fed += h
@@ -423,8 +315,8 @@ def test_graph_replay_with_slots_and_hops_rewritten(form, dev):
     captures (capture + instantiation costs milliseconds of host time, a replay tens of microseconds)."""
     net, _, S, n, T = form
     calls = 5
-    clips, _ = _clips(S, calls * T, 8700, dev)
-    e = _emb(S, 8800, dev)
+    clips, _ = su.clips(S, calls * T, 8700, dev)
+    e = su.emb(S, 8800, dev)
     xbuf, ebuf = torch.empty(n, 2, HOP * T + LA, device=dev), torch.empty(n, 256, device=dev)
     slots = torch.empty(n, dtype=torch.int32, device=dev)
     hops = torch.empty(n, dtype=torch.int32, device=dev)
@@ -432,9 +324,9 @@ def test_graph_replay_with_slots_and_hops_rewritten(form, dev):
     sg, sdir = net.init_buffers(S, dev), net.init_buffers(S, dev)
     fed = [0] * S
     host = []
-    for c, sl in enumerate(_subsets(S, n, calls, 8900)):
-        hh = _hops(n, T, 9000 + c)
-        xbuf.copy_(torch.stack([_chunk(clips[s], fed[s], T) for s in sl]))
+    for c, sl in enumerate(su.subsets(S, n, calls, 8900)):
+        hh = su.hop_mix(n, T, 9000 + c)
+        xbuf.copy_(torch.stack([su.chunk(clips[s], fed[s], T) for s in sl]))
         ebuf.copy_(e[sl])
         slots.copy_(torch.tensor(sl, dtype=torch.int32))
         hops.copy_(torch.tensor(hh, dtype=torch.int32))
@@ -442,13 +334,13 @@ def test_graph_replay_with_slots_and_hops_rewritten(form, dev):
         yd.fill_(SENTINEL)
         torch.cuda.synchronize()
         t0 = time.perf_counter()
-        _forward(net, sg, xbuf, ebuf, slots, hops, yg, T, L2H_FLAG_GRAPH, dev)
+        net._launch("slots_hops", xbuf, ebuf, sg, yg, T, L2H_FLAG_GRAPH, slots=slots, hops=hops)
         host.append(time.perf_counter() - t0)
-        _forward(net, sdir, xbuf, ebuf, slots, hops, yd, T, 0, dev)
+        net._launch("slots_hops", xbuf, ebuf, sdir, yd, T, slots=slots, hops=hops)
         for s, h in zip(sl, hh):
             fed[s] += h
         torch.cuda.synchronize()
-        assert torch.equal(_bits(yg), _bits(yd)), c
-    assert torch.equal(_bits(sg.buf), _bits(sdir.buf))
+        assert torch.equal(su.bits(yg), su.bits(yd)), c
+    assert torch.equal(su.bits(sg.buf), su.bits(sdir.buf))
     assert sg.stream_pos() == fed
     assert max(host[1:]) < 0.5 * host[0], ("a replay took as long as a capture: new graph per hop mix?", host)

@@ -5,15 +5,8 @@ import ctypes
 import pytest
 import torch
 
-FAKE_DEV = ctypes.c_void_p(0x10000)          # never dereferenced: every call below fails its argument checks first
-
-
-@pytest.fixture(scope="module")
-def eng(tsh_params):
-    from lookoncetohear_b200 import Net, build, _cabi
-    build.build()
-    net = Net(**tsh_params)
-    return net, net._engine(), _cabi.lib()
+import serving_util as su
+from serving_util import FAKE_DEV, eng  # noqa: F401
 
 
 def _slots(*s):
@@ -38,9 +31,7 @@ def test_offsets_query_keeps_the_first_16_and_adds_the_clock(eng):
 
 def test_sepstate_layout_names_the_clock(eng):
     net, _, _ = eng
-    from lookoncetohear_b200.net import SepState
-    hb, stride, offs = net._state_layout()
-    st = SepState(torch.zeros(hb // 4 + 3 * stride), 3, 3, hb, stride, offs)
+    st = su.host_state(net, 3)
     pos, calls = st._clocks()
     pos.copy_(torch.tensor([5, 0, 1 << 40]))
     calls.copy_(torch.tensor([3, 0, 8], dtype=torch.int32))
@@ -88,9 +79,7 @@ def test_forward_active_argument_errors(eng):
 
 def test_python_arguments_raise_value_error(eng):
     net, _, _ = eng
-    from lookoncetohear_b200.net import SepState
-    hb, stride, offs = net._state_layout()
-    st = SepState(torch.zeros(hb // 4 + 2 * stride), 2, 3, hb, stride, offs)
+    st = su.host_state(net, 2)
     with pytest.raises(ValueError):
         st.reset_streams([0])                   # no engine behind a hand-made state
     st._net = net

@@ -2,32 +2,17 @@
 (predict(..., active=) / l2h_sep_forward_active) and moved between states (copy_streams_from).  The oracle of each
 behaviour is bit-exact: the same stream run on its own in a state of the same batch size, where the kernel forms are the
 same (B = 2: the fused one-hop tail; B = 2 with fused_tail = 0: the separate kernels; B = 32: the tensor-core chain)."""
-import ctypes
-
 import pytest
 import torch
 import torch.nn.functional as F
 
-from lookoncetohear_b200 import Net, synth, _cabi
+from lookoncetohear_b200 import synth
 from oracle import restate as rs
+import serving_util as su
+from serving_util import HOP, LA, dev, model  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-HOP, LA = 128, 64
 FORMS = [pytest.param((2, 1), id="B2-fused"), pytest.param((2, 0), id="B2-separate"), pytest.param((32, 1), id="B32-tc")]
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda", 0)
-
-
-@pytest.fixture(scope="module")
-def model(tsh_params, dev):
-    torch.manual_seed(0)
-    net = Net(**tsh_params).eval()
-    sd = {k: v.detach().clone() for k, v in net.state_dict().items()}
-    return net.to(dev), sd
 
 
 @pytest.fixture(params=FORMS)
@@ -35,23 +20,8 @@ def form(request, model):
     """(net, sd, B): the network switched to the kernel form under test for the test's duration."""
     B, fused = request.param
     net, sd = model
-    net.set_option("fused_tail", fused)
-    yield net, sd, B
-    net.set_option("fused_tail", 1)
-
-
-def _clips(n, hops, seed, dev):
-    x, tgt = synth.mixture(n, HOP * hops, seed0=seed)
-    return F.pad(x, (0, LA)).to(dev), tgt
-
-
-def _emb(n, seed, dev):
-    return synth.embedding(n, seed0=seed)[:, 0].to(dev)
-
-
-def _chunk(clip, t):
-    """hop t of one padded clip [2, N]: its 128 samples + the 64 look-ahead samples"""
-    return clip[:, HOP * t:HOP * t + HOP + LA]
+    with su.switched(net, {"fused_tail": fused}):
+        yield net, sd, B
 
 
 def _hop(net, st, x, e, active=None):
@@ -70,15 +40,15 @@ def test_admit_into_running_state(form, dev):
     the admission."""
     net, _, B = form
     s = B - 1
-    other, _ = _clips(B, 110, 100, dev)
-    xc, _ = _clips(1, 70, 200, dev)
-    e_other, e_x = _emb(B, 300, dev), _emb(1, 400, dev)[0]
+    other, _ = su.clips(B, 110, 100, dev)
+    xc, _ = su.clips(1, 70, 200, dev)
+    e_other, e_x = su.emb(B, 300, dev), su.emb(1, 400, dev)[0]
 
     def inputs(t, x_hop):            # slot s carries X's hop x_hop (None: its original stream's hop t)
-        x = torch.stack([_chunk(other[b], t) for b in range(B)])
+        x = torch.stack([su.chunk(other[b], t) for b in range(B)])
         e = e_other.clone()
         if x_hop is not None:
-            x[s], e[s] = _chunk(xc[0], x_hop), e_x
+            x[s], e[s] = su.chunk(xc[0], x_hop), e_x
         return x, e
 
     st_a, st_b = net.init_buffers(B, dev), net.init_buffers(B, dev)
@@ -104,16 +74,6 @@ def test_admit_into_running_state(form, dev):
             assert torch.equal(_rec(st_a, b), _rec(st_b, b)), b
 
 
-def _forward_active(net, st, x, e, y, mask, flags, dev):
-    """l2h_sep_forward_active on fixed buffers (a service's staging buffers; with L2H_FLAG_GRAPH one cached graph)."""
-    B = x.shape[0]
-    ws, _ = net._workspace(dev, B, 1)
-    _cabi.check(_cabi.lib().l2h_sep_forward_active(
-        net._engine(), x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], e.data_ptr(), st.buf.data_ptr(), y.data_ptr(),
-        y.stride(0), y.stride(1), y.shape[-1], B, 1, ws.data_ptr(), ws.numel(), flags,
-        torch.cuda.current_stream(dev).cuda_stream, mask.data_ptr()))
-
-
 @pytest.mark.parametrize("graph", [False, True], ids=["direct", "graph"])
 def test_skip_hops(form, dev, graph):
     """Stream X in slot s misses hops 3, 4, 17 and 60: across each its record does not change and its rows of y are not
@@ -121,9 +81,9 @@ def test_skip_hops(form, dev, graph):
     L2H_FLAG_GRAPH the mask is rewritten in place and the same cached graph (the same argument set) is replayed."""
     net, _, B = form
     s, skip, T = B // 2, {3, 4, 17, 60}, 70
-    other, _ = _clips(B, T, 500, dev)
-    xc, _ = _clips(1, T, 600, dev)
-    e = _emb(B, 700, dev)
+    other, _ = su.clips(B, T, 500, dev)
+    xc, _ = su.clips(1, T, 600, dev)
+    e = su.emb(B, 700, dev)
     net._sync_weights(dev)
     xbuf = torch.empty(B, 2, HOP + LA, device=dev)
     ybuf = torch.empty(B, 2, HOP, device=dev)
@@ -133,11 +93,11 @@ def test_skip_hops(form, dev, graph):
     got, fed = [], 0
     for t in range(T):
         for b in range(B):
-            xbuf[b] = _chunk(xc[0], fed) if b == s else _chunk(other[b], t)
+            xbuf[b] = su.chunk(xc[0], fed) if b == s else su.chunk(other[b], t)
         mask[s] = 0 if t in skip else 1
         ybuf.fill_(1234.5)
         before = _rec(st, s)
-        _forward_active(net, st, xbuf, e, ybuf, mask, flags, dev)
+        net._launch("forward_active", xbuf, e, st, ybuf, 1, flags, mask=mask)
         if t in skip:
             assert torch.equal(_rec(st, s), before), f"record changed on skipped hop {t}"
             assert bool((ybuf[s] == 1234.5).all()), f"y written on skipped hop {t}"
@@ -148,7 +108,7 @@ def test_skip_hops(form, dev, graph):
     assert st.stream_pos()[s] == T - len(skip) and st.header() == (T, T)
     ref_st = net.init_buffers(B, dev)
     for j in range(fed):
-        x = torch.stack([_chunk(xc[0], j) if b == s else _chunk(other[b], j) for b in range(B)])
+        x = torch.stack([su.chunk(xc[0], j) if b == s else su.chunk(other[b], j) for b in range(B)])
         y = _hop(net, ref_st, x, e)
         assert torch.equal(got[j], y[s]), f"active hop {j}"
     assert torch.equal(_rec(st, s), _rec(ref_st, s))
@@ -160,9 +120,9 @@ def test_copy_between_states(form, dev):
     agrees with five one-hop calls."""
     net, sd, B = form
     s = B - 1
-    xo, _ = _clips(B, 63, 800, dev)
-    xp, _ = _clips(B, 49, 900, dev)
-    e1, e2 = _emb(B, 1000, dev), _emb(B, 1100, dev)
+    xo, _ = su.clips(B, 63, 800, dev)
+    xp, _ = su.clips(B, 49, 900, dev)
+    e1, e2 = su.emb(B, 1000, dev), su.emb(B, 1100, dev)
     s1 = net.init_buffers(B, dev)
     s2 = net.init_buffers(B, dev).load_reference(rs.sep_init_state(sd, B))
     for t in range(13):
@@ -196,8 +156,8 @@ def test_copy_between_states(form, dev):
 def test_copy_between_devices(model):
     net, _ = model
     d0, d1 = torch.device("cuda", 0), torch.device("cuda", 1)
-    xo, _ = _clips(2, 20, 1200, d0)
-    e = _emb(2, 1300, d0)
+    xo, _ = su.clips(2, 20, 1200, d0)
+    e = su.emb(2, 1300, d0)
     a = net.init_buffers(2, d0)
     for t in range(10):
         _hop(net, a, xo[..., HOP * t:HOP * t + HOP + LA], e)
@@ -216,11 +176,11 @@ def test_admitted_skipping_stream_vs_oracle(form, dev):
     """A stream admitted at hop 10 that then misses two hops, against the reference implementation fed the chunks it got."""
     net, sd, B = form
     s, T = 0, 40
-    other, _ = _clips(B, T, 1400, dev)
+    other, _ = su.clips(B, T, 1400, dev)
     n_fed = T - 10 - 2
     x_cpu, tgt = synth.mixture(1, HOP * n_fed, seed0=1500)
     xc = F.pad(x_cpu, (0, LA)).to(dev)
-    e = _emb(B, 1600, dev)
+    e = su.emb(B, 1600, dev)
     st = net.init_buffers(B, dev)
     got, fed = [], 0
     for t in range(T):
@@ -229,7 +189,7 @@ def test_admitted_skipping_stream_vs_oracle(form, dev):
         x = other[..., HOP * t:HOP * t + HOP + LA].clone()
         active = None
         if t >= 10:
-            x[s] = _chunk(xc[0], fed)
+            x[s] = su.chunk(xc[0], fed)
             active = torch.ones(B, dtype=torch.bool, device=dev)
             active[s] = t not in (13, 25)
         y = _hop(net, st, x, e, active)

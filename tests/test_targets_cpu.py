@@ -1,24 +1,12 @@
 """Host-side checks of calls that extract several targets per mixture (l2h_sep_forward_targets, Net.predict_targets /
 forward_targets): the argument errors the C call returns before it touches the device, the Python ValueErrors, and the
 header's description (no GPU needed; the handle below never commits weights)."""
-import ctypes
-import os
-import re
 
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-FAKE_DEV = ctypes.c_void_p(0x10000)          # never dereferenced: every call below fails its argument checks first
-L2H_FLAG_TAPS = 1
-
-
-@pytest.fixture(scope="module")
-def eng(tsh_params):
-    from lookoncetohear_b200 import Net, build, _cabi
-    build.build()
-    net = Net(**tsh_params)
-    return net, net._engine(), _cabi.lib()
+import serving_util as su
+from serving_util import FAKE_DEV, L2H_FLAG_TAPS, eng  # noqa: F401
 
 
 def _call(L, h, batch, n_targets, frames, flags=0, p=FAKE_DEV, emb=FAKE_DEV, y=FAKE_DEV):
@@ -47,9 +35,7 @@ def test_forward_targets_argument_errors(eng):
 
 def test_python_targets_raise_value_error(eng):
     net, _, _ = eng
-    from lookoncetohear_b200.net import SepState
-    hb, stride, offs = net._state_layout()
-    st6 = SepState(torch.zeros(hb // 4 + 6 * stride), 6, 3, hb, stride, offs)
+    st6 = su.host_state(net, 6)
     x = torch.zeros(2, 2, 192)
     for bad in (torch.zeros(2, 256), torch.zeros(2, 3, 128), torch.zeros(3, 3, 256), torch.zeros(2, 0, 256),
                 torch.zeros(2, 3, 256, 1), [[0.0] * 256] * 2):
@@ -68,14 +54,13 @@ def test_python_targets_raise_value_error(eng):
 
 
 def test_header_documents_forward_targets():
-    hdr = open(os.path.join(ROOT, "include", "lookonce_b200.h")).read()
-    decl = re.search(r"int l2h_sep_forward_targets\((.*?)\);", hdr, flags=re.S)
+    hdr = su.header()
+    decl, args = su.declaration(hdr, "l2h_sep_forward_targets")
     assert decl, "l2h_sep_forward_targets is not declared"
-    args = [a.split()[-1].lstrip("*") for a in " ".join(decl.group(1).split()).split(",")]
     assert args == ["handle", "x_dev", "x_batch_stride", "x_ch_stride", "x_len", "emb_dev", "state_dev", "y_dev",
                     "y_batch_stride", "y_ch_stride", "y_len", "batch", "n_targets", "frames", "workspace_dev",
                     "workspace_bytes", "flags", "stream"]
-    doc = " ".join(re.sub(r"\n\s*\*", " ", hdr[:decl.start()].rsplit("/*", 1)[1]).split())
+    doc = su.doc_before(hdr, decl.start())
     for phrase in ("i*K + k", "l2h_sep_state_bytes(handle, batch*K)", "l2h_sep_workspace_bytes(handle, batch*K, frames, flags)",
                    "lead record", "not a standalone stream", "n_targets == 1 is l2h_sep_forward", "L2H_FLAG_GRAPH",
                    "L2H_FLAG_TAPS", "slot lists", "l2h_sep_stream_host", "no compact record"):

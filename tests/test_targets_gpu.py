@@ -11,13 +11,12 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from lookoncetohear_b200 import Net, synth, _cabi
+from lookoncetohear_b200 import synth
 from oracle import restate as rs
+import serving_util as su
+from serving_util import HOP, LA, L2H_FLAG_GRAPH, dev, model  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-HOP, LA = 128, 64
-L2H_FLAG_GRAPH = 2
-DEFAULTS = {"fused_tail": 1, "back_many": 1, "fuse_ih": 0}
 # (mixtures, targets, hops per call, engine options, exact)
 FORMS = [pytest.param((1, 2, 1, {}, False), id="fused-tail-1x2"),
          pytest.param((2, 3, 1, {}, False), id="fused-tail-2x3"),
@@ -33,74 +32,25 @@ FORMS = [pytest.param((1, 2, 1, {}, False), id="fused-tail-1x2"),
          pytest.param((16, 3, 2, {"fuse_ih": 1}, True), id="T2-tc-lstm-x-16x3")]
 
 
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda", 0)
-
-
-@pytest.fixture(scope="module")
-def model(tsh_params, dev):
-    torch.manual_seed(0)
-    net = Net(**tsh_params).eval()
-    sd = {k: v.detach().clone() for k, v in net.state_dict().items()}
-    return net.to(dev), sd
-
-
-def _switched(net, opts):
-    for k, v in opts.items():
-        net.set_option(k, v)
-
-
 @pytest.fixture(params=FORMS)
 def form(request, model):
     """(net, sd, B, K, T, exact): the network switched to the kernel form under test for the test's duration."""
     B, K, T, opts, exact = request.param
     net, sd = model
-    _switched(net, opts)
-    yield net, sd, B, K, T, exact
-    _switched(net, {k: DEFAULTS[k] for k in opts})
-
-
-def _clips(n, hops, seed, dev):
-    x, tgt = synth.mixture(n, HOP * hops, seed0=seed)
-    return F.pad(x, (0, LA)).to(dev), tgt
-
-
-def _embeds(B, K, seed, dev):
-    return synth.embedding(B * K, seed0=seed)[:, 0].view(B, K, 256).to(dev)
-
-
-def _chunk(clips, t, T):
-    """hops t .. t+T-1 of padded clips [B, 2, N]: their 128*T samples + the 64 look-ahead samples"""
-    return clips[..., HOP * t:HOP * (t + T) + LA]
-
-
-def _bits(t):
-    """a float tensor as its bit patterns: records hold NaN (the embedding of a fresh stream), which torch.equal rejects"""
-    return t.contiguous().view(torch.int32)
-
-
-def _foreign(st, K):
-    """[records, stride] bool: the conv tails and block 0 of the non-lead records, which a targets call does not own"""
-    L = st.lay
-    m = torch.zeros(st.batch, st.stride, dtype=torch.bool, device=st.buf.device)
-    nonlead = [r for r in range(st.batch) if r % K]
-    m[nonlead, L["st_conv"]:L["st_deconv"]] = True
-    m[nonlead, L["st_blk"]:L["st_blk"] + L["bk_stride"]] = True
-    return m
+    with su.switched(net, opts):
+        yield net, sd, B, K, T, exact
 
 
 def _owned(st, K):
     """every record as bits, the regions a targets call does not own cleared"""
-    r = _bits(st._rec()).clone()
-    r[_foreign(st, K)] = 0
+    r = su.bits(st._rec()).clone()
+    r[su.foreign(st, K)] = 0
     return r
 
 
 def _owned_values(st, K):
     r = st._rec().clone()
-    r[_foreign(st, K)] = 0
+    r[su.foreign(st, K)] = 0
     return r
 
 
@@ -114,12 +64,12 @@ def test_targets_equal_duplicated_dense_call(form, dev):
     """4 consecutive calls: y and the owned part of every record equal the duplicated dense call's."""
     net, _, B, K, T, exact = form
     calls = 4
-    clips, _ = _clips(B, calls * T, 7100, dev)
-    emb = _embeds(B, K, 7200, dev)
+    clips, _ = su.clips(B, calls * T, 7100, dev)
+    emb = su.embeds(B, K, 7200, dev)
     got, ref = net.init_buffers(B * K, dev), net.init_buffers(B * K, dev)
     with torch.no_grad():
         for c in range(calls):
-            x = _chunk(clips, c * T, T)
+            x = su.chunk(clips, c * T, T)
             y, _ = net.predict_targets(x, emb, got, pad=False)
             y_ref, _ = net.predict(x.repeat_interleave(K, 0), emb.reshape(B * K, 256), ref, pad=False)
             assert y.shape == (B, K, 2, HOP * T)
@@ -139,24 +89,21 @@ def test_non_lead_regions_are_never_read(model, dev, B, K, T, opts):
     """NaN in the conv tails and block 0 of every non-lead record: the outputs stay finite and equal those of a state
     without the NaN, and those regions still hold NaN afterwards."""
     net, _ = model
-    _switched(net, opts)
-    try:
-        clips, _ = _clips(B, 3 * T, 7300, dev)
-        emb = _embeds(B, K, 7400, dev)
+    with su.switched(net, opts):
+        clips, _ = su.clips(B, 3 * T, 7300, dev)
+        emb = su.embeds(B, K, 7400, dev)
         clean, poisoned = net.init_buffers(B * K, dev), net.init_buffers(B * K, dev)
-        foreign = _foreign(poisoned, K)
+        foreign = su.foreign(poisoned, K)
         poisoned._rec()[foreign] = float("nan")
         with torch.no_grad():
             for c in range(3):
-                x = _chunk(clips, c * T, T)
+                x = su.chunk(clips, c * T, T)
                 y, _ = net.predict_targets(x, emb, clean, pad=False)
                 yp, _ = net.predict_targets(x, emb, poisoned, pad=False)
                 assert bool(torch.isfinite(yp).all()), f"call {c}"
                 assert torch.equal(yp, y), f"call {c}"
         assert bool(torch.isnan(poisoned._rec()[foreign]).all())
         assert torch.equal(_owned(poisoned, K), _owned(clean, K))
-    finally:
-        _switched(net, {k: DEFAULTS[k] for k in opts})
 
 
 @pytest.mark.parametrize("T", [1, 3])
@@ -164,16 +111,16 @@ def test_one_target_is_forward(model, dev, T):
     """n_targets = 1 is l2h_sep_forward bit for bit: outputs and the whole state."""
     net, _ = model
     B = 3
-    clips, _ = _clips(B, 3 * T, 7500, dev)
-    emb = _embeds(B, 1, 7600, dev)
+    clips, _ = su.clips(B, 3 * T, 7500, dev)
+    emb = su.embeds(B, 1, 7600, dev)
     got, ref = net.init_buffers(B, dev), net.init_buffers(B, dev)
     with torch.no_grad():
         for c in range(3):
-            x = _chunk(clips, c * T, T)
+            x = su.chunk(clips, c * T, T)
             y, _ = net.predict_targets(x, emb, got, pad=False)
             y_ref, _ = net.predict(x, emb[:, 0], ref, pad=False)
             assert torch.equal(y[:, 0], y_ref), f"call {c}"
-    assert torch.equal(_bits(got.buf), _bits(ref.buf))
+    assert torch.equal(su.bits(got.buf), su.bits(ref.buf))
 
 
 def test_streaming_equals_whole_clip(model, dev):
@@ -182,12 +129,12 @@ def test_streaming_equals_whole_clip(model, dev):
     B, K, hops = 1, 2, 500
     x, _ = synth.mixture(B, HOP * hops, seed0=7700)
     x = x.to(dev)
-    emb = _embeds(B, K, 7800, dev)
+    emb = su.embeds(B, K, 7800, dev)
     xp = F.pad(x, (0, LA))
     st = net.init_buffers(B * K, dev)
     with torch.no_grad():
         y = net.forward_targets(x, emb)
-        ys = torch.cat([net.predict_targets(_chunk(xp, t, 1), emb, st, pad=False)[0] for t in range(hops)], -1)
+        ys = torch.cat([net.predict_targets(su.chunk(xp, t, 1), emb, st, pad=False)[0] for t in range(hops)], -1)
     assert y.shape == ys.shape == (B, K, 2, HOP * hops)
     assert rs.rel_l2(ys.cpu(), y.cpu()) < 1e-4
 
@@ -197,14 +144,14 @@ def test_embedding_change_touches_only_its_target(model, dev):
     bit-identical to a run without the change."""
     net, _ = model
     B, K, calls = 2, 3, 8
-    clips, _ = _clips(B, calls, 7900, dev)
-    emb = _embeds(B, K, 8000, dev)
+    clips, _ = su.clips(B, calls, 7900, dev)
+    emb = su.embeds(B, K, 8000, dev)
     emb2 = emb.clone()
-    emb2[1, 2] = _embeds(1, 1, 8100, dev)[0, 0]
+    emb2[1, 2] = su.embeds(1, 1, 8100, dev)[0, 0]
     a, b = net.init_buffers(B * K, dev), net.init_buffers(B * K, dev)
     with torch.no_grad():
         for c in range(calls):
-            x = _chunk(clips, c, 1)
+            x = su.chunk(clips, c, 1)
             ya, _ = net.predict_targets(x, emb, a, pad=False)
             yb, _ = net.predict_targets(x, emb if c < calls // 2 else emb2, b, pad=False)
             changed = torch.zeros(B, K, dtype=torch.bool)
@@ -218,31 +165,23 @@ def test_group_reset_equals_fresh_group(model, dev):
     """reset_streams of a whole group and then continuing equals the group in a fresh state fed the same calls."""
     net, _ = model
     B, K = 2, 2
-    clips, _ = _clips(B, 10, 8200, dev)
-    emb = _embeds(B, K, 8300, dev)
+    clips, _ = su.clips(B, 10, 8200, dev)
+    emb = su.embeds(B, K, 8300, dev)
     st = net.init_buffers(B * K, dev)
     fresh = net.init_buffers(B * K, dev)
     group = [K * 1 + k for k in range(K)]
     with torch.no_grad():
         for c in range(4):
-            net.predict_targets(_chunk(clips, c, 1), emb, st, pad=False)
+            net.predict_targets(su.chunk(clips, c, 1), emb, st, pad=False)
         st.reset_streams(group)
         for c in range(4):
-            x = _chunk(clips, 4 + c, 1)
+            x = su.chunk(clips, 4 + c, 1)
             x_fresh = x.clone()
-            x_fresh[1] = _chunk(clips, c, 1)[1]          # group 1 starts from the clip's beginning again
+            x_fresh[1] = su.chunk(clips, c, 1)[1]          # group 1 starts from the clip's beginning again
             y, _ = net.predict_targets(x_fresh, emb, st, pad=False)
             y_ref, _ = net.predict_targets(x_fresh, emb, fresh, pad=False)
             assert torch.equal(y[1], y_ref[1]), f"call {c}"
     assert torch.equal(_owned(st, K)[group], _owned(fresh, K)[group])
-
-
-def _forward_targets(net, st, x, e, y, B, K, T, flags, dev):
-    ws, _ = net._workspace(dev, B * K, T)
-    _cabi.check(_cabi.lib().l2h_sep_forward_targets(
-        net._engine(), x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], e.data_ptr(), st.buf.data_ptr(), y.data_ptr(),
-        y.stride(1), y.stride(2), y.shape[-1], B, K, T, ws.data_ptr(), ws.numel(), flags,
-        torch.cuda.current_stream(dev).cuda_stream))
 
 
 @pytest.mark.parametrize("B, K, T", [pytest.param(2, 2, 1, id="one-hop"), pytest.param(8, 3, 1, id="tc-mid"),
@@ -252,18 +191,18 @@ def test_graph_replay_equals_direct_launches(model, dev, B, K, T):
     direct launches: outputs and the whole state."""
     net, _ = model
     calls = 4
-    clips, _ = _clips(B, calls * T, 8400, dev)
+    clips, _ = su.clips(B, calls * T, 8400, dev)
     net._sync_weights(dev)
     xbuf, ebuf = torch.empty(B, 2, HOP * T + LA, device=dev), torch.empty(B * K, 256, device=dev)
     yg, yd = torch.empty(B, K, 2, HOP * T, device=dev), torch.empty(B, K, 2, HOP * T, device=dev)
     sg, sdir = net.init_buffers(B * K, dev), net.init_buffers(B * K, dev)
     for c in range(calls):
-        xbuf.copy_(_chunk(clips, c * T, T))
-        ebuf.copy_(_embeds(B, K, 8500 + 10 * (c // 2), dev).reshape(B * K, 256))      # the embeddings change once
-        _forward_targets(net, sg, xbuf, ebuf, yg, B, K, T, L2H_FLAG_GRAPH, dev)
-        _forward_targets(net, sdir, xbuf, ebuf, yd, B, K, T, 0, dev)
+        xbuf.copy_(su.chunk(clips, c * T, T))
+        ebuf.copy_(su.embeds(B, K, 8500 + 10 * (c // 2), dev).reshape(B * K, 256))      # the embeddings change once
+        net._launch("targets", xbuf, ebuf, sg, yg, T, L2H_FLAG_GRAPH, K=K)
+        net._launch("targets", xbuf, ebuf, sdir, yd, T, K=K)
         assert torch.equal(yg, yd), c
-    assert torch.equal(_bits(sg.buf), _bits(sdir.buf))
+    assert torch.equal(su.bits(sg.buf), su.bits(sdir.buf))
 
 
 def test_offline_batch_split_equals_duplicated_forward(model, dev):
@@ -273,7 +212,7 @@ def test_offline_batch_split_equals_duplicated_forward(model, dev):
     B, K = 2, 2
     x, _ = synth.mixture(B, 64000, seed0=8600)
     x = x.to(dev)
-    emb = _embeds(B, K, 8700, dev)
+    emb = su.embeds(B, K, 8700, dev)
     keep = net.max_frames_per_launch
     net.max_frames_per_launch = 500 * K           # one mixture (K target rows of 500 frames) per launch
     try:
@@ -291,7 +230,7 @@ def test_targets_vs_oracle(model, dev):
     net, sd = model
     B, K = 2, 2
     x, tgt = synth.mixture(B, HOP * 40, seed0=8800)
-    emb = _embeds(B, K, 8900, dev)
+    emb = su.embeds(B, K, 8900, dev)
     with torch.no_grad():
         y = net.forward_targets(x.to(dev), emb).cpu()
     for i in range(B):

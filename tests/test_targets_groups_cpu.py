@@ -2,23 +2,13 @@
 Net.advance_targets): the argument errors the C call returns before it touches the device, the Python ValueErrors and the
 header's description (no GPU needed; the handle below never commits weights)."""
 import ctypes
-import os
 import re
 
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-FAKE_DEV = ctypes.c_void_p(0x10000)          # never dereferenced: every call below fails its argument checks first
-L2H_FLAG_TAPS = 1
-
-
-@pytest.fixture(scope="module")
-def eng(tsh_params):
-    from lookoncetohear_b200 import Net, build, _cabi
-    build.build()
-    net = Net(**tsh_params)
-    return net, net._engine(), _cabi.lib()
+import serving_util as su
+from serving_util import FAKE_DEV, L2H_FLAG_TAPS, eng  # noqa: F401
 
 
 def _call(L, h, state_batch, n, k, frames, groups=ctypes.c_void_p(0x30000), hops=None, flags=0, p=FAKE_DEV, emb=FAKE_DEV,
@@ -53,9 +43,7 @@ def test_forward_targets_groups_argument_errors(eng, hops):
 
 def test_python_advance_targets_raise_value_error(eng):
     net, _, _ = eng
-    from lookoncetohear_b200.net import SepState
-    hb, stride, offs = net._state_layout()
-    st = SepState(torch.zeros(hb // 4 + 8 * stride), 8, 3, hb, stride, offs)      # G = 4 groups of K = 2
+    st = su.host_state(net, 8)                                                    # G = 4 groups of K = 2
     x = torch.zeros(2, 2, 128 * 3 + 64)                                           # n = 2, T = 3
     emb = torch.zeros(2, 2, 256)
     for bad in (torch.zeros(2, 256), torch.zeros(2, 2, 128), torch.zeros(3, 2, 256), torch.zeros(2, 0, 256),
@@ -82,21 +70,20 @@ def test_python_advance_targets_raise_value_error(eng):
 
 
 def test_header_documents_forward_targets_groups():
-    hdr = open(os.path.join(ROOT, "include", "lookonce_b200.h")).read()
-    decl = re.search(r"int l2h_sep_forward_targets_groups\((.*?)\);", hdr, flags=re.S)
+    hdr = su.header()
+    decl, args = su.declaration(hdr, "l2h_sep_forward_targets_groups")
     assert decl, "l2h_sep_forward_targets_groups is not declared"
-    args = [a.split()[-1].lstrip("*") for a in " ".join(decl.group(1).split()).split(",")]
     assert args == ["handle", "x_dev", "x_batch_stride", "x_ch_stride", "x_len", "emb_dev", "state_dev", "state_batch",
                     "groups_dev", "hops_dev", "n", "n_targets", "frames", "y_dev", "y_batch_stride", "y_ch_stride", "y_len",
                     "workspace_dev", "workspace_bytes", "flags", "stream"]
     prev = re.search(r"int l2h_sep_forward_targets\(", hdr)
     assert prev and prev.start() < decl.start(), "declared after l2h_sep_forward_targets"
-    doc = " ".join(re.sub(r"\n\s*\*", " ", hdr[:decl.start()].rsplit("/*", 1)[1]).split())
+    doc = su.doc_before(hdr, decl.start())
     for phrase in ("g*K + k", "lead record", "groups_dev", "outside [0, G)", "hops_dev", "NULL", "128*h + 63", "128*h - 1",
                    "h = 0 stores nothing", "outside [0, frames] counts as 0", "l2h_sep_workspace_bytes(handle, n*K, frames, flags)",
                    "(n, K, T)", "L2H_FLAG_GRAPH", "L2H_FLAG_TAPS", "n_targets == 1 is l2h_sep_forward_slots_hops"):
         assert phrase in doc, phrase
     # the targets call's description points at this one for slot lists and hop counts
-    targets_doc = " ".join(re.sub(r"\n\s*\*", " ", hdr[:prev.start()].rsplit("/*", 1)[1]).split())
+    targets_doc = su.doc_before(hdr, prev.start())
     assert "l2h_sep_forward_targets_groups" in targets_doc
     assert "#define L2H_ABI_VERSION 1" in hdr

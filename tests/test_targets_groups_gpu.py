@@ -11,14 +11,12 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from lookoncetohear_b200 import Net, synth, _cabi
+from lookoncetohear_b200 import synth
 from oracle import restate as rs
+import serving_util as su
+from serving_util import HOP, LA, L2H_FLAG_GRAPH, SENTINEL, dev, model  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-HOP, LA = 128, 64
-L2H_FLAG_GRAPH = 2
-SENTINEL = float("nan")
-DEFAULTS = {"fused_tail": 1, "back_many": 1, "fuse_ih": 0}
 # (listed groups, targets, hops per call, engine options): the forms of tests/test_targets_gpu.py
 FORMS = [pytest.param((1, 2, 1, {}), id="fused-tail-1x2"),
          pytest.param((2, 3, 1, {}), id="fused-tail-2x3"),
@@ -40,147 +38,21 @@ RAGGED = [pytest.param((2, 2, 3, {}), id="T3-2x2"),
           pytest.param((16, 3, 2, {"fuse_ih": 1}), id="T2-tc-lstm-x-16x3")]
 
 
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda", 0)
-
-
-@pytest.fixture(scope="module")
-def model(tsh_params, dev):
-    torch.manual_seed(0)
-    net = Net(**tsh_params).eval()
-    sd = {k: v.detach().clone() for k, v in net.state_dict().items()}
-    net = net.to(dev)
-    net._sync_weights(dev)
-    return net, sd
-
-
-def _switched(net, opts):
-    for k, v in opts.items():
-        net.set_option(k, v)
-
-
-def _form(request, model):
-    n, K, T, opts = request.param
-    net, sd = model
-    _switched(net, opts)
-    return net, sd, n, K, T, opts
-
-
 @pytest.fixture(params=FORMS)
 def form(request, model):
     """(net, sd, n, K, T): the network switched to the kernel form under test for the test's duration."""
-    net, sd, n, K, T, opts = _form(request, model)
-    yield net, sd, n, K, T
-    _switched(net, {k: DEFAULTS[k] for k in opts})
+    n, K, T, opts = request.param
+    net, sd = model
+    with su.switched(net, opts):
+        yield net, sd, n, K, T
 
 
 @pytest.fixture(params=RAGGED)
 def ragged(request, model):
-    net, sd, n, K, T, opts = _form(request, model)
-    yield net, sd, n, K, T
-    _switched(net, {k: DEFAULTS[k] for k in opts})
-
-
-def _clips(n, hops, seed, dev):
-    x, tgt = synth.mixture(n, HOP * hops, seed0=seed)
-    return F.pad(x, (0, LA)).to(dev), tgt
-
-
-def _embeds(G, K, seed, dev):
-    return synth.embedding(G * K, seed0=seed)[:, 0].view(G, K, 256).to(dev)
-
-
-def _chunk(clip, t, T):
-    """hops t .. t+T-1 of one padded clip [2, N]: their 128*T samples + the 64 look-ahead samples"""
-    return clip[:, HOP * t:HOP * (t + T) + LA]
-
-
-def _subsets(G, n, calls, seed):
-    """a different unsorted list of n distinct groups for every call"""
-    g = torch.Generator().manual_seed(seed)
-    return [torch.randperm(G, generator=g)[:n].tolist() for _ in range(calls)]
-
-
-def _hops(n, T, seed):
-    """n hop counts in [0, T] that include 0, 1 and T (n >= 3), else 1 and T"""
-    g = torch.Generator().manual_seed(seed)
-    h = torch.randint(0, T + 1, (n,), generator=g)
-    fixed = [0, 1, T] if n >= 3 else [1, T]
-    h[torch.randperm(n, generator=g)[:len(fixed)]] = torch.tensor(fixed)
-    return h.tolist()
-
-
-def _bits(t):
-    """a float tensor as its bit patterns: records hold NaN (the embedding of a fresh stream), which torch.equal rejects"""
-    return t.contiguous().view(torch.int32)
-
-
-def _records(st):
-    """every record as bits, the gate memo's weight generation word cleared: copy_streams_from invalidates the memo of the
-    records it writes (by design), so the oracle's records carry generation 0 where a groups call keeps it"""
-    r = _bits(st._rec()).clone()
-    r[:, st.lay["st_emb"] + 256] = 0
-    return r
-
-
-def _recs(groups, K):
-    return [g * K + k for g in groups for k in range(K)]
-
-
-def _foreign(st, K):
-    """[records, stride] bool: the conv tails and block 0 of the non-lead records, which a targets call does not own"""
-    L = st.lay
-    m = torch.zeros(st.batch, st.stride, dtype=torch.bool, device=st.buf.device)
-    nonlead = [r for r in range(st.batch) if r % K]
-    m[nonlead, L["st_conv"]:L["st_deconv"]] = True
-    m[nonlead, L["st_blk"]:L["st_blk"] + L["bk_stride"]] = True
-    return m
-
-
-def _oracle(net, st, compact, x, emb, groups, K):
-    """copy the listed groups' records into a compact state of n*K records, predict_targets there, copy them back"""
-    recs = _recs(groups, K)
-    compact.copy_streams_from(st, recs, list(range(len(recs))))
-    y, _ = net.predict_targets(x, emb, compact, pad=False)
-    st.copy_streams_from(compact, list(range(len(recs))), recs)
-    return y
-
-
-def _warm_state(net, G, n, K, T, seed, dev):
-    """a state of G groups with history and different clocks, advanced through the oracle; and the groups' clip positions"""
-    clips, _ = _clips(G, 2 * T, seed, dev)
-    emb = _embeds(G, K, seed + 1, dev)
-    st = net.init_buffers(G * K, dev)
-    compact = net.init_buffers(n * K, dev)
-    fed = [0] * G
-    with torch.no_grad():
-        for sl in _subsets(G, n, 2, seed + 2):
-            _oracle(net, st, compact, torch.stack([_chunk(clips[g], fed[g], T) for g in sl]), emb[sl], sl, K)
-            for g in sl:
-                fed[g] += T
-    return st, fed
-
-
-def _copy(net, st, dev):
-    twin = net.init_buffers(st.batch, dev)
-    twin.buf.copy_(st.buf)
-    return twin
-
-
-def _forward_groups(net, st, x, e, groups, hops, y, K, T, flags, dev):
-    """l2h_sep_forward_targets_groups on fixed buffers: x [n, 2, 128*T + 64], e [n*K, 256], y [n, K, 2, 128*T]"""
-    n = x.shape[0]
-    ws, _ = net._workspace(dev, n * K, T)
-    _cabi.check(_cabi.lib().l2h_sep_forward_targets_groups(
-        net._engine(), x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], e.data_ptr(), st.buf.data_ptr(), st.batch,
-        groups.data_ptr(), None if hops is None else hops.data_ptr(), n, K, T, y.data_ptr(), y.stride(1), y.stride(2),
-        y.shape[-1], ws.data_ptr(), ws.numel(), flags, torch.cuda.current_stream(dev).cuda_stream))
-
-
-def _i32(v, dev):
-    return torch.tensor(v, dtype=torch.int32, device=dev)
+    n, K, T, opts = request.param
+    net, sd = model
+    with su.switched(net, opts):
+        yield net, sd, n, K, T
 
 
 # ---- every form against copy / predict_targets / copy back ----------------------------------------------------------
@@ -189,27 +61,27 @@ def test_groups_equal_copy_run_copy_back(form, dev):
     bit for bit, unlisted records are untouched, and so are the conv tails and block 0 of the non-lead records."""
     net, _, n, K, T = form
     G = n + 3
-    st, fed = _warm_state(net, G, n, K, T, 4100, dev)
-    ref = _copy(net, st, dev)
+    st, fed = su.warm_groups(net, G, n, K, T, 4100, dev)
+    ref = su.copy(net, st)
     compact = net.init_buffers(n * K, dev)
-    clips, _ = _clips(G, 8 * T, 4100, dev)
-    emb = _embeds(G, K, 4101, dev)                      # the warm-up's embeddings: the gate memos stay valid
-    foreign = _foreign(st, K)
+    clips, _ = su.clips(G, 8 * T, 4100, dev)
+    emb = su.embeds(G, K, 4101, dev)                      # the warm-up's embeddings: the gate memos stay valid
+    foreign = su.foreign(st, K)
     with torch.no_grad():
-        for c, sl in enumerate(_subsets(G, n, 4, 4200)):
-            x = torch.stack([_chunk(clips[g], fed[g], T) for g in sl])
-            before = _bits(st._rec()).clone()
+        for c, sl in enumerate(su.subsets(G, n, 4, 4200)):
+            x = torch.stack([su.chunk(clips[g], fed[g], T) for g in sl])
+            before = su.bits(st._rec()).clone()
             y = net.advance_targets(x, emb[sl], st, sl)
-            y_ref = _oracle(net, ref, compact, x, emb[sl], sl, K)
+            y_ref = su.oracle(net, ref, su.recs(sl, K), x, emb[sl], compact)
             for g in sl:
                 fed[g] += T
             assert y.shape == (n, K, 2, HOP * T)
-            assert torch.equal(_bits(y), _bits(y_ref)), f"call {c}: y"
-            listed = _recs(sl, K)
+            assert torch.equal(su.bits(y), su.bits(y_ref)), f"call {c}: y"
+            listed = su.recs(sl, K)
             unlisted = [r for r in range(G * K) if r not in listed]
-            assert torch.equal(_bits(st._rec())[unlisted], before[unlisted]), f"call {c}: an unlisted record changed"
-            assert torch.equal(_records(st), _records(ref)), f"call {c}: records"
-            assert torch.equal(_bits(st._rec())[foreign], before[foreign]), f"call {c}: a non-lead conv tail or block 0"
+            assert torch.equal(su.bits(st._rec())[unlisted], before[unlisted]), f"call {c}: an unlisted record changed"
+            assert torch.equal(su.records(st), su.records(ref)), f"call {c}: records"
+            assert torch.equal(su.bits(st._rec())[foreign], before[foreign]), f"call {c}: a non-lead conv tail or block 0"
     assert st.stream_pos() == ref.stream_pos() == [fed[r // K] for r in range(G * K)]
 
 
@@ -217,51 +89,35 @@ def test_groups_equal_copy_run_copy_back(form, dev):
 def test_all_hops_T_equal_no_hop_list(ragged, dev):
     net, _, n, K, T = ragged
     G = n + 2
-    st, _ = _warm_state(net, G, n, K, T, 4300, dev)
-    twin = _copy(net, st, dev)
-    clips, _ = _clips(n, T, 4400, dev)
-    e = _embeds(n, K, 4500, dev).reshape(n * K, 256)
-    groups = _i32(_subsets(G, n, 1, 4600)[0], dev)
+    st, _ = su.warm_groups(net, G, n, K, T, 4300, dev)
+    twin = su.copy(net, st)
+    clips, _ = su.clips(n, T, 4400, dev)
+    e = su.embeds(n, K, 4500, dev).reshape(n * K, 256)
+    groups = su.i32(su.subsets(G, n, 1, 4600)[0], dev)
     y = torch.full((n, K, 2, HOP * T), SENTINEL, device=dev)
     y_ref = torch.full_like(y, SENTINEL)
-    _forward_groups(net, st, clips.contiguous(), e, groups, _i32([T] * n, dev), y, K, T, 0, dev)
-    _forward_groups(net, twin, clips.contiguous(), e, groups, None, y_ref, K, T, 0, dev)
+    net._launch("targets_groups", clips.contiguous(), e, st, y, T, slots=groups, hops=su.i32([T] * n, dev), K=K)
+    net._launch("targets_groups", clips.contiguous(), e, twin, y_ref, T, slots=groups, K=K)
     torch.cuda.synchronize()
-    assert torch.equal(_bits(y), _bits(y_ref))
-    assert torch.equal(_bits(st.buf), _bits(twin.buf))
+    assert torch.equal(su.bits(y), su.bits(y_ref))
+    assert torch.equal(su.bits(st.buf), su.bits(twin.buf))
 
 
 def test_zero_hops_and_outside_groups_store_nothing(ragged, dev):
     net, _, n, K, T = ragged
     G = n + 2
-    st, _ = _warm_state(net, G, n, K, T, 4700, dev)
-    before = _bits(st._rec()).clone()
-    clips, _ = _clips(n, T, 4800, dev)
-    e = _embeds(n, K, 4900, dev).reshape(n * K, 256)
-    sl = _subsets(G, n, 1, 5000)[0]
+    st, _ = su.warm_groups(net, G, n, K, T, 4700, dev)
+    before = su.bits(st._rec()).clone()
+    clips, _ = su.clips(n, T, 4800, dev)
+    e = su.embeds(n, K, 4900, dev).reshape(n * K, 256)
+    sl = su.subsets(G, n, 1, 5000)[0]
     for groups, hops in ((sl, [0] * n), ([-1 - i if i % 2 else G + i for i in range(n)], [T] * n),
                          (sl, [T + 1 + i if i % 2 else -1 - i for i in range(n)])):      # counts outside [0, T] count as 0
         y = torch.full((n, K, 2, HOP * T), SENTINEL, device=dev)
-        _forward_groups(net, st, clips.contiguous(), e, _i32(groups, dev), _i32(hops, dev), y, K, T, 0, dev)
+        net._launch("targets_groups", clips.contiguous(), e, st, y, T, slots=su.i32(groups, dev), hops=su.i32(hops, dev), K=K)
         torch.cuda.synchronize()
         assert bool(torch.isnan(y).all()), (groups, hops, "a y row was written")
-        assert torch.equal(_bits(st._rec()), before), (groups, hops, "a record changed")
-
-
-def _ring_mask(st, frames):
-    """bool [stride]: the ring rows of a record holding the given frames (every block, head, K and V)"""
-    L = st.lay
-    m = torch.zeros(st.stride, dtype=torch.bool, device=st.buf.device)
-    for blk in range(st.n_blocks):
-        base = L["st_blk"] + blk * L["bk_stride"]
-        for h in range(4):
-            for f in frames:
-                slot = f % L["ring"]
-                k0 = base + L["bk_k"] + (h * L["ring"] + slot) * L["k_ld"]
-                v0 = base + L["bk_v"] + (h * L["ring"] + slot) * L["v_dim"]
-                m[k0:k0 + L["k_ld"]] = True
-                m[v0:v0 + L["v_dim"]] = True
-    return m
+        assert torch.equal(su.bits(st._rec()), before), (groups, hops, "a record changed")
 
 
 def test_mixed_hops_match_uniform_call_where_they_advance(ragged, dev):
@@ -270,40 +126,40 @@ def test_mixed_hops_match_uniform_call_where_they_advance(ragged, dev):
     as before; every record of a group advances its clock by h_i (its calls by 1 if h_i > 0)."""
     net, _, n, K, T = ragged
     G = n + 2
-    st, _ = _warm_state(net, G, n, K, T, 5100, dev)
-    twin = _copy(net, st, dev)
+    st, _ = su.warm_groups(net, G, n, K, T, 5100, dev)
+    twin = su.copy(net, st)
     before = st._rec().clone()
     pos0, calls0 = st.stream_pos(), st._clocks()[1].cpu().tolist()
-    clips, _ = _clips(n, T, 5200, dev)
+    clips, _ = su.clips(n, T, 5200, dev)
     x = clips.contiguous().clone()
-    hops = _hops(n, T, 5300)
+    hops = su.hop_mix(n, T, 5300)
     for i, h in enumerate(hops):
         x[i, :, HOP * h + LA:] = float("nan")
-    e = _embeds(n, K, 5400, dev).reshape(n * K, 256)
-    sl = _subsets(G, n, 1, 5500)[0]
+    e = su.embeds(n, K, 5400, dev).reshape(n * K, 256)
+    sl = su.subsets(G, n, 1, 5500)[0]
     y = torch.full((n, K, 2, HOP * T), SENTINEL, device=dev)
     y_ref = torch.full_like(y, SENTINEL)
-    _forward_groups(net, st, x, e, _i32(sl, dev), _i32(hops, dev), y, K, T, 0, dev)
-    _forward_groups(net, twin, clips.contiguous(), e, _i32(sl, dev), None, y_ref, K, T, 0, dev)
+    net._launch("targets_groups", x, e, st, y, T, slots=su.i32(sl, dev), hops=su.i32(hops, dev), K=K)
+    net._launch("targets_groups", clips.contiguous(), e, twin, y_ref, T, slots=su.i32(sl, dev), K=K)
     torch.cuda.synchronize()
-    ring_all = _ring_mask(st, range(st.lay["ring"]))
+    ring_all = su.ring_mask(st, range(st.lay["ring"]))
     for i, (g, h) in enumerate(zip(sl, hops)):
-        assert torch.equal(_bits(y[i, ..., :HOP * h]), _bits(y_ref[i, ..., :HOP * h])), (i, h)
+        assert torch.equal(su.bits(y[i, ..., :HOP * h]), su.bits(y_ref[i, ..., :HOP * h])), (i, h)
         assert bool(torch.isnan(y[i, ..., HOP * h:]).all()), (i, h, "y written past the group's hops")
-        for r in _recs([g], K):
-            new = _ring_mask(st, range(pos0[r], pos0[r] + h))
-            assert torch.equal(_bits(st._rec()[r][new]), _bits(twin._rec()[r][new])), (i, h, r, "ring rows of the new frames")
+        for r in su.recs([g], K):
+            new = su.ring_mask(st, range(pos0[r], pos0[r] + h))
+            assert torch.equal(su.bits(st._rec()[r][new]), su.bits(twin._rec()[r][new])), (i, h, r, "ring rows of the new frames")
             other = ring_all & ~new
-            assert torch.equal(_bits(st._rec()[r][other]), _bits(before[r][other])), (i, h, r, "another ring row changed")
+            assert torch.equal(su.bits(st._rec()[r][other]), su.bits(before[r][other])), (i, h, r, "another ring row changed")
             if h == 0:
-                assert torch.equal(_bits(st._rec()[r]), _bits(before[r])), (i, r, "h = 0 stored something")
+                assert torch.equal(su.bits(st._rec()[r]), su.bits(before[r])), (i, r, "h = 0 stored something")
             if h == T:
-                assert torch.equal(_bits(st._rec()[r]), _bits(twin._rec()[r])), (i, r, "h = T")
-    unlisted = [r for r in range(G * K) if r not in _recs(sl, K)]
-    assert torch.equal(_bits(st._rec()[unlisted]), _bits(before[unlisted]))
+                assert torch.equal(su.bits(st._rec()[r]), su.bits(twin._rec()[r])), (i, r, "h = T")
+    unlisted = [r for r in range(G * K) if r not in su.recs(sl, K)]
+    assert torch.equal(su.bits(st._rec()[unlisted]), su.bits(before[unlisted]))
     pos, calls = st.stream_pos(), st._clocks()[1].cpu().tolist()
     for g, h in zip(sl, hops):
-        for r in _recs([g], K):
+        for r in su.recs([g], K):
             assert pos[r] == pos0[r] + h and calls[r] == calls0[r] + (1 if h > 0 else 0), (g, r, h)
 
 
@@ -312,22 +168,18 @@ def test_mixed_hops_match_uniform_call_where_they_advance(ragged, dev):
 def test_one_target_is_slots_hops(model, dev, n, T):
     net, _ = model
     S = n + 3
-    clips, _ = _clips(n, 3 * T, 5600, dev)
-    e = _embeds(n, 1, 5700, dev).reshape(n, 256)
+    clips, _ = su.clips(n, 3 * T, 5600, dev)
+    e = su.embeds(n, 1, 5700, dev).reshape(n, 256)
     a, b = net.init_buffers(S, dev), net.init_buffers(S, dev)
     ya, yb = torch.full((n, 1, 2, HOP * T), SENTINEL, device=dev), torch.full((n, 2, HOP * T), SENTINEL, device=dev)
-    ws, _ = net._workspace(dev, n, T)
-    for c, sl in enumerate(_subsets(S, n, 3, 5800)):
+    for c, sl in enumerate(su.subsets(S, n, 3, 5800)):
         x = clips[..., HOP * T * c:HOP * T * (c + 1) + LA].contiguous()
-        groups, hops = _i32(sl, dev), _i32(_hops(n, T, 5900 + c), dev)
-        _forward_groups(net, a, x, e, groups, hops, ya, 1, T, 0, dev)
-        _cabi.check(_cabi.lib().l2h_sep_forward_slots_hops(
-            net._engine(), x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], e.data_ptr(), b.buf.data_ptr(), S,
-            groups.data_ptr(), hops.data_ptr(), n, T, yb.data_ptr(), yb.stride(0), yb.stride(1), yb.shape[-1], ws.data_ptr(),
-            ws.numel(), 0, torch.cuda.current_stream(dev).cuda_stream))
+        groups, hops = su.i32(sl, dev), su.i32(su.hop_mix(n, T, 5900 + c), dev)
+        net._launch("targets_groups", x, e, a, ya, T, slots=groups, hops=hops, K=1)
+        net._launch("slots_hops", x, e, b, yb, T, slots=groups, hops=hops)
         torch.cuda.synchronize()
-        assert torch.equal(_bits(ya[:, 0]), _bits(yb)), c
-    assert torch.equal(_bits(a.buf), _bits(b.buf))
+        assert torch.equal(su.bits(ya[:, 0]), su.bits(yb)), c
+    assert torch.equal(su.bits(a.buf), su.bits(b.buf))
 
 
 # ---- graph replay with the lists rewritten in place --------------------------------------------------------------------
@@ -339,19 +191,19 @@ def test_graph_replay_with_groups_and_hops_rewritten(model, dev, n, K, T):
     twin state, bit for bit.  Only the first tick captures: the graph cached for (n, K, T) reads the lists when it runs."""
     net, _ = model
     G, calls = n + 3, 5
-    clips, _ = _clips(G, calls * T, 6000, dev)
-    emb = _embeds(G, K, 6100, dev)
+    clips, _ = su.clips(G, calls * T, 6000, dev)
+    emb = su.embeds(G, K, 6100, dev)
     xbuf, ebuf = torch.empty(n, 2, HOP * T + LA, device=dev), torch.empty(n * K, 256, device=dev)
     groups, hops = torch.empty(n, dtype=torch.int32, device=dev), torch.empty(n, dtype=torch.int32, device=dev)
     yg, yd = torch.empty(n, K, 2, HOP * T, device=dev), torch.empty(n, K, 2, HOP * T, device=dev)
     sg, sdir = net.init_buffers(G * K, dev), net.init_buffers(G * K, dev)
     fed = [0] * G
     host = []
-    for c, sl in enumerate(_subsets(G, n, calls, 6200)):
-        hh = _hops(n, T, 6300 + c) if T > 1 else [1] * n
+    for c, sl in enumerate(su.subsets(G, n, calls, 6200)):
+        hh = su.hop_mix(n, T, 6300 + c) if T > 1 else [1] * n
         listed = list(sl)
         listed[c % n] = G + c if c % 2 else -1 - c            # one group misses the tick
-        xbuf.copy_(torch.stack([_chunk(clips[g], fed[g], T) for g in sl]))
+        xbuf.copy_(torch.stack([su.chunk(clips[g], fed[g], T) for g in sl]))
         ebuf.copy_(emb[sl].reshape(n * K, 256))
         groups.copy_(torch.tensor(listed, dtype=torch.int32))
         hops.copy_(torch.tensor(hh, dtype=torch.int32))
@@ -359,16 +211,16 @@ def test_graph_replay_with_groups_and_hops_rewritten(model, dev, n, K, T):
         yd.fill_(SENTINEL)
         torch.cuda.synchronize()
         t0 = time.perf_counter()
-        _forward_groups(net, sg, xbuf, ebuf, groups, hops, yg, K, T, L2H_FLAG_GRAPH, dev)
+        net._launch("targets_groups", xbuf, ebuf, sg, yg, T, L2H_FLAG_GRAPH, slots=groups, hops=hops, K=K)
         host.append(time.perf_counter() - t0)
-        _forward_groups(net, sdir, xbuf, ebuf, groups, hops, yd, K, T, 0, dev)
+        net._launch("targets_groups", xbuf, ebuf, sdir, yd, T, slots=groups, hops=hops, K=K)
         for i, g in enumerate(listed):
             if 0 <= g < G:
                 fed[g] += hh[i]
         torch.cuda.synchronize()
-        assert torch.equal(_bits(yg), _bits(yd)), c
+        assert torch.equal(su.bits(yg), su.bits(yd)), c
         assert bool(torch.isnan(yg[c % n]).all()), (c, "the missing group wrote y")
-    assert torch.equal(_bits(sg.buf), _bits(sdir.buf))
+    assert torch.equal(su.bits(sg.buf), su.bits(sdir.buf))
     assert sg.stream_pos() == [fed[r // K] for r in range(G * K)]
     assert max(host[1:]) < 0.5 * host[0], ("a replay took as long as a capture: new graph per tick?", host)
 
@@ -381,7 +233,7 @@ def test_streaming_with_missed_hops_equals_whole_clip(model, dev):
     net, sd = model
     G, K, total = 2, 2, 40
     x, tgt = synth.mixture(G, HOP * total, seed0=6400)
-    emb = _embeds(G, K, 6500, dev)
+    emb = su.embeds(G, K, 6500, dev)
     xp = F.pad(x.to(dev), (0, LA + HOP * total))          # a call's x rows span its longest backlog
     st = net.init_buffers(G * K, dev)
     gen = torch.Generator().manual_seed(6600)
@@ -402,7 +254,7 @@ def test_streaming_with_missed_hops_equals_whole_clip(model, dev):
             if T == 0:
                 continue
             catch_ups += T > 1
-            xs = torch.stack([_chunk(xp[g], fed[g], T) for g in range(G)])
+            xs = torch.stack([su.chunk(xp[g], fed[g], T) for g in range(G)])
             y = net.advance_targets(xs, emb, st, list(range(G)), hops=h)
             for g in range(G):
                 outs[g].append(y[g, ..., :HOP * h[g]])

@@ -24,45 +24,12 @@ power limit, which belong with the numbers.
 import argparse
 import ctypes
 import json
-import os
-import statistics
-import subprocess
 import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-from lookoncetohear_b200 import Net, synth, _cabi  # noqa: E402
-from lookoncetohear_b200.configs import TSH_PARAMS  # noqa: E402
-
-HOP, LA = 128, 64
-L2H_FLAG_GRAPH = 2
-
-
-def median_ms(fn, reps, windows=5):
-    out = []
-    for _ in range(windows):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        for i in range(reps):
-            fn(i)
-        b.record()
-        torch.cuda.synchronize()
-        out.append(a.elapsed_time(b) / reps)
-    return statistics.median(out)
-
-
-def gpu_info():
-    info = {"gpu": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30)
-        info["power_limit_and_max_sm_clock"] = q.stdout.strip().splitlines()[0]
-    except (OSError, subprocess.SubprocessError, IndexError):
-        info["power_limit_and_max_sm_clock"] = "unavailable"
-    return info
+from bench_common import HOP, LA, L2H_FLAG_GRAPH, emit, gpu_info, median_ms, setup_net
+from lookoncetohear_b200 import synth, _cabi
 
 
 def main():
@@ -71,16 +38,10 @@ def main():
     ap.add_argument("--reps", type=int, default=20, help="ticks per timed window")
     ap.add_argument("--out", default=None, help="also write the JSON here")
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("bench_ragged_backlog: needs a CUDA device")
-    dev = torch.device("cuda", 0)
+    net, dev = setup_net("bench_ragged_backlog")
     S, R = args.slots, args.reps
     cases = [(n, T) for n in (4, 16, 64) for T in (2, 4, 8) if n <= S]
-    torch.manual_seed(0)
-    net = Net(**TSH_PARAMS).eval().to(dev)
-    net._sync_weights(dev)
     L, h = _cabi.lib(), net._engine()
-    st_ptr = torch.cuda.current_stream(dev).cuda_stream
 
     def ws_bytes(n, T):
         b = ctypes.c_size_t()
@@ -114,47 +75,31 @@ def main():
         dslots = {d: torch.empty(n, dtype=torch.int32, device=dev) for d in range(1, T + 1)}
         debuf = {d: torch.empty(n, 256, device=dev) for d in range(1, T + 1)}
 
-        def call(sl, hp, eb, m, d, flags=L2H_FLAG_GRAPH):
-            xd = x[d]
-            if hp is None:
-                _cabi.check(L.l2h_sep_forward_slots_frames(
-                    h, xd.data_ptr(), xd.stride(0), xd.stride(1), HOP * d + LA, eb.data_ptr(), big.buf.data_ptr(), S,
-                    sl.data_ptr(), m, d, y.data_ptr(), y.stride(0), y.stride(1), HOP * d, ws.data_ptr(), ws.numel(),
-                    flags, st_ptr))
-            else:
-                _cabi.check(L.l2h_sep_forward_slots_hops(
-                    h, xd.data_ptr(), xd.stride(0), xd.stride(1), HOP * d + LA, eb.data_ptr(), big.buf.data_ptr(), S,
-                    sl.data_ptr(), hp.data_ptr(), m, d, y.data_ptr(), y.stride(0), y.stride(1), HOP * d, ws.data_ptr(),
-                    ws.numel(), L2H_FLAG_GRAPH, st_ptr))
+        def call(entry, sl, eb, m, d, flags=L2H_FLAG_GRAPH, hp=None):
+            net._launch(entry, x[d][:m], eb, big, y[:m, :, :HOP * d], d, flags, slots=sl, hops=hp, ws=ws)
 
         def run_ragged(i):
             slots.copy_(lists[i % R])
             hops.copy_(mixes[i % R])
             ebuf.copy_(embs[i % R])
-            call(slots, hops, ebuf, n, T)
+            call("slots_hops", slots, ebuf, n, T, hp=hops)
 
         def run_per_depth(i, flags=L2H_FLAG_GRAPH):
             for d, (sl, eb) in groups[i % R].items():
                 m = sl.shape[0]
                 dslots[d][:m].copy_(sl)
                 debuf[d][:m].copy_(eb)
-                if d == 1:
-                    _cabi.check(L.l2h_sep_forward_slots(
-                        h, x[1].data_ptr(), x[1].stride(0), x[1].stride(1), HOP + LA, debuf[1].data_ptr(),
-                        big.buf.data_ptr(), S, dslots[1].data_ptr(), m, y.data_ptr(), y.stride(0), y.stride(1), HOP,
-                        ws.data_ptr(), ws.numel(), flags, st_ptr))
-                else:
-                    call(dslots[d], None, debuf[d], m, d, flags)
+                call("slots" if d == 1 else "slots_frames", dslots[d], debuf[d], m, d, flags)
 
         def run_equal_ragged(i):
             slots.copy_(lists[i % R])
             ebuf.copy_(embs[i % R])
-            call(slots, full, ebuf, n, T)
+            call("slots_hops", slots, ebuf, n, T, hp=full)
 
         def run_equal_frames(i):
             slots.copy_(lists[i % R])
             ebuf.copy_(embs[i % R])
-            call(slots, None, ebuf, n, T)
+            call("slots_frames", slots, ebuf, n, T)
 
         fns = {"ragged_ms": run_ragged, "per_depth_ms": run_per_depth,
                "per_depth_direct_ms": lambda i: run_per_depth(i, 0), "equal_ragged_ms": run_equal_ragged,
@@ -169,11 +114,7 @@ def main():
         r["mean_calls_per_depth_tick"] = sum(len(gi) for gi in groups) / R
         res["cases"][f"n{n}_T{T}"] = r
         print(json.dumps({f"n{n}_T{T}": r}), file=sys.stderr)
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        with open(args.out, "w") as f:
-            f.write(line + "\n")
+    emit(res, args.out)
 
 
 if __name__ == "__main__":

@@ -18,48 +18,14 @@ the GPU's name and power limit, which belong with the numbers.
 """
 import argparse
 import ctypes
-import json
-import os
-import statistics
-import subprocess
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from bench_common import HOP, LA, L2H_FLAG_GRAPH, emit, gpu_info, median_ms, setup_net
+from lookoncetohear_b200 import synth, _cabi
+from lookoncetohear_b200.configs import TSH_PARAMS
 
-from lookoncetohear_b200 import Net, synth, _cabi  # noqa: E402
-from lookoncetohear_b200.configs import TSH_PARAMS  # noqa: E402
-
-HOP, LA = 128, 64
-L2H_FLAG_GRAPH = 2
 FC = 97 * 64          # floats of one block's h (or c) per record
-
-
-def median_ms(fn, reps, windows=5):
-    """median over `windows` of the device time of `reps` calls of fn, per call (ms)"""
-    out = []
-    for _ in range(windows):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        for i in range(reps):
-            fn(i)
-        b.record()
-        torch.cuda.synchronize()
-        out.append(a.elapsed_time(b) / reps)
-    return statistics.median(out)
-
-
-def gpu_info():
-    info = {"gpu": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30)
-        info["power_limit_and_max_sm_clock"] = q.stdout.strip().splitlines()[0]
-    except (OSError, subprocess.SubprocessError, IndexError):
-        info["power_limit_and_max_sm_clock"] = "unavailable"
-    return info
 
 
 def main():
@@ -68,18 +34,12 @@ def main():
     ap.add_argument("--reps", type=int, default=20, help="calls (catch-up: backlogs) per timed window")
     ap.add_argument("--out", default=None, help="also write the JSON here")
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("bench_slot_frames: needs a CUDA device")
-    dev = torch.device("cuda", 0)
+    net, dev = setup_net("bench_slot_frames")
     S, R = args.slots, args.reps
     catch_up = [(n, k) for n in (1, 4, 16) for k in (2, 4, 8) if n <= S]
     cadence = [(n, T) for n in (64, 256) for T in (1, 2, 4) if n <= S]
     max_t = max([k for _, k in catch_up] + [T for _, T in cadence])
-    torch.manual_seed(0)
-    net = Net(**TSH_PARAMS).eval().to(dev)
-    net._sync_weights(dev)
     L, h = _cabi.lib(), net._engine()
-    st_ptr = torch.cuda.current_stream(dev).cuda_stream
     n_blocks = TSH_PARAMS["B"]
 
     def ws_bytes(n, T):
@@ -97,11 +57,8 @@ def main():
 
     def slot_call(slots, ebuf, n, T, x_off=0):
         """T hops of the n listed rows; x_off: the first hop of x (and y) this call consumes (chained one-hop calls)"""
-        xp, yp = x.data_ptr() + 4 * HOP * x_off, y.data_ptr() + 4 * HOP * x_off
-        _cabi.check(L.l2h_sep_forward_slots_frames(h, xp, x.stride(0), x.stride(1), HOP * T + LA, ebuf.data_ptr(),
-                                                   big.buf.data_ptr(), S, slots.data_ptr(), n, T, yp, y.stride(0),
-                                                   y.stride(1), HOP * T, ws.data_ptr(), ws.numel(), L2H_FLAG_GRAPH,
-                                                   st_ptr))
+        net._launch("slots_frames", x[:n, :, HOP * x_off:HOP * (x_off + T) + LA], ebuf, big,
+                    y[:n, :, HOP * x_off:HOP * (x_off + T)], T, L2H_FLAG_GRAPH, slots=slots, ws=ws)
 
     def lists_for(n):
         lists = torch.stack([torch.randperm(S, generator=g)[:n] for _ in range(R)]).to(dev, torch.int32)
@@ -139,9 +96,7 @@ def main():
             slot_call(slots, ebuf, n, T)
 
         def run_dense(i):
-            _cabi.check(L.l2h_sep_forward(h, x.data_ptr(), x.stride(0), x.stride(1), HOP * T + LA, e.data_ptr(),
-                                          dense.buf.data_ptr(), y.data_ptr(), y.stride(0), y.stride(1), HOP * T, n, T,
-                                          ws.data_ptr(), ws.numel(), L2H_FLAG_GRAPH, st_ptr))
+            net._launch("forward", x[:n, :, :HOP * T + LA], e, dense, y[:n, :, :HOP * T], T, L2H_FLAG_GRAPH, ws=ws)
 
         for fn in (run_slots, run_dense):
             for i in range(R):
@@ -155,11 +110,7 @@ def main():
         r["hc_copy_share"] = hc / r["workspace_bytes"]
         res["cadence"][f"n{n}_T{T}"] = r
         del dense
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        with open(args.out, "w") as f:
-            f.write(line + "\n")
+    emit(res, args.out)
 
 
 if __name__ == "__main__":

@@ -12,47 +12,11 @@ Each figure is the median over 5 windows of `--hops` hops timed with CUDA events
 with the GPU's name and power limit, which belong with the numbers.
 """
 import argparse
-import json
-import os
-import statistics
-import subprocess
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-from lookoncetohear_b200 import Net, synth, _cabi  # noqa: E402
-from lookoncetohear_b200.configs import TSH_PARAMS  # noqa: E402
-
-HOP, LA = 128, 64
-L2H_FLAG_GRAPH = 2
-
-
-def median_ms(fn, reps, windows=5):
-    """median over `windows` of the device time of `reps` calls of fn, per call (ms)"""
-    out = []
-    for _ in range(windows):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        for i in range(reps):
-            fn(i)
-        b.record()
-        torch.cuda.synchronize()
-        out.append(a.elapsed_time(b) / reps)
-    return statistics.median(out)
-
-
-def gpu_info():
-    info = {"gpu": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30)
-        info["power_limit_and_max_sm_clock"] = q.stdout.strip().splitlines()[0]
-    except (OSError, subprocess.SubprocessError, IndexError):
-        info["power_limit_and_max_sm_clock"] = "unavailable"
-    return info
+from bench_common import HOP, LA, L2H_FLAG_GRAPH, emit, gpu_info, median_ms, setup_net
+from lookoncetohear_b200 import synth
 
 
 def main():
@@ -61,15 +25,8 @@ def main():
     ap.add_argument("--hops", type=int, default=20, help="hops per timed window")
     ap.add_argument("--out", default=None, help="also write the JSON here")
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("bench_slot_list: needs a CUDA device")
-    dev = torch.device("cuda", 0)
+    net, dev = setup_net("bench_slot_list")
     S, K = args.slots, args.hops
-    torch.manual_seed(0)
-    net = Net(**TSH_PARAMS).eval().to(dev)
-    net._sync_weights(dev)
-    L, h = _cabi.lib(), net._engine()
-    st_ptr = torch.cuda.current_stream(dev).cuda_stream
     g = torch.Generator().manual_seed(7000)
     x = (0.1 * torch.randn(S, 2, HOP + LA, generator=g)).to(dev)
     e = synth.embedding(8, seed0=8000)[:, 0].repeat((S + 7) // 8, 1)[:S].contiguous().to(dev)
@@ -93,20 +50,14 @@ def main():
         def run_slots(i):
             slots.copy_(lists[i % K])
             ebuf.copy_(embs[i % K])
-            _cabi.check(L.l2h_sep_forward_slots(h, x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], ebuf.data_ptr(),
-                                                big.buf.data_ptr(), S, slots.data_ptr(), n, y.data_ptr(), y.stride(0),
-                                                y.stride(1), HOP, ws.data_ptr(), ws.numel(), L2H_FLAG_GRAPH, st_ptr))
+            net._launch("slots", x[:n], ebuf, big, y[:n], 1, L2H_FLAG_GRAPH, slots=slots, ws=ws)
 
         def run_dense(i):
-            _cabi.check(L.l2h_sep_forward(h, x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], e.data_ptr(),
-                                          dense.buf.data_ptr(), y.data_ptr(), y.stride(0), y.stride(1), HOP, n, 1,
-                                          ws.data_ptr(), ws.numel(), L2H_FLAG_GRAPH, st_ptr))
+            net._launch("forward", x[:n], e, dense, y[:n], 1, L2H_FLAG_GRAPH, ws=ws)
 
         def run_mask(i):
             mask.copy_(masks[i % K])
-            _cabi.check(L.l2h_sep_forward_active(h, x.data_ptr(), x.stride(0), x.stride(1), x.shape[-1], e.data_ptr(),
-                                                 big.buf.data_ptr(), y.data_ptr(), y.stride(0), y.stride(1), HOP, S, 1,
-                                                 ws.data_ptr(), ws.numel(), L2H_FLAG_GRAPH, st_ptr, mask.data_ptr()))
+            net._launch("forward_active", x, e, big, y, 1, L2H_FLAG_GRAPH, mask=mask, ws=ws)
 
         for fn in (run_slots, run_dense, run_mask):      # warm: graph capture, every listed slot's gate built
             for i in range(K):
@@ -117,11 +68,7 @@ def main():
         r = res[f"n{n}"]
         r["slots_over_dense"] = r["slots_ms"] / r["dense_ms"]
         del dense
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        with open(args.out, "w") as f:
-            f.write(line + "\n")
+    emit(res, args.out)
 
 
 if __name__ == "__main__":

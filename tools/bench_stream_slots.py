@@ -11,46 +11,11 @@ Reports, as one JSON object, each figure the median of 5 windows timed with CUDA
 and the GPU's name and power limit, which belong with the numbers.
 """
 import argparse
-import json
-import os
-import statistics
-import subprocess
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-from lookoncetohear_b200 import Net, synth  # noqa: E402
-from lookoncetohear_b200.configs import TSH_PARAMS  # noqa: E402
-
-HOP, LA = 128, 64
-
-
-def median_ms(fn, reps, windows=5):
-    """median over `windows` of the device time of `reps` calls of fn, per call (ms)"""
-    out = []
-    for _ in range(windows):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        for i in range(reps):
-            fn(i)
-        b.record()
-        torch.cuda.synchronize()
-        out.append(a.elapsed_time(b) / reps)
-    return statistics.median(out)
-
-
-def gpu_info():
-    info = {"gpu": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30)
-        info["power_limit_and_max_sm_clock"] = q.stdout.strip().splitlines()[0]
-    except (OSError, subprocess.SubprocessError, IndexError):
-        info["power_limit_and_max_sm_clock"] = "unavailable"
-    return info
+from bench_common import HOP, LA, emit, gpu_info, median_ms, setup_net
+from lookoncetohear_b200 import synth
 
 
 def main():
@@ -59,12 +24,8 @@ def main():
     ap.add_argument("--hops", type=int, default=20, help="hops per timed window")
     ap.add_argument("--out", default=None, help="also write the JSON here")
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("bench_stream_slots: needs a CUDA device")
-    dev = torch.device("cuda", 0)
+    net, dev = setup_net("bench_stream_slots")
     B, K = args.streams, args.hops
-    torch.manual_seed(0)
-    net = Net(**TSH_PARAMS).eval().to(dev)
     g = torch.Generator().manual_seed(5000)
     n_hops = K + 10
     x = (0.1 * torch.randn(B, 2, HOP * n_hops + LA, generator=g)).to(dev)
@@ -98,11 +59,7 @@ def main():
     rec_bytes = st.stride * 4
     res["record_bytes"] = rec_bytes
     res["reset_GBps_32"] = 32 * rec_bytes / (res["reset_us_32"] * 1e-6) / 1e9
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        with open(args.out, "w") as f:
-            f.write(line + "\n")
+    emit(res, args.out)
 
 
 if __name__ == "__main__":

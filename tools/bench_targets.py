@@ -14,65 +14,16 @@ shape (max relative L2 over the target rows).  Printed as one JSON object with t
 clock, which belong with the numbers.
 """
 import argparse
-import json
-import os
-import statistics
-import subprocess
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from bench_common import HOP, LA, L2H_FLAG_GRAPH, alternate, emit, gpu_info, rel_l2, setup_net
+from lookoncetohear_b200 import synth
 
-from lookoncetohear_b200 import Net, synth, _cabi  # noqa: E402
-from lookoncetohear_b200.configs import TSH_PARAMS  # noqa: E402
-
-HOP, LA = 128, 64
-L2H_FLAG_GRAPH = 2
 HOP_CASES = [(1, 2), (1, 3), (16, 2), (64, 2), (64, 3), (128, 2)]
 
 
-def window_ms(fn, reps):
-    """device time of `reps` calls of fn, per call (ms)"""
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for i in range(reps):
-        fn(i)
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / reps
-
-
-def alternate(fa, fb, reps, windows=5):
-    """medians of `windows` windows of fa and fb, timed alternately"""
-    ta, tb = [], []
-    for _ in range(windows):
-        ta.append(window_ms(fa, reps))
-        tb.append(window_ms(fb, reps))
-    return statistics.median(ta), statistics.median(tb)
-
-
-def gpu_info():
-    info = {"gpu": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30)
-        info["power_limit_and_max_sm_clock"] = q.stdout.strip().splitlines()[0]
-    except (OSError, subprocess.SubprocessError, IndexError):
-        info["power_limit_and_max_sm_clock"] = "unavailable"
-    return info
-
-
-def rel_l2(a, b):
-    """max over rows of ||a - b|| / ||b||"""
-    a, b = a.reshape(a.shape[0], -1).double(), b.reshape(b.shape[0], -1).double()
-    return float(((a - b).norm(dim=1) / b.norm(dim=1)).max())
-
-
 def one_hop(net, dev, M, K, reps):
-    L, h = _cabi.lib(), net._engine()
-    st_ptr = torch.cuda.current_stream(dev).cuda_stream
     n = M * K
     x, _ = synth.mixture(M, HOP * (reps + 1), seed0=9000)
     x = torch.nn.functional.pad(x, (0, LA)).to(dev)
@@ -85,15 +36,11 @@ def one_hop(net, dev, M, K, reps):
 
     def run_targets(i):
         xb.copy_(x[..., HOP * (i % reps):HOP * (i % reps) + HOP + LA])
-        _cabi.check(L.l2h_sep_forward_targets(h, xb.data_ptr(), xb.stride(0), xb.stride(1), HOP + LA, e.data_ptr(),
-                                              st_t.buf.data_ptr(), yt.data_ptr(), yt.stride(1), yt.stride(2), HOP, M, K,
-                                              1, ws.data_ptr(), ws.numel(), L2H_FLAG_GRAPH, st_ptr))
+        net._launch("targets", xb, e, st_t, yt, 1, L2H_FLAG_GRAPH, K=K, ws=ws)
 
     def run_dense(i):
         xbd.copy_(xd[..., HOP * (i % reps):HOP * (i % reps) + HOP + LA])
-        _cabi.check(L.l2h_sep_forward(h, xbd.data_ptr(), xbd.stride(0), xbd.stride(1), HOP + LA, e.data_ptr(),
-                                      st_d.buf.data_ptr(), yd.data_ptr(), yd.stride(0), yd.stride(1), HOP, n, 1,
-                                      ws.data_ptr(), ws.numel(), L2H_FLAG_GRAPH, st_ptr))
+        net._launch("forward", xbd, e, st_d, yd, 1, L2H_FLAG_GRAPH, ws=ws)
 
     err = 0.0
     for i in range(reps):                      # warm-up from fresh states, in step: the outputs must agree
@@ -101,7 +48,7 @@ def one_hop(net, dev, M, K, reps):
         run_dense(i)
         err = max(err, rel_l2(yt.reshape(n, 2, HOP), yd))
     torch.cuda.synchronize()
-    t_ms, d_ms = alternate(run_targets, run_dense, reps)
+    t_ms, d_ms = alternate({"t": run_targets, "d": run_dense}, reps).values()
     return {"targets_ms": t_ms, "dense_ms": d_ms, "targets_over_dense": t_ms / d_ms, "max_rel_l2": err}
 
 
@@ -123,7 +70,7 @@ def offline(net, dev, M, K, seconds):
         run_dense(0)
         torch.cuda.synchronize()
         err = rel_l2(out["t"].reshape(M * K, 2, -1), out["d"])
-        t_ms, d_ms = alternate(run_targets, run_dense, 1)
+        t_ms, d_ms = alternate({"t": run_targets, "d": run_dense}, 1).values()
     return {"targets_ms": t_ms, "dense_ms": d_ms, "targets_over_dense": t_ms / d_ms, "max_rel_l2": err}
 
 
@@ -132,22 +79,13 @@ def main():
     ap.add_argument("--hops", type=int, default=20, help="hops per timed window")
     ap.add_argument("--out", default=None, help="also write the JSON here")
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("bench_targets: needs a CUDA device")
-    dev = torch.device("cuda", 0)
-    torch.manual_seed(0)
-    net = Net(**TSH_PARAMS).eval().to(dev)
-    net._sync_weights(dev)
+    net, dev = setup_net("bench_targets")
     res = dict(gpu_info(), hops_per_window=args.hops)
     with torch.no_grad():
         for M, K in HOP_CASES:
             res[f"hop_{M}x{K}"] = one_hop(net, dev, M, K, args.hops)
     res["offline_32x3_4s"] = offline(net, dev, 32, 3, 4)
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        with open(args.out, "w") as f:
-            f.write(line + "\n")
+    emit(res, args.out)
 
 
 if __name__ == "__main__":

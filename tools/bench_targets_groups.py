@@ -17,69 +17,19 @@ their outputs are compared during the warm-up (max relative L2 over target rows)
 GPU's name, power limit and max SM clock, which belong with the numbers.
 """
 import argparse
-import json
-import os
-import statistics
-import subprocess
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from bench_common import HOP, LA, L2H_FLAG_GRAPH, alternate, emit, gpu_info, rel_l2, setup_net
+from lookoncetohear_b200 import synth
 
-from lookoncetohear_b200 import Net, synth, _cabi  # noqa: E402
-from lookoncetohear_b200.configs import TSH_PARAMS  # noqa: E402
-
-HOP, LA = 128, 64
-L2H_FLAG_GRAPH = 2
 STATES = {2: 256, 3: 255}                      # records per state: 128 groups of 2, 85 groups of 3
 CASES = [(8, 2), (32, 2), (64, 2), (128, 2), (8, 3), (32, 3), (64, 3)]
 RAGGED = (32, 2, 4)                            # (n, K, T)
 TICKS = 8                                      # distinct precomputed ticks, cycled
 
 
-def window_ms(fn, reps):
-    """device time of `reps` calls of fn, per call (ms)"""
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for i in range(reps):
-        fn(i)
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / reps
-
-
-def alternate(fns, reps, windows=5):
-    """medians of `windows` windows of every fn, timed in turn"""
-    t = {k: [] for k in fns}
-    for _ in range(windows):
-        for k, fn in fns.items():
-            t[k].append(window_ms(fn, reps))
-    return {k: statistics.median(v) for k, v in t.items()}
-
-
-def gpu_info():
-    info = {"gpu": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30)
-        info["power_limit_and_max_sm_clock"] = q.stdout.strip().splitlines()[0]
-    except (OSError, subprocess.SubprocessError, IndexError):
-        info["power_limit_and_max_sm_clock"] = "unavailable"
-    return info
-
-
-def rel_l2(a, b):
-    """max over rows of ||a - b|| / ||b||, over the rows b has written"""
-    a, b = a.reshape(a.shape[0], -1).double(), b.reshape(b.shape[0], -1).double()
-    nb = b.norm(dim=1)
-    live = nb > 0
-    return float(((a - b).norm(dim=1)[live] / nb[live]).max()) if bool(live.any()) else 0.0
-
-
 def case(net, dev, n, K, T, reps, ragged):
-    L, h, sp = _cabi.lib(), net._engine(), torch.cuda.current_stream(dev).cuda_stream
     S = STATES[K]
     G = S // K
     g = torch.Generator().manual_seed(9400 + 10 * n + K)
@@ -109,25 +59,18 @@ def case(net, dev, n, K, T, reps, ragged):
     def run_groups(i):
         j = i % TICKS
         xb.copy_(xa[j]); eb.copy_(ea[j]); gb.copy_(groups[j]); hab.copy_(hops_a[j])
-        _cabi.check(L.l2h_sep_forward_targets_groups(
-            h, xb.data_ptr(), xb.stride(0), xb.stride(1), xb.shape[-1], eb.data_ptr(), st_a.buf.data_ptr(), S, gb.data_ptr(),
-            hab.data_ptr() if ragged else None, n, K, T, ya.data_ptr(), ya.stride(1), ya.stride(2), HOP * T, ws.data_ptr(),
-            ws.numel(), L2H_FLAG_GRAPH, sp))
+        net._launch("targets_groups", xb, eb, st_a, ya, T, L2H_FLAG_GRAPH, slots=gb, hops=hab if ragged else None, K=K,
+                    ws=ws)
 
     def run_dense(i):          # the dense state's rows are the same n groups every tick: their embeddings stay put
         j = i % TICKS
         xb.copy_(xa[j]); eb.copy_(ea[0])
-        _cabi.check(L.l2h_sep_forward_targets(
-            h, xb.data_ptr(), xb.stride(0), xb.stride(1), xb.shape[-1], eb.data_ptr(), st_b.buf.data_ptr(), yb.data_ptr(),
-            yb.stride(1), yb.stride(2), HOP * T, n, K, T, ws.data_ptr(), ws.numel(), L2H_FLAG_GRAPH, sp))
+        net._launch("targets", xb, eb, st_b, yb, T, L2H_FLAG_GRAPH, K=K, ws=ws)
 
     def run_slots(i):
         j = i % TICKS
         xcb.copy_(xc[j]); eb.copy_(ea[j]); slb.copy_(slots[j]); hcb.copy_(hops_c[j])
-        _cabi.check(L.l2h_sep_forward_slots_hops(
-            h, xcb.data_ptr(), xcb.stride(0), xcb.stride(1), xcb.shape[-1], eb.data_ptr(), st_c.buf.data_ptr(), S,
-            slb.data_ptr(), hcb.data_ptr() if ragged else None, n * K, T, yc.data_ptr(), yc.stride(0), yc.stride(1),
-            HOP * T, ws.data_ptr(), ws.numel(), L2H_FLAG_GRAPH, sp))
+        net._launch("slots_hops", xcb, eb, st_c, yc, T, L2H_FLAG_GRAPH, slots=slb, hops=hcb if ragged else None, ws=ws)
 
     err = 0.0
     for i in range(reps):                      # warm-up (graph capture, gate memos), (a) and (c) in step
@@ -155,23 +98,14 @@ def main():
     ap.add_argument("--hops", type=int, default=20, help="ticks per timed window")
     ap.add_argument("--out", default=None, help="also write the JSON here")
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("bench_targets_groups: needs a CUDA device")
-    dev = torch.device("cuda", 0)
-    torch.manual_seed(0)
-    net = Net(**TSH_PARAMS).eval().to(dev)
-    net._sync_weights(dev)
+    net, dev = setup_net("bench_targets_groups")
     res = dict(gpu_info(), ticks_per_window=args.hops)
     with torch.no_grad():
         for n, K in CASES:
             res[f"hop_n{n}_K{K}"] = case(net, dev, n, K, 1, args.hops, False)
         n, K, T = RAGGED
         res[f"ragged_n{n}_K{K}_T{T}"] = case(net, dev, n, K, T, args.hops, True)
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        with open(args.out, "w") as f:
-            f.write(line + "\n")
+    emit(res, args.out)
 
 
 if __name__ == "__main__":
