@@ -253,24 +253,15 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
     int32_t* lens = nullptr;
     if (mixed) {
         lens = reinterpret_cast<int32_t*>(wsp + ws.LENS);
-        for (int b0 = 0; b0 < B; b0 += LENS_PER_LAUNCH) {
-            const int n = std::min(LENS_PER_LAUNCH, B - b0);
-            LensBlock blk;
-            memcpy(blk.v, lens_host + b0, sizeof(int32_t) * n);
-            eput_lens_kernel<<<1, 256, 0, st>>>(lens + b0, blk, n);
-            CK(cudaGetLastError());
-        }
+        CK(launch_eput_lens(st, lens, lens_host, B));
     }
 
-    estd_kernel<<<B, 256, 0, st>>>(x, N, lens, INV);
-    CK(cudaGetLastError());
+    CK(launch_estd(st, B, x, N, lens, INV));
     CK(cudaMemsetAsync(GN, 0, sizeof(double) * 2 * B, st));
-    efront_kernel<<<dim3(T, B), 256, 0, st>>>(x, N, lens, INV, X, GN, e->w, T);
-    CK(cudaGetLastError());
+    CK(launch_efront(st, B, x, N, lens, INV, X, GN, e->w, T));
     {
         const int64_t per_b = (int64_t)T * NF * CH, total4 = (int64_t)B * per_b / 4;
-        egn_apply_kernel<<<(unsigned)((total4 + 255) / 256), 256, 0, st>>>(X, GN, per_b, total4, lens, e->w);
-        CK(cudaGetLastError());
+        CK(launch_egn_apply(st, X, GN, per_b, total4, lens, e->w));
     }
 
     for (int blk = 0; blk < e->n_blocks; ++blk) {
@@ -297,10 +288,8 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
             g.b = pk.bplanes(inter ? PL.ih2 : PL.ih1, 256); g.N = 512; g.K = 256; g.passes = passes;
             g.bias = inter ? W.b2 : W.b1; g.C = GX; g.ldc = 512; g.c_seq_stride = (int64_t)steps * 512;
             CKU(umma::launch(g, st, &_why));
-            if (inter && lens != nullptr) {             // windows past an utterance's own frames: zero state, zero h
-                einter_mask_kernel<<<dim3(NF, B), 128, 0, st>>>(GX, lens, steps);
-                CK(cudaGetLastError());
-            }
+            // windows past an utterance's own frames: zero state, zero h
+            if (inter && lens != nullptr) CK(launch_einter_mask(st, B, GX, lens, steps));
             LstmArgs l{};
             l.gx = GX; l.gx_ld = 512; l.out = HC; l.out_ld = 128; l.whh = inter ? W.whh2 : W.whh1;
             l.nseq = nseq; l.L = steps; l.inner_count = 1; l.outer_stride = steps; l.inner_stride = 0; l.step_stride = 1;
@@ -332,8 +321,7 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
             g.bias = W.bqkv; g.prelu_vec = W.slope_qkv; g.C = QKV; g.ldc = NQKV; g.c_seq_stride = 0;
             CKU(umma::launch(g, st, &_why));
         }
-        eqkv_ln_kernel<<<dim3(T, B), 384, 0, st>>>(QKV, QN, KP, VP, k_plane, v_plane, W, T, Tp);
-        CK(cudaGetLastError());
+        CK(launch_eqkv_ln(st, B, QKV, QN, KP, VP, k_plane, v_plane, W, T, Tp));
         {
             umma::GemmDesc g;                          // S = Q K^T / sqrt(520), per (utterance, head)
             g.a0.base = QN; g.a0.channels = QK; g.a0.n_pos = T; g.a0.pos_stride = QK; g.a0.n_inner = Z; g.a0.inner_stride = (int64_t)Tp * QK;
@@ -344,8 +332,7 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
             g.C = S; g.ldc = Tp; g.c_seq_stride = (int64_t)T * Tp;
             CKU(umma::launch(g, st, &_why));
         }
-        softmax_rows_kernel<<<(unsigned)((int64_t)Z * T), 128, 0, st>>>(S, Tp, T, T, (int64_t)T * Tp, lens);
-        CK(cudaGetLastError());
+        CK(launch_softmax_rows(st, Z, S, Tp, T, T, (int64_t)T * Tp, lens));
         {
             umma::GemmDesc g;                          // O = P V (V is the MN-major B operand: [frame][f*16+c])
             g.a0.base = S; g.a0.channels = T; g.a0.n_pos = T; g.a0.pos_stride = Tp; g.a0.n_inner = Z; g.a0.inner_stride = (int64_t)T * Tp;
@@ -356,8 +343,7 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
             g.C = O; g.ldc = VDIM; g.c_seq_stride = (int64_t)Tp * VDIM;
             CKU(umma::launch(g, st, &_why));
         }
-        eattn_out_kernel<<<dim3((unsigned)std::min<int64_t>((int64_t)T * B, NUM_SMS * 4)), 256, EAOUT_SMEM, st>>>(O, X, W, T, Tp, T * B);
-        CK(cudaGetLastError());
+        CK(launch_eattn_out(st, eattn_out_ctas(T, B), O, X, W, T, Tp, T * B));
     }
     // ---- head: Linear(4160 -> 256) over rows (b,t) [features f*64+c], LN, mean over T -----------
     {
@@ -369,8 +355,7 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
         g.bias = e->w.bh; g.C = HD; g.ldc = 256;
         CKU(umma::launch(g, st, &_why));
     }
-    ehead_kernel<<<B, 256, 0, st>>>(HD, out, e->w, T, lens);
-    CK(cudaGetLastError());
+    CK(launch_ehead(st, B, HD, out, e->w, T, lens));
     return 0;
 }
 

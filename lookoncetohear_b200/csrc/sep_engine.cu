@@ -354,8 +354,8 @@ struct ChainForm {
     bool walkers;       // front_many_kernel / back_many_kernel: CTAs (clusters) walk (stream, chunk-of-frames) items
     bool qkv_many;      // many frames: the persistent qkv_many_kernel, on at most qkv_ctas CTAs (one wave)
     int qkv_ctas;
-    bool attn_tiled;    // enough query tiles to fill the GPU: attn_tile_kernel (one pass over 57 rows serves 8 queries)
-    int nsplit;         // attn_splits
+    AttnForm attn;      // clusters while they fit one wave (attn_splits), else attn_tile_kernel where enough query tiles fill the
+                        // GPU (one pass over 57 rows serves 8 queries), else attn_kernel
     RecForm intra, inter;
     // programmatic dependent launch pays on the latency chain of a few rows; with many rows early-launched dependents park
     // on the SMs the big kernels need, so tensor-core chains take it only where option "tc_pdl" asks: bit 0 the many-stream
@@ -377,8 +377,8 @@ static ChainForm chain_form(const SepEngine* e, int B, int T, uint32_t flags, bo
         static int wave[64] = {};
         f.qkv_ctas = resident_ctas(wave, qkv_many_kernel_t<Map>, QKV_THREADS, QKV_MANY_SMEM);
     }
-    f.attn_tiled = T > 1 && (int64_t)B * NHEAD * ((T + ATT_TQ - 1) / ATT_TQ) >= NUM_SMS;
-    f.nsplit = attn_splits(B, T);
+    const bool attn_tiled = T > 1 && (int64_t)B * NHEAD * ((T + ATT_TQ - 1) / ATT_TQ) >= NUM_SMS;
+    f.attn = attn_splits(B, T) > 1 ? AttnForm::cluster : attn_tiled ? AttnForm::tile : AttnForm::query;
     const auto rec = [e](int64_t seqdirs) { const bool tc = seqdirs >= e->tcl_min_seqdirs; return RecForm{tc, tc && e->fuse_ih}; };
     f.intra = rec((int64_t)B * T * 2);      // (stream, frame) sequences over F, both directions
     f.inter = rec((int64_t)B * NF);         // (stream, bin) sequences over T
@@ -600,15 +600,14 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
     const BlockRows<Map> R0 = c.rows_of(0);           // the front runs over block 0's rows
     const int gate_ctas = c.K > 1 ? 0 : 1;            // the front's speaker-gate memo CTAs (one per row); fan_out() builds them here
     if (f.fused_tail) {      // the frame as 13 row tiles: spectrum of the tile's bins, conv, and block 0's input projection
-        CK(launch_k(false, front1_kernel_t<Map>, dim3(TAIL_TILES + gate_ctas, R0.B), dim3(256), FRONT1_SMEM, st, a.x, a.xbs, a.xcs, a.x_len,
-                    R0.X, a.state, R0.recs, e->w, e->bw[0], c.GX, a.pos_rel, a.emb, c.PRE, a.active));
+        CK(launch_front1(false, st, R0.B, gate_ctas, a.x, a.xbs, a.xcs, a.x_len, R0.X, a.state, R0.recs, e->w, e->bw[0], c.GX, a.pos_rel,
+                         a.emb, c.PRE, a.active));
     } else if (f.walkers) {
-        const ChunkWalk g = front_many_walk(R0.B, T);
-        CK(launch_k(false, front_many_kernel_t<Map>, dim3(g.workers + gate_ctas * R0.B, 1), dim3(256), FRONT_SMEM, st, a.x, a.xbs, a.xcs,
-                    a.x_len, R0.X, a.state, R0.recs, e->w, T, a.pos_rel, a.emb, c.PRE, g.chunk, g.n_chunks, R0.B, g.workers, a.active));
+        CK(launch_front_many(false, st, gate_ctas, front_many_walk(R0.B, T), a.x, a.xbs, a.xcs, a.x_len, R0.X, a.state, R0.recs, e->w, T,
+                             a.pos_rel, a.emb, c.PRE, R0.B, a.active));
     } else {
-        CK(launch_k(false, front_kernel_t<Map>, dim3(T + gate_ctas, R0.B), dim3(256), FRONT_SMEM, st, a.x, a.xbs, a.xcs, a.x_len, R0.X,
-                    a.state, R0.recs, e->w, T, a.pos_rel, a.emb, c.PRE, 0, 1, 0, a.active));
+        CK(launch_front(false, st, R0.B, gate_ctas, a.x, a.xbs, a.xcs, a.x_len, R0.X, a.state, R0.recs, e->w, T, a.pos_rel, a.emb, c.PRE,
+                        0, 1, 0, a.active));
     }
     MARK("front");
     if (int rc = c.do_tap()) return rc;
@@ -654,10 +653,9 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
             MARK("mid");
         } else if (f.row_mid && f.mid_split) {
             float* GI = c.GX; float* HN = c.GX + R.rows * 256;         // the BiLSTM is done with GX
-            CK(launch_k(f.pdl, mid_a_kernel, mid_grid_for(R.B, 2), dim3(256), MID_A_SMEM, st, (const float*)c.Y, R.X, GI, W, R.B, (int64_t)0, 1));
-            CK(launch_k(f.pdl, mid_b_kernel_t<Map>, mid_grid_for(R.B, 3), dim3(256), MID_B_SMEM, st, (const float*)GI, HN, (int64_t)0, 1, a.state,
-                        R.recs, b, W, R.B, a.active));
-            CK(launch_k(f.pdl, mid_c_kernel, mid_grid_for(R.B, 4), dim3(256), MID_C_SMEM, st, (const float*)HN, R.X, c.QKVRAW, W, R.B, (int64_t)0, 1));
+            CK(launch_mid_a(f.pdl, st, c.Y, R.X, GI, W, R.B, 0, 1));
+            CK(launch_mid_b(f.pdl, st, GI, HN, 0, 1, a.state, R.recs, b, W, R.B, a.active));
+            CK(launch_mid_c(f.pdl, st, HN, R.X, c.QKVRAW, W, R.B, 0, 1));
             MARK("mid");
         } else if (f.fused_tail) {
             NextIh nx{};      // the next block's input projection, where that block reads it from GX
@@ -693,8 +691,7 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
         }
         // ---- attention --------------------------------------------------------------------------
         if (T > 1) {
-            CK(launch_k(f.pdl, kv_gather_kernel_t<Map>, dim3(ATT - 1, R.B * NHEAD), dim3(128), 0, st, (const float*)a.state, R.recs, b, c.KALL,
-                        c.VALL, T));
+            CK(launch_kv_gather(f.pdl, st, R.B, a.state, R.recs, b, c.KALL, c.VALL, T));
             MARK("kv_gather");
         }
         if (f.tc && !f.tc_mid) {      // Q|K|V projections of all rows as one tensor-core GEMM (+ bias + PReLU per column)
@@ -702,46 +699,31 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
                                       st, false)) return rc;
         }
         if (f.qkv_many) {      // many frames: persistent form (LayerNorm parameters staged once per CTA), one wave
-            const int64_t grid_q = std::min<int64_t>(f.qkv_ctas, (int64_t)R.B * T);
-            CK(launch_k(f.qkv_pdl, qkv_many_kernel_t<Map>, dim3((unsigned)grid_q), dim3(QKV_THREADS), QKV_MANY_SMEM, st, (const float*)c.QKVRAW,
-                        c.Q, c.KALL, c.VALL, a.state, R.recs, b, W, T, R.B * T, a.active));
+            const int grid_q = (int)std::min<int64_t>(f.qkv_ctas, (int64_t)R.B * T);
+            CK(launch_qkv_many(f.qkv_pdl, st, grid_q, c.QKVRAW, c.Q, c.KALL, c.VALL, a.state, R.recs, b, W, T, R.B * T, a.active));
         } else {
             const bool pre = f.tc || f.row_mid;      // the projections are in QKVRAW already
-            CK(launch_k(f.pdl, qkv_kernel_t<Map>, dim3(T, R.B), dim3(QKV_THREADS), pre ? QKV_PRE_SMEM : QKV_SMEM, st, (const float*)R.X,
-                        (const float*)(pre ? c.QKVRAW : nullptr), c.Q, c.KALL, c.VALL, a.state, R.recs, b, W, T, 0, a.active));
+            CK(launch_qkv(f.pdl, st, R.B, R.X, pre ? c.QKVRAW : nullptr, c.Q, c.KALL, c.VALL, a.state, R.recs, b, W, T, 0, a.active));
         }
         MARK("qkv");
-        if (f.nsplit > 1) {
-            CK(launch_cluster(f.pdl, dim3(1, ATT_CL, 1), attn_cluster_kernel_t<Map>, dim3(T, NHEAD * ATT_CL, R.B), dim3(256), 0, st,
-                              (const float*)c.Q, (const float*)c.KALL, (const float*)c.VALL, (const float*)a.state, R.recs, b, c.Z, T, 0));
-        } else if (f.attn_tiled) {
-            CK(launch_k(f.pdl, attn_tile_kernel, dim3((T + ATT_TQ - 1) / ATT_TQ, NHEAD, R.B), dim3(256), 0, st, (const float*)c.Q,
-                        (const float*)c.KALL, (const float*)c.VALL, c.Z, T));
-        } else {
-            CK(launch_k(f.pdl, attn_kernel_t<Map>, dim3(T, NHEAD, R.B), dim3(256), 0, st, (const float*)c.Q, (const float*)c.KALL,
-                        (const float*)c.VALL, (const float*)a.state, R.recs, b, c.Z, T, 0));
-        }
+        CK(launch_attention(f.attn, f.pdl, st, R.B, c.Q, c.KALL, c.VALL, a.state, R.recs, b, c.Z, T, 0));
         MARK("attn");
         if (f.tc) {      // Linear(64->64) + PReLU of all rows on the tensor cores, then LayerNorm(6208) + residual (+ gate) per frame
             if (int rc = tc_rows_gemm(e, b, PL_P, c.Z, 64, 64, 64, nullptr, nullptr, W.bp, nullptr, nullptr, c.Y, 64, R.rows, st, f.gemm_pdl,
                                       W.slopes + 3)) return rc;
-            CK(launch_k(f.gemm_pdl, ln_frame_res_kernel_t<Map>, dim3(T, R.B), dim3(256), 0, st, (const float*)c.Y, R.X, (const float*)a.state,
-                        R.recs, W, R.gate, T));
+            CK(launch_ln_frame_res(f.gemm_pdl, st, R.B, c.Y, R.X, a.state, R.recs, W, R.gate, T));
         } else {
-            CK(launch_k(f.pdl, attn_out_kernel_t<Map>, dim3(T, R.B), dim3(256), AOUT_SMEM, st, (const float*)c.Z, R.X, (const float*)a.state,
-                        R.recs, W, R.gate, T));
+            CK(launch_attn_out(f.pdl, st, R.B, c.Z, R.X, a.state, R.recs, W, R.gate, T));
         }
         MARK("attn_out");
         if (int rc = c.do_tap()) return rc;
     }
     if (c.fans_out_before(e->n_blocks)) { if (int rc = c.fan_out()) return rc; }
     if (f.walkers) {
-        const ChunkWalk g = back_many_walk(a.B, T);
-        CK(launch_cluster(f.pdl, dim3(BACK_CL, 1, 1), back_many_kernel_t<Map>, dim3(BACK_CL * g.workers, 1), dim3(256), BACK_MANY_SMEM, st,
-                          (const float*)c.X, a.y, a.ybs, a.ycs, a.y_len, a.state, recs, e->w, T, a.pos_rel, g.chunk, g.n_chunks, a.B, a.active));
+        CK(launch_back_many(f.pdl, st, back_many_walk(a.B, T), c.X, a.y, a.ybs, a.ycs, a.y_len, a.state, recs, e->w, T, a.pos_rel, a.B,
+                            a.active));
     } else {
-        CK(launch_cluster(f.pdl, dim3(BACK_CL, 1, 1), back_kernel_t<Map>, dim3(BACK_CL * T, a.B), dim3(256), BACK_SMEM, st, (const float*)c.X,
-                          a.y, a.ybs, a.ycs, a.y_len, a.state, recs, e->w, T, a.pos_rel, 0, 1, 0, (int64_t)0, a.active));
+        CK(launch_back(f.pdl, st, a.B, c.X, a.y, a.ybs, a.ycs, a.y_len, a.state, recs, e->w, T, a.pos_rel, 0, 1, 0, 0, a.active));
     }
     MARK("back");
     return 0;
@@ -811,7 +793,7 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
     if ((size_t)slot * K * sizeof(float) > a.ws_bytes) return fail(1, "workspace too small for the pipelined stream");
     const int64_t ss = stream_stride(e->n_blocks);
     const int rows = B * NF;
-    const int nsplit = attn_splits(B, 1);
+    const AttnForm attn = attn_splits(B, 1) > 1 ? AttnForm::cluster : AttnForm::query;
     // programmatic dependent launch, per stage: the kernel's prologue (weight staging) overlaps its stream predecessor's
     // tail; every kernel reaches griddepcontrol.wait before it touches activations or state.  Off by default: a parked
     // dependent holds shared memory and CTA slots the running kernels need, on the serial stage too (mid_b -> mid_b of the
@@ -888,9 +870,8 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
                         // position the device derives from the state header)
                         cudaStream_t sF = sFront(k);
                         // the speaker-gate memo CTA (blockIdx.x == 1) rides with hop 0 only: one builder of ST_GATE per group
-                        CK(launch_k((ppdl & 1) != 0, front_kernel, dim3(k == 0 ? 2 : 1, B), dim3(256), FRONT_SMEM, sF, a.x, a.xbs, a.xcs,
-                                    a.x_len, a.wsp + (int64_t)k * slot + ws.X, state, ss, e->w, 1, a.pos_rel, a.emb, PRE, k, K, k * HOP,
-                                    all_active));
+                        CK(launch_front((ppdl & 1) != 0, sF, B, k == 0 ? 1 : 0, a.x, a.xbs, a.xcs, a.x_len, a.wsp + (int64_t)k * slot + ws.X,
+                                        state, ss, e->w, 1, a.pos_rel, a.emb, PRE, k, K, k * HOP, all_active));
                         if (k == 0) {                  // ... and every attn_out lane of block 0 (the gate's only reader) waits for it once
                             cudaEvent_t gate_ev;
                             if (int rc = record(&gate_ev, sF)) return rc;
@@ -914,7 +895,7 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
                 // only the W_hh product + cell (mid_b) is serial per block; the rest rides on the parallel lanes.
                 // GI / H' live in the hop's GX slot, which the BiLSTM has finished with.  One CTA per (stream, row
                 // tile) walks the batch's hops: its 100 KB of weights are staged once per batch, not once per hop.
-                CK(launch_k((ppdl & 8) != 0, mid_a_kernel, mid_grid_for(B, 2), dim3(256), MID_A_SMEM, st_a, (const float*)Y, X, GX, W, B, slot, nh));
+                CK(launch_mid_a((ppdl & 8) != 0, st_a, Y, X, GX, W, B, slot, nh));
                 cudaEvent_t ev_a;
                 if (int rc = record(&ev_a, st_a)) return rc;
                 for (int k = k0; k < k1; ++k) a_done[b][k] = ev_a;
@@ -924,8 +905,7 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
             {
                 float* wsp = a.wsp + (int64_t)k0 * slot;
                 float* GI = wsp + ws.GX; float* HN = GI + (int64_t)rows * 256;
-                CK(launch_k((ppdl & 16) != 0, mid_b_kernel, mid_grid_for(B, 3), dim3(256), MID_B_SMEM, sB1(b), (const float*)GI, HN, slot,
-                            k1 - k0, state, ss, b, W, B, all_active));
+                CK(launch_mid_b((ppdl & 16) != 0, sB1(b), GI, HN, slot, k1 - k0, state, ss, b, W, B, all_active));
             }
             cudaEvent_t midb_done;
             if (int rc = record(&midb_done, sB1(b))) return rc;
@@ -933,8 +913,8 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
             cudaStream_t st_c = sBc(b, k0 / mb);
             float* wsp0 = a.wsp + (int64_t)k0 * slot;
             CK(cudaStreamWaitEvent(st_c, midb_done, 0));
-            CK(launch_k((ppdl & 32) != 0, mid_c_kernel, mid_grid_for(B, 4), dim3(256), MID_C_SMEM, st_c,      // as mid_a: a CTA walks the hops of its tile
-                        (const float*)(wsp0 + ws.GX + (int64_t)rows * 256), wsp0 + ws.X, wsp0 + ws.QKVRAW, W, B, slot, k1 - k0));
+            CK(launch_mid_c((ppdl & 32) != 0, st_c, wsp0 + ws.GX + (int64_t)rows * 256, wsp0 + ws.X, wsp0 + ws.QKVRAW, W, B, slot,
+                            k1 - k0));      // as mid_a: a CTA walks the hops of its tile
             cudaEvent_t midc_done;
             if (int rc = record(&midc_done, st_c)) return rc;
             for (int k = k0; k < k1; ++k) {
@@ -946,24 +926,15 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
                 // attention (one per attention lane) must be done
                 for (int d = 0; d < e->pipe_tlanes && k - PIPE_QKV_AHEAD - 1 - d >= 0; ++d)
                     CK(cudaStreamWaitEvent(st_q, att_done[b][k - PIPE_QKV_AHEAD - 1 - d], 0));
-                CK(launch_k((ppdl & 64) != 0, qkv_kernel, dim3(1, B), dim3(QKV_THREADS), QKV_PRE_SMEM, st_q, (const float*)X,
-                            (const float*)QKVRAW, Q, (float*)nullptr, (float*)nullptr, state, ss, b, W, 1, k, all_active));
+                CK(launch_qkv((ppdl & 64) != 0, st_q, B, X, QKVRAW, Q, nullptr, nullptr, state, ss, b, W, 1, k, all_active));
                 if (int rc = record(&qkv_done[b][k], st_q)) return rc;
                 // the attention reads this hop's ring row and the 49 before it: the other qkv lanes' latest hops must be in
                 cudaStream_t st_t = sBa(b, k);
                 for (int d = 0; d < e->pipe_qlanes && d <= k; ++d) CK(cudaStreamWaitEvent(st_t, qkv_done[b][k - d], 0));
-                if (nsplit > 1) {
-                    CK(launch_cluster((ppdl & 128) != 0, dim3(1, ATT_CL, 1), attn_cluster_kernel, dim3(1, NHEAD * ATT_CL, B),
-                                      dim3(256), 0, st_t, (const float*)Q, (const float*)nullptr, (const float*)nullptr,
-                                      (const float*)state, ss, b, Z, 1, k));
-                } else {
-                    CK(launch_k((ppdl & 128) != 0, attn_kernel, dim3(1, NHEAD, B), dim3(256), 0, st_t, (const float*)Q,
-                                (const float*)nullptr, (const float*)nullptr, (const float*)state, ss, b, Z, 1, k));
-                }
+                CK(launch_attention(attn, (ppdl & 128) != 0, st_t, B, Q, nullptr, nullptr, state, ss, b, Z, 1, k));
                 if (int rc = record(&att_done[b][k], st_t)) return rc;
                 CK(cudaStreamWaitEvent(sBo(b, k), att_done[b][k], 0));
-                CK(launch_k((ppdl & 256) != 0, attn_out_kernel, dim3(1, B), dim3(256), AOUT_SMEM, sBo(b, k), (const float*)Z, X,
-                            (const float*)state, ss, W, b == 0 ? 1 : 0, 1));
+                CK(launch_attn_out((ppdl & 256) != 0, sBo(b, k), B, Z, X, state, ss, W, b == 0 ? 1 : 0, 1));
                 if (int rc = record(&out_done[b][k], sBo(b, k))) return rc;
             }
         }
@@ -972,9 +943,8 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
             cudaStream_t sBack = sBackL(k);
             // this hop's output and the three before it (deconv / overlap-add context) sit on different attn_out lanes
             for (int d = 0; d <= 3 && d <= k; ++d) CK(cudaStreamWaitEvent(sBack, out_done[2][k - d], 0));
-            CK(launch_cluster((ppdl & 512) != 0, dim3(BACK_CL, 1, 1), back_kernel, dim3(BACK_CL, B), dim3(256), BACK_SMEM, sBack,
-                              (const float*)X, a.y, a.ybs, a.ycs, a.y_len, state, ss, e->w, 1, a.pos_rel, k, K, k * HOP, slot,
-                              all_active));
+            CK(launch_back((ppdl & 512) != 0, sBack, B, X, a.y, a.ybs, a.ycs, a.y_len, state, ss, e->w, 1, a.pos_rel, k, K, k * HOP, slot,
+                           all_active));
         }
     }
     for (int i = 1; i < PIPE_STREAMS; ++i)                             // join

@@ -1,5 +1,7 @@
 // Launch geometry of the separator kernels, shared by the engine (sep_engine.cu) and the kernel tests
-// (tests/kernels/kernel_harness.cu), so that the tests launch every kernel exactly as the engine does.
+// (tests/kernels/kernel_harness.cu), so that the tests launch every kernel exactly as the engine does.  A kernel launched
+// from more than one place has one launcher here, the only place that states its grid, block, dynamic shared memory and
+// cluster shape; it takes the kernel's own arguments in the kernel's order, after what only the geometry needs.
 #pragma once
 #include <algorithm>
 #include <utility>
@@ -54,6 +56,104 @@ static inline cudaError_t set_sep_smem() {
     for (const auto& k : kernels)
         if (cudaError_t e = cudaFuncSetAttribute(k.first, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k.second)) return e;
     return cudaSuccess;
+}
+
+// front_kernel: grid (T + gate, B), the T frames and, with gate = 1, each stream's speaker-gate memo CTA
+template <class Map>
+inline cudaError_t launch_front(bool pdl, cudaStream_t st, int B, int gate, const float* x, int64_t x_bstride, int64_t x_cstride,
+                                int x_len, float* X, float* state, Map recs, const SepWeights& w, int T, int pos_rel, const float* emb,
+                                float* spk_pre, int frame_k, int frames_total, int sample_off, const uint8_t* active) {
+    return launch_k(pdl, front_kernel_t<Map>, dim3(T + gate, B), dim3(256), FRONT_SMEM, st, x, x_bstride, x_cstride, x_len, X, state,
+                    recs, w, T, pos_rel, emb, spk_pre, frame_k, frames_total, sample_off, active);
+}
+// front_many_kernel: g.workers CTAs walk the chunks, then `gate` speaker-gate CTAs per stream
+template <class Map>
+inline cudaError_t launch_front_many(bool pdl, cudaStream_t st, int gate, const ChunkWalk& g, const float* x, int64_t x_bstride,
+                                     int64_t x_cstride, int x_len, float* X, float* state, Map recs, const SepWeights& w, int T,
+                                     int pos_rel, const float* emb, float* spk_pre, int n_streams, const uint8_t* active) {
+    return launch_k(pdl, front_many_kernel_t<Map>, dim3(g.workers + gate * n_streams, 1), dim3(256), FRONT_SMEM, st, x, x_bstride,
+                    x_cstride, x_len, X, state, recs, w, T, pos_rel, emb, spk_pre, g.chunk, g.n_chunks, n_streams, g.workers, active);
+}
+// front1_kernel: grid (TAIL_TILES + gate, B), the frame's 13 bin tiles and, with gate = 1, the speaker-gate CTA
+template <class Map>
+inline cudaError_t launch_front1(bool pdl, cudaStream_t st, int B, int gate, const float* x, int64_t x_bstride, int64_t x_cstride,
+                                 int x_len, float* X, float* state, Map recs, const SepWeights& w, const BlockWeights& w0, float* GX,
+                                 int pos_rel, const float* emb, float* spk_pre, const uint8_t* active) {
+    return launch_k(pdl, front1_kernel_t<Map>, dim3(TAIL_TILES + gate, B), dim3(256), FRONT1_SMEM, st, x, x_bstride, x_cstride, x_len,
+                    X, state, recs, w, w0, GX, pos_rel, emb, spk_pre, active);
+}
+// the middle section in three kernels, each persistent over (stream, row tile) items
+inline cudaError_t launch_mid_a(bool pdl, cudaStream_t st, const float* Y, float* X, float* GI, const BlockWeights& w, int n_streams,
+                                int64_t hop_stride, int n_hops) {
+    return launch_k(pdl, mid_a_kernel, mid_grid_for(n_streams, 2), dim3(256), MID_A_SMEM, st, Y, X, GI, w, n_streams, hop_stride, n_hops);
+}
+template <class Map>
+inline cudaError_t launch_mid_b(bool pdl, cudaStream_t st, const float* GI, float* Hn, int64_t hop_stride, int n_hops, float* state,
+                                Map recs, int blk, const BlockWeights& w, int n_streams, const uint8_t* active) {
+    return launch_k(pdl, mid_b_kernel_t<Map>, mid_grid_for(n_streams, 3), dim3(256), MID_B_SMEM, st, GI, Hn, hop_stride, n_hops, state,
+                    recs, blk, w, n_streams, active);
+}
+inline cudaError_t launch_mid_c(bool pdl, cudaStream_t st, const float* Hn, float* X, float* QKV, const BlockWeights& w, int n_streams,
+                                int64_t hop_stride, int n_hops) {
+    return launch_k(pdl, mid_c_kernel, mid_grid_for(n_streams, 4), dim3(256), MID_C_SMEM, st, Hn, X, QKV, w, n_streams, hop_stride, n_hops);
+}
+// qkv_kernel: grid (T, B); the projections run inside (pre == nullptr) or are given, with less shared memory
+template <class Map>
+inline cudaError_t launch_qkv(bool pdl, cudaStream_t st, int B, const float* X, const float* pre, float* Q, float* Kall, float* Vall,
+                              float* state, Map recs, int blk, const BlockWeights& w, int T, int frame_k, const uint8_t* active) {
+    return launch_k(pdl, qkv_kernel_t<Map>, dim3(T, B), dim3(QKV_THREADS), pre ? QKV_PRE_SMEM : QKV_SMEM, st, X, pre, Q, Kall, Vall,
+                    state, recs, blk, w, T, frame_k, active);
+}
+// qkv_many_kernel: `ctas` persistent CTAs walk the frames
+template <class Map>
+inline cudaError_t launch_qkv_many(bool pdl, cudaStream_t st, int ctas, const float* pre, float* Q, float* Kall, float* Vall,
+                                   float* state, Map recs, int blk, const BlockWeights& w, int T, int n_frames, const uint8_t* active) {
+    return launch_k(pdl, qkv_many_kernel_t<Map>, dim3(ctas), dim3(QKV_THREADS), QKV_MANY_SMEM, st, pre, Q, Kall, Vall, state, recs, blk,
+                    w, T, n_frames, active);
+}
+template <class Map>
+inline cudaError_t launch_kv_gather(bool pdl, cudaStream_t st, int B, const float* state, Map recs, int blk, float* Kall, float* Vall,
+                                    int T) {
+    return launch_k(pdl, kv_gather_kernel_t<Map>, dim3(ATT - 1, B * NHEAD), dim3(128), 0, st, state, recs, blk, Kall, Vall, T);
+}
+// attn_kernel (a CTA per query frame and head), attn_tile_kernel (ATT_TQ query frames per CTA; the linear scratch only, no
+// frame_k) or attn_cluster_kernel (each window split over an ATT_CL-CTA cluster)
+enum class AttnForm { query, tile, cluster };
+template <class Map>
+inline cudaError_t launch_attention(AttnForm form, bool pdl, cudaStream_t st, int B, const float* Q, const float* Kall,
+                                    const float* Vall, const float* state, Map recs, int blk, float* Z, int T, int frame_k) {
+    if (form == AttnForm::cluster)
+        return launch_cluster(pdl, dim3(1, ATT_CL, 1), attn_cluster_kernel_t<Map>, dim3(T, NHEAD * ATT_CL, B), dim3(256), 0, st, Q, Kall,
+                              Vall, state, recs, blk, Z, T, frame_k);
+    if (form == AttnForm::tile)
+        return launch_k(pdl, attn_tile_kernel, dim3((T + ATT_TQ - 1) / ATT_TQ, NHEAD, B), dim3(256), 0, st, Q, Kall, Vall, Z, T);
+    return launch_k(pdl, attn_kernel_t<Map>, dim3(T, NHEAD, B), dim3(256), 0, st, Q, Kall, Vall, state, recs, blk, Z, T, frame_k);
+}
+template <class Map>
+inline cudaError_t launch_attn_out(bool pdl, cudaStream_t st, int B, const float* Z, float* X, const float* state, Map recs,
+                                   const BlockWeights& w, int apply_gate, int T) {
+    return launch_k(pdl, attn_out_kernel_t<Map>, dim3(T, B), dim3(256), AOUT_SMEM, st, Z, X, state, recs, w, apply_gate, T);
+}
+template <class Map>
+inline cudaError_t launch_ln_frame_res(bool pdl, cudaStream_t st, int B, const float* P, float* X, const float* state, Map recs,
+                                       const BlockWeights& w, int apply_gate, int T) {
+    return launch_k(pdl, ln_frame_res_kernel_t<Map>, dim3(T, B), dim3(256), 0, st, P, X, state, recs, w, apply_gate, T);
+}
+// back_kernel: a cluster of BACK_CL per frame and stream
+template <class Map>
+inline cudaError_t launch_back(bool pdl, cudaStream_t st, int B, const float* X, float* y, int64_t y_bstride, int64_t y_cstride,
+                               int y_len, float* state, Map recs, const SepWeights& w, int T, int pos_rel, int frame_k, int frames_total,
+                               int sample_off, int64_t hist_stride, const uint8_t* active) {
+    return launch_cluster(pdl, dim3(BACK_CL, 1, 1), back_kernel_t<Map>, dim3(BACK_CL * T, B), dim3(256), BACK_SMEM, st, X, y, y_bstride,
+                          y_cstride, y_len, state, recs, w, T, pos_rel, frame_k, frames_total, sample_off, hist_stride, active);
+}
+// back_many_kernel: g.workers clusters of BACK_CL walk the chunks
+template <class Map>
+inline cudaError_t launch_back_many(bool pdl, cudaStream_t st, const ChunkWalk& g, const float* X, float* y, int64_t y_bstride,
+                                    int64_t y_cstride, int y_len, float* state, Map recs, const SepWeights& w, int T, int pos_rel,
+                                    int n_streams, const uint8_t* active) {
+    return launch_cluster(pdl, dim3(BACK_CL, 1, 1), back_many_kernel_t<Map>, dim3(BACK_CL * g.workers, 1), dim3(256), BACK_MANY_SMEM,
+                          st, X, y, y_bstride, y_cstride, y_len, state, recs, w, T, pos_rel, g.chunk, g.n_chunks, n_streams, active);
 }
 
 }  // namespace l2h

@@ -6,8 +6,8 @@
 // tests/test_embed_kernels_gpu.py can drive each kernel directly with arbitrary shapes and compare it element by element
 // with a float64 reference.
 //
-// The argument structs below are plain C (mirrored with ctypes in the tests); every function fills the engine's own
-// descriptor and calls the engine's own launcher (or launches the kernel with the engine's own geometry).  Built by
+// The argument structs below are plain C (mirrored with ctypes in the tests); every function checks its arguments, fills
+// the engine's own descriptor and calls the engine's own launcher.  Built by
 // lookoncetohear_b200/build.py as lib/libl2h_kernel_harness.so with hidden visibility, so this library's copy of the
 // l2h symbols never binds to the product library's copy.
 #include <cstdio>
@@ -160,39 +160,39 @@ KH_API int kh_split_planes(const float* src, int64_t row_stride, int64_t col_str
                                    static_cast<__nv_bfloat16*>(lo), static_cast<cudaStream_t>(stream));
 }
 
-// `passes` applies to the tensor-core variants only
-KH_API int kh_lstm(const KhLstm* k, int variant, int passes, char* why, int why_len, void* stream) {
-    put_why(why, why_len, nullptr);
+// the dynamic shared memory of every kernel launched here that needs more than the default, set once per device (the
+// separator's dense forms with the engine's own list)
+static cudaError_t configure() {
     static thread_local int configured_dev = -1;
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return (int)e;
-    if (configured_dev != dev) {
-        e = configure_lstm();
-        if (e == cudaSuccess) e = configure_tc_lstm();
-        if (e != cudaSuccess) { put_why(why, why_len, "kernel attributes"); return (int)e; }
-        configured_dev = dev;
-    }
+    if (e != cudaSuccess || configured_dev == dev) return e;
+    e = configure_lstm();
+    if (e == cudaSuccess) e = configure_tc_lstm();
+    if (e == cudaSuccess) e = set_sep_smem<int64_t>();
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(emb::eattn_out_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)emb::EAOUT_SMEM);
+    if (e == cudaSuccess) configured_dev = dev;
+    return e;
+}
+
+// `passes` applies to the tensor-core variants only
+KH_API int kh_lstm(const KhLstm* k, int variant, int passes, char* why, int why_len, void* stream) {
+    put_why(why, why_len, nullptr);
+    cudaError_t e = configure();
+    if (e != cudaSuccess) { put_why(why, why_len, "kernel attributes"); return (int)e; }
     const LstmArgs a = to_lstm(*k);
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
-    // the forced kernels get the launchers' own argument checks
-    if (variant >= KH_LSTM_REC3_PRE && variant <= KH_LSTM_REC4_4 && (a.nseq <= 0 || a.L <= 0 || !lstm_state_ok(a))) {
-        put_why(why, why_len, "refused by the launcher's checks");
-        return (int)cudaErrorInvalidValue;
-    }
+    static const LstmRec forced[] = {LstmRec::rec3_pre, LstmRec::rec3_ring, LstmRec::rec4_2, LstmRec::rec4_4};   // KH_LSTM_REC*
     switch (variant) {
         case KH_LSTM_AUTO: e = launch_lstm_rec(a, st); break;
-        case KH_LSTM_REC3_PRE:
-            if ((size_t)a.L * 1024 > 200 * 1024) { put_why(why, why_len, "L too long for the preloaded kernel"); return (int)cudaErrorInvalidValue; }
-            e = launch_k(false, lstm_rec3_kernel<1, true>, dim3(a.nseq, a.ndir), dim3(128), (size_t)a.L * 1024, st, a);
+        case KH_LSTM_REC3_PRE: case KH_LSTM_REC3_RING: case KH_LSTM_REC4_2: case KH_LSTM_REC4_4: {
+            // the forced kernels get the launcher's own argument checks
+            const char* no = (a.nseq <= 0 || a.L <= 0 || !lstm_state_ok(a)) ? "refused by the launcher's checks"
+                             : (variant == KH_LSTM_REC3_PRE && !lstm_rec_preloads(a.L)) ? "L too long for the preloaded kernel" : nullptr;
+            if (no) { put_why(why, why_len, no); return (int)cudaErrorInvalidValue; }
+            e = launch_lstm_variant(forced[variant - KH_LSTM_REC3_PRE], a, st, false);
             break;
-        case KH_LSTM_REC3_RING: e = launch_k(false, lstm_rec3_kernel<1, false>, dim3(a.nseq, a.ndir), dim3(128), 0, st, a); break;
-        case KH_LSTM_REC4_2:
-            e = launch_k(false, lstm_rec4_kernel<2>, dim3((a.nseq + 1) / 2, a.ndir), dim3(128), lstm_rec4_smem(2), st, a);
-            break;
-        case KH_LSTM_REC4_4:
-            e = launch_k(false, lstm_rec4_kernel<4>, dim3((a.nseq + 3) / 4, a.ndir), dim3(128), lstm_rec4_smem(4), st, a);
-            break;
+        }
         case KH_LSTM_TC: e = launch_tc_lstm(a, passes, st); break;
         case KH_LSTM_TC_X: {
             tcl::LstmXArgs xa{};
@@ -239,17 +239,6 @@ KH_API int kh_sep_layout(int n_blocks, int64_t* out) {
     return n;
 }
 
-// dynamic shared memory of the separator kernels (dense forms), set once per device with the engine's own list
-static cudaError_t configure_sep() {
-    static thread_local int configured_dev = -1;
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess || configured_dev == dev) return e;
-    e = set_sep_smem<int64_t>();
-    if (e == cudaSuccess) configured_dev = dev;
-    return e;
-}
-
 // CTAs of attn_cluster_kernel the current device holds at once: the engine splits a call's windows over 8-CTA
 // clusters while B * T * NHEAD * ATT_CL fits in this (attn_splits)
 KH_API int kh_attn_cluster_resident() { return attn_cluster_resident(); }
@@ -259,27 +248,24 @@ KH_API int kh_attn_cluster_resident() { return attn_cluster_resident(); }
 KH_API int kh_qkv(const KhSepWeights* w, const float* X, const float* pre, float* Q, float* Kall, float* Vall, float* state,
                   int64_t sstride, int blk, int B, int T, int frame_k, const uint8_t* active, void* stream) {
     if (B <= 0 || T <= 0 || frame_k < 0) return (int)cudaErrorInvalidValue;
-    cudaError_t e = configure_sep();
-    if (e != cudaSuccess) return (int)e;
-    return (int)launch_k(false, qkv_kernel, dim3(T, B), dim3(QKV_THREADS), QKV_SMEM, static_cast<cudaStream_t>(stream), X, pre,
-                         Q, Kall, Vall, state, sstride, blk, to_block(*w), T, frame_k, active);
+    if (cudaError_t e = configure()) return (int)e;
+    return (int)launch_qkv(false, static_cast<cudaStream_t>(stream), B, X, pre, Q, Kall, Vall, state, sstride, blk, to_block(*w), T,
+                           frame_k, active);
 }
 
 // qkv_many_kernel over frames 0 .. n_frames-1 (frame fi = stream fi / T, row fi % T) with `grid` persistent CTAs
 KH_API int kh_qkv_many(const KhSepWeights* w, const float* pre, float* Q, float* Kall, float* Vall, float* state,
                        int64_t sstride, int blk, int T, int grid, int n_frames, const uint8_t* active, void* stream) {
     if (T <= 0 || grid <= 0 || n_frames <= 0) return (int)cudaErrorInvalidValue;
-    cudaError_t e = configure_sep();
-    if (e != cudaSuccess) return (int)e;
-    return (int)launch_k(false, qkv_many_kernel, dim3(grid), dim3(QKV_THREADS), QKV_MANY_SMEM, static_cast<cudaStream_t>(stream),
-                         pre, Q, Kall, Vall, state, sstride, blk, to_block(*w), T, n_frames, active);
+    if (cudaError_t e = configure()) return (int)e;
+    return (int)launch_qkv_many(false, static_cast<cudaStream_t>(stream), grid, pre, Q, Kall, Vall, state, sstride, blk, to_block(*w),
+                                T, n_frames, active);
 }
 
 // kv_gather_kernel: grid (ATT - 1, B * NHEAD), 128 threads
 KH_API int kh_kv_gather(const float* state, int64_t sstride, int blk, float* Kall, float* Vall, int B, int T, void* stream) {
     if (B <= 0 || T <= 1) return (int)cudaErrorInvalidValue;
-    return (int)launch_k(false, kv_gather_kernel, dim3(ATT - 1, B * NHEAD), dim3(128), 0, static_cast<cudaStream_t>(stream),
-                         state, sstride, blk, Kall, Vall, T);
+    return (int)launch_kv_gather(false, static_cast<cudaStream_t>(stream), B, state, sstride, blk, Kall, Vall, T);
 }
 
 // One attention form: T == 1 reads the ring (window of frame clock + frame_k), T > 1 the linear scratch.  The tile form
@@ -287,38 +273,25 @@ KH_API int kh_kv_gather(const float* state, int64_t sstride, int blk, float* Kal
 KH_API int kh_attention(int form, const float* Q, const float* Kall, const float* Vall, const float* state, int64_t sstride,
                         int blk, float* Z, int B, int T, int frame_k, void* stream) {
     if (B <= 0 || T <= 0 || frame_k < 0 || (T > 1 && frame_k != 0)) return (int)cudaErrorInvalidValue;
-    const cudaStream_t st = static_cast<cudaStream_t>(stream);
-    switch (form) {
-        case KH_ATTN_QUERY:
-            return (int)launch_k(false, attn_kernel, dim3(T, NHEAD, B), dim3(256), 0, st, Q, Kall, Vall, state, sstride, blk, Z, T,
+    if (form < KH_ATTN_QUERY || form > KH_ATTN_CLUSTER || (form == KH_ATTN_TILE && T == 1)) return (int)cudaErrorInvalidValue;
+    static const AttnForm forms[] = {AttnForm::query, AttnForm::tile, AttnForm::cluster};      // by KhAttnForm
+    return (int)launch_attention(forms[form], false, static_cast<cudaStream_t>(stream), B, Q, Kall, Vall, state, sstride, blk, Z, T,
                                  frame_k);
-        case KH_ATTN_TILE:
-            if (T == 1) return (int)cudaErrorInvalidValue;
-            return (int)launch_k(false, attn_tile_kernel, dim3((T + ATT_TQ - 1) / ATT_TQ, NHEAD, B), dim3(256), 0, st, Q, Kall,
-                                 Vall, Z, T);
-        case KH_ATTN_CLUSTER:
-            return (int)launch_cluster(false, dim3(1, ATT_CL, 1), attn_cluster_kernel, dim3(T, NHEAD * ATT_CL, B), dim3(256), 0,
-                                       st, Q, Kall, Vall, state, sstride, blk, Z, T, frame_k);
-        default: return (int)cudaErrorInvalidValue;
-    }
 }
 
 // attn_out_kernel: grid (T, B); X [B][T][97][64] updated in place; the gate is ST_GATE of each stream's record
 KH_API int kh_attn_out(const KhSepWeights* w, const float* Z, float* X, const float* state, int64_t sstride, int B, int T,
                        int apply_gate, void* stream) {
     if (B <= 0 || T <= 0) return (int)cudaErrorInvalidValue;
-    cudaError_t e = configure_sep();
-    if (e != cudaSuccess) return (int)e;
-    return (int)launch_k(false, attn_out_kernel, dim3(T, B), dim3(256), AOUT_SMEM, static_cast<cudaStream_t>(stream), Z, X,
-                         state, sstride, to_block(*w), apply_gate, T);
+    if (cudaError_t e = configure()) return (int)e;
+    return (int)launch_attn_out(false, static_cast<cudaStream_t>(stream), B, Z, X, state, sstride, to_block(*w), apply_gate, T);
 }
 
 // ln_frame_res_kernel: grid (T, B); P [B][T][97][64] = the projection after PReLU
 KH_API int kh_ln_frame_res(const KhSepWeights* w, const float* P, float* X, const float* state, int64_t sstride, int B, int T,
                            int apply_gate, void* stream) {
     if (B <= 0 || T <= 0) return (int)cudaErrorInvalidValue;
-    return (int)launch_k(false, ln_frame_res_kernel, dim3(T, B), dim3(256), 0, static_cast<cudaStream_t>(stream), P, X, state,
-                         sstride, to_block(*w), apply_gate, T);
+    return (int)launch_ln_frame_res(false, static_cast<cudaStream_t>(stream), B, P, X, state, sstride, to_block(*w), apply_gate, T);
 }
 
 // ---- the separator's front and back (sep_kernels.cuh, hop_kernels.cuh) ----------------------------------------------
@@ -347,12 +320,10 @@ KH_API int kh_front(const KhSepFrontBack* w, const float* x, int64_t x_bstride, 
     const bool group = frames_total > 1;
     if (B <= 0 || T <= 0 || (group && (T != 1 || frame_k < 0 || frame_k >= frames_total)) || (!group && frame_k != 0))
         return (int)cudaErrorInvalidValue;
-    cudaError_t e = configure_sep();
-    if (e != cudaSuccess) return (int)e;
-    const dim3 grid(group ? (frame_k == 0 ? 2 : 1) : T + 1, B);
-    return (int)launch_k(false, front_kernel, grid, dim3(256), FRONT_SMEM, static_cast<cudaStream_t>(stream), x, x_bstride,
-                         x_cstride, x_len, X, state, sstride, to_sep(*w), T, pos_rel, emb, spk_pre, group ? frame_k : 0,
-                         group ? frames_total : 1, group ? frame_k * HOP : 0, active);
+    if (cudaError_t e = configure()) return (int)e;
+    return (int)launch_front(false, static_cast<cudaStream_t>(stream), B, group ? (frame_k == 0 ? 1 : 0) : 1, x, x_bstride, x_cstride,
+                             x_len, X, state, sstride, to_sep(*w), T, pos_rel, emb, spk_pre, group ? frame_k : 0,
+                             group ? frames_total : 1, group ? frame_k * HOP : 0, active);
 }
 
 // the engine's front_many_kernel geometry for (B, T) (sep_launch.cuh)
@@ -366,12 +337,10 @@ KH_API int kh_front_many(const KhSepFrontBack* w, const float* x, int64_t x_bstr
                          float* state, int64_t sstride, int B, int T, int pos_rel, const float* emb, float* spk_pre, int chunk,
                          int n_workers, const uint8_t* active, void* stream) {
     if (B <= 0 || T <= 0 || chunk <= 0 || n_workers <= 0) return (int)cudaErrorInvalidValue;
-    cudaError_t e = configure_sep();
-    if (e != cudaSuccess) return (int)e;
-    const int n_chunks = (T + chunk - 1) / chunk;
-    return (int)launch_k(false, front_many_kernel, dim3(n_workers + B, 1), dim3(256), FRONT_SMEM, static_cast<cudaStream_t>(stream),
-                         x, x_bstride, x_cstride, x_len, X, state, sstride, to_sep(*w), T, pos_rel, emb, spk_pre, chunk, n_chunks,
-                         B, n_workers, active);
+    if (cudaError_t e = configure()) return (int)e;
+    const ChunkWalk g{chunk, (T + chunk - 1) / chunk, n_workers};
+    return (int)launch_front_many(false, static_cast<cudaStream_t>(stream), 1, g, x, x_bstride, x_cstride, x_len, X, state, sstride,
+                                  to_sep(*w), T, pos_rel, emb, spk_pre, B, active);
 }
 
 // front1_kernel: one frame as 13 tiles of 8 bins plus the speaker-gate CTA, grid (14, B); GX [B][97][512]
@@ -379,12 +348,11 @@ KH_API int kh_front1(const KhSepFrontBack* w, const float* x, int64_t x_bstride,
                      float* GX, float* state, int64_t sstride, int B, int pos_rel, const float* emb, float* spk_pre,
                      const uint8_t* active, void* stream) {
     if (B <= 0) return (int)cudaErrorInvalidValue;
-    cudaError_t e = configure_sep();
-    if (e != cudaSuccess) return (int)e;
+    if (cudaError_t e = configure()) return (int)e;
     BlockWeights w0{};
     w0.ln1_g = w->ln1_g; w0.ln1_b = w->ln1_b; w0.wih1_t = w->wih1_t; w0.b1 = w->b1;
-    return (int)launch_k(false, front1_kernel, dim3(TAIL_TILES + 1, B), dim3(256), FRONT1_SMEM, static_cast<cudaStream_t>(stream),
-                         x, x_bstride, x_cstride, x_len, X, state, sstride, to_sep(*w), w0, GX, pos_rel, emb, spk_pre, active);
+    return (int)launch_front1(false, static_cast<cudaStream_t>(stream), B, 1, x, x_bstride, x_cstride, x_len, X, state, sstride,
+                              to_sep(*w), w0, GX, pos_rel, emb, spk_pre, active);
 }
 
 // back_kernel in clusters of BACK_CL.  frames_total <= 1: an ordinary call of T frames, grid (4 T, B); it advances the
@@ -396,12 +364,10 @@ KH_API int kh_back(const KhSepFrontBack* w, const float* X, float* y, int64_t y_
     const bool group = frames_total > 1;
     if (B <= 0 || T <= 0 || (group && (T != 1 || frame_k < 0 || frame_k >= frames_total)) || (!group && frame_k != 0))
         return (int)cudaErrorInvalidValue;
-    cudaError_t e = configure_sep();
-    if (e != cudaSuccess) return (int)e;
-    return (int)launch_cluster(false, dim3(BACK_CL, 1, 1), back_kernel, dim3(BACK_CL * T, B), dim3(256), BACK_SMEM,
-                               static_cast<cudaStream_t>(stream), X, y, y_bstride, y_cstride, y_len, state, sstride, to_sep(*w), T,
-                               pos_rel, group ? frame_k : 0, group ? frames_total : 1, group ? frame_k * HOP : 0,
-                               group ? hist_stride : (int64_t)0, active);
+    if (cudaError_t e = configure()) return (int)e;
+    return (int)launch_back(false, static_cast<cudaStream_t>(stream), B, X, y, y_bstride, y_cstride, y_len, state, sstride, to_sep(*w),
+                            T, pos_rel, group ? frame_k : 0, group ? frames_total : 1, group ? frame_k * HOP : 0,
+                            group ? hist_stride : 0, active);
 }
 
 // the engine's back_many_kernel geometry for (B, T) (sep_launch.cuh)
@@ -415,16 +381,14 @@ KH_API int kh_back_many(const KhSepFrontBack* w, const float* X, float* y, int64
                         float* state, int64_t sstride, int B, int T, int pos_rel, int chunk, int n_cl, const uint8_t* active,
                         void* stream) {
     if (B <= 0 || T <= 0 || chunk <= 0 || n_cl <= 0) return (int)cudaErrorInvalidValue;
-    cudaError_t e = configure_sep();
-    if (e != cudaSuccess) return (int)e;
-    const int n_chunks = (T + chunk - 1) / chunk;
-    return (int)launch_cluster(false, dim3(BACK_CL, 1, 1), back_many_kernel, dim3(BACK_CL * n_cl, 1), dim3(256), BACK_MANY_SMEM,
-                               static_cast<cudaStream_t>(stream), X, y, y_bstride, y_cstride, y_len, state, sstride, to_sep(*w), T,
-                               pos_rel, chunk, n_chunks, B, active);
+    if (cudaError_t e = configure()) return (int)e;
+    const ChunkWalk g{chunk, (T + chunk - 1) / chunk, n_cl};
+    return (int)launch_back_many(false, static_cast<cudaStream_t>(stream), g, X, y, y_bstride, y_cstride, y_len, state, sstride,
+                                 to_sep(*w), T, pos_rel, B, active);
 }
 
 // ---- the enrollment network's own kernels (embed_kernels.cuh) --------------------------------------------------------
-// Launched with embed_forward_impl's geometry.  Every `lens` (device, [B] int32) may be null: the equal-length path.
+// Launched through embed_forward_impl's launchers.  Every `lens` (device, [B] int32) may be null: the equal-length path.
 // The fields of EmbWeights that estd / efront / egn_apply / ehead read, and of EmbBlockWeights that eqkv_ln and eattn_out
 // read.
 struct KhEmbWeights {
@@ -464,85 +428,62 @@ KH_API int kh_embed_layout(int64_t* out) {
 // estd_kernel: grid B, 256 threads; x [B][2][N]
 KH_API int kh_estd(const float* x, int N, const int32_t* lens, float* inv_std, int B, void* stream) {
     if (B <= 0 || N <= 0) return (int)cudaErrorInvalidValue;
-    return (int)launch_k(false, emb::estd_kernel, dim3(B), dim3(256), 0, static_cast<cudaStream_t>(stream), x, N, lens, inv_std);
+    return (int)emb::launch_estd(static_cast<cudaStream_t>(stream), B, x, N, lens, inv_std);
 }
 
 // efront_kernel: grid (T, B), 256 threads; the caller zeroes gn_sums [B][2] (double)
 KH_API int kh_efront(const KhEmbWeights* w, const float* x, int N, const int32_t* lens, const float* inv_std, float* X,
                      double* gn_sums, int B, int T, void* stream) {
     if (B <= 0 || T <= 0) return (int)cudaErrorInvalidValue;
-    return (int)launch_k(false, emb::efront_kernel, dim3(T, B), dim3(256), 0, static_cast<cudaStream_t>(stream), x, N, lens,
-                         inv_std, X, gn_sums, to_emb(*w), T);
+    return (int)emb::launch_efront(static_cast<cudaStream_t>(stream), B, x, N, lens, inv_std, X, gn_sums, to_emb(*w), T);
 }
 
 // egn_apply_kernel: ceil(total4 / 256) CTAs of 256 threads
 KH_API int kh_egn_apply(const KhEmbWeights* w, float* X, const double* gn_sums, int64_t per_b, int64_t total4,
                         const int32_t* lens, void* stream) {
     if (per_b <= 0 || total4 <= 0) return (int)cudaErrorInvalidValue;
-    return (int)launch_k(false, emb::egn_apply_kernel, dim3((unsigned)((total4 + 255) / 256)), dim3(256), 0,
-                         static_cast<cudaStream_t>(stream), X, gn_sums, per_b, total4, lens, to_emb(*w));
+    return (int)emb::launch_egn_apply(static_cast<cudaStream_t>(stream), X, gn_sums, per_b, total4, lens, to_emb(*w));
 }
 
 // eqkv_ln_kernel: grid (T, B), 384 threads; QKV [B][T][65][128]
 KH_API int kh_eqkv_ln(const KhEmbBlock* w, const float* QKV, float* Qn, void* Kp, void* Vp, int64_t k_plane, int64_t v_plane,
                       int B, int T, int Tp, void* stream) {
     if (B <= 0 || T <= 0 || Tp < T) return (int)cudaErrorInvalidValue;
-    return (int)launch_k(false, emb::eqkv_ln_kernel, dim3(T, B), dim3(384), 0, static_cast<cudaStream_t>(stream), QKV, Qn,
-                         static_cast<__nv_bfloat16*>(Kp), static_cast<__nv_bfloat16*>(Vp), k_plane, v_plane, to_emb_block(*w),
-                         T, Tp);
+    return (int)emb::launch_eqkv_ln(static_cast<cudaStream_t>(stream), B, QKV, Qn, static_cast<__nv_bfloat16*>(Kp),
+                                    static_cast<__nv_bfloat16*>(Vp), k_plane, v_plane, to_emb_block(*w), T, Tp);
 }
 
 // softmax_rows_kernel: one CTA of 128 threads per row, Z * rows_per_z rows
 KH_API int kh_softmax_rows(float* S, int64_t ld, int n, int rows_per_z, int64_t z_stride, int Z, const int32_t* lens,
                            void* stream) {
     if (Z <= 0 || rows_per_z <= 0 || n <= 0 || ld < n) return (int)cudaErrorInvalidValue;
-    return (int)launch_k(false, emb::softmax_rows_kernel, dim3((unsigned)((int64_t)Z * rows_per_z)), dim3(128), 0,
-                         static_cast<cudaStream_t>(stream), S, ld, n, rows_per_z, z_stride, lens);
+    return (int)emb::launch_softmax_rows(static_cast<cudaStream_t>(stream), Z, S, ld, n, rows_per_z, z_stride, lens);
 }
 
 // the engine's eattn_out_kernel grid for (T, B)
-KH_API int kh_eattn_out_grid(int T, int B) { return (int)std::min<int64_t>((int64_t)T * B, NUM_SMS * 4); }
+KH_API int kh_eattn_out_grid(int T, int B) { return emb::eattn_out_ctas(T, B); }
 
 // eattn_out_kernel with `grid` persistent CTAs over frames 0 .. n_frames-1 (frame item = b * T + t)
 KH_API int kh_eattn_out(const KhEmbBlock* w, const float* O, float* X, int T, int Tp, int n_frames, int grid, void* stream) {
     if (T <= 0 || Tp < T || n_frames <= 0 || grid <= 0) return (int)cudaErrorInvalidValue;
-    static thread_local int configured_dev = -1;
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return (int)e;
-    if (configured_dev != dev) {
-        e = cudaFuncSetAttribute(emb::eattn_out_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)emb::EAOUT_SMEM);
-        if (e != cudaSuccess) return (int)e;
-        configured_dev = dev;
-    }
-    return (int)launch_k(false, emb::eattn_out_kernel, dim3(grid), dim3(256), emb::EAOUT_SMEM, static_cast<cudaStream_t>(stream),
-                         O, X, to_emb_block(*w), T, Tp, n_frames);
+    if (cudaError_t e = configure()) return (int)e;
+    return (int)emb::launch_eattn_out(static_cast<cudaStream_t>(stream), grid, O, X, to_emb_block(*w), T, Tp, n_frames);
 }
 
 // ehead_kernel: grid B, 256 threads; HD [B][T][256]
 KH_API int kh_ehead(const KhEmbWeights* w, const float* HD, float* out, int B, int T, const int32_t* lens, void* stream) {
     if (B <= 0 || T <= 0) return (int)cudaErrorInvalidValue;
-    return (int)launch_k(false, emb::ehead_kernel, dim3(B), dim3(256), 0, static_cast<cudaStream_t>(stream), HD, out, to_emb(*w),
-                         T, lens);
+    return (int)emb::launch_ehead(static_cast<cudaStream_t>(stream), B, HD, out, to_emb(*w), T, lens);
 }
 
 // einter_mask_kernel: grid (NF, B), 128 threads; gx [(b*NF + f)][steps][512]
 KH_API int kh_einter_mask(float* gx, const int32_t* lens, int B, int steps, void* stream) {
     if (B <= 0 || steps <= 0 || lens == nullptr) return (int)cudaErrorInvalidValue;
-    return (int)launch_k(false, emb::einter_mask_kernel, dim3(emb::NF, B), dim3(128), 0, static_cast<cudaStream_t>(stream), gx,
-                         lens, steps);
+    return (int)emb::launch_einter_mask(static_cast<cudaStream_t>(stream), B, gx, lens, steps);
 }
 
 // eput_lens_kernel: the host lengths lens_host[0 .. n-1] to dst, one launch per block of LENS_PER_LAUNCH, as the engine loops
 KH_API int kh_eput_lens(int32_t* dst, const int32_t* lens_host, int n, void* stream) {
     if (n <= 0) return (int)cudaErrorInvalidValue;
-    for (int b0 = 0; b0 < n; b0 += emb::LENS_PER_LAUNCH) {
-        const int m = std::min(emb::LENS_PER_LAUNCH, n - b0);
-        emb::LensBlock blk;
-        memcpy(blk.v, lens_host + b0, sizeof(int32_t) * m);
-        const cudaError_t e = launch_k(false, emb::eput_lens_kernel, dim3(1), dim3(256), 0, static_cast<cudaStream_t>(stream),
-                                       dst + b0, blk, m);
-        if (e != cudaSuccess) return (int)e;
-    }
-    return 0;
+    return (int)emb::launch_eput_lens(static_cast<cudaStream_t>(stream), dst, lens_host, n);
 }
