@@ -17,9 +17,10 @@
  *   l2h_sep_forward_slots_frames / l2h_sep_forward_slots_hops
  *        <- several Net.predict hops for a list of a state's streams, the same number for every row or one per row
  *           (Net.advance_slots)
- *   l2h_sep_forward_targets / l2h_sep_forward_targets_groups
- *        <- Net.predict for several enrolled speakers of each mixture, for a whole state or a list of its listener
- *           groups (Net.predict_targets, Net.advance_targets)
+ *   l2h_sep_forward_targets / l2h_sep_forward_targets_groups / l2h_sep_forward_targets_rows
+ *        <- Net.predict for several enrolled speakers of each mixture, for a whole state, a list of its listener
+ *           groups, or listeners with different numbers of speakers (Net.predict_targets, Net.advance_targets,
+ *           Net.advance_target_rows)
  *   l2h_sep_stream_host
  *        <- the chunk loop around Net.predict(chunk, embed, state, pad=False)  (SURVEY.md 3.3)
  *           with host buffers: H2D of each chunk and D2H of each result inside the call
@@ -254,6 +255,44 @@ int l2h_sep_forward_targets_groups(void* handle, const float* x_dev, int64_t x_b
                                    const int32_t* groups_dev, const int32_t* hops_dev, int32_t n, int32_t n_targets,
                                    int32_t frames, float* y_dev, int64_t y_batch_stride, int64_t y_ch_stride,
                                    int32_t y_len, void* workspace_dev, size_t workspace_bytes, uint32_t flags, void* stream);
+/* l2h_sep_forward_targets_groups for listeners who enrolled different numbers of speakers: every listener lists its own
+ * target rows and their records, so one call, and one cached graph, serves any mix of one-, two- and three-speaker
+ * listeners.  The front and block 0 run once per call row (listener), blocks 1 .. B-1 and the back once per target row.
+ *   x_dev      [n] call rows of 128*frames + 64 samples (x_len): call row i is one listener's mixture
+ *   emb_dev    [R][256], R = n_rows: target row r's embedding
+ *   y_dev      [R] target rows; y_batch_stride is the stride between consecutive target rows
+ *   records_dev [R] int32 of DEVICE memory: target row r continues record records_dev[r] of the state.  An entry outside
+ *              [0, state_batch) marks a row that is computed but stores nothing.  Records need not be adjacent, aligned or
+ *              in order, so any free records of a state serve a new listener; a record listed twice is a caller error the
+ *              call does not detect.
+ *   offsets_dev [n+1] int32 of DEVICE memory: call row i owns target rows offsets_dev[i] .. offsets_dev[i+1]-1.  Rows from
+ *              offsets_dev[n] to R-1 belong to no listener and store nothing, so one fixed R carries any number of live
+ *              targets.  The offsets are clamped on the device to be non-decreasing and <= R: a bad list gives empty
+ *              listeners, never a read out of bounds.
+ *   hops_dev   [n] int32 of DEVICE memory, or NULL: every call row advances `frames` hops.  Otherwise call row i advances
+ *              h = hops_dev[i] hops, from 0 to `frames`, with the read, write and store rules of
+ *              l2h_sep_forward_targets_groups: it reads only x samples 0 .. 128*h + 63, its target rows receive y samples
+ *              0 .. 128*h - 1 only, and h = 0 stores nothing; every target row of the listener uses the same count.
+ *   state_dev  a state of state_batch records.  A listener's lead record is records_dev[offsets_dev[i]], the record of its
+ *              first target row: it also holds the listener's conv tails and block 0's K/V rings and (h, c), as the lead
+ *              record g*K of a groups call does; the listener's other records never hold them.  A listener with no target
+ *              row, or with a lead record outside the state, stores nothing at all.  The records of a listener advance
+ *              together, so their clocks must start equal: start a listener's records together (l2h_sep_state_reset_streams
+ *              of all of them); adding a record to a running listener is not supported.
+ *   workspace  l2h_sep_workspace_bytes(handle, n_rows, frames, flags)
+ * All three lists are read when the kernels run: with L2H_FLAG_GRAPH one graph cached for (n, R, T) serves every tick, and
+ * its key holds the list pointers, not their contents, so a caller rewrites records_dev, offsets_dev and hops_dev in place
+ * before every tick.  Every kernel form is chosen for the R target rows, and block 0 runs those forms over the n call rows,
+ * so with offsets i*K and records g_i*K + k this is l2h_sep_forward_targets_groups, bit for bit.  Not supported: activity
+ * masks, the pipelined wavefront graph and l2h_sep_stream_host / _dev, taps.
+ * Errors 1, before anything is enqueued: null pointers, n, n_rows or frames <= 0, n_rows > state_batch, n > n_rows,
+ * n_rows*frames*97 rows beyond the limit of one call, L2H_FLAG_TAPS. */
+int l2h_sep_forward_targets_rows(void* handle, const float* x_dev, int64_t x_batch_stride, int64_t x_ch_stride,
+                                 int32_t x_len, const float* emb_dev, void* state_dev, int32_t state_batch,
+                                 const int32_t* records_dev, const int32_t* offsets_dev, const int32_t* hops_dev,
+                                 int32_t n, int32_t n_rows, int32_t frames, float* y_dev, int64_t y_batch_stride,
+                                 int64_t y_ch_stride, int32_t y_len, void* workspace_dev, size_t workspace_bytes,
+                                 uint32_t flags, void* stream);
 
 /* Streaming with HOST buffers (the end-to-end path).  Per round: H2D of the round's samples (+64
  * look-ahead) from pinned memory, the kernel chains, D2H of the new samples; one stream synchronise at

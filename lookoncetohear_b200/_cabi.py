@@ -84,6 +84,12 @@ _SIGS = {
                                                      ctypes.c_int32, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64,
                                                      ctypes.c_int32, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_uint32,
                                                      ctypes.c_void_p]),
+    "l2h_sep_forward_targets_rows": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64,
+                                                   ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
+                                                   ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
+                                                   ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int64,
+                                                   ctypes.c_int64, ctypes.c_int32, ctypes.c_void_p, ctypes.c_size_t,
+                                                   ctypes.c_uint32, ctypes.c_void_p]),
     "l2h_sep_stream_host": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p,
                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
                                           ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p,

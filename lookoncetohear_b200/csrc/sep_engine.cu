@@ -236,9 +236,10 @@ static Workspace carve(int n_blocks, int B, int T, uint32_t flags) {
     // the listed records' carried inter-LSTM state of every block for a slot-list call (gather_h_kernel): h for one-hop
     // calls in the tensor-core form, h and c ([n_blocks][B][97][64] each) for every multi-hop call
     ws.HG = alloc((T > 1 ? 2 : tc_mid_form(B, T, flags) ? 1 : 0) * (int64_t)n_blocks * B * FC);
-    // a call over a list of groups (l2h_sep_forward_targets_groups): the record and hop lists of its target rows
-    // (group_rows_kernel), two int32 per row.  Reserved for every call, so that one size query serves every kind of call.
-    ws.LISTS = alloc(2 * (int64_t)B);
+    // a call over listed groups or target rows (l2h_sep_forward_targets_groups / _rows): the lists target_lists_kernel
+    // builds, five int32 per target row and one more (records, hops, owners, the leads of at most B listeners, the clamped
+    // offsets).  Reserved for every call, so that one size query serves every kind of call.
+    ws.LISTS = alloc(5 * (int64_t)B + 1);
     ws.total = (cur + 511) & ~int64_t(511);      // a multiple of one GX row: pipelined hops address their slots as rows of one tensor
     return ws;
 }
@@ -328,10 +329,15 @@ struct ChainArgs {
     Profiler* prof = nullptr;
     const uint8_t* active = nullptr;     // one-hop calls: [B] device mask of the streams that advance (null: all)
     const int32_t* slots = nullptr;      // [B] device list, row b -> record slots[b] (null: row b -> record b); with targets > 1
-                                         // the [B / targets] group list of l2h_sep_forward_targets_groups
+                                         // the [B / targets] group list of l2h_sep_forward_targets_groups; with targets == 0
+                                         // the [B] record list of l2h_sep_forward_targets_rows
     int state_batch = 0;                 // records in the state (slot lists only)
     const int32_t* hops = nullptr;       // slot lists: [B] device list of the frames each row advances (null: all T); per group
-    int targets = 1;                     // l2h_sep_forward_targets: rows per mixture (B counts target rows; x has B / targets)
+                                         // or listener (one per mixture) with targets != 1
+    int targets = 1;                     // l2h_sep_forward_targets: rows per mixture (B counts target rows; x has B / targets);
+                                         // 0: per listener, from `offsets`
+    const int32_t* offsets = nullptr;    // targets == 0: [calls + 1] device list, mixture i owns target rows offsets[i] ..
+    int calls = 0;                       // offsets[i+1]-1 (l2h_sep_forward_targets_rows); calls: the mixtures
 };
 
 // few streams, one hop (the latency path): everything after the BiLSTM as one 16-CTA cluster kernel per stream, while all
@@ -397,7 +403,6 @@ struct BlockRows {
     int64_t ss;         // record stride
     Map recs;           // record map
     float* X;           // the block's input and output
-    int scale;          // the recurrences take the form of scale x this block's sequences: the call's
     bool ih_written;    // GX holds the intra input projection already: front1_kernel / the previous tail_kernel wrote it
     int gate;           // 1: this block's attn_out (tail_kernel) builds the speaker gate
 };
@@ -410,56 +415,75 @@ template <class Map>
 struct Chain {
     static constexpr bool slots = std::is_same_v<Map, Records>;
     SepEngine* e; const ChainArgs& a; cudaStream_t st; const ChainForm& f; Map recs;
-    int K;              // targets per mixture
+    int K;              // targets per mixture; 0: per listener (l2h_sep_forward_targets_rows)
+    int M;              // mixtures: the rows of block 0 when the chain fans out
+    bool fans;          // several targets per mixture: block 0 runs over the M mixtures, fan_out() makes the target rows
     int64_t ss;         // record stride
-    Map lead;           // K > 1: the record map of block 0's rows, the groups' lead records (rows_of)
+    Map lead;           // fans: the record map of block 0's rows, the mixtures' lead records (rows_of)
+    int64_t lead_ss;    // ... and its record stride
     float *X, *GX, *Y, *Z, *Q, *KALL, *VALL, *PRE, *QKVRAW, *TAPS, *HG, *CG, *sbase;
-    int32_t* lists;     // a list of groups: the target rows' record list, then their hop list (group_rows)
+    float* X0;          // fans: block 0's input and output, the mixtures' rows
+    int32_t* lists;     // listed groups or rows: the lists target_lists() builds (target_lists_kernel), B entries each:
+                        // the target rows' records, their hops, their owners, then the M leads and the M + 1 row offsets
     int tap = 0;
 
     Chain(SepEngine* e_, const ChainArgs& a_, cudaStream_t st_, const ChainForm& f_, Map recs_, const Workspace& ws)
-        : e(e_), a(a_), st(st_), f(f_), recs(recs_), K(a_.targets), ss(stream_stride(e_->n_blocks)) {
+        : e(e_), a(a_), st(st_), f(f_), recs(recs_), K(a_.targets), M(K > 0 ? a_.B / K : a_.calls), fans(K != 1),
+          ss(stream_stride(e_->n_blocks)) {
         float* w = a.wsp;
         X = w + ws.X; GX = w + ws.GX; Y = w + ws.Y; Z = w + ws.Z; Q = w + ws.Q; KALL = w + ws.KALL; VALL = w + ws.VALL;
         PRE = w + ws.PRE; QKVRAW = w + ws.QKVRAW; TAPS = w + ws.TAPS; HG = w + ws.HG;
         CG = HG + (int64_t)e->n_blocks * a.B * FC;
         lists = reinterpret_cast<int32_t*>(w + ws.LISTS);
         sbase = a.state + sizeof(StateHeader) / 4;
-        if constexpr (slots) lead = Records{ss * K, a.slots, a.state_batch / K, a.hops, a.T};      // a.slots: the groups
-        else lead = recs * K;
+        if constexpr (slots) { lead = Records{ss, lists + 3 * (int64_t)a.B, a.state_batch, a.hops, a.T}; lead_ss = ss; }
+        else { lead = recs * K; lead_ss = ss * K; }
+        // block 0's rows go in room of GX that block 0 leaves unused; with more than 8/9 as many mixtures as target rows
+        // (many single-target listeners) there is none, and they go in X, which fan_out() moves to GX before fanning out
+        const int64_t rows0 = (int64_t)M * a.T * NF;
+        X0 = rows0 * (512 + 64) <= (int64_t)a.B * a.T * NF * 512 ? GX + rows0 * 512 : X;
     }
 
     // Several targets per mixture (l2h_sep_forward_targets): B counts target rows, K per mixture, row i*K + k = target k of
     // mixture i.  The front and block 0 do not depend on the speaker (its gate applies after block 0), so they run once
-    // per mixture: over B / K rows, on the lead records i*K (record stride K*ss), without the gate, into room in GX that
-    // block 0 leaves unused.  fan_out() then builds every target row's gate memo and its gated copy of block 0's output
-    // in X, and blocks 1 .. n_blocks-1 and the back run over all B rows.  Every form was chosen for the B rows, and
-    // block 0 runs those same forms, so a target row gets the arithmetic of a dense call with its mixture duplicated.
-    // Over a list of groups (l2h_sep_forward_targets_groups) block 0's map is the group list with record stride K*ss and
-    // the groups' hop counts, which addresses lead record g*K; the target rows' map is the list group_rows() builds.
+    // per mixture: over M = B / K rows, on the lead records i*K (record stride K*ss), without the gate, into X0.
+    // fan_out() then builds every target row's gate memo and its gated copy of block 0's output in X, and blocks 1 ..
+    // n_blocks-1 and the back run over all B rows.  Every form was chosen for the B rows, and block 0 runs those same
+    // forms, so a target row gets the arithmetic of a dense call with its mixture duplicated.
+    // Over listed groups or rows (l2h_sep_forward_targets_groups / _rows) block 0's map is the lead list target_lists()
+    // builds, with the listeners' hop counts, and the target rows' map is its record list: a listener's rows need not be
+    // K, adjacent or in order.
     BlockRows<Map> rows_of(int b) const {
-        const bool lead_rows = K > 1 && b == 0;
-        BlockRows<Map> r{lead_rows ? a.B / K : a.B, 0, lead_rows ? ss * K : ss, lead_rows ? lead : recs, X, lead_rows ? K : 1,
-                         f.fused_tail && !fans_out_before(b), (b == 0 && e->n_blocks > 1 && K == 1) ? 1 : 0};
+        const bool lead_rows = fans && b == 0;
+        BlockRows<Map> r{lead_rows ? M : a.B, 0, lead_rows ? lead_ss : ss, lead_rows ? lead : recs, lead_rows ? X0 : X,
+                         f.fused_tail && !fans_out_before(b), (b == 0 && e->n_blocks > 1 && !fans) ? 1 : 0};
         r.rows = (int64_t)r.B * a.T * NF;
-        if (lead_rows) r.X = GX + r.rows * 512;
         return r;
     }
-    bool fans_out_before(int b) const { return K > 1 && b == 1; }      // b == n_blocks: before the back
+    bool fans_out_before(int b) const { return fans && b == 1; }      // b == n_blocks: before the back
     int fan_out() {
+        const float* x0 = X0;
+        if (X0 == X) {      // block 0 ran in X: GX is free after it
+            CK(cudaMemcpyAsync(GX, X, (size_t)M * a.T * FC * sizeof(float), cudaMemcpyDeviceToDevice, st));
+            x0 = GX;
+        }
+        const int32_t* owner = nullptr;      // dense targets: row r belongs to mixture r / K
+        if constexpr (slots) owner = lists + 2 * (int64_t)a.B;
         CK(launch_k(f.pdl, spk_gate_kernel_t<Map>, dim3(a.B), dim3(256), 0, st, a.emb, PRE, a.state, recs, e->w));
-        CK(launch_k(f.pdl, gate_fanout_kernel_t<Map>, dim3(a.T, a.B), dim3(256), 0, st, (const float*)rows_of(0).X, X,
-                    (const float*)a.state, recs, K, a.T, e->n_blocks > 1 ? 1 : 0));
+        CK(launch_k(f.pdl, gate_fanout_kernel_t<Map>, dim3(a.T, a.B), dim3(256), 0, st, x0, X, (const float*)a.state, recs, owner, K,
+                    a.T, e->n_blocks > 1 ? 1 : 0));
         MARK("gate_fanout");
         return 0;
     }
-    // a list of groups: the target rows' record list (and hop list) from the group list, before any kernel reads them
-    int group_rows() {
+    // listed groups or rows: the target rows' lists and the leads, before any kernel reads them
+    int target_lists() {
         if constexpr (slots) {
-            if (K > 1) {
-                CK(launch_k(false, group_rows_kernel, dim3((unsigned)((a.B + 255) / 256)), dim3(256), 0, st, a.slots, a.hops,
-                            a.state_batch / K, K, a.B, lists, lists + a.B));
-                MARK("group_rows");
+            if (fans) {
+                const int64_t B = a.B;
+                CK(launch_k(false, target_lists_kernel, dim3(1), dim3(1024), 0, st, a.offsets ? a.slots : nullptr, a.offsets,
+                            a.offsets ? nullptr : a.slots, a.hops, M, K, a.B, a.state_batch, lists, lists + B, lists + 2 * B,
+                            lists + 3 * B, lists + 4 * B));
+                MARK("target_lists");
             }
         }
         return 0;
@@ -519,7 +543,7 @@ struct Chain {
                 if (inter && R.recs.hops) CK(launch_k(false, inter_gate_mask_kernel, dim3(a.T, R.B), dim3(256), 0, st, GX, R.recs, a.T));
             }
             if (rf.tc) CK(launch_tc_lstm(l, e->tc_passes, st, f.pdl));
-            else CK(launch_lstm_rec(l, st, f.pdl, l.nseq * R.scale));
+            else CK(launch_lstm_rec(l, st, f.pdl, l.nseq / R.B * a.B));      // the form of the call's sequences
         }
         MARK(inter ? "lstm_inter" : "lstm_intra");
         return 0;
@@ -528,13 +552,13 @@ struct Chain {
     // Slot lists: one-hop tensor-core chains read the listed records' h of every block for the inter-step GEMMs, and
     // multi-hop calls carry their (h, c) through the inter recurrences, from a copy in the workspace (HG, CG) that
     // gather_hc() takes before block 0 and scatter_hc() stores back after the last block's inter recurrence.  Block b's
-    // part holds the rows of rows_of(b) (inter_hc): over a list of groups, block 0's part holds the lead rows.
+    // part holds the rows of rows_of(b) (inter_hc): over listed groups or rows, block 0's part holds the lead rows.
     // hc_copy: gather_h_kernel or scatter_hc_kernel over the blocks from b0 on that share rows_of(b0)'s record map.  The
     // kernels address block `blk` of a record from the state pointer they get, so a pointer b0 blocks further makes their
     // block 0 block b0 of the records.
     int hc_copy(bool scatter, int b0) {
         const BlockRows<Map> R = rows_of(b0);
-        const int nb = (K > 1 && b0 == 0) ? 1 : e->n_blocks - b0;
+        const int nb = (fans && b0 == 0) ? 1 : e->n_blocks - b0;
         const int64_t o = (int64_t)b0 * R.B * FC;
         const dim3 grid((unsigned)(((int64_t)nb * R.B * FC / 4 + 255) / 256));      // one thread per float4 of h (and c)
         if (scatter)
@@ -549,7 +573,7 @@ struct Chain {
         if constexpr (slots) {
             if (f.tc_mid || a.T > 1) {
                 if (int rc = hc_copy(false, 0)) return rc;
-                if (K > 1 && e->n_blocks > 1) { if (int rc = hc_copy(false, 1)) return rc; }
+                if (fans && e->n_blocks > 1) { if (int rc = hc_copy(false, 1)) return rc; }
             }
         }
         return 0;
@@ -576,7 +600,7 @@ struct Chain {
     int scatter_hc() {
         if constexpr (slots) {
             if (int rc = hc_copy(true, 0)) return rc;
-            if (K > 1 && e->n_blocks > 1) { if (int rc = hc_copy(true, 1)) return rc; }
+            if (fans && e->n_blocks > 1) { if (int rc = hc_copy(true, 1)) return rc; }
         }
         return 0;
     }
@@ -595,10 +619,10 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
     const ChainForm f = chain_form<Map>(e, a.B, T, a.flags, a.prof != nullptr);
     Chain<Map> c(e, a, st, f, recs, ws);
     MARK("start");
-    if (int rc = c.group_rows()) return rc;
+    if (int rc = c.target_lists()) return rc;
     if (int rc = c.gather_hc()) return rc;
     const BlockRows<Map> R0 = c.rows_of(0);           // the front runs over block 0's rows
-    const int gate_ctas = c.K > 1 ? 0 : 1;            // the front's speaker-gate memo CTAs (one per row); fan_out() builds them here
+    const int gate_ctas = c.fans ? 0 : 1;             // the front's speaker-gate memo CTAs (one per row); fan_out() builds them here
     if (f.fused_tail) {      // the frame as 13 row tiles: spectrum of the tile's bins, conv, and block 0's input projection
         CK(launch_front1(false, st, R0.B, gate_ctas, a.x, a.xbs, a.xcs, a.x_len, R0.X, a.state, R0.recs, e->w, e->bw[0], c.GX, a.pos_rel,
                          a.emb, c.PRE, a.active));
@@ -732,8 +756,8 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
 
 static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
     const int64_t ss = stream_stride(e->n_blocks);
-    if (a.slots && a.targets > 1) {      // a list of groups: the target rows' record (and hop) lists that Chain::group_rows
-                                         // builds in the workspace at the start of the call
+    if (a.slots && a.targets != 1) {     // listed groups or rows: the target rows' record (and hop) lists that
+                                         // Chain::target_lists builds in the workspace at the start of the call
         const int32_t* lists = reinterpret_cast<const int32_t*>(a.wsp + carve(e->n_blocks, a.B, a.T, a.flags).LISTS);
         return enqueue_chain_t(e, a, st, Records{ss, lists, a.state_batch, a.hops ? lists + a.B : nullptr, a.T});
     }
@@ -977,7 +1001,7 @@ static void drop_graphs(SepEngine* e) {
 static std::vector<int64_t> graph_key(const ChainArgs& a, int t) {
     return {(int64_t)a.x, a.xbs, a.xcs, a.x_len, (int64_t)a.emb, (int64_t)a.state, (int64_t)a.y,
             a.ybs, a.ycs, a.y_len, a.B, t, (int64_t)a.wsp, (int64_t)a.flags, a.pos_rel, (int64_t)a.active,
-            (int64_t)a.slots, a.state_batch, (int64_t)a.hops, a.targets};
+            (int64_t)a.slots, a.state_batch, (int64_t)a.hops, a.targets, (int64_t)a.offsets, a.calls};
 }
 
 // Launch the graph cached under `key` on `st`.  The first time a key is seen, `enqueue(cap)` is captured on the private
@@ -1366,6 +1390,34 @@ int l2h_sep_forward_targets_groups(void* handle, const float* x, int64_t xbs, in
     a.state_batch = state_batch;
     a.hops = hops_dev;
     a.targets = n_targets;
+    return run_chain(e, a, static_cast<cudaStream_t>(stream), (flags & L2H_FLAG_GRAPH) != 0);
+}
+
+int l2h_sep_forward_targets_rows(void* handle, const float* x, int64_t xbs, int64_t xcs, int32_t x_len, const float* emb,
+                                 void* state, int32_t state_batch, const int32_t* records_dev, const int32_t* offsets_dev,
+                                 const int32_t* hops_dev, int32_t n, int32_t n_rows, int32_t frames, float* y, int64_t ybs,
+                                 int64_t ycs, int32_t y_len, void* ws, size_t ws_bytes, uint32_t flags, void* stream) {
+    SepEngine* e = static_cast<SepEngine*>(handle);
+    if (!e || !x || !emb || !state || !y || !ws || !records_dev || !offsets_dev) return fail(1, "null argument");
+    if (n <= 0 || n_rows <= 0 || frames <= 0)
+        return fail(1, "a target rows call needs n, n_rows and frames > 0 (n = " + std::to_string(n) + ", n_rows = " +
+                           std::to_string(n_rows) + ", frames = " + std::to_string(frames) + ")");
+    if (n_rows > state_batch)
+        return fail(1, "a target rows call needs n_rows <= state_batch (n_rows = " + std::to_string(n_rows) + ", state_batch = " +
+                           std::to_string(state_batch) + ")");
+    if (n > n_rows)      // the mixtures' rows of the front and block 0 live in the workspace of the n_rows target rows
+        return fail(1, "a target rows call needs n <= n_rows (n = " + std::to_string(n) + ", n_rows = " + std::to_string(n_rows) + ")");
+    if ((int64_t)n_rows * frames * NF > 0x7fffffff / 2) return fail(1, "n_rows*frames too large for one call; split the rows");
+    if (flags & L2H_FLAG_TAPS) return fail(1, "a target rows call cannot be combined with L2H_FLAG_TAPS");
+    if (int rc_dev = check_device(e)) return rc_dev;
+    ChainArgs a{x, xbs, xcs, x_len, emb, static_cast<float*>(state), y, ybs, ycs, y_len, n_rows, frames,
+                static_cast<float*>(ws), ws_bytes, flags & ~L2H_FLAG_GRAPH, 0};
+    a.slots = records_dev;
+    a.state_batch = state_batch;
+    a.hops = hops_dev;
+    a.targets = 0;
+    a.offsets = offsets_dev;
+    a.calls = n;
     return run_chain(e, a, static_cast<cudaStream_t>(stream), (flags & L2H_FLAG_GRAPH) != 0);
 }
 

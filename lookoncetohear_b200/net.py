@@ -362,16 +362,19 @@ class Net(nn.Module):
     def _stream_workspace(self, device, batch, chunks_per_call):
         return self._cached_workspace(device, _cabi.lib().l2h_sep_stream_workspace_bytes, batch, chunks_per_call)
 
-    def _launch(self, entry, x, emb, state, y, frames, flags=0, mask=None, slots=None, hops=None, K=1, ws=None):
+    def _launch(self, entry, x, emb, state, y, frames, flags=0, mask=None, slots=None, hops=None, K=1, ws=None,
+                offsets=None):
         """Run the separator forward C entry point `entry` on the current stream of x's device, on the caller's tensors as
         they are (a service's fixed buffers keep the cached graph's key).  entry: "forward", "forward_active", "slots",
-        "slots_frames", "slots_hops", "targets" or "targets_groups" (l2h_sep_forward, l2h_sep_forward_<entry>).
+        "slots_frames", "slots_hops", "targets", "targets_groups" or "targets_rows" (l2h_sep_forward,
+        l2h_sep_forward_<entry>).
 
         x [rows_x, M, N]; emb [rows, 256]; y [rows, S, N], or for the targets calls [rows_x, K, S, N], passed as its
-        [rows, S, N] view; rows = rows_x * K.  mask: the [rows] uint8 activity mask of forward_active (None: all);
-        slots: the int32 slot list (the group list of targets_groups); hops: the int32 hop counts (None: every row all
-        frames).  ws: a workspace to use, else the net's own, sized for rows and frames.  A rejected argument raises
-        ValueError, except on the dense entries, where every error is a RuntimeError."""
+        [rows, S, N] view; rows = rows_x * K, or for targets_rows the target rows of y.  mask: the [rows] uint8 activity
+        mask of forward_active (None: all); slots: the int32 slot list (the group list of targets_groups, the record list
+        of targets_rows); offsets: the int32 [rows_x + 1] row offsets of targets_rows; hops: the int32 hop counts (None:
+        every row all frames).  ws: a workspace to use, else the net's own, sized for rows and frames.  A rejected argument
+        raises ValueError, except on the dense entries, where every error is a RuntimeError."""
         dev = x.device
         self._sync_weights(dev)
         if y.dim() == 4:
@@ -397,6 +400,8 @@ class Net(nn.Module):
                 args = (*head, *listed, hop_list, n, frames, *out, *tail)
             elif entry == "targets":
                 args = (*head, *out, n, K, frames, *tail)
+            elif entry == "targets_rows":
+                args = (*head, *listed, offsets.data_ptr(), hop_list, n, y.shape[0], frames, *out, *tail)
             else:
                 args = (*head, *listed, hop_list, n, K, frames, *out, *tail)
             fn = getattr(_cabi.lib(), "l2h_sep_" + entry if entry.startswith("forward") else "l2h_sep_forward_" + entry)
@@ -486,13 +491,17 @@ class Net(nn.Module):
     _LIST_WORDS = {"slot": ("integer slot indices", "slots lists {} records for {} input rows",
                             "a slot lies outside [0, {end})"),
                    "hop": ("integer hop counts", "hops gives {} counts for {} input rows",
-                           "a hop count lies outside [0, {last}] (the call's {last} hops)")}
+                           "a hop count lies outside [0, {last}] (the call's {last} hops)"),
+                   "record": ("integer record indices", "records lists {} records for {} target rows",
+                              "a record lies outside [0, {end})"),
+                   "offset": ("integer row offsets", "offsets gives {} entries for {} = input rows + 1",
+                              "an offset lies outside [0, {last}] (the call's {last} target rows)")}
 
     @classmethod
     def _device_list(cls, values, dev, n, end, distinct, noun):
-        """`values` (slots, groups or hop counts of a call of n rows) as the [n] int32 device tensor the engine reads.  A
+        """`values` (slots, groups, records, offsets or hop counts of a call of n rows) as the [n] int32 device tensor the engine reads.  A
         CUDA int32 tensor is used as it is (its entries are read when the kernels run); anything else is checked here (n
-        ints in [0, end), each listed once if `distinct`) and uploaded.  noun: "slot" or "hop", for the messages."""
+        ints in [0, end), each listed once if `distinct`) and uploaded.  noun: a key of _LIST_WORDS, for the messages."""
         entries, count, outside = cls._LIST_WORDS[noun]
         if isinstance(values, torch.Tensor) and values.is_cuda:
             if values.dtype != torch.int32 or tuple(values.shape) != (n,) or not values.is_contiguous():
@@ -684,6 +693,51 @@ class Net(nn.Module):
             hops = self._hop_counts(hops, x.device, n, frames)
         groups = self._slot_list(groups, x.device, n, state.batch // K)
         return self._run_targets("targets_groups", x, embeds, state, frames, out_len, groups, hops)
+
+    def advance_target_rows(self, x, embeds, state, records, offsets, hops=None):
+        """Advance listeners who each enrolled their own number of speakers by T hops each, in one call
+        (l2h_sep_forward_targets_rows): advance_targets without its one K for every listener.  x [n, M, 128*T + 64] (the
+        pad=False shape), row i listener i's mixture; embeds [R, 256], one row per target row; listener i owns target rows
+        offsets[i] .. offsets[i+1]-1, and target row r continues record records[r] of `state`.  Returns y [R, S, 128*T]:
+        row r is target row r's speaker.  Rows from offsets[n] on belong to no listener: they store nothing and their y rows
+        are left unwritten, so one fixed R carries any number of live targets.
+
+        A listener's lead record, records[offsets[i]], also holds its mixture's front and block 0; its other records never
+        do, so reset a listener's records together (reset_streams of all of them) before its first call.  Records need not
+        be adjacent or in order.  Host lists (sequences or CPU tensors) are checked and uploaded: `records` R distinct ints
+        in [0, state.batch); `offsets` n + 1 ints from 0, non-decreasing, at most R; `hops` as for advance_targets (None:
+        every listener advances T hops; else h_i in [0, T], and listener i's rows receive y[r, :, :128*h_i] only).  CUDA
+        int32 tensors are used in place and read when the kernels run: there a record outside the state marks a row that
+        stores nothing, and the engine clamps the offsets to be non-decreasing and at most R.  With fixed tensors rewritten in
+        place every tick, one cached graph per (n, R, T) serves every mix of listeners."""
+        if x.dim() != 3:
+            raise ValueError(f"advance_target_rows needs x of shape [n, channels, {self.stft_chunk_size}*T+"
+                             f"{self.stft_pad_size}], got {tuple(x.shape)}")
+        if not isinstance(embeds, torch.Tensor) or embeds.dim() != 2 or embeds.shape[1] != self.embed_dim:
+            shape = tuple(embeds.shape) if isinstance(embeds, torch.Tensor) else type(embeds).__name__
+            raise ValueError(f"embeds must have shape [R, {self.embed_dim}], one row per target row, got {shape}")
+        frames, out_len = self._frames(x.shape[-1], who="advance_target_rows", per=" per row")
+        if not isinstance(state, SepState):
+            raise TypeError("state must come from Net.init_buffers()")
+        n, R = x.shape[0], embeds.shape[0]
+        if not 0 < n <= R <= state.batch:
+            raise ValueError(f"advance_target_rows needs 0 < n <= R <= state.batch, got n = {n} listeners, R = {R} target "
+                             f"rows and a state of {state.batch} records")
+        dev = x.device
+        if hops is not None:
+            hops = self._hop_counts(hops, dev, n, frames)
+        records = self._device_list(records, dev, R, state.batch, True, "record")
+        on_host = not (isinstance(offsets, torch.Tensor) and offsets.is_cuda)
+        offsets_dev = self._device_list(offsets, dev, n + 1, R + 1, False, "offset")
+        if on_host:
+            o = torch.as_tensor(offsets).tolist()
+            if o[0] != 0 or any(b < a for a, b in zip(o, o[1:])):
+                raise ValueError(f"offsets must start at 0 and never decrease, got {o}")
+        self._require_cuda(x)
+        y = torch.empty(R, self.num_src, out_len, dtype=torch.float32, device=dev)
+        self._launch("targets_rows", x.contiguous().float(), embeds.to(dev, torch.float32).contiguous(), state, y, frames,
+                     slots=records, hops=hops, offsets=offsets_dev)
+        return y
 
     def stream_dev(self, x_dev, embed_dev, chunks_per_call=1, state=None, n_calls=None, out=None):
         """Streaming over a device-resident clip (l2h_sep_stream_dev): x_dev [B,M,N] is consumed
