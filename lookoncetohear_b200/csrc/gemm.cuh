@@ -360,22 +360,35 @@ inline cudaError_t launch_rows_gemm_cfg(const GemmArgs& g, cudaStream_t st, bool
     return launch_k(pdl, rows_gemm_kernel<BM, BN, TM, TN>, grid, dim3(NT), smem, st, g);
 }
 
+// The kernel launch_rows_gemm runs for a problem (none: the problem is refused).
+enum class RowsGemmForm { none, tile16x64, tile64x64, tile64x128, big64, big128 };
+
 // Pick a tile by problem size: small M (one streaming frame = 97 rows) wants many small CTAs,
 // large M wants the 64x128 tile.  N must be a multiple of 64; K a multiple of 64.
 // `shape`: 0 = by size (below); 1 = 64x64 tiles, 2 = the persistent 128-row form, whatever M is (the pipelined graph's 4-hop
 // batches of 388 rows: fewer, fatter CTAs compete less with the other stages' kernels)
-inline cudaError_t launch_rows_gemm(const GemmArgs& g, cudaStream_t st, bool pdl = false, int shape = 0) {
-    if (g.N % 64 != 0 || g.K % 64 != 0 || g.M <= 0) return cudaErrorInvalidValue;
-    if (g.ln_g && g.K != 64) return cudaErrorInvalidValue;
-    if (shape == 1) return launch_rows_gemm_cfg<64, 64, 4, 4>(g, st, pdl);
-    if (g.M <= 2048 && shape == 0) return launch_rows_gemm_cfg<16, 64, 2, 4>(g, st, pdl);     // 128 threads
+inline RowsGemmForm rows_gemm_form(const GemmArgs& g, int shape) {
+    if (g.N % 64 != 0 || g.K % 64 != 0 || g.M <= 0) return RowsGemmForm::none;
+    if (g.ln_g && g.K != 64) return RowsGemmForm::none;
+    if (shape == 1) return RowsGemmForm::tile64x64;
+    if (g.M <= 2048 && shape == 0) return RowsGemmForm::tile16x64;
     {   // large M: persistent kernel with the weight slab resident in shared memory (when it fits)
         const int bn = (g.N % 128 == 0) ? 128 : 64;
         const size_t smem = ((size_t)g.K * bn + (size_t)GK * 132) * sizeof(float);
-        if (smem <= 200 * 1024) return bn == 128 ? launch_rows_gemm_big<128>(g, st, pdl) : launch_rows_gemm_big<64>(g, st, pdl);
+        if (smem <= 200 * 1024) return bn == 128 ? RowsGemmForm::big128 : RowsGemmForm::big64;
     }
-    if (g.N % 128 == 0) return launch_rows_gemm_cfg<64, 128, 4, 8>(g, st, pdl); // 256 threads
-    return launch_rows_gemm_cfg<64, 64, 4, 4>(g, st, pdl);                      // 256 threads
+    return g.N % 128 == 0 ? RowsGemmForm::tile64x128 : RowsGemmForm::tile64x64;
+}
+
+inline cudaError_t launch_rows_gemm(const GemmArgs& g, cudaStream_t st, bool pdl = false, int shape = 0) {
+    switch (rows_gemm_form(g, shape)) {
+        case RowsGemmForm::tile16x64: return launch_rows_gemm_cfg<16, 64, 2, 4>(g, st, pdl);      // 128 threads
+        case RowsGemmForm::tile64x64: return launch_rows_gemm_cfg<64, 64, 4, 4>(g, st, pdl);      // 256 threads
+        case RowsGemmForm::tile64x128: return launch_rows_gemm_cfg<64, 128, 4, 8>(g, st, pdl);    // 256 threads
+        case RowsGemmForm::big64: return launch_rows_gemm_big<64>(g, st, pdl);
+        case RowsGemmForm::big128: return launch_rows_gemm_big<128>(g, st, pdl);
+        default: return cudaErrorInvalidValue;
+    }
 }
 
 }  // namespace l2h

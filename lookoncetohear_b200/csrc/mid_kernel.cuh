@@ -19,6 +19,7 @@
 // epilogue.  Weights and activations are stored in k-slices padded by 4 floats so that the 8 lanes of a
 // quarter-warp (one LDS.128 phase) hit 32 distinct banks.
 #pragma once
+#include <algorithm>
 #include "common.cuh"
 #include "sep_kernels.cuh"
 
@@ -52,6 +53,24 @@ static_assert((MID_W3A % 4) == 0 && (MID_W3B % 4) == 0 && (MID_W5 % 4) == 0 && (
 __host__ __device__ constexpr int mid_aidx(int ks, int k, int r) { return (k / ks) * (ks * MID_RT + 4) + (k % ks) * MID_RT + r; }
 // index of weight (k, n) in a k-sliced [K][N] matrix
 __host__ __device__ constexpr int mid_widx(int ks, int n_cols, int k, int n) { return (k / ks) * (ks * n_cols + 4) + (k % ks) * n_cols + n; }
+
+// host: BlockWeights::mid_pack (MID_PACK floats, padding zeroed) from the five matrices as the engine stores them, W^T
+// [K][N]: wl1_t [128][64], wih2_t and whh2_t [64][256] (gate column j*4 + q), wl2_t [64][64], wqkv_t [64][NQKV]
+inline void mid_pack_weights(const float* wl1_t, const float* wih2_t, const float* whh2_t, const float* wl2_t, const float* wqkv_t,
+                             float* dst) {
+    std::fill(dst, dst + MID_PACK, 0.f);
+    for (int k = 0; k < M1_K; ++k)
+        for (int n = 0; n < M1_N; ++n) dst[MID_W1 + mid_widx(M1_KS, M1_N, k, n)] = wl1_t[(int64_t)k * 64 + n];
+    for (int k = 0; k < M3_K; ++k)
+        for (int n = 0; n < M3_N; ++n) {
+            dst[MID_W3A + mid_widx(M3_KS, M3_N, k, n)] = wih2_t[(int64_t)k * 256 + n];
+            dst[MID_W3B + mid_widx(M3_KS, M3_N, k, n)] = whh2_t[(int64_t)k * 256 + n];
+        }
+    for (int k = 0; k < M5_K; ++k)
+        for (int n = 0; n < M5_N; ++n) dst[MID_W5 + mid_widx(M5_KS, M5_N, k, n)] = wl2_t[(int64_t)k * 64 + n];
+    for (int k = 0; k < M6_K; ++k)
+        for (int n = 0; n < M6_N; ++n) dst[MID_W6 + mid_widx(M6_KS, M6_N, k, n)] = wqkv_t[(int64_t)k * NQKV + n];
+}
 
 // sum v[] over the KQ adjacent lanes of a group; lane kq keeps the kq-th chunk of NV / KQ values in v[0 ..)
 template <int HALF, int BIT, int NV>

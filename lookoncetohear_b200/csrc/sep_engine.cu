@@ -254,8 +254,7 @@ static int set_attrs() {
     if (g_attr_done[dev_ord]) return 0;
     CK(set_sep_smem<int64_t>());
     CK(set_sep_smem<Records>());      // the slot-list forms (l2h_sep_forward_slots)
-    CK(cudaFuncSetAttribute(mid_a_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_A_SMEM));
-    CK(cudaFuncSetAttribute(mid_c_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_C_SMEM));
+    CK(set_mid_split_smem());
     CK(configure_rows_gemm());
     CK(configure_lstm());
     CK(umma::configure());
@@ -669,8 +668,7 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
                 const cudaError_t ce = umma::launch(q, st, &why);
                 if (ce != cudaSuccess) return fail(3, std::string("umma_gemm (inter step): ") + cudaGetErrorString(ce) + " " + why);
             }
-            CK(launch_k(f.mid_pdl, lstm_cell_rows_kernel_t<Map>, dim3((unsigned)((R.rows * 64 + 255) / 256)), dim3(256), 0, st,
-                        (const float*)c.GX, a.state, R.recs, b, c.Y, (int)R.rows, a.active));
+            CK(launch_lstm_cell_rows(f.mid_pdl, st, c.GX, a.state, R.recs, b, c.Y, R.rows, a.active));
             if (int rc = c.dense(b, PL_L2, R, f.mid_pdl)) return rc;
             if (int rc = tc_rows_gemm(e, b, PL_QKV, R.X, 64, 64, NQKV, nullptr, nullptr, W.bqkv, W.slope_vec, nullptr, c.QKVRAW, NQKV, R.rows,
                                       st, f.mid_pdl)) return rc;
@@ -693,8 +691,7 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
             if (int rc = c.do_tap()) return rc;
             continue;
         } else if (f.row_mid) {
-            CK(launch_k(f.pdl, mid_kernel_t<Map>, mid_grid_for(R.B, 1), dim3(256), MID_SMEM, st, (const float*)c.Y, R.X, c.QKVRAW, a.state, R.recs,
-                        b, W, R.B, a.active));
+            CK(launch_mid(f.pdl, st, c.Y, R.X, c.QKVRAW, a.state, R.recs, b, W, R.B, a.active));
             MARK("mid");
         } else {
             if (int rc = c.dense(b, PL_L1, R, f.pdl)) return rc;
@@ -1132,20 +1129,8 @@ int l2h_sep_commit_weights(void* handle, void* stream) {
     float* h = e->pack.host.data();
     for (const auto& m : e->mid_src)        // per-column PReLU slopes of the fused Q|K|V projection
         for (int n = 0; n < NQKV; ++n) h[m.slope_vec + n] = h[m.slopes + (n < NHEAD * QE ? 0 : (n < 2 * NHEAD * QE ? 1 : 2))];
-    for (const auto& m : e->mid_src) {      // k-sliced, bank-padded copies for mid_kernel (layout: mid_kernel.cuh)
-        std::fill(h + m.dst, h + m.dst + MID_PACK, 0.f);
-        for (int k = 0; k < M1_K; ++k)
-            for (int n = 0; n < M1_N; ++n) h[m.dst + MID_W1 + mid_widx(M1_KS, M1_N, k, n)] = h[m.wl1 + (int64_t)k * 64 + n];
-        for (int k = 0; k < M3_K; ++k)
-            for (int n = 0; n < M3_N; ++n) {
-                h[m.dst + MID_W3A + mid_widx(M3_KS, M3_N, k, n)] = h[m.wih2 + (int64_t)k * 256 + n];
-                h[m.dst + MID_W3B + mid_widx(M3_KS, M3_N, k, n)] = h[m.whh2t + (int64_t)k * 256 + n];
-            }
-        for (int k = 0; k < M5_K; ++k)
-            for (int n = 0; n < M5_N; ++n) h[m.dst + MID_W5 + mid_widx(M5_KS, M5_N, k, n)] = h[m.wl2 + (int64_t)k * 64 + n];
-        for (int k = 0; k < M6_K; ++k)
-            for (int n = 0; n < M6_N; ++n) h[m.dst + MID_W6 + mid_widx(M6_KS, M6_N, k, n)] = h[m.wqkv + (int64_t)k * NQKV + n];
-    }
+    for (const auto& m : e->mid_src)        // k-sliced, bank-padded copies for mid_kernel (layout: mid_kernel.cuh)
+        mid_pack_weights(h + m.wl1, h + m.wih2, h + m.whh2t, h + m.wl2, h + m.wqkv, h + m.dst);
     int cur = -1;
     CK(cudaGetDevice(&cur));
     if (e->pack.dev != nullptr && e->pack.device != cur)    // the module moved to another GPU: everything device-side is rebuilt there

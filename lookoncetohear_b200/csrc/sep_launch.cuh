@@ -58,6 +58,13 @@ static inline cudaError_t set_sep_smem() {
     return cudaSuccess;
 }
 
+// dynamic shared memory of mid_a_kernel and mid_c_kernel, which address no records (one form serves every call)
+static inline cudaError_t set_mid_split_smem() {
+    cudaError_t e = cudaFuncSetAttribute(mid_a_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_A_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(mid_c_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_C_SMEM);
+    return e;
+}
+
 // front_kernel: grid (T + gate, B), the T frames and, with gate = 1, each stream's speaker-gate memo CTA
 template <class Map>
 inline cudaError_t launch_front(bool pdl, cudaStream_t st, int B, int gate, const float* x, int64_t x_bstride, int64_t x_cstride,
@@ -82,6 +89,13 @@ inline cudaError_t launch_front1(bool pdl, cudaStream_t st, int B, int gate, con
     return launch_k(pdl, front1_kernel_t<Map>, dim3(TAIL_TILES + gate, B), dim3(256), FRONT1_SMEM, st, x, x_bstride, x_cstride, x_len,
                     X, state, recs, w, w0, GX, pos_rel, emb, spk_pre, active);
 }
+// the middle section in one kernel, persistent over (stream, row tile) items, one CTA per SM
+template <class Map>
+inline cudaError_t launch_mid(bool pdl, cudaStream_t st, const float* Y, float* X, float* QKV, float* state, Map recs, int blk,
+                              const BlockWeights& w, int n_streams, const uint8_t* active) {
+    return launch_k(pdl, mid_kernel_t<Map>, mid_grid_for(n_streams, 1), dim3(256), MID_SMEM, st, Y, X, QKV, state, recs, blk, w,
+                    n_streams, active);
+}
 // the middle section in three kernels, each persistent over (stream, row tile) items
 inline cudaError_t launch_mid_a(bool pdl, cudaStream_t st, const float* Y, float* X, float* GI, const BlockWeights& w, int n_streams,
                                 int64_t hop_stride, int n_hops) {
@@ -96,6 +110,13 @@ inline cudaError_t launch_mid_b(bool pdl, cudaStream_t st, const float* GI, floa
 inline cudaError_t launch_mid_c(bool pdl, cudaStream_t st, const float* Hn, float* X, float* QKV, const BlockWeights& w, int n_streams,
                                 int64_t hop_stride, int n_hops) {
     return launch_k(pdl, mid_c_kernel, mid_grid_for(n_streams, 4), dim3(256), MID_C_SMEM, st, Hn, X, QKV, w, n_streams, hop_stride, n_hops);
+}
+// lstm_cell_rows_kernel: one thread per (row, hidden unit)
+template <class Map>
+inline cudaError_t launch_lstm_cell_rows(bool pdl, cudaStream_t st, const float* gates, float* state, Map recs, int blk, float* Hout,
+                                         int64_t rows, const uint8_t* active) {
+    return launch_k(pdl, lstm_cell_rows_kernel_t<Map>, dim3((unsigned)((rows * 64 + 255) / 256)), dim3(256), 0, st, gates, state, recs,
+                    blk, Hout, (int)rows, active);
 }
 // qkv_kernel: grid (T, B); the projections run inside (pre == nullptr) or are given, with less shared memory
 template <class Map>

@@ -78,15 +78,32 @@ class EmbBlock(ctypes.Structure):
     _fields_ = [(n, ctypes.c_void_p) for n in ("gq", "bq", "gk", "bk", "gv", "bv", "wp_t", "bp", "slope_p", "gp", "bpn")]
 
 
+class RowsGemm(ctypes.Structure):
+    """GemmArgs (gemm.cuh) field for field"""
+    _fields_ = [("A", ctypes.c_void_p), ("lda", ctypes.c_int64), ("a_rows_per_seq", ctypes.c_int32),
+                ("a_seq_stride", ctypes.c_int64), ("Wt", ctypes.c_void_p), ("bias", ctypes.c_void_p), ("C", ctypes.c_void_p),
+                ("ldc", ctypes.c_int64), ("c_rows_per_seq", ctypes.c_int32), ("c_seq_stride", ctypes.c_int64),
+                ("c_inner", ctypes.c_int32), ("c_inner_stride", ctypes.c_int64)] + \
+               [(n, ctypes.c_void_p) for n in ("R", "ln_g", "ln_b", "prelu", "prelu_vec")] + \
+               [("M", ctypes.c_int32), ("N", ctypes.c_int32), ("K", ctypes.c_int32)]
+
+
+class MidWeights(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_void_p) for n in ("mid_pack", "bl1", "ln2_g", "ln2_b", "b2", "bl2", "bqkv", "slopes")]
+
+
 MIRRORS = {"kh_sizeof_asource": ASource, "kh_sizeof_gemm": Gemm, "kh_sizeof_plan": Plan, "kh_sizeof_lstm": Lstm,
            "kh_sizeof_sep_weights": SepWeights, "kh_sizeof_sep_front_back": SepFrontBack,
-           "kh_sizeof_emb_weights": EmbWeights, "kh_sizeof_emb_block": EmbBlock}
+           "kh_sizeof_emb_weights": EmbWeights, "kh_sizeof_emb_block": EmbBlock, "kh_sizeof_rows_gemm": RowsGemm,
+           "kh_sizeof_mid_weights": MidWeights}
+MID_SYMBOLS = ("kh_rows_gemm", "kh_rows_gemm_form", "kh_mid_layout", "kh_mid_pack", "kh_mid", "kh_mid_a", "kh_mid_b",
+               "kh_mid_c", "kh_lstm_cell_rows")
 EMBED_SYMBOLS = ("kh_embed_layout", "kh_estd", "kh_efront", "kh_egn_apply", "kh_eqkv_ln", "kh_softmax_rows",
                  "kh_eattn_out_grid", "kh_eattn_out", "kh_ehead", "kh_einter_mask", "kh_eput_lens")
 SYMBOLS = ("kh_gemm", "kh_gemm_plan", "kh_split_planes", "kh_lstm", "kh_launch_count", "kh_sep_layout", "kh_qkv",
            "kh_qkv_many", "kh_kv_gather", "kh_attention", "kh_attn_out", "kh_ln_frame_res",
            "kh_attn_cluster_resident", "kh_front", "kh_front_many", "kh_front_many_geometry", "kh_front1", "kh_back",
-           "kh_back_many", "kh_back_many_geometry") + EMBED_SYMBOLS + tuple(MIRRORS)
+           "kh_back_many", "kh_back_many_geometry") + EMBED_SYMBOLS + MID_SYMBOLS + tuple(MIRRORS)
 EMBED_LAYOUT_NAMES = ("NFFT", "HOP", "NF", "CH", "QK", "VDIM", "FC", "NQKV", "DFT_LD", "EAOUT_SMEM", "LENS_PER_LAUNCH")
 
 ATTN_FORMS = {"query": 0, "tile": 1, "cluster": 2}
@@ -150,6 +167,19 @@ def lib():
             "kh_einter_mask": [P, P, I, I, P],
             "kh_eput_lens": [P, P, I, P],
         })
+        MW = ctypes.POINTER(MidWeights)
+        sigs.update({
+            "kh_rows_gemm": [ctypes.POINTER(RowsGemm), I, IP, P],
+            "kh_rows_gemm_form": [I, I, I, I],
+            "kh_mid_layout": [ctypes.POINTER(ctypes.c_int64)],
+            "kh_mid": [MW, P, P, P, P, I64, I, I, P, P],
+            "kh_mid_a": [MW, P, P, P, I, I64, I, P],
+            "kh_mid_b": [MW, P, P, I64, I, P, I64, I, I, P, P],
+            "kh_mid_c": [MW, P, P, P, I, I64, I, P],
+            "kh_lstm_cell_rows": [P, P, I64, I, P, I64, P, P],
+        })
+        L.kh_mid_pack.restype = None
+        L.kh_mid_pack.argtypes = [P] * 6
         for s, args in sigs.items():
             getattr(L, s).restype = ctypes.c_int
             getattr(L, s).argtypes = args
@@ -922,3 +952,250 @@ def eattention64(X2, pk, blk=0, **mut):
         P, _ = softmax64(S, [T] * T)
         O[:, h] = P @ r["V"][0][h]
     return eattn_out64(O, X2, q("wp_t"), q("bp"), q("slope_p"), q("gp"), q("bpn"), **mut)[0]
+
+
+# ---- the separator's CUDA-core rows GEMM (gemm.cuh) and its one-hop middle section (mid_kernel.cuh) -------------------
+# The weights are in the engine's stored layout: W^T [K][N]; the inter-LSTM gates in unit-major columns j*4 + q
+# (q = i, f, g, o); the Q|K|V projection's PReLU slopes by column group (Q 0-23, K 24-47, V 48-111).  Each reference
+# returns, next to every value, an element-wise bound on the kernel's fp32 rounding: u = 2^-24, a sum of n terms within
+# u sqrt(n) sum |terms|, input bounds carried through (a LayerNorm's through |g| / sigma, as in _ln_bound64).
+ROWS_GEMM_FORMS = {0: None, 1: "tile16x64", 2: "tile64x64", 3: "tile64x128", 4: "big64", 5: "big128"}    # RowsGemmForm
+MID_LAYOUT_NAMES = ("MID_PACK", "MID_RT", "MID_W1", "MID_W3A", "MID_W3B", "MID_W5", "MID_W6", "MID_SMEM", "MID_A_SMEM",
+                    "MID_B_SMEM", "MID_C_SMEM", "NUM_SMS")
+# (region, K, N, KS) of the five k-sliced matrices of BlockWeights::mid_pack (mid_kernel.cuh: M1 .. M6)
+MID_MATRICES = (("MID_W1", 128, 64, 8), ("MID_W3A", 64, 256, 8), ("MID_W3B", 64, 256, 8), ("MID_W5", 64, 64, 4),
+                ("MID_W6", 64, NQKV, 8))
+SLOPE_GROUPS = (24, 48)          # first column of the K and of the V group
+
+
+def rows_gemm(desc, shape=0):
+    """(cudaError_t, RowsGemmForm name) of one kh_rows_gemm call"""
+    form = ctypes.c_int()
+    rc = lib().kh_rows_gemm(ctypes.byref(desc), shape, ctypes.byref(form), stream())
+    return rc, ROWS_GEMM_FORMS[form.value]
+
+
+def rows_gemm_form(M, N, K, shape=0):
+    return ROWS_GEMM_FORMS[lib().kh_rows_gemm_form(M, N, K, shape)]
+
+
+def mid_layout():
+    """kh_mid_layout as {name: value} (MID_LAYOUT_NAMES; offsets in floats, *_SMEM in bytes)"""
+    out = (ctypes.c_int64 * 16)()
+    n = lib().kh_mid_layout(out)
+    return dict(zip(MID_LAYOUT_NAMES, list(out)[:n]))
+
+
+def mid_widx(ks, n_cols, k, n):
+    """index of weight (k, n) in a k-sliced [K][N] matrix (mid_kernel.cuh: slices of ks rows padded by 4 floats)"""
+    return (k // ks) * (ks * n_cols + 4) + (k % ks) * n_cols + n
+
+
+def mid_pack(wl1_t, wih2_t, whh2_t, wl2_t, wqkv_t):
+    """BlockWeights::mid_pack from the five W^T matrices, by the engine's own packing (kh_mid_pack; host memory)"""
+    src = [t.detach().float().contiguous().cpu() for t in (wl1_t, wih2_t, whh2_t, wl2_t, wqkv_t)]
+    dst = torch.full((mid_layout()["MID_PACK"],), float("nan"))
+    lib().kh_mid_pack(*[t.data_ptr() for t in src], dst.data_ptr())
+    return dst
+
+
+def mid_unpack(packed, lay):
+    """the five W^T matrices read back from a mid_pack through mid_widx"""
+    out = []
+    for region, K, N, ks in MID_MATRICES:
+        k = torch.arange(K)[:, None]
+        n = torch.arange(N)[None, :]
+        out.append(packed[lay[region] + mid_widx(ks, N, k, n)])
+    return out
+
+
+def mid(w, Y, X, QKV, state, sstride, blk, B, active=None):
+    return lib().kh_mid(ctypes.byref(w), ptr(Y), ptr(X), ptr(QKV), ptr(state), sstride, blk, B, ptr(active), stream())
+
+
+def mid_a(w, Y, X, GI, B, hop_stride=0, n_hops=1):
+    return lib().kh_mid_a(ctypes.byref(w), ptr(Y), ptr(X), ptr(GI), B, hop_stride, n_hops, stream())
+
+
+def mid_b(w, GI, Hn, state, sstride, blk, B, hop_stride=0, n_hops=1, active=None):
+    return lib().kh_mid_b(ctypes.byref(w), ptr(GI), ptr(Hn), hop_stride, n_hops, ptr(state), sstride, blk, B, ptr(active),
+                          stream())
+
+
+def mid_c(w, Hn, X, QKV, B, hop_stride=0, n_hops=1):
+    return lib().kh_mid_c(ctypes.byref(w), ptr(Hn), ptr(X), ptr(QKV), B, hop_stride, n_hops, stream())
+
+
+def lstm_cell_rows(gates, state, sstride, blk, Hout, rows, active=None):
+    return lib().kh_lstm_cell_rows(ptr(gates), ptr(state), sstride, blk, ptr(Hout), rows, ptr(active), stream())
+
+
+def rows_offsets(M, ld, rows_per_seq=0, seq_stride=0):
+    """[M] offset (floats) of GEMM row m: m * ld, or windowed (seq = m / rows_per_seq, p = m % rows_per_seq) at
+    seq * seq_stride + p * ld (gemm.cuh: a_rows_per_seq / c_rows_per_seq with c_inner <= 1)"""
+    m = torch.arange(M, dtype=torch.int64)
+    if rows_per_seq <= 0:
+        return m * ld
+    return (m // rows_per_seq) * seq_stride + (m % rows_per_seq) * ld
+
+
+def _layer_norm_mut(x, g, b, unbiased=False, eps_outside=False, eps=1e-5):
+    """layer_norm64 with the LayerNorm mutants: unbiased variance, eps added outside the sqrt"""
+    x = x.double()
+    mu = x.mean(-1, keepdim=True)
+    var = ((x - mu) ** 2).mean(-1, keepdim=True)
+    if unbiased:
+        var = var * x.shape[-1] / (x.shape[-1] - 1)
+    sd = torch.sqrt(var) + eps if eps_outside else torch.sqrt(var + eps)
+    return (x - mu) / sd * g.double() + b.double()
+
+
+def rows_gemm64(A, Wt, bias=None, ln=None, R=None, ln_chain=8, unbiased=False, eps_outside=False, no_transpose=False,
+                drop_bias=False, drop_residual=False):
+    """C = [LN(A)] W + bias [+ R] of the logical rows A [M][K] (fp32), Wt [K][N], ln = (g, b) over K = 64 channels, R
+    [M][N] the residual.  ln_chain: the LayerNorm statistics' longest rounding chain (rows GEMM: 4 values per lane and a
+    4-level shuffle tree = 8).  Mutants: unbiased / eps_outside (LayerNorm), no_transpose (W^T's memory read as W [N][K]),
+    drop_bias, drop_residual.  Returns (C, bound)."""
+    K, N = Wt.shape
+    a = A.double()
+    ae = torch.zeros_like(a)
+    if ln is not None:
+        g, b = ln[0].double(), ln[1].double()
+        if unbiased or eps_outside:
+            a = _layer_norm_mut(A, g, b, unbiased, eps_outside)
+        else:
+            a, ae = _ln_bound64(a, g, b, ln_chain)
+    W = Wt.double().reshape(N, K).T if no_transpose else Wt.double()
+    out = a @ W
+    terms = a.abs() @ W.abs()
+    if bias is not None and not drop_bias:
+        out = out + bias.double()
+        terms = terms + bias.double().abs()
+    if R is not None and not drop_residual:
+        out = out + R.double()
+        terms = terms + R.double().abs()
+    return out, ae @ W.abs() + U32 * (math.sqrt(K + 2) * terms + out.abs())
+
+
+def _sigmoid_err(x, s):
+    """__fdividef(1, 1 + __expf(-x)) (fast_sigmoid) and its ex2.approx.ftz form (lstm_cell_rows): __expf is within
+    2 + 1.16 |x| ulp (CUDA C Programming Guide, intrinsic functions; the 1.16 |x| is the rounding of x log2 e), which
+    moves s = 1 / (1 + e) by s (1 - s) times that relative error; 1 + e rounds once and __fdividef adds 2 ulp"""
+    return s * (1 - s) * (2 + 1.16 * x.abs()) * 2.0 ** -23 + 5 * U32 * s
+
+
+def _tanh_err(x, t):
+    """fast_tanh = 2 fast_sigmoid(2x) - 1: twice the sigmoid's error at 2x, and the subtraction's rounding"""
+    s = (t + 1) / 2
+    return 2 * _sigmoid_err(2 * x, s) + U32
+
+
+def cell64(G, Ge, c, ce, swap_if=False, drop_c=False):
+    """one LSTM cell step from the gate pre-activations G [..][256] (column j*4 + q, q = i, f, g, o) with bounds Ge and
+    the carried c [..][64] (bound ce): c' = f c + i g, h' = o tanh(c').  Mutants: swap_if (i and f exchanged), drop_c
+    (c carried as 0).  Returns (h', bound, c', bound)."""
+    G = G.double().view(*G.shape[:-1], 64, 4)
+    Ge = Ge.double().view(*G.shape)
+    c = torch.zeros_like(c.double()) if drop_c else c.double()
+    qi, qf = (1, 0) if swap_if else (0, 1)
+    xi, xf, xg, xo = G[..., qi], G[..., qf], G[..., 2], G[..., 3]
+    ei, ef, eg, eo = Ge[..., qi], Ge[..., qf], Ge[..., 2], Ge[..., 3]
+    i, f, g, o = torch.sigmoid(xi), torch.sigmoid(xf), torch.tanh(xg), torch.sigmoid(xo)
+    ie = i * (1 - i) * ei + _sigmoid_err(xi, i)
+    fe = f * (1 - f) * ef + _sigmoid_err(xf, f)
+    ge = (1 - g * g) * eg + _tanh_err(xg, g)
+    oe = o * (1 - o) * eo + _sigmoid_err(xo, o)
+    c2 = f * c + i * g
+    c2e = c.abs() * fe + f * ce + g.abs() * ie + i * ge + U32 * (2 * (f * c).abs() + 2 * (i * g).abs())
+    t = torch.tanh(c2)
+    h = o * t
+    he = t.abs() * oe + o * ((1 - t * t) * c2e + _tanh_err(c2, t)) + U32 * h.abs()
+    return h, he, c2, c2e
+
+
+def lstm_cell64(gates, c, **mutant):
+    """lstm_cell_rows_kernel of exact fp32 gates [rows][256] and c [rows][64]: (h', bound, c', bound)"""
+    return cell64(gates, torch.zeros_like(gates.double()), c, torch.zeros_like(c.double()), **mutant)
+
+
+def mid_a64(Y, X, p, drop_residual=False, drop_bias=False, unbiased=False, eps_outside=False):
+    """X1 = X + Y W_l1 + b_l1 and GI = LN(X1) W_ih + b of rows Y [..][128], X [..][64]; p: the block's weights
+    (wl1_t, bl1, ln2_g, ln2_b, wih2_t, b2, ...).  The LayerNorm's statistics: 2 values per lane, a 5-level warp tree.
+    Returns (X1, bound, GI, bound)."""
+    W1, b1 = p["wl1_t"].double(), p["bl1"].double()
+    x = torch.zeros_like(X.double()) if drop_residual else X.double()
+    X1 = x + Y.double() @ W1 + (0 if drop_bias else b1)
+    X1e = U32 * (math.sqrt(130) * (X.double().abs() + Y.double().abs() @ W1.abs() + b1.abs()) + X1.abs())
+    g, b = p["ln2_g"].double(), p["ln2_b"].double()
+    if unbiased or eps_outside:
+        xn, xne = _layer_norm_mut(X1, g, b, unbiased, eps_outside), torch.zeros_like(X1)
+    else:
+        xn, xne = _ln_bound64(X1, g, b, 6, ye=X1e)
+    Wih, b2 = p["wih2_t"].double(), p["b2"].double()
+    GI = xn @ Wih + b2
+    GIe = xne @ Wih.abs() + U32 * (math.sqrt(66) * (xn.abs() @ Wih.abs() + b2.abs()) + GI.abs())
+    return X1, X1e, GI, GIe
+
+
+def mid_gates64(GI, GIe, h, he, p):
+    """g = GI + h W_hh (the kernels' operand order: (h W_hh) + ((x W_ih) + b)) and its bound"""
+    Whh = p["whh2_t"].double()
+    G = GI.double() + h.double() @ Whh
+    return G, GIe + he @ Whh.abs() + U32 * (math.sqrt(65) * (h.double().abs() @ Whh.abs() + GI.double().abs()) + G.abs())
+
+
+def mid_c64(X1, X1e, H, He, p, drop_residual=False, drop_bias=False, slope_groups=SLOPE_GROUPS):
+    """X2 = X1 + H W_l2 + b_l2 and P = PReLU(X2 W_qkv + b_qkv) with the slope of each column's group.  Mutants:
+    drop_residual, drop_bias (b_l2), slope_groups (other group boundaries).  Returns (X2, bound, P, bound)."""
+    W2, b2 = p["wl2_t"].double(), p["bl2"].double()
+    x1 = torch.zeros_like(X1.double()) if drop_residual else X1.double()
+    X2 = x1 + H.double() @ W2 + (0 if drop_bias else b2)
+    X2e = X1e + He @ W2.abs() + U32 * (math.sqrt(66) * (X1.double().abs() + H.double().abs() @ W2.abs() + b2.abs()) + X2.abs())
+    Wq, bq, s = p["wqkv_t"].double(), p["bqkv"].double(), p["slopes"].double()
+    col = torch.arange(NQKV)
+    a = torch.where(col < slope_groups[0], s[0], torch.where(col < slope_groups[1], s[1], s[2]))
+    Z = X2 @ Wq + bq
+    Ze = X2e @ Wq.abs() + U32 * (math.sqrt(65) * (X2.abs() @ Wq.abs() + bq.abs()) + Z.abs())
+    P = prelu64(Z, a)
+    return X2, X2e, P, Ze * torch.clamp(a.abs(), min=1.0) + U32 * P.abs()
+
+
+def mid64(Y, X, h, c, p, swap_if=False, drop_c=False, whh_new_h=False, drop_residual=False, drop_bias=False,
+          slope_groups=SLOPE_GROUPS, unbiased=False, eps_outside=False):
+    """the one-hop middle section of rows Y [..][128], X [..][64] with the carried (h, c) [..][64]: X1 = X + Y W_l1 + b;
+    the inter-LSTM step from LN(X1) and (h, c); X2 = X1 + h' W_l2 + b; P = PReLU(X2 W_qkv + b).  Mutants: those of
+    mid_a64, cell64 and mid_c64 (drop_residual / drop_bias apply to both Linears), whh_new_h (h W_hh taken from the new
+    h: the state read after it was overwritten).  Returns a dict of X1, GI, h, c, X2, P and their bounds (key + "_b")."""
+    X1, X1e, GI, GIe = mid_a64(Y, X, p, drop_residual, drop_bias, unbiased, eps_outside)
+    zero = torch.zeros_like(h.double())
+    G, Ge = mid_gates64(GI, GIe, h, zero, p)
+    h2, h2e, c2, c2e = cell64(G, Ge, c, zero, swap_if, drop_c)
+    if whh_new_h:
+        G, Ge = mid_gates64(GI, GIe, h2.float(), zero, p)
+        h2, h2e, c2, c2e = cell64(G, Ge, c, zero, swap_if, drop_c)
+    X2, X2e, P, Pe = mid_c64(X1, X1e, h2, h2e, p, drop_residual, drop_bias, slope_groups)
+    return dict(X1=X1, X1_b=X1e, GI=GI, GI_b=GIe, h=h2, h_b=h2e, c=c2, c_b=c2e, X2=X2, X2_b=X2e, P=P, P_b=Pe)
+
+
+def mid_b64(GIs, h, c, p, GIe=None, no_advance=False, store_first=False):
+    """mid_b_kernel over the hops of GIs [n_hops][..][256] from the carried (h, c): per hop g = GI + h W_hh, the cell,
+    H'_j = h'.  GIe: the bounds of GIs (None: exact fp32 inputs).  Mutants: no_advance (every hop from the carried h),
+    store_first (the state after the first hop is what is stored).  Returns (H' [n_hops][..][64], bounds, the stored
+    (h, c) and their bounds)."""
+    h = h.double()
+    c = c.double()
+    he, ce = torch.zeros_like(h), torch.zeros_like(c)
+    h0 = h
+    Hs, Hes, stored = [], [], None
+    for j in range(GIs.shape[0]):
+        gie = torch.zeros_like(GIs[j].double()) if GIe is None else GIe[j]
+        hin, hine = (h0, torch.zeros_like(h0)) if no_advance else (h, he)
+        G, Ge = mid_gates64(GIs[j], gie, hin, hine, p)
+        h, he, c, ce = cell64(G, Ge, c, ce)
+        Hs.append(h)
+        Hes.append(he)
+        if j == 0 and store_first:
+            stored = (h, he, c, ce)
+    if stored is None:
+        stored = (h, he, c, ce)
+    return torch.stack(Hs), torch.stack(Hes), stored

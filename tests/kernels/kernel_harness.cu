@@ -1,10 +1,10 @@
 // Test-only C entry points into the engine's tensor-core GEMM (umma::launch), LSTM recurrences (lstm.cuh,
 // tc_lstm.cuh), the separator's attention section (sep_kernels.cuh), its front and back (sep_kernels.cuh,
-// hop_kernels.cuh) and the enrollment network's own kernels (embed_kernels.cuh: estd, efront, egn_apply, eqkv_ln,
-// softmax_rows, eattn_out, ehead, einter_mask, eput_lens), so that tests/test_umma_gemm_gpu.py,
-// tests/test_lstm_kernels_gpu.py, tests/test_attention_kernels_gpu.py, tests/test_front_back_kernels_gpu.py and
-// tests/test_embed_kernels_gpu.py can drive each kernel directly with arbitrary shapes and compare it element by element
-// with a float64 reference.
+// hop_kernels.cuh), its CUDA-core rows GEMM (gemm.cuh), its one-hop middle section (mid_kernel.cuh: mid_kernel, mid_a,
+// mid_b, mid_c) and the tensor-core chain's cell kernel (sep_kernels.cuh: lstm_cell_rows), and the enrollment network's
+// own kernels (embed_kernels.cuh: estd, efront, egn_apply, eqkv_ln, softmax_rows, eattn_out, ehead, einter_mask,
+// eput_lens), so that the kernel-level tests (tests/test_*_kernels_gpu.py) can drive each kernel directly with arbitrary
+// shapes and compare it element by element with a float64 reference.
 //
 // The argument structs below are plain C (mirrored with ctypes in the tests); every function checks its arguments, fills
 // the engine's own descriptor and calls the engine's own launcher.  Built by
@@ -12,6 +12,7 @@
 // l2h symbols never binds to the product library's copy.
 #include <cstdio>
 #include "umma_gemm.cu"
+#include "gemm.cuh"
 #include "tc_lstm.cuh"
 #include "sep_launch.cuh"
 #include "embed_kernels.cuh"
@@ -169,7 +170,9 @@ static cudaError_t configure() {
     if (e != cudaSuccess || configured_dev == dev) return e;
     e = configure_lstm();
     if (e == cudaSuccess) e = configure_tc_lstm();
+    if (e == cudaSuccess) e = configure_rows_gemm();
     if (e == cudaSuccess) e = set_sep_smem<int64_t>();
+    if (e == cudaSuccess) e = set_mid_split_smem();
     if (e == cudaSuccess) e = cudaFuncSetAttribute(emb::eattn_out_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)emb::EAOUT_SMEM);
     if (e == cudaSuccess) configured_dev = dev;
     return e;
@@ -385,6 +388,120 @@ KH_API int kh_back_many(const KhSepFrontBack* w, const float* X, float* y, int64
     const ChunkWalk g{chunk, (T + chunk - 1) / chunk, n_cl};
     return (int)launch_back_many(false, static_cast<cudaStream_t>(stream), g, X, y, y_bstride, y_cstride, y_len, state, sstride,
                                  to_sep(*w), T, pos_rel, B, active);
+}
+
+// ---- the separator's CUDA-core rows GEMM (gemm.cuh) -------------------------------------------------------------------
+// GemmArgs field for field
+struct KhRowsGemm {
+    const float* A;
+    int64_t lda;
+    int32_t a_rows_per_seq;
+    int64_t a_seq_stride;
+    const float *Wt, *bias;
+    float* C;
+    int64_t ldc;
+    int32_t c_rows_per_seq;
+    int64_t c_seq_stride;
+    int32_t c_inner;
+    int64_t c_inner_stride;
+    const float *R, *ln_g, *ln_b, *prelu, *prelu_vec;
+    int32_t M, N, K;
+};
+
+static GemmArgs to_rows_gemm(const KhRowsGemm& k) {
+    GemmArgs g{};
+    g.A = k.A; g.lda = k.lda; g.a_rows_per_seq = k.a_rows_per_seq; g.a_seq_stride = k.a_seq_stride;
+    g.Wt = k.Wt; g.bias = k.bias; g.C = k.C; g.ldc = k.ldc;
+    g.c_rows_per_seq = k.c_rows_per_seq; g.c_seq_stride = k.c_seq_stride; g.c_inner = k.c_inner; g.c_inner_stride = k.c_inner_stride;
+    g.R = k.R; g.ln_g = k.ln_g; g.ln_b = k.ln_b; g.prelu = k.prelu; g.prelu_vec = k.prelu_vec;
+    g.M = k.M; g.N = k.N; g.K = k.K;
+    return g;
+}
+
+KH_API int kh_sizeof_rows_gemm() { return (int)sizeof(KhRowsGemm); }
+
+// the kernel launch_rows_gemm runs for (M, N, K, shape) without a LayerNorm prologue, as RowsGemmForm (0: refused)
+KH_API int kh_rows_gemm_form(int M, int N, int K, int shape) {
+    GemmArgs g{};
+    g.M = M; g.N = N; g.K = K;
+    return (int)rows_gemm_form(g, shape);
+}
+
+// launch_rows_gemm(g, stream, no PDL, shape); *form (may be null) = the kernel it chose (RowsGemmForm)
+KH_API int kh_rows_gemm(const KhRowsGemm* k, int shape, int* form, void* stream) {
+    const GemmArgs g = to_rows_gemm(*k);
+    if (form) *form = (int)rows_gemm_form(g, shape);
+    if (shape < 0 || shape > 2 || g.A == nullptr || g.Wt == nullptr || g.C == nullptr || g.lda < g.K) return (int)cudaErrorInvalidValue;
+    if (cudaError_t e = configure()) return (int)e;
+    return (int)launch_rows_gemm(g, static_cast<cudaStream_t>(stream), false, shape);
+}
+
+// ---- the separator's one-hop middle section (mid_kernel.cuh) and the tensor-core chain's cell (sep_kernels.cuh) -------
+// The fields of BlockWeights that mid_kernel, mid_a, mid_b and mid_c read.
+struct KhMidWeights {
+    const float *mid_pack, *bl1, *ln2_g, *ln2_b, *b2, *bl2, *bqkv, *slopes;
+};
+
+static BlockWeights to_mid(const KhMidWeights& k) {
+    BlockWeights w{};
+    w.mid_pack = k.mid_pack; w.bl1 = k.bl1; w.ln2_g = k.ln2_g; w.ln2_b = k.ln2_b; w.b2 = k.b2; w.bl2 = k.bl2; w.bqkv = k.bqkv;
+    w.slopes = k.slopes;
+    return w;
+}
+
+KH_API int kh_sizeof_mid_weights() { return (int)sizeof(KhMidWeights); }
+
+// MID_PACK, MID_RT, MID_W1, MID_W3A, MID_W3B, MID_W5, MID_W6, MID_SMEM, MID_A_SMEM, MID_B_SMEM, MID_C_SMEM (bytes), NUM_SMS;
+// returns the count written (12)
+KH_API int kh_mid_layout(int64_t* out) {
+    const int64_t v[] = {MID_PACK, MID_RT, MID_W1, MID_W3A, MID_W3B, MID_W5, MID_W6, (int64_t)MID_SMEM, (int64_t)MID_A_SMEM,
+                         (int64_t)MID_B_SMEM, (int64_t)MID_C_SMEM, NUM_SMS};
+    const int n = (int)(sizeof(v) / sizeof(v[0]));
+    for (int i = 0; i < n; ++i) out[i] = v[i];
+    return n;
+}
+
+// the engine's k-sliced packing (host arrays; dst holds MID_PACK floats)
+KH_API void kh_mid_pack(const float* wl1_t, const float* wih2_t, const float* whh2_t, const float* wl2_t, const float* wqkv_t,
+                        float* dst) {
+    mid_pack_weights(wl1_t, wih2_t, whh2_t, wl2_t, wqkv_t, dst);
+}
+
+// mid_kernel over B streams' [B][97] rows of Y [..][128], X [..][64] (updated in place) and QKV [..][112]; the carried
+// (h, c) of block blk of record b at state + header + b * sstride
+KH_API int kh_mid(const KhMidWeights* w, const float* Y, float* X, float* QKV, float* state, int64_t sstride, int blk, int B,
+                  const uint8_t* active, void* stream) {
+    if (B <= 0 || blk < 0 || sstride <= 0) return (int)cudaErrorInvalidValue;
+    if (cudaError_t e = configure()) return (int)e;
+    return (int)launch_mid(false, static_cast<cudaStream_t>(stream), Y, X, QKV, state, sstride, blk, to_mid(*w), B, active);
+}
+
+// mid_a / mid_b / mid_c over n_hops hops whose buffers sit hop_stride floats apart
+KH_API int kh_mid_a(const KhMidWeights* w, const float* Y, float* X, float* GI, int B, int64_t hop_stride, int n_hops, void* stream) {
+    if (B <= 0 || n_hops <= 0 || hop_stride < 0) return (int)cudaErrorInvalidValue;
+    if (cudaError_t e = configure()) return (int)e;
+    return (int)launch_mid_a(false, static_cast<cudaStream_t>(stream), Y, X, GI, to_mid(*w), B, hop_stride, n_hops);
+}
+
+KH_API int kh_mid_b(const KhMidWeights* w, const float* GI, float* Hn, int64_t hop_stride, int n_hops, float* state, int64_t sstride,
+                    int blk, int B, const uint8_t* active, void* stream) {
+    if (B <= 0 || n_hops <= 0 || hop_stride < 0 || blk < 0 || sstride <= 0) return (int)cudaErrorInvalidValue;
+    if (cudaError_t e = configure()) return (int)e;
+    return (int)launch_mid_b(false, static_cast<cudaStream_t>(stream), GI, Hn, hop_stride, n_hops, state, sstride, blk, to_mid(*w), B,
+                             active);
+}
+
+KH_API int kh_mid_c(const KhMidWeights* w, const float* Hn, float* X, float* QKV, int B, int64_t hop_stride, int n_hops, void* stream) {
+    if (B <= 0 || n_hops <= 0 || hop_stride < 0) return (int)cudaErrorInvalidValue;
+    if (cudaError_t e = configure()) return (int)e;
+    return (int)launch_mid_c(false, static_cast<cudaStream_t>(stream), Hn, X, QKV, to_mid(*w), B, hop_stride, n_hops);
+}
+
+// lstm_cell_rows_kernel: gates [rows][256] (column j*4 + q), row r = stream r / 97, bin r % 97; Hout [rows][64]
+KH_API int kh_lstm_cell_rows(const float* gates, float* state, int64_t sstride, int blk, float* Hout, int64_t rows,
+                             const uint8_t* active, void* stream) {
+    if (rows <= 0 || rows * 64 > 0x7fffffff || blk < 0 || sstride <= 0) return (int)cudaErrorInvalidValue;
+    return (int)launch_lstm_cell_rows(false, static_cast<cudaStream_t>(stream), gates, state, sstride, blk, Hout, rows, active);
 }
 
 // ---- the enrollment network's own kernels (embed_kernels.cuh) --------------------------------------------------------

@@ -1,6 +1,6 @@
 """The kernel harness library (tests/kernels/) and the float64 references the kernel-level GPU tests
 (test_umma_gemm_gpu.py, test_lstm_kernels_gpu.py, test_attention_kernels_gpu.py, test_front_back_kernels_gpu.py,
-test_embed_kernels_gpu.py) rely on.  The enrollment references (estd64, efront64, egn64, eqkv_ln64, softmax64,
+test_embed_kernels_gpu.py, test_rows_gemm_kernels_gpu.py, test_mid_kernels_gpu.py) rely on.  The enrollment references (estd64, efront64, egn64, eqkv_ln64, softmax64,
 eattn_out64, ehead64) are pinned to oracle/restate.py; each of their mutants is shown to miss the reference by more than
 10x its bound, and einter_mask_expected's mutants to change it.  No device needed."""
 import ctypes
@@ -469,3 +469,144 @@ def test_embed_mutants_differ(embed_params):
     assert torch.equal(ref.view(2, kh.E_NF, steps, 512)[0, :, :Tb - 3], gx.view(2, kh.E_NF, steps, 512)[0, :, :Tb - 3])
     for m in (dict(start=4), dict(start=2), dict(fwd_only=True), dict(pad=(float("-inf"), 0.0, float("-inf"), 0.0))):
         assert not torch.equal(kh.einter_mask_expected(gx, lens, steps, **m), ref), m
+
+
+# ---- the rows GEMM and the one-hop middle section (test_rows_gemm_kernels_gpu.py, test_mid_kernels_gpu.py) -----------
+def _mid_params(seed=0):
+    """random block weights in the engine's stored layouts (W^T, gate columns j*4 + q), distinct PReLU slopes"""
+    g = torch.Generator().manual_seed(seed)
+    r = lambda *s, scale=1.0: scale * torch.randn(*s, generator=g)
+    return dict(wl1_t=r(128, 64, scale=128 ** -0.5), bl1=r(64, scale=0.3), ln2_g=1 + r(64, scale=0.2),
+                ln2_b=r(64, scale=0.2), wih2_t=r(64, 256, scale=0.25), whh2_t=r(64, 256, scale=0.25), b2=r(256, scale=0.3),
+                wl2_t=r(64, 64, scale=0.125), bl2=r(64, scale=0.3), wqkv_t=r(64, kh.NQKV, scale=0.125),
+                bqkv=r(kh.NQKV, scale=0.3), slopes=torch.tensor([0.25, -0.3, 0.6, 0.1]))
+
+
+def _torch_gate_rows(w):
+    """engine gate columns j*4 + q of W^T [K][256] -> torch.nn.LSTMCell rows q*64 + j of W [256][K]"""
+    return w.T.reshape(64, 4, -1).transpose(0, 1).reshape(256, -1)
+
+
+def test_rows_gemm_reference_is_layer_norm_and_linear():
+    torch.manual_seed(1)
+    A, Wt, b, R = torch.randn(37, 64), torch.randn(64, 256) / 8, torch.randn(256), torch.randn(37, 256)
+    ln = torch.nn.LayerNorm(64).double()
+    with torch.no_grad():
+        ln.weight.copy_(1 + 0.2 * torch.randn(64))
+        ln.bias.copy_(0.2 * torch.randn(64))
+        lin = torch.nn.Linear(64, 256).double()
+        lin.weight.copy_(Wt.T)
+        lin.bias.copy_(b)
+        want = lin(ln(A.double())) + R.double()
+    got, bound = kh.rows_gemm64(A, Wt, b, (ln.weight.float(), ln.bias.float()), R)
+    assert torch.allclose(got, want, rtol=0, atol=1e-12)
+    assert bool((bound > 0).all())
+    # windowed rows: sequence s, row p at s * seq_stride + p * ld
+    assert kh.rows_offsets(5, 64, 2, 1000).tolist() == [0, 64, 1000, 1064, 2000]
+    assert kh.rows_offsets(3, 72).tolist() == [0, 72, 144]
+
+
+def test_mid_references_are_the_torch_modules():
+    """mid64 is nn.Linear(128, 64) + residual, nn.LayerNorm(64), nn.LSTMCell(64, 64) (gates permuted to j*4 + q),
+    nn.Linear(64, 64) + residual and nn.Linear(64, 112) + nn.PReLU per Q / K / V group; mid_b64 over hops is the
+    LSTMCell stepped; lstm_cell64 is the LSTMCell's cell from given pre-activations."""
+    p = _mid_params()
+    torch.manual_seed(2)
+    n = 23
+    Y, X, h, c = torch.randn(n, 128), torch.randn(n, 64), 0.5 * torch.randn(n, 64), torch.randn(n, 64)
+    d = lambda t: t.double()
+    with torch.no_grad():
+        l1 = torch.nn.Linear(128, 64).double()
+        l1.weight.copy_(p["wl1_t"].T); l1.bias.copy_(p["bl1"])
+        ln = torch.nn.LayerNorm(64).double()
+        ln.weight.copy_(p["ln2_g"]); ln.bias.copy_(p["ln2_b"])
+        cell = torch.nn.LSTMCell(64, 64).double()
+        cell.weight_ih.copy_(_torch_gate_rows(p["wih2_t"])); cell.weight_hh.copy_(_torch_gate_rows(p["whh2_t"]))
+        cell.bias_ih.copy_(_torch_gate_rows(p["b2"][None, :])[:, 0]); cell.bias_hh.zero_()
+        l2 = torch.nn.Linear(64, 64).double()
+        l2.weight.copy_(p["wl2_t"].T); l2.bias.copy_(p["bl2"])
+        lq = torch.nn.Linear(64, kh.NQKV).double()
+        lq.weight.copy_(p["wqkv_t"].T); lq.bias.copy_(p["bqkv"])
+        X1 = d(X) + l1(d(Y))
+        h2, c2 = cell(ln(X1), (d(h), d(c)))
+        X2 = X1 + l2(h2)
+        Z = lq(X2)
+        P = torch.cat([torch.nn.PReLU(init=float(p["slopes"][i])).double()(Z[:, a:b])
+                       for i, (a, b) in enumerate(((0, 24), (24, 48), (48, kh.NQKV)))], 1)
+        r = kh.mid64(Y, X, h, c, p)
+        for k, want in (("X1", X1), ("h", h2), ("c", c2), ("X2", X2), ("P", P)):
+            assert torch.allclose(r[k], want, rtol=0, atol=1e-12), k
+            assert bool((r[k + "_b"] > 0).all()), k
+        # three hops of mid_b from the same GI rows
+        GIs = torch.stack([kh.mid_a64(torch.randn(n, 128), torch.randn(n, 64), p)[2].float() for _ in range(3)])
+        H, _, (hs, _, cs, _) = kh.mid_b64(GIs, h, c, p)
+        hh, cc = d(h), d(c)
+        for j in range(3):
+            g = d(GIs[j]) + hh @ d(p["whh2_t"])
+            cell_only = torch.nn.LSTMCell(256, 64, bias=False).double()
+            cell_only.weight_ih.copy_(_torch_gate_rows(torch.eye(256)))
+            cell_only.weight_hh.zero_()
+            hh, cc = cell_only(g, (hh, cc))
+            assert torch.allclose(H[j], hh, rtol=0, atol=1e-12)
+        assert torch.allclose(hs, hh, rtol=0, atol=1e-12) and torch.allclose(cs, cc, rtol=0, atol=1e-12)
+        gates = 2 * torch.randn(n, 256)
+        hl, _, cl, _ = kh.lstm_cell64(gates, c)
+        hw, cw = cell_only(d(gates), (torch.zeros(n, 64, dtype=torch.float64), d(c)))
+        assert torch.allclose(hl, hw, rtol=0, atol=1e-12) and torch.allclose(cl, cw, rtol=0, atol=1e-12)
+
+
+def test_mid_pack_round_trips_through_mid_widx():
+    """kh_mid_pack (the engine's own packing at commit) puts W^T[k][n] of each matrix at region + mid_widx(KS, N, k, n)
+    and zero in every padding float"""
+    lay = kh.mid_layout()
+    assert lay["MID_RT"] == 8 and lay["NUM_SMS"] == 132
+    p = _mid_params(3)
+    mats = [p[k] for k in ("wl1_t", "wih2_t", "whh2_t", "wl2_t", "wqkv_t")]
+    packed = kh.mid_pack(*mats)
+    for got, want in zip(kh.mid_unpack(packed, lay), mats):
+        assert torch.equal(got, want)
+    used = torch.zeros(lay["MID_PACK"], dtype=torch.bool)
+    for region, K, N, ks in kh.MID_MATRICES:
+        used[lay[region] + kh.mid_widx(ks, N, torch.arange(K)[:, None], torch.arange(N)[None, :])] = True
+    assert int(used.sum()) == sum(K * N for _, K, N, _ in kh.MID_MATRICES)
+    assert bool((packed[~used] == 0).all())
+
+
+def _ratio(a, b, bound):
+    return float(((a - b).abs() / bound).max())
+
+
+def test_rows_gemm_and_mid_mutants_differ():
+    """every mutated reference the GPU tests use misses the reference by >= 10x its bound, on at least one of the outputs
+    of the kernel it stands for, on test-like data; the eps placement shows on a row of small spread"""
+    torch.manual_seed(4)
+    A = torch.randn(40, 64)
+    A[3] = 0.5 + 0.01 * torch.randn(64)
+    Wt, b, R = torch.randn(64, 64) / 8, 0.3 * torch.randn(64), torch.randn(40, 64)
+    ln = (1 + 0.2 * torch.randn(64), 0.2 * torch.randn(64))
+    ref, bound = kh.rows_gemm64(A, Wt, b, ln, R)
+    for m in ("unbiased", "eps_outside", "no_transpose", "drop_bias", "drop_residual"):
+        assert _ratio(kh.rows_gemm64(A, Wt, b, ln, R, **{m: True})[0], ref, bound) >= 10, m
+    assert _ratio(ref[:-16], ref[16:], bound[16:]) >= 10                 # rows offset by one 16-row tile
+    p = _mid_params(5)
+    n = 97
+    Y, X, h, c = torch.randn(n, 128), torch.randn(n, 64), 0.5 * torch.randn(n, 64), torch.randn(n, 64)
+    Y[7] = 0
+    X[7] = 0.4 - p["bl1"] + 0.01 * torch.randn(64)                        # X1 of row 7: spread 0.01
+    r = kh.mid64(Y, X, h, c, p)
+    muts = dict(unbiased=("h", "c", "P"), eps_outside=("h", "c", "P"), swap_if=("h", "c", "P"), drop_c=("h", "c", "P"),
+                whh_new_h=("h", "c", "P"), drop_residual=("X2", "P"), drop_bias=("X2", "P"), slope_groups=("P",))
+    for m, keys in muts.items():
+        mr = kh.mid64(Y, X, h, c, p, **{m: (20, 48) if m == "slope_groups" else True})
+        assert max(_ratio(mr[k], r[k], r[k + "_b"]) for k in keys) >= 10, m
+    GIs = torch.stack([kh.mid_a64(torch.randn(n, 128), torch.randn(n, 64), p)[2].float() for _ in range(3)])
+    H, Hb, (hs, hb, cs, cb) = kh.mid_b64(GIs, h, c, p)
+    H2 = kh.mid_b64(GIs, h, c, p, no_advance=True)[0]
+    assert _ratio(H2[1:], H[1:], Hb[1:]) >= 10
+    _, _, (hs2, _, cs2, _) = kh.mid_b64(GIs, h, c, p, store_first=True)
+    assert _ratio(hs2, hs, hb) >= 10 and _ratio(cs2, cs, cb) >= 10
+    gates = 2 * torch.randn(n, 256)
+    hl, hlb, cl, clb = kh.lstm_cell64(gates, c)
+    for m in ("swap_if", "drop_c"):
+        hm, _, cm, _ = kh.lstm_cell64(gates, c, **{m: True})
+        assert _ratio(hm, hl, hlb) >= 10 and _ratio(cm, cl, clb) >= 10, m
