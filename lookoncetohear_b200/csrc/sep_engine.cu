@@ -259,25 +259,7 @@ static int set_attrs() {
     CK(configure_lstm());
     CK(umma::configure());
     CK(configure_tc_lstm());
-    {   // tail_kernel: 16 CTAs per cluster is a non-portable size; ask whether this device can place it
-        g_tail_clusters[dev_ord] = 0;
-        if (cudaFuncSetAttribute(tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TAIL_SMEM) == cudaSuccess &&
-            cudaFuncSetAttribute(tail_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess) {
-            cudaLaunchConfig_t cfg{};
-            cfg.gridDim = dim3(TAIL_CL, 1); cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = TAIL_SMEM;
-            cudaLaunchAttribute at[1];
-            at[0].id = cudaLaunchAttributeClusterDimension;
-            at[0].val.clusterDim.x = TAIL_CL; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-            cfg.attrs = at; cfg.numAttrs = 1;
-            int ncl = 0;
-            if (cudaOccupancyMaxActiveClusters(&ncl, tail_kernel, &cfg) == cudaSuccess) g_tail_clusters[dev_ord] = ncl;
-        }
-        if (g_tail_clusters[dev_ord] > 0 &&      // the slot-list form: same resources, so the same cluster count
-            (cudaFuncSetAttribute(tail_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TAIL_SMEM) != cudaSuccess ||
-             cudaFuncSetAttribute(tail_kernel_t<Records>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess))
-            g_tail_clusters[dev_ord] = 0;
-        cudaGetLastError();
-    }
+    g_tail_clusters[dev_ord] = set_tail_attrs();
     g_attr_done[dev_ord] = true;
     return 0;
 }
@@ -685,8 +667,7 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
                 const BlockWeights& Wn = e->bw[b + 1];
                 nx.ln_g = Wn.ln1_g; nx.ln_b = Wn.ln1_b; nx.wih_t = Wn.wih1_t; nx.bias = Wn.b1; nx.GX = c.GX;
             }
-            CK(launch_cluster(f.pdl, dim3(TAIL_CL, 1, 1), tail_kernel_t<Map>, dim3(TAIL_CL, R.B), dim3(256), TAIL_SMEM, st, (const float*)c.Y, R.X,
-                              a.state, R.recs, b, W, nx, R.gate, 0, a.active));
+            CK(launch_tail(f.pdl, st, R.B, c.Y, R.X, a.state, R.recs, b, W, nx, R.gate, 0, a.active));
             MARK("tail");
             if (int rc = c.do_tap()) return rc;
             continue;

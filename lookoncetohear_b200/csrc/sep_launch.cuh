@@ -65,6 +65,29 @@ static inline cudaError_t set_mid_split_smem() {
     return e;
 }
 
+// tail_kernel: 16 CTAs per cluster is a non-portable size.  Sets the dynamic shared memory and the non-portable cluster
+// size of both Map forms on the current device and returns how many clusters the device can hold at once (0: it cannot
+// be scheduled, and callers keep the separate kernels).  Clears the error state it may leave.
+static inline int set_tail_attrs() {
+    int ncl = 0;
+    if (cudaFuncSetAttribute(tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TAIL_SMEM) == cudaSuccess &&
+        cudaFuncSetAttribute(tail_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess) {
+        cudaLaunchConfig_t cfg{};
+        cfg.gridDim = dim3(TAIL_CL, 1); cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = TAIL_SMEM;
+        cudaLaunchAttribute at[1];
+        at[0].id = cudaLaunchAttributeClusterDimension;
+        at[0].val.clusterDim.x = TAIL_CL; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+        cfg.attrs = at; cfg.numAttrs = 1;
+        if (cudaOccupancyMaxActiveClusters(&ncl, tail_kernel, &cfg) != cudaSuccess) ncl = 0;
+    }
+    if (ncl > 0 &&      // the slot-list form: same resources, so the same cluster count
+        (cudaFuncSetAttribute(tail_kernel_t<Records>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TAIL_SMEM) != cudaSuccess ||
+         cudaFuncSetAttribute(tail_kernel_t<Records>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess))
+        ncl = 0;
+    cudaGetLastError();
+    return ncl;
+}
+
 // front_kernel: grid (T + gate, B), the T frames and, with gate = 1, each stream's speaker-gate memo CTA
 template <class Map>
 inline cudaError_t launch_front(bool pdl, cudaStream_t st, int B, int gate, const float* x, int64_t x_bstride, int64_t x_cstride,
@@ -110,6 +133,13 @@ inline cudaError_t launch_mid_b(bool pdl, cudaStream_t st, const float* GI, floa
 inline cudaError_t launch_mid_c(bool pdl, cudaStream_t st, const float* Hn, float* X, float* QKV, const BlockWeights& w, int n_streams,
                                 int64_t hop_stride, int n_hops) {
     return launch_k(pdl, mid_c_kernel, mid_grid_for(n_streams, 4), dim3(256), MID_C_SMEM, st, Hn, X, QKV, w, n_streams, hop_stride, n_hops);
+}
+// tail_kernel: one cluster of TAIL_CL CTAs per stream, grid (TAIL_CL, B); set_tail_attrs() must have returned > 0
+template <class Map>
+inline cudaError_t launch_tail(bool pdl, cudaStream_t st, int B, const float* Y, float* X, float* state, Map recs, int blk,
+                               const BlockWeights& w, const NextIh& nx, int apply_gate, int frame_k, const uint8_t* active) {
+    return launch_cluster(pdl, dim3(TAIL_CL, 1, 1), tail_kernel_t<Map>, dim3(TAIL_CL, B), dim3(256), TAIL_SMEM, st, Y, X, state, recs,
+                          blk, w, nx, apply_gate, frame_k, active);
 }
 // lstm_cell_rows_kernel: one thread per (row, hidden unit)
 template <class Map>

@@ -92,18 +92,27 @@ class MidWeights(ctypes.Structure):
     _fields_ = [(n, ctypes.c_void_p) for n in ("mid_pack", "bl1", "ln2_g", "ln2_b", "b2", "bl2", "bqkv", "slopes")]
 
 
+class TailWeights(ctypes.Structure):
+    """KhTailWeights: the fields of BlockWeights that tail_kernel reads, then the next block's input projection (nx_wih_t
+    null: no next block)"""
+    _fields_ = [(n, ctypes.c_void_p) for n in ("mid_pack", "bl1", "ln2_g", "ln2_b", "b2", "bl2", "bqkv", "slopes", "lnq_g",
+                                                "lnq_b", "lnk_g", "lnk_b", "lnv_g", "lnv_b", "wp_t", "bp", "lnp_g", "lnp_b",
+                                                "nx_ln_g", "nx_ln_b", "nx_wih_t", "nx_bias")]
+
+
 MIRRORS = {"kh_sizeof_asource": ASource, "kh_sizeof_gemm": Gemm, "kh_sizeof_plan": Plan, "kh_sizeof_lstm": Lstm,
            "kh_sizeof_sep_weights": SepWeights, "kh_sizeof_sep_front_back": SepFrontBack,
            "kh_sizeof_emb_weights": EmbWeights, "kh_sizeof_emb_block": EmbBlock, "kh_sizeof_rows_gemm": RowsGemm,
-           "kh_sizeof_mid_weights": MidWeights}
+           "kh_sizeof_mid_weights": MidWeights, "kh_sizeof_tail_weights": TailWeights}
 MID_SYMBOLS = ("kh_rows_gemm", "kh_rows_gemm_form", "kh_mid_layout", "kh_mid_pack", "kh_mid", "kh_mid_a", "kh_mid_b",
                "kh_mid_c", "kh_lstm_cell_rows")
+TAIL_SYMBOLS = ("kh_tail_clusters", "kh_tail", "kh_tail_slots")
 EMBED_SYMBOLS = ("kh_embed_layout", "kh_estd", "kh_efront", "kh_egn_apply", "kh_eqkv_ln", "kh_softmax_rows",
                  "kh_eattn_out_grid", "kh_eattn_out", "kh_ehead", "kh_einter_mask", "kh_eput_lens")
 SYMBOLS = ("kh_gemm", "kh_gemm_plan", "kh_split_planes", "kh_lstm", "kh_launch_count", "kh_sep_layout", "kh_qkv",
            "kh_qkv_many", "kh_kv_gather", "kh_attention", "kh_attn_out", "kh_ln_frame_res",
            "kh_attn_cluster_resident", "kh_front", "kh_front_many", "kh_front_many_geometry", "kh_front1", "kh_back",
-           "kh_back_many", "kh_back_many_geometry") + EMBED_SYMBOLS + MID_SYMBOLS + tuple(MIRRORS)
+           "kh_back_many", "kh_back_many_geometry") + EMBED_SYMBOLS + MID_SYMBOLS + TAIL_SYMBOLS + tuple(MIRRORS)
 EMBED_LAYOUT_NAMES = ("NFFT", "HOP", "NF", "CH", "QK", "VDIM", "FC", "NQKV", "DFT_LD", "EAOUT_SMEM", "LENS_PER_LAUNCH")
 
 ATTN_FORMS = {"query": 0, "tile": 1, "cluster": 2}
@@ -177,6 +186,12 @@ def lib():
             "kh_mid_b": [MW, P, P, I64, I, P, I64, I, I, P, P],
             "kh_mid_c": [MW, P, P, P, I, I64, I, P],
             "kh_lstm_cell_rows": [P, P, I64, I, P, I64, P, P],
+        })
+        TW = ctypes.POINTER(TailWeights)
+        sigs.update({
+            "kh_tail_clusters": [],
+            "kh_tail": [TW, P, P, P, P, I64, I, I, I, I, P, P],
+            "kh_tail_slots": [TW, P, P, P, P, I64, P, I, P, I, I, I, P],
         })
         L.kh_mid_pack.restype = None
         L.kh_mid_pack.argtypes = [P] * 6
@@ -1161,18 +1176,21 @@ def mid_c64(X1, X1e, H, He, p, drop_residual=False, drop_bias=False, slope_group
 
 
 def mid64(Y, X, h, c, p, swap_if=False, drop_c=False, whh_new_h=False, drop_residual=False, drop_bias=False,
-          slope_groups=SLOPE_GROUPS, unbiased=False, eps_outside=False):
+          slope_groups=SLOPE_GROUPS, unbiased=False, eps_outside=False, hb=None, cb=None):
     """the one-hop middle section of rows Y [..][128], X [..][64] with the carried (h, c) [..][64]: X1 = X + Y W_l1 + b;
-    the inter-LSTM step from LN(X1) and (h, c); X2 = X1 + h' W_l2 + b; P = PReLU(X2 W_qkv + b).  Mutants: those of
-    mid_a64, cell64 and mid_c64 (drop_residual / drop_bias apply to both Linears), whh_new_h (h W_hh taken from the new
-    h: the state read after it was overwritten).  Returns a dict of X1, GI, h, c, X2, P and their bounds (key + "_b")."""
+    the inter-LSTM step from LN(X1) and (h, c); X2 = X1 + h' W_l2 + b; P = PReLU(X2 W_qkv + b).  hb / cb: bounds of the
+    carried (h, c) (None: exact).  Mutants: those of mid_a64, cell64 and mid_c64 (drop_residual / drop_bias apply to both
+    Linears), whh_new_h (h W_hh taken from the new h: the state read after it was overwritten).  Returns a dict of X1, GI,
+    h, c, X2, P and their bounds (key + "_b")."""
     X1, X1e, GI, GIe = mid_a64(Y, X, p, drop_residual, drop_bias, unbiased, eps_outside)
     zero = torch.zeros_like(h.double())
-    G, Ge = mid_gates64(GI, GIe, h, zero, p)
-    h2, h2e, c2, c2e = cell64(G, Ge, c, zero, swap_if, drop_c)
+    hb = zero if hb is None else hb.double()
+    cb = zero if cb is None else cb.double()
+    G, Ge = mid_gates64(GI, GIe, h, hb, p)
+    h2, h2e, c2, c2e = cell64(G, Ge, c, cb, swap_if, drop_c)
     if whh_new_h:
         G, Ge = mid_gates64(GI, GIe, h2.float(), zero, p)
-        h2, h2e, c2, c2e = cell64(G, Ge, c, zero, swap_if, drop_c)
+        h2, h2e, c2, c2e = cell64(G, Ge, c, cb, swap_if, drop_c)
     X2, X2e, P, Pe = mid_c64(X1, X1e, h2, h2e, p, drop_residual, drop_bias, slope_groups)
     return dict(X1=X1, X1_b=X1e, GI=GI, GI_b=GIe, h=h2, h_b=h2e, c=c2, c_b=c2e, X2=X2, X2_b=X2e, P=P, P_b=Pe)
 
@@ -1199,3 +1217,168 @@ def mid_b64(GIs, h, c, p, GIe=None, no_advance=False, store_first=False):
     if stored is None:
         stored = (h, he, c, ce)
     return torch.stack(Hs), torch.stack(Hes), stored
+
+
+# ---- the fused one-hop tail of a block (hop_kernels.cuh: tail_kernel; tfgridnet_causal.py:518-588, :250, :505-512) ---
+# tail_kernel runs, for one frame of each stream, the middle section (mid64), the Q/K/V LayerNorms, the 50-frame
+# attention over the K/V ring, the output projection with its LayerNorm(6208), the residual, the speaker gate and the next
+# block's input projection.  One 16-CTA cluster per stream: CTA p < 13 owns bins 8p .. 8p + 7 (the last tile: bin 96
+# alone) and combines the LayerNorm statistics of all tiles from their (mean, M2); CTA r attends with head r / 4 over
+# window rows TAIL_PART_ROWS[r % 4] .. TAIL_PART_ROWS[r % 4 + 1] - 1 (row j = frame pos - 49 + j; the last part's last
+# row is the one this launch writes), and the tile CTAs merge each head's four partials by their maxima.
+TAIL_CL, TAIL_TILES = 16, 13
+TAIL_PART_ROWS = (0, 13, 26, 38, 50)
+# the longest rounding chains of the kernel's LayerNorm statistics: phase Q sums 8 values per lane over a 4-level
+# shuffle tree and combines 13 tiles one after the other; phase O sums 2 values per thread over a block tree (5 + 3
+# levels) and 13 tiles over a 5-level warp tree
+TAIL_Q_CHAIN, TAIL_O_CHAIN = 32, 24
+# absolute error of a normalised Q/K/V value from everything before the statistics (the 64-term projection of X2, whose
+# rows of low X1 spread carry the LayerNorm(64)'s amplified rounding, over the group's spread ~0.5), and of an output
+# value from the attention and the projection (|score| ~ 1 or ~80, 50-row sums, a 64-term projection over the spread of
+# the LayerNorm(6208)'s input)
+TAIL_QKV_TOL, TAIL_X_TOL = 5e-5, 2e-4
+
+
+def tail_clusters():
+    """how many tail_kernel clusters the device holds at once (0: it cannot be scheduled)"""
+    return lib().kh_tail_clusters()
+
+
+def tail(w, Y, X, GX, state, sstride, blk, B, apply_gate, frame_k=0, active=None):
+    return lib().kh_tail(ctypes.byref(w), ptr(Y), ptr(X), ptr(GX), ptr(state), sstride, blk, B, apply_gate, frame_k,
+                         ptr(active), stream())
+
+
+def tail_slots(w, Y, X, GX, state, sstride, slots, batch, hops, blk, B, apply_gate):
+    return lib().kh_tail_slots(ctypes.byref(w), ptr(Y), ptr(X), ptr(GX), ptr(state), sstride, ptr(slots), batch, ptr(hops),
+                               blk, B, apply_gate, stream())
+
+
+def chan_ln64(y, g, b, d, tiles="exact"):
+    """LayerNorm (biased variance, eps 1e-5 inside the sqrt) over y [97 * d] (element f*d + e), with the statistics
+    combined from the 13 row tiles' (mean, M2) as tail_kernel combines them (Chan): mean = sum n_p m_p / N, M2 = sum
+    (M2_p + n_p (m_p - mean)^2).  tiles="exact" equals layer_norm64.  Mutants: "equal" (every tile weighted as 8 rows,
+    also the 1-row last tile), "no_between" (M2 without the between-tile term), "per_tile" (each tile normalised by its
+    own statistics)."""
+    y = y.double()
+    t = y.view(NF, d)
+    parts = [t[p * 8:(p + 1) * 8].reshape(-1) for p in range(TAIL_TILES)]
+    if tiles == "per_tile":
+        out = torch.cat([(q - q.mean()) / torch.sqrt(((q - q.mean()) ** 2).mean() + 1e-5) for q in parts])
+        return out * g.double() + b.double()
+    n = [float(q.numel()) for q in parts]
+    wts = [8.0 * d] * len(parts) if tiles == "equal" else n
+    N = float(NF * d)
+    m = [q.mean() for q in parts]
+    m2 = [((q - mq) ** 2).sum() for q, mq in zip(parts, m)]
+    mean = sum(wp * mp for wp, mp in zip(wts, m)) / N
+    M2 = sum(m2) if tiles == "no_between" else sum(a + wp * (mp - mean) ** 2 for a, wp, mp in zip(m2, wts, m))
+    return (y - mean) / torch.sqrt(M2 / N + 1e-5) * g.double() + b.double()
+
+
+def tail64(Y, X, h, c, p, hist_k, hist_v, gate=None, nxt=None, hist_tol=0.0, hb=None, cb=None, stale=None, shift=False,
+           no_rescale=False, qkv_stats="exact", ln_per_tile=False, heads_transposed=False, gate_first=False, drop_gate=False,
+           ih_from_x2=False, **mid_mutant):
+    """tail_kernel for one stream at clock pos, in float64, with a bound on each output's fp32 error.
+    Y [97][128] (the intra BiLSTM's output), X [97][64] (the block input), (h, c) [97][64] the carried inter-LSTM state
+    (bounds hb / cb); p: the block weights (mid64's, lnq_g .. lnv_b of >= 582 / 1552 values, wp_t, bp, lnp_g, lnp_b);
+    hist_k [50][4][>= 582] and hist_v [50][4][1552]: the K / V rows of frames pos - 50 .. pos - 1 (zero rows before the
+    stream start; row 0 is read only by the shift mutant), exact up to hist_tol.  gate [97][64]: the speaker gate of the
+    block output (None: no gate); nxt: the next block's (ln_g, ln_b, wih_t, bias) (None: no phase G).
+
+    Bounds.  (h, c): mid64's element-wise bounds.  Q/K/V, per (Q/K/V, head) group: TAIL_QKV_TOL |g|max, plus the
+    statistics' rounding chain TAIL_Q_CHAIN u |mean| / sigma |g|max (what a group of mean >> spread costs) and P's own
+    rounding 4 u |P|max / sigma |g|max.  X: TAIL_X_TOL, twice the largest Q/K/V group bound and the window rows' hist_tol
+    (a K/V or q error moves a score and so Z by about as much), and the LayerNorm(6208)'s chain TAIL_O_CHAIN u |mean| /
+    sigma |g|max, times max(1, |gate|).  GX: ih64's bound, plus X's bound carried through the LayerNorm(64) and |W_ih|.
+
+    Mutants: those of mid64 (keyword arguments), stale = (k [4][>= 582], v [4][1552]) the newest row read before this hop
+    wrote it (the slot's old content), shift (the window one frame earlier: pos - 50 .. pos - 1), no_rescale (each part's
+    partial taken with its own max, merged without exp(m_p - max)), qkv_stats = "equal" / "no_between" (chan_ln64),
+    ln_per_tile (LayerNorm(6208) per row tile), heads_transposed (projection column c0 + e*4 + h), gate_first (X2 gate +
+    LN), drop_gate, ih_from_x2 (phase G applied to X2).
+
+    Returns a dict of X, K [4][582], V [4][1552], Q [4][582], h, c, X2, P, Z, GX (with nxt) and the bounds of X, K, V, Q,
+    h, c and GX (key + "_b", the shape of the value)."""
+    m = mid64(Y, X, h, c, p, hb=hb, cb=cb, **mid_mutant)
+    P = m["P"]
+    # phase Q: head split and LayerNorm over (F, E) per (Q/K/V, head)
+    qkv, qkv_b = [], []
+    for d, c0, key in ((QE, 0, "lnq"), (QE, 24, "lnk"), (VD, 48, "lnv")):
+        n = NF * d
+        g, b = p[key + "_g"][:n].double(), p[key + "_b"][:n].double()
+        cols = P[:, c0:c0 + NHEAD * d]
+        if heads_transposed:
+            y = cols.reshape(NF, d, NHEAD).permute(2, 0, 1).reshape(NHEAD, n)
+        else:
+            y = cols.reshape(NF, NHEAD, d).permute(1, 0, 2).reshape(NHEAD, n)
+        qkv.append(torch.stack([chan_ln64(y[hh], g, b, d, qkv_stats) for hh in range(NHEAD)]))
+        mu, sd = y.mean(-1, keepdim=True), y.std(-1, unbiased=False, keepdim=True)
+        tol = g.abs().max() * (TAIL_QKV_TOL + U32 * (TAIL_Q_CHAIN * mu.abs() + 4 * y.abs().max(-1, keepdim=True)[0]) / sd)
+        qkv_b.append(tol.expand(NHEAD, n))
+    (q, k, v), (qb, kb, vb) = qkv, qkv_b
+    # phase A: the window of frames pos - 49 .. pos (shift: pos - 50 .. pos - 1)
+    hk, hv = hist_k[..., :QK_DIM].double(), hist_v.double()
+    k_new, v_new = (k, v) if stale is None else (stale[0][..., :QK_DIM].double(), stale[1].double())
+    Kw, Vw = (hk, hv) if shift else (torch.cat([hk[1:], k_new[None]]), torch.cat([hv[1:], v_new[None]]))
+    o = []
+    for hh in range(NHEAD):
+        s = Kw[:, hh] @ q[hh] / math.sqrt(QK_DIM)                         # [50]
+        if no_rescale:
+            e = torch.cat([torch.exp(s[a:z] - s[a:z].max()) for a, z in zip(TAIL_PART_ROWS[:-1], TAIL_PART_ROWS[1:])])
+        else:
+            e = torch.exp(s - s.max())
+        o.append(e / e.sum() @ Vw[:, hh])
+    Z = merge_heads64(torch.stack(o)[None])[0]
+    # phase O: Linear + PReLU, LayerNorm(6208), residual, gate
+    Pp = prelu64(Z @ p["wp_t"].double() + p["bp"].double(), float(p["slopes"][3]))
+    lg, lb = p["lnp_g"].double(), p["lnp_b"].double()
+    y = chan_ln64(Pp.reshape(FC), lg, lb, CH, "per_tile" if ln_per_tile else "exact").view(NF, CH)
+    X2 = m["X2"]
+    res = X2 + y
+    xtol = TAIL_X_TOL + 2 * max(float(t.max()) for t in qkv_b) + 2 * hist_tol + \
+        TAIL_O_CHAIN * U32 * float(Pp.mean().abs() / Pp.std(unbiased=False) * lg.abs().max())
+    if gate is None or drop_gate:
+        Xo = res
+    else:
+        gt = gate.double()
+        Xo = X2 * gt + y if gate_first else res * gt
+        xtol *= max(1.0, float(gt.abs().max()))
+    Xb = torch.full_like(Xo, xtol)
+    out = dict(X=Xo, X_b=Xb, K=k, K_b=kb, V=v, V_b=vb, Q=q, Q_b=qb, h=m["h"], h_b=m["h_b"], c=m["c"], c_b=m["c_b"], X2=X2,
+               P=P, Z=Z)
+    if nxt is not None:
+        ng, nb, wih_t, bias = nxt
+        src = X2 if ih_from_x2 else Xo
+        GX, GXb = ih64(src, ng, nb, wih_t, bias)
+        sd = src.std(-1, unbiased=False, keepdim=True)
+        xh = (src - src.mean(-1, keepdim=True)) / sd
+        carried = ((ng.double().abs() * 2 * xtol + (ng.double() * xh).abs() * xtol) / sd) @ wih_t.double().abs()
+        out.update(GX=GX, GX_b=GXb + carried)
+    return out
+
+
+# tail64's mutants that need no data of their own (stale=(k, v) needs the slot's old rows), by name
+TAIL_MUTANTS = {"shift": dict(shift=True), "no_rescale": dict(no_rescale=True), "qkv_equal_weights": dict(qkv_stats="equal"),
+                "qkv_no_between": dict(qkv_stats="no_between"), "ln_per_tile": dict(ln_per_tile=True),
+                "heads_transposed": dict(heads_transposed=True), "gate_first": dict(gate_first=True),
+                "drop_gate": dict(drop_gate=True), "ih_from_x2": dict(ih_from_x2=True), "eps_outside": dict(eps_outside=True),
+                "swap_if": dict(swap_if=True), "drop_c": dict(drop_c=True)}
+
+
+def tail_chain64(Ys, Xs, h, c, p, hist_k, hist_v, gates=None, nxt=None, **mutant):
+    """len(Ys) consecutive hops of tail64 on one stream: hop j runs at clock pos + j on Ys[j], Xs[j] and the (h, c) hop
+    j - 1 left, and its window holds the K/V rows hops 0 .. j - 1 wrote (exact up to their bounds).  hist_k / hist_v: the
+    rows of frames pos - 50 .. pos - 1.  Returns the list of tail64's outputs."""
+    K, V = hist_k[..., :QK_DIM].double(), hist_v.double()
+    hb = cb = None
+    tol = 0.0
+    outs = []
+    for j in range(len(Ys)):
+        r = tail64(Ys[j], Xs[j], h, c, p, K[j:j + ATT], V[j:j + ATT], None if gates is None else gates[j], nxt, tol, hb, cb,
+                   **mutant)
+        outs.append(r)
+        K, V = torch.cat([K, r["K"][None]]), torch.cat([V, r["V"][None]])
+        tol = max(tol, float(r["K_b"].max()), float(r["V_b"].max()))
+        h, c, hb, cb = r["h"], r["c"], r["h_b"], r["c_b"]
+    return outs

@@ -1,7 +1,8 @@
 // Test-only C entry points into the engine's tensor-core GEMM (umma::launch), LSTM recurrences (lstm.cuh,
 // tc_lstm.cuh), the separator's attention section (sep_kernels.cuh), its front and back (sep_kernels.cuh,
 // hop_kernels.cuh), its CUDA-core rows GEMM (gemm.cuh), its one-hop middle section (mid_kernel.cuh: mid_kernel, mid_a,
-// mid_b, mid_c) and the tensor-core chain's cell kernel (sep_kernels.cuh: lstm_cell_rows), and the enrollment network's
+// mid_b, mid_c), the fused one-hop tail of a block (hop_kernels.cuh: tail_kernel, both record maps), the tensor-core
+// chain's cell kernel (sep_kernels.cuh: lstm_cell_rows), and the enrollment network's
 // own kernels (embed_kernels.cuh: estd, efront, egn_apply, eqkv_ln, softmax_rows, eattn_out, ehead, einter_mask,
 // eput_lens), so that the kernel-level tests (tests/test_*_kernels_gpu.py) can drive each kernel directly with arbitrary
 // shapes and compare it element by element with a float64 reference.
@@ -161,8 +162,11 @@ KH_API int kh_split_planes(const float* src, int64_t row_stride, int64_t col_str
                                    static_cast<__nv_bfloat16*>(lo), static_cast<cudaStream_t>(stream));
 }
 
+// 16-CTA tail_kernel clusters the configured device holds at once (set_tail_attrs; 0: tail_kernel cannot be scheduled)
+static thread_local int tail_clusters = 0;
+
 // the dynamic shared memory of every kernel launched here that needs more than the default, set once per device (the
-// separator's dense forms with the engine's own list)
+// separator's dense forms with the engine's own list, and both forms of tail_kernel)
 static cudaError_t configure() {
     static thread_local int configured_dev = -1;
     int dev = 0;
@@ -174,6 +178,7 @@ static cudaError_t configure() {
     if (e == cudaSuccess) e = set_sep_smem<int64_t>();
     if (e == cudaSuccess) e = set_mid_split_smem();
     if (e == cudaSuccess) e = cudaFuncSetAttribute(emb::eattn_out_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)emb::EAOUT_SMEM);
+    if (e == cudaSuccess) tail_clusters = set_tail_attrs();
     if (e == cudaSuccess) configured_dev = dev;
     return e;
 }
@@ -502,6 +507,62 @@ KH_API int kh_lstm_cell_rows(const float* gates, float* state, int64_t sstride, 
                              const uint8_t* active, void* stream) {
     if (rows <= 0 || rows * 64 > 0x7fffffff || blk < 0 || sstride <= 0) return (int)cudaErrorInvalidValue;
     return (int)launch_lstm_cell_rows(false, static_cast<cudaStream_t>(stream), gates, state, sstride, blk, Hout, rows, active);
+}
+
+// ---- the fused one-hop tail of a block (hop_kernels.cuh: tail_kernel) -------------------------------------------------
+// The fields of BlockWeights that tail_kernel reads (the middle section's, slopes[3] = the output PReLU, the Q/K/V
+// LayerNorms with the Q/K vectors read as QK_LD floats, the output projection and its LayerNorm), and the next block's
+// input projection (NextIh; nx_wih_t == null: no next block, GX untouched).
+struct KhTailWeights {
+    const float *mid_pack, *bl1, *ln2_g, *ln2_b, *b2, *bl2, *bqkv, *slopes;
+    const float *lnq_g, *lnq_b, *lnk_g, *lnk_b, *lnv_g, *lnv_b;
+    const float *wp_t, *bp, *lnp_g, *lnp_b;
+    const float *nx_ln_g, *nx_ln_b, *nx_wih_t, *nx_bias;
+};
+
+static BlockWeights to_tail(const KhTailWeights& k) {
+    BlockWeights w{};
+    w.mid_pack = k.mid_pack; w.bl1 = k.bl1; w.ln2_g = k.ln2_g; w.ln2_b = k.ln2_b; w.b2 = k.b2; w.bl2 = k.bl2; w.bqkv = k.bqkv;
+    w.slopes = k.slopes;
+    w.lnq_g = k.lnq_g; w.lnq_b = k.lnq_b; w.lnk_g = k.lnk_g; w.lnk_b = k.lnk_b; w.lnv_g = k.lnv_g; w.lnv_b = k.lnv_b;
+    w.wp_t = k.wp_t; w.bp = k.bp; w.lnp_g = k.lnp_g; w.lnp_b = k.lnp_b;
+    return w;
+}
+
+static NextIh to_next(const KhTailWeights& k, float* GX) {
+    NextIh nx{};
+    if (k.nx_wih_t != nullptr) { nx.ln_g = k.nx_ln_g; nx.ln_b = k.nx_ln_b; nx.wih_t = k.nx_wih_t; nx.bias = k.nx_bias; nx.GX = GX; }
+    return nx;
+}
+
+KH_API int kh_sizeof_tail_weights() { return (int)sizeof(KhTailWeights); }
+
+// 16-CTA tail_kernel clusters the current device holds at once (set_tail_attrs): the engine fuses a block's tail while
+// the call's rows fit in one wave of them
+KH_API int kh_tail_clusters() { return configure() == cudaSuccess ? tail_clusters : 0; }
+
+// tail_kernel, dense map: row b of Y [B][97][128], X [B][97][64] (updated in place) and GX [B][97][512] is record b at
+// state + header + b * sstride; block blk
+KH_API int kh_tail(const KhTailWeights* w, const float* Y, float* X, float* GX, float* state, int64_t sstride, int blk, int B,
+                   int apply_gate, int frame_k, const uint8_t* active, void* stream) {
+    if (B <= 0 || blk < 0 || sstride <= 0 || frame_k < 0 || (w->nx_wih_t != nullptr && GX == nullptr)) return (int)cudaErrorInvalidValue;
+    if (cudaError_t e = configure()) return (int)e;
+    if (tail_clusters <= 0) return (int)cudaErrorInvalidConfiguration;
+    return (int)launch_tail(false, static_cast<cudaStream_t>(stream), B, Y, X, state, sstride, blk, to_tail(*w), to_next(*w, GX), apply_gate,
+                            frame_k, active);
+}
+
+// tail_kernel_t<Records>: row b is record slots[b] of a state of `batch` records of sstride floats; hops (device, [B]) may
+// be null; the call is one frame
+KH_API int kh_tail_slots(const KhTailWeights* w, const float* Y, float* X, float* GX, float* state, int64_t sstride,
+                         const int32_t* slots, int batch, const int32_t* hops, int blk, int B, int apply_gate, void* stream) {
+    if (B <= 0 || batch <= 0 || blk < 0 || sstride <= 0 || slots == nullptr || (w->nx_wih_t != nullptr && GX == nullptr))
+        return (int)cudaErrorInvalidValue;
+    if (cudaError_t e = configure()) return (int)e;
+    if (tail_clusters <= 0) return (int)cudaErrorInvalidConfiguration;
+    const Records recs{sstride, slots, batch, hops, 1};
+    return (int)launch_tail(false, static_cast<cudaStream_t>(stream), B, Y, X, state, recs, blk, to_tail(*w), to_next(*w, GX), apply_gate,
+                            0, nullptr);
 }
 
 // ---- the enrollment network's own kernels (embed_kernels.cuh) --------------------------------------------------------

@@ -1,6 +1,6 @@
 """The kernel harness library (tests/kernels/) and the float64 references the kernel-level GPU tests
 (test_umma_gemm_gpu.py, test_lstm_kernels_gpu.py, test_attention_kernels_gpu.py, test_front_back_kernels_gpu.py,
-test_embed_kernels_gpu.py, test_rows_gemm_kernels_gpu.py, test_mid_kernels_gpu.py) rely on.  The enrollment references (estd64, efront64, egn64, eqkv_ln64, softmax64,
+test_embed_kernels_gpu.py, test_rows_gemm_kernels_gpu.py, test_mid_kernels_gpu.py, test_tail_kernel_gpu.py) rely on.  The enrollment references (estd64, efront64, egn64, eqkv_ln64, softmax64,
 eattn_out64, ehead64) are pinned to oracle/restate.py; each of their mutants is shown to miss the reference by more than
 10x its bound, and einter_mask_expected's mutants to change it.  No device needed."""
 import ctypes
@@ -610,3 +610,109 @@ def test_rows_gemm_and_mid_mutants_differ():
     for m in ("swap_if", "drop_c"):
         hm, _, cm, _ = kh.lstm_cell64(gates, c, **{m: True})
         assert _ratio(hm, hl, hlb) >= 10 and _ratio(cm, cl, clb) >= 10, m
+
+
+# ---- the fused one-hop tail (test_tail_kernel_gpu.py) ------------------------------------------------------------------
+def _tail_block(sd64, blk):
+    """block blk's weights in the engine's stored layouts (sep_engine.cu: W^T, gate columns j*4 + q, slopes Q K V proj)"""
+    g = lambda k: sd64[f"tfgridnet.blocks.{blk}." + k]
+    pk = kh.packed_from_torch
+    p = dict(wl1_t=g("intra_linear.weight").T, bl1=g("intra_linear.bias"), ln2_g=g("inter_norm.norm.weight"),
+             ln2_b=g("inter_norm.norm.bias"), wih2_t=pk(g("inter_rnn.weight_ih_l0")).T,
+             whh2_t=pk(g("inter_rnn.weight_hh_l0")).T, b2=pk(g("inter_rnn.bias_ih_l0") + g("inter_rnn.bias_hh_l0")),
+             wl2_t=g("inter_linear.weight").T, bl2=g("inter_linear.bias"),
+             wqkv_t=torch.cat([g(f"attn_conv_{n}.0.weight") for n in "QKV"]).T,
+             bqkv=torch.cat([g(f"attn_conv_{n}.0.bias") for n in "QKV"]),
+             slopes=torch.stack([g(f"attn_conv_{n}.1.weight")[0] for n in "QKV"] + [g("attn_concat_proj.1.weight")[0]]),
+             wp_t=g("attn_concat_proj.0.weight").T, bp=g("attn_concat_proj.0.bias"),
+             lnp_g=g("attn_concat_proj.3.norm.weight"), lnp_b=g("attn_concat_proj.3.norm.bias"))
+    for n in "QKV":
+        p[f"ln{n.lower()}_g"], p[f"ln{n.lower()}_b"] = g(f"attn_conv_{n}.3.norm.weight"), g(f"attn_conv_{n}.3.norm.bias")
+    ih = (g("intra_norm.norm.weight"), g("intra_norm.norm.bias"),
+          torch.cat([pk(g("intra_rnn.weight_ih_l0")).T, pk(g("intra_rnn.weight_ih_l0_reverse")).T], 1),
+          torch.cat([pk(g("intra_rnn.bias_ih_l0") + g("intra_rnn.bias_hh_l0")),
+                     pk(g("intra_rnn.bias_ih_l0_reverse") + g("intra_rnn.bias_hh_l0_reverse"))]))
+    return p, ih
+
+
+def _intra(sd64, blk, X):
+    """the block's intra BiLSTM output [97][128] of X [97][64] (oracle/restate.py::sep_block's first half)"""
+    from oracle import restate
+    g = lambda k: sd64[f"tfgridnet.blocks.{blk}." + k]
+    A = restate._ln(X, g("intra_norm.norm.weight"), g("intra_norm.norm.bias"))[None]
+    yf, _, _ = restate._lstm_seq(A, g("intra_rnn.weight_ih_l0"), g("intra_rnn.weight_hh_l0"), g("intra_rnn.bias_ih_l0"),
+                                 g("intra_rnn.bias_hh_l0"))
+    yb, _, _ = restate._lstm_seq(A, g("intra_rnn.weight_ih_l0_reverse"), g("intra_rnn.weight_hh_l0_reverse"),
+                                 g("intra_rnn.bias_ih_l0_reverse"), g("intra_rnn.bias_hh_l0_reverse"), reverse=True)
+    return torch.cat([yf[0], yb[0]], -1)
+
+
+def _ring_rows(buf):
+    """the oracle's K_buf / V_buf [4][49][n] (frames pos - 49 .. pos - 1) as tail64's rows of frames pos - 50 .. pos - 1"""
+    k, v = buf["K_buf"].permute(1, 0, 2), buf["V_buf"].permute(1, 0, 2)
+    return torch.cat([torch.zeros_like(k[:1]), k]), torch.cat([torch.zeros_like(v[:1]), v])
+
+
+def test_tail_reference_is_the_model(tsh_params):
+    """tail64 (and tail_chain64 over 3 hops) reproduces oracle/restate.py::sep_block for T = 1 with carried buffers: the
+    block output, the new K_buf / V_buf rows and (h0, c0); its GX is the next block's intra input projection of that
+    output (the gate applied first, as sep_core applies it to the next block's input)"""
+    from oracle import restate
+    sd64 = restate.cast_sd(_net_sd(tsh_params, seed=3), torch.float64)
+    hp = restate.sep_hparams(sd64)
+    p, _ = _tail_block(sd64, 0)
+    _, ih1 = _tail_block(sd64, 1)
+    g = torch.Generator().manual_seed(11)
+    r = lambda *s: torch.randn(*s, generator=g, dtype=torch.float64)
+    buf = dict(K_buf=r(4, 49, kh.QK_DIM), V_buf=r(4, 49, kh.V_DIM), h0=0.5 * r(1, kh.NF, 64), c0=r(1, kh.NF, 64))
+    gate = 1 + 0.5 * r(kh.NF, 64)
+    X = [r(kh.NF, 64) for _ in range(3)]
+    Y = [_intra(sd64, 0, x) for x in X]
+    hk, hv = _ring_rows(buf)
+    chain = kh.tail_chain64(Y, X, buf["h0"][0], buf["c0"][0], p, hk, hv, gates=[gate] * 3, nxt=ih1)
+    one = kh.tail64(Y[0], X[0], buf["h0"][0], buf["c0"][0], p, hk, hv, gate, ih1)
+    for t in range(3):
+        want = restate.sep_block(sd64, "tfgridnet.blocks.0.", X[t][None, None], buf, hp, 50)[0, 0]
+        got = chain[t]
+        for k, ref in (("X", want * gate), ("K", buf["K_buf"][:, -1]), ("V", buf["V_buf"][:, -1]), ("h", buf["h0"][0]),
+                       ("c", buf["c0"][0])):
+            assert torch.allclose(got[k], ref, rtol=0, atol=1e-12), (t, k)
+            assert bool((got[k + "_b"] > 0).all()), (t, k)
+            if t == 0:
+                assert torch.equal(one[k], got[k]), k
+        # the next block's intra gates of its input (the gated output): columns d*256 + j*4 + q
+        A = restate._ln(want * gate, ih1[0], ih1[1])
+        blk1 = lambda k: sd64["tfgridnet.blocks.1." + k]
+        gx = torch.cat([kh.packed_from_torch((A @ blk1(f"intra_rnn.weight_ih_l0{s}").T + blk1(f"intra_rnn.bias_ih_l0{s}")
+                                              + blk1(f"intra_rnn.bias_hh_l0{s}")).T).T for s in ("", "_reverse")], 1)
+        assert torch.allclose(got["GX"], gx, rtol=0, atol=1e-12), t
+    assert torch.allclose(kh.chan_ln64(X[0].reshape(-1)[:kh.NF * 6], p["lnq_g"], p["lnq_b"], 6),
+                          kh.layer_norm64(X[0].reshape(-1)[:kh.NF * 6], p["lnq_g"], p["lnq_b"]), rtol=0, atol=1e-12)
+
+
+def test_tail_mutants_differ():
+    """every mutated tail64 misses the reference by >= 10x its bound on at least one output (X, K, V, h, c or GX), on
+    test-like data: a young stream's window (zero rows), X1 of small spread on rows 7 and 96, a K head of mean >> spread"""
+    p = _mid_params(6)
+    g = torch.Generator().manual_seed(8)
+    r = lambda *s, scale=1.0: scale * torch.randn(*s, generator=g)
+    p.update(lnq_g=1 + r(kh.QK_DIM, scale=0.2), lnq_b=r(kh.QK_DIM, scale=0.2), lnk_g=1 + r(kh.QK_DIM, scale=0.2),
+             lnk_b=r(kh.QK_DIM, scale=0.2), lnv_g=1 + r(kh.V_DIM, scale=0.2), lnv_b=r(kh.V_DIM, scale=0.2),
+             wp_t=r(64, 64, scale=0.25), bp=r(64, scale=0.1), lnp_g=1 + r(kh.FC, scale=0.2), lnp_b=r(kh.FC, scale=0.2))
+    p["bqkv"][36:42] = 5.0                                  # K head 2: mean 5, spread ~0.1
+    p["wqkv_t"][:, 36:42] *= 0.1
+    Y, X, h, c = r(kh.NF, 128), r(kh.NF, 64), r(kh.NF, 64, scale=0.5), r(kh.NF, 64)
+    for f in (7, 96):
+        Y[f] = 0
+        X[f] = 0.4 - p["bl1"] + 0.01 * r(64)
+    hk, hv = torch.zeros(50, kh.NHEAD, kh.QK_DIM), torch.zeros(50, kh.NHEAD, kh.V_DIM)
+    hk[20:], hv[20:] = r(30, kh.NHEAD, kh.QK_DIM), r(30, kh.NHEAD, kh.V_DIM)     # frames before the start: zero rows
+    gate = 1 + 0.5 * r(kh.NF, 64)
+    gate[::5] *= -1
+    nxt = (1 + r(64, scale=0.2), r(64, scale=0.2), r(64, 512, scale=0.125), r(512, scale=0.3))
+    stale = (r(kh.NHEAD, kh.QK_DIM), r(kh.NHEAD, kh.V_DIM))
+    ref = kh.tail64(Y, X, h, c, p, hk, hv, gate, nxt)
+    keys = ("X", "K", "V", "h", "c", "GX")
+    for name, kw in list(kh.TAIL_MUTANTS.items()) + [("stale", dict(stale=stale))]:
+        mr = kh.tail64(Y, X, h, c, p, hk, hv, gate, nxt, **kw)
+        assert max(_ratio(mr[k], ref[k], ref[k + "_b"]) for k in keys) >= 10, name
