@@ -450,9 +450,8 @@ struct Chain {
         }
         const int32_t* owner = nullptr;      // dense targets: row r belongs to mixture r / K
         if constexpr (slots) owner = lists + 2 * (int64_t)a.B;
-        CK(launch_k(f.pdl, spk_gate_kernel_t<Map>, dim3(a.B), dim3(256), 0, st, a.emb, PRE, a.state, recs, e->w));
-        CK(launch_k(f.pdl, gate_fanout_kernel_t<Map>, dim3(a.T, a.B), dim3(256), 0, st, x0, X, (const float*)a.state, recs, owner, K,
-                    a.T, e->n_blocks > 1 ? 1 : 0));
+        CK(launch_spk_gate(f.pdl, st, a.B, a.emb, PRE, a.state, recs, e->w));
+        CK(launch_gate_fanout(f.pdl, st, a.B, x0, X, (const float*)a.state, recs, owner, K, a.T, e->n_blocks > 1 ? 1 : 0));
         MARK("gate_fanout");
         return 0;
     }
@@ -460,10 +459,8 @@ struct Chain {
     int target_lists() {
         if constexpr (slots) {
             if (fans) {
-                const int64_t B = a.B;
-                CK(launch_k(false, target_lists_kernel, dim3(1), dim3(1024), 0, st, a.offsets ? a.slots : nullptr, a.offsets,
-                            a.offsets ? nullptr : a.slots, a.hops, M, K, a.B, a.state_batch, lists, lists + B, lists + 2 * B,
-                            lists + 3 * B, lists + 4 * B));
+                CK(launch_target_lists(st, a.offsets ? a.slots : nullptr, a.offsets, a.offsets ? nullptr : a.slots, a.hops, M, K, a.B,
+                                       a.state_batch, lists));
                 MARK("target_lists");
             }
         }
@@ -521,7 +518,7 @@ struct Chain {
             }
             MARK(inter ? "gemm_ih_inter" : "gemm_ih_intra");
             if constexpr (slots) {
-                if (inter && R.recs.hops) CK(launch_k(false, inter_gate_mask_kernel, dim3(a.T, R.B), dim3(256), 0, st, GX, R.recs, a.T));
+                if (inter && R.recs.hops) CK(launch_inter_gate_mask(st, R.B, GX, R.recs, a.T));
             }
             if (rf.tc) CK(launch_tc_lstm(l, e->tc_passes, st, f.pdl));
             else CK(launch_lstm_rec(l, st, f.pdl, l.nseq / R.B * a.B));      // the form of the call's sequences
@@ -534,20 +531,13 @@ struct Chain {
     // multi-hop calls carry their (h, c) through the inter recurrences, from a copy in the workspace (HG, CG) that
     // gather_hc() takes before block 0 and scatter_hc() stores back after the last block's inter recurrence.  Block b's
     // part holds the rows of rows_of(b) (inter_hc): over listed groups or rows, block 0's part holds the lead rows.
-    // hc_copy: gather_h_kernel or scatter_hc_kernel over the blocks from b0 on that share rows_of(b0)'s record map.  The
-    // kernels address block `blk` of a record from the state pointer they get, so a pointer b0 blocks further makes their
-    // block 0 block b0 of the records.
+    // hc_copy: gather_h_kernel or scatter_hc_kernel over the blocks from b0 on that share rows_of(b0)'s record map
+    // (launch_gather_h / launch_scatter_hc: block b0 of the records, block b0's part of HG and CG).
     int hc_copy(bool scatter, int b0) {
         const BlockRows<Map> R = rows_of(b0);
         const int nb = (fans && b0 == 0) ? 1 : e->n_blocks - b0;
-        const int64_t o = (int64_t)b0 * R.B * FC;
-        const dim3 grid((unsigned)(((int64_t)nb * R.B * FC / 4 + 255) / 256));      // one thread per float4 of h (and c)
-        if (scatter)
-            CK(launch_k(false, scatter_hc_kernel, grid, dim3(256), 0, st, a.state + b0 * BK_STRIDE, R.recs, nb, R.B,
-                        (const float*)HG + o, (const float*)CG + o));
-        else
-            CK(launch_k(false, gather_h_kernel, grid, dim3(256), 0, st, (const float*)a.state + b0 * BK_STRIDE, R.recs, nb, R.B,
-                        HG + o, a.T > 1 ? CG + o : nullptr));
+        if (scatter) CK(launch_scatter_hc(st, b0, a.state, R.recs, nb, R.B, HG, CG));
+        else CK(launch_gather_h(st, b0, a.state, R.recs, nb, R.B, HG, a.T > 1 ? CG : nullptr));
         return 0;
     }
     int gather_hc() {
@@ -573,8 +563,7 @@ struct Chain {
     int h_last(int b, const BlockRows<Map>& R) {      // a ragged row's h is that of its own last frame
         if constexpr (slots) {
             if (R.recs.hops)
-                CK(launch_k(false, inter_h_last_kernel, dim3(R.B), dim3(256), 0, st, (const float*)Y, HG + (int64_t)b * R.B * FC, R.recs,
-                            a.T));
+                CK(launch_inter_h_last(st, R.B, Y, HG + (int64_t)b * R.B * FC, R.recs, a.T));
         }
         return 0;
     }

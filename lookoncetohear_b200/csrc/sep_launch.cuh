@@ -207,4 +207,32 @@ inline cudaError_t launch_back_many(bool pdl, cudaStream_t st, const ChunkWalk& 
                           st, X, y, y_bstride, y_cstride, y_len, state, recs, w, T, pos_rel, g.chunk, g.n_chunks, n_streams, active);
 }
 
+// The slot-list helpers.  gather_h_kernel / scatter_hc_kernel copy blocks b0 .. b0 + n_blocks - 1 of the records, between
+// the state and the copies Hg, Cg [blocks][n_streams][97][64] (Cg may be null for the gather): the kernels address
+// block blk of a record from the state pointer they get, so a pointer b0 blocks further makes their block 0 block b0;
+// one thread per float4 of a block's h (and c).
+inline dim3 hc_copy_grid(int n_blocks, int n_streams) {
+    return dim3((unsigned)(((int64_t)n_blocks * n_streams * FC / 4 + 255) / 256));
+}
+inline cudaError_t launch_gather_h(cudaStream_t st, int b0, const float* state, Records recs, int n_blocks, int n_streams, float* Hg,
+                                   float* Cg) {
+    const int64_t o = (int64_t)b0 * n_streams * FC;
+    return launch_k(false, gather_h_kernel, hc_copy_grid(n_blocks, n_streams), dim3(256), 0, st, state + b0 * BK_STRIDE, recs,
+                    n_blocks, n_streams, Hg + o, Cg ? Cg + o : nullptr);
+}
+inline cudaError_t launch_scatter_hc(cudaStream_t st, int b0, float* state, Records recs, int n_blocks, int n_streams, const float* Hg,
+                                     const float* Cg) {
+    const int64_t o = (int64_t)b0 * n_streams * FC;
+    return launch_k(false, scatter_hc_kernel, hc_copy_grid(n_blocks, n_streams), dim3(256), 0, st, state + b0 * BK_STRIDE, recs,
+                    n_blocks, n_streams, Hg + o, Cg + o);
+}
+// inter_gate_mask_kernel: grid (T, B)
+inline cudaError_t launch_inter_gate_mask(cudaStream_t st, int B, float* gx, Records recs, int T) {
+    return launch_k(false, inter_gate_mask_kernel, dim3(T, B), dim3(256), 0, st, gx, recs, T);
+}
+// inter_h_last_kernel: one CTA per row; Hg = the block's part of gather_h_kernel's copy
+inline cudaError_t launch_inter_h_last(cudaStream_t st, int B, const float* Y, float* Hg, Records recs, int T) {
+    return launch_k(false, inter_h_last_kernel, dim3(B), dim3(256), 0, st, Y, Hg, recs, T);
+}
+
 }  // namespace l2h

@@ -130,4 +130,28 @@ target_lists_kernel(const int32_t* __restrict__ records, const int32_t* __restri
 constexpr auto spk_gate_kernel = spk_gate_kernel_t<int64_t>;
 constexpr auto gate_fanout_kernel = gate_fanout_kernel_t<int64_t>;
 
+// Launchers of the kernels above, shared by the engine (sep_engine.cu) and the kernel tests (tests/kernels/
+// kernel_harness.cu), in the convention of sep_launch.cuh.
+// spk_gate_kernel: one CTA per target row
+template <class Map>
+inline cudaError_t launch_spk_gate(bool pdl, cudaStream_t st, int rows, const float* emb, float* spk_pre, float* state, Map recs,
+                                   const SepWeights& w) {
+    return launch_k(pdl, spk_gate_kernel_t<Map>, dim3(rows), dim3(256), 0, st, emb, spk_pre, state, recs, w);
+}
+// gate_fanout_kernel: grid (T, target rows)
+template <class Map>
+inline cudaError_t launch_gate_fanout(bool pdl, cudaStream_t st, int rows, const float* X0, float* X, const float* state, Map recs,
+                                      const int32_t* owner, int n_targets, int T, int apply_gate) {
+    return launch_k(pdl, gate_fanout_kernel_t<Map>, dim3(T, rows), dim3(256), 0, st, X0, X, state, recs, owner, n_targets, T,
+                    apply_gate);
+}
+// target_lists_kernel: one CTA of 1024 threads.  `lists` is the call's int32 buffer of 5 rows + 1 entries (rows >= n):
+// rec [rows], rec_hops [rows], owner [rows], lead [n] at 3 rows, start [n + 1] at 4 rows.
+inline cudaError_t launch_target_lists(cudaStream_t st, const int32_t* records, const int32_t* offsets, const int32_t* groups,
+                                       const int32_t* hops, int n, int K, int rows, int batch, int32_t* lists) {
+    const int64_t R = rows;
+    return launch_k(false, target_lists_kernel, dim3(1), dim3(1024), 0, st, records, offsets, groups, hops, n, K, rows, batch, lists,
+                    lists + R, lists + 2 * R, lists + 3 * R, lists + 4 * R);
+}
+
 }  // namespace l2h

@@ -57,7 +57,7 @@ class Lstm(ctypes.Structure):
                 ("inner_stride", ctypes.c_int64), ("step_stride", ctypes.c_int64), ("out_outer_stride", ctypes.c_int64),
                 ("out_inner_stride", ctypes.c_int64), ("out_step_stride", ctypes.c_int64),
                 ("x", ctypes.c_void_p), ("x_ld", ctypes.c_int64), ("wih_hi", ctypes.c_void_p), ("wih_lo", ctypes.c_void_p),
-                ("bias", ctypes.c_void_p), ("ln_g", ctypes.c_void_p), ("ln_b", ctypes.c_void_p)]
+                ("bias", ctypes.c_void_p), ("ln_g", ctypes.c_void_p), ("ln_b", ctypes.c_void_p), ("steps", ctypes.c_void_p)]
 
 
 class SepWeights(ctypes.Structure):
@@ -100,19 +100,27 @@ class TailWeights(ctypes.Structure):
                                                 "nx_ln_g", "nx_ln_b", "nx_wih_t", "nx_bias")]
 
 
+class Records(ctypes.Structure):
+    """KhRecords = Records (sep_kernels.cuh): row b is record slots[b] of `batch` records of `stride` floats"""
+    _fields_ = [("stride", ctypes.c_int64), ("slots", ctypes.c_void_p), ("batch", ctypes.c_int32), ("hops", ctypes.c_void_p),
+                ("frames", ctypes.c_int32)]
+
+
 MIRRORS = {"kh_sizeof_asource": ASource, "kh_sizeof_gemm": Gemm, "kh_sizeof_plan": Plan, "kh_sizeof_lstm": Lstm,
            "kh_sizeof_sep_weights": SepWeights, "kh_sizeof_sep_front_back": SepFrontBack,
            "kh_sizeof_emb_weights": EmbWeights, "kh_sizeof_emb_block": EmbBlock, "kh_sizeof_rows_gemm": RowsGemm,
-           "kh_sizeof_mid_weights": MidWeights, "kh_sizeof_tail_weights": TailWeights}
+           "kh_sizeof_mid_weights": MidWeights, "kh_sizeof_tail_weights": TailWeights, "kh_sizeof_records": Records}
 MID_SYMBOLS = ("kh_rows_gemm", "kh_rows_gemm_form", "kh_mid_layout", "kh_mid_pack", "kh_mid", "kh_mid_a", "kh_mid_b",
                "kh_mid_c", "kh_lstm_cell_rows")
 TAIL_SYMBOLS = ("kh_tail_clusters", "kh_tail", "kh_tail_slots")
+TARGETS_SYMBOLS = ("kh_target_lists", "kh_spk_gate", "kh_gate_fanout", "kh_gather_h", "kh_scatter_hc", "kh_inter_gate_mask",
+                   "kh_inter_h_last")
 EMBED_SYMBOLS = ("kh_embed_layout", "kh_estd", "kh_efront", "kh_egn_apply", "kh_eqkv_ln", "kh_softmax_rows",
                  "kh_eattn_out_grid", "kh_eattn_out", "kh_ehead", "kh_einter_mask", "kh_eput_lens")
 SYMBOLS = ("kh_gemm", "kh_gemm_plan", "kh_split_planes", "kh_lstm", "kh_launch_count", "kh_sep_layout", "kh_qkv",
            "kh_qkv_many", "kh_kv_gather", "kh_attention", "kh_attn_out", "kh_ln_frame_res",
            "kh_attn_cluster_resident", "kh_front", "kh_front_many", "kh_front_many_geometry", "kh_front1", "kh_back",
-           "kh_back_many", "kh_back_many_geometry") + EMBED_SYMBOLS + MID_SYMBOLS + TAIL_SYMBOLS + tuple(MIRRORS)
+           "kh_back_many", "kh_back_many_geometry") + EMBED_SYMBOLS + MID_SYMBOLS + TAIL_SYMBOLS + TARGETS_SYMBOLS + tuple(MIRRORS)
 EMBED_LAYOUT_NAMES = ("NFFT", "HOP", "NF", "CH", "QK", "VDIM", "FC", "NQKV", "DFT_LD", "EAOUT_SMEM", "LENS_PER_LAUNCH")
 
 ATTN_FORMS = {"query": 0, "tile": 1, "cluster": 2}
@@ -192,6 +200,16 @@ def lib():
             "kh_tail_clusters": [],
             "kh_tail": [TW, P, P, P, P, I64, I, I, I, I, P, P],
             "kh_tail_slots": [TW, P, P, P, P, I64, P, I, P, I, I, I, P],
+        })
+        RP = ctypes.POINTER(Records)
+        sigs.update({
+            "kh_target_lists": [P, P, P, P, I, I, I, I, P, P],
+            "kh_spk_gate": [FB, P, P, P, I64, RP, I, P],
+            "kh_gate_fanout": [P, P, P, I64, RP, P, I, I, I, I, P],
+            "kh_gather_h": [P, RP, I, I, I, P, P, P],
+            "kh_scatter_hc": [P, RP, I, I, I, P, P, P],
+            "kh_inter_gate_mask": [P, RP, I, P],
+            "kh_inter_h_last": [P, P, RP, I, P],
         })
         L.kh_mid_pack.restype = None
         L.kh_mid_pack.argtypes = [P] * 6
@@ -1382,3 +1400,190 @@ def tail_chain64(Ys, Xs, h, c, p, hist_k, hist_v, gates=None, nxt=None, **mutant
         tol = max(tol, float(r["K_b"].max()), float(r["V_b"].max()))
         h, c, hb, cb = r["h"], r["c"], r["h_b"], r["c_b"]
     return outs
+
+
+# ---- the several-target kernels (targets_kernels.cuh) and the slot-list helpers (sep_kernels.cuh) --------------------
+# target_lists_kernel builds, at the start of a call over a state's listeners, which record each target row uses, the
+# frames it advances, the listener that owns it, each listener's lead record and the clamped row offsets; spk_gate_kernel
+# and gate_fanout_kernel give every target row its speaker-gate memo and its gated copy of block 0's output.  The slot-list
+# helpers copy the listed records' carried inter-LSTM (h, c) to and from the workspace, and mask the frames a ragged row
+# does not advance.  Every reference here is exact (integer lists, copies, one fp32 multiply per element).
+INT_MAX = 2 ** 31 - 1
+TARGET_LISTS_MUTANTS = ("no_carry", "no_clamp", "owner_off_by_one", "lead_unvalidated")
+FANOUT_MUTANTS = ("owner_mod", "gate_unowned")
+
+
+def records_map(stride, slots, batch, hops=None, frames=1):
+    """a Records map over device int32 tensors slots [rows] and hops [rows] (or None)"""
+    return Records(stride, ptr(slots), batch, ptr(hops), frames)
+
+
+def _byref(s):
+    return None if s is None else ctypes.byref(s)
+
+
+def target_lists(records, offsets, groups, hops, n, K, rows, batch, lists):
+    return lib().kh_target_lists(ptr(records), ptr(offsets), ptr(groups), ptr(hops), n, K, rows, batch, ptr(lists), stream())
+
+
+def spk_gate(w, emb, spk_pre, state, sstride, recs, rows):
+    """recs None: the dense map (row r = record r, sstride floats apart)"""
+    return lib().kh_spk_gate(ctypes.byref(w), ptr(emb), ptr(spk_pre), ptr(state), sstride, _byref(recs), rows, stream())
+
+
+def gate_fanout(X0, X, state, sstride, recs, owner, n_targets, T, apply_gate, rows):
+    """recs and owner None: the dense map, row r of mixture r / n_targets"""
+    return lib().kh_gate_fanout(ptr(X0), ptr(X), ptr(state), sstride, _byref(recs), ptr(owner), n_targets, T, apply_gate, rows,
+                                stream())
+
+
+def gather_h(state, recs, b0, n_blocks, B, Hg, Cg):
+    return lib().kh_gather_h(ptr(state), ctypes.byref(recs), b0, n_blocks, B, ptr(Hg), ptr(Cg), stream())
+
+
+def scatter_hc(state, recs, b0, n_blocks, B, Hg, Cg):
+    return lib().kh_scatter_hc(ptr(state), ctypes.byref(recs), b0, n_blocks, B, ptr(Hg), ptr(Cg), stream())
+
+
+def inter_gate_mask(gx, recs, B):
+    return lib().kh_inter_gate_mask(ptr(gx), ctypes.byref(recs), B, stream())
+
+
+def inter_h_last(Y, Hg, recs, B):
+    return lib().kh_inter_h_last(ptr(Y), ptr(Hg), ctypes.byref(recs), B, stream())
+
+
+def row_frames(hops, b, T):
+    """the frames row b advances (sep_kernels.cuh row_frames): all T without hops, hops[b] if it lies in [0, T], else 0"""
+    if hops is None:
+        return T
+    h = int(hops[b])
+    return h if 0 <= h <= T else 0
+
+
+def target_lists_ref(records, offsets, groups, hops, n, K, rows, batch, mutant=None):
+    """target_lists_kernel of int lists: records + offsets (a rows call) or groups (K rows per group).  Returns rec, owner,
+    lead, rec_hops (None without hops) and start (None without offsets).  Mutants (TARGET_LISTS_MUTANTS): no_carry (the
+    running maximum restarts at every 1024-entry pass), no_clamp (offsets not clamped to [0, rows]),
+    owner_off_by_one (the owner search counts start < r instead of <= r), lead_unvalidated (a listener whose lead record is
+    invalid still stores through its other rows)."""
+    def listed(i, r, first):
+        if records is None:
+            g = groups[i]
+            return g * K + (r - first) if 0 <= g < batch // K else -1
+        s = records[r] if 0 <= r < rows else -1              # (only the no_clamp mutant reads outside the list)
+        return s if 0 <= s < batch else -1
+    start = None
+    if offsets is not None:
+        start, run = [], (-math.inf if mutant == "no_clamp" else 0)
+        for i in range(n + 1):
+            if mutant == "no_carry" and i % 1024 == 0:
+                run = 0
+            v = offsets[i] if mutant == "no_clamp" else min(max(offsets[i], 0), rows)
+            run = max(run, v)
+            start.append(run)
+    first = (lambda i: start[i]) if start is not None else (lambda i: i * K)
+    lead = [listed(i, first(i), first(i)) if first(i) < first(i + 1) else -1 for i in range(n)]
+    rec, owner = [], []
+    for r in range(rows):
+        if start is not None:                                 # the kernel's binary search over start[0 .. n]
+            lo, hi = 0, n + 1
+            while lo < hi:
+                mid = (lo + hi) >> 1
+                if (start[mid] < r) if mutant == "owner_off_by_one" else (start[mid] <= r):
+                    lo = mid + 1
+                else:
+                    hi = mid
+            i = lo - 1 if lo - 1 < n else -1
+        else:
+            i = r // K if r // K < n else -1
+        owner.append(i)
+        ok = i >= 0 and (mutant == "lead_unvalidated" or lead[i] >= 0)
+        rec.append(listed(i, r, first(i)) if ok else -1)
+    rec_hops = None if hops is None else [hops[i] if i >= 0 else 0 for i in owner]
+    return dict(rec=rec, owner=owner, lead=lead, rec_hops=rec_hops, start=start)
+
+
+def _partition(g, n, used):
+    """n + 1 non-decreasing offsets from 0 to `used`, with empty listeners"""
+    cuts = sorted(g.randrange(used + 1) for _ in range(n - 1))
+    off = [0] + cuts + [used]
+    for j in range(3, n, 7):                                  # every 7th listener from the 4th on empty
+        off[j + 1] = off[j]
+    return off
+
+
+def target_lists_cases(T=3):
+    """the target_lists_kernel problems the GPU test runs (and the CPU test shows every mutant differs on): name, the
+    lists, n, K, rows, batch, and `catches`, the mutants that must differ from the reference on the case"""
+    import random
+    bad_records = (-1, None, INT_MAX, -INT_MAX)              # None: batch
+    bad_hops = (-1, 0, T, T + 1, INT_MAX, -INT_MAX)
+    cases = []
+
+    def rows_case(name, n, rows, spare, seed, hops=True, edits=(), invalid_lead=False, catches=()):
+        g = random.Random(seed)
+        batch = rows + 7
+        recs = g.sample(range(batch), rows)
+        for j in range(5, rows, 37):                          # bad records: -1, batch, +-(2^31 - 1)
+            b = bad_records[(j // 37) % 4]
+            recs[j] = batch if b is None else b
+        off = _partition(g, n, rows - spare)
+        for kind, j in edits:
+            if kind == "neg":
+                off[j] = -5 - j
+            elif kind == "above":
+                off[j] = rows + 100
+            elif kind == "dec":                              # below its predecessor (and below the running maximum)
+                off[j] = max(off[j - 1] - 3, 0)
+        if invalid_lead:                                      # the first listener of >= 2 valid rows: its lead invalid
+            for i in range(n):
+                a, z = off[i], off[i + 1]
+                if 0 <= a and z - a >= 2 and z <= rows and off[i] == max(off[:i + 1]) and all(
+                        0 <= recs[r] < batch for r in range(a + 1, z)):
+                    recs[a] = -1
+                    break
+        hp = [g.choice(bad_hops) if g.random() < 0.3 else g.randrange(T + 1) for _ in range(n)] if hops else None
+        cases.append(dict(name=name, records=recs, offsets=off, groups=None, hops=hp, n=n, K=0, rows=rows, batch=batch,
+                          catches=set(catches) | {"owner_off_by_one"}))
+
+    rows_case("rows_n1", 1, 1, 0, 1)
+    rows_case("rows_n1_spare", 1, 8, 3, 2, invalid_lead=True, catches=("lead_unvalidated",))
+    rows_case("rows_n31", 31, 100, 6, 3, invalid_lead=True, catches=("lead_unvalidated",))
+    rows_case("rows_n31_bad", 31, 64, 0, 4, hops=False, edits=(("neg", 0), ("dec", 9), ("neg", 15), ("above", 29)),
+              catches=("no_clamp",))
+    rows_case("rows_n1023", 1023, 2048, 17, 5, edits=(("dec", 500), ("neg", 0)), invalid_lead=True,
+              catches=("no_clamp", "lead_unvalidated"))
+    rows_case("rows_n1024", 1024, 3000, 40, 6, hops=False, edits=(("dec", 1024),), catches=("no_carry",))
+    rows_case("rows_n1025", 1025, 2100, 0, 7, edits=(("dec", 1024), ("dec", 1025)), catches=("no_carry",))
+    rows_case("rows_n2500", 2500, 4096, 100, 8, edits=(("neg", 0), ("dec", 1024), ("dec", 2048), ("above", 2490)),
+              invalid_lead=True, catches=("no_carry", "no_clamp", "lead_unvalidated"))
+
+    def groups_case(name, n, K, n_groups, seed, hops=True):
+        g = random.Random(seed)
+        batch = n_groups * K                                  # the engine guarantees batch % K == 0
+        grp = [g.randrange(n_groups) for _ in range(n)]
+        for j in range(1, n, 5):                              # groups outside [0, batch / K)
+            grp[j] = (-1, n_groups, INT_MAX, -INT_MAX)[(j // 5) % 4]
+        hp = [g.choice(bad_hops) if g.random() < 0.3 else g.randrange(T + 1) for _ in range(n)] if hops else None
+        cases.append(dict(name=name, records=None, offsets=None, groups=grp, hops=hp, n=n, K=K, rows=n * K, batch=batch,
+                          catches=set()))
+
+    groups_case("groups_n1_K2", 1, 2, 2, 11)
+    groups_case("groups_n31_K3", 31, 3, 10, 12)
+    groups_case("groups_n1500_K2", 1500, 2, 1500, 13, hops=False)
+    return cases
+
+
+def gate_fanout_ref(X0, gates, owner, K, apply_gate, mutant=None):
+    """gate_fanout_kernel: X0 [mixtures][T][97][64] and gates [rows][97][64] (the gate of each target row's record) ->
+    X [rows][T][97][64], row r = X0[i] (times the gate if apply_gate and i >= 0) with i = owner[r] (owner None: r / K),
+    mixture 0 for i = -1; fp32 products, as the kernel's (exact).  Mutants (FANOUT_MUTANTS): owner_mod (owner r % K),
+    gate_unowned (a row without owner gated too)."""
+    rows = gates.shape[0]
+    out = torch.empty((rows,) + tuple(X0.shape[1:]), dtype=torch.float32)
+    for r in range(rows):
+        i = (r % K if mutant == "owner_mod" else r // K) if owner is None else int(owner[r])
+        v = X0[max(i, 0)].float()
+        out[r] = v * gates[r].float()[None] if apply_gate and (i >= 0 or mutant == "gate_unowned") else v
+    return out

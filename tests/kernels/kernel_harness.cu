@@ -2,9 +2,10 @@
 // tc_lstm.cuh), the separator's attention section (sep_kernels.cuh), its front and back (sep_kernels.cuh,
 // hop_kernels.cuh), its CUDA-core rows GEMM (gemm.cuh), its one-hop middle section (mid_kernel.cuh: mid_kernel, mid_a,
 // mid_b, mid_c), the fused one-hop tail of a block (hop_kernels.cuh: tail_kernel, both record maps), the tensor-core
-// chain's cell kernel (sep_kernels.cuh: lstm_cell_rows), and the enrollment network's
-// own kernels (embed_kernels.cuh: estd, efront, egn_apply, eqkv_ln, softmax_rows, eattn_out, ehead, einter_mask,
-// eput_lens), so that the kernel-level tests (tests/test_*_kernels_gpu.py) can drive each kernel directly with arbitrary
+// chain's cell kernel (sep_kernels.cuh: lstm_cell_rows), the enrollment network's own kernels (embed_kernels.cuh: estd,
+// efront, egn_apply, eqkv_ln, softmax_rows, eattn_out, ehead, einter_mask, eput_lens), the several-target kernels
+// (targets_kernels.cuh: target_lists, spk_gate, gate_fanout) and the slot-list helpers (sep_kernels.cuh: gather_h,
+// scatter_hc, inter_gate_mask, inter_h_last), so that the kernel-level tests (tests/test_*_kernels_gpu.py) can drive each kernel directly with arbitrary
 // shapes and compare it element by element with a float64 reference.
 //
 // The argument structs below are plain C (mirrored with ctypes in the tests); every function checks its arguments, fills
@@ -17,6 +18,7 @@
 #include "tc_lstm.cuh"
 #include "sep_launch.cuh"
 #include "embed_kernels.cuh"
+#include "targets_kernels.cuh"      // last, as in the engine
 
 #define KH_API extern "C" __attribute__((visibility("default")))
 
@@ -68,6 +70,7 @@ struct KhLstm {
     const void* wih_hi;
     const void* wih_lo;
     const float *bias, *ln_g, *ln_b;
+    const int32_t* steps;       // KH_LSTM_TC_X only (LstmXArgs::steps); must be null for the other variants
 };
 
 enum KhLstmVariant {
@@ -190,6 +193,7 @@ KH_API int kh_lstm(const KhLstm* k, int variant, int passes, char* why, int why_
     if (e != cudaSuccess) { put_why(why, why_len, "kernel attributes"); return (int)e; }
     const LstmArgs a = to_lstm(*k);
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (k->steps != nullptr && variant != KH_LSTM_TC_X) { put_why(why, why_len, "steps apply to tc_x only"); return (int)cudaErrorInvalidValue; }
     static const LstmRec forced[] = {LstmRec::rec3_pre, LstmRec::rec3_ring, LstmRec::rec4_2, LstmRec::rec4_4};   // KH_LSTM_REC*
     switch (variant) {
         case KH_LSTM_AUTO: e = launch_lstm_rec(a, st); break;
@@ -206,7 +210,7 @@ KH_API int kh_lstm(const KhLstm* k, int variant, int passes, char* why, int why_
             tcl::LstmXArgs xa{};
             xa.l = a; xa.x = k->x; xa.x_ld = k->x_ld;
             xa.wih_hi = static_cast<const __nv_bfloat16*>(k->wih_hi); xa.wih_lo = static_cast<const __nv_bfloat16*>(k->wih_lo);
-            xa.bias = k->bias; xa.ln_g = k->ln_g; xa.ln_b = k->ln_b;
+            xa.bias = k->bias; xa.ln_g = k->ln_g; xa.ln_b = k->ln_b; xa.steps = k->steps;
             e = launch_tc_lstm_x(xa, passes, st);
             break;
         }
@@ -664,4 +668,78 @@ KH_API int kh_einter_mask(float* gx, const int32_t* lens, int B, int steps, void
 KH_API int kh_eput_lens(int32_t* dst, const int32_t* lens_host, int n, void* stream) {
     if (n <= 0) return (int)cudaErrorInvalidValue;
     return (int)emb::launch_eput_lens(static_cast<cudaStream_t>(stream), dst, lens_host, n);
+}
+
+// ---- the several-target kernels (targets_kernels.cuh) and the slot-list helpers (sep_kernels.cuh) --------------------
+// Records field for field: row b is record slots[b] of a state of `batch` records of `stride` floats; hops (device, one
+// entry per row) may be null
+struct KhRecords {
+    int64_t stride;
+    const int32_t* slots;
+    int32_t batch;
+    const int32_t* hops;
+    int32_t frames;
+};
+
+static Records to_records(const KhRecords& k) { return Records{k.stride, k.slots, k.batch, k.hops, k.frames}; }
+static bool records_ok(const KhRecords* r) { return r && r->stride > 0 && r->slots != nullptr && r->batch > 0 && r->frames > 0; }
+
+KH_API int kh_sizeof_records() { return (int)sizeof(KhRecords); }
+
+// target_lists_kernel over n listeners and `rows` target rows (n <= rows): records + offsets (the rows call) or groups
+// (offsets and records null, K targets per group); lists = 5 rows + 1 int32, laid out as launch_target_lists states
+KH_API int kh_target_lists(const int32_t* records, const int32_t* offsets, const int32_t* groups, const int32_t* hops, int n, int K,
+                           int rows, int batch, int32_t* lists, void* stream) {
+    const bool by_rows = records != nullptr && offsets != nullptr && groups == nullptr;
+    const bool by_groups = records == nullptr && offsets == nullptr && groups != nullptr && K > 0;
+    if (!(by_rows || by_groups) || n <= 0 || rows < n || batch <= 0 || lists == nullptr) return (int)cudaErrorInvalidValue;
+    return (int)launch_target_lists(static_cast<cudaStream_t>(stream), records, offsets, groups, hops, n, K, rows, batch, lists);
+}
+
+// spk_gate_kernel over `rows` rows: recs == null -> the dense map (row r = record r, sstride floats apart), otherwise the
+// Records map (sstride unused).  emb [rows][256], spk_pre [rows][6208].
+KH_API int kh_spk_gate(const KhSepFrontBack* w, const float* emb, float* spk_pre, float* state, int64_t sstride, const KhRecords* recs,
+                       int rows, void* stream) {
+    if (rows <= 0 || (recs == nullptr && sstride <= 0) || (recs != nullptr && !records_ok(recs))) return (int)cudaErrorInvalidValue;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (recs == nullptr) return (int)launch_spk_gate(false, st, rows, emb, spk_pre, state, sstride, to_sep(*w));
+    return (int)launch_spk_gate(false, st, rows, emb, spk_pre, state, to_records(*recs), to_sep(*w));
+}
+
+// gate_fanout_kernel: X [rows][T][97][64] from X0 [mixtures][T][97][64]; the dense map (recs == null: owner must be null,
+// row r is mixture r / n_targets) or the Records map with an owner list
+KH_API int kh_gate_fanout(const float* X0, float* X, const float* state, int64_t sstride, const KhRecords* recs, const int32_t* owner,
+                          int n_targets, int T, int apply_gate, int rows, void* stream) {
+    const bool dense = recs == nullptr && owner == nullptr && sstride > 0 && n_targets > 0;
+    const bool listed = recs != nullptr && owner != nullptr && records_ok(recs);
+    if (!(dense || listed) || rows <= 0 || T <= 0) return (int)cudaErrorInvalidValue;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (dense) return (int)launch_gate_fanout(false, st, rows, X0, X, state, sstride, owner, n_targets, T, apply_gate);
+    return (int)launch_gate_fanout(false, st, rows, X0, X, state, to_records(*recs), owner, n_targets, T, apply_gate);
+}
+
+// gather_h_kernel over blocks b0 .. b0 + n_blocks - 1 of B rows' records into Hg (Cg: may be null), each
+// [b0 + n_blocks][B][97][64]
+KH_API int kh_gather_h(const float* state, const KhRecords* recs, int b0, int n_blocks, int B, float* Hg, float* Cg, void* stream) {
+    if (!records_ok(recs) || b0 < 0 || n_blocks <= 0 || B <= 0 || Hg == nullptr) return (int)cudaErrorInvalidValue;
+    return (int)launch_gather_h(static_cast<cudaStream_t>(stream), b0, state, to_records(*recs), n_blocks, B, Hg, Cg);
+}
+
+// scatter_hc_kernel: the inverse copy, into the records of the rows that store
+KH_API int kh_scatter_hc(float* state, const KhRecords* recs, int b0, int n_blocks, int B, const float* Hg, const float* Cg,
+                         void* stream) {
+    if (!records_ok(recs) || b0 < 0 || n_blocks <= 0 || B <= 0 || Hg == nullptr || Cg == nullptr) return (int)cudaErrorInvalidValue;
+    return (int)launch_scatter_hc(static_cast<cudaStream_t>(stream), b0, state, to_records(*recs), n_blocks, B, Hg, Cg);
+}
+
+// inter_gate_mask_kernel: gx [B][T][97][256], T = recs->frames
+KH_API int kh_inter_gate_mask(float* gx, const KhRecords* recs, int B, void* stream) {
+    if (!records_ok(recs) || B <= 0) return (int)cudaErrorInvalidValue;
+    return (int)launch_inter_gate_mask(static_cast<cudaStream_t>(stream), B, gx, to_records(*recs), recs->frames);
+}
+
+// inter_h_last_kernel: Y [B][T][97][64] -> Hg [B][97][64], T = recs->frames
+KH_API int kh_inter_h_last(const float* Y, float* Hg, const KhRecords* recs, int B, void* stream) {
+    if (!records_ok(recs) || B <= 0) return (int)cudaErrorInvalidValue;
+    return (int)launch_inter_h_last(static_cast<cudaStream_t>(stream), B, Y, Hg, to_records(*recs), recs->frames);
 }

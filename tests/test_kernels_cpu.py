@@ -1,6 +1,7 @@
 """The kernel harness library (tests/kernels/) and the float64 references the kernel-level GPU tests
 (test_umma_gemm_gpu.py, test_lstm_kernels_gpu.py, test_attention_kernels_gpu.py, test_front_back_kernels_gpu.py,
-test_embed_kernels_gpu.py, test_rows_gemm_kernels_gpu.py, test_mid_kernels_gpu.py, test_tail_kernel_gpu.py) rely on.  The enrollment references (estd64, efront64, egn64, eqkv_ln64, softmax64,
+test_embed_kernels_gpu.py, test_rows_gemm_kernels_gpu.py, test_mid_kernels_gpu.py, test_tail_kernel_gpu.py,
+test_targets_kernels_gpu.py) rely on.  The enrollment references (estd64, efront64, egn64, eqkv_ln64, softmax64,
 eattn_out64, ehead64) are pinned to oracle/restate.py; each of their mutants is shown to miss the reference by more than
 10x its bound, and einter_mask_expected's mutants to change it.  No device needed."""
 import ctypes
@@ -716,3 +717,58 @@ def test_tail_mutants_differ():
     for name, kw in list(kh.TAIL_MUTANTS.items()) + [("stale", dict(stale=stale))]:
         mr = kh.tail64(Y, X, h, c, p, hk, hv, gate, nxt, **kw)
         assert max(_ratio(mr[k], ref[k], ref[k + "_b"]) for k in keys) >= 10, name
+
+
+def test_target_lists_reference_is_the_plain_definition():
+    """On a valid list (monotone offsets inside [0, rows], every record in the state) target_lists_ref is the obvious
+    reading: listener i owns rows offsets[i] .. offsets[i+1]-1, each storing through its own record."""
+    import random
+    g = random.Random(3)
+    n, rows, batch = 40, 150, 200
+    off = sorted(g.randrange(rows - 10) for _ in range(n - 1))
+    off = [0] + off + [rows - 10]
+    recs = g.sample(range(batch), rows)
+    hops = [g.randrange(4) for _ in range(n)]
+    ref = kh.target_lists_ref(recs, off, None, hops, n, 0, rows, batch)
+    owner = [next((i for i in range(n) if off[i] <= r < off[i + 1]), -1) for r in range(rows)]
+    assert ref["owner"] == owner and ref["start"] == off
+    assert ref["rec"] == [recs[r] if owner[r] >= 0 else -1 for r in range(rows)]
+    assert ref["rec_hops"] == [hops[i] if i >= 0 else 0 for i in owner]
+    assert ref["lead"] == [recs[off[i]] if off[i] < off[i + 1] else -1 for i in range(n)]
+    grp = kh.target_lists_ref(None, None, [2, -1, 0], None, 3, 4, 12, 12)
+    assert grp["rec"] == [8, 9, 10, 11, -1, -1, -1, -1, 0, 1, 2, 3] and grp["lead"] == [8, -1, 0] and grp["start"] is None
+
+
+def test_target_lists_mutants_differ():
+    """Every mutant of target_lists_ref differs from the reference on each case of the GPU test
+    (test_targets_kernels_gpu.py) that names it, and every mutant is named by some case."""
+    named = set()
+    for c in kh.target_lists_cases():
+        args = (c["records"], c["offsets"], c["groups"], c["hops"], c["n"], c["K"], c["rows"], c["batch"])
+        ref = kh.target_lists_ref(*args)
+        for m in c["catches"]:
+            assert kh.target_lists_ref(*args, mutant=m) != ref, (c["name"], m)
+        named |= c["catches"]
+        assert c["rows"] >= c["n"]
+    assert named == set(kh.TARGET_LISTS_MUTANTS)
+
+
+def test_gate_fanout_reference_and_mutants():
+    """gate_fanout_ref copies X0 of the owner (mixture 0 for no owner) times the row's gate; the owner r % K mutant differs
+    on a dense fan-out of 3 x 3 rows, the gated unowned row on a listed one with apply_gate"""
+    g = torch.Generator().manual_seed(5)
+    X0 = torch.randn(3, 2, kh.NF, kh.CH, generator=g)
+    gates = 1 + 0.5 * torch.randn(9, kh.NF, kh.CH, generator=g)
+    out = kh.gate_fanout_ref(X0, gates, None, 3, 1)
+    assert torch.equal(out[4], X0[1] * gates[4][None])
+    assert not torch.equal(kh.gate_fanout_ref(X0, gates, None, 3, 0, mutant="owner_mod"), kh.gate_fanout_ref(X0, gates, None, 3, 0))
+    owner = [0, -1, 2, 1, -1, 0, 2, 1, 0]
+    lst = kh.gate_fanout_ref(X0, gates, owner, 3, 1)
+    assert torch.equal(lst[1], X0[0]) and torch.equal(lst[2], X0[2] * gates[2][None])
+    assert not torch.equal(kh.gate_fanout_ref(X0, gates, owner, 3, 1, mutant="gate_unowned"), lst)
+    assert torch.equal(kh.gate_fanout_ref(X0, gates, owner, 3, 0), torch.stack([X0[max(i, 0)] for i in owner]))
+
+
+def test_row_frames_is_the_kernels_rule():
+    assert [kh.row_frames([-1, 0, 1, 3, 4, kh.INT_MAX, -kh.INT_MAX], b, 3) for b in range(7)] == [0, 0, 1, 3, 0, 0, 0]
+    assert kh.row_frames(None, 0, 5) == 5
