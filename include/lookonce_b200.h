@@ -456,6 +456,47 @@ int l2h_render_binaural(const float* src_dev, const float* rir_dev, const float*
 int l2h_resample(const float* x_dev, int64_t x_row_stride, int32_t n_in, int32_t n_rows, const int32_t* orig_freq,
                  int32_t new_freq, float* y_dev, int64_t y_row_stride, int32_t y_capacity, void* stream);
 
+/* Streaming resampling for a list of a state's slots: devices at 48, 32, 24 or 8 kHz into and out of the 16 kHz
+ * separator, one push of `block` input samples per 8 ms tick.  With the rates reduced by their gcd to o and q and
+ * w = ceil(6 o / (0.99 min(o, q))) taps per side (as in l2h_resample), `block` must be a positive multiple of o, and each
+ * push yields out_block = block * q / o samples.  A stream's output is z, the l2h_resample output of everything it has
+ * been pushed as one signal, delayed by delay = D = floor(w q / o) samples, with zeros before z's start: after k pushes
+ * it has returned k * out_block samples, and every one of them is bit for bit the matching sample of z (the ones of z
+ * whose taps have all arrived).  Equal rates, and rates whose 8 ms is not a whole number of samples (44.1 kHz family),
+ * are refused.
+ *
+ * The state is [n_slots][channels][hist + keep] fp32 of DEVICE memory: per channel the trailing input samples the next
+ * push reads, then the last `keep` outputs.  All zeros is a fresh stream (zero samples before its start), so a slot is
+ * reset by zeroing its rows and moved by copying them.
+ *
+ * l2h_resample_stream_layout: hist (H), delay (D) and out_block of a stream.  Errors: 1 = null pointer, a rate <= 0, equal
+ * rates, a block that is not a positive multiple of o, keep < 0; 2 = the staged window of one push (hist + block + keep +
+ * out_block samples) exceeds the kernel's shared memory.
+ *
+ * l2h_resample_stream: row i of a call pushes h = hops_dev[i] blocks (`blocks` = T, the call's maximum, when hops_dev is
+ * NULL) into slot slots_dev[i] of the state:
+ *   x_dev      [n][channels][blocks * block] fp32, strides in floats; row i reads only its first h * block samples
+ *   y_dev      [n][channels][keep + blocks * out_block] fp32; row i receives y[i][c][0 .. keep + h * out_block): the last
+ *              keep + h * out_block samples of its stream's delayed output (the keep window, then the h new pushes' samples;
+ *              what precedes the stream's start reads as 0).  Its later samples are not written.  Must not overlap x or
+ *              the state.
+ *   slots_dev  [n] int32 of DEVICE memory read when the kernel runs, like l2h_sep_forward_slots_hops's list: an entry
+ *              outside [0, n_slots) marks a row that stores nothing (neither its y row nor any state row).  A slot listed
+ *              twice is a caller error the call does not detect.
+ *   hops_dev   [n] int32 of DEVICE memory read when the kernel runs, or NULL (every row pushes `blocks`).  h = 0, or an entry
+ *              outside [0, blocks], stores nothing.
+ * So a service passes the same slot and hop tensors to the resampler and the separator, and a call captured in a CUDA graph
+ * serves any list of the same n rewritten in place.  One launch; nothing on the host is read from the device.
+ * Errors, returned before anything is enqueued: 1 = null pointers, n, channels, blocks or n_slots <= 0, n > n_slots,
+ * channel or row strides under the lengths above, and the layout's errors 1; 2 = the staged window of one row (hist +
+ * blocks * block + keep + blocks * out_block samples) exceeds the kernel's shared memory.  Asynchronous on `stream`. */
+int l2h_resample_stream_layout(int32_t orig_freq, int32_t new_freq, int32_t block, int32_t keep, int32_t* hist,
+                               int32_t* delay, int32_t* out_block);
+int l2h_resample_stream(const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, float* y_dev, int64_t y_row_stride,
+                        int64_t y_ch_stride, int32_t n, int32_t channels, int32_t blocks, const int32_t* slots_dev,
+                        const int32_t* hops_dev, float* state_dev, int32_t n_slots, int32_t orig_freq, int32_t new_freq,
+                        int32_t block, int32_t keep, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -5,12 +5,13 @@ net), behind the reference's own Python call signatures.
     from lookoncetohear_b200 import Net            # drop-in for src.models.tfgridnet_realtime.net.Net
     from lookoncetohear_b200 import EmbedTFGridNet # drop-in for src.models.tfgridnet_orig.tfgridnet.EmbedTFGridNet
     from lookoncetohear_b200 import resample       # for torchaudio.functional.resample(x, orig, new) at its defaults
+    from lookoncetohear_b200 import StreamResampler  # the same, pushed a block per tick into a state of slots
 
 Compute happens only in lib/liblookonce_b200.so (hand-written sm_90a CUDA, C ABI declared in
 include/lookonce_b200.h); importing this package never falls back to PyTorch math.
 """
 from .embed import EmbedTFGridNet  # noqa: F401
 from .net import Net, SepState  # noqa: F401
-from .render import resample  # noqa: F401
+from .render import StreamResampler, resample  # noqa: F401
 
-__all__ = ["Net", "SepState", "EmbedTFGridNet", "resample"]
+__all__ = ["Net", "SepState", "EmbedTFGridNet", "resample", "StreamResampler"]

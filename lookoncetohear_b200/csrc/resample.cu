@@ -50,6 +50,38 @@ struct RsLaunch {
     RsRate rate[RS_MAX_RATES];
 };
 
+// One output sample: the 2w + 1 taps xp[0 .. 2w] (input samples c - w .. c + w, c = floor(m o / q)) weighted for the
+// phase r = (m o) mod q.  Tap t = 0 always has u >= w du >= 6, so xp[0] never enters the sum.  Both kernels call this,
+// so a streamed sample is the whole-signal sample bit for bit.
+__device__ __forceinline__ float rs_output(const float* xp, int64_t r, const RsRate& g) {
+    const double u0 = (double)r * g.du_r + g.w * g.du;                // u of tap n = c - w
+    float acc = 0.f;
+    for (int t = 0; t <= 2 * g.w; ++t) {
+        const float u = (float)fma(-(double)t, g.du, u0);
+        if (fabsf(u) < (float)RS_WIDTH) {
+            const float sinc = u == 0.f ? 1.f : sinpif(u) / (3.14159265358979f * u);
+            const float win = 0.5f + 0.5f * cospif(u * (1.f / RS_WIDTH));     // cos^2(pi u / 12)
+            acc = fmaf(g.scale * sinc * win, xp[t], acc);
+        }
+    }
+    return acc;
+}
+
+// the filter of orig -> new_freq Hz for rows of n_in samples (n_out 0 when n_in is not known)
+static RsRate rs_rate(int32_t orig, int32_t new_freq, int32_t n_in) {
+    RsRate g;
+    const int32_t gd = std::gcd(orig, new_freq);
+    g.o = orig / gd;
+    g.q = new_freq / gd;
+    const double base = std::min(g.o, g.q) * RS_ROLLOFF;
+    g.w = (int32_t)std::ceil(RS_WIDTH * (double)g.o / base);
+    g.n_out = (int32_t)(((int64_t)new_freq * n_in + orig - 1) / orig);
+    g.scale = (float)(base / g.o);
+    g.du = base / g.o;
+    g.du_r = base / ((double)g.o * g.q);
+    return g;
+}
+
 __global__ void __launch_bounds__(RS_TILE)
 resample_kernel(const float* __restrict__ x, int64_t x_stride, int n_in, float* __restrict__ y, int64_t y_stride, int cap,
                 const __grid_constant__ RsLaunch L) {
@@ -83,18 +115,89 @@ resample_kernel(const float* __restrict__ x, int64_t x_stride, int n_in, float* 
     float acc = 0.f;
     if (m < g.n_out) {
         const int64_t mo = (int64_t)m * g.o, c = mo / g.q;
-        const double u0 = (double)(mo - c * g.q) * g.du_r + g.w * g.du;    // u of tap n = c - w
-        const float* xp = xs + (c - g.w - lo);
-        for (int t = 0; t <= 2 * g.w; ++t) {
-            const float u = (float)fma(-(double)t, g.du, u0);
-            if (fabsf(u) < (float)RS_WIDTH) {
-                const float sinc = u == 0.f ? 1.f : sinpif(u) / (3.14159265358979f * u);
-                const float win = 0.5f + 0.5f * cospif(u * (1.f / RS_WIDTH));     // cos^2(pi u / 12)
-                acc = fmaf(g.scale * sinc * win, xp[t], acc);
-            }
-        }
+        acc = rs_output(xs + (c - g.w - lo), mo - c * g.q, g);
     }
     yr[m] = acc;
+}
+
+// ---- streaming: per-slot state, pushes of `block` input samples ------------------------------------------------------
+// A stream's output is the whole-signal output z of everything it was pushed, delayed by D = floor(w q / o) samples
+// (z'[j] = z[j - D], zero before z's start): after k pushes exactly the k * out_block - D samples of z whose taps have all
+// arrived are final.  A slot's state row per channel is [H + keep] floats: the last H = ceil(D o / q) + w input samples,
+// which the next push's outputs read, then the last `keep` outputs.  The oldest history word sits under tap 0 of the
+// push's first output only, which always weighs zero (rs_output), so it holds the number of outputs the stream has made,
+// capped at D, instead: a zeroed row is a fresh stream and knows which of its first outputs precede z's start.
+struct RsStream {
+    RsRate g;
+    int32_t block, out_block;  // input samples per push (a multiple of o) and the outputs each push yields
+    int32_t delay, hist, keep; // D, H and the output samples repeated from the previous call
+};
+
+// One CTA = one (call row, channel): stage the slot's history and the row's h pushes, compute the h * out_block outputs
+// with their absolute phase ((j - D) o mod q: pushes are whole periods), write keep + outputs, then store the new history
+// and keep tail.  A slot is listed once per call, so no other CTA touches its rows.
+__global__ void __launch_bounds__(RS_TILE)
+resample_stream_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, float* __restrict__ y, int64_t y_row,
+                       int64_t y_ch, int C, int T, const int32_t* __restrict__ slots, const int32_t* __restrict__ hops,
+                       float* __restrict__ state, int n_slots, const __grid_constant__ RsStream s) {
+    extern __shared__ float sm[];
+    const int row = blockIdx.x / C, ch = blockIdx.x - row * C, tid = threadIdx.x;
+    const int slot = slots[row], h = hops ? hops[row] : T;
+    if (slot < 0 || slot >= n_slots || h <= 0 || h > T) return;          // a row that stores nothing
+    const RsRate& g = s.g;
+    const int H = s.hist, keep = s.keep, D = s.delay, n_win = H + h * s.block, n_new = h * s.out_block;
+    float* st = state + ((int64_t)slot * C + ch) * (H + keep);
+    const float* xr = x + (int64_t)row * x_row + (int64_t)ch * x_ch;
+    float* yr = y + (int64_t)row * y_row + (int64_t)ch * y_ch;
+    float* win = sm;                                 // [H + h * block]: the history, then the row's new samples
+    float* out = sm + H + T * s.block;               // [keep + h * out_block]: the keep tail, then the new outputs
+    const float made = st[0];
+    const int before = made >= (float)D ? D : (made > 0.f ? (int)made : 0);
+    for (int i = tid; i < n_win; i += blockDim.x) win[i] = i == 0 ? 0.f : (i < H ? st[i] : xr[i - H]);
+    for (int i = tid; i < keep; i += blockDim.x) out[i] = st[H + i];
+    __syncthreads();
+    for (int j = tid; j < n_new; j += blockDim.x) {
+        float v = 0.f;                                                   // before z's start
+        if (before + j >= D) {
+            const int64_t a = (int64_t)(j - D) * g.o;
+            const int64_t c = a >= 0 ? a / g.q : -((-a + g.q - 1) / g.q);  // floor(a / q): tap c + H of win is x[m o / q]
+            v = rs_output(win + (H + c - g.w), a - c * g.q, g);
+        }
+        out[keep + j] = v;
+    }
+    __syncthreads();
+    for (int i = tid; i < keep + n_new; i += blockDim.x) yr[i] = out[i];
+    for (int i = tid; i < H + keep; i += blockDim.x)
+        st[i] = i == 0 ? (float)min(D, before + n_new) : (i < H ? win[n_win - H + i] : out[n_new + i - H]);
+}
+
+// the stream of orig -> new_freq Hz in pushes of `block` samples with `keep` repeated outputs, for calls of up to `blocks`
+// pushes per row: 0, or an error code (1 invalid, 2 the window of a row exceeds shared memory) with its message
+static int rs_stream(const char* who, int32_t orig, int32_t new_freq, int32_t block, int32_t keep, int32_t blocks,
+                     RsStream* s) {
+    const std::string rates = std::to_string(orig) + " -> " + std::to_string(new_freq) + " Hz";
+    if (orig <= 0 || new_freq <= 0) return fail(1, std::string(who) + ": rates must be positive, got " + rates);
+    if (orig == new_freq) return fail(1, std::string(who) + ": " + rates + " needs no resampling");
+    s->g = rs_rate(orig, new_freq, 0);
+    const RsRate& g = s->g;
+    if (block <= 0 || block % g.o != 0)
+        return fail(1, std::string(who) + ": block " + std::to_string(block) + " is not a positive multiple of " +
+                           std::to_string(g.o) + ", the input samples of one period of " + rates);
+    if (keep < 0) return fail(1, std::string(who) + ": keep " + std::to_string(keep) + " is negative");
+    const int64_t out_block = (int64_t)block / g.o * g.q, delay = (int64_t)g.w * g.q / g.o;
+    const int64_t hist = (delay * g.o + g.q - 1) / g.q + g.w;
+    const int64_t floats = hist + (int64_t)blocks * block + keep + (int64_t)blocks * out_block;
+    if (floats * (int64_t)sizeof(float) > RS_SMEM_BYTES)
+        return fail(2, std::string(who) + ": " + rates + " in blocks of " + std::to_string(block) + " with keep " +
+                           std::to_string(keep) + " and " + std::to_string(blocks) + " blocks per row is too large: " +
+                           std::to_string(floats) + " staged samples per row exceed shared memory (" +
+                           std::to_string(RS_SMEM_BYTES / sizeof(float)) + ")");
+    s->block = block;
+    s->out_block = (int32_t)out_block;
+    s->delay = (int32_t)delay;
+    s->hist = (int32_t)hist;
+    s->keep = keep;
+    return 0;
 }
 }  // namespace l2h
 
@@ -149,20 +252,49 @@ extern "C" int l2h_resample(const float* x_dev, int64_t x_row_stride, int32_t n_
         }
         L.run[L.n_run++] = (uint32_t)(r - row0) << 8 | (uint32_t)idx;
         if (idx < n_rates) continue;
-        const int32_t gd = std::gcd(orig, new_freq);
-        RsRate& g = L.rate[n_rates];
+        const RsRate& g = L.rate[n_rates] = rs_rate(orig, new_freq, n_in);
         rate_hz[n_rates++] = orig;
-        g.o = orig / gd;
-        g.q = new_freq / gd;
-        const double base = std::min(g.o, g.q) * RS_ROLLOFF;
-        g.w = (int32_t)std::ceil(RS_WIDTH * (double)g.o / base);
-        g.n_out = (int32_t)(((int64_t)new_freq * n_in + orig - 1) / orig);
-        g.scale = (float)(base / g.o);
-        g.du = base / g.o;
-        g.du_r = base / ((double)g.o * g.q);
         if (g.o != g.q) smem = std::max(smem, (int)((((int64_t)(threads - 1) * g.o) / g.q + 2 * g.w + 2) * sizeof(float)));
     }
     if (e == cudaSuccess) e = launch(n_rows);
     if (e != cudaSuccess) return fail(3, std::string("l2h_resample: ") + cudaGetErrorString(e));
+    return 0;
+}
+
+extern "C" int l2h_resample_stream_layout(int32_t orig_freq, int32_t new_freq, int32_t block, int32_t keep, int32_t* hist,
+                                          int32_t* delay, int32_t* out_block) {
+    using namespace l2h;
+    if (!hist || !delay || !out_block) return fail(1, "l2h_resample_stream_layout: null pointer");
+    RsStream s;
+    if (int rc = rs_stream("l2h_resample_stream_layout", orig_freq, new_freq, block, keep, 1, &s)) return rc;
+    *hist = s.hist;
+    *delay = s.delay;
+    *out_block = s.out_block;
+    return 0;
+}
+
+extern "C" int l2h_resample_stream(const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, float* y_dev,
+                                   int64_t y_row_stride, int64_t y_ch_stride, int32_t n, int32_t channels, int32_t blocks,
+                                   const int32_t* slots_dev, const int32_t* hops_dev, float* state_dev, int32_t n_slots,
+                                   int32_t orig_freq, int32_t new_freq, int32_t block, int32_t keep, void* stream) {
+    using namespace l2h;
+    if (!x_dev || !y_dev || !slots_dev || !state_dev) return fail(1, "l2h_resample_stream: null pointer");
+    if (n <= 0 || channels <= 0 || blocks <= 0 || n_slots <= 0)
+        return fail(1, "l2h_resample_stream: n, channels, blocks and n_slots must be positive");
+    if (n > n_slots) return fail(1, "l2h_resample_stream: a call needs n <= n_slots");
+    if ((int64_t)n * channels > INT32_MAX) return fail(1, "l2h_resample_stream: n * channels is too large");
+    RsStream s;
+    if (int rc = rs_stream("l2h_resample_stream", orig_freq, new_freq, block, keep, blocks, &s)) return rc;
+    const int64_t x_len = (int64_t)blocks * block, y_len = keep + (int64_t)blocks * s.out_block;
+    if (x_ch_stride < x_len || x_row_stride / channels < x_ch_stride || y_ch_stride < y_len ||
+        y_row_stride / channels < y_ch_stride)
+        return fail(1, "l2h_resample_stream: bad stride: rows and channels of x (" + std::to_string(x_len) + " samples) and y (" +
+                           std::to_string(y_len) + ") must not overlap");
+    const int smem = (int)((s.hist + x_len + y_len) * sizeof(float));
+    resample_stream_kernel<<<(unsigned)(n * channels), RS_TILE, smem, static_cast<cudaStream_t>(stream)>>>(
+        x_dev, x_row_stride, x_ch_stride, y_dev, y_row_stride, y_ch_stride, channels, blocks, slots_dev, hops_dev, state_dev,
+        n_slots, s);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(3, std::string("l2h_resample_stream: ") + cudaGetErrorString(e));
     return 0;
 }

@@ -262,6 +262,41 @@ class SepState(dict):
         return self.copy_streams_from(staged, list(range(len(ss))), list(ds))
 
 
+# the wording of device_list's errors per list: what its entries are, a wrong count, an entry outside [0, end)
+_LIST_WORDS = {"slot": ("integer slot indices", "slots lists {} records for {} input rows",
+                        "a slot lies outside [0, {end})"),
+               "hop": ("integer hop counts", "hops gives {} counts for {} input rows",
+                       "a hop count lies outside [0, {last}] (the call's {last} hops)"),
+               "record": ("integer record indices", "records lists {} records for {} target rows",
+                          "a record lies outside [0, {end})"),
+               "offset": ("integer row offsets", "offsets gives {} entries for {} = input rows + 1",
+                          "an offset lies outside [0, {last}] (the call's {last} target rows)")}
+
+
+def device_list(values, dev, n, end, distinct, noun):
+    """`values` (slots, groups, records, offsets or hop counts of a call of n rows) as the [n] int32 device tensor the engine
+    reads (the separator's calls and StreamResampler).  A CUDA int32 tensor is used as it is (its entries are read when the
+    kernels run); anything else is checked here (n ints in [0, end), each listed once if `distinct`) and uploaded.  noun: a
+    key of _LIST_WORDS, for the messages."""
+    entries, count, outside = _LIST_WORDS[noun]
+    if isinstance(values, torch.Tensor) and values.is_cuda:
+        if values.dtype != torch.int32 or tuple(values.shape) != (n,) or not values.is_contiguous():
+            raise ValueError(f"a CUDA {noun} list must be a contiguous int32 tensor of shape ({n},)")
+        if values.device != dev:
+            raise ValueError(f"{noun}s must live on the input's device {dev}, not {values.device}")
+        return values
+    v = torch.as_tensor(values)
+    if v.dtype.is_floating_point or v.dtype.is_complex or v.dtype == torch.bool or v.dim() != 1:
+        raise ValueError(f"{noun}s must be a sequence or 1-d tensor of {entries}")
+    if v.numel() != n:
+        raise ValueError(count.format(v.numel(), n))
+    if n > 0 and (int(v.min()) < 0 or int(v.max()) >= end):
+        raise ValueError(outside.format(end=end, last=end - 1))
+    if distinct and len(set(v.tolist())) != n:
+        raise ValueError(f"a {noun} is listed twice")
+    return v.to(torch.int32).to(dev)
+
+
 class Net(nn.Module):
     """CUDA (H100) replacement of the reference ``Net`` (net.py:20-76)."""
 
@@ -487,48 +522,15 @@ class Net(nn.Module):
             raise ValueError(f"active must have shape ({batch},), got {tuple(active.shape)}")
         return active.contiguous().view(torch.uint8)
 
-    # the wording of _device_list's errors per list: what its entries are, a wrong count, an entry outside [0, end)
-    _LIST_WORDS = {"slot": ("integer slot indices", "slots lists {} records for {} input rows",
-                            "a slot lies outside [0, {end})"),
-                   "hop": ("integer hop counts", "hops gives {} counts for {} input rows",
-                           "a hop count lies outside [0, {last}] (the call's {last} hops)"),
-                   "record": ("integer record indices", "records lists {} records for {} target rows",
-                              "a record lies outside [0, {end})"),
-                   "offset": ("integer row offsets", "offsets gives {} entries for {} = input rows + 1",
-                              "an offset lies outside [0, {last}] (the call's {last} target rows)")}
-
-    @classmethod
-    def _device_list(cls, values, dev, n, end, distinct, noun):
-        """`values` (slots, groups, records, offsets or hop counts of a call of n rows) as the [n] int32 device tensor the engine reads.  A
-        CUDA int32 tensor is used as it is (its entries are read when the kernels run); anything else is checked here (n
-        ints in [0, end), each listed once if `distinct`) and uploaded.  noun: a key of _LIST_WORDS, for the messages."""
-        entries, count, outside = cls._LIST_WORDS[noun]
-        if isinstance(values, torch.Tensor) and values.is_cuda:
-            if values.dtype != torch.int32 or tuple(values.shape) != (n,) or not values.is_contiguous():
-                raise ValueError(f"a CUDA {noun} list must be a contiguous int32 tensor of shape ({n},)")
-            if values.device != dev:
-                raise ValueError(f"{noun}s must live on the input's device {dev}, not {values.device}")
-            return values
-        v = torch.as_tensor(values)
-        if v.dtype.is_floating_point or v.dtype.is_complex or v.dtype == torch.bool or v.dim() != 1:
-            raise ValueError(f"{noun}s must be a sequence or 1-d tensor of {entries}")
-        if v.numel() != n:
-            raise ValueError(count.format(v.numel(), n))
-        if n > 0 and (int(v.min()) < 0 or int(v.max()) >= end):
-            raise ValueError(outside.format(end=end, last=end - 1))
-        if distinct and len(set(v.tolist())) != n:
-            raise ValueError(f"a {noun} is listed twice")
-        return v.to(torch.int32).to(dev)
-
     @classmethod
     def _slot_list(cls, slots, dev, n, batch):
         """slots (or groups) of a call of n rows: n distinct ints in [0, batch), or a CUDA int32 list used in place"""
-        return cls._device_list(slots, dev, n, batch, True, "slot")
+        return device_list(slots, dev, n, batch, True, "slot")
 
     @classmethod
     def _hop_counts(cls, hops, dev, n, frames):
         """hop counts of a call of n rows and `frames` hops: n ints in [0, frames], or a CUDA int32 list used in place"""
-        return cls._device_list(hops, dev, n, frames + 1, False, "hop")
+        return device_list(hops, dev, n, frames + 1, False, "hop")
 
     def _frames(self, n, pad=False, who="pad=False", per=""):
         """(frames, output samples) of a call on n input samples: pad=True rounds up to whole hops and returns n samples;
@@ -726,9 +728,9 @@ class Net(nn.Module):
         dev = x.device
         if hops is not None:
             hops = self._hop_counts(hops, dev, n, frames)
-        records = self._device_list(records, dev, R, state.batch, True, "record")
+        records = device_list(records, dev, R, state.batch, True, "record")
         on_host = not (isinstance(offsets, torch.Tensor) and offsets.is_cuda)
-        offsets_dev = self._device_list(offsets, dev, n + 1, R + 1, False, "offset")
+        offsets_dev = device_list(offsets, dev, n + 1, R + 1, False, "offset")
         if on_host:
             o = torch.as_tensor(offsets).tolist()
             if o[0] != 0 or any(b < a for a, b in zip(o, o[1:])):

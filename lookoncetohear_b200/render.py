@@ -3,7 +3,8 @@ reference's simulators and dataset do on the CPU (src/datasets/multi_ch_simulato
 src/datasets/MixLibriSpeechNoisyEnrollNorm.py:179-202 noise scaling / peak normalisation / mixture), and the band-limited
 resampler of the responses and the dataset's audio (`torchaudio.functional.resample` at its defaults,
 multi_ch_simulator.py:49, MixLibriSpeechNoisyEnrollNorm.py:69-75).  The arithmetic is `l2h_render_binaural` and
-`l2h_resample` (hand-written CUDA); no CPU fallback."""
+`l2h_resample` (hand-written CUDA); and its streaming form for listeners whose devices run at another rate than the
+separator's 16 kHz (`StreamResampler`, `l2h_resample_stream`).  No CPU fallback."""
 import ctypes
 import math
 import numbers
@@ -11,6 +12,7 @@ import numbers
 import torch
 
 from . import _cabi
+from .net import device_list
 
 
 def _rates(freq, shape, what):
@@ -66,6 +68,99 @@ def resample(x, orig_freq, new_freq, lowpass_filter_width=6, rolloff=0.99, resam
         _cabi.check(_cabi.lib().l2h_resample(xr.data_ptr(), n, n, rows, rates, new, y.data_ptr(), n_out, n_out,
                                              torch.cuda.current_stream(dev).cuda_stream))
     return y.view(*lead, n_out).to(x.dtype)
+
+
+def _whole(v, what, low=1):
+    """v as an int >= low, or ValueError"""
+    if isinstance(v, bool) or not isinstance(v, numbers.Integral) or int(v) < low or int(v) >= 2 ** 31:
+        raise ValueError(f"{what} must be an integer >= {low} (below 2**31), got {v!r}")
+    return int(v)
+
+
+class StreamResampler:
+    """`resample` for streams pushed a block at a time, one state row per (slot, channel): devices at 48, 32, 24 or 8 kHz
+    into and out of the 16 kHz separator, every tick one call over the same slot list and hop counts as
+    `Net.advance_slots` (l2h_resample_stream).
+
+    Each push of `block` input samples (a multiple of o, the input samples of one period of the reduced rates) yields
+    `out_block` = block * new / orig output samples.  The stream's output is `resample` of everything it has been pushed,
+    delayed by `delay` samples (zeros before its start), bit for bit; the delay is what the window's taps on the far side
+    need (6 samples at 48 -> 16 kHz, 21 at 16 -> 48 kHz).  Each output row first repeats the last `keep` samples of the
+    stream's previous output: with keep=64, a push of 384 samples at 48 kHz returns the 192 samples of a one-hop
+    `predict(..., pad=False)` chunk.  Equal rates and the 44.1 kHz family (whose 8 ms is no whole number of samples) are
+    refused.
+
+    `state` [slots, channels, hist + keep] is a plain float32 tensor on `device`: all zeros is a fresh stream, so a listener
+    is reset by zeroing its rows (`reset`) and moved by copying them."""
+
+    def __init__(self, orig_freq, new_freq, slots, channels, block, keep=0, device=None):
+        orig, new = _whole(orig_freq, "orig_freq"), _whole(new_freq, "new_freq")
+        self.n_slots, self.channels = _whole(slots, "slots"), _whole(channels, "channels")
+        self.block, self.keep = _whole(block, "block"), _whole(keep, "keep", 0)
+        hist, delay, out_block = ctypes.c_int32(), ctypes.c_int32(), ctypes.c_int32()
+        self._check(_cabi.lib().l2h_resample_stream_layout(orig, new, self.block, self.keep, ctypes.byref(hist),
+                                                           ctypes.byref(delay), ctypes.byref(out_block)))
+        self.orig_freq, self.new_freq = orig, new
+        self.hist, self.delay, self.out_block = hist.value, delay.value, out_block.value
+        dev = torch.device("cuda") if device is None else torch.device(device)
+        if dev.type != "cuda":
+            raise RuntimeError("lookoncetohear_b200.StreamResampler needs a CUDA device (no CPU fallback)")
+        if dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+        self.state = torch.zeros(self.n_slots, self.channels, self.hist + self.keep, dtype=torch.float32, device=dev)
+
+    @staticmethod
+    def _check(rc):
+        if rc == 2:                     # a window too large for the kernel: still the caller's sizes
+            raise ValueError(_cabi.lib().l2h_last_error().decode())
+        _cabi.check_args(rc)
+
+    def __call__(self, x, slots, hops=None, out=None):
+        """x [n, channels, block * T] CUDA tensor: row i pushes hops[i] blocks (T without `hops`) into slot slots[i].
+        Returns y [n, channels, keep + T * out_block] float32 (`out`, if given): row i receives y[i, :, :keep + h_i *
+        out_block], the last keep + h_i * out_block samples of its stream's delayed output; its later samples are left
+        unwritten.  A row with h_i = 0, or whose CUDA slot entry lies outside [0, slots), stores nothing: neither its y row
+        nor its state rows change.
+
+        `slots` and `hops` follow Net.advance_slots: n distinct ints in [0, slots) and n ints in [0, T] (sequences or CPU
+        tensors, checked and uploaded), or contiguous CUDA int32 tensors of shape (n,) used in place and read when the
+        kernel runs, so a call captured in a CUDA graph serves any list rewritten in place."""
+        dev = self.state.device
+        if not isinstance(x, torch.Tensor) or not x.is_cuda:
+            raise RuntimeError("StreamResampler needs CUDA tensors (no CPU fallback)")
+        if x.device != dev:
+            raise ValueError(f"x must live on the state's device {dev}, not {x.device}")
+        if (not x.is_floating_point() or x.dim() != 3 or x.shape[0] < 1 or x.shape[1] != self.channels
+                or x.shape[2] < self.block or x.shape[2] % self.block):
+            raise ValueError(f"x must be a floating-point tensor [n, {self.channels}, {self.block} * T] with n, T >= 1, got "
+                             f"{x.dtype} {tuple(x.shape)}")
+        n, C, L = x.shape
+        T = L // self.block
+        y_len = self.keep + T * self.out_block
+        if x.dtype != torch.float32 or x.stride(2) != 1 or x.stride(1) < L or x.stride(0) < C * x.stride(1):
+            x = x.to(torch.float32).contiguous()
+        slots = device_list(slots, dev, n, self.n_slots, True, "slot")
+        if hops is not None:
+            hops = device_list(hops, dev, n, T + 1, False, "hop")
+        if out is None:
+            out = torch.empty(n, C, y_len, dtype=torch.float32, device=dev)
+        elif (not isinstance(out, torch.Tensor) or out.dtype != torch.float32 or out.device != dev
+              or tuple(out.shape) != (n, C, y_len) or out.stride(2) != 1 or out.stride(1) < y_len
+              or out.stride(0) < C * out.stride(1)):
+            raise ValueError(f"out must be a float32 tensor [{n}, {C}, {y_len}] on {dev} with unit sample stride and rows "
+                             "and channels that do not overlap")
+        with torch.cuda.device(dev):
+            self._check(_cabi.lib().l2h_resample_stream(
+                x.data_ptr(), x.stride(0), x.stride(1), out.data_ptr(), out.stride(0), out.stride(1), n, C, T,
+                slots.data_ptr(), None if hops is None else hops.data_ptr(), self.state.data_ptr(), self.n_slots,
+                self.orig_freq, self.new_freq, self.block, self.keep, torch.cuda.current_stream(dev).cuda_stream))
+        return out
+
+    def reset(self, slots):
+        """Make the listed slots fresh streams (their state rows zero); the other slots keep their history."""
+        idx = torch.as_tensor(slots).cpu().reshape(-1)
+        idx = device_list(idx, self.state.device, idx.numel(), self.n_slots, False, "slot")
+        self.state.index_fill_(0, idx.long(), 0.0)
 
 
 def render_binaural(srcs, rirs, noise=None, noise_scale=None, rir_sr=None, sr=16000):
