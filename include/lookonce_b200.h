@@ -497,6 +497,72 @@ int l2h_resample_stream(const float* x_dev, int64_t x_row_stride, int64_t x_ch_s
                         const int32_t* hops_dev, float* state_dev, int32_t n_slots, int32_t orig_freq, int32_t new_freq,
                         int32_t block, int32_t keep, void* stream);
 
+/* Streaming resampling of pushes of any length, for a list of a state's slots: devices at 44.1, 22.05 or 11.025 kHz (whose
+ * 8 ms is no whole number of samples), and clients that send 10 ms packets, at any rate, into and out of the 16 kHz
+ * separator.  With o, q and w as in l2h_resample_stream and D = floor(w q / o), a stream that has been pushed N samples
+ * in all has returned exactly floor(N q / o) samples, and they are bit for bit the first floor(N q / o) samples of z
+ * delayed by D (z the l2h_resample output of everything it was pushed as one signal, zeros before z's start): the same
+ * output and delay as l2h_resample_stream with keep 0, whose pushes of whole periods give the same bits.
+ *
+ * The state is [n_slots][channels][row_floats] fp32 of DEVICE memory: per channel the count of outputs made (capped at D)
+ * and the input count modulo o, both exact in a float, then the last ceil((D + 1) o / q) + w + 1 input samples.  All
+ * zeros is a fresh stream, so a slot is reset by zeroing its rows and moved by copying them.
+ *
+ * l2h_resample_packets_layout: row_floats, delay (D) and max_out = ceil(max_in q / o), the most samples one push of up to
+ * max_in samples returns.  Errors: 1 = null pointer, a rate <= 0, equal rates, max_in <= 0; 2 = the staged window of one
+ * push (the history and max_in samples) exceeds the kernel's shared memory.
+ *
+ * l2h_resample_packets: row i of a call pushes c_i * unit samples, c_i = counts_dev[i], into slot slots_dev[i]:
+ *   x_dev           [n][channels][max_in] fp32, strides in floats; row i reads only its first c_i * unit samples
+ *   y_dev           [n][channels][max_out] fp32; row i receives y[i][c][0 .. m_i), the m_i samples its push makes final.
+ *                   Its later samples are not written.  Must not overlap x or the state.
+ *   counts_dev      [n] int32 of DEVICE memory read when the kernel runs; c_i * unit outside [0, max_in] counts as 0.
+ *                   unit = 1 counts samples; unit = 128 takes the separator's hop counts (l2h_hop_fifo's hops_dev) as they
+ *                   are, for the way back out of it.
+ *   out_counts_dev  [n] int32 of DEVICE memory: m_i, 0 for a row that stores nothing.
+ *   slots_dev       [n] int32 of DEVICE memory read when the kernel runs, like l2h_resample_stream's: an entry outside
+ *                   [0, n_slots) marks a row that stores nothing (no y sample, no state row).  So does a push of 0 samples.
+ * One launch; nothing on the host is read from the device, and a call captured in a CUDA graph serves any lists of the
+ * same n rewritten in place.  Errors, returned before anything is enqueued: 1 = null pointers, n, channels, unit or n_slots
+ * <= 0, n > n_slots, channel or row strides under the lengths above, and the layout's errors 1; 2 = as for the layout.
+ * Asynchronous on `stream`. */
+int l2h_resample_packets_layout(int32_t orig_freq, int32_t new_freq, int32_t max_in, int32_t* row_floats, int32_t* delay,
+                                int32_t* max_out);
+int l2h_resample_packets(const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, float* y_dev, int64_t y_row_stride,
+                         int64_t y_ch_stride, int32_t n, int32_t channels, int32_t max_in, const int32_t* counts_dev,
+                         int32_t unit, int32_t* out_counts_dev, const int32_t* slots_dev, float* state_dev, int32_t n_slots,
+                         int32_t orig_freq, int32_t new_freq, void* stream);
+
+/* A per-slot hop FIFO: 16 kHz pieces of any length in, the separator's chunks and per-row hop counts out, so one tick runs
+ * from device memory (packets in, l2h_resample_packets, l2h_hop_fifo, l2h_sep_forward_slots_hops, l2h_resample_packets
+ * with unit 128) with no count read back to the host.  A slot's signal is 64 zeros, then every sample appended since it
+ * was reset; p is its read position (0 when fresh), and the slot holds the samples past p + 64.
+ *
+ * l2h_hop_fifo: row i appends c_i * unit samples of x row i to slot slots_dev[i] (c_i = counts_dev[i], the count and slot
+ * rules of l2h_resample_packets), then pops h_i = min(frames, floor(held / 128)) hops, held counted after the append:
+ *   chunk_dev   [n][channels][128 * frames + 64] fp32; row i receives chunk[i][c][0 .. 128 h_i + 64), samples
+ *               [p, p + 128 h_i + 64) of its slot's signal (the l2h_sep_forward_slots_hops chunk of h_i hops), and p
+ *               advances by 128 h_i: the last 64 samples stay as the next chunk's start.  Its later samples are not written.
+ *   hops_dev    [n] int32 of DEVICE memory: h_i, 0 for a row whose slot lies outside [0, n_slots) (it stores nothing).
+ * So the same slot list and hops_dev go straight to l2h_sep_forward_slots_hops, and a row with count 0 still drains the
+ * whole hops its slot holds.  Samples past the slot's `capacity` are dropped (the held ones stay intact) and added to the
+ * slot's dropped-sample counter, which shows a client that sends faster than it is served; nothing is read or written out
+ * of bounds.
+ *
+ * The state is [n_slots][channels][row_floats] fp32 of DEVICE memory: per channel three int32 words stored in the floats'
+ * bits (p modulo the ring, the samples held, the samples dropped, saturating at 2^31 - 1), then a ring of 64 + capacity
+ * samples.  All zeros is an empty FIFO, so a slot is reset by zeroing its rows and moved by copying them.
+ * l2h_hop_fifo_layout: row_floats = 3 + 64 + capacity.  Errors: 1 = null pointer, capacity < 128 (one hop).
+ *
+ * One launch.  Errors, returned before anything is enqueued: 1 = null pointers, n, channels, max_in, unit, frames or
+ * n_slots <= 0, n > n_slots, channel or row strides under the lengths above, and the layout's errors.  Asynchronous on
+ * `stream`. */
+int l2h_hop_fifo_layout(int32_t capacity, int32_t* row_floats);
+int l2h_hop_fifo(const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, int32_t max_in, const int32_t* counts_dev,
+                 int32_t unit, float* chunk_dev, int64_t chunk_row_stride, int64_t chunk_ch_stride, int32_t* hops_dev,
+                 int32_t n, int32_t channels, int32_t frames, const int32_t* slots_dev, float* state_dev, int32_t n_slots,
+                 int32_t capacity, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -199,6 +199,128 @@ static int rs_stream(const char* who, int32_t orig, int32_t new_freq, int32_t bl
     s->keep = keep;
     return 0;
 }
+
+// ---- packets: pushes of any number of samples ------------------------------------------------------------------------
+// A stream pushed N samples in all has returned floor(N q / o) of them, each the sample of z' above (the same D).  Output j
+// reads taps up to floor((j - D) o / q) + w, and D o / q >= w - (o - 1) / q, so every tap of j <= floor(N q / o) - 1 has
+// arrived.  Relative to the last period boundary at or before the stream's input count N0 (phase p = N0 mod o), the push
+// makes the outputs floor(p q / o) .. floor((p + n) q / o) - 1, so the phase is all the clock a stream needs.  A state row
+// per channel is [RP_HEAD + H]: the outputs made (capped at D) and the phase, exact in floats, then the last H = ceil((D +
+// 1) o / q) + w + 1 input samples, enough for the taps of a push's first output at any phase.
+constexpr int RP_HEAD = 2;
+
+struct RsPackets {
+    RsRate g;
+    int32_t delay, hist;       // D, H
+    int32_t max_in, unit;      // row i pushes counts[i] * unit samples, counted as 0 outside [0, max_in]
+};
+
+// One CTA = one (call row, channel): stage the slot's history and the row's new samples, compute the new outputs with
+// their phase relative to the period boundary, write them, then store the new history, phase and count.
+__global__ void __launch_bounds__(RS_TILE)
+resample_packets_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, float* __restrict__ y, int64_t y_row,
+                        int64_t y_ch, int C, const int32_t* __restrict__ counts, int32_t* __restrict__ out_counts,
+                        const int32_t* __restrict__ slots, float* __restrict__ state, int n_slots,
+                        const __grid_constant__ RsPackets s) {
+    extern __shared__ float win[];                   // [H + n]: the history, then the row's new samples
+    const int row = blockIdx.x / C, ch = blockIdx.x - row * C, tid = threadIdx.x;
+    const int slot = slots[row];
+    const int64_t pushed = (int64_t)counts[row] * s.unit;
+    const int n = pushed >= 0 && pushed <= s.max_in ? (int)pushed : 0;
+    if (slot < 0 || slot >= n_slots || n == 0) {                        // a row that stores nothing
+        if (ch == 0 && tid == 0) out_counts[row] = 0;
+        return;
+    }
+    const RsRate& g = s.g;
+    const int H = s.hist, D = s.delay;
+    float* st = state + ((int64_t)slot * C + ch) * (RP_HEAD + H);
+    const float made = st[0], phase = st[1];
+    const int before = made >= (float)D ? D : (made > 0.f ? (int)made : 0);
+    const int p = phase >= (float)(g.o - 1) ? g.o - 1 : (phase > 0.f ? (int)phase : 0);
+    const int64_t j0 = (int64_t)p * g.q / g.o;                         // the push's outputs j0 .. j0 + n_new - 1
+    const int n_new = (int)((int64_t)(p + n) * g.q / g.o - j0);
+    if (ch == 0 && tid == 0) out_counts[row] = n_new;
+    const float* xr = x + (int64_t)row * x_row + (int64_t)ch * x_ch;
+    float* yr = y + (int64_t)row * y_row + (int64_t)ch * y_ch;
+    for (int i = tid; i < H + n; i += blockDim.x) win[i] = i < H ? st[RP_HEAD + i] : xr[i - H];
+    __syncthreads();
+    // win[H - p] is the input at the period boundary: output j (relative to it) centres on its input c = floor((j - D) o / q)
+    for (int k = tid; k < n_new; k += blockDim.x) {
+        float v = 0.f;                                                  // before z's start
+        if (before + k >= D) {
+            const int64_t a = (j0 + k - D) * g.o;
+            const int64_t c = a >= 0 ? a / g.q : -((-a + g.q - 1) / g.q);  // floor(a / q)
+            v = rs_output(win + (H - p + c - g.w), a - c * g.q, g);
+        }
+        yr[k] = v;
+    }
+    for (int i = tid; i < H; i += blockDim.x) st[RP_HEAD + i] = win[n + i];
+    if (tid == 0) {
+        st[0] = (float)min(D, before + n_new);
+        st[1] = (float)((p + n) % g.o);
+    }
+}
+
+// the packet stream of orig -> new_freq Hz for pushes of up to max_in samples: 0, or an error code (1 invalid, 2 the
+// window of a row exceeds shared memory) with its message
+static int rs_packets(const char* who, int32_t orig, int32_t new_freq, int32_t max_in, RsPackets* s, int32_t* max_out) {
+    const std::string rates = std::to_string(orig) + " -> " + std::to_string(new_freq) + " Hz";
+    if (orig <= 0 || new_freq <= 0) return fail(1, std::string(who) + ": rates must be positive, got " + rates);
+    if (orig == new_freq) return fail(1, std::string(who) + ": " + rates + " needs no resampling");
+    if (max_in <= 0) return fail(1, std::string(who) + ": max_in " + std::to_string(max_in) + " is not positive");
+    s->g = rs_rate(orig, new_freq, 0);
+    const RsRate& g = s->g;
+    const int64_t delay = (int64_t)g.w * g.q / g.o;
+    const int64_t hist = ((delay + 1) * g.o + g.q - 1) / g.q + g.w + 1;
+    const int64_t out = ((int64_t)max_in * g.q + g.o - 1) / g.o;
+    const int64_t floats = hist + max_in;
+    if (floats * (int64_t)sizeof(float) > RS_SMEM_BYTES)
+        return fail(2, std::string(who) + ": " + rates + " in pushes of up to " + std::to_string(max_in) +
+                           " samples is too large: " + std::to_string(floats) + " staged samples per row (history and "
+                           "push) exceed shared memory (" + std::to_string(RS_SMEM_BYTES / sizeof(float)) + ")");
+    s->delay = (int32_t)delay;
+    s->hist = (int32_t)hist;
+    s->max_in = max_in;
+    *max_out = (int32_t)out;
+    return 0;
+}
+
+// ---- the hop FIFO: 16 kHz pieces of any length -> separator chunks and hop counts ------------------------------------
+// A slot's row per channel is [FF_HEAD + 64 + capacity]: the read position, the samples held and the samples dropped (int32
+// words), then a ring of 64 + capacity samples.  The 64 samples before the read position are the carry, the held ones
+// follow it.  All zeros is an empty FIFO whose carry is 64 zeros.
+constexpr int FF_HEAD = 3, FF_HOP = 128, FF_CARRY = 64;
+
+__global__ void __launch_bounds__(RS_TILE)
+hop_fifo_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, int max_in, const int32_t* __restrict__ counts,
+                int unit, float* __restrict__ chunk, int64_t c_row, int64_t c_ch, int32_t* __restrict__ hops, int C, int T,
+                const int32_t* __restrict__ slots, float* __restrict__ state, int n_slots, int capacity) {
+    const int row = blockIdx.x / C, ch = blockIdx.x - row * C, tid = threadIdx.x;
+    const int slot = slots[row];
+    if (slot < 0 || slot >= n_slots) {                                  // a row that stores nothing
+        if (ch == 0 && tid == 0) hops[row] = 0;
+        return;
+    }
+    const int64_t pushed = (int64_t)counts[row] * unit;
+    const int n = pushed >= 0 && pushed <= max_in ? (int)pushed : 0;
+    const int R = FF_CARRY + capacity;
+    float* st = state + ((int64_t)slot * C + ch) * (FF_HEAD + R);
+    float* ring = st + FF_HEAD;
+    const int pos = min(max(__float_as_int(st[0]), 0), R - 1), held = min(max(__float_as_int(st[1]), 0), capacity);
+    const int kept = min(n, capacity - held), h = min(T, (held + kept) / FF_HOP);
+    const float* xr = x + (int64_t)row * x_row + (int64_t)ch * x_ch;
+    for (int i = tid; i < kept; i += blockDim.x) ring[(pos + held + i) % R] = xr[i];
+    __syncthreads();                                                    // the appended samples, visible to the block
+    float* cr = chunk + (int64_t)row * c_row + (int64_t)ch * c_ch;
+    for (int i = tid; i < h * FF_HOP + FF_CARRY; i += blockDim.x) cr[i] = ring[(pos + R - FF_CARRY + i) % R];
+    if (tid == 0) {
+        if (ch == 0) hops[row] = h;
+        st[0] = __int_as_float((pos + h * FF_HOP) % R);
+        st[1] = __int_as_float(held + kept - h * FF_HOP);
+        const int dropped = __float_as_int(st[2]);
+        st[2] = __int_as_float(n - kept > INT32_MAX - dropped ? INT32_MAX : dropped + (n - kept));
+    }
+}
 }  // namespace l2h
 
 extern "C" int l2h_resample(const float* x_dev, int64_t x_row_stride, int32_t n_in, int32_t n_rows, const int32_t* orig_freq,
@@ -296,5 +418,84 @@ extern "C" int l2h_resample_stream(const float* x_dev, int64_t x_row_stride, int
         n_slots, s);
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(3, std::string("l2h_resample_stream: ") + cudaGetErrorString(e));
+    return 0;
+}
+
+extern "C" int l2h_resample_packets_layout(int32_t orig_freq, int32_t new_freq, int32_t max_in, int32_t* row_floats,
+                                           int32_t* delay, int32_t* max_out) {
+    using namespace l2h;
+    if (!row_floats || !delay || !max_out) return fail(1, "l2h_resample_packets_layout: null pointer");
+    RsPackets s;
+    int32_t out;
+    if (int rc = rs_packets("l2h_resample_packets_layout", orig_freq, new_freq, max_in, &s, &out)) return rc;
+    *row_floats = RP_HEAD + s.hist;
+    *delay = s.delay;
+    *max_out = out;
+    return 0;
+}
+
+extern "C" int l2h_resample_packets(const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, float* y_dev,
+                                    int64_t y_row_stride, int64_t y_ch_stride, int32_t n, int32_t channels, int32_t max_in,
+                                    const int32_t* counts_dev, int32_t unit, int32_t* out_counts_dev,
+                                    const int32_t* slots_dev, float* state_dev, int32_t n_slots, int32_t orig_freq,
+                                    int32_t new_freq, void* stream) {
+    using namespace l2h;
+    if (!x_dev || !y_dev || !counts_dev || !out_counts_dev || !slots_dev || !state_dev)
+        return fail(1, "l2h_resample_packets: null pointer");
+    if (n <= 0 || channels <= 0 || unit <= 0 || n_slots <= 0)
+        return fail(1, "l2h_resample_packets: n, channels, unit and n_slots must be positive");
+    if (n > n_slots) return fail(1, "l2h_resample_packets: a call needs n <= n_slots");
+    if ((int64_t)n * channels > INT32_MAX) return fail(1, "l2h_resample_packets: n * channels is too large");
+    RsPackets s;
+    int32_t max_out;
+    if (int rc = rs_packets("l2h_resample_packets", orig_freq, new_freq, max_in, &s, &max_out)) return rc;
+    s.unit = unit;
+    if (x_ch_stride < max_in || x_row_stride / channels < x_ch_stride || y_ch_stride < max_out ||
+        y_row_stride / channels < y_ch_stride)
+        return fail(1, "l2h_resample_packets: bad stride: rows and channels of x (" + std::to_string(max_in) +
+                           " samples) and y (" + std::to_string(max_out) + ") must not overlap");
+    const int smem = (int)((s.hist + max_in) * sizeof(float));
+    resample_packets_kernel<<<(unsigned)(n * channels), RS_TILE, smem, static_cast<cudaStream_t>(stream)>>>(
+        x_dev, x_row_stride, x_ch_stride, y_dev, y_row_stride, y_ch_stride, channels, counts_dev, out_counts_dev, slots_dev,
+        state_dev, n_slots, s);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(3, std::string("l2h_resample_packets: ") + cudaGetErrorString(e));
+    return 0;
+}
+
+extern "C" int l2h_hop_fifo_layout(int32_t capacity, int32_t* row_floats) {
+    using namespace l2h;
+    if (!row_floats) return fail(1, "l2h_hop_fifo_layout: null pointer");
+    if (capacity < FF_HOP || capacity > INT32_MAX - FF_HEAD - FF_CARRY)
+        return fail(1, "l2h_hop_fifo_layout: capacity " + std::to_string(capacity) + " cannot hold one hop of " +
+                           std::to_string(FF_HOP) + " samples");
+    *row_floats = FF_HEAD + FF_CARRY + capacity;
+    return 0;
+}
+
+extern "C" int l2h_hop_fifo(const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, int32_t max_in,
+                            const int32_t* counts_dev, int32_t unit, float* chunk_dev, int64_t chunk_row_stride,
+                            int64_t chunk_ch_stride, int32_t* hops_dev, int32_t n, int32_t channels, int32_t frames,
+                            const int32_t* slots_dev, float* state_dev, int32_t n_slots, int32_t capacity, void* stream) {
+    using namespace l2h;
+    if (!x_dev || !counts_dev || !chunk_dev || !hops_dev || !slots_dev || !state_dev)
+        return fail(1, "l2h_hop_fifo: null pointer");
+    if (n <= 0 || channels <= 0 || max_in <= 0 || unit <= 0 || frames <= 0 || n_slots <= 0)
+        return fail(1, "l2h_hop_fifo: n, channels, max_in, unit, frames and n_slots must be positive");
+    if (n > n_slots) return fail(1, "l2h_hop_fifo: a call needs n <= n_slots");
+    if ((int64_t)n * channels > INT32_MAX) return fail(1, "l2h_hop_fifo: n * channels is too large");
+    int32_t row_floats;
+    if (int rc = l2h_hop_fifo_layout(capacity, &row_floats)) return rc;
+    const int64_t c_len = (int64_t)frames * FF_HOP + FF_CARRY;
+    if (c_len > INT32_MAX) return fail(1, "l2h_hop_fifo: frames is too large");
+    if (x_ch_stride < max_in || x_row_stride / channels < x_ch_stride || chunk_ch_stride < c_len ||
+        chunk_row_stride / channels < chunk_ch_stride)
+        return fail(1, "l2h_hop_fifo: bad stride: rows and channels of x (" + std::to_string(max_in) + " samples) and chunk (" +
+                           std::to_string(c_len) + ") must not overlap");
+    hop_fifo_kernel<<<(unsigned)(n * channels), RS_TILE, 0, static_cast<cudaStream_t>(stream)>>>(
+        x_dev, x_row_stride, x_ch_stride, max_in, counts_dev, unit, chunk_dev, chunk_row_stride, chunk_ch_stride, hops_dev,
+        channels, frames, slots_dev, state_dev, n_slots, capacity);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(3, std::string("l2h_hop_fifo: ") + cudaGetErrorString(e));
     return 0;
 }

@@ -270,14 +270,16 @@ _LIST_WORDS = {"slot": ("integer slot indices", "slots lists {} records for {} i
                "record": ("integer record indices", "records lists {} records for {} target rows",
                           "a record lies outside [0, {end})"),
                "offset": ("integer row offsets", "offsets gives {} entries for {} = input rows + 1",
-                          "an offset lies outside [0, {last}] (the call's {last} target rows)")}
+                          "an offset lies outside [0, {last}] (the call's {last} target rows)"),
+               "count": ("integer sample counts", "counts gives {} counts for {} input rows",
+                         "a count lies outside [0, {last}] (the units one input row holds)")}
 
 
 def device_list(values, dev, n, end, distinct, noun):
-    """`values` (slots, groups, records, offsets or hop counts of a call of n rows) as the [n] int32 device tensor the engine
-    reads (the separator's calls and StreamResampler).  A CUDA int32 tensor is used as it is (its entries are read when the
-    kernels run); anything else is checked here (n ints in [0, end), each listed once if `distinct`) and uploaded.  noun: a
-    key of _LIST_WORDS, for the messages."""
+    """`values` (slots, groups, records, offsets, hop or sample counts of a call of n rows) as the [n] int32 device tensor
+    the engine reads (the separator's calls and the streaming resamplers and FIFO).  A CUDA int32 tensor is used as it is
+    (its entries are read when the kernels run); anything else is checked here (n ints in [0, end), each listed once if
+    `distinct`) and uploaded.  noun: a key of _LIST_WORDS, for the messages."""
     entries, count, outside = _LIST_WORDS[noun]
     if isinstance(values, torch.Tensor) and values.is_cuda:
         if values.dtype != torch.int32 or tuple(values.shape) != (n,) or not values.is_contiguous():
