@@ -421,6 +421,9 @@ int l2h_embed_forward_lengths(void* handle, const float* x_dev, int32_t n_max, c
  *   output_sisnr  = mean over channels of SI-SNR(est, target)                 (torchmetrics definition, zero-mean)
  *   si_snr_i      = mean over channels of SI-SNR(est, target) - SI-SNR(mixture, target)   (0 if mixture_dev is NULL)
  *   embedding_sim = cosine similarity of emb and emb_gt                        (0 if either is NULL)
+ * SI-SNR is computed in double in torchmetrics' order: the means, then the centred sums and alpha, then the residual
+ * energy |alpha t~ - p~|^2 directly (three passes over each row), so a DC offset on the signals costs no precision.
+ * The cosine clamps each norm to 1e-8 separately, as F.cosine_similarity does.
  * est / target / mixture: [batch][channels][n_samples] fp32 contiguous on the device (est = the separator's output
  * buffer); emb / emb_gt: [batch][emb_dim].  Asynchronous on `stream`; the caller copies 3 floats per mixture back. */
 int l2h_eval_metrics(const float* est_dev, const float* target_dev, const float* mixture_dev, int32_t batch, int32_t channels,

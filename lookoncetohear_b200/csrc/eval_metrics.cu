@@ -4,8 +4,12 @@
 //   si_snr_i      = mean over ears of SI-SNR(estimate, target) - SI-SNR(mixture, target)
 //   embedding_sim = cosine_similarity(embedding, embedding_gt)
 // so that the device->host traffic of an evaluation step shrinks from the separated audio to three floats per mixture.
-// SI-SNR as torchmetrics' scale_invariant_signal_noise_ratio (zero-mean; alpha = (<p,t>+eps)/(<t,t>+eps);
-// 10 log10((|alpha t|^2+eps)/(|alpha t - p|^2+eps)), eps = float32 eps).  All sums in double.
+// SI-SNR as torchmetrics' scale_invariant_signal_noise_ratio, in its order and all in double, per channel row:
+//   1. the means of estimate, target (and mixture);
+//   2. the centred sums <p~,t~>, <t~,t~> and alpha = (<p~,t~>+eps)/(<t~,t~>+eps);
+//   3. the residual energy |alpha t~ - p~|^2 summed directly;
+// then 10 log10((alpha^2 <t~,t~>+eps)/(|alpha t~ - p~|^2+eps)), eps = float32 eps.  Three passes over the row instead of
+// one-pass raw sums: spt - sp st / n and friends cancel catastrophically once the signals carry a DC offset.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string>
@@ -27,13 +31,10 @@ __device__ __forceinline__ double blk_sum(double v, double* red) {
     return t;
 }
 
-__device__ __forceinline__ double si_snr_from_sums(double n, double sp, double st, double spp, double stt, double spt) {
-    const double eps = 1.1920928955078125e-07;          // torch.finfo(torch.float32).eps
-    const double pt = spt - sp * st / n, tt = stt - st * st / n, pp = spp - sp * sp / n;
-    const double alpha = (pt + eps) / (tt + eps);
-    const double sig = alpha * alpha * tt;
-    const double noise = sig - 2.0 * alpha * pt + pp;
-    return 10.0 * log10((sig + eps) / (fmax(noise, 0.0) + eps));
+constexpr double SI_EPS = 1.1920928955078125e-07;          // torch.finfo(torch.float32).eps
+
+__device__ __forceinline__ double si_snr_db(double sig, double noise) {
+    return 10.0 * log10((sig + SI_EPS) / (noise + SI_EPS));
 }
 
 // one CTA per mixture; 256 threads
@@ -45,19 +46,32 @@ eval_metrics_kernel(const float* __restrict__ est, const float* __restrict__ tgt
     double acc_s = 0.0, acc_i = 0.0;
     for (int c = 0; c < ch; ++c) {
         const int64_t off = ((int64_t)b * ch + c) * n;
-        double sp = 0, st = 0, sm = 0, spp = 0, stt = 0, smm = 0, spt = 0, smt = 0;
+        const float *p = est + off, *t = tgt + off, *m = mix ? mix + off : nullptr;
+        double sp = 0, st = 0, sm = 0;
         for (int i = tid; i < n; i += 256) {
-            const double p = est[off + i], t = tgt[off + i];
-            sp += p; st += t; spp += p * p; stt += t * t; spt += p * t;
-            if (mix) { const double m = mix[off + i]; sm += m; smm += m * m; smt += m * t; }
+            sp += p[i]; st += t[i];
+            if (m) sm += m[i];
         }
-        sp = blk_sum(sp, red); st = blk_sum(st, red); spp = blk_sum(spp, red); stt = blk_sum(stt, red); spt = blk_sum(spt, red);
-        const double s_est = si_snr_from_sums((double)n, sp, st, spp, stt, spt);
+        const double mp = blk_sum(sp, red) / n, mt = blk_sum(st, red) / n, mm = m ? blk_sum(sm, red) / n : 0.0;
+        double spt = 0, stt = 0, smt = 0;
+        for (int i = tid; i < n; i += 256) {
+            const double tc = t[i] - mt;
+            spt += (p[i] - mp) * tc; stt += tc * tc;
+            if (m) smt += (m[i] - mm) * tc;
+        }
+        const double tt = blk_sum(stt, red);
+        const double ap = (blk_sum(spt, red) + SI_EPS) / (tt + SI_EPS);
+        const double am = m ? (blk_sum(smt, red) + SI_EPS) / (tt + SI_EPS) : 0.0;
+        double rp = 0, rm = 0;
+        for (int i = tid; i < n; i += 256) {
+            const double tc = t[i] - mt;
+            const double ep = ap * tc - (p[i] - mp);
+            rp += ep * ep;
+            if (m) { const double em = am * tc - (m[i] - mm); rm += em * em; }
+        }
+        const double s_est = si_snr_db(ap * ap * tt, blk_sum(rp, red));
         acc_s += s_est;
-        if (mix) {
-            sm = blk_sum(sm, red); smm = blk_sum(smm, red); smt = blk_sum(smt, red);
-            acc_i += s_est - si_snr_from_sums((double)n, sm, st, smm, stt, smt);
-        }
+        if (m) acc_i += s_est - si_snr_db(am * am * tt, blk_sum(rm, red));
     }
     double cs = 0.0;
     if (emb && emb_gt) {

@@ -346,12 +346,18 @@ def render_binaural(srcs, rirs, noise=None, noise_scale=None, rir_sr=None, sr=16
     Returns (events [B, S, 2, N], mixture [B, 2, N], norm [B]); the target of a sample is events[:, tgt_idx]."""
     if not srcs.is_cuda:
         raise RuntimeError("lookoncetohear_b200.render.render_binaural needs CUDA tensors (no CPU fallback)")
+    if srcs.dim() != 3:
+        raise ValueError(f"srcs must be [B, S, N], got {tuple(srcs.shape)}")
+    B, S, N = srcs.shape
+    if rirs.dim() != 4 or tuple(rirs.shape[:3]) != (B, S, 2) or rirs.shape[3] < 1:
+        raise ValueError(f"rirs must be [B, S, 2, L >= 1] = [{B}, {S}, 2, L], got {tuple(rirs.shape)}")
+    if noise is not None and tuple(noise.shape) != (B, 2, N):
+        raise ValueError(f"noise must be [B, 2, N] = [{B}, 2, {N}], got {tuple(noise.shape)}")
+    if noise_scale is not None and noise_scale.numel() != B:
+        raise ValueError(f"noise_scale must have one element per batch item ({B}), got {noise_scale.numel()}")
     dev = srcs.device
     src = srcs.contiguous().float()
     rir = rirs.to(dev, torch.float32).contiguous()
-    B, S, N = src.shape
-    if rir.shape[:3] != (B, S, 2):
-        raise ValueError(f"rirs must be [B, S, 2, L], got {tuple(rir.shape)}")
     if rir_sr is not None:
         per_item = torch.as_tensor(rir_sr).detach().cpu().reshape(-1)
         if per_item.numel() not in (1, B):

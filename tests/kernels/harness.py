@@ -12,6 +12,7 @@ bf16 weights times split activations.
 import ctypes
 import math
 
+import numpy as np
 import torch
 
 from lookoncetohear_b200 import build as _build
@@ -1587,3 +1588,272 @@ def gate_fanout_ref(X0, gates, owner, K, apply_gate, mutant=None):
         v = X0[max(i, 0)].float()
         out[r] = v * gates[r].float()[None] if apply_gate and (i >= 0 or mutant == "gate_unowned") else v
     return out
+
+
+# ---- binaural renderer (csrc/render.cu) and evaluation metrics (csrc/eval_metrics.cu) --------------------------------
+U32 = 2.0 ** -24                    # unit roundoff of fp32
+U64 = 2.0 ** -53                    # unit roundoff of float64
+F32_EPS = 1.1920928955078125e-07    # torch.finfo(torch.float32).eps, torchmetrics' SI-SNR epsilon
+FIR_MUTANTS = ("drop_chunk_tap", "tile_shift", "left_both", "src_se")
+MIX_MUTANTS = ("peak_ear0", "noise_unnormalised")
+METRICS_MUTANTS = ("no_centre", "one_pass", "f64_eps", "first_ear", "si_i_sign", "clamp_product")
+
+
+def fir64(src, rir, exact=False, mutant=None):
+    """fir_kernel: events [B, S, 2, N] = convolve(src[b, s], rir[b, s, ear])[:N] from src [B, S, N] and rir [B, S, 2, L],
+    in float64 (fftconvolve).  exact: data whose products lie on the 2^-8 grid (integers, or halves times quarters),
+    rounded to the nearest multiple of 2^-8 (+0.0, never -0.0), which is exact while every sum stays far below 2^45.  Mutants (FIR_MUTANTS): drop_chunk_tap (tap k of a 256-tap chunk with
+    k % 256 == 255 left out), tile_shift (every tile's source window one sample early: y[o] = F[o - 1]), left_both (both
+    ears with the left-ear response), src_se (event (s, ear) reads source row 2 s + ear of the flattened [B * S] sources,
+    NaN past the last)."""
+    from scipy.signal import fftconvolve
+    src, rir = np.asarray(src, np.float64), np.asarray(rir, np.float64).copy()
+    B, S, N = src.shape
+    x = np.broadcast_to(src[:, :, None, :], (B, S, 2, N))
+    if mutant == "src_se":
+        flat = np.concatenate([src.reshape(B * S, N), np.full((2 * S, N), np.nan)])
+        x = flat[np.arange(B)[:, None, None] * S + 2 * np.arange(S)[None, :, None] + np.arange(2)[None, None, :]]
+    if mutant == "drop_chunk_tap":
+        rir[..., 255::256] = 0.0
+    if mutant == "left_both":
+        rir[:, :, 1] = rir[:, :, 0]
+    y = fftconvolve(x, rir, axes=-1)[..., :N]
+    if exact:
+        y = np.rint(y * 256.0) / 256.0 + 0.0
+    if mutant == "tile_shift":
+        y = np.concatenate([np.zeros_like(y[..., :1]), y[..., :-1]], axis=-1)
+    return y
+
+
+def fir_bound64(src, rir):
+    """per-sample bound on one fp32 running sum of the L products: (L + 1) 2^-24 sum_k |h_k| |x_(o-k)|"""
+    return (rir.shape[-1] + 1) * U32 * fir64(np.abs(src), np.abs(rir))
+
+
+def mix64(ev, noise=None, scale=None, fp32=False, mutant=None):
+    """mix_peak_kernel + mix_norm_kernel: (events [B, S, 2, N], mixture [B, 2, N], norm [B]) from the un-normalised events
+    ev [B, S, 2, N], noise [B, 2, N] or None and scale [B] or None (= 1).
+    fp32: the kernels' fp32 model -- the peak of |v| with v = fl(sc noise) (0 without noise) plus each event in order,
+    nf = max(peak, 1), events fl32(e / nf), the mixture fl32(fl32(sc / nf) noise) plus each normalised event in order;
+    otherwise the same in float64 (the reference's arithmetic).  Mutants (MIX_MUTANTS): peak_ear0 (the peak over ear 0
+    only), noise_unnormalised (the mixture's noise not divided by nf)."""
+    dt = np.float32 if fp32 else np.float64
+    ev = np.asarray(ev).astype(dt)
+    B, S, _, N = ev.shape
+    sc = np.ones(B, dt) if scale is None else np.asarray(scale).astype(dt)
+    nz = None if noise is None else np.asarray(noise).astype(dt)
+    v = np.zeros((B, 2, N), dt) if nz is None else sc[:, None, None] * nz
+    for s in range(S):
+        v = v + ev[:, s]
+    peak = np.abs(v[:, :1] if mutant == "peak_ear0" else v).reshape(B, -1).max(1)
+    nf = np.maximum(peak, dt(1))
+    e = ev / nf[:, None, None, None]
+    m = np.zeros((B, 2, N), dt) if nz is None else (sc if mutant == "noise_unnormalised" else sc / nf)[:, None, None] * nz
+    for s in range(S):
+        m = m + e[:, s]
+    return e, m, nf
+
+
+def mix_bound64(e, noise, scale, nf):
+    """per-sample bound on the kernel's fp32 mixture against sc noise / nf + sum_s e_s in float64 (e, nf: the kernel's
+    own events and norm): one rounding for sc / nf, one for the product (none if fused with the first add), S for the
+    adds: (S + 3) 2^-24 (|sc noise| / nf + sum |e_s|), the extra unit covering gamma_(S+2)'s slack"""
+    S = e.shape[1]
+    a = np.abs(np.asarray(e, np.float64)).sum(1)
+    if noise is not None:
+        sc = np.ones(len(nf)) if scale is None else np.asarray(scale, np.float64)
+        a = a + np.abs(sc[:, None, None] * np.asarray(noise, np.float64)) / np.asarray(nf, np.float64)[:, None, None]
+    return (S + 3) * U32 * a
+
+
+def render_int_inputs(B, S, N, L, seed, noise=False):
+    """integer-valued sources and responses (|x|, |h| <= 8 up to L = 4097, <= 4 beyond): every partial sum of the FIR and
+    of the peak is an integer below 2^24, so the fp32 kernels are exact in any order.  noise: integer noise in [-8, 8]
+    and power-of-two scales 2^-3 .. 2^2 (sc noise then stays on a 2^-3 grid: the peak's sums are exact too)."""
+    rng = np.random.default_rng(seed)
+    a = 8 if L <= 4097 else 4
+    src = rng.integers(-a, a + 1, (B, S, N)).astype(np.float32)
+    rir = rng.integers(-a, a + 1, (B, S, 2, L)).astype(np.float32)
+    if not noise:
+        return src, rir, None, None
+    return src, rir, rng.integers(-8, 9, (B, 2, N)).astype(np.float32), (2.0 ** rng.integers(-3, 3, B)).astype(np.float32)
+
+
+# (B, S, N, L, noise, mutants that must miss the exact comparison).  L on and around the 256-tap chunk edges, N on and
+# around the 1024-sample tiles, below 4 and past 132 * 256 / 2 = 16896 (the mixing kernels' grid-stride loop), L > N.
+RENDER_EXACT_CASES = (
+    (1, 1, 1, 1, False, ("left_both",)),
+    (2, 1, 3, 2, False, FIR_MUTANTS[1:]),
+    (3, 4, 4, 255, False, FIR_MUTANTS[1:]),
+    (2, 4, 5, 256, False, FIR_MUTANTS[1:]),
+    (1, 1, 1023, 257, False, FIR_MUTANTS[:3]),
+    (2, 2, 1024, 511, False, FIR_MUTANTS),
+    (1, 4, 1025, 512, False, FIR_MUTANTS),
+    (2, 1, 16896, 513, False, FIR_MUTANTS),
+    (1, 2, 16897, 4096, False, FIR_MUTANTS),
+    (1, 1, 80000, 4097, False, FIR_MUTANTS[:3]),
+    (1, 1, 80000, 16384, False, FIR_MUTANTS[:3]),
+    (300, 1, 1025, 257, False, FIR_MUTANTS),
+    (7, 4, 3, 4096, False, FIR_MUTANTS[1:]),
+    (2, 4, 1000, 16384, False, FIR_MUTANTS),
+    (3, 4, 1025, 257, True, FIR_MUTANTS + ("noise_unnormalised",)),
+    (2, 2, 17000, 300, True, FIR_MUTANTS + ("noise_unnormalised",)),
+    (1, 1, 3, 5, True, ("left_both", "tile_shift", "noise_unnormalised")),
+)
+
+
+def render_peak_inputs(N=20000):
+    """Four items of two events, a three-tap response, no noise: item 0's mixture peaks at exactly 1.0 (events unchanged),
+    item 1's at -64 on ear 0's sample 0, item 2's stays below 1 (events unchanged), item 3's -- the last item's -- at 64
+    on ear 1's last sample.  Every other |mixture| sample is at most 8."""
+    rng = np.random.default_rng(11)
+    src = rng.integers(-1, 2, (4, 2, N)).astype(np.float32)
+    rir = rng.integers(-1, 2, (4, 2, 2, 3)).astype(np.float32)
+    src[0], rir[0] = 0.0, 0.0
+    src[0, 0, 5], rir[0, 0, 1, 0] = 1.0, 1.0
+    src[1, 1, 0], rir[1, 1, 0, 0] = -8.0, 8.0
+    src[2, 1] = 0.0
+    src[2, 0] *= 0.5
+    rir[2, 0] = (0.25, -0.25, 0.25)
+    src[3, 0, -1], rir[3, 0, 1] = 8.0, (8.0, 0.0, 0.0)
+    rir[3, 1, 1] = 0.0
+    return src, rir
+
+
+def si_snr64(p, t, mutant=None):
+    """SI-SNR in dB over the last axis, centred and in float64, as oracle/restate.py::si_sdr (torchmetrics).  Mutants
+    (METRICS_MUTANTS): no_centre, one_pass (raw sums: pt = spt - sp st / n, ..., noise = alpha^2 tt - 2 alpha pt + pp),
+    f64_eps (float64's epsilon for float32's)."""
+    p, t = np.asarray(p, np.float64), np.asarray(t, np.float64)
+    eps = np.finfo(np.float64).eps if mutant == "f64_eps" else F32_EPS
+    if mutant == "one_pass":
+        n = p.shape[-1]
+        sp, st = p.sum(-1), t.sum(-1)
+        pt, tt, pp = (p * t).sum(-1) - sp * st / n, (t * t).sum(-1) - st * st / n, (p * p).sum(-1) - sp * sp / n
+        alpha = (pt + eps) / (tt + eps)
+        sig = alpha * alpha * tt
+        return 10 * np.log10((sig + eps) / (np.maximum(sig - 2 * alpha * pt + pp, 0.0) + eps))
+    if mutant != "no_centre":
+        p, t = p - p.mean(-1, keepdims=True), t - t.mean(-1, keepdims=True)
+    alpha = ((p * t).sum(-1, keepdims=True) + eps) / ((t * t).sum(-1, keepdims=True) + eps)
+    ts = alpha * t
+    r = ts - p
+    return 10 * np.log10(((ts * ts).sum(-1) + eps) / ((r * r).sum(-1) + eps))
+
+
+def si_snr_err64(p, t):
+    """bound on the double-precision error, in dB, of SI-SNR computed in the centred order (means, centred sums and alpha,
+    residual energy summed directly), from the centred signals alone, so it does not grow with a DC offset: the energies'
+    relative errors stay below 4 (n + 2) u64 (1 + sqrt(sig / noise)) each (the sums' n u64, the residual's cancellation
+    u64 (|alpha t~| + |p~|) per sample, through Cauchy-Schwarz), and 10 log10 turns a relative error r into 10 r / ln 10 dB"""
+    p, t = np.asarray(p, np.float64), np.asarray(t, np.float64)
+    n = p.shape[-1]
+    p, t = p - p.mean(-1, keepdims=True), t - t.mean(-1, keepdims=True)
+    alpha = ((p * t).sum(-1, keepdims=True) + F32_EPS) / ((t * t).sum(-1, keepdims=True) + F32_EPS)
+    sig, noise = ((alpha * t) ** 2).sum(-1) + F32_EPS, ((alpha * t - p) ** 2).sum(-1) + F32_EPS
+    return 10 / math.log(10) * 8 * (n + 2) * U64 * (1 + np.sqrt(sig / noise))
+
+
+def cos64(x, y, mutant=None):
+    """F.cosine_similarity over the last axis in float64: <x, y> / (max(|x|, 1e-8) max(|y|, 1e-8)).  Mutant
+    clamp_product: <x, y> / max(|x| |y|, 1e-8)."""
+    x, y = np.asarray(x, np.float64), np.asarray(y, np.float64)
+    nx, ny = np.sqrt((x * x).sum(-1)), np.sqrt((y * y).sum(-1))
+    den = np.maximum(nx * ny, 1e-8) if mutant == "clamp_product" else np.maximum(nx, 1e-8) * np.maximum(ny, 1e-8)
+    return (x * y).sum(-1) / den
+
+
+def eval_metrics64(est, tgt, mix=None, emb=None, emb_gt=None, mutant=None):
+    """eval_metrics_kernel in float64: est / tgt / mix [B, C, n], emb / emb_gt [B, D] -> ([B, 3] (mean over channels of
+    SI-SNR(est, tgt), mean of SI-SNR(est, tgt) - SI-SNR(mix, tgt) (0 without mix), cosine (0 without embeddings)),
+    [B, 3] bound on the kernel's error: its fp32 rounding plus si_snr_err64 of each term, or the cosine's double
+    rounding 2 (D + 4) u64 (sum |x y| / den + |cos|)).  Mutants: METRICS_MUTANTS (first_ear: ear 0 instead of the mean;
+    si_i_sign: si_snr_i negated)."""
+    s = si_snr64(est, tgt, mutant)
+    err = si_snr_err64(est, tgt)
+    out, bound = np.zeros((s.shape[0], 3)), np.zeros((s.shape[0], 3))
+    red = (lambda a: a[:, 0]) if mutant == "first_ear" else (lambda a: a.mean(1))
+    out[:, 0], bound[:, 0] = red(s), err.mean(1)
+    if mix is not None:
+        out[:, 1] = red(s - si_snr64(mix, tgt, mutant)) * (-1 if mutant == "si_i_sign" else 1)
+        bound[:, 1] = (err + si_snr_err64(mix, tgt)).mean(1)
+    if emb is not None:
+        x, y = np.asarray(emb, np.float64), np.asarray(emb_gt, np.float64)
+        out[:, 2] = cos64(x, y, mutant)
+        den = np.maximum(np.sqrt((x * x).sum(-1)), 1e-8) * np.maximum(np.sqrt((y * y).sum(-1)), 1e-8)
+        bound[:, 2] = 2 * (x.shape[-1] + 4) * U64 * (np.abs(x * y).sum(-1) / den + np.abs(out[:, 2]))
+    return out, U32 * (np.abs(out) + bound) + bound
+
+
+def worst_ratio(got, ref, bound):
+    """max |got - ref| / bound, where a zero bound asks for equality (inf if not met)"""
+    d = np.abs(np.asarray(got, np.float64) - np.asarray(ref, np.float64))
+    with np.errstate(divide="ignore", invalid="ignore"):
+        r = np.where(bound > 0, d / np.where(bound > 0, bound, 1.0), np.where(d == 0, 0.0, np.inf))
+    return float(r.max()) if r.size else 0.0
+
+
+EMB_KINDS = ("random", "zero", "tiny", "parallel", "antiparallel", "huge", "tiny_vs_unit")
+
+
+def metrics_inputs(B, C, n, seed, snr=(20.0,), dc=(0.0,), target="noise", mixture=True, D=None):
+    """est, tgt, mix (or None), emb, emb_gt (or None), fp32.  The target: 0.1 N(0, 1) ("noise"), zeros ("silent") or one
+    random constant per row ("constant").  Item b's estimate is dc_b 0.1 + 1.7 t + white noise at snr_b + 3 c dB on ear c
+    (snr_b = snr[b % len(snr)], dc_b = dc[b // len(snr) % len(dc)], offsets in units of the target's RMS 0.1); the
+    mixture t + 0.1 N(0, 1) + dc_b 0.05.  Embeddings of dimension D cycle through EMB_KINDS: zero (emb = 0), tiny (both
+    of norm 1e-9), parallel (emb_gt = 3 emb), antiparallel (emb_gt = -emb / 2), huge (elements near 1e18),
+    tiny_vs_unit (norms 1e-9 and 1)."""
+    rng = np.random.default_rng(seed)
+    if target == "noise":
+        t = 0.1 * rng.standard_normal((B, C, n))
+    elif target == "silent":
+        t = np.zeros((B, C, n))
+    else:
+        t = np.broadcast_to(rng.uniform(-1, 1, (B, C, 1)), (B, C, n))
+    t = t.astype(np.float32).astype(np.float64)
+    sb = np.array([snr[b % len(snr)] for b in range(B)])[:, None] + 3.0 * np.arange(C)[None, :]
+    db = np.array([dc[b // len(snr) % len(dc)] for b in range(B)])[:, None, None]
+    w = 0.17 * 10.0 ** (-sb / 20)
+    est = (db * 0.1 + 1.7 * t + w[:, :, None] * rng.standard_normal((B, C, n))).astype(np.float32)
+    mix = (t + 0.1 * rng.standard_normal((B, C, n)) + db * 0.05).astype(np.float32) if mixture else None
+    emb = emb_gt = None
+    if D is not None:
+        x, y = rng.standard_normal((B, D)), rng.standard_normal((B, D))
+        for b in range(B):
+            k = EMB_KINDS[b % len(EMB_KINDS)]
+            nx = np.linalg.norm(x[b])
+            if k == "zero":
+                x[b] = 0.0
+            elif k == "tiny":
+                x[b], y[b] = x[b] * 1e-9 / nx, y[b] * 1e-9 / np.linalg.norm(y[b])
+            elif k == "parallel":
+                y[b] = 3.0 * x[b]
+            elif k == "antiparallel":
+                y[b] = -0.5 * x[b]
+            elif k == "huge":
+                x[b], y[b] = x[b] * 1e18, y[b] * 1e18
+            elif k == "tiny_vs_unit":
+                x[b], y[b] = x[b] * 1e-9 / nx, y[b] / np.linalg.norm(y[b])
+        emb, emb_gt = x.astype(np.float32), y.astype(np.float32)
+    return est, t.astype(np.float32), mix, emb, emb_gt
+
+
+# (id, metrics_inputs arguments, mutants that must miss the bound by >= 10x on the case)
+METRICS_CASES = (
+    ("snr_sweep", dict(B=5, C=2, n=80000, seed=1, snr=(-30.0, 0.0, 30.0, 60.0, 90.0), D=256), ("first_ear", "si_i_sign")),
+    ("dc_offsets", dict(B=8, C=2, n=80000, seed=2, snr=(60.0, 84.0), dc=(0.0, 1.0, 100.0, 1000.0), D=1000),
+     ("no_centre", "one_pass", "first_ear", "si_i_sign", "clamp_product")),
+    ("dc_long", dict(B=1, C=2, n=2 ** 20 + 3, seed=3, snr=(84.0,), dc=(1000.0,), D=257),
+     ("no_centre", "one_pass", "first_ear", "si_i_sign")),
+    ("one_ear", dict(B=5, C=1, n=257, seed=4, snr=(-10.0, 10.0, 40.0), dc=(0.0, 1.0), D=1), ("si_i_sign",)),
+    ("three_ears", dict(B=5, C=3, n=255, seed=5, snr=(0.0, 25.0, 50.0), D=255), ("first_ear", "si_i_sign", "clamp_product")),
+    ("n2", dict(B=1, C=2, n=2, seed=6, D=257), ()),
+    ("n3_b300", dict(B=300, C=2, n=3, seed=7, snr=(-30.0, 0.0, 30.0, 90.0), D=1000), ("clamp_product",)),
+    ("n256", dict(B=5, C=3, n=256, seed=8, snr=(10.0, 70.0), D=257), ("first_ear", "si_i_sign", "clamp_product")),
+    ("silent_target", dict(B=2, C=2, n=1000, seed=9, target="silent", D=256), ("f64_eps",)),
+    ("constant_target", dict(B=2, C=3, n=1001, seed=10, target="constant", dc=(100.0,), D=256), ("f64_eps",)),
+    ("no_mixture", dict(B=5, C=2, n=2 ** 20 + 3, seed=11, snr=(90.0, 30.0), dc=(1.0, 1000.0), mixture=False, D=256),
+     ("no_centre", "one_pass", "first_ear")),
+    ("no_embeddings", dict(B=300, C=2, n=257, seed=12, snr=(-30.0, 0.0, 45.0, 90.0), dc=(0.0, 100.0)),
+     ("no_centre", "first_ear", "si_i_sign")),
+)
