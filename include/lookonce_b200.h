@@ -26,6 +26,8 @@
  *           with host buffers: H2D of each chunk and D2H of each result inside the call
  *   l2h_embed_create / l2h_embed_load_weight / l2h_embed_commit_weights / l2h_embed_forward
  *        <- EmbedTFGridNet.__init__/forward     src/models/tfgridnet_orig/tfgridnet.py:88-127
+ *   l2h_enroll_capture / l2h_embed_forward_slots
+ *        <- EmbedTFGridNet.forward of a listener's own recent stream (EnrollCapture, EmbedTFGridNet.enroll)
  *
  * Conventions follow the reference's only FFI (src/datasets/motion_simulator.py:30-95): every
  * function returns int (0 = OK, non-zero = error, text via l2h_last_error()), handles are opaque
@@ -414,6 +416,28 @@ int l2h_embed_forward(void* handle, const float* x_dev, float* emb_dev, int32_t 
  * length outside [192, n_max], or a workspace smaller than the query.  Asynchronous on `stream`. */
 int l2h_embed_forward_lengths(void* handle, const float* x_dev, int32_t n_max, const int32_t* lengths_host, int32_t batch,
                               float* emb_dev, void* workspace_dev, size_t workspace_bytes, void* stream);
+/* Enrollment from listeners' own streams: row b embeds the last used_b = min(lengths_host[b], captured) samples that slot
+ * s = slots[b] of an enrollment capture (l2h_enroll_capture below) holds, read from its ring in place, with no gather copy
+ * and nothing read back to the host.  Row b is l2h_embed_forward_lengths of those samples in a batch padded to n_max, bit
+ * for bit.
+ *   capture_dev  the capture's state [n_slots][2][row_floats] (l2h_enroll_capture_layout(capacity)), written by earlier
+ *                work on `stream`
+ *   slots_host / slots_dev  exactly one is non-NULL: a HOST array of `batch` distinct slots in [0, n_slots), read during the
+ *                call only, or `batch` int32 of DEVICE memory read when the kernels run, where an entry outside [0, n_slots)
+ *                marks a row that embeds nothing
+ *   lengths_host HOST array of `batch` lengths in [192, n_max], read during the call only
+ *   emb_dev      row b goes to emb_dev + b * emb_row_stride (>= 256 floats), so it can land in a row of the separator's
+ *                embedding staging buffer.  A row with used_b < 192 (the slot captured too little) is not written: its
+ *                listener keeps the embedding it had.
+ *   used_dev     [batch] int32 of DEVICE memory: used_b, or 0 for a row that was not written
+ *   workspace    l2h_embed_workspace_bytes(batch, n_max), as for l2h_embed_forward_lengths; n_max <= capacity
+ * Errors, returned before anything is enqueued and before the weights are checked: 1 = a null pointer, both or neither slot
+ * list, batch or n_slots <= 0, batch > n_slots, capacity < 192, n_max outside [192, capacity], emb_row_stride < 256, a length
+ * outside [192, n_max], a host slot outside [0, n_slots) or listed twice, or a workspace smaller than the query.
+ * Asynchronous on `stream`. */
+int l2h_embed_forward_slots(void* handle, const float* capture_dev, int32_t n_slots, int32_t capacity, const int32_t* slots_host,
+                            const int32_t* slots_dev, const int32_t* lengths_host, int32_t batch, int32_t n_max, float* emb_dev,
+                            int64_t emb_row_stride, int32_t* used_dev, void* workspace_dev, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Evaluation epilogue on the device (replaces the CPU metric code after `outputs.cpu()` in
@@ -565,6 +589,31 @@ int l2h_hop_fifo(const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, 
                  int32_t unit, float* chunk_dev, int64_t chunk_row_stride, int64_t chunk_ch_stride, int32_t* hops_dev,
                  int32_t n, int32_t channels, int32_t frames, const int32_t* slots_dev, float* state_dev, int32_t n_slots,
                  int32_t capacity, void* stream);
+
+/* A per-slot enrollment capture: the recent 16 kHz input of each listener, kept on the device as it streams, so an
+ * enrollment (l2h_embed_forward_slots) needs no copy of the audio on the host.
+ *
+ * l2h_enroll_capture: row i appends samples 64 .. 64 + 128 h - 1 of its chunk, h = hops_dev[i], to slot slots_dev[i]: the
+ * hops' new samples, without the look-ahead that the next chunk repeats.  It takes the chunk, slot and hop tensors that
+ * l2h_hop_fifo gives l2h_sep_forward_slots_hops:
+ *   chunk_dev   [n][channels][128 * frames + 64] fp32, strides in floats; row i reads only samples 64 .. 128 h + 63
+ *   slots_dev   [n] int32 of DEVICE memory read when the kernel runs: an entry outside [0, n_slots) marks a row that stores
+ *               nothing.  A slot listed twice is a caller error the call does not detect.
+ *   hops_dev    [n] int32 of DEVICE memory read when the kernel runs: h = 0, or an entry outside [0, frames], stores nothing.
+ * So a call captured in a CUDA graph with l2h_hop_fifo and l2h_sep_forward_slots_hops serves any lists of the same n
+ * rewritten in place.  A slot keeps its last `capacity` samples.
+ *
+ * The state is [n_slots][channels][row_floats] fp32 of DEVICE memory: per channel two int32 words stored in the floats' bits
+ * (the write position in the ring, the samples captured since reset, capped at capacity), then a ring of capacity samples.
+ * All zeros is an empty capture, so a slot is reset by zeroing its rows and moved by copying them.
+ * l2h_enroll_capture_layout: row_floats = 2 + capacity.  Errors: 1 = null pointer, capacity < 192 (the shortest enrollment).
+ *
+ * One launch.  Errors, returned before anything is enqueued: 1 = null pointers, n, channels, frames or n_slots <= 0,
+ * n > n_slots, channel or row strides under the chunk's length, and the layout's errors.  Asynchronous on `stream`. */
+int l2h_enroll_capture_layout(int32_t capacity, int32_t* row_floats);
+int l2h_enroll_capture(const float* chunk_dev, int64_t chunk_row_stride, int64_t chunk_ch_stride, int32_t n, int32_t channels,
+                       int32_t frames, const int32_t* slots_dev, const int32_t* hops_dev, float* state_dev, int32_t n_slots,
+                       int32_t capacity, void* stream);
 
 #ifdef __cplusplus
 }

@@ -202,28 +202,11 @@ static EWs ecarve(int B, int N) {
             return fail(3, std::string(#expr) + ": " + cudaGetErrorString(_e) + " " + _why);       \
     } while (0)
 
-// The shortest utterance: T = 1 + n / HOP >= KS frames for the 4-frame unfold.
-constexpr int MIN_SAMPLES = HOP * (KS - 1);
-
-// x [B][2][N]; utterance b is x[b, :, :lens_host[b]] (lens_host null: every utterance is N long).  Every argument is
-// checked before the committed-weights check and before any device work.
-static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B, int N, const int32_t* lens_host, float* wsp,
-                              size_t ws_bytes, cudaStream_t st) {
-    if (B <= 0) return fail(1, "need batch >= 1");
-    if (N < MIN_SAMPLES) return fail(1, "utterance too short for the 4-frame unfold: need at least 192 samples");
-    bool mixed = false;                        // some utterance shorter than N: the padded-frame path
-    if (lens_host != nullptr)
-        for (int b = 0; b < B; ++b) {
-            if (lens_host[b] < MIN_SAMPLES || lens_host[b] > N)
-                return fail(1, "length " + std::to_string(lens_host[b]) + " of utterance " + std::to_string(b) + " is outside [192, n_max = " +
-                                   std::to_string(N) + "]");
-            mixed |= lens_host[b] != N;
-        }
-    const EWs ws = ecarve(B, N);
+// The checks every forward form makes once its own arguments are checked: the workspace, the batch, the weights and the
+// device; then the kernels' attributes.  Nothing is enqueued.
+static int embed_ready(EmbedEngine* e, int B, const EWs& ws, size_t ws_bytes) {
     if ((size_t)ws.total * sizeof(float) > ws_bytes) return fail(1, "workspace too small");
-    const int T = ws.T, Tp = ws.Tp;
-    const int64_t rows = (int64_t)B * T * NF;
-    if (rows * 2 > 0x7fffffff) return fail(1, "batch too large for one call; split it (l2h_embed_max_batch)");
+    if ((int64_t)B * ws.T * NF * 2 > 0x7fffffff) return fail(1, "batch too large for one call; split it (l2h_embed_max_batch)");
     if (!e->pack.committed) return fail(4, "weights not committed");
     int cur_dev = -1;
     CK(cudaGetDevice(&cur_dev));
@@ -238,6 +221,16 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
         CK(cudaFuncSetAttribute(eattn_out_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)EAOUT_SMEM));
         e->attrs_dev = cur_dev;
     }
+    return 0;
+}
+
+// The chain from the audio (read through xm, estd and efront only) to out [B][256].  lens: the device lengths, or null
+// when every utterance is N long.
+template <class XMap>
+static int embed_chain(EmbedEngine* e, const XMap& xm, const int32_t* lens, float* out, int B, int N, const EWs& ws, float* wsp,
+                       cudaStream_t st) {
+    const int T = ws.T, Tp = ws.Tp;
+    const int64_t rows = (int64_t)B * T * NF;
     float* INV = wsp + ws.INV; double* GN = reinterpret_cast<double*>(wsp + ws.GN);
     float* X = wsp + ws.X; float* GX = wsp + ws.GX; float* HC = wsp + ws.HC;
     float* QKV = wsp + ws.QKV; float* QN = wsp + ws.QN;
@@ -249,16 +242,9 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
     const int passes = e->passes;
     const WeightPack& pk = e->pack;
 
-    // lengths on the device only for a mixed batch; equal lengths run exactly the equal-length path
-    int32_t* lens = nullptr;
-    if (mixed) {
-        lens = reinterpret_cast<int32_t*>(wsp + ws.LENS);
-        CK(launch_eput_lens(st, lens, lens_host, B));
-    }
-
-    CK(launch_estd(st, B, x, N, lens, INV));
+    CK(launch_estd_map(st, B, xm, N, lens, INV));
     CK(cudaMemsetAsync(GN, 0, sizeof(double) * 2 * B, st));
-    CK(launch_efront(st, B, x, N, lens, INV, X, GN, e->w, T));
+    CK(launch_efront_map(st, B, xm, N, lens, INV, X, GN, e->w, T));
     {
         const int64_t per_b = (int64_t)T * NF * CH, total4 = (int64_t)B * per_b / 4;
         CK(launch_egn_apply(st, X, GN, per_b, total4, lens, e->w));
@@ -359,6 +345,73 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
     return 0;
 }
 
+// x [B][2][N]; utterance b is x[b, :, :lens_host[b]] (lens_host null: every utterance is N long).  Every argument is
+// checked before the committed-weights check and before any device work.
+static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B, int N, const int32_t* lens_host, float* wsp,
+                              size_t ws_bytes, cudaStream_t st) {
+    if (B <= 0) return fail(1, "need batch >= 1");
+    if (N < MIN_SAMPLES) return fail(1, "utterance too short for the 4-frame unfold: need at least 192 samples");
+    bool mixed = false;                        // some utterance shorter than N: the padded-frame path
+    if (lens_host != nullptr)
+        for (int b = 0; b < B; ++b) {
+            if (lens_host[b] < MIN_SAMPLES || lens_host[b] > N)
+                return fail(1, "length " + std::to_string(lens_host[b]) + " of utterance " + std::to_string(b) + " is outside [192, n_max = " +
+                                   std::to_string(N) + "]");
+            mixed |= lens_host[b] != N;
+        }
+    const EWs ws = ecarve(B, N);
+    if (int rc = embed_ready(e, B, ws, ws_bytes)) return rc;
+    // lengths on the device only for a mixed batch; equal lengths run exactly the equal-length path
+    int32_t* lens = nullptr;
+    if (mixed) {
+        lens = reinterpret_cast<int32_t*>(wsp + ws.LENS);
+        CK(launch_eput_lens(st, lens, lens_host, B));
+    }
+    return embed_chain(e, XDense{x}, lens, out, B, N, ws, wsp, st);
+}
+
+// Row b embeds the last used[b] = min(lengths_host[b], captured) samples of slot slots[b] of an enrollment capture
+// [n_slots][2][EC_HEAD + capacity], read from the ring in place (XRing), into emb + b * emb_row_stride; a row with
+// used[b] == 0 (under 192 samples captured, or a device slot outside the capture) is left untouched.  Padded to N = n_max
+// with the workspace of l2h_embed_forward_lengths: the slot list XRing reads sits in HD (free until the head's GEMM), the
+// embeddings before their scatter in QKV (free after the last block).
+static int embed_slots_impl(EmbedEngine* e, const float* capture, int n_slots, int capacity, const int32_t* slots_host,
+                            const int32_t* slots_dev, const int32_t* lens_host, int B, int N, float* emb, int64_t emb_row_stride,
+                            int32_t* used, float* wsp, size_t ws_bytes, cudaStream_t st) {
+    if (B <= 0 || n_slots <= 0) return fail(1, "need batch >= 1 and n_slots >= 1");
+    if (B > n_slots) return fail(1, "a call needs batch <= n_slots");
+    if (capacity < MIN_SAMPLES || capacity > INT32_MAX - EC_HEAD)
+        return fail(1, "capture capacity " + std::to_string(capacity) + " cannot hold the 192 samples of the shortest enrollment");
+    if (N < MIN_SAMPLES || N > capacity)
+        return fail(1, "n_max = " + std::to_string(N) + " is outside [192, capacity = " + std::to_string(capacity) + "]");
+    if (emb_row_stride < 256) return fail(1, "emb_row_stride " + std::to_string(emb_row_stride) + " < 256: rows would overlap");
+    for (int b = 0; b < B; ++b)
+        if (lens_host[b] < MIN_SAMPLES || lens_host[b] > N)
+            return fail(1, "length " + std::to_string(lens_host[b]) + " of row " + std::to_string(b) + " is outside [192, n_max = " +
+                               std::to_string(N) + "]");
+    if (slots_host != nullptr) {
+        std::vector<char> seen(n_slots, 0);
+        for (int b = 0; b < B; ++b) {
+            const int s = slots_host[b];
+            if (s < 0 || s >= n_slots)
+                return fail(1, "slot " + std::to_string(s) + " of row " + std::to_string(b) + " is outside the capture's [0, " +
+                                   std::to_string(n_slots) + ")");
+            if (seen[s]) return fail(1, "slot " + std::to_string(s) + " is listed twice");
+            seen[s] = 1;
+        }
+    }
+    const EWs ws = ecarve(B, N);
+    if (int rc = embed_ready(e, B, ws, ws_bytes)) return rc;
+    int32_t* lens = reinterpret_cast<int32_t*>(wsp + ws.LENS);
+    int32_t* slots = reinterpret_cast<int32_t*>(wsp + ws.HD);
+    float* rows = wsp + ws.QKV;
+    const int64_t row_floats = EC_HEAD + (int64_t)capacity;
+    CK(launch_eslot_rows(st, slots_host, slots_dev, lens_host, B, capture, row_floats, n_slots, capacity, slots, lens, used));
+    if (int rc = embed_chain(e, XRing{capture, row_floats, capacity, slots, used}, lens, rows, B, N, ws, wsp, st)) return rc;
+    CK(launch_eput_rows(st, B, rows, emb, emb_row_stride, used));
+    return 0;
+}
+
 }  // namespace l2h
 
 using namespace l2h;
@@ -441,6 +494,16 @@ int l2h_embed_forward_lengths(void* handle, const float* x_dev, int32_t n_max, c
     if (!e || !x_dev || !emb_dev || !ws) return fail(1, "null argument");
     return embed_forward_impl(e, x_dev, emb_dev, batch, n_max, lengths_host, static_cast<float*>(ws), ws_bytes,
                               static_cast<cudaStream_t>(stream));
+}
+
+int l2h_embed_forward_slots(void* handle, const float* capture_dev, int32_t n_slots, int32_t capacity, const int32_t* slots_host,
+                            const int32_t* slots_dev, const int32_t* lengths_host, int32_t batch, int32_t n_max, float* emb_dev,
+                            int64_t emb_row_stride, int32_t* used_dev, void* ws, size_t ws_bytes, void* stream) {
+    EmbedEngine* e = static_cast<EmbedEngine*>(handle);
+    if (!e || !capture_dev || !lengths_host || !emb_dev || !used_dev || !ws) return fail(1, "null argument");
+    if ((slots_host == nullptr) == (slots_dev == nullptr)) return fail(1, "give exactly one of slots_host and slots_dev");
+    return embed_slots_impl(e, capture_dev, n_slots, capacity, slots_host, slots_dev, lengths_host, batch, n_max, emb_dev,
+                            emb_row_stride, used_dev, static_cast<float*>(ws), ws_bytes, static_cast<cudaStream_t>(stream));
 }
 
 int l2h_embed_forward(void* handle, const float* x_dev, float* emb_dev, int32_t batch, int32_t n_samples, void* ws,

@@ -25,6 +25,7 @@
 
 #include "../../include/lookonce_b200.h"
 #include "host_errors.h"
+#include "enroll_capture.cuh"
 
 namespace l2h {
 
@@ -321,6 +322,31 @@ hop_fifo_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, int ma
         st[2] = __int_as_float(n - kept > INT32_MAX - dropped ? INT32_MAX : dropped + (n - kept));
     }
 }
+
+// ---- the enrollment capture: the hops' new samples into a per-slot ring (layout: enroll_capture.cuh) -----------------
+// Row i appends samples EC_CARRY .. EC_CARRY + 128 h - 1 of its chunk (the hops' new samples, no look-ahead repeat) to slot
+// slots[i], h = hops[i]; a slot outside [0, n_slots) or h outside [1, T] stores nothing.  grid n * C, a CTA per (row,
+// channel).
+__global__ void __launch_bounds__(256)
+enroll_capture_kernel(const float* __restrict__ chunk, int64_t c_row, int64_t c_ch, int C, int T,
+                      const int32_t* __restrict__ slots, const int32_t* __restrict__ hops, float* __restrict__ state,
+                      int n_slots, int capacity) {
+    const int row = blockIdx.x / C, ch = blockIdx.x - row * C, tid = threadIdx.x;
+    const int slot = slots[row], h = hops[row];
+    if (slot < 0 || slot >= n_slots || h <= 0 || h > T) return;
+    float* st = state + ((int64_t)slot * C + ch) * (EC_HEAD + capacity);
+    const CaptureRow r = capture_row(state, EC_HEAD + capacity, C, slot, ch, capacity);
+    float* ring = st + EC_HEAD;
+    const int n = h * EC_HOP, skip = n > capacity ? n - capacity : 0;   // only the last `capacity` samples survive
+    const float* src = chunk + (int64_t)row * c_row + (int64_t)ch * c_ch + EC_CARRY;
+    for (int i = skip + tid; i < n; i += blockDim.x) ring[(int)(((int64_t)r.wpos + i) % capacity)] = src[i];
+    __syncthreads();                                                    // every thread has read the head
+    if (tid == 0) {
+        st[0] = __int_as_float((int)(((int64_t)r.wpos + n) % capacity));
+        st[1] = __int_as_float(min(r.captured + n, capacity));
+    }
+}
+
 }  // namespace l2h
 
 extern "C" int l2h_resample(const float* x_dev, int64_t x_row_stride, int32_t n_in, int32_t n_rows, const int32_t* orig_freq,
@@ -497,5 +523,38 @@ extern "C" int l2h_hop_fifo(const float* x_dev, int64_t x_row_stride, int64_t x_
         channels, frames, slots_dev, state_dev, n_slots, capacity);
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(3, std::string("l2h_hop_fifo: ") + cudaGetErrorString(e));
+    return 0;
+}
+
+extern "C" int l2h_enroll_capture_layout(int32_t capacity, int32_t* row_floats) {
+    using namespace l2h;
+    if (!row_floats) return fail(1, "l2h_enroll_capture_layout: null pointer");
+    if (capacity < EC_MIN_CAPACITY || capacity > INT32_MAX - EC_HEAD)
+        return fail(1, "l2h_enroll_capture_layout: capacity " + std::to_string(capacity) + " cannot hold the " +
+                           std::to_string(EC_MIN_CAPACITY) + " samples of the shortest enrollment");
+    *row_floats = EC_HEAD + capacity;
+    return 0;
+}
+
+extern "C" int l2h_enroll_capture(const float* chunk_dev, int64_t chunk_row_stride, int64_t chunk_ch_stride, int32_t n,
+                                  int32_t channels, int32_t frames, const int32_t* slots_dev, const int32_t* hops_dev,
+                                  float* state_dev, int32_t n_slots, int32_t capacity, void* stream) {
+    using namespace l2h;
+    if (!chunk_dev || !slots_dev || !hops_dev || !state_dev) return fail(1, "l2h_enroll_capture: null pointer");
+    if (n <= 0 || channels <= 0 || frames <= 0 || n_slots <= 0)
+        return fail(1, "l2h_enroll_capture: n, channels, frames and n_slots must be positive");
+    if (n > n_slots) return fail(1, "l2h_enroll_capture: a call needs n <= n_slots");
+    if ((int64_t)n * channels > INT32_MAX) return fail(1, "l2h_enroll_capture: n * channels is too large");
+    int32_t row_floats;
+    if (int rc = l2h_enroll_capture_layout(capacity, &row_floats)) return rc;
+    const int64_t c_len = (int64_t)frames * EC_HOP + EC_CARRY;
+    if (c_len > INT32_MAX) return fail(1, "l2h_enroll_capture: frames is too large");
+    if (chunk_ch_stride < c_len || chunk_row_stride / channels < chunk_ch_stride)
+        return fail(1, "l2h_enroll_capture: bad stride: rows and channels of the chunk (" + std::to_string(c_len) +
+                           " samples) must not overlap");
+    enroll_capture_kernel<<<(unsigned)(n * channels), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        chunk_dev, chunk_row_stride, chunk_ch_stride, channels, frames, slots_dev, hops_dev, state_dev, n_slots, capacity);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(3, std::string("l2h_enroll_capture: ") + cudaGetErrorString(e));
     return 0;
 }

@@ -170,6 +170,69 @@ class EmbedTFGridNet(nn.Module):
             out[ii] = oc
         return out
 
+    def enroll(self, capture, slots, lengths, out=None, used=None):
+        """Embed listeners from their own streams: row b is the embedding of the last min(lengths[b], captured) samples
+        that slot slots[b] of `capture` (a 2-channel `EnrollCapture`) holds, read from its ring in place on the caller's
+        stream, with no host copy of the audio and nothing read back.  It equals, bit for bit, ``forward(x, lengths)``
+        of those samples gathered into a batch padded to max(lengths).
+
+        `slots` follows Net.advance_slots: n distinct ints in [0, capture slots) (a sequence or CPU tensor, checked
+        here), or a contiguous CUDA int32 tensor of shape (n,) used in place and read when the kernels run, where an
+        entry outside the capture marks a row that embeds nothing.  `lengths`: n ints in [192, capture.capacity].
+
+        Returns `out` [n, 256] float32: a new tensor, or the one given, which may be a view with any row stride >= 256 --
+        rows of the separator's embedding staging buffer.  A row whose slot captured fewer than 192 samples is not
+        written (NaN in a new tensor), so in the staging buffer that listener keeps its embedding.  `used` (a contiguous
+        CUDA int32 tensor of shape (n,), optional) receives the samples each row used, 0 for a row not written."""
+        from .net import device_list
+        from .render import EnrollCapture
+        if not isinstance(capture, EnrollCapture):
+            raise TypeError("capture must be an EnrollCapture")
+        if capture.channels != self.num_ch:
+            raise ValueError(f"enrollment needs a capture of {self.num_ch} channels, got {capture.channels}")
+        dev = capture.state.device
+        if isinstance(slots, torch.Tensor) and slots.is_cuda:
+            n = slots.shape[0] if slots.dim() == 1 else -1
+            slots = device_list(slots, dev, n, capture.n_slots, True, "slot")
+        else:
+            v = torch.as_tensor(slots)
+            n = v.shape[0] if v.dim() == 1 else -1
+            slots = device_list(v, torch.device("cpu"), n, capture.n_slots, True, "slot").contiguous()
+        if n < 1:
+            raise ValueError("slots must list at least one slot")
+        lens = check_lengths(lengths, n, capture.capacity)
+        if out is None:
+            out = torch.full((n, self.embed_dim), float("nan"), dtype=torch.float32, device=dev)
+        elif (not isinstance(out, torch.Tensor) or out.dtype != torch.float32 or out.device != dev
+              or tuple(out.shape) != (n, self.embed_dim) or out.stride(1) != 1 or out.stride(0) < self.embed_dim):
+            raise ValueError(f"out must be a float32 tensor [{n}, {self.embed_dim}] on {dev} with unit column stride and a "
+                             f"row stride >= {self.embed_dim}")
+        if used is None:
+            used = torch.empty(n, dtype=torch.int32, device=dev)
+        elif (not isinstance(used, torch.Tensor) or used.dtype != torch.int32 or used.device != dev
+              or tuple(used.shape) != (n,) or not used.is_contiguous()):
+            raise ValueError(f"used must be a contiguous int32 tensor of shape ({n},) on {dev}")
+        self._sync_weights(dev)
+        L, h = _cabi.lib(), self._engine()
+        host = not slots.is_cuda
+        n_max = max(lens)
+        per = self.max_batch(n_max)
+        for b0 in range(0, n, per):
+            nb = min(per, n - b0)
+            ws = ctypes.c_size_t()
+            _cabi.check(L.l2h_embed_workspace_bytes(h, nb, n_max, ctypes.byref(ws)))
+            if self._ws is None or self._ws.numel() < ws.value or self._ws.device != dev:
+                self._ws = torch.empty(ws.value, dtype=torch.uint8, device=dev)
+            sl = slots[b0:b0 + nb]
+            sl_host = ctypes.cast(sl.data_ptr(), ctypes.POINTER(ctypes.c_int32)) if host else None
+            with torch.cuda.device(dev):
+                _cabi.check_args(L.l2h_embed_forward_slots(
+                    h, capture.state.data_ptr(), capture.n_slots, capture.capacity, sl_host,
+                    None if host else sl.data_ptr(), (ctypes.c_int32 * nb)(*lens[b0:b0 + nb]), nb, n_max,
+                    out[b0].data_ptr(), out.stride(0), used[b0:].data_ptr(), self._ws.data_ptr(), self._ws.numel(),
+                    torch.cuda.current_stream(dev).cuda_stream))
+        return out
+
 
 MIN_SAMPLES = 192          # 1 + n // 64 >= 4 STFT frames for the 4-frame unfold
 

@@ -6,7 +6,8 @@ multi_ch_simulator.py:49, MixLibriSpeechNoisyEnrollNorm.py:69-75).  The arithmet
 `l2h_resample` (hand-written CUDA); and its streaming form for listeners whose devices run at another rate than the
 separator's 16 kHz (`StreamResampler`, `l2h_resample_stream`), with pushes of any length (`PacketResampler`,
 `l2h_resample_packets`) and the per-slot FIFO that turns them into separator chunks and hop counts (`HopFifo`,
-`l2h_hop_fifo`).  No CPU fallback."""
+`l2h_hop_fifo`); and the per-slot capture that keeps each listener's recent input for enrollment (`EnrollCapture`,
+`l2h_enroll_capture`).  No CPU fallback."""
 import ctypes
 import math
 import numbers
@@ -334,6 +335,60 @@ class HopFifo:
 
     def reset(self, slots):
         """Make the listed slots empty FIFOs with a zero carry; the other slots keep what they hold."""
+        _reset(self.state, slots)
+
+
+class EnrollCapture:
+    """Per-slot capture of each listener's recent 16 kHz input on the device (l2h_enroll_capture), so a "look" can be
+    enrolled from the stream itself (`EmbedTFGridNet.enroll`) with no copy of the audio kept on the host.
+
+    Each call appends the hops' new samples of a row's chunk, samples 64 .. 64 + 128 h - 1 (no look-ahead repeat), to its
+    slot; a slot keeps its last `capacity` samples and counts what it captured since reset, capped at `capacity`
+    (`captured`).  It takes the chunk, slots and hops that `HopFifo` hands `Net.advance_slots`, so it runs in the same
+    tick and the same CUDA graph.
+
+    `state` [slots, channels, 2 + capacity] is a float32 tensor on `device` (two int32 words in its first floats): all
+    zeros is an empty capture, so a listener is reset by zeroing its rows (`reset`) and moved by copying them.  `capacity`
+    must hold the 192 samples of the shortest enrollment."""
+
+    HOP, CARRY = 128, 64
+
+    def __init__(self, slots, channels, capacity, device=None):
+        self.n_slots, self.channels = _whole(slots, "slots"), _whole(channels, "channels")
+        self.capacity = _whole(capacity, "capacity")
+        row = ctypes.c_int32()
+        _cabi.check_args(_cabi.lib().l2h_enroll_capture_layout(self.capacity, ctypes.byref(row)))
+        dev = _cuda_device(device, "EnrollCapture")
+        self.state = torch.zeros(self.n_slots, self.channels, row.value, dtype=torch.float32, device=dev)
+
+    def __call__(self, chunk, slots, hops):
+        """chunk [n, channels, 128 * T + 64] CUDA tensor: row i appends samples 64 .. 64 + 128 * hops[i] - 1 to slot
+        slots[i].  A row whose CUDA slot entry lies outside [0, slots), or whose CUDA hop entry lies outside [1, T],
+        stores nothing.
+
+        `slots` and `hops` follow Net.advance_slots: n distinct ints in [0, slots) and n ints in [0, T] (sequences or CPU
+        tensors, checked and uploaded), or contiguous CUDA int32 tensors of shape (n,) used in place and read when the
+        kernel runs (HopFifo's hops), so a call captured in a CUDA graph serves any lists rewritten in place."""
+        dev = self.state.device
+        chunk = _rows_in(chunk, dev, self.channels, "EnrollCapture")
+        n, C, L = chunk.shape
+        if L < self.HOP + self.CARRY or (L - self.CARRY) % self.HOP:
+            raise ValueError(f"chunk rows must hold 128 * T + 64 samples with T >= 1, got {L}")
+        T = (L - self.CARRY) // self.HOP
+        slots = device_list(slots, dev, n, self.n_slots, True, "slot")
+        hops = device_list(hops, dev, n, T + 1, False, "hop")
+        with torch.cuda.device(dev):
+            _cabi.check_args(_cabi.lib().l2h_enroll_capture(
+                chunk.data_ptr(), chunk.stride(0), chunk.stride(1), n, C, T, slots.data_ptr(), hops.data_ptr(),
+                self.state.data_ptr(), self.n_slots, self.capacity, torch.cuda.current_stream(dev).cuda_stream))
+
+    @property
+    def captured(self):
+        """[slots] int32 CUDA view of the state: the samples each slot captured since its reset, capped at capacity"""
+        return self.state[:, 0, 1].view(torch.int32)
+
+    def reset(self, slots):
+        """Make the listed slots empty captures; the other slots keep what they hold."""
         _reset(self.state, slots)
 
 
