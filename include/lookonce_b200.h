@@ -438,6 +438,28 @@ int l2h_embed_forward_lengths(void* handle, const float* x_dev, int32_t n_max, c
 int l2h_embed_forward_slots(void* handle, const float* capture_dev, int32_t n_slots, int32_t capacity, const int32_t* slots_host,
                             const int32_t* slots_dev, const int32_t* lengths_host, int32_t batch, int32_t n_max, float* emb_dev,
                             int64_t emb_row_stride, int32_t* used_dev, void* workspace_dev, size_t workspace_bytes, void* stream);
+/* Enrollment from a capture in slices: l2h_embed_forward_slots cut into an ordered plan of units, each one stage of one or
+ * a few kernel launches, so a service can put a bounded amount of enrollment work between its ticks.  *units receives the
+ * number of units of the plan for (batch, n_max, window): 2 + num_blocks * (8 + w), where w = ceil((1 + n_max / 64 - 3) /
+ * window) windows of the inter-frame recurrence, or w = 1 for window = 0 or a window at least that long.  Error 1: a null
+ * pointer, batch <= 0, n_max < 192 or window < 0. */
+int l2h_embed_slots_units(void* handle, int32_t batch, int32_t n_max, int32_t window, int32_t* units);
+/* Enqueues units [first_unit, first_unit + n_units) of that plan on `stream`.  The other arguments are those of
+ * l2h_embed_forward_slots, and all units run in one call equal it, bit for bit, for every window.
+ *   - Every unit runs exactly once, in order; every call passes the same arguments and the same workspace.
+ *   - Between calls the stream may run any work that does not touch that workspace, emb_dev rows or used_dev: ticks that
+ *     keep writing the capture and ticks that read the staging rows emb_dev points into included.  The embedding is that
+ *     of the samples the capture held when unit 0 ran.
+ *   - used_dev is final after unit 0.  emb_dev rows are written by the last unit only: until then a listener keeps the
+ *     embedding it had.
+ *   - The workspace is l2h_embed_workspace_bytes(batch, n_max), as for l2h_embed_forward_slots: the (h, c) the windows of
+ *     the recurrence carry live in it.
+ * Errors, returned before anything is enqueued: every error of l2h_embed_forward_slots (host slot lists are checked on
+ * every call), and 1 = window < 0, n_units < 1, or a unit range outside the plan.  Asynchronous on `stream`. */
+int l2h_embed_forward_slots_units(void* handle, const float* capture_dev, int32_t n_slots, int32_t capacity,
+                                  const int32_t* slots_host, const int32_t* slots_dev, const int32_t* lengths_host, int32_t batch,
+                                  int32_t n_max, float* emb_dev, int64_t emb_row_stride, int32_t* used_dev, void* workspace_dev,
+                                  size_t workspace_bytes, int32_t window, int32_t first_unit, int32_t n_units, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Evaluation epilogue on the device (replaces the CPU metric code after `outputs.cpu()` in

@@ -168,6 +168,14 @@ _SIGS = {
                                               ctypes.POINTER(ctypes.c_int32), ctypes.c_void_p, ctypes.POINTER(ctypes.c_int32),
                                               ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
                                               ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
+    "l2h_embed_slots_units": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
+                                            ctypes.POINTER(ctypes.c_int32)]),
+    "l2h_embed_forward_slots_units": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
+                                                    ctypes.POINTER(ctypes.c_int32), ctypes.c_void_p,
+                                                    ctypes.POINTER(ctypes.c_int32), ctypes.c_int32, ctypes.c_int32,
+                                                    ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p,
+                                                    ctypes.c_size_t, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
+                                                    ctypes.c_void_p]),
 }
 
 

@@ -224,11 +224,33 @@ static int embed_ready(EmbedEngine* e, int B, const EWs& ws, size_t ws_bytes) {
     return 0;
 }
 
+// The unit plan: the chain below as an ordered list of units, each one stage of one or a few launches, so that a caller
+// can enqueue it in pieces (l2h_embed_forward_slots_units).  In order:
+//   unit 0          [eslot_rows,] estd, the GroupNorm memset, efront, egn_apply: the only unit that reads the audio
+//   per block       intra: W_ih GEMM | recurrence | ConvTranspose + residual GEMM
+//                   inter: W_ih GEMM (+ einter_mask) | the recurrence in windows | ConvTranspose + residual GEMM
+//                   attention: Q|K|V GEMM + eqkv_ln | S GEMM + softmax_rows | P.V GEMM + eattn_out
+//   last unit       head GEMM, ehead[, eput_rows]: the only unit that writes the embeddings
+// The inter recurrence runs `window` steps per unit (forward steps [kW, (k+1)W) and the reverse direction over the
+// mirrored range), with each direction's (h, c) carried between units in fp32 in QKV, which is free from the block's
+// previous attention to its own Q|K|V GEMM.  window = 0, or one at least as long as the recurrence, makes the whole
+// recurrence one unit: the launch of the unsliced chain.
+static int inter_windows(int steps, int window) { return (window <= 0 || window >= steps) ? 1 : (steps + window - 1) / window; }
+static int embed_units(int n_blocks, int T, int window) { return 2 + n_blocks * (8 + inter_windows(T - KS + 1, window)); }
+
+// Which units of the plan a call enqueues: take() is called once per unit, in plan order.
+struct Units {
+    int first = 0, end = INT32_MAX;     // [first, end)
+    int window = 0;
+    int next = 0;
+    bool take() { const int u = next++; return u >= first && u < end; }
+};
+
 // The chain from the audio (read through xm, estd and efront only) to out [B][256].  lens: the device lengths, or null
-// when every utterance is N long.
+// when every utterance is N long.  Enqueues the units of `u` only.
 template <class XMap>
 static int embed_chain(EmbedEngine* e, const XMap& xm, const int32_t* lens, float* out, int B, int N, const EWs& ws, float* wsp,
-                       cudaStream_t st) {
+                       cudaStream_t st, Units u = Units{}) {
     const int T = ws.T, Tp = ws.Tp;
     const int64_t rows = (int64_t)B * T * NF;
     float* INV = wsp + ws.INV; double* GN = reinterpret_cast<double*>(wsp + ws.GN);
@@ -242,10 +264,10 @@ static int embed_chain(EmbedEngine* e, const XMap& xm, const int32_t* lens, floa
     const int passes = e->passes;
     const WeightPack& pk = e->pack;
 
-    CK(launch_estd_map(st, B, xm, N, lens, INV));
-    CK(cudaMemsetAsync(GN, 0, sizeof(double) * 2 * B, st));
-    CK(launch_efront_map(st, B, xm, N, lens, INV, X, GN, e->w, T));
-    {
+    if (u.take()) {
+        CK(launch_estd_map(st, B, xm, N, lens, INV));
+        CK(cudaMemsetAsync(GN, 0, sizeof(double) * 2 * B, st));
+        CK(launch_efront_map(st, B, xm, N, lens, INV, X, GN, e->w, T));
         const int64_t per_b = (int64_t)T * NF * CH, total4 = (int64_t)B * per_b / 4;
         CK(launch_egn_apply(st, X, GN, per_b, total4, lens, e->w));
     }
@@ -273,15 +295,44 @@ static int embed_chain(EmbedEngine* e, const XMap& xm, const int32_t* lens, floa
             g.rows_per_seq = steps; g.nseq = nseq;
             g.b = pk.bplanes(inter ? PL.ih2 : PL.ih1, 256); g.N = 512; g.K = 256; g.passes = passes;
             g.bias = inter ? W.b2 : W.b1; g.C = GX; g.ldc = 512; g.c_seq_stride = (int64_t)steps * 512;
-            CKU(umma::launch(g, st, &_why));
-            // windows past an utterance's own frames: zero state, zero h
-            if (inter && lens != nullptr) CK(launch_einter_mask(st, B, GX, lens, steps));
+            if (u.take()) {
+                CKU(umma::launch(g, st, &_why));
+                // windows past an utterance's own frames: zero state, zero h
+                if (inter && lens != nullptr) CK(launch_einter_mask(st, B, GX, lens, steps));
+            }
             LstmArgs l{};
             l.gx = GX; l.gx_ld = 512; l.out = HC; l.out_ld = 128; l.whh = inter ? W.whh2 : W.whh1;
             l.nseq = nseq; l.L = steps; l.inner_count = 1; l.outer_stride = steps; l.inner_stride = 0; l.step_stride = 1;
             l.ndir = 2;
-            if ((int64_t)l.nseq * l.ndir >= e->tcl_min_seqdirs) CK(launch_tc_lstm(l, passes, st));   // many sequences: recurrence on the tensor cores
-            else CK(launch_lstm_rec(l, st));
+            const bool tc = (int64_t)l.nseq * l.ndir >= e->tcl_min_seqdirs;   // many sequences: recurrence on the tensor cores
+            const int n_win = inter ? inter_windows(steps, u.window) : 1;
+            if (n_win == 1) {
+                if (u.take()) {
+                    if (tc) CK(launch_tc_lstm(l, passes, st));
+                    else CK(launch_lstm_rec(l, st));
+                }
+            } else {
+                // Window k: each direction as its own one-direction launch of the kernel (and variant) the whole
+                // recurrence takes, so every step computes what it computes there.  The reverse direction is run as
+                // a forward one over rows that step backwards from the window's last position.
+                const LstmRec v = lstm_rec_variant(l, l.nseq);
+                float* hc_state = QKV;                          // [dir][h | c][nseq][64]
+                const int64_t hc_plane = (int64_t)nseq * 64;
+                for (int k = 0; k < n_win; ++k) {
+                    if (!u.take()) continue;
+                    if (k == 0) CK(cudaMemsetAsync(hc_state, 0, sizeof(float) * 4 * hc_plane, st));
+                    const int s0 = k * u.window, len = std::min(u.window, steps - s0);
+                    for (int dir = 0; dir < 2; ++dir) {
+                        LstmArgs d = l;
+                        const int64_t row0 = dir == 0 ? s0 : steps - 1 - s0;
+                        d.ndir = 1; d.L = len; d.step_stride = dir == 0 ? 1 : -1;
+                        d.gx = GX + row0 * 512 + dir * 256; d.out = HC + row0 * 128 + dir * 64; d.whh = l.whh + dir * 256 * 64;
+                        d.h_state = hc_state + 2 * dir * hc_plane; d.c_state = d.h_state + hc_plane; d.hc_outer_stride = 64;
+                        if (tc) CK(launch_tc_lstm(d, passes, st));
+                        else CK(launch_lstm_variant(v, d, st, false));
+                    }
+                }
+            }
             // ---- ConvTranspose1d(128->64, k=4) + residual: output position p reads h rows p-3 .. p; rows outside the
             // sequence are the zero-filled halo of the tensor map ----------------------------------------------------
             umma::GemmDesc c;
@@ -295,10 +346,10 @@ static int embed_chain(EmbedEngine* e, const XMap& xm, const int32_t* lens, floa
             c.bias = inter ? W.bl2 : W.bl1; c.C = X; c.R = X;
             if (!inter) { c.ldc = 64; c.c_seq_stride = (int64_t)NF * 64; }                 // row ((b,t), f) -> X[b][t][f]
             else { c.ldc = (int64_t)NF * 64; c.c_inner = NF; c.c_seq_stride = (int64_t)T * NF * 64; c.c_inner_stride = 64; }   // ((b,f), t)
-            CKU(umma::launch(c, st, &_why));
+            if (u.take()) CKU(umma::launch(c, st, &_why));
         }
         // ---- full self-attention over frames ------------------------------------------------
-        {
+        if (u.take()) {
             umma::GemmDesc g;                          // Q|K|V 1x1 convs of all heads + PReLU
             g.a0.base = X; g.a0.channels = 64; g.a0.n_pos = rows; g.a0.pos_stride = 64;
             umma::set_plain_chunks(g, 64);
@@ -306,9 +357,9 @@ static int embed_chain(EmbedEngine* e, const XMap& xm, const int32_t* lens, floa
             g.b = pk.bplanes(PL.qkv, 64); g.N = NQKV; g.K = 64; g.passes = passes;
             g.bias = W.bqkv; g.prelu_vec = W.slope_qkv; g.C = QKV; g.ldc = NQKV; g.c_seq_stride = 0;
             CKU(umma::launch(g, st, &_why));
+            CK(launch_eqkv_ln(st, B, QKV, QN, KP, VP, k_plane, v_plane, W, T, Tp));
         }
-        CK(launch_eqkv_ln(st, B, QKV, QN, KP, VP, k_plane, v_plane, W, T, Tp));
-        {
+        if (u.take()) {
             umma::GemmDesc g;                          // S = Q K^T / sqrt(520), per (utterance, head)
             g.a0.base = QN; g.a0.channels = QK; g.a0.n_pos = T; g.a0.pos_stride = QK; g.a0.n_inner = Z; g.a0.inner_stride = (int64_t)Tp * QK;
             umma::set_plain_chunks(g, QK);
@@ -317,9 +368,9 @@ static int embed_chain(EmbedEngine* e, const XMap& xm, const int32_t* lens, floa
             g.N = T; g.K = QK; g.passes = passes; g.alpha = 1.f / sqrtf((float)QK);
             g.C = S; g.ldc = Tp; g.c_seq_stride = (int64_t)T * Tp;
             CKU(umma::launch(g, st, &_why));
+            CK(launch_softmax_rows(st, Z, S, Tp, T, T, (int64_t)T * Tp, lens));
         }
-        CK(launch_softmax_rows(st, Z, S, Tp, T, T, (int64_t)T * Tp, lens));
-        {
+        if (u.take()) {
             umma::GemmDesc g;                          // O = P V (V is the MN-major B operand: [frame][f*16+c])
             g.a0.base = S; g.a0.channels = T; g.a0.n_pos = T; g.a0.pos_stride = Tp; g.a0.n_inner = Z; g.a0.inner_stride = (int64_t)T * Tp;
             umma::set_plain_chunks(g, T);
@@ -328,11 +379,11 @@ static int embed_chain(EmbedEngine* e, const XMap& xm, const int32_t* lens, floa
             g.N = VDIM; g.K = T; g.passes = passes;
             g.C = O; g.ldc = VDIM; g.c_seq_stride = (int64_t)Tp * VDIM;
             CKU(umma::launch(g, st, &_why));
+            CK(launch_eattn_out(st, eattn_out_ctas(T, B), O, X, W, T, Tp, T * B));
         }
-        CK(launch_eattn_out(st, eattn_out_ctas(T, B), O, X, W, T, Tp, T * B));
     }
     // ---- head: Linear(4160 -> 256) over rows (b,t) [features f*64+c], LN, mean over T -----------
-    {
+    if (u.take()) {
         umma::GemmDesc g;
         g.a0.base = X; g.a0.channels = FC; g.a0.n_pos = (int64_t)B * T; g.a0.pos_stride = FC;
         umma::set_plain_chunks(g, FC);
@@ -340,8 +391,9 @@ static int embed_chain(EmbedEngine* e, const XMap& xm, const int32_t* lens, floa
         g.b = pk.bplanes(e->head_plane, FC); g.N = 256; g.K = FC; g.passes = passes;
         g.bias = e->w.bh; g.C = HD; g.ldc = 256;
         CKU(umma::launch(g, st, &_why));
+        CK(launch_ehead(st, B, HD, out, e->w, T, lens));
     }
-    CK(launch_ehead(st, B, HD, out, e->w, T, lens));
+    if (u.next != embed_units(e->n_blocks, T, u.window)) return fail(3, "enrollment unit plan out of step with its count");
     return 0;
 }
 
@@ -374,10 +426,12 @@ static int embed_forward_impl(EmbedEngine* e, const float* x, float* out, int B,
 // [n_slots][2][EC_HEAD + capacity], read from the ring in place (XRing), into emb + b * emb_row_stride; a row with
 // used[b] == 0 (under 192 samples captured, or a device slot outside the capture) is left untouched.  Padded to N = n_max
 // with the workspace of l2h_embed_forward_lengths: the slot list XRing reads sits in HD (free until the head's GEMM), the
-// embeddings before their scatter in QKV (free after the last block).
+// embeddings before their scatter in QKV (free after the last block).  Enqueues units [first_unit, first_unit + n_units) of
+// the plan for `window` (embed_units); n_units < 0: all of them.
 static int embed_slots_impl(EmbedEngine* e, const float* capture, int n_slots, int capacity, const int32_t* slots_host,
                             const int32_t* slots_dev, const int32_t* lens_host, int B, int N, float* emb, int64_t emb_row_stride,
-                            int32_t* used, float* wsp, size_t ws_bytes, cudaStream_t st) {
+                            int32_t* used, float* wsp, size_t ws_bytes, cudaStream_t st, int window = 0, int first_unit = 0,
+                            int n_units = -1) {
     if (B <= 0 || n_slots <= 0) return fail(1, "need batch >= 1 and n_slots >= 1");
     if (B > n_slots) return fail(1, "a call needs batch <= n_slots");
     if (capacity < MIN_SAMPLES || capacity > INT32_MAX - EC_HEAD)
@@ -401,14 +455,24 @@ static int embed_slots_impl(EmbedEngine* e, const float* capture, int n_slots, i
         }
     }
     const EWs ws = ecarve(B, N);
+    const int total = embed_units(e->n_blocks, ws.T, window);
+    if (n_units < 0) n_units = total;
+    if (window < 0) return fail(1, "window " + std::to_string(window) + " < 0");
+    if (first_unit < 0 || n_units < 1 || first_unit > total - n_units)
+        return fail(1, "units [" + std::to_string(first_unit) + ", " + std::to_string((int64_t)first_unit + n_units) +
+                           ") are outside the plan's [0, " + std::to_string(total) + ")");
     if (int rc = embed_ready(e, B, ws, ws_bytes)) return rc;
     int32_t* lens = reinterpret_cast<int32_t*>(wsp + ws.LENS);
     int32_t* slots = reinterpret_cast<int32_t*>(wsp + ws.HD);
     float* rows = wsp + ws.QKV;
     const int64_t row_floats = EC_HEAD + (int64_t)capacity;
-    CK(launch_eslot_rows(st, slots_host, slots_dev, lens_host, B, capture, row_floats, n_slots, capacity, slots, lens, used));
-    if (int rc = embed_chain(e, XRing{capture, row_floats, capacity, slots, used}, lens, rows, B, N, ws, wsp, st)) return rc;
-    CK(launch_eput_rows(st, B, rows, emb, emb_row_stride, used));
+    Units u;
+    u.first = first_unit; u.end = first_unit + n_units; u.window = window;
+    if (u.first == 0)      // unit 0 also lists the rows
+        CK(launch_eslot_rows(st, slots_host, slots_dev, lens_host, B, capture, row_floats, n_slots, capacity, slots, lens, used));
+    if (int rc = embed_chain(e, XRing{capture, row_floats, capacity, slots, used}, lens, rows, B, N, ws, wsp, st, u)) return rc;
+    if (u.end == total)    // the last unit also scatters the embeddings
+        CK(launch_eput_rows(st, B, rows, emb, emb_row_stride, used));
     return 0;
 }
 
@@ -504,6 +568,26 @@ int l2h_embed_forward_slots(void* handle, const float* capture_dev, int32_t n_sl
     if ((slots_host == nullptr) == (slots_dev == nullptr)) return fail(1, "give exactly one of slots_host and slots_dev");
     return embed_slots_impl(e, capture_dev, n_slots, capacity, slots_host, slots_dev, lengths_host, batch, n_max, emb_dev,
                             emb_row_stride, used_dev, static_cast<float*>(ws), ws_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int l2h_embed_slots_units(void* handle, int32_t batch, int32_t n_max, int32_t window, int32_t* units) {
+    EmbedEngine* e = static_cast<EmbedEngine*>(handle);
+    if (!e || !units || batch <= 0 || n_max < emb::MIN_SAMPLES || window < 0) return fail(1, "bad argument");
+    *units = embed_units(e->n_blocks, 1 + n_max / emb::HOP, window);
+    return 0;
+}
+
+int l2h_embed_forward_slots_units(void* handle, const float* capture_dev, int32_t n_slots, int32_t capacity,
+                                  const int32_t* slots_host, const int32_t* slots_dev, const int32_t* lengths_host, int32_t batch,
+                                  int32_t n_max, float* emb_dev, int64_t emb_row_stride, int32_t* used_dev, void* ws,
+                                  size_t ws_bytes, int32_t window, int32_t first_unit, int32_t n_units, void* stream) {
+    EmbedEngine* e = static_cast<EmbedEngine*>(handle);
+    if (!e || !capture_dev || !lengths_host || !emb_dev || !used_dev || !ws) return fail(1, "null argument");
+    if ((slots_host == nullptr) == (slots_dev == nullptr)) return fail(1, "give exactly one of slots_host and slots_dev");
+    if (n_units < 1) return fail(1, "n_units " + std::to_string(n_units) + " < 1");
+    return embed_slots_impl(e, capture_dev, n_slots, capacity, slots_host, slots_dev, lengths_host, batch, n_max, emb_dev,
+                            emb_row_stride, used_dev, static_cast<float*>(ws), ws_bytes, static_cast<cudaStream_t>(stream), window,
+                            first_unit, n_units);
 }
 
 int l2h_embed_forward(void* handle, const float* x_dev, float* emb_dev, int32_t batch, int32_t n_samples, void* ws,

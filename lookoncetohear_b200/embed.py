@@ -184,6 +184,46 @@ class EmbedTFGridNet(nn.Module):
         rows of the separator's embedding staging buffer.  A row whose slot captured fewer than 192 samples is not
         written (NaN in a new tensor), so in the staging buffer that listener keeps its embedding.  `used` (a contiguous
         CUDA int32 tensor of shape (n,), optional) receives the samples each row used, 0 for a row not written."""
+        dev, slots, n, lens, out, used = self._enroll_args(capture, slots, lengths, out, used)
+        L, h = _cabi.lib(), self._engine()
+        host = not slots.is_cuda
+        n_max = max(lens)
+        per = self.max_batch(n_max)
+        for b0 in range(0, n, per):
+            nb = min(per, n - b0)
+            ws = ctypes.c_size_t()
+            _cabi.check(L.l2h_embed_workspace_bytes(h, nb, n_max, ctypes.byref(ws)))
+            if self._ws is None or self._ws.numel() < ws.value or self._ws.device != dev:
+                self._ws = torch.empty(ws.value, dtype=torch.uint8, device=dev)
+            sl = slots[b0:b0 + nb]
+            sl_host = ctypes.cast(sl.data_ptr(), ctypes.POINTER(ctypes.c_int32)) if host else None
+            with torch.cuda.device(dev):
+                _cabi.check_args(L.l2h_embed_forward_slots(
+                    h, capture.state.data_ptr(), capture.n_slots, capture.capacity, sl_host,
+                    None if host else sl.data_ptr(), (ctypes.c_int32 * nb)(*lens[b0:b0 + nb]), nb, n_max,
+                    out[b0].data_ptr(), out.stride(0), used[b0:].data_ptr(), self._ws.data_ptr(), self._ws.numel(),
+                    torch.cuda.current_stream(dev).cuda_stream))
+        return out
+
+    def enroll_job(self, capture, slots, lengths, out=None, used=None, window=None):
+        """``enroll`` in slices: returns an `EnrollJob` whose ``step(n)`` enqueues the next n units of the enrollment on
+        the current stream, so a service can put a bounded amount of enrollment work between its ticks.  Arguments,
+        checks and results are those of ``enroll``, bit for bit, whatever the window and however the units are stepped.
+
+        The inter-frame recurrence, the one stage whose length grows with the utterance, runs `window` steps per unit
+        (default `DEFAULT_WINDOW`, 0: the whole recurrence is one unit).  The job owns its workspace and keeps its tensors
+        alive, so ``enroll``, ``forward`` and other jobs may run between its steps, as may ticks that keep writing the
+        capture: the embedding is that of the samples held when the first unit ran.  `used` is final after the first unit
+        of each ``max_batch`` cut; `out` rows are written by the last unit of their cut only."""
+        if window is None:
+            window = DEFAULT_WINDOW
+        if isinstance(window, bool) or not isinstance(window, numbers.Integral) or window < 0:
+            raise ValueError(f"window must be an int >= 0, got {window!r}")
+        dev, slots, n, lens, out, used = self._enroll_args(capture, slots, lengths, out, used)
+        return EnrollJob(self, capture, dev, slots, n, lens, out, used, int(window))
+
+    def _enroll_args(self, capture, slots, lengths, out, used):
+        """The checks of ``enroll``: (device, slot list tensor, n, lengths, out, used), the weights committed."""
         from .net import device_list
         from .render import EnrollCapture
         if not isinstance(capture, EnrollCapture):
@@ -213,28 +253,75 @@ class EmbedTFGridNet(nn.Module):
               or tuple(used.shape) != (n,) or not used.is_contiguous()):
             raise ValueError(f"used must be a contiguous int32 tensor of shape ({n},) on {dev}")
         self._sync_weights(dev)
-        L, h = _cabi.lib(), self._engine()
-        host = not slots.is_cuda
-        n_max = max(lens)
-        per = self.max_batch(n_max)
+        return dev, slots, n, lens, out, used
+
+
+# Inter-recurrence steps per unit of an EnrollJob: 0, the whole recurrence as one unit.  Measured at 5 s (DESIGN.md
+# section 7, tools/bench_enroll_slices.py), that unit is at most 7 % (8 listeners) to 25 % (1 listener) longer than the
+# largest GEMM unit, which no window splits, while windows cost 7-39 % more device time in all.
+DEFAULT_WINDOW = 0
+
+
+class EnrollJob:
+    """An enrollment enqueued in slices (``EmbedTFGridNet.enroll_job``).  ``units``: the units of the whole job (those of
+    every ``max_batch`` cut, run one cut after another); ``done``: whether all were enqueued; ``step(n=1)`` enqueues the
+    next n units on the current stream; ``run()`` enqueues the rest.  ``out`` and ``used`` are the tensors ``enroll``
+    would return and fill."""
+
+    def __init__(self, net, capture, dev, slots, n, lens, out, used, window):
+        L, h = _cabi.lib(), net._engine()
+        self.net, self.capture, self.dev, self.window = net, capture, dev, window
+        self.slots, self.lens, self.out, self.used = slots, lens, out, used
+        self._host = not slots.is_cuda
+        self.n_max = max(lens)
+        per = net.max_batch(self.n_max)
+        self._cuts = []                                    # (first row, rows, units)
         for b0 in range(0, n, per):
             nb = min(per, n - b0)
-            ws = ctypes.c_size_t()
-            _cabi.check(L.l2h_embed_workspace_bytes(h, nb, n_max, ctypes.byref(ws)))
-            if self._ws is None or self._ws.numel() < ws.value or self._ws.device != dev:
-                self._ws = torch.empty(ws.value, dtype=torch.uint8, device=dev)
-            sl = slots[b0:b0 + nb]
-            sl_host = ctypes.cast(sl.data_ptr(), ctypes.POINTER(ctypes.c_int32)) if host else None
-            with torch.cuda.device(dev):
-                _cabi.check_args(L.l2h_embed_forward_slots(
-                    h, capture.state.data_ptr(), capture.n_slots, capture.capacity, sl_host,
-                    None if host else sl.data_ptr(), (ctypes.c_int32 * nb)(*lens[b0:b0 + nb]), nb, n_max,
-                    out[b0].data_ptr(), out.stride(0), used[b0:].data_ptr(), self._ws.data_ptr(), self._ws.numel(),
-                    torch.cuda.current_stream(dev).cuda_stream))
-        return out
+            u = ctypes.c_int32()
+            _cabi.check_args(L.l2h_embed_slots_units(h, nb, self.n_max, window, ctypes.byref(u)))
+            self._cuts.append((b0, nb, u.value))
+        ws = ctypes.c_size_t()
+        _cabi.check(L.l2h_embed_workspace_bytes(h, self._cuts[0][1], self.n_max, ctypes.byref(ws)))
+        self._ws = torch.empty(ws.value, dtype=torch.uint8, device=dev)    # the job's own: shared by its cuts in turn
+        self.units = sum(c[2] for c in self._cuts)
+        self._next = 0
+
+    @property
+    def done(self):
+        return self._next >= self.units
+
+    def step(self, n=1):
+        """Enqueue the next n units (fewer if fewer remain) on the current stream; returns how many were enqueued."""
+        if isinstance(n, bool) or not isinstance(n, numbers.Integral) or n < 1:
+            raise ValueError(f"n must be an int >= 1, got {n!r}")
+        L, h = _cabi.lib(), self.net._engine()
+        end = min(self.units, self._next + int(n))
+        start, base = self._next, 0
+        for b0, nb, units in self._cuts:
+            lo, hi = max(start, base), min(end, base + units)
+            if lo < hi:
+                sl = self.slots[b0:b0 + nb]
+                sl_host = ctypes.cast(sl.data_ptr(), ctypes.POINTER(ctypes.c_int32)) if self._host else None
+                with torch.cuda.device(self.dev):
+                    _cabi.check_args(L.l2h_embed_forward_slots_units(
+                        h, self.capture.state.data_ptr(), self.capture.n_slots, self.capture.capacity, sl_host,
+                        None if self._host else sl.data_ptr(), (ctypes.c_int32 * nb)(*self.lens[b0:b0 + nb]), nb,
+                        self.n_max, self.out[b0].data_ptr(), self.out.stride(0), self.used[b0:].data_ptr(),
+                        self._ws.data_ptr(), self._ws.numel(), self.window, lo - base, hi - lo,
+                        torch.cuda.current_stream(self.dev).cuda_stream))
+                self._next = hi
+            base += units
+        return end - start
+
+    def run(self):
+        """Enqueue every unit not yet enqueued; returns ``out``."""
+        if not self.done:
+            self.step(self.units - self._next)
+        return self.out
 
 
-MIN_SAMPLES = 192          # 1 + n // 64 >= 4 STFT frames for the 4-frame unfold
+MIN_SAMPLES = 192         # 1 + n // 64 >= 4 STFT frames for the 4-frame unfold
 
 
 def check_lengths(lengths, batch, n_max):
