@@ -16,7 +16,8 @@ include/lookonce_b200.h); importing this package never falls back to PyTorch mat
 """
 from .embed import EmbedTFGridNet, EnrollJob  # noqa: F401
 from .net import Net, SepState  # noqa: F401
-from .render import EnrollCapture, HopFifo, PacketResampler, StreamResampler, resample  # noqa: F401
+from .render import resample  # noqa: F401
+from .stream import EnrollCapture, HopFifo, PacketResampler, StreamResampler  # noqa: F401
 
 __all__ = ["Net", "SepState", "EmbedTFGridNet", "resample", "StreamResampler", "PacketResampler", "HopFifo",
            "EnrollCapture", "EnrollJob"]

@@ -15,17 +15,24 @@
 // their own `orig`: a launch takes, as its kernel parameter, a table of up to RS_MAX_RATES distinct rates and up to
 // RS_MAX_RUNS runs of consecutive rows with the same rate (no per-row table in device memory); a CTA finds its row's
 // run by binary search.
+//
+// The file also holds the per-slot stages of the serving front end, which share one scaffold (slot_row, slot_call):
+// the streaming resamplers (pushes of whole periods, resample_stream_kernel; pushes of any length,
+// resample_packets_kernel), the hop FIFO that turns 16 kHz pieces into separator chunks (hop_fifo_kernel) and the
+// enrollment capture (enroll_capture_kernel).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include <algorithm>
 #include <cmath>
+#include <initializer_list>
 #include <numeric>
 #include <string>
 
 #include "../../include/lookonce_b200.h"
 #include "host_errors.h"
 #include "enroll_capture.cuh"
+#include "sep_layout.h"
 
 namespace l2h {
 
@@ -36,6 +43,7 @@ constexpr int RS_MAX_ROWS = 65535;        // rows per launch (grid.y)
 constexpr int RS_SMEM_BYTES = 48 * 1024;  // staged input window per CTA
 constexpr int RS_WIDTH = 6;               // zero crossings of the sinc on each side (lowpass_filter_width)
 constexpr double RS_ROLLOFF = 0.99;
+static_assert(CHUNK_HOP == HOP && CHUNK_CARRY == LOOKAHEAD, "the FIFO and the capture cut the separator's chunks");
 
 struct RsRate {
     int32_t o, q;   // reduced rates; o == q (== 1): the row is copied
@@ -75,7 +83,7 @@ static RsRate rs_rate(int32_t orig, int32_t new_freq, int32_t n_in) {
     g.o = orig / gd;
     g.q = new_freq / gd;
     const double base = std::min(g.o, g.q) * RS_ROLLOFF;
-    g.w = (int32_t)std::ceil(RS_WIDTH * (double)g.o / base);
+    g.w = (int32_t)std::min(std::ceil(RS_WIDTH * (double)g.o / base), (double)INT32_MAX);   // refused by the size checks
     g.n_out = (int32_t)(((int64_t)new_freq * n_in + orig - 1) / orig);
     g.scale = (float)(base / g.o);
     g.du = base / g.o;
@@ -121,6 +129,38 @@ resample_kernel(const float* __restrict__ x, int64_t x_stride, int n_in, float* 
     yr[m] = acc;
 }
 
+// ---- the per-slot scaffold -------------------------------------------------------------------------------------------
+// A per-slot stage keeps a state [n_slots][C][row_floats], all zeros for a fresh slot, and runs one CTA per (call row,
+// channel).  The slot list is read on the device, and a row whose slot lies outside the state stores nothing.
+struct SlotRow {
+    int row, ch;
+    bool live;   // the row's slot lies inside the state
+    float* st;   // its state row of channel ch (when live)
+};
+
+L2H_DEVINL SlotRow slot_row(int C, const int32_t* slots, int n_slots, float* state, int64_t row_floats) {
+    const int row = blockIdx.x / C, ch = blockIdx.x - row * C, slot = slots[row];
+    return {row, ch, !(slot < 0 || slot >= n_slots), state + ((int64_t)slot * C + ch) * row_floats};
+}
+
+// row `row`, channel `ch` of a strided [n][C][*] tensor
+template <class T>
+L2H_DEVINL T* row_ch(T* p, int64_t row_stride, int64_t ch_stride, int row, int ch) {
+    return p + (int64_t)row * row_stride + (int64_t)ch * ch_stride;
+}
+
+// a count word of a state row, stored as a float, clamped into [0, hi]
+L2H_DEVINL int clamp_word(float v, int hi) { return v >= (float)hi ? hi : (v > 0.f ? (int)v : 0); }
+
+// Sample jd + D of the delayed output z' below: zero before z's start (!started), else rs_output at input c = floor(jd o /
+// q), which sits at win[origin + c].
+L2H_DEVINL float rs_delayed(const float* win, int origin, int64_t jd, bool started, const RsRate& g) {
+    if (!started) return 0.f;
+    const int64_t a = jd * g.o;
+    const int64_t c = a >= 0 ? a / g.q : -((-a + g.q - 1) / g.q);       // floor(a / q)
+    return rs_output(win + (origin + c - g.w), a - c * g.q, g);
+}
+
 // ---- streaming: per-slot state, pushes of `block` input samples ------------------------------------------------------
 // A stream's output is the whole-signal output z of everything it was pushed, delayed by D = floor(w q / o) samples
 // (z'[j] = z[j - D], zero before z's start): after k pushes exactly the k * out_block - D samples of z whose taps have all
@@ -142,54 +182,56 @@ resample_stream_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch,
                        int64_t y_ch, int C, int T, const int32_t* __restrict__ slots, const int32_t* __restrict__ hops,
                        float* __restrict__ state, int n_slots, const __grid_constant__ RsStream s) {
     extern __shared__ float sm[];
-    const int row = blockIdx.x / C, ch = blockIdx.x - row * C, tid = threadIdx.x;
-    const int slot = slots[row], h = hops ? hops[row] : T;
-    if (slot < 0 || slot >= n_slots || h <= 0 || h > T) return;          // a row that stores nothing
-    const RsRate& g = s.g;
-    const int H = s.hist, keep = s.keep, D = s.delay, n_win = H + h * s.block, n_new = h * s.out_block;
-    float* st = state + ((int64_t)slot * C + ch) * (H + keep);
-    const float* xr = x + (int64_t)row * x_row + (int64_t)ch * x_ch;
-    float* yr = y + (int64_t)row * y_row + (int64_t)ch * y_ch;
+    const int tid = threadIdx.x, H = s.hist, keep = s.keep, D = s.delay;
+    const SlotRow r = slot_row(C, slots, n_slots, state, H + keep);
+    const int h = hops ? hops[r.row] : T;
+    if (!r.live || h <= 0 || h > T) return;                            // a row that stores nothing
+    const int n_win = H + h * s.block, n_new = h * s.out_block;
+    float* st = r.st;
+    const float* xr = row_ch(x, x_row, x_ch, r.row, r.ch);
+    float* yr = row_ch(y, y_row, y_ch, r.row, r.ch);
     float* win = sm;                                 // [H + h * block]: the history, then the row's new samples
     float* out = sm + H + T * s.block;               // [keep + h * out_block]: the keep tail, then the new outputs
-    const float made = st[0];
-    const int before = made >= (float)D ? D : (made > 0.f ? (int)made : 0);
+    const int before = clamp_word(st[0], D);
     for (int i = tid; i < n_win; i += blockDim.x) win[i] = i == 0 ? 0.f : (i < H ? st[i] : xr[i - H]);
     for (int i = tid; i < keep; i += blockDim.x) out[i] = st[H + i];
     __syncthreads();
-    for (int j = tid; j < n_new; j += blockDim.x) {
-        float v = 0.f;                                                   // before z's start
-        if (before + j >= D) {
-            const int64_t a = (int64_t)(j - D) * g.o;
-            const int64_t c = a >= 0 ? a / g.q : -((-a + g.q - 1) / g.q);  // floor(a / q): tap c + H of win is x[m o / q]
-            v = rs_output(win + (H + c - g.w), a - c * g.q, g);
-        }
-        out[keep + j] = v;
-    }
+    // win[H] is x[0] of the push: output j centres on x[floor((j - D) o / q)]
+    for (int j = tid; j < n_new; j += blockDim.x) out[keep + j] = rs_delayed(win, H, j - D, before + j >= D, s.g);
     __syncthreads();
     for (int i = tid; i < keep + n_new; i += blockDim.x) yr[i] = out[i];
     for (int i = tid; i < H + keep; i += blockDim.x)
         st[i] = i == 0 ? (float)min(D, before + n_new) : (i < H ? win[n_win - H + i] : out[n_new + i - H]);
 }
 
+static std::string rs_rates(int32_t orig, int32_t new_freq) { return std::to_string(orig) + " -> " + std::to_string(new_freq) + " Hz"; }
+
+// the filter of a stream of orig -> new_freq Hz and its delay D = floor(w q / o): 0, or 1 with its message
+static int rs_streaming(const std::string& who, int32_t orig, int32_t new_freq, RsRate* g, int64_t* delay) {
+    if (orig <= 0 || new_freq <= 0) return fail(1, who + ": rates must be positive, got " + rs_rates(orig, new_freq));
+    if (orig == new_freq) return fail(1, who + ": " + rs_rates(orig, new_freq) + " needs no resampling");
+    *g = rs_rate(orig, new_freq, 0);
+    *delay = (int64_t)g->w * g->q / g->o;
+    return 0;
+}
+
 // the stream of orig -> new_freq Hz in pushes of `block` samples with `keep` repeated outputs, for calls of up to `blocks`
 // pushes per row: 0, or an error code (1 invalid, 2 the window of a row exceeds shared memory) with its message
-static int rs_stream(const char* who, int32_t orig, int32_t new_freq, int32_t block, int32_t keep, int32_t blocks,
+static int rs_stream(const std::string& who, int32_t orig, int32_t new_freq, int32_t block, int32_t keep, int32_t blocks,
                      RsStream* s) {
-    const std::string rates = std::to_string(orig) + " -> " + std::to_string(new_freq) + " Hz";
-    if (orig <= 0 || new_freq <= 0) return fail(1, std::string(who) + ": rates must be positive, got " + rates);
-    if (orig == new_freq) return fail(1, std::string(who) + ": " + rates + " needs no resampling");
-    s->g = rs_rate(orig, new_freq, 0);
+    int64_t delay;
+    if (int rc = rs_streaming(who, orig, new_freq, &s->g, &delay)) return rc;
     const RsRate& g = s->g;
+    const std::string rates = rs_rates(orig, new_freq);
     if (block <= 0 || block % g.o != 0)
-        return fail(1, std::string(who) + ": block " + std::to_string(block) + " is not a positive multiple of " +
-                           std::to_string(g.o) + ", the input samples of one period of " + rates);
-    if (keep < 0) return fail(1, std::string(who) + ": keep " + std::to_string(keep) + " is negative");
-    const int64_t out_block = (int64_t)block / g.o * g.q, delay = (int64_t)g.w * g.q / g.o;
+        return fail(1, who + ": block " + std::to_string(block) + " is not a positive multiple of " + std::to_string(g.o) +
+                           ", the input samples of one period of " + rates);
+    if (keep < 0) return fail(1, who + ": keep " + std::to_string(keep) + " is negative");
+    const int64_t out_block = (int64_t)block / g.o * g.q;
     const int64_t hist = (delay * g.o + g.q - 1) / g.q + g.w;
     const int64_t floats = hist + (int64_t)blocks * block + keep + (int64_t)blocks * out_block;
     if (floats * (int64_t)sizeof(float) > RS_SMEM_BYTES)
-        return fail(2, std::string(who) + ": " + rates + " in blocks of " + std::to_string(block) + " with keep " +
+        return fail(2, who + ": " + rates + " in blocks of " + std::to_string(block) + " with keep " +
                            std::to_string(keep) + " and " + std::to_string(blocks) + " blocks per row is too large: " +
                            std::to_string(floats) + " staged samples per row exceed shared memory (" +
                            std::to_string(RS_SMEM_BYTES / sizeof(float)) + ")");
@@ -224,37 +266,26 @@ resample_packets_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch
                         const int32_t* __restrict__ slots, float* __restrict__ state, int n_slots,
                         const __grid_constant__ RsPackets s) {
     extern __shared__ float win[];                   // [H + n]: the history, then the row's new samples
-    const int row = blockIdx.x / C, ch = blockIdx.x - row * C, tid = threadIdx.x;
-    const int slot = slots[row];
-    const int64_t pushed = (int64_t)counts[row] * s.unit;
+    const int tid = threadIdx.x, H = s.hist, D = s.delay;
+    const SlotRow r = slot_row(C, slots, n_slots, state, RP_HEAD + H);
+    const int64_t pushed = (int64_t)counts[r.row] * s.unit;
     const int n = pushed >= 0 && pushed <= s.max_in ? (int)pushed : 0;
-    if (slot < 0 || slot >= n_slots || n == 0) {                        // a row that stores nothing
-        if (ch == 0 && tid == 0) out_counts[row] = 0;
+    if (!r.live || n == 0) {                                            // a row that stores nothing
+        if (r.ch == 0 && tid == 0) out_counts[r.row] = 0;
         return;
     }
     const RsRate& g = s.g;
-    const int H = s.hist, D = s.delay;
-    float* st = state + ((int64_t)slot * C + ch) * (RP_HEAD + H);
-    const float made = st[0], phase = st[1];
-    const int before = made >= (float)D ? D : (made > 0.f ? (int)made : 0);
-    const int p = phase >= (float)(g.o - 1) ? g.o - 1 : (phase > 0.f ? (int)phase : 0);
+    float* st = r.st;
+    const int before = clamp_word(st[0], D), p = clamp_word(st[1], g.o - 1);
     const int64_t j0 = (int64_t)p * g.q / g.o;                         // the push's outputs j0 .. j0 + n_new - 1
     const int n_new = (int)((int64_t)(p + n) * g.q / g.o - j0);
-    if (ch == 0 && tid == 0) out_counts[row] = n_new;
-    const float* xr = x + (int64_t)row * x_row + (int64_t)ch * x_ch;
-    float* yr = y + (int64_t)row * y_row + (int64_t)ch * y_ch;
+    if (r.ch == 0 && tid == 0) out_counts[r.row] = n_new;
+    const float* xr = row_ch(x, x_row, x_ch, r.row, r.ch);
+    float* yr = row_ch(y, y_row, y_ch, r.row, r.ch);
     for (int i = tid; i < H + n; i += blockDim.x) win[i] = i < H ? st[RP_HEAD + i] : xr[i - H];
     __syncthreads();
     // win[H - p] is the input at the period boundary: output j (relative to it) centres on its input c = floor((j - D) o / q)
-    for (int k = tid; k < n_new; k += blockDim.x) {
-        float v = 0.f;                                                  // before z's start
-        if (before + k >= D) {
-            const int64_t a = (j0 + k - D) * g.o;
-            const int64_t c = a >= 0 ? a / g.q : -((-a + g.q - 1) / g.q);  // floor(a / q)
-            v = rs_output(win + (H - p + c - g.w), a - c * g.q, g);
-        }
-        yr[k] = v;
-    }
+    for (int k = tid; k < n_new; k += blockDim.x) yr[k] = rs_delayed(win, H - p, j0 + k - D, before + k >= D, g);
     for (int i = tid; i < H; i += blockDim.x) st[RP_HEAD + i] = win[n + i];
     if (tid == 0) {
         st[0] = (float)min(D, before + n_new);
@@ -264,19 +295,17 @@ resample_packets_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch
 
 // the packet stream of orig -> new_freq Hz for pushes of up to max_in samples: 0, or an error code (1 invalid, 2 the
 // window of a row exceeds shared memory) with its message
-static int rs_packets(const char* who, int32_t orig, int32_t new_freq, int32_t max_in, RsPackets* s, int32_t* max_out) {
-    const std::string rates = std::to_string(orig) + " -> " + std::to_string(new_freq) + " Hz";
-    if (orig <= 0 || new_freq <= 0) return fail(1, std::string(who) + ": rates must be positive, got " + rates);
-    if (orig == new_freq) return fail(1, std::string(who) + ": " + rates + " needs no resampling");
-    if (max_in <= 0) return fail(1, std::string(who) + ": max_in " + std::to_string(max_in) + " is not positive");
-    s->g = rs_rate(orig, new_freq, 0);
+static int rs_packets(const std::string& who, int32_t orig, int32_t new_freq, int32_t max_in, RsPackets* s,
+                      int32_t* max_out) {
+    int64_t delay;
+    if (int rc = rs_streaming(who, orig, new_freq, &s->g, &delay)) return rc;
+    if (max_in <= 0) return fail(1, who + ": max_in " + std::to_string(max_in) + " is not positive");
     const RsRate& g = s->g;
-    const int64_t delay = (int64_t)g.w * g.q / g.o;
     const int64_t hist = ((delay + 1) * g.o + g.q - 1) / g.q + g.w + 1;
     const int64_t out = ((int64_t)max_in * g.q + g.o - 1) / g.o;
     const int64_t floats = hist + max_in;
     if (floats * (int64_t)sizeof(float) > RS_SMEM_BYTES)
-        return fail(2, std::string(who) + ": " + rates + " in pushes of up to " + std::to_string(max_in) +
+        return fail(2, who + ": " + rs_rates(orig, new_freq) + " in pushes of up to " + std::to_string(max_in) +
                            " samples is too large: " + std::to_string(floats) + " staged samples per row (history and "
                            "push) exceed shared memory (" + std::to_string(RS_SMEM_BYTES / sizeof(float)) + ")");
     s->delay = (int32_t)delay;
@@ -288,63 +317,101 @@ static int rs_packets(const char* who, int32_t orig, int32_t new_freq, int32_t m
 
 // ---- the hop FIFO: 16 kHz pieces of any length -> separator chunks and hop counts ------------------------------------
 // A slot's row per channel is [FF_HEAD + 64 + capacity]: the read position, the samples held and the samples dropped (int32
-// words), then a ring of 64 + capacity samples.  The 64 samples before the read position are the carry, the held ones
-// follow it.  All zeros is an empty FIFO whose carry is 64 zeros.
-constexpr int FF_HEAD = 3, FF_HOP = 128, FF_CARRY = 64;
+// words), then a ring of 64 + capacity samples.  The 64 (CHUNK_CARRY) samples before the read position are the carry, the
+// held ones follow it.  All zeros is an empty FIFO whose carry is 64 zeros.
+constexpr int FF_HEAD = 3;
 
 __global__ void __launch_bounds__(RS_TILE)
 hop_fifo_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, int max_in, const int32_t* __restrict__ counts,
                 int unit, float* __restrict__ chunk, int64_t c_row, int64_t c_ch, int32_t* __restrict__ hops, int C, int T,
                 const int32_t* __restrict__ slots, float* __restrict__ state, int n_slots, int capacity) {
-    const int row = blockIdx.x / C, ch = blockIdx.x - row * C, tid = threadIdx.x;
-    const int slot = slots[row];
-    if (slot < 0 || slot >= n_slots) {                                  // a row that stores nothing
-        if (ch == 0 && tid == 0) hops[row] = 0;
+    const int tid = threadIdx.x, R = CHUNK_CARRY + capacity;
+    const SlotRow r = slot_row(C, slots, n_slots, state, FF_HEAD + R);
+    if (!r.live) {                                                      // a row that stores nothing
+        if (r.ch == 0 && tid == 0) hops[r.row] = 0;
         return;
     }
-    const int64_t pushed = (int64_t)counts[row] * unit;
+    const int64_t pushed = (int64_t)counts[r.row] * unit;
     const int n = pushed >= 0 && pushed <= max_in ? (int)pushed : 0;
-    const int R = FF_CARRY + capacity;
-    float* st = state + ((int64_t)slot * C + ch) * (FF_HEAD + R);
+    float* st = r.st;
     float* ring = st + FF_HEAD;
     const int pos = min(max(__float_as_int(st[0]), 0), R - 1), held = min(max(__float_as_int(st[1]), 0), capacity);
-    const int kept = min(n, capacity - held), h = min(T, (held + kept) / FF_HOP);
-    const float* xr = x + (int64_t)row * x_row + (int64_t)ch * x_ch;
+    const int kept = min(n, capacity - held), h = min(T, (held + kept) / CHUNK_HOP);
+    const float* xr = row_ch(x, x_row, x_ch, r.row, r.ch);
     for (int i = tid; i < kept; i += blockDim.x) ring[(pos + held + i) % R] = xr[i];
     __syncthreads();                                                    // the appended samples, visible to the block
-    float* cr = chunk + (int64_t)row * c_row + (int64_t)ch * c_ch;
-    for (int i = tid; i < h * FF_HOP + FF_CARRY; i += blockDim.x) cr[i] = ring[(pos + R - FF_CARRY + i) % R];
+    float* cr = row_ch(chunk, c_row, c_ch, r.row, r.ch);
+    for (int i = tid; i < h * CHUNK_HOP + CHUNK_CARRY; i += blockDim.x) cr[i] = ring[(pos + R - CHUNK_CARRY + i) % R];
     if (tid == 0) {
-        if (ch == 0) hops[row] = h;
-        st[0] = __int_as_float((pos + h * FF_HOP) % R);
-        st[1] = __int_as_float(held + kept - h * FF_HOP);
+        if (r.ch == 0) hops[r.row] = h;
+        st[0] = __int_as_float((pos + h * CHUNK_HOP) % R);
+        st[1] = __int_as_float(held + kept - h * CHUNK_HOP);
         const int dropped = __float_as_int(st[2]);
         st[2] = __int_as_float(n - kept > INT32_MAX - dropped ? INT32_MAX : dropped + (n - kept));
     }
 }
 
 // ---- the enrollment capture: the hops' new samples into a per-slot ring (layout: enroll_capture.cuh) -----------------
-// Row i appends samples EC_CARRY .. EC_CARRY + 128 h - 1 of its chunk (the hops' new samples, no look-ahead repeat) to slot
-// slots[i], h = hops[i]; a slot outside [0, n_slots) or h outside [1, T] stores nothing.  grid n * C, a CTA per (row,
-// channel).
-__global__ void __launch_bounds__(256)
+// Row i appends samples CHUNK_CARRY .. CHUNK_CARRY + 128 h - 1 of its chunk (the hops' new samples, no look-ahead repeat)
+// to slot slots[i], h = hops[i]; a slot outside [0, n_slots) or h outside [1, T] stores nothing.  grid n * C, a CTA per
+// (row, channel).
+__global__ void __launch_bounds__(RS_TILE)
 enroll_capture_kernel(const float* __restrict__ chunk, int64_t c_row, int64_t c_ch, int C, int T,
                       const int32_t* __restrict__ slots, const int32_t* __restrict__ hops, float* __restrict__ state,
                       int n_slots, int capacity) {
-    const int row = blockIdx.x / C, ch = blockIdx.x - row * C, tid = threadIdx.x;
-    const int slot = slots[row], h = hops[row];
-    if (slot < 0 || slot >= n_slots || h <= 0 || h > T) return;
-    float* st = state + ((int64_t)slot * C + ch) * (EC_HEAD + capacity);
-    const CaptureRow r = capture_row(state, EC_HEAD + capacity, C, slot, ch, capacity);
+    const int tid = threadIdx.x;
+    const SlotRow sr = slot_row(C, slots, n_slots, state, EC_HEAD + capacity);
+    const int h = hops[sr.row];
+    if (!sr.live || h <= 0 || h > T) return;
+    float* st = sr.st;
+    const CaptureRow r = capture_row(st, capacity);
     float* ring = st + EC_HEAD;
-    const int n = h * EC_HOP, skip = n > capacity ? n - capacity : 0;   // only the last `capacity` samples survive
-    const float* src = chunk + (int64_t)row * c_row + (int64_t)ch * c_ch + EC_CARRY;
+    const int n = h * CHUNK_HOP, skip = n > capacity ? n - capacity : 0;   // only the last `capacity` samples survive
+    const float* src = row_ch(chunk, c_row, c_ch, sr.row, sr.ch) + CHUNK_CARRY;
     for (int i = skip + tid; i < n; i += blockDim.x) ring[(int)(((int64_t)r.wpos + i) % capacity)] = src[i];
     __syncthreads();                                                    // every thread has read the head
     if (tid == 0) {
         st[0] = __int_as_float((int)(((int64_t)r.wpos + n) % capacity));
         st[1] = __int_as_float(min(r.captured + n, capacity));
     }
+}
+
+// ---- the host side of the per-slot calls ------------------------------------------------------------------------------
+// The checks every per-slot call makes first, in this order: its pointers, its sizes (`sizes` names them), n <= n_slots,
+// and a grid of n * channels CTAs.  0, or 1 with its message.
+static int slot_call(const std::string& who, std::initializer_list<const void*> ptrs, const char* sizes,
+                     std::initializer_list<int32_t> values, int32_t n, int32_t channels, int32_t n_slots) {
+    for (const void* p : ptrs) if (!p) return fail(1, who + ": null pointer");
+    for (int32_t v : values) if (v <= 0) return fail(1, who + ": " + sizes + " must be positive");
+    if (n > n_slots) return fail(1, who + ": a call needs n <= n_slots");
+    if ((int64_t)n * channels > INT32_MAX) return fail(1, who + ": n * channels is too large");
+    return 0;
+}
+
+// a strided [n][channels][len] operand of a per-slot call
+struct Rows { const char* name; int64_t row, ch, len; };
+
+// 0 when no two rows or channels of any operand overlap, else 1 with its message
+static int disjoint(const std::string& who, int32_t channels, std::initializer_list<Rows> ops) {
+    bool ok = true;
+    std::string what;
+    for (const Rows& r : ops) {
+        ok = ok && r.ch >= r.len && r.row / channels >= r.ch;
+        what += (what.empty() ? "" : " and ") + std::string(r.name) + " (" + std::to_string(r.len) + " samples)";
+    }
+    return ok ? 0 : fail(1, who + ": bad stride: rows and channels of " + what + " must not overlap");
+}
+
+// the samples of a separator chunk of `frames` hops: 0, or 1 when they do not fit an int32
+static int chunk_len(const std::string& who, int32_t frames, int64_t* len) {
+    *len = (int64_t)frames * CHUNK_HOP + CHUNK_CARRY;
+    return *len > INT32_MAX ? fail(1, who + ": frames is too large") : 0;
+}
+
+// the error of the launch just made: 0, or 3 with its message
+static int launched(const std::string& who) {
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail(3, who + ": " + cudaGetErrorString(e));
 }
 
 }  // namespace l2h
@@ -363,13 +430,11 @@ extern "C" int l2h_resample(const float* x_dev, int64_t x_row_stride, int32_t n_
         if (r > 0 && orig == orig_freq[r - 1]) continue;
         const int64_t n_out = ((int64_t)new_freq * n_in + orig - 1) / orig;
         if (n_out > y_capacity)
-            return fail(1, "l2h_resample: row " + std::to_string(r) + " (" + std::to_string(orig) + " -> " + std::to_string(new_freq) +
-                               " Hz) has " + std::to_string(n_out) + " output samples, capacity " + std::to_string(y_capacity));
-        const int32_t gd = std::gcd(orig, new_freq), o = orig / gd, q = new_freq / gd;
-        const int64_t w = (int64_t)std::ceil(RS_WIDTH * (double)o / (std::min(o, q) * RS_ROLLOFF));
-        if ((((int64_t)(RS_TILE - 1) * o) / q + 2 * w + 2) * (int64_t)sizeof(float) > RS_SMEM_BYTES)
-            return fail(2, "l2h_resample: reduced rate ratio " + std::to_string(o) + "/" + std::to_string(q) + " (" + std::to_string(orig) +
-                               " -> " + std::to_string(new_freq) + " Hz) is too large: the input window of a tile exceeds shared memory");
+            return fail(1, "l2h_resample: row " + std::to_string(r) + " (" + rs_rates(orig, new_freq) + ") has " + std::to_string(n_out) + " output samples, capacity " + std::to_string(y_capacity));
+        const RsRate g = rs_rate(orig, new_freq, 0);
+        if ((((int64_t)(RS_TILE - 1) * g.o) / g.q + 2 * (int64_t)g.w + 2) * (int64_t)sizeof(float) > RS_SMEM_BYTES)
+            return fail(2, "l2h_resample: reduced rate ratio " + std::to_string(g.o) + "/" + std::to_string(g.q) + " (" +
+                               rs_rates(orig, new_freq) + ") is too large: the input window of a tile exceeds shared memory");
     }
     if (y_capacity == 0) return 0;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -426,25 +491,20 @@ extern "C" int l2h_resample_stream(const float* x_dev, int64_t x_row_stride, int
                                    const int32_t* slots_dev, const int32_t* hops_dev, float* state_dev, int32_t n_slots,
                                    int32_t orig_freq, int32_t new_freq, int32_t block, int32_t keep, void* stream) {
     using namespace l2h;
-    if (!x_dev || !y_dev || !slots_dev || !state_dev) return fail(1, "l2h_resample_stream: null pointer");
-    if (n <= 0 || channels <= 0 || blocks <= 0 || n_slots <= 0)
-        return fail(1, "l2h_resample_stream: n, channels, blocks and n_slots must be positive");
-    if (n > n_slots) return fail(1, "l2h_resample_stream: a call needs n <= n_slots");
-    if ((int64_t)n * channels > INT32_MAX) return fail(1, "l2h_resample_stream: n * channels is too large");
+    const std::string who = "l2h_resample_stream";
+    if (int rc = slot_call(who, {x_dev, y_dev, slots_dev, state_dev}, "n, channels, blocks and n_slots",
+                           {n, channels, blocks, n_slots}, n, channels, n_slots))
+        return rc;
     RsStream s;
-    if (int rc = rs_stream("l2h_resample_stream", orig_freq, new_freq, block, keep, blocks, &s)) return rc;
+    if (int rc = rs_stream(who, orig_freq, new_freq, block, keep, blocks, &s)) return rc;
     const int64_t x_len = (int64_t)blocks * block, y_len = keep + (int64_t)blocks * s.out_block;
-    if (x_ch_stride < x_len || x_row_stride / channels < x_ch_stride || y_ch_stride < y_len ||
-        y_row_stride / channels < y_ch_stride)
-        return fail(1, "l2h_resample_stream: bad stride: rows and channels of x (" + std::to_string(x_len) + " samples) and y (" +
-                           std::to_string(y_len) + ") must not overlap");
+    if (int rc = disjoint(who, channels, {{"x", x_row_stride, x_ch_stride, x_len}, {"y", y_row_stride, y_ch_stride, y_len}}))
+        return rc;
     const int smem = (int)((s.hist + x_len + y_len) * sizeof(float));
     resample_stream_kernel<<<(unsigned)(n * channels), RS_TILE, smem, static_cast<cudaStream_t>(stream)>>>(
         x_dev, x_row_stride, x_ch_stride, y_dev, y_row_stride, y_ch_stride, channels, blocks, slots_dev, hops_dev, state_dev,
         n_slots, s);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(3, std::string("l2h_resample_stream: ") + cudaGetErrorString(e));
-    return 0;
+    return launched(who);
 }
 
 extern "C" int l2h_resample_packets_layout(int32_t orig_freq, int32_t new_freq, int32_t max_in, int32_t* row_floats,
@@ -466,36 +526,30 @@ extern "C" int l2h_resample_packets(const float* x_dev, int64_t x_row_stride, in
                                     const int32_t* slots_dev, float* state_dev, int32_t n_slots, int32_t orig_freq,
                                     int32_t new_freq, void* stream) {
     using namespace l2h;
-    if (!x_dev || !y_dev || !counts_dev || !out_counts_dev || !slots_dev || !state_dev)
-        return fail(1, "l2h_resample_packets: null pointer");
-    if (n <= 0 || channels <= 0 || unit <= 0 || n_slots <= 0)
-        return fail(1, "l2h_resample_packets: n, channels, unit and n_slots must be positive");
-    if (n > n_slots) return fail(1, "l2h_resample_packets: a call needs n <= n_slots");
-    if ((int64_t)n * channels > INT32_MAX) return fail(1, "l2h_resample_packets: n * channels is too large");
+    const std::string who = "l2h_resample_packets";
+    if (int rc = slot_call(who, {x_dev, y_dev, counts_dev, out_counts_dev, slots_dev, state_dev},
+                           "n, channels, unit and n_slots", {n, channels, unit, n_slots}, n, channels, n_slots))
+        return rc;
     RsPackets s;
     int32_t max_out;
-    if (int rc = rs_packets("l2h_resample_packets", orig_freq, new_freq, max_in, &s, &max_out)) return rc;
+    if (int rc = rs_packets(who, orig_freq, new_freq, max_in, &s, &max_out)) return rc;
     s.unit = unit;
-    if (x_ch_stride < max_in || x_row_stride / channels < x_ch_stride || y_ch_stride < max_out ||
-        y_row_stride / channels < y_ch_stride)
-        return fail(1, "l2h_resample_packets: bad stride: rows and channels of x (" + std::to_string(max_in) +
-                           " samples) and y (" + std::to_string(max_out) + ") must not overlap");
+    if (int rc = disjoint(who, channels, {{"x", x_row_stride, x_ch_stride, max_in}, {"y", y_row_stride, y_ch_stride, max_out}}))
+        return rc;
     const int smem = (int)((s.hist + max_in) * sizeof(float));
     resample_packets_kernel<<<(unsigned)(n * channels), RS_TILE, smem, static_cast<cudaStream_t>(stream)>>>(
         x_dev, x_row_stride, x_ch_stride, y_dev, y_row_stride, y_ch_stride, channels, counts_dev, out_counts_dev, slots_dev,
         state_dev, n_slots, s);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(3, std::string("l2h_resample_packets: ") + cudaGetErrorString(e));
-    return 0;
+    return launched(who);
 }
 
 extern "C" int l2h_hop_fifo_layout(int32_t capacity, int32_t* row_floats) {
     using namespace l2h;
     if (!row_floats) return fail(1, "l2h_hop_fifo_layout: null pointer");
-    if (capacity < FF_HOP || capacity > INT32_MAX - FF_HEAD - FF_CARRY)
+    if (capacity < CHUNK_HOP || capacity > INT32_MAX - FF_HEAD - CHUNK_CARRY)
         return fail(1, "l2h_hop_fifo_layout: capacity " + std::to_string(capacity) + " cannot hold one hop of " +
-                           std::to_string(FF_HOP) + " samples");
-    *row_floats = FF_HEAD + FF_CARRY + capacity;
+                           std::to_string(CHUNK_HOP) + " samples");
+    *row_floats = FF_HEAD + CHUNK_CARRY + capacity;
     return 0;
 }
 
@@ -504,26 +558,22 @@ extern "C" int l2h_hop_fifo(const float* x_dev, int64_t x_row_stride, int64_t x_
                             int64_t chunk_ch_stride, int32_t* hops_dev, int32_t n, int32_t channels, int32_t frames,
                             const int32_t* slots_dev, float* state_dev, int32_t n_slots, int32_t capacity, void* stream) {
     using namespace l2h;
-    if (!x_dev || !counts_dev || !chunk_dev || !hops_dev || !slots_dev || !state_dev)
-        return fail(1, "l2h_hop_fifo: null pointer");
-    if (n <= 0 || channels <= 0 || max_in <= 0 || unit <= 0 || frames <= 0 || n_slots <= 0)
-        return fail(1, "l2h_hop_fifo: n, channels, max_in, unit, frames and n_slots must be positive");
-    if (n > n_slots) return fail(1, "l2h_hop_fifo: a call needs n <= n_slots");
-    if ((int64_t)n * channels > INT32_MAX) return fail(1, "l2h_hop_fifo: n * channels is too large");
+    const std::string who = "l2h_hop_fifo";
+    if (int rc = slot_call(who, {x_dev, counts_dev, chunk_dev, hops_dev, slots_dev, state_dev},
+                           "n, channels, max_in, unit, frames and n_slots", {n, channels, max_in, unit, frames, n_slots}, n,
+                           channels, n_slots))
+        return rc;
     int32_t row_floats;
+    int64_t c_len;
     if (int rc = l2h_hop_fifo_layout(capacity, &row_floats)) return rc;
-    const int64_t c_len = (int64_t)frames * FF_HOP + FF_CARRY;
-    if (c_len > INT32_MAX) return fail(1, "l2h_hop_fifo: frames is too large");
-    if (x_ch_stride < max_in || x_row_stride / channels < x_ch_stride || chunk_ch_stride < c_len ||
-        chunk_row_stride / channels < chunk_ch_stride)
-        return fail(1, "l2h_hop_fifo: bad stride: rows and channels of x (" + std::to_string(max_in) + " samples) and chunk (" +
-                           std::to_string(c_len) + ") must not overlap");
+    if (int rc = chunk_len(who, frames, &c_len)) return rc;
+    if (int rc = disjoint(who, channels, {{"x", x_row_stride, x_ch_stride, max_in},
+                                          {"chunk", chunk_row_stride, chunk_ch_stride, c_len}}))
+        return rc;
     hop_fifo_kernel<<<(unsigned)(n * channels), RS_TILE, 0, static_cast<cudaStream_t>(stream)>>>(
         x_dev, x_row_stride, x_ch_stride, max_in, counts_dev, unit, chunk_dev, chunk_row_stride, chunk_ch_stride, hops_dev,
         channels, frames, slots_dev, state_dev, n_slots, capacity);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(3, std::string("l2h_hop_fifo: ") + cudaGetErrorString(e));
-    return 0;
+    return launched(who);
 }
 
 extern "C" int l2h_enroll_capture_layout(int32_t capacity, int32_t* row_floats) {
@@ -540,21 +590,16 @@ extern "C" int l2h_enroll_capture(const float* chunk_dev, int64_t chunk_row_stri
                                   int32_t channels, int32_t frames, const int32_t* slots_dev, const int32_t* hops_dev,
                                   float* state_dev, int32_t n_slots, int32_t capacity, void* stream) {
     using namespace l2h;
-    if (!chunk_dev || !slots_dev || !hops_dev || !state_dev) return fail(1, "l2h_enroll_capture: null pointer");
-    if (n <= 0 || channels <= 0 || frames <= 0 || n_slots <= 0)
-        return fail(1, "l2h_enroll_capture: n, channels, frames and n_slots must be positive");
-    if (n > n_slots) return fail(1, "l2h_enroll_capture: a call needs n <= n_slots");
-    if ((int64_t)n * channels > INT32_MAX) return fail(1, "l2h_enroll_capture: n * channels is too large");
+    const std::string who = "l2h_enroll_capture";
+    if (int rc = slot_call(who, {chunk_dev, slots_dev, hops_dev, state_dev}, "n, channels, frames and n_slots",
+                           {n, channels, frames, n_slots}, n, channels, n_slots))
+        return rc;
     int32_t row_floats;
+    int64_t c_len;
     if (int rc = l2h_enroll_capture_layout(capacity, &row_floats)) return rc;
-    const int64_t c_len = (int64_t)frames * EC_HOP + EC_CARRY;
-    if (c_len > INT32_MAX) return fail(1, "l2h_enroll_capture: frames is too large");
-    if (chunk_ch_stride < c_len || chunk_row_stride / channels < chunk_ch_stride)
-        return fail(1, "l2h_enroll_capture: bad stride: rows and channels of the chunk (" + std::to_string(c_len) +
-                           " samples) must not overlap");
-    enroll_capture_kernel<<<(unsigned)(n * channels), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    if (int rc = chunk_len(who, frames, &c_len)) return rc;
+    if (int rc = disjoint(who, channels, {{"chunk", chunk_row_stride, chunk_ch_stride, c_len}})) return rc;
+    enroll_capture_kernel<<<(unsigned)(n * channels), RS_TILE, 0, static_cast<cudaStream_t>(stream)>>>(
         chunk_dev, chunk_row_stride, chunk_ch_stride, channels, frames, slots_dev, hops_dev, state_dev, n_slots, capacity);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(3, std::string("l2h_enroll_capture: ") + cudaGetErrorString(e));
-    return 0;
+    return launched(who);
 }

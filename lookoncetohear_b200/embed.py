@@ -16,6 +16,8 @@ import torch
 import torch.nn as nn
 
 from . import _cabi
+from .net import device_list
+from .stream import EnrollCapture
 
 
 class _Affine4D(nn.Module):
@@ -123,20 +125,24 @@ class EmbedTFGridNet(nn.Module):
         _cabi.check(_cabi.lib().l2h_embed_max_batch(self._engine(), int(n_samples), ctypes.byref(per)))
         return max(1, per.value)
 
+    def _workspace(self, nb, n, dev):
+        """the engine's shared workspace on dev, grown to what a call of nb utterances of n samples needs"""
+        ws = ctypes.c_size_t()
+        _cabi.check(_cabi.lib().l2h_embed_workspace_bytes(self._engine(), nb, n, ctypes.byref(ws)))
+        if self._ws is None or self._ws.numel() < ws.value or self._ws.device != dev:
+            self._ws = torch.empty(ws.value, dtype=torch.uint8, device=dev)
+        return self._ws
+
     def _run(self, x, out, lens):
         """One engine call: x [nb, M, n] contiguous on the device, lens None or nb ints, out [nb, embed_dim]."""
         dev = x.device
         nb, _, n = x.shape
-        L, h = _cabi.lib(), self._engine()
-        ws = ctypes.c_size_t()
-        _cabi.check(L.l2h_embed_workspace_bytes(h, nb, n, ctypes.byref(ws)))
-        if self._ws is None or self._ws.numel() < ws.value or self._ws.device != dev:
-            self._ws = torch.empty(ws.value, dtype=torch.uint8, device=dev)
+        ws = self._workspace(nb, n, dev)
         lens_c = None if lens is None else (ctypes.c_int32 * nb)(*lens)
         with torch.cuda.device(dev):
-            _cabi.check(L.l2h_embed_forward_lengths(h, x.data_ptr(), n, lens_c, nb, out.data_ptr(),
-                                                    self._ws.data_ptr(), self._ws.numel(),
-                                                    torch.cuda.current_stream(dev).cuda_stream))
+            _cabi.check(_cabi.lib().l2h_embed_forward_lengths(self._engine(), x.data_ptr(), n, lens_c, nb, out.data_ptr(),
+                                                              ws.data_ptr(), ws.numel(),
+                                                              torch.cuda.current_stream(dev).cuda_stream))
 
     def forward(self, input, lengths=None):
         """input [B, M, N] -> [B, embed_dim]   (reference tfgridnet.py:100-127).
@@ -185,24 +191,12 @@ class EmbedTFGridNet(nn.Module):
         written (NaN in a new tensor), so in the staging buffer that listener keeps its embedding.  `used` (a contiguous
         CUDA int32 tensor of shape (n,), optional) receives the samples each row used, 0 for a row not written."""
         dev, slots, n, lens, out, used = self._enroll_args(capture, slots, lengths, out, used)
-        L, h = _cabi.lib(), self._engine()
-        host = not slots.is_cuda
         n_max = max(lens)
         per = self.max_batch(n_max)
         for b0 in range(0, n, per):
             nb = min(per, n - b0)
-            ws = ctypes.c_size_t()
-            _cabi.check(L.l2h_embed_workspace_bytes(h, nb, n_max, ctypes.byref(ws)))
-            if self._ws is None or self._ws.numel() < ws.value or self._ws.device != dev:
-                self._ws = torch.empty(ws.value, dtype=torch.uint8, device=dev)
-            sl = slots[b0:b0 + nb]
-            sl_host = ctypes.cast(sl.data_ptr(), ctypes.POINTER(ctypes.c_int32)) if host else None
-            with torch.cuda.device(dev):
-                _cabi.check_args(L.l2h_embed_forward_slots(
-                    h, capture.state.data_ptr(), capture.n_slots, capture.capacity, sl_host,
-                    None if host else sl.data_ptr(), (ctypes.c_int32 * nb)(*lens[b0:b0 + nb]), nb, n_max,
-                    out[b0].data_ptr(), out.stride(0), used[b0:].data_ptr(), self._ws.data_ptr(), self._ws.numel(),
-                    torch.cuda.current_stream(dev).cuda_stream))
+            _slots_call(_cabi.lib().l2h_embed_forward_slots, self, capture, slots, lens, out, used, b0, nb, n_max,
+                        self._workspace(nb, n_max, dev))
         return out
 
     def enroll_job(self, capture, slots, lengths, out=None, used=None, window=None):
@@ -224,8 +218,6 @@ class EmbedTFGridNet(nn.Module):
 
     def _enroll_args(self, capture, slots, lengths, out, used):
         """The checks of ``enroll``: (device, slot list tensor, n, lengths, out, used), the weights committed."""
-        from .net import device_list
-        from .render import EnrollCapture
         if not isinstance(capture, EnrollCapture):
             raise TypeError("capture must be an EnrollCapture")
         if capture.channels != self.num_ch:
@@ -256,6 +248,21 @@ class EmbedTFGridNet(nn.Module):
         return dev, slots, n, lens, out, used
 
 
+def _slots_call(entry, net, capture, slots, lens, out, used, b0, nb, n_max, ws, *tail):
+    """entry (l2h_embed_forward_slots, or ..._units with `tail` = window, first unit, units) over rows b0 .. b0 + nb - 1
+    of an enrollment from `capture`: a host or CUDA slot list, the rows' lengths padded to n_max, workspace ws, on the
+    current stream of the capture's device"""
+    dev = capture.state.device
+    sl = slots[b0:b0 + nb]
+    sl_host = None if sl.is_cuda else ctypes.cast(sl.data_ptr(), ctypes.POINTER(ctypes.c_int32))
+    with torch.cuda.device(dev):
+        _cabi.check_args(entry(
+            net._engine(), capture.state.data_ptr(), capture.n_slots, capture.capacity, sl_host,
+            sl.data_ptr() if sl.is_cuda else None, (ctypes.c_int32 * nb)(*lens[b0:b0 + nb]), nb, n_max,
+            out[b0].data_ptr(), out.stride(0), used[b0:].data_ptr(), ws.data_ptr(), ws.numel(), *tail,
+            torch.cuda.current_stream(dev).cuda_stream))
+
+
 # Inter-recurrence steps per unit of an EnrollJob: 0, the whole recurrence as one unit.  Measured at 5 s (DESIGN.md
 # section 7, tools/bench_enroll_slices.py), that unit is at most 7 % (8 listeners) to 25 % (1 listener) longer than the
 # largest GEMM unit, which no window splits, while windows cost 7-39 % more device time in all.
@@ -272,7 +279,6 @@ class EnrollJob:
         L, h = _cabi.lib(), net._engine()
         self.net, self.capture, self.dev, self.window = net, capture, dev, window
         self.slots, self.lens, self.out, self.used = slots, lens, out, used
-        self._host = not slots.is_cuda
         self.n_max = max(lens)
         per = net.max_batch(self.n_max)
         self._cuts = []                                    # (first row, rows, units)
@@ -295,21 +301,13 @@ class EnrollJob:
         """Enqueue the next n units (fewer if fewer remain) on the current stream; returns how many were enqueued."""
         if isinstance(n, bool) or not isinstance(n, numbers.Integral) or n < 1:
             raise ValueError(f"n must be an int >= 1, got {n!r}")
-        L, h = _cabi.lib(), self.net._engine()
         end = min(self.units, self._next + int(n))
         start, base = self._next, 0
         for b0, nb, units in self._cuts:
             lo, hi = max(start, base), min(end, base + units)
             if lo < hi:
-                sl = self.slots[b0:b0 + nb]
-                sl_host = ctypes.cast(sl.data_ptr(), ctypes.POINTER(ctypes.c_int32)) if self._host else None
-                with torch.cuda.device(self.dev):
-                    _cabi.check_args(L.l2h_embed_forward_slots_units(
-                        h, self.capture.state.data_ptr(), self.capture.n_slots, self.capture.capacity, sl_host,
-                        None if self._host else sl.data_ptr(), (ctypes.c_int32 * nb)(*self.lens[b0:b0 + nb]), nb,
-                        self.n_max, self.out[b0].data_ptr(), self.out.stride(0), self.used[b0:].data_ptr(),
-                        self._ws.data_ptr(), self._ws.numel(), self.window, lo - base, hi - lo,
-                        torch.cuda.current_stream(self.dev).cuda_stream))
+                _slots_call(_cabi.lib().l2h_embed_forward_slots_units, self.net, self.capture, self.slots, self.lens,
+                            self.out, self.used, b0, nb, self.n_max, self._ws, self.window, lo - base, hi - lo)
                 self._next = hi
             base += units
         return end - start

@@ -11,7 +11,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from lookoncetohear_b200 import Net, SepState, synth
+from lookoncetohear_b200 import Net, SepState, resample, synth
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HOP, LA = 128, 64
@@ -100,6 +100,18 @@ def hop_mix(n, T, seed):
 
 def i32(v, dev):
     return torch.tensor(v, dtype=torch.int32, device=dev)
+
+
+def signals(S, C, n, seed, dev):
+    """[S, C, n] seeded signals on dev"""
+    return (0.1 * torch.randn(S, C, n, generator=torch.Generator().manual_seed(seed))).to(dev)
+
+
+def delayed(whole, orig, new, D, n=None):
+    """resample of the whole signals [S, C, N], delayed by D samples (zeros first): its first n samples, or as many as
+    the resampled signals hold"""
+    z = resample(whole, orig, new)
+    return F.pad(z, (D, 0))[..., :z.shape[-1] if n is None else n]
 
 
 # ---- states ----------------------------------------------------------------------------------------------------------

@@ -9,25 +9,14 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from lookoncetohear_b200 import HopFifo, PacketResampler, StreamResampler, resample, synth
+from lookoncetohear_b200 import HopFifo, PacketResampler, StreamResampler, synth
 from oracle import resample as ors
-from serving_util import bits, dev, i32, model  # noqa: F401
+from serving_util import SENTINEL as NAN, bits, delayed, dev, i32, model, signals  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
 RATES = [44100, 22050, 11025, 48000, 32000, 24000, 8000]
 PAIRS = [(r, 16000) for r in RATES] + [(16000, r) for r in RATES]
-NAN = float("nan")
-
-
-def signals(S, C, n, seed, dev):
-    return (0.1 * torch.randn(S, C, n, generator=torch.Generator().manual_seed(seed))).to(dev)
-
-
-def delayed(whole, orig, new, D, keep):
-    """the first `keep` samples of resample of the whole signals [S, C, N], delayed by D samples (zeros first)"""
-    z = resample(whole, orig, new)
-    return F.pad(z, (D, 0))[..., :keep]
 
 
 @pytest.mark.parametrize("orig,new", PAIRS)

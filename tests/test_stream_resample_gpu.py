@@ -9,23 +9,12 @@ import torch.nn.functional as F
 
 from lookoncetohear_b200 import StreamResampler, resample, synth
 from oracle import resample as ors
-from serving_util import bits, dev, hop_mix, i32, model  # noqa: F401
+from serving_util import SENTINEL as NAN, bits, delayed, dev, hop_mix, i32, model, signals  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
 PAIRS = [(48000, 16000), (32000, 16000), (24000, 16000), (8000, 16000),
          (16000, 48000), (16000, 32000), (16000, 24000), (16000, 8000)]
-NAN = float("nan")
-
-
-def signals(S, C, n, seed, dev):
-    return (0.1 * torch.randn(S, C, n, generator=torch.Generator().manual_seed(seed))).to(dev)
-
-
-def delayed(whole, orig, new, D):
-    """resample of the whole signals [S, C, N], delayed by D samples (zeros first), same length"""
-    z = resample(whole, orig, new)
-    return F.pad(z, (D, 0))[..., :z.shape[-1]]
 
 
 def run_ticks(rs, sig, ticks, n, T, seed):

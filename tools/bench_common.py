@@ -67,6 +67,19 @@ def alternate(fns, reps, windows=5):
     return {k: statistics.median(v) for k, v in t.items()}
 
 
+def graphed(fn):
+    """fn() captured as a CUDA graph (after a warm-up call on a side stream); returns the graph's replay"""
+    side = torch.cuda.Stream()
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        fn()
+    torch.cuda.current_stream().wait_stream(side)
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        fn()
+    return g.replay
+
+
 def rel_l2(a, b):
     """max over rows of ||a - b|| / ||b||, over the rows b has written (norm > 0)"""
     a, b = a.reshape(a.shape[0], -1).double(), b.reshape(b.shape[0], -1).double()

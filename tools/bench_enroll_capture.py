@@ -29,24 +29,11 @@ import time
 
 import torch
 
-from bench_common import L2H_FLAG_GRAPH, alternate, emit, gpu_info, setup_net
+from bench_common import L2H_FLAG_GRAPH, alternate, emit, gpu_info, graphed, setup_net
 from lookoncetohear_b200 import EmbedTFGridNet, EnrollCapture, HopFifo, synth
 from lookoncetohear_b200.configs import EMBED_PARAMS
 
 T, HOP, CARRY, SR = 3, 128, 64, 16000
-
-
-def graphed(fn):
-    """fn() captured as a CUDA graph (after a warm-up call on a side stream); returns the graph's replay"""
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        fn()
-    torch.cuda.current_stream().wait_stream(side)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        fn()
-    return g.replay
 
 
 def host_ms(fn, reps):

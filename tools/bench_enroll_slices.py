@@ -27,25 +27,13 @@ import sys
 
 import torch
 
-from bench_common import L2H_FLAG_GRAPH, emit, gpu_info, setup_net
+from bench_common import L2H_FLAG_GRAPH, emit, gpu_info, graphed, setup_net
 from lookoncetohear_b200 import EmbedTFGridNet, EnrollCapture, HopFifo, synth
 from lookoncetohear_b200.configs import EMBED_PARAMS
 from lookoncetohear_b200.embed import DEFAULT_WINDOW
 
 T, HOP, CARRY, SR, PERIOD_MS = 3, 128, 64, 16000, 8.0
 WINDOWS = (0, 64, 128, 256)
-
-
-def graphed(fn):
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        fn()
-    torch.cuda.current_stream().wait_stream(side)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        fn()
-    return g.replay
 
 
 def ev():

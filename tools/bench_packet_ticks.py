@@ -25,7 +25,7 @@ import sys
 import numpy as np
 import torch
 
-from bench_common import L2H_FLAG_GRAPH, alternate, emit, gpu_info, setup_net
+from bench_common import L2H_FLAG_GRAPH, alternate, emit, gpu_info, graphed, setup_net
 from lookoncetohear_b200 import HopFifo, PacketResampler, synth
 
 T, CAP, PACKET = 3, 1024, 441
@@ -56,19 +56,6 @@ class HostFifo:
         self.buf[slot] = torch.gather(self.buf[slot], 2, src[:, None].expand(-1, self.buf.shape[1], -1))
         self.fill[sl] = fill - 128 * h
         return chunk, torch.from_numpy(h.astype(np.int32)).to(dev)
-
-
-def graphed(fn):
-    """fn() captured as a CUDA graph (after a warm-up call on a side stream); returns the graph's replay"""
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        fn()
-    torch.cuda.current_stream().wait_stream(side)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        fn()
-    return g.replay
 
 
 def main():

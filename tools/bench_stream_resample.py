@@ -22,7 +22,7 @@ import sys
 
 import torch
 
-from bench_common import HOP, LA, L2H_FLAG_GRAPH, alternate, emit, gpu_info, setup_net
+from bench_common import HOP, L2H_FLAG_GRAPH, LA, alternate, emit, gpu_info, graphed, setup_net
 from lookoncetohear_b200 import StreamResampler, resample, synth
 
 
@@ -48,19 +48,6 @@ class Recipe:
         else:
             out.copy_(new)
         self.hist.index_copy_(0, idx, xin[..., -self.hc:])
-
-
-def graphed(fn):
-    """fn() captured as a CUDA graph (after a warm-up call on a side stream); returns the graph's replay"""
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        fn()
-    torch.cuda.current_stream().wait_stream(side)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        fn()
-    return g.replay
 
 
 def main():
