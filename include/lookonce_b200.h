@@ -21,6 +21,9 @@
  *        <- Net.predict for several enrolled speakers of each mixture, for a whole state, a list of its listener
  *           groups, or listeners with different numbers of speakers (Net.predict_targets, Net.advance_targets,
  *           Net.advance_target_rows)
+ *   l2h_sep_forward_targets_rows_history / l2h_sep_join_targets / l2h_sep_state_move_lead
+ *        <- adding a speaker to a running listener, warmed from its recent block-0 output, and dropping one
+ *           (Net.advance_target_rows(history=), Net.join_targets, SepState.move_lead)
  *   l2h_sep_stream_host
  *        <- the chunk loop around Net.predict(chunk, embed, state, pad=False)  (SURVEY.md 3.3)
  *           with host buffers: H2D of each chunk and D2H of each result inside the call
@@ -122,6 +125,15 @@ int l2h_sep_state_offsets(void* handle, int64_t* out, int32_t n);
  * The copied records' gate memo is invalidated (it is rebuilt at their next call).  A stream moves to another device by a
  * host copy of its record (SepState views) into an initialised state there. */
 int l2h_sep_state_reset_streams(void* handle, void* state_dev, int32_t batch, const int32_t* slots_host, int32_t n, void* stream);
+/* l2h_sep_state_move_lead: record new_host[i] takes over as its listener's lead from record old_host[i] (a record of the same
+ * listener): the speaker-independent part of old_host[i] -- block 0's K/V rings and (h, c), and the current copy of its conv
+ * tails, which goes into the copy new_host[i]'s own parity makes current -- is copied into new_host[i].  Its blocks
+ * 1 .. B-1, back tails, embedding, gate memo and clock stay as they are.  The two clocks must be equal: the call waits for
+ * `stream`, reads them and refuses the call (1) if any pair differs.  Then old_host[i] may be dropped from the listener's
+ * rows.  Errors 1, before anything is enqueued: null pointers, batch or n <= 0, n > batch, a record outside [0, batch) or
+ * listed twice in one list, a record in both lists, different clocks. */
+int l2h_sep_state_move_lead(void* handle, void* state_dev, int32_t batch, const int32_t* old_host, const int32_t* new_host,
+                            int32_t n, void* stream);
 int l2h_sep_state_copy_streams(void* handle, void* dst_state_dev, int32_t dst_batch, const int32_t* dst_slots_host,
                                const void* src_state_dev, int32_t src_batch, const int32_t* src_slots_host, int32_t n,
                                void* stream);
@@ -279,8 +291,9 @@ int l2h_sep_forward_targets_groups(void* handle, const float* x_dev, int64_t x_b
  *              first target row: it also holds the listener's conv tails and block 0's K/V rings and (h, c), as the lead
  *              record g*K of a groups call does; the listener's other records never hold them.  A listener with no target
  *              row, or with a lead record outside the state, stores nothing at all.  The records of a listener advance
- *              together, so their clocks must start equal: start a listener's records together (l2h_sep_state_reset_streams
- *              of all of them); adding a record to a running listener is not supported.
+ *              together, so their clocks must be equal: start a listener's records together (l2h_sep_state_reset_streams
+ *              of all of them), or add a record to a running listener with l2h_sep_join_targets below.  Dropping a
+ *              non-lead row is leaving it out of the next call; dropping the lead is l2h_sep_state_move_lead first.
  *   workspace  l2h_sep_workspace_bytes(handle, n_rows, frames, flags)
  * All three lists are read when the kernels run: with L2H_FLAG_GRAPH one graph cached for (n, R, T) serves every tick, and
  * its key holds the list pointers, not their contents, so a caller rewrites records_dev, offsets_dev and hops_dev in place
@@ -295,6 +308,50 @@ int l2h_sep_forward_targets_rows(void* handle, const float* x_dev, int64_t x_bat
                                  int32_t n, int32_t n_rows, int32_t frames, float* y_dev, int64_t y_batch_stride,
                                  int64_t y_ch_stride, int32_t y_len, void* workspace_dev, size_t workspace_bytes,
                                  uint32_t flags, void* stream);
+/* Adding and dropping the targets of a running listener (INTEGRATION.md section 1).
+ *
+ * A block-0 history is hist_dev [state_batch][hist_frames][97*64] fp32 of DEVICE memory (24.8 KB per frame and record),
+ * keyed by record: the ring of the last hist_frames frames of block 0's output (before the speaker gate) of a listener's
+ * lead record, frame n of the record's own clock in slot n mod hist_frames.  Only leads' rings are written.
+ *
+ * l2h_sep_forward_targets_rows_history: l2h_sep_forward_targets_rows that also writes, for every listener that stores,
+ * its h frames of block 0's output into its lead's ring (its last hist_frames of them when h > hist_frames).  y, the state and every other output are those of
+ * l2h_sep_forward_targets_rows, bit for bit; the workspace is the same.  With L2H_FLAG_GRAPH the cached graph's key holds
+ * hist_dev and hist_frames.  Errors 1, before anything is enqueued: those of l2h_sep_forward_targets_rows, a null hist_dev,
+ * hist_frames < 1. */
+int l2h_sep_forward_targets_rows_history(void* handle, const float* x_dev, int64_t x_batch_stride, int64_t x_ch_stride,
+                                         int32_t x_len, const float* emb_dev, void* state_dev, int32_t state_batch,
+                                         const int32_t* records_dev, const int32_t* offsets_dev, const int32_t* hops_dev,
+                                         int32_t n, int32_t n_rows, int32_t frames, float* y_dev, int64_t y_batch_stride,
+                                         int64_t y_ch_stride, int32_t y_len, void* workspace_dev, size_t workspace_bytes,
+                                         uint32_t flags, void* stream, float* hist_dev, int32_t hist_frames);
+/* l2h_sep_join_targets: J new target records, each brought up to the clock of a running listener's lead, so that the next
+ * targets-rows call can list it among that listener's rows.  Row j:
+ *   records_dev[j]  the record that joins; leads_dev[j] the lead record of the listener it joins.  Both [J] int32 lists of
+ *              DEVICE memory, read when the kernels run (with L2H_FLAG_GRAPH the cached graph's key holds the pointers).
+ *              A row whose record or lead lies outside [0, state_batch), whose record is another row's record, or whose
+ *              record is a listed lead stores nothing (used 0).
+ *   W_j        the frames the row replays: min(frames, hist_frames, p), p the lead's clock; 0 without a history.
+ *   record     becomes a fresh record (as l2h_sep_state_reset_streams leaves it) with clock p - W_j, its gate memo is built
+ *              from emb_dev[j] ([J][256]), and blocks 1 .. B-1 and the back then run over frames p - W_j .. p - 1 of the
+ *              lead's history (the gate applied, as a targets call applies it): the record ends at clock p with its K/V
+ *              rings, (h, c) and deconv / iSTFT tails warmed.  With a history covering the whole stream it is the record
+ *              the target would have had, had it been listed from the start.  W_j = 0 (frames == 0, hist_dev NULL, or a
+ *              lead at clock 0) is a cold join: fresh deep state at the lead's clock, nothing computed past the gate memo.
+ *              The frames replayed must be in the lead's ring: every call that advanced the lead over them wrote it.
+ *   y_dev      [J][num_src][*]: row j receives samples 0 .. 128*W_j - 1 (the replayed frames' output); the rest is not
+ *              written.  May be NULL when no frame is replayed.
+ *   used_dev   [J] int32 of DEVICE memory receiving W_j (0 for a row that stores nothing), or NULL.
+ *   workspace  l2h_sep_workspace_bytes(handle, J, max(1, min(frames, hist_frames)), flags)
+ * The lead's record is only read.  The header advances as for any call when frames are replayed.  A join reads its leads'
+ * clocks and rings and shares the header's call counter with every call on the state, so it must be ordered with the
+ * state's ticks on one stream (or by events), never run beside one.
+ * Errors 1, before anything is enqueued: null pointers (y_dev only when frames are replayed), J <= 0, J > state_batch,
+ * frames < 0, hist_frames < 1 with a history, J*frames*97 rows beyond the limit of one call, L2H_FLAG_TAPS. */
+int l2h_sep_join_targets(void* handle, const int32_t* records_dev, const int32_t* leads_dev, const float* emb_dev, int32_t J,
+                         void* state_dev, int32_t state_batch, const float* hist_dev, int32_t hist_frames, int32_t frames,
+                         float* y_dev, int64_t y_batch_stride, int64_t y_ch_stride, int32_t* used_dev, void* workspace_dev,
+                         size_t workspace_bytes, uint32_t flags, void* stream);
 
 /* Streaming with HOST buffers (the end-to-end path).  Per round: H2D of the round's samples (+64
  * look-ahead) from pinned memory, the kernel chains, D2H of the new samples; one stream synchronise at

@@ -10,14 +10,15 @@ net), behind the reference's own Python call signatures.
     from lookoncetohear_b200 import HopFifo          # 16 kHz pieces of any length -> separator chunks and hop counts
     from lookoncetohear_b200 import EnrollCapture    # each listener's recent input, kept for EmbedTFGridNet.enroll
     from lookoncetohear_b200 import EnrollJob        # EmbedTFGridNet.enroll_job: an enrollment enqueued in slices
+    from lookoncetohear_b200 import TargetHistory    # Net.target_history: block 0's recent output, for Net.join_targets
 
 Compute happens only in lib/liblookonce_b200.so (hand-written sm_90a CUDA, C ABI declared in
 include/lookonce_b200.h); importing this package never falls back to PyTorch math.
 """
 from .embed import EmbedTFGridNet, EnrollJob  # noqa: F401
-from .net import Net, SepState  # noqa: F401
+from .net import Net, SepState, TargetHistory  # noqa: F401
 from .render import resample  # noqa: F401
 from .stream import EnrollCapture, HopFifo, PacketResampler, StreamResampler  # noqa: F401
 
-__all__ = ["Net", "SepState", "EmbedTFGridNet", "resample", "StreamResampler", "PacketResampler", "HopFifo",
+__all__ = ["Net", "SepState", "TargetHistory", "EmbedTFGridNet", "resample", "StreamResampler", "PacketResampler", "HopFifo",
            "EnrollCapture", "EnrollJob"]

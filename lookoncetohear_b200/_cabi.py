@@ -90,6 +90,18 @@ _SIGS = {
                                                    ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int64,
                                                    ctypes.c_int64, ctypes.c_int32, ctypes.c_void_p, ctypes.c_size_t,
                                                    ctypes.c_uint32, ctypes.c_void_p]),
+    "l2h_sep_forward_targets_rows_history": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64,
+                                                           ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
+                                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
+                                                           ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int64,
+                                                           ctypes.c_int64, ctypes.c_int32, ctypes.c_void_p, ctypes.c_size_t,
+                                                           ctypes.c_uint32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32]),
+    "l2h_sep_join_targets": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
+                                           ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
+                                           ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p,
+                                           ctypes.c_size_t, ctypes.c_uint32, ctypes.c_void_p]),
+    "l2h_sep_state_move_lead": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.POINTER(ctypes.c_int32),
+                                              ctypes.POINTER(ctypes.c_int32), ctypes.c_int32, ctypes.c_void_p]),
     "l2h_sep_stream_host": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p,
                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
                                           ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p,

@@ -319,6 +319,11 @@ struct ChainArgs {
                                          // 0: per listener, from `offsets`
     const int32_t* offsets = nullptr;    // targets == 0: [calls + 1] device list, mixture i owns target rows offsets[i] ..
     int calls = 0;                       // offsets[i+1]-1 (l2h_sep_forward_targets_rows); calls: the mixtures
+    float* hist = nullptr;               // a block-0 history [state_batch][hist_frames][97*64]: listed rows calls write their
+    int hist_frames = 0;                 // leads' frames into it, joins replay frames from it
+    const int32_t* leads = nullptr;      // a join (l2h_sep_join_targets): [B] device list, row j replays the history of leads[j]
+    int32_t* used = nullptr;             // ... and writes the frames it replays here (may be null)
+    int join_frames = 0;                 // ... at most this many (0: a cold join)
 };
 
 // few streams, one hop (the latency path): everything after the BiLSTM as one 16-CTA cluster kernel per stream, while all
@@ -406,11 +411,12 @@ struct Chain {
     float* X0;          // fans: block 0's input and output, the mixtures' rows
     int32_t* lists;     // listed groups or rows: the lists target_lists() builds (target_lists_kernel), B entries each:
                         // the target rows' records, their hops, their owners, then the M leads and the M + 1 row offsets
+    bool joins;         // a join (l2h_sep_join_targets): no front and no block 0; X0 holds frames of the leads' histories
     int tap = 0;
 
     Chain(SepEngine* e_, const ChainArgs& a_, cudaStream_t st_, const ChainForm& f_, Map recs_, const Workspace& ws)
         : e(e_), a(a_), st(st_), f(f_), recs(recs_), K(a_.targets), M(K > 0 ? a_.B / K : a_.calls), fans(K != 1),
-          ss(stream_stride(e_->n_blocks)) {
+          ss(stream_stride(e_->n_blocks)), joins(a_.leads != nullptr) {
         float* w = a.wsp;
         X = w + ws.X; GX = w + ws.GX; Y = w + ws.Y; Z = w + ws.Z; Q = w + ws.Q; KALL = w + ws.KALL; VALL = w + ws.VALL;
         PRE = w + ws.PRE; QKVRAW = w + ws.QKVRAW; TAPS = w + ws.TAPS; HG = w + ws.HG;
@@ -449,8 +455,13 @@ struct Chain {
             x0 = GX;
         }
         const int32_t* owner = nullptr;      // dense targets: row r belongs to mixture r / K
-        if constexpr (slots) owner = lists + 2 * (int64_t)a.B;
-        CK(launch_spk_gate(f.pdl, st, a.B, a.emb, PRE, a.state, recs, e->w));
+        if constexpr (slots) {
+            owner = lists + 2 * (int64_t)a.B;
+            // a rows call with a history: block 0's frames of every lead into its ring
+            if (a.hist && !joins) CK(launch_history_put(f.pdl, st, M, x0, a.state, lead, a.hist, a.hist_frames, a.T));
+        }
+        // a join built its rows' gate memos before the chain (enqueue_join)
+        if (!joins) CK(launch_spk_gate(f.pdl, st, a.B, a.emb, PRE, a.state, recs, e->w));
         CK(launch_gate_fanout(f.pdl, st, a.B, x0, X, (const float*)a.state, recs, owner, K, a.T, e->n_blocks > 1 ? 1 : 0));
         MARK("gate_fanout");
         return 0;
@@ -458,7 +469,11 @@ struct Chain {
     // listed groups or rows: the target rows' lists and the leads, before any kernel reads them
     int target_lists() {
         if constexpr (slots) {
-            if (fans) {
+            if (joins) {      // the lists and the fresh records are join_start_kernel's (enqueue_join); here block 0's output
+                              // of the replayed frames, from the leads' histories
+                CK(launch_history_get(f.pdl, st, a.B, a.hist, a.hist_frames, a.state, recs, a.leads, X0, a.T));
+                MARK("history_get");
+            } else if (fans) {
                 CK(launch_target_lists(st, a.offsets ? a.slots : nullptr, a.offsets, a.offsets ? nullptr : a.slots, a.hops, M, K, a.B,
                                        a.state_batch, lists));
                 MARK("target_lists");
@@ -543,7 +558,7 @@ struct Chain {
     int gather_hc() {
         if constexpr (slots) {
             if (f.tc_mid || a.T > 1) {
-                if (int rc = hc_copy(false, 0)) return rc;
+                if (!joins) { if (int rc = hc_copy(false, 0)) return rc; }
                 if (fans && e->n_blocks > 1) { if (int rc = hc_copy(false, 1)) return rc; }
             }
         }
@@ -569,7 +584,7 @@ struct Chain {
     }
     int scatter_hc() {
         if constexpr (slots) {
-            if (int rc = hc_copy(true, 0)) return rc;
+            if (!joins) { if (int rc = hc_copy(true, 0)) return rc; }
             if (fans && e->n_blocks > 1) { if (int rc = hc_copy(true, 1)) return rc; }
         }
         return 0;
@@ -593,7 +608,9 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
     if (int rc = c.gather_hc()) return rc;
     const BlockRows<Map> R0 = c.rows_of(0);           // the front runs over block 0's rows
     const int gate_ctas = c.fans ? 0 : 1;             // the front's speaker-gate memo CTAs (one per row); fan_out() builds them here
-    if (f.fused_tail) {      // the frame as 13 row tiles: spectrum of the tile's bins, conv, and block 0's input projection
+    if (c.joins) {
+        // a join starts at block 1: target_lists() filled block 0's output from the histories
+    } else if (f.fused_tail) {      // the frame as 13 row tiles: spectrum of the tile's bins, conv, and block 0's input projection
         CK(launch_front1(false, st, R0.B, gate_ctas, a.x, a.xbs, a.xcs, a.x_len, R0.X, a.state, R0.recs, e->w, e->bw[0], c.GX, a.pos_rel,
                          a.emb, c.PRE, a.active));
     } else if (f.walkers) {
@@ -606,7 +623,7 @@ static int enqueue_chain_t(SepEngine* e, const ChainArgs& a, cudaStream_t st, Ma
     MARK("front");
     if (int rc = c.do_tap()) return rc;
 
-    for (int b = 0; b < e->n_blocks; ++b) {
+    for (int b = c.joins ? 1 : 0; b < e->n_blocks; ++b) {
         if (c.fans_out_before(b)) { if (int rc = c.fan_out()) return rc; }
         const BlockRows<Map> R = c.rows_of(b);
         const BlockWeights& W = e->bw[b];
@@ -730,6 +747,26 @@ static int enqueue_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
     }
     if (a.slots) return enqueue_chain_t(e, a, st, Records{ss, a.slots, a.state_batch, a.hops, a.T});
     return enqueue_chain_t(e, a, st, ss);
+}
+
+// A join (l2h_sep_join_targets, rows a.B = J, frames a.T = max(1, a.join_frames)): the rows' fresh records at their leads'
+// clocks and the rows' lists (join_start_kernel), their gate memos, and, when frames are replayed, the chain from block 1
+// over them (Chain::joins) as a ragged listed-rows call: row j advances its used[j] frames.
+static int enqueue_join(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
+    if (!e->pack.committed) return fail(4, "weights not committed");
+    const Workspace ws = carve(e->n_blocks, a.B, a.T, a.flags);
+    if ((size_t)ws.total * sizeof(float) > a.ws_bytes) return fail(1, "workspace too small");
+    if (int rc = set_attrs()) return rc;
+    const int64_t ss = stream_stride(e->n_blocks);
+    int32_t* lists = reinterpret_cast<int32_t*>(a.wsp + ws.LISTS);
+    CK(launch_join_start(st, a.B, a.state, ss, a.state_batch, a.slots, a.leads, a.join_frames, lists, a.used));
+    CK(launch_spk_gate(false, st, a.B, a.emb, a.wsp + ws.PRE, a.state, Records{ss, lists, a.state_batch, nullptr, a.T}, e->w));
+    if (a.join_frames == 0) return 0;      // a cold join
+    return enqueue_chain_t(e, a, st, Records{ss, lists, a.state_batch, lists + a.B, a.T});
+}
+
+static int enqueue_call(SepEngine* e, const ChainArgs& a, cudaStream_t st) {
+    return a.leads ? enqueue_join(e, a, st) : enqueue_chain(e, a, st);
 }
 
 // ---- wavefront pipeline over (block, frame) for one-frame calls ---------------------------------------
@@ -968,7 +1005,8 @@ static void drop_graphs(SepEngine* e) {
 static std::vector<int64_t> graph_key(const ChainArgs& a, int t) {
     return {(int64_t)a.x, a.xbs, a.xcs, a.x_len, (int64_t)a.emb, (int64_t)a.state, (int64_t)a.y,
             a.ybs, a.ycs, a.y_len, a.B, t, (int64_t)a.wsp, (int64_t)a.flags, a.pos_rel, (int64_t)a.active,
-            (int64_t)a.slots, a.state_batch, (int64_t)a.hops, a.targets, (int64_t)a.offsets, a.calls};
+            (int64_t)a.slots, a.state_batch, (int64_t)a.hops, a.targets, (int64_t)a.offsets, a.calls,
+            (int64_t)a.hist, a.hist_frames, (int64_t)a.leads, (int64_t)a.used, a.join_frames};
 }
 
 // Launch the graph cached under `key` on `st`.  The first time a key is seen, `enqueue(cap)` is captured on the private
@@ -1007,11 +1045,11 @@ static int run_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_t st
 static int run_chain(SepEngine* e, const ChainArgs& a, cudaStream_t st, bool use_graph) {
     if (!use_graph || (a.flags & L2H_FLAG_TAPS)) {
         const long long before = g_launches;
-        const int rc = enqueue_chain(e, a, st);
+        const int rc = enqueue_call(e, a, st);
         e->launch_count += g_launches - before;
         return rc;
     }
-    return run_graph(e, graph_key(a, a.T), e->cap_stream, st, [&](cudaStream_t cs) { return enqueue_chain(e, a, cs); });
+    return run_graph(e, graph_key(a, a.T), e->cap_stream, st, [&](cudaStream_t cs) { return enqueue_call(e, a, cs); });
 }
 
 }  // namespace l2h
@@ -1212,6 +1250,47 @@ int l2h_sep_state_copy_streams(void* handle, void* dst_state, int32_t dst_batch,
     return 0;
 }
 
+int l2h_sep_state_move_lead(void* handle, void* state, int32_t batch, const int32_t* old_host, const int32_t* new_host, int32_t n,
+                            void* stream) {
+    SepEngine* e = static_cast<SepEngine*>(handle);
+    if (!e || !state || !old_host || !new_host) return fail(1, "null argument");
+    if (batch <= 0 || n <= 0 || n > batch) return fail(1, "batch and the record count must be positive, records at most batch");
+    if (int rc = check_slots(old_host, n, batch, "move_lead (old leads)")) return rc;
+    if (int rc = check_slots(new_host, n, batch, "move_lead (new leads)")) return rc;
+    std::vector<char> is_old((size_t)batch, 0);
+    for (int32_t i = 0; i < n; ++i) is_old[(size_t)old_host[i]] = 1;
+    for (int32_t i = 0; i < n; ++i)
+        if (is_old[(size_t)new_host[i]])
+            return fail(1, "move_lead: record " + std::to_string(new_host[i]) + " is both an old and a new lead");
+    if (int rc = check_device(e)) return rc;
+    const int64_t ss = stream_stride(e->n_blocks);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    float* rec = static_cast<float*>(state) + sizeof(StateHeader) / 4;
+    // the clocks, as the work queued before this call leaves them: a lead moves only between records of one listener
+    std::vector<long long> clk(2 * (size_t)n);
+    for (int32_t i = 0; i < n; ++i) {
+        CK(cudaMemcpyAsync(&clk[2 * i], rec + (int64_t)old_host[i] * ss + ST_POS, sizeof(long long), cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(&clk[2 * i + 1], rec + (int64_t)new_host[i] * ss + ST_POS, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    }
+    CK(cudaStreamSynchronize(st));
+    for (int32_t i = 0; i < n; ++i)
+        if (clk[2 * i] != clk[2 * i + 1])
+            return fail(1, "move_lead: records " + std::to_string(old_host[i]) + " and " + std::to_string(new_host[i]) +
+                               " have different clocks (" + std::to_string(clk[2 * i]) + " and " + std::to_string(clk[2 * i + 1]) +
+                               " frames)");
+    for (int32_t i0 = 0; i0 < n; i0 += MOVE_MAX_PAIRS) {
+        const int32_t k = std::min<int32_t>(MOVE_MAX_PAIRS, n - i0);
+        PairList pl{};
+        std::copy(old_host + i0, old_host + i0 + k, pl.from);
+        std::copy(new_host + i0, new_host + i0 + k, pl.to);
+        const unsigned per_rec = (unsigned)std::max(1, 2 * NUM_SMS / k);      // as reset_streams: ~2 CTAs per SM over all records
+        move_lead_kernel<<<dim3(per_rec, k), 256, 0, st>>>(static_cast<float*>(state), ss, pl);
+        CK(cudaGetLastError());
+        e->launch_count += 1;
+    }
+    return 0;
+}
+
 int l2h_sep_workspace_bytes(void* handle, int32_t batch, int32_t frames, uint32_t flags, size_t* bytes) {
     SepEngine* e = static_cast<SepEngine*>(handle);
     if (!e || !bytes || batch <= 0 || frames <= 0) return fail(1, "bad argument");
@@ -1348,10 +1427,10 @@ int l2h_sep_forward_targets_groups(void* handle, const float* x, int64_t xbs, in
     return run_chain(e, a, static_cast<cudaStream_t>(stream), (flags & L2H_FLAG_GRAPH) != 0);
 }
 
-int l2h_sep_forward_targets_rows(void* handle, const float* x, int64_t xbs, int64_t xcs, int32_t x_len, const float* emb,
-                                 void* state, int32_t state_batch, const int32_t* records_dev, const int32_t* offsets_dev,
-                                 const int32_t* hops_dev, int32_t n, int32_t n_rows, int32_t frames, float* y, int64_t ybs,
-                                 int64_t ycs, int32_t y_len, void* ws, size_t ws_bytes, uint32_t flags, void* stream) {
+static int targets_rows(void* handle, const float* x, int64_t xbs, int64_t xcs, int32_t x_len, const float* emb, void* state,
+                        int32_t state_batch, const int32_t* records_dev, const int32_t* offsets_dev, const int32_t* hops_dev,
+                        int32_t n, int32_t n_rows, int32_t frames, float* y, int64_t ybs, int64_t ycs, int32_t y_len, void* ws,
+                        size_t ws_bytes, uint32_t flags, void* stream, float* hist, int32_t hist_frames) {
     SepEngine* e = static_cast<SepEngine*>(handle);
     if (!e || !x || !emb || !state || !y || !ws || !records_dev || !offsets_dev) return fail(1, "null argument");
     if (n <= 0 || n_rows <= 0 || frames <= 0)
@@ -1373,6 +1452,57 @@ int l2h_sep_forward_targets_rows(void* handle, const float* x, int64_t xbs, int6
     a.targets = 0;
     a.offsets = offsets_dev;
     a.calls = n;
+    a.hist = hist;
+    a.hist_frames = hist_frames;
+    return run_chain(e, a, static_cast<cudaStream_t>(stream), (flags & L2H_FLAG_GRAPH) != 0);
+}
+
+int l2h_sep_forward_targets_rows(void* handle, const float* x, int64_t xbs, int64_t xcs, int32_t x_len, const float* emb,
+                                 void* state, int32_t state_batch, const int32_t* records_dev, const int32_t* offsets_dev,
+                                 const int32_t* hops_dev, int32_t n, int32_t n_rows, int32_t frames, float* y, int64_t ybs,
+                                 int64_t ycs, int32_t y_len, void* ws, size_t ws_bytes, uint32_t flags, void* stream) {
+    return targets_rows(handle, x, xbs, xcs, x_len, emb, state, state_batch, records_dev, offsets_dev, hops_dev, n, n_rows, frames, y,
+                        ybs, ycs, y_len, ws, ws_bytes, flags, stream, nullptr, 0);
+}
+
+int l2h_sep_forward_targets_rows_history(void* handle, const float* x, int64_t xbs, int64_t xcs, int32_t x_len, const float* emb,
+                                         void* state, int32_t state_batch, const int32_t* records_dev, const int32_t* offsets_dev,
+                                         const int32_t* hops_dev, int32_t n, int32_t n_rows, int32_t frames, float* y, int64_t ybs,
+                                         int64_t ycs, int32_t y_len, void* ws, size_t ws_bytes, uint32_t flags, void* stream,
+                                         float* hist_dev, int32_t hist_frames) {
+    if (!hist_dev) return fail(1, "null argument: hist_dev");
+    if (hist_frames < 1) return fail(1, "a history needs hist_frames >= 1 (hist_frames = " + std::to_string(hist_frames) + ")");
+    return targets_rows(handle, x, xbs, xcs, x_len, emb, state, state_batch, records_dev, offsets_dev, hops_dev, n, n_rows, frames, y,
+                        ybs, ycs, y_len, ws, ws_bytes, flags, stream, hist_dev, hist_frames);
+}
+
+int l2h_sep_join_targets(void* handle, const int32_t* records_dev, const int32_t* leads_dev, const float* emb, int32_t J, void* state,
+                         int32_t state_batch, const float* hist_dev, int32_t hist_frames, int32_t frames, float* y, int64_t ybs,
+                         int64_t ycs, int32_t* used_dev, void* ws, size_t ws_bytes, uint32_t flags, void* stream) {
+    SepEngine* e = static_cast<SepEngine*>(handle);
+    if (!e || !records_dev || !leads_dev || !emb || !state || !ws) return fail(1, "null argument");
+    if (J <= 0 || J > state_batch)
+        return fail(1, "a join needs 0 < J <= state_batch (J = " + std::to_string(J) + ", state_batch = " + std::to_string(state_batch) +
+                           ")");
+    if (frames < 0) return fail(1, "a join needs frames >= 0 (frames = " + std::to_string(frames) + ")");
+    if (hist_dev && hist_frames < 1)
+        return fail(1, "a history needs hist_frames >= 1 (hist_frames = " + std::to_string(hist_frames) + ")");
+    const int replay = hist_dev ? std::min(frames, hist_frames) : 0;      // the most frames a row replays
+    if (replay > 0 && !y) return fail(1, "null argument: y_dev (the join replays frames)");
+    if ((int64_t)J * replay * NF > 0x7fffffff / 2) return fail(1, "J*frames too large for one call; split the rows");
+    if (flags & L2H_FLAG_TAPS) return fail(1, "a join cannot be combined with L2H_FLAG_TAPS");
+    if (int rc_dev = check_device(e)) return rc_dev;
+    ChainArgs a{nullptr, 0, 0, 0, emb, static_cast<float*>(state), y, ybs, ycs, HOP * replay, J, std::max(1, replay),
+                static_cast<float*>(ws), ws_bytes, flags & ~L2H_FLAG_GRAPH, 0};
+    a.slots = records_dev;
+    a.state_batch = state_batch;
+    a.targets = 0;
+    a.calls = J;
+    a.hist = const_cast<float*>(hist_dev);
+    a.hist_frames = hist_dev ? hist_frames : 0;
+    a.leads = leads_dev;
+    a.used = used_dev;
+    a.join_frames = replay;
     return run_chain(e, a, static_cast<cudaStream_t>(stream), (flags & L2H_FLAG_GRAPH) != 0);
 }
 

@@ -154,4 +154,118 @@ inline cudaError_t launch_target_lists(cudaStream_t st, const int32_t* records, 
                     lists + R, lists + 2 * R, lists + 3 * R, lists + 4 * R);
 }
 
+// ---- adding and dropping the targets of a running listener (l2h_sep_forward_targets_rows_history, l2h_sep_join_targets,
+// l2h_sep_state_move_lead) ---------------------------------------------------------------------------------------------
+// A block-0 history is [state batch][F][97*64] fp32, keyed by record: the ring of the last F frames of block 0's ungated
+// output of a lead record, frame n of the record's own clock in slot n mod F.
+
+// Rows tick: listener i's last min(h_i, F) frames of block 0's output X0 [M][T][97][64] (frames h_i - F <= t < h_i) go into
+// the ring of its lead record, at the lead's clock from before the call: no two CTAs write one slot, and a tick of more
+// frames than the ring holds leaves its last F.  `lead` is the map of block 0's rows (the lead list and the listeners'
+// hop counts): a listener that stores nothing writes nothing.  grid (T, M), 256 threads.
+__global__ void __launch_bounds__(256)
+history_put_kernel(const float* __restrict__ X0, const float* __restrict__ state, Records lead, float* __restrict__ hist, int F,
+                   int T) {
+    griddep_launch();
+    griddep_wait();
+    const int t = blockIdx.x, i = blockIdx.y;
+    const RowRecord r = row_record(lead, nullptr, i);
+    const int h = row_frames(lead, i, T);
+    if (!r.stores || t >= h || t + F < h) return;
+    const long long fr = rec_pos(state + r.off) + t;
+    const float4* src = reinterpret_cast<const float4*>(X0 + ((int64_t)i * T + t) * FC);
+    float4* dst = reinterpret_cast<float4*>(hist + ((int64_t)__ldg(lead.slots + i) * F + (int)(fr % F)) * FC);
+    for (int j = threadIdx.x; j < FC / 4; j += 256) dst[j] = src[j];
+}
+
+// Join, first kernel: row j is live when records[j] and leads[j] both lie in [0, batch), and records[j] is neither another
+// row's record nor any row's lead (such rows would race with each other; they store nothing).  Its record becomes a fresh record,
+// as reset_streams_kernel leaves it, except for its clock: p - W_j, where p is the clock of leads[j] and W_j = min(w_max, p)
+// the frames the row replays.  CTA 0 of each row also writes the row's entries of the call's lists: rec[j] (the record, -1
+// for a row that is not live), used[j] = W_j (0 if not live), owner[j] (j, -1 if not live), and used_out[j] if given.
+// grid (any, J), 256 threads.
+static_assert(ST_GEN % 4 == 0 && ST_CALLS == ST_GEN + 1 && ST_POS == ST_GEN + 2, "one float4 holds the memo generation and clock");
+__global__ void __launch_bounds__(256)
+join_start_kernel(float* __restrict__ state, int64_t ss, int batch, const int32_t* __restrict__ records,
+                  const int32_t* __restrict__ leads, int w_max, int32_t* __restrict__ rec, int32_t* __restrict__ used,
+                  int32_t* __restrict__ owner, int32_t* __restrict__ used_out, int J) {
+    const int j = blockIdx.y;
+    const int s = __ldg(records + j), l = __ldg(leads + j);
+    bool clash = false;
+    for (int k = threadIdx.x; k < J; k += blockDim.x) clash |= (k != j && __ldg(records + k) == s) || __ldg(leads + k) == s;
+    const bool live = !__syncthreads_or(clash) && (unsigned)s < (unsigned)batch && (unsigned)l < (unsigned)batch;
+    const long long p = live ? rec_pos(stream_rec(state, ss, l)) : 0;
+    const int W = (int)min((long long)w_max, p);
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        rec[j] = live ? s : -1;
+        used[j] = live ? W : 0;
+        owner[j] = live ? j : -1;
+        if (used_out != nullptr) used_out[j] = live ? W : 0;
+    }
+    if (!live) return;
+    float4* r = reinterpret_cast<float4*>(stream_rec(state, ss, s));
+    const long long start = p - W;
+    const float nan = __int_as_float(0x7fc00000);
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < ss / 4; i += (int64_t)gridDim.x * blockDim.x)
+        r[i] = i < SPK / 4 ? make_float4(nan, nan, nan, nan)
+             : i == ST_GEN / 4 ? make_float4(0.f, 0.f, __int_as_float((int)(start & 0xffffffffLL)), __int_as_float((int)(start >> 32)))
+                               : make_float4(0.f, 0.f, 0.f, 0.f);
+}
+
+// Join, the replayed frames: X0[j][t] = frame (clock of record j) + t of the ring of leads[j], for t < used[j]; the other
+// frames (and rows that are not live) are zero.  `recs` is the join's row map (rec, used).  grid (T, J), 256 threads.
+__global__ void __launch_bounds__(256)
+history_get_kernel(const float* __restrict__ hist, int F, const float* __restrict__ state, Records recs,
+                   const int32_t* __restrict__ leads, float* __restrict__ X0, int T) {
+    griddep_launch();
+    griddep_wait();
+    const int t = blockIdx.x, j = blockIdx.y;
+    const RowRecord r = row_record(recs, nullptr, j);
+    float4* dst = reinterpret_cast<float4*>(X0 + ((int64_t)j * T + t) * FC);
+    if (!r.stores || t >= row_frames(recs, j, T)) {
+        for (int i = threadIdx.x; i < FC / 4; i += 256) dst[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+        return;
+    }
+    const long long fr = rec_pos(state + r.off) + t;
+    const float4* src = reinterpret_cast<const float4*>(hist + ((int64_t)__ldg(leads + j) * F + (int)(fr % F)) * FC);
+    for (int i = threadIdx.x; i < FC / 4; i += 256) dst[i] = src[i];
+}
+
+// l2h_sep_state_move_lead: the speaker-independent part of record olds[i] goes to record news[i]: block 0 (K/V rings and
+// (h, c)) whole, and the current copy of the conv tails (parity of olds[i]'s calls) into the copy news[i]'s parity makes
+// current.  Nothing else of news[i] changes.  grid (any, n), 256 threads.
+constexpr int MOVE_MAX_PAIRS = RESET_MAX_SLOTS / 2;      // the kernel parameters stay under 4 KB
+struct PairList { int32_t from[MOVE_MAX_PAIRS], to[MOVE_MAX_PAIRS]; };
+__global__ void __launch_bounds__(256)
+move_lead_kernel(float* __restrict__ state, int64_t ss, PairList pairs) {
+    constexpr int64_t CONV = 2 * 4 * NF;                   // one parity of the conv tails
+    static_assert(CONV % 4 == 0, "float4 copies");
+    const float* src = stream_rec(state, ss, pairs.from[blockIdx.y]);
+    float* dst = stream_rec(state, ss, pairs.to[blockIdx.y]);
+    const float4* s0 = reinterpret_cast<const float4*>(src + ST_BLK);
+    float4* d0 = reinterpret_cast<float4*>(dst + ST_BLK);
+    const float4* sc = reinterpret_cast<const float4*>(src + ST_CONV + rec_par(src) * CONV);
+    float4* dc = reinterpret_cast<float4*>(dst + ST_CONV + rec_par(dst) * CONV);
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < BK_STRIDE / 4 + CONV / 4; i += (int64_t)gridDim.x * blockDim.x) {
+        if (i < BK_STRIDE / 4) d0[i] = s0[i];
+        else dc[i - BK_STRIDE / 4] = sc[i - BK_STRIDE / 4];
+    }
+}
+
+inline cudaError_t launch_history_put(bool pdl, cudaStream_t st, int M, const float* X0, const float* state, Records lead, float* hist,
+                                      int F, int T) {
+    return launch_k(pdl, history_put_kernel, dim3(T, M), dim3(256), 0, st, X0, state, lead, hist, F, T);
+}
+inline cudaError_t launch_join_start(cudaStream_t st, int J, float* state, int64_t ss, int batch, const int32_t* records,
+                                     const int32_t* leads, int w_max, int32_t* lists, int32_t* used_out) {
+    const int64_t R = J;
+    const unsigned per_rec = (unsigned)std::max(1, 2 * NUM_SMS / J);      // as reset_streams: ~2 CTAs per SM over all records
+    return launch_k(false, join_start_kernel, dim3(per_rec, J), dim3(256), 0, st, state, ss, batch, records, leads, w_max, lists,
+                    lists + R, lists + 2 * R, used_out, J);
+}
+inline cudaError_t launch_history_get(bool pdl, cudaStream_t st, int J, const float* hist, int F, const float* state, Records recs,
+                                      const int32_t* leads, float* X0, int T) {
+    return launch_k(pdl, history_get_kernel, dim3(T, J), dim3(256), 0, st, hist, F, state, recs, leads, X0, T);
+}
+
 }  // namespace l2h

@@ -261,6 +261,62 @@ class SepState(dict):
         staged._rec().copy_(src_state._rec()[list(ss)].cpu().to(dev))
         return self.copy_streams_from(staged, list(range(len(ss))), list(ds))
 
+    def move_lead(self, old, new):
+        """Hand the lead of a listener from record old[i] to record new[i], another record of the same listener, so that
+        old[i] can be dropped from its rows (l2h_sep_state_move_lead): block 0's rings and (h, c) and the current conv tails
+        of old[i] are copied into new[i], whose own blocks 1 .., back tails, gate memo and clock stay.  The clocks must be
+        equal (ValueError otherwise); the call waits for the current stream to read them.  Move a TargetHistory's rings
+        with it (TargetHistory.move)."""
+        h, L = self._engine_call()
+        o, nw = self._slots(old), self._slots(new)
+        if len(o) != len(nw):
+            raise ValueError("move_lead: old and new differ in length")
+        with torch.cuda.device(self.buf.device):
+            _cabi.check_args(L.l2h_sep_state_move_lead(h, self.buf.data_ptr(), self.batch, o, nw, len(o),
+                                                       torch.cuda.current_stream(self.buf.device).cuda_stream))
+        return self
+
+
+class TargetHistory:
+    """The block-0 history of a state's listeners (Net.target_history): ``buf`` [state.batch, frames, 97*64] fp32 on the
+    state's device, record r's row the ring of the last `frames` frames of block 0's output (before the speaker gate) of
+    r as a listener's lead, frame n of r's own clock in slot n mod frames.  advance_target_rows(history=) writes the rings
+    of the leads it advances; Net.join_targets replays them.  24.8 KB per frame and record: 64 frames x 256 records take
+    407 MB."""
+
+    def __init__(self, state, frames):
+        if not isinstance(state, SepState):
+            raise TypeError("state must come from Net.init_buffers()")
+        if isinstance(frames, bool) or not isinstance(frames, int) or frames < 1:
+            raise ValueError(f"a history needs frames >= 1, got {frames!r}")
+        self.state, self.frames = state, frames
+        self.buf = torch.zeros(state.batch, frames, 97 * 64, dtype=torch.float32, device=state.buf.device)
+
+    def check(self, state):
+        """ValueError unless this is a history of `state` of the layout the engine reads"""
+        if state is not self.state and state.buf.data_ptr() != self.state.buf.data_ptr():
+            raise ValueError("this history belongs to another state")
+        shape = (state.batch, self.frames, 97 * 64)
+        if (tuple(self.buf.shape) != shape or self.buf.dtype != torch.float32 or not self.buf.is_contiguous()
+                or self.buf.device != state.buf.device):
+            raise ValueError(f"a history must be a contiguous float32 tensor of shape {shape} on {state.buf.device}, got "
+                             f"{tuple(self.buf.shape)} {self.buf.dtype} on {self.buf.device}")
+
+    def reset(self, records):
+        """Zero the rings of `records` (a listener starting afresh in them)."""
+        r = torch.as_tensor(SepState._slots(records)[:], dtype=torch.int64, device=self.buf.device)
+        self.buf.index_fill_(0, r, 0.0)
+        return self
+
+    def move(self, src, dst):
+        """The ring of record src[i] becomes record dst[i]'s, with SepState.move_lead."""
+        s = torch.as_tensor(SepState._slots(src)[:], dtype=torch.int64, device=self.buf.device)
+        d = torch.as_tensor(SepState._slots(dst)[:], dtype=torch.int64, device=self.buf.device)
+        if s.numel() != d.numel():
+            raise ValueError("move: src and dst differ in length")
+        self.buf.index_copy_(0, d, self.buf.index_select(0, s))
+        return self
+
 
 # the wording of device_list's errors per list: what its entries are, a wrong count, an entry outside [0, end)
 _LIST_WORDS = {"slot": ("integer slot indices", "slots lists {} records for {} input rows",
@@ -271,6 +327,8 @@ _LIST_WORDS = {"slot": ("integer slot indices", "slots lists {} records for {} i
                           "a record lies outside [0, {end})"),
                "offset": ("integer row offsets", "offsets gives {} entries for {} = input rows + 1",
                           "an offset lies outside [0, {last}] (the call's {last} target rows)"),
+               "lead": ("integer record indices", "leads lists {} records for {} joining records",
+                        "a lead lies outside [0, {end})"),
                "count": ("integer sample counts", "counts gives {} counts for {} input rows",
                          "a count lies outside [0, {last}] (the units one input row holds)")}
 
@@ -400,7 +458,7 @@ class Net(nn.Module):
         return self._cached_workspace(device, _cabi.lib().l2h_sep_stream_workspace_bytes, batch, chunks_per_call)
 
     def _launch(self, entry, x, emb, state, y, frames, flags=0, mask=None, slots=None, hops=None, K=1, ws=None,
-                offsets=None):
+                offsets=None, history=None):
         """Run the separator forward C entry point `entry` on the current stream of x's device, on the caller's tensors as
         they are (a service's fixed buffers keep the cached graph's key).  entry: "forward", "forward_active", "slots",
         "slots_frames", "slots_hops", "targets", "targets_groups" or "targets_rows" (l2h_sep_forward,
@@ -410,8 +468,9 @@ class Net(nn.Module):
         [rows, S, N] view; rows = rows_x * K, or for targets_rows the target rows of y.  mask: the [rows] uint8 activity
         mask of forward_active (None: all); slots: the int32 slot list (the group list of targets_groups, the record list
         of targets_rows); offsets: the int32 [rows_x + 1] row offsets of targets_rows; hops: the int32 hop counts (None:
-        every row all frames).  ws: a workspace to use, else the net's own, sized for rows and frames.  A rejected argument
-        raises ValueError, except on the dense entries, where every error is a RuntimeError."""
+        every row all frames).  ws: a workspace to use, else the net's own, sized for rows and frames.  history: with
+        targets_rows, a TargetHistory the call writes (l2h_sep_forward_targets_rows_history).  A rejected argument raises
+        ValueError, except on the dense entries, where every error is a RuntimeError."""
         dev = x.device
         self._sync_weights(dev)
         if y.dim() == 4:
@@ -439,6 +498,9 @@ class Net(nn.Module):
                 args = (*head, *out, n, K, frames, *tail)
             elif entry == "targets_rows":
                 args = (*head, *listed, offsets.data_ptr(), hop_list, n, y.shape[0], frames, *out, *tail)
+                if history is not None:
+                    entry = "targets_rows_history"
+                    args = (*args, history.buf.data_ptr(), history.frames)
             else:
                 args = (*head, *listed, hop_list, n, K, frames, *out, *tail)
             fn = getattr(_cabi.lib(), "l2h_sep_" + entry if entry.startswith("forward") else "l2h_sep_forward_" + entry)
@@ -698,7 +760,7 @@ class Net(nn.Module):
         groups = self._slot_list(groups, x.device, n, state.batch // K)
         return self._run_targets("targets_groups", x, embeds, state, frames, out_len, groups, hops)
 
-    def advance_target_rows(self, x, embeds, state, records, offsets, hops=None):
+    def advance_target_rows(self, x, embeds, state, records, offsets, hops=None, history=None):
         """Advance listeners who each enrolled their own number of speakers by T hops each, in one call
         (l2h_sep_forward_targets_rows): advance_targets without its one K for every listener.  x [n, M, 128*T + 64] (the
         pad=False shape), row i listener i's mixture; embeds [R, 256], one row per target row; listener i owns target rows
@@ -707,13 +769,18 @@ class Net(nn.Module):
         are left unwritten, so one fixed R carries any number of live targets.
 
         A listener's lead record, records[offsets[i]], also holds its mixture's front and block 0; its other records never
-        do, so reset a listener's records together (reset_streams of all of them) before its first call.  Records need not
-        be adjacent or in order.  Host lists (sequences or CPU tensors) are checked and uploaded: `records` R distinct ints
+        do, so reset a listener's records together (reset_streams of all of them) before its first call, or add a record
+        to a running listener with join_targets.  Drop a target by leaving its row out of the next call; drop a lead with
+        state.move_lead first.  Records need not be adjacent or in order.  Host lists (sequences or CPU tensors) are checked and uploaded: `records` R distinct ints
         in [0, state.batch); `offsets` n + 1 ints from 0, non-decreasing, at most R; `hops` as for advance_targets (None:
         every listener advances T hops; else h_i in [0, T], and listener i's rows receive y[r, :, :128*h_i] only).  CUDA
         int32 tensors are used in place and read when the kernels run: there a record outside the state marks a row that
         stores nothing, and the engine clamps the offsets to be non-decreasing and at most R.  With fixed tensors rewritten in
-        place every tick, one cached graph per (n, R, T) serves every mix of listeners."""
+        place every tick, one cached graph per (n, R, T) serves every mix of listeners.
+
+        history: None, or a TargetHistory of `state` (target_history): the call also writes each listener's advanced
+        frames of block 0's output into its lead's ring, for join_targets to replay; y and the state are those of the call
+        without it, bit for bit."""
         if x.dim() != 3:
             raise ValueError(f"advance_target_rows needs x of shape [n, channels, {self.stft_chunk_size}*T+"
                              f"{self.stft_pad_size}], got {tuple(x.shape)}")
@@ -730,6 +797,10 @@ class Net(nn.Module):
         dev = x.device
         if hops is not None:
             hops = self._hop_counts(hops, dev, n, frames)
+        if history is not None:
+            if not isinstance(history, TargetHistory):
+                raise TypeError("history must come from Net.target_history()")
+            history.check(state)
         records = device_list(records, dev, R, state.batch, True, "record")
         on_host = not (isinstance(offsets, torch.Tensor) and offsets.is_cuda)
         offsets_dev = device_list(offsets, dev, n + 1, R + 1, False, "offset")
@@ -740,8 +811,89 @@ class Net(nn.Module):
         self._require_cuda(x)
         y = torch.empty(R, self.num_src, out_len, dtype=torch.float32, device=dev)
         self._launch("targets_rows", x.contiguous().float(), embeds.to(dev, torch.float32).contiguous(), state, y, frames,
-                     slots=records, hops=hops, offsets=offsets_dev)
+                     slots=records, hops=hops, offsets=offsets_dev, history=history)
         return y
+
+    def target_history(self, state, frames):
+        """A block-0 history of `frames` frames for the listeners of `state` (TargetHistory), zeroed: pass it to every
+        advance_target_rows of those listeners, and join_targets can bring a new target up to a listener's clock."""
+        return TargetHistory(state, frames)
+
+    def join_targets(self, state, records, leads, embeds, history=None, frames=None, out=None, used=None, flags=0, ws=None):
+        """Add target records to running listeners (l2h_sep_join_targets): record records[j] joins the listener whose lead
+        record is leads[j], with embedding embeds[j] ([J, 256]).  The record becomes a fresh record at the lead's clock p
+        minus W_j = min(frames, history.frames, p), its gate memo is built, and blocks 1 .. B-1 and the back replay those
+        W_j frames of the lead's history, so it ends at clock p, warm.  With a history that covers the whole stream it is
+        the record the target would have had from the start.  frames: None (history.frames, or 0 without a history); 0 or
+        no history is a cold join (fresh deep state at the lead's clock).  Then list records[j] among the listener's rows
+        in the next advance_target_rows.
+
+        Returns (y [J, S, 128*frames], used [J] int32 on the device): row j of y holds the output of the W_j replayed
+        frames in its first 128*W_j samples, the rest is left unwritten; used[j] = W_j.  out / used: fixed tensors to write
+        instead (a service's buffers keep the cached graph's key with flags=L2H_FLAG_GRAPH).  Host lists are checked:
+        records J distinct ints and leads J ints in [0, state.batch), no record equal to any listed lead.  CUDA int32
+        tensors are used in place and read when the kernels run: there a record or lead outside the state, a record
+        listed twice or a record equal to a listed lead marks a row that stores nothing (used 0).
+
+        ws: a uint8 CUDA tensor of at least l2h_sep_workspace_bytes(J, max(1, min(frames, history.frames))) bytes to use,
+        else the net's own workspace, grown if the join needs more than it holds.  The ticks' cached graphs are keyed on
+        their workspace, so a service passes its own buffer here (or one to the ticks) and no tick recaptures its graph
+        after a join.  A join reads its leads' clocks and rings and counts as a call of its state: enqueue it on the
+        stream of that state's ticks, never beside one."""
+        if not isinstance(state, SepState):
+            raise TypeError("state must come from Net.init_buffers()")
+        if not isinstance(embeds, torch.Tensor) or embeds.dim() != 2 or embeds.shape[1] != self.embed_dim:
+            shape = tuple(embeds.shape) if isinstance(embeds, torch.Tensor) else type(embeds).__name__
+            raise ValueError(f"embeds must have shape [J, {self.embed_dim}], one row per joining record, got {shape}")
+        J = embeds.shape[0]
+        if not 0 < J <= state.batch:
+            raise ValueError(f"join_targets needs 0 < J <= state.batch, got J = {J} and a state of {state.batch} records")
+        if history is not None:
+            if not isinstance(history, TargetHistory):
+                raise TypeError("history must come from Net.target_history()")
+            history.check(state)
+        if frames is None:
+            frames = history.frames if history is not None else 0
+        if isinstance(frames, bool) or not isinstance(frames, int) or frames < 0:
+            raise ValueError(f"frames must be an int >= 0, got {frames!r}")
+        dev = state.buf.device
+        # a CUDA list is read when the kernels run: join_start_kernel makes a clashing row store nothing
+        if not (isinstance(records, torch.Tensor) and records.is_cuda) and not (isinstance(leads, torch.Tensor) and leads.is_cuda):
+            r, l = torch.as_tensor(records).flatten().tolist(), torch.as_tensor(leads).flatten().tolist()
+            if set(r) & set(l):
+                raise ValueError(f"a joining record is a listed lead: {sorted(set(r) & set(l))}")
+        records = device_list(records, dev, J, state.batch, True, "record")
+        leads = device_list(leads, dev, J, state.batch, False, "lead")
+        replay = min(frames, history.frames) if history is not None else 0
+        y = out if out is not None else torch.empty(J, self.num_src, 128 * frames, dtype=torch.float32, device=dev)
+        if (not isinstance(y, torch.Tensor) or y.dim() != 3 or y.shape[0] != J or y.shape[1] != self.num_src
+                or y.shape[2] < 128 * replay or y.stride(2) != 1 or y.dtype != torch.float32 or y.device != dev):
+            shape = (tuple(y.shape), y.dtype, y.device) if isinstance(y, torch.Tensor) else type(y).__name__
+            raise ValueError(f"out must be a float32 tensor [J, {self.num_src}, >= {128 * replay}] with unit sample stride on "
+                             f"{dev}, got {shape}")
+        if used is None:
+            used = torch.empty(J, dtype=torch.int32, device=dev)
+        elif used.dtype != torch.int32 or tuple(used.shape) != (J,) or used.device != dev or not used.is_contiguous():
+            raise ValueError(f"used must be a contiguous int32 tensor of shape ({J},) on {dev}")
+        self._require_cuda(state.buf)
+        self._sync_weights(dev)
+        if ws is None:
+            ws, ws_bytes = self._workspace(dev, J, max(1, replay), flags)
+        else:
+            need = ctypes.c_size_t()
+            _cabi.check(_cabi.lib().l2h_sep_workspace_bytes(self._engine(), J, max(1, replay), flags, ctypes.byref(need)))
+            if (not isinstance(ws, torch.Tensor) or ws.dtype != torch.uint8 or ws.device != dev or not ws.is_contiguous()
+                    or ws.numel() < need.value):
+                raise ValueError(f"ws must be a contiguous uint8 tensor of at least {need.value} bytes on {dev}")
+            ws_bytes = ws.numel()
+        with torch.cuda.device(dev):
+            _cabi.check_args(_cabi.lib().l2h_sep_join_targets(
+                self._engine(), records.data_ptr(), leads.data_ptr(), embeds.to(dev, torch.float32).contiguous().data_ptr(), J,
+                state.buf.data_ptr(), state.batch, None if history is None else history.buf.data_ptr(),
+                0 if history is None else history.frames, frames, y.data_ptr() if y.numel() else None, y.stride(0),
+                y.stride(1), used.data_ptr(), ws.data_ptr(), ws_bytes, flags,
+                torch.cuda.current_stream(dev).cuda_stream))
+        return y, used
 
     def stream_dev(self, x_dev, embed_dev, chunks_per_call=1, state=None, n_calls=None, out=None):
         """Streaming over a device-resident clip (l2h_sep_stream_dev): x_dev [B,M,N] is consumed
