@@ -31,6 +31,9 @@
  *        <- EmbedTFGridNet.__init__/forward     src/models/tfgridnet_orig/tfgridnet.py:88-127
  *   l2h_enroll_capture / l2h_embed_forward_slots
  *        <- EmbedTFGridNet.forward of a listener's own recent stream (EnrollCapture, EmbedTFGridNet.enroll)
+ *   l2h_target_mix / l2h_target_mix_set
+ *        <- summing each listener's target voices, and a little of its mixture, into one output row with fades
+ *           (TargetMixer)
  *
  * Conventions follow the reference's only FFI (src/datasets/motion_simulator.py:30-95): every
  * function returns int (0 = OK, non-zero = error, text via l2h_last_error()), handles are opaque
@@ -693,6 +696,73 @@ int l2h_enroll_capture_layout(int32_t capacity, int32_t* row_floats);
 int l2h_enroll_capture(const float* chunk_dev, int64_t chunk_row_stride, int64_t chunk_ch_stride, int32_t n, int32_t channels,
                        int32_t frames, const int32_t* slots_dev, const int32_t* hops_dev, float* state_dev, int32_t n_slots,
                        int32_t capacity, void* stream);
+
+/* A per-listener target mixer: the separated voices of each listener (the target rows of l2h_sep_forward_targets_rows) and,
+ * optionally, a little of its unprocessed mixture ("transparency") summed into one row per listener, each term scaled by
+ * a gain that ramps smoothly when it changes, so a voice that joins or drops fades in or out instead of clicking.
+ *
+ * The state is [n_records + n_slots][channels][row_floats] fp32 of DEVICE memory: one ramp per separator record and
+ * channel, then one per listener slot and channel for the ambient term.  A ramp (g0, g1, F, p) goes from g0 to g1 over F
+ * samples, p of them mixed already (words 2 and 3 are int32 words stored in the floats' bits: F + 1, 0 for a row never
+ * set, and p).  The sample at ramp position q (q = p for the next one mixed) is mixed at
+ *     G(q) = g1                                              if q + 1 >= F   (F = 0: an immediate change)
+ *          = g0 + (g1 - g0) (1 - cos(pi (q + 1) / F)) / 2     otherwise       (a raised cosine, fp32, cospif)
+ * so a ramp ends exactly at g1, and a sample's gain depends only on its position in the ramp.  All
+ * zeros is a fresh row: a record settled at gain 1, a slot settled at ambient gain 0.  So a row is reset by zeroing it and
+ * moved by copying it.  A record's or slot's channels are written only by the CTAs of that channel.
+ * l2h_target_mix_layout: row_floats = 4.  Errors: 1 = null pointer.
+ *
+ * l2h_target_mix: listener row i (h = hops_dev[i], or frames without hops) writes, for s < 128 h,
+ *     out[i][c][s] = sum over its target rows r, in row order, of G_r(s) y[r][c][s]  +  A_i(s) chunk[i][c][s]
+ *   y_dev        [R][channels][128 * frames] fp32, strides in floats: the y of l2h_sep_forward_targets_rows
+ *   chunk_dev    [n][channels][128 * frames + 64] fp32, the separator's input of the same call, or NULL: no ambient term.
+ *                chunk[i][c][0 .. 128 h) is exactly the stretch of the mixture that y[r][c][0 .. 128 h) estimates, with
+ *                the same 64-sample look-ahead delay, so the ambient term is time-aligned with no buffer of its own.
+ *   out_dev      [n][channels][128 * frames] fp32: row i receives out[i][c][0 .. 128 h); its later samples are not
+ *                written.  Must not overlap y or the chunk.
+ *   records_dev  [R] int32 of DEVICE memory: target row r's gain is record records[r]'s ramp; a record outside
+ *                [0, n_records) marks a row that is skipped.  A record listed twice is a caller error the call does not
+ *                detect.
+ *   offsets_dev  [n + 1] int32 of DEVICE memory: row i owns target rows offsets[i] .. offsets[i+1]-1, the offsets clamped
+ *                as l2h_sep_forward_targets_rows clamps them (non-decreasing, at most R); rows from offsets[n] on belong to
+ *                nobody and are not read.
+ *   hops_dev     [n] int32 of DEVICE memory, or NULL (every row mixes frames hops)
+ *   slots_dev    [n] int32 of DEVICE memory: row i's ambient gain is slot slots[i]'s ramp.
+ * G_r(s) and A_i(s) are the ramps' G at positions p + s; the call advances every ramp it mixes by 128 h (the ambient ramp
+ * too when chunk_dev is NULL: it keeps the listener's clock).  Each sample's sum starts at -0 and takes, with fmaf in the
+ * order above, every term whose gain at that sample is nonzero.  fmaf(g, x, -0) is g x exactly, so the first such term
+ * starts the sum with nothing added to a zero: one target at unity gain gives y itself, and several at unity with no
+ * ambient give their fp32 sum in row order, bit for bit.  A sample that no term enters is -0, so a row that stores but
+ * has no live term writes zeros.  A term at gain 0 never reaches a sample, not even as the sign of a zero or a NaN in its
+ * input, and a term whose gain is 0 for every sample of the call is not read at all.  So the output depends only on the
+ * samples' gains, and cutting the hops differently changes no bit of it.  A row whose slot lies outside [0, n_slots), or whose h lies outside [1, frames], stores nothing and
+ * advances no ramp.  The output of l2h_sep_forward_targets_groups (K targets per group) is served as y [n K][channels]
+ * [128 frames] with offsets i K and records g_i K + k.  All lists are read when the kernel runs, so a call captured in a
+ * CUDA graph with l2h_hop_fifo, l2h_sep_forward_targets_rows and l2h_resample_packets serves any lists of the same n and R
+ * rewritten in place.  One launch.  Errors, returned before anything is enqueued: 1 = null pointers (chunk_dev may be
+ * NULL), n, R, channels, frames, n_records or n_slots <= 0, n > R, n > n_slots, channel or row strides under the lengths
+ * above, out overlapping y or the chunk.  y and the chunk share the one `channels` count, so a chunk whose channels differ
+ * from y's cannot be passed here (TargetMixer refuses it by shape).  Asynchronous on `stream`.
+ *
+ * l2h_target_mix_set: entry e sets the ramp of state row rows_dev[e] (a record b as row b, a slot s as row n_records + s) in
+ * every channel to (g0, gains_dev[e], fades_dev[e], 0): a fade to gains_dev[e] over fades_dev[e] samples, starting at
+ * starts_dev[e], or, with starts_dev NULL, at the gain of the last sample mixed (a fresh row: its rest gain), so changing a
+ * ramp halfway never jumps.  rows_dev, gains_dev, starts_dev and fades_dev are [n] arrays of DEVICE memory read when the
+ * kernel runs, so a set can run from a CUDA graph; a row outside [0, n_records + n_slots), or a fade outside
+ * [0, 2^31 - 2], marks an entry that stores nothing.  A row listed twice is a caller error the call does not detect.
+ * Enqueue a set on the stream of the mixer's calls, between them: a set that runs while a mix call reads the same ramps
+ * races with it.  One launch.  Errors, returned before anything is enqueued: 1 = null pointers (starts_dev may be NULL),
+ * n_records, n_slots, channels or n <= 0.  The fades live in device memory and are read when the kernel runs, so a
+ * negative fade is no argument error: it marks an entry that stores nothing (TargetMixer refuses it in host lists).
+ * Asynchronous on `stream`. */
+int l2h_target_mix_layout(int32_t* row_floats);
+int l2h_target_mix(const float* y_dev, int64_t y_row_stride, int64_t y_ch_stride, const float* chunk_dev,
+                   int64_t chunk_row_stride, int64_t chunk_ch_stride, float* out_dev, int64_t out_row_stride,
+                   int64_t out_ch_stride, int32_t n, int32_t R, int32_t channels, int32_t frames, const int32_t* records_dev,
+                   const int32_t* offsets_dev, const int32_t* hops_dev, const int32_t* slots_dev, float* state_dev,
+                   int32_t n_records, int32_t n_slots, void* stream);
+int l2h_target_mix_set(float* state_dev, int32_t n_records, int32_t n_slots, int32_t channels, const int32_t* rows_dev,
+                       int32_t n, const float* gains_dev, const float* starts_dev, const int32_t* fades_dev, void* stream);
 
 #ifdef __cplusplus
 }

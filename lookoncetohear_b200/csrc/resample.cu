@@ -18,8 +18,9 @@
 //
 // The file also holds the per-slot stages of the serving front end, which share one scaffold (slot_row, slot_call):
 // the streaming resamplers (pushes of whole periods, resample_stream_kernel; pushes of any length,
-// resample_packets_kernel), the hop FIFO that turns 16 kHz pieces into separator chunks (hop_fifo_kernel) and the
-// enrollment capture (enroll_capture_kernel).
+// resample_packets_kernel), the hop FIFO that turns 16 kHz pieces into separator chunks (hop_fifo_kernel), the
+// enrollment capture (enroll_capture_kernel) and the target mixer that sums a listener's separated voices and its ambient
+// mixture into one row (target_mix_kernel, target_mix_set_kernel).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -28,6 +29,7 @@
 #include <initializer_list>
 #include <numeric>
 #include <string>
+#include <utility>
 
 #include "../../include/lookonce_b200.h"
 #include "host_errors.h"
@@ -376,6 +378,175 @@ enroll_capture_kernel(const float* __restrict__ chunk, int64_t c_row, int64_t c_
     }
 }
 
+// ---- the target mixer: a listener's target rows, gain-ramped, and its ambient mixture summed into one row -------------
+// The state is [n_records + n_slots][C][TM_FLOATS]: one ramp per (separator record, channel), then one per (listener slot,
+// channel) for the ambient term.  A ramp (g0, g1, F, p) goes from g0 to g1 over F samples, p of them mixed already: the
+// sample at position q of the ramp is mixed at ramp_level(q + 1), so the gain of a sample depends only on (g0, g1, F) and
+// q, never on how the ramp was cut into calls.  Word 2 holds F + 1 (0: never set, settled at the row's rest gain, 1 for a
+// record and 0 for a slot), so all zeros is a fresh row.
+constexpr int TM_FLOATS = 4;     // g0, g1, then int32 words F + 1 and p
+constexpr int TM_THREADS = 128;
+constexpr int TM_TERMS = 64;     // target rows staged per pass
+
+struct Ramp {
+    float g0, g1;
+    int F, p;    // p in [0, F]
+};
+
+L2H_DEVINL Ramp ramp_of(const float* w, float rest) {
+    const int f1 = __float_as_int(w[2]);
+    if (f1 <= 0) return {rest, rest, 0, 0};
+    const int F = f1 - 1;
+    return {w[0], w[1], F, min(max(__float_as_int(w[3]), 0), F)};
+}
+
+// the gain after q samples of the ramp: g1 from q = F on, a raised cosine from g0 before
+L2H_DEVINL float ramp_level(const Ramp& r, int64_t q) {
+    if (q >= r.F) return r.g1;
+    return r.g0 + (r.g1 - r.g0) * (1.f - cospif((float)q / (float)r.F)) * 0.5f;
+}
+
+// a ramp that mixes 0 into every one of the next n samples (a raised cosine is monotone, so its ends decide)
+L2H_DEVINL bool ramp_mute(const Ramp& r, int n) {
+    return ramp_level(r, (int64_t)r.p + 1) == 0.f && ramp_level(r, (int64_t)r.p + n) == 0.f;
+}
+
+// the word p of a ramp after n more samples (only a running ramp changes)
+L2H_DEVINL void ramp_advance(float* w, const Ramp& r, int n) {
+    if (r.p < r.F) w[3] = __int_as_float((int)min((int64_t)r.F, (int64_t)r.p + n));
+}
+
+// V consecutive floats (V = 1 or 4; 4 only where every operand is 16-byte aligned)
+template <int V> struct Vec { float v[V]; };
+template <int V> L2H_DEVINL Vec<V> vload(const float* p) {
+    Vec<V> a;
+    if constexpr (V == 4) {
+        const float4 f = *reinterpret_cast<const float4*>(p);
+        a.v[0] = f.x; a.v[1] = f.y; a.v[2] = f.z; a.v[3] = f.w;
+    } else {
+        a.v[0] = *p;
+    }
+    return a;
+}
+template <int V> L2H_DEVINL void vstore(float* p, const Vec<V>& a) {
+    if constexpr (V == 4) *reinterpret_cast<float4*>(p) = make_float4(a.v[0], a.v[1], a.v[2], a.v[3]);
+    else *p = a.v[0];
+}
+
+// acc += gain * x over V samples at ramp position q0, each sample's gain from the ramp.  A sample whose gain is 0 is left
+// as it is, so whether a term enters a sample depends only on that sample's gain, never on how the hops were cut.
+template <int V> L2H_DEVINL void mix_term(Vec<V>& acc, const Vec<V>& x, const Ramp& r, int64_t q0) {
+    const bool flat = (int64_t)r.p + 1 >= r.F;
+#pragma unroll
+    for (int k = 0; k < V; ++k) {
+        const float g = flat ? r.g1 : ramp_level(r, q0 + k + 1);
+        if (g != 0.f) acc.v[k] = fmaf(g, x.v[k], acc.v[k]);
+    }
+}
+
+// max over the block of v (TM_THREADS threads)
+L2H_DEVINL int block_max(int v, int* red) {
+    for (int d = 16; d > 0; d >>= 1) v = max(v, __shfl_xor_sync(0xffffffffu, v, d));
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    v = red[0];
+    for (int w = 1; w < TM_THREADS / 32; ++w) v = max(v, red[w]);
+    __syncthreads();
+    return v;
+}
+
+// One CTA = one (listener row, channel).  Row i owns target rows start .. end - 1, start = the running maximum of the
+// offsets clamped to [0, R] (the separator's clamp, targets_kernels.cuh), and writes out[i][c][0 .. 128 h) with h = hops[i]
+// (T without hops): the sum in row order of its live target rows scaled by their records' ramps, then the ambient term
+// (chunk row i scaled by its slot's ramp).  Each sample's sum starts at -0 and takes, with fmaf, every term whose gain at
+// that sample is nonzero: fmaf(g, x, -0) is g x exactly, so the first such term starts the sum with nothing added to a
+// zero, and a sample with none is -0.  A term whose gain is 0 over all 128 h samples is not read.  Target rows are staged
+// TM_TERMS at a time; a later pass continues the sum from `out`, which the same thread wrote.  Each staged term's ramp word is read once, by the thread that stages it, which also advances it.
+template <int V>
+__global__ void __launch_bounds__(TM_THREADS)
+target_mix_kernel(const float* __restrict__ y, int64_t y_row, int64_t y_ch, const float* __restrict__ chunk, int64_t c_row,
+                  int64_t c_ch, float* __restrict__ out, int64_t o_row, int64_t o_ch, int C, int R, int T,
+                  const int32_t* __restrict__ records, const int32_t* __restrict__ offsets,
+                  const int32_t* __restrict__ hops, const int32_t* __restrict__ slots, float* __restrict__ state,
+                  int n_records, int n_slots) {
+    __shared__ Ramp ramp[TM_TERMS];
+    __shared__ int term_row[TM_TERMS];   // the staged target rows, -1 for a row that mixes nothing
+    __shared__ int red[TM_THREADS / 32];
+    const int tid = threadIdx.x;
+    const SlotRow sr = slot_row(C, slots, n_slots, state + (int64_t)n_records * C * TM_FLOATS, TM_FLOATS);
+    const int h = hops ? hops[sr.row] : T;
+    if (!sr.live || h <= 0 || h > T) return;                           // a row that stores nothing
+    const int n = h * CHUNK_HOP, i = sr.row, ch = sr.ch;
+    int lo = 0, hi = 0;                                                 // max of the clamped offsets 0 .. i and 0 .. i + 1
+    for (int j = tid; j <= i + 1; j += TM_THREADS) {
+        const int v = min(max(offsets[j], 0), R);
+        hi = max(hi, v);
+        if (j <= i) lo = max(lo, v);
+    }
+    const int start = block_max(lo, red), end = block_max(hi, red);
+    const Ramp amb = ramp_of(sr.st, 0.f);
+    const bool amb_live = chunk != nullptr && !ramp_mute(amb, n);
+    const float* cr = chunk ? row_ch(chunk, c_row, c_ch, i, ch) : nullptr;
+    float* orow = row_ch(out, o_row, o_ch, i, ch);
+    bool started = false;                                               // out holds a partial sum (uniform)
+    for (int r0 = start;; r0 += TM_TERMS) {
+        const int cnt = max(0, min(TM_TERMS, end - r0));
+        const bool last = r0 + TM_TERMS >= end;
+        if (tid < cnt) {
+            const int rec = records[r0 + tid];
+            int row = -1;
+            if (rec >= 0 && rec < n_records) {
+                float* w = state + ((int64_t)rec * C + ch) * TM_FLOATS;
+                const Ramp g = ramp_of(w, 1.f);
+                ramp[tid] = g;
+                if (!ramp_mute(g, n)) row = r0 + tid;
+                ramp_advance(w, g, n);
+            }
+            term_row[tid] = row;
+        }
+        __syncthreads();
+        bool any = false;
+        for (int t = 0; t < cnt; ++t) any = any || term_row[t] >= 0;
+        if (any || (last && (amb_live || !started))) {
+            for (int s = tid * V; s < n; s += TM_THREADS * V) {
+                Vec<V> acc;
+                if (started) acc = vload<V>(orow + s);
+                else
+                    for (int k = 0; k < V; ++k) acc.v[k] = -0.f;             // the identity of the sum
+                for (int t = 0; t < cnt; ++t) {
+                    const int row = term_row[t];
+                    if (row >= 0)
+                        mix_term<V>(acc, vload<V>(row_ch(y, y_row, y_ch, row, ch) + s), ramp[t], (int64_t)ramp[t].p + s);
+                }
+                if (last && amb_live) mix_term<V>(acc, vload<V>(cr + s), amb, (int64_t)amb.p + s);
+                vstore<V>(orow + s, acc);
+            }
+            started = true;
+        }
+        if (last) break;
+        __syncthreads();                                                // the staged terms are read before the next pass
+    }
+    if (tid == 0) ramp_advance(sr.st, amb, n);                         // every thread read the ambient ramp above
+}
+
+// Entry e of a gain set (j = e * C + ch): the ramp of state row rows[e] becomes (start, gains[e], fades[e], 0), start =
+// starts[e], or without starts the gain of the last sample mixed.  A row outside the state, or a fade outside [0, 2^31 - 2],
+// stores nothing.
+__global__ void __launch_bounds__(RS_TILE)
+target_mix_set_kernel(float* __restrict__ state, int n_records, int n_rows, int C, const int32_t* __restrict__ rows, int n,
+                      const float* __restrict__ gains, const float* __restrict__ starts, const int32_t* __restrict__ fades) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n * C) return;
+    const int e = j / C, ch = j - e * C, row = rows[e], F = fades[e];
+    if (row < 0 || row >= n_rows || F < 0 || F == INT32_MAX) return;
+    float* w = state + ((int64_t)row * C + ch) * TM_FLOATS;
+    const Ramp g = ramp_of(w, row < n_records ? 1.f : 0.f);
+    w[0] = starts ? starts[e] : ramp_level(g, g.p);
+    w[1] = gains[e];
+    w[2] = __int_as_float(F + 1);
+    w[3] = __int_as_float(0);
+}
+
 // ---- the host side of the per-slot calls ------------------------------------------------------------------------------
 // The checks every per-slot call makes first, in this order: its pointers, its sizes (`sizes` names them), n <= n_slots,
 // and a grid of n * channels CTAs.  0, or 1 with its message.
@@ -406,6 +577,12 @@ static int disjoint(const std::string& who, int32_t channels, std::initializer_l
 static int chunk_len(const std::string& who, int32_t frames, int64_t* len) {
     *len = (int64_t)frames * CHUNK_HOP + CHUNK_CARRY;
     return *len > INT32_MAX ? fail(1, who + ": frames is too large") : 0;
+}
+
+// the bytes [first, last) that `rows` rows of a strided operand span
+static std::pair<uintptr_t, uintptr_t> span(const void* p, int64_t rows, int32_t channels, const Rows& r) {
+    const uintptr_t a = reinterpret_cast<uintptr_t>(p);
+    return {a, a + (uintptr_t)(((rows - 1) * r.row + (int64_t)(channels - 1) * r.ch + r.len) * (int64_t)sizeof(float))};
 }
 
 // the error of the launch just made: 0, or 3 with its message
@@ -601,5 +778,62 @@ extern "C" int l2h_enroll_capture(const float* chunk_dev, int64_t chunk_row_stri
     if (int rc = disjoint(who, channels, {{"chunk", chunk_row_stride, chunk_ch_stride, c_len}})) return rc;
     enroll_capture_kernel<<<(unsigned)(n * channels), RS_TILE, 0, static_cast<cudaStream_t>(stream)>>>(
         chunk_dev, chunk_row_stride, chunk_ch_stride, channels, frames, slots_dev, hops_dev, state_dev, n_slots, capacity);
+    return launched(who);
+}
+
+extern "C" int l2h_target_mix_layout(int32_t* row_floats) {
+    using namespace l2h;
+    if (!row_floats) return fail(1, "l2h_target_mix_layout: null pointer");
+    *row_floats = TM_FLOATS;
+    return 0;
+}
+
+extern "C" int l2h_target_mix(const float* y_dev, int64_t y_row_stride, int64_t y_ch_stride, const float* chunk_dev,
+                              int64_t chunk_row_stride, int64_t chunk_ch_stride, float* out_dev, int64_t out_row_stride,
+                              int64_t out_ch_stride, int32_t n, int32_t R, int32_t channels, int32_t frames,
+                              const int32_t* records_dev, const int32_t* offsets_dev, const int32_t* hops_dev,
+                              const int32_t* slots_dev, float* state_dev, int32_t n_records, int32_t n_slots, void* stream) {
+    using namespace l2h;
+    const std::string who = "l2h_target_mix";
+    if (int rc = slot_call(who, {y_dev, out_dev, records_dev, offsets_dev, slots_dev, state_dev},
+                           "n, R, channels, frames, n_records and n_slots", {n, R, channels, frames, n_records, n_slots}, n,
+                           channels, n_slots))
+        return rc;
+    if (n > R) return fail(1, who + ": a call needs n <= R (every listener row owns its target rows)");
+    int64_t c_len;
+    if (int rc = chunk_len(who, frames, &c_len)) return rc;
+    const int64_t len = (int64_t)frames * CHUNK_HOP;
+    const Rows y{"y", y_row_stride, y_ch_stride, len}, out{"out", out_row_stride, out_ch_stride, len},
+        ck{"chunk", chunk_row_stride, chunk_ch_stride, c_len};
+    if (int rc = chunk_dev ? disjoint(who, channels, {y, ck, out}) : disjoint(who, channels, {y, out})) return rc;
+    const auto o = span(out_dev, n, channels, out), a = span(y_dev, R, channels, y);
+    const auto b = chunk_dev ? span(chunk_dev, n, channels, ck) : std::make_pair(uintptr_t(0), uintptr_t(0));
+    if ((o.first < a.second && a.first < o.second) || (o.first < b.second && b.first < o.second))
+        return fail(1, who + ": out must not overlap y or the chunk");
+    bool vec = true;                                    // float4 loads and stores where every operand allows them
+    for (const Rows& r : {y, out, ck}) vec = vec && r.row % 4 == 0 && r.ch % 4 == 0;
+    for (const void* p : {(const void*)y_dev, (const void*)out_dev, (const void*)chunk_dev})
+        vec = vec && reinterpret_cast<uintptr_t>(p) % 16 == 0;
+    const auto kernel = vec ? target_mix_kernel<4> : target_mix_kernel<1>;
+    kernel<<<(unsigned)(n * channels), TM_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
+        y_dev, y_row_stride, y_ch_stride, chunk_dev, chunk_row_stride, chunk_ch_stride, out_dev, out_row_stride,
+        out_ch_stride, channels, R, frames, records_dev, offsets_dev, hops_dev, slots_dev, state_dev, n_records, n_slots);
+    return launched(who);
+}
+
+extern "C" int l2h_target_mix_set(float* state_dev, int32_t n_records, int32_t n_slots, int32_t channels,
+                                  const int32_t* rows_dev, int32_t n, const float* gains_dev, const float* starts_dev,
+                                  const int32_t* fades_dev, void* stream) {
+    using namespace l2h;
+    const std::string who = "l2h_target_mix_set";
+    for (const void* p : {(const void*)state_dev, (const void*)rows_dev, (const void*)gains_dev, (const void*)fades_dev})
+        if (!p) return fail(1, who + ": null pointer");
+    if (n_records <= 0 || n_slots <= 0 || channels <= 0 || n <= 0)
+        return fail(1, who + ": n_records, n_slots, channels and n must be positive");
+    if ((int64_t)n_records + n_slots > INT32_MAX || (int64_t)n * channels > INT32_MAX)
+        return fail(1, who + ": n_records + n_slots or n * channels is too large");
+    const int jobs = n * channels;
+    target_mix_set_kernel<<<(unsigned)((jobs + RS_TILE - 1) / RS_TILE), RS_TILE, 0, static_cast<cudaStream_t>(stream)>>>(
+        state_dev, n_records, n_records + n_slots, channels, rows_dev, n, gains_dev, starts_dev, fades_dev);
     return launched(who);
 }

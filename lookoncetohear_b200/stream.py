@@ -2,11 +2,14 @@
 `Net.advance_slots`: streaming resampling for listeners whose devices run at another rate than the separator's 16 kHz
 (`StreamResampler`, `l2h_resample_stream`), with pushes of any length (`PacketResampler`, `l2h_resample_packets`), the
 per-slot FIFO that turns 16 kHz pieces into separator chunks and hop counts (`HopFifo`, `l2h_hop_fifo`), and the
-per-slot capture that keeps each listener's recent input for enrollment (`EnrollCapture`, `l2h_enroll_capture`).
+per-slot capture that keeps each listener's recent input for enrollment (`EnrollCapture`, `l2h_enroll_capture`), and
+the per-listener mixer that sums the separated voices and the ambient mixture into one row with fades (`TargetMixer`,
+`l2h_target_mix`).
 
 Each stage keeps a float32 state [slots, channels, row floats] on a CUDA device.  All zeros is a fresh slot, so a
 listener is reset by zeroing its rows (`reset`) and moved by copying them.  No CPU fallback."""
 import ctypes
+import math
 import numbers
 
 import torch
@@ -45,14 +48,15 @@ class _SlotStage:
     def __init__(self, slots, channels):
         self.n_slots, self.channels = _whole(slots, "slots"), _whole(channels, "channels")
 
-    def _allocate(self, row_floats, device):
-        """a zero state of rows of row_floats on `device` (the current CUDA device for None or "cuda")"""
+    def _allocate(self, row_floats, device, rows=None):
+        """a zero state of `rows` (else n_slots) rows of row_floats on `device` (the current CUDA device for None or
+        "cuda")"""
         dev = torch.device("cuda") if device is None else torch.device(device)
         if dev.type != "cuda":
             raise RuntimeError(f"lookoncetohear_b200.{type(self).__name__} needs a CUDA device (no CPU fallback)")
         if dev.index is None:
             dev = torch.device("cuda", torch.cuda.current_device())
-        self.state = torch.zeros(self.n_slots, self.channels, row_floats, dtype=torch.float32, device=dev)
+        self.state = torch.zeros(rows or self.n_slots, self.channels, row_floats, dtype=torch.float32, device=dev)
 
     def reset(self, slots):
         """Make the listed slots fresh (their state rows zero); the other slots keep what they hold."""
@@ -304,3 +308,173 @@ class EnrollCapture(_SlotStage):
     def captured(self):
         """[slots] int32 CUDA view of the state: the samples each slot captured since its reset, capped at capacity"""
         return self.state[:, 0, 1].view(torch.int32)
+
+
+class TargetMixer(_SlotStage):
+    """Per-listener mixing of the separated voices on the device (l2h_target_mix): each listener's target rows of
+    `Net.advance_target_rows`, each scaled by its record's gain, plus optionally its unprocessed mixture scaled by its
+    slot's ambient gain ("transparency"), summed into one row per listener for the up-resampler and the client.
+
+    Every gain is a ramp: set_gains / set_ambient fade it to a new value over `fade` samples along a raised cosine, so a
+    joined voice fades in and a dropped one fades out instead of clicking.  The gain of a sample depends only on the
+    ramp and the sample's position since the ramp started: how the ramp is cut into ticks and hop counts never changes a
+    bit of the output, and a ramp advances only by the samples its listener mixes.
+
+    `state` [records + slots, channels, 4] is a float32 tensor on `device`: one ramp per separator record, then one per
+    listener slot.  All zeros is a fresh row, a record at gain 1 and a slot at ambient gain 0, so rows are reset by
+    zeroing them (`reset`) and moved by copying them."""
+
+    GAIN_MAX = 16.0
+
+    def __init__(self, records, slots, channels, device=None):
+        super().__init__(slots, channels)
+        self.n_records = _whole(records, "records")
+        if self.n_records + self.n_slots >= 2 ** 31:
+            raise ValueError("records + slots must be below 2**31")
+        self._allocate(*_layout(_cabi.lib().l2h_target_mix_layout), device, rows=self.n_records + self.n_slots)
+
+    def reset(self, records=(), slots=()):
+        """Make the listed records (gain 1) and slots (ambient gain 0) fresh; the other rows keep their ramps."""
+        dev = self.state.device
+        rows = []
+        for values, end, noun, base in ((records, self.n_records, "record", 0), (slots, self.n_slots, "slot", self.n_records)):
+            v = torch.as_tensor(values).cpu().reshape(-1)
+            if v.numel():
+                rows.append(device_list(v, dev, v.numel(), end, False, noun).long() + base)
+        if rows:
+            self.state.index_fill_(0, torch.cat(rows), 0.0)
+
+    def __call__(self, y, records, offsets, slots, hops=None, chunk=None, out=None):
+        """y [R, channels, 128 * T] CUDA tensor, the target rows of Net.advance_target_rows; listener row i owns target
+        rows offsets[i] .. offsets[i+1]-1, target row r has record records[r]'s gain, and slots[i] is the listener's
+        slot.  Returns out [n, channels, 128 * T] float32 (`out`, if given, written in place): row i receives, for
+        s < 128 h (h = hops[i], T without hops), the sum in row order of its live target rows times their gains, plus
+        chunk[i, :, s] times its slot's ambient gain when `chunk` is given.  Its later samples are left unwritten.
+
+        chunk [n, channels, 128 * T + 64] is the separator's input of the same call: its first 128 h samples are exactly
+        the stretch of the mixture that y's rows estimate, with the same 64-sample look-ahead delay, so the ambient term
+        needs no buffer of its own.  A term enters only the samples where its gain is nonzero, so one target at gain 1
+        returns its y row bit for bit, NaN in a muted term's samples never reaches out, and a term whose gain is 0 over
+        the call is not read.  A listener with no live term gets zeros (-0).
+
+        Lists follow Net.advance_target_rows: host lists are checked and uploaded (`records` R distinct ints in
+        [0, records); `offsets` n + 1 ints from 0, non-decreasing, at most R; `slots` n distinct ints in [0, slots);
+        `hops` n ints in [0, T]); contiguous CUDA int32 tensors are used in place and read when the kernel runs, where a
+        record outside the mixer marks a row that is skipped, the offsets are clamped as the separator clamps them, and
+        a slot outside the mixer or a hop count outside [1, T] marks a listener that stores nothing and advances no
+        ramp.  So a call captured in a CUDA graph with the FIFO, the separator and the up-resampler serves any lists
+        rewritten in place.  The output of Net.advance_targets, y [n, K, S, 128 T], is y.view(n K, S, 128 T) with offsets
+        i K and records g_i K + k."""
+        y = self._rows_in(y, self.HOP)
+        dev = self.state.device
+        R, C, L = y.shape
+        T = L // self.HOP
+        n = len(slots) if not isinstance(slots, torch.Tensor) else slots.numel()
+        if not 0 < n <= R:
+            raise ValueError(f"a mix needs 0 < n <= R, got n = {n} listeners and R = {R} target rows")
+        records = device_list(records, dev, R, self.n_records, True, "record")
+        on_host = not (isinstance(offsets, torch.Tensor) and offsets.is_cuda)
+        o = torch.as_tensor(offsets).tolist() if on_host else None
+        offsets = device_list(offsets, dev, n + 1, R + 1, False, "offset")
+        if on_host:
+            if o[0] != 0 or any(b < a for a, b in zip(o, o[1:])):
+                raise ValueError(f"offsets must start at 0 and never decrease, got {o}")
+        slots = device_list(slots, dev, n, self.n_slots, True, "slot")
+        if hops is not None:
+            hops = device_list(hops, dev, n, T + 1, False, "hop")
+        if chunk is not None:
+            chunk = self._rows_in(chunk)
+            if tuple(chunk.shape) != (n, C, L + self.CARRY):
+                raise ValueError(f"chunk must have shape [{n}, {C}, {L + self.CARRY}] (the separator's input of the call, "
+                                 f"with y's channels), got {tuple(chunk.shape)}")
+        out = self._rows_out(out, (n, C, L))
+        ck = (None, 0, 0) if chunk is None else (chunk.data_ptr(), chunk.stride(0), chunk.stride(1))
+        with torch.cuda.device(dev):
+            _check(_cabi.lib().l2h_target_mix(
+                y.data_ptr(), y.stride(0), y.stride(1), *ck, out.data_ptr(), out.stride(0), out.stride(1), n, R, C, T,
+                records.data_ptr(), offsets.data_ptr(), None if hops is None else hops.data_ptr(), slots.data_ptr(),
+                self.state.data_ptr(), self.n_records, self.n_slots, self._stream()))
+        return out
+
+    def set_gains(self, records, gains, fade=0, start=None):
+        """Fade the gains of the listed records to `gains` over `fade` samples (0: at once), starting at `start`, or,
+        without it, at the gain of the last sample each record mixed, so changing a ramp halfway never jumps.  Join a
+        voice with set_gains([b], [1.0], fade=480, start=0.0); drop one with set_gains([b], [0.0], fade=480), keep
+        listing b until fading[b] is false, then leave its row out.
+
+        `gains`, `fade` and `start` are numbers or one per record.  Host values are checked (gains and starts finite, in
+        [0, 16]; fades ints >= 0) and uploaded; CUDA tensors (int32 records and fades, float32 gains and starts, shape
+        (n,)) are used in place and read when the kernel runs, so a set can be captured in a CUDA graph.  Enqueue a set
+        on the mixer's stream between its calls."""
+        self._set(records, self.n_records, "record", 0, gains, fade, start)
+
+    def set_ambient(self, slots, gains, fade=0, start=None):
+        """set_gains for the ambient gains of the listed slots (the share of the unprocessed mixture each listener hears;
+        0 when fresh)."""
+        self._set(slots, self.n_slots, "slot", self.n_records, gains, fade, start)
+
+    def _set(self, rows, end, noun, base, gains, fade, start):
+        dev = self.state.device
+        n = rows.numel() if isinstance(rows, torch.Tensor) else len(rows)
+        if n < 1:
+            raise ValueError(f"set needs at least one {noun}")
+        rows = device_list(rows, dev, n, end, True, noun)
+        # record b is state row b, slot s is state row records + s; a CUDA entry outside [0, end) stays outside the state
+        rows = torch.where((rows >= 0) & (rows < end), rows + base, -1).to(torch.int32)
+        gains = self._values(gains, n, torch.float32, "gains")
+        fades = self._values(fade, n, torch.int32, "fade")
+        starts = None if start is None else self._values(start, n, torch.float32, "start")
+        with torch.cuda.device(dev):
+            _check(_cabi.lib().l2h_target_mix_set(
+                self.state.data_ptr(), self.n_records, self.n_slots, self.channels, rows.data_ptr(), n,
+                gains.data_ptr(), None if starts is None else starts.data_ptr(), fades.data_ptr(), self._stream()))
+
+    def _values(self, v, n, dtype, what):
+        """v as an [n] `dtype` tensor on the state's device: a CUDA tensor used in place, else numbers checked and
+        uploaded (a single number for every entry)"""
+        dev = self.state.device
+        if isinstance(v, torch.Tensor) and v.is_cuda:
+            if v.dtype != dtype or tuple(v.shape) != (n,) or not v.is_contiguous() or v.device != dev:
+                raise ValueError(f"a CUDA {what} tensor must be a contiguous {dtype} tensor of shape ({n},) on {dev}")
+            return v
+        vals = v.tolist() if isinstance(v, torch.Tensor) else v
+        vals = list(vals) if isinstance(vals, (list, tuple)) else [vals] * n
+        if len(vals) != n:
+            raise ValueError(f"{what} gives {len(vals)} values for {n} entries")
+        if dtype == torch.int32:
+            vals = [_whole(f, what, 0) for f in vals]
+            if max(vals) >= 2 ** 31 - 1:
+                raise ValueError(f"{what} must be below 2**31 - 1 samples")
+        else:
+            for g in vals:
+                if (isinstance(g, bool) or not isinstance(g, numbers.Real) or not math.isfinite(g)
+                        or not 0.0 <= g <= self.GAIN_MAX):
+                    raise ValueError(f"{what} must be finite numbers in [0, {self.GAIN_MAX:g}], got {g!r}")
+        return torch.tensor(vals, dtype=dtype).to(dev)
+
+    def _words(self):
+        """(g0, g1, F, p, set) of channel 0 of every row, p clamped into [0, F]"""
+        w = self.state[:, 0]
+        f1 = w[:, 2].view(torch.int32)
+        F = (f1 - 1).clamp(min=0)
+        p = torch.minimum(w[:, 3].view(torch.int32).clamp(min=0), F)
+        return w[:, 0], w[:, 1], F, p, f1 > 0
+
+    @property
+    def level(self):
+        """[records + slots] float32 CUDA tensor: the gain of the last sample each row mixed (entry b: record b; entry
+        records + s: slot s's ambient gain), computed on the device, never synchronising.  It follows the kernel's ramp
+        up to the rounding of torch's cos against the kernel's cospif."""
+        g0, g1, F, p, is_set = self._words()
+        x = p.float() / F.clamp(min=1).float()
+        ramp = g0 + (g1 - g0) * (1.0 - torch.cos(math.pi * x)) * 0.5
+        lvl = torch.where(p >= F, g1, ramp)
+        rest = torch.zeros_like(lvl)
+        rest[:self.n_records] = 1.0
+        return torch.where(is_set, lvl, rest)
+
+    @property
+    def fading(self):
+        """[records + slots] bool CUDA tensor: the rows whose ramp has samples left to mix, never synchronising"""
+        _, _, F, p, is_set = self._words()
+        return is_set & (p < F)
