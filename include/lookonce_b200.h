@@ -34,6 +34,8 @@
  *   l2h_target_mix / l2h_target_mix_set
  *        <- summing each listener's target voices, and a little of its mixture, into one output row with fades
  *           (TargetMixer)
+ *   l2h_limiter
+ *        <- keeping each listener's output under a ceiling, with one gain for both ears (Limiter)
  *
  * Conventions follow the reference's only FFI (src/datasets/motion_simulator.py:30-95): every
  * function returns int (0 = OK, non-zero = error, text via l2h_last_error()), handles are opaque
@@ -763,6 +765,52 @@ int l2h_target_mix(const float* y_dev, int64_t y_row_stride, int64_t y_ch_stride
                    int32_t n_records, int32_t n_slots, void* stream);
 int l2h_target_mix_set(float* state_dev, int32_t n_records, int32_t n_slots, int32_t channels, const int32_t* rows_dev,
                        int32_t n, const float* gains_dev, const float* starts_dev, const int32_t* fades_dev, void* stream);
+
+/* A per-slot look-ahead peak limiter: each listener's output kept under a ceiling, with one gain for all channels at each
+ * sample, so interaural level ratios are preserved.  Put it after the up-resampler, on the samples the device plays:
+ * band-limited upsampling of a limited 16 kHz signal can overshoot the ceiling between its samples.
+ *
+ * Gains live in an integer log domain of Q = 65536 quanta per octave of amplitude.  At input sample k of a slot,
+ * La = lookahead samples and `release_step` quanta of recovery per sample:
+ *     p[k] = max over channels of |x[c][k]|;   q[k] = 0 if p <= ceiling, else ceil(Q log2(p / ceiling)) + 1,
+ *            and 150 Q (a gain of exactly 0) when a channel's sample is not finite
+ *     s[k] = max q[k - La .. k]          r[k] = max(s[k], r[k - 1] - release_step)          a[k] = sum r[k - La .. k]
+ *     y[c][k] = 2^(-a[k] / (Q (La + 1))) x[c][k - La]        (0 where x[c][k - La] is not finite)
+ * The fp32 gain is exp2f of the fraction times an exact power of two, the same for every channel.
+ * So every written sample has |y| <= ceiling exactly, whatever the input; while no reduction is pending (a = 0) the gain
+ * is exactly 1 and y is x delayed by La samples, bit for bit; and, the recurrence being exact integer arithmetic, cutting
+ * a stream into other pushes changes no bit of the output or the state.  A non-finite sample mutes the output around it,
+ * and the gain then recovers at the release rate from 150 octaves (about 900 dB): zeroing the slot's rows ends it at once.
+ *
+ * The state is [n_slots][channels][row_floats] fp32 of DEVICE memory.  Per channel: four head words, the channel's last La
+ * input samples, then the last La q and the last La r (int32 words stored in the floats' bits).  The head words and the q
+ * and r histories are channel 0's only: r of the last sample (int32), the slot's ceiling (float; 0: the call's), the
+ * samples written with a > 0 since the slot was fresh (int32, saturating at 2^31 - 1) and the gain reduction in dB at the
+ * last sample written (float).  A ceiling written into word 1 (a positive normal float; anything else means the call's)
+ * applies to samples pushed after it.  All zeros is a fresh
+ * slot, whose delay line starts with La zeros, so a slot is reset by zeroing its rows and moved by copying them.
+ * l2h_limiter_layout: row_floats = 4 + 3 La.  Errors: 1 = null pointer, channels <= 0, lookahead < 0; 2 = the staging of
+ * a one-sample push ((channels + 2) (La + 1) words) exceeds the kernel's shared memory.
+ *
+ * l2h_limiter: row i pushes m_i = counts_dev[i] * unit samples of x row i into slot slots_dev[i]:
+ *   x_dev       [n][channels][max_in] fp32, strides in floats; row i reads only its first m_i samples
+ *   y_dev       [n][channels][max_in] fp32; row i receives y[i][c][0 .. m_i), its slot's next m_i output samples.  Its later
+ *               samples are not written.  Must not overlap x or the state.
+ *   counts_dev  [n] int32 of DEVICE memory read when the kernel runs; m_i outside [0, max_in] counts as 0.  unit = 1 takes
+ *               l2h_resample_packets' out counts, unit = 128 the separator's hop counts (l2h_hop_fifo's hops_dev).
+ *   slots_dev   [n] int32 of DEVICE memory read when the kernel runs: an entry outside [0, n_slots) marks a row that stores
+ *               nothing (no y sample, no state row).  So does a push of 0 samples.  A slot listed twice is a caller error
+ *               the call does not detect.
+ * One launch, one CTA per row over all its channels; nothing on the host is read from the device, and a call captured in
+ * a CUDA graph serves any lists of the same n rewritten in place.  Errors, returned before anything is enqueued:
+ * 1 = null pointers, n, channels, max_in, unit or n_slots <= 0, n > n_slots, a ceiling that is not a positive normal float,
+ * release_step outside [1, 150 Q], lookahead < 0, channel or row strides under max_in, y overlapping x; 2 = the staging of
+ * a row ((channels + 2) (La + max_in) words) exceeds the kernel's shared memory.  Asynchronous on `stream`. */
+int l2h_limiter_layout(int32_t channels, int32_t lookahead, int32_t* row_floats);
+int l2h_limiter(const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, int32_t max_in, const int32_t* counts_dev,
+                int32_t unit, float* y_dev, int64_t y_row_stride, int64_t y_ch_stride, int32_t n, int32_t channels,
+                const int32_t* slots_dev, float* state_dev, int32_t n_slots, float ceiling, int32_t lookahead,
+                int32_t release_step, void* stream);
 
 #ifdef __cplusplus
 }

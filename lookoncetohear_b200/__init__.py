@@ -12,6 +12,7 @@ net), behind the reference's own Python call signatures.
     from lookoncetohear_b200 import EnrollJob        # EmbedTFGridNet.enroll_job: an enrollment enqueued in slices
     from lookoncetohear_b200 import TargetHistory    # Net.target_history: block 0's recent output, for Net.join_targets
     from lookoncetohear_b200 import TargetMixer      # each listener's voices and ambient mixture into one row, with fades
+    from lookoncetohear_b200 import Limiter          # each listener's output kept under a ceiling, one gain for both ears
 
 Compute happens only in lib/liblookonce_b200.so (hand-written sm_90a CUDA, C ABI declared in
 include/lookonce_b200.h); importing this package never falls back to PyTorch math.
@@ -19,7 +20,7 @@ include/lookonce_b200.h); importing this package never falls back to PyTorch mat
 from .embed import EmbedTFGridNet, EnrollJob  # noqa: F401
 from .net import Net, SepState, TargetHistory  # noqa: F401
 from .render import resample  # noqa: F401
-from .stream import EnrollCapture, HopFifo, PacketResampler, StreamResampler, TargetMixer  # noqa: F401
+from .stream import EnrollCapture, HopFifo, PacketResampler, Limiter, StreamResampler, TargetMixer  # noqa: F401
 
 __all__ = ["Net", "SepState", "TargetHistory", "EmbedTFGridNet", "resample", "StreamResampler", "PacketResampler", "HopFifo",
-           "EnrollCapture", "EnrollJob", "TargetMixer"]
+           "EnrollCapture", "EnrollJob", "TargetMixer", "Limiter"]

@@ -19,12 +19,14 @@
 // The file also holds the per-slot stages of the serving front end, which share one scaffold (slot_row, slot_call):
 // the streaming resamplers (pushes of whole periods, resample_stream_kernel; pushes of any length,
 // resample_packets_kernel), the hop FIFO that turns 16 kHz pieces into separator chunks (hop_fifo_kernel), the
-// enrollment capture (enroll_capture_kernel) and the target mixer that sums a listener's separated voices and its ambient
-// mixture into one row (target_mix_kernel, target_mix_set_kernel).
+// enrollment capture (enroll_capture_kernel), the target mixer that sums a listener's separated voices and its ambient
+// mixture into one row (target_mix_kernel, target_mix_set_kernel), and the look-ahead limiter that keeps each listener's
+// output under a ceiling with one gain for all channels (limiter_kernel).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include <algorithm>
+#include <cfloat>
 #include <cmath>
 #include <initializer_list>
 #include <numeric>
@@ -547,6 +549,137 @@ target_mix_set_kernel(float* __restrict__ state, int n_records, int n_rows, int 
     w[3] = __int_as_float(0);
 }
 
+// ---- the limiter: a look-ahead peak limiter per slot, one gain for all channels ---------------------------------------
+// Gains live in an integer log domain, LM_Q quanta per octave of amplitude, so the release recurrence is exact integer
+// arithmetic: computed as a parallel max-scan it is still the same bits under any cut into calls.  Per input sample k:
+//   q[k] = 0 if p <= ceiling, else ceil(LM_Q log2(p / ceiling)) + 1      p = max over channels of |x[c][k]|
+//          (LM_MUTE for a non-finite sample); the + 1 covers the rounding of the fp32 gain and product
+//   s[k] = max q[k - La .. k]                                             hold
+//   r[k] = max(s[k], r[k - 1] - step)                                     release, `step` quanta per sample
+//   a[k] = sum r[k - La .. k]                                             smoothing box of La + 1
+//   y[c][k] = 2^(-a[k] / (LM_Q (La + 1))) x[c][k - La]                    0 where x is not finite, or a mutes
+// A peak at P keeps r >= q[P] over [P, P + La], so the box at P + La, which scales x[P], is at least q[P]: |y| <= ceiling.
+// A slot's state row per channel is [LM_HEAD + 3 La]: the head words (channel 0's only: r of the last sample, the slot's
+// ceiling (0: the call's), the samples written with a > 0, saturating, and the dB of reduction at the last sample), the
+// channel's last La input samples, then (channel 0's only) the last La q and the last La r.  All zeros is a fresh slot.
+constexpr int LM_HEAD = 4;
+constexpr int LM_Q = 1 << 16;
+constexpr int LM_MUTE_OCT = 150;                        // a reduction of 150 octaves is a gain of exactly 0
+constexpr int LM_MUTE = LM_MUTE_OCT * LM_Q;            // the q of a non-finite sample, and every q's and r's cap
+
+// the maximum of v over the block's threads before this one (INT64_MIN for thread 0); every thread of the block calls it
+L2H_DEVINL int64_t block_exclusive_max(int64_t v, int64_t* warp_max) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    int64_t inc = v;
+    for (int d = 1; d < 32; d <<= 1) {
+        const int64_t o = __shfl_up_sync(0xffffffffu, inc, d);
+        if (lane >= d) inc = max(inc, o);
+    }
+    int64_t ex = __shfl_up_sync(0xffffffffu, inc, 1);
+    if (lane == 0) ex = INT64_MIN;
+    if (lane == 31) warp_max[w] = inc;
+    __syncthreads();
+    for (int i = 0; i < w; ++i) ex = max(ex, warp_max[i]);
+    return ex;
+}
+
+// One CTA = one call row over all C channels (the gain is linked).  The slot's C channel rows are consecutive, so the
+// scaffold's slot_row finds them as one row of C row_floats.  Row i pushes n = counts[i] * unit samples (0 outside
+// [0, max_in]: the row stores nothing) and writes y[i][c][0 .. n).
+__global__ void __launch_bounds__(RS_TILE)
+limiter_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, int max_in, const int32_t* __restrict__ counts,
+               int unit, float* __restrict__ y, int64_t y_row, int64_t y_ch, int C, const int32_t* __restrict__ slots,
+               float* __restrict__ state, int n_slots, float ceiling, int La, int step) {
+    extern __shared__ float sm[];
+    __shared__ int64_t warp_max[RS_TILE / 32];
+    __shared__ int limited;
+    const int tid = threadIdx.x;
+    const int64_t rf = LM_HEAD + 3 * (int64_t)La;
+    const SlotRow sr = slot_row(1, slots, n_slots, state, C * rf);
+    const int64_t pushed = (int64_t)counts[sr.row] * unit;
+    const int n = pushed >= 0 && pushed <= max_in ? (int)pushed : 0;
+    if (!sr.live || n == 0) return;                                     // a row that stores nothing
+    float* st = sr.st;                                                  // channel c's row at st + c rf
+    const int W = La + n;
+    float* xs = sm;                                                     // [C][W]: each channel's delay line, then x
+    int* qs = reinterpret_cast<int*>(sm + (int64_t)C * W);              // [W]: the last La q, then the new ones
+    int* rs = qs + W;                                                   // [W]: the last La r, then s, then r
+    const float cw = st[1];
+    const float lim = cw >= FLT_MIN && cw <= FLT_MAX ? cw : ceiling;     // the slot's ceiling, else the call's
+    const int64_t r_in = min(max(__float_as_int(st[0]), 0), LM_MUTE);
+    for (int c = 0; c < C; ++c) {
+        const float* d = st + c * rf + LM_HEAD;
+        const float* xr = row_ch(x, x_row, x_ch, sr.row, c);
+        for (int i = tid; i < W; i += blockDim.x) xs[(int64_t)c * W + i] = i < La ? d[i] : xr[i - La];
+    }
+    for (int i = tid; i < La; i += blockDim.x) {
+        qs[i] = min(max(__float_as_int(st[LM_HEAD + La + i]), 0), LM_MUTE);
+        rs[i] = min(max(__float_as_int(st[LM_HEAD + 2 * La + i]), 0), LM_MUTE);
+    }
+    if (tid == 0) limited = 0;
+    __syncthreads();
+    for (int k = tid; k < n; k += blockDim.x) {
+        float p = 0.f;
+        bool finite = true;
+        for (int c = 0; c < C; ++c) {
+            const float v = xs[(int64_t)c * W + La + k];
+            finite = finite && isfinite(v);
+            p = fmaxf(p, fabsf(v));
+        }
+        int q = 0;
+        if (!finite) q = LM_MUTE;
+        else if (p > lim) q = (int)fmin((double)LM_MUTE, ceil(LM_Q * log2((double)p / (double)lim)) + 1.0);
+        qs[La + k] = q;
+    }
+    __syncthreads();
+    // hold and release over contiguous pieces of the push, one per thread: r[k] = max(r_in - (k + 1) step,
+    // max_{j <= k} (s[j] + j step) - k step), the running max carried across the pieces by a block scan
+    const int per = (n + blockDim.x - 1) / blockDim.x, k0 = min(n, tid * per), k1 = min(n, k0 + per);
+    int64_t run = INT64_MIN;
+    for (int k = k0; k < k1; ++k) {
+        int s = 0;
+        for (int j = k; j <= k + La; ++j) s = max(s, qs[j]);             // q[k - La .. k]
+        rs[La + k] = s;
+        run = max(run, s + (int64_t)k * step);
+    }
+    run = block_exclusive_max(run, warp_max);
+    for (int k = k0; k < k1; ++k) {
+        run = max(run, rs[La + k] + (int64_t)k * step);
+        rs[La + k] = (int)max(r_in - (int64_t)(k + 1) * step, run - (int64_t)k * step);
+    }
+    __syncthreads();
+    const double inv = 1.0 / ((double)LM_Q * (La + 1));
+    int mine = 0;
+    for (int k = tid; k < n; k += blockDim.x) {
+        int64_t a = 0;
+        for (int j = k; j <= k + La; ++j) a += rs[j];                    // r[k - La .. k], exact in any order
+        // the gain 2^-e as 2^-f 2^-i (i = floor(e)): the power of two scales exactly, so a gain below the normal range
+        // keeps its precision
+        const double e = (double)a * inv;
+        const int ei = (int)e;
+        const float gf = a == 0 ? 1.f : (a >= (int64_t)LM_MUTE * (La + 1) ? 0.f : exp2f(-(float)(e - ei)));
+        mine += a > 0;
+        for (int c = 0; c < C; ++c) {
+            const float v = xs[(int64_t)c * W + k];                     // x[c][k - La]
+            row_ch(y, y_row, y_ch, sr.row, c)[k] = isfinite(v) ? (ei ? ldexpf(gf * v, -ei) : gf * v) : 0.f;
+        }
+        if (k == n - 1) st[3] = (float)(e * 6.020599913279624);        // 20 log10(2) dB per octave
+    }
+    if (mine) atomicAdd(&limited, mine);
+    for (int c = 0; c < C; ++c)
+        for (int i = tid; i < La; i += blockDim.x) st[c * rf + LM_HEAD + i] = xs[(int64_t)c * W + n + i];
+    for (int i = tid; i < La; i += blockDim.x) {
+        st[LM_HEAD + La + i] = __int_as_float(qs[n + i]);
+        st[LM_HEAD + 2 * La + i] = __int_as_float(rs[n + i]);
+    }
+    __syncthreads();                                                    // every thread counted
+    if (tid == 0) {
+        st[0] = __int_as_float(rs[La + n - 1]);
+        const int before = max(__float_as_int(st[2]), 0);
+        st[2] = __int_as_float(limited > INT32_MAX - before ? INT32_MAX : before + limited);
+    }
+}
+
 // ---- the host side of the per-slot calls ------------------------------------------------------------------------------
 // The checks every per-slot call makes first, in this order: its pointers, its sizes (`sizes` names them), n <= n_slots,
 // and a grid of n * channels CTAs.  0, or 1 with its message.
@@ -835,5 +968,57 @@ extern "C" int l2h_target_mix_set(float* state_dev, int32_t n_records, int32_t n
     const int jobs = n * channels;
     target_mix_set_kernel<<<(unsigned)((jobs + RS_TILE - 1) / RS_TILE), RS_TILE, 0, static_cast<cudaStream_t>(stream)>>>(
         state_dev, n_records, n_records + n_slots, channels, rows_dev, n, gains_dev, starts_dev, fades_dev);
+    return launched(who);
+}
+
+namespace l2h {
+// the staged floats of a limiter row of `max_in` samples: 0, or an error code (1 invalid, 2 the staging exceeds shared
+// memory) with its message
+static int lm_staging(const std::string& who, int32_t channels, int32_t lookahead, int32_t max_in, int* smem) {
+    if (channels <= 0) return fail(1, who + ": channels must be positive");
+    if (lookahead < 0) return fail(1, who + ": lookahead " + std::to_string(lookahead) + " is negative");
+    const int64_t floats = ((int64_t)channels + 2) * ((int64_t)lookahead + max_in);
+    if (floats * (int64_t)sizeof(float) > RS_SMEM_BYTES)
+        return fail(2, who + ": " + std::to_string(channels) + " channels with a look-ahead of " + std::to_string(lookahead) +
+                           " samples and pushes of up to " + std::to_string(max_in) + " samples are too large: " +
+                           std::to_string(floats) + " staged words per row exceed shared memory (" +
+                           std::to_string(RS_SMEM_BYTES / sizeof(float)) + ")");
+    *smem = (int)(floats * sizeof(float));
+    return 0;
+}
+}  // namespace l2h
+
+extern "C" int l2h_limiter_layout(int32_t channels, int32_t lookahead, int32_t* row_floats) {
+    using namespace l2h;
+    if (!row_floats) return fail(1, "l2h_limiter_layout: null pointer");
+    int smem;
+    if (int rc = lm_staging("l2h_limiter_layout", channels, lookahead, 1, &smem)) return rc;
+    *row_floats = LM_HEAD + 3 * lookahead;
+    return 0;
+}
+
+extern "C" int l2h_limiter(const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, int32_t max_in,
+                           const int32_t* counts_dev, int32_t unit, float* y_dev, int64_t y_row_stride, int64_t y_ch_stride,
+                           int32_t n, int32_t channels, const int32_t* slots_dev, float* state_dev, int32_t n_slots,
+                           float ceiling, int32_t lookahead, int32_t release_step, void* stream) {
+    using namespace l2h;
+    const std::string who = "l2h_limiter";
+    if (int rc = slot_call(who, {x_dev, counts_dev, y_dev, slots_dev, state_dev}, "n, channels, max_in, unit and n_slots",
+                           {n, channels, max_in, unit, n_slots}, n, channels, n_slots))
+        return rc;
+    if (!(ceiling >= FLT_MIN && ceiling <= FLT_MAX))
+        return fail(1, who + ": ceiling " + std::to_string(ceiling) + " is not a positive normal float");
+    if (release_step <= 0 || release_step > LM_MUTE)
+        return fail(1, who + ": release_step " + std::to_string(release_step) + " lies outside [1, " +
+                           std::to_string(LM_MUTE) + "]");
+    int smem;
+    if (int rc = lm_staging(who, channels, lookahead, max_in, &smem)) return rc;
+    const Rows x{"x", x_row_stride, x_ch_stride, max_in}, y{"y", y_row_stride, y_ch_stride, max_in};
+    if (int rc = disjoint(who, channels, {x, y})) return rc;
+    const auto a = span(x_dev, n, channels, x), b = span(y_dev, n, channels, y);
+    if (a.first < b.second && b.first < a.second) return fail(1, who + ": y must not overlap x");
+    limiter_kernel<<<(unsigned)n, RS_TILE, smem, static_cast<cudaStream_t>(stream)>>>(
+        x_dev, x_row_stride, x_ch_stride, max_in, counts_dev, unit, y_dev, y_row_stride, y_ch_stride, channels, slots_dev,
+        state_dev, n_slots, ceiling, lookahead, release_step);
     return launched(who);
 }

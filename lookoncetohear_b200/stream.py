@@ -2,9 +2,10 @@
 `Net.advance_slots`: streaming resampling for listeners whose devices run at another rate than the separator's 16 kHz
 (`StreamResampler`, `l2h_resample_stream`), with pushes of any length (`PacketResampler`, `l2h_resample_packets`), the
 per-slot FIFO that turns 16 kHz pieces into separator chunks and hop counts (`HopFifo`, `l2h_hop_fifo`), and the
-per-slot capture that keeps each listener's recent input for enrollment (`EnrollCapture`, `l2h_enroll_capture`), and
+per-slot capture that keeps each listener's recent input for enrollment (`EnrollCapture`, `l2h_enroll_capture`),
 the per-listener mixer that sums the separated voices and the ambient mixture into one row with fades (`TargetMixer`,
-`l2h_target_mix`).
+`l2h_target_mix`), and the per-listener look-ahead limiter that keeps the output under a ceiling with one gain for both
+ears (`Limiter`, `l2h_limiter`).
 
 Each stage keeps a float32 state [slots, channels, row floats] on a CUDA device.  All zeros is a fresh slot, so a
 listener is reset by zeroing its rows (`reset`) and moved by copying them.  No CPU fallback."""
@@ -478,3 +479,103 @@ class TargetMixer(_SlotStage):
         """[records + slots] bool CUDA tensor: the rows whose ramp has samples left to mix, never synchronising"""
         _, _, F, p, is_set = self._words()
         return is_set & (p < F)
+
+
+class Limiter(_SlotStage):
+    """A per-slot look-ahead peak limiter on the device (l2h_limiter): each listener's output kept under `ceiling`, with
+    one gain for all channels at each sample, so the interaural level ratios the binaural output carries are preserved.
+    Place it after the up-resampler, on the samples the device plays: band-limited upsampling of a signal limited at
+    16 kHz can overshoot the ceiling between its samples.
+
+    Every written sample satisfies |y| <= ceiling exactly, whatever the input.  Output is the slot's signal delayed by
+    La = round(lookahead * rate) samples (La / rate of added latency; 44 samples at 44.1 kHz for the 1 ms default), times
+    a gain that is exactly 1 while no reduction is pending, so below the ceiling y is the delayed input bit for bit.  A
+    peak is met by a gain reduction that starts La samples ahead of it, and the reduction then recovers at `release` dB
+    per second.  The gain is computed in an integer log domain, so cutting a stream into other pushes changes no bit of
+    the output or the state.  A non-finite sample is written as 0 and mutes the output around it; the gain then recovers
+    at the release rate from about 900 dB of reduction, and `reset` ends the mute at once.
+
+    `state` [slots, channels, 4 + 3 La] is a float32 tensor on `device`: all zeros is a fresh slot, so a listener is reset
+    by zeroing its rows (`reset`) and moved by copying them."""
+
+    Q = 65536                                  # log-gain quanta per octave of amplitude (l2h_limiter)
+    MUTE = 150 * Q                             # the cap of a reduction, a gain of exactly 0
+    DB_PER_OCTAVE = 20 * math.log10(2)
+
+    def __init__(self, slots, channels, rate, ceiling=10 ** (-1 / 20), lookahead=0.001, release=80.0, device=None):
+        super().__init__(slots, channels)
+        self.rate = _whole(rate, "rate")
+        self.ceiling = self._level(ceiling, "ceiling")
+        if isinstance(lookahead, bool) or not isinstance(lookahead, numbers.Real) or not 0 <= lookahead < 2 ** 31 / self.rate:
+            raise ValueError(f"lookahead must be a number of seconds >= 0, got {lookahead!r}")
+        if (isinstance(release, bool) or not isinstance(release, numbers.Real) or not math.isfinite(release)
+                or release <= 0):
+            raise ValueError(f"release must be a positive number of dB per second, got {release!r}")
+        self.lookahead = round(lookahead * self.rate)
+        self.release_step = max(1, round(release / self.DB_PER_OCTAVE * self.Q / self.rate))
+        if self.release_step > self.MUTE:
+            raise ValueError(f"release {release!r} dB/s recovers more than the whole range in one sample")
+        self._allocate(*_layout(_cabi.lib().l2h_limiter_layout, self.channels, self.lookahead), device)
+
+    @staticmethod
+    def _level(v, what, zero=False):
+        """v rounded to float32, where it must be a positive normal number (or 0 if `zero`), or ValueError"""
+        ok = not isinstance(v, bool) and isinstance(v, numbers.Real) and math.isfinite(v)
+        f = float(torch.tensor(float(v), dtype=torch.float32)) if ok else math.nan
+        if not (ok and (2.0 ** -126 <= f < math.inf or (zero and v == 0))):
+            raise ValueError(f"{what} must be a positive amplitude that float32 holds as a normal number, got {v!r}")
+        return f
+
+    def __call__(self, x, counts, slots, unit=1, out=None):
+        """x [n, channels, L] CUDA tensor: row i pushes its first counts[i] * unit samples into slot slots[i] and receives
+        as many back, y[i, :, :counts[i] * unit]: its slot's signal delayed by La samples times the linked gain.  Returns
+        y [n, channels, L] float32 (`out`, if given, written in place; it must not overlap x).  Its later samples are left
+        unwritten.
+
+        `counts`/`unit` follow the packet stages: lim(y44, n44, slots) after PacketResampler up,
+        lim(y48, hops, slots, unit=384) after a 48 kHz StreamResampler up, lim(mix, hops, slots, unit=128) on the mixer's
+        16 kHz output.  Host lists are checked (slots n distinct ints in [0, slots), counts n ints in [0, L // unit]) and
+        uploaded; contiguous CUDA int32 tensors are used in place and read when the kernel runs, where a slot outside
+        [0, slots) or a count * unit outside [0, L] marks a row that stores nothing (neither its out row nor its state
+        rows change).  So a call captured in the tick's CUDA graph serves any lists rewritten in place."""
+        x = self._rows_in(x)
+        dev = self.state.device
+        n, C, L = x.shape
+        unit = _whole(unit, "unit")
+        slots = device_list(slots, dev, n, self.n_slots, True, "slot")
+        counts = device_list(counts, dev, n, L // unit + 1, False, "count")
+        out = self._rows_out(out, (n, C, L))
+        with torch.cuda.device(dev):
+            _check(_cabi.lib().l2h_limiter(
+                x.data_ptr(), x.stride(0), x.stride(1), L, counts.data_ptr(), unit, out.data_ptr(), out.stride(0),
+                out.stride(1), n, C, slots.data_ptr(), self.state.data_ptr(), self.n_slots, self.ceiling,
+                self.lookahead, self.release_step, self._stream()))
+        return out
+
+    def set_ceiling(self, slots, values):
+        """Give the listed slots their own ceilings (a hearing-safety cap per user): `values` one number or one per slot,
+        positive finite amplitudes, or 0 for the limiter's `ceiling`.  It applies to the samples pushed after the set.
+        Enqueued on the current stream; `reset` returns a slot to the default."""
+        dev = self.state.device
+        idx = torch.as_tensor(slots).cpu().reshape(-1)
+        n = idx.numel()
+        if n < 1:
+            raise ValueError("set_ceiling needs at least one slot")
+        idx = device_list(idx, dev, n, self.n_slots, True, "slot")
+        vals = values.tolist() if isinstance(values, torch.Tensor) else values
+        vals = list(vals) if isinstance(vals, (list, tuple)) else [vals] * n
+        if len(vals) != n:
+            raise ValueError(f"values gives {len(vals)} ceilings for {n} slots")
+        vals = [self._level(v, "a ceiling", zero=True) for v in vals]
+        self.state[idx.long(), 0, 1] = torch.tensor(vals, dtype=torch.float32).to(dev)
+
+    @property
+    def reduction(self):
+        """[slots] float32 CUDA view of the state: the dB of gain reduction at the last sample each slot wrote"""
+        return self.state[:, 0, 3]
+
+    @property
+    def limited(self):
+        """[slots] int32 CUDA view of the state: the samples each slot wrote with a gain reduction since its reset
+        (saturating at 2**31 - 1)"""
+        return self.state[:, 0, 2].view(torch.int32)
