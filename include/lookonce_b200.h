@@ -36,6 +36,8 @@
  *           (TargetMixer)
  *   l2h_limiter
  *        <- keeping each listener's output under a ceiling, with one gain for both ears (Limiter)
+ *   l2h_leveler
+ *        <- bringing each voice a listener hears to one loudness, with one gain for both ears (Leveler)
  *
  * Conventions follow the reference's only FFI (src/datasets/motion_simulator.py:30-95): every
  * function returns int (0 = OK, non-zero = error, text via l2h_last_error()), handles are opaque
@@ -811,6 +813,64 @@ int l2h_limiter(const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, i
                 int32_t unit, float* y_dev, int64_t y_row_stride, int64_t y_ch_stride, int32_t n, int32_t channels,
                 const int32_t* slots_dev, float* state_dev, int32_t n_slots, float ceiling, int32_t lookahead,
                 int32_t release_step, void* stream);
+
+/* A per-row loudness leveler: brings each voice a listener hears to one loudness, with one gain for all channels, so
+ * interaural level ratios are preserved.  A row is a separator record (the target rows of l2h_sep_forward_targets_rows,
+ * before the mixer) or a listener slot (the mixer's sum).  It works on the separator's 16 kHz grid of 128-sample hops,
+ * with no look-ahead and no added delay.  Per hop of a row, over its channels:
+ *     each channel passes the two BS.1770 pre-filters ("K-weighting") for 16 kHz, derived from the analog prototypes as
+ *       libebur128 derives them: a high shelf (f0 = 1681.974450955533 Hz, G = 3.999843853973347 dB, Q = 0.7071752369554196,
+ *       Vb = Vh^0.4996667741545416), then a high-pass (f0 = 38.13547087602444 Hz, Q = 0.5003270373238773), K = tan(pi f0 / fs);
+ *     P = the mean square of the weighted samples over the hop, summed over the channels; its loudness -0.691 + 10 log10 P
+ *       LUFS;
+ *     gate: a hop updates the estimate only when its loudness is at least `gate` and, once the row has an estimate, at
+ *       least the estimate's loudness + `relative` (so pauses and a silent target's residual never pull the gain up);
+ *     estimate: E <- E + w (P - E), w = max(alpha, 1 / (n + 1)) with n the gated hops before: the plain mean of the first
+ *       hops, then an exponential average;
+ *     gain (dB, one per row): 0 until the row has settle_hops gated hops; in the hop that reaches them,
+ *       d = clamp(target - L(E), min_gain, max_gain); after that it moves toward d by at most rise_step dB up and
+ *       fall_step dB down per hop (a hop that fails the gate still moves it toward the d of the held estimate);
+ *     apply: sample k = 1 .. 128 of the hop is multiplied, in every channel, by 10^(g_k / 20) with
+ *       g_k = g_prev + (g_new - g_prev) k / 128; a g_k of 0 dB is exactly 1.0f.
+ * With min_gain = max_gain = 0 every written sample is its input bit for bit.  A hop with a sample that is not finite,
+ * or whose magnitude is 2^32 or more, is not measured: its filters, estimate, count and gain keep their values (its samples
+ * are written as x times the held gain, and a limiter downstream mutes a non-finite one), so the state stays finite.  A
+ * hop's result depends only on the state at its start and its samples, so cutting hops into other calls changes no bit.
+ *
+ * The state is [n_rows][channels][row_floats] fp32 of DEVICE memory.  Per channel: three head words, then the channel's
+ * shelf and high-pass states (two each).  The head words are channel 0's only: the estimate E (mean-square power), the
+ * gated hops n (an int32 word stored in the float's bits, saturating at 2^31 - 1) and the gain in dB at the last sample
+ * written.  All zeros is a fresh row, so a row is reset by zeroing it and moved by copying it.
+ * l2h_leveler_layout: row_floats = 7.  Errors: 1 = null pointer, channels <= 0.
+ *
+ * l2h_leveler: call row r (one CTA each, over all its channels) levels y[r][c][0 .. 128 h) into out[r][c][0 .. 128 h):
+ *   y_dev        [R][channels][128 * frames] fp32, strides in floats
+ *   out_dev      the same shape; its rows' later samples, and the rows that store nothing, are not written.  out may be
+ *                y itself (the same pointer and strides), which levels in place; any other overlap is refused.
+ *   records_dev  [R] int32 of DEVICE memory: row r keeps its state in row records[r]; a record outside [0, n_rows) marks
+ *                a row that stores nothing and advances nothing.  A record listed twice is a caller error the call does
+ *                not detect.
+ *   offsets_dev  [n + 1] int32 of DEVICE memory: listener i owns rows offsets[i] .. offsets[i+1]-1, the offsets clamped as
+ *                l2h_sep_forward_targets_rows and l2h_target_mix clamp them; rows from offsets[n] on belong to nobody and
+ *                store nothing.  NULL: listener i owns row i alone (rows from n on store nothing), the placement on the
+ *                mixer's sum with records = slots.
+ *   hops_dev     [n] int32 of DEVICE memory, or NULL (frames hops): listener i's rows level h = hops[i] hops; h outside
+ *                [1, frames] stores nothing.
+ *   alpha        1 - exp(-128 / (window * 16000)) for an averaging window in seconds; rise_step and fall_step in dB per
+ *                hop (dB/s * 128 / 16000); settle_hops in hops.
+ * All lists are read when the kernel runs, so a call captured in a CUDA graph with the FIFO, the rows call and the mixer
+ * serves any lists of the same n and R rewritten in place.  One launch; nothing is read back to the host.  Errors,
+ * returned before anything is enqueued: 1 = null pointers (offsets_dev and hops_dev may be NULL), n, R, channels, frames
+ * or n_rows <= 0, n > R, n > n_rows, 128 frames above 2^31 - 1, a target, gate, relative, min_gain or max_gain that is
+ * not finite, relative > 0, alpha outside (0, 1], min_gain > max_gain or a gain outside [-40, 40] dB, rise_step or
+ * fall_step negative or not finite, settle_hops < 1, channel or row strides under 128 frames, out overlapping y other than
+ * as y itself.  Asynchronous on `stream`. */
+int l2h_leveler_layout(int32_t channels, int32_t* row_floats);
+int l2h_leveler(const float* y_dev, int64_t y_row_stride, int64_t y_ch_stride, float* out_dev, int64_t out_row_stride,
+                int64_t out_ch_stride, int32_t n, int32_t R, int32_t channels, int32_t frames, const int32_t* records_dev,
+                const int32_t* offsets_dev, const int32_t* hops_dev, float* state_dev, int32_t n_rows, float target,
+                float gate, float relative, float alpha, int32_t settle_hops, float min_gain, float max_gain,
+                float rise_step, float fall_step, void* stream);
 
 #ifdef __cplusplus
 }

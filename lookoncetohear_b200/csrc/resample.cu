@@ -20,8 +20,9 @@
 // the streaming resamplers (pushes of whole periods, resample_stream_kernel; pushes of any length,
 // resample_packets_kernel), the hop FIFO that turns 16 kHz pieces into separator chunks (hop_fifo_kernel), the
 // enrollment capture (enroll_capture_kernel), the target mixer that sums a listener's separated voices and its ambient
-// mixture into one row (target_mix_kernel, target_mix_set_kernel), and the look-ahead limiter that keeps each listener's
-// output under a ceiling with one gain for all channels (limiter_kernel).
+// mixture into one row (target_mix_kernel, target_mix_set_kernel), the look-ahead limiter that keeps each listener's
+// output under a ceiling with one gain for all channels (limiter_kernel), and the leveler that brings each voice to one
+// loudness with one gain for all channels (leveler_kernel).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -680,6 +681,121 @@ limiter_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, int max
     }
 }
 
+// ---- the leveler: a gated, K-weighted loudness leveler per row, one gain for all channels ------------------------------
+// A row (a separator record, or a listener slot on the mixer's sum) is leveled hop by hop on the 16 kHz grid.  Each
+// channel's samples pass the two BS.1770 pre-filters (a high shelf, then a high-pass, in transposed direct form II); the
+// hop's power P is the mean square of the weighted samples summed over the channels, its loudness -0.691 + 10 log10 P
+// LUFS.  A hop at or above `gate`, and, once the row has an estimate, at or above the estimate's loudness + `relative`,
+// updates the estimate E += w (P - E), w = max(alpha, 1 / (n + 1)) over the n gated hops before it.  The gain (dB) stays
+// where it is until the row has `settle` gated hops, takes d = clamp(target - L(E), min_gain, max_gain) in the hop that
+// reaches them, and then moves toward d by at most `rise` dB up and `fall` dB down per hop.  Sample k = 1 .. 128 of the hop
+// is scaled in every channel by the gain interpolated in dB from the hop's start to its end; a gain of 0 dB is exactly 1.
+// A hop with a sample that is not finite, or whose magnitude reaches 2^32 (where the weighted squares could overflow), is
+// not measured: filters, estimate, count and gain keep their values, so the state stays finite.  A hop's result depends
+// only on the state at its start and its samples, so cutting the hops into other calls changes no bit.
+// A row's state per channel is [LV_HEAD + 4]: the head words (channel 0's only: E, n as an int32 word, the gain in dB),
+// then the channel's shelf and high-pass states.  All zeros is a fresh row.
+constexpr int LV_HEAD = 3;
+constexpr int LV_FLOATS = LV_HEAD + 4;
+constexpr int LV_THREADS = TM_THREADS;                  // one thread per sample of a hop; block_max's block
+constexpr float LV_BIG = 4294967296.f;                  // 2^32
+constexpr float LV_LOG2_10_20 = 0.16609640474436813f;   // log2(10) / 20: dB to an octave of amplitude
+static_assert(LV_THREADS == CHUNK_HOP, "the leveler runs one thread per sample of a hop");
+
+struct LvParams {
+    float sb0, sb1, sb2, sa1, sa2;   // the shelf
+    float ha1, ha2;                  // the high-pass, whose numerator is 1, -2, 1
+    float target, gate, relative, alpha, min_gain, max_gain, rise, fall;
+    int settle;
+};
+
+L2H_DEVINL float lv_lufs(float power) { return -0.691f + 10.f * log10f(power); }
+
+// One CTA = one call row over all C channels (the gain is linked).  Listener i owns rows start .. end - 1 (the separator's
+// clamp: the first j with offsets[j] > r ends the listeners at or before row r), or row i alone without offsets; its rows
+// level their first 128 h samples, h = hops[i] (T without hops).  Row r keeps its state in row records[r].  y and out may
+// be the same tensor: each hop's samples are read before they are written.
+__global__ void __launch_bounds__(LV_THREADS)
+leveler_kernel(const float* y, int64_t y_row, int64_t y_ch, float* out, int64_t o_row, int64_t o_ch, int n, int C, int T,
+               const int32_t* __restrict__ records, const int32_t* __restrict__ offsets, const int32_t* __restrict__ hops,
+               float* __restrict__ state, int n_rows, const __grid_constant__ LvParams p) {
+    __shared__ int red[LV_THREADS / 32];
+    __shared__ float part[LV_THREADS];
+    __shared__ float g_from, g_to;                                      // the hop's gain in dB at its start and its end
+    const int tid = threadIdx.x;
+    const SlotRow sr = slot_row(1, records, n_rows, state, (int64_t)C * LV_FLOATS);
+    const int r = sr.row;
+    int i = r;
+    if (offsets) {
+        int first = n + 1;
+        for (int j = tid; j <= n; j += LV_THREADS)
+            if (offsets[j] > r) { first = j; break; }
+        i = -block_max(-first, red) - 1;
+    }
+    const int h = i >= 0 && i < n ? (hops ? hops[i] : T) : 0;
+    if (!sr.live || h <= 0 || h > T) return;                            // a row that stores nothing
+    float* st = sr.st;                                                  // channel c's row at st + c LV_FLOATS
+    float E = st[0], g = st[2];
+    int cnt = max(__float_as_int(st[1]), 0);
+    for (int t = 0; t < h; ++t) {
+        const int64_t s = (int64_t)t * CHUNK_HOP + tid;
+        bool bad = false;
+        for (int c = 0; c < C; ++c) bad = bad || !(fabsf(row_ch(y, y_row, y_ch, r, c)[s]) < LV_BIG);
+        const bool measured = !__syncthreads_or(bad);
+        if (measured) {
+            float acc = 0.f;
+            for (int c = tid; c < C; c += LV_THREADS) {
+                float* f = st + (int64_t)c * LV_FLOATS + LV_HEAD;
+                float s1 = f[0], s2 = f[1], h1 = f[2], h2 = f[3];
+                const float* xr = row_ch(y, y_row, y_ch, r, c) + (int64_t)t * CHUNK_HOP;
+#pragma unroll 16
+                for (int k = 0; k < CHUNK_HOP; ++k) {
+                    const float x = xr[k];
+                    const float u = fmaf(p.sb0, x, s1);
+                    s1 = fmaf(p.sb1, x, fmaf(-p.sa1, u, s2));
+                    s2 = fmaf(p.sb2, x, -p.sa2 * u);
+                    const float w = u + h1;
+                    h1 = fmaf(-2.f, u, fmaf(-p.ha1, w, h2));
+                    h2 = fmaf(-p.ha2, w, u);
+                    acc = fmaf(w, w, acc);
+                }
+                f[0] = s1; f[1] = s2; f[2] = h1; f[3] = h2;
+            }
+            part[tid] = acc;
+            __syncthreads();
+        }
+        if (tid == 0) {
+            const float g0 = g;
+            if (measured) {
+                float P = 0.f;
+                for (int c = 0; c < min(C, LV_THREADS); ++c) P += part[c];   // channel order: the same bits every call
+                P *= 1.f / CHUNK_HOP;
+                const float L = lv_lufs(P);
+                const int before = cnt;
+                if (L >= p.gate && (cnt == 0 || L >= lv_lufs(E) + p.relative)) {
+                    E = fmaf(fmaxf(p.alpha, 1.f / (float)(cnt + 1)), P - E, E);
+                    cnt += cnt < INT32_MAX;
+                }
+                if (cnt >= p.settle) {
+                    const float d = fminf(fmaxf(p.target - lv_lufs(E), p.min_gain), p.max_gain);
+                    g = before < p.settle ? d : g + fminf(fmaxf(d - g, -p.fall), p.rise);
+                }
+            }
+            g_from = g0;
+            g_to = g;
+        }
+        __syncthreads();
+        const float gk = fmaf(g_to - g_from, (float)(tid + 1) * (1.f / CHUNK_HOP), g_from);
+        const float lin = gk == 0.f ? 1.f : exp2f(gk * LV_LOG2_10_20);
+        for (int c = 0; c < C; ++c) row_ch(out, o_row, o_ch, r, c)[s] = row_ch(y, y_row, y_ch, r, c)[s] * lin;
+    }
+    if (tid == 0) {
+        st[0] = E;
+        st[1] = __int_as_float(cnt);
+        st[2] = g;
+    }
+}
+
 // ---- the host side of the per-slot calls ------------------------------------------------------------------------------
 // The checks every per-slot call makes first, in this order: its pointers, its sizes (`sizes` names them), n <= n_slots,
 // and a grid of n * channels CTAs.  0, or 1 with its message.
@@ -1020,5 +1136,79 @@ extern "C" int l2h_limiter(const float* x_dev, int64_t x_row_stride, int64_t x_c
     limiter_kernel<<<(unsigned)n, RS_TILE, smem, static_cast<cudaStream_t>(stream)>>>(
         x_dev, x_row_stride, x_ch_stride, max_in, counts_dev, unit, y_dev, y_row_stride, y_ch_stride, channels, slots_dev,
         state_dev, n_slots, ceiling, lookahead, release_step);
+    return launched(who);
+}
+
+namespace l2h {
+// The BS.1770 pre-filters at `rate` Hz from their analog prototypes, as libebur128 derives them (at 48 kHz they are the
+// recommendation's table): a high shelf, then a high-pass whose numerator is 1, -2, 1.
+static void lv_filters(double rate, LvParams* p) {
+    double K = std::tan(M_PI * 1681.974450955533 / rate);
+    const double Q = 0.7071752369554196, Vh = std::pow(10.0, 3.999843853973347 / 20.0);
+    const double Vb = std::pow(Vh, 0.4996667741545416), a0 = 1.0 + K / Q + K * K;
+    p->sb0 = (float)((Vh + Vb * K / Q + K * K) / a0);
+    p->sb1 = (float)(2.0 * (K * K - Vh) / a0);
+    p->sb2 = (float)((Vh - Vb * K / Q + K * K) / a0);
+    p->sa1 = (float)(2.0 * (K * K - 1.0) / a0);
+    p->sa2 = (float)((1.0 - K / Q + K * K) / a0);
+    K = std::tan(M_PI * 38.13547087602444 / rate);
+    const double Qh = 0.5003270373238773, ah = 1.0 + K / Qh + K * K;
+    p->ha1 = (float)(2.0 * (K * K - 1.0) / ah);
+    p->ha2 = (float)((1.0 - K / Qh + K * K) / ah);
+}
+}  // namespace l2h
+
+extern "C" int l2h_leveler_layout(int32_t channels, int32_t* row_floats) {
+    using namespace l2h;
+    if (!row_floats) return fail(1, "l2h_leveler_layout: null pointer");
+    if (channels <= 0) return fail(1, "l2h_leveler_layout: channels must be positive");
+    *row_floats = LV_FLOATS;
+    return 0;
+}
+
+extern "C" int l2h_leveler(const float* y_dev, int64_t y_row_stride, int64_t y_ch_stride, float* out_dev,
+                           int64_t out_row_stride, int64_t out_ch_stride, int32_t n, int32_t R, int32_t channels,
+                           int32_t frames, const int32_t* records_dev, const int32_t* offsets_dev, const int32_t* hops_dev,
+                           float* state_dev, int32_t n_rows, float target, float gate, float relative, float alpha,
+                           int32_t settle_hops, float min_gain, float max_gain, float rise_step, float fall_step,
+                           void* stream) {
+    using namespace l2h;
+    const std::string who = "l2h_leveler";
+    if (int rc = slot_call(who, {y_dev, out_dev, records_dev, state_dev}, "n, R, channels, frames and n_rows",
+                           {n, R, channels, frames, n_rows}, n, channels, n_rows))
+        return rc;
+    if (n > R) return fail(1, who + ": a call needs n <= R (every listener row owns its rows)");
+    if ((int64_t)frames * CHUNK_HOP > INT32_MAX) return fail(1, who + ": frames is too large");
+    for (float v : {target, gate, relative, min_gain, max_gain})
+        if (!std::isfinite(v)) return fail(1, who + ": target, gate, relative, min_gain and max_gain must be finite");
+    if (relative > 0.f) return fail(1, who + ": relative " + std::to_string(relative) + " dB is above 0");
+    if (!(alpha > 0.f && alpha <= 1.f)) return fail(1, who + ": alpha " + std::to_string(alpha) + " lies outside (0, 1]");
+    if (!(min_gain <= max_gain && min_gain >= -40.f && max_gain <= 40.f))
+        return fail(1, who + ": the gain range [" + std::to_string(min_gain) + ", " + std::to_string(max_gain) +
+                           "] dB is empty or leaves [-40, 40]");
+    if (!(rise_step >= 0.f && fall_step >= 0.f && std::isfinite(rise_step) && std::isfinite(fall_step)))
+        return fail(1, who + ": rise_step and fall_step must be finite and not negative");
+    if (settle_hops < 1) return fail(1, who + ": settle_hops " + std::to_string(settle_hops) + " is below 1");
+    const int64_t len = (int64_t)frames * CHUNK_HOP;
+    const Rows y{"y", y_row_stride, y_ch_stride, len}, out{"out", out_row_stride, out_ch_stride, len};
+    if (int rc = disjoint(who, channels, {y, out})) return rc;
+    const bool in_place = out_dev == y_dev && out_row_stride == y_row_stride && out_ch_stride == y_ch_stride;
+    const auto a = span(y_dev, R, channels, y), b = span(out_dev, R, channels, out);
+    if (!in_place && a.first < b.second && b.first < a.second)
+        return fail(1, who + ": out must be y itself (same pointer and strides) or not overlap it");
+    LvParams p;
+    lv_filters(16000.0, &p);
+    p.target = target;
+    p.gate = gate;
+    p.relative = relative;
+    p.alpha = alpha;
+    p.min_gain = min_gain;
+    p.max_gain = max_gain;
+    p.rise = rise_step;
+    p.fall = fall_step;
+    p.settle = settle_hops;
+    leveler_kernel<<<(unsigned)R, LV_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
+        y_dev, y_row_stride, y_ch_stride, out_dev, out_row_stride, out_ch_stride, n, channels, frames, records_dev,
+        offsets_dev, hops_dev, state_dev, n_rows, p);
     return launched(who);
 }

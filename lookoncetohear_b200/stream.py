@@ -4,8 +4,9 @@
 per-slot FIFO that turns 16 kHz pieces into separator chunks and hop counts (`HopFifo`, `l2h_hop_fifo`), and the
 per-slot capture that keeps each listener's recent input for enrollment (`EnrollCapture`, `l2h_enroll_capture`),
 the per-listener mixer that sums the separated voices and the ambient mixture into one row with fades (`TargetMixer`,
-`l2h_target_mix`), and the per-listener look-ahead limiter that keeps the output under a ceiling with one gain for both
-ears (`Limiter`, `l2h_limiter`).
+`l2h_target_mix`), the per-listener look-ahead limiter that keeps the output under a ceiling with one gain for both
+ears (`Limiter`, `l2h_limiter`), and the per-row leveler that brings each voice to one loudness with one gain for both
+ears (`Leveler`, `l2h_leveler`).
 
 Each stage keeps a float32 state [slots, channels, row floats] on a CUDA device.  All zeros is a fresh slot, so a
 listener is reset by zeroing its rows (`reset`) and moved by copying them.  No CPU fallback."""
@@ -579,3 +580,113 @@ class Limiter(_SlotStage):
         """[slots] int32 CUDA view of the state: the samples each slot wrote with a gain reduction since its reset
         (saturating at 2**31 - 1)"""
         return self.state[:, 0, 2].view(torch.int32)
+
+
+class Leveler(_SlotStage):
+    """A per-row loudness leveler on the device (l2h_leveler): each voice a listener hears brought to one loudness, with
+    one gain for all channels, so the interaural level ratios the binaural output carries are preserved.  A row is a
+    separator record (level the target rows of `Net.advance_target_rows` before the mixer, so voices that are 15-20 dB
+    apart in the mixture reach the mixer at one level), or a listener slot (level the mixer's sum, records = slots).
+
+    It works on the separator's 16 kHz grid, hop by hop, with no look-ahead and no added delay.  Each hop's loudness is
+    measured as BS.1770 defines it (K-weighted mean square, summed over the channels, in LUFS).  Hops that pass the
+    absolute `gate` and, once the row has an estimate, the `relative` gate below it update the estimate: the plain mean
+    of the first hops, then an exponential average over `window` seconds.  Pauses and a silent target's residual fail
+    the gate and never pull the gain up.  The gain (dB) stays at 0 until the row has `settle` seconds of gated hops, then
+    takes clamp(target - estimate, min_gain, max_gain) at once, and afterwards follows it at most `rise` dB/s up and
+    `fall` dB/s down.  The gain is interpolated in dB across each hop.  A hop's result depends only on the row's state and
+    its samples, so cutting hops into other ticks changes no bit; with min_gain = max_gain = 0 the output is the input bit
+    for bit.  A hop with a non-finite sample is not measured and leaves the state as it was.
+
+    The defaults are choices, not values tuned on trained separator output.
+
+    `state` [rows, channels, 7] is a float32 tensor on `device`: all zeros is a fresh row, so rows are reset by zeroing
+    them (`reset`) and moved by copying them."""
+
+    HOP_S = 128 / 16000                         # seconds per hop of the 16 kHz grid
+
+    def __init__(self, rows, channels, target=-20.0, gate=-50.0, relative=-20.0, window=3.0, settle=0.256,
+                 min_gain=-12.0, max_gain=12.0, rise=3.0, fall=10.0, device=None):
+        super().__init__(rows, channels)
+        num = {k: self._number(v, k) for k, v in (("target", target), ("gate", gate), ("relative", relative),
+                                                   ("window", window), ("settle", settle), ("min_gain", min_gain),
+                                                   ("max_gain", max_gain), ("rise", rise), ("fall", fall))}
+        if num["relative"] > 0:
+            raise ValueError(f"relative must be at most 0 LU, got {relative!r}")
+        if num["window"] <= 0 or num["settle"] <= 0:
+            raise ValueError(f"window and settle must be positive seconds, got {window!r} and {settle!r}")
+        if not -40.0 <= num["min_gain"] <= num["max_gain"] <= 40.0:
+            raise ValueError(f"the gain range must satisfy -40 <= min_gain <= max_gain <= 40 dB, got {min_gain!r}, "
+                             f"{max_gain!r}")
+        if num["rise"] < 0 or num["fall"] < 0:
+            raise ValueError(f"rise and fall must be dB/s >= 0, got {rise!r} and {fall!r}")
+        self.target, self.gate, self.relative = num["target"], num["gate"], num["relative"]
+        self.min_gain, self.max_gain = num["min_gain"], num["max_gain"]
+        self.alpha = -math.expm1(-self.HOP_S / num["window"])
+        self.settle_hops = max(1, round(num["settle"] / self.HOP_S))
+        self.rise_step, self.fall_step = num["rise"] * self.HOP_S, num["fall"] * self.HOP_S
+        if self.settle_hops >= 2 ** 31 or self.alpha <= 0:
+            raise ValueError(f"settle {settle!r} s or window {window!r} s is out of range")
+        self._allocate(*_layout(_cabi.lib().l2h_leveler_layout, self.channels), device)
+
+    @staticmethod
+    def _number(v, what):
+        if isinstance(v, bool) or not isinstance(v, numbers.Real) or not math.isfinite(v):
+            raise ValueError(f"{what} must be a finite number, got {v!r}")
+        return float(v)
+
+    def __call__(self, y, records, offsets=None, hops=None, out=None):
+        """y [R, channels, 128 * T] CUDA tensor: row r is leveled with the state of row records[r].  Returns out [R,
+        channels, 128 * T] float32 (`out`, if given, written in place; out=y levels y in place): listener i owns rows
+        offsets[i] .. offsets[i+1]-1 (without offsets, row i alone) and its rows receive their first 128 h samples, h =
+        hops[i] (T without hops).  Their later samples, and rows that store nothing, are left unwritten.
+
+        Lists follow TargetMixer: host lists are checked and uploaded (`records` R distinct ints in [0, rows); `offsets`
+        n + 1 ints from 0, non-decreasing, at most R; `hops` n ints in [0, T], n = R without offsets); contiguous CUDA
+        int32 tensors are used in place and read when the kernel runs, where a record outside the leveler marks a row
+        that stores nothing and advances nothing, the offsets are clamped as the separator clamps them, rows from
+        offsets[n] on store nothing, and a hop count outside [1, T] stores nothing.  So a call captured in a CUDA graph
+        with the FIFO, the separator and the mixer serves any lists rewritten in place.  Before the mixer:
+        lev(y, records, offsets, hops=hops, out=y); on the mixer's sum: lev(mix, slots, hops=hops, out=mix)."""
+        y = self._rows_in(y, self.HOP)
+        dev = self.state.device
+        R, C, L = y.shape
+        T = L // self.HOP
+        records = device_list(records, dev, R, self.n_slots, True, "record")
+        if offsets is None:
+            n = R
+        else:
+            n = (offsets.numel() if isinstance(offsets, torch.Tensor) else len(offsets)) - 1
+            if not 0 < n <= R:
+                raise ValueError(f"offsets must hold n + 1 entries with 0 < n <= R = {R}, got {n + 1}")
+            on_host = not (isinstance(offsets, torch.Tensor) and offsets.is_cuda)
+            o = torch.as_tensor(offsets).tolist() if on_host else None
+            offsets = device_list(offsets, dev, n + 1, R + 1, False, "offset")
+            if on_host and (o[0] != 0 or any(b < a for a, b in zip(o, o[1:]))):
+                raise ValueError(f"offsets must start at 0 and never decrease, got {o}")
+        if n > self.n_slots:
+            raise ValueError(f"a call of {n} listeners needs n <= rows = {self.n_slots}")
+        if hops is not None:
+            hops = device_list(hops, dev, n, T + 1, False, "hop")
+        out = self._rows_out(out, (R, C, L))
+        with torch.cuda.device(dev):
+            _check(_cabi.lib().l2h_leveler(
+                y.data_ptr(), y.stride(0), y.stride(1), out.data_ptr(), out.stride(0), out.stride(1), n, R, C, T,
+                records.data_ptr(), None if offsets is None else offsets.data_ptr(),
+                None if hops is None else hops.data_ptr(), self.state.data_ptr(), self.n_slots, self.target, self.gate,
+                self.relative, self.alpha, self.settle_hops, self.min_gain, self.max_gain, self.rise_step,
+                self.fall_step, self._stream()))
+        return out
+
+    @property
+    def loudness(self):
+        """[rows] float32 CUDA tensor: the loudness (LUFS) of each row's estimate, -inf before its first gated hop;
+        computed on the device, never synchronising"""
+        w = self.state[:, 0]
+        lufs = -0.691 + 10.0 * torch.log10(w[:, 0].clamp(min=torch.finfo(torch.float32).tiny))
+        return torch.where(w[:, 1].view(torch.int32) > 0, lufs, torch.full_like(lufs, -math.inf))
+
+    @property
+    def gain(self):
+        """[rows] float32 CUDA view of the state: each row's gain in dB at the last sample it wrote"""
+        return self.state[:, 0, 2]
