@@ -38,6 +38,9 @@
  *        <- keeping each listener's output under a ceiling, with one gain for both ears (Limiter)
  *   l2h_leveler
  *        <- bringing each voice a listener hears to one loudness, with one gain for both ears (Leveler)
+ *   l2h_band_compressor
+ *        <- fitting each listener's output to their hearing: gain per band and per ear, compression per band linked across
+ *           the ears (BandCompressor)
  *
  * Conventions follow the reference's only FFI (src/datasets/motion_simulator.py:30-95): every
  * function returns int (0 = OK, non-zero = error, text via l2h_last_error()), handles are opaque
@@ -871,6 +874,67 @@ int l2h_leveler(const float* y_dev, int64_t y_row_stride, int64_t y_ch_stride, f
                 const int32_t* offsets_dev, const int32_t* hops_dev, float* state_dev, int32_t n_rows, float target,
                 float gate, float relative, float alpha, int32_t settle_hops, float min_gain, float max_gain,
                 float rise_step, float fall_step, void* stream);
+
+/* A per-slot multiband compressor: fits each listener's output to their hearing with a gain per band and per ear, and
+ * compression per band that is the same for every channel, so the dynamics keep the interaural level differences.  It
+ * works on the separator's 16 kHz grid of 128-sample hops, on the mixer's sum (one row per slot).
+ *
+ * The bank (l2h_band_compressor_design) has K bands, 1 <= K <= 16, cut at K - 1 edges that rise strictly inside
+ * (0, 8000) Hz; each band is a linear-phase FIR of L taps, L odd in [33, 255], with a delay of D = (L - 1) / 2 samples.
+ * With LP_j = scipy.signal.firwin(L, edge_j, fs=16000) (a Hamming-windowed sinc scaled to a DC gain of 1), band 0 is
+ * LP_1, band j is LP_{j+1} - LP_j and band K - 1 is delta[n - D] - LP_{K-1}, all computed in float64, so the bands sum to
+ * delta[n - D].  Per hop of a slot, over its channels:
+ *     stage: the hop's 128 samples of each channel follow the slot's last L - 1 staged samples; a sample that is not
+ *       finite, or whose magnitude is 2^32 or more, enters as 0, and the hop is then not measured;
+ *     filter: band[c][b][k] = sum_j h_b[j] x_c[k - j];
+ *     measure: P_b = the mean square of band b over the hop's samples, averaged over the channels; the detector
+ *       S_b <- S_b + a (P_b - S_b), a = attack if P_b > S_b, else release; L_b = 10 log10 S_b dBFS (a full-scale sine
+ *       reads -3.01);
+ *     gain: R_b = slope_b max(0, L_b - knee_b) dB, shared by the channels; channel c's band b ends the hop at
+ *       g_cb = clamp(gain_cb - R_b, -40, 40) dB;
+ *     apply: sample k = 1 .. 128 is sum_b 10^(g_k / 20) band[c][b][k], summed in band order, with g_k = g_prev + (g_cb -
+ *       g_prev) k / 128 from the gain at the previous hop's end; a g_k of 0 dB is exactly 1.0f;
+ *     bypass: when every g of the slot is exactly 0 dB at the hop's start and end, the output is the staged input delayed
+ *       by D samples, bit for bit.
+ * A hop's result depends only on the state at its start and its samples, so cutting hops into other calls changes no bit.
+ *
+ * The state is [n_slots][channels][row_floats] fp32 of DEVICE memory.  Per channel: the channel's K profile gains (dB),
+ * its K current gains (dB, at the last sample written), then K words of channel 0's only: S_b (mean square), then K more:
+ * knee_b (dBFS), then K more: slope_b = 1 - 1 / ratio_b, then the channel's last L - 1 staged samples.  All zeros is a
+ * fresh slot with a flat 0 dB profile and no compression, so a slot is reset by zeroing its rows and moved by copying
+ * them; a profile is set by writing its words, and takes effect from the next hop, across one hop's dB ramp.
+ *
+ * l2h_band_compressor_design: writes the bank, out [bands][taps] fp32 of HOST memory, from edges_hz [bands - 1] (HOST
+ * memory; may be NULL when bands = 1).  Uploads nothing.  Errors: 1 = null pointer, bands outside [1, 16], taps not odd
+ * in [33, 255], edges that do not rise strictly inside (0, 8000).
+ * l2h_band_compressor_layout: row_floats = 5 bands + taps - 1.  Errors: 1 = null pointer, channels <= 0, bands outside
+ * [1, 16], taps not odd in [33, 255]; 2 = the staging of a row (taps 4 ceil(bands / 4) + channels (taps + 127) +
+ * channels bands 130 words) exceeds the kernel's shared memory.
+ *
+ * l2h_band_compressor: call row i (one CTA each, over all its channels) compresses y[i][c][0 .. 128 h) into
+ * out[i][c][0 .. 128 h) with the state of slot slots[i]:
+ *   y_dev        [n][channels][128 * frames] fp32, strides in floats
+ *   out_dev      the same shape; its rows' later samples, and the rows that store nothing, are not written.  out may be y
+ *                itself (the same pointer and strides): each hop is staged before anything of it is written.  Any other
+ *                overlap is refused.
+ *   slots_dev    [n] int32 of DEVICE memory: an entry outside [0, n_slots) marks a row that stores nothing and advances
+ *                nothing.  A slot listed twice is a caller error the call does not detect.
+ *   hops_dev     [n] int32 of DEVICE memory, or NULL (frames hops): row i compresses h = hops[i] hops; h outside
+ *                [1, frames] stores nothing.
+ *   taps_dev     [bands][taps] fp32 of DEVICE memory: the bank, read when the kernel runs.
+ *   attack, release  the detector's coefficients per hop, 1 - exp(-0.008 / tau) for a time constant tau in seconds.
+ * All lists are read when the kernel runs, so a call captured in a CUDA graph with the FIFO, the rows call and the mixer
+ * serves any lists of the same n rewritten in place.  One launch; nothing is read back to the host.  Errors, returned
+ * before anything is enqueued: 1 = null pointers (hops_dev may be NULL), n, channels, frames or n_slots <= 0,
+ * n > n_slots, 128 frames above 2^31 - 1, attack or release outside (0, 1], bands outside [1, 16], taps not odd in
+ * [33, 255], channel or row strides under 128 frames, out overlapping y other than as y itself; 2 = the staging of a
+ * row exceeds the kernel's shared memory (as in the layout).  Asynchronous on `stream`. */
+int l2h_band_compressor_design(int32_t bands, const float* edges_hz, int32_t taps, float* out);
+int l2h_band_compressor_layout(int32_t channels, int32_t bands, int32_t taps, int32_t* row_floats);
+int l2h_band_compressor(const float* y_dev, int64_t y_row_stride, int64_t y_ch_stride, float* out_dev,
+                        int64_t out_row_stride, int64_t out_ch_stride, int32_t n, int32_t channels, int32_t frames,
+                        const int32_t* slots_dev, const int32_t* hops_dev, const float* taps_dev, int32_t bands,
+                        int32_t taps, float* state_dev, int32_t n_slots, float attack, float release, void* stream);
 
 #ifdef __cplusplus
 }

@@ -14,6 +14,7 @@ net), behind the reference's own Python call signatures.
     from lookoncetohear_b200 import TargetMixer      # each listener's voices and ambient mixture into one row, with fades
     from lookoncetohear_b200 import Limiter          # each listener's output kept under a ceiling, one gain for both ears
     from lookoncetohear_b200 import Leveler          # each voice brought to one loudness, one gain for both ears
+    from lookoncetohear_b200 import BandCompressor   # each listener's output fitted to their hearing, per band and ear
 
 Compute happens only in lib/liblookonce_b200.so (hand-written sm_90a CUDA, C ABI declared in
 include/lookonce_b200.h); importing this package never falls back to PyTorch math.
@@ -21,7 +22,8 @@ include/lookonce_b200.h); importing this package never falls back to PyTorch mat
 from .embed import EmbedTFGridNet, EnrollJob  # noqa: F401
 from .net import Net, SepState, TargetHistory  # noqa: F401
 from .render import resample  # noqa: F401
-from .stream import EnrollCapture, HopFifo, PacketResampler, Leveler, Limiter, StreamResampler, TargetMixer  # noqa: F401
+from .stream import BandCompressor, EnrollCapture, HopFifo, PacketResampler, Leveler, Limiter, StreamResampler, TargetMixer  # noqa: F401
 
 __all__ = ["Net", "SepState", "TargetHistory", "EmbedTFGridNet", "resample", "StreamResampler", "PacketResampler", "HopFifo",
-           "EnrollCapture", "EnrollJob", "TargetMixer", "Limiter", "Leveler"]
+           "EnrollCapture", "EnrollJob", "TargetMixer", "Limiter", "Leveler",
+           "BandCompressor"]

@@ -21,8 +21,9 @@
 // resample_packets_kernel), the hop FIFO that turns 16 kHz pieces into separator chunks (hop_fifo_kernel), the
 // enrollment capture (enroll_capture_kernel), the target mixer that sums a listener's separated voices and its ambient
 // mixture into one row (target_mix_kernel, target_mix_set_kernel), the look-ahead limiter that keeps each listener's
-// output under a ceiling with one gain for all channels (limiter_kernel), and the leveler that brings each voice to one
-// loudness with one gain for all channels (leveler_kernel).
+// output under a ceiling with one gain for all channels (limiter_kernel), the leveler that brings each voice to one
+// loudness with one gain for all channels (leveler_kernel), and the multiband compressor that fits each listener's output
+// to their hearing, per band and per ear, with its compression linked across the channels (band_compressor_kernel).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -33,6 +34,7 @@
 #include <numeric>
 #include <string>
 #include <utility>
+#include <vector>
 
 #include "../../include/lookonce_b200.h"
 #include "host_errors.h"
@@ -796,6 +798,153 @@ leveler_kernel(const float* y, int64_t y_row, int64_t y_ch, float* out, int64_t 
     }
 }
 
+// ---- the band compressor: per-band gain and compression per slot, the compression linked across channels --------------
+// A slot (a listener, on the mixer's 16 kHz sum) is split hop by hop into K bands by linear-phase FIRs of L taps (the
+// bank of l2h_band_compressor_design, [K][L], summing to a delay of D = (L - 1) / 2 samples).  Per hop: the band's linked
+// level P_b is its mean square over the hop's samples and the channels; the detector S_b moves toward it by `attack` when
+// P_b > S_b, else by `release`; the compression R_b = slope_b max(0, 10 log10 S_b - knee_b) dB is the same for every
+// channel, and channel c's band b takes g = clamp(gain_cb - R_b, -40, 40) dB at the hop's end.  Sample k = 1 .. 128 of
+// the hop is the sum in band order of each band's sample times 10^(g_k / 20), g_k interpolated in dB from the gain at the
+// previous hop's end (a g_k of 0 dB is exactly 1).  When every gain of the slot is 0 dB at the hop's start and end, the
+// output is the staged input delayed by D, bit for bit.  A sample that is not finite, or whose magnitude reaches 2^32,
+// is staged as 0, and its hop is not measured (the detector keeps its values), so the state stays finite.  A hop's result
+// depends only on the state at its start and its samples, so cutting hops into other calls changes no bit.
+// A slot's state per channel is [5 K + L - 1]: the channel's K profile gains (dB) and its K current gains (dB, at the last
+// sample written); then, channel 0's only, S_b, knee_b (dBFS) and slope_b = 1 - 1 / ratio; then the channel's last L - 1
+// staged samples.  All zeros is a fresh slot: flat 0 dB and no compression.
+constexpr int BC_THREADS = CHUNK_HOP;                   // one thread per sample of a hop
+constexpr int BC_MAX_BANDS = 16;
+constexpr int BC_MIN_TAPS = 33, BC_MAX_TAPS = 255;
+constexpr float BC_RANGE = 40.f;                        // the gains' clamp, dB
+static_assert(BC_MAX_BANDS <= BC_THREADS, "one thread per band updates the detectors");
+
+// One CTA = one call row over all C channels (the compression is linked).  Row i compresses the first 128 h samples of
+// y[i] into out[i], h = hops[i] (T without hops), with the state of slot slots[i].  Each hop is staged before anything of
+// it is written, so out may be y itself.  KP = bc_padded(K) accumulators per thread.
+template <int KP>
+__global__ void __launch_bounds__(BC_THREADS)
+band_compressor_kernel(const float* y, int64_t y_row, int64_t y_ch, float* out, int64_t o_row, int64_t o_ch, int C, int T,
+                       const int32_t* __restrict__ slots, const int32_t* __restrict__ hops, const float* __restrict__ bank,
+                       int K, int L, float* __restrict__ state, int n_slots, float attack, float release) {
+    extern __shared__ float4 sm4[];
+    __shared__ float part[BC_THREADS / 32][KP];
+    __shared__ float S[KP];
+    const int tid = threadIdx.x, H = L - 1, W = H + CHUNK_HOP, D = H / 2, CK = C * K;
+    const int64_t rf = 5 * K + H;
+    const SlotRow sr = slot_row(1, slots, n_slots, state, C * rf);
+    const int h = hops ? hops[sr.row] : T;
+    if (!sr.live || h <= 0 || h > T) return;                            // a row that stores nothing
+    float* st = sr.st;                                                  // channel c's row at st + c rf
+    float* taps = reinterpret_cast<float*>(sm4);                        // [L][KP]: tap j of band b, zero past K
+    float* win = taps + L * KP;                                         // [C][W]: the last H staged samples, then the hop
+    float* band = win + C * W;                                          // [C][K][128]: the hop's band signals
+    float* g0 = band + CK * CHUNK_HOP;                                  // [C][K]: the gains (dB) at the hop's start
+    float* g1 = g0 + CK;                                                // [C][K]: and at its end
+    for (int i = tid; i < L * KP; i += BC_THREADS) {
+        const int j = i / KP, b = i - j * KP;
+        taps[i] = b < K ? bank[b * L + j] : 0.f;
+    }
+    for (int c = 0; c < C; ++c)
+        for (int i = tid; i < H; i += BC_THREADS) win[c * W + i] = st[c * rf + 5 * K + i];
+    for (int i = tid; i < CK; i += BC_THREADS) {
+        const int c = i / K;
+        g0[i] = st[c * rf + K + (i - c * K)];
+    }
+    if (tid < K) S[tid] = st[2 * K + tid];
+    for (int t = 0; t < h; ++t) {
+        const int64_t s = (int64_t)t * CHUNK_HOP + tid;
+        bool bad = false;
+        for (int c = 0; c < C; ++c) {
+            const float v = row_ch(y, y_row, y_ch, sr.row, c)[s];
+            const bool ok = fabsf(v) < LV_BIG;
+            bad = bad || !ok;
+            win[c * W + H + tid] = ok ? v : 0.f;
+        }
+        const bool measured = !__syncthreads_or(bad);                   // and the staged hop is visible to the block
+        float sq[KP];
+#pragma unroll
+        for (int b = 0; b < KP; ++b) sq[b] = 0.f;
+        for (int c = 0; c < C; ++c) {
+            float acc[KP];
+#pragma unroll
+            for (int b = 0; b < KP; ++b) acc[b] = 0.f;
+            const float* xk = win + c * W + H + tid;                   // xk[-j] is the sample j before this one
+#pragma unroll 4
+            for (int j = 0; j < L; ++j) {
+                const float x = xk[-j];
+                const float4* tp = reinterpret_cast<const float4*>(taps + j * KP);
+#pragma unroll
+                for (int q = 0; q < KP / 4; ++q) {
+                    const float4 w = tp[q];
+                    acc[4 * q] = fmaf(w.x, x, acc[4 * q]);
+                    acc[4 * q + 1] = fmaf(w.y, x, acc[4 * q + 1]);
+                    acc[4 * q + 2] = fmaf(w.z, x, acc[4 * q + 2]);
+                    acc[4 * q + 3] = fmaf(w.w, x, acc[4 * q + 3]);
+                }
+            }
+#pragma unroll
+            for (int b = 0; b < KP; ++b) {
+                if (b < K) band[(c * K + b) * CHUNK_HOP + tid] = acc[b];
+                sq[b] = fmaf(acc[b], acc[b], sq[b]);
+            }
+        }
+        if (measured) {                                                 // the same order of sums every call
+#pragma unroll
+            for (int b = 0; b < KP; ++b) {
+                float v = sq[b];
+                for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
+                if ((tid & 31) == 0) part[tid >> 5][b] = v;
+            }
+            __syncthreads();
+            if (tid < K) {
+                float P = part[0][tid];
+                for (int w = 1; w < BC_THREADS / 32; ++w) P += part[w][tid];
+                P *= 1.f / (float)(CHUNK_HOP * C);
+                const float old = S[tid];
+                S[tid] = fmaf(P > old ? attack : release, P - old, old);
+            }
+        }
+        __syncthreads();                                                // the detectors, and every band sample
+        bool live = false;
+        for (int i = tid; i < CK; i += BC_THREADS) {
+            const int c = i / K, b = i - c * K;
+            const float R = st[4 * K + b] * fmaxf(0.f, 10.f * log10f(S[b]) - st[3 * K + b]);
+            g1[i] = fminf(fmaxf(st[c * rf + b] - R, -BC_RANGE), BC_RANGE);
+            live = live || g0[i] != 0.f || g1[i] != 0.f;
+        }
+        live = __syncthreads_or(live);                                  // and every gain is visible to the block
+        const float f = (float)(tid + 1) * (1.f / CHUNK_HOP);
+        for (int c = 0; c < C; ++c) {
+            float o = win[c * W + H + tid - D];                         // the staged input delayed by D
+            if (live) {
+                o = 0.f;
+                for (int b = 0; b < K; ++b) {
+                    const float a = g0[c * K + b], gk = fmaf(g1[c * K + b] - a, f, a);
+                    const float lin = gk == 0.f ? 1.f : exp2f(gk * LV_LOG2_10_20);
+                    o = fmaf(lin, band[(c * K + b) * CHUNK_HOP + tid], o);
+                }
+            }
+            row_ch(out, o_row, o_ch, sr.row, c)[s] = o;
+        }
+        for (int c = 0; c < C; ++c) {                                   // the last H staged samples become the history
+            const float a = tid < H ? win[c * W + CHUNK_HOP + tid] : 0.f;
+            const float b = tid + BC_THREADS < H ? win[c * W + CHUNK_HOP + BC_THREADS + tid] : 0.f;
+            __syncthreads();                                            // every thread has read the channel's window
+            if (tid < H) win[c * W + tid] = a;
+            if (tid + BC_THREADS < H) win[c * W + BC_THREADS + tid] = b;
+        }
+        for (int i = tid; i < CK; i += BC_THREADS) g0[i] = g1[i];
+    }
+    __syncthreads();                                                    // the history and the gains
+    for (int c = 0; c < C; ++c)
+        for (int i = tid; i < H; i += BC_THREADS) st[c * rf + 5 * K + i] = win[c * W + i];
+    for (int i = tid; i < CK; i += BC_THREADS) {
+        const int c = i / K;
+        st[c * rf + K + (i - c * K)] = g0[i];
+    }
+    if (tid < K) st[2 * K + tid] = S[tid];
+}
+
 // ---- the host side of the per-slot calls ------------------------------------------------------------------------------
 // The checks every per-slot call makes first, in this order: its pointers, its sizes (`sizes` names them), n <= n_slots,
 // and a grid of n * channels CTAs.  0, or 1 with its message.
@@ -1210,5 +1359,104 @@ extern "C" int l2h_leveler(const float* y_dev, int64_t y_row_stride, int64_t y_c
     leveler_kernel<<<(unsigned)R, LV_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
         y_dev, y_row_stride, y_ch_stride, out_dev, out_row_stride, out_ch_stride, n, channels, frames, records_dev,
         offsets_dev, hops_dev, state_dev, n_rows, p);
+    return launched(who);
+}
+
+namespace l2h {
+// the bank's shape and a call's staging (taps, windows, band signals and gains): 0, or an error code (1 invalid, 2 the
+// staging exceeds shared memory) with its message
+static int bc_staging(const std::string& who, int32_t channels, int32_t bands, int32_t taps, int* kp, int* smem) {
+    if (channels <= 0) return fail(1, who + ": channels must be positive");
+    if (bands < 1 || bands > BC_MAX_BANDS)
+        return fail(1, who + ": bands " + std::to_string(bands) + " lies outside [1, " + std::to_string(BC_MAX_BANDS) + "]");
+    if (taps < BC_MIN_TAPS || taps > BC_MAX_TAPS || taps % 2 == 0)
+        return fail(1, who + ": taps " + std::to_string(taps) + " is not odd in [" + std::to_string(BC_MIN_TAPS) + ", " +
+                           std::to_string(BC_MAX_TAPS) + "]");
+    *kp = (bands + 3) / 4 * 4;                          // the kernel reads each tap row as float4
+    const int64_t floats = (int64_t)taps * *kp + (int64_t)channels * (taps - 1 + CHUNK_HOP) +
+                           (int64_t)channels * bands * (CHUNK_HOP + 2);
+    if (floats * (int64_t)sizeof(float) > RS_SMEM_BYTES)
+        return fail(2, who + ": " + std::to_string(channels) + " channels of " + std::to_string(bands) + " bands of " +
+                           std::to_string(taps) + " taps are too large: " + std::to_string(floats) +
+                           " staged words per row exceed shared memory (" + std::to_string(RS_SMEM_BYTES / sizeof(float)) +
+                           ")");
+    *smem = (int)(floats * sizeof(float));
+    return 0;
+}
+}  // namespace l2h
+
+extern "C" int l2h_band_compressor_design(int32_t bands, const float* edges_hz, int32_t taps, float* out) {
+    using namespace l2h;
+    const std::string who = "l2h_band_compressor_design";
+    if (!out || (bands > 1 && !edges_hz)) return fail(1, who + ": null pointer");
+    int kp, smem;
+    if (int rc = bc_staging(who, 1, bands, taps, &kp, &smem)) return rc;   // one channel always fits
+    for (int j = 0; j + 1 < bands; ++j) {
+        const float e = edges_hz[j];
+        if (!(e > 0.f && e < 8000.f) || (j > 0 && !(e > edges_hz[j - 1])))
+            return fail(1, who + ": the edges must rise strictly inside (0, 8000) Hz, got edge " + std::to_string(j) + " = " +
+                               std::to_string(e));
+    }
+    // LP_j: scipy.signal.firwin(taps, edge_j, fs=16000), a Hamming-windowed sinc scaled to a DC gain of 1; band 0 is LP_1,
+    // band j LP_{j+1} - LP_j, the last band the delay D minus LP_{K-1}, all in float64
+    const int L = taps, D = (L - 1) / 2;
+    std::vector<double> prev(L, 0.0), lp(L);
+    for (int b = 0; b < bands; ++b) {
+        if (b + 1 < bands) {
+            const double cut = edges_hz[b] / 8000.0;
+            double sum = 0.0;
+            for (int i = 0; i < L; ++i) {
+                const double m = i - D, u = M_PI * cut * m;
+                const double win = 0.54 - 0.46 * std::cos(2.0 * M_PI * i / (L - 1));
+                lp[i] = cut * (m == 0 ? 1.0 : std::sin(u) / u) * win;
+                sum += lp[i];
+            }
+            for (double& v : lp) v /= sum;
+        } else {
+            for (int i = 0; i < L; ++i) lp[i] = i == D ? 1.0 : 0.0;
+        }
+        for (int i = 0; i < L; ++i) out[(int64_t)b * L + i] = (float)(lp[i] - prev[i]);
+        prev.swap(lp);
+    }
+    return 0;
+}
+
+extern "C" int l2h_band_compressor_layout(int32_t channels, int32_t bands, int32_t taps, int32_t* row_floats) {
+    using namespace l2h;
+    if (!row_floats) return fail(1, "l2h_band_compressor_layout: null pointer");
+    int kp, smem;
+    if (int rc = bc_staging("l2h_band_compressor_layout", channels, bands, taps, &kp, &smem)) return rc;
+    *row_floats = 5 * bands + taps - 1;
+    return 0;
+}
+
+extern "C" int l2h_band_compressor(const float* y_dev, int64_t y_row_stride, int64_t y_ch_stride, float* out_dev,
+                                   int64_t out_row_stride, int64_t out_ch_stride, int32_t n, int32_t channels, int32_t frames,
+                                   const int32_t* slots_dev, const int32_t* hops_dev, const float* taps_dev, int32_t bands,
+                                   int32_t taps, float* state_dev, int32_t n_slots, float attack, float release,
+                                   void* stream) {
+    using namespace l2h;
+    const std::string who = "l2h_band_compressor";
+    if (int rc = slot_call(who, {y_dev, out_dev, slots_dev, taps_dev, state_dev}, "n, channels, frames and n_slots",
+                           {n, channels, frames, n_slots}, n, channels, n_slots))
+        return rc;
+    if ((int64_t)frames * CHUNK_HOP > INT32_MAX) return fail(1, who + ": frames is too large");
+    if (!(attack > 0.f && attack <= 1.f) || !(release > 0.f && release <= 1.f))
+        return fail(1, who + ": attack " + std::to_string(attack) + " and release " + std::to_string(release) +
+                           " must lie in (0, 1]");
+    int kp, smem;
+    if (int rc = bc_staging(who, channels, bands, taps, &kp, &smem)) return rc;
+    const int64_t len = (int64_t)frames * CHUNK_HOP;
+    const Rows y{"y", y_row_stride, y_ch_stride, len}, out{"out", out_row_stride, out_ch_stride, len};
+    if (int rc = disjoint(who, channels, {y, out})) return rc;
+    const bool in_place = out_dev == y_dev && out_row_stride == y_row_stride && out_ch_stride == y_ch_stride;
+    const auto a = span(y_dev, n, channels, y), b = span(out_dev, n, channels, out);
+    if (!in_place && a.first < b.second && b.first < a.second)
+        return fail(1, who + ": out must be y itself (same pointer and strides) or not overlap it");
+    const auto kernel = kp == 4 ? band_compressor_kernel<4> : kp == 8 ? band_compressor_kernel<8>
+                      : kp == 12 ? band_compressor_kernel<12> : band_compressor_kernel<16>;
+    kernel<<<(unsigned)n, BC_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
+        y_dev, y_row_stride, y_ch_stride, out_dev, out_row_stride, out_ch_stride, channels, frames, slots_dev, hops_dev,
+        taps_dev, bands, taps, state_dev, n_slots, attack, release);
     return launched(who);
 }

@@ -5,8 +5,9 @@ per-slot FIFO that turns 16 kHz pieces into separator chunks and hop counts (`Ho
 per-slot capture that keeps each listener's recent input for enrollment (`EnrollCapture`, `l2h_enroll_capture`),
 the per-listener mixer that sums the separated voices and the ambient mixture into one row with fades (`TargetMixer`,
 `l2h_target_mix`), the per-listener look-ahead limiter that keeps the output under a ceiling with one gain for both
-ears (`Limiter`, `l2h_limiter`), and the per-row leveler that brings each voice to one loudness with one gain for both
-ears (`Leveler`, `l2h_leveler`).
+ears (`Limiter`, `l2h_limiter`), the per-row leveler that brings each voice to one loudness with one gain for both
+ears (`Leveler`, `l2h_leveler`), and the per-listener multiband compressor that fits the output to each ear's hearing
+(`BandCompressor`, `l2h_band_compressor`).
 
 Each stage keeps a float32 state [slots, channels, row floats] on a CUDA device.  All zeros is a fresh slot, so a
 listener is reset by zeroing its rows (`reset`) and moved by copying them.  No CPU fallback."""
@@ -690,3 +691,138 @@ class Leveler(_SlotStage):
     def gain(self):
         """[rows] float32 CUDA view of the state: each row's gain in dB at the last sample it wrote"""
         return self.state[:, 0, 2]
+
+
+class BandCompressor(_SlotStage):
+    """A per-slot multiband compressor on the device (l2h_band_compressor): each listener's output fitted to their hearing,
+    with a gain per band and per ear and compression per band ("wide dynamic range compression") that is the same for
+    both ears, so the dynamics keep the interaural level differences the binaural output carries.  Hearing loss depends on
+    frequency and often differs between the ears; a profile sets both per listener (`set_profile`).
+
+    It runs on the mixer's 16 kHz sum, one row per slot: cmp(mix, slots, hops=hops, out=mix).  The separated audio holds
+    nothing above 8 kHz, so 16 kHz loses nothing and is the cheapest place for it; the limiter stays after the
+    up-resampler.  The bank (`design`) splits the band at `edges` Hz into linear-phase FIR bands of `taps` taps that sum
+    to a delay of `delay` = (taps - 1) / 2 samples: 64 samples (4 ms) at the defaults, five octave-wide bands.  Per hop
+    of 128 samples each band's level, averaged over the channels, drives a detector that follows it with time constants
+    `attack` (level rising) and `release` (falling) in seconds; a band's compression is slope * max(0, level - knee) dB
+    with slope = 1 - 1 / ratio, and ear c's band b takes clamp(gain_cb - compression_b, -40, 40) dB at the hop's end,
+    interpolated in dB across the hop.  While every gain of a slot is 0 dB, as in a fresh slot, the output is the input
+    delayed by `delay` samples, bit for bit.  A hop's result depends only on the slot's state and its samples, so cutting
+    hops into other ticks changes no bit.  A non-finite sample, or one of magnitude 2^32 or more, enters as 0, and its hop
+    is not measured.
+
+    `taps` is the bank on the device, [bands, taps] float32.  `state` [slots, channels, 5 bands + taps - 1] is a float32
+    tensor on `device`: all zeros is a fresh slot with a flat 0 dB profile and no compression, so a listener is reset by
+    zeroing its rows (`reset`) and moved by copying them."""
+
+    RATE = 16000
+    RANGE = 40.0                                # the gains' clamp, dB
+    HOP_S = 128 / 16000                         # seconds per hop of the 16 kHz grid
+
+    def __init__(self, slots, channels, edges=(500, 1000, 2000, 4000), taps=129, attack=0.005, release=0.08,
+                 device=None):
+        super().__init__(slots, channels)
+        bank = self.design(edges, taps)
+        self.edges = tuple(float(e) for e in torch.as_tensor(edges, dtype=torch.float32).reshape(-1).tolist())
+        self.bands, self.n_taps = bank.shape
+        self.delay = (self.n_taps - 1) // 2
+        coef = {}
+        for what, tau in (("attack", attack), ("release", release)):
+            if (isinstance(tau, bool) or not isinstance(tau, numbers.Real) or not math.isfinite(tau) or tau <= 0
+                    or float(torch.tensor(-math.expm1(-self.HOP_S / tau), dtype=torch.float32)) <= 0):
+                raise ValueError(f"{what} must be a positive number of seconds, got {tau!r}")
+            coef[what] = -math.expm1(-self.HOP_S / tau)
+        self.attack, self.release = float(attack), float(release)
+        self.attack_coef, self.release_coef = coef["attack"], coef["release"]
+        self._allocate(*_layout(_cabi.lib().l2h_band_compressor_layout, self.channels, self.bands, self.n_taps), device)
+        self.taps = bank.to(self.state.device)
+
+    @staticmethod
+    def design(edges=(500, 1000, 2000, 4000), taps=129):
+        """The bank of K = len(edges) + 1 bands cut at `edges` Hz (rising strictly inside (0, 8000)), each a linear-phase
+        FIR of `taps` taps (odd, 33 to 255), as a [K, taps] float32 CPU tensor (l2h_band_compressor_design): with LP_j =
+        scipy.signal.firwin(taps, edge_j, fs=16000), band 0 is LP_1, band j is LP_{j+1} - LP_j and the last band is a
+        delay of (taps - 1) / 2 samples minus LP_{K-1}, computed in float64, so the bands sum to that delay."""
+        try:
+            e = torch.as_tensor(edges, dtype=torch.float32).reshape(-1).contiguous()
+        except (TypeError, ValueError, RuntimeError):
+            raise ValueError(f"edges must be a sequence of numbers of Hz, got {edges!r}") from None
+        if isinstance(edges, (str, bytes)) or e.numel() >= 16:
+            raise ValueError(f"edges must be at most 15 numbers of Hz (at most 16 bands), got {edges!r}")
+        L = _whole(taps, "taps")
+        out = torch.empty(e.numel() + 1, L, dtype=torch.float32)
+        _check(_cabi.lib().l2h_band_compressor_design(e.numel() + 1, e.data_ptr() if e.numel() else None, L,
+                                                      out.data_ptr()))
+        return out
+
+    def __call__(self, y, slots, hops=None, out=None):
+        """y [n, channels, 128 * T] CUDA tensor, the mixer's sum: row i is compressed with the state of slot slots[i].
+        Returns out [n, channels, 128 * T] float32 (`out`, if given, written in place; out=y compresses y in place): row
+        i receives its first 128 h samples, h = hops[i] (T without hops).  Its later samples, and rows that store nothing,
+        are left unwritten.
+
+        Lists follow Leveler on the mixer's sum: host lists are checked and uploaded (`slots` n distinct ints in
+        [0, slots), `hops` n ints in [0, T]); contiguous CUDA int32 tensors are used in place and read when the kernel
+        runs, where a slot outside [0, slots) or a hop count outside [1, T] marks a row that stores nothing and advances
+        nothing.  So a call captured in the tick's CUDA graph serves any lists rewritten in place."""
+        y = self._rows_in(y, self.HOP)
+        dev = self.state.device
+        n, C, L = y.shape
+        T = L // self.HOP
+        slots = device_list(slots, dev, n, self.n_slots, True, "slot")
+        if hops is not None:
+            hops = device_list(hops, dev, n, T + 1, False, "hop")
+        out = self._rows_out(out, (n, C, L))
+        with torch.cuda.device(dev):
+            _check(_cabi.lib().l2h_band_compressor(
+                y.data_ptr(), y.stride(0), y.stride(1), out.data_ptr(), out.stride(0), out.stride(1), n, C, T,
+                slots.data_ptr(), None if hops is None else hops.data_ptr(), self.taps.data_ptr(), self.bands,
+                self.n_taps, self.state.data_ptr(), self.n_slots, self.attack_coef, self.release_coef, self._stream()))
+        return out
+
+    def set_profile(self, slots, gains, knees=0.0, ratios=1.0):
+        """Fit the listed slots: `gains` in dB per band, [K] for every slot and both ears, [n, K] per slot for both ears,
+        or [n, channels, K] per slot and ear, each in [-40, 40]; `knees` in dBFS and `ratios` >= 1 per band, each a
+        number, [K] or [n, K].  A band compresses by (1 - 1 / ratio) dB per dB its level lies above its knee.  Enqueued on
+        the current stream; it takes effect from the next hop, across one hop's dB ramp, and `reset` returns a slot to
+        the flat profile."""
+        dev, K, C = self.state.device, self.bands, self.channels
+        idx = torch.as_tensor(slots).cpu().reshape(-1)
+        n = idx.numel()
+        if n < 1:
+            raise ValueError("set_profile needs at least one slot")
+        idx = device_list(idx, dev, n, self.n_slots, True, "slot")
+        g = self._table(gains, "gains", n, [(K,), (n, K), (n, C, K)], lambda v: -self.RANGE <= v <= self.RANGE)
+        kn = self._table(knees, "knees", n, [(), (K,), (n, K)], math.isfinite)
+        ra = self._table(ratios, "ratios", n, [(), (K,), (n, K)], lambda v: v >= 1)
+        g = (g.reshape(1, 1, K) if g.dim() == 1 else g.reshape(n, -1, K)).expand(n, C, K)
+        kn, ra = ((t.expand(K) if t.dim() == 0 else t).reshape(-1, K).expand(n, K) for t in (kn, ra))
+        rows = idx.long()
+        self.state[rows, :, :K] = g.float().to(dev)
+        self.state[rows, 0, 3 * K:4 * K] = kn.float().to(dev)
+        self.state[rows, 0, 4 * K:5 * K] = (1.0 - 1.0 / ra).float().to(dev)
+
+    @staticmethod
+    def _table(v, what, n, shapes, ok):
+        """v as a float64 CPU tensor of one of `shapes` whose every entry passes `ok`, or ValueError"""
+        try:
+            t = torch.as_tensor(v.detach().cpu() if isinstance(v, torch.Tensor) else v, dtype=torch.float64)
+        except (TypeError, ValueError, RuntimeError):
+            t = None
+        if t is None or tuple(t.shape) not in shapes or isinstance(v, bool):
+            raise ValueError(f"{what} must be numbers of shape {' or '.join(str(list(s)) for s in shapes)}, got {v!r}")
+        if not all(ok(x) for x in t.reshape(-1).tolist()):
+            raise ValueError(f"{what} holds a value out of range, got {t.tolist()}")
+        return t
+
+    @property
+    def level(self):
+        """[slots, bands] float32 CUDA tensor: each band's detector level in dBFS (a full-scale sine reads -3.01), -inf
+        before the slot's first measured hop; computed on the device, never synchronising"""
+        K = self.bands
+        return 10.0 * torch.log10(self.state[:, 0, 2 * K:3 * K])
+
+    @property
+    def gain(self):
+        """[slots, channels, bands] float32 CUDA view of the state: each band's gain in dB at the last sample written"""
+        return self.state[:, :, self.bands:2 * self.bands]
