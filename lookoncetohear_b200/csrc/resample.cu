@@ -16,8 +16,11 @@
 // RS_MAX_RUNS runs of consecutive rows with the same rate (no per-row table in device memory); a CTA finds its row's
 // run by binary search.
 //
-// The file also holds the per-slot stages of the serving front end, which share one scaffold (slot_row, slot_call):
-// the streaming resamplers (pushes of whole periods, resample_stream_kernel; pushes of any length,
+// The file also holds the per-slot stages of the serving front end, which share one scaffold: on the device slot_row
+// and row_ch find a call row's state and operands, row_hops and row_pushed its hop or sample count, int_word, clamp_word
+// and add_word read and count state words, and hop_gain turns a hop's dB gains into sample gains; on the host slot_call,
+// disjoint, overlap, hop_lens and staging check a call before it is launched, and launched after.  The stages are the
+// streaming resamplers (pushes of whole periods, resample_stream_kernel; pushes of any length,
 // resample_packets_kernel), the hop FIFO that turns 16 kHz pieces into separator chunks (hop_fifo_kernel), the
 // enrollment capture (enroll_capture_kernel), the target mixer that sums a listener's separated voices and its ambient
 // mixture into one row (target_mix_kernel, target_mix_set_kernel), the look-ahead limiter that keeps each listener's
@@ -33,7 +36,6 @@
 #include <initializer_list>
 #include <numeric>
 #include <string>
-#include <utility>
 #include <vector>
 
 #include "../../include/lookonce_b200.h"
@@ -138,7 +140,9 @@ resample_kernel(const float* __restrict__ x, int64_t x_stride, int n_in, float* 
 
 // ---- the per-slot scaffold -------------------------------------------------------------------------------------------
 // A per-slot stage keeps a state [n_slots][C][row_floats], all zeros for a fresh slot, and runs one CTA per (call row,
-// channel).  The slot list is read on the device, and a row whose slot lies outside the state stores nothing.
+// channel), or per call row where its channels share a gain.  The slot, hop and count lists are read on the device: a
+// row whose slot lies outside the state, whose hop count lies outside [1, T] or whose push lies outside [0, max_in]
+// stores nothing.
 struct SlotRow {
     int row, ch;
     bool live;   // the row's slot lies inside the state
@@ -156,8 +160,41 @@ L2H_DEVINL T* row_ch(T* p, int64_t row_stride, int64_t ch_stride, int row, int c
     return p + (int64_t)row * row_stride + (int64_t)ch * ch_stride;
 }
 
+// the hops row `row` takes, hops[row] (T without a hop list): 0 for a count outside [1, T], a row that stores nothing
+L2H_DEVINL int row_hops(const int32_t* hops, int row, int T) {
+    const int h = hops ? hops[row] : T;
+    return h >= 1 && h <= T ? h : 0;
+}
+
+// the samples row `row` pushes, counts[row] * unit: 0 for a push outside [0, max_in], a push of nothing
+L2H_DEVINL int row_pushed(const int32_t* counts, int row, int unit, int max_in) {
+    const int64_t pushed = (int64_t)counts[row] * unit;
+    return pushed >= 0 && pushed <= max_in ? (int)pushed : 0;
+}
+
 // a count word of a state row, stored as a float, clamped into [0, hi]
 L2H_DEVINL int clamp_word(float v, int hi) { return v >= (float)hi ? hi : (v > 0.f ? (int)v : 0); }
+
+// an int32 word of a state row, clamped into [0, hi]
+L2H_DEVINL int int_word(float w, int hi) { return min(max(__float_as_int(w), 0), hi); }
+
+// the int32 counter word w (a negative one counts as 0) plus add >= 0, saturating at INT32_MAX
+L2H_DEVINL float add_word(float w, int add) {
+    const int before = max(__float_as_int(w), 0);
+    return __int_as_float(add > INT32_MAX - before ? INT32_MAX : before + add);
+}
+
+// The leveler's and the compressor's gains are in dB, interpolated across each hop.  A sample of magnitude HG_BIG (2^32)
+// or more is not measured: its squares could overflow.
+constexpr float HG_BIG = 4294967296.f;
+constexpr float HG_LOG2_10_20 = 0.16609640474436813f;   // log2(10) / 20: dB to an octave of amplitude
+
+// the linear gain of the calling thread's sample k = threadIdx.x + 1 of a hop (one thread per sample), interpolated in dB
+// from g0 at the hop's start to g1 at its end; a gain of 0 dB is exactly 1
+L2H_DEVINL float hop_gain(float g0, float g1) {
+    const float gk = fmaf(g1 - g0, (float)(threadIdx.x + 1) * (1.f / CHUNK_HOP), g0);
+    return gk == 0.f ? 1.f : exp2f(gk * HG_LOG2_10_20);
+}
 
 // Sample jd + D of the delayed output z' below: zero before z's start (!started), else rs_output at input c = floor(jd o /
 // q), which sits at win[origin + c].
@@ -191,8 +228,8 @@ resample_stream_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch,
     extern __shared__ float sm[];
     const int tid = threadIdx.x, H = s.hist, keep = s.keep, D = s.delay;
     const SlotRow r = slot_row(C, slots, n_slots, state, H + keep);
-    const int h = hops ? hops[r.row] : T;
-    if (!r.live || h <= 0 || h > T) return;                            // a row that stores nothing
+    const int h = row_hops(hops, r.row, T);
+    if (h == 0 || !r.live) return;                                      // a row that stores nothing
     const int n_win = H + h * s.block, n_new = h * s.out_block;
     float* st = r.st;
     const float* xr = row_ch(x, x_row, x_ch, r.row, r.ch);
@@ -213,6 +250,16 @@ resample_stream_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch,
 
 static std::string rs_rates(int32_t orig, int32_t new_freq) { return std::to_string(orig) + " -> " + std::to_string(new_freq) + " Hz"; }
 
+// the shared-memory bytes of a per-slot call that stages `floats` per row, into *smem unless it is null (a layout
+// query): 0, or 2 when they exceed shared memory, with the message "who: what: <floats> staged <unit> exceed ...""
+static int staging(const std::string& who, int64_t floats, const std::string& what, const char* unit, int* smem) {
+    if (floats * (int64_t)sizeof(float) > RS_SMEM_BYTES)
+        return fail(2, who + ": " + what + ": " + std::to_string(floats) + " staged " + unit + " exceed shared memory (" +
+                           std::to_string(RS_SMEM_BYTES / sizeof(float)) + ")");
+    if (smem) *smem = (int)(floats * sizeof(float));
+    return 0;
+}
+
 // the filter of a stream of orig -> new_freq Hz and its delay D = floor(w q / o): 0, or 1 with its message
 static int rs_streaming(const std::string& who, int32_t orig, int32_t new_freq, RsRate* g, int64_t* delay) {
     if (orig <= 0 || new_freq <= 0) return fail(1, who + ": rates must be positive, got " + rs_rates(orig, new_freq));
@@ -223,9 +270,10 @@ static int rs_streaming(const std::string& who, int32_t orig, int32_t new_freq, 
 }
 
 // the stream of orig -> new_freq Hz in pushes of `block` samples with `keep` repeated outputs, for calls of up to `blocks`
-// pushes per row: 0, or an error code (1 invalid, 2 the window of a row exceeds shared memory) with its message
+// pushes per row, and the bytes of a row's window: 0, or an error code (1 invalid, 2 the window exceeds shared memory)
+// with its message
 static int rs_stream(const std::string& who, int32_t orig, int32_t new_freq, int32_t block, int32_t keep, int32_t blocks,
-                     RsStream* s) {
+                     RsStream* s, int* smem) {
     int64_t delay;
     if (int rc = rs_streaming(who, orig, new_freq, &s->g, &delay)) return rc;
     const RsRate& g = s->g;
@@ -237,11 +285,9 @@ static int rs_stream(const std::string& who, int32_t orig, int32_t new_freq, int
     const int64_t out_block = (int64_t)block / g.o * g.q;
     const int64_t hist = (delay * g.o + g.q - 1) / g.q + g.w;
     const int64_t floats = hist + (int64_t)blocks * block + keep + (int64_t)blocks * out_block;
-    if (floats * (int64_t)sizeof(float) > RS_SMEM_BYTES)
-        return fail(2, who + ": " + rates + " in blocks of " + std::to_string(block) + " with keep " +
-                           std::to_string(keep) + " and " + std::to_string(blocks) + " blocks per row is too large: " +
-                           std::to_string(floats) + " staged samples per row exceed shared memory (" +
-                           std::to_string(RS_SMEM_BYTES / sizeof(float)) + ")");
+    const std::string what = rates + " in blocks of " + std::to_string(block) + " with keep " + std::to_string(keep) +
+                             " and " + std::to_string(blocks) + " blocks per row is too large";
+    if (int rc = staging(who, floats, what, "samples per row", smem)) return rc;
     s->block = block;
     s->out_block = (int32_t)out_block;
     s->delay = (int32_t)delay;
@@ -275,8 +321,7 @@ resample_packets_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch
     extern __shared__ float win[];                   // [H + n]: the history, then the row's new samples
     const int tid = threadIdx.x, H = s.hist, D = s.delay;
     const SlotRow r = slot_row(C, slots, n_slots, state, RP_HEAD + H);
-    const int64_t pushed = (int64_t)counts[r.row] * s.unit;
-    const int n = pushed >= 0 && pushed <= s.max_in ? (int)pushed : 0;
+    const int n = row_pushed(counts, r.row, s.unit, s.max_in);
     if (!r.live || n == 0) {                                            // a row that stores nothing
         if (r.ch == 0 && tid == 0) out_counts[r.row] = 0;
         return;
@@ -300,21 +345,19 @@ resample_packets_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch
     }
 }
 
-// the packet stream of orig -> new_freq Hz for pushes of up to max_in samples: 0, or an error code (1 invalid, 2 the
-// window of a row exceeds shared memory) with its message
+// the packet stream of orig -> new_freq Hz for pushes of up to max_in samples, and the bytes of a row's window: 0, or an
+// error code (1 invalid, 2 the window exceeds shared memory) with its message
 static int rs_packets(const std::string& who, int32_t orig, int32_t new_freq, int32_t max_in, RsPackets* s,
-                      int32_t* max_out) {
+                      int32_t* max_out, int* smem) {
     int64_t delay;
     if (int rc = rs_streaming(who, orig, new_freq, &s->g, &delay)) return rc;
     if (max_in <= 0) return fail(1, who + ": max_in " + std::to_string(max_in) + " is not positive");
     const RsRate& g = s->g;
     const int64_t hist = ((delay + 1) * g.o + g.q - 1) / g.q + g.w + 1;
     const int64_t out = ((int64_t)max_in * g.q + g.o - 1) / g.o;
-    const int64_t floats = hist + max_in;
-    if (floats * (int64_t)sizeof(float) > RS_SMEM_BYTES)
-        return fail(2, who + ": " + rs_rates(orig, new_freq) + " in pushes of up to " + std::to_string(max_in) +
-                           " samples is too large: " + std::to_string(floats) + " staged samples per row (history and "
-                           "push) exceed shared memory (" + std::to_string(RS_SMEM_BYTES / sizeof(float)) + ")");
+    if (int rc = staging(who, hist + max_in, rs_rates(orig, new_freq) + " in pushes of up to " + std::to_string(max_in) +
+                                                 " samples is too large", "samples per row (history and push)", smem))
+        return rc;
     s->delay = (int32_t)delay;
     s->hist = (int32_t)hist;
     s->max_in = max_in;
@@ -338,11 +381,10 @@ hop_fifo_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, int ma
         if (r.ch == 0 && tid == 0) hops[r.row] = 0;
         return;
     }
-    const int64_t pushed = (int64_t)counts[r.row] * unit;
-    const int n = pushed >= 0 && pushed <= max_in ? (int)pushed : 0;
+    const int n = row_pushed(counts, r.row, unit, max_in);
     float* st = r.st;
     float* ring = st + FF_HEAD;
-    const int pos = min(max(__float_as_int(st[0]), 0), R - 1), held = min(max(__float_as_int(st[1]), 0), capacity);
+    const int pos = int_word(st[0], R - 1), held = int_word(st[1], capacity);
     const int kept = min(n, capacity - held), h = min(T, (held + kept) / CHUNK_HOP);
     const float* xr = row_ch(x, x_row, x_ch, r.row, r.ch);
     for (int i = tid; i < kept; i += blockDim.x) ring[(pos + held + i) % R] = xr[i];
@@ -353,8 +395,7 @@ hop_fifo_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, int ma
         if (r.ch == 0) hops[r.row] = h;
         st[0] = __int_as_float((pos + h * CHUNK_HOP) % R);
         st[1] = __int_as_float(held + kept - h * CHUNK_HOP);
-        const int dropped = __float_as_int(st[2]);
-        st[2] = __int_as_float(n - kept > INT32_MAX - dropped ? INT32_MAX : dropped + (n - kept));
+        st[2] = add_word(st[2], n - kept);
     }
 }
 
@@ -368,8 +409,8 @@ enroll_capture_kernel(const float* __restrict__ chunk, int64_t c_row, int64_t c_
                       int n_slots, int capacity) {
     const int tid = threadIdx.x;
     const SlotRow sr = slot_row(C, slots, n_slots, state, EC_HEAD + capacity);
-    const int h = hops[sr.row];
-    if (!sr.live || h <= 0 || h > T) return;
+    const int h = row_hops(hops, sr.row, T);
+    if (h == 0 || !sr.live) return;
     float* st = sr.st;
     const CaptureRow r = capture_row(st, capacity);
     float* ring = st + EC_HEAD;
@@ -402,7 +443,7 @@ L2H_DEVINL Ramp ramp_of(const float* w, float rest) {
     const int f1 = __float_as_int(w[2]);
     if (f1 <= 0) return {rest, rest, 0, 0};
     const int F = f1 - 1;
-    return {w[0], w[1], F, min(max(__float_as_int(w[3]), 0), F)};
+    return {w[0], w[1], F, int_word(w[3], F)};
 }
 
 // the gain after q samples of the ramp: g1 from q = F on, a raised cosine from g0 before
@@ -479,8 +520,8 @@ target_mix_kernel(const float* __restrict__ y, int64_t y_row, int64_t y_ch, cons
     __shared__ int red[TM_THREADS / 32];
     const int tid = threadIdx.x;
     const SlotRow sr = slot_row(C, slots, n_slots, state + (int64_t)n_records * C * TM_FLOATS, TM_FLOATS);
-    const int h = hops ? hops[sr.row] : T;
-    if (!sr.live || h <= 0 || h > T) return;                           // a row that stores nothing
+    const int h = row_hops(hops, sr.row, T);
+    if (h == 0 || !sr.live) return;                                     // a row that stores nothing
     const int n = h * CHUNK_HOP, i = sr.row, ch = sr.ch;
     int lo = 0, hi = 0;                                                 // max of the clamped offsets 0 .. i and 0 .. i + 1
     for (int j = tid; j <= i + 1; j += TM_THREADS) {
@@ -599,8 +640,7 @@ limiter_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, int max
     const int tid = threadIdx.x;
     const int64_t rf = LM_HEAD + 3 * (int64_t)La;
     const SlotRow sr = slot_row(1, slots, n_slots, state, C * rf);
-    const int64_t pushed = (int64_t)counts[sr.row] * unit;
-    const int n = pushed >= 0 && pushed <= max_in ? (int)pushed : 0;
+    const int n = row_pushed(counts, sr.row, unit, max_in);
     if (!sr.live || n == 0) return;                                     // a row that stores nothing
     float* st = sr.st;                                                  // channel c's row at st + c rf
     const int W = La + n;
@@ -609,15 +649,15 @@ limiter_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, int max
     int* rs = qs + W;                                                   // [W]: the last La r, then s, then r
     const float cw = st[1];
     const float lim = cw >= FLT_MIN && cw <= FLT_MAX ? cw : ceiling;     // the slot's ceiling, else the call's
-    const int64_t r_in = min(max(__float_as_int(st[0]), 0), LM_MUTE);
+    const int64_t r_in = int_word(st[0], LM_MUTE);
     for (int c = 0; c < C; ++c) {
         const float* d = st + c * rf + LM_HEAD;
         const float* xr = row_ch(x, x_row, x_ch, sr.row, c);
         for (int i = tid; i < W; i += blockDim.x) xs[(int64_t)c * W + i] = i < La ? d[i] : xr[i - La];
     }
     for (int i = tid; i < La; i += blockDim.x) {
-        qs[i] = min(max(__float_as_int(st[LM_HEAD + La + i]), 0), LM_MUTE);
-        rs[i] = min(max(__float_as_int(st[LM_HEAD + 2 * La + i]), 0), LM_MUTE);
+        qs[i] = int_word(st[LM_HEAD + La + i], LM_MUTE);
+        rs[i] = int_word(st[LM_HEAD + 2 * La + i], LM_MUTE);
     }
     if (tid == 0) limited = 0;
     __syncthreads();
@@ -678,8 +718,7 @@ limiter_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, int max
     __syncthreads();                                                    // every thread counted
     if (tid == 0) {
         st[0] = __int_as_float(rs[La + n - 1]);
-        const int before = max(__float_as_int(st[2]), 0);
-        st[2] = __int_as_float(limited > INT32_MAX - before ? INT32_MAX : before + limited);
+        st[2] = add_word(st[2], limited);
     }
 }
 
@@ -700,8 +739,6 @@ limiter_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, int max
 constexpr int LV_HEAD = 3;
 constexpr int LV_FLOATS = LV_HEAD + 4;
 constexpr int LV_THREADS = TM_THREADS;                  // one thread per sample of a hop; block_max's block
-constexpr float LV_BIG = 4294967296.f;                  // 2^32
-constexpr float LV_LOG2_10_20 = 0.16609640474436813f;   // log2(10) / 20: dB to an octave of amplitude
 static_assert(LV_THREADS == CHUNK_HOP, "the leveler runs one thread per sample of a hop");
 
 struct LvParams {
@@ -734,15 +771,16 @@ leveler_kernel(const float* y, int64_t y_row, int64_t y_ch, float* out, int64_t 
             if (offsets[j] > r) { first = j; break; }
         i = -block_max(-first, red) - 1;
     }
-    const int h = i >= 0 && i < n ? (hops ? hops[i] : T) : 0;
-    if (!sr.live || h <= 0 || h > T) return;                            // a row that stores nothing
+    if (i < 0 || i >= n) return;                                        // a row of no listener
+    const int h = row_hops(hops, i, T);
+    if (h == 0 || !sr.live) return;                                     // a row that stores nothing
     float* st = sr.st;                                                  // channel c's row at st + c LV_FLOATS
     float E = st[0], g = st[2];
-    int cnt = max(__float_as_int(st[1]), 0);
+    int cnt = int_word(st[1], INT32_MAX);
     for (int t = 0; t < h; ++t) {
         const int64_t s = (int64_t)t * CHUNK_HOP + tid;
         bool bad = false;
-        for (int c = 0; c < C; ++c) bad = bad || !(fabsf(row_ch(y, y_row, y_ch, r, c)[s]) < LV_BIG);
+        for (int c = 0; c < C; ++c) bad = bad || !(fabsf(row_ch(y, y_row, y_ch, r, c)[s]) < HG_BIG);
         const bool measured = !__syncthreads_or(bad);
         if (measured) {
             float acc = 0.f;
@@ -787,8 +825,7 @@ leveler_kernel(const float* y, int64_t y_row, int64_t y_ch, float* out, int64_t 
             g_to = g;
         }
         __syncthreads();
-        const float gk = fmaf(g_to - g_from, (float)(tid + 1) * (1.f / CHUNK_HOP), g_from);
-        const float lin = gk == 0.f ? 1.f : exp2f(gk * LV_LOG2_10_20);
+        const float lin = hop_gain(g_from, g_to);
         for (int c = 0; c < C; ++c) row_ch(out, o_row, o_ch, r, c)[s] = row_ch(y, y_row, y_ch, r, c)[s] * lin;
     }
     if (tid == 0) {
@@ -832,8 +869,8 @@ band_compressor_kernel(const float* y, int64_t y_row, int64_t y_ch, float* out, 
     const int tid = threadIdx.x, H = L - 1, W = H + CHUNK_HOP, D = H / 2, CK = C * K;
     const int64_t rf = 5 * K + H;
     const SlotRow sr = slot_row(1, slots, n_slots, state, C * rf);
-    const int h = hops ? hops[sr.row] : T;
-    if (!sr.live || h <= 0 || h > T) return;                            // a row that stores nothing
+    const int h = row_hops(hops, sr.row, T);
+    if (h == 0 || !sr.live) return;                                     // a row that stores nothing
     float* st = sr.st;                                                  // channel c's row at st + c rf
     float* taps = reinterpret_cast<float*>(sm4);                        // [L][KP]: tap j of band b, zero past K
     float* win = taps + L * KP;                                         // [C][W]: the last H staged samples, then the hop
@@ -856,7 +893,7 @@ band_compressor_kernel(const float* y, int64_t y_row, int64_t y_ch, float* out, 
         bool bad = false;
         for (int c = 0; c < C; ++c) {
             const float v = row_ch(y, y_row, y_ch, sr.row, c)[s];
-            const bool ok = fabsf(v) < LV_BIG;
+            const bool ok = fabsf(v) < HG_BIG;
             bad = bad || !ok;
             win[c * W + H + tid] = ok ? v : 0.f;
         }
@@ -913,16 +950,12 @@ band_compressor_kernel(const float* y, int64_t y_row, int64_t y_ch, float* out, 
             live = live || g0[i] != 0.f || g1[i] != 0.f;
         }
         live = __syncthreads_or(live);                                  // and every gain is visible to the block
-        const float f = (float)(tid + 1) * (1.f / CHUNK_HOP);
         for (int c = 0; c < C; ++c) {
             float o = win[c * W + H + tid - D];                         // the staged input delayed by D
             if (live) {
                 o = 0.f;
-                for (int b = 0; b < K; ++b) {
-                    const float a = g0[c * K + b], gk = fmaf(g1[c * K + b] - a, f, a);
-                    const float lin = gk == 0.f ? 1.f : exp2f(gk * LV_LOG2_10_20);
-                    o = fmaf(lin, band[(c * K + b) * CHUNK_HOP + tid], o);
-                }
+                for (int b = 0; b < K; ++b)
+                    o = fmaf(hop_gain(g0[c * K + b], g1[c * K + b]), band[(c * K + b) * CHUNK_HOP + tid], o);
             }
             row_ch(out, o_row, o_ch, sr.row, c)[s] = o;
         }
@@ -971,16 +1004,24 @@ static int disjoint(const std::string& who, int32_t channels, std::initializer_l
     return ok ? 0 : fail(1, who + ": bad stride: rows and channels of " + what + " must not overlap");
 }
 
-// the samples of a separator chunk of `frames` hops: 0, or 1 when they do not fit an int32
-static int chunk_len(const std::string& who, int32_t frames, int64_t* len) {
-    *len = (int64_t)frames * CHUNK_HOP + CHUNK_CARRY;
-    return *len > INT32_MAX ? fail(1, who + ": frames is too large") : 0;
+// the samples of `frames` hops (len) and of a separator chunk of them (c_len: the carry, then the hops): 0, or 1 when
+// they do not fit an int32
+static int hop_lens(const std::string& who, int32_t frames, int64_t* len, int64_t* c_len) {
+    *len = (int64_t)frames * CHUNK_HOP;
+    *c_len = *len + CHUNK_CARRY;
+    return *c_len > INT32_MAX ? fail(1, who + ": frames is too large") : 0;
 }
 
-// the bytes [first, last) that `rows` rows of a strided operand span
-static std::pair<uintptr_t, uintptr_t> span(const void* p, int64_t rows, int32_t channels, const Rows& r) {
-    const uintptr_t a = reinterpret_cast<uintptr_t>(p);
-    return {a, a + (uintptr_t)(((rows - 1) * r.row + (int64_t)(channels - 1) * r.ch + r.len) * (int64_t)sizeof(float))};
+// whether n_out rows of `out` at po share a byte with n_in rows of `in` at pi (none when pi is null); out may be `in`
+// itself (the same pointer and strides) where `in_place`
+static bool overlap(const void* po, int64_t n_out, const Rows& out, const void* pi, int64_t n_in, const Rows& in,
+                    int32_t channels, bool in_place) {
+    if (!pi || (in_place && po == pi && out.row == in.row && out.ch == in.ch)) return false;
+    const auto end = [channels](const void* p, int64_t rows, const Rows& r) {    // the end of the bytes the rows span
+        return reinterpret_cast<uintptr_t>(p) +
+               (uintptr_t)(((rows - 1) * r.row + (int64_t)(channels - 1) * r.ch + r.len) * (int64_t)sizeof(float));
+    };
+    return reinterpret_cast<uintptr_t>(po) < end(pi, n_in, in) && reinterpret_cast<uintptr_t>(pi) < end(po, n_out, out);
 }
 
 // the error of the launch just made: 0, or 3 with its message
@@ -1054,7 +1095,7 @@ extern "C" int l2h_resample_stream_layout(int32_t orig_freq, int32_t new_freq, i
     using namespace l2h;
     if (!hist || !delay || !out_block) return fail(1, "l2h_resample_stream_layout: null pointer");
     RsStream s;
-    if (int rc = rs_stream("l2h_resample_stream_layout", orig_freq, new_freq, block, keep, 1, &s)) return rc;
+    if (int rc = rs_stream("l2h_resample_stream_layout", orig_freq, new_freq, block, keep, 1, &s, nullptr)) return rc;
     *hist = s.hist;
     *delay = s.delay;
     *out_block = s.out_block;
@@ -1071,11 +1112,11 @@ extern "C" int l2h_resample_stream(const float* x_dev, int64_t x_row_stride, int
                            {n, channels, blocks, n_slots}, n, channels, n_slots))
         return rc;
     RsStream s;
-    if (int rc = rs_stream(who, orig_freq, new_freq, block, keep, blocks, &s)) return rc;
+    int smem;
+    if (int rc = rs_stream(who, orig_freq, new_freq, block, keep, blocks, &s, &smem)) return rc;
     const int64_t x_len = (int64_t)blocks * block, y_len = keep + (int64_t)blocks * s.out_block;
     if (int rc = disjoint(who, channels, {{"x", x_row_stride, x_ch_stride, x_len}, {"y", y_row_stride, y_ch_stride, y_len}}))
         return rc;
-    const int smem = (int)((s.hist + x_len + y_len) * sizeof(float));
     resample_stream_kernel<<<(unsigned)(n * channels), RS_TILE, smem, static_cast<cudaStream_t>(stream)>>>(
         x_dev, x_row_stride, x_ch_stride, y_dev, y_row_stride, y_ch_stride, channels, blocks, slots_dev, hops_dev, state_dev,
         n_slots, s);
@@ -1088,7 +1129,7 @@ extern "C" int l2h_resample_packets_layout(int32_t orig_freq, int32_t new_freq, 
     if (!row_floats || !delay || !max_out) return fail(1, "l2h_resample_packets_layout: null pointer");
     RsPackets s;
     int32_t out;
-    if (int rc = rs_packets("l2h_resample_packets_layout", orig_freq, new_freq, max_in, &s, &out)) return rc;
+    if (int rc = rs_packets("l2h_resample_packets_layout", orig_freq, new_freq, max_in, &s, &out, nullptr)) return rc;
     *row_floats = RP_HEAD + s.hist;
     *delay = s.delay;
     *max_out = out;
@@ -1107,11 +1148,11 @@ extern "C" int l2h_resample_packets(const float* x_dev, int64_t x_row_stride, in
         return rc;
     RsPackets s;
     int32_t max_out;
-    if (int rc = rs_packets(who, orig_freq, new_freq, max_in, &s, &max_out)) return rc;
+    int smem;
+    if (int rc = rs_packets(who, orig_freq, new_freq, max_in, &s, &max_out, &smem)) return rc;
     s.unit = unit;
     if (int rc = disjoint(who, channels, {{"x", x_row_stride, x_ch_stride, max_in}, {"y", y_row_stride, y_ch_stride, max_out}}))
         return rc;
-    const int smem = (int)((s.hist + max_in) * sizeof(float));
     resample_packets_kernel<<<(unsigned)(n * channels), RS_TILE, smem, static_cast<cudaStream_t>(stream)>>>(
         x_dev, x_row_stride, x_ch_stride, y_dev, y_row_stride, y_ch_stride, channels, counts_dev, out_counts_dev, slots_dev,
         state_dev, n_slots, s);
@@ -1139,9 +1180,9 @@ extern "C" int l2h_hop_fifo(const float* x_dev, int64_t x_row_stride, int64_t x_
                            channels, n_slots))
         return rc;
     int32_t row_floats;
-    int64_t c_len;
+    int64_t len, c_len;
     if (int rc = l2h_hop_fifo_layout(capacity, &row_floats)) return rc;
-    if (int rc = chunk_len(who, frames, &c_len)) return rc;
+    if (int rc = hop_lens(who, frames, &len, &c_len)) return rc;
     if (int rc = disjoint(who, channels, {{"x", x_row_stride, x_ch_stride, max_in},
                                           {"chunk", chunk_row_stride, chunk_ch_stride, c_len}}))
         return rc;
@@ -1170,9 +1211,9 @@ extern "C" int l2h_enroll_capture(const float* chunk_dev, int64_t chunk_row_stri
                            {n, channels, frames, n_slots}, n, channels, n_slots))
         return rc;
     int32_t row_floats;
-    int64_t c_len;
+    int64_t len, c_len;
     if (int rc = l2h_enroll_capture_layout(capacity, &row_floats)) return rc;
-    if (int rc = chunk_len(who, frames, &c_len)) return rc;
+    if (int rc = hop_lens(who, frames, &len, &c_len)) return rc;
     if (int rc = disjoint(who, channels, {{"chunk", chunk_row_stride, chunk_ch_stride, c_len}})) return rc;
     enroll_capture_kernel<<<(unsigned)(n * channels), RS_TILE, 0, static_cast<cudaStream_t>(stream)>>>(
         chunk_dev, chunk_row_stride, chunk_ch_stride, channels, frames, slots_dev, hops_dev, state_dev, n_slots, capacity);
@@ -1198,15 +1239,13 @@ extern "C" int l2h_target_mix(const float* y_dev, int64_t y_row_stride, int64_t 
                            channels, n_slots))
         return rc;
     if (n > R) return fail(1, who + ": a call needs n <= R (every listener row owns its target rows)");
-    int64_t c_len;
-    if (int rc = chunk_len(who, frames, &c_len)) return rc;
-    const int64_t len = (int64_t)frames * CHUNK_HOP;
+    int64_t len, c_len;
+    if (int rc = hop_lens(who, frames, &len, &c_len)) return rc;
     const Rows y{"y", y_row_stride, y_ch_stride, len}, out{"out", out_row_stride, out_ch_stride, len},
         ck{"chunk", chunk_row_stride, chunk_ch_stride, c_len};
     if (int rc = chunk_dev ? disjoint(who, channels, {y, ck, out}) : disjoint(who, channels, {y, out})) return rc;
-    const auto o = span(out_dev, n, channels, out), a = span(y_dev, R, channels, y);
-    const auto b = chunk_dev ? span(chunk_dev, n, channels, ck) : std::make_pair(uintptr_t(0), uintptr_t(0));
-    if ((o.first < a.second && a.first < o.second) || (o.first < b.second && b.first < o.second))
+    if (overlap(out_dev, n, out, y_dev, R, y, channels, false) ||
+        overlap(out_dev, n, out, chunk_dev, n, ck, channels, false))
         return fail(1, who + ": out must not overlap y or the chunk");
     bool vec = true;                                    // float4 loads and stores where every operand allows them
     for (const Rows& r : {y, out, ck}) vec = vec && r.row % 4 == 0 && r.ch % 4 == 0;
@@ -1242,22 +1281,17 @@ namespace l2h {
 static int lm_staging(const std::string& who, int32_t channels, int32_t lookahead, int32_t max_in, int* smem) {
     if (channels <= 0) return fail(1, who + ": channels must be positive");
     if (lookahead < 0) return fail(1, who + ": lookahead " + std::to_string(lookahead) + " is negative");
-    const int64_t floats = ((int64_t)channels + 2) * ((int64_t)lookahead + max_in);
-    if (floats * (int64_t)sizeof(float) > RS_SMEM_BYTES)
-        return fail(2, who + ": " + std::to_string(channels) + " channels with a look-ahead of " + std::to_string(lookahead) +
-                           " samples and pushes of up to " + std::to_string(max_in) + " samples are too large: " +
-                           std::to_string(floats) + " staged words per row exceed shared memory (" +
-                           std::to_string(RS_SMEM_BYTES / sizeof(float)) + ")");
-    *smem = (int)(floats * sizeof(float));
-    return 0;
+    return staging(who, ((int64_t)channels + 2) * ((int64_t)lookahead + max_in),
+                   std::to_string(channels) + " channels with a look-ahead of " + std::to_string(lookahead) +
+                       " samples and pushes of up to " + std::to_string(max_in) + " samples are too large",
+                   "words per row", smem);
 }
 }  // namespace l2h
 
 extern "C" int l2h_limiter_layout(int32_t channels, int32_t lookahead, int32_t* row_floats) {
     using namespace l2h;
     if (!row_floats) return fail(1, "l2h_limiter_layout: null pointer");
-    int smem;
-    if (int rc = lm_staging("l2h_limiter_layout", channels, lookahead, 1, &smem)) return rc;
+    if (int rc = lm_staging("l2h_limiter_layout", channels, lookahead, 1, nullptr)) return rc;
     *row_floats = LM_HEAD + 3 * lookahead;
     return 0;
 }
@@ -1280,8 +1314,7 @@ extern "C" int l2h_limiter(const float* x_dev, int64_t x_row_stride, int64_t x_c
     if (int rc = lm_staging(who, channels, lookahead, max_in, &smem)) return rc;
     const Rows x{"x", x_row_stride, x_ch_stride, max_in}, y{"y", y_row_stride, y_ch_stride, max_in};
     if (int rc = disjoint(who, channels, {x, y})) return rc;
-    const auto a = span(x_dev, n, channels, x), b = span(y_dev, n, channels, y);
-    if (a.first < b.second && b.first < a.second) return fail(1, who + ": y must not overlap x");
+    if (overlap(y_dev, n, y, x_dev, n, x, channels, false)) return fail(1, who + ": y must not overlap x");
     limiter_kernel<<<(unsigned)n, RS_TILE, smem, static_cast<cudaStream_t>(stream)>>>(
         x_dev, x_row_stride, x_ch_stride, max_in, counts_dev, unit, y_dev, y_row_stride, y_ch_stride, channels, slots_dev,
         state_dev, n_slots, ceiling, lookahead, release_step);
@@ -1327,7 +1360,8 @@ extern "C" int l2h_leveler(const float* y_dev, int64_t y_row_stride, int64_t y_c
                            {n, R, channels, frames, n_rows}, n, channels, n_rows))
         return rc;
     if (n > R) return fail(1, who + ": a call needs n <= R (every listener row owns its rows)");
-    if ((int64_t)frames * CHUNK_HOP > INT32_MAX) return fail(1, who + ": frames is too large");
+    int64_t len, c_len;
+    if (int rc = hop_lens(who, frames, &len, &c_len)) return rc;
     for (float v : {target, gate, relative, min_gain, max_gain})
         if (!std::isfinite(v)) return fail(1, who + ": target, gate, relative, min_gain and max_gain must be finite");
     if (relative > 0.f) return fail(1, who + ": relative " + std::to_string(relative) + " dB is above 0");
@@ -1338,12 +1372,9 @@ extern "C" int l2h_leveler(const float* y_dev, int64_t y_row_stride, int64_t y_c
     if (!(rise_step >= 0.f && fall_step >= 0.f && std::isfinite(rise_step) && std::isfinite(fall_step)))
         return fail(1, who + ": rise_step and fall_step must be finite and not negative");
     if (settle_hops < 1) return fail(1, who + ": settle_hops " + std::to_string(settle_hops) + " is below 1");
-    const int64_t len = (int64_t)frames * CHUNK_HOP;
     const Rows y{"y", y_row_stride, y_ch_stride, len}, out{"out", out_row_stride, out_ch_stride, len};
     if (int rc = disjoint(who, channels, {y, out})) return rc;
-    const bool in_place = out_dev == y_dev && out_row_stride == y_row_stride && out_ch_stride == y_ch_stride;
-    const auto a = span(y_dev, R, channels, y), b = span(out_dev, R, channels, out);
-    if (!in_place && a.first < b.second && b.first < a.second)
+    if (overlap(out_dev, R, out, y_dev, R, y, channels, true))
         return fail(1, who + ": out must be y itself (same pointer and strides) or not overlap it");
     LvParams p;
     lv_filters(16000.0, &p);
@@ -1375,13 +1406,8 @@ static int bc_staging(const std::string& who, int32_t channels, int32_t bands, i
     *kp = (bands + 3) / 4 * 4;                          // the kernel reads each tap row as float4
     const int64_t floats = (int64_t)taps * *kp + (int64_t)channels * (taps - 1 + CHUNK_HOP) +
                            (int64_t)channels * bands * (CHUNK_HOP + 2);
-    if (floats * (int64_t)sizeof(float) > RS_SMEM_BYTES)
-        return fail(2, who + ": " + std::to_string(channels) + " channels of " + std::to_string(bands) + " bands of " +
-                           std::to_string(taps) + " taps are too large: " + std::to_string(floats) +
-                           " staged words per row exceed shared memory (" + std::to_string(RS_SMEM_BYTES / sizeof(float)) +
-                           ")");
-    *smem = (int)(floats * sizeof(float));
-    return 0;
+    return staging(who, floats, std::to_string(channels) + " channels of " + std::to_string(bands) + " bands of " +
+                                    std::to_string(taps) + " taps are too large", "words per row", smem);
 }
 }  // namespace l2h
 
@@ -1389,8 +1415,8 @@ extern "C" int l2h_band_compressor_design(int32_t bands, const float* edges_hz, 
     using namespace l2h;
     const std::string who = "l2h_band_compressor_design";
     if (!out || (bands > 1 && !edges_hz)) return fail(1, who + ": null pointer");
-    int kp, smem;
-    if (int rc = bc_staging(who, 1, bands, taps, &kp, &smem)) return rc;   // one channel always fits
+    int kp;
+    if (int rc = bc_staging(who, 1, bands, taps, &kp, nullptr)) return rc;   // one channel always fits
     for (int j = 0; j + 1 < bands; ++j) {
         const float e = edges_hz[j];
         if (!(e > 0.f && e < 8000.f) || (j > 0 && !(e > edges_hz[j - 1])))
@@ -1424,8 +1450,8 @@ extern "C" int l2h_band_compressor_design(int32_t bands, const float* edges_hz, 
 extern "C" int l2h_band_compressor_layout(int32_t channels, int32_t bands, int32_t taps, int32_t* row_floats) {
     using namespace l2h;
     if (!row_floats) return fail(1, "l2h_band_compressor_layout: null pointer");
-    int kp, smem;
-    if (int rc = bc_staging("l2h_band_compressor_layout", channels, bands, taps, &kp, &smem)) return rc;
+    int kp;
+    if (int rc = bc_staging("l2h_band_compressor_layout", channels, bands, taps, &kp, nullptr)) return rc;
     *row_floats = 5 * bands + taps - 1;
     return 0;
 }
@@ -1440,18 +1466,16 @@ extern "C" int l2h_band_compressor(const float* y_dev, int64_t y_row_stride, int
     if (int rc = slot_call(who, {y_dev, out_dev, slots_dev, taps_dev, state_dev}, "n, channels, frames and n_slots",
                            {n, channels, frames, n_slots}, n, channels, n_slots))
         return rc;
-    if ((int64_t)frames * CHUNK_HOP > INT32_MAX) return fail(1, who + ": frames is too large");
+    int64_t len, c_len;
+    if (int rc = hop_lens(who, frames, &len, &c_len)) return rc;
     if (!(attack > 0.f && attack <= 1.f) || !(release > 0.f && release <= 1.f))
         return fail(1, who + ": attack " + std::to_string(attack) + " and release " + std::to_string(release) +
                            " must lie in (0, 1]");
     int kp, smem;
     if (int rc = bc_staging(who, channels, bands, taps, &kp, &smem)) return rc;
-    const int64_t len = (int64_t)frames * CHUNK_HOP;
     const Rows y{"y", y_row_stride, y_ch_stride, len}, out{"out", out_row_stride, out_ch_stride, len};
     if (int rc = disjoint(who, channels, {y, out})) return rc;
-    const bool in_place = out_dev == y_dev && out_row_stride == y_row_stride && out_ch_stride == y_ch_stride;
-    const auto a = span(y_dev, n, channels, y), b = span(out_dev, n, channels, out);
-    if (!in_place && a.first < b.second && b.first < a.second)
+    if (overlap(out_dev, n, out, y_dev, n, y, channels, true))
         return fail(1, who + ": out must be y itself (same pointer and strides) or not overlap it");
     const auto kernel = kp == 4 ? band_compressor_kernel<4> : kp == 8 ? band_compressor_kernel<8>
                       : kp == 12 ? band_compressor_kernel<12> : band_compressor_kernel<16>;

@@ -357,6 +357,18 @@ def device_list(values, dev, n, end, distinct, noun):
     return v.to(torch.int32).to(dev)
 
 
+def device_offsets(offsets, dev, n, R):
+    """The row offsets of a call of n listeners over R rows as the [n + 1] int32 device tensor: device_list's checks
+    (entries in [0, R]), and host lists must also start at 0 and never decrease.  A CUDA tensor is used as it is; the
+    kernels clamp its entries as the separator does."""
+    values = device_list(offsets, dev, n + 1, R + 1, False, "offset")
+    if not (isinstance(offsets, torch.Tensor) and offsets.is_cuda):
+        o = torch.as_tensor(offsets).tolist()
+        if o[0] != 0 or any(b < a for a, b in zip(o, o[1:])):
+            raise ValueError(f"offsets must start at 0 and never decrease, got {o}")
+    return values
+
+
 class Net(nn.Module):
     """CUDA (H100) replacement of the reference ``Net`` (net.py:20-76)."""
 
@@ -802,16 +814,11 @@ class Net(nn.Module):
                 raise TypeError("history must come from Net.target_history()")
             history.check(state)
         records = device_list(records, dev, R, state.batch, True, "record")
-        on_host = not (isinstance(offsets, torch.Tensor) and offsets.is_cuda)
-        offsets_dev = device_list(offsets, dev, n + 1, R + 1, False, "offset")
-        if on_host:
-            o = torch.as_tensor(offsets).tolist()
-            if o[0] != 0 or any(b < a for a, b in zip(o, o[1:])):
-                raise ValueError(f"offsets must start at 0 and never decrease, got {o}")
+        offsets = device_offsets(offsets, dev, n, R)
         self._require_cuda(x)
         y = torch.empty(R, self.num_src, out_len, dtype=torch.float32, device=dev)
         self._launch("targets_rows", x.contiguous().float(), embeds.to(dev, torch.float32).contiguous(), state, y, frames,
-                     slots=records, hops=hops, offsets=offsets_dev, history=history)
+                     slots=records, hops=hops, offsets=offsets, history=history)
         return y
 
     def target_history(self, state, frames):

@@ -18,7 +18,7 @@ import numbers
 import torch
 
 from . import _cabi
-from .net import device_list
+from .net import device_list, device_offsets
 
 
 def _whole(v, what, low=1):
@@ -26,6 +26,14 @@ def _whole(v, what, low=1):
     if isinstance(v, bool) or not isinstance(v, numbers.Integral) or int(v) < low or int(v) >= 2 ** 31:
         raise ValueError(f"{what} must be an integer >= {low} (below 2**31), got {v!r}")
     return int(v)
+
+
+def _real(v, what, ok=math.isfinite, must="a finite number"):
+    """v as a float when it is a real number, not a bool, that passes `ok` (by default: finite; a range test also
+    refuses NaN), else ValueError "{what} must be {must}"."""
+    if isinstance(v, bool) or not isinstance(v, numbers.Real) or not ok(v):
+        raise ValueError(f"{what} must be {must}, got {v!r}")
+    return float(v)
 
 
 def _check(rc):
@@ -47,6 +55,7 @@ class _SlotStage:
     checks of the row tensors a call reads and writes."""
 
     HOP, CARRY = 128, 64      # a separator chunk of h hops: 64 samples carried from the last chunk, then 128 h new ones
+    HOP_S = 128 / 16000       # seconds per hop of the 16 kHz grid
 
     def __init__(self, slots, channels):
         self.n_slots, self.channels = _whole(slots, "slots"), _whole(channels, "channels")
@@ -63,12 +72,27 @@ class _SlotStage:
 
     def reset(self, slots):
         """Make the listed slots fresh (their state rows zero); the other slots keep what they hold."""
-        idx = torch.as_tensor(slots).cpu().reshape(-1)
-        idx = device_list(idx, self.state.device, idx.numel(), self.n_slots, False, "slot")
-        self.state.index_fill_(0, idx.long(), 0.0)
+        self.state.index_fill_(0, self._indices(slots, self.n_slots, "slot"), 0.0)
 
-    def _stream(self):
-        return torch.cuda.current_stream(self.state.device).cuda_stream
+    def _indices(self, values, end, noun, distinct=False, need=None):
+        """host indices into [0, end) (each listed once if `distinct`), checked and uploaded as an int64 tensor on the
+        state's device; `need` names a call that needs at least one"""
+        idx = torch.as_tensor(values).cpu().reshape(-1)
+        if need and idx.numel() < 1:
+            raise ValueError(f"{need} needs at least one {noun}")
+        return device_list(idx, self.state.device, idx.numel(), end, distinct, noun).long()
+
+    def _hops(self, hops, n, T):
+        """an optional hop list of n rows in [0, T], as device_list uploads it"""
+        return None if hops is None else device_list(hops, self.state.device, n, T + 1, False, "hop")
+
+    def _run(self, entry, *args):
+        """the C entry `entry` called on the state's device and its current stream, each tensor argument passed as its
+        data pointer"""
+        dev = self.state.device
+        with torch.cuda.device(dev):
+            args = [a.data_ptr() if isinstance(a, torch.Tensor) else a for a in args]
+            _check(getattr(_cabi.lib(), entry)(*args, torch.cuda.current_stream(dev).cuda_stream))
 
     def _rows_in(self, x, block=None):
         """x [n, channels, L] (n, L >= 1; L a multiple of `block` if given) as float32 on the state's device with unit
@@ -153,14 +177,10 @@ class StreamResampler(_SlotStage):
         n, C, L = x.shape
         T = L // self.block
         slots = device_list(slots, dev, n, self.n_slots, True, "slot")
-        if hops is not None:
-            hops = device_list(hops, dev, n, T + 1, False, "hop")
+        hops = self._hops(hops, n, T)
         out = self._rows_out(out, (n, C, self.keep + T * self.out_block))
-        with torch.cuda.device(dev):
-            _check(_cabi.lib().l2h_resample_stream(
-                x.data_ptr(), x.stride(0), x.stride(1), out.data_ptr(), out.stride(0), out.stride(1), n, C, T,
-                slots.data_ptr(), None if hops is None else hops.data_ptr(), self.state.data_ptr(), self.n_slots,
-                self.orig_freq, self.new_freq, self.block, self.keep, self._stream()))
+        self._run("l2h_resample_stream", x, x.stride(0), x.stride(1), out, out.stride(0), out.stride(1), n, C, T, slots,
+                  hops, self.state, self.n_slots, self.orig_freq, self.new_freq, self.block, self.keep)
         return out
 
 
@@ -206,11 +226,8 @@ class PacketResampler(_SlotStage):
         counts = device_list(counts, dev, n, self.max_in // unit + 1, False, "count")
         out = self._rows_out(out, (n, C, self.max_out))
         out_counts = self._ints_out(out_counts, n, "out_counts")
-        with torch.cuda.device(dev):
-            _check(_cabi.lib().l2h_resample_packets(
-                x.data_ptr(), x.stride(0), x.stride(1), out.data_ptr(), out.stride(0), out.stride(1), n, C, L,
-                counts.data_ptr(), unit, out_counts.data_ptr(), slots.data_ptr(), self.state.data_ptr(), self.n_slots,
-                self.orig_freq, self.new_freq, self._stream()))
+        self._run("l2h_resample_packets", x, x.stride(0), x.stride(1), out, out.stride(0), out.stride(1), n, C, L, counts,
+                  unit, out_counts, slots, self.state, self.n_slots, self.orig_freq, self.new_freq)
         return out, out_counts
 
 
@@ -250,11 +267,8 @@ class HopFifo(_SlotStage):
         counts = device_list(counts, dev, n, L // unit + 1, False, "count")
         out = self._rows_out(out, (n, C, self.HOP * self.frames + self.CARRY))
         hops = self._ints_out(hops, n, "hops")
-        with torch.cuda.device(dev):
-            _check(_cabi.lib().l2h_hop_fifo(
-                x.data_ptr(), x.stride(0), x.stride(1), L, counts.data_ptr(), unit, out.data_ptr(), out.stride(0),
-                out.stride(1), hops.data_ptr(), n, C, self.frames, slots.data_ptr(), self.state.data_ptr(), self.n_slots,
-                self.capacity, self._stream()))
+        self._run("l2h_hop_fifo", x, x.stride(0), x.stride(1), L, counts, unit, out, out.stride(0), out.stride(1), hops, n,
+                  C, self.frames, slots, self.state, self.n_slots, self.capacity)
         return out, hops
 
     @property
@@ -302,10 +316,8 @@ class EnrollCapture(_SlotStage):
         T = (L - self.CARRY) // self.HOP
         slots = device_list(slots, dev, n, self.n_slots, True, "slot")
         hops = device_list(hops, dev, n, T + 1, False, "hop")
-        with torch.cuda.device(dev):
-            _check(_cabi.lib().l2h_enroll_capture(
-                chunk.data_ptr(), chunk.stride(0), chunk.stride(1), n, C, T, slots.data_ptr(), hops.data_ptr(),
-                self.state.data_ptr(), self.n_slots, self.capacity, self._stream()))
+        self._run("l2h_enroll_capture", chunk, chunk.stride(0), chunk.stride(1), n, C, T, slots, hops, self.state,
+                  self.n_slots, self.capacity)
 
     @property
     def captured(self):
@@ -338,12 +350,10 @@ class TargetMixer(_SlotStage):
 
     def reset(self, records=(), slots=()):
         """Make the listed records (gain 1) and slots (ambient gain 0) fresh; the other rows keep their ramps."""
-        dev = self.state.device
-        rows = []
-        for values, end, noun, base in ((records, self.n_records, "record", 0), (slots, self.n_slots, "slot", self.n_records)):
-            v = torch.as_tensor(values).cpu().reshape(-1)
-            if v.numel():
-                rows.append(device_list(v, dev, v.numel(), end, False, noun).long() + base)
+        rows = [self._indices(values, end, noun) + base
+                for values, end, noun, base in ((records, self.n_records, "record", 0),
+                                                (slots, self.n_slots, "slot", self.n_records))
+                if torch.as_tensor(values).numel()]
         if rows:
             self.state.index_fill_(0, torch.cat(rows), 0.0)
 
@@ -376,27 +386,18 @@ class TargetMixer(_SlotStage):
         if not 0 < n <= R:
             raise ValueError(f"a mix needs 0 < n <= R, got n = {n} listeners and R = {R} target rows")
         records = device_list(records, dev, R, self.n_records, True, "record")
-        on_host = not (isinstance(offsets, torch.Tensor) and offsets.is_cuda)
-        o = torch.as_tensor(offsets).tolist() if on_host else None
-        offsets = device_list(offsets, dev, n + 1, R + 1, False, "offset")
-        if on_host:
-            if o[0] != 0 or any(b < a for a, b in zip(o, o[1:])):
-                raise ValueError(f"offsets must start at 0 and never decrease, got {o}")
+        offsets = device_offsets(offsets, dev, n, R)
         slots = device_list(slots, dev, n, self.n_slots, True, "slot")
-        if hops is not None:
-            hops = device_list(hops, dev, n, T + 1, False, "hop")
+        hops = self._hops(hops, n, T)
         if chunk is not None:
             chunk = self._rows_in(chunk)
             if tuple(chunk.shape) != (n, C, L + self.CARRY):
                 raise ValueError(f"chunk must have shape [{n}, {C}, {L + self.CARRY}] (the separator's input of the call, "
                                  f"with y's channels), got {tuple(chunk.shape)}")
         out = self._rows_out(out, (n, C, L))
-        ck = (None, 0, 0) if chunk is None else (chunk.data_ptr(), chunk.stride(0), chunk.stride(1))
-        with torch.cuda.device(dev):
-            _check(_cabi.lib().l2h_target_mix(
-                y.data_ptr(), y.stride(0), y.stride(1), *ck, out.data_ptr(), out.stride(0), out.stride(1), n, R, C, T,
-                records.data_ptr(), offsets.data_ptr(), None if hops is None else hops.data_ptr(), slots.data_ptr(),
-                self.state.data_ptr(), self.n_records, self.n_slots, self._stream()))
+        ck = (None, 0, 0) if chunk is None else (chunk, chunk.stride(0), chunk.stride(1))
+        self._run("l2h_target_mix", y, y.stride(0), y.stride(1), *ck, out, out.stride(0), out.stride(1), n, R, C, T, records,
+                  offsets, hops, slots, self.state, self.n_records, self.n_slots)
         return out
 
     def set_gains(self, records, gains, fade=0, start=None):
@@ -427,10 +428,8 @@ class TargetMixer(_SlotStage):
         gains = self._values(gains, n, torch.float32, "gains")
         fades = self._values(fade, n, torch.int32, "fade")
         starts = None if start is None else self._values(start, n, torch.float32, "start")
-        with torch.cuda.device(dev):
-            _check(_cabi.lib().l2h_target_mix_set(
-                self.state.data_ptr(), self.n_records, self.n_slots, self.channels, rows.data_ptr(), n,
-                gains.data_ptr(), None if starts is None else starts.data_ptr(), fades.data_ptr(), self._stream()))
+        self._run("l2h_target_mix_set", self.state, self.n_records, self.n_slots, self.channels, rows, n, gains, starts,
+                  fades)
 
     def _values(self, v, n, dtype, what):
         """v as an [n] `dtype` tensor on the state's device: a CUDA tensor used in place, else numbers checked and
@@ -450,9 +449,7 @@ class TargetMixer(_SlotStage):
                 raise ValueError(f"{what} must be below 2**31 - 1 samples")
         else:
             for g in vals:
-                if (isinstance(g, bool) or not isinstance(g, numbers.Real) or not math.isfinite(g)
-                        or not 0.0 <= g <= self.GAIN_MAX):
-                    raise ValueError(f"{what} must be finite numbers in [0, {self.GAIN_MAX:g}], got {g!r}")
+                _real(g, what, lambda g: 0.0 <= g <= self.GAIN_MAX, f"finite numbers in [0, {self.GAIN_MAX:g}]")
         return torch.tensor(vals, dtype=dtype).to(dev)
 
     def _words(self):
@@ -508,11 +505,8 @@ class Limiter(_SlotStage):
         super().__init__(slots, channels)
         self.rate = _whole(rate, "rate")
         self.ceiling = self._level(ceiling, "ceiling")
-        if isinstance(lookahead, bool) or not isinstance(lookahead, numbers.Real) or not 0 <= lookahead < 2 ** 31 / self.rate:
-            raise ValueError(f"lookahead must be a number of seconds >= 0, got {lookahead!r}")
-        if (isinstance(release, bool) or not isinstance(release, numbers.Real) or not math.isfinite(release)
-                or release <= 0):
-            raise ValueError(f"release must be a positive number of dB per second, got {release!r}")
+        _real(lookahead, "lookahead", lambda s: 0 <= s < 2 ** 31 / self.rate, "a number of seconds >= 0")
+        _real(release, "release", lambda r: 0 < r < math.inf, "a positive number of dB per second")
         self.lookahead = round(lookahead * self.rate)
         self.release_step = max(1, round(release / self.DB_PER_OCTAVE * self.Q / self.rate))
         if self.release_step > self.MUTE:
@@ -522,10 +516,10 @@ class Limiter(_SlotStage):
     @staticmethod
     def _level(v, what, zero=False):
         """v rounded to float32, where it must be a positive normal number (or 0 if `zero`), or ValueError"""
-        ok = not isinstance(v, bool) and isinstance(v, numbers.Real) and math.isfinite(v)
-        f = float(torch.tensor(float(v), dtype=torch.float32)) if ok else math.nan
-        if not (ok and (2.0 ** -126 <= f < math.inf or (zero and v == 0))):
-            raise ValueError(f"{what} must be a positive amplitude that float32 holds as a normal number, got {v!r}")
+        must = "a positive amplitude that float32 holds as a normal number"
+        f = float(torch.tensor(_real(v, what, must=must), dtype=torch.float32))
+        if not (2.0 ** -126 <= f < math.inf or (zero and v == 0)):
+            raise ValueError(f"{what} must be {must}, got {v!r}")
         return f
 
     def __call__(self, x, counts, slots, unit=1, out=None):
@@ -547,29 +541,22 @@ class Limiter(_SlotStage):
         slots = device_list(slots, dev, n, self.n_slots, True, "slot")
         counts = device_list(counts, dev, n, L // unit + 1, False, "count")
         out = self._rows_out(out, (n, C, L))
-        with torch.cuda.device(dev):
-            _check(_cabi.lib().l2h_limiter(
-                x.data_ptr(), x.stride(0), x.stride(1), L, counts.data_ptr(), unit, out.data_ptr(), out.stride(0),
-                out.stride(1), n, C, slots.data_ptr(), self.state.data_ptr(), self.n_slots, self.ceiling,
-                self.lookahead, self.release_step, self._stream()))
+        self._run("l2h_limiter", x, x.stride(0), x.stride(1), L, counts, unit, out, out.stride(0), out.stride(1), n, C, slots,
+                  self.state, self.n_slots, self.ceiling, self.lookahead, self.release_step)
         return out
 
     def set_ceiling(self, slots, values):
         """Give the listed slots their own ceilings (a hearing-safety cap per user): `values` one number or one per slot,
         positive finite amplitudes, or 0 for the limiter's `ceiling`.  It applies to the samples pushed after the set.
         Enqueued on the current stream; `reset` returns a slot to the default."""
-        dev = self.state.device
-        idx = torch.as_tensor(slots).cpu().reshape(-1)
+        idx = self._indices(slots, self.n_slots, "slot", True, "set_ceiling")
         n = idx.numel()
-        if n < 1:
-            raise ValueError("set_ceiling needs at least one slot")
-        idx = device_list(idx, dev, n, self.n_slots, True, "slot")
         vals = values.tolist() if isinstance(values, torch.Tensor) else values
         vals = list(vals) if isinstance(vals, (list, tuple)) else [vals] * n
         if len(vals) != n:
             raise ValueError(f"values gives {len(vals)} ceilings for {n} slots")
         vals = [self._level(v, "a ceiling", zero=True) for v in vals]
-        self.state[idx.long(), 0, 1] = torch.tensor(vals, dtype=torch.float32).to(dev)
+        self.state[idx, 0, 1] = torch.tensor(vals, dtype=torch.float32).to(self.state.device)
 
     @property
     def reduction(self):
@@ -604,12 +591,10 @@ class Leveler(_SlotStage):
     `state` [rows, channels, 7] is a float32 tensor on `device`: all zeros is a fresh row, so rows are reset by zeroing
     them (`reset`) and moved by copying them."""
 
-    HOP_S = 128 / 16000                         # seconds per hop of the 16 kHz grid
-
     def __init__(self, rows, channels, target=-20.0, gate=-50.0, relative=-20.0, window=3.0, settle=0.256,
                  min_gain=-12.0, max_gain=12.0, rise=3.0, fall=10.0, device=None):
         super().__init__(rows, channels)
-        num = {k: self._number(v, k) for k, v in (("target", target), ("gate", gate), ("relative", relative),
+        num = {k: _real(v, k) for k, v in (("target", target), ("gate", gate), ("relative", relative),
                                                    ("window", window), ("settle", settle), ("min_gain", min_gain),
                                                    ("max_gain", max_gain), ("rise", rise), ("fall", fall))}
         if num["relative"] > 0:
@@ -629,12 +614,6 @@ class Leveler(_SlotStage):
         if self.settle_hops >= 2 ** 31 or self.alpha <= 0:
             raise ValueError(f"settle {settle!r} s or window {window!r} s is out of range")
         self._allocate(*_layout(_cabi.lib().l2h_leveler_layout, self.channels), device)
-
-    @staticmethod
-    def _number(v, what):
-        if isinstance(v, bool) or not isinstance(v, numbers.Real) or not math.isfinite(v):
-            raise ValueError(f"{what} must be a finite number, got {v!r}")
-        return float(v)
 
     def __call__(self, y, records, offsets=None, hops=None, out=None):
         """y [R, channels, 128 * T] CUDA tensor: row r is leveled with the state of row records[r].  Returns out [R,
@@ -660,23 +639,14 @@ class Leveler(_SlotStage):
             n = (offsets.numel() if isinstance(offsets, torch.Tensor) else len(offsets)) - 1
             if not 0 < n <= R:
                 raise ValueError(f"offsets must hold n + 1 entries with 0 < n <= R = {R}, got {n + 1}")
-            on_host = not (isinstance(offsets, torch.Tensor) and offsets.is_cuda)
-            o = torch.as_tensor(offsets).tolist() if on_host else None
-            offsets = device_list(offsets, dev, n + 1, R + 1, False, "offset")
-            if on_host and (o[0] != 0 or any(b < a for a, b in zip(o, o[1:]))):
-                raise ValueError(f"offsets must start at 0 and never decrease, got {o}")
+            offsets = device_offsets(offsets, dev, n, R)
         if n > self.n_slots:
             raise ValueError(f"a call of {n} listeners needs n <= rows = {self.n_slots}")
-        if hops is not None:
-            hops = device_list(hops, dev, n, T + 1, False, "hop")
+        hops = self._hops(hops, n, T)
         out = self._rows_out(out, (R, C, L))
-        with torch.cuda.device(dev):
-            _check(_cabi.lib().l2h_leveler(
-                y.data_ptr(), y.stride(0), y.stride(1), out.data_ptr(), out.stride(0), out.stride(1), n, R, C, T,
-                records.data_ptr(), None if offsets is None else offsets.data_ptr(),
-                None if hops is None else hops.data_ptr(), self.state.data_ptr(), self.n_slots, self.target, self.gate,
-                self.relative, self.alpha, self.settle_hops, self.min_gain, self.max_gain, self.rise_step,
-                self.fall_step, self._stream()))
+        self._run("l2h_leveler", y, y.stride(0), y.stride(1), out, out.stride(0), out.stride(1), n, R, C, T, records,
+                  offsets, hops, self.state, self.n_slots, self.target, self.gate, self.relative, self.alpha,
+                  self.settle_hops, self.min_gain, self.max_gain, self.rise_step, self.fall_step)
         return out
 
     @property
@@ -717,7 +687,6 @@ class BandCompressor(_SlotStage):
 
     RATE = 16000
     RANGE = 40.0                                # the gains' clamp, dB
-    HOP_S = 128 / 16000                         # seconds per hop of the 16 kHz grid
 
     def __init__(self, slots, channels, edges=(500, 1000, 2000, 4000), taps=129, attack=0.005, release=0.08,
                  device=None):
@@ -726,12 +695,14 @@ class BandCompressor(_SlotStage):
         self.edges = tuple(float(e) for e in torch.as_tensor(edges, dtype=torch.float32).reshape(-1).tolist())
         self.bands, self.n_taps = bank.shape
         self.delay = (self.n_taps - 1) // 2
+        def coef_of(tau):                       # the per-hop step of a detector with time constant tau seconds
+            return -math.expm1(-self.HOP_S / tau)
+
         coef = {}
         for what, tau in (("attack", attack), ("release", release)):
-            if (isinstance(tau, bool) or not isinstance(tau, numbers.Real) or not math.isfinite(tau) or tau <= 0
-                    or float(torch.tensor(-math.expm1(-self.HOP_S / tau), dtype=torch.float32)) <= 0):
-                raise ValueError(f"{what} must be a positive number of seconds, got {tau!r}")
-            coef[what] = -math.expm1(-self.HOP_S / tau)
+            _real(tau, what, lambda t: 0 < t < math.inf and float(torch.tensor(coef_of(t), dtype=torch.float32)) > 0,
+                  "a positive number of seconds")
+            coef[what] = coef_of(tau)
         self.attack, self.release = float(attack), float(release)
         self.attack_coef, self.release_coef = coef["attack"], coef["release"]
         self._allocate(*_layout(_cabi.lib().l2h_band_compressor_layout, self.channels, self.bands, self.n_taps), device)
@@ -770,14 +741,10 @@ class BandCompressor(_SlotStage):
         n, C, L = y.shape
         T = L // self.HOP
         slots = device_list(slots, dev, n, self.n_slots, True, "slot")
-        if hops is not None:
-            hops = device_list(hops, dev, n, T + 1, False, "hop")
+        hops = self._hops(hops, n, T)
         out = self._rows_out(out, (n, C, L))
-        with torch.cuda.device(dev):
-            _check(_cabi.lib().l2h_band_compressor(
-                y.data_ptr(), y.stride(0), y.stride(1), out.data_ptr(), out.stride(0), out.stride(1), n, C, T,
-                slots.data_ptr(), None if hops is None else hops.data_ptr(), self.taps.data_ptr(), self.bands,
-                self.n_taps, self.state.data_ptr(), self.n_slots, self.attack_coef, self.release_coef, self._stream()))
+        self._run("l2h_band_compressor", y, y.stride(0), y.stride(1), out, out.stride(0), out.stride(1), n, C, T, slots, hops,
+                  self.taps, self.bands, self.n_taps, self.state, self.n_slots, self.attack_coef, self.release_coef)
         return out
 
     def set_profile(self, slots, gains, knees=0.0, ratios=1.0):
@@ -787,32 +754,29 @@ class BandCompressor(_SlotStage):
         the current stream; it takes effect from the next hop, across one hop's dB ramp, and `reset` returns a slot to
         the flat profile."""
         dev, K, C = self.state.device, self.bands, self.channels
-        idx = torch.as_tensor(slots).cpu().reshape(-1)
-        n = idx.numel()
-        if n < 1:
-            raise ValueError("set_profile needs at least one slot")
-        idx = device_list(idx, dev, n, self.n_slots, True, "slot")
-        g = self._table(gains, "gains", n, [(K,), (n, K), (n, C, K)], lambda v: -self.RANGE <= v <= self.RANGE)
-        kn = self._table(knees, "knees", n, [(), (K,), (n, K)], math.isfinite)
-        ra = self._table(ratios, "ratios", n, [(), (K,), (n, K)], lambda v: v >= 1)
+        rows = self._indices(slots, self.n_slots, "slot", True, "set_profile")
+        n = rows.numel()
+        g = self._table(gains, "gains", n, [(K,), (n, K), (n, C, K)], lambda v: -self.RANGE <= v <= self.RANGE,
+                        f"dB in [{-self.RANGE:g}, {self.RANGE:g}]")
+        kn = self._table(knees, "knees", n, [(), (K,), (n, K)], math.isfinite, "finite dBFS")
+        ra = self._table(ratios, "ratios", n, [(), (K,), (n, K)], lambda v: v >= 1, "ratios >= 1")
         g = (g.reshape(1, 1, K) if g.dim() == 1 else g.reshape(n, -1, K)).expand(n, C, K)
         kn, ra = ((t.expand(K) if t.dim() == 0 else t).reshape(-1, K).expand(n, K) for t in (kn, ra))
-        rows = idx.long()
         self.state[rows, :, :K] = g.float().to(dev)
         self.state[rows, 0, 3 * K:4 * K] = kn.float().to(dev)
         self.state[rows, 0, 4 * K:5 * K] = (1.0 - 1.0 / ra).float().to(dev)
 
     @staticmethod
-    def _table(v, what, n, shapes, ok):
-        """v as a float64 CPU tensor of one of `shapes` whose every entry passes `ok`, or ValueError"""
+    def _table(v, what, n, shapes, ok, must):
+        """v as a float64 CPU tensor of one of `shapes` whose every entry is `must` (passes `ok`), or ValueError"""
         try:
             t = torch.as_tensor(v.detach().cpu() if isinstance(v, torch.Tensor) else v, dtype=torch.float64)
         except (TypeError, ValueError, RuntimeError):
             t = None
         if t is None or tuple(t.shape) not in shapes or isinstance(v, bool):
             raise ValueError(f"{what} must be numbers of shape {' or '.join(str(list(s)) for s in shapes)}, got {v!r}")
-        if not all(ok(x) for x in t.reshape(-1).tolist()):
-            raise ValueError(f"{what} holds a value out of range, got {t.tolist()}")
+        for x in t.reshape(-1).tolist():
+            _real(x, f"every entry of {what}", ok, must)
         return t
 
     @property
