@@ -1,7 +1,8 @@
 """Scaffolding shared by the serving tests (slot lists, multi-hop and ragged slot lists, per-stream clocks, several targets
-per mixture and their groups): fixtures, seeded inputs, state comparisons, the copy / run / copy back oracle, and the
-header parsing of the host-side tests.  Not a test module: each test file imports what it uses, the fixtures by name, so
-`model` is built once per test file.  Fixed-buffer launches go through Net._launch, which names the C entry point."""
+per mixture and their groups) and the per-slot stages: fixtures, seeded inputs, state comparisons, the copy / run / copy
+back oracle, graph replays against eager twins, the 44.1 kHz tick on the separator, and the header parsing of the
+host-side tests.  Not a test module: each test file imports what it uses, the fixtures by name, so `model` is built
+once per test file.  Fixed-buffer launches go through Net._launch, which names the C entry point."""
 import contextlib
 import ctypes
 import os
@@ -11,7 +12,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from lookoncetohear_b200 import Net, SepState, resample, synth
+from lookoncetohear_b200 import HopFifo, Limiter, Net, PacketResampler, SepState, TargetMixer, resample, synth
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HOP, LA = 128, 64
@@ -215,6 +216,119 @@ def warm_groups(net, G, n, K, T, seed, dev):
             for g in sl:
                 fed[g] += T
     return st, fed
+
+
+# ---- one CUDA graph against an eager twin ----------------------------------------------------------------------------
+def captured(fn, warm=None):
+    """a CUDA graph of fn(), captured after one run of warm() (default: fn) on a side stream"""
+    side = torch.cuda.Stream()
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        (warm or fn)()
+    torch.cuda.current_stream().wait_stream(side)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        fn()
+    return graph
+
+
+def refill(bufs):
+    """the float buffers of the dict to SENTINEL and the int buffers to -1, so a sample a replay does not write shows"""
+    for v in bufs.values():
+        v.fill_(SENTINEL) if v.is_floating_point() else v.fill_(-1)
+
+
+def assert_same(got, want, live, twin, where):
+    """the buffers got[k] and want[k] (floats as bits) and the states of the stages live[k] and twin[k] equal"""
+    for k in got:
+        a, b = got[k], want[k]
+        assert torch.equal(bits(a), bits(b)) if a.is_floating_point() else torch.equal(a, b), (where, k)
+    for k in live:
+        assert torch.equal(bits(live[k].state), bits(twin[k].state)), (where, k)
+
+
+# ---- the 44.1 kHz tick on the separator ------------------------------------------------------------------------------
+TICK_S, TICK_T, TICK_N = 4, 2, 3                         # slots, hops per tick, listeners (on slots 0 .. TICK_N - 1)
+TICK_RECS, TICK_OFFSETS = [0, 1, 2, 3], [0, 1, 3, 4]     # listener 1 hears two voices
+
+
+def separator_tick(net, dev, build=None, rows=None, mixed=None, after=None, bufs=None, each=None):
+    """24 ticks of 44.1 kHz packets of 0, 441 or 882 samples (seeds 60 + t) from three listeners: down, FIFO,
+    advance_target_rows, the mixer, up to 44.1 kHz and the limiter, captured in one CUDA graph after a warm-up that
+    pushes nothing (every state stays as it was) and replayed with x and the counts rewritten in place.  After every
+    replay the buffers and every stage's state are bit for bit those of the same chain run eagerly from the same states.
+
+    A test adds its own stages: build(o) adds them to a fresh chain o and sets it up; rows, mixed and after, called as
+    f(o, b, y, slots, rec, off), run them on the separator's rows y, on the mixer's sum b["mix"] and at the end of the
+    tick.  `bufs` gives its extra buffers by name and width (None: an int32 count per listener), and each(b, t) sees
+    the live buffers after every tick's comparison.  Returns the live stages."""
+    S, T, n, C = TICK_S, TICK_T, TICK_N, 2
+    x16, _ = clips(n, 40, 9900, dev)
+    x44 = resample(x16[..., :HOP * 40].reshape(n * C, -1), 16000, 44100).reshape(n, C, -1).contiguous()
+    e = emb(len(TICK_RECS), 9910, dev)
+    widths = {"y16": 320, "oc": None, "chunk": HOP * T + LA, "hops": None, "mix": HOP * T, "y44": 353 * T,
+              "oc44": None, "out": 353 * T, **(bufs or {})}
+
+    def fresh():
+        """[n, C, w] of SENTINEL for a width w, [n] int32 zeros for a width None"""
+        return {k: torch.zeros(n, dtype=torch.int32, device=dev) if w is None else
+                torch.full((n, C, w), SENTINEL, device=dev) for k, w in widths.items()}
+
+    def chain():
+        o = {"down": PacketResampler(44100, 16000, S, C, 882, device=dev), "fifo": HopFifo(S, C, T, 2048, device=dev),
+             "mix": TargetMixer(S, S, C, device=dev), "up": PacketResampler(16000, 44100, S, C, HOP * T, device=dev),
+             "lim": Limiter(S, C, 44100, device=dev)}
+        if build:
+            build(o)
+        return o
+
+    def tick(o, b, st, x, counts, slots, rec, off):
+        o["down"](x, counts, slots, out=b["y16"], out_counts=b["oc"])
+        o["fifo"](b["y16"], b["oc"], slots, out=b["chunk"], hops=b["hops"])
+        y = net.advance_target_rows(b["chunk"], e, st, rec, off, hops=b["hops"])
+        if rows:
+            rows(o, b, y, slots, rec, off)
+        o["mix"](y, rec, off, slots, hops=b["hops"], chunk=b["chunk"], out=b["mix"])
+        if mixed:
+            mixed(o, b, y, slots, rec, off)
+        o["up"](b["mix"], b["hops"], slots, unit=HOP, out=b["y44"], out_counts=b["oc44"])
+        o["lim"](b["y44"], b["oc44"], slots, out=b["out"])
+        if after:
+            after(o, b, y, slots, rec, off)
+
+    def lists():
+        return i32(list(range(n)), dev), i32(TICK_RECS, dev), i32(TICK_OFFSETS, dev)
+
+    live, b = chain(), fresh()
+    st = net.init_buffers(S, dev)
+    x = torch.zeros(n, C, 882, device=dev)
+    counts = i32([0] * n, dev)
+    ls = lists()
+    with torch.no_grad():
+        graph = captured(lambda: tick(live, b, st, x, counts, *ls))
+        torch.cuda.synchronize()
+        twin, st_twin = chain(), copy(net, st)
+        for k in live:
+            twin[k].state.copy_(live[k].state)
+        pos = [0] * n
+        for t in range(24):
+            g = torch.Generator().manual_seed(60 + t)
+            cn = [[0, 441, 882][int(k)] for k in torch.randint(0, 3, (n,), generator=g)]
+            cn = [min(c, x44.shape[-1] - pos[i]) for i, c in enumerate(cn)]
+            x.fill_(0.0)
+            for i in range(n):
+                x[i, :, :cn[i]] = x44[i, :, pos[i]:pos[i] + cn[i]]
+                pos[i] += cn[i]
+            counts.copy_(i32(cn, dev))
+            refill(b)
+            graph.replay()
+            want = fresh()
+            tick(twin, want, st_twin, x, i32(cn, dev), *lists())
+            assert_same(b, want, live, twin, t)
+            if each:
+                each(b, t)
+    torch.cuda.synchronize()
+    return live
 
 
 # ---- the header ------------------------------------------------------------------------------------------------------

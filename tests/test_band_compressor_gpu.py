@@ -11,7 +11,7 @@ import pytest
 import torch
 
 import serving_util as su
-from lookoncetohear_b200 import BandCompressor, HopFifo, Leveler, Limiter, PacketResampler, TargetMixer, resample
+from lookoncetohear_b200 import BandCompressor, Leveler
 from serving_util import HOP, SENTINEL, dev, model  # noqa: F401
 from test_band_compressor_cpu import BANK, model_hop, model_state, set_profile, speech
 
@@ -231,79 +231,18 @@ def test_full_tick_on_the_separator(model, dev):
     """44.1 kHz packets down, FIFO, advance_target_rows, the leveler on the rows, the mixer, the compressor in place on the
     mixer's sum, up to 44.1 kHz and the limiter, all in one captured graph replayed with counts rewritten in place: bit
     for bit the eager chain"""
-    net, _ = model
-    S, T, n = 4, 2, 3
-    recs, offsets = [0, 1, 2, 3], [0, 1, 3, 4]                      # listener 1 hears two voices
-    clips, _ = su.clips(n, 40, 9900, dev)
-    x44 = resample(clips[..., :HOP * 40].reshape(n * C, -1), 16000, 44100).reshape(n, C, -1).contiguous()
-    e = su.emb(len(recs), 9910, dev)
-
-    def chain():
-        o = {"down": PacketResampler(44100, 16000, S, C, 882, device=dev), "fifo": HopFifo(S, C, T, 2048, device=dev),
-             "lev": Leveler(S, C, gate=-90.0, settle=0.04, min_gain=-40.0, device=dev),
-             "mix": TargetMixer(S, S, C, device=dev), "cmp": BandCompressor(S, C, device=dev),
-             "up": PacketResampler(16000, 44100, S, C, HOP * T, device=dev), "lim": Limiter(S, C, 44100, device=dev)}
+    def build(o):
+        o["lev"] = Leveler(su.TICK_S, C, gate=-90.0, settle=0.04, min_gain=-40.0, device=dev)
+        o["cmp"] = BandCompressor(su.TICK_S, C, device=dev)
         o["cmp"].set_profile([0, 1, 2], [[0.0, 4.0, 10.0, 15.0, 8.0]] * 3, knees=-40.0, ratios=[1.5, 2, 2, 2.5, 2])
-        return o
 
-    def bufs():
-        return {"y16": torch.full((n, C, 320), SENTINEL, device=dev), "oc": torch.zeros(n, dtype=torch.int32, device=dev),
-                "chunk": torch.full((n, C, HOP * T + 64), SENTINEL, device=dev),
-                "hops": torch.zeros(n, dtype=torch.int32, device=dev),
-                "mix": torch.full((n, C, HOP * T), SENTINEL, device=dev),
-                "y44": torch.full((n, C, 353 * T), SENTINEL, device=dev),
-                "oc44": torch.zeros(n, dtype=torch.int32, device=dev),
-                "out": torch.full((n, C, 353 * T), SENTINEL, device=dev)}
-
-    def tick(o, b, st, x, counts, slots, rec, off):
-        o["down"](x, counts, slots, out=b["y16"], out_counts=b["oc"])
-        o["fifo"](b["y16"], b["oc"], slots, out=b["chunk"], hops=b["hops"])
-        y = net.advance_target_rows(b["chunk"], e, st, rec, off, hops=b["hops"])
+    def rows(o, b, y, slots, rec, off):
         o["lev"](y, rec, off, hops=b["hops"], out=y)
-        o["mix"](y, rec, off, slots, hops=b["hops"], chunk=b["chunk"], out=b["mix"])
-        o["cmp"](b["mix"], slots, hops=b["hops"], out=b["mix"])
-        o["up"](b["mix"], b["hops"], slots, unit=HOP, out=b["y44"], out_counts=b["oc44"])
-        o["lim"](b["y44"], b["oc44"], slots, out=b["out"])
 
-    live, b = chain(), bufs()
-    st = net.init_buffers(S, dev)
-    x = torch.zeros(n, C, 882, device=dev)
-    slots, counts = su.i32([0, 1, 2], dev), su.i32([0] * n, dev)
-    rec, off = su.i32(recs, dev), su.i32(offsets, dev)
-    with torch.no_grad():
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            tick(live, b, st, x, counts, slots, rec, off)               # nothing pushed: every state stays as it was
-        torch.cuda.current_stream().wait_stream(side)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            tick(live, b, st, x, counts, slots, rec, off)
-        torch.cuda.synchronize()
-        twin, st_twin = chain(), su.copy(net, st)
-        for k in live:
-            twin[k].state.copy_(live[k].state)
-        pos = [0] * n
-        for t in range(24):
-            g = torch.Generator().manual_seed(60 + t)
-            cn = [[0, 441, 882][int(k)] for k in torch.randint(0, 3, (n,), generator=g)]
-            cn = [min(c, x44.shape[-1] - pos[i]) for i, c in enumerate(cn)]
-            x.fill_(0.0)
-            for i in range(n):
-                x[i, :, :cn[i]] = x44[i, :, pos[i]:pos[i] + cn[i]]
-                pos[i] += cn[i]
-            counts.copy_(su.i32(cn, dev))
-            for v in b.values():
-                v.fill_(SENTINEL) if v.is_floating_point() else v.fill_(-1)
-            graph.replay()
-            want = bufs()
-            tick(twin, want, st_twin, x, su.i32(cn, dev), su.i32([0, 1, 2], dev), su.i32(recs, dev),
-                 su.i32(offsets, dev))
-            for k in b:
-                assert torch.equal(su.bits(b[k]), su.bits(want[k])), (t, k)
-            for k in live:
-                assert torch.equal(su.bits(live[k].state), su.bits(twin[k].state)), (t, k)
-    torch.cuda.synchronize()
+    def mixed(o, b, y, slots, rec, off):
+        o["cmp"](b["mix"], slots, hops=b["hops"], out=b["mix"])
+
+    live = su.separator_tick(model[0], dev, build, rows=rows, mixed=mixed)
     assert bool(torch.isfinite(live["cmp"].level[:3]).all()) and float(live["cmp"].gain[:3].abs().max()) > 1
     print(f"\nmixed voices (untrained weights): band levels {live['cmp'].level[:3].tolist()} dBFS, "
           f"gains {live['cmp'].gain[:3, 0].tolist()} dB")

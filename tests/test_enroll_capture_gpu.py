@@ -8,7 +8,7 @@ import torch
 
 from lookoncetohear_b200 import EmbedTFGridNet, EnrollCapture, HopFifo, synth
 from oracle import restate as rs
-from serving_util import bits, dev, i32, model  # noqa: F401
+from serving_util import assert_same, bits, captured, dev, i32, model  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -65,26 +65,18 @@ def test_graph_replay_fifo_then_capture(dev):
     S, C, n, T, max_in, capacity = 6, 2, 4, 3, 400, 900
 
     def pair():
-        return HopFifo(S, C, T, 2048, device=dev), EnrollCapture(S, C, capacity, device=dev)
+        return {"fifo": HopFifo(S, C, T, 2048, device=dev), "cap": EnrollCapture(S, C, capacity, device=dev)}
 
-    def tick(objs, x, counts, slots, chunk, hops):
-        fifo, cap = objs
-        fifo(x, counts, slots, out=chunk, hops=hops)
-        cap(chunk, slots, hops)
+    def tick(o, x, counts, slots, chunk, hops):
+        o["fifo"](x, counts, slots, out=chunk, hops=hops)
+        o["cap"](chunk, slots, hops)
 
     live, twin = pair(), pair()
     x = torch.zeros(n, C, max_in, device=dev)
     counts, slots = i32([0] * n, dev), i32(list(range(n)), dev)
     chunk = torch.zeros(n, C, HOP * T + CARRY, device=dev)
     hops = torch.zeros(n, dtype=torch.int32, device=dev)
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        tick(live, x, counts, slots, chunk, hops)                 # pushes of nothing: the states stay empty
-    torch.cuda.current_stream().wait_stream(side)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        tick(live, x, counts, slots, chunk, hops)
+    graph = captured(lambda: tick(live, x, counts, slots, chunk, hops))   # pushes of nothing: the states stay empty
     g = torch.Generator().manual_seed(90)
     fed = [torch.zeros(C, 0, device=dev) for _ in range(S)]
     for t in range(200):
@@ -101,10 +93,9 @@ def test_graph_replay_fifo_then_capture(dev):
             if 0 <= s < S:
                 fed[s] = torch.cat([fed[s], x[i, :, :m]], 1)
     torch.cuda.synchronize()
-    assert live[0].dropped.sum().item() == 0
-    for a, b in zip(live, twin):
-        assert torch.equal(bits(a.state), bits(b.state))
-    fifo, cap = live
+    fifo, cap = live["fifo"], live["cap"]
+    assert fifo.dropped.sum().item() == 0
+    assert_same({}, {}, live, twin, "after 200 ticks")
     for s in range(S):
         popped = fed[s].shape[1] - int(fifo.held[s])
         k = min(popped, capacity)

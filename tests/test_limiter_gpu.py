@@ -11,7 +11,7 @@ import pytest
 import torch
 
 import serving_util as su
-from lookoncetohear_b200 import HopFifo, Limiter, PacketResampler, TargetMixer, resample
+from lookoncetohear_b200 import Limiter, PacketResampler
 from serving_util import HOP, SENTINEL, dev, model  # noqa: F401
 from test_limiter_cpu import CEILING, cuts, loud, model_push, model_state
 
@@ -211,14 +211,7 @@ def test_graph_replay_with_lists_rewritten(dev):
     x = torch.zeros(n, C, L, device=dev)
     slots, counts = su.i32(list(range(n)), dev), su.i32([0] * n, dev)
     y = torch.full((n, C, L), SENTINEL, device=dev)
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        live(x, counts, slots, out=y)
-    torch.cuda.current_stream().wait_stream(side)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        live(x, counts, slots, out=y)
+    graph = su.captured(lambda: live(x, counts, slots, out=y))
     src = loud_inputs(L * 12, dev)
     for t in range(12):
         g = torch.Generator().manual_seed(50 + t)
@@ -233,8 +226,7 @@ def test_graph_replay_with_lists_rewritten(dev):
         graph.replay()
         want = torch.full_like(y, SENTINEL)
         twin(x, su.i32(cn, dev), su.i32(sl, dev), out=want)
-        assert torch.equal(su.bits(y), su.bits(want)), t
-        assert torch.equal(su.bits(live.state), su.bits(twin.state)), t
+        su.assert_same({"y": y}, {"y": want}, {"lim": live}, {"lim": twin}, t)
 
 
 # ---- 8. the 44.1 kHz tick on the separator --------------------------------------------------------------------------
@@ -242,91 +234,32 @@ def test_full_tick_on_the_separator(model, dev):
     """44.1 kHz packets down, FIFO, advance_target_rows, the mixer at gains up to 16, up to 44.1 kHz and the limiter, all
     in one captured graph replayed with counts rewritten in place: under the ceiling and bit for bit the eager chain.
     It also limits the mixer's 16 kHz output before `up` and reports how far upsampling takes that over the ceiling."""
-    net, _ = model
-    S, T, n = 4, 2, 3
-    recs, offsets = [0, 1, 2, 3], [0, 1, 3, 4]                      # listener 1 hears two voices
-    R = len(recs)
-    clips, _ = su.clips(n, 40, 9900, dev)
-    x44 = resample(clips[..., :HOP * 40].reshape(n * C, -1), 16000, 44100).reshape(n, C, -1).contiguous()
-    e = su.emb(R, 9910, dev)
+    S, T = su.TICK_S, su.TICK_T
+    peak = {"post": 0.0, "pre": 0.0, "played": 0}
 
-    def chain():
-        objs = {"down": PacketResampler(44100, 16000, S, C, 882, device=dev), "fifo": HopFifo(S, C, T, 2048, device=dev),
-                "mix": TargetMixer(S, S, C, device=dev), "up": PacketResampler(16000, 44100, S, C, HOP * T, device=dev),
-                "lim": Limiter(S, C, 44100, device=dev), "lim16": Limiter(S, C, 16000, device=dev),
-                "up16": PacketResampler(16000, 44100, S, C, HOP * T, device=dev)}
-        objs["mix"].set_gains(recs, [16.0, 12.0, 16.0, 4.0])
-        return objs
+    def build(o):
+        o["mix"].set_gains(su.TICK_RECS, [16.0, 12.0, 16.0, 4.0])
+        o["lim16"] = Limiter(S, C, 16000, device=dev)
+        o["up16"] = PacketResampler(16000, 44100, S, C, HOP * T, device=dev)
 
-    def bufs():
-        return {"y16": torch.full((n, C, 320), SENTINEL, device=dev), "oc": torch.zeros(n, dtype=torch.int32, device=dev),
-                "chunk": torch.full((n, C, HOP * T + 64), SENTINEL, device=dev),
-                "hops": torch.zeros(n, dtype=torch.int32, device=dev),
-                "mix": torch.full((n, C, HOP * T), SENTINEL, device=dev),
-                "y44": torch.full((n, C, 353 * T), SENTINEL, device=dev),
-                "oc44": torch.zeros(n, dtype=torch.int32, device=dev),
-                "out": torch.full((n, C, 353 * T), SENTINEL, device=dev),
-                "m16": torch.full((n, C, HOP * T), SENTINEL, device=dev),
-                "pre": torch.full((n, C, 353 * T), SENTINEL, device=dev),
-                "ocp": torch.zeros(n, dtype=torch.int32, device=dev)}
-
-    def tick(o, b, st, x, counts, slots, rec, off):
-        o["down"](x, counts, slots, out=b["y16"], out_counts=b["oc"])
-        o["fifo"](b["y16"], b["oc"], slots, out=b["chunk"], hops=b["hops"])
-        y = net.advance_target_rows(b["chunk"], e, st, rec, off, hops=b["hops"])
-        o["mix"](y, rec, off, slots, hops=b["hops"], chunk=b["chunk"], out=b["mix"])
-        o["up"](b["mix"], b["hops"], slots, unit=HOP, out=b["y44"], out_counts=b["oc44"])
-        o["lim"](b["y44"], b["oc44"], slots, out=b["out"])
-        o["lim16"](b["mix"], b["hops"], slots, unit=HOP, out=b["m16"])          # limiting before `up` instead
+    def after(o, b, y, slots, rec, off):                                    # limiting before `up` instead
+        o["lim16"](b["mix"], b["hops"], slots, unit=HOP, out=b["m16"])
         o["up16"](b["m16"], b["hops"], slots, unit=HOP, out=b["pre"], out_counts=b["ocp"])
 
-    live, b = chain(), bufs()
-    st = net.init_buffers(S, dev)
-    x = torch.zeros(n, C, 882, device=dev)
-    slots, counts = su.i32([0, 1, 2], dev), su.i32([0] * n, dev)
-    rec, off = su.i32(recs, dev), su.i32(offsets, dev)
-    with torch.no_grad():
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            tick(live, b, st, x, counts, slots, rec, off)               # nothing pushed: every state stays as it was
-        torch.cuda.current_stream().wait_stream(side)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            tick(live, b, st, x, counts, slots, rec, off)
-        torch.cuda.synchronize()
-        twin, st_twin = chain(), su.copy(net, st)
-        for k in live:
-            twin[k].state.copy_(live[k].state)
-        pos, over_post, over_pre, played = [0] * n, 0.0, 0.0, 0
-        for t in range(24):
-            g = torch.Generator().manual_seed(60 + t)
-            cn = [[0, 441, 882][int(k)] for k in torch.randint(0, 3, (n,), generator=g)]
-            cn = [min(c, x44.shape[-1] - pos[i]) for i, c in enumerate(cn)]
-            x.fill_(0.0)
-            for i in range(n):
-                x[i, :, :cn[i]] = x44[i, :, pos[i]:pos[i] + cn[i]]
-                pos[i] += cn[i]
-            counts.copy_(su.i32(cn, dev))
-            for v in b.values():
-                v.fill_(SENTINEL) if v.is_floating_point() else v.fill_(-1)
-            graph.replay()
-            want = bufs()
-            tick(twin, want, st_twin, x, su.i32(cn, dev), su.i32([0, 1, 2], dev), su.i32(recs, dev),
-                 su.i32(offsets, dev))
-            for k in b:
-                assert torch.equal(su.bits(b[k]), su.bits(want[k])), (t, k)
-            for k in live:
-                assert torch.equal(su.bits(live[k].state), su.bits(twin[k].state)), (t, k)
-            oc, ocp = b["oc44"].cpu().tolist(), b["ocp"].cpu().tolist()
-            for i in range(n):
-                if oc[i]:
-                    z = b["out"][i, :, :oc[i]]
-                    assert bool(torch.isfinite(z).all()) and float(z.abs().max()) <= CEILING, (t, i)
-                    over_post = max(over_post, float(z.abs().max()))
-                    played += oc[i]
-                if ocp[i]:
-                    over_pre = max(over_pre, float(b["pre"][i, :, :ocp[i]].abs().max()))
-    assert played > 0 and int(live["lim"].limited.sum()) > 0             # the gains of 16 did call for limiting
-    print(f"\n44.1 kHz tick: limiter after up peaks at {20 * math.log10(over_post / CEILING):+.2f} dB re the ceiling; "
-          f"limiting at 16 kHz before up peaks at {20 * math.log10(over_pre / CEILING):+.2f} dB")
+    def each(b, t):
+        oc, ocp = b["oc44"].cpu().tolist(), b["ocp"].cpu().tolist()
+        for i in range(su.TICK_N):
+            if oc[i]:
+                z = b["out"][i, :, :oc[i]]
+                assert bool(torch.isfinite(z).all()) and float(z.abs().max()) <= CEILING, (t, i)
+                peak["post"] = max(peak["post"], float(z.abs().max()))
+                peak["played"] += oc[i]
+            if ocp[i]:
+                peak["pre"] = max(peak["pre"], float(b["pre"][i, :, :ocp[i]].abs().max()))
+
+    live = su.separator_tick(model[0], dev, build, after=after, each=each,
+                             bufs={"m16": HOP * T, "pre": 353 * T, "ocp": None})
+    assert peak["played"] > 0 and int(live["lim"].limited.sum()) > 0     # the gains of 16 did call for limiting
+    post, pre = (20 * math.log10(peak[k] / CEILING) for k in ("post", "pre"))
+    print(f"\n44.1 kHz tick: limiter after up peaks at {post:+.2f} dB re the ceiling; "
+          f"limiting at 16 kHz before up peaks at {pre:+.2f} dB")

@@ -12,6 +12,7 @@ import torch.nn.functional as F
 from lookoncetohear_b200 import HopFifo, PacketResampler, StreamResampler, synth
 from oracle import resample as ors
 from serving_util import SENTINEL as NAN, bits, delayed, dev, i32, model, signals  # noqa: F401
+from serving_util import assert_same, captured, refill
 
 pytestmark = pytest.mark.gpu
 
@@ -151,8 +152,9 @@ def test_graph_replay_with_lists_rewritten_in_place(dev):
     S, C, n, T = 8, 2, 5, 2
 
     def chain():
-        return (PacketResampler(44100, 16000, S, C, 882, device=dev), HopFifo(S, C, T, 1024, device=dev),
-                PacketResampler(16000, 44100, S, C, 128 * T, device=dev))
+        return {"down": PacketResampler(44100, 16000, S, C, 882, device=dev),
+                "fifo": HopFifo(S, C, T, 1024, device=dev),
+                "up": PacketResampler(16000, 44100, S, C, 128 * T, device=dev)}
 
     def bufs():
         return {"y16": torch.full((n, C, 320), NAN, device=dev), "oc": torch.zeros(n, dtype=torch.int32, device=dev),
@@ -160,25 +162,17 @@ def test_graph_replay_with_lists_rewritten_in_place(dev):
                 "hops": torch.zeros(n, dtype=torch.int32, device=dev),
                 "y44": torch.full((n, C, 353 * T), NAN, device=dev), "oc44": torch.zeros(n, dtype=torch.int32, device=dev)}
 
-    def tick(objs, b, x, counts, slots):
-        down, fifo, up = objs
-        down(x, counts, slots, out=b["y16"], out_counts=b["oc"])
-        fifo(b["y16"], b["oc"], slots, out=b["chunk"], hops=b["hops"])
-        up(b["chunk"][..., 64:], b["hops"], slots, unit=128, out=b["y44"], out_counts=b["oc44"])
+    def tick(o, b, x, counts, slots):
+        o["down"](x, counts, slots, out=b["y16"], out_counts=b["oc"])
+        o["fifo"](b["y16"], b["oc"], slots, out=b["chunk"], hops=b["hops"])
+        o["up"](b["chunk"][..., 64:], b["hops"], slots, unit=128, out=b["y44"], out_counts=b["oc44"])
 
     live, twin = chain(), chain()
-    assert live[2].max_out == 353 * T
+    assert live["up"].max_out == 353 * T
     x = torch.zeros(n, C, 882, device=dev)
     counts, slots = i32([0] * n, dev), i32(list(range(n)), dev)
     b = bufs()
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        tick(live, b, x, counts, slots)                          # pushes of nothing: the states stay fresh
-    torch.cuda.current_stream().wait_stream(side)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        tick(live, b, x, counts, slots)
+    graph = captured(lambda: tick(live, b, x, counts, slots))     # pushes of nothing: the states stay fresh
     g = torch.Generator().manual_seed(51)
     for t in range(10):
         sl = torch.randperm(S, generator=g)[:n].tolist()
@@ -187,15 +181,11 @@ def test_graph_replay_with_lists_rewritten_in_place(dev):
         x.copy_(signals(n, C, 882, 60 + t, dev))
         slots.copy_(i32(sl, dev))
         counts.copy_(i32(cn, dev))
-        for v in b.values():
-            v.fill_(NAN) if v.is_floating_point() else v.fill_(-1)
+        refill(b)
         graph.replay()
         want = bufs()
         tick(twin, want, x, i32(cn, dev), i32(sl, dev))
-        for k in b:
-            assert torch.equal(bits(b[k]), bits(want[k])) if b[k].is_floating_point() else torch.equal(b[k], want[k]), (t, k)
-        for a, c in zip(live, twin):
-            assert torch.equal(bits(a.state), bits(c.state)), t
+        assert_same(b, want, live, twin, t)
 
 
 def test_python_call_checks(dev):

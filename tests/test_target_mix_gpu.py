@@ -242,8 +242,9 @@ def test_graph_replay_with_lists_and_sets_rewritten(dev):
     S, C, T, n, NR, R = 6, 2, 2, 4, 10, 7
 
     def chain():
-        return (PacketResampler(44100, 16000, S, C, 882, device=dev), HopFifo(S, C, T, 1024, device=dev),
-                TargetMixer(NR, S, C, device=dev), PacketResampler(16000, 44100, S, C, HOP * T, device=dev))
+        return {"down": PacketResampler(44100, 16000, S, C, 882, device=dev),
+                "fifo": HopFifo(S, C, T, 1024, device=dev), "mix": TargetMixer(NR, S, C, device=dev),
+                "up": PacketResampler(16000, 44100, S, C, HOP * T, device=dev)}
 
     def bufs():
         return {"y16": torch.full((n, C, 320), SENTINEL, device=dev), "oc": torch.zeros(n, dtype=torch.int32, device=dev),
@@ -253,14 +254,13 @@ def test_graph_replay_with_lists_and_sets_rewritten(dev):
                 "y44": torch.full((n, C, 353 * T), SENTINEL, device=dev),
                 "oc44": torch.zeros(n, dtype=torch.int32, device=dev)}
 
-    def tick(objs, b, x, counts, slots, y, rec, off, sets):
-        down, fifo, mix, up = objs
-        mix.set_gains(sets["rows"], sets["gains"], sets["fades"], sets["starts"])
-        mix.set_ambient(sets["slots"], sets["amb"], sets["fades"][:1].contiguous())
-        down(x, counts, slots, out=b["y16"], out_counts=b["oc"])
-        fifo(b["y16"], b["oc"], slots, out=b["chunk"], hops=b["hops"])
-        mix(y, rec, off, slots, hops=b["hops"], chunk=b["chunk"], out=b["mix"])
-        up(b["mix"], b["hops"], slots, unit=HOP, out=b["y44"], out_counts=b["oc44"])
+    def tick(o, b, x, counts, slots, y, rec, off, sets):
+        o["mix"].set_gains(sets["rows"], sets["gains"], sets["fades"], sets["starts"])
+        o["mix"].set_ambient(sets["slots"], sets["amb"], sets["fades"][:1].contiguous())
+        o["down"](x, counts, slots, out=b["y16"], out_counts=b["oc"])
+        o["fifo"](b["y16"], b["oc"], slots, out=b["chunk"], hops=b["hops"])
+        o["mix"](y, rec, off, slots, hops=b["hops"], chunk=b["chunk"], out=b["mix"])
+        o["up"](b["mix"], b["hops"], slots, unit=HOP, out=b["y44"], out_counts=b["oc44"])
 
     def lists(t):
         g = torch.Generator().manual_seed(70 + t)
@@ -284,14 +284,7 @@ def test_graph_replay_with_lists_and_sets_rewritten(dev):
     sets = {"rows": su.i32([-1, -1], dev), "gains": torch.zeros(2, device=dev), "fades": su.i32([0, 0], dev),
             "starts": torch.zeros(2, device=dev), "slots": su.i32([-1], dev), "amb": torch.zeros(1, device=dev)}
     b = bufs()
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        tick(live, b, x, counts, slots, y, rec, off, sets)               # nothing pushed, nothing set: states stay fresh
-    torch.cuda.current_stream().wait_stream(side)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        tick(live, b, x, counts, slots, y, rec, off, sets)
+    graph = su.captured(lambda: tick(live, b, x, counts, slots, y, rec, off, sets))   # nothing pushed or set
     for t in range(12):
         sl, cn, rl, ol, st = lists(t)
         x.copy_(su.signals(n, C, 882, 80 + t, dev))
@@ -301,17 +294,13 @@ def test_graph_replay_with_lists_and_sets_rewritten(dev):
         sets["rows"].copy_(su.i32(st["rows"], dev)); sets["gains"].copy_(torch.tensor(st["gains"]))
         sets["fades"].copy_(su.i32(st["fades"], dev)); sets["starts"].copy_(torch.tensor(st["starts"]))
         sets["slots"].copy_(su.i32(st["slots"], dev)); sets["amb"].copy_(torch.tensor(st["amb"]))
-        for v in b.values():
-            v.fill_(SENTINEL) if v.is_floating_point() else v.fill_(-1)
+        su.refill(b)
         graph.replay()
         want = bufs()
         eager = {k: (su.i32(st[k], dev) if k in ("rows", "fades", "slots") else torch.tensor(st[k], device=dev))
                  for k in st}
         tick(twin, want, x, su.i32(cn, dev), su.i32(sl, dev), y, su.i32(rl, dev), su.i32(ol, dev), eager)
-        for k in b:
-            assert torch.equal(su.bits(b[k]), su.bits(want[k])), (t, k)
-        for a, c in zip(live, twin):
-            assert torch.equal(su.bits(a.state), su.bits(c.state)), t
+        su.assert_same(b, want, live, twin, t)
 
 
 # ---- 6. on the separator ---------------------------------------------------------------------------------------------
