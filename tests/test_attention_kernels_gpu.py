@@ -36,103 +36,31 @@ import pytest
 import torch
 
 from kernels import harness as kh
+from kernels.scaffold import SENTINEL, Guarded, Ledger, Records, bits, dev, is_sentinel, lay, ratio  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
-SENTINEL = 0x7FC0DEAD
-SENSITIVITY = 10.0
 N_BLOCKS, BLK = 2, 1
 BIG = 2 ** 31 + 7
 CLOCKS = ([0, 50, 56, BIG, 111], [1, 48, 49, 55, 57, BIG])      # each set: < 49, the 50 / 56 boundaries, > 2^31
 TOL = {"qkv": 1e-5, "unit": 5e-6, "wide": 6e-5, "attn_out": 2e-5, "ln_frame_res": 1e-5, "chain": 1e-5}
 NF, CH, NH, ATT, RING = kh.NF, kh.CH, kh.NHEAD, kh.ATT, kh.RING
 QK_DIM, QK_LD, V_DIM, FC = kh.QK_DIM, kh.QK_LD, kh.V_DIM, kh.FC
-GUARD = 4096                                                     # sentinel floats after every output buffer
-WORST = {}                                                       # (kernel, regime) -> worst error / bound, for the summary
+LEDGER = Ledger()                                                # keys (kernel, regime); bounds absolute: TOL
 
 
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    kh.lib()
-    return torch.device("cuda", 0)
-
-
-@pytest.fixture(scope="module")
-def lay(dev):
-    return kh.sep_layout(N_BLOCKS)
-
-
-def sentinel(n, dev):
-    return torch.full((n,), SENTINEL, dtype=torch.int32, device=dev).view(torch.float32)
-
-
-def bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def buf(shape, dev):
-    """a sentinel buffer of `shape` followed by GUARD sentinel floats; returns (view, whole)"""
-    n = math.prod(shape)
-    whole = sentinel(n + GUARD, dev)
-    return whole[:n].view(shape), whole
-
-
-def guard_ok(whole):
-    return bool((bits(whole[-GUARD:]) == SENTINEL).all())
-
-
-class State:
+class State(Records):
     """One state of len(clocks) streams and N_BLOCKS blocks, every float the sentinel except the streams' clocks."""
 
     def __init__(self, lay, clocks, dev):
-        self.lay, self.clocks, self.B = lay, list(clocks), len(clocks)
-        self.hdr, self.ss = lay["HEADER_BYTES"] // 4, lay["STREAM_STRIDE"]
-        self.t = sentinel(self.hdr + self.B * self.ss, dev)
-        i64 = self.t.view(torch.int64)
+        super().__init__(lay, len(clocks), dev)
+        self.clocks, self.B = list(clocks), len(clocks)
         for b, c in enumerate(self.clocks):
-            o = self.hdr + b * self.ss + lay["ST_POS"]
-            assert o % 2 == 0
-            i64[o // 2] = c
+            self.pos(b).fill_(c)
 
-    def rec(self, b, t=None):
-        t = self.t if t is None else t
-        return t[self.hdr + b * self.ss:self.hdr + (b + 1) * self.ss]
-
-    def rings(self, b, t=None, blk=BLK):
-        """views K [4][56][584], V [4][56][1552] of stream b's rings in block blk"""
-        r = self.rec(b, t)
-        o = self.lay["ST_BLK"] + blk * self.lay["BK_STRIDE"]
-        k = r[o + self.lay["BK_K"]:o + self.lay["BK_K"] + NH * RING * QK_LD].view(NH, RING, QK_LD)
-        v = r[o + self.lay["BK_V"]:o + self.lay["BK_V"] + NH * RING * V_DIM].view(NH, RING, V_DIM)
-        return k, v
-
-    def gate(self, b):
-        o = self.lay["ST_GATE"]
-        return self.rec(b)[o:o + FC]
-
-
-def unchanged_except(st, before, written):
-    """the state equals `before` bit for bit outside the ring rows written = {(b, slot)} (all heads, K and V)"""
-    exp = before.clone()
-    for b, slot in written:
-        for now, then in zip(st.rings(b), st.rings(b, exp)):
-            then[:, slot] = now[:, slot]
-    return torch.equal(bits(st.t), bits(exp))
-
-
-def check(err, tol, mutants, key):
-    """err within tol; every mutant error >= SENSITIVITY x tol.  Records the worst ratios."""
-    WORST[key] = max(WORST.get(key, 0.0), err / tol)
-    print(f"[{key}] err {err:.2e} = {err / tol:.3f} x bound; mutants / bound: "
-          + ", ".join(f"{m} {e / tol:.0f}" for m, e in mutants.items()))
-    assert err <= tol, (key, err, tol)
-    for m, e in mutants.items():
-        assert e >= SENSITIVITY * tol, (key, m, e, tol)
-
-
-def maxdiff(got, ref):
-    return float((got.double().cpu() - ref).abs().max())
+    def rings(self, b, t=None):
+        """views K [4][56][584], V [4][56][1552] of stream b's rings in block BLK"""
+        return self.ring(b, BLK, "k", t), self.ring(b, BLK, "v", t)
 
 
 # ---- weights ---------------------------------------------------------------------------------------------------------
@@ -188,39 +116,46 @@ def qkv_outputs(st, Q, K, V, T, frame_k, active):
     return q, ring, written
 
 
-def check_qkv(st, before, Q, Qw, K, Kw, V, Vw, T, frame_k, active, refs, tol, key):
-    """assert everything a qkv launch must (and must not) have written; returns the max error against each reference"""
+def qkv_buffers(B, T, dev):
+    """Q [B][4][T][584] and the K, V scratch [B][4][49 + T][584 / 1552] of a T-frame call"""
+    return (Guarded((B, NH, T, QK_LD), dev), Guarded((B, NH, ATT - 1 + T, QK_LD), dev),
+            Guarded((B, NH, ATT - 1 + T, V_DIM), dev))
+
+
+def check_qkv(st, before, Q, K, V, T, frame_k, active, refs, tol, key):
+    """assert everything a qkv launch must (and must not) have written, and its error against each reference"""
     B = st.B
-    q, ring, written = qkv_outputs(st, Q, K, V, T, frame_k, active)
-    assert guard_ok(Qw) and guard_ok(Kw) and guard_ok(Vw)
+    q, ring, written = qkv_outputs(st, Q.t, K.t, V.t, T, frame_k, active)
+    assert Q.ok() and K.ok() and V.ok()
+    K, V = K.t, V.t
     assert bool((bits(q[..., QK_DIM:]) == 0).all()), "Q pad columns"
     assert len(written) == len(ring), "a ring slot written twice"
-    assert unchanged_except(st, before, written), "state written outside the expected ring rows"
+    rows = st.index(*(r[:, slot] for b, slot in written for r in st.rings(b)))
+    assert st.same_outside(rows, before), "state written outside the expected ring rows"
     got = {"q": q[..., :QK_DIM]}
     if T > 1:
         ks = K.view(B, NH, ATT - 1 + T, QK_LD)
         vs = V.view(B, NH, ATT - 1 + T, V_DIM)
-        assert bool((bits(ks[:, :, :ATT - 1]) == SENTINEL).all()) and bool((bits(vs[:, :, :ATT - 1]) == SENTINEL).all()), \
-            "history rows of the scratch written"
+        assert is_sentinel(ks[:, :, :ATT - 1]) and is_sentinel(vs[:, :, :ATT - 1]), "history rows of the scratch written"
         assert bool((bits(ks[:, :, ATT - 1:, QK_DIM:]) == 0).all()), "scratch pad columns"
         got["k"] = ks[:, :, ATT - 1:, :QK_DIM].permute(0, 2, 1, 3).reshape(B * T, NH, QK_DIM)
         got["v"] = vs[:, :, ATT - 1:].permute(0, 2, 1, 3).reshape(B * T, NH, V_DIM)
     else:
-        assert bool((bits(K) == SENTINEL).all()) and bool((bits(V) == SENTINEL).all()), "scratch written by a one-frame call"
+        assert is_sentinel(K) and is_sentinel(V), "scratch written by a one-frame call"
     for _, _, kr, _ in ring:
         assert bool((bits(kr[:, QK_DIM:]) == 0).all()), "ring pad columns"
     idx = [b * T + t for b, t, _, _ in ring]
     errs = {}
     for name, (rq, rk, rv) in refs.items():
-        e = maxdiff(got["q"], rq)
+        e = ratio(got["q"], rq, tol)
         if T > 1:
-            e = max(e, maxdiff(got["k"], rk), maxdiff(got["v"], rv))
+            e = max(e, ratio(got["k"], rk, tol), ratio(got["v"], rv, tol))
         if ring:
-            e = max(e, maxdiff(torch.stack([r[2][:, :QK_DIM] for r in ring]), rk[idx]),
-                    maxdiff(torch.stack([r[3] for r in ring]), rv[idx]))
+            e = max(e, ratio(torch.stack([r[2][:, :QK_DIM] for r in ring]), rk[idx], tol),
+                    ratio(torch.stack([r[3] for r in ring]), rv[idx], tol))
         errs[name] = e
     err = errs.pop("ref")
-    check(err, tol, errs, key)
+    LEDGER.check(key, err, errs)
 
 
 QKV_T = [(1, 0), (1, 5), (2, 0), (49, 0), (50, 0), (51, 0), (70, 0)]
@@ -238,12 +173,10 @@ def test_qkv_kernel(mode, T, frame_k, masked, dev, lay):
     pre = kh.qkv_proj64(X, w.wqkv_t, w.bqkv, w.slopes).float()
     active = torch.tensor([1, 0, 1, 1, 0, 1][:B], dtype=torch.uint8) if masked else None
     st = State(lay, clocks, dev)
-    before = st.t.clone()
-    Q, Qw = buf((B, NH, T, QK_LD), dev)
-    K, Kw = buf((B, NH, ATT - 1 + T, QK_LD), dev)
-    V, Vw = buf((B, NH, ATT - 1 + T, V_DIM), dev)
+    before = st.snapshot()
+    Q, K, V = qkv_buffers(B, T, dev)
     dX, dpre = X.to(dev), pre.to(dev)
-    rc = kh.qkv(w.c, dX, dpre if mode == "pre" else None, Q, K, V, st.t, st.ss, BLK, B, T, frame_k,
+    rc = kh.qkv(w.c, dX, dpre if mode == "pre" else None, Q.t, K.t, V.t, st.t, st.ss, BLK, B, T, frame_k,
                 None if active is None else active.to(dev))
     torch.cuda.synchronize()
     assert rc == 0
@@ -252,7 +185,7 @@ def test_qkv_kernel(mode, T, frame_k, masked, dev, lay):
             "heads_transposed": w.qkv_ref(**src, heads_transposed=True)}
     if mode == "proj":
         refs["swap_qk_slopes"] = w.qkv_ref(**src, swap_qk_slopes=True)
-    check_qkv(st, before, Q, Qw, K, Kw, V, Vw, T, frame_k, active, refs, TOL["qkv"], ("qkv_" + mode, "-"))
+    check_qkv(st, before, Q, K, V, T, frame_k, active, refs, TOL["qkv"], ("qkv_" + mode, "-"))
 
 
 MANY = [(3, 13), (4, 60)]
@@ -274,21 +207,19 @@ def test_qkv_many_kernel(B, T, grid, dev, lay):
     out = []
     for kernel in ("many", "one"):
         st = State(lay, clocks, dev)
-        before = st.t.clone()
-        Q, Qw = buf((B, NH, T, QK_LD), dev)
-        K, Kw = buf((B, NH, ATT - 1 + T, QK_LD), dev)
-        V, Vw = buf((B, NH, ATT - 1 + T, V_DIM), dev)
+        before = st.snapshot()
+        Q, K, V = qkv_buffers(B, T, dev)
         if kernel == "many":
-            rc = kh.qkv_many(w.c, pre.to(dev), Q, K, V, st.t, st.ss, BLK, T, grid, n_frames, dact)
+            rc = kh.qkv_many(w.c, pre.to(dev), Q.t, K.t, V.t, st.t, st.ss, BLK, T, grid, n_frames, dact)
         else:
-            rc = kh.qkv(w.c, None, pre.to(dev), Q, K, V, st.t, st.ss, BLK, B, T, 0, dact)
+            rc = kh.qkv(w.c, None, pre.to(dev), Q.t, K.t, V.t, st.t, st.ss, BLK, B, T, 0, dact)
         torch.cuda.synchronize()
         assert rc == 0
-        out.append((st.t, Qw, Kw, Vw))
+        out.append((st.t, Q.whole, K.whole, V.whole))
         if kernel == "many":
             refs = {"ref": w.qkv_ref(pre=pre), "unbiased": w.qkv_ref(pre=pre, unbiased=True),
                     "heads_transposed": w.qkv_ref(pre=pre, heads_transposed=True)}
-            check_qkv(st, before, Q, Qw, K, Kw, V, Vw, T, 0, active, refs, TOL["qkv"], ("qkv_many", "-"))
+            check_qkv(st, before, Q, K, V, T, 0, active, refs, TOL["qkv"], ("qkv_many", "-"))
     for a, b in zip(*out):
         assert torch.equal(bits(a), bits(b)), "qkv_many_kernel and qkv_kernel differ"
 
@@ -382,12 +313,12 @@ def run_attention(form, hist, st, T, frame_k, dev, scratch=True):
     if T > 1:
         k, v = hist.scratch(T)
         K, V = k.to(dev).contiguous(), v.to(dev).contiguous()
-    Z, Zw = buf((B, T, NF, CH), dev)
-    rc = kh.attention(form, Q, K, V, st.t, st.ss, BLK, Z, B, T, frame_k)
+    Z = Guarded((B, T, NF, CH), dev)
+    rc = kh.attention(form, Q, K, V, st.t, st.ss, BLK, Z.t, B, T, frame_k)
     torch.cuda.synchronize()
     assert rc == 0, (form, T, frame_k)
-    assert guard_ok(Zw)
-    return Z
+    assert Z.ok()
+    return Z.t
 
 
 @pytest.mark.parametrize("regime", ["unit", "wide"])
@@ -402,13 +333,13 @@ def test_attention_ring(form, clocks, frame_k, regime, dev, lay):
     hist = History(cl, 10, regime, seed=300 + frame_k)
     st = State(lay, cl, dev)
     hist.fill_ring(st, lambda b: kh.Ring.window(cl[b] + frame_k))
-    before = st.t.clone()
+    before = st.snapshot()
     Z = run_attention(form, hist, st, 1, frame_k, dev)
-    assert torch.equal(bits(st.t), bits(before)), "state written"
+    assert st.same_outside(st.index(), before), "state written"
     frames = lambda b: [cl[b] + frame_k]
     ref = hist.reference(frames)
-    mut = {m: maxdiff(Z, r) for m, r in hist.mutants(frames, regime).items()}
-    check(maxdiff(Z, ref), TOL[regime], mut, (form + "_ring", regime))
+    mut = {m: ratio(Z, r, TOL[regime]) for m, r in hist.mutants(frames, regime).items()}
+    LEDGER.check((form + "_ring", regime), ratio(Z, ref, TOL[regime]), mut)
     Zs = run_attention(form, hist, st, frame_k + 2, 0, dev)
     assert torch.equal(bits(Zs[:, frame_k]), bits(Z[:, 0])), "ring and scratch forms of one window differ"
 
@@ -427,8 +358,8 @@ def test_attention_scratch(form, T, regime, dev, lay):
     st = State(lay, cl, dev)
     Z = run_attention(form, hist, st, T, 0, dev)
     frames = lambda b: [cl[b] + t for t in range(T)]
-    mut = {m: maxdiff(Z, r) for m, r in hist.mutants(frames, regime).items()}
-    check(maxdiff(Z, hist.reference(frames)), TOL[regime], mut, (form + "_scratch", regime))
+    mut = {m: ratio(Z, r, TOL[regime]) for m, r in hist.mutants(frames, regime).items()}
+    LEDGER.check((form + "_scratch", regime), ratio(Z, hist.reference(frames), TOL[regime]), mut)
 
 
 @pytest.mark.parametrize("T", [2, 70])
@@ -441,16 +372,16 @@ def test_kv_gather(clocks, T, dev, lay):
     hist = History(cl, T + 2, "unit", seed=500 + T)
     st = State(lay, cl, dev)
     hist.fill_ring(st, lambda b: range(cl[b] - ATT + 1, cl[b]), zero_history=False)
-    before = st.t.clone()
-    K, Kw = buf((B, NH, ATT - 1 + T, QK_LD), dev)
-    V, Vw = buf((B, NH, ATT - 1 + T, V_DIM), dev)
-    assert kh.kv_gather(st.t, st.ss, BLK, K, V, B, T) == 0
+    before = st.snapshot()
+    _, K, V = qkv_buffers(B, T, dev)
+    assert kh.kv_gather(st.t, st.ss, BLK, K.t, V.t, B, T) == 0
     torch.cuda.synchronize()
-    assert torch.equal(bits(st.t), bits(before)) and guard_ok(Kw) and guard_ok(Vw)
+    assert st.same_outside(st.index(), before) and K.ok() and V.ok()
+    K, V = K.t, V.t
     rk, rv = hist.scratch(T)
     assert torch.equal(bits(K[:, :, :ATT - 1].cpu()), bits(rk[:, :, :ATT - 1]))
     assert torch.equal(bits(V[:, :, :ATT - 1].cpu()), bits(rv[:, :, :ATT - 1]))
-    assert bool((bits(K[:, :, ATT - 1:]) == SENTINEL).all()) and bool((bits(V[:, :, ATT - 1:]) == SENTINEL).all())
+    assert is_sentinel(K[:, :, ATT - 1:]) and is_sentinel(V[:, :, ATT - 1:])
 
 
 # ---- attn_out_kernel / ln_frame_res_kernel ---------------------------------------------------------------------------
@@ -471,16 +402,16 @@ def test_attention_output(kernel, T, apply_gate, dev, lay):
     st = State(lay, cl, dev)
     if apply_gate:
         for b in range(B):
-            st.gate(b).copy_(gate[b])
-    before = st.t.clone()
-    dX, dXw = buf((B, T, NF, CH), dev)
-    dX.copy_(X)
+            st.gate(b).copy_(gate[b].view(NF, CH))
+    before = st.snapshot()
+    dX = Guarded((B, T, NF, CH), dev, X)
     src = (Z if kernel == "attn_out" else P).to(dev)
     src0 = src.clone()
     fn = kh.attn_out if kernel == "attn_out" else kh.ln_frame_res
-    assert fn(w.c, src, dX, st.t, st.ss, B, T, apply_gate) == 0
+    assert fn(w.c, src, dX.t, st.t, st.ss, B, T, apply_gate) == 0
     torch.cuda.synchronize()
-    assert torch.equal(bits(st.t), bits(before)) and torch.equal(bits(src), bits(src0)) and guard_ok(dXw)
+    assert st.same_outside(st.index(), before) and torch.equal(bits(src), bits(src0)) and dX.ok()
+    dX = dX.t
     gt = gate[:, None].expand(B, T, FC).reshape(B * T, NF, CH) if apply_gate else None
     g64, b64 = w.lnp
 
@@ -493,7 +424,8 @@ def test_attention_output(kernel, T, apply_gate, dev, lay):
     mutants = {"per_bin": ref(per_bin=True), "unbiased": ref(unbiased=True)}
     if apply_gate:
         mutants["gate_first"] = ref(gate_first=True)
-    check(maxdiff(dX, ref()), TOL[kernel], {m: maxdiff(dX, r) for m, r in mutants.items()}, (kernel, f"gate{apply_gate}"))
+    LEDGER.check((kernel, f"gate{apply_gate}"), ratio(dX, ref(), TOL[kernel]),
+                 {m: ratio(dX, r, TOL[kernel]) for m, r in mutants.items()})
 
 
 # ---- a kernel-level hop chain ----------------------------------------------------------------------------------------
@@ -516,21 +448,19 @@ def test_hop_chain_equals_one_call(dev, lay):
     Zh = {f: torch.empty(B, T, NF, CH, device=dev) for f in forms}
     for k in range(T):
         Xk = dX[:, k].contiguous()
-        Qk, _ = buf((B, NH, 1, QK_LD), dev)
+        Qk = Guarded((B, NH, 1, QK_LD), dev).t
         assert kh.qkv(w.c, Xk, None, Qk, None, None, hop.t, hop.ss, BLK, B, 1, k) == 0
         for f in forms:
-            Zk, _ = buf((B, 1, NF, CH), dev)
+            Zk = Guarded((B, 1, NF, CH), dev).t
             assert kh.attention(f, Qk, None, None, hop.t, hop.ss, BLK, Zk, B, 1, k) == 0
             Zh[f][:, k] = Zk[:, 0]
         Qh[:, :, k] = Qk[:, :, 0]
-    Q, _ = buf((B, NH, T, QK_LD), dev)
-    K, _ = buf((B, NH, ATT - 1 + T, QK_LD), dev)
-    V, _ = buf((B, NH, ATT - 1 + T, V_DIM), dev)
+    Q, K, V = (b.t for b in qkv_buffers(B, T, dev))
     assert kh.kv_gather(one.t, one.ss, BLK, K, V, B, T) == 0
     assert kh.qkv(w.c, dX, None, Q, K, V, one.t, one.ss, BLK, B, T, 0) == 0
     Z1 = {}
     for f in forms + ("tile",):
-        Z1[f], _ = buf((B, T, NF, CH), dev)
+        Z1[f] = Guarded((B, T, NF, CH), dev).t
         assert kh.attention(f, Q, K, V, one.t, one.ss, BLK, Z1[f], B, T, 0) == 0
     torch.cuda.synchronize()
     assert torch.equal(bits(Qh), bits(Q))
@@ -552,15 +482,14 @@ def test_hop_chain_equals_one_call(dev, lay):
     frames = lambda b: [cl[b] + t for t in range(T)]
     ref = hist.reference(frames)
     for f in forms + ("tile",):
-        check(maxdiff(Z1[f], ref), TOL["chain"], {"shift": maxdiff(Z1[f], hist.reference(frames, lo=-ATT, hi=-1))},
-              (f + "_chain", "unit"))
+        LEDGER.check((f + "_chain", "unit"), ratio(Z1[f], ref, TOL["chain"]),
+                     {"shift": ratio(Z1[f], hist.reference(frames, lo=-ATT, hi=-1), TOL["chain"])})
 
 
 def test_summary(dev):
     """prints the worst error / bound per kernel and regime over the tests above (run in the same session), and how many
     attn_cluster_kernel CTAs the device holds at once: the engine picks the cluster form while B * T * 4 * 8 fit"""
-    for k, v in sorted(WORST.items()):
-        print(f"worst {k[0]:>20s} {k[1]:>6s}: {v:.3f} x bound")
+    LEDGER.summary()
     resident = kh.lib().kh_attn_cluster_resident()
     sms = torch.cuda.get_device_properties(dev).multi_processor_count
     print(f"attn_cluster_kernel: {resident} resident CTAs on {sms} SMs; the cluster form up to B * T = {resident // 32}")

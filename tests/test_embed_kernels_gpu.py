@@ -8,7 +8,7 @@ einter_mask_kernel and eput_lens_kernel run through tests/kernels/kernel_harness
 einter_mask_expected) restate the model (tfgridnet.py:100-127, espnet2's GridNet block) for one utterance of its own
 length; a CPU test pins them to oracle/restate.py.  Every float a kernel must not read or write holds a NaN sentinel:
 x past each utterance's length, the DFT table's two pad columns, Q/K/V rows T .. Tp-1, O rows t >= T, HD rows
-t >= T_b, the guard floats after every buffer.  Padded frames a kernel must leave alone must survive bit for bit.
+t >= T_b, the guard floats around every buffer.  Padded frames a kernel must leave alone must survive bit for bit.
 
 Bounds (element-wise, computed by the references; u = 2^-24): estd one fp32 rounding of a double result; efront the
 128-term DFT (plus the fp32 table and the scaled sample, u (sqrt(128) + 2)) carried through the 36-term conv plus bias
@@ -36,28 +36,18 @@ import pytest
 import torch
 
 from kernels import harness as kh
+from kernels.scaffold import Guarded, Ledger, bits, dev, is_sentinel, ratio, sentinel  # noqa: F401
 from lookoncetohear_b200 import EmbedTFGridNet, _cabi, synth
 from lookoncetohear_b200.configs import EMBED_PARAMS
 from oracle import restate as rs
 
 pytestmark = pytest.mark.gpu
 
-SENTINEL = 0x7FC0DEAD
-SENSITIVITY = 10.0
-GUARD = 1024
 NF, CH, FC, NH, QK, VDIM, HOP = kh.E_NF, kh.E_CH, kh.E_FC, kh.E_NH, kh.E_QK, kh.E_VDIM, kh.E_HOP
 # mixed lengths: the shortest (T_b = 4: one inter window), 255, 256, 64 k + 63, the longest (not first)
 LENS_MIXED = [1343, 192, 4000, 255, 256]
 CASES = {"mixed": (LENS_MIXED, max(LENS_MIXED)), "equal": (None, 1100)}      # equal: N not a multiple of 64
-WORST = {}                                                                   # kernel -> worst error / bound
-MARGIN = {}                                                                  # kernel -> smallest mutant error / bound
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    kh.lib()
-    return torch.device("cuda", 0)
+LEDGER = Ledger()
 
 
 @pytest.fixture(scope="module")
@@ -68,46 +58,7 @@ def w(dev):
 @pytest.fixture(scope="module", autouse=True)
 def summary():
     yield
-    print("\n[embed kernels] worst error / bound: " + ", ".join(f"{k} {v:.3f}" for k, v in sorted(WORST.items())))
-    print("[embed kernels] smallest mutant error / bound: " + ", ".join(f"{k} {v:.3g}" for k, v in sorted(MARGIN.items())))
-
-
-def sentinel(n, dev):
-    return torch.full((n,), SENTINEL, dtype=torch.int32, device=dev).view(torch.float32)
-
-
-def bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def buf(shape, dev):
-    """a sentinel buffer of `shape` followed by GUARD sentinel floats; returns (view, whole)"""
-    n = math.prod(shape)
-    whole = sentinel(n + GUARD, dev)
-    return whole[:n].view(shape), whole
-
-
-def guard_ok(whole):
-    return bool((bits(whole[-GUARD:]) == SENTINEL).all())
-
-
-def ratio(got, ref, bound):
-    """max |got - ref| / bound (an exact value has bound 0: any difference is infinitely far outside)"""
-    d = (got.double().cpu() - ref.double()).abs()
-    r = d / bound.double().clamp_min(1e-300)
-    r[d == 0] = 0
-    return float(r.max()) if r.numel() else 0.0
-
-
-def check(key, err, mutants):
-    """err (error / bound) <= 1; every mutant's error / bound >= SENSITIVITY.  Records the worst ratios."""
-    WORST[key] = max(WORST.get(key, 0.0), err)
-    if mutants:
-        MARGIN[key] = min([MARGIN.get(key, math.inf)] + list(mutants.values()))
-    print(f"[{key}] err {err:.3f} x bound; mutants / bound: " + ", ".join(f"{m} {e:.3g}" for m, e in mutants.items()))
-    assert err <= 1.0, (key, err)
-    for m, e in mutants.items():
-        assert e >= SENSITIVITY, (key, m, e)
+    LEDGER.summary()
 
 
 def lens_dev(lens, dev):
@@ -166,17 +117,18 @@ def test_estd(case, dev):
     lens, N = CASES[case]
     x, xd = signal(lens, N, dev, 10)
     B = x.shape[0]
-    inv, whole = buf((B,), dev)
-    assert kh.estd(xd, N, lens_dev(lens, dev), inv, B) == 0
+    inv = Guarded((B,), dev)
+    assert kh.estd(xd, N, lens_dev(lens, dev), inv.t, B) == 0
     torch.cuda.synchronize()
-    assert guard_ok(whole)
+    assert inv.ok()
+    inv = inv.t
     err, mut = 0.0, {"biased": 0.0, "mic0": 0.0}
     for b, n in enumerate(own(lens, N, B)):
         ref, bound = kh.estd64(x[b], n)
         err = max(err, ratio(inv[b:b + 1], ref.view(1), bound.view(1)))
         mut["biased"] = max(mut["biased"], ratio(inv[b:b + 1], kh.estd64(x[b], n, unbiased=False)[0].view(1), bound.view(1)))
         mut["mic0"] = max(mut["mic0"], ratio(inv[b:b + 1], kh.estd64(x[b], n, mic0_only=True)[0].view(1), bound.view(1)))
-    check("estd", err, mut)
+    LEDGER.check("estd", err, mut)
 
 
 @pytest.mark.parametrize("case", list(CASES))
@@ -187,12 +139,13 @@ def test_efront(case, dev, w):
     x, xd = signal(lens, N, dev, 11)
     B, T = x.shape[0], kh.e_frames(N)
     inv = torch.stack([kh.estd64(x[b], n)[0] for b, n in enumerate(own(lens, N, B))]).float()
-    X, whole = buf((B, T, NF, CH), dev)
+    X = Guarded((B, T, NF, CH), dev)
     gn = torch.zeros(2 * B + 2, dtype=torch.float64, device=dev)
     gn[2 * B:] = float("nan")
-    assert kh.efront(w.c, xd, N, lens_dev(lens, dev), inv.to(dev), X, gn, B, T) == 0
+    assert kh.efront(w.c, xd, N, lens_dev(lens, dev), inv.to(dev), X.t, gn, B, T) == 0
     torch.cuda.synchronize()
-    assert guard_ok(whole) and bool(gn[2 * B:].isnan().all())
+    assert X.ok() and bool(gn[2 * B:].isnan().all())
+    X = X.t
     muts = dict(edge_repeat=dict(edge_repeat=True), reflect_at_N=dict(reflect_at=N), symmetric_hann=dict(symmetric_hann=True),
                 reim_interleaved=dict(reim_interleaved=True), conv_flip_time=dict(conv_flip_time=True))
     err, errs, mut = 0.0, 0.0, {k: 0.0 for k in muts}
@@ -206,8 +159,8 @@ def test_efront(case, dev, w):
             mut[k] = max(mut[k], ratio(X[b], kh.efront64(x[b], n, T, inv[b], w.Wc, bc, **m)["X"], ref["X_bound"]))
     if lens is None:
         del mut["reflect_at_N"]                        # the same thing on the equal-length path
-    check("efront", err, mut)
-    check("efront GN sums", errs, {})
+    LEDGER.check("efront", err, mut)
+    LEDGER.check("efront GN sums", errs, {})
 
 
 @pytest.mark.parametrize("case", list(CASES))
@@ -223,11 +176,11 @@ def test_egn_apply(case, dev, w):
     for b, n in enumerate(own(lens, N, B)):
         r = X0[b, :kh.e_frames(n)].double()
         sums[2 * b], sums[2 * b + 1] = r.sum(), (r * r).sum()
-    X, whole = buf((B, T, NF, CH), dev)
-    X.copy_(X0.to(dev))
-    assert kh.egn_apply(w.c, X, sums.to(dev), T * FC, total4, lens_dev(lens, dev)) == 0
+    X = Guarded((B, T, NF, CH), dev, X0)
+    assert kh.egn_apply(w.c, X.t, sums.to(dev), T * FC, total4, lens_dev(lens, dev)) == 0
     torch.cuda.synchronize()
-    assert guard_ok(whole)
+    assert X.ok()
+    X = X.t
     err, mut = 0.0, {"padded_count": 0.0, "unbiased": 0.0}
     for b, n in enumerate(own(lens, N, B)):
         Tb = kh.e_frames(n)
@@ -239,7 +192,7 @@ def test_egn_apply(case, dev, w):
             mut[k] = max(mut[k], ratio(X[b], m, bound))
     if lens is None:
         del mut["padded_count"]
-    check("egn_apply", err, mut)
+    LEDGER.check("egn_apply", err, mut)
 
 
 # ---- eqkv_ln ---------------------------------------------------------------------------------------------------------
@@ -248,15 +201,15 @@ def test_eqkv_ln(B, T, Tp, dev, w):
     g = torch.Generator().manual_seed(13 + T)
     QKV = torch.randn(B, T, NF, kh.E_NQKV, generator=g) * 1.3 + 0.2
     Z = B * NH
-    Qn, qw = buf((Z, Tp, QK), dev)
     k_plane, v_plane = Z * Tp * QK, Z * Tp * VDIM
-    Kf, kw = buf((k_plane,), dev)                  # two bf16 planes = one float per element
-    Vf, vw = buf((v_plane,), dev)
-    Kp, Vp = Kf.view(torch.bfloat16).view(2, Z, Tp, QK), Vf.view(torch.bfloat16).view(2, Z, Tp, VDIM)
+    Qg = Guarded((Z, Tp, QK), dev)
+    Kg, Vg = Guarded((k_plane,), dev), Guarded((v_plane,), dev)         # two bf16 planes = one float per element
+    Qn = Qg.t
+    Kp, Vp = Kg.t.view(torch.bfloat16).view(2, Z, Tp, QK), Vg.t.view(torch.bfloat16).view(2, Z, Tp, VDIM)
     assert kh.eqkv_ln(w.cb, QKV.to(dev), Qn, Kp, Vp, k_plane, v_plane, B, T, Tp) == 0
     torch.cuda.synchronize()
-    assert guard_ok(qw) and guard_ok(kw) and guard_ok(vw)
-    assert bool((bits(Qn[:, T:]) == SENTINEL).all())
+    assert Qg.ok() and Kg.ok() and Vg.ok()
+    assert is_sentinel(Qn[:, T:])
     for P, n in ((Kp, QK), (Vp, VDIM)):                            # rows T .. Tp-1 of both planes keep the sentinel
         fresh = sentinel(P.numel() // 2, dev).view(torch.int16).view(P.shape)
         assert torch.equal(P.view(torch.int16)[:, :, T:], fresh[:, :, T:])
@@ -282,7 +235,7 @@ def test_eqkv_ln(B, T, Tp, dev, w):
             for k in muts:
                 mut[k] = max(mut[k], ratio(got[name], mrefs[k][name][0], bound))
     for name in "QKV":
-        check(f"eqkv_ln {name}", errs[name], mut if name == "V" else {})
+        LEDGER.check(f"eqkv_ln {name}", errs[name], mut if name == "V" else {})
 
 
 # ---- softmax_rows ----------------------------------------------------------------------------------------------------
@@ -303,17 +256,17 @@ def test_softmax_rows(case, dev):
     Z = B * NH
     g = torch.Generator().manual_seed(14)
     S0 = (torch.rand(Z * T, Tp, generator=g) * 2 - 1) * scale if scale > 10 else scale * torch.randn(Z * T, Tp, generator=g)
-    S, whole = buf((Z * T, Tp), dev)
-    S.copy_(S0.to(dev))
-    assert kh.softmax_rows(S, Tp, T, T, T * Tp, Z, lens_dev(lens, dev)) == 0
+    S = Guarded((Z * T, Tp), dev, S0)
+    assert kh.softmax_rows(S.t, Tp, T, T, T * Tp, Z, lens_dev(lens, dev)) == 0
     torch.cuda.synchronize()
-    assert guard_ok(whole)
+    assert S.ok()
+    S = S.t
     ncols = kh.softmax_row_lens(Z, T, lens, T)
     ref, bound = kh.softmax64(S0, ncols)
     mut = {"pad_not_zeroed": ratio(S, kh.softmax64(S0, ncols, zero_pad=False)[0], bound)}
     if lens is not None:
         mut["len_z_mod_NH"] = ratio(S, kh.softmax64(S0, kh.softmax_row_lens(Z, T, lens, T, by_mod=True))[0], bound)
-    check("softmax_rows", ratio(S, ref, bound), mut)
+    LEDGER.check("softmax_rows", ratio(S, ref, bound), mut)
 
 
 # ---- eattn_out -------------------------------------------------------------------------------------------------------
@@ -329,13 +282,12 @@ def test_eattn_out(B, T, Tp, grid, dev, w):
     g = torch.Generator().manual_seed(15 + T)
     O0 = torch.randn(B, NH, T, VDIM, generator=g)
     X0 = torch.randn(B, T, NF, CH, generator=g)
-    O, ow = buf((B, NH, Tp, VDIM), dev)
-    O[:, :, :T] = O0.to(dev)
-    X, xw = buf((B, T, NF, CH), dev)
-    X.copy_(X0.to(dev))
-    assert kh.eattn_out(w.cb, O, X, T, Tp, T * B, grid) == 0
+    O, X = Guarded((B, NH, Tp, VDIM), dev), Guarded((B, T, NF, CH), dev, X0)
+    O.t[:, :, :T] = O0.to(dev)
+    assert kh.eattn_out(w.cb, O.t, X.t, T, Tp, T * B, grid) == 0
     torch.cuda.synchronize()
-    assert guard_ok(ow) and guard_ok(xw)
+    assert O.ok() and X.ok()
+    X = X.t
     a = [w.b(k) for k in ("wp_t", "bp", "slope_p", "gp", "bpn")]
     muts = dict(heads_cf=dict(heads_cf=True), ignore_slope=dict(ignore_slope=True), ln_per_bin=dict(ln_per_bin=True))
     err, mut = 0.0, {k: 0.0 for k in muts}
@@ -345,7 +297,7 @@ def test_eattn_out(B, T, Tp, grid, dev, w):
         err = max(err, ratio(X[b], ref, bound))
         for k, m in muts.items():
             mut[k] = max(mut[k], ratio(X[b], kh.eattn_out64(Ob, X0[b], *a, **m)[0], bound))
-    check("eattn_out", err, mut)
+    LEDGER.check("eattn_out", err, mut)
 
 
 # ---- ehead -----------------------------------------------------------------------------------------------------------
@@ -362,10 +314,11 @@ def test_ehead(case, dev, w):
     HDd = HD0.clone()
     for b, n in enumerate(own(lens, N, B)):
         HDd[b, kh.e_frames(n):] = float("nan")                       # never read
-    out, whole = buf((B, 256), dev)
-    assert kh.ehead(w.c, HDd.to(dev), out, B, T, lens_dev(lens, dev)) == 0
+    out = Guarded((B, 256), dev)
+    assert kh.ehead(w.c, HDd.to(dev), out.t, B, T, lens_dev(lens, dev)) == 0
     torch.cuda.synchronize()
-    assert guard_ok(whole)
+    assert out.ok()
+    out = out.t
     err, mut = 0.0, {"div_T": 0.0, "mean_before_ln": 0.0}
     for b, n in enumerate(own(lens, N, B)):
         Tb = kh.e_frames(n)
@@ -375,7 +328,7 @@ def test_ehead(case, dev, w):
             mut[k] = max(mut[k], ratio(out[b], kh.ehead64(HD0[b], Tb, w.p["lnh_g"], w.p["lnh_b"], **{k: True})[0], bound))
     if lens is None:
         del mut["div_T"]
-    check("ehead", err, mut)
+    LEDGER.check("ehead", err, mut)
 
 
 # ---- einter_mask, eput_lens ------------------------------------------------------------------------------------------
@@ -386,31 +339,31 @@ def test_einter_mask(dev):
     B = len(lens)
     g = torch.Generator().manual_seed(17)
     gx0 = torch.randn(B * NF, steps, 512, generator=g)
-    gx, whole = buf((B * NF, steps, 512), dev)
-    gx.copy_(gx0.to(dev))
-    assert kh.einter_mask(gx, lens_dev(lens, dev), B, steps) == 0
+    gx = Guarded((B * NF, steps, 512), dev, gx0)
+    assert kh.einter_mask(gx.t, lens_dev(lens, dev), B, steps) == 0
     torch.cuda.synchronize()
-    assert guard_ok(whole)
-    got = gx.cpu()
+    assert gx.ok()
+    got = gx.t.cpu()
     ref = kh.einter_mask_expected(gx0, lens, steps)
     assert torch.equal(bits(got), bits(ref))
     ilong = lens.index(N)
     assert torch.equal(bits(got.view(B, NF, -1)[ilong]), bits(gx0.view(B, NF, -1)[ilong]))
     for m in (dict(start=4), dict(start=2), dict(fwd_only=True), dict(pad=(float("-inf"), 0.0, float("-inf"), 0.0))):
         assert not torch.equal(bits(got), bits(kh.einter_mask_expected(gx0, lens, steps, **m))), m
-    check("einter_mask", 0.0, {"start_Tb-4": math.inf, "start_Tb-2": math.inf, "fwd_only": math.inf, "gate_order": math.inf})
+    LEDGER.check("einter_mask", 0.0, {"start_Tb-4": math.inf, "start_Tb-2": math.inf, "fwd_only": math.inf,
+                                      "gate_order": math.inf})
 
 
 @pytest.mark.parametrize("n", [1, 1000, 1001])
 def test_eput_lens(n, dev):
     lens = [192 + 37 * i for i in range(n)]
-    dst = torch.full((n + 64,), SENTINEL, dtype=torch.int32, device=dev)
+    dst = Guarded((n,), dev)
     n0 = kh.lib().kh_launch_count()
-    assert kh.eput_lens(dst, lens, n) == 0
+    assert kh.eput_lens(dst.t, lens, n) == 0
     torch.cuda.synchronize()
     assert kh.lib().kh_launch_count() - n0 == (n + kh.E_LENS_PER_LAUNCH - 1) // kh.E_LENS_PER_LAUNCH
-    assert dst[:n].cpu().tolist() == lens
-    assert bool((dst[n:] == SENTINEL).all())
+    assert bits(dst.t).cpu().tolist() == lens
+    assert dst.ok()
 
 
 # ---- the -inf premise on the recurrences -----------------------------------------------------------------------------
@@ -431,7 +384,7 @@ def test_masked_windows_leave_zero_state(variant, passes, dev):
 
     def run(gx_, nseq, steps):
         gd = gx_.contiguous().to(dev)
-        out = torch.full((nseq, steps, 128), SENTINEL, dtype=torch.int32, device=dev).view(torch.float32)
+        out = sentinel(nseq * steps * 128, dev).view(nseq, steps, 128)
         a = kh.Lstm()
         a.gx, a.gx_ld, a.out, a.out_ld, a.whh = gd.data_ptr(), 512, out.data_ptr(), 128, whh.data_ptr()
         a.nseq, a.L, a.inner_count, a.ndir = nseq, steps, 1, 2

@@ -36,21 +36,18 @@ group form), 0.34 (front_many_kernel), 0.10 (front1_kernel X) and 0.17 (its GX),
 unbiased variance, which moves a value by only |LN| / 12416); every other mutant misses by more than 3500x.
 """
 import math
-import subprocess
 
 import pytest
 import torch
 
 from kernels import harness as kh
+from kernels.scaffold import SENTINEL, Guarded, Ledger, Records, bits, dev, is_sentinel, lay, ratio  # noqa: F401
 from lookoncetohear_b200.configs import TSH_PARAMS
 
 pytestmark = pytest.mark.gpu
 
-SENTINEL = 0x7FC0DEAD
-SENSITIVITY = 10.0
 N_BLOCKS = 2
-GUARD = 4096
-NF, CH, FC, HOP, NROW, SPK = kh.NF, kh.CH, kh.FC, kh.HOP, kh.NROW, kh.SPK
+NF, CH, FC, HOP, SPK = kh.NF, kh.CH, kh.FC, kh.HOP, kh.SPK
 GEN = 5
 # per stream: frames consumed, calls (bit 0 = parity of the tails it reads), speaker-gate memo key
 STREAMS = [dict(pos=0, calls=0, memo="nan"),              # a fresh stream: zero tails
@@ -61,65 +58,12 @@ STREAMS = [dict(pos=0, calls=0, memo="nan"),              # a fresh stream: zero
 MASK = [1, 1, 0, 1, 0]
 HDR_POS, HDR_CALLS = 40, 9
 CLIPS = {"abs": (0, 0), "rel0": (1, 0), "rel37": (1, 37)}          # (pos_rel, header pos - clip_base)
-WORST = {}                                                          # kernel -> worst error / bound, for the summary
-MARGIN = {}                                                         # kernel -> smallest mutant error / bound
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    kh.lib()
-    return torch.device("cuda", 0)
-
-
-@pytest.fixture(scope="module")
-def lay(dev):
-    return kh.sep_layout(N_BLOCKS)
+LEDGER = Ledger()
 
 
 @pytest.fixture(scope="module")
 def w(dev):
     return Weights(dev)
-
-
-def sentinel(n, dev):
-    return torch.full((n,), SENTINEL, dtype=torch.int32, device=dev).view(torch.float32)
-
-
-def bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def buf(shape, dev):
-    """a sentinel buffer of `shape` followed by GUARD sentinel floats; returns (view, whole)"""
-    n = math.prod(shape)
-    whole = sentinel(n + GUARD, dev)
-    return whole[:n].view(shape), whole
-
-
-def guard_ok(whole):
-    return bool((bits(whole[-GUARD:]) == SENTINEL).all())
-
-
-def is_sentinel(t):
-    return bool((bits(t) == SENTINEL).all())
-
-
-def ratio(got, ref, bound):
-    """max |got - ref| / bound (an exact value has bound 0: any difference is infinitely far outside)"""
-    d = (got.double().cpu() - ref).abs()
-    return float((d / bound.clamp_min(1e-300)).max())
-
-
-def check(key, err, mutants):
-    """err (error / bound) <= 1; every mutant's error / bound >= SENSITIVITY.  Records the worst ratios."""
-    WORST[key] = max(WORST.get(key, 0.0), err)
-    if mutants:
-        MARGIN[key] = min([MARGIN.get(key, math.inf)] + list(mutants.values()))
-    print(f"[{key}] err {err:.3f} x bound; mutants / bound: " + ", ".join(f"{m} {e:.0f}" for m, e in mutants.items()))
-    assert err <= 1.0, (key, err)
-    for m, e in mutants.items():
-        assert e >= SENSITIVITY, (key, m, e)
 
 
 # ---- weights ---------------------------------------------------------------------------------------------------------
@@ -162,18 +106,17 @@ class Weights:
 
 
 # ---- state -----------------------------------------------------------------------------------------------------------
-class State:
+class State(Records):
     """One state of B streams (STREAMS cycled, positions spread) and N_BLOCKS blocks, every float the sentinel except
     the header, the streams' clocks, tails (both parity copies, different data; zero for a fresh stream) and gate memo
     keys.  rel = header pos - clip_base."""
 
     def __init__(self, lay, B, dev, rel, emb, seed):
-        self.lay, self.B, self.dev = lay, B, dev
-        self.hdr, self.ss = lay["HEADER_BYTES"] // 4, lay["STREAM_STRIDE"]
-        self.t = sentinel(self.hdr + B * self.ss, dev)
-        i64, i32 = self.t.view(torch.int64), self.t.view(torch.int32)
+        super().__init__(lay, B, dev)
+        self.B = B
+        i64 = self.t.view(torch.int64)
         i64[0], i64[1], i64[2] = HDR_POS, HDR_CALLS, HDR_POS - rel
-        i32[6] = 0                                                  # done: the last-CTA counter
+        self.t.view(torch.int32)[6] = 0                             # done: the last-CTA counter
         g = torch.Generator().manual_seed(seed)
         self.streams = []
         for b in range(B):
@@ -181,9 +124,8 @@ class State:
             if s["pos"] and b >= len(STREAMS):
                 s["pos"] += 1000 * b                                # never the header's pos
             self.streams.append(s)
-            o = self.hdr + b * self.ss
-            i64[(o + lay["ST_POS"]) // 2] = s["pos"]
-            i32[o + lay["ST_CALLS"]] = s["calls"]
+            self.pos(b).fill_(s["pos"])
+            self.calls(b).fill_(s["calls"])
             fresh = s["calls"] == 0
             for view, scale in ((self.conv(b), 1.5), (self.deconv(b), 0.7), (self.istft(b), 1.5)):
                 v = torch.zeros(view.shape) if fresh else scale * torch.randn(view.shape, generator=g)
@@ -192,31 +134,8 @@ class State:
             if s["memo"] != "nan":
                 if s["memo"] == "elem":
                     e[77] += 0.5
-                self.rec(b)[lay["ST_EMB"]:lay["ST_EMB"] + SPK] = e.to(dev)
-                i32[o + lay["ST_GEN"]] = GEN - 1 if s["memo"] == "gen" else GEN
-
-    def rec(self, b, t=None):
-        t = self.t if t is None else t
-        return t[self.hdr + b * self.ss:self.hdr + (b + 1) * self.ss]
-
-    def _f(self, b, name, shape, t=None):
-        o = self.lay[name]
-        return self.rec(b, t)[o:o + math.prod(shape)].view(shape)
-
-    def conv(self, b, t=None):
-        return self._f(b, "ST_CONV", (2, 2, 4, NF), t)
-
-    def deconv(self, b, t=None):
-        return self._f(b, "ST_DECONV", (2, 2, NF, CH), t)
-
-    def istft(self, b, t=None):
-        return self._f(b, "ST_ISTFT", (2, 2, NROW), t)
-
-    def gate(self, b, t=None):
-        return self._f(b, "ST_GATE", (NF, CH), t)
-
-    def emb(self, b, t=None):
-        return self._f(b, "ST_EMB", (SPK,), t)
+                self.emb(b).copy_(e.to(dev))
+                self.gen(b).fill_(GEN - 1 if s["memo"] == "gen" else GEN)
 
     def par(self, b):
         return self.streams[b]["calls"] & 1
@@ -226,21 +145,16 @@ class State:
         i64 = t[:self.hdr].view(torch.int64)
         return int(i64[0]), int(i64[1]), int(i64[2]), int(t[:self.hdr].view(torch.int32)[6])
 
-    def clock(self, b, t=None):
-        r = self.rec(b, t)
-        return int(r[self.lay["ST_POS"]:self.lay["ST_POS"] + 2].view(torch.int64)[0]), int(r.view(torch.int32)[self.lay["ST_CALLS"]])
-
     def advance(self, t, T, active):
         """t with the header and every active stream's clock advanced by one call of T frames (finish_call)"""
         t = t.clone()
-        i64, i32 = t.view(torch.int64), t.view(torch.int32)
+        i64 = t.view(torch.int64)
         i64[0] += T
         i64[1] += 1
         for b in range(self.B):
             if active is None or active[b]:
-                o = self.hdr + b * self.ss
-                i64[(o + self.lay["ST_POS"]) // 2] += T
-                i32[o + self.lay["ST_CALLS"]] += 1
+                self.pos(b, t)[0] += T
+                self.calls(b, t)[0] += 1
         return t
 
 
@@ -267,12 +181,10 @@ class Inputs:
 
 
 # ---- checks ----------------------------------------------------------------------------------------------------------
-def check_front(key, w, st, before, inp, T, X, Xw, prew, frame_rows=None):
-    """X (rows frame_rows of a group, or the whole call) against front64 and its mutants for every stream, active or not;
-    the new conv tail of each active stream; the gate memo; and nothing else of the state written.  Returns the state the
-    launch must have left (bits), for equality checks."""
-    assert guard_ok(Xw) and guard_ok(prew)
-    exp = before.clone()
+def check_front(key, w, st, before, inp, T, X):
+    """X against front64 and its mutants for every stream, active or not; the new conv tail of each active stream; the
+    gate memo; and nothing else of the state written"""
+    exp, written = before.clone(), []
     err, muts = 0.0, {}
 
     def mut(name, r):
@@ -296,28 +208,26 @@ def check_front(key, w, st, before, inp, T, X, Xw, prew, frame_rows=None):
         if inp.live(b):
             got = st.conv(b)[par ^ 1]
             err = max(err, ratio(got, ref["tail"], ref["tail_bound"]))
-            st.conv(b, exp)[par ^ 1] = got
+            written.append(got)
             if s["memo"] != "match":
                 g, gb = w.gate(inp.emb[b])
                 got = st.gate(b)
                 e = ratio(got, g, gb)
                 gm = {"cf_order": ratio(got, w.gate(inp.emb[b], cf_order=True)[0], gb),
                       "unbiased": ratio(got, w.gate(inp.emb[b], unbiased=True)[0], gb)}
-                check("gate", e, gm)
-                st.gate(b, exp).copy_(got)
+                LEDGER.check("gate", e, gm)
+                written.append(got)
                 st.emb(b, exp).copy_(inp.demb[b])
-                st.rec(b, exp).view(torch.int32)[st.lay["ST_GEN"]] = GEN
-    check(key, err, muts)
-    assert torch.equal(bits(st.t), bits(exp)), "state written outside the new conv tails and the rebuilt gates"
-    return exp
+                st.gen(b, exp).fill_(GEN)
+    LEDGER.check(key, err, muts)
+    assert st.same_outside(st.index(*written), exp), "state written outside the new conv tails and the rebuilt gates"
 
 
-def check_back(key, w, st, before, inp, T, y, yw, y_len, advanced=True):
+def check_back(key, w, st, before, inp, T, y, y_len, advanced=True):
     """y against back64 and its mutants (active streams: the call's samples below y_len; everything else sentinel), the
     new deconv tail (bit-exact) and iSTFT tail of each active stream, the clocks advanced once, and nothing else written"""
-    assert guard_ok(yw)
     exp = st.advance(before, T, inp.active) if advanced else before.clone()
-    err, muts = 0.0, {}
+    written, err, muts = [], 0.0, {}
     y = y.cpu()
     for b in range(st.B):
         if not inp.live(b):
@@ -344,10 +254,9 @@ def check_back(key, w, st, before, inp, T, y, yw, y_len, advanced=True):
         assert torch.equal(bits(st.deconv(b)[par ^ 1].cpu()), bits(ref["deconv_tail"].float())), ("deconv tail", b)
         got_i = st.istft(b)[par ^ 1]
         err = max(err, ratio(got_i, ref["istft_tail"], ref["istft_bound"]))
-        st.deconv(b, exp)[par ^ 1] = st.deconv(b)[par ^ 1]
-        st.istft(b, exp)[par ^ 1] = got_i
-    check(key, err, muts)
-    assert torch.equal(bits(st.t), bits(exp)), "state written outside the new tails and the clocks"
+        written += [st.deconv(b)[par ^ 1], got_i]
+    LEDGER.check(key, err, muts)
+    assert st.same_outside(st.index(*written), exp), "state written outside the new tails and the clocks"
 
 
 def setup(lay, dev, B, T, clip, masked, seed, xcut=64):
@@ -357,28 +266,31 @@ def setup(lay, dev, B, T, clip, masked, seed, xcut=64):
 
 
 def run_front(kind, w, st, inp, T, dev, **kw):
-    X, Xw = buf((st.B, T, NF, CH), dev)
-    pre, prew = buf((st.B, FC), dev)
+    """X and the gate scratch of one launch, their guards intact"""
+    X, pre = Guarded((st.B, T, NF, CH), dev), Guarded((st.B, FC), dev)
     if kind == "front":
-        rc = kh.front(w.c, inp.dx, inp.x_len, X, st.t, st.ss, st.B, T, inp.pos_rel, inp.demb, pre, active=inp.dact)
+        rc = kh.front(w.c, inp.dx, inp.x_len, X.t, st.t, st.ss, st.B, T, inp.pos_rel, inp.demb, pre.t, active=inp.dact)
     else:
-        rc = kh.front_many(w.c, inp.dx, inp.x_len, X, st.t, st.ss, st.B, T, inp.pos_rel, inp.demb, pre, kw["chunk"],
+        rc = kh.front_many(w.c, inp.dx, inp.x_len, X.t, st.t, st.ss, st.B, T, inp.pos_rel, inp.demb, pre.t, kw["chunk"],
                            kw["workers"], active=inp.dact)
     torch.cuda.synchronize()
     assert rc == 0, (kind, rc)
-    return X, Xw, pre, prew
+    assert X.ok() and pre.ok()
+    return X.t, pre.t
 
 
 def run_back(kind, w, st, inp, T, y_len, dev, **kw):
-    y, yw = buf((st.B, 2, inp.s0 + HOP * T + 256), dev)
+    """y of one launch, its guards intact"""
+    y = Guarded((st.B, 2, inp.s0 + HOP * T + 256), dev)
     dX = inp.X.to(dev)
     if kind == "back":
-        rc = kh.back(w.c, dX, y, y_len, st.t, st.ss, st.B, T, inp.pos_rel, active=inp.dact)
+        rc = kh.back(w.c, dX, y.t, y_len, st.t, st.ss, st.B, T, inp.pos_rel, active=inp.dact)
     else:
-        rc = kh.back_many(w.c, dX, y, y_len, st.t, st.ss, st.B, T, inp.pos_rel, kw["chunk"], kw["n_cl"], active=inp.dact)
+        rc = kh.back_many(w.c, dX, y.t, y_len, st.t, st.ss, st.B, T, inp.pos_rel, kw["chunk"], kw["n_cl"], active=inp.dact)
     torch.cuda.synchronize()
     assert rc == 0, (kind, rc)
-    return y, yw
+    assert y.ok()
+    return y.t
 
 
 TS = [1, 2, 3, 5, 37]
@@ -394,9 +306,9 @@ def test_front_kernel(T, clip, masked, dev, lay, w):
     """an ordinary call of T frames: X of every stream (inactive ones too) against front64, the new conv tails of the
     active streams in the other parity copy, the gate rebuilt exactly for the active streams whose memo key differs"""
     inp, st = setup(lay, dev, 5, T, clip, masked, seed=10 * T, xcut=XCUT[T])
-    before = st.t.clone()
-    X, Xw, _, prew = run_front("front", w, st, inp, T, dev)
-    check_front("front_kernel", w, st, before, inp, T, X, Xw, prew)
+    before = st.snapshot()
+    X, _ = run_front("front", w, st, inp, T, dev)
+    check_front("front_kernel", w, st, before, inp, T, X)
     assert st.header(before) == st.header()
 
 
@@ -418,10 +330,10 @@ def test_front_many_kernel(T, geom, dev, lay, w):
     out = []
     for kind in ("many", "front"):
         inp, st = setup(lay, dev, B, T, "rel37", True, seed=20 + T)
-        before = st.t.clone()
-        X, Xw, pre, prew = run_front(kind, w, st, inp, T, dev, chunk=chunk, workers=workers)
+        before = st.snapshot()
+        X, pre = run_front(kind, w, st, inp, T, dev, chunk=chunk, workers=workers)
         if kind == "many":
-            check_front("front_many_kernel", w, st, before, inp, T, X, Xw, prew)
+            check_front("front_many_kernel", w, st, before, inp, T, X)
         out.append((X, st.t, pre))
     for a, b in zip(*out):
         assert torch.equal(bits(a), bits(b)), "front_many_kernel and front_kernel differ"
@@ -434,22 +346,21 @@ def test_front1_kernel(clip, masked, dev, lay, w):
     """one frame over 13 bin tiles: X and the new conv tails within front64's bounds (and within them of front_kernel's
     X), block 0's input projection GX within ih64 of the kernel's own X, the gate as front_kernel builds it"""
     inp, st = setup(lay, dev, 5, 1, clip, masked, seed=30, xcut=37)
-    before = st.t.clone()
-    X, Xw = buf((st.B, 1, NF, CH), dev)
-    GX, GXw = buf((st.B, NF, 512), dev)
-    pre, prew = buf((st.B, FC), dev)
-    rc = kh.front1(w.c, inp.dx, inp.x_len, X, GX, st.t, st.ss, st.B, inp.pos_rel, inp.demb, pre, active=inp.dact)
+    before = st.snapshot()
+    X, GX, pre = Guarded((st.B, 1, NF, CH), dev), Guarded((st.B, NF, 512), dev), Guarded((st.B, FC), dev)
+    rc = kh.front1(w.c, inp.dx, inp.x_len, X.t, GX.t, st.t, st.ss, st.B, inp.pos_rel, inp.demb, pre.t, active=inp.dact)
     torch.cuda.synchronize()
     assert rc == 0
-    assert guard_ok(GXw)
-    check_front("front1_kernel", w, st, before, inp, 1, X, Xw, prew)
+    assert X.ok() and GX.ok() and pre.ok()
+    X, GX = X.t, GX.t
+    check_front("front1_kernel", w, st, before, inp, 1, X)
     err = 0.0
     for b in range(st.B):
         ref, bound = kh.ih64(X[b, 0].cpu(), w.ln1_g, w.ln1_b, w.wih1_t, w.b1)
         err = max(err, ratio(GX[b], ref, bound))
-    check("front1_kernel GX", err, {})
+    LEDGER.check("front1_kernel GX", err, {})
     st0 = State(lay, st.B, dev, inp.rel, inp.emb, 31)
-    X0, _, _, _ = run_front("front", w, st0, inp, 1, dev)
+    X0, _ = run_front("front", w, st0, inp, 1, dev)
     for b in range(st.B):
         ref = w.front(inp.x[b], inp.x_len, inp.s0, 1, st.conv(b, before)[st.par(b)].cpu())
         assert ratio(X[b], X0[b].double().cpu(), 2 * ref["X_bound"]) <= 1.0, b
@@ -464,9 +375,9 @@ def test_back_kernel(T, clip, masked, dev, lay, w):
     sentinel elsewhere, the new tails in the other parity copy, the clocks advanced exactly once"""
     inp, st = setup(lay, dev, 5, T, clip, masked, seed=40 + T)
     y_len = inp.s0 + HOP * (T - 1) + YCUT[T]
-    before = st.t.clone()
-    y, yw = run_back("back", w, st, inp, T, y_len, dev)
-    check_back("back_kernel", w, st, before, inp, T, y, yw, y_len)
+    before = st.snapshot()
+    y = run_back("back", w, st, inp, T, y_len, dev)
+    check_back("back_kernel", w, st, before, inp, T, y, y_len)
     pos, ncalls, _, done = st.header()
     assert (pos, ncalls, done) == (HDR_POS + T, HDR_CALLS + 1, 0)
 
@@ -477,9 +388,9 @@ def test_back_kernel_y_len(cut, dev, lay, w):
     T = 3
     inp, st = setup(lay, dev, 5, T, "rel37", False, seed=50 + cut)
     y_len = inp.s0 + HOP * (T - 1) + cut
-    before = st.t.clone()
-    y, yw = run_back("back", w, st, inp, T, y_len, dev)
-    check_back("back_kernel", w, st, before, inp, T, y, yw, y_len)
+    before = st.snapshot()
+    y = run_back("back", w, st, inp, T, y_len, dev)
+    check_back("back_kernel", w, st, before, inp, T, y, y_len)
 
 
 # ---- back_many_kernel ------------------------------------------------------------------------------------------------
@@ -497,10 +408,10 @@ def test_back_many_kernel(T, geom, dev, lay, w):
     for kind in ("many", "back"):
         inp, st = setup(lay, dev, B, T, "rel37", True, seed=60 + T)
         y_len = inp.s0 + HOP * T - 5
-        before = st.t.clone()
-        y, yw = run_back(kind, w, st, inp, T, y_len, dev, chunk=chunk, n_cl=n_cl)
+        before = st.snapshot()
+        y = run_back(kind, w, st, inp, T, y_len, dev, chunk=chunk, n_cl=n_cl)
         if kind == "many":
-            check_back("back_many_kernel", w, st, before, inp, T, y, yw, y_len)
+            check_back("back_many_kernel", w, st, before, inp, T, y, y_len)
         out.append((y, st.t))
     for a, b in zip(*out):
         assert torch.equal(bits(a), bits(b)), "back_many_kernel and back_kernel differ"
@@ -518,15 +429,15 @@ def test_many_streams_engine_geometry(T, dev, lay, w):
     res = {}
     for kind in ("many", "one"):
         inp, st = setup(lay, dev, B, T, "rel0", True, seed=70 + T)
-        before = st.t.clone()
-        X, Xw, pre, prew = run_front("front" if kind == "one" else "many", w, st, inp, T, dev, chunk=fc, workers=fw)
+        before = st.snapshot()
+        X, pre = run_front("front" if kind == "one" else "many", w, st, inp, T, dev, chunk=fc, workers=fw)
         if kind == "many":
-            check_front("front_many_kernel", w, st, before, inp, T, X, Xw, prew)
-        mid = st.t.clone()
+            check_front("front_many_kernel", w, st, before, inp, T, X)
+        mid = st.snapshot()
         y_len = inp.s0 + HOP * T
-        y, yw = run_back("back" if kind == "one" else "many", w, st, inp, T, y_len, dev, chunk=bc, n_cl=bn)
+        y = run_back("back" if kind == "one" else "many", w, st, inp, T, y_len, dev, chunk=bc, n_cl=bn)
         if kind == "many":
-            check_back("back_many_kernel", w, st, mid, inp, T, y, yw, y_len)
+            check_back("back_many_kernel", w, st, mid, inp, T, y, y_len)
         res[kind] = (X, pre, y, st.t)
     for a, b in zip(res["many"], res["one"]):
         assert torch.equal(bits(a), bits(b))
@@ -543,32 +454,32 @@ def test_group_form_equals_one_call(K, dev, lay, w):
     res = {}
     for form in ("group", "call"):
         inp, st = setup(lay, dev, B, K, "rel37", False, seed=80 + K)
-        before = st.t.clone()
+        before = st.snapshot()
         y_len = inp.s0 + HOP * K - 3
-        y, yw = buf((B, 2, inp.s0 + HOP * K + 256), dev)
-        pre, prew = buf((B, FC), dev)
         if form == "group":
-            ws, wsw = buf((K * slot,), dev)
-            Xk = [ws[k * slot:k * slot + B * FC].view(B, 1, NF, CH) for k in range(K)]
+            y, pre, ws = Guarded((B, 2, inp.s0 + HOP * K + 256), dev), Guarded((B, FC), dev), Guarded((K * slot,), dev)
+            Xk = [ws.t[k * slot:k * slot + B * FC].view(B, 1, NF, CH) for k in range(K)]
             for k in range(K):
-                assert kh.front(w.c, inp.dx, inp.x_len, Xk[k], st.t, st.ss, B, 1, inp.pos_rel, inp.demb, pre, frame_k=k,
-                                frames_total=K) == 0
+                assert kh.front(w.c, inp.dx, inp.x_len, Xk[k], st.t, st.ss, B, 1, inp.pos_rel, inp.demb, pre.t,
+                                frame_k=k, frames_total=K) == 0
             torch.cuda.synchronize()
             X = torch.cat(Xk, dim=1)
-            assert guard_ok(wsw) and all(is_sentinel(ws[k * slot + B * FC:(k + 1) * slot]) for k in range(K))
-            check_front("front_kernel group", w, st, before, inp, K, X, sentinel(GUARD, dev), prew)
+            assert ws.ok() and pre.ok() and all(is_sentinel(ws.t[k * slot + B * FC:(k + 1) * slot]) for k in range(K))
+            check_front("front_kernel group", w, st, before, inp, K, X)
             for k in range(K):
                 Xk[k].copy_(inp.X[:, k:k + 1].to(dev))             # the back's input rows, in the same slots
-            mid = st.t.clone()
+            mid = st.snapshot()
             for k in range(K):
-                assert kh.back(w.c, Xk[k], y, y_len, st.t, st.ss, B, 1, inp.pos_rel, frame_k=k, frames_total=K,
+                assert kh.back(w.c, Xk[k], y.t, y_len, st.t, st.ss, B, 1, inp.pos_rel, frame_k=k, frames_total=K,
                                hist_stride=slot) == 0
             torch.cuda.synchronize()
-            check_back("back_kernel group", w, st, mid, inp, K, y, yw, y_len, advanced=False)
+            assert y.ok()
+            y, pre = y.t, pre.t
+            check_back("back_kernel group", w, st, mid, inp, K, y, y_len, advanced=False)
             state = st.advance(st.t, K, None)
         else:
-            X, _, pre, prew = run_front("front", w, st, inp, K, dev)
-            y, yw = run_back("back", w, st, inp, K, y_len, dev)
+            X, pre = run_front("front", w, st, inp, K, dev)
+            y = run_back("back", w, st, inp, K, y_len, dev)
             state = st.t
         res[form] = (X, y, pre, state)
     for name, a, b in zip(("X", "y", "gate scratch", "state"), res["group"], res["call"]):
@@ -578,13 +489,4 @@ def test_group_form_equals_one_call(K, dev, lay, w):
 def test_summary(dev):
     """prints the worst error / bound per kernel and the smallest mutant error / bound over the tests above (run in the
     same session) with the device's name and power limit"""
-    p = torch.cuda.get_device_properties(dev)
-    try:
-        pl = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", str(dev.index)],
-                            capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        pl = "unknown"
-    print(f"device: {p.name}, power limit {pl}")
-    for k, v in sorted(WORST.items()):
-        print(f"worst {k:>22s}: {v:.3f} x bound; smallest mutant margin {MARGIN.get(k, math.nan):.1f}")
-    assert all(v <= 1.0 for v in WORST.values()) and all(v >= SENSITIVITY for v in MARGIN.values())
+    LEDGER.summary()

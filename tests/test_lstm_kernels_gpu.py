@@ -20,19 +20,11 @@ import pytest
 import torch
 
 from kernels import harness as kh
+from kernels.scaffold import SENSITIVITY, SENTINEL, dev, sentinel  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
-SENTINEL = 0x7FC0DEAD
 TOL = {"cuda": 1.5e-6, "tc": 2e-5, "tc_x": 5e-5}    # |h - h64| bound per family (passes = 3 for the tensor cores)
-SENSITIVITY = 10.0
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    kh.lib()
-    return torch.device("cuda", 0)
 
 
 @dataclass
@@ -113,10 +105,10 @@ class Problem:
 
     def run(self, variant, passes=3, h_state=True):
         s, dev = self.s, self.dev
-        out = torch.zeros(self.rows_o * self.out_ld, dtype=torch.int32, device=dev).fill_(SENTINEL).view(torch.float32)
+        out = sentinel(self.rows_o * self.out_ld, dev)
         h = c = None
         if s.state and h_state:
-            h = torch.zeros(self.n_hc, dtype=torch.int32, device=dev).fill_(SENTINEL).view(torch.float32)
+            h = sentinel(self.n_hc, dev)
             c = h.clone()
             h[self.hc_idx.to(dev)] = self.h0.to(dev)
             c[self.hc_idx.to(dev)] = self.c0.to(dev)

@@ -35,64 +35,32 @@ import pytest
 import torch
 
 from kernels import harness as kh
+from kernels.scaffold import Guarded, dev  # noqa: F401
 from lookoncetohear_b200 import _cabi
 from lookoncetohear_b200.metrics import eval_metrics
 from lookoncetohear_b200.render import render_binaural
 
 pytestmark = pytest.mark.gpu
 
-SENTINEL = 0x7FC0DEAD
-GUARD = 1024
 
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    _cabi.lib()
-    return torch.device("cuda", 0)
-
-
-def bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-class Guarded:
-    """a device buffer of `shape` floats between GUARD sentinel floats on each side (init: its values, or the sentinel)"""
-
-    def __init__(self, shape, dev, init=None):
-        n = int(np.prod(shape))
-        self.whole = torch.full((n + 2 * GUARD,), SENTINEL, dtype=torch.int32, device=dev).view(torch.float32)
-        self.t = self.whole[GUARD:GUARD + n].view(shape)
-        if init is not None:
-            self.t.copy_(torch.from_numpy(np.ascontiguousarray(init, np.float32)).view(shape))
-
-    def ptr(self):
-        return self.t.data_ptr()
-
-    def guards_ok(self):
-        return bool((bits(self.whole[:GUARD]) == SENTINEL).all()) and bool((bits(self.whole[-GUARD:]) == SENTINEL).all())
-
-    def np(self):
-        return self.t.cpu().numpy()
+def ptr(g):
+    """the device pointer of a Guarded buffer, or NULL"""
+    return None if g is None else g.t.data_ptr()
 
 
 def render(src, rir, noise, scale, dev, norm=True):
     """l2h_render_binaural on guarded copies -> (events, mixture, norm or None) as numpy fp32; every guard intact"""
     B, S, N = src.shape
-    ins = [Guarded(x.shape, dev, x) for x in (src, rir, noise, scale) if x is not None]
-    g_src, g_rir = ins[0], ins[1]
-    g_nz = ins[2] if noise is not None else None
-    g_sc = ins[-1] if scale is not None else None
+    g_src, g_rir, g_nz, g_sc = (None if x is None else Guarded(x.shape, dev, x) for x in (src, rir, noise, scale))
     ev, mix, scratch = Guarded((B, S, 2, N), dev), Guarded((B, 2, N), dev), Guarded((B,), dev)
     nrm = Guarded((B,), dev) if norm else None
-    rc = _cabi.lib().l2h_render_binaural(g_src.ptr(), g_rir.ptr(), g_nz.ptr() if g_nz else None, g_sc.ptr() if g_sc else None,
-                                         B, S, N, rir.shape[-1], ev.ptr(), mix.ptr(), nrm.ptr() if nrm else None,
-                                         scratch.ptr(), torch.cuda.current_stream(dev).cuda_stream)
+    rc = _cabi.lib().l2h_render_binaural(ptr(g_src), ptr(g_rir), ptr(g_nz), ptr(g_sc), B, S, N, rir.shape[-1], ptr(ev),
+                                         ptr(mix), ptr(nrm), ptr(scratch), torch.cuda.current_stream(dev).cuda_stream)
     assert rc == 0, _cabi.lib().l2h_last_error().decode()
     torch.cuda.synchronize(dev)
-    for g in ins + [ev, mix, scratch] + ([nrm] if nrm else []):
-        assert g.guards_ok(), "a guard lost its sentinel"
-    return ev.np(), mix.np(), nrm.np() if nrm else None
+    for g in (g_src, g_rir, g_nz, g_sc, ev, mix, scratch, nrm):
+        assert g is None or g.ok(), "a guard lost its sentinel"
+    return ev.t.cpu().numpy(), mix.t.cpu().numpy(), nrm.t.cpu().numpy() if nrm else None
 
 
 def same_bits(a, b):
@@ -191,14 +159,14 @@ def metrics(est, tgt, mix, emb, emb_gt, dev):
     B, C, n = est.shape
     ins = {k: Guarded(v.shape, dev, v) for k, v in dict(est=est, tgt=tgt, mix=mix, emb=emb, emb_gt=emb_gt).items() if v is not None}
     out = Guarded((B, 3), dev)
-    p = lambda k: ins[k].ptr() if k in ins else None
+    p = lambda k: ptr(ins.get(k))
     rc = _cabi.lib().l2h_eval_metrics(p("est"), p("tgt"), p("mix"), B, C, n, p("emb"), p("emb_gt"),
-                                      emb.shape[1] if emb is not None else 0, out.ptr(), torch.cuda.current_stream(dev).cuda_stream)
+                                      emb.shape[1] if emb is not None else 0, ptr(out), torch.cuda.current_stream(dev).cuda_stream)
     assert rc == 0, _cabi.lib().l2h_last_error().decode()
     torch.cuda.synchronize(dev)
     for g in list(ins.values()) + [out]:
-        assert g.guards_ok(), "a guard lost its sentinel"
-    return out.np()
+        assert g.ok(), "a guard lost its sentinel"
+    return out.t.cpu().numpy()
 
 
 @pytest.mark.parametrize("case", kh.METRICS_CASES, ids=lambda c: c[0])

@@ -13,7 +13,7 @@ the residual.  Each value has its own bound: u = 2^-24, u sqrt(n) sum |terms| fo
 rounding carried through |g| / sigma.  The LayerNorm problems include a constant row, whose normalised row is exactly
 ln_b (so its output is bit for bit that of a launch without the LayerNorm on the row ln_b), a row of mean 10^3 and unit
 spread, and a row of spread 0.01 (where eps inside or outside the sqrt differs).  Every float the kernel must not write
-holds the NaN sentinel 0x7FC0DEAD and must survive: rows past M, the guard floats after C, the gaps between hop slots;
+holds the NaN sentinel 0x7FC0DEAD and must survive: rows past M, the guard floats around C, the gaps between hop slots;
 every float it must not read is NaN too: A's padding columns (lda > K) and the hop slots' gaps.  All forms accumulate k in
 order, then add the bias, then the residual, so every form gives the same bits on the same problem.
 
@@ -29,30 +29,13 @@ import pytest
 import torch
 
 from kernels import harness as kh
+from kernels.scaffold import Guarded, Ledger, bits, dev, ratio  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
-SENTINEL = 0x7FC0DEAD
-SENSITIVITY = 10.0
-GUARD = 1024
 TILE = 16
 REACHABLE = {"tile16x64", "tile64x64", "big128"}
-WORST, MUTANT_MIN = {}, {}
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    kh.lib()
-    return torch.device("cuda", 0)
-
-
-def sentinel(n, dev):
-    return torch.full((n,), SENTINEL, dtype=torch.int32, device=dev).view(torch.float32)
-
-
-def bits(t):
-    return t.contiguous().view(torch.int32)
+LEDGER = Ledger()
 
 
 # kind -> (K, N, lda, LayerNorm, residual in place): the engine's four dense layers (sep_engine.cu: Chain::dense); the
@@ -90,15 +73,16 @@ class Problem:
         """one launch (ln=False: without the LayerNorm; A: other rows); asserts that nothing outside C's rows changed
         and that no NaN was read; returns (the form launched, C's rows [M][N])"""
         A = self.A if A is None else A
-        abuf = sentinel(self.n_a + GUARD, dev)
+        ag = Guarded((self.n_a,), dev)
+        cg = ag if self.shared else Guarded((self.n_c,), dev)
+        abuf, cbuf = ag.t, cg.t
         ai = (self.a_off[:, None] + torch.arange(self.K)[None, :]).to(dev)
         abuf[ai] = A.to(dev)
-        cbuf = abuf if self.shared else sentinel(self.n_c + GUARD, dev)
         ci = (self.c_off[:, None] + torch.arange(self.N)[None, :]).to(dev)
         if self.res:
             cbuf[ci] = self.R.to(dev)
         before = cbuf.clone()
-        abefore = abuf.clone()
+        abefore = ag.whole.clone()
         w = {k: v.to(dev) for k, v in (("Wt", self.Wt), ("bias", self.bias))}
         d = kh.RowsGemm()
         d.A, d.lda, d.Wt, d.bias, d.C, d.ldc = abuf.data_ptr(), self.lda, w["Wt"].data_ptr(), w["bias"].data_ptr(), \
@@ -121,31 +105,22 @@ class Problem:
         got = cbuf[ci].clone()
         exp = before.clone()
         exp[ci] = got
-        assert torch.equal(bits(cbuf), bits(exp)), f"{self.kind} M={self.M} shape {shape}: C written outside its rows"
+        assert torch.equal(bits(cbuf), bits(exp)) and cg.ok(), \
+            f"{self.kind} M={self.M} shape {shape}: C written outside its rows"
         if not self.shared:
-            assert torch.equal(bits(abuf), bits(abefore)), "A written"
+            assert torch.equal(bits(ag.whole), bits(abefore)), "A written"
         assert bool(torch.isfinite(got).all()), "a NaN sentinel was read"
         return form, got
 
 
-def ratio(got, ref, bound):
-    return float(((got.double().cpu() - ref).abs() / bound).max())
-
-
-def check(key, got, p):
+def compare(key, got, p):
     """got within the reference's per-element bound; every mutant misses it by >= SENSITIVITY x"""
     ref, bound = p.ref()
-    r = ratio(got, ref, bound)
-    WORST[key] = max(WORST.get(key, 0.0), r)
     names = ["no_transpose", "drop_bias"] + (["unbiased", "eps_outside"] if p.ln is not None else []) + \
             (["drop_residual"] if p.res else [])
     mut = {m: ratio(got, p.ref(**{m: True})[0], bound) for m in names}
     mut["tile_offset"] = ratio(got[TILE:], ref[:-TILE], bound[TILE:])
-    MUTANT_MIN[key] = min(MUTANT_MIN.get(key, math.inf), min(mut.values()))
-    print(f"[{key}] err / bound {r:.3f}; mutants / bound: " + ", ".join(f"{m} {v:.0f}" for m, v in mut.items()))
-    assert r <= 1.0, (key, r)
-    for m, v in mut.items():
-        assert v >= SENSITIVITY, (key, m, v)
+    LEDGER.check(key, ratio(got, ref, bound), mut)
 
 
 @pytest.mark.parametrize("M", [97, 194, 1261, 2047, 2048])
@@ -155,7 +130,7 @@ def test_dense_layers(kind, M, dev):
     assert kh.rows_gemm_form(M, p.N, p.K) == "tile16x64"
     form, got = p.run(dev)
     assert form == "tile16x64"
-    check(kind, got, p)
+    compare(kind, got, p)
     if p.ln is not None:
         # the constant row's normalised row is exactly ln_b: bit for bit the launch without LayerNorm on ln_b
         A2 = p.A.clone()
@@ -185,7 +160,7 @@ def test_pipeline_windowed_forms(B, hops, dev):
         form, got = p.run(dev, shape, windowed=win)
         assert form == kh.rows_gemm_form(p.M, p.N, p.K, shape) and form in REACHABLE, (shape, form)
         forms.add(form)
-        check(f"pipeline {form}", got, p)
+        compare(f"pipeline {form}", got, p)
         outs[shape] = got
     assert forms == ({"tile16x64", "tile64x64", "big128"} if p.M <= 2048 else {"tile64x64", "big128"})
     for shape in (1, 2):
@@ -202,6 +177,4 @@ def test_forms_agree_on_plain_rows(dev):
 
 
 def test_summary(dev):
-    print("worst error / bound: " + ", ".join(f"{k} {v:.3f}" for k, v in sorted(WORST.items())))
-    print("smallest mutant error / bound: " + ", ".join(f"{k} {v:.0f}" for k, v in sorted(MUTANT_MIN.items())))
-    assert all(v <= 1.0 for v in WORST.values()) and all(v >= SENSITIVITY for v in MUTANT_MIN.values())
+    LEDGER.summary()

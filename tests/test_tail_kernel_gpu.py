@@ -15,7 +15,7 @@ gate on the block output and ih64 of that output.  Each state holds streams with
 50, 55, 56, 57, 111, 2^31 + 7} and two blocks at a record stride with a gap; the kernel runs on block 1.  Every float
 the kernel must neither write nor read holds the NaN sentinel 0x7FC0DEAD: the 6 spare ring slots and the slot this hop
 writes (a kernel that reads the newest row before it is written, or a spare slot, turns NaN), block 0, the other fields
-of each record, the gains' padding and guard floats after every buffer.  Scores are ~1 ("unit") or spread over +-80
+of each record, the gains' padding and guard floats around every buffer.  Scores are ~1 ("unit") or spread over +-80
 ("wide", where each part of a head's window has its own max); the "edge" weights give one K head and the
 LayerNorm(6208)'s input a mean >> spread, and two rows of each stream (7 and 96, the last tile's only row) an X1 of
 spread 0.01, where eps inside or outside the sqrt differs.
@@ -51,31 +51,17 @@ import pytest
 import torch
 
 from kernels import harness as kh
+from kernels.scaffold import SENTINEL, Guarded, Ledger, Records, bits, dev, is_sentinel, lay, ratio  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
-SENTINEL = 0x7FC0DEAD
-SENSITIVITY = 10.0
-GUARD = 1024
 N_BLOCKS, BLK = 2, 1
 BIG = 2 ** 31 + 7
 CLOCKS = (0, 1, 48, 49, 50, 55, 56, 57, 111, BIG)
 NF, CH, NH, ATT, RING = kh.NF, kh.CH, kh.NHEAD, kh.ATT, kh.RING
 QK_DIM, QK_LD, V_DIM, FC, NQKV = kh.QK_DIM, kh.QK_LD, kh.V_DIM, kh.FC, kh.NQKV
 LOW_SPREAD_ROWS = (7, 96)
-WORST, MUTANT_MIN = {}, {}
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    kh.lib()
-    return torch.device("cuda", 0)
-
-
-@pytest.fixture(scope="module")
-def lay(dev):
-    return kh.sep_layout(N_BLOCKS)
+LEDGER = Ledger()
 
 
 @pytest.fixture(scope="module")
@@ -83,43 +69,6 @@ def ncl(dev):
     n = kh.tail_clusters()
     assert n > 0, "tail_kernel's 16-CTA cluster cannot be scheduled: one-hop calls lose their 8-launch path"
     return n
-
-
-def sentinel(n, dev):
-    return torch.full((n,), SENTINEL, dtype=torch.int32, device=dev).view(torch.float32)
-
-
-def bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def ratio(got, ref, bound):
-    return float(((got.double().cpu() - ref.double()).abs() / bound).max())
-
-
-def record(key, errs, muts):
-    """errs: {output: error / bound}; muts: {mutant: error / bound, the largest over the outputs}"""
-    worst = max(errs.values())
-    WORST[key] = max(WORST.get(key, 0.0), worst)
-    if muts:
-        MUTANT_MIN[key] = min(MUTANT_MIN.get(key, math.inf), min(muts.values()))
-    print(f"[{key}] err / bound " + ", ".join(f"{k} {v:.3f}" for k, v in errs.items()) + "; mutants / bound: "
-          + ", ".join(f"{m} {v:.0f}" for m, v in muts.items()))
-    assert worst <= 1.0, (key, errs)
-    for m, v in muts.items():
-        assert v >= SENSITIVITY, (key, m, v)
-
-
-def buf(rows, cols, dev, init=None):
-    """a [rows][cols] sentinel buffer followed by GUARD sentinel floats (init: its rows' values)"""
-    whole = sentinel(rows * cols + GUARD, dev)
-    if init is not None:
-        whole[:rows * cols] = init.reshape(-1).to(dev)
-    return whole[:rows * cols].view(rows, cols), whole
-
-
-def guard_ok(whole):
-    return bool((bits(whole[-GUARD:]) == SENTINEL).all())
 
 
 class Weights:
@@ -192,78 +141,53 @@ class Stream:
         self.stale[0][:, QK_DIM:] = 0
 
 
-class State:
+class State(Records):
     """len(streams) records a gap apart, N_BLOCKS blocks, every float the sentinel except each record's clock, gate, block
     BLK's (h, c) and the ring rows of frames pos - 49 .. pos - 1 of block BLK"""
 
     def __init__(self, lay, streams, dev):
-        self.lay, self.B = lay, len(streams)
-        self.hdr, self.ss = lay["HEADER_BYTES"] // 4, lay["STREAM_STRIDE"] + 36
-        self.ring = kh.Ring(lay)
-        self.t = sentinel(self.hdr + self.B * self.ss + GUARD, dev)
+        super().__init__(lay, len(streams), dev, gap=36)
+        self.B = len(streams)
         for b, s in enumerate(streams):
             self.put(b, s)
-        self.before = self.t.clone()
-
-    def rec(self, b):
-        return self.hdr + b * self.ss
+        self.before = self.snapshot()
 
     def put(self, b, s):
-        o = self.rec(b)
-        self.t.view(torch.int64)[(o + self.lay["ST_POS"]) // 2] = s.pos
-        self.t[o + self.lay["ST_GATE"]:o + self.lay["ST_GATE"] + FC] = s.gate.reshape(-1).to(self.t.device)
-        self.hc(b, "h")[:] = s.h.reshape(-1).to(self.t.device)
-        self.hc(b, "c")[:] = s.c.reshape(-1).to(self.t.device)
+        self.pos(b).fill_(s.pos)
+        self.gate(b).copy_(s.gate)
+        self.hc(b, BLK, "h").copy_(s.h)
+        self.hc(b, BLK, "c").copy_(s.c)
         for j in range(1, ATT):
             n = s.pos - ATT + j
             for hh in range(NH):
                 self.row(b, "k", hh, n)[:] = s.hk[j, hh].to(self.t.device)
                 self.row(b, "v", hh, n)[:] = s.hv[j, hh].to(self.t.device)
 
-    def set_pos(self, b, pos):
-        self.t.view(torch.int64)[(self.rec(b) + self.lay["ST_POS"]) // 2] = pos
-
-    def hc(self, b, which):
-        o = self.rec(b) + self.lay["ST_BLK"] + BLK * self.lay["BK_STRIDE"] + self.lay["BK_H" if which == "h" else "BK_C"]
-        return self.t[o:o + NF * 64]
-
     def row(self, b, which, hh, n):
-        o = self.rec(b) + self.ring.row(BLK, which, hh, n)
-        return self.t[o:o + (QK_LD if which == "k" else V_DIM)]
+        return self.ring(b, BLK, which)[hh, kh.Ring.slot(n)]
 
     def written(self, b, pos):
-        """flat indices of what a storing launch at clock pos writes in record b: (h, c) and slot pos % 56 of K and V"""
-        idx = [torch.arange(NF * 64) + (self.hc(b, w).data_ptr() - self.t.data_ptr()) // 4 for w in ("h", "c")]
-        for which in ("k", "v"):
-            for hh in range(NH):
-                rw = self.row(b, which, hh, pos)
-                idx.append(torch.arange(rw.numel()) + (rw.data_ptr() - self.t.data_ptr()) // 4)
-        return torch.cat(idx).to(self.t.device)
+        """what a storing launch at clock pos writes in record b: (h, c) and slot pos % 56 of K and V"""
+        return [self.hc(b, BLK, "h"), self.hc(b, BLK, "c")] + [self.ring(b, BLK, w)[:, kh.Ring.slot(pos)] for w in "kv"]
 
-    def only_written(self, stores, before=None):
-        """the state equals `before` outside what the launch at the current clocks writes for the records in `stores`
-        ({record: pos})"""
-        exp = (self.before if before is None else before).clone()
-        for b, pos in stores.items():
-            i = self.written(b, pos)
-            exp[i] = self.t[i]
-        return torch.equal(bits(self.t), bits(exp))
+    def only_written(self, stores):
+        """the state equals its initial image outside what the launch at the current clocks writes for the records in
+        `stores` ({record: pos})"""
+        return self.same_outside(self.index(*(v for b, pos in stores.items() for v in self.written(b, pos))), self.before)
 
 
 def launch(W, st, streams, B, apply_gate, has_next, dev, active=None):
     """kh.tail over the streams' rows; returns X [B][97][64], GX [B][97][512] (None without next block)"""
-    Y = torch.stack([s.Y for s in streams])
-    dY, Yw = buf(B * NF, 128, dev, Y)
-    dX, Xw = buf(B * NF, 64, dev, torch.stack([s.X for s in streams]))
-    dG, Gw = buf(B * NF, 512, dev)
-    y0 = Yw.clone()
-    rc = kh.tail(W.c_next if has_next else W.c_last, dY, dX, dG, st.t, st.ss, BLK, B, apply_gate, 0, active)
+    dY = Guarded((B * NF, 128), dev, torch.stack([s.Y for s in streams]))
+    dX, dG = Guarded((B * NF, 64), dev, torch.stack([s.X for s in streams])), Guarded((B * NF, 512), dev)
+    y0 = dY.whole.clone()
+    rc = kh.tail(W.c_next if has_next else W.c_last, dY.t, dX.t, dG.t, st.t, st.ss, BLK, B, apply_gate, 0, active)
     torch.cuda.synchronize()
     assert rc == 0
-    assert torch.equal(bits(Yw), bits(y0)) and guard_ok(Xw) and guard_ok(Gw)
+    assert torch.equal(bits(dY.whole), bits(y0)) and dX.ok() and dG.ok()
     if not has_next:
-        assert bool((bits(Gw) == SENTINEL).all()), "GX written without a next block"
-    return dX.view(B, NF, 64).clone(), (dG.view(B, NF, 512).clone() if has_next else None)
+        assert is_sentinel(dG.t), "GX written without a next block"
+    return dX.t.view(B, NF, 64).clone(), (dG.t.view(B, NF, 512).clone() if has_next else None)
 
 
 def mutants_for(regime, apply_gate, has_next):
@@ -284,7 +208,7 @@ def stream_outputs(st, b, pos, X, GX):
     k = torch.stack([st.row(b, "k", hh, pos) for hh in range(NH)])
     v = torch.stack([st.row(b, "v", hh, pos) for hh in range(NH)])
     assert bool((bits(k[:, QK_DIM:]) == 0).all()), "K pad columns 582, 583"
-    got = dict(X=X[b], K=k[:, :QK_DIM], V=v, h=st.hc(b, "h").view(NF, 64), c=st.hc(b, "c").view(NF, 64))
+    got = dict(X=X[b], K=k[:, :QK_DIM], V=v, h=st.hc(b, BLK, "h"), c=st.hc(b, BLK, "c"))
     if GX is not None:
         got["GX"] = GX[b]
     return got
@@ -330,17 +254,17 @@ def test_tail_kernel(B, regime, apply_gate, has_next, edge, weights, lay, ncl, d
             mr = kh.tail64(s.Y, s.X, s.h, s.c, W.p, s.hk, s.hv, gate, nxt, **kw)
             ref_b = {k + "_b": r[k + "_b"] for k in keys if k != "GX"}
             muts[m] = max(muts.get(m, 0.0), max(outputs_ratio(dict(mr, **ref_b), got, keys, GXb).values()))
-    record(f"tail {regime}{' edge' if edge else ''}", errs, muts)
+    LEDGER.check(f"tail {regime}{' edge' if edge else ''}", errs, muts)
     # the same mid_tile as mid_kernel: (h, c) bit for bit
     st2 = State(lay, streams, dev)
-    dY, _ = buf(B * NF, 128, dev, torch.stack([s.Y for s in streams]))
-    dX, _ = buf(B * NF, 64, dev, torch.stack([s.X for s in streams]))
-    dQ, _ = buf(B * NF, NQKV, dev)
-    assert kh.mid(W.c_mid, dY, dX, dQ, st2.t, st2.ss, BLK, B, act.to(dev)) == 0
+    dY = Guarded((B * NF, 128), dev, torch.stack([s.Y for s in streams]))
+    dX = Guarded((B * NF, 64), dev, torch.stack([s.X for s in streams]))
+    dQ = Guarded((B * NF, NQKV), dev)
+    assert kh.mid(W.c_mid, dY.t, dX.t, dQ.t, st2.t, st2.ss, BLK, B, act.to(dev)) == 0
     torch.cuda.synchronize()
     for b in live:
         for w in ("h", "c"):
-            assert torch.equal(bits(st.hc(b, w)), bits(st2.hc(b, w))), (b, w)
+            assert torch.equal(bits(st.hc(b, BLK, w)), bits(st2.hc(b, BLK, w))), (b, w)
 
 
 @pytest.mark.parametrize("hops", ["none", "list"])
@@ -357,15 +281,14 @@ def test_tail_kernel_records(hops, weights, lay, dev):
     recs = [Stream(W, CLOCKS[(3 * i) % len(CLOCKS)], "unit", seed=5000 + i) for i in range(batch)]
     calls = [Stream(W, 0, "unit", seed=6000 + b) for b in range(n)]          # the rows' Y and X
     st = State(lay, recs, dev)
-    Y = torch.stack([s.Y for s in calls])
-    dY, _ = buf(n * NF, 128, dev, Y)
-    dX, Xw = buf(n * NF, 64, dev, torch.stack([s.X for s in calls]))
-    dG, Gw = buf(n * NF, 512, dev)
+    dY = Guarded((n * NF, 128), dev, torch.stack([s.Y for s in calls]))
+    dX, dG = Guarded((n * NF, 64), dev, torch.stack([s.X for s in calls])), Guarded((n * NF, 512), dev)
     dslots = torch.tensor(slots, dtype=torch.int32, device=dev)
     dhops = None if hop is None else torch.tensor(hop, dtype=torch.int32, device=dev)
-    assert kh.tail_slots(W.c_next, dY, dX, dG, st.t, st.ss, dslots, batch, dhops, BLK, n, 1) == 0
+    assert kh.tail_slots(W.c_next, dY.t, dX.t, dG.t, st.t, st.ss, dslots, batch, dhops, BLK, n, 1) == 0
     torch.cuda.synchronize()
-    assert guard_ok(Xw) and guard_ok(Gw)
+    assert dX.ok() and dG.ok()
+    dX, dG = dX.t, dG.t
     assert st.only_written({slots[b]: recs[slots[b]].pos for b in stores}), "a row that stores nothing wrote its record"
     # the dense form over the same records, in call-row order (row b = record slots[b], record 0 for the out-of-range row)
     dense = [recs[sl] if 0 <= sl < batch else recs[0] for sl in slots]
@@ -378,8 +301,8 @@ def test_tail_kernel_records(hops, weights, lay, dev):
     for b in stores:
         assert torch.equal(bits(dX.view(n, NF, 64)[b]), bits(X[b])), b
         assert torch.equal(bits(dG.view(n, NF, 512)[b]), bits(GX[b])), b
-        a, d = st.written(slots[b], recs[slots[b]].pos), sd.written(b, dense[b].pos)
-        assert torch.equal(bits(st.t[a]), bits(sd.t[d])), b
+        for a, d in zip(st.written(slots[b], recs[slots[b]].pos), sd.written(b, dense[b].pos)):
+            assert torch.equal(bits(a), bits(d)), b
 
 
 def test_tail_kernel_chain(weights, lay, dev):
@@ -398,7 +321,7 @@ def test_tail_kernel_chain(weights, lay, dev):
         hop_streams = []
         for b, s in enumerate(streams):
             s.Y, s.X = Ys[b][j], Xs[b][j]
-            st.set_pos(b, clocks[b] + j)
+            st.pos(b).fill_(clocks[b] + j)
             hop_streams.append(s)
         X, _ = launch(W, st, hop_streams, B, 1, False, dev)
         outs.append(X)
@@ -415,13 +338,11 @@ def test_tail_kernel_chain(weights, lay, dev):
             errs["V"] = max(errs.get("V", 0.0), ratio(v, ref[j]["V"], ref[j]["V_b"]))
             muts["shift"] = max(muts.get("shift", 0.0), ratio(outs[j][b], shifted[j]["X"], ref[j]["X_b"]))
         last = ref[-1]
-        errs["h"] = max(errs.get("h", 0.0), ratio(st.hc(b, "h").view(NF, 64), last["h"], last["h_b"]))
-        errs["c"] = max(errs.get("c", 0.0), ratio(st.hc(b, "c").view(NF, 64), last["c"], last["c_b"]))
-    record("tail chain", errs, muts)
+        errs["h"] = max(errs.get("h", 0.0), ratio(st.hc(b, BLK, "h"), last["h"], last["h_b"]))
+        errs["c"] = max(errs.get("c", 0.0), ratio(st.hc(b, BLK, "c"), last["c"], last["c_b"]))
+    LEDGER.check("tail chain", errs, muts)
 
 
 def test_summary(dev, ncl):
     print(f"tail_kernel: {ncl} clusters of 16 CTAs resident at once")
-    print("worst error / bound: " + ", ".join(f"{k} {v:.3f}" for k, v in sorted(WORST.items())))
-    print("smallest mutant error / bound: " + ", ".join(f"{k} {v:.0f}" for k, v in sorted(MUTANT_MIN.items())))
-    assert all(v <= 1.0 for v in WORST.values()) and all(v >= SENSITIVITY for v in MUTANT_MIN.values())
+    LEDGER.summary()

@@ -20,7 +20,7 @@ inter_h_last_kernel are exact for T_b in {-1, 0, 1, T - 1, T, T + 1}, T in {1, 2
 recurrence with per-sequence step counts (LstmXArgs::steps, passes 1-3) must give, for a sequence of T_b steps, the
 outputs of its first T_b steps and its final c bit-identical to a run of T_b steps, and c0 for T_b outside [1, L].
 
-Every buffer is followed by guard floats holding the sentinel 0x7FC0DEAD, every float a kernel must not write holds it
+Every buffer sits between guard floats holding the sentinel 0x7FC0DEAD, every float a kernel must not write holds it
 too and must keep it bit for bit, and each state is compared whole with the one the launch must leave.  Mutants: the
 scan without the carry between passes, the offsets unclamped, the owner search off by one (start < r), an unvalidated
 lead (target_lists); the owner r % K and a gated row without owner (gate_fanout); the gate in (c, f) order and with
@@ -36,89 +36,21 @@ import pytest
 import torch
 
 from kernels import harness as kh
+from kernels.scaffold import SENTINEL, Guarded, Ledger, Records, bits, dev, is_sentinel, lay, ratio, sentinel  # noqa: F401
 from lookoncetohear_b200.configs import TSH_PARAMS
 
 pytestmark = pytest.mark.gpu
 
-SENTINEL = 0x7FC0DEAD
-SENSITIVITY = 10.0
-GUARD = 1024
 N_BLOCKS = 3
 GAP = 132                   # floats between two records (a multiple of 4: the kernels read float4s)
 GEN = 5
 NF, CH, FC, SPK = kh.NF, kh.CH, kh.FC, kh.SPK
 INT_MAX = kh.INT_MAX
-WORST, MARGIN = {}, {}
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    kh.lib()
-    return torch.device("cuda", 0)
-
-
-@pytest.fixture(scope="module")
-def lay(dev):
-    return kh.sep_layout(N_BLOCKS)
-
-
-def sentinel(n, dev):
-    return torch.full((n,), SENTINEL, dtype=torch.int32, device=dev).view(torch.float32)
-
-
-def bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def guarded(shape, dev):
-    """a sentinel buffer of `shape` followed by GUARD sentinel floats; returns (view, whole)"""
-    n = math.prod(shape)
-    whole = sentinel(n + GUARD, dev)
-    return whole[:n].view(shape), whole
-
-
-def guard_ok(whole):
-    return bool((bits(whole[-GUARD:]) == SENTINEL).all())
+LEDGER = Ledger()
 
 
 def i32(v, dev):
     return torch.tensor(v, dtype=torch.int32, device=dev)
-
-
-def ratio(got, ref, bound):
-    d = (got.double().cpu() - ref).abs()
-    return float((d / bound.clamp_min(1e-300)).max())
-
-
-class State:
-    """`batch` records of lay's layout, ss = STREAM_STRIDE + GAP floats apart, every float the sentinel"""
-
-    def __init__(self, lay, batch, dev):
-        self.lay, self.batch = lay, batch
-        self.hdr, self.ss = lay["HEADER_BYTES"] // 4, lay["STREAM_STRIDE"] + GAP
-        self.t = sentinel(self.hdr + batch * self.ss + GUARD, dev)
-
-    def rec(self, k, t=None):
-        t = self.t if t is None else t
-        return t[self.hdr + k * self.ss:self.hdr + (k + 1) * self.ss]
-
-    def field(self, k, off, n, t=None):
-        return self.rec(k, t)[off:off + n]
-
-    def gate(self, k, t=None):
-        return self.field(k, self.lay["ST_GATE"], FC, t).view(NF, CH)
-
-    def emb(self, k, t=None):
-        return self.field(k, self.lay["ST_EMB"], SPK, t)
-
-    def gen(self, k, t=None):
-        return self.rec(k, t).view(torch.int32)[self.lay["ST_GEN"]:self.lay["ST_GEN"] + 1]
-
-    def hc(self, k, blk, which, t=None):
-        """block blk's carried h or c of record k, [97][64]"""
-        o = self.lay["ST_BLK"] + blk * self.lay["BK_STRIDE"] + self.lay["BK_H" if which == "h" else "BK_C"]
-        return self.field(k, o, FC, t).view(NF, CH)
 
 
 def records(st, slots, hops, T, dev):
@@ -138,9 +70,9 @@ LIST_CASES = kh.target_lists_cases()
 
 
 def lists_expected(ref, n, rows):
-    """the 5 rows + 1 + GUARD ints the launch must leave: rec, rec_hops (or the sentinel), owner, lead [n], start [n + 1]
-    (or the sentinel)"""
-    out = [SENTINEL] * (5 * rows + 1 + GUARD)
+    """the 5 rows + 1 ints the launch must leave: rec, rec_hops (or the sentinel), owner, lead [n], start [n + 1] (or the
+    sentinel)"""
+    out = [SENTINEL] * (5 * rows + 1)
     out[0:rows] = ref["rec"]
     if ref["rec_hops"] is not None:
         out[rows:2 * rows] = ref["rec_hops"]
@@ -156,10 +88,11 @@ def test_target_lists(case, dev):
     c = case
     n, K, rows, batch = c["n"], c["K"], c["rows"], c["batch"]
     args = [None if c[k] is None else i32(c[k], dev) for k in ("records", "offsets", "groups", "hops")]
-    lists = torch.full((5 * rows + 1 + GUARD,), SENTINEL, dtype=torch.int32, device=dev)
-    assert kh.target_lists(*args, n, K, rows, batch, lists) == 0
+    lists = Guarded((5 * rows + 1,), dev)
+    assert kh.target_lists(*args, n, K, rows, batch, lists.t) == 0
     torch.cuda.synchronize()
-    got = lists.cpu().tolist()
+    assert lists.ok(), c["name"]
+    got = bits(lists.t).cpu().tolist()
     ref = kh.target_lists_ref(c["records"], c["offsets"], c["groups"], c["hops"], n, K, rows, batch)
     exp = lists_expected(ref, n, rows)
     if got != exp:
@@ -217,7 +150,7 @@ GATE_T = 3
 @pytest.mark.parametrize("form", ["dense", "records", "records_hops"])
 def test_spk_gate(form, gw, lay, dev):
     batch = len(MEMO)
-    st = State(lay, batch, dev)
+    st = Records(lay, batch, dev, GAP)
     g = torch.Generator().manual_seed(21)
     if form == "dense":
         slots, hops = list(range(batch)), None
@@ -238,19 +171,20 @@ def test_spk_gate(form, gw, lay, dev):
         st.emb(k).copy_(e.to(dev))
         st.gen(k).fill_(GEN - 1 if kind == "gen" else GEN)
         st.gate(k).copy_((1 + 0.5 * torch.randn(NF, CH, generator=g)).to(dev))      # an old gate
-    before = st.t.clone()
-    pre, pre_w = guarded((rows, FC), dev)
+    before = st.snapshot()
+    pre = Guarded((rows, FC), dev)
     demb = emb.to(dev)
     recs, keep = (None, None) if form == "dense" else records(st, slots, hops, GATE_T, dev)
-    assert kh.spk_gate(gw.c, demb, pre, st.t, st.ss, recs, rows) == 0
+    assert kh.spk_gate(gw.c, demb, pre.t, st.t, st.ss, recs, rows) == 0
     torch.cuda.synchronize()
-    assert guard_ok(pre_w)
-    exp = before.clone()
+    assert pre.ok()
+    pre = pre.t
+    exp, written = before.clone(), []
     err, perr, muts, rebuilt = 0.0, 0.0, {}, []
     for b in range(rows):
         writes = stores(slots, hops, b, batch, GATE_T) and MEMO[slots[b]] != "match"
         if not writes:
-            assert bool((bits(pre[b]) == SENTINEL).all()), (form, b, "spk_pre row written")
+            assert is_sentinel(pre[b]), (form, b, "spk_pre row written")
             continue
         k = slots[b]
         rebuilt.append(k)
@@ -261,23 +195,18 @@ def test_spk_gate(form, gw, lay, dev):
             muts[m] = min(muts.get(m, math.inf), ratio(got, gw.gate(emb[b], **kw)[0], bound))
         p, pb = gw.pre(emb[b])
         perr = max(perr, ratio(pre[b], p, pb))
-        st.gate(k, exp).copy_(got)
+        written.append(got)
         st.emb(k, exp).copy_(demb[b])
         st.gen(k, exp).fill_(GEN)
-    assert torch.equal(bits(st.t), bits(exp)), (form, "state written outside the rebuilt memos")
+    assert st.same_outside(st.index(*written), exp), (form, "state written outside the rebuilt memos")
     expect_rebuilt = {"dense": [0, 2, 3, 4, 6, 7, 8], "records": [3, 2, 4, 6, 7, 8],
                       "records_hops": [3, 7, 8]}[form]
     assert sorted(rebuilt) == sorted(expect_rebuilt), (form, rebuilt)
     if form != "dense":
         assert torch.equal(bits(st.rec(0)), bits(st.rec(0, before))), "record 0 written"
-    WORST["gate"] = max(WORST.get("gate", 0.0), err)
-    WORST["spk_pre"] = max(WORST.get("spk_pre", 0.0), perr)
-    MARGIN["gate"] = min([MARGIN.get("gate", math.inf)] + list(muts.values()))
-    print(f"[spk_gate {form}] rebuilt records {sorted(rebuilt)}; gate err {err:.3f} x bound, spk_pre {perr:.3f}; "
-          "mutants / bound: " + ", ".join(f"{m} {e:.1f}" for m, e in muts.items()))
-    assert err <= 1.0 and perr <= 1.0
-    for m, e in muts.items():
-        assert e >= SENSITIVITY, (m, e)
+    print(f"[spk_gate {form}] rebuilt records {sorted(rebuilt)}")
+    LEDGER.check("gate", err, muts)
+    LEDGER.check("spk_pre", perr, {})
 
 
 # ---- gate_fanout_kernel ----------------------------------------------------------------------------------------------
@@ -290,28 +219,28 @@ FAN_OWNER = [0, 1, -1, 2, -1, 1, 0, 2]
 @pytest.mark.parametrize("apply_gate", [0, 1])
 @pytest.mark.parametrize("form", ["dense", "listed"])
 def test_gate_fanout(form, apply_gate, T, lay, dev):
-    st = State(lay, FAN_BATCH, dev)
+    st = Records(lay, FAN_BATCH, dev, GAP)
     g = torch.Generator().manual_seed(31 + T)
     for k in range(FAN_BATCH):
         st.gate(k).copy_((1 + 0.5 * torch.randn(NF, CH, generator=g)).to(dev))
-    before = st.t.clone()
+    before = st.snapshot()
     K = 3
     if form == "dense":
         M, rows, owner, slots = 3, 9, None, list(range(9))
     else:
         M, rows, owner, slots = 3, len(FAN_SLOTS), FAN_OWNER, FAN_SLOTS
     X0 = torch.randn(M, T, NF, CH, generator=g)
-    X, Xw = guarded((rows, T, NF, CH), dev)
+    X = Guarded((rows, T, NF, CH), dev)
     gates = torch.stack([st.gate(s if 0 <= s < FAN_BATCH else 0).cpu() for s in slots])
     if form == "dense":
-        rc = kh.gate_fanout(X0.to(dev), X, st.t, st.ss, None, None, K, T, apply_gate, rows)
+        rc = kh.gate_fanout(X0.to(dev), X.t, st.t, st.ss, None, None, K, T, apply_gate, rows)
     else:
         recs, keep = records(st, slots, None, T, dev)
-        rc = kh.gate_fanout(X0.to(dev), X, st.t, st.ss, recs, i32(owner, dev), K, T, apply_gate, rows)
+        rc = kh.gate_fanout(X0.to(dev), X.t, st.t, st.ss, recs, i32(owner, dev), K, T, apply_gate, rows)
     assert rc == 0
     torch.cuda.synchronize()
-    assert guard_ok(Xw) and torch.equal(bits(st.t), bits(before))
-    got = bits(X.cpu())
+    assert X.ok() and st.same_outside(st.index(), before)
+    got = bits(X.t.cpu())
     assert torch.equal(got, bits(kh.gate_fanout_ref(X0, gates, owner, K, apply_gate))), (form, apply_gate, T)
     caught = []
     for m in kh.FANOUT_MUTANTS:
@@ -330,7 +259,7 @@ HC_FORMS = [(0, 1), (0, 2), (0, 3), (1, 1), (1, 2)]
 
 
 def hc_state(lay, dev, seed):
-    st = State(lay, HC_BATCH, dev)
+    st = Records(lay, HC_BATCH, dev, GAP)
     g = torch.Generator().manual_seed(seed)
     for k in range(HC_BATCH):
         for blk in range(N_BLOCKS):
@@ -347,13 +276,12 @@ def test_gather_h(b0, nb, hops, with_c, lay, dev):
     hp = HC_HOPS if hops else None
     B = len(HC_SLOTS)
     recs, keep = records(st, HC_SLOTS, hp, HC_T, dev)
-    before = st.t.clone()
-    Hg, Hw = guarded((N_BLOCKS, B, NF, CH), dev)
-    Cg, Cw = guarded((N_BLOCKS, B, NF, CH), dev)
-    assert kh.gather_h(st.t, recs, b0, nb, B, Hg, Cg if with_c else None) == 0
+    before = st.snapshot()
+    Hg, Cg = Guarded((N_BLOCKS, B, NF, CH), dev), Guarded((N_BLOCKS, B, NF, CH), dev)
+    assert kh.gather_h(st.t, recs, b0, nb, B, Hg.t, Cg.t if with_c else None) == 0
     torch.cuda.synchronize()
-    assert guard_ok(Hw) and guard_ok(Cw) and torch.equal(bits(st.t), bits(before))
-    for which, buf in (("h", Hg), ("c", Cg)):
+    assert Hg.ok() and Cg.ok() and st.same_outside(st.index(), before)
+    for which, buf in (("h", Hg.t), ("c", Cg.t)):
         for blk in range(N_BLOCKS):
             for b in range(B):
                 s = HC_SLOTS[b]
@@ -362,7 +290,7 @@ def test_gather_h(b0, nb, hops, with_c, lay, dev):
                     # an out-of-range row reads record 0 (a copy nothing stores back)
                     assert torch.equal(got, bits(st.hc(s if 0 <= s < HC_BATCH else 0, blk, which))), (which, blk, b)
                 else:
-                    assert bool((got == SENTINEL).all()), (which, blk, b, "written outside the call's blocks")
+                    assert is_sentinel(got), (which, blk, b, "written outside the call's blocks")
 
 
 @pytest.mark.parametrize("hops", [None, "ragged"])
@@ -372,7 +300,7 @@ def test_scatter_hc(b0, nb, hops, lay, dev):
     hp = HC_HOPS if hops else None
     B = len(HC_SLOTS)
     recs, keep = records(st, HC_SLOTS, hp, HC_T, dev)
-    before = st.t.clone()
+    before = st.snapshot()
     g = torch.Generator().manual_seed(44)
     Hg = torch.randn(N_BLOCKS, B, NF, CH, generator=g).to(dev)
     Cg = torch.randn(N_BLOCKS, B, NF, CH, generator=g).to(dev)
@@ -388,7 +316,7 @@ def test_scatter_hc(b0, nb, hops, lay, dev):
             st.hc(HC_SLOTS[b], blk, "h", exp).copy_(Hg[blk, b])
             st.hc(HC_SLOTS[b], blk, "c", exp).copy_(Cg[blk, b])
     assert n_stored == (2 if hops else 5)
-    assert torch.equal(bits(st.t), bits(exp)), "state written outside the storing rows' blocks b0 .. b0 + nb - 1"
+    assert st.same_outside(st.index(), exp), "state written outside the storing rows' blocks b0 .. b0 + nb - 1"
 
 
 # ---- inter_gate_mask_kernel / inter_h_last_kernel --------------------------------------------------------------------
@@ -397,18 +325,18 @@ def test_scatter_hc(b0, nb, hops, lay, dev):
 def test_inter_gate_mask_and_h_last(T, ragged, lay, dev):
     hops = [-1, 0, 1, T - 1, T, T + 1] if ragged else None
     B = 6
-    st = State(lay, B, dev)
+    st = Records(lay, B, dev, GAP)
     recs, keep = records(st, list(range(B)), hops, T, dev)
     g = torch.Generator().manual_seed(51 + T)
     gx0 = torch.randn(B, T, NF, 256, generator=g)
-    gx, gxw = guarded((B, T, NF, 256), dev)
-    gx.copy_(gx0.to(dev))
-    assert kh.inter_gate_mask(gx, recs, B) == 0
+    gx = Guarded((B, T, NF, 256), dev, gx0)
+    assert kh.inter_gate_mask(gx.t, recs, B) == 0
     Y = torch.randn(B, T, NF, CH, generator=g)
-    Hg, Hw = guarded((B, NF, CH), dev)
-    assert kh.inter_h_last(Y.to(dev), Hg, recs, B) == 0
+    Hg = Guarded((B, NF, CH), dev)
+    assert kh.inter_h_last(Y.to(dev), Hg.t, recs, B) == 0
     torch.cuda.synchronize()
-    assert guard_ok(gxw) and guard_ok(Hw)
+    assert gx.ok() and Hg.ok()
+    gx, Hg = gx.t, Hg.t
     exp = gx0.clone()
     for b in range(B):
         Tb = kh.row_frames(hops, b, T)
@@ -419,7 +347,7 @@ def test_inter_gate_mask_and_h_last(T, ragged, lay, dev):
         if 0 < Tb < T:
             assert torch.equal(got, bits(Y[b, Tb - 1])), (b, Tb)
         else:
-            assert bool((got == SENTINEL).all()), (b, Tb, "h of a row that ends with the recurrence written")
+            assert is_sentinel(got), (b, Tb, "h of a row that ends with the recurrence written")
     assert torch.equal(bits(gx.cpu()), bits(exp))
 
 
@@ -497,6 +425,4 @@ def test_tc_lstm_steps_refused_elsewhere(dev):
 
 
 def test_summary():
-    for k, v in sorted(WORST.items()):
-        print(f"worst {k:>8s}: {v:.3f} x bound; smallest mutant margin {MARGIN.get(k, math.nan):.1f}")
-    assert all(v <= 1.0 for v in WORST.values()) and all(v >= SENSITIVITY for v in MARGIN.values())
+    LEDGER.summary()

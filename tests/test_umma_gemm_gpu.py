@@ -23,6 +23,7 @@ import pytest
 import torch
 
 from kernels import harness as kh
+from kernels.scaffold import SENTINEL, dev, sentinel  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -31,15 +32,7 @@ TOL = {3: 5 * 2.0 ** -18, 2: 2.0 ** -9 + 2.0 ** -16, 1: 2.0 ** -8 + 2.0 ** -17}
 CA = 4.0                       # fp32 accumulation term of bound (a), in units of 2^-24 sqrt(K)
 CB = 5.0                       # bound (b), in units of 2^-24 K^0.3 (the measured growth of the accumulation error with K)
 LN_TOL = 2.0 ** -19            # fp32 LayerNorm of the row, relative to the products (bound (a) of LN cases)
-SENTINEL = 0x7FC0DEAD          # a quiet NaN with a payload no kernel produces
 WRONG_MARGIN = 20.0
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    kh.lib()
-    return torch.device("cuda", 0)
 
 
 @dataclass
@@ -188,7 +181,7 @@ def run_case(c, dev, seed=0):
     ldc = width * c.c_inner if c.c_inner > 1 else width
     off, seq_stride, inner_stride = _row_offsets(c, ldc, width)
     total = int(off.max()) + ldc + 64
-    Cbuf = torch.full((total,), 0, dtype=torch.int32, device=dev).fill_(SENTINEL).view(torch.float32)
+    Cbuf = sentinel(total, dev)
     idx = (off[:, None] + torch.arange(c.N)[None, :]).to(dev)
     Rbuf = None
     if c.res:
@@ -389,7 +382,7 @@ def test_split_planes_bit_exact(dev):
 def _valid_desc(dev, keep):
     A = torch.randn(256, 64, device=dev)
     planes = torch.zeros(2 * 64 * 64, dtype=torch.bfloat16, device=dev)
-    C = torch.full((256 * 64,), 0, dtype=torch.int32, device=dev).fill_(SENTINEL).view(torch.float32)
+    C = sentinel(256 * 64, dev)
     s = torch.ones(64, device=dev)
     keep += [A, planes, C, s]
     d = kh.Gemm()
