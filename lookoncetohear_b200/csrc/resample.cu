@@ -260,6 +260,13 @@ static int staging(const std::string& who, int64_t floats, const std::string& wh
     return 0;
 }
 
+// Lets `kernel` take RS_SMEM_BYTES of dynamic shared memory on the current device.  A kernel with static shared memory
+// of its own cannot launch by default when the two together pass 48 KB, which a staging just under RS_SMEM_BYTES does.
+template <class Kernel>
+static cudaError_t full_staging(Kernel kernel) {
+    return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RS_SMEM_BYTES);
+}
+
 // the filter of a stream of orig -> new_freq Hz and its delay D = floor(w q / o): 0, or 1 with its message
 static int rs_streaming(const std::string& who, int32_t orig, int32_t new_freq, RsRate* g, int64_t* delay) {
     if (orig <= 0 || new_freq <= 0) return fail(1, who + ": rates must be positive, got " + rs_rates(orig, new_freq));
@@ -813,7 +820,7 @@ leveler_kernel(const float* y, int64_t y_row, int64_t y_ch, float* out, int64_t 
                 const float L = lv_lufs(P);
                 const int before = cnt;
                 if (L >= p.gate && (cnt == 0 || L >= lv_lufs(E) + p.relative)) {
-                    E = fmaf(fmaxf(p.alpha, 1.f / (float)(cnt + 1)), P - E, E);
+                    E = fmaf(fmaxf(p.alpha, 1.f / (float)(cnt + 1ll)), P - E, E);   // no overflow at INT32_MAX
                     cnt += cnt < INT32_MAX;
                 }
                 if (cnt >= p.settle) {
@@ -1315,6 +1322,8 @@ extern "C" int l2h_limiter(const float* x_dev, int64_t x_row_stride, int64_t x_c
     const Rows x{"x", x_row_stride, x_ch_stride, max_in}, y{"y", y_row_stride, y_ch_stride, max_in};
     if (int rc = disjoint(who, channels, {x, y})) return rc;
     if (overlap(y_dev, n, y, x_dev, n, x, channels, false)) return fail(1, who + ": y must not overlap x");
+    if (smem > RS_SMEM_BYTES - 1024)                                    // then the static words need the opt-in
+        if (cudaError_t e = full_staging(limiter_kernel)) return fail(3, who + ": " + cudaGetErrorString(e));
     limiter_kernel<<<(unsigned)n, RS_TILE, smem, static_cast<cudaStream_t>(stream)>>>(
         x_dev, x_row_stride, x_ch_stride, max_in, counts_dev, unit, y_dev, y_row_stride, y_ch_stride, channels, slots_dev,
         state_dev, n_slots, ceiling, lookahead, release_step);
@@ -1479,6 +1488,8 @@ extern "C" int l2h_band_compressor(const float* y_dev, int64_t y_row_stride, int
         return fail(1, who + ": out must be y itself (same pointer and strides) or not overlap it");
     const auto kernel = kp == 4 ? band_compressor_kernel<4> : kp == 8 ? band_compressor_kernel<8>
                       : kp == 12 ? band_compressor_kernel<12> : band_compressor_kernel<16>;
+    if (smem > RS_SMEM_BYTES - 1024)                                    // then the static words need the opt-in
+        if (cudaError_t e = full_staging(kernel)) return fail(3, who + ": " + cudaGetErrorString(e));
     kernel<<<(unsigned)n, BC_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
         y_dev, y_row_stride, y_ch_stride, out_dev, out_row_stride, out_ch_stride, channels, frames, slots_dev, hops_dev,
         taps_dev, bands, taps, state_dev, n_slots, attack, release);

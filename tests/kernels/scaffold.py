@@ -59,8 +59,9 @@ class Guarded:
 
 def ratio(got, ref, bound):
     """max |got - ref| / bound: 0 where got equals ref exactly (so 0 / 0 is 0), inf where a bound of 0 is missed, and 0
-    over no elements"""
-    d = (got.double().cpu() - ref.double().cpu()).abs()
+    over no elements; tensors or numpy arrays"""
+    got, ref = (torch.as_tensor(v).double().cpu() for v in (got, ref))
+    d = (got - ref).abs()
     r = d / torch.as_tensor(bound, dtype=torch.float64)
     r[d == 0] = 0
     return float(r.max()) if r.numel() else 0.0

@@ -10,6 +10,7 @@ import pytest
 import torch
 from scipy.signal import firwin
 
+from kernels.scaffold import SENSITIVITY, ratio
 from lookoncetohear_b200 import BandCompressor
 from serving_util import declaration, doc_before, header
 
@@ -50,30 +51,156 @@ def set_profile(st, gains, knees=0.0, ratios=1.0):
     st["slope"] = 1.0 - 1.0 / np.broadcast_to(np.asarray(ratios, dtype=np.float64), (K,))
 
 
-def model_hop(st, x, bank, attack=ATTACK, release=RELEASE):
-    """l2h_band_compressor on one hop of one slot: x [C, 128] float64 (float32 values), bank [K, L]; returns the hop's
-    output and advances st"""
-    C = x.shape[0]
-    K, L = bank.shape
-    D = (L - 1) // 2
+# Mutants of the model, each a plausible kernel bug (model_hop(mutant=...)): the gain ramp one sample early, the
+# detector's level from channel 0 only, the level not divided by C, the taps applied in reverse (a correlation), the
+# second copy of the history rotation dropped (only histories longer than one thread's 128 samples), release for attack.
+MUTANTS = ("early", "unlinked", "undivided", "reversed", "history", "attack")
+
+
+def bands(st, x, bank, mutant=None):
+    """the staged window [C, L - 1 + 128], the band signals [C, K, 128] and whether every sample is measured"""
     with np.errstate(invalid="ignore"):
         ok = np.abs(x) < BIG
     w = np.concatenate([st["hist"], np.where(ok, x, 0.0)], 1)
-    band = np.stack([[np.convolve(w[c], bank[b], "valid") for b in range(K)] for c in range(C)])   # [C, K, 128]
-    if ok.all():
-        P = (band ** 2).mean(axis=(0, 2))
-        st["S"] = st["S"] + np.where(P > st["S"], attack, release) * (P - st["S"])
-    with np.errstate(divide="ignore"):
-        level = 10 * np.log10(st["S"])
-    R = st["slope"] * np.maximum(0.0, level - st["knee"])
-    g0, g1 = st["g"], np.clip(st["prof"] - R[None], -40.0, 40.0)
-    if not g0.any() and not g1.any():
-        y = w[:, L - 1 - D:L - 1 - D + HOP]
+    taps = bank[:, ::-1] if mutant == "reversed" else bank
+    band = np.stack([[np.convolve(w[c], taps[b], "valid") for b in range(len(taps))] for c in range(len(w))])
+    return w, band, bool(ok.all())
+
+
+def detect(S, band, attack=ATTACK, release=RELEASE, mutant=None):
+    """the detectors after a measured hop: the linked level P [K] and the new S [K]"""
+    if mutant == "unlinked":
+        P = (band[:1] ** 2).mean(axis=(0, 2))
+    elif mutant == "undivided":
+        P = (band ** 2).sum(axis=(0, 2)) / HOP
     else:
-        gk = g0[:, :, None] + (g1 - g0)[:, :, None] * np.arange(1, HOP + 1) / HOP
-        y = (np.where(gk == 0, 1.0, 10 ** (gk / 20)) * band).sum(1)
-    st["hist"], st["g"] = w[:, HOP:], g1
+        P = (band ** 2).mean(axis=(0, 2))
+    up = np.where(P > S, release if mutant == "attack" else attack, release)
+    return P, S + up * (P - S)
+
+
+def end_gains(st, S):
+    """each channel's band gains (dB) at the end of a hop whose detectors end at S"""
+    with np.errstate(divide="ignore"):
+        level = 10 * np.log10(S)
+    R = st["slope"] * np.maximum(0.0, level - st["knee"])
+    return np.clip(st["prof"] - R[None], -40.0, 40.0)
+
+
+def ramp(g0, g1, mutant=None):
+    """the dB gain of samples k = 1 .. 128 (k = 0 .. 127 for the early mutant), [..., 128]"""
+    k = np.arange(HOP) + (mutant != "early")
+    return g0[..., None] + (g1 - g0)[..., None] * k / HOP
+
+
+def hop_out(w, band, g0, g1, mutant=None):
+    """the hop's output from the gains at its start and end: the window delayed by D where both are 0 dB everywhere"""
+    H = w.shape[1] - HOP
+    if not g0.any() and not g1.any():
+        return w[:, H - H // 2:H - H // 2 + HOP]
+    gk = ramp(g0, g1, mutant)
+    return (np.where(gk == 0, 1.0, 10 ** (gk / 20)) * band).sum(1)
+
+
+def model_hop(st, x, bank, attack=ATTACK, release=RELEASE, mutant=None):
+    """l2h_band_compressor on one hop of one slot: x [C, 128] float64 (float32 values), bank [K, L]; returns the hop's
+    output and advances st"""
+    w, band, ok = bands(st, x, bank, mutant)
+    if ok:
+        st["S"] = detect(st["S"], band, attack, release, mutant)[1]
+    g0, g1 = st["g"], end_gains(st, st["S"])
+    y = hop_out(w, band, g0, g1, mutant)
+    hist = w[:, HOP:]
+    if mutant == "history" and hist.shape[1] > HOP:
+        hist = np.concatenate([hist[:, :HOP], st["hist"][:, HOP:]], 1)
+    st["hist"], st["g"] = hist, g1
     return y
+
+
+# ---- the kernel's state row and the error bound of one hop ----------------------------------------------------------
+U = 2.0 ** -24                       # the unit roundoff of fp32
+LOG2_10_20 = math.log2(10) / 20
+LOG2_10_20_F32 = float(np.float32(LOG2_10_20))
+
+
+def gamma(n):
+    return n * U / (1 - n * U)
+
+
+def from_row(row, K):
+    """a slot's state rows [C, 5 K + L - 1] as the kernel keeps them (fp32) -> the model's state"""
+    r = np.asarray(row, np.float32).astype(np.float64)
+    return {"prof": r[:, :K].copy(), "g": r[:, K:2 * K].copy(), "S": r[0, 2 * K:3 * K].copy(),
+            "knee": r[0, 3 * K:4 * K].copy(), "slope": r[0, 4 * K:5 * K].copy(), "hist": r[:, 5 * K:].copy()}
+
+
+def to_row(st):
+    """the model's state -> the kernel's fp32 rows; the head words only channel 0 keeps are 0 in the other channels"""
+    C, K = st["prof"].shape
+    row = np.zeros((C, 5 * K + st["hist"].shape[1]), np.float32)
+    row[:, :K], row[:, K:2 * K], row[:, 5 * K:] = st["prof"], st["g"], st["hist"]
+    row[0, 2 * K:3 * K], row[0, 3 * K:4 * K], row[0, 4 * K:5 * K] = st["S"], st["knee"], st["slope"]
+    return row
+
+
+def hop_bound(st, x, bank, S1, g1, attack=ATTACK, release=RELEASE):
+    """The kernel's error bounds for one hop from state st, given the detectors S1 and gains g1 it ended the hop with:
+    {"S": S1 against detect(), "g": g1 against end_gains(st, S1), "y": the output against hop_out(st g, g1)}.
+      band: an L-term fp32 FMA chain, beta = gamma_L sum |h| |x|;
+      P: 128 C squares of band signals within beta, summed at depth C + 8, then one scaling by fl(1 / (128 C));
+      S: fmaf(coef, fl(P - S), S), and, where |P - S| is within P's error, either coefficient;
+      g: 10 log10f(S1) (2 ulp), then the knee's difference, the slope's product and the profile's difference;
+      y: gk = fmaf(fl(g1 - g0), k / 128, g0), exp2f (2 ulp) of fl(gk fl(log2(10) / 20)), then the K-term FMA band sum;
+         0 where g0 and g1 are 0 dB everywhere (the delayed input)."""
+    C = x.shape[0]
+    K, L = bank.shape
+    w, band, ok = bands(st, x, bank)
+    aw = np.abs(w)
+    beta = gamma(L) * np.stack([[np.convolve(aw[c], np.abs(bank[b]), "valid") for b in range(K)] for c in range(C)])
+    out = {}
+    if ok:
+        P, S = detect(st["S"], band, attack, release)
+        big = np.abs(band) + beta
+        eP = ((2 * np.abs(band) * beta + beta ** 2).sum(axis=(0, 2)) + gamma(C + 8) * (big ** 2).sum(axis=(0, 2))) \
+            / (HOP * C) * (1 + 3 * U) + 2 * U * P
+        d = np.abs(P - st["S"])
+        c = np.maximum(attack, release)
+        eS = c * (eP * (1 + U) + U * d) + U * (np.abs(S) + c * eP) + np.where(d <= eP, abs(attack - release) * (d + eP), 0)
+        out["S"] = eS
+    else:
+        out["S"] = np.zeros(K)                      # the detectors keep their bits
+    with np.errstate(divide="ignore", invalid="ignore"):
+        lg = np.where(S1 > 0, np.log10(np.where(S1 > 0, S1, 1.0)), 0.0)
+    t = 10 * lg
+    et = 10 * 2 * 2.0 ** -23 * np.abs(lg) + U * np.abs(t)
+    R = np.where(S1 > 0, st["slope"] * np.maximum(0.0, t - st["knee"]), 0.0)      # 10 log10f(0) = -inf: R is 0
+    eR = np.where(S1 > 0, np.abs(st["slope"]) * (et + U * np.abs(t - st["knee"])) + U * np.abs(R), 0.0)
+    out["g"] = eR[None] + U * np.abs(st["prof"] - R[None]) * (R != 0)[None]
+    g0 = st["g"]
+    if not g0.any() and not g1.any():
+        out["y"] = np.zeros((C, HOP))
+        return out
+    gk = ramp(g0, g1)
+    egk = U * np.abs(g1 - g0)[..., None] + U * np.abs(gk)
+    earg = LOG2_10_20 * egk + np.abs(gk) * (abs(LOG2_10_20_F32 - LOG2_10_20) + U * LOG2_10_20_F32)
+    lin = np.where(gk == 0, 1.0, 10 ** (gk / 20))
+    elin = lin * (math.log(2) * earg + 2.0 ** -22) * (1 + 4 * U)
+    out["y"] = (lin * beta + np.abs(band) * elin).sum(1) + gamma(K) * ((lin + elin) * (np.abs(band) + beta)).sum(1)
+    return out
+
+
+def hop_errors(st, x, bank, got, mutant=None, attack=ATTACK, release=RELEASE):
+    """error / bound of a hop run from state st, got = {"y", "S", "g", "hist"} (its output and the state it ended with),
+    against the model or one of its mutants from st: S against detect(), g against end_gains() of got's S, y against
+    hop_out() of st's and got's gains; the history must match bit for bit (inf where it does not)"""
+    b = hop_bound(st, x, bank, got["S"], got["g"], attack, release)
+    w, band, ok = bands(st, x, bank, mutant)
+    S = detect(st["S"], band, attack, release, mutant)[1] if ok else st["S"]
+    m = {k: v.copy() for k, v in st.items()}
+    model_hop(m, x, bank, attack, release, mutant)
+    return {"y": ratio(got["y"], hop_out(w, band, st["g"], got["g"], mutant), b["y"]),
+            "S": ratio(got["S"], S, b["S"]), "g": ratio(got["g"], end_gains(st, got["S"]), b["g"]),
+            "hist": 0.0 if np.array_equal(got["hist"], m["hist"]) else math.inf}
 
 
 def model_run(x, ticks, bank, st=None, **kw):
@@ -198,6 +325,54 @@ def test_cutting_into_ticks_changes_nothing():
     runs = [model_run(x, t, BANK, st={k: v.copy() for k, v in st0.items()}) for t in ([90], cuts(90, 5), cuts(90, 6))]
     for y, st, _ in runs[1:]:
         assert np.array_equal(y, runs[0][0]) and all(np.array_equal(st[k], runs[0][1][k]) for k in st)
+
+
+def random_bank(K, L, seed):
+    """a seeded asymmetric bank [K, L] of fp32 values: unlike the designed one, it shows the order of the taps"""
+    return np.random.default_rng(seed).uniform(-0.3, 0.3, (K, L)).astype(np.float32).astype(np.float64)
+
+
+def test_state_row_round_trips():
+    C, K, L = 3, 4, 37
+    row = (np.arange(C * (5 * K + L - 1)).reshape(C, -1) * 0.37 - 5).astype(np.float32)
+    row[1:, 2 * K:5 * K] = 0
+    st = from_row(row, K)
+    assert st["S"].tolist() == row[0, 2 * K:3 * K].tolist() and np.array_equal(st["hist"], row[:, 5 * K:])
+    assert np.array_equal(to_row(st).view(np.int32), row.view(np.int32))
+
+
+def mutant_case():
+    """a hop of 2 channels through a random bank of 161 taps (a history of 160 samples): the detectors attack, every
+    gain moves, and the channels differ"""
+    C, K, L = 2, 4, 161
+    bank = random_bank(K, L, 3)
+    st = model_state(C, K, L)
+    set_profile(st, np.array([[6, -3, 9, 2], [1, 4, -5, 8]]), knees=-60.0, ratios=[2, 3, 1.5, 4])
+    st["S"], st["g"] = np.full(K, 1e-5), np.full((C, K), 3.0)
+    x = speech(C, 3, 7, db=-3.0)
+    st["hist"] = x[:, :L - 1].copy()
+    return st, x[:, 2 * HOP:], bank
+
+
+def test_bounds_are_zero_where_the_arithmetic_is_exact():
+    st, x, bank = mutant_case()
+    st["hist"][:] = 0
+    st["S"][:] = 0
+    b = hop_bound(st, np.zeros_like(x), bank, np.zeros(4), end_gains(st, np.zeros(4)))
+    assert all(not v.any() for v in b.values())                  # silence: every band, level and gain is exact
+    st["g"][:], st["prof"][:] = 0, 0
+    b = hop_bound(st, x, bank, np.zeros(4), np.zeros((2, 4)))
+    assert not b["y"].any() and not b["g"].any()                 # 0 dB at both ends: the delayed input
+
+
+def test_mutants_miss_their_bounds():
+    st, x, bank = mutant_case()
+    m = {k: v.copy() for k, v in st.items()}
+    y = model_hop(m, x, bank)
+    got = {"y": y, "S": m["S"], "g": m["g"], "hist": m["hist"]}
+    assert max(hop_errors(st, x, bank, got).values()) == 0
+    for mutant in MUTANTS:
+        assert max(hop_errors(st, x, bank, got, mutant).values()) >= SENSITIVITY, mutant
 
 
 # ---- the library -----------------------------------------------------------------------------------------------------

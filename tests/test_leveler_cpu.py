@@ -9,6 +9,7 @@ import pytest
 import torch
 from scipy.signal import lfilter
 
+from kernels.scaffold import SENSITIVITY, ratio
 from lookoncetohear_b200 import Leveler
 from serving_util import declaration, doc_before, header
 
@@ -47,23 +48,198 @@ def model_state(C):
     return {"shelf": np.zeros((C, 2)), "hp": np.zeros((C, 2)), "E": 0.0, "n": 0, "g": 0.0}
 
 
-def model_hop(st, x, p=DEFAULTS):
-    """l2h_leveler on one hop of one row: x [C, 128] float64 (float32 values), returns the leveled hop; advances st"""
+FILTERS32 = tuple(f.astype(np.float32).astype(np.float64) for f in FILTERS)     # the coefficients lv_filters rounds
+INT32_MAX = 2 ** 31 - 1
+
+# Mutants of the model, each a plausible kernel bug (model_hop(mutant=...)): the gain ramp one sample early, the
+# estimate's weight max(alpha, 1 / n), the relative gate ignored, d taken one hop after `settle`, the power of channel 0
+# only, the rise clamp dropped.
+MUTANTS = ("early", "weight", "relative", "settle", "channel0", "rise")
+
+
+def measured(x):
+    return bool(np.isfinite(x).all() and np.abs(x).max() < BIG)
+
+
+def gain_step(g, E, n, before, p=DEFAULTS, mutant=None):
+    """the gain (dB) at the end of a measured hop that started at g with `before` gated hops and ends with n and E"""
+    settle = p["settle"] + (mutant == "settle")
+    if n < settle:
+        return g
+    d = min(max(p["target"] - lufs(E), p["min_gain"]), p["max_gain"])
+    if before < settle:
+        return d
+    return g + (max(d - g, -p["fall"]) if mutant == "rise" else min(max(d - g, -p["fall"]), p["rise"]))
+
+
+def hop_out(x, g0, g1, mutant=None):
+    k = np.arange(HOP) + (mutant != "early")
+    gk = g0 + (g1 - g0) * k / HOP
+    return x * np.where(gk == 0, 1.0, 10 ** (gk / 20))
+
+
+def model_hop(st, x, p=DEFAULTS, coefs=FILTERS, mutant=None, gated=None):
+    """l2h_leveler on one hop of one row: x [C, 128] float64 (float32 values), returns the leveled hop; advances st.
+    coefs: the filters (FILTERS32: the kernel's fp32 coefficients); gated: the gates' decision, when not the model's.
+    The gated-hop count saturates at INT32_MAX, and a negative count word counts as 0, as in the kernel."""
     g0 = st["g"]
-    if np.isfinite(x).all() and np.abs(x).max() < BIG:
-        sb, sa, hb, ha = FILTERS
+    st["n"] = max(st["n"], 0)
+    if measured(x):
+        sb, sa, hb, ha = coefs
         u, st["shelf"] = lfilter(sb, sa, x, axis=1, zi=st["shelf"])
         w, st["hp"] = lfilter(hb, ha, u, axis=1, zi=st["hp"])
-        P = float((w ** 2).sum()) / HOP
+        P = float(((w[:1] if mutant == "channel0" else w) ** 2).sum()) / HOP
         L, before = lufs(P), st["n"]
-        if L >= p["gate"] and (st["n"] == 0 or L >= lufs(st["E"]) + p["relative"]):
-            st["E"] += max(p["alpha"], 1 / (st["n"] + 1)) * (P - st["E"])
-            st["n"] += 1
-        if st["n"] >= p["settle"]:
-            d = min(max(p["target"] - lufs(st["E"]), p["min_gain"]), p["max_gain"])
-            st["g"] = d if before < p["settle"] else st["g"] + min(max(d - st["g"], -p["fall"]), p["rise"])
-    gk = g0 + (st["g"] - g0) * np.arange(1, HOP + 1) / HOP
-    return x * np.where(gk == 0, 1.0, 10 ** (gk / 20))
+        if gated is None:
+            gated = L >= p["gate"] and (st["n"] == 0 or mutant == "relative" or L >= lufs(st["E"]) + p["relative"])
+        if gated:
+            n = max(st["n"], 1) if mutant == "weight" else st["n"] + 1
+            st["E"] += max(p["alpha"], 1 / n) * (P - st["E"])
+            st["n"] = min(st["n"] + 1, INT32_MAX)
+        st["g"] = gain_step(st["g"], st["E"], st["n"], before, p, mutant)
+    return hop_out(x, g0, st["g"], mutant)
+
+
+# ---- the kernel's state row and the error bound of one hop ----------------------------------------------------------
+U = 2.0 ** -24                       # the unit roundoff of fp32
+LOG2_10_20 = math.log2(10) / 20
+LOG2_10_20_F32 = float(np.float32(LOG2_10_20))
+
+
+def from_row(row):
+    """a row's state [C, 7] as the kernel keeps it (fp32) -> the model's state; the count word as the int32 it holds"""
+    r = np.ascontiguousarray(row, np.float32)
+    return {"E": float(r[0, 0]), "n": int(r[0, 1:2].view(np.int32)[0]), "g": float(r[0, 2]),
+            "shelf": r[:, 3:5].astype(np.float64), "hp": r[:, 5:7].astype(np.float64)}
+
+
+def to_row(st):
+    C = st["shelf"].shape[0]
+    row = np.zeros((C, FLOATS), np.float32)
+    row[0, 0], row[0, 2] = st["E"], st["g"]
+    row[0, 1:2].view(np.int32)[0] = st["n"]
+    row[:, 3:5], row[:, 5:7] = st["shelf"], st["hp"]
+    return row
+
+
+def lufs_err(v, ev=0.0):
+    """the error of the kernel's -0.691f + 10 log10f(v) at a v within ev of the float64 v: log10f's 2 ulp, the product's
+    and the sum's roundings, -0.691f's own, and ev carried through the logarithm"""
+    if v <= 0:
+        return 0.0 if ev == 0 else math.inf
+    lg = math.log10(v)
+    return (10 * 10 / math.log(10) * ev / v if ev else 0.0) + 20 * 2.0 ** -23 * abs(lg) + U * abs(10 * lg) \
+        + U * abs(lufs(v)) + abs(float(np.float32(-0.691)) + 0.691)
+
+
+def filter_bound(st, x, coefs=FILTERS32):
+    """The two sections in transposed direct form II, one fmaf per step as the kernel runs them: (the float64 states
+    [C, 4], their error bounds, the per-channel sums of the squared weighted samples [C] and their bounds).  Each step's
+    roundings (u |value| per rounded result) are carried to later steps through the powers of the sections' state
+    matrix M, in absolute value: |M^m| stays small where |M|^m, with the high-pass's poles near 1, would not.  The
+    error of u = fl(sb0 x + s1) enters as one of s1.  A thread accumulates channels c, c + 128, ... into one sum, so a
+    channel's rounding terms are counted against its thread's running sum."""
+    (sb0, sb1, sb2), (_, sa1, sa2), _, (_, ha1, ha2) = coefs
+    M = np.array([[-sa1, 1, 0, 0], [-sa2, 0, 0, 0], [-2 - ha1, 0, -ha1, 1], [1 - ha2, 0, -ha2, 0]])
+    Mp = [np.eye(4)]
+    for _ in range(HOP):
+        Mp.append(M @ Mp[-1])
+    Mp = np.array(Mp)                                          # [HOP + 1, 4, 4]
+    cM = np.abs(Mp[:, 0] + Mp[:, 2])                           # w = u + h1 = s1 + h1 + sb0 x: [HOP + 1, 4]
+    C = len(x)
+    s1, s2 = st["shelf"][:, 0].copy(), st["shelf"][:, 1].copy()
+    h1, h2 = st["hp"][:, 0].copy(), st["hp"][:, 1].copy()
+    a, b, W = np.zeros((C, HOP, 4)), np.zeros((C, HOP, 4)), np.zeros((C, HOP))
+    for k in range(HOP):
+        xk = x[:, k]
+        u = sb0 * xk + s1
+        inner = -sa1 * u + s2
+        s1n = sb1 * xk + inner
+        prod = -sa2 * u
+        s2 = sb2 * xk + prod
+        w = u + h1
+        inner2 = -ha1 * w + h2
+        h1n = -2 * u + inner2
+        h2 = -ha2 * w + u
+        a[:, k, 0] = U * np.abs(u)
+        b[:, k] = np.stack([U * (np.abs(inner) + np.abs(s1n)), U * (np.abs(prod) + np.abs(s2)),
+                            U * (np.abs(inner2) + np.abs(h1n) + abs(ha1) * np.abs(w)),
+                            U * (np.abs(h2) + abs(ha2) * np.abs(w))], 1)
+        s1, h1, W[:, k] = s1n, h1n, w
+    j = np.arange(HOP)
+    e = np.einsum("jst,cjt->cs", np.abs(Mp[HOP - j]), a) + np.einsum("jst,cjt->cs", np.abs(Mp[HOP - 1 - j]), b)
+    lag = j[:, None] - j[None, :]                              # k - j
+    Ta = np.where((lag > 0)[..., None], cM[np.clip(lag, 0, HOP)], 0.0)
+    Tb = np.where((lag > 0)[..., None], cM[np.clip(lag - 1, 0, HOP)], 0.0)
+    ew = np.einsum("kjs,cjs->ck", Ta, a) + np.einsum("kjs,cjs->ck", Tb, b) + a[:, :, 0] + U * np.abs(W)
+    A = (W * W).sum(1)
+    eA = (2 * np.abs(W) * ew + ew * ew).sum(1) + U * np.cumsum(W * W, 1).sum(1)
+    for c in range(128, C):                                    # the sums of the thread's earlier channels
+        eA[c] += HOP * U * (A[c % 128:c:128] + eA[c % 128:c:128]).sum()
+    grow = 1 + 8 * U
+    return np.stack([s1, s2, h1, h2], 1), e * grow, A, eA * grow
+
+
+def hop_errors(st, x, p, got, mutant=None, coefs=FILTERS32):
+    """error / bound of a hop run from state st, got = from_row() of the state it ended with plus its output "y", against
+    the model or one of its mutants from st.  The count word must match exactly; where the float64 loudness lies within
+    its bound of a gate, the kernel's branch (shown by its count, or by its estimate at a saturated count) is taken.
+      filters: filter_bound's running bounds;  P: the per-channel sums within their bounds, summed over min(C, 128)
+      thread sums from 0;  E: fmaf(w, fl(P - E), E), w = max(alpha, fl(1 / fl(n + 1))) within 2 roundings of 1 / (n + 1);
+      g: from the kernel's own E, lufs_err, then the target's, d - g's and the step's roundings;
+      y: from the kernel's own start and end gains: fmaf(fl(g1 - g0), k / 128, g0), exp2f (2 ulp), the product."""
+    g0, n0 = st["g"], max(st["n"], 0)
+    out = {}
+    if not measured(x):
+        same = got["E"] == st["E"] and got["n"] == n0 and got["g"] == g0 and \
+            np.array_equal(got["shelf"], st["shelf"]) and np.array_equal(got["hp"], st["hp"])
+        out["state"] = 0.0 if same else math.inf
+        g1, eg = got["g"], 0.0
+    else:
+        ref, ef, A, eA = filter_bound(st, x, coefs)
+        out["filters"] = ratio(np.concatenate([got["shelf"], got["hp"]], 1), ref, ef)
+        m = min(len(x), 128)
+        P, eP = A.sum() / HOP, (eA.sum() + gamma(m) * (A + eA).sum()) / HOP
+        L, eL = lufs(P), lufs_err(P, eP)
+        ambiguous = abs(L - p["gate"]) <= eL or (
+            n0 > 0 and abs(L - lufs(st["E"]) - p["relative"]) <= eL + lufs_err(st["E"]) + U * abs(lufs(st["E"]) + p["relative"]))
+        took = got["n"] != n0 if n0 < INT32_MAX else got["E"] != st["E"]
+        mst = dict(st, shelf=st["shelf"].copy(), hp=st["hp"].copy())
+        model_hop(mst, x, p, coefs, mutant, gated=took if ambiguous else None)
+        out["n"] = 0.0 if got["n"] == mst["n"] else math.inf
+        if mst["n"] != n0 or (n0 == INT32_MAX and mst["E"] != st["E"]):          # gated
+            wgt = max(p["alpha"], 1 / (n0 + 1))
+            d = abs(P - st["E"])
+            eE = wgt * (eP + U * (d + eP)) + 2 * U * wgt * d + U * abs(mst["E"])
+            if mutant == "channel0":
+                eE += wgt * eP                                                   # its own P, not the bound's
+            out["E"] = ratio(got["E"], mst["E"], eE * (1 + 4 * U))
+        else:
+            out["E"] = 0.0 if got["E"] == st["E"] else math.inf
+        g1 = gain_step(g0, got["E"], mst["n"], n0, p, mutant)
+        settle = p["settle"] + (mutant == "settle")
+        eg = 0.0
+        if mst["n"] >= settle:
+            LE = lufs(got["E"])
+            t = p["target"] - LE
+            d = min(max(t, p["min_gain"]), p["max_gain"])
+            eg = lufs_err(got["E"]) + U * abs(t)
+            if n0 >= settle:
+                eg += U * abs(d - g0) + U * abs(g1)
+        out["g"] = ratio(got["g"], g1, eg * (1 + 4 * U))
+    gk = g0 + (got["g"] - g0) * np.arange(1, HOP + 1) / HOP
+    egk = U * abs(got["g"] - g0) + U * np.abs(gk)
+    earg = LOG2_10_20 * egk + np.abs(gk) * (abs(LOG2_10_20_F32 - LOG2_10_20) + U * LOG2_10_20_F32)
+    lin = np.where(gk == 0, 1.0, 10 ** (gk / 20))
+    elin = lin * (math.log(2) * earg + 2.0 ** -22)
+    y = hop_out(x, g0, got["g"], mutant)
+    exact = g0 == 0 and got["g"] == 0                              # a gain of 0 dB is exactly 1
+    out["y"] = ratio(got["y"], y, 0.0 if exact else (np.abs(x) * elin + U * np.abs(y)) * (1 + 4 * U))
+    return out
+
+
+def gamma(n):
+    return n * U / (1 - n * U)
 
 
 def model_run(x, ticks, p=DEFAULTS, st=None):
@@ -185,6 +361,56 @@ def test_identity_at_zero_gain_range():
     x = voice(2, 100, 8)
     y, st, _ = model_run(x, [100], dict(DEFAULTS, min_gain=0.0, max_gain=0.0))
     assert np.array_equal(y, x) and st["g"] == 0 and st["n"] > 0
+
+
+def test_state_row_round_trips():
+    row = (np.arange(3 * FLOATS).reshape(3, FLOATS) * 0.37 - 2).astype(np.float32)
+    row[1:, :3] = 0
+    row[0, 1:2].view(np.int32)[0] = -5
+    st = from_row(row)
+    assert st["n"] == -5 and st["E"] == row[0, 0] and np.array_equal(st["hp"], row[:, 5:])
+    assert np.array_equal(to_row(st).view(np.int32), row.view(np.int32))
+
+
+P_MUT = dict(DEFAULTS, settle=4, alpha=float(np.float32(0.01)), rise=0.05, fall=0.05)
+
+
+def mutant_cases():
+    """mutant -> (state, hop): a gated, rate-limited hop of two channels at different levels (the ramp, the weight,
+    channel 0's power, the rise clamp); a hop over the absolute gate and 30 dB under the estimate (the relative gate);
+    the hop that reaches `settle` (d one hop late)"""
+    x = voice(2, 40, 9, db=-6.0)
+    st = model_state(2)
+    model_run(x[:, :30 * HOP], [30], P_MUT, st)
+    hop = x[:, 30 * HOP:31 * HOP]
+    a = dict(st, n=5, g=-6.0, E=st["E"] * 0.5)
+    b = dict(st, n=5, E=st["E"] * 1000)
+    c = dict(st, n=P_MUT["settle"] - 1)
+    return {"early": (a, hop), "weight": (a, hop), "channel0": (a, hop), "rise": (a, hop), "relative": (b, hop),
+            "settle": (c, hop)}
+
+
+def kernel_like(st, x, p):
+    """the model's own hop as a kernel's result: its end state and output"""
+    m = dict(st, shelf=st["shelf"].copy(), hp=st["hp"].copy())
+    y = model_hop(m, x, p, FILTERS32)
+    return dict(m, y=y)
+
+
+def test_bounds_are_zero_where_the_arithmetic_is_exact():
+    st, x = model_state(3), np.zeros((3, HOP))
+    errs = hop_errors(st, x, P_MUT, kernel_like(st, x, P_MUT))
+    assert all(v == 0 for v in errs.values())
+    x = voice(3, 1, 4)                                            # 0 dB at both ends: the input itself
+    got = kernel_like(st, x, P_MUT)
+    assert np.array_equal(got["y"], x) and hop_errors(st, x, P_MUT, dict(got, y=x * (1 + U)))["y"] == math.inf
+
+
+def test_mutants_miss_their_bounds():
+    for mutant, (st, x) in mutant_cases().items():
+        got = kernel_like(st, x, P_MUT)
+        assert max(hop_errors(st, x, P_MUT, got).values()) < 1e-6, mutant      # lfilter's float64 roundings
+        assert max(hop_errors(st, x, P_MUT, got, mutant).values()) >= SENSITIVITY, mutant
 
 
 # ---- the library -----------------------------------------------------------------------------------------------------

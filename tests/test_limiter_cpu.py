@@ -2,12 +2,14 @@
 of tests/test_limiter_gpu.py) with its own checks; the layout; the argument errors of both C entries, returned before
 anything is enqueued; the Python checks of Limiter; the header; the exports."""
 import ctypes
+import itertools
 import math
 
 import numpy as np
 import pytest
 import torch
 
+from kernels.scaffold import SENSITIVITY, ratio
 from lookoncetohear_b200 import Limiter
 from serving_util import FAKE_DEV, declaration, doc_before, header
 
@@ -24,30 +26,122 @@ def model_state(C, La):
             "limited": 0, "db": 0.0}
 
 
-def model_push(st, x, ceiling, La, step):
-    """l2h_limiter on one slot: x [C, n] float64 (float32 values) pushed, returns y [C, n]; advances st"""
-    C, n = x.shape
-    lim = st["ceil"] if st["ceil"] > 0 else ceiling
+FLT_MIN, FLT_MAX = float(np.finfo(np.float32).tiny), float(np.finfo(np.float32).max)
+INT32_MAX = 2 ** 31 - 1
+U = 2.0 ** -24
+
+# Mutants of the model, each a plausible kernel bug (model_push(mutant=...)): the hold one sample short, the box one
+# sample short, r carried in from 0, the slot's ceiling ignored, a non-finite sample's level taken as 0 instead of muting.
+MUTANTS = ("hold", "box", "carry", "ceiling", "nonfinite")
+
+
+def q_words(x, lim, mutant=None):
+    """each sample's q [n] and where Q log2(p / ceiling) lies within 1e-9 of an integer, so that the device's double
+    log2 may round the other way [n]"""
     finite = np.isfinite(x)
     p = np.abs(np.where(finite, x, 0.0)).max(0)
-    q = np.zeros(n, np.int64)
+    q = np.zeros(p.shape, np.int64)
+    near = np.zeros(p.shape, bool)
     over = p > lim
-    with np.errstate(divide="ignore"):
-        q[over] = np.minimum(MUTE, np.ceil(Q * np.log2(p[over] / lim)) + 1).astype(np.int64)
-    q[~finite.all(0)] = MUTE
-    qa = np.concatenate([st["qh"], q])
+    v = Q * np.log2(p[over] / lim)
+    q[over] = np.minimum(MUTE, np.ceil(v) + 1).astype(np.int64)
+    near[over] = np.abs(v - np.round(v)) < 1e-9
+    if mutant != "nonfinite":
+        q[~finite.all(0)] = MUTE
+    return q, near
+
+
+def model_push(st, x, ceiling, La, step, mutant=None, q=None, trace=None):
+    """l2h_limiter on one slot: x [C, n] float64 (float32 values) pushed, returns y [C, n]; advances st.  As in the
+    kernel, the slot's ceiling applies where it is a positive normal float, history and r words count within [0, MUTE]
+    and the count of limited samples saturates; q: the push's q words, when not the model's own; trace: a dict that
+    receives the box sums a."""
+    C, n = x.shape
+    c = st["ceil"]
+    lim = c if FLT_MIN <= c <= FLT_MAX and mutant != "ceiling" else ceiling
+    if q is None:
+        q = q_words(x, lim, mutant)[0]
+    qa = np.concatenate([np.clip(st["qh"], 0, MUTE), q])
     s = np.lib.stride_tricks.sliding_window_view(qa, La + 1).max(1)                # q[k - La .. k]
+    if mutant == "hold" and La:
+        s = np.lib.stride_tricks.sliding_window_view(qa[1:], La).max(1)
     k = np.arange(n, dtype=np.int64)
-    r = np.maximum(st["r"] - (k + 1) * step, np.maximum.accumulate(s + k * step) - k * step)
-    ra = np.concatenate([st["rh"], r])
+    r_in = 0 if mutant == "carry" else min(max(st["r"], 0), MUTE)
+    r = np.maximum(r_in - (k + 1) * step, np.maximum.accumulate(s + k * step) - k * step)
+    ra = np.concatenate([np.clip(st["rh"], 0, MUTE), r])
     a = np.lib.stride_tricks.sliding_window_view(ra, La + 1).sum(1)                # r[k - La .. k]
+    if mutant == "box" and La:
+        a = np.lib.stride_tricks.sliding_window_view(ra[1:], La).sum(1)
     g = np.where(a >= MUTE * (La + 1), 0.0, 2.0 ** (-a / (Q * (La + 1))))
     xs = np.concatenate([st["xd"], x], 1)
     xd = xs[:, :n]
     y = np.where(np.isfinite(xd), g * np.where(np.isfinite(xd), xd, 0.0), 0.0)
-    st.update(xd=xs[:, n:], qh=qa[n:], rh=ra[n:], r=int(r[-1]), limited=min(2 ** 31 - 1, st["limited"] + int((a > 0).sum())),
+    st.update(xd=xs[:, n:], qh=qa[n:], rh=ra[n:], r=int(r[-1]),
+              limited=min(INT32_MAX, max(st["limited"], 0) + int((a > 0).sum())),
               db=float(a[-1] / (Q * (La + 1)) * 20 * math.log10(2)))
+    if trace is not None:
+        trace["a"] = a
     return y
+
+
+def from_row(row, La):
+    """a slot's state rows [C, 4 + 3 La] as the kernel keeps them (fp32) -> the model's state; int32 words as they are"""
+    r = np.ascontiguousarray(row, np.float32)
+    i = r.view(np.int32)
+    return {"xd": r[:, HEAD:HEAD + La].astype(np.float64), "qh": i[0, HEAD + La:HEAD + 2 * La].astype(np.int64),
+            "rh": i[0, HEAD + 2 * La:].astype(np.int64), "r": int(i[0, 0]), "ceil": float(r[0, 1]),
+            "limited": int(i[0, 2]), "db": float(r[0, 3])}
+
+
+def to_row(st, C):
+    La = st["qh"].shape[0]
+    row = np.zeros((C, HEAD + 3 * La), np.float32)
+    i = row.view(np.int32)
+    i[0, 0], row[0, 1], i[0, 2], row[0, 3] = st["r"], st["ceil"], st["limited"], st["db"]
+    row[:, HEAD:HEAD + La] = st["xd"]
+    i[0, HEAD + La:HEAD + 2 * La], i[0, HEAD + 2 * La:] = st["qh"], st["rh"]
+    return row
+
+
+def push_bound(x, xd, a, La):
+    """the bound of each output sample of a push whose box sums are a [n] (the model's), its delayed inputs xd [C, n]:
+    0 where a = 0 (the input itself), where a mutes (exactly 0) and where x is not finite (0); else the gain 2^-e as
+    exp2f of the fraction's fp32 rounding (2 ulp) times 2^-floor(e), the product's rounding, and 2^-149 where ldexpf
+    rounds a subnormal result"""
+    e = a / (Q * (La + 1))
+    f = e - np.floor(e)
+    gf = 2.0 ** -f
+    eg = gf * math.log(2) * (U * f + 2.0 ** -50) + 2.0 ** -23
+    b = 2.0 ** -np.floor(e) * np.abs(np.where(np.isfinite(xd), xd, 0.0)) * (eg + U * gf) * (1 + 4 * U) + 2.0 ** -149
+    return np.where((a == 0) | (a >= MUTE * (La + 1)) | ~np.isfinite(xd), 0.0, b)
+
+
+def push_errors(st, x, ceiling, La, step, got, mutant=None):
+    """error / bound of a push run from state st, got = from_row() of the state it ended with plus its output "y":
+    every integer word and the delay line bit for bit (inf where one differs), y within push_bound and the reduction
+    word within its double-to-float rounding.  Where q is within 1e-9 of a quantum's edge either q is accepted: the
+    variant whose words match the kernel's is compared."""
+    c = st["ceil"]
+    lim = c if FLT_MIN <= c <= FLT_MAX and mutant != "ceiling" else ceiling
+    q, near = q_words(x, lim, mutant)
+    best = None
+    for bump in itertools.product((0, 1), repeat=min(int(near.sum()), 4)):
+        qv = q.copy()
+        qv[np.flatnonzero(near)[:len(bump)]] -= np.array(bump, np.int64)
+        m = {k: (v.copy() if isinstance(v, np.ndarray) else v) for k, v in st.items()}
+        tr = {}
+        y = model_push(m, x, ceiling, La, step, mutant, qv, tr)
+        same = all(np.array_equal(got[k], m[k]) for k in ("qh", "rh")) and got["r"] == m["r"] and \
+            got["limited"] == m["limited"] and np.float32(got["ceil"]).view(np.int32) == np.float32(st["ceil"]).view(np.int32)
+        same = same and np.array_equal(np.asarray(got["xd"], np.float32).view(np.int32),
+                                       np.asarray(m["xd"], np.float32).view(np.int32))
+        xd = np.concatenate([st["xd"], x], 1)[:, :x.shape[1]]
+        errs = {"words": 0.0 if same else math.inf,
+                "y": ratio(got["y"], y, push_bound(x, xd, tr["a"], La)),
+                "db": ratio(got["db"], m["db"], U * abs(m["db"]) * (1 + 2.0 ** -20))}
+        if best is None or max(errs.values()) < max(best.values()):
+            best = errs
+    return best
 
 
 def model_run(x, pushes, ceiling=CEILING, La=16, step=20):
@@ -105,6 +199,48 @@ def test_model_split_invariance():
         y2, st2 = model_run(x, cuts(40000, seed), La=44, step=19)
         assert np.array_equal(y, y2)
         assert all(np.array_equal(st[k], st2[k]) for k in st)
+
+
+def test_state_row_round_trips():
+    row = (np.arange(3 * (HEAD + 3 * 5)).reshape(3, -1) * 0.37 - 2).astype(np.float32)
+    i = row.view(np.int32)
+    i[0, 0], i[0, 2], i[0, HEAD + 5:] = -7, INT32_MAX - 3, np.arange(10) * 70000 - 3
+    row[1:, :HEAD], row[1:, HEAD + 5:] = 0, 0
+    st = from_row(row, 5)
+    assert st["r"] == -7 and st["limited"] == INT32_MAX - 3 and st["qh"][0] == -3
+    assert np.array_equal(to_row(st, 3).view(np.int32), i)
+
+
+def mutant_case():
+    """a push of 2 channels with peaks over the slot's own ceiling and a NaN, from a slot releasing a large r"""
+    La = 8
+    st = model_state(2, La)
+    st.update(r=3 * Q, ceil=0.5, rh=np.full(La, 3 * Q), qh=np.full(La, Q))
+    x = loud(2, 300, 11, peak=12.0)
+    x[1, 250] = np.nan
+    return st, x, La
+
+
+def kernel_like(st, x, La, step=20):
+    m = {k: (v.copy() if isinstance(v, np.ndarray) else v) for k, v in st.items()}
+    y = model_push(m, x, CEILING, La, step)
+    return dict(m, y=y, db=float(np.float32(m["db"])))
+
+
+def test_bounds_are_zero_where_the_arithmetic_is_exact():
+    st = model_state(2, 4)
+    x = loud(2, 200, 12, peak=0.5)                                 # under the ceiling: a = 0, the input delayed
+    assert not push_bound(x, x, np.zeros(200, np.int64), 4).any()
+    assert not push_bound(x, x, np.full(200, MUTE * 5), 4).any()  # muted: exactly 0
+    assert max(push_errors(st, x, CEILING, 4, 20, kernel_like(st, x, 4)).values()) == 0
+
+
+def test_mutants_miss_their_bounds():
+    st, x, La = mutant_case()
+    got = kernel_like(st, x, La, 2000)
+    assert max(push_errors(st, x, CEILING, La, 2000, got).values()) <= 1.0
+    for mutant in MUTANTS:
+        assert max(push_errors(st, x, CEILING, La, 2000, got, mutant).values()) >= SENSITIVITY, mutant
 
 
 def test_model_release_and_mute():
