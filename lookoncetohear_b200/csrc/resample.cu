@@ -394,13 +394,14 @@ hop_fifo_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, int ma
     const int pos = int_word(st[0], R - 1), held = int_word(st[1], capacity);
     const int kept = min(n, capacity - held), h = min(T, (held + kept) / CHUNK_HOP);
     const float* xr = row_ch(x, x_row, x_ch, r.row, r.ch);
-    for (int i = tid; i < kept; i += blockDim.x) ring[(pos + held + i) % R] = xr[i];
+    // ring indices in int64: pos + held + i reaches 2 capacity + 62, which passes INT32_MAX from capacity ~2^30 on
+    for (int i = tid; i < kept; i += blockDim.x) ring[((int64_t)pos + held + i) % R] = xr[i];
     __syncthreads();                                                    // the appended samples, visible to the block
     float* cr = row_ch(chunk, c_row, c_ch, r.row, r.ch);
-    for (int i = tid; i < h * CHUNK_HOP + CHUNK_CARRY; i += blockDim.x) cr[i] = ring[(pos + R - CHUNK_CARRY + i) % R];
+    for (int i = tid; i < h * CHUNK_HOP + CHUNK_CARRY; i += blockDim.x) cr[i] = ring[((int64_t)pos + R - CHUNK_CARRY + i) % R];
     if (tid == 0) {
         if (r.ch == 0) hops[r.row] = h;
-        st[0] = __int_as_float((pos + h * CHUNK_HOP) % R);
+        st[0] = __int_as_float((int)(((int64_t)pos + h * CHUNK_HOP) % R));
         st[1] = __int_as_float(held + kept - h * CHUNK_HOP);
         st[2] = add_word(st[2], n - kept);
     }
@@ -427,7 +428,7 @@ enroll_capture_kernel(const float* __restrict__ chunk, int64_t c_row, int64_t c_
     __syncthreads();                                                    // every thread has read the head
     if (tid == 0) {
         st[0] = __int_as_float((int)(((int64_t)r.wpos + n) % capacity));
-        st[1] = __int_as_float(min(r.captured + n, capacity));
+        st[1] = __int_as_float((int)min((int64_t)r.captured + n, (int64_t)capacity));
     }
 }
 

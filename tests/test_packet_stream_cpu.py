@@ -1,9 +1,13 @@
 """Packet streams without a GPU: the layout queries (l2h_resample_packets_layout, l2h_hop_fifo_layout) against the sizes of
 their definitions for every rate pair, the argument errors of l2h_resample_packets and l2h_hop_fifo, returned before anything
-touches the device, and the checks of lookoncetohear_b200.PacketResampler and HopFifo that run before any CUDA call."""
+touches the device, and the checks of lookoncetohear_b200.PacketResampler and HopFifo that run before any CUDA call.  Also
+the exact host models of one push through the hop FIFO and the enrollment capture (fifo_push, capture_push), with their
+own checks."""
+import collections
 import ctypes
 import math
 
+import numpy as np
 import pytest
 import torch
 
@@ -72,6 +76,98 @@ def test_history_covers_every_phase(orig, new):
 def test_the_44k_family(lib, orig, new, w, delay):
     assert rate(orig, new)[2] == w
     assert layout(lib, orig, new, 882)[1][1] == delay
+
+
+# ---- host models of the hop FIFO and the enrollment capture ----------------------------------------------------------
+# One row of one channel, from a given state row: the head words as Python ints (the int32 words of the state) and a ring
+# that is any indexable of floats.  Each returns what the kernel writes: its chunk and hop count, the new head, and the
+# ring words written as {ring index: value}.  Python ints cannot overflow, so the models hold at any capacity.
+INT32_MAX = 2 ** 31 - 1
+FF_HEAD, EC_HEAD, HOP, CARRY = 3, 2, 128, 64
+
+
+def clamp(w, hi):
+    """an int32 head word clamped into [0, hi]"""
+    return min(max(w, 0), hi)
+
+
+def fifo_push(head, ring, x, capacity, T):
+    """hop_fifo_kernel for one (row, channel) of a live slot: head (pos, held, dropped), the pushed samples x (empty for
+    a count outside [0, max_in]).  Returns (chunk [128 h + 64], h, new head, writes)."""
+    R = CARRY + capacity
+    pos, held = clamp(head[0], R - 1), clamp(head[1], capacity)
+    n = len(x)
+    kept = min(n, capacity - held)
+    writes = {(pos + held + i) % R: x[i] for i in range(kept)}
+    h = min(T, (held + kept) // HOP)
+    chunk = [writes.get(k, ring[k]) for k in ((pos + R - CARRY + i) % R for i in range(HOP * h + CARRY))]
+    dropped = min(max(head[2], 0) + n - kept, INT32_MAX)
+    return chunk, h, ((pos + HOP * h) % R, held + kept - HOP * h, dropped), writes
+
+
+def capture_push(head, new, capacity):
+    """enroll_capture_kernel for one (row, channel) of a live slot with h in [1, T]: head (wpos, captured), the hops'
+    new samples `new` (chunk samples 64 .. 64 + 128 h - 1).  Returns (new head, writes): only the last `capacity` samples
+    are written."""
+    wpos, captured = clamp(head[0], capacity - 1), clamp(head[1], capacity)
+    n = len(new)
+    writes = {(wpos + i) % capacity: new[i] for i in range(max(0, n - capacity), n)}
+    return ((wpos + n) % capacity, min(captured + n, capacity)), writes
+
+
+def test_fifo_model_is_the_stream_it_was_pushed():
+    """pushes that fill, overflow and drain: each chunk is the kept samples after 64 zeros, read at the popped position,
+    and the dropped count is everything not kept"""
+    rng = np.random.default_rng(11)
+    capacity, T = 300, 2
+    ring, head = [0.0] * (CARRY + capacity), (0, 0, 0)
+    kept_all, pos, dropped = [], 0, 0
+    for n in [0, 1, 127, 300, 300, 17, 0, 0, 0, 256, 5, 400]:
+        x = rng.standard_normal(n).tolist()
+        chunk, h, new_head, writes = fifo_push(head, ring, x, capacity, T)
+        kept = min(n, capacity - head[1])
+        kept_all += x[:kept]
+        dropped += n - kept
+        stream = [0.0] * CARRY + kept_all
+        assert chunk == stream[pos:pos + HOP * h + CARRY]
+        assert h == min(T, (head[1] + kept) // HOP) and new_head[1:] == (head[1] + kept - HOP * h, dropped)
+        pos += HOP * h
+        for k, v in writes.items():
+            ring[k] = v
+        head = new_head
+    assert dropped > 0 and head[1] < capacity
+
+
+def test_fifo_model_clamps_and_saturates():
+    ring = list(range(CARRY + 200))
+    _, h, head, w = fifo_push((10 ** 6, 10 ** 6, INT32_MAX - 3), ring, [1.0] * 9, 200, 5)   # pos, held past their clamps
+    assert h == 1 and head == ((CARRY + 199 + HOP) % (CARRY + 200), 200 - HOP, INT32_MAX) and not w
+    _, h, head, w = fifo_push((-4, -1, -9), ring, [1.0] * 9, 200, 5)                       # negative words count as 0
+    assert h == 0 and head == (0, 9, 0) and sorted(w) == list(range(9))
+    cap = 2 ** 30 + 64                                      # the int32 overflow: indices past INT32_MAX, kept in the ring
+    R = CARRY + cap
+    chunk, h, head, w = fifo_push((R - 1, cap - 100, 0), collections.defaultdict(float), [2.0] * 300, cap, 3)
+    assert h == 3 and head == (HOP * 3 - 1, cap - 384, 200) and min(w) == cap - 101 and max(w) == cap - 2
+    assert (R - 1) + (cap - 100) > INT32_MAX and 2 * R - 65 > INT32_MAX
+
+
+def test_capture_model_keeps_the_last_capacity_samples():
+    cap = 200
+    ring, head = [None] * cap, (0, 0)
+    pushed = []
+    rng = np.random.default_rng(12)
+    for n in (128, 256, 128 * 3, 128):
+        new = rng.standard_normal(n).tolist()
+        head, w = capture_push(head, new, cap)
+        pushed += new
+        assert len(w) == min(n, cap)
+        for k, v in w.items():
+            ring[k] = v
+        assert head == (len(pushed) % cap, min(len(pushed), cap))
+        k = min(len(pushed), cap)
+        assert [ring[(head[0] - k + i) % cap] for i in range(k)] == pushed[-k:]
+    assert capture_push((-3, -3), [1.0] * 128, cap)[0] == (128, 128)
+    assert capture_push((cap + 5, INT32_MAX), [1.0] * 128, cap)[0] == ((cap - 1 + 128) % cap, cap)
 
 
 def test_fifo_layout(lib):

@@ -1,14 +1,16 @@
 """Packet streams on the GPU (l2h_resample_packets / PacketResampler, l2h_hop_fifo / HopFifo): ragged pushes of any length
 against `resample` of each stream's whole input delayed by D, bit for bit, and against the float64 restatement
 oracle/resample.py; whole-period pushes against StreamResampler; the FIFO's chunks, hop counts, draining and overflow
-against a host model; 48 kHz packets through the FIFO against StreamResampler(keep=64); graph replays with the lists
-rewritten in place; and a tick of 44.1 kHz listeners sending 10 ms packets, down -> FIFO -> separator -> up, against the
-same chain built from whole-signal resampling and the same hop schedule."""
+against the host model of test_packet_stream_cpu.py, every state row bit for bit; 48 kHz packets through the FIFO against
+StreamResampler(keep=64); graph replays with the lists rewritten in place; and a tick of 44.1 kHz listeners sending 10 ms
+packets, down -> FIFO -> separator -> up, against the same chain built from whole-signal resampling and the same hop
+schedule."""
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
+import test_packet_stream_cpu as ps
 from lookoncetohear_b200 import HopFifo, PacketResampler, StreamResampler, synth
 from oracle import resample as ors
 from serving_util import SENTINEL as NAN, bits, delayed, dev, i32, model, signals  # noqa: F401
@@ -90,8 +92,7 @@ def test_fifo_chunks_hops_drain_and_overflow(dev):
     fifo = HopFifo(S, C, T, cap, device=dev)
     assert fifo.state.shape == (S, C, 3 + 64 + cap) and not fifo.state.any()
     g = torch.Generator().manual_seed(606)
-    sig = [torch.zeros(C, 0) for _ in range(S)]                 # everything each slot kept
-    pos, held, dropped = [0] * S, [0] * S, [0] * S
+    held, dropped = [0] * S, [0] * S
     drained = overflowed = 0
     for t in range(60):
         sl = torch.randperm(S, generator=g)[:n].tolist()
@@ -109,19 +110,22 @@ def test_fifo_chunks_hops_drain_and_overflow(dev):
             if not 0 <= s < S:
                 assert hops[i] == 0 and torch.isnan(chunk[i]).all()
                 continue
-            kept = min(m, cap - held[s])
-            dropped[s] += m - kept
-            overflowed += m > kept
-            sig[s] = torch.cat([sig[s], x[i, :, :kept].cpu()], -1)
-            held[s] += kept
-            h = min(T, held[s] // 128)
+            for c in range(C):                                  # the host model from the row before the call
+                row = before[s, c].cpu().numpy().copy()
+                want, h, head, writes = ps.fifo_push(row[:3].view(np.int32).tolist(), row[3:], x[i, c, :m].cpu().numpy(),
+                                                     cap, T)
+                assert hops[i] == h, (t, i, s)
+                got = chunk[i, c].cpu().numpy()
+                assert np.array_equal(got[:128 * h + 64].view(np.int32), np.array(want, np.float32).view(np.int32)), (t, i, s)
+                assert np.isnan(got[128 * h + 64:]).all()
+                row[:3] = np.array(head, np.int32).view(np.float32)
+                for k, v in writes.items():
+                    row[3 + k] = v
+                assert np.array_equal(fifo.state[s, c].cpu().numpy().view(np.int32), row.view(np.int32)), (t, i, s, c)
+            held[s] = head[1]
+            dropped[s] = head[2]
+            overflowed += head[2] > int(before[s, 0, 2].view(torch.int32))
             drained += m == 0 and h > 0
-            assert hops[i] == h, (t, i, s)
-            want = F.pad(sig[s], (64, 0))[:, pos[s]:pos[s] + 128 * h + 64]
-            assert torch.equal(bits(chunk[i, :, :128 * h + 64].cpu()), bits(want)), (t, i, s)
-            assert torch.isnan(chunk[i, :, 128 * h + 64:]).all()
-            pos[s] += 128 * h
-            held[s] -= 128 * h
         assert fifo.held.tolist() == held and fifo.dropped.tolist() == dropped, t
         listed = {s for s in sl if 0 <= s < S}
         for s in set(range(S)) - listed:

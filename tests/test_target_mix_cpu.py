@@ -1,5 +1,6 @@
 """Host-side checks of the target mixer, no device: a float64 numpy model of the mix (l2h_target_mix) and of its gain
-ramps (the reference of tests/test_target_mix_gpu.py) with its own checks; the layout; the argument errors of both C
+ramps (the reference of tests/test_target_mix_gpu.py and test_stream_stage_kernels_gpu.py), the bound on the device's
+error from it and its mutants, with their own checks; the layout; the argument errors of both C
 entries, returned before anything is enqueued; the Python checks of TargetMixer; the header; the exports."""
 import ctypes
 import math
@@ -42,14 +43,23 @@ def model_state(records, slots, C):
     return np.zeros((records + slots, C, WORDS))
 
 
-def model_set(state, n_records, rows, gains, fades, starts=None):
-    """l2h_target_mix_set over state rows (records b, slots n_records + s)"""
+def model_set(state, n_records, rows, gains, fades, starts=None, with_bound=False, mutant=None):
+    """l2h_target_mix_set over state rows (records b, slots n_records + s).  With with_bound, returns [rows, C]: a bound
+    on the device's error in each row's start word, which is 0 where `starts` gives it or the set stores nothing.
+    `mutant` "set_start" starts a set without starts one sample late."""
+    bound = np.zeros(state.shape[:2])
     for e, r in enumerate(rows):
         if not (0 <= r < state.shape[0]) or not (0 <= fades[e] < 2 ** 31 - 1):
             continue
         for c in range(state.shape[1]):
-            g = level(state[r, c], 1.0 if r < n_records else 0.0) if starts is None else starts[e]
+            if starts is None:
+                g0, g1, F, p = ramp(state[r, c], 1.0 if r < n_records else 0.0)
+                G, E = ramp_gains(g0, g1, F, [p + (mutant == "set_start")])
+                g, bound[r, c] = G[0], E[0]
+            else:
+                g = starts[e]
             state[r, c] = (g, gains[e], fades[e] + 1, 0)
+    return bound if with_bound else None
 
 
 def clamped_starts(offsets, R):
@@ -57,12 +67,52 @@ def clamped_starts(offsets, R):
     return np.maximum.accumulate(np.clip(np.asarray(offsets), 0, R)).tolist()
 
 
-def model_mix(state, n_records, y, records, offsets, slots, hops=None, chunk=None, out=None):
+# The device's error.  The build has no --use_fast_math, so (float)q / (float)F is an IEEE division (0.5 ulp) and cospif
+# is the CUDA Math API's (1 ulp, its documented maximum); every other operation rounds once, to fp32.
+U = 2.0 ** -24                                              # the unit roundoff of fp32
+MIX_MUTANTS = ("q", "linear", "ambient_64", "reversed", "p_frozen", "set_start")
+
+
+def ramp_gains(g0, g1, F, k, mutant=None):
+    """(G, E): the ramp's levels after k samples (an array; the sample at ramp position q is mixed at k = q + 1) and a
+    bound on the error of the device's fp32 ramp_level at each.  At or past the ramp's end the device takes g1 itself:
+    E = 0."""
+    k = np.asarray(k, np.float64)
+    D = g1 - g0
+    flat = k >= F
+    Fs = max(F, 1)
+    t = k / Fs
+    c = np.cos(np.pi * t)
+    d = 1 - c
+    G = np.where(flat, g1, g0 + D * (t if mutant == "linear" else d / 2))
+    # (float)k and (float)F round past 2^24, then the quotient: t's error, then cospif's 1 ulp plus the slope times it
+    et = t * (np.where(k >= 2 ** 24, U, 0) + (U if F >= 2 ** 24 else 0) + U) * (1 + 4 * U)
+    ec = 2 * U * np.abs(c) + np.pi * et + 2.0 ** -149
+    ed = ec + U * (d + ec)                                  # 1 - cospif
+    ep = abs(D) * ed + d * U * abs(D) + U * abs(D) * (d + ed)   # (g1 - g0) * (1 - cospif), then * 0.5 exactly
+    E = (ep / 2 + U * (np.abs(G) + ep / 2)) * (1 + 8 * U)   # g0 + ..., rounded
+    return G, np.where(flat, 0.0, E)
+
+
+def _exact_sum(a, b):
+    """a + b in float64 and whether that sum is exact (two-sum)"""
+    s = a + b
+    bb = s - a
+    return s, (a - (s - bb)) + (b - bb) == 0
+
+
+def model_mix(state, n_records, y, records, offsets, slots, hops=None, chunk=None, out=None, with_bound=False,
+              mutant=None):
     """l2h_target_mix on numpy: y [R, C, 128 T], chunk [n, C, 128 T + 64] or None.  Returns out [n, C, 128 T] (NaN where
-    nothing is written, unless `out` is given) and advances the state's ramps."""
+    nothing is written, unless `out` is given) and advances the state's ramps.  With with_bound, returns (out, bound):
+    per sample, a bound on |device - out| for the sequential fmaf sum from -0 in row order, then the ambient term.  Each
+    term adds its fp32 gain's error times |x|, and each fmaf one rounding of its result, which is 0 where the gain is
+    exact, the sum so far has no error and the new sum is an fp32 number.  A sample no term enters is -0.  `mutant`
+    (MIX_MUTANTS) computes a subtly wrong mix instead ("reversed": the fp32 sum in reverse order)."""
     R, C, L = y.shape
     T, n, n_slots = L // HOP, len(slots), state.shape[0] - n_records
     out = np.full((n, C, L), np.nan) if out is None else out
+    bound = np.zeros((n, C, L))
     start = clamped_starts(offsets, R)
     for i in range(n):
         h = T if hops is None else hops[i]
@@ -71,20 +121,31 @@ def model_mix(state, n_records, y, records, offsets, slots, hops=None, chunk=Non
         m = HOP * h
         terms = [(y[r], state[records[r]], 1.0) for r in range(start[i], start[i + 1]) if 0 <= records[r] < n_records]
         if chunk is not None:
-            terms.append((chunk[i], state[n_records + slots[i]], 0.0))
-        acc = np.zeros((C, m))
-        for x, w, rest in terms:
-            for c in range(C):
+            terms.append((chunk[i, :, 64:] if mutant == "ambient_64" else chunk[i], state[n_records + slots[i]], 0.0))
+        for c in range(C):
+            acc, err = np.full(m, -0.0), np.zeros(m)
+            acc32 = np.full(m, -0.0, np.float32)
+            for x, w, rest in (terms[::-1] if mutant == "reversed" else terms):
                 g0, g1, F, p = ramp(w[c], rest)
-                g = np.array([gain(g0, g1, F, p + s) for s in range(m)])
-                live = g != 0                                   # a term enters only the samples where its gain is not 0
-                acc[c, live] += g[live] * x[c, :m][live]
-        out[i, :, :m] = acc
+                G, E = ramp_gains(g0, g1, F, p + np.arange(m) + (0 if mutant == "q" else 1), mutant)
+                live = G != 0                               # a term enters only the samples where its gain is not 0
+                xs = np.where(live, x[c, :m], 0.0)
+                new, exact = _exact_sum(acc, G * xs)
+                ex = exact & (err == 0) & (E == 0) & (np.float32(new) == new)
+                ea = E * np.abs(xs)
+                err = np.where(live, err + ea + np.where(ex, 0.0, U * (np.abs(new) + err + ea)), err)
+                acc = np.where(live, new, acc)
+                acc32 = np.where(live, np.float32(acc32 + np.float32(G * xs)), acc32)
+            out[i, c, :m] = acc32 if mutant == "reversed" else acc
+            bound[i, c, :m] = err
+        if mutant == "p_frozen":
+            continue
         for _, w, rest in terms + ([] if chunk is not None else [(None, state[n_records + slots[i]], 0.0)]):
             for c in range(C):
-                if w[c, 2] > 0:
-                    w[c, 3] = min(int(w[c, 2]) - 1, int(w[c, 3]) + m)
-    return out
+                g0, g1, F, p = ramp(w[c], rest)
+                if w[c, 2] > 0 and p < F:                   # only a running ramp advances, from its clamped p
+                    w[c, 3] = min(F, p + m)
+    return (out, bound) if with_bound else out
 
 
 # ---- the model's own checks ------------------------------------------------------------------------------------------
@@ -170,6 +231,87 @@ def test_model_fresh_rows_and_store_rules():
     out = model_mix(st, 3, y, [0, 1, 2], [0, 2, 3], [0, 5], hops=[0, 1])            # h = 0, slot outside: nothing
     assert np.isnan(out).all()
     assert clamped_starts([2, 1, 9, 0], 3) == [2, 2, 3, 3]
+
+
+def _ramped_case(seed, C=2, T=2):
+    """one listener of three running ramps and an ambient ramp, one hop count T"""
+    g = np.random.default_rng(seed)
+    st = model_state(4, 2, C)
+    model_set(st, 4, [0, 1, 3, 4 + 1], [0.25, 1.5, 0.0, 0.75], [700, 97, 2 ** 31 - 2, 300], [1.0, 0.0, 0.5, 0.0])
+    st[1, :, 3] = 40
+    y = np.float32(g.standard_normal((3, C, HOP * T))).astype(np.float64)
+    ck = np.float32(g.standard_normal((1, C, HOP * T + CARRY))).astype(np.float64)
+    return st, y, ck
+
+
+def _fp32_mix(state, y, chunk, records):
+    """an fp32 emulation of one listener's mix (numpy's float32 cos for cospif), for the bound's own check"""
+    f = np.float32
+    C, m = y.shape[1], y.shape[2]
+    out = np.full((C, m), f(-0.0))
+    for x, w, rest in [(y[r], state[records[r]], 1.0) for r in range(len(records))] + [(chunk, state[-1], 0.0)]:
+        for c in range(C):
+            g0, g1, F, p = ramp(w[c], rest)
+            k = p + np.arange(m) + 1
+            lv = f(g0) + (f(g1) - f(g0)) * (f(1) - np.cos(f(np.pi) * (k.astype(f) / f(F)))) * f(0.5)
+            gk = np.where(k >= F, f(g1), lv.astype(f))
+            live = gk != 0
+            out[c] = np.where(live, (out[c].astype(np.float64) + gk.astype(np.float64) * x[c, :m]).astype(f), out[c])
+    return out
+
+
+def test_mix_bound_covers_fp32_and_is_zero_where_exact():
+    st, y, ck = _ramped_case(1)
+    model_set(st, 4, [5], [0.75], [300], [0.0])          # the ambient ramp of slot 1, used by listener 0 below
+    emu = _fp32_mix(st.copy(), y, ck[0], [0, 1, 3])
+    st2 = st.copy()
+    st2[4] = st[5]                                       # the listener's slot is 0
+    out, bound = model_mix(st2, 4, y, [0, 1, 3], [0, 3], [0], chunk=ck, with_bound=True)
+    assert (bound[0] > 0).all() and np.all(np.abs(emu - out[0]) <= bound[0])
+    assert bound.max() < 1e-5
+    # rest gains of 1 and integer samples: every fmaf exact, the bound 0, a sample no term enters -0
+    st = model_state(3, 1, 1)
+    yi = np.arange(3 * HOP, dtype=np.float64).reshape(3, 1, HOP) - 100
+    yi[2, 0, 5] = 0
+    out, bound = model_mix(st, 3, yi, [0, 1, 2], [0, 3], [0], with_bound=True)
+    assert not bound.any() and np.array_equal(out[0], yi.sum(0))
+    model_set(st, 3, [0, 1, 2], [0.0, 0.0, 0.0], [0, 0, 0], [0.0, 0.0, 0.0])
+    out, bound = model_mix(st, 3, yi, [0, 1, 2], [0, 3], [0], with_bound=True)
+    assert not bound.any() and np.signbit(out).all() and not out.any()
+
+
+def _cancelling_case():
+    """rest gains of 1: rows 2^25, -2^25, b (the row order's fp32 sum is b exactly; the reverse order loses b)"""
+    st = model_state(3, 1, 1)
+    b = np.float32(np.random.default_rng(3).standard_normal(HOP)).astype(np.float64)
+    y = np.stack([np.full(HOP, 2.0 ** 25), np.full(HOP, -2.0 ** 25), b])[:, None]
+    return st, y
+
+
+@pytest.mark.parametrize("mutant", MIX_MUTANTS)
+def test_mix_mutants_miss_their_bound(mutant):
+    from kernels.scaffold import SENSITIVITY, ratio
+    if mutant == "reversed":
+        st, y = _cancelling_case()
+        want, bound = model_mix(st.copy(), 3, y, [0, 1, 2], [0, 3], [0], with_bound=True)
+        assert not bound.any()
+        got = model_mix(st.copy(), 3, y, [0, 1, 2], [0, 3], [0], mutant=mutant)
+        assert ratio(got, want, bound) >= SENSITIVITY
+        return
+    st, y, ck = _ramped_case(2)
+    if mutant == "set_start":
+        a, b = st.copy(), st.copy()
+        bound = model_set(a, 4, [1, 0], [0.5, 0.5], [10, 10], with_bound=True)
+        model_set(b, 4, [1, 0], [0.5, 0.5], [10, 10], mutant=mutant)
+        assert ratio(b[:2, :, 0], a[:2, :, 0], bound[:2]) >= SENSITIVITY
+        return
+    a, b = st.copy(), st.copy()
+    want, bound = model_mix(a, 4, y, [0, 1, 3], [0, 3], [1], chunk=ck, with_bound=True)
+    got = model_mix(b, 4, y, [0, 1, 3], [0, 3], [1], chunk=ck, mutant=mutant)
+    if mutant == "p_frozen":
+        assert not np.array_equal(a, b) and np.array_equal(want, got)
+    else:
+        assert ratio(got, want, bound) >= SENSITIVITY
 
 
 # ---- the library -----------------------------------------------------------------------------------------------------
