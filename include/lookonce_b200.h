@@ -41,6 +41,8 @@
  *   l2h_band_compressor
  *        <- fitting each listener's output to their hearing: gain per band and per ear, compression per band linked across
  *           the ears (BandCompressor)
+ *   l2h_band_compressor_lr
+ *        <- the same on a Linkwitz-Riley crossover bank, whose delay is shorter (BandCompressor(bank="lr4" or "lr8"))
  *
  * Conventions follow the reference's only FFI (src/datasets/motion_simulator.py:30-95): every
  * function returns int (0 = OK, non-zero = error, text via l2h_last_error()), handles are opaque
@@ -935,6 +937,55 @@ int l2h_band_compressor(const float* y_dev, int64_t y_row_stride, int64_t y_ch_s
                         int64_t out_row_stride, int64_t out_ch_stride, int32_t n, int32_t channels, int32_t frames,
                         const int32_t* slots_dev, const int32_t* hops_dev, const float* taps_dev, int32_t bands,
                         int32_t taps, float* state_dev, int32_t n_slots, float attack, float release, void* stream);
+
+/* The band compressor on a Linkwitz-Riley crossover bank: the same per-slot compressor as l2h_band_compressor, with a bank
+ * of IIR crossovers in place of the linear-phase FIRs, so the delay it adds is short and falls with frequency (with the
+ * default edges 500, 1000, 2000 and 4000 Hz at order 4: 1.83 ms at 250 Hz, 1.09 ms at 1 kHz, 0.41 ms at 2.8 kHz, 0.19 ms at
+ * 6 kHz, against the FIR bank's 4 ms at every frequency), for weaker band separation and a non-linear phase.
+ *
+ * The bank (l2h_band_compressor_lr_design) has K bands, 1 <= K <= 16, cut at K - 1 edges that rise strictly inside
+ * (0, 8000) Hz, with crossovers of order N = 4 or 8.  At edge e, LP_e = (Butterworth low-pass of order N / 2)^2, HP_e =
+ * (Butterworth high-pass of order N / 2)^2 and AP_e is the allpass on the same poles, each by the bilinear transform
+ * prewarped at the edge, as scipy.signal.butter(N / 2, edge, fs=16000) designs it, so LP_e + HP_e = AP_e.  Band b (from 0)
+ * is HP_1 .. HP_b, then LP_{b+1} for every band but the last, then AP_{b+2} .. AP_{K-1} (edges counted from 1), so the
+ * bands sum to the allpass cascade AP_1 .. AP_{K-1}: magnitude 1 at every frequency, no pure delay.  Every coefficient is
+ * derived in float64 and rounded to fp32 at the end.  Each band is a cascade of S = N / 2 (K - 1) second-order sections
+ * (b0, b1, b2, a1, a2; y = b0 x + s1, s1 <- b1 x - a1 y + s2, s2 <- b2 x - a2 y, transposed direct form II with fp32
+ * states), the shorter cascades ending in identity sections (1, 0, 0, 0, 0).  K = 1 has no sections: its band is the input.
+ * Per hop of a slot, over its channels, as l2h_band_compressor:
+ *     stage: a sample that is not finite, or whose magnitude is 2^32 or more, enters as 0, and the hop is then not measured;
+ *     filter: band[c][b] = channel c's staged samples through band b's sections, sample by sample;
+ *     measure, gain: as l2h_band_compressor, P_b, S_b, R_b and g_cb;
+ *     apply: sample k = 1 .. 128 is sum_b 10^(g_k / 20) band[c][b][k], summed in band order from -0, with g_k ramped as
+ *       there; a g_k of 0 dB is exactly 1.0f.  There is no bypass: at 0 dB everywhere the output is the bands' sum, the
+ *       allpass cascade of the input, not the input; with K = 1 it is the input bit for bit.
+ * A hop's result depends only on the state at its start and its samples, so cutting hops into other calls changes no bit.
+ *
+ * The state is [n_slots][channels][row_floats] fp32 of DEVICE memory.  Per channel the first 5 K words are those of
+ * l2h_band_compressor (profile gains, current gains, then channel 0's S_b, knee_b and slope_b), then the two states of
+ * each section of each band, [K][S][2].  All zeros is a fresh slot with a flat 0 dB profile and no compression; a slot is
+ * reset by zeroing its rows, moved by copying them, and fitted by writing the same words as for l2h_band_compressor.
+ *
+ * l2h_band_compressor_lr_design: writes the bank, out [bands][S][5] fp32 of HOST memory, S = order / 2 (bands - 1), from
+ * edges_hz [bands - 1] (HOST memory; may be NULL when bands = 1).  Uploads nothing.  Errors: 1 = null pointer, bands
+ * outside [1, 16], order not 4 or 8, edges that do not rise strictly inside (0, 8000).
+ * l2h_band_compressor_lr_layout: row_floats = 5 bands + 2 bands S.  Errors: 1 = null pointer, channels <= 0, bands outside
+ * [1, 16], order not 4 or 8; 2 = the staging of a row (5 bands S + channels 128 + channels bands 130 words) exceeds the
+ * kernel's shared memory.
+ *
+ * l2h_band_compressor_lr: the arguments of l2h_band_compressor, with sos_dev [bands][S][5] fp32 of DEVICE memory (the
+ * bank, read when the kernel runs) and order in place of taps_dev and taps.  The same list rules: a slot outside
+ * [0, n_slots), or a hop count outside [1, frames], stores nothing and advances nothing; out may be y itself.  All lists
+ * are read when the kernel runs, so a call captured in a CUDA graph serves any lists of the same n rewritten in place.
+ * One launch; nothing is read back to the host.  Errors, returned before anything is enqueued: those of
+ * l2h_band_compressor, with order not 4 or 8 in place of the taps; 2 = the staging of a row exceeds the kernel's shared
+ * memory (as in the layout).  Asynchronous on `stream`. */
+int l2h_band_compressor_lr_design(int32_t bands, const float* edges_hz, int32_t order, float* out);
+int l2h_band_compressor_lr_layout(int32_t channels, int32_t bands, int32_t order, int32_t* row_floats);
+int l2h_band_compressor_lr(const float* y_dev, int64_t y_row_stride, int64_t y_ch_stride, float* out_dev,
+                           int64_t out_row_stride, int64_t out_ch_stride, int32_t n, int32_t channels, int32_t frames,
+                           const int32_t* slots_dev, const int32_t* hops_dev, const float* sos_dev, int32_t bands,
+                           int32_t order, float* state_dev, int32_t n_slots, float attack, float release, void* stream);
 
 #ifdef __cplusplus
 }

@@ -36,6 +36,7 @@
 #include <initializer_list>
 #include <numeric>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/lookonce_b200.h"
@@ -863,9 +864,36 @@ constexpr int BC_MIN_TAPS = 33, BC_MAX_TAPS = 255;
 constexpr float BC_RANGE = 40.f;                        // the gains' clamp, dB
 static_assert(BC_MAX_BANDS <= BC_THREADS, "one thread per band updates the detectors");
 
-// One CTA = one call row over all C channels (the compression is linked).  Row i compresses the first 128 h samples of
-// y[i] into out[i], h = hops[i] (T without hops), with the state of slot slots[i].  Each hop is staged before anything of
-// it is written, so out may be y itself.  KP = bc_padded(K) accumulators per thread.
+// The steps both banks share, one thread per sample of the hop.  measure: sq[b] is the thread's sample of band b squared
+// and summed over the channels in channel order; the block sums it over the samples (a warp shuffle, then the warps in
+// order) into P_b and moves the detector S_b toward it.  The caller syncs before and after.
+template <int KP>
+L2H_DEVINL void bc_measure(const float (&sq)[KP], float (*part)[KP], float* S, int K, int C, float attack, float release) {
+    const int tid = threadIdx.x;
+#pragma unroll
+    for (int b = 0; b < KP; ++b) {
+        float v = sq[b];
+        for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
+        if ((tid & 31) == 0) part[tid >> 5][b] = v;
+    }
+    __syncthreads();
+    if (tid < K) {
+        float P = part[0][tid];
+        for (int w = 1; w < BC_THREADS / 32; ++w) P += part[w][tid];
+        P *= 1.f / (float)(CHUNK_HOP * C);
+        const float old = S[tid];
+        S[tid] = fmaf(P > old ? attack : release, P - old, old);
+    }
+}
+
+// gain: element i = c K + b of the gains (dB) at the hop's end, from the detectors S and the slot's state rows st (rf
+// words per channel)
+L2H_DEVINL float bc_gain(const float* st, int64_t rf, const float* S, int K, int i) {
+    const int c = i / K, b = i - c * K;
+    const float R = st[4 * K + b] * fmaxf(0.f, 10.f * log10f(S[b]) - st[3 * K + b]);
+    return fminf(fmaxf(st[c * rf + b] - R, -BC_RANGE), BC_RANGE);
+}
+
 template <int KP>
 __global__ void __launch_bounds__(BC_THREADS)
 band_compressor_kernel(const float* y, int64_t y_row, int64_t y_ch, float* out, int64_t o_row, int64_t o_ch, int C, int T,
@@ -933,28 +961,11 @@ band_compressor_kernel(const float* y, int64_t y_row, int64_t y_ch, float* out, 
                 sq[b] = fmaf(acc[b], acc[b], sq[b]);
             }
         }
-        if (measured) {                                                 // the same order of sums every call
-#pragma unroll
-            for (int b = 0; b < KP; ++b) {
-                float v = sq[b];
-                for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
-                if ((tid & 31) == 0) part[tid >> 5][b] = v;
-            }
-            __syncthreads();
-            if (tid < K) {
-                float P = part[0][tid];
-                for (int w = 1; w < BC_THREADS / 32; ++w) P += part[w][tid];
-                P *= 1.f / (float)(CHUNK_HOP * C);
-                const float old = S[tid];
-                S[tid] = fmaf(P > old ? attack : release, P - old, old);
-            }
-        }
+        if (measured) bc_measure<KP>(sq, part, S, K, C, attack, release);   // the same order of sums every call
         __syncthreads();                                                // the detectors, and every band sample
         bool live = false;
         for (int i = tid; i < CK; i += BC_THREADS) {
-            const int c = i / K, b = i - c * K;
-            const float R = st[4 * K + b] * fmaxf(0.f, 10.f * log10f(S[b]) - st[3 * K + b]);
-            g1[i] = fminf(fmaxf(st[c * rf + b] - R, -BC_RANGE), BC_RANGE);
+            g1[i] = bc_gain(st, rf, S, K, i);
             live = live || g0[i] != 0.f || g1[i] != 0.f;
         }
         live = __syncthreads_or(live);                                  // and every gain is visible to the block
@@ -979,6 +990,132 @@ band_compressor_kernel(const float* y, int64_t y_row, int64_t y_ch, float* out, 
     __syncthreads();                                                    // the history and the gains
     for (int c = 0; c < C; ++c)
         for (int i = tid; i < H; i += BC_THREADS) st[c * rf + 5 * K + i] = win[c * W + i];
+    for (int i = tid; i < CK; i += BC_THREADS) {
+        const int c = i / K;
+        st[c * rf + K + (i - c * K)] = g0[i];
+    }
+    if (tid < K) st[2 * K + tid] = S[tid];
+}
+
+// ---- the Linkwitz-Riley band compressor: the same per-hop steps on an IIR crossover bank with a short delay ------------
+// The bank (l2h_band_compressor_lr_design) cuts the band at the K - 1 edges with Linkwitz-Riley crossovers of order
+// N = 4 or 8: at edge e, LP_e and HP_e are a Butterworth filter of order N / 2 applied twice and AP_e is the allpass on
+// the same poles, so LP_e + HP_e = AP_e.  Band b is HP_1 .. HP_b, then LP_{b+1} (every band but the last), then
+// AP_{b+2} .. AP_{K-1}, so the bands sum to the allpass cascade AP_1 .. AP_{K-1}: flat in magnitude, with a delay that
+// falls with frequency.  Each band is a cascade of S = N / 2 (K - 1) biquads, [K][S][5] (b0, b1, b2, a1, a2), the
+// shorter cascades ending in identity sections; they run in transposed direct form II with fp32 states, one thread per
+// (channel, band), sample by sample through the whole cascade.  The stage, measure, gain and apply steps are the FIR
+// kernel's, the measure and the gain through the same helpers (bc_measure, bc_gain).  There is no bypass: at 0 dB
+// every band is scaled by exactly 1, and the output is the bands' sum in band order, started from -0, so that K = 1
+// (no sections) returns its staged input bit for bit.
+// A slot's state per channel is [5 K + 2 K S]: the FIR bank's 5 K head words, then the two states of each band's
+// sections, [K][S][2].  All zeros is a fresh slot.
+
+// one band of one channel through the hop's 128 samples: x the staged hop, cf [S][5] its sections in shared memory,
+// z [S][2] their states (read and written back), yb the band's 128 samples.  S is a compile-time count, so the cascade
+// unrolls without a branch and the sections of neighbouring samples overlap.  The states stay in registers, and the
+// coefficients too while S <= LR_REG_SECTIONS.
+constexpr int LR_REG_SECTIONS = 16;
+template <int S>
+L2H_DEVINL void lr_band(const float* x, const float* cf, float* z, float* yb) {
+    constexpr int SR = S > 0 ? S : 1;
+    constexpr bool REGS = S <= LR_REG_SECTIONS;
+    float z1[SR], z2[SR], c[REGS ? SR : 1][5];
+#pragma unroll
+    for (int q = 0; q < S; ++q) {
+        z1[q] = z[2 * q];
+        z2[q] = z[2 * q + 1];
+        if (REGS)
+            for (int j = 0; j < 5; ++j) c[REGS ? q : 0][j] = cf[5 * q + j];
+    }
+#pragma unroll 4
+    for (int k = 0; k < CHUNK_HOP; ++k) {
+        float v = x[k];
+#pragma unroll
+        for (int q = 0; q < S; ++q) {
+            const float* cq = REGS ? c[REGS ? q : 0] : cf + 5 * q;
+            const float u = fmaf(cq[0], v, z1[q]);
+            z1[q] = fmaf(cq[1], v, fmaf(-cq[3], u, z2[q]));
+            z2[q] = fmaf(cq[2], v, -cq[4] * u);
+            v = u;
+        }
+        yb[k] = v;
+    }
+#pragma unroll
+    for (int q = 0; q < S; ++q) {
+        z[2 * q] = z1[q];
+        z[2 * q + 1] = z2[q];
+    }
+}
+
+// One CTA = one call row over all C channels, as band_compressor_kernel.  One instantiation per band count K and order
+// N: KP = bc_padded(K) accumulators per thread, and each band's NS = N / 2 (K - 1) sections known at compile time.
+template <int K, int N>
+__global__ void __launch_bounds__(BC_THREADS)
+band_compressor_lr_kernel(const float* y, int64_t y_row, int64_t y_ch, float* out, int64_t o_row, int64_t o_ch, int C,
+                          int T, const int32_t* __restrict__ slots, const int32_t* __restrict__ hops,
+                          const float* __restrict__ sos, float* __restrict__ state, int n_slots, float attack,
+                          float release) {
+    constexpr int KP = (K + 3) / 4 * 4, NS = N / 2 * (K - 1);
+    extern __shared__ float4 sm4[];
+    __shared__ float part[BC_THREADS / 32][KP];
+    __shared__ float S[KP];
+    const int tid = threadIdx.x, CK = C * K;
+    const int64_t rf = 5 * K + 2 * K * NS;
+    const SlotRow sr = slot_row(1, slots, n_slots, state, C * rf);
+    const int h = row_hops(hops, sr.row, T);
+    if (h == 0 || !sr.live) return;                                     // a row that stores nothing
+    float* st = sr.st;                                                  // channel c's row at st + c rf
+    float* coef = reinterpret_cast<float*>(sm4);                        // [K][NS][5]: the bank
+    float* win = coef + K * NS * 5;                                     // [C][128]: the staged hop
+    float* band = win + C * CHUNK_HOP;                                  // [C][K][128]: the hop's band signals
+    float* g0 = band + CK * CHUNK_HOP;                                  // [C][K]: the gains (dB) at the hop's start
+    float* g1 = g0 + CK;                                                // [C][K]: and at its end
+    for (int i = tid; i < K * NS * 5; i += BC_THREADS) coef[i] = sos[i];
+    for (int i = tid; i < CK; i += BC_THREADS) {
+        const int c = i / K;
+        g0[i] = st[c * rf + K + (i - c * K)];
+    }
+    if (tid < K) S[tid] = st[2 * K + tid];
+    for (int t = 0; t < h; ++t) {
+        const int64_t s = (int64_t)t * CHUNK_HOP + tid;
+        bool bad = false;
+        for (int c = 0; c < C; ++c) {
+            const float v = row_ch(y, y_row, y_ch, sr.row, c)[s];
+            const bool ok = fabsf(v) < HG_BIG;
+            bad = bad || !ok;
+            win[c * CHUNK_HOP + tid] = ok ? v : 0.f;
+        }
+        const bool measured = !__syncthreads_or(bad);                   // and the staged hop is visible to the block
+        for (int i = tid; i < CK; i += BC_THREADS) {
+            const int c = i / K, b = i - c * K;
+            lr_band<NS>(win + c * CHUNK_HOP, coef + b * NS * 5, st + c * rf + 5 * K + 2 * b * NS, band + i * CHUNK_HOP);
+        }
+        __syncthreads();                                                // every band sample
+        float sq[KP];
+#pragma unroll
+        for (int b = 0; b < KP; ++b) sq[b] = 0.f;
+        for (int c = 0; c < C; ++c) {
+#pragma unroll
+            for (int b = 0; b < KP; ++b) {
+                const float v = b < K ? band[(c * K + b) * CHUNK_HOP + tid] : 0.f;
+                sq[b] = fmaf(v, v, sq[b]);
+            }
+        }
+        if (measured) bc_measure<KP>(sq, part, S, K, C, attack, release);
+        __syncthreads();                                                // the detectors
+        for (int i = tid; i < CK; i += BC_THREADS) g1[i] = bc_gain(st, rf, S, K, i);
+        __syncthreads();                                                // every gain
+        for (int c = 0; c < C; ++c) {
+            float o = -0.f;                                             // so that o + -0 is o, -0 included
+            for (int b = 0; b < K; ++b)
+                o = fmaf(hop_gain(g0[c * K + b], g1[c * K + b]), band[(c * K + b) * CHUNK_HOP + tid], o);
+            row_ch(out, o_row, o_ch, sr.row, c)[s] = o;
+        }
+        __syncthreads();                                                // every thread has read the gains and the bands
+        for (int i = tid; i < CK; i += BC_THREADS) g0[i] = g1[i];
+    }
+    __syncthreads();                                                    // the gains
     for (int i = tid; i < CK; i += BC_THREADS) {
         const int c = i / K;
         st[c * rf + K + (i - c * K)] = g0[i];
@@ -1494,5 +1631,120 @@ extern "C" int l2h_band_compressor(const float* y_dev, int64_t y_row_stride, int
     kernel<<<(unsigned)n, BC_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
         y_dev, y_row_stride, y_ch_stride, out_dev, out_row_stride, out_ch_stride, channels, frames, slots_dev, hops_dev,
         taps_dev, bands, taps, state_dev, n_slots, attack, release);
+    return launched(who);
+}
+
+namespace l2h {
+// the Linkwitz-Riley bank's shape and a call's staging (the sections, the staged hop, band signals and gains): 0, or
+// an error code (1 invalid, 2 the staging exceeds shared memory) with its message; *ns the sections per band
+static int lr_staging(const std::string& who, int32_t channels, int32_t bands, int32_t order, int* ns, int* smem) {
+    if (channels <= 0) return fail(1, who + ": channels must be positive");
+    if (bands < 1 || bands > BC_MAX_BANDS)
+        return fail(1, who + ": bands " + std::to_string(bands) + " lies outside [1, " + std::to_string(BC_MAX_BANDS) + "]");
+    if (order != 4 && order != 8) return fail(1, who + ": order " + std::to_string(order) + " is not 4 or 8");
+    *ns = order / 2 * (bands - 1);
+    const int64_t floats = (int64_t)bands * *ns * 5 + (int64_t)channels * CHUNK_HOP +
+                           (int64_t)channels * bands * (CHUNK_HOP + 2);
+    return staging(who, floats, std::to_string(channels) + " channels of " + std::to_string(bands) + " bands of order " +
+                                    std::to_string(order) + " are too large", "words per row", smem);
+}
+
+// the biquads (b0, b1, b2, a1, a2) of a Butterworth filter of order n (even) cut at f Hz, by the bilinear transform
+// prewarped at f, as scipy.signal.butter(n, f, fs=16000) designs it; `kind` 'l' low-pass, 'h' high-pass, 'a' the allpass
+// on the same poles.  Section k holds the poles at angles pi (2 k + 1) / (2 n) from the negative real axis.
+static std::vector<double> lr_butter(int n, double f, char kind) {
+    std::vector<double> out;
+    const double K = std::tan(M_PI * f / 16000.0), K2 = K * K;
+    for (int k = 0; k < n / 2; ++k) {
+        const double d = 2.0 * std::sin(M_PI * (2 * k + 1) / (2.0 * n));   // 1 / Q
+        const double norm = 1.0 / (1.0 + d * K + K2);
+        const double a1 = 2.0 * (K2 - 1.0) * norm, a2 = (1.0 - d * K + K2) * norm;
+        if (kind == 'l') out.insert(out.end(), {K2 * norm, 2.0 * K2 * norm, K2 * norm, a1, a2});
+        else if (kind == 'h') out.insert(out.end(), {norm, -2.0 * norm, norm, a1, a2});
+        else out.insert(out.end(), {a2, a1, 1.0, a1, a2});
+    }
+    return out;
+}
+
+using LrKernel = decltype(&band_compressor_lr_kernel<1, 4>);
+
+template <int N, int... K>
+static LrKernel lr_kernel_of(int bands, std::integer_sequence<int, K...>) {
+    static const LrKernel table[] = {band_compressor_lr_kernel<K + 1, N>...};
+    return table[bands - 1];
+}
+
+// the instantiation for `bands` in [1, BC_MAX_BANDS] and `order` 4 or 8
+static LrKernel lr_kernel(int bands, int order) {
+    const auto K = std::make_integer_sequence<int, BC_MAX_BANDS>{};
+    return order == 4 ? lr_kernel_of<4>(bands, K) : lr_kernel_of<8>(bands, K);
+}
+}  // namespace l2h
+
+extern "C" int l2h_band_compressor_lr_design(int32_t bands, const float* edges_hz, int32_t order, float* out) {
+    using namespace l2h;
+    const std::string who = "l2h_band_compressor_lr_design";
+    if (!out || (bands > 1 && !edges_hz)) return fail(1, who + ": null pointer");
+    int ns;
+    if (int rc = lr_staging(who, 1, bands, order, &ns, nullptr)) return rc;
+    for (int j = 0; j + 1 < bands; ++j) {
+        const float e = edges_hz[j];
+        if (!(e > 0.f && e < 8000.f) || (j > 0 && !(e > edges_hz[j - 1])))
+            return fail(1, who + ": the edges must rise strictly inside (0, 8000) Hz, got edge " + std::to_string(j) + " = " +
+                               std::to_string(e));
+    }
+    // band b: HP of edges 0 .. b - 1, the LP of edge b (not the last band), the AP of edges b + 1 .. K - 2, each LR
+    // filter the Butterworth sections twice; then identity sections up to ns, all in float64
+    const int n = order / 2;
+    for (int b = 0; b < bands; ++b) {
+        std::vector<double> sec;
+        const auto add = [&](const std::vector<double>& v, int times) {
+            for (int r = 0; r < times; ++r) sec.insert(sec.end(), v.begin(), v.end());
+        };
+        for (int e = 0; e < b; ++e) add(lr_butter(n, edges_hz[e], 'h'), 2);
+        if (b + 1 < bands) add(lr_butter(n, edges_hz[b], 'l'), 2);
+        for (int e = b + 1; e + 1 < bands; ++e) add(lr_butter(n, edges_hz[e], 'a'), 1);
+        while ((int)sec.size() < 5 * ns) sec.insert(sec.end(), {1.0, 0.0, 0.0, 0.0, 0.0});
+        for (int i = 0; i < 5 * ns; ++i) out[(int64_t)b * 5 * ns + i] = (float)sec[i];
+    }
+    return 0;
+}
+
+extern "C" int l2h_band_compressor_lr_layout(int32_t channels, int32_t bands, int32_t order, int32_t* row_floats) {
+    using namespace l2h;
+    if (!row_floats) return fail(1, "l2h_band_compressor_lr_layout: null pointer");
+    int ns;
+    if (int rc = lr_staging("l2h_band_compressor_lr_layout", channels, bands, order, &ns, nullptr)) return rc;
+    *row_floats = 5 * bands + 2 * bands * ns;
+    return 0;
+}
+
+extern "C" int l2h_band_compressor_lr(const float* y_dev, int64_t y_row_stride, int64_t y_ch_stride, float* out_dev,
+                                      int64_t out_row_stride, int64_t out_ch_stride, int32_t n, int32_t channels,
+                                      int32_t frames, const int32_t* slots_dev, const int32_t* hops_dev,
+                                      const float* sos_dev, int32_t bands, int32_t order, float* state_dev,
+                                      int32_t n_slots, float attack, float release, void* stream) {
+    using namespace l2h;
+    const std::string who = "l2h_band_compressor_lr";
+    if (int rc = slot_call(who, {y_dev, out_dev, slots_dev, sos_dev, state_dev}, "n, channels, frames and n_slots",
+                           {n, channels, frames, n_slots}, n, channels, n_slots))
+        return rc;
+    int64_t len, c_len;
+    if (int rc = hop_lens(who, frames, &len, &c_len)) return rc;
+    if (!(attack > 0.f && attack <= 1.f) || !(release > 0.f && release <= 1.f))
+        return fail(1, who + ": attack " + std::to_string(attack) + " and release " + std::to_string(release) +
+                           " must lie in (0, 1]");
+    int ns, smem;
+    if (int rc = lr_staging(who, channels, bands, order, &ns, &smem)) return rc;
+    const Rows y{"y", y_row_stride, y_ch_stride, len}, out{"out", out_row_stride, out_ch_stride, len};
+    if (int rc = disjoint(who, channels, {y, out})) return rc;
+    if (overlap(out_dev, n, out, y_dev, n, y, channels, true))
+        return fail(1, who + ": out must be y itself (same pointer and strides) or not overlap it");
+    const auto kernel = lr_kernel(bands, order);
+    if (smem > RS_SMEM_BYTES - 1024)                                    // then the static words need the opt-in
+        if (cudaError_t e = full_staging(kernel)) return fail(3, who + ": " + cudaGetErrorString(e));
+    kernel<<<(unsigned)n, BC_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
+        y_dev, y_row_stride, y_ch_stride, out_dev, out_row_stride, out_ch_stride, channels, frames, slots_dev, hops_dev,
+        sos_dev, state_dev, n_slots, attack, release);
     return launched(who);
 }

@@ -681,20 +681,38 @@ class BandCompressor(_SlotStage):
     hops into other ticks changes no bit.  A non-finite sample, or one of magnitude 2^32 or more, enters as 0, and its hop
     is not measured.
 
-    `taps` is the bank on the device, [bands, taps] float32.  `state` [slots, channels, 5 bands + taps - 1] is a float32
-    tensor on `device`: all zeros is a fresh slot with a flat 0 dB profile and no compression, so a listener is reset by
-    zeroing its rows (`reset`) and moved by copying them."""
+    `bank` chooses the filters: "fir" (the default, above), or "lr4" / "lr8", a Linkwitz-Riley crossover tree of order 4
+    or 8 (`design_lr`; l2h_band_compressor_lr) whose bands sum to an allpass: flat in magnitude, with a delay that is
+    short and falls with frequency (1.83 ms at 250 Hz down to 0.19 ms at 6 kHz for "lr4" at the default edges, against
+    the FIR bank's 4 ms), for weaker band separation and a non-linear phase (INTEGRATION.md, "Choosing the compressor's
+    bank").  An LR bank has no pure delay (`delay` is 0) and no bypass: at 0 dB its output is the allpass cascade of the
+    input.  `taps` applies to the FIR bank only.
+
+    `taps` is the bank on the device: [bands, taps] float32 FIR taps, or [bands, S, 5] float32 second-order sections for
+    an LR bank.  `state` [slots, channels, row] is a float32 tensor on `device` (row = 5 bands + taps - 1 for the FIR
+    bank, 5 bands + 2 bands S for an LR bank): all zeros is a fresh slot with a flat 0 dB profile and no compression, so
+    a listener is reset by zeroing its rows (`reset`) and moved by copying them."""
 
     RATE = 16000
     RANGE = 40.0                                # the gains' clamp, dB
+    BANKS = {"fir": None, "lr4": 4, "lr8": 8}   # bank -> LR order
 
     def __init__(self, slots, channels, edges=(500, 1000, 2000, 4000), taps=129, attack=0.005, release=0.08,
-                 device=None):
+                 device=None, bank="fir"):
         super().__init__(slots, channels)
-        bank = self.design(edges, taps)
+        if not isinstance(bank, str) or bank not in self.BANKS:
+            raise ValueError(f"bank must be one of {', '.join(map(repr, self.BANKS))}, got {bank!r}")
+        self.bank, self.order = bank, self.BANKS[bank]
+        if self.order is None:
+            table = self.design(edges, taps)
+            self.bands, self.n_taps = table.shape
+            self.delay = (self.n_taps - 1) // 2
+        else:
+            if isinstance(taps, bool) or taps != 129:
+                raise ValueError(f"taps applies to the FIR bank only, got taps={taps!r} with bank={bank!r}")
+            table = self.design_lr(edges, self.order)
+            self.bands, self.n_taps, self.delay = table.shape[0], None, 0
         self.edges = tuple(float(e) for e in torch.as_tensor(edges, dtype=torch.float32).reshape(-1).tolist())
-        self.bands, self.n_taps = bank.shape
-        self.delay = (self.n_taps - 1) // 2
         def coef_of(tau):                       # the per-hop step of a detector with time constant tau seconds
             return -math.expm1(-self.HOP_S / tau)
 
@@ -705,8 +723,43 @@ class BandCompressor(_SlotStage):
             coef[what] = coef_of(tau)
         self.attack, self.release = float(attack), float(release)
         self.attack_coef, self.release_coef = coef["attack"], coef["release"]
-        self._allocate(*_layout(_cabi.lib().l2h_band_compressor_layout, self.channels, self.bands, self.n_taps), device)
-        self.taps = bank.to(self.state.device)
+        if self.order is None:
+            self._allocate(*_layout(_cabi.lib().l2h_band_compressor_layout, self.channels, self.bands, self.n_taps), device)
+        else:
+            self._allocate(*_layout(_cabi.lib().l2h_band_compressor_lr_layout, self.channels, self.bands, self.order),
+                           device)
+        self._bank = torch.zeros(max(1, table.numel()), device=self.state.device)   # one band: a pointer to no words
+        self._bank[:table.numel()].copy_(table.reshape(-1))
+        self.taps = self._bank[:table.numel()].view(table.shape)
+
+    @staticmethod
+    def _edges(edges):
+        """edges as a contiguous float32 CPU tensor of at most 15 entries, or ValueError"""
+        try:
+            e = torch.as_tensor(edges, dtype=torch.float32).reshape(-1).contiguous()
+        except (TypeError, ValueError, RuntimeError):
+            raise ValueError(f"edges must be a sequence of numbers of Hz, got {edges!r}") from None
+        if isinstance(edges, (str, bytes)) or e.numel() >= 16:
+            raise ValueError(f"edges must be at most 15 numbers of Hz (at most 16 bands), got {edges!r}")
+        return e
+
+    @staticmethod
+    def design_lr(edges=(500, 1000, 2000, 4000), order=4):
+        """The Linkwitz-Riley bank of K = len(edges) + 1 bands cut at `edges` Hz (rising strictly inside (0, 8000)) with
+        crossovers of `order` 4 or 8, as a [K, S, 5] float32 CPU tensor of second-order sections (b0, b1, b2, a1, a2),
+        S = order / 2 (K - 1) (l2h_band_compressor_lr_design): at each edge LP = (Butterworth low-pass)^2, HP =
+        (Butterworth high-pass)^2 of order / 2, as scipy.signal.butter designs them at fs=16000, and AP the allpass on the
+        same poles; band j is the HPs of the edges below it, its own LP (every band but the last) and the APs of the edges
+        above that, padded with identity sections, computed in float64, so the bands sum to the product of the APs."""
+        e = BandCompressor._edges(edges)
+        if isinstance(order, bool) or order not in (4, 8):
+            raise ValueError(f"order must be 4 or 8, got {order!r}")
+        N = int(order)
+        S = N // 2 * e.numel()
+        buf = torch.empty(max(1, (e.numel() + 1) * S * 5), dtype=torch.float32)    # one band: no sections, no words
+        _check(_cabi.lib().l2h_band_compressor_lr_design(e.numel() + 1, e.data_ptr() if e.numel() else None, N,
+                                                         buf.data_ptr()))
+        return buf[:(e.numel() + 1) * S * 5].view(e.numel() + 1, S, 5)
 
     @staticmethod
     def design(edges=(500, 1000, 2000, 4000), taps=129):
@@ -714,12 +767,7 @@ class BandCompressor(_SlotStage):
         FIR of `taps` taps (odd, 33 to 255), as a [K, taps] float32 CPU tensor (l2h_band_compressor_design): with LP_j =
         scipy.signal.firwin(taps, edge_j, fs=16000), band 0 is LP_1, band j is LP_{j+1} - LP_j and the last band is a
         delay of (taps - 1) / 2 samples minus LP_{K-1}, computed in float64, so the bands sum to that delay."""
-        try:
-            e = torch.as_tensor(edges, dtype=torch.float32).reshape(-1).contiguous()
-        except (TypeError, ValueError, RuntimeError):
-            raise ValueError(f"edges must be a sequence of numbers of Hz, got {edges!r}") from None
-        if isinstance(edges, (str, bytes)) or e.numel() >= 16:
-            raise ValueError(f"edges must be at most 15 numbers of Hz (at most 16 bands), got {edges!r}")
+        e = BandCompressor._edges(edges)
         L = _whole(taps, "taps")
         out = torch.empty(e.numel() + 1, L, dtype=torch.float32)
         _check(_cabi.lib().l2h_band_compressor_design(e.numel() + 1, e.data_ptr() if e.numel() else None, L,
@@ -743,8 +791,9 @@ class BandCompressor(_SlotStage):
         slots = device_list(slots, dev, n, self.n_slots, True, "slot")
         hops = self._hops(hops, n, T)
         out = self._rows_out(out, (n, C, L))
-        self._run("l2h_band_compressor", y, y.stride(0), y.stride(1), out, out.stride(0), out.stride(1), n, C, T, slots, hops,
-                  self.taps, self.bands, self.n_taps, self.state, self.n_slots, self.attack_coef, self.release_coef)
+        entry, shape = ("l2h_band_compressor", self.n_taps) if self.order is None else ("l2h_band_compressor_lr", self.order)
+        self._run(entry, y, y.stride(0), y.stride(1), out, out.stride(0), out.stride(1), n, C, T, slots, hops, self._bank,
+                  self.bands, shape, self.state, self.n_slots, self.attack_coef, self.release_coef)
         return out
 
     def set_profile(self, slots, gains, knees=0.0, ratios=1.0):
