@@ -43,6 +43,9 @@
  *           the ears (BandCompressor)
  *   l2h_band_compressor_lr
  *        <- the same on a Linkwitz-Riley crossover bank, whose delay is shorter (BandCompressor(bank="lr4" or "lr8"))
+ *   l2h_jitter_buffer
+ *        <- putting a device's packets back in sequence order and concealing lost ones, over a lossy network
+ *           (JitterBuffer)
  *
  * Conventions follow the reference's only FFI (src/datasets/motion_simulator.py:30-95): every
  * function returns int (0 = OK, non-zero = error, text via l2h_last_error()), handles are opaque
@@ -986,6 +989,88 @@ int l2h_band_compressor_lr(const float* y_dev, int64_t y_row_stride, int64_t y_c
                            int64_t out_row_stride, int64_t out_ch_stride, int32_t n, int32_t channels, int32_t frames,
                            const int32_t* slots_dev, const int32_t* hops_dev, const float* sos_dev, int32_t bands,
                            int32_t order, float* state_dev, int32_t n_slots, float attack, float release, void* stream);
+
+/* A per-slot jitter buffer: the first stage of a tick for devices that send packets of P samples with RTP's 16-bit
+ * sequence numbers over a lossy network (UDP over Wi-Fi or BLE).  It puts packets back in sequence order, drops late and
+ * duplicate ones and conceals lost ones, so every later stage sees one continuous stream at the device's rate.  A tick:
+ *     l2h_jitter_buffer(x, seqs, counts -> y, out_counts)                     device rate, in order, losses concealed
+ *     l2h_resample_packets(y, counts = out_counts, unit = P -> y16, n16)      (a 16 kHz device skips this)
+ *     l2h_hop_fifo(y16, counts = n16, unit = 1 -> chunk, hops)
+ *     l2h_sep_forward_slots_hops(chunk, slots, hops)
+ * all from device memory and capturable in one CUDA graph.
+ *
+ * Sequence numbers are compared in serial-number arithmetic (RFC 1982): with `next` the number of the next packet to
+ * decide, a packet s lies d = (s - next) mod 2^16, taken in [-2^15, 2^15), ahead of it, so a stream that wraps from 65535 to
+ * 0 passes unchanged.  A row's packets are processed one at a time, in row order:
+ *   - the first packet of a fresh slot sets next := s;
+ *   - d < 0: late, dropped and counted in `late`;
+ *   - a packet already held: a duplicate, dropped and counted in `duplicate`;
+ *   - 0 <= d < window: held;
+ *   - d >= window: a restart (a device reboot, a long outage): the held packets are discarded and counted in `dropped`,
+ *     next := s, the packet is held, the restart is counted in `restarts`, and the packet fades in as after a loss run.
+ * Then, while next is held it is released and next advances; while next is missing and a packet at least next + depth + 1
+ * is held, next is declared lost (counted in `lost`), released as concealment, and next advances.  So depth = 0
+ * conceals a gap as soon as any later packet arrives, and each step up waits one more packet for a late arrival.
+ * In-order traffic is released on arrival: with no loss, duplicate or reordering the output is the input bit for bit,
+ * with no added delay.  The window counts from next: the decided packets a call does not write (at most max_out per row
+ * per call) wait in a backlog of up to `window` more, which the slot's next call writes first (also with count 0).  So
+ * every decision is a function of the arrival sequence alone, and cutting the same arrivals into other calls, or another
+ * max_out, changes only where the output is cut, bit for bit.  A release that finds the backlog full discards its oldest
+ * packet and counts it in `dropped`; a service that writes what it decides every tick never reaches that.
+ *
+ * Concealment (after ITU-T G.711 Appendix I: pitch-period repetition with fading), one decision per slot for all channels,
+ * so the repeated period keeps its interaural time and level differences.  Lags tau_min = round(0.0025 rate) ..
+ * tau_max = round(0.015 rate) (66-400 Hz), correlation window Wc = round(0.020 rate), round(v) = floor(v + 0.5):
+ *   - at the first lost packet of a run, with s the fp32 channel sum (channels in order) of the last Wc + tau_max written
+ *     samples (concealment included), tau is the first maximiser over the lags of
+ *         sum_k s[N - Wc + k] s[N - Wc + k - tau] / sqrt(max(sum_k s[N - Wc + k - tau]^2, FLT_MIN)),  k = 0 .. Wc - 1
+ *     over the lags whose numerator is positive (each lag's sums in fp32, k ascending, fmaf), tau_max when none is;
+ *   - channel c plays e_c[k] = g(k) x_c[N - tau + (k mod tau)], the last period looped, with g = 1 for k < round(0.010
+ *     rate), (B - k) / (B - A) in fp32 from A = round(0.010 rate) to B = round(0.060 rate), and exactly 0 from B on;
+ *   - the first real packet after a run, or after a restart (which searches a period first when no run is going), starts
+ *     with a raised-cosine crossfade over Lr = min(round(0.004 rate), P) samples from the continuing concealment e (with
+ *     its gain) to the packet r: v = e + w (r - e), w = 0.5 - 0.5 cospif((i + 1) / (Lr + 1)), i < Lr (fmaf);
+ *   - a sample that is not finite, or whose magnitude is 2^32 or more, enters as 0.
+ *
+ * The state is [n_slots][channels][row_floats] fp32 of DEVICE memory, row_floats = 16 + R + R P + H + tau_max with
+ * R = 2 window and H = Wc + tau_max: per channel sixteen head words and R ring tags (channel 0's only), a ring of R
+ * packets, the last H samples written and the period being repeated.  The head words are int32 words in the floats' bits:
+ * 0 started, 1 next, 2 the ring position of the oldest packet not written, 3 the packets decided and not written,
+ * 4 the concealed samples into the current run (capped at B), 5 the run's lag (0: no run), 6 lost, 7 late, 8 duplicate,
+ * 9 dropped, 10 restarts (saturating at 2^31 - 1; a negative one counts as 0), 11 the packets held, 12 the lag of the
+ * last run (`pitch`).  A tag is 0 (empty), s + 1 for a stored packet s (with bit 17 set for a released one that fades
+ * in) or -1 (a released loss); a released entry plays its packet whatever its number (a restart may lie between it and
+ * next, and its packets still play), and a released entry with any other tag is concealed.  All zeros is a fresh
+ * slot, so a slot is reset by zeroing its rows and moved by copying them.
+ *
+ * l2h_jitter_buffer_layout: row_floats.  Errors: 1 = null pointer, channels <= 0, rate outside [8000, 384000], packet < 1,
+ * window outside [1, 4096], depth outside [0, window - 1], max_out < 1, a slot row of more than 2^31 - 1 floats; 2 = the
+ * staging of a row (channels (H + max_out P) + H + channels tau_max + R + 1 + max_out words) exceeds the kernel's shared
+ * memory.
+ *
+ * l2h_jitter_buffer: row i pushes packets j < c_i = counts_dev[i] of x row i into slot slots_dev[i]:
+ *   x_dev           [n][channels][max_in P] fp32, strides in floats; packet j of row i is x[i][c][j P .. (j + 1) P)
+ *   seqs_dev        [n][max_in] int32 of DEVICE memory read when the kernel runs: packet j's sequence number; an entry
+ *                   outside [0, 65535] marks a packet that is skipped
+ *   counts_dev      [n] int32 of DEVICE memory read when the kernel runs: c_i in packets
+ *   y_dev           [n][channels][max_out P] fp32; row i receives y[i][c][0 .. m_i P), its slot's next m_i packets.  Its
+ *                   later samples are not written.  Must not overlap x or the state.
+ *   out_counts_dev  [n] int32 of DEVICE memory: m_i, in packets
+ *   slots_dev       [n] int32 of DEVICE memory read when the kernel runs: an entry outside [0, n_slots), or a count outside
+ *                   [0, max_in], marks a row that stores nothing and gets out count 0.  A slot listed twice is a caller
+ *                   error the call does not detect.
+ * One launch, one CTA per row over all its channels; nothing on the host is read from the device, and a call captured in
+ * a CUDA graph serves any lists of the same n rewritten in place.  Errors, returned before anything is enqueued:
+ * 1 = null pointers, n, channels, max_in or n_slots <= 0, n > n_slots, the layout's errors 1, channel or row strides under
+ * the lengths above, y overlapping x; 2 = the staging of a row (as in the layout, with max_in in place of 1) exceeds the
+ * kernel's shared memory.  Asynchronous on `stream`. */
+int l2h_jitter_buffer_layout(int32_t channels, int32_t rate, int32_t packet, int32_t depth, int32_t window, int32_t max_out,
+                             int32_t* row_floats);
+int l2h_jitter_buffer(const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, int32_t max_in, const int32_t* seqs_dev,
+                      const int32_t* counts_dev, float* y_dev, int64_t y_row_stride, int64_t y_ch_stride,
+                      int32_t* out_counts_dev, int32_t n, int32_t channels, const int32_t* slots_dev, float* state_dev,
+                      int32_t n_slots, int32_t rate, int32_t packet, int32_t depth, int32_t window, int32_t max_out,
+                      void* stream);
 
 #ifdef __cplusplus
 }

@@ -15,6 +15,7 @@ net), behind the reference's own Python call signatures.
     from lookoncetohear_b200 import Limiter          # each listener's output kept under a ceiling, one gain for both ears
     from lookoncetohear_b200 import Leveler          # each voice brought to one loudness, one gain for both ears
     from lookoncetohear_b200 import BandCompressor   # each listener's output fitted to their hearing, per band and ear
+    from lookoncetohear_b200 import JitterBuffer     # packets back in sequence order, lost ones concealed
 
 Compute happens only in lib/liblookonce_b200.so (hand-written sm_90a CUDA, C ABI declared in
 include/lookonce_b200.h); importing this package never falls back to PyTorch math.
@@ -22,8 +23,8 @@ include/lookonce_b200.h); importing this package never falls back to PyTorch mat
 from .embed import EmbedTFGridNet, EnrollJob  # noqa: F401
 from .net import Net, SepState, TargetHistory  # noqa: F401
 from .render import resample  # noqa: F401
-from .stream import BandCompressor, EnrollCapture, HopFifo, PacketResampler, Leveler, Limiter, StreamResampler, TargetMixer  # noqa: F401
+from .stream import BandCompressor, EnrollCapture, HopFifo, JitterBuffer, PacketResampler, Leveler, Limiter, StreamResampler, TargetMixer  # noqa: F401
 
 __all__ = ["Net", "SepState", "TargetHistory", "EmbedTFGridNet", "resample", "StreamResampler", "PacketResampler", "HopFifo",
            "EnrollCapture", "EnrollJob", "TargetMixer", "Limiter", "Leveler",
-           "BandCompressor"]
+           "BandCompressor", "JitterBuffer"]

@@ -26,7 +26,8 @@
 // mixture into one row (target_mix_kernel, target_mix_set_kernel), the look-ahead limiter that keeps each listener's
 // output under a ceiling with one gain for all channels (limiter_kernel), the leveler that brings each voice to one
 // loudness with one gain for all channels (leveler_kernel), and the multiband compressor that fits each listener's output
-// to their hearing, per band and per ear, with its compression linked across the channels (band_compressor_kernel).
+// to their hearing, per band and per ear, with its compression linked across the channels (band_compressor_kernel), and
+// the jitter buffer that puts a device's packets back in sequence order and conceals lost ones (jitter_buffer_kernel).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -1746,5 +1747,320 @@ extern "C" int l2h_band_compressor_lr(const float* y_dev, int64_t y_row_stride, 
     kernel<<<(unsigned)n, BC_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
         y_dev, y_row_stride, y_ch_stride, out_dev, out_row_stride, out_ch_stride, channels, frames, slots_dev, hops_dev,
         sos_dev, state_dev, n_slots, attack, release);
+    return launched(who);
+}
+
+// ---- the jitter buffer: packets back in sequence order, losses concealed ----------------------------------------------
+// Packets of P samples carry RTP's 16-bit sequence numbers, compared in serial-number arithmetic (RFC 1982).  A slot keeps
+// `next`, the sequence number of the next packet to decide, a window of the W numbers next .. next + W - 1 (the packets
+// stored there wait for their turn), and a backlog of up to W decided packets its calls have not written yet, so a packet
+// is placed, released or declared lost from the arrivals alone: cutting them into other calls, or another max_out,
+// changes no decision.  Thread 0 runs each row's arrivals in order on ring tags staged in shared memory; all threads then
+// copy the stored packets into the ring and write the decided ones, concealing a lost one by repeating the last pitch
+// period (found by a normalised autocorrelation over the lags in parallel, each lag's sums in one fixed order) with a gain
+// that holds for 10 ms and falls to 0 by 60 ms, and fading the first real packet after a run or a restart in from the
+// continuing concealment along a raised cosine.
+//
+// A slot's row per channel is [JB_HEAD + R + R P + H + tau_max] floats, R = 2 W: the head words and the R ring tags
+// (channel 0's only), the ring of R packets, the last H = Wc + tau_max written samples, and the period being repeated.
+// A tag is 0 (empty), s + 1 for a stored packet s (| JB_RECOVER for a released one that fades in), or JB_LOST (a
+// released loss); a backlog entry with any other tag is concealed.  The backlog occupies ring positions head .. head + pend - 1, the window the W after it.
+namespace l2h {
+constexpr int JB_HEAD = 16;
+constexpr int JB_LOST = -1;
+constexpr int JB_RECOVER = 1 << 17;
+constexpr int JB_SEQ = 1 << 16;
+constexpr int JB_MAX_WINDOW = 4096;
+// head words (int32 in the floats' bits): started, next, head, pend, run (concealed samples into the run, capped at its
+// silent point), tau (0: no run), then the counters lost, late, duplicate, dropped, restarts, and held and pitch
+enum { JB_STARTED, JB_NEXT, JB_POS, JB_PEND, JB_RUN, JB_TAU, JB_C_LOST, JB_C_LATE, JB_C_DUP, JB_C_DROPPED, JB_C_RESTARTS,
+       JB_HELD, JB_PITCH };
+
+struct JbParams {
+    int32_t P, W, R, D, M, max_out;   // packet, window, ring (2 W), depth, arrivals per row, packets written per row
+    int32_t tmin, tmax, wc, hist;     // lags, correlation window, history H = wc + tmax
+    int32_t lr, ga, gb;               // crossfade samples; a run's gain is 1 before sample ga, 0 from sample gb
+    int64_t rf;                       // floats per channel row
+};
+
+// a sample as it enters: 0 when it is not finite or its magnitude is 2^32 or more
+L2H_DEVINL float jb_clean(float v) { return fabsf(v) < HG_BIG ? v : 0.f; }
+
+// the gain of concealed sample k of a run
+L2H_DEVINL float jb_gain(int k, const JbParams& p) {
+    return k < p.ga ? 1.f : (k >= p.gb ? 0.f : (float)(p.gb - k) / (float)(p.gb - p.ga));
+}
+
+// The lag of the period that ends at the history win[c][base + H] (every thread calls it): the first maximiser over
+// tmin .. tmax of sum_k s[k] s[k - t] / sqrt(max(sum_k s[k - t]^2, FLT_MIN)) over the last wc samples of the channel
+// sum s, tmax when no numerator is positive.
+L2H_DEVINL int jb_pitch(const float* win, int64_t WL, int base, int C, float* sum, float* sc, int* lt, int* tau,
+                        const JbParams& p) {
+    const int tid = threadIdx.x, H = p.hist;
+    for (int i = tid; i < H; i += blockDim.x) {
+        float a = win[base + i];
+        for (int c = 1; c < C; ++c) a += win[c * WL + base + i];
+        sum[i] = a;
+    }
+    __syncthreads();
+    float best = -1.f;
+    int bt = p.tmax;
+    const float* a = sum + H - p.wc;
+    for (int t = p.tmin + tid; t <= p.tmax; t += blockDim.x) {
+        const float* b = a - t;
+        float num = 0.f, en = 0.f;
+        for (int k = 0; k < p.wc; ++k) {
+            num = fmaf(a[k], b[k], num);
+            en = fmaf(b[k], b[k], en);
+        }
+        if (num > 0.f) {
+            const float score = num / sqrtf(fmaxf(en, FLT_MIN));
+            if (score > best) best = score, bt = t;
+        }
+    }
+    sc[tid] = best;
+    lt[tid] = bt;
+    __syncthreads();
+    if (tid == 0) {
+        float b0 = -1.f;
+        int t0 = p.tmax;
+        for (int i = 0; i < (int)blockDim.x; ++i)
+            if (sc[i] > b0 || (sc[i] == b0 && lt[i] < t0)) b0 = sc[i], t0 = lt[i];
+        *tau = t0;
+    }
+    __syncthreads();
+    return *tau;
+}
+
+// One CTA = one call row over all C channels (one decision per slot).  Row i pushes packets j < counts[i] of x row i
+// with sequence numbers seqs[i][j] and writes y[i][c][0 .. out_counts[i] P).
+__global__ void __launch_bounds__(RS_TILE)
+jitter_buffer_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, const int32_t* __restrict__ seqs,
+                     const int32_t* __restrict__ counts, float* __restrict__ y, int64_t y_row, int64_t y_ch,
+                     int32_t* __restrict__ out_counts, int C, const int32_t* __restrict__ slots, float* __restrict__ state,
+                     int n_slots, const __grid_constant__ JbParams p) {
+    extern __shared__ float sm[];
+    __shared__ float sc[RS_TILE];
+    __shared__ int lt[RS_TILE];
+    __shared__ int n_out_s, tau_s;
+    const int tid = threadIdx.x, P = p.P, R = p.R, W = p.W, H = p.hist;
+    const int64_t rf = p.rf, WL = H + (int64_t)p.max_out * P;
+    const SlotRow sr = slot_row(1, slots, n_slots, state, C * rf);
+    const int cnt = counts[sr.row];
+    if (!sr.live || cnt < 0 || cnt > p.M) {                             // a row that stores nothing
+        if (tid == 0) out_counts[sr.row] = 0;
+        return;
+    }
+    float* st = sr.st;                                                  // channel c's row at st + c rf
+    float* win = sm;                                                    // [C][WL]: the history, then the packets written
+    float* sum = win + C * WL;                                          // [H]: the channel sum of a search
+    float* per = sum + H;                                               // [C][tmax]: the period being repeated
+    int* tg = reinterpret_cast<int*>(per + (int64_t)C * p.tmax);        // [R]: the ring tags
+    int* cp = tg + R;                                                   // [M]: the ring slot of each arrival, or -1
+    int* kind = cp + p.M;                                               // [max_out]: the tag of each packet written
+    const int64_t o_ring = JB_HEAD + R, o_hist = o_ring + (int64_t)R * P, o_per = o_hist + H;
+    for (int i = tid; i < R; i += blockDim.x) tg[i] = __float_as_int(st[JB_HEAD + i]);
+    for (int c = 0; c < C; ++c) {
+        for (int i = tid; i < H; i += blockDim.x) win[c * WL + i] = st[c * rf + o_hist + i];
+        for (int i = tid; i < p.tmax; i += blockDim.x) per[c * p.tmax + i] = st[c * rf + o_per + i];
+    }
+    __syncthreads();
+    if (tid == 0) {
+        int started = __float_as_int(st[JB_STARTED]) != 0, next = int_word(st[JB_NEXT], JB_SEQ - 1);
+        int pos = int_word(st[JB_POS], R - 1), pend = int_word(st[JB_PEND], W);
+        int lost = 0, late = 0, dup = 0, dropped = 0, restarts = 0;
+        const auto slot = [&](int d) { return (pos + pend + d) % R; };
+        const auto held = [&](int d) { return tg[slot(d)] == ((next + d) & (JB_SEQ - 1)) + 1; };
+        int far = -1;                                                   // the farthest stored packet in the window
+        for (int d = 0; d < W; ++d) if (held(d)) far = d;
+        const int32_t* sq = seqs + (int64_t)sr.row * p.M;
+        for (int j = 0; j < cnt; ++j) {
+            cp[j] = -1;
+            const int s = sq[j];
+            if (s < 0 || s >= JB_SEQ) continue;                         // no sequence number: skipped
+            if (!started) started = 1, next = s;
+            int d = (s - next) & (JB_SEQ - 1);
+            if (d >= JB_SEQ / 2) d -= JB_SEQ;
+            bool recover = false;
+            if (d < 0) { late = min(late + 1, INT32_MAX - 1); continue; }
+            if (d < W) {
+                if (held(d)) { dup = min(dup + 1, INT32_MAX - 1); continue; }
+            } else {                                                    // beyond the window: a restart
+                for (int e = 0; e < W; ++e) {
+                    if (held(e)) dropped = min(dropped + 1, INT32_MAX - 1);
+                    tg[slot(e)] = 0;
+                }
+                restarts = min(restarts + 1, INT32_MAX - 1);
+                next = s, d = 0, far = -1, recover = true;
+            }
+            const int at = slot(d);
+            tg[at] = s + 1;
+            for (int k = 0; k < j; ++k) if (cp[k] == at) cp[k] = -1;    // a slot freed and reused in this call
+            cp[j] = at;
+            far = max(far, d);
+            for (;;) {                                                  // the release rule
+                int t;
+                if (held(0)) t = (next + 1) | (recover ? JB_RECOVER : 0), recover = false;
+                else if (far >= p.D + 1) t = JB_LOST, lost = min(lost + 1, INT32_MAX - 1);
+                else break;
+                if (pend == W) {                                        // the backlog is full: its oldest goes
+                    tg[pos] = 0;
+                    pos = (pos + 1) % R, --pend;
+                    dropped = min(dropped + 1, INT32_MAX - 1);
+                }
+                tg[(pos + pend) % R] = t;
+                ++pend, next = (next + 1) & (JB_SEQ - 1), --far;
+            }
+        }
+        const int n_out = min(pend, p.max_out);
+        for (int k = 0; k < n_out; ++k) {                               // what each written packet is
+            // a released packet plays whatever its number: a restart may lie between it and next; a malformed tag conceals
+            const int at = (pos + k) % R, t = tg[at], s1 = t & ~JB_RECOVER;
+            kind[k] = s1 >= 1 && s1 <= JB_SEQ ? t : JB_LOST;
+            tg[at] = 0;
+        }
+        pos = (pos + n_out) % R, pend -= n_out;
+        int nheld = 0;
+        for (int d = 0; d < W; ++d) nheld += held(d);
+        st[JB_STARTED] = __int_as_float(started);
+        st[JB_NEXT] = __int_as_float(next);
+        st[JB_POS] = __int_as_float(pos);
+        st[JB_PEND] = __int_as_float(pend);
+        st[JB_C_LOST] = add_word(st[JB_C_LOST], lost);
+        st[JB_C_LATE] = add_word(st[JB_C_LATE], late);
+        st[JB_C_DUP] = add_word(st[JB_C_DUP], dup);
+        st[JB_C_DROPPED] = add_word(st[JB_C_DROPPED], dropped);
+        st[JB_C_RESTARTS] = add_word(st[JB_C_RESTARTS], restarts);
+        st[JB_HELD] = __int_as_float(nheld);
+        out_counts[sr.row] = n_out;
+        n_out_s = n_out;
+    }
+    __syncthreads();
+    const int n_out = n_out_s;
+    for (int i = tid; i < R; i += blockDim.x) st[JB_HEAD + i] = __int_as_float(tg[i]);
+    const int64_t per_row = (int64_t)C * P;
+    for (int64_t e = tid; e < (int64_t)cnt * per_row; e += blockDim.x) {   // the stored packets into the ring
+        const int j = (int)(e / per_row), r = (int)(e - j * per_row), c = r / P, i = r - c * P;
+        if (cp[j] >= 0) st[c * rf + o_ring + (int64_t)cp[j] * P + i] = jb_clean(row_ch(x, x_row, x_ch, sr.row, c)[(int64_t)j * P + i]);
+    }
+    __syncthreads();                                                    // the ring, visible to the block
+    int run = int_word(st[JB_RUN], p.gb), tau = __float_as_int(st[JB_TAU]);
+    if (tau < p.tmin || tau > p.tmax) tau = 0;
+    const int pos0 = int_word(st[JB_POS], R - 1) - n_out;               // the ring slot of the first packet written
+    for (int k = 0; k < n_out; ++k) {
+        const int t = kind[k], base = k * P;
+        if (tau == 0 && t != JB_LOST && !(t & JB_RECOVER)) {            // a packet in order: copied as it is
+            const int at = (pos0 + k + R) % R;
+            for (int e = tid; e < C * P; e += blockDim.x) {
+                const int c = e / P, i = e - c * P;
+                const float v = st[c * rf + o_ring + (int64_t)at * P + i];
+                win[c * WL + H + base + i] = v;
+                row_ch(y, y_row, y_ch, sr.row, c)[base + i] = v;
+            }
+            __syncthreads();
+            continue;
+        }
+        if (tau == 0) {                                                 // a run starts: find its period
+            tau = jb_pitch(win, WL, base, C, sum, sc, lt, &tau_s, p);
+            run = 0;
+            for (int e = tid; e < C * tau; e += blockDim.x) {
+                const int c = e / tau, i = e - c * tau;
+                per[c * p.tmax + i] = win[c * WL + base + H - tau + i];
+            }
+            if (tid == 0) st[JB_PITCH] = __int_as_float(tau);
+            __syncthreads();
+        }
+        const int at = (pos0 + k + R) % R;
+        for (int e = tid; e < C * P; e += blockDim.x) {
+            const int c = e / P, i = e - c * P;
+            const int q = min(run + i, p.gb);
+            const float cont = jb_gain(q, p) * per[c * p.tmax + (run + i) % tau];
+            float v = cont;
+            if (t != JB_LOST) {                                         // the fade from the concealment to the packet
+                const float r = st[c * rf + o_ring + (int64_t)at * P + i];
+                if (i < p.lr) v = fmaf(0.5f - 0.5f * cospif((float)(i + 1) / (float)(p.lr + 1)), r - cont, cont);
+                else v = r;
+            }
+            win[c * WL + H + base + i] = v;
+            row_ch(y, y_row, y_ch, sr.row, c)[base + i] = v;
+        }
+        if (t == JB_LOST) run = min(run + P, p.gb);
+        else tau = 0, run = 0;
+        __syncthreads();
+    }
+    for (int c = 0; c < C; ++c) {
+        for (int i = tid; i < H; i += blockDim.x) st[c * rf + o_hist + i] = win[c * WL + (int64_t)n_out * P + i];
+        for (int i = tid; i < p.tmax; i += blockDim.x) st[c * rf + o_per + i] = per[c * p.tmax + i];
+    }
+    if (tid == 0) {
+        st[JB_RUN] = __int_as_float(tau ? run : 0);
+        st[JB_TAU] = __int_as_float(tau);
+    }
+}
+
+// the parameters of a jitter buffer and the shared-memory bytes of a call of `arrivals` packets per row: 0, or an error
+// code (1 invalid, 2 the staging exceeds shared memory) with its message
+static int jb_params(const std::string& who, int32_t channels, int32_t rate, int32_t packet, int32_t depth, int32_t window,
+                     int32_t max_out, int32_t arrivals, JbParams* p, int* smem) {
+    if (channels <= 0) return fail(1, who + ": channels must be positive");
+    if (rate < 8000 || rate > 384000) return fail(1, who + ": rate " + std::to_string(rate) + " lies outside [8000, 384000] Hz");
+    if (packet < 1) return fail(1, who + ": packet " + std::to_string(packet) + " is not positive");
+    if (window < 1 || window > JB_MAX_WINDOW)
+        return fail(1, who + ": window " + std::to_string(window) + " lies outside [1, " + std::to_string(JB_MAX_WINDOW) + "]");
+    if (depth < 0 || depth >= window)
+        return fail(1, who + ": depth " + std::to_string(depth) + " lies outside [0, window - 1 = " + std::to_string(window - 1) + "]");
+    if (max_out < 1) return fail(1, who + ": max_out " + std::to_string(max_out) + " is not positive");
+    const auto samples = [rate](double s) { return (int32_t)std::floor(s * rate + 0.5); };
+    p->P = packet, p->W = window, p->R = 2 * window, p->D = depth, p->M = arrivals, p->max_out = max_out;
+    p->tmin = samples(0.0025), p->tmax = samples(0.015), p->wc = samples(0.020);
+    p->hist = p->wc + p->tmax;
+    p->lr = std::min(samples(0.004), packet);
+    p->ga = samples(0.010), p->gb = samples(0.060);
+    p->rf = JB_HEAD + p->R + (int64_t)p->R * packet + p->hist + p->tmax;
+    if ((int64_t)channels * p->rf > INT32_MAX)
+        return fail(1, who + ": a slot of " + std::to_string(channels) + " channels, window " + std::to_string(window) +
+                           " and packets of " + std::to_string(packet) + " samples is too large");
+    const int64_t floats = (int64_t)channels * (p->hist + (int64_t)max_out * packet) + p->hist +
+                           (int64_t)channels * p->tmax + p->R + arrivals + max_out;
+    return staging(who, floats, std::to_string(channels) + " channels at " + std::to_string(rate) + " Hz with " +
+                                    std::to_string(max_out) + " packets of " + std::to_string(packet) +
+                                    " samples written per row are too large", "words per row", smem);
+}
+}  // namespace l2h
+
+extern "C" int l2h_jitter_buffer_layout(int32_t channels, int32_t rate, int32_t packet, int32_t depth, int32_t window,
+                                        int32_t max_out, int32_t* row_floats) {
+    using namespace l2h;
+    if (!row_floats) return fail(1, "l2h_jitter_buffer_layout: null pointer");
+    JbParams p;
+    if (int rc = jb_params("l2h_jitter_buffer_layout", channels, rate, packet, depth, window, max_out, 1, &p, nullptr))
+        return rc;
+    *row_floats = (int32_t)p.rf;
+    return 0;
+}
+
+extern "C" int l2h_jitter_buffer(const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, int32_t max_in,
+                                 const int32_t* seqs_dev, const int32_t* counts_dev, float* y_dev, int64_t y_row_stride,
+                                 int64_t y_ch_stride, int32_t* out_counts_dev, int32_t n, int32_t channels,
+                                 const int32_t* slots_dev, float* state_dev, int32_t n_slots, int32_t rate, int32_t packet,
+                                 int32_t depth, int32_t window, int32_t max_out, void* stream) {
+    using namespace l2h;
+    const std::string who = "l2h_jitter_buffer";
+    if (int rc = slot_call(who, {x_dev, seqs_dev, counts_dev, y_dev, out_counts_dev, slots_dev, state_dev},
+                           "n, channels, max_in and n_slots", {n, channels, max_in, n_slots}, n, channels, n_slots))
+        return rc;
+    JbParams p;
+    int smem;
+    if (int rc = jb_params(who, channels, rate, packet, depth, window, max_out, max_in, &p, &smem)) return rc;
+    const Rows x{"x", x_row_stride, x_ch_stride, (int64_t)max_in * packet},
+        y{"y", y_row_stride, y_ch_stride, (int64_t)max_out * packet};
+    if (x.len > INT32_MAX) return fail(1, who + ": max_in * packet is too large");
+    if (int rc = disjoint(who, channels, {x, y})) return rc;
+    if (overlap(y_dev, n, y, x_dev, n, x, channels, false)) return fail(1, who + ": y must not overlap x");
+    if (smem > RS_SMEM_BYTES - 4096)                                    // then the static words need the opt-in
+        if (cudaError_t e = full_staging(jitter_buffer_kernel)) return fail(3, who + ": " + cudaGetErrorString(e));
+    jitter_buffer_kernel<<<(unsigned)n, RS_TILE, smem, static_cast<cudaStream_t>(stream)>>>(
+        x_dev, x_row_stride, x_ch_stride, seqs_dev, counts_dev, y_dev, y_row_stride, y_ch_stride, out_counts_dev, channels,
+        slots_dev, state_dev, n_slots, p);
     return launched(who);
 }

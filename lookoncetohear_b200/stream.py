@@ -6,8 +6,9 @@ per-slot capture that keeps each listener's recent input for enrollment (`Enroll
 the per-listener mixer that sums the separated voices and the ambient mixture into one row with fades (`TargetMixer`,
 `l2h_target_mix`), the per-listener look-ahead limiter that keeps the output under a ceiling with one gain for both
 ears (`Limiter`, `l2h_limiter`), the per-row leveler that brings each voice to one loudness with one gain for both
-ears (`Leveler`, `l2h_leveler`), and the per-listener multiband compressor that fits the output to each ear's hearing
-(`BandCompressor`, `l2h_band_compressor`).
+ears (`Leveler`, `l2h_leveler`), the per-listener multiband compressor that fits the output to each ear's hearing
+(`BandCompressor`, `l2h_band_compressor`), and the per-slot jitter buffer that puts a device's packets back in sequence
+order and conceals lost ones (`JitterBuffer`, `l2h_jitter_buffer`).
 
 Each stage keeps a float32 state [slots, channels, row floats] on a CUDA device.  All zeros is a fresh slot, so a
 listener is reset by zeroing its rows (`reset`) and moved by copying them.  No CPU fallback."""
@@ -839,3 +840,133 @@ class BandCompressor(_SlotStage):
     def gain(self):
         """[slots, channels, bands] float32 CUDA view of the state: each band's gain in dB at the last sample written"""
         return self.state[:, :, self.bands:2 * self.bands]
+
+
+class JitterBuffer(_SlotStage):
+    """A per-slot jitter buffer on the device (l2h_jitter_buffer): the first stage of a tick for devices that send packets
+    of `packet` samples at `rate` Hz with RTP's 16-bit sequence numbers over a lossy network.  It puts the packets back in
+    sequence order, drops late and duplicate ones, and conceals lost ones, so every later stage sees one continuous
+    stream at the device's rate: jb(x, seqs, counts, slots) -> (y, out_counts), then PacketResampler (unit=packet) or,
+    for a 16 kHz device, HopFifo (unit=packet).
+
+    Arrivals are processed one at a time in row order.  `next` is the sequence number of the next packet to decide (the
+    first packet of a fresh slot sets it), and d = (s - next) mod 2**16 taken in [-2**15, 2**15).  A packet with d < 0 is
+    late, one already held a duplicate, and one with d >= `window` restarts the slot (the held packets are dropped, next
+    := s, and the packet fades in).  Others are held.  Then, while next is held it is released; while it is missing and a
+    packet at least `depth` + 1 past it is held, it is declared lost and released as concealment.  In-order traffic is
+    therefore released on arrival, bit for bit with no added delay, and `depth` is the reordering a gap waits for.  A
+    call writes at most `max_out` released packets per row; the rest wait (a backlog of up to `window` packets) and are
+    written first by the slot's next call.  Decisions depend on the arrivals alone: cutting them into other calls, or
+    another max_out, moves only where the output is cut.
+
+    A lost packet repeats the last pitch period (2.5-15 ms, found by normalised autocorrelation over the last 20 ms of
+    the channel sum, one lag for all channels) at gain 1 for 10 ms, falling linearly to 0 at 60 ms and silent after; the
+    first real packet after a run or a restart fades in from the continuing concealment along a raised cosine over
+    min(4 ms, packet).  A non-finite sample, or one of magnitude 2**32 or more, enters as 0.
+
+    `state` [slots, channels, row] is a float32 tensor on `device`: all zeros is a fresh slot, so a listener is reset by
+    zeroing its rows (`reset`) and moved by copying them.  The counters are int32 views that never synchronise."""
+
+    SEQ = 1 << 16
+    LOST, LATE, DUPLICATE, DROPPED, RESTARTS, HELD, PITCH = 6, 7, 8, 9, 10, 11, 12   # head words of channel 0
+
+    def __init__(self, slots, channels, rate, packet, depth=1, window=16, max_out=4, device=None):
+        super().__init__(slots, channels)
+        self.rate, self.packet = _whole(rate, "rate"), _whole(packet, "packet")
+        self.depth, self.window = _whole(depth, "depth", 0), _whole(window, "window")
+        self.max_out = _whole(max_out, "max_out")
+        if self.depth >= self.window:
+            raise ValueError(f"depth must be below window = {self.window} packets, got {depth!r}")
+        self._allocate(*_layout(_cabi.lib().l2h_jitter_buffer_layout, self.channels, self.rate, self.packet, self.depth,
+                                self.window, self.max_out), device)
+
+    def __call__(self, x, seqs, counts, slots, out=None, out_counts=None):
+        """x [n, channels, M * packet] CUDA tensor: row i pushes its packets j < counts[i], x[i, :, j P:(j + 1) P], with
+        sequence numbers seqs[i, j], into slot slots[i].  Returns (y [n, channels, max_out * packet] float32, out_counts [n]
+        int32 CUDA) (`out` and `out_counts`, if given, written in place): row i receives y[i, :, :out_counts[i] * packet],
+        its slot's next packets in sequence order; its later samples are left unwritten.
+
+        Host lists are checked and uploaded (`slots` n distinct ints in [0, slots), `counts` n ints in [0, M], `seqs` [n, M]
+        int32 values whose first counts[i] entries of row i lie in [0, 65535], so a short row may be padded with -1; with
+        counts on the device every entry is checked); contiguous CUDA int32 tensors are used in place and read when the kernel runs, where a slot
+        outside [0, slots) or a count outside [0, M] marks a row that stores nothing and gets out count 0, and a sequence
+        number outside [0, 65535] marks a packet that is skipped.  So a call captured in the tick's CUDA graph serves any
+        lists rewritten in place."""
+        x = self._rows_in(x, self.packet)
+        dev = self.state.device
+        n, C, L = x.shape
+        M = L // self.packet
+        slots = device_list(slots, dev, n, self.n_slots, True, "slot")
+        host_counts = None if isinstance(counts, torch.Tensor) and counts.is_cuda else counts
+        counts = device_list(counts, dev, n, M + 1, False, "count")
+        seqs = self._seqs(seqs, n, M, host_counts)
+        out = self._rows_out(out, (n, C, self.max_out * self.packet))
+        out_counts = self._ints_out(out_counts, n, "out_counts")
+        self._run("l2h_jitter_buffer", x, x.stride(0), x.stride(1), M, seqs, counts, out, out.stride(0), out.stride(1),
+                  out_counts, n, C, slots, self.state, self.n_slots, self.rate, self.packet, self.depth, self.window,
+                  self.max_out)
+        return out, out_counts
+
+    def _seqs(self, seqs, n, M, counts=None):
+        """the [n, M] int32 sequence numbers on the state's device: a CUDA tensor used in place, else checked (the
+        entries each row pushes, given host `counts`, else all of them) and uploaded"""
+        dev = self.state.device
+        if isinstance(seqs, torch.Tensor) and seqs.is_cuda:
+            if seqs.dtype != torch.int32 or tuple(seqs.shape) != (n, M) or not seqs.is_contiguous() or seqs.device != dev:
+                raise ValueError(f"a CUDA seqs tensor must be a contiguous int32 tensor of shape ({n}, {M}) on {dev}")
+            return seqs
+        v = torch.as_tensor(seqs)
+        if v.dtype.is_floating_point or v.dtype.is_complex or v.dtype == torch.bool or tuple(v.shape) != (n, M):
+            raise ValueError(f"seqs must be integers of shape ({n}, {M}), got {tuple(v.shape)} {v.dtype}")
+        if v.numel() and (int(v.min()) < -2 ** 31 or int(v.max()) >= 2 ** 31):
+            raise ValueError("sequence numbers must be int32 values")
+        pushed = torch.ones(n, M, dtype=torch.bool) if counts is None else \
+            torch.arange(M)[None] < torch.as_tensor(counts).reshape(n, 1)
+        if bool(((v < 0) | (v >= self.SEQ))[pushed].any()):
+            raise ValueError("the sequence numbers of pushed packets must lie in [0, 65535]")
+        return v.to(torch.int32).contiguous().to(dev)
+
+    def _word(self, k):
+        return self.state[:, 0, k].view(torch.int32)
+
+    @property
+    def lost(self):
+        """[slots] int32 CUDA view: packets declared lost and concealed since the slot's reset (saturating)"""
+        return self._word(self.LOST)
+
+    @property
+    def late(self):
+        """[slots] int32 CUDA view: packets that arrived after their turn and were dropped (saturating)"""
+        return self._word(self.LATE)
+
+    @property
+    def duplicate(self):
+        """[slots] int32 CUDA view: packets that arrived while the same number was held and were dropped (saturating)"""
+        return self._word(self.DUPLICATE)
+
+    @property
+    def dropped(self):
+        """[slots] int32 CUDA view: held packets a restart discarded, and released ones a full backlog discarded
+        (saturating)"""
+        return self._word(self.DROPPED)
+
+    @property
+    def restarts(self):
+        """[slots] int32 CUDA view: arrivals beyond the window that restarted the slot (saturating)"""
+        return self._word(self.RESTARTS)
+
+    @property
+    def held(self):
+        """[slots] int32 CUDA view: packets stored and waiting for their turn"""
+        return self._word(self.HELD)
+
+    @property
+    def next(self):
+        """[slots] int32 CUDA view: the sequence number of the next packet to decide (released packets a call has not
+        written yet, `max_out` per row, play before it)"""
+        return self._word(1)
+
+    @property
+    def pitch(self):
+        """[slots] int32 CUDA view: the lag, in samples, of the last concealment run (0 before the first)"""
+        return self._word(self.PITCH)
