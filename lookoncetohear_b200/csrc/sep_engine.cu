@@ -977,8 +977,7 @@ static int enqueue_pipeline(SepEngine* e, const ChainArgs& a, int K, cudaStream_
     }
     for (int i = 1; i < PIPE_STREAMS; ++i)                             // join
         if (int rc = edge(e->pipe_streams[i], origin)) return rc;
-    advance_header_kernel<<<1, 256, 0, origin>>>(state, ss, B, K);       // every clock: pos += K, calls += 1, after every hop of the group
-    CK(cudaGetLastError());
+    CK(launch_advance_header(origin, state, ss, B, K));       // every clock: pos += K, calls += 1, after every hop of the group
     return 0;
 }
 
@@ -1177,10 +1176,7 @@ int l2h_sep_state_bytes(void* handle, int32_t batch, size_t* bytes) {
 int l2h_sep_state_init(void* handle, void* state, int32_t batch, void* stream) {
     SepEngine* e = static_cast<SepEngine*>(handle);
     if (!e || !state || batch <= 0) return fail(1, "bad argument");
-    const int64_t ss = stream_stride(e->n_blocks);
-    const int64_t total = sizeof(StateHeader) / 4 + (int64_t)batch * ss;
-    state_init_kernel<<<592, 256, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<float*>(state), total, ss, batch);
-    CK(cudaGetLastError());
+    CK(launch_state_init(static_cast<cudaStream_t>(stream), static_cast<float*>(state), stream_stride(e->n_blocks), batch));
     e->launch_count += 1;
     return 0;
 }
@@ -1204,18 +1200,11 @@ int l2h_sep_state_reset_streams(void* handle, void* state, int32_t batch, const 
     if (batch <= 0 || n <= 0 || n > batch) return fail(1, "batch and the slot count must be positive, slots at most batch");
     if (int rc = check_slots(slots_host, n, batch, "reset_streams")) return rc;
     if (int rc = check_device(e)) return rc;
-    const int64_t ss = stream_stride(e->n_blocks);
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    for (int32_t i0 = 0; i0 < n; i0 += RESET_MAX_SLOTS) {       // one launch for up to RESET_MAX_SLOTS records
-        const int32_t k = std::min<int32_t>(RESET_MAX_SLOTS, n - i0);
-        SlotList sl{};
-        std::copy(slots_host + i0, slots_host + i0 + k, sl.s);
-        // ~2 CTAs per SM over all records: each record is 6 MB of stores
-        const unsigned per_rec = (unsigned)std::max(1, 2 * NUM_SMS / k);
-        reset_streams_kernel<<<dim3(per_rec, k), 256, 0, st>>>(static_cast<float*>(state), ss, sl);
-        CK(cudaGetLastError());
-        e->launch_count += 1;
-    }
+    const long long before = g_launches;
+    const cudaError_t ce = launch_reset_streams(static_cast<cudaStream_t>(stream), static_cast<float*>(state),
+                                                stream_stride(e->n_blocks), slots_host, n);
+    e->launch_count += g_launches - before;
+    CK(ce);
     return 0;
 }
 
@@ -1278,16 +1267,10 @@ int l2h_sep_state_move_lead(void* handle, void* state, int32_t batch, const int3
             return fail(1, "move_lead: records " + std::to_string(old_host[i]) + " and " + std::to_string(new_host[i]) +
                                " have different clocks (" + std::to_string(clk[2 * i]) + " and " + std::to_string(clk[2 * i + 1]) +
                                " frames)");
-    for (int32_t i0 = 0; i0 < n; i0 += MOVE_MAX_PAIRS) {
-        const int32_t k = std::min<int32_t>(MOVE_MAX_PAIRS, n - i0);
-        PairList pl{};
-        std::copy(old_host + i0, old_host + i0 + k, pl.from);
-        std::copy(new_host + i0, new_host + i0 + k, pl.to);
-        const unsigned per_rec = (unsigned)std::max(1, 2 * NUM_SMS / k);      // as reset_streams: ~2 CTAs per SM over all records
-        move_lead_kernel<<<dim3(per_rec, k), 256, 0, st>>>(static_cast<float*>(state), ss, pl);
-        CK(cudaGetLastError());
-        e->launch_count += 1;
-    }
+    const long long before = g_launches;
+    const cudaError_t ce = launch_move_lead(st, static_cast<float*>(state), ss, old_host, new_host, n);
+    e->launch_count += g_launches - before;
+    CK(ce);
     return 0;
 }
 
@@ -1594,8 +1577,7 @@ int l2h_sep_stream_dev(void* handle, const float* x_dev, int32_t x_len, const fl
     if (!e || !x_dev || !emb || !state || !y_dev || !ws) return fail(1, "null argument");
     if (n_calls <= 0 || cpc <= 0) return fail(1, "n_calls and chunks_per_call must be positive");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    set_clip_base_kernel<<<1, 1, 0, st>>>(static_cast<float*>(state));
-    CK(cudaGetLastError());
+    CK(launch_set_clip_base(st, static_cast<float*>(state)));
     e->launch_count += 1;
     ChainArgs a{x_dev, (int64_t)NMIC * x_len, x_len, x_len, emb, static_cast<float*>(state), y_dev,
                 (int64_t)NSRC * y_len, y_len, y_len, batch, cpc, static_cast<float*>(ws), ws_bytes, 0, 1};

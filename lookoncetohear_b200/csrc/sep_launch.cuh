@@ -235,4 +235,34 @@ inline cudaError_t launch_inter_h_last(cudaStream_t st, int B, const float* Y, f
     return launch_k(false, inter_h_last_kernel, dim3(B), dim3(256), 0, st, Y, Hg, recs, T);
 }
 
+// The state kernels (l2h_sep_state_init, l2h_sep_state_reset_streams, l2h_sep_stream_dev and the pipelined graph).  Their
+// launchers sit here rather than beside the kernels in sep_kernels.cuh: defined there, they changed the code nvcc
+// generated for kernels that do not use them.
+// state_init_kernel: the whole state of B records of `stride` floats, 592 CTAs of 256 threads
+inline cudaError_t launch_state_init(cudaStream_t st, float* state, int64_t stride, int B) {
+    const int64_t total = (int64_t)(sizeof(StateHeader) / 4) + (int64_t)B * stride;
+    return launch_k(false, state_init_kernel, dim3(592), dim3(256), 0, st, state, total, stride, B);
+}
+// reset_streams_kernel over the host list slots[0 .. n-1]: one launch per RESET_MAX_SLOTS of them, each of ~2 CTAs per SM
+// over all its records (each record is 6 MB of stores)
+inline cudaError_t launch_reset_streams(cudaStream_t st, float* state, int64_t sstride, const int32_t* slots, int n) {
+    for (int i0 = 0; i0 < n; i0 += RESET_MAX_SLOTS) {
+        const int k = std::min(RESET_MAX_SLOTS, n - i0);
+        SlotList sl{};
+        std::copy(slots + i0, slots + i0 + k, sl.s);
+        const unsigned per_rec = (unsigned)std::max(1, 2 * NUM_SMS / k);
+        if (cudaError_t e = launch_k(false, reset_streams_kernel, dim3(per_rec, k), dim3(256), 0, st, state, sstride, sl)) return e;
+    }
+    return cudaSuccess;
+}
+// advance_header_kernel, the pipelined graph's last node: the header and each of the n_streams dense records advance by
+// `frames` frames and one call.  One CTA of 256 threads.
+inline cudaError_t launch_advance_header(cudaStream_t st, float* state, int64_t sstride, int n_streams, int frames) {
+    return launch_k(false, advance_header_kernel, dim3(1), dim3(256), 0, st, state, sstride, n_streams, frames);
+}
+// set_clip_base_kernel: one thread
+inline cudaError_t launch_set_clip_base(cudaStream_t st, float* state) {
+    return launch_k(false, set_clip_base_kernel, dim3(1), dim3(1), 0, st, state);
+}
+
 }  // namespace l2h

@@ -252,6 +252,19 @@ move_lead_kernel(float* __restrict__ state, int64_t ss, PairList pairs) {
     }
 }
 
+// move_lead_kernel over the host pairs from[i] -> to[i], i < n: one launch per MOVE_MAX_PAIRS of them, each of ~2 CTAs per
+// SM over all its pairs, as reset_streams
+inline cudaError_t launch_move_lead(cudaStream_t st, float* state, int64_t ss, const int32_t* from, const int32_t* to, int n) {
+    for (int i0 = 0; i0 < n; i0 += MOVE_MAX_PAIRS) {
+        const int k = std::min(MOVE_MAX_PAIRS, n - i0);
+        PairList pl{};
+        std::copy(from + i0, from + i0 + k, pl.from);
+        std::copy(to + i0, to + i0 + k, pl.to);
+        const unsigned per_rec = (unsigned)std::max(1, 2 * NUM_SMS / k);
+        if (cudaError_t e = launch_k(false, move_lead_kernel, dim3(per_rec, k), dim3(256), 0, st, state, ss, pl)) return e;
+    }
+    return cudaSuccess;
+}
 inline cudaError_t launch_history_put(bool pdl, cudaStream_t st, int M, const float* X0, const float* state, Records lead, float* hist,
                                       int F, int T) {
     return launch_k(pdl, history_put_kernel, dim3(T, M), dim3(256), 0, st, X0, state, lead, hist, F, T);

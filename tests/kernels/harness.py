@@ -118,10 +118,15 @@ TARGETS_SYMBOLS = ("kh_target_lists", "kh_spk_gate", "kh_gate_fanout", "kh_gathe
                    "kh_inter_h_last")
 EMBED_SYMBOLS = ("kh_embed_layout", "kh_estd", "kh_efront", "kh_egn_apply", "kh_eqkv_ln", "kh_softmax_rows",
                  "kh_eattn_out_grid", "kh_eattn_out", "kh_ehead", "kh_einter_mask", "kh_eput_lens")
+STATE_SYMBOLS = ("kh_state_limits", "kh_state_init", "kh_reset_streams", "kh_advance_header", "kh_set_clip_base", "kh_move_lead",
+                 "kh_join_start", "kh_history_put", "kh_history_get", "kh_eslot_rows", "kh_eput_rows", "kh_estd_ring",
+                 "kh_efront_ring")
 SYMBOLS = ("kh_gemm", "kh_gemm_plan", "kh_split_planes", "kh_lstm", "kh_launch_count", "kh_sep_layout", "kh_qkv",
            "kh_qkv_many", "kh_kv_gather", "kh_attention", "kh_attn_out", "kh_ln_frame_res",
            "kh_attn_cluster_resident", "kh_front", "kh_front_many", "kh_front_many_geometry", "kh_front1", "kh_back",
-           "kh_back_many", "kh_back_many_geometry") + EMBED_SYMBOLS + MID_SYMBOLS + TAIL_SYMBOLS + TARGETS_SYMBOLS + tuple(MIRRORS)
+           "kh_back_many", "kh_back_many_geometry") + EMBED_SYMBOLS + MID_SYMBOLS + TAIL_SYMBOLS + TARGETS_SYMBOLS + \
+          STATE_SYMBOLS + tuple(MIRRORS)
+STATE_LIMIT_NAMES = ("RESET_MAX_SLOTS", "MOVE_MAX_PAIRS", "SLOT_ROWS_PER_LAUNCH", "MIN_SAMPLES", "EC_HEAD")
 EMBED_LAYOUT_NAMES = ("NFFT", "HOP", "NF", "CH", "QK", "VDIM", "FC", "NQKV", "DFT_LD", "EAOUT_SMEM", "LENS_PER_LAUNCH")
 
 ATTN_FORMS = {"query": 0, "tile": 1, "cluster": 2}
@@ -211,6 +216,21 @@ def lib():
             "kh_scatter_hc": [P, RP, I, I, I, P, P, P],
             "kh_inter_gate_mask": [P, RP, I, P],
             "kh_inter_h_last": [P, P, RP, I, P],
+        })
+        sigs.update({
+            "kh_state_limits": [ctypes.POINTER(ctypes.c_int64)],
+            "kh_state_init": [P, I64, I, P],
+            "kh_reset_streams": [P, I64, I, P, I, P],
+            "kh_advance_header": [P, I64, I, I, P],
+            "kh_set_clip_base": [P, P],
+            "kh_move_lead": [P, I64, I, P, P, I, P],
+            "kh_join_start": [P, I64, I, P, P, I, I, P, P, P],
+            "kh_history_put": [P, P, RP, P, I, I, P],
+            "kh_history_get": [P, I, P, RP, P, P, I, P],
+            "kh_eslot_rows": [P, P, P, I, P, I, I, P, P, P, P],
+            "kh_eput_rows": [P, P, I64, P, I, P],
+            "kh_estd_ring": [P, I, P, P, I, P, P, I, P],
+            "kh_efront_ring": [EW, P, I, P, P, I, P, P, P, P, I, I, P],
         })
         L.kh_mid_pack.restype = None
         L.kh_mid_pack.argtypes = [P] * 6
@@ -1857,3 +1877,364 @@ METRICS_CASES = (
     ("no_embeddings", dict(B=300, C=2, n=257, seed=12, snr=(-30.0, 0.0, 45.0, 90.0), dc=(0.0, 100.0)),
      ("no_centre", "first_ear", "si_i_sign")),
 )
+
+
+# ---- the kernels that own a separator state's records (sep_kernels.cuh, targets_kernels.cuh) and the enrollment rows of
+# a capture (embed_kernels.cuh) -----------------------------------------------------------------------------------------
+# Every output is a copy, a fill or an integer, so each reference is exact.  The references work on int32 numpy arrays
+# holding the bits of the floats (a state, a ring, a list); `lay` is sep_layout()'s dict, `hdr` the header in floats and
+# `ss` the record stride.  A record's clock is the int64 in floats ST_POS, ST_POS + 1 (low word first).
+NAN_BITS = 0x7FC00000                # the quiet NaN the kernels write into a fresh record's embedding (the gate-memo key)
+HDR_POS, HDR_NCALLS, HDR_CLIP, HDR_DONE = 0, 2, 4, 6      # StateHeader fields, in floats
+CONV_PARITY = 2 * 4 * NF             # floats of one parity of the conv tails
+STATE_INIT_MUTANTS = ("from_zero", "emb_zero")
+RESET_MUTANTS = ("clock_kept", "first_chunk_only")
+ADVANCE_MUTANTS = ("pos32", "done_kept")
+JOIN_MUTANTS = ("clock_p", "no_clamp", "no_lead_clash", "no_record_clash")
+HIST_PUT_MUTANTS = ("first_F", "clock_after", "clock32")
+HIST_GET_MUTANTS = ("lead_clock", "no_zero", "clock32")
+MOVE_MUTANTS = ("src_parity", "all_blocks")
+SLOT_ROWS_MUTANTS = ("short_live", "no_clamp")
+PUT_ROWS_MUTANTS = ("dead_written",)
+RING_MUTANTS = ("no_wrap",)
+
+
+def state_limits():
+    """kh_state_limits as {name: value} (STATE_LIMIT_NAMES)"""
+    out = (ctypes.c_int64 * 8)()
+    n = lib().kh_state_limits(out)
+    return dict(zip(STATE_LIMIT_NAMES, list(out)[:n]))
+
+
+def _i32(v):
+    return (ctypes.c_int32 * len(v))(*v)
+
+
+def state_init(state, stride, B):
+    return lib().kh_state_init(ptr(state), stride, B, stream())
+
+
+def reset_streams(state, sstride, batch, slots):
+    return lib().kh_reset_streams(ptr(state), sstride, batch, _i32(slots), len(slots), stream())
+
+
+def advance_header(state, sstride, n_streams, frames):
+    return lib().kh_advance_header(ptr(state), sstride, n_streams, frames, stream())
+
+
+def set_clip_base(state):
+    return lib().kh_set_clip_base(ptr(state), stream())
+
+
+def move_lead(state, ss, batch, src, dst):
+    return lib().kh_move_lead(ptr(state), ss, batch, _i32(src), _i32(dst), len(src), stream())
+
+
+def join_start(state, ss, batch, records, leads, w_max, J, lists, used_out):
+    """records, leads: device int32 [J]; lists: device int32 [3 J] (rec, used, owner); used_out: device [J] or None"""
+    return lib().kh_join_start(ptr(state), ss, batch, ptr(records), ptr(leads), w_max, J, ptr(lists), ptr(used_out), stream())
+
+
+def history_put(X0, state, lead, hist, F, M):
+    """lead: the Records map of the listeners' lead records and hop counts, frames = T"""
+    return lib().kh_history_put(ptr(X0), ptr(state), ctypes.byref(lead), ptr(hist), F, M, stream())
+
+
+def history_get(hist, F, state, recs, leads, X0, J):
+    """recs: the join's Records map (slots = rec, hops = used, frames = T)"""
+    return lib().kh_history_get(ptr(hist), F, ptr(state), ctypes.byref(recs), ptr(leads), ptr(X0), J, stream())
+
+
+def eslot_rows(slots_host, slots_dev, lens_host, n, capture, n_slots, capacity, slots_out, lens, used):
+    return lib().kh_eslot_rows(None if slots_host is None else _i32(slots_host), ptr(slots_dev), _i32(lens_host), n, ptr(capture),
+                               n_slots, capacity, ptr(slots_out), ptr(lens), ptr(used), stream())
+
+
+def eput_rows(src, dst, row_stride, used, B):
+    return lib().kh_eput_rows(ptr(src), ptr(dst), row_stride, ptr(used), B, stream())
+
+
+def estd_ring(capture, capacity, slots, used, N, lens, inv_std, B):
+    return lib().kh_estd_ring(ptr(capture), capacity, ptr(slots), ptr(used), N, ptr(lens), ptr(inv_std), B, stream())
+
+
+def efront_ring(w, capture, capacity, slots, used, N, lens, inv_std, X, gn_sums, B, T):
+    return lib().kh_efront_ring(ctypes.byref(w), ptr(capture), capacity, ptr(slots), ptr(used), N, ptr(lens), ptr(inv_std),
+                                ptr(X), ptr(gn_sums), B, T, stream())
+
+
+def get64(a, i):
+    """the int64 in int32 words a[i] (low), a[i + 1] (high)"""
+    return (int(a[i]) & 0xFFFFFFFF) | (int(a[i + 1]) << 32)
+
+
+def put64(a, i, v):
+    v &= (1 << 64) - 1
+    lo, hi = v & 0xFFFFFFFF, v >> 32
+    a[i], a[i + 1] = lo - (1 << 32) if lo >= 1 << 31 else lo, hi - (1 << 32) if hi >= 1 << 31 else hi
+
+
+def fresh_record(ss, lay, clock=0):
+    """a record as reset_streams_kernel leaves it (clock 0) and join_start_kernel (its clock): the embedding NaN, every other
+    float 0, the clock words set"""
+    r = np.zeros(ss, dtype=np.int32)
+    r[:SPK] = NAN_BITS
+    put64(r, lay["ST_POS"], clock)
+    return r
+
+
+def state_init_ref(hdr, ss, B, mutant=None):
+    """state_init_kernel: the header 0, in each record the SPK embedding floats NaN and the rest 0.  Mutants
+    (STATE_INIT_MUTANTS): from_zero (records counted from float 0, not from the end of the header), emb_zero (no NaN)."""
+    i = np.arange(hdr + B * ss, dtype=np.int64)
+    o = i % ss if mutant == "from_zero" else (i - hdr) % ss
+    nan = (i >= hdr) & (o < SPK) & (mutant != "emb_zero")
+    return np.where(nan, NAN_BITS, 0).astype(np.int32)
+
+
+def reset_streams_ref(state, hdr, ss, lay, slots, mutant=None):
+    """reset_streams_kernel: each listed record becomes fresh_record(ss) (clock 0, calls 0), whole stride.  Mutants
+    (RESET_MUTANTS): clock_kept (the calls and clock words left as they were), first_chunk_only (slots past the first
+    RESET_MAX_SLOTS skipped)."""
+    out = state.copy()
+    lim = state_limits()["RESET_MAX_SLOTS"] if mutant == "first_chunk_only" else len(slots)
+    for s in slots[:lim]:
+        r = out[hdr + s * ss:hdr + (s + 1) * ss]
+        keep = r[lay["ST_CALLS"]:lay["ST_POS"] + 2].copy()
+        r[:] = fresh_record(ss, lay)
+        if mutant == "clock_kept":
+            r[lay["ST_CALLS"]:lay["ST_POS"] + 2] = keep
+    return out
+
+
+def _add64(a, i, d, bits32=False):
+    if bits32:                       # the low word wraps, the high word stays
+        a[i] = np.int32(((int(a[i]) + d + (1 << 31)) % (1 << 32)) - (1 << 31))
+    else:
+        put64(a, i, get64(a, i) + d)
+
+
+def advance_header_ref(state, hdr, ss, lay, n_streams, frames, mutant=None):
+    """advance_header_kernel: header pos += frames, ncalls += 1, done = 0; each of records 0 .. n_streams-1: clock +=
+    frames, calls += 1 (int32, wrapping).  Mutants (ADVANCE_MUTANTS): pos32 (every clock carried in 32 bits), done_kept."""
+    out = state.copy()
+    _add64(out, HDR_POS, frames, mutant == "pos32")
+    _add64(out, HDR_NCALLS, 1)
+    if mutant != "done_kept":
+        out[HDR_DONE] = 0
+    for b in range(n_streams):
+        o = hdr + b * ss
+        _add64(out, o + lay["ST_POS"], frames, mutant == "pos32")
+        out[o + lay["ST_CALLS"]] = np.int32(((int(out[o + lay["ST_CALLS"]]) + 1 + (1 << 31)) % (1 << 32)) - (1 << 31))
+    return out
+
+
+def set_clip_base_ref(state):
+    out = state.copy()
+    out[HDR_CLIP:HDR_CLIP + 2] = out[HDR_POS:HDR_POS + 2]
+    return out
+
+
+def join_start_ref(records, leads, clocks, batch, w_max, mutant=None):
+    """join_start_kernel of int lists: row j is live when records[j] and leads[j] lie in [0, batch) and records[j] is no
+    other row's record and no row's lead (its own included); W_j = min(w_max, p) with p = clocks[leads[j]].  Returns rec,
+    used, owner (the lists) and start {record: its new clock p - W_j}.  Mutants (JOIN_MUTANTS): clock_p (the new clock p),
+    no_clamp (W = w_max), no_lead_clash, no_record_clash."""
+    J = len(records)
+    rec, used, owner, start = [], [], [], {}
+    for j in range(J):
+        s, l = records[j], leads[j]
+        clash = (mutant != "no_record_clash" and any(k != j and records[k] == s for k in range(J))) or \
+            (mutant != "no_lead_clash" and any(leads[k] == s for k in range(J)))
+        live = not clash and 0 <= s < batch and 0 <= l < batch
+        p = clocks[l] if live else 0
+        W = w_max if mutant == "no_clamp" else min(w_max, p)
+        rec.append(s if live else -1)
+        used.append(W if live else 0)
+        owner.append(j if live else -1)
+        if live:
+            start[s] = p if mutant == "clock_p" else p - W
+    return dict(rec=rec, used=used, owner=owner, start=start)
+
+
+def _slot(clock, t, F, mutant):
+    fr = clock + t
+    return (fr % (1 << 32)) % F if mutant == "clock32" else fr % F
+
+
+def history_put_ref(hist, X0, leads, hops, clocks, F, T, batch, mutant=None):
+    """history_put_kernel: hist [batch][F][...] after listener i's last min(h_i, F) frames t (h_i - F <= t < h_i, h_i =
+    row_frames(hops, i, T)) went to slot (clocks[l] + t) mod F of its lead l, when l lies in [0, batch) and h_i > 0.  Mutants
+    (HIST_PUT_MUTANTS): first_F (the first min(h_i, F) frames), clock_after (the slot from the clock after the tick,
+    clocks[l] + h_i), clock32 (the slot from the clock's low 32 bits)."""
+    out = hist.copy()
+    for i, l in enumerate(leads):
+        h = row_frames(hops, i, T)
+        if not (0 <= l < batch and h > 0):
+            continue
+        c = clocks[l] + (h if mutant == "clock_after" else 0)
+        for t in (range(min(h, F)) if mutant == "first_F" else range(max(0, h - F), h)):
+            out[l, _slot(c, t, F, mutant)] = X0[i, t]
+    return out
+
+
+def history_get_ref(hist, rec, used, leads, clocks, F, T, batch, mutant=None):
+    """history_get_kernel: X0 [J][T][...], row j's frame t < used_j = row_frames(used, j, T) is slot (clocks[rec_j] + t) mod F
+    of the ring of leads[j] when rec_j lies in [0, batch) and used_j > 0; every other frame 0.  Mutants (HIST_GET_MUTANTS):
+    lead_clock (the slot from the lead's clock), no_zero (a live row's frames t >= used_j replayed too), clock32."""
+    out = np.zeros((len(rec), T) + hist.shape[2:], dtype=hist.dtype)
+    for j, s in enumerate(rec):
+        h = row_frames(used, j, T)
+        if not (0 <= s < batch and h > 0):
+            continue
+        c = clocks[leads[j]] if mutant == "lead_clock" else clocks[s]
+        for t in range(T if mutant == "no_zero" else h):
+            out[j, t] = hist[leads[j], _slot(c, t, F, mutant)]
+    return out
+
+
+def move_lead_ref(state, hdr, ss, lay, n_blocks, src, dst, mutant=None, conv_parity=CONV_PARITY):
+    """move_lead_kernel: for each pair, block 0 of record src[i] (BK_STRIDE floats from ST_BLK) and the conv tails of its
+    current parity (calls & 1, conv_parity floats) go to record dst[i], the tails into dst[i]'s current parity.  Mutants (MOVE_MUTANTS):
+    src_parity (the tails into src[i]'s parity), all_blocks (blocks 1 and up copied too)."""
+    out = state.copy()
+    nblk = n_blocks if mutant == "all_blocks" else 1
+    for a, b in zip(src, dst):
+        ra, rb = out[hdr + a * ss:hdr + (a + 1) * ss], out[hdr + b * ss:hdr + (b + 1) * ss]
+        o = lay["ST_BLK"]
+        rb[o:o + nblk * lay["BK_STRIDE"]] = ra[o:o + nblk * lay["BK_STRIDE"]]
+        pa, pb = int(ra[lay["ST_CALLS"]]) & 1, int(rb[lay["ST_CALLS"]]) & 1
+        if mutant == "src_parity":
+            pb = pa
+        c = lay["ST_CONV"]
+        rb[c + pb * conv_parity:c + (pb + 1) * conv_parity] = ra[c + pa * conv_parity:c + (pa + 1) * conv_parity]
+    return out
+
+
+def eslot_rows_ref(slots, lens, captured, n_slots, capacity, min_samples, mutant=None):
+    """eslot_rows_kernel: row i of slot s = slots[i] (in: 0 <= s < n_slots), captured[s] the capture head's raw count,
+    clamped to [0, capacity]: used = min(lens[i], captured) if that is >= min_samples else 0 (0 for a slot outside),
+    lens_out = used or min_samples, slots_out = s or 0.  Mutants (SLOT_ROWS_MUTANTS): short_live (a row below
+    min_samples kept live), no_clamp (the raw count)."""
+    out_s, out_l, out_u = [], [], []
+    for s, n in zip(slots, lens):
+        inside = 0 <= s < n_slots
+        c = captured[s] if inside else 0
+        if mutant != "no_clamp":
+            c = min(max(c, 0), capacity)
+        u = min(n, c)
+        use = u if (u > 0 if mutant == "short_live" else u >= min_samples) else 0
+        out_s.append(s if inside else 0)
+        out_l.append(use if use > 0 else min_samples)
+        out_u.append(use)
+    return dict(slots=out_s, lens=out_l, used=out_u)
+
+
+def eput_rows_ref(dst, src, used, row_stride, mutant=None):
+    """eput_rows_kernel: dst row b (row_stride floats apart) = src[b] [256] for used[b] > 0.  Mutant (PUT_ROWS_MUTANTS):
+    dead_written (every row written)."""
+    out = dst.copy()
+    for b, u in enumerate(used):
+        if u > 0 or mutant == "dead_written":
+            out[b * row_stride:b * row_stride + 256] = src[b]
+    return out
+
+
+def ring_utterance(rings, wpos, n, capacity, mutant=None):
+    """XRing's utterance of n samples: rings [2][capacity] of one slot, the head's write position clamped to
+    [0, capacity - 1]; the n samples before it, oldest first, wrapping past the ring's start.  Mutant (RING_MUTANTS):
+    no_wrap (the start wpos - n not wrapped, so sample s reads ring index wpos - n + s; one below 0 reads 0)."""
+    w = min(max(wpos, 0), capacity - 1)
+    start = w - n
+    if mutant != "no_wrap" and start < 0:
+        start += capacity
+    idx = np.arange(n) + start
+    idx = np.where(idx >= capacity, idx - capacity, idx)
+    out = np.zeros((2, n), dtype=rings.dtype)
+    ok = idx >= 0
+    out[:, ok] = rings[:, idx[ok]]
+    return out
+
+
+# The clocks the state tests set: around 2^31 and 2^32, where a clock carried in 32 bits goes wrong, and 2^40 + 7
+CLOCKS = (0, 1, 49, 2 ** 31 - 1, 2 ** 31 + 3, 2 ** 32 - 1, 2 ** 32 + 5, 2 ** 40 + 7)
+HIST_F = (1, 7, 50, 64)          # 7 and 50 do not divide 2^32: a 32-bit clock puts a frame into another slot
+
+
+def join_start_case(w_max):
+    """a join over a state of 30 records: leads 10 .. 19 at clocks 0, 1, 49, 50, 51 and the 2^31 / 2^32 / 2^40 ones,
+    duplicated records, a record that is another row's lead or its own, records and leads -1, batch and 2^31 - 1, and
+    two rows on one lead.  Returns records, leads, clocks [batch], batch, w_max and `catches`."""
+    batch = 30
+    clocks = [2 ** 33 + 17 * k for k in range(batch)]
+    for k, c in enumerate((0, 1, 49, 50, 51, 2 ** 31 - 1, 2 ** 31 + 3, 2 ** 32 - 1, 2 ** 32 + 5, 2 ** 40 + 7)):
+        clocks[10 + k] = c
+    rows = [(k, 10 + k) for k in range(10)] + [
+        (20, 19),                    # a second row on lead 19
+        (21, 18), (21, 17),          # one record listed twice
+        (18, 15),                    # the lead of row 8
+        (22, 22),                    # its own lead
+        (-1, 10), (batch, 10), (INT_MAX, 10), (23, -1), (24, batch), (25, INT_MAX),
+        (26, 11)]                    # a second row on lead 11
+    catches = {"no_lead_clash", "no_record_clash"} | ({"clock_p", "no_clamp"} if w_max > 0 else set())
+    return dict(records=[r for r, _ in rows], leads=[l for _, l in rows], clocks=clocks, batch=batch, w_max=w_max,
+                catches=catches)
+
+
+def history_put_case(F):
+    """ten listeners of a tick of T = F + 6 frames into rings of F: ragged hop counts (T, 0, -1, T + 1, 1, F, F + 1,
+    T - 1), leads 0 .. 6 at clocks around 2^31, 2^32 and 2^40, and leads -1, batch and 2^31 - 1"""
+    T, batch = F + 6, 8
+    leads = [0, 1, 2, 3, 4, 5, 6, -1, batch, INT_MAX]
+    hops = [T, 0, -1, T + 1, 1, F, F + 1, T - 1, T, T]
+    clocks = [2 ** 32 - 1, 2 ** 32 + 5, 49, 2 ** 31 - 1, 2 ** 40 + 7, 2 ** 31 + 3, 0, 1]
+    catches = {1: {"first_F"}, 64: {"first_F", "clock_after"}}.get(F, set(HIST_PUT_MUTANTS))
+    return dict(leads=leads, hops=hops, clocks=clocks, F=F, T=T, batch=batch, catches=catches)
+
+
+def history_get_case(F):
+    """eight join rows over T = 6 frames: used T, 1, T - 1, 0, T + 1 and -1; records -1 and batch; leads 4 and 5 (whose
+    clocks differ from the rows'), and -1 and 2^31 - 1 on rows that store nothing"""
+    T, batch = 6, 8
+    rec = [0, 1, 2, 3, -1, batch, 6, 7]
+    used = [T, 1, T - 1, 0, T, T, T + 1, -1]
+    leads = [4, 5, 4, 5, -1, INT_MAX, 4, 5]
+    clocks = [2 ** 32 + 5, 2 ** 40 + 7, 2 ** 31 + 3, 2 ** 32 - 1, 49, 2 ** 31 - 1, 1, 0]
+    catches = {1: {"no_zero"}, 64: {"lead_clock", "no_zero"}}.get(F, set(HIST_GET_MUTANTS))
+    return dict(rec=rec, used=used, leads=leads, clocks=clocks, F=F, T=T, batch=batch, catches=catches)
+
+
+SLOT_CAPTURED = (-5, 0, 191, 192, 500, 1000, 1001, INT_MAX, -INT_MAX, 700)
+SLOT_LENS = (192, 191, 150, 300, 1000, 1200, INT_MAX, 0, -3)
+
+
+def eslot_rows_case(n, device, limit):
+    """n rows of a capture of 500 slots of capacity 1000; each slot's raw captured count from SLOT_CAPTURED (negative,
+    below MIN_SAMPLES, above capacity), lengths from SLOT_LENS; a device list also lists slots -1, n_slots and 2^31 - 1.
+    Row 0 is one only the clamp decides (captured 1001, length 1200), row 1 one only the MIN_SAMPLES rule does
+    (captured 191).  `limit` = SLOT_ROWS_PER_LAUNCH: the rows cross it when n does."""
+    import random
+    g = random.Random(n * 2 + device)
+    n_slots, capacity = 500, 1000
+    captured = [SLOT_CAPTURED[s % len(SLOT_CAPTURED)] for s in range(n_slots)]
+    slots = [g.randrange(n_slots) for _ in range(n)]
+    lens = [SLOT_LENS[i % len(SLOT_LENS)] for i in range(n)]
+    if device:
+        for i, s in zip(range(2, n, 7), (-1, n_slots, INT_MAX) * n):
+            slots[i] = s
+    slots[0], lens[0] = 6, 1200                             # captured 1001
+    if n > 1:
+        slots[1], lens[1] = 2, 400                          # captured 191
+        if n > limit:
+            slots[limit], lens[limit] = 16, 1200            # the second launch's first row: captured 1001 again
+    catches = {"no_clamp"} | ({"short_live"} if n > 1 else set())
+    return dict(slots=slots, lens=lens, captured=captured, n_slots=n_slots, capacity=capacity, device=device, catches=catches)
+
+
+def ring_cases(min_samples):
+    """XRing calls: (capacity, rows of (raw write position, n, live)).  Write positions 0, n - 1, n, capacity - 1 and one
+    past the ring (clamped), n == capacity, capacity == MIN_SAMPLES, and a row that is not live."""
+    m = min_samples
+    return [dict(name="cap1000", capacity=1000, rows=[(0, 700, True), (699, 700, True), (700, 700, True), (999, 700, True),
+                                                      (300, 1000, True), (5000, 640, True), (10, 400, False), (250, 193, True)]),
+            dict(name="cap_min", capacity=m, rows=[(0, m, True), (100, m, True), (m - 1, m, True), (m - 1, m, False)])]

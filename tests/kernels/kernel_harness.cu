@@ -5,8 +5,11 @@
 // chain's cell kernel (sep_kernels.cuh: lstm_cell_rows), the enrollment network's own kernels (embed_kernels.cuh: estd,
 // efront, egn_apply, eqkv_ln, softmax_rows, eattn_out, ehead, einter_mask, eput_lens), the several-target kernels
 // (targets_kernels.cuh: target_lists, spk_gate, gate_fanout) and the slot-list helpers (sep_kernels.cuh: gather_h,
-// scatter_hc, inter_gate_mask, inter_h_last), so that the kernel-level tests (tests/test_*_kernels_gpu.py) can drive each kernel directly with arbitrary
-// shapes and compare it element by element with a float64 reference.
+// scatter_hc, inter_gate_mask, inter_h_last), the kernels that own a separator state's records (sep_kernels.cuh:
+// state_init, reset_streams, advance_header, set_clip_base; targets_kernels.cuh: join_start, history_put, history_get,
+// move_lead), the enrollment-from-capture kernels (embed_kernels.cuh: eslot_rows, eput_rows, and estd / efront over the
+// capture ring's XRing map), so that the kernel-level tests (tests/test_*_kernels_gpu.py) can drive each kernel directly
+// with arbitrary shapes and compare it element by element with a float64 or exact reference.
 //
 // The argument structs below are plain C (mirrored with ctypes in the tests); every function checks its arguments, fills
 // the engine's own descriptor and calls the engine's own launcher.  Built by
@@ -742,4 +745,118 @@ KH_API int kh_inter_gate_mask(float* gx, const KhRecords* recs, int B, void* str
 KH_API int kh_inter_h_last(const float* Y, float* Hg, const KhRecords* recs, int B, void* stream) {
     if (!records_ok(recs) || B <= 0) return (int)cudaErrorInvalidValue;
     return (int)launch_inter_h_last(static_cast<cudaStream_t>(stream), B, Y, Hg, to_records(*recs), recs->frames);
+}
+
+// ---- the kernels that own a separator state's records (sep_kernels.cuh, targets_kernels.cuh) -------------------------
+// RESET_MAX_SLOTS, MOVE_MAX_PAIRS, SLOT_ROWS_PER_LAUNCH, MIN_SAMPLES (embed_kernels.cuh), EC_HEAD; returns the count
+// written (5)
+KH_API int kh_state_limits(int64_t* out) {
+    const int64_t v[] = {RESET_MAX_SLOTS, MOVE_MAX_PAIRS, emb::SLOT_ROWS_PER_LAUNCH, emb::MIN_SAMPLES, EC_HEAD};
+    const int n = (int)(sizeof(v) / sizeof(v[0]));
+    for (int i = 0; i < n; ++i) out[i] = v[i];
+    return n;
+}
+
+// state_init_kernel over a state of B records of `stride` floats
+KH_API int kh_state_init(float* state, int64_t stride, int B, void* stream) {
+    if (state == nullptr || stride <= 0 || B <= 0) return (int)cudaErrorInvalidValue;
+    return (int)launch_state_init(static_cast<cudaStream_t>(stream), state, stride, B);
+}
+
+// reset_streams_kernel over the host list slots_host[0 .. n-1], each in [0, batch); records sstride floats apart, a
+// multiple of 4 that holds at least the SPK floats of the embedding
+static bool slots_in(const int32_t* s, int n, int batch) {
+    for (int i = 0; i < n; ++i)
+        if (s[i] < 0 || s[i] >= batch) return false;
+    return true;
+}
+KH_API int kh_reset_streams(float* state, int64_t sstride, int batch, const int32_t* slots_host, int n, void* stream) {
+    if (state == nullptr || slots_host == nullptr || sstride < SPK || sstride % 4 != 0 || batch <= 0 || n <= 0 ||
+        !slots_in(slots_host, n, batch))
+        return (int)cudaErrorInvalidValue;
+    return (int)launch_reset_streams(static_cast<cudaStream_t>(stream), state, sstride, slots_host, n);
+}
+
+// advance_header_kernel: the header and the n_streams dense records advance by `frames` frames and one call
+KH_API int kh_advance_header(float* state, int64_t sstride, int n_streams, int frames, void* stream) {
+    if (state == nullptr || sstride <= 0 || n_streams <= 0) return (int)cudaErrorInvalidValue;
+    return (int)launch_advance_header(static_cast<cudaStream_t>(stream), state, sstride, n_streams, frames);
+}
+
+// set_clip_base_kernel: header clip_base = header pos
+KH_API int kh_set_clip_base(float* state, void* stream) {
+    if (state == nullptr) return (int)cudaErrorInvalidValue;
+    return (int)launch_set_clip_base(static_cast<cudaStream_t>(stream), state);
+}
+
+// move_lead_kernel over the host pairs from_host[i] -> to_host[i], i < n, each in [0, batch); records ss floats apart
+KH_API int kh_move_lead(float* state, int64_t ss, int batch, const int32_t* from_host, const int32_t* to_host, int n, void* stream) {
+    if (state == nullptr || from_host == nullptr || to_host == nullptr || ss < ST_BLK + BK_STRIDE || ss % 4 != 0 || batch <= 0 ||
+        n <= 0 || !slots_in(from_host, n, batch) || !slots_in(to_host, n, batch))
+        return (int)cudaErrorInvalidValue;
+    return (int)launch_move_lead(static_cast<cudaStream_t>(stream), state, ss, from_host, to_host, n);
+}
+
+// join_start_kernel over J rows (device lists records and leads, any values); lists = 3 J int32: rec, used, owner;
+// used_out (device, J) may be null
+KH_API int kh_join_start(float* state, int64_t ss, int batch, const int32_t* records, const int32_t* leads, int w_max, int J,
+                         int32_t* lists, int32_t* used_out, void* stream) {
+    if (state == nullptr || records == nullptr || leads == nullptr || lists == nullptr || ss <= 0 || ss % 4 != 0 || batch <= 0 ||
+        J <= 0 || w_max < 0)
+        return (int)cudaErrorInvalidValue;
+    return (int)launch_join_start(static_cast<cudaStream_t>(stream), J, state, ss, batch, records, leads, w_max, lists, used_out);
+}
+
+// history_put_kernel over M listeners: X0 [M][T][97][64] into hist [batch][F][97][64]; `lead` maps listener i to its lead
+// record (lead->slots) and its hop count (lead->hops), with lead->frames = T
+KH_API int kh_history_put(const float* X0, const float* state, const KhRecords* lead, float* hist, int F, int M, void* stream) {
+    if (!records_ok(lead) || X0 == nullptr || hist == nullptr || F <= 0 || M <= 0) return (int)cudaErrorInvalidValue;
+    return (int)launch_history_put(false, static_cast<cudaStream_t>(stream), M, X0, state, to_records(*lead), hist, F, lead->frames);
+}
+
+// history_get_kernel over J rows: X0 [J][T][97][64] from hist; `recs` is the join's row map (slots = rec, hops = used,
+// frames = T); leads[j] must lie in [0, batch) for every row that stores
+KH_API int kh_history_get(const float* hist, int F, const float* state, const KhRecords* recs, const int32_t* leads, float* X0, int J,
+                          void* stream) {
+    if (!records_ok(recs) || hist == nullptr || leads == nullptr || X0 == nullptr || F <= 0 || J <= 0) return (int)cudaErrorInvalidValue;
+    return (int)launch_history_get(false, static_cast<cudaStream_t>(stream), J, hist, F, state, to_records(*recs), leads, X0,
+                                   recs->frames);
+}
+
+// ---- enrollment from a capture (embed_kernels.cuh) -------------------------------------------------------------------
+// eslot_rows_kernel over n rows: slots from the host list (each in [0, n_slots), as the engine requires) or the device
+// list (any values), exactly one of them; lens_host any values; capture [n_slots][2][EC_HEAD + capacity]
+KH_API int kh_eslot_rows(const int32_t* slots_host, const int32_t* slots_dev, const int32_t* lens_host, int n, const float* capture,
+                         int n_slots, int capacity, int32_t* slots_out, int32_t* lens, int32_t* used, void* stream) {
+    if ((slots_host == nullptr) == (slots_dev == nullptr) || lens_host == nullptr || capture == nullptr || n <= 0 || n_slots <= 0 ||
+        capacity <= 0 || capacity > INT32_MAX - EC_HEAD || (slots_host != nullptr && !slots_in(slots_host, n, n_slots)))
+        return (int)cudaErrorInvalidValue;
+    return (int)emb::launch_eslot_rows(static_cast<cudaStream_t>(stream), slots_host, slots_dev, lens_host, n, capture,
+                                       EC_HEAD + (int64_t)capacity, n_slots, capacity, slots_out, lens, used);
+}
+
+// eput_rows_kernel: src [B][256] to the dst rows of live rows, row_stride floats apart
+KH_API int kh_eput_rows(const float* src, float* dst, int64_t row_stride, const int32_t* used, int B, void* stream) {
+    if (src == nullptr || dst == nullptr || used == nullptr || row_stride < 256 || B <= 0) return (int)cudaErrorInvalidValue;
+    return (int)emb::launch_eput_rows(static_cast<cudaStream_t>(stream), B, src, dst, row_stride, used);
+}
+
+// estd_kernel / efront_kernel over the capture ring (XRing): utterance b is the last lens[b] samples of slot slots[b]
+// (device lists: slots in [0, n_slots), lens[b] in [MIN_SAMPLES, capacity], as eslot_rows leaves them); used[b] == 0
+// marks a row that is not live
+static emb::XRing to_ring(const float* capture, int capacity, const int32_t* slots, const int32_t* used) {
+    return emb::XRing{capture, EC_HEAD + (int64_t)capacity, capacity, slots, used};
+}
+KH_API int kh_estd_ring(const float* capture, int capacity, const int32_t* slots, const int32_t* used, int N, const int32_t* lens,
+                        float* inv_std, int B, void* stream) {
+    if (capture == nullptr || slots == nullptr || used == nullptr || lens == nullptr || capacity <= 0 || N <= 0 || B <= 0)
+        return (int)cudaErrorInvalidValue;
+    return (int)emb::launch_estd_map(static_cast<cudaStream_t>(stream), B, to_ring(capture, capacity, slots, used), N, lens, inv_std);
+}
+KH_API int kh_efront_ring(const KhEmbWeights* w, const float* capture, int capacity, const int32_t* slots, const int32_t* used, int N,
+                          const int32_t* lens, const float* inv_std, float* X, double* gn_sums, int B, int T, void* stream) {
+    if (capture == nullptr || slots == nullptr || used == nullptr || lens == nullptr || capacity <= 0 || N <= 0 || B <= 0 || T <= 0)
+        return (int)cudaErrorInvalidValue;
+    return (int)emb::launch_efront_map(static_cast<cudaStream_t>(stream), B, to_ring(capture, capacity, slots, used), N, lens, inv_std,
+                                       X, gn_sums, to_emb(*w), T);
 }

@@ -1,7 +1,7 @@
 """The kernel harness library (tests/kernels/) and the float64 references the kernel-level GPU tests
 (test_umma_gemm_gpu.py, test_lstm_kernels_gpu.py, test_attention_kernels_gpu.py, test_front_back_kernels_gpu.py,
 test_embed_kernels_gpu.py, test_rows_gemm_kernels_gpu.py, test_mid_kernels_gpu.py, test_tail_kernel_gpu.py,
-test_targets_kernels_gpu.py) rely on.  The enrollment references (estd64, efront64, egn64, eqkv_ln64, softmax64,
+test_targets_kernels_gpu.py, test_state_kernels_gpu.py, test_embed_slot_kernels_gpu.py) rely on.  The enrollment references (estd64, efront64, egn64, eqkv_ln64, softmax64,
 eattn_out64, ehead64) are pinned to oracle/restate.py; each of their mutants is shown to miss the reference by more than
 10x its bound, and einter_mask_expected's mutants to change it.  No device needed."""
 import ctypes
@@ -772,3 +772,189 @@ def test_gate_fanout_reference_and_mutants():
 def test_row_frames_is_the_kernels_rule():
     assert [kh.row_frames([-1, 0, 1, 3, 4, kh.INT_MAX, -kh.INT_MAX], b, 3) for b in range(7)] == [0, 0, 1, 3, 0, 0, 0]
     assert kh.row_frames(None, 0, 5) == 5
+
+
+# ---- the state-record kernels and the enrollment rows of a capture (test_state_kernels_gpu.py,
+# test_embed_slot_kernels_gpu.py) ---------------------------------------------------------------------------------------
+_LAY = dict(ST_CALLS=257, ST_POS=258, ST_GEN=256, ST_BLK=300, BK_STRIDE=40, ST_CONV=264)
+
+
+def _state(hdr, ss, B, seed):
+    import numpy as np
+    return np.random.default_rng(seed).integers(-2 ** 31, 2 ** 31, hdr + B * ss, dtype=np.int64).astype(np.int32)
+
+
+def test_state_references_are_the_plain_definition():
+    """state_init, reset, advance_header and set_clip_base references against element loops on small synthetic
+    layouts, and each of their mutants changes them"""
+    import numpy as np
+    hdr, ss, B = 16, 300, 3
+    ref = kh.state_init_ref(hdr, ss, B)
+    loop = [0] * hdr + [kh.NAN_BITS if o < kh.SPK else 0 for b in range(B) for o in range(ss)]
+    assert ref.tolist() == loop
+    for m in kh.STATE_INIT_MUTANTS:
+        assert not np.array_equal(kh.state_init_ref(hdr, ss, B, mutant=m), ref), m
+    st = _state(hdr, ss, 5, 1)
+    out = kh.reset_streams_ref(st, hdr, ss, _LAY, [3, 1])
+    for b in range(5):
+        r = out[hdr + b * ss:hdr + (b + 1) * ss].tolist()
+        if b in (3, 1):
+            assert r == [kh.NAN_BITS] * kh.SPK + [0] * (ss - kh.SPK)
+        else:
+            assert r == st[hdr + b * ss:hdr + (b + 1) * ss].tolist()
+    assert not np.array_equal(kh.reset_streams_ref(st, hdr, ss, _LAY, [3, 1], mutant="clock_kept"), out)
+    st = _state(hdr, ss, 5, 2)
+    for i, c in ((0, 2 ** 32 - 3), (hdr + 2 * ss + 258, 2 ** 32 - 1)):
+        kh.put64(st, i, c)
+    st[hdr + 2 * ss + 257] = 2 ** 31 - 1
+    out = kh.advance_header_ref(st, hdr, ss, _LAY, 3, 5)
+    assert kh.get64(out, 0) == 2 ** 32 + 2 and kh.get64(out, 2) == kh.get64(st, 2) + 1 and out[6] == 0
+    assert kh.get64(out, hdr + 2 * ss + 258) == 2 ** 32 + 4 and out[hdr + 2 * ss + 257] == -2 ** 31
+    assert np.array_equal(out[hdr + 3 * ss:], st[hdr + 3 * ss:])
+    for m in kh.ADVANCE_MUTANTS:
+        assert not np.array_equal(kh.advance_header_ref(st, hdr, ss, _LAY, 3, 5, mutant=m), out), m
+    cb = kh.set_clip_base_ref(st)
+    assert kh.get64(cb, kh.HDR_CLIP) == kh.get64(st, kh.HDR_POS) and np.array_equal(cb[6:], st[6:])
+
+
+def test_reset_first_chunk_mutant_needs_a_second_chunk():
+    import numpy as np
+    lim = kh.state_limits()["RESET_MAX_SLOTS"]
+    hdr, ss = 16, 264
+    st = _state(hdr, ss, lim + 1, 3)
+    slots = list(range(lim + 1))[::-1]
+    ref = kh.reset_streams_ref(st, hdr, ss, _LAY, slots)
+    assert np.array_equal(kh.reset_streams_ref(st, hdr, ss, _LAY, slots[:lim], mutant="first_chunk_only"),
+                          kh.reset_streams_ref(st, hdr, ss, _LAY, slots[:lim]))
+    assert not np.array_equal(kh.reset_streams_ref(st, hdr, ss, _LAY, slots, mutant="first_chunk_only"), ref)
+
+
+def test_join_start_reference_and_mutants():
+    """join_start_ref against the rule written out per row, on every case of the GPU test; each mutant differs on the
+    cases that name it, and every mutant is named"""
+    named = set()
+    for w_max in (0, 1, 50):
+        c = kh.join_start_case(w_max)
+        recs, leads, batch = c["records"], c["leads"], c["batch"]
+        ref = kh.join_start_ref(recs, leads, c["clocks"], batch, w_max)
+        for j, (s, l) in enumerate(zip(recs, leads)):
+            live = recs.count(s) == 1 and s not in leads and 0 <= s < batch and 0 <= l < batch
+            W = min(w_max, c["clocks"][l]) if live else 0
+            assert (ref["rec"][j], ref["used"][j], ref["owner"][j]) == ((s, W, j) if live else (-1, 0, -1)), (w_max, j)
+            if live:
+                assert ref["start"][s] == c["clocks"][l] - W
+        assert sum(r >= 0 for r in ref["rec"]) == 12
+        for m in c["catches"]:
+            assert kh.join_start_ref(recs, leads, c["clocks"], batch, w_max, mutant=m) != ref, (w_max, m)
+        named |= c["catches"]
+    assert named == set(kh.JOIN_MUTANTS)
+
+
+def test_history_references_and_mutants():
+    """history_put_ref writes listener i's frame t to slot (clock + t) mod F for its last min(h, F) frames;
+    history_get_ref reads them back by the row's own clock.  A put of one frame per tick then a get equals the frames in
+    order, and every mutant differs on the cases that name it."""
+    import numpy as np
+    named_put, named_get = set(), set()
+    for F in kh.HIST_F:
+        c = kh.history_put_case(F)
+        T, batch = c["T"], c["batch"]
+        X0 = np.arange(len(c["leads"]) * T, dtype=np.int32).reshape(len(c["leads"]), T, 1) + 1
+        hist = np.zeros((batch, F, 1), dtype=np.int32)
+        ref = kh.history_put_ref(hist, X0, c["leads"], c["hops"], c["clocks"], F, T, batch)
+        for i, l in enumerate(c["leads"]):
+            h = kh.row_frames(c["hops"], i, T)
+            if 0 <= l < batch and h > 0:
+                for t in range(max(0, h - F), h):
+                    assert ref[l, (c["clocks"][l] + t) % F, 0] == X0[i, t, 0]
+        for m in c["catches"]:
+            assert not np.array_equal(kh.history_put_ref(hist, X0, c["leads"], c["hops"], c["clocks"], F, T, batch, m), ref), (F, m)
+        named_put |= c["catches"]
+        g = kh.history_get_case(F)
+        H = np.arange(g["batch"] * F, dtype=np.int32).reshape(g["batch"], F, 1) + 1
+        got = kh.history_get_ref(H, g["rec"], g["used"], g["leads"], g["clocks"], F, g["T"], g["batch"])
+        for j, s in enumerate(g["rec"]):
+            h = kh.row_frames(g["used"], j, g["T"])
+            for t in range(g["T"]):
+                live = 0 <= s < g["batch"] and t < h
+                assert got[j, t, 0] == (H[g["leads"][j], (g["clocks"][s] + t) % F, 0] if live else 0), (F, j, t)
+        for m in g["catches"]:
+            assert not np.array_equal(kh.history_get_ref(H, g["rec"], g["used"], g["leads"], g["clocks"], F, g["T"], g["batch"],
+                                                         m), got), (F, m)
+        named_get |= g["catches"]
+    assert named_put == set(kh.HIST_PUT_MUTANTS) and named_get == set(kh.HIST_GET_MUTANTS)
+    # round trip: ticks of one frame starting at 2^32 - 4 put into a ring of 7, then read back from clock p - W
+    F, p0, n = 7, 2 ** 32 - 4, 10
+    hist = np.zeros((1, F, 1), dtype=np.int32)
+    for k in range(n):
+        hist = kh.history_put_ref(hist, np.full((1, 1, 1), 100 + k, dtype=np.int32), [0], None, [p0 + k], F, 1, 1)
+    W = 5
+    back = kh.history_get_ref(hist, [0], [W], [0], [p0 + n - W], F, W, 1)
+    assert back[0, :, 0].tolist() == [100 + k for k in range(n - W, n)]
+
+
+def test_move_lead_reference_and_mutants():
+    import numpy as np
+    lay = dict(_LAY, ST_BLK=320, BK_STRIDE=20, ST_CONV=264)
+    hdr, ss, nb = 16, 320 + 3 * 20, 3
+    st = _state(hdr, ss, 4, 4)
+    for b, calls in enumerate((2, 5, 7, 4)):
+        st[hdr + b * ss + lay["ST_CALLS"]] = calls
+    for src, dst in ((0, 1), (1, 3), (2, 0), (1, 2)):
+        ref = kh.move_lead_ref(st, hdr, ss, lay, nb, [src], [dst], conv_parity=8)
+        exp = st.copy()
+        a, b = hdr + src * ss, hdr + dst * ss
+        exp[b + 320:b + 340] = st[a + 320:a + 340]
+        pa, pb = st[a + lay["ST_CALLS"]] & 1, st[b + lay["ST_CALLS"]] & 1
+        exp[b + 264 + 8 * pb:b + 272 + 8 * pb] = st[a + 264 + 8 * pa:a + 272 + 8 * pa]
+        assert np.array_equal(ref, exp), (src, dst)
+        assert not np.array_equal(kh.move_lead_ref(st, hdr, ss, lay, nb, [src], [dst], mutant="all_blocks", conv_parity=8), ref)
+        assert np.array_equal(kh.move_lead_ref(st, hdr, ss, lay, nb, [src], [dst], mutant="src_parity", conv_parity=8), ref) == (pa == pb)
+
+
+def test_eslot_rows_reference_and_mutants():
+    lim = kh.state_limits()
+    named = set()
+    for n in (1, lim["SLOT_ROWS_PER_LAUNCH"], lim["SLOT_ROWS_PER_LAUNCH"] + 1):
+        for device in (False, True):
+            c = kh.eslot_rows_case(n, device, lim["SLOT_ROWS_PER_LAUNCH"])
+            args = (c["slots"], c["lens"], c["captured"], c["n_slots"], c["capacity"], lim["MIN_SAMPLES"])
+            ref = kh.eslot_rows_ref(*args)
+            for i, (s, ln) in enumerate(zip(c["slots"], c["lens"])):
+                cap = min(max(c["captured"][s], 0), c["capacity"]) if 0 <= s < c["n_slots"] else 0
+                u = min(ln, cap)
+                use = u if u >= lim["MIN_SAMPLES"] else 0
+                assert (ref["slots"][i], ref["lens"][i], ref["used"][i]) == \
+                    (s if 0 <= s < c["n_slots"] else 0, use or lim["MIN_SAMPLES"], use)
+            assert device or all(0 <= s < c["n_slots"] for s in c["slots"])
+            for m in c["catches"]:
+                assert kh.eslot_rows_ref(*args, mutant=m) != ref, (n, device, m)
+            named |= c["catches"]
+    assert named == set(kh.SLOT_ROWS_MUTANTS)
+    import numpy as np
+    dst = np.zeros(3 * 300, dtype=np.int32)
+    src = np.arange(3 * 256, dtype=np.int32).reshape(3, 256) + 1
+    out = kh.eput_rows_ref(dst, src, [5, 0, 192], 300)
+    assert out[:256].tolist() == src[0].tolist() and not out[300:900 - 44 - 256].any() and out[600:856].tolist() == src[2].tolist()
+    assert not np.array_equal(kh.eput_rows_ref(dst, src, [5, 0, 192], 300, mutant="dead_written"), out)
+
+
+def test_ring_utterance_is_the_last_samples_written():
+    """Write samples 1, 2, ... into a ring one at a time, as the capture does: the utterance of the last n samples is
+    n consecutive values ending at the last one written, whatever the write position; the unwrapped mutant differs exactly
+    when the utterance wraps"""
+    import numpy as np
+    for cap in (192, 1000):
+        for total in (cap - 1, cap, cap + 37, 3 * cap + 5):
+            rings = np.zeros((2, cap), dtype=np.int64)
+            for k in range(1, total + 1):
+                rings[0, (k - 1) % cap], rings[1, (k - 1) % cap] = k, -k
+            wpos = total % cap
+            for n in (192, cap // 2 + 1, min(cap, total)):
+                if n > min(cap, total):
+                    continue
+                u = kh.ring_utterance(rings, wpos, n, cap)
+                assert u[0].tolist() == list(range(total - n + 1, total + 1)) and u[1].tolist() == [-v for v in u[0]]
+                assert np.array_equal(kh.ring_utterance(rings, wpos, n, cap, mutant="no_wrap"), u) == (wpos >= n)
+    for c in kh.ring_cases(192):
+        assert any(w < n for w, n, live in c["rows"] if live), c["name"]
