@@ -46,6 +46,9 @@
  *   l2h_jitter_buffer
  *        <- putting a device's packets back in sequence order and concealing lost ones, over a lossy network
  *           (JitterBuffer)
+ *   l2h_jitter_buffer_timed
+ *        <- the same, releasing missing packets on the server's clock, so an uplink gap is concealed as it happens
+ *           (JitterBuffer(deadline=...))
  *
  * Conventions follow the reference's only FFI (src/datasets/motion_simulator.py:30-95): every
  * function returns int (0 = OK, non-zero = error, text via l2h_last_error()), handles are opaque
@@ -1071,6 +1074,48 @@ int l2h_jitter_buffer(const float* x_dev, int64_t x_row_stride, int64_t x_ch_str
                       int32_t* out_counts_dev, int32_t n, int32_t channels, const int32_t* slots_dev, float* state_dev,
                       int32_t n_slots, int32_t rate, int32_t packet, int32_t depth, int32_t window, int32_t max_out,
                       void* stream);
+
+/* The jitter buffer released on time: l2h_jitter_buffer with wall-clock deadlines, so a gap in a device's uplink is
+ * concealed as it happens instead of when the uplink recovers, and a long outage ends in a restart with no added
+ * latency.  A missing packet is declared lost by the arrival rule above or by its deadline on the server's clock,
+ * whichever comes first.
+ *
+ * Clock.  now = *now_dev, read when the kernel runs, is the server's clock at the call in microseconds, an int32 that
+ * wraps; clocks are compared in serial arithmetic (mod 2^32, only differences under 2^31 us matter).  Every packet pushed
+ * in a call is taken to have arrived at that call's now.
+ * Anchor.  A slot keeps the highest-numbered packet ever placed in its window, the anchor (a_s, a_t): its sequence
+ * number and the now of the call it arrived in.  The first packet of a fresh slot sets it, and so does a restart; late and duplicate
+ * packets never move it.
+ * Deadline.  Packet s is expected at a_t + (s - a_s) period, with period = round(1e6 P / rate) us and s - a_s taken in
+ * [-2^15, 2^15) (products mod 2^32).  Packet next expires once now - expected(next) >= deadline_us.
+ * A row's work: first its arrivals run exactly as in l2h_jitter_buffer (except for a stalled slot, below).  Then the
+ * release rule runs once more at now, with a third way to release next: next has expired and the slot has not stalled.
+ * That release is a loss, counted in `lost` and in `expired`, and concealed as any loss is; held packets that follow it
+ * are released too.  So a deadline <= e period declares a gap lost as soon as a packet e past it arrives, as depth does.
+ * Stall.  Deadline releases stop once the concealment has gone silent: once next - a_s - 1 >= S, S = ceil(B / P)
+ * packets (60 ms; 6 at 44.1 kHz / 441 and at 16 kHz / 160).  From then on the slot releases nothing, and its next arrival
+ * with s - next >= 0 restarts the slot at s through the restart rule (counted in `restarts`, faded in), so no silent
+ * backlog is released and a long outage adds no latency.  A packet behind next is still late.
+ * With a deadline that no call reaches the output, the out counts and head words 0-12 equal l2h_jitter_buffer's, bit for
+ * bit.  Over one sequence of (arrivals, now) calls another max_out changes only where the output is cut; splitting one
+ * call's arrivals into two calls at the same now can change decisions (the deadline rule runs after each call).
+ * A slot's deadlines are checked only in calls that list it: a service that runs deadlines lists every live slot in
+ * every tick, with count 0 when the slot sent nothing.
+ *
+ * State: the layout of l2h_jitter_buffer_layout, with channel 0's head words 13 a_s, 14 a_t and 15 expired (saturating
+ * at 2^31 - 1), which l2h_jitter_buffer leaves as they are.  One slot's state is meant for one of the two entries.
+ *
+ * l2h_jitter_buffer_timed: the arguments of l2h_jitter_buffer, plus
+ *   now_dev         [1] int32 of DEVICE memory read when the kernel runs: the clock, so a call captured in a CUDA graph
+ *                   serves any clock rewritten in place
+ *   deadline_us     >= 0, in microseconds
+ * Errors: those of l2h_jitter_buffer, and 1 = now_dev null, deadline_us < 0.  Asynchronous on `stream`. */
+int l2h_jitter_buffer_timed(const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, int32_t max_in,
+                            const int32_t* seqs_dev, const int32_t* counts_dev, float* y_dev, int64_t y_row_stride,
+                            int64_t y_ch_stride, int32_t* out_counts_dev, int32_t n, int32_t channels,
+                            const int32_t* slots_dev, float* state_dev, int32_t n_slots, int32_t rate, int32_t packet,
+                            int32_t depth, int32_t window, int32_t max_out, const int32_t* now_dev, int32_t deadline_us,
+                            void* stream);
 
 #ifdef __cplusplus
 }

@@ -204,6 +204,12 @@ _SIGS = {
                                         ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
                                         ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
                                         ctypes.c_void_p]),
+    "l2h_jitter_buffer_timed": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int32,
+                                              ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64,
+                                              ctypes.c_int64, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
+                                              ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
+                                              ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
+                                              ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p]),
     "l2h_embed_create": (ctypes.c_int, [ctypes.POINTER(EmbedConfig), c_void_pp]),
     "l2h_embed_destroy": (ctypes.c_int, [ctypes.c_void_p]),
     "l2h_embed_set_option": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_int32]),

@@ -27,7 +27,8 @@
 // output under a ceiling with one gain for all channels (limiter_kernel), the leveler that brings each voice to one
 // loudness with one gain for all channels (leveler_kernel), and the multiband compressor that fits each listener's output
 // to their hearing, per band and per ear, with its compression linked across the channels (band_compressor_kernel), and
-// the jitter buffer that puts a device's packets back in sequence order and conceals lost ones (jitter_buffer_kernel).
+// the jitter buffer that puts a device's packets back in sequence order and conceals lost ones (jitter_buffer_kernel, and
+// jitter_buffer_kernel_t<true>, which also releases missing packets on deadlines from the server's clock).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -1772,9 +1773,10 @@ constexpr int JB_RECOVER = 1 << 17;
 constexpr int JB_SEQ = 1 << 16;
 constexpr int JB_MAX_WINDOW = 4096;
 // head words (int32 in the floats' bits): started, next, head, pend, run (concealed samples into the run, capped at its
-// silent point), tau (0: no run), then the counters lost, late, duplicate, dropped, restarts, and held and pitch
+// silent point), tau (0: no run), then the counters lost, late, duplicate, dropped, restarts, and held and pitch; the
+// timed form adds the anchor (the highest packet placed and the clock of its call) and the counter expired
 enum { JB_STARTED, JB_NEXT, JB_POS, JB_PEND, JB_RUN, JB_TAU, JB_C_LOST, JB_C_LATE, JB_C_DUP, JB_C_DROPPED, JB_C_RESTARTS,
-       JB_HELD, JB_PITCH };
+       JB_HELD, JB_PITCH, JB_ANCHOR_SEQ, JB_ANCHOR_T, JB_C_EXPIRED };
 
 struct JbParams {
     int32_t P, W, R, D, M, max_out;   // packet, window, ring (2 W), depth, arrivals per row, packets written per row
@@ -1782,6 +1784,21 @@ struct JbParams {
     int32_t lr, ga, gb;               // crossfade samples; a run's gain is 1 before sample ga, 0 from sample gb
     int64_t rf;                       // floats per channel row
 };
+
+// the timed form's clock: the server's clock (µs, int32 that wraps) read when the kernel runs, the deadline (µs), the
+// packet period (µs, mod 2^32) and the stall S (packets past the anchor after which deadline releases stop)
+struct JbClock {
+    const int32_t* now;
+    int32_t deadline;
+    uint32_t period;
+    int32_t stall;
+};
+
+// a difference of 16-bit sequence numbers in serial arithmetic: v mod 2^16 taken in [-2^15, 2^15)
+L2H_DEVINL int jb_ser(int v) {
+    v &= JB_SEQ - 1;
+    return v >= JB_SEQ / 2 ? v - JB_SEQ : v;
+}
 
 // a sample as it enters: 0 when it is not finite or its magnitude is 2^32 or more
 L2H_DEVINL float jb_clean(float v) { return fabsf(v) < HG_BIG ? v : 0.f; }
@@ -1833,12 +1850,15 @@ L2H_DEVINL int jb_pitch(const float* win, int64_t WL, int base, int C, float* su
 }
 
 // One CTA = one call row over all C channels (one decision per slot).  Row i pushes packets j < counts[i] of x row i
-// with sequence numbers seqs[i][j] and writes y[i][c][0 .. out_counts[i] P).
+// with sequence numbers seqs[i][j] and writes y[i][c][0 .. out_counts[i] P).  Timed: the arrivals also keep the anchor,
+// an arrival at or past next restarts a stalled slot, and after them a missing next is also released as a loss once its
+// deadline on the clock has passed (`ck`; unused untimed).
+template <bool Timed>
 __global__ void __launch_bounds__(RS_TILE)
-jitter_buffer_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, const int32_t* __restrict__ seqs,
-                     const int32_t* __restrict__ counts, float* __restrict__ y, int64_t y_row, int64_t y_ch,
-                     int32_t* __restrict__ out_counts, int C, const int32_t* __restrict__ slots, float* __restrict__ state,
-                     int n_slots, const __grid_constant__ JbParams p) {
+jitter_buffer_kernel_t(const float* __restrict__ x, int64_t x_row, int64_t x_ch, const int32_t* __restrict__ seqs,
+                       const int32_t* __restrict__ counts, float* __restrict__ y, int64_t y_row, int64_t y_ch,
+                       int32_t* __restrict__ out_counts, int C, const int32_t* __restrict__ slots, float* __restrict__ state,
+                       int n_slots, const __grid_constant__ JbParams p, const JbClock ck) {
     extern __shared__ float sm[];
     __shared__ float sc[RS_TILE];
     __shared__ int lt[RS_TILE];
@@ -1873,26 +1893,37 @@ jitter_buffer_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, c
         const auto held = [&](int d) { return tg[slot(d)] == ((next + d) & (JB_SEQ - 1)) + 1; };
         int far = -1;                                                   // the farthest stored packet in the window
         for (int d = 0; d < W; ++d) if (held(d)) far = d;
+        // timed: the anchor (a_s, a_t), the clock of this call and the deadline releases
+        int a_s = 0, expired = 0;
+        uint32_t a_t = 0, now = 0;
+        if constexpr (Timed) {
+            a_s = int_word(st[JB_ANCHOR_SEQ], JB_SEQ - 1), a_t = (uint32_t)__float_as_int(st[JB_ANCHOR_T]);
+            now = (uint32_t)*ck.now;
+        }
+        // the concealment has gone silent: no deadline releases, and the next arrival at or past next restarts
+        const auto stalled = [&] { return Timed && jb_ser(next - a_s - 1) >= ck.stall; };
         const int32_t* sq = seqs + (int64_t)sr.row * p.M;
         for (int j = 0; j < cnt; ++j) {
             cp[j] = -1;
             const int s = sq[j];
             if (s < 0 || s >= JB_SEQ) continue;                         // no sequence number: skipped
-            if (!started) started = 1, next = s;
+            if (!started) started = 1, next = s, a_s = s;
             int d = (s - next) & (JB_SEQ - 1);
             if (d >= JB_SEQ / 2) d -= JB_SEQ;
             bool recover = false;
             if (d < 0) { late = min(late + 1, INT32_MAX - 1); continue; }
-            if (d < W) {
+            if (d < W && !stalled()) {
                 if (held(d)) { dup = min(dup + 1, INT32_MAX - 1); continue; }
-            } else {                                                    // beyond the window: a restart
+            } else {                                                    // beyond the window (or stalled): a restart
                 for (int e = 0; e < W; ++e) {
                     if (held(e)) dropped = min(dropped + 1, INT32_MAX - 1);
                     tg[slot(e)] = 0;
                 }
                 restarts = min(restarts + 1, INT32_MAX - 1);
-                next = s, d = 0, far = -1, recover = true;
+                next = s, d = 0, far = -1, recover = true, a_s = s;
             }
+            if constexpr (Timed)                                        // the first packet, a restart, or a new highest
+                if (jb_ser(s - a_s) >= 0) a_s = s, a_t = now;
             const int at = slot(d);
             tg[at] = s + 1;
             for (int k = 0; k < j; ++k) if (cp[k] == at) cp[k] = -1;    // a slot freed and reused in this call
@@ -1904,6 +1935,25 @@ jitter_buffer_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, c
                 else if (far >= p.D + 1) t = JB_LOST, lost = min(lost + 1, INT32_MAX - 1);
                 else break;
                 if (pend == W) {                                        // the backlog is full: its oldest goes
+                    tg[pos] = 0;
+                    pos = (pos + 1) % R, --pend;
+                    dropped = min(dropped + 1, INT32_MAX - 1);
+                }
+                tg[(pos + pend) % R] = t;
+                ++pend, next = (next + 1) & (JB_SEQ - 1), --far;
+            }
+        }
+        if constexpr (Timed) {
+            // the release rule once more at now, with a third way to release next: it expired (packet s is expected at
+            // a_t + (s - a_s) period) and the slot has not stalled
+            while (started) {
+                int t;
+                if (held(0)) t = next + 1;
+                else if (far >= p.D + 1) t = JB_LOST, lost = min(lost + 1, INT32_MAX - 1);
+                else if (!stalled() && (int)(now - (a_t + (uint32_t)jb_ser(next - a_s) * ck.period)) >= ck.deadline)
+                    t = JB_LOST, lost = min(lost + 1, INT32_MAX - 1), expired = min(expired + 1, INT32_MAX - 1);
+                else break;
+                if (pend == W) {
                     tg[pos] = 0;
                     pos = (pos + 1) % R, --pend;
                     dropped = min(dropped + 1, INT32_MAX - 1);
@@ -1932,6 +1982,11 @@ jitter_buffer_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, c
         st[JB_C_DROPPED] = add_word(st[JB_C_DROPPED], dropped);
         st[JB_C_RESTARTS] = add_word(st[JB_C_RESTARTS], restarts);
         st[JB_HELD] = __int_as_float(nheld);
+        if constexpr (Timed) {
+            st[JB_ANCHOR_SEQ] = __int_as_float(a_s);
+            st[JB_ANCHOR_T] = __int_as_float((int)a_t);
+            st[JB_C_EXPIRED] = add_word(st[JB_C_EXPIRED], expired);
+        }
         out_counts[sr.row] = n_out;
         n_out_s = n_out;
     }
@@ -2039,13 +2094,15 @@ extern "C" int l2h_jitter_buffer_layout(int32_t channels, int32_t rate, int32_t 
     return 0;
 }
 
-extern "C" int l2h_jitter_buffer(const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, int32_t max_in,
-                                 const int32_t* seqs_dev, const int32_t* counts_dev, float* y_dev, int64_t y_row_stride,
-                                 int64_t y_ch_stride, int32_t* out_counts_dev, int32_t n, int32_t channels,
-                                 const int32_t* slots_dev, float* state_dev, int32_t n_slots, int32_t rate, int32_t packet,
-                                 int32_t depth, int32_t window, int32_t max_out, void* stream) {
-    using namespace l2h;
-    const std::string who = "l2h_jitter_buffer";
+namespace l2h {
+constexpr auto jitter_buffer_kernel = jitter_buffer_kernel_t<false>;
+
+// both entries: the checks of l2h_jitter_buffer, then one launch of the untimed kernel (now_dev null) or the timed one
+static int jb_call(const std::string& who, const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, int32_t max_in,
+                   const int32_t* seqs_dev, const int32_t* counts_dev, float* y_dev, int64_t y_row_stride,
+                   int64_t y_ch_stride, int32_t* out_counts_dev, int32_t n, int32_t channels, const int32_t* slots_dev,
+                   float* state_dev, int32_t n_slots, int32_t rate, int32_t packet, int32_t depth, int32_t window,
+                   int32_t max_out, const int32_t* now_dev, int32_t deadline_us, void* stream) {
     if (int rc = slot_call(who, {x_dev, seqs_dev, counts_dev, y_dev, out_counts_dev, slots_dev, state_dev},
                            "n, channels, max_in and n_slots", {n, channels, max_in, n_slots}, n, channels, n_slots))
         return rc;
@@ -2057,10 +2114,43 @@ extern "C" int l2h_jitter_buffer(const float* x_dev, int64_t x_row_stride, int64
     if (x.len > INT32_MAX) return fail(1, who + ": max_in * packet is too large");
     if (int rc = disjoint(who, channels, {x, y})) return rc;
     if (overlap(y_dev, n, y, x_dev, n, x, channels, false)) return fail(1, who + ": y must not overlap x");
+    JbClock ck{now_dev, deadline_us, 0, 0};
+    if (now_dev) {
+        // period = round(1e6 packet / rate) µs, exactly, taken mod 2^32 as the clock is; S = ceil(gb / packet)
+        ck.period = (uint32_t)((2000000 * (int64_t)packet + rate) / (2 * (int64_t)rate));
+        ck.stall = (p.gb + packet - 1) / packet;
+    }
+    const auto kernel = now_dev ? jitter_buffer_kernel_t<true> : jitter_buffer_kernel;
     if (smem > RS_SMEM_BYTES - 4096)                                    // then the static words need the opt-in
-        if (cudaError_t e = full_staging(jitter_buffer_kernel)) return fail(3, who + ": " + cudaGetErrorString(e));
-    jitter_buffer_kernel<<<(unsigned)n, RS_TILE, smem, static_cast<cudaStream_t>(stream)>>>(
+        if (cudaError_t e = full_staging(kernel)) return fail(3, who + ": " + cudaGetErrorString(e));
+    kernel<<<(unsigned)n, RS_TILE, smem, static_cast<cudaStream_t>(stream)>>>(
         x_dev, x_row_stride, x_ch_stride, seqs_dev, counts_dev, y_dev, y_row_stride, y_ch_stride, out_counts_dev, channels,
-        slots_dev, state_dev, n_slots, p);
+        slots_dev, state_dev, n_slots, p, ck);
     return launched(who);
+}
+}  // namespace l2h
+
+extern "C" int l2h_jitter_buffer(const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, int32_t max_in,
+                                 const int32_t* seqs_dev, const int32_t* counts_dev, float* y_dev, int64_t y_row_stride,
+                                 int64_t y_ch_stride, int32_t* out_counts_dev, int32_t n, int32_t channels,
+                                 const int32_t* slots_dev, float* state_dev, int32_t n_slots, int32_t rate, int32_t packet,
+                                 int32_t depth, int32_t window, int32_t max_out, void* stream) {
+    return l2h::jb_call("l2h_jitter_buffer", x_dev, x_row_stride, x_ch_stride, max_in, seqs_dev, counts_dev, y_dev,
+                        y_row_stride, y_ch_stride, out_counts_dev, n, channels, slots_dev, state_dev, n_slots, rate, packet,
+                        depth, window, max_out, nullptr, 0, stream);
+}
+
+extern "C" int l2h_jitter_buffer_timed(const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, int32_t max_in,
+                                       const int32_t* seqs_dev, const int32_t* counts_dev, float* y_dev,
+                                       int64_t y_row_stride, int64_t y_ch_stride, int32_t* out_counts_dev, int32_t n,
+                                       int32_t channels, const int32_t* slots_dev, float* state_dev, int32_t n_slots,
+                                       int32_t rate, int32_t packet, int32_t depth, int32_t window, int32_t max_out,
+                                       const int32_t* now_dev, int32_t deadline_us, void* stream) {
+    using namespace l2h;
+    const std::string who = "l2h_jitter_buffer_timed";
+    if (!now_dev) return fail(1, who + ": null pointers");
+    if (deadline_us < 0) return fail(1, who + ": deadline_us " + std::to_string(deadline_us) + " is negative");
+    return jb_call(who, x_dev, x_row_stride, x_ch_stride, max_in, seqs_dev, counts_dev, y_dev, y_row_stride, y_ch_stride,
+                   out_counts_dev, n, channels, slots_dev, state_dev, n_slots, rate, packet, depth, window, max_out,
+                   now_dev, deadline_us, stream);
 }

@@ -864,27 +864,42 @@ class JitterBuffer(_SlotStage):
     first real packet after a run or a restart fades in from the continuing concealment along a raised cosine over
     min(4 ms, packet).  A non-finite sample, or one of magnitude 2**32 or more, enters as 0.
 
+    With `deadline` (microseconds; l2h_jitter_buffer_timed) the buffer also releases on time: every call takes `now`,
+    the server's clock in microseconds, and a missing packet is declared lost either by the rule above or once its
+    deadline has passed, whichever comes first.  A slot anchors its clock on the highest packet it has placed: packet s
+    is expected at the anchor's arrival time plus (s - anchor) packet periods, and the packet at next expires once now
+    lies `deadline` past that.  After its arrivals, each call releases every expired packet as a loss (counted in `lost`
+    and `expired`), so a gap in a device's uplink is concealed as it happens.  Once the concealment has gone silent (60 ms
+    of packets past the anchor) the slot releases nothing more, and its next arrival at or past next restarts it, so a
+    long outage adds no latency.  A slot's deadlines are checked only in calls that list it: list every live slot in
+    every tick, with count 0 when it sent nothing.  With a deadline no call reaches, the output is the untimed buffer's.
+
     `state` [slots, channels, row] is a float32 tensor on `device`: all zeros is a fresh slot, so a listener is reset by
     zeroing its rows (`reset`) and moved by copying them.  The counters are int32 views that never synchronise."""
 
     SEQ = 1 << 16
     LOST, LATE, DUPLICATE, DROPPED, RESTARTS, HELD, PITCH = 6, 7, 8, 9, 10, 11, 12   # head words of channel 0
+    EXPIRED = 15
 
-    def __init__(self, slots, channels, rate, packet, depth=1, window=16, max_out=4, device=None):
+    def __init__(self, slots, channels, rate, packet, depth=1, window=16, max_out=4, device=None, deadline=None):
         super().__init__(slots, channels)
         self.rate, self.packet = _whole(rate, "rate"), _whole(packet, "packet")
         self.depth, self.window = _whole(depth, "depth", 0), _whole(window, "window")
         self.max_out = _whole(max_out, "max_out")
+        self.deadline = None if deadline is None else _whole(deadline, "deadline", 0)
         if self.depth >= self.window:
             raise ValueError(f"depth must be below window = {self.window} packets, got {depth!r}")
         self._allocate(*_layout(_cabi.lib().l2h_jitter_buffer_layout, self.channels, self.rate, self.packet, self.depth,
                                 self.window, self.max_out), device)
 
-    def __call__(self, x, seqs, counts, slots, out=None, out_counts=None):
+    def __call__(self, x, seqs, counts, slots, out=None, out_counts=None, now=None):
         """x [n, channels, M * packet] CUDA tensor: row i pushes its packets j < counts[i], x[i, :, j P:(j + 1) P], with
         sequence numbers seqs[i, j], into slot slots[i].  Returns (y [n, channels, max_out * packet] float32, out_counts [n]
         int32 CUDA) (`out` and `out_counts`, if given, written in place): row i receives y[i, :, :out_counts[i] * packet],
         its slot's next packets in sequence order; its later samples are left unwritten.
+
+        `now` is required exactly when the buffer has a deadline: the server's clock in microseconds, a host int (taken
+        mod 2**32) or a CUDA int32 tensor of shape (1,) used in place and read when the kernel runs.
 
         Host lists are checked and uploaded (`slots` n distinct ints in [0, slots), `counts` n ints in [0, M], `seqs` [n, M]
         int32 values whose first counts[i] entries of row i lie in [0, 65535], so a short row may be padded with -1; with
@@ -893,6 +908,7 @@ class JitterBuffer(_SlotStage):
         number outside [0, 65535] marks a packet that is skipped.  So a call captured in the tick's CUDA graph serves any
         lists rewritten in place."""
         x = self._rows_in(x, self.packet)
+        now = self._now(now)
         dev = self.state.device
         n, C, L = x.shape
         M = L // self.packet
@@ -902,10 +918,32 @@ class JitterBuffer(_SlotStage):
         seqs = self._seqs(seqs, n, M, host_counts)
         out = self._rows_out(out, (n, C, self.max_out * self.packet))
         out_counts = self._ints_out(out_counts, n, "out_counts")
-        self._run("l2h_jitter_buffer", x, x.stride(0), x.stride(1), M, seqs, counts, out, out.stride(0), out.stride(1),
-                  out_counts, n, C, slots, self.state, self.n_slots, self.rate, self.packet, self.depth, self.window,
-                  self.max_out)
+        args = (x, x.stride(0), x.stride(1), M, seqs, counts, out, out.stride(0), out.stride(1), out_counts, n, C, slots,
+                self.state, self.n_slots, self.rate, self.packet, self.depth, self.window, self.max_out)
+        if now is None:
+            self._run("l2h_jitter_buffer", *args)
+        else:
+            self._run("l2h_jitter_buffer_timed", *args, now, self.deadline)
         return out, out_counts
+
+    def _now(self, now):
+        """the clock of a call as a CUDA int32 tensor of shape (1,) on the state's device (None without a deadline), or
+        ValueError"""
+        if self.deadline is None:
+            if now is not None:
+                raise ValueError("now is given to a JitterBuffer without a deadline")
+            return None
+        dev = self.state.device
+        if isinstance(now, torch.Tensor) and now.is_cuda:
+            if now.dtype != torch.int32 or tuple(now.shape) != (1,) or now.device != dev:
+                raise ValueError(f"a CUDA now tensor must be an int32 tensor of shape (1,) on {dev}")
+            return now
+        if now is None:
+            raise ValueError("a JitterBuffer with a deadline needs now, the server's clock in microseconds")
+        if isinstance(now, bool) or not isinstance(now, numbers.Integral):
+            raise ValueError(f"now must be an int of microseconds or a CUDA int32 tensor of shape (1,), got {now!r}")
+        v = int(now) % 2 ** 32
+        return torch.tensor([v - 2 ** 32 if v >= 2 ** 31 else v], dtype=torch.int32).to(dev)
 
     def _seqs(self, seqs, n, M, counts=None):
         """the [n, M] int32 sequence numbers on the state's device: a CUDA tensor used in place, else checked (the
@@ -970,3 +1008,9 @@ class JitterBuffer(_SlotStage):
     def pitch(self):
         """[slots] int32 CUDA view: the lag, in samples, of the last concealment run (0 before the first)"""
         return self._word(self.PITCH)
+
+    @property
+    def expired(self):
+        """[slots] int32 CUDA view: packets declared lost because their deadline passed, a part of `lost` (saturating;
+        0 without a deadline)"""
+        return self._word(self.EXPIRED)
