@@ -49,6 +49,9 @@
  *   l2h_jitter_buffer_timed
  *        <- the same, releasing missing packets on the server's clock, so an uplink gap is concealed as it happens
  *           (JitterBuffer(deadline=...))
+ *   l2h_jitter_buffer_adaptive
+ *        <- the same, with each listener's deadline drawn from the measured lateness of their own packets
+ *           (JitterBuffer(deadline=(lo, hi)))
  *
  * Conventions follow the reference's only FFI (src/datasets/motion_simulator.py:30-95): every
  * function returns int (0 = OK, non-zero = error, text via l2h_last_error()), handles are opaque
@@ -1116,6 +1119,60 @@ int l2h_jitter_buffer_timed(const float* x_dev, int64_t x_row_stride, int64_t x_
                             const int32_t* slots_dev, float* state_dev, int32_t n_slots, int32_t rate, int32_t packet,
                             int32_t depth, int32_t window, int32_t max_out, const int32_t* now_dev, int32_t deadline_us,
                             void* stream);
+
+/* The jitter buffer with adaptive deadlines: l2h_jitter_buffer_timed whose deadline each slot draws from the measured
+ * lateness of its own packets, between lo_us and hi_us, so a listener on a clean link waits little for a loss and one
+ * on a jittery link loses few packets to `late`.
+ *
+ * Arrivals.  arrivals_dev [n][max_in] int32 (may be null) holds each packet's arrival time on the server's clock in
+ * us, with the clock's wrap and serial arithmetic.  Without it every arrival is the call's now; an arrival after now
+ * (serial) is taken as now.  The anchor (a_s, a_t) is kept as in l2h_jitter_buffer_timed, except that a_t is the
+ * arrival time of the packet that set it, not the now of its call.
+ * Lateness.  With the anchor in force before packet s is placed, its lateness is
+ *     l = arrival - (a_t + (s - a_s) period)   us, s - a_s in [-2^15, 2^15), in serial int32,
+ * the quantity the release rule compares with the deadline.  It is measured for every packet placed in the window and
+ * for every late packet (d < 0; late packets are the evidence that the deadline is too short), except that nothing is
+ * measured for a slot's first packet, a duplicate, a packet that restarts the slot, or a packet that arrives while the
+ * slot is stalled (an outage is not jitter).
+ * Statistics, in exact integer arithmetic, so that the same timestamped arrivals cut into other calls give the same
+ * statistics.  A slot keeps 64 int32 bins h_0 .. h_63 of width w = max(1, ceil(hi_us / 64)) us (a bin read outside
+ * [0, 2^30] is clamped to it) and k, the packets measured (saturating at 2^31 - 1).  Lateness l falls in bin
+ * b = clamp(floor(l / w), 0, 63): early packets land in bin 0, lateness of hi_us or more in bin 63.  With the memory
+ * N = max(1, round(5e6 / period)) packets (about 5 s) each measured packet, in arrival order, with m = min(k + 1, N):
+ *     h_i -= floor(h_i / m) for every i;  h_b += floor(2^24 / m);  k += 1
+ * so the first packets are weighted as a plain mean and later ones forget exponentially; the bins sum to about 2^24.
+ * Deadline.  Once per call, after its arrivals and before the release at now, each listed slot that has started
+ * recomputes its deadline: with the tail T_b = sum_{i > b} h_i, the total T = sum_i h_i (int64) and
+ * r = round(late_rate 2^16), b is the smallest bin with T_b 2^16 <= r T, and the deadline is clamp((b + 1) w, lo_us,
+ * hi_us).  While k < ceil(1 / late_rate) it is hi_us: a (1 - late_rate) quantile needs that many samples.
+ * The release at now is then l2h_jitter_buffer_timed's rule with the slot's deadline; the stall S, restarts,
+ * concealment, backlog and max_out are unchanged.  With lo_us == hi_us == D and no arrivals_dev (or every arrival the
+ * now of its call) the output, the out counts and head words 0-15 equal l2h_jitter_buffer_timed's at deadline D, bit
+ * for bit.  A slot's deadlines are checked only in calls that list it: a service lists every live slot in every tick.
+ *
+ * State: [n_slots][channels][row_floats] with row_floats from l2h_jitter_buffer_adaptive_layout, 66 words more than
+ * l2h_jitter_buffer_layout's.  The first row_floats - 66 words of each channel's row are laid out as in
+ * l2h_jitter_buffer_timed; channel 0's last 66 words are the statistics block: 64 bins, k, and the deadline of the last
+ * call (0 until the slot has started; the other channels leave these words unused).  All zeros is a fresh slot, so a
+ * slot is reset by zeroing its rows and moved by copying them.
+ *
+ * l2h_jitter_buffer_adaptive_layout: the arguments and errors of l2h_jitter_buffer_layout.
+ *
+ * l2h_jitter_buffer_adaptive: the arguments of l2h_jitter_buffer_timed with deadline_us replaced by
+ *   arrivals_dev    [n][max_in] int32 of DEVICE memory read when the kernel runs, or null: packet j's arrival time, so a
+ *                   call captured in a CUDA graph serves any arrival times rewritten in place
+ *   lo_us, hi_us    0 <= lo_us <= hi_us, the bounds of every slot's deadline, in microseconds
+ *   late_rate       in (0, 0.5]: the fraction of measured packets the deadline may leave late
+ * Errors: those of l2h_jitter_buffer (the staging of a row also holds max_in more words), and 1 = now_dev null,
+ * lo_us < 0, hi_us < lo_us, late_rate outside (0, 0.5].  Asynchronous on `stream`. */
+int l2h_jitter_buffer_adaptive_layout(int32_t channels, int32_t rate, int32_t packet, int32_t depth, int32_t window,
+                                      int32_t max_out, int32_t* row_floats);
+int l2h_jitter_buffer_adaptive(const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, int32_t max_in,
+                               const int32_t* seqs_dev, const int32_t* counts_dev, float* y_dev, int64_t y_row_stride,
+                               int64_t y_ch_stride, int32_t* out_counts_dev, int32_t n, int32_t channels,
+                               const int32_t* slots_dev, float* state_dev, int32_t n_slots, int32_t rate, int32_t packet,
+                               int32_t depth, int32_t window, int32_t max_out, const int32_t* now_dev,
+                               const int32_t* arrivals_dev, int32_t lo_us, int32_t hi_us, double late_rate, void* stream);
 
 #ifdef __cplusplus
 }

@@ -210,6 +210,15 @@ _SIGS = {
                                               ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
                                               ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
                                               ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p]),
+    "l2h_jitter_buffer_adaptive_layout": (ctypes.c_int, [ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
+                                                        ctypes.c_int32, ctypes.c_int32, ctypes.POINTER(ctypes.c_int32)]),
+    "l2h_jitter_buffer_adaptive": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int32,
+                                                 ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64,
+                                                 ctypes.c_int64, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
+                                                 ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
+                                                 ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
+                                                 ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
+                                                 ctypes.c_double, ctypes.c_void_p]),
     "l2h_embed_create": (ctypes.c_int, [ctypes.POINTER(EmbedConfig), c_void_pp]),
     "l2h_embed_destroy": (ctypes.c_int, [ctypes.c_void_p]),
     "l2h_embed_set_option": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_int32]),

@@ -1794,6 +1794,23 @@ struct JbClock {
     int32_t stall;
 };
 
+// The adaptive form: the timed form whose deadline is drawn per slot from a histogram of the lateness of its packets.
+// Channel 0's row ends in a block of JB_STATS words (int32): JB_BINS bins summing to about JB_UNIT, the packets
+// measured (saturating), and the deadline of the slot's last call.
+constexpr int JB_BINS = 64;
+constexpr int JB_STATS = JB_BINS + 2;
+constexpr int JB_UNIT = 1 << 24;
+constexpr int JB_BIN_MAX = 1 << 30;    // a bin read from the state is clamped to [0, JB_BIN_MAX]
+enum { JB_UNTIMED, JB_TIMED, JB_ADAPTIVE };
+
+// the adaptive form's parameters: the arrival times [n][M] (µs, or null: every packet arrives at now), the bounds of the
+// deadline, the bin width w = max(1, ceil(hi / 64)), r = round(late_rate 2^16), the warm-up ceil(1 / late_rate)
+// (packets measured before the quantile is used) and the memory N = max(1, round(5e6 / period)) in packets
+struct JbAdapt {
+    const int32_t* arrivals;
+    int32_t lo, hi, w, r, warm, mem;
+};
+
 // a difference of 16-bit sequence numbers in serial arithmetic: v mod 2^16 taken in [-2^15, 2^15)
 L2H_DEVINL int jb_ser(int v) {
     v &= JB_SEQ - 1;
@@ -1849,16 +1866,58 @@ L2H_DEVINL int jb_pitch(const float* win, int64_t WL, int base, int C, float* su
     return *tau;
 }
 
+// the histogram bin of a lateness of l µs: floor(l / w) clamped to [0, JB_BINS - 1]
+L2H_DEVINL int jb_bin(int l, int w) { return l < 0 ? 0 : min(l / w, JB_BINS - 1); }
+
+// The adaptive form's statistics, run by warp 0 of a row whose slot has started (every lane calls it): the `nm`
+// lateness bins mb[] of this call, in arrival order, enter the slot's block sb (lane l owns bins 2 l and 2 l + 1); then
+// the deadline is found by a suffix scan over the bins.  Returns the deadline (on every lane) and writes the block.
+L2H_DEVINL int jb_stats(float* sb, const int* mb, int nm, const JbAdapt& ad) {
+    const int lane = threadIdx.x;
+    int h0 = min(max(__float_as_int(sb[2 * lane]), 0), JB_BIN_MAX);
+    int h1 = min(max(__float_as_int(sb[2 * lane + 1]), 0), JB_BIN_MAX);
+    int k = max(__float_as_int(sb[JB_BINS]), 0);
+    for (int j = 0; j < nm; ++j) {                                      // packet k is weighted 1 / min(k + 1, N)
+        const int m = min(k, ad.mem - 1) + 1, b = mb[j];
+        h0 -= h0 / m;
+        h1 -= h1 / m;
+        if (b == 2 * lane) h0 += JB_UNIT / m;
+        if (b == 2 * lane + 1) h1 += JB_UNIT / m;
+        k += k < INT32_MAX;
+    }
+    const int64_t pair = (int64_t)h0 + h1;
+    int64_t suf = pair;                                                 // bins 2 lane .. 63
+    for (int o = 1; o < 32; o <<= 1) {
+        const int64_t v = __shfl_down_sync(~0u, suf, o);
+        if (lane + o < 32) suf += v;
+    }
+    const int64_t total = __shfl_sync(~0u, suf, 0), lim = (int64_t)ad.r * total;
+    const int64_t t1 = suf - pair, t0 = t1 + h1;                        // the tails beyond bins 2 lane + 1 and 2 lane
+    const unsigned q0 = __ballot_sync(~0u, (t0 << 16) <= lim), q1 = __ballot_sync(~0u, (t1 << 16) <= lim);
+    // the smallest bin whose tail holds at most the fraction: q1 always holds on lane 31 (its tail is 0)
+    const int b = min(q0 ? 2 * (__ffs(q0) - 1) : JB_BINS, 2 * (__ffs(q1) - 1) + 1);
+    const int dl = k < ad.warm ? ad.hi : (int)min(max((int64_t)(b + 1) * ad.w, (int64_t)ad.lo), (int64_t)ad.hi);
+    sb[2 * lane] = __int_as_float(h0);
+    sb[2 * lane + 1] = __int_as_float(h1);
+    if (lane == 0) {
+        sb[JB_BINS] = __int_as_float(k);
+        sb[JB_BINS + 1] = __int_as_float(dl);
+    }
+    return dl;
+}
+
 // One CTA = one call row over all C channels (one decision per slot).  Row i pushes packets j < counts[i] of x row i
 // with sequence numbers seqs[i][j] and writes y[i][c][0 .. out_counts[i] P).  Timed: the arrivals also keep the anchor,
 // an arrival at or past next restarts a stalled slot, and after them a missing next is also released as a loss once its
-// deadline on the clock has passed (`ck`; unused untimed).
-template <bool Timed>
-__global__ void __launch_bounds__(RS_TILE)
-jitter_buffer_kernel_t(const float* __restrict__ x, int64_t x_row, int64_t x_ch, const int32_t* __restrict__ seqs,
+// deadline on the clock has passed (`ck`; unused untimed).  Adaptive: as timed, with each packet's own arrival time, the
+// lateness of the measured arrivals kept in the slot's statistics block by warp 0 between thread 0's arrivals and its
+// release at now, and the deadline the block gives (`ad`; unused otherwise).
+template <int Mode>
+L2H_DEVINL void jb_row(const float* __restrict__ x, int64_t x_row, int64_t x_ch, const int32_t* __restrict__ seqs,
                        const int32_t* __restrict__ counts, float* __restrict__ y, int64_t y_row, int64_t y_ch,
                        int32_t* __restrict__ out_counts, int C, const int32_t* __restrict__ slots, float* __restrict__ state,
-                       int n_slots, const __grid_constant__ JbParams p, const JbClock ck) {
+                       int n_slots, const JbParams& p, const JbClock& ck, const JbAdapt& ad) {
+    constexpr bool Timed = Mode != JB_UNTIMED, Adaptive = Mode == JB_ADAPTIVE;
     extern __shared__ float sm[];
     __shared__ float sc[RS_TILE];
     __shared__ int lt[RS_TILE];
@@ -1885,14 +1944,18 @@ jitter_buffer_kernel_t(const float* __restrict__ x, int64_t x_row, int64_t x_ch,
         for (int i = tid; i < p.tmax; i += blockDim.x) per[c * p.tmax + i] = st[c * rf + o_per + i];
     }
     __syncthreads();
-    if (tid == 0) {
+    // thread 0's bookkeeping; in the adaptive form warp 0 enters too, and between thread 0's arrivals and its release
+    // at now it keeps the slot's statistics and finds its deadline
+    __shared__ int nm_s;
+    if (Adaptive ? tid < 32 : tid == 0) {
         int started = __float_as_int(st[JB_STARTED]) != 0, next = int_word(st[JB_NEXT], JB_SEQ - 1);
         int pos = int_word(st[JB_POS], R - 1), pend = int_word(st[JB_PEND], W);
         int lost = 0, late = 0, dup = 0, dropped = 0, restarts = 0;
         const auto slot = [&](int d) { return (pos + pend + d) % R; };
         const auto held = [&](int d) { return tg[slot(d)] == ((next + d) & (JB_SEQ - 1)) + 1; };
         int far = -1;                                                   // the farthest stored packet in the window
-        for (int d = 0; d < W; ++d) if (held(d)) far = d;
+        if (!Adaptive || tid == 0)
+            for (int d = 0; d < W; ++d) if (held(d)) far = d;
         // timed: the anchor (a_s, a_t), the clock of this call and the deadline releases
         int a_s = 0, expired = 0;
         uint32_t a_t = 0, now = 0;
@@ -1903,92 +1966,122 @@ jitter_buffer_kernel_t(const float* __restrict__ x, int64_t x_row, int64_t x_ch,
         // the concealment has gone silent: no deadline releases, and the next arrival at or past next restarts
         const auto stalled = [&] { return Timed && jb_ser(next - a_s - 1) >= ck.stall; };
         const int32_t* sq = seqs + (int64_t)sr.row * p.M;
-        for (int j = 0; j < cnt; ++j) {
-            cp[j] = -1;
-            const int s = sq[j];
-            if (s < 0 || s >= JB_SEQ) continue;                         // no sequence number: skipped
-            if (!started) started = 1, next = s, a_s = s;
-            int d = (s - next) & (JB_SEQ - 1);
-            if (d >= JB_SEQ / 2) d -= JB_SEQ;
-            bool recover = false;
-            if (d < 0) { late = min(late + 1, INT32_MAX - 1); continue; }
-            if (d < W && !stalled()) {
-                if (held(d)) { dup = min(dup + 1, INT32_MAX - 1); continue; }
-            } else {                                                    // beyond the window (or stalled): a restart
-                for (int e = 0; e < W; ++e) {
-                    if (held(e)) dropped = min(dropped + 1, INT32_MAX - 1);
-                    tg[slot(e)] = 0;
+        int* mb = kind + p.max_out;                                     // adaptive: [M] the bins of the measured arrivals
+        int nm = 0;
+        if (!Adaptive || tid == 0) {                                    // the arrivals
+            for (int j = 0; j < cnt; ++j) {
+                cp[j] = -1;
+                const int s = sq[j];
+                if (s < 0 || s >= JB_SEQ) continue;                         // no sequence number: skipped
+                // adaptive: the packet's arrival (now without arrival times, or when it lies after now), and the
+                // bin of its lateness against the anchor in force (for the packets measured: not the slot's first)
+                uint32_t arr = now;
+                const bool first = !started;
+                if constexpr (Adaptive)
+                    if (ad.arrivals) {
+                        const uint32_t a = (uint32_t)ad.arrivals[(int64_t)sr.row * p.M + j];
+                        if ((int)(a - now) < 0) arr = a;
+                    }
+                const auto measure = [&] {
+                    mb[nm++] = jb_bin((int)(arr - (a_t + (uint32_t)jb_ser(s - a_s) * ck.period)), ad.w);
+                };
+                if (!started) started = 1, next = s, a_s = s;
+                int d = (s - next) & (JB_SEQ - 1);
+                if (d >= JB_SEQ / 2) d -= JB_SEQ;
+                bool recover = false;
+                if (d < 0) {
+                    late = min(late + 1, INT32_MAX - 1);
+                    if constexpr (Adaptive) if (!stalled()) measure();     // a late packet is measured
+                    continue;
                 }
-                restarts = min(restarts + 1, INT32_MAX - 1);
-                next = s, d = 0, far = -1, recover = true, a_s = s;
-            }
-            if constexpr (Timed)                                        // the first packet, a restart, or a new highest
-                if (jb_ser(s - a_s) >= 0) a_s = s, a_t = now;
-            const int at = slot(d);
-            tg[at] = s + 1;
-            for (int k = 0; k < j; ++k) if (cp[k] == at) cp[k] = -1;    // a slot freed and reused in this call
-            cp[j] = at;
-            far = max(far, d);
-            for (;;) {                                                  // the release rule
-                int t;
-                if (held(0)) t = (next + 1) | (recover ? JB_RECOVER : 0), recover = false;
-                else if (far >= p.D + 1) t = JB_LOST, lost = min(lost + 1, INT32_MAX - 1);
-                else break;
-                if (pend == W) {                                        // the backlog is full: its oldest goes
-                    tg[pos] = 0;
-                    pos = (pos + 1) % R, --pend;
-                    dropped = min(dropped + 1, INT32_MAX - 1);
+                if (d < W && !stalled()) {
+                    if (held(d)) { dup = min(dup + 1, INT32_MAX - 1); continue; }
+                    if constexpr (Adaptive) if (!first) measure();
+                } else {                                                    // beyond the window (or stalled): a restart
+                    for (int e = 0; e < W; ++e) {
+                        if (held(e)) dropped = min(dropped + 1, INT32_MAX - 1);
+                        tg[slot(e)] = 0;
+                    }
+                    restarts = min(restarts + 1, INT32_MAX - 1);
+                    next = s, d = 0, far = -1, recover = true, a_s = s;
                 }
-                tg[(pos + pend) % R] = t;
-                ++pend, next = (next + 1) & (JB_SEQ - 1), --far;
-            }
-        }
-        if constexpr (Timed) {
-            // the release rule once more at now, with a third way to release next: it expired (packet s is expected at
-            // a_t + (s - a_s) period) and the slot has not stalled
-            while (started) {
-                int t;
-                if (held(0)) t = next + 1;
-                else if (far >= p.D + 1) t = JB_LOST, lost = min(lost + 1, INT32_MAX - 1);
-                else if (!stalled() && (int)(now - (a_t + (uint32_t)jb_ser(next - a_s) * ck.period)) >= ck.deadline)
-                    t = JB_LOST, lost = min(lost + 1, INT32_MAX - 1), expired = min(expired + 1, INT32_MAX - 1);
-                else break;
-                if (pend == W) {
-                    tg[pos] = 0;
-                    pos = (pos + 1) % R, --pend;
-                    dropped = min(dropped + 1, INT32_MAX - 1);
+                if constexpr (Timed)                            // the first packet, a restart, or a new highest
+                    if (jb_ser(s - a_s) >= 0) a_s = s, a_t = arr;
+                const int at = slot(d);
+                tg[at] = s + 1;
+                for (int k = 0; k < j; ++k) if (cp[k] == at) cp[k] = -1;    // a slot freed and reused in this call
+                cp[j] = at;
+                far = max(far, d);
+                for (;;) {                                                  // the release rule
+                    int t;
+                    if (held(0)) t = (next + 1) | (recover ? JB_RECOVER : 0), recover = false;
+                    else if (far >= p.D + 1) t = JB_LOST, lost = min(lost + 1, INT32_MAX - 1);
+                    else break;
+                    if (pend == W) {                                        // the backlog is full: its oldest goes
+                        tg[pos] = 0;
+                        pos = (pos + 1) % R, --pend;
+                        dropped = min(dropped + 1, INT32_MAX - 1);
+                    }
+                    tg[(pos + pend) % R] = t;
+                    ++pend, next = (next + 1) & (JB_SEQ - 1), --far;
                 }
-                tg[(pos + pend) % R] = t;
-                ++pend, next = (next + 1) & (JB_SEQ - 1), --far;
             }
         }
-        const int n_out = min(pend, p.max_out);
-        for (int k = 0; k < n_out; ++k) {                               // what each written packet is
-            // a released packet plays whatever its number: a restart may lie between it and next; a malformed tag conceals
-            const int at = (pos + k) % R, t = tg[at], s1 = t & ~JB_RECOVER;
-            kind[k] = s1 >= 1 && s1 <= JB_SEQ ? t : JB_LOST;
-            tg[at] = 0;
+        int deadline = ck.deadline;
+        if constexpr (Adaptive) {                                       // a slot that has started: its statistics
+            if (tid == 0) nm_s = started ? nm : -1;
+            __syncwarp();
+            deadline = nm_s >= 0 ? jb_stats(st + rf - JB_STATS, mb, nm_s, ad) : ad.hi;
         }
-        pos = (pos + n_out) % R, pend -= n_out;
-        int nheld = 0;
-        for (int d = 0; d < W; ++d) nheld += held(d);
-        st[JB_STARTED] = __int_as_float(started);
-        st[JB_NEXT] = __int_as_float(next);
-        st[JB_POS] = __int_as_float(pos);
-        st[JB_PEND] = __int_as_float(pend);
-        st[JB_C_LOST] = add_word(st[JB_C_LOST], lost);
-        st[JB_C_LATE] = add_word(st[JB_C_LATE], late);
-        st[JB_C_DUP] = add_word(st[JB_C_DUP], dup);
-        st[JB_C_DROPPED] = add_word(st[JB_C_DROPPED], dropped);
-        st[JB_C_RESTARTS] = add_word(st[JB_C_RESTARTS], restarts);
-        st[JB_HELD] = __int_as_float(nheld);
-        if constexpr (Timed) {
-            st[JB_ANCHOR_SEQ] = __int_as_float(a_s);
-            st[JB_ANCHOR_T] = __int_as_float((int)a_t);
-            st[JB_C_EXPIRED] = add_word(st[JB_C_EXPIRED], expired);
+        if (!Adaptive || tid == 0) {
+            if constexpr (Timed) {
+                // the release rule once more at now, with a third way to release next: it expired (packet s is
+                // expected at a_t + (s - a_s) period) and the slot has not stalled
+                while (started) {
+                    int t;
+                    if (held(0)) t = next + 1;
+                    else if (far >= p.D + 1) t = JB_LOST, lost = min(lost + 1, INT32_MAX - 1);
+                    else if (!stalled() && (int)(now - (a_t + (uint32_t)jb_ser(next - a_s) * ck.period)) >= deadline)
+                        t = JB_LOST, lost = min(lost + 1, INT32_MAX - 1), expired = min(expired + 1, INT32_MAX - 1);
+                    else break;
+                    if (pend == W) {
+                        tg[pos] = 0;
+                        pos = (pos + 1) % R, --pend;
+                        dropped = min(dropped + 1, INT32_MAX - 1);
+                    }
+                    tg[(pos + pend) % R] = t;
+                    ++pend, next = (next + 1) & (JB_SEQ - 1), --far;
+                }
+            }
+            const int n_out = min(pend, p.max_out);
+            for (int k = 0; k < n_out; ++k) {                               // what each written packet is
+                // a released packet plays whatever its number: a restart may lie between it and next; a malformed
+                // tag conceals
+                const int at = (pos + k) % R, t = tg[at], s1 = t & ~JB_RECOVER;
+                kind[k] = s1 >= 1 && s1 <= JB_SEQ ? t : JB_LOST;
+                tg[at] = 0;
+            }
+            pos = (pos + n_out) % R, pend -= n_out;
+            int nheld = 0;
+            for (int d = 0; d < W; ++d) nheld += held(d);
+            st[JB_STARTED] = __int_as_float(started);
+            st[JB_NEXT] = __int_as_float(next);
+            st[JB_POS] = __int_as_float(pos);
+            st[JB_PEND] = __int_as_float(pend);
+            st[JB_C_LOST] = add_word(st[JB_C_LOST], lost);
+            st[JB_C_LATE] = add_word(st[JB_C_LATE], late);
+            st[JB_C_DUP] = add_word(st[JB_C_DUP], dup);
+            st[JB_C_DROPPED] = add_word(st[JB_C_DROPPED], dropped);
+            st[JB_C_RESTARTS] = add_word(st[JB_C_RESTARTS], restarts);
+            st[JB_HELD] = __int_as_float(nheld);
+            if constexpr (Timed) {
+                st[JB_ANCHOR_SEQ] = __int_as_float(a_s);
+                st[JB_ANCHOR_T] = __int_as_float((int)a_t);
+                st[JB_C_EXPIRED] = add_word(st[JB_C_EXPIRED], expired);
+            }
+            out_counts[sr.row] = n_out;
+            n_out_s = n_out;
         }
-        out_counts[sr.row] = n_out;
-        n_out_s = n_out;
     }
     __syncthreads();
     const int n_out = n_out_s;
@@ -2053,10 +2146,30 @@ jitter_buffer_kernel_t(const float* __restrict__ x, int64_t x_row, int64_t x_ch,
     }
 }
 
-// the parameters of a jitter buffer and the shared-memory bytes of a call of `arrivals` packets per row: 0, or an error
-// code (1 invalid, 2 the staging exceeds shared memory) with its message
+template <bool Timed>
+__global__ void __launch_bounds__(RS_TILE)
+jitter_buffer_kernel_t(const float* __restrict__ x, int64_t x_row, int64_t x_ch, const int32_t* __restrict__ seqs,
+                       const int32_t* __restrict__ counts, float* __restrict__ y, int64_t y_row, int64_t y_ch,
+                       int32_t* __restrict__ out_counts, int C, const int32_t* __restrict__ slots, float* __restrict__ state,
+                       int n_slots, const __grid_constant__ JbParams p, const JbClock ck) {
+    jb_row<Timed ? JB_TIMED : JB_UNTIMED>(x, x_row, x_ch, seqs, counts, y, y_row, y_ch, out_counts, C, slots, state,
+                                          n_slots, p, ck, JbAdapt{});
+}
+
+__global__ void __launch_bounds__(RS_TILE)
+jitter_buffer_adaptive_kernel(const float* __restrict__ x, int64_t x_row, int64_t x_ch, const int32_t* __restrict__ seqs,
+                              const int32_t* __restrict__ counts, float* __restrict__ y, int64_t y_row, int64_t y_ch,
+                              int32_t* __restrict__ out_counts, int C, const int32_t* __restrict__ slots,
+                              float* __restrict__ state, int n_slots, const __grid_constant__ JbParams p, const JbClock ck,
+                              const __grid_constant__ JbAdapt ad) {
+    jb_row<JB_ADAPTIVE>(x, x_row, x_ch, seqs, counts, y, y_row, y_ch, out_counts, C, slots, state, n_slots, p, ck, ad);
+}
+
+// the parameters of a jitter buffer and the shared-memory bytes of a call of `arrivals` packets per row (the adaptive
+// form's rows end in the statistics block and stage the bins of the arrivals too): 0, or an error code (1 invalid, 2 the
+// staging exceeds shared memory) with its message
 static int jb_params(const std::string& who, int32_t channels, int32_t rate, int32_t packet, int32_t depth, int32_t window,
-                     int32_t max_out, int32_t arrivals, JbParams* p, int* smem) {
+                     int32_t max_out, int32_t arrivals, JbParams* p, int* smem, bool adaptive = false) {
     if (channels <= 0) return fail(1, who + ": channels must be positive");
     if (rate < 8000 || rate > 384000) return fail(1, who + ": rate " + std::to_string(rate) + " lies outside [8000, 384000] Hz");
     if (packet < 1) return fail(1, who + ": packet " + std::to_string(packet) + " is not positive");
@@ -2071,12 +2184,12 @@ static int jb_params(const std::string& who, int32_t channels, int32_t rate, int
     p->hist = p->wc + p->tmax;
     p->lr = std::min(samples(0.004), packet);
     p->ga = samples(0.010), p->gb = samples(0.060);
-    p->rf = JB_HEAD + p->R + (int64_t)p->R * packet + p->hist + p->tmax;
+    p->rf = JB_HEAD + p->R + (int64_t)p->R * packet + p->hist + p->tmax + (adaptive ? JB_STATS : 0);
     if ((int64_t)channels * p->rf > INT32_MAX)
         return fail(1, who + ": a slot of " + std::to_string(channels) + " channels, window " + std::to_string(window) +
                            " and packets of " + std::to_string(packet) + " samples is too large");
     const int64_t floats = (int64_t)channels * (p->hist + (int64_t)max_out * packet) + p->hist +
-                           (int64_t)channels * p->tmax + p->R + arrivals + max_out;
+                           (int64_t)channels * p->tmax + p->R + arrivals + max_out + (adaptive ? arrivals : 0);
     return staging(who, floats, std::to_string(channels) + " channels at " + std::to_string(rate) + " Hz with " +
                                     std::to_string(max_out) + " packets of " + std::to_string(packet) +
                                     " samples written per row are too large", "words per row", smem);
@@ -2094,21 +2207,35 @@ extern "C" int l2h_jitter_buffer_layout(int32_t channels, int32_t rate, int32_t 
     return 0;
 }
 
+extern "C" int l2h_jitter_buffer_adaptive_layout(int32_t channels, int32_t rate, int32_t packet, int32_t depth,
+                                                 int32_t window, int32_t max_out, int32_t* row_floats) {
+    using namespace l2h;
+    if (!row_floats) return fail(1, "l2h_jitter_buffer_adaptive_layout: null pointer");
+    JbParams p;
+    if (int rc = jb_params("l2h_jitter_buffer_adaptive_layout", channels, rate, packet, depth, window, max_out, 1, &p,
+                           nullptr, true))
+        return rc;
+    *row_floats = (int32_t)p.rf;
+    return 0;
+}
+
 namespace l2h {
 constexpr auto jitter_buffer_kernel = jitter_buffer_kernel_t<false>;
 
-// both entries: the checks of l2h_jitter_buffer, then one launch of the untimed kernel (now_dev null) or the timed one
+// the three entries: the checks of l2h_jitter_buffer, then one launch of the untimed kernel (now_dev null), the timed one
+// or, with `ad` (whose lo, hi and late rate r are set), the adaptive one
 static int jb_call(const std::string& who, const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, int32_t max_in,
                    const int32_t* seqs_dev, const int32_t* counts_dev, float* y_dev, int64_t y_row_stride,
                    int64_t y_ch_stride, int32_t* out_counts_dev, int32_t n, int32_t channels, const int32_t* slots_dev,
                    float* state_dev, int32_t n_slots, int32_t rate, int32_t packet, int32_t depth, int32_t window,
-                   int32_t max_out, const int32_t* now_dev, int32_t deadline_us, void* stream) {
+                   int32_t max_out, const int32_t* now_dev, int32_t deadline_us, void* stream, JbAdapt* ad = nullptr) {
     if (int rc = slot_call(who, {x_dev, seqs_dev, counts_dev, y_dev, out_counts_dev, slots_dev, state_dev},
                            "n, channels, max_in and n_slots", {n, channels, max_in, n_slots}, n, channels, n_slots))
         return rc;
     JbParams p;
     int smem;
-    if (int rc = jb_params(who, channels, rate, packet, depth, window, max_out, max_in, &p, &smem)) return rc;
+    if (int rc = jb_params(who, channels, rate, packet, depth, window, max_out, max_in, &p, &smem, ad != nullptr))
+        return rc;
     const Rows x{"x", x_row_stride, x_ch_stride, (int64_t)max_in * packet},
         y{"y", y_row_stride, y_ch_stride, (int64_t)max_out * packet};
     if (x.len > INT32_MAX) return fail(1, who + ": max_in * packet is too large");
@@ -2119,6 +2246,19 @@ static int jb_call(const std::string& who, const float* x_dev, int64_t x_row_str
         // period = round(1e6 packet / rate) µs, exactly, taken mod 2^32 as the clock is; S = ceil(gb / packet)
         ck.period = (uint32_t)((2000000 * (int64_t)packet + rate) / (2 * (int64_t)rate));
         ck.stall = (p.gb + packet - 1) / packet;
+    }
+    if (ad) {
+        // w = max(1, ceil(hi / 64)); N = max(1, round(5e6 / period)) with the period before it is taken mod 2^32
+        const int64_t period = (2000000 * (int64_t)packet + rate) / (2 * (int64_t)rate);
+        ad->w = (int32_t)std::max<int64_t>(1, ((int64_t)ad->hi + JB_BINS - 1) / JB_BINS);
+        ad->mem = (int32_t)std::max<int64_t>(1, (10000000 + period) / (2 * period));
+        if (smem > RS_SMEM_BYTES - 4096)
+            if (cudaError_t e = full_staging(jitter_buffer_adaptive_kernel))
+                return fail(3, who + ": " + cudaGetErrorString(e));
+        jitter_buffer_adaptive_kernel<<<(unsigned)n, RS_TILE, smem, static_cast<cudaStream_t>(stream)>>>(
+            x_dev, x_row_stride, x_ch_stride, seqs_dev, counts_dev, y_dev, y_row_stride, y_ch_stride, out_counts_dev,
+            channels, slots_dev, state_dev, n_slots, p, ck, *ad);
+        return launched(who);
     }
     const auto kernel = now_dev ? jitter_buffer_kernel_t<true> : jitter_buffer_kernel;
     if (smem > RS_SMEM_BYTES - 4096)                                    // then the static words need the opt-in
@@ -2153,4 +2293,27 @@ extern "C" int l2h_jitter_buffer_timed(const float* x_dev, int64_t x_row_stride,
     return jb_call(who, x_dev, x_row_stride, x_ch_stride, max_in, seqs_dev, counts_dev, y_dev, y_row_stride, y_ch_stride,
                    out_counts_dev, n, channels, slots_dev, state_dev, n_slots, rate, packet, depth, window, max_out,
                    now_dev, deadline_us, stream);
+}
+
+extern "C" int l2h_jitter_buffer_adaptive(const float* x_dev, int64_t x_row_stride, int64_t x_ch_stride, int32_t max_in,
+                                          const int32_t* seqs_dev, const int32_t* counts_dev, float* y_dev,
+                                          int64_t y_row_stride, int64_t y_ch_stride, int32_t* out_counts_dev, int32_t n,
+                                          int32_t channels, const int32_t* slots_dev, float* state_dev, int32_t n_slots,
+                                          int32_t rate, int32_t packet, int32_t depth, int32_t window, int32_t max_out,
+                                          const int32_t* now_dev, const int32_t* arrivals_dev, int32_t lo_us,
+                                          int32_t hi_us, double late_rate, void* stream) {
+    using namespace l2h;
+    const std::string who = "l2h_jitter_buffer_adaptive";
+    if (!now_dev) return fail(1, who + ": null pointers");
+    if (lo_us < 0 || hi_us < lo_us)
+        return fail(1, who + ": lo_us " + std::to_string(lo_us) + " and hi_us " + std::to_string(hi_us) +
+                           " do not satisfy 0 <= lo_us <= hi_us");
+    if (!(late_rate > 0.0 && late_rate <= 0.5))
+        return fail(1, who + ": late_rate " + std::to_string(late_rate) + " lies outside (0, 0.5]");
+    // r = round(late_rate 2^16); the warm-up ceil(1 / late_rate), at most 2^31 - 1
+    JbAdapt ad{arrivals_dev, lo_us, hi_us, 0, (int32_t)std::floor(late_rate * 65536.0 + 0.5),
+               (int32_t)std::min(std::ceil(1.0 / late_rate), (double)INT32_MAX), 0};
+    return jb_call(who, x_dev, x_row_stride, x_ch_stride, max_in, seqs_dev, counts_dev, y_dev, y_row_stride, y_ch_stride,
+                   out_counts_dev, n, channels, slots_dev, state_dev, n_slots, rate, packet, depth, window, max_out,
+                   now_dev, 0, stream, &ad);
 }

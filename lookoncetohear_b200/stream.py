@@ -874,6 +874,15 @@ class JitterBuffer(_SlotStage):
     long outage adds no latency.  A slot's deadlines are checked only in calls that list it: list every live slot in
     every tick, with count 0 when it sent nothing.  With a deadline no call reaches, the output is the untimed buffer's.
 
+    With `deadline=(lo, hi)` (l2h_jitter_buffer_adaptive) each slot draws its own deadline from the measured lateness of
+    its packets: a packet's lateness is its arrival time minus the time the anchor expects it, and a slot keeps a
+    64-bin histogram of it over about the last 5 s of packets, in exact integer arithmetic.  Once per call the slot's
+    deadline becomes the smallest bin edge that leaves at most `late_rate` of the measured packets later than it,
+    clamped to [lo, hi]; it is `hi` until 1 / late_rate packets have been measured.  A slot's first packet, duplicates,
+    restarts and arrivals while the slot is stalled are not measured; late packets are.  Each call may take `arrivals`,
+    the packets' arrival times on the server's clock (else each arrives at `now`).  `deadline_us` reads each slot's
+    current deadline.  With lo == hi and no arrival times the output is the timed buffer's at that deadline.
+
     `state` [slots, channels, row] is a float32 tensor on `device`: all zeros is a fresh slot, so a listener is reset by
     zeroing its rows (`reset`) and moved by copying them.  The counters are int32 views that never synchronise."""
 
@@ -881,18 +890,34 @@ class JitterBuffer(_SlotStage):
     LOST, LATE, DUPLICATE, DROPPED, RESTARTS, HELD, PITCH = 6, 7, 8, 9, 10, 11, 12   # head words of channel 0
     EXPIRED = 15
 
-    def __init__(self, slots, channels, rate, packet, depth=1, window=16, max_out=4, device=None, deadline=None):
+    def __init__(self, slots, channels, rate, packet, depth=1, window=16, max_out=4, device=None, deadline=None,
+                 late_rate=None):
         super().__init__(slots, channels)
         self.rate, self.packet = _whole(rate, "rate"), _whole(packet, "packet")
         self.depth, self.window = _whole(depth, "depth", 0), _whole(window, "window")
         self.max_out = _whole(max_out, "max_out")
-        self.deadline = None if deadline is None else _whole(deadline, "deadline", 0)
+        self.adaptive = isinstance(deadline, (tuple, list))
+        if self.adaptive:
+            if len(deadline) != 2:
+                raise ValueError(f"an adaptive deadline is a pair (lo, hi) of microseconds, got {deadline!r}")
+            lo, hi = _whole(deadline[0], "deadline lo", 0), _whole(deadline[1], "deadline hi", 0)
+            if lo > hi:
+                raise ValueError(f"deadline (lo, hi) needs lo <= hi, got {deadline!r}")
+            self.deadline = (lo, hi)
+            self.late_rate = _real(0.02 if late_rate is None else late_rate, "late_rate", lambda v: 0 < v <= 0.5,
+                                   "a number in (0, 0.5]")
+        else:
+            if late_rate is not None:
+                raise ValueError("late_rate is given only with an adaptive deadline=(lo, hi)")
+            self.deadline = None if deadline is None else _whole(deadline, "deadline", 0)
+            self.late_rate = None
         if self.depth >= self.window:
             raise ValueError(f"depth must be below window = {self.window} packets, got {depth!r}")
-        self._allocate(*_layout(_cabi.lib().l2h_jitter_buffer_layout, self.channels, self.rate, self.packet, self.depth,
-                                self.window, self.max_out), device)
+        query = _cabi.lib().l2h_jitter_buffer_adaptive_layout if self.adaptive else _cabi.lib().l2h_jitter_buffer_layout
+        self._allocate(*_layout(query, self.channels, self.rate, self.packet, self.depth, self.window, self.max_out),
+                       device)
 
-    def __call__(self, x, seqs, counts, slots, out=None, out_counts=None, now=None):
+    def __call__(self, x, seqs, counts, slots, out=None, out_counts=None, now=None, arrivals=None):
         """x [n, channels, M * packet] CUDA tensor: row i pushes its packets j < counts[i], x[i, :, j P:(j + 1) P], with
         sequence numbers seqs[i, j], into slot slots[i].  Returns (y [n, channels, max_out * packet] float32, out_counts [n]
         int32 CUDA) (`out` and `out_counts`, if given, written in place): row i receives y[i, :, :out_counts[i] * packet],
@@ -900,6 +925,11 @@ class JitterBuffer(_SlotStage):
 
         `now` is required exactly when the buffer has a deadline: the server's clock in microseconds, a host int (taken
         mod 2**32) or a CUDA int32 tensor of shape (1,) used in place and read when the kernel runs.
+
+        `arrivals` (adaptive deadline only; optional) [n, M]: each packet's arrival time on the same clock, in
+        microseconds, a host integer array (taken mod 2**32, checked and uploaded) or a contiguous CUDA int32 tensor
+        used in place and read when the kernel runs.  An arrival after `now` is taken as now; without `arrivals` every
+        packet arrives at now.
 
         Host lists are checked and uploaded (`slots` n distinct ints in [0, slots), `counts` n ints in [0, M], `seqs` [n, M]
         int32 values whose first counts[i] entries of row i lie in [0, 65535], so a short row may be padded with -1; with
@@ -912,6 +942,7 @@ class JitterBuffer(_SlotStage):
         dev = self.state.device
         n, C, L = x.shape
         M = L // self.packet
+        arrivals = self._arrivals(arrivals, n, M)
         slots = device_list(slots, dev, n, self.n_slots, True, "slot")
         host_counts = None if isinstance(counts, torch.Tensor) and counts.is_cuda else counts
         counts = device_list(counts, dev, n, M + 1, False, "count")
@@ -922,9 +953,33 @@ class JitterBuffer(_SlotStage):
                 self.state, self.n_slots, self.rate, self.packet, self.depth, self.window, self.max_out)
         if now is None:
             self._run("l2h_jitter_buffer", *args)
+        elif self.adaptive:
+            self._run("l2h_jitter_buffer_adaptive", *args, now, arrivals, *self.deadline, self.late_rate)
         else:
             self._run("l2h_jitter_buffer_timed", *args, now, self.deadline)
         return out, out_counts
+
+    def _arrivals(self, arrivals, n, M):
+        """the [n, M] int32 arrival times on the state's device (None: every packet arrives at now): a CUDA tensor used
+        in place, else integers taken mod 2**32 and uploaded; ValueError without an adaptive deadline"""
+        if arrivals is None:
+            return None
+        if not self.adaptive:
+            raise ValueError("arrivals are given only to a JitterBuffer with an adaptive deadline=(lo, hi)")
+        dev = self.state.device
+        if isinstance(arrivals, torch.Tensor) and arrivals.is_cuda:
+            if (arrivals.dtype != torch.int32 or tuple(arrivals.shape) != (n, M) or not arrivals.is_contiguous()
+                    or arrivals.device != dev):
+                raise ValueError(f"a CUDA arrivals tensor must be a contiguous int32 tensor of shape ({n}, {M}) on {dev}")
+            return arrivals
+        try:
+            v = torch.as_tensor(arrivals)
+        except (TypeError, ValueError, RuntimeError, OverflowError):
+            raise ValueError("arrivals must be integers of microseconds (each within int64)") from None
+        if v.dtype.is_floating_point or v.dtype.is_complex or v.dtype == torch.bool or tuple(v.shape) != (n, M):
+            raise ValueError(f"arrivals must be integers of shape ({n}, {M}), got {tuple(v.shape)} {v.dtype}")
+        w = v.to(torch.int64).remainder(2 ** 32)
+        return torch.where(w >= 2 ** 31, w - 2 ** 32, w).to(torch.int32).contiguous().to(dev)
 
     def _now(self, now):
         """the clock of a call as a CUDA int32 tensor of shape (1,) on the state's device (None without a deadline), or
@@ -1008,6 +1063,14 @@ class JitterBuffer(_SlotStage):
     def pitch(self):
         """[slots] int32 CUDA view: the lag, in samples, of the last concealment run (0 before the first)"""
         return self._word(self.PITCH)
+
+    @property
+    def deadline_us(self):
+        """[slots] int32 CUDA view (adaptive deadline only): each slot's deadline in microseconds, as its last call
+        found it from the slot's statistics (0 before the slot's first packet); read it beside `expired` and `late`"""
+        if not self.adaptive:
+            raise ValueError("deadline_us belongs to a JitterBuffer with an adaptive deadline=(lo, hi)")
+        return self._word(self.state.shape[2] - 1)
 
     @property
     def expired(self):
